@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- KV-cache transfer GB/s (+ decode TTFT delta) for the prefill->decode hand-off.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 Workload = BASELINE.json configs[1]: Llama-3-8B bf16, 4 k-token context, paged KV block_size=16
@@ -13,8 +13,7 @@ A "step" is one gather -> NVLink -> scatter of that request's KV.
   N > 1      rank 0 = prefill GPU, ranks 1..N-1 = decode GPUs, one process per GPU, pools mapped into each other through
              CUDA IPC.  --direction pull (default): every decode GPU launches the transfer kernel itself and READS its
              blocks from the prefill pool over NVLink (the decode-side READ of vLLM's NixlConnector); --direction push:
-             rank 0 launches ONE kernel that stores to all decode pools (measured: SM-issued peer stores cap at 706 GB/s
-             per destination, peer loads reach 775; profiles/r02_copylab_{push,pull}.jsonl).
+             rank 0 launches ONE kernel that stores to all decode pools.
 
   value      GB/s of destination bytes, kernel launched through the C ABI with block tables already in HBM; K launches back
              to back, each bracketed by its own pair of CUDA events: the step time is the MEDIAN of the K per-launch device
@@ -67,7 +66,7 @@ DIRECTION = "pull"
 
 
 def configure(args):
-    """Non-default workloads (other BASELINE configs) for the numbers under profiles/; the driver uses defaults."""
+    """Non-default workloads (other BASELINE configs); the headline number uses the defaults."""
     global NL, KV_HEADS, INNER, REGION, SRC_REGION, CTX_TOKENS, N_BLOCKS, POOL_BLOCKS, BYTES_PER_DST, MODEL_NAME, CAST
     global REPLICATE, NVLS, TOPOLOGY, DIRECTION
     if args.model == "llama70b-tp4":       # configs[3]: 80 layers, 2 of 8 KV heads per rank -> 8 KiB regions
@@ -96,14 +95,14 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, copy read+write)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3; not measured)"
 
 
-NVLINK_PEER_GBS_GUIDE = 770.0   # B200_PROFILING.md: measured peer copy per direction on this pool; nominal 900
+NVLINK_PEER_GBS_NOMINAL = 450.0   # H100 SXM data sheet: NVLink 4, 900 GB/s bidirectional = 450 per direction
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -247,7 +246,7 @@ def workload_config(n_gpus):
             "layout": "LayerSeparate/BlockIsSecondDim (vLLM [2,num_blocks,16,8,128] per layer)",
             "pool_blocks": POOL_BLOCKS,
             "block_tables": "random permutation (seeded), non-contiguous on both sides",
-            "cache": f"inputs larger than L2 ({(BYTES_PER_DST + BYTES_PER_DST * SRC_REGION // REGION) / 2**20:.0f} MiB touched per step vs 126 MB L2), no flush needed",
+            "cache": f"inputs larger than L2 ({(BYTES_PER_DST + BYTES_PER_DST * SRC_REGION // REGION) / 2**20:.0f} MiB touched per step vs 50 MB L2), no flush needed",
             "bytes_per_destination": BYTES_PER_DST}
 
 
@@ -526,6 +525,8 @@ def run_ours(args):
     launches0 = K.launch_count()
     value_ms_med, value_ms_mean = timed_leg(launch, K_steps, W)
     launches_value = K.launch_count() - launches0
+    if args.dump_outputs and is_dst:   # what the last timed C-ABI launch left (untimed; before the e2e leg rewrites it)
+        dump_outputs(torch, args.dump_outputs, dst_bufs, dids[my_dst_index], dev, f"rank{rank}_", n_dst * n_src)
 
     # ================= leg 2: `e2e` -- host API, host block tables every step =================
     e2e_times = []
@@ -624,20 +625,20 @@ def run_ours(args):
         if world == 1:
             alg = BYTES_PER_DST * SRC_REGION // REGION + BYTES_PER_DST   # B_src read once + B_dst written, per launch (SURVEY §8d)
             roof = {"bound": "hbm", "achieved": round(alg / (ms_per_step * 1e-3) / 1e9, 2), "peak": peak, "unit": "GB/s",
-                    "frac": round(alg / (ms_per_step * 1e-3) / 1e9 / peak, 4), "traffic": ncu_traffic("n1"), "peak_source": peak_src,
+                    "frac": round(alg / (ms_per_step * 1e-3) / 1e9 / peak, 4), "peak_source": peak_src,
                     "kernel": f"kvbm_paged_copy_kernel<{CAST}>", "algorithmic_bytes_per_launch": alg,
                     "frac_of_mean_step": round(alg / (value_ms_mean * 1e-3) / 1e9 / peak, 4)}
         else:
             # NVLink: bytes that cross the source GPU's port per step / step time, against a contiguous peer copy measured
-            # on THIS box in this process (gpu_baselines.memcpy_whole) -- else the guide's 770 GB/s
+            # in this run (gpu_baselines.memcpy_whole) -- else the data sheet's 450 GB/s per direction
             measured = gb.get("memcpy_whole", {}).get("gbs")
-            nv_peak = measured or NVLINK_PEER_GBS_GUIDE
+            nv_peak = measured or NVLINK_PEER_GBS_NOMINAL
             per_src = value / n_src
             roof = {"bound": "nvlink", "achieved": round(per_src, 2), "peak": round(nv_peak, 1), "unit": "GB/s",
-                    "frac": round(per_src / nv_peak, 4), "frac_of_nominal_900": round(per_src / 900.0, 4),
-                    "traffic": ncu_traffic("n2") if world == 2 else None, "sources": n_src,
+                    "frac": round(per_src / nv_peak, 4), "frac_of_nominal_450": round(per_src / NVLINK_PEER_GBS_NOMINAL, 4),
+                    "sources": n_src,
                     "peak_source": ("contiguous cudaMemcpyAsync rank0 -> rank1 measured in this run (gpu_baselines.memcpy_whole)" if measured else
-                                    "B200_PROFILING.md measured peer copy 770 GB/s per direction") + "; nominal 900",
+                                    "H100 SXM data sheet, not measured") + "; nominal 450 per direction",
                     "kernel": "kvbm_paged_copy_kernel<0>", "algorithmic_bytes_per_launch": (total_dst_bytes // n_src) // (n_dst if pull else 1),
                     "launches_per_step": n_dst if pull else 1,
                     "hbm_read_gbs_source": round((BYTES_PER_DST * SRC_REGION // REGION) * (1 if REPLICATE else n_dst) / (ms_per_step * 1e-3) / 1e9, 2)}
@@ -705,6 +706,28 @@ def run_ours(args):
     if world > 1:
         dist.destroy_process_group()
     return 0 if ok else 1
+
+
+def dump_outputs(torch, out_dir, dst_bufs, did, dev, prefix, n_dests, sample_budget=40 << 20, seed=2025):
+    """Writes what the timed `value` leg (C-ABI paged_copy launches) left in this destination pool (every destination rank
+    writes its own files):
+      <prefix>region_sums.npy     float64 [NL, OUTER, N_BLOCKS]: sum of (i + 1) * byte[i] over every moved (layer, K/V,
+                                  block) region, in block-table order (exact: below 2**53)
+      <prefix>regions_sample.npy  float32 [k, REGION]: every byte of a fixed sample of k moved regions (seeded; k keeps
+                                  the samples of all destinations within `sample_budget` bytes), one value per byte"""
+    os.makedirs(out_dir, exist_ok=True)
+    d = torch.as_tensor(np.asarray(did, dtype=np.int64), device=dev)
+    w = torch.arange(1, REGION + 1, dtype=torch.int64, device=dev)
+    sums = torch.stack([(buf.view(OUTER, POOL_BLOCKS, REGION).index_select(1, d).long() * w).sum(dim=2) for buf in dst_bufs])
+    np.save(os.path.join(out_dir, prefix + "region_sums.npy"), sums.cpu().numpy().astype(np.float64))
+    n = NL * OUTER * N_BLOCKS
+    k = max(1, min(n, sample_budget // (4 * REGION * n_dests)))
+    pick = np.sort(np.random.default_rng(seed).choice(n, size=k, replace=False))
+    rows = []
+    for flat in pick:
+        l, o, b = np.unravel_index(flat, (NL, OUTER, N_BLOCKS))
+        rows.append(dst_bufs[l].view(OUTER, POOL_BLOCKS, REGION)[o, int(did[b])])
+    np.save(os.path.join(out_dir, prefix + "regions_sample.npy"), torch.stack(rows).float().cpu().numpy())
 
 
 # -----------------------------------------------------------------------------------------------------
@@ -835,7 +858,7 @@ def gpu_baselines(torch, K, mgr, h_src, h_dst, sid, did, dev, world, iters=5):
         R = C.CDLL(ref_so)
         R.kvbm_kernels_launch_vectorized_copy.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p]
         res["ref_k1_flow"] = dict(timed(lambda: k1_flow(R.kvbm_kernels_launch_vectorized_copy)),
-                                  what="the reference's tensor_kernels.cu K1 (compiled unmodified for sm_100) driven like "
+                                  what="the reference's tensor_kernels.cu K1 (compiled unmodified for sm_90) driven like "
                                        "kvbm-physical executor/cuda.rs:234-327: host pointer tables, 2 x H2D, launch, host sync")
     res["ours_k1_flow"] = dict(timed(lambda: k1_flow(K.vectorized_copy)),
                                what="the same flow through this library's drop-in K1 symbol")
@@ -916,7 +939,7 @@ def nccl_bcast_baseline():
     """The reference's replicate path: one grouped ncclBcast per region (kvbm-engine collectives/nccl.rs:321-356), as the
     stand-alone binary benchmarks/nccl_bcast_baseline (single process, one communicator per GPU).  Run on 64 blocks
     (4096 regions, 128 MiB): with the full 256-block request (16 384 broadcasts per rank in ONE group) NCCL 2.27 does not
-    finish within minutes on this box (profiles/r02_nccl_bcast_n2_*.json), and the rate is flat in the size anyway."""
+    finish within minutes, and the rate is flat in the size anyway."""
     exe = os.path.join(ROOT, "benchmarks", "nccl_bcast_baseline")
     if not os.path.exists(exe):
         return {"unavailable": "benchmarks/nccl_bcast_baseline not built (needs nccl.h at build time)"}
@@ -933,16 +956,6 @@ def nccl_bcast_baseline():
         return {"unavailable": str(e)[:160]}
 
 
-def ncu_traffic(which):
-    """dram (N=1) / NVLink (N=2) bytes per launch of the dominant kernel from the committed ncu summary (profiles/), or None."""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    try:
-        d = json.load(open(p))
-        return d["paged_copy_n1_dram_bytes_per_launch"] if which == "n1" else d.get("paged_copy_n2_nvlink_bytes_per_launch")
-    except Exception:
-        return None
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -951,7 +964,7 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--quick", action="store_true", help="skip the untimed extras (sorted tables, GPU baselines, mode self-test)")
-    # non-default workloads (other BASELINE configs); results of these runs live in profiles/
+    # non-default workloads (other BASELINE configs)
     ap.add_argument("--model", default="llama8b", choices=["llama8b", "llama70b-tp4", "mixtral"])
     ap.add_argument("--ctx", type=int, default=4096, help="context tokens (blocks = ctx/16)")
     ap.add_argument("--cast", default="none", choices=["none", "fp8"])
@@ -962,7 +975,11 @@ def main():
                     help="N > 1: pull = every decode GPU launches and reads the prefill pool (default); push = the prefill GPU stores to all")
     ap.add_argument("--topology", default="fanout", choices=["fanout", "pairs"],
                     help="fanout: rank 0 -> ranks 1..N-1 (default); pairs: rank r -> rank r+N/2 (TP-sharded prefill -> decode)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed C-ABI steps, write what they left in each destination pool as DIR/<name>.npy (see dump_outputs)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs applies to --impl ours (the CPU reference arm keeps no device outputs)")
     configure(args)
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else max(args.warmup, 1)
     if args.impl == "reference":

@@ -1,4 +1,4 @@
-// copylab -- design-space study of the paged KV copy on one B200 (and, with --peer, over NVLink to GPU 1).
+// copylab -- design-space study of the paged KV copy on one H100 (and, with --peer, over NVLink to GPU 1).
 // Bench-only: nothing here ships.  Stand-alone (cudart only) so a GPU call does not pay a torch import.
 //
 //   benchmarks/copylab [--peer push|pull] [--blocks 256] [--pool 1024] [--iters 30] [--only NAME]
@@ -7,7 +7,7 @@
 // (random block tables both sides).  Prints one JSON object per variant:
 //   ws_*      warp-specialised TMA ring: producer warp (descriptors + cp.async.bulk g2s), consumer warp (s2g), dynamic
 //             or static tile scheduler
-//   simt_*    SIMT gather/scatter, one CTA per region, U independent 16 B (or 32 B) loads in flight per thread
+//   simt_*    SIMT gather/scatter, one CTA per region, U independent 16 B loads in flight per thread
 //   lib       the product library's kvbm_kernels_paged_copy_v2 (dlopen dynamo_b200/libkvbm_kernels.so)
 //   ref_k1    the reference K1 recompiled (oracle/_ref), device pointer tables
 //   memcpy    cudaMemcpyAsync of the same byte count, contiguous
@@ -76,7 +76,7 @@ using kvbm::ptx::mbar_arrive;
 // sched: 0 static (item = first + k*stride in batches of B), 1 dynamic (atomic tickets of B items)
 // ------------------------------------------------------------------------------------------------------------
 struct WsParams {
-  int S, P, B, sched, store_mode, guide;  // store_mode 0 = TMA bulk store, 1 = SIMT st.v4 from smem by the consumer warp, 2 = st.v8 (256-bit)
+  int S, P, B, sched, store_mode, guide;  // store_mode 0 = TMA bulk store, 1 = SIMT st.v4 from smem by the consumer warp
   uint32_t* counter;               // [0] tickets, [1] finished rings
   unsigned long long* times;       // optional [grid*R][3]: start, first data, end
 };
@@ -202,23 +202,12 @@ __global__ void __launch_bounds__(256, 1) ws_copy_kernel(const __grid_constant__
           ptx::bulk_wait_read_n(wp.P);
           if (q >= static_cast<uint32_t>(wp.P)) mbar_arrive(empty0 + 8 * ((q - wp.P) % S));
         }
-      } else if (wp.store_mode == 1) {
+      } else {
         uint4* d4 = reinterpret_cast<uint4*>(dst);
         for (uint32_t i = lane; i < (bytes >> 4); i += 32) {
           uint4 v;
           asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(sa + i * 16));
           ptx::st_stream_v4(d4 + i, v);
-        }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(empty0 + 8 * slot);
-      } else {
-        for (uint32_t i = lane; i < (bytes >> 5); i += 32) {
-          uint4 a, b;
-          asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w) : "r"(sa + i * 32));
-          asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w) : "r"(sa + i * 32 + 16));
-          asm volatile("st.global.L1::no_allocate.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(dst + i * 32), "r"(a.x), "r"(a.y), "r"(a.z),
-                       "r"(a.w), "r"(b.x), "r"(b.y), "r"(b.z), "r"(b.w)
-                       : "memory");
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(empty0 + 8 * slot);
@@ -269,7 +258,7 @@ __global__ void __launch_bounds__(512, 1) ws_engine_kernel(const __grid_constant
 // ------------------------------------------------------------------------------------------------------------
 // simt: one CTA per `rpc` regions; T threads; each thread keeps U x 16 B loads in flight
 // ------------------------------------------------------------------------------------------------------------
-template <int U, bool V8>
+template <int U>
 __global__ void __launch_bounds__(256) simt_copy_kernel(const __grid_constant__ Job job, uint32_t regions, uint32_t rpc)
 {
   for (uint32_t rr = 0; rr < rpc; ++rr) {
@@ -278,30 +267,11 @@ __global__ void __launch_bounds__(256) simt_copy_kernel(const __grid_constant__ 
     uint64_t s, d;
     uint32_t bytes;
     item_addr(job, r * job.tiles_per_region, s, d, bytes);  // tiles_per_region == 1 for this kernel
-    constexpr int W = V8 ? 32 : 16;
-    const uint32_t n = job.src.region / W;
+    const uint32_t n = job.src.region / 16;
     const uint8_t* sp = reinterpret_cast<const uint8_t*>(s);
     uint8_t* dp = reinterpret_cast<uint8_t*>(d);
     for (uint32_t base = 0; base < n; base += U * blockDim.x) {
-      if (V8) {
-        uint32_t v[U][8];
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-          const uint32_t i = base + u * blockDim.x + threadIdx.x;
-          if (i < n)
-            asm volatile("ld.global.L1::no_allocate.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                         : "=r"(v[u][0]), "=r"(v[u][1]), "=r"(v[u][2]), "=r"(v[u][3]), "=r"(v[u][4]), "=r"(v[u][5]), "=r"(v[u][6]), "=r"(v[u][7])
-                         : "l"(sp + static_cast<size_t>(i) * 32));
-        }
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-          const uint32_t i = base + u * blockDim.x + threadIdx.x;
-          if (i < n)
-            asm volatile("st.global.L1::no_allocate.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(dp + static_cast<size_t>(i) * 32), "r"(v[u][0]),
-                         "r"(v[u][1]), "r"(v[u][2]), "r"(v[u][3]), "r"(v[u][4]), "r"(v[u][5]), "r"(v[u][6]), "r"(v[u][7])
-                         : "memory");
-        }
-      } else {
+      {
         uint4 v[U];
 #pragma unroll
         for (int u = 0; u < U; ++u) {
@@ -522,49 +492,48 @@ int main(int argc, char** argv)
     if (!remote && quick) {
       for (int guide : {1, 2, 4})
         for (int B : {8, 4}) {
-          cfgs.push_back({148, 1, 6, 2, B, 2, 32768, 0, guide});
+          cfgs.push_back({132, 1, 6, 2, B, 2, 32768, 0, guide});
           cfgs.push_back({132, 1, 6, 1, B, 2, 16384, 0, guide});
-          cfgs.push_back({74, 2, 6, 2, B, 2, 16384, 0, guide});
-          cfgs.push_back({148, 1, 12, 4, B, 2, 16384, 0, guide});
+          cfgs.push_back({66, 2, 6, 2, B, 2, 16384, 0, guide});
+          cfgs.push_back({132, 1, 12, 4, B, 2, 16384, 0, guide});
         }
-      cfgs.push_back({148, 1, 6, 2, 2, 1, 32768, 0});
+      cfgs.push_back({132, 1, 6, 2, 2, 1, 32768, 0});
       cfgs.push_back({132, 1, 6, 1, 8, 1, 16384, 0});
-      cfgs.push_back({74, 2, 6, 2, 8, 1, 16384, 0});
-      cfgs.push_back({37, 4, 3, 1, 4, 2, 16384, 0, 2});
+      cfgs.push_back({66, 2, 6, 2, 8, 1, 16384, 0});
+      cfgs.push_back({33, 4, 3, 1, 4, 2, 16384, 0, 2});
       cfgs.push_back({32, 4, 3, 1, 4, 2, 16384, 0, 2});
       cfgs.push_back({16, 4, 3, 1, 4, 2, 16384, 0, 2});
       cfgs.push_back({16, 2, 6, 2, 4, 2, 16384, 0, 2});
       cfgs.push_back({8, 4, 3, 1, 4, 2, 16384, 0, 2});
     } else if (!remote) {
       for (int sched : {1, 0})
-        for (int grid : {148, 74}) {
+        for (int grid : {132, 66}) {
           cfgs.push_back({grid, 1, 6, 2, 8, sched, 32768, 0});
           cfgs.push_back({grid, 2, 3, 1, 8, sched, 32768, 0});
           cfgs.push_back({grid, 2, 6, 2, 8, sched, 16384, 0});
           cfgs.push_back({grid, 1, 12, 4, 8, sched, 16384, 0});
           cfgs.push_back({grid, 4, 3, 1, 8, sched, 16384, 0});
         }
-      for (int grid : {111, 132, 296})
+      for (int grid : {111, 132, 264})
         for (int tile : {32768, 16384}) cfgs.push_back({grid, 1, tile == 32768 ? 3 : 6, 1, 8, 1, tile, 0});
-      cfgs.push_back({148, 1, 6, 2, 4, 1, 32768, 0});
-      cfgs.push_back({148, 1, 6, 2, 2, 1, 32768, 0});
-      cfgs.push_back({148, 1, 6, 2, 16, 1, 32768, 0});
-      cfgs.push_back({148, 1, 6, 2, 32, 1, 32768, 0});
-      cfgs.push_back({148, 1, 6, 1, 8, 1, 32768, 0});
-      cfgs.push_back({148, 1, 6, 3, 8, 1, 32768, 0});
-      cfgs.push_back({148, 1, 4, 1, 8, 1, 32768, 0});
-      cfgs.push_back({148, 1, 3, 1, 8, 1, 32768, 0});
-      cfgs.push_back({148, 1, 2, 1, 8, 1, 32768, 0});
-      cfgs.push_back({148, 1, 4, 1, 8, 1, 16384, 0});
-      cfgs.push_back({148, 1, 8, 2, 8, 1, 8192, 0});
-      cfgs.push_back({148, 2, 8, 2, 8, 1, 8192, 0});
-      cfgs.push_back({148, 1, 6, 2, 8, 1, 32768, 1});
-      cfgs.push_back({148, 2, 3, 1, 8, 1, 32768, 1});
-      cfgs.push_back({148, 4, 3, 1, 8, 1, 16384, 1});
-      cfgs.push_back({148, 4, 3, 1, 8, 1, 16384, 2});
+      cfgs.push_back({132, 1, 6, 2, 4, 1, 32768, 0});
+      cfgs.push_back({132, 1, 6, 2, 2, 1, 32768, 0});
+      cfgs.push_back({132, 1, 6, 2, 16, 1, 32768, 0});
+      cfgs.push_back({132, 1, 6, 2, 32, 1, 32768, 0});
+      cfgs.push_back({132, 1, 6, 1, 8, 1, 32768, 0});
+      cfgs.push_back({132, 1, 6, 3, 8, 1, 32768, 0});
+      cfgs.push_back({132, 1, 4, 1, 8, 1, 32768, 0});
+      cfgs.push_back({132, 1, 3, 1, 8, 1, 32768, 0});
+      cfgs.push_back({132, 1, 2, 1, 8, 1, 32768, 0});
+      cfgs.push_back({132, 1, 4, 1, 8, 1, 16384, 0});
+      cfgs.push_back({132, 1, 8, 2, 8, 1, 8192, 0});
+      cfgs.push_back({132, 2, 8, 2, 8, 1, 8192, 0});
+      cfgs.push_back({132, 1, 6, 2, 8, 1, 32768, 1});
+      cfgs.push_back({132, 2, 3, 1, 8, 1, 32768, 1});
+      cfgs.push_back({132, 4, 3, 1, 8, 1, 16384, 1});
     } else {
-      for (int store : {0, 1, 2})
-        for (int grid : {148, 74, 32, 16}) {
+      for (int store : {0, 1})
+        for (int grid : {132, 66, 32, 16}) {
           cfgs.push_back({grid, 1, 6, 2, 4, 2, 32768, store, 2});
           cfgs.push_back({grid, 2, 6, 3, 4, 2, 16384, store, 2});
           cfgs.push_back({grid, 4, 6, 3, 4, 2, 8192, store, 2});
@@ -635,16 +604,13 @@ int main(int argc, char** argv)
       snprintf(cfg, sizeof cfg, "\"threads\":%d,\"rpc\":%d,", threads, rpc);
       report(name, cfg, t, bad);
     };
-    run("simt_u1", simt_copy_kernel<1, false>, 128, 1);
-    run("simt_u4", simt_copy_kernel<4, false>, 128, 1);
-    run("simt_u8", simt_copy_kernel<8, false>, 128, 1);
-    run("simt_u8", simt_copy_kernel<8, false>, 256, 1);
-    run("simt_u16", simt_copy_kernel<16, false>, 128, 1);
-    run("simt_u4", simt_copy_kernel<4, false>, 256, 1);
-    run("simt_u4", simt_copy_kernel<4, false>, 256, 2);
-    run("simt_v8_u4", simt_copy_kernel<4, true>, 128, 1);
-    run("simt_v8_u8", simt_copy_kernel<8, true>, 128, 1);
-    run("simt_v8_u4", simt_copy_kernel<4, true>, 256, 1);
+    run("simt_u1", simt_copy_kernel<1>, 128, 1);
+    run("simt_u4", simt_copy_kernel<4>, 128, 1);
+    run("simt_u8", simt_copy_kernel<8>, 128, 1);
+    run("simt_u8", simt_copy_kernel<8>, 256, 1);
+    run("simt_u16", simt_copy_kernel<16>, 128, 1);
+    run("simt_u4", simt_copy_kernel<4>, 256, 1);
+    run("simt_u4", simt_copy_kernel<4>, 256, 2);
   }
 
   // ---------------- the product library and the reference K1 ----------------
@@ -711,7 +677,7 @@ int main(int argc, char** argv)
     struct C {
       int grid, R, S, P, B, tile;
     };
-    const C cs[] = {{132, 1, 6, 1, 8, 16384}, {74, 2, 6, 2, 8, 16384}, {148, 1, 6, 2, 8, 32768}, {148, 2, 3, 1, 8, 16384}, {16, 2, 6, 2, 4, 16384}, {16, 4, 3, 1, 4, 16384}};
+    const C cs[] = {{132, 1, 6, 1, 8, 16384}, {66, 2, 6, 2, 8, 16384}, {132, 1, 6, 2, 8, 32768}, {132, 2, 3, 1, 8, 16384}, {16, 2, 6, 2, 4, 16384}, {16, 4, 3, 1, 4, 16384}};
     for (const C& c : cs) {
       Job j = job;
       j.tile = c.tile;
@@ -770,8 +736,8 @@ int main(int argc, char** argv)
       CK(cudaHostAlloc(reinterpret_cast<void**>(&h_word), 64, cudaHostAllocMapped));
       const V vs[] = {{"default_pool", 0, 0, 0, 0, 0, 0, 0},      {"default_ws", 1, 0, 0, 0, 0, 0, 0},       {"static", 0, 1, 0, 0, 0, 0, 0},
                       {"ws_done_flag", 1, 0, 0, 0, 0, 0, 0, 1},    {"ws_done_flag_host_word", 1, 0, 0, 0, 0, 0, 0, 3},
-                      {"r1_148", 1, 0, 2, 148, 0, 0, 0},           {"r1_132_p1", 1, 0, 2, 132, 6, 16384, 1},  {"r2_74_p1", 1, 0, 4, 74, 6, 16384, 1},
-                      {"r1_148_t32", 1, 0, 2, 148, 6, 32768, 2},   {"r2_148", 1, 0, 4, 148, 3, 16384, 1},     {"r4_74", 1, 0, 8, 74, 3, 16384, 1}};
+                      {"r1_132", 1, 0, 2, 132, 0, 0, 0},           {"r1_132_p1", 1, 0, 2, 132, 6, 16384, 1},  {"r2_66_p1", 1, 0, 4, 66, 6, 16384, 1},
+                      {"r1_132_t32", 1, 0, 2, 132, 6, 32768, 2},   {"r2_132", 1, 0, 4, 132, 3, 16384, 1},     {"r4_66", 1, 0, 8, 66, 3, 16384, 1}};
       for (const V& v : vs) {
         kvbm_paged_copy_opts o{};
         o.sync_workspace = v.ws ? ws : nullptr;

@@ -1,9 +1,8 @@
-"""Writes the SASS of the library's kernels under profiles/ (no GPU needed: cuobjdump reads the sm_100a cubin in the .so).
+"""Writes the SASS of the library's kernels under profiles/ (no GPU needed: cuobjdump reads the sm_90a cubin in the .so).
 
-    python benchmarks/dump_sass.py            -> profiles/r02_sass_<kernel>.txt + profiles/r02_sass_summary.md
-The summary counts the mnemonics that prove what the kernel is built from (B200_PROFILING.md "What proves a
-Blackwell-native kernel"): UBLKCP = cp.async.bulk (TMA 1-D bulk), SYNCS = mbarrier, UTMACMDFLUSH / fences,
-F2FP = fp8<->bf16 converts, LDG/STG widths for the SIMT kernels."""
+    python benchmarks/dump_sass.py            -> profiles/sass_<kernel>.txt + profiles/sass_summary.md
+The summary counts the mnemonics that show what the kernel is built from: UBLKCP = cp.async.bulk (TMA 1-D bulk),
+SYNCS = mbarrier, UTMACMDFLUSH / fences, F2FP = fp8<->bf16 converts, LDG/STG widths for the SIMT kernels."""
 import collections
 import os
 import re
@@ -20,6 +19,8 @@ KEYS = ["UBLKCP.S.G", "UBLKCP.G.S", "SYNCS.ARRIVE.TRANS64", "SYNCS.PHASECHK.TRAN
 
 def main():
     txt = subprocess.run(["cuobjdump", "-sass", SO], capture_output=True, text=True, check=True).stdout
+    out = os.path.join(ROOT, "profiles")
+    os.makedirs(out, exist_ok=True)
     parts = re.split(r"\n\s*Function : ", txt)
     rows = []
     for p in parts[1:]:
@@ -30,11 +31,11 @@ def main():
         body = p
         ops = collections.Counter(m.group(1) for m in re.finditer(r"^\s*/\*[0-9a-f]+\*/\s+(?:@!?U?P\d\s+)?([A-Z][A-Z0-9_.]+)", body, re.M))
         regs = re.search(r"REG:(\d+)", body)
-        with open(os.path.join(ROOT, "profiles", f"r02_sass_{tag}.txt"), "w") as f:
+        with open(os.path.join(out, f"sass_{tag}.txt"), "w") as f:
             f.write("Function : " + p)
         rows.append((tag, name, sum(ops.values()), {k: sum(v for o, v in ops.items() if o.startswith(k)) for k in KEYS}))
-    with open(os.path.join(ROOT, "profiles", "r02_sass_summary.md"), "w") as f:
-        f.write("# SASS of the sm_100a kernels in dynamo_b200/libkvbm_kernels.so (`python benchmarks/dump_sass.py`)\n\n")
+    with open(os.path.join(out, "sass_summary.md"), "w") as f:
+        f.write("# SASS of the sm_90a kernels in dynamo_b200/libkvbm_kernels.so (`python benchmarks/dump_sass.py`)\n\n")
         f.write("| kernel | instructions | " + " | ".join(KEYS) + " |\n|---|---:|" + "---:|" * len(KEYS) + "\n")
         for tag, name, total, c in rows:
             f.write(f"| `{tag}` | {total} | " + " | ".join(str(c[k]) for k in KEYS) + " |\n")

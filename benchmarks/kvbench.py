@@ -1,8 +1,8 @@
 """kvbench -- the reference's own KV transfer benchmark (lib/kvbm-kernels/examples/kvbench.rs), re-run on
 this box against BOTH libraries through the identical C ABI:
 
-    impl=ours       dynamo_b200/libkvbm_kernels.so            (sm_100a TMA ring)
-    impl=reference  oracle/_ref/libkvbm_kernels_ref.so         (tensor_kernels.cu compiled unmodified for sm_100)
+    impl=ours       dynamo_b200/libkvbm_kernels.so            (sm_90a TMA ring)
+    impl=reference  oracle/_ref/libkvbm_kernels_ref.so         (tensor_kernels.cu compiled unmodified for sm_90)
 
 Same model (Llama 3.1 70B bf16: 80 layers, 8 KV heads, head_dim 128, K+V), same patterns (fc_to_fc: one copy
 per block; lw_to_fc: one copy per (block, layer, outer)), same backends (vectorized = K1 with device pointer

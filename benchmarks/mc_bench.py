@@ -140,7 +140,7 @@ for mode, name in ((1, "multicast_st"), (2, "multicast_tma")):
 if a.sweep:
     res["sweep"] = []
     for mode in (1, 2):
-        for ctas in (16, 32, 48, 74, 111, 148):
+        for ctas in (16, 32, 48, 66, 111, 132):
             for warps, stages, tile in ((4, 6, 16384), (8, 6, 8192), (8, 8, 4096), (4, 12, 8192), (2, 6, 32768), (16, 6, 4096)):
                 fn = lambda: run_mc(mode, ctas, warps, stages, tile)  # noqa: E731
                 try:

@@ -4,7 +4,7 @@
 // communicator per visible GPU (ncclCommInitAll), vLLM layer-separate pools, Llama-3-8B geometry.
 // Prints one JSON line; compare with `bench.py --replicate [--nvls]`.  Not part of the product libraries.
 //
-//   nvcc -O2 -std=c++17 -gencode arch=compute_100a,code=sm_100a -o benchmarks/nccl_bcast_baseline \
+//   nvcc -O2 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o benchmarks/nccl_bcast_baseline \
 //        benchmarks/nccl_bcast_baseline.cu -lnccl
 #include <cuda_runtime_api.h>
 #include <nccl.h>

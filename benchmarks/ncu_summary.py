@@ -1,6 +1,6 @@
 """Summarises .ncu-rep captures (read here, no GPU needed) into a small JSON + markdown table for profiles/.
 
-    python benchmarks/ncu_summary.py gpurun_out/prof_ours.ncu-rep [more.ncu-rep ...] --out profiles/r01_ncu_summary
+    python benchmarks/ncu_summary.py prof_ours.ncu-rep [more.ncu-rep ...] --out profiles/ncu_summary
 """
 import argparse
 import csv

@@ -30,7 +30,7 @@ ap.add_argument("--pool", type=int, default=2048)
 ap.add_argument("--layer-us", type=float, default=40.0)
 ap.add_argument("--ctas", type=int, default=16)
 ap.add_argument("--iters", type=int, default=10)
-ap.add_argument("--standin-blocks", type=int, default=148 * 4)
+ap.add_argument("--standin-blocks", type=int, default=132 * 4)
 ap.add_argument("--fma", type=int, default=0, help="dependent FMA pairs per 16 B: >0 makes the stand-in compute-bound instead of HBM-saturating")
 ap.add_argument("--warps", type=int, default=0)
 ap.add_argument("--stages", type=int, default=0)
@@ -93,7 +93,7 @@ if a.standin == "gemm":
 
 def compute_layer(flag_ptr=0, value=0):
     if a.standin == "gemm":
-        # a real prefill-shaped layer: one cuBLAS bf16 GEMM (tcgen05 kernel, ~1 CTA/SM, large smem); the ready flag is
+        # a real prefill-shaped layer: one cuBLAS bf16 GEMM (wgmma kernel on sm_90, ~1 CTA/SM, large smem); the ready flag is
         # released by a stream mem-op right behind it
         torch.matmul(gA, gB, out=gC)
         if flag_ptr:

@@ -90,19 +90,19 @@ def main():
         # diagnostics: loads only / stores only (half the traffic; GB/s printed as if both directions moved)
         (4, 3, 1, 16384, 0, 0, 2), (4, 6, 1, 8192, 0, 0, 2), (8, 3, 1, 8192, 0, 0, 2), (2, 3, 1, 32768, 0, 0, 2),
         (4, 3, 1, 16384, 0, 0, 3), (4, 3, 2, 16384, 0, 0, 3), (4, 6, 3, 8192, 0, 0, 3), (4, 6, 5, 8192, 0, 0, 3), (8, 3, 2, 8192, 0, 0, 3),
-        (4, 3, 1, 16384, 74, 0, 0), (4, 3, 1, 16384, 32, 0, 0), (4, 3, 1, 16384, 16, 0, 0), (8, 3, 1, 8192, 16, 0, 1),
+        (4, 3, 1, 16384, 66, 0, 0), (4, 3, 1, 16384, 32, 0, 0), (4, 3, 1, 16384, 16, 0, 0), (8, 3, 1, 8192, 16, 0, 1),
     ]
     if a.fine:
         cfgs = []
         for shape in [(4, 3, 1, 16384), (4, 6, 3, 8192), (2, 3, 1, 32768), (8, 3, 1, 8192), (2, 6, 3, 16384), (4, 4, 2, 8192)]:
-            for ctas in (64, 74, 96, 111, 128, 148):
+            for ctas in (64, 66, 96, 111, 128, 132):
                 cfgs.append((*shape, ctas, 0, 0))
         for hint in (1, 2, 3):
-            cfgs += [(4, 3, 1, 16384, 74, hint, 0), (4, 3, 1, 16384, 148, hint, 0), (2, 3, 1, 32768, 74, hint, 0)]
+            cfgs += [(4, 3, 1, 16384, 66, hint, 0), (4, 3, 1, 16384, 132, hint, 0), (2, 3, 1, 32768, 66, hint, 0)]
     if a.peer:   # NVLink-bound: how few SMs saturate the link, and how many stores must be in flight
         cfgs = [(4, 3, 1, 16384, 0, 0, 0), (4, 6, 3, 8192, 0, 0, 0), (4, 6, 5, 8192, 0, 0, 0), (2, 6, 4, 16384, 0, 0, 0),
                 (4, 3, 1, 16384, 0, 0, 1), (8, 3, 1, 8192, 0, 0, 1),
-                (4, 3, 1, 16384, 74, 0, 0), (4, 3, 1, 16384, 32, 0, 0), (4, 3, 1, 16384, 16, 0, 0), (4, 3, 1, 16384, 8, 0, 0),
+                (4, 3, 1, 16384, 66, 0, 0), (4, 3, 1, 16384, 32, 0, 0), (4, 3, 1, 16384, 16, 0, 0), (4, 3, 1, 16384, 8, 0, 0),
                 (4, 6, 4, 8192, 32, 0, 0), (4, 6, 4, 8192, 16, 0, 0), (4, 6, 4, 8192, 8, 0, 0), (2, 6, 4, 16384, 16, 0, 0),
                 (2, 6, 4, 16384, 8, 0, 0), (4, 12, 10, 4096, 16, 0, 0), (8, 3, 1, 8192, 16, 0, 1), (8, 3, 1, 8192, 32, 0, 1),
                 (4, 3, 2, 16384, 16, 0, 0), (1, 6, 4, 32768, 16, 0, 0), (1, 6, 4, 32768, 32, 0, 0)]

@@ -1,20 +1,20 @@
-"""Decode-visible TTFT under the reference's own hand-off model, from the committed bench lines.
+"""Decode-visible TTFT under the reference's own hand-off model, from bench.py result lines.
 
 The mocker models the prefill->decode hand-off as  delay_ms = tokens * kv_bytes_per_token / (bw * 1e9) * 1e3
-(/root/reference/lib/mocker/src/common/utils.rs:14-40; default bw 64 GB/s "inter-node InfiniBand",
+(lib/mocker/src/common/utils.rs:14-40; default bw 64 GB/s "inter-node InfiniBand",
 components/src/dynamo/mocker/utils/kv_cache.py:30-33) and TTFT = T_prefill + T_transfer + T_first_decode.
 Only T_transfer differs between data planes, so the TTFT drop of a decode worker is the difference of transfer
 times.  This script tabulates it for the measured fan-outs.
 
-    python benchmarks/ttft_model.py > profiles/r01_ttft.md
+    python benchmarks/ttft_model.py bench_n1.json bench_n2.json ... > ttft.md
 """
-import glob
 import json
 import os
+import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 rows = []
-for f in sorted(glob.glob(os.path.join(ROOT, "profiles", "r01_bench_n*.json"))):
+for f in sys.argv[1:]:
     try:
         d = json.loads(open(f).read().strip().splitlines()[-1])
     except Exception:
@@ -36,7 +36,7 @@ for (n, rep), (name, d) in best.items():
         cpu1 = d["cpu_baseline"].get("single_thread_value")
 print("# Decode-visible TTFT change from the KV hand-off alone (Llama-3-8B bf16, 4 k-token prompt, 512 MiB of KV per decode worker)\n")
 print("`T_transfer = tokens * kv_bytes_per_token / BW` (lib/mocker/src/common/utils.rs:14-40); measured columns are the p50 of the")
-print("end-to-end step (`e2e.p50_ms`, host API, host block tables) of the bench lines under profiles/.\n")
+print("end-to-end step (`e2e.p50_ms`, host API, host block tables) of the bench lines given.\n")
 print("| fan-out | payload | ours: all destinations complete (ms, p50) | mocker default 64 GB/s, per destination (ms) | NVLink figure of the docs 450 GB/s (ms) | "
       "reference CPU path, all host threads, destinations one after another (ms) | TTFT drop of the LAST decode worker vs CPU path (ms) | file |")
 print("|---|---|---:|---:|---:|---:|---:|---|")

@@ -11,16 +11,18 @@ and ONLY `T_transfer` differs between the data planes compared:
 
   mocker64   tokens * kv_bytes_per_token / 64 GB/s     the mocker's default `--kv-transfer-bandwidth`
              (components/src/dynamo/mocker/utils/kv_cache.py:30-33), a pure delay
-  cpu        the reference's CPU memcpy path at the rate measured on the B200 host (bench.py cpu_baseline),
+  cpu        the reference's CPU memcpy path at the rate of a bench.py cpu_baseline (--cpu-bench),
              one transfer at a time per prefill host
-  ours       latency + bytes / BW fitted to the measured 1 -> 1 NVLink pushes (profiles/r01_fanout_n2.jsonl),
+  ours       latency + bytes / BW fitted to measured 1 -> 1 NVLink pushes (--sweep, benchmarks/fanout_sweep.py output),
              one transfer at a time per prefill GPU (its NVLink egress is the shared resource)
+  ours_pull  with --pull-bench (a bench.py --gpus 2 line): the same latency, the pull direction's measured rate
+Without those files the model falls back to the H100 SXM data sheet's NVLink rate and an assumed CPU rate, and says so.
 
 The decode worker is chosen by the KV router restated in libkvbm_router.so (`RadixTree.find_matches`, XXH3 block hashes):
 best prefix overlap wins, ties go to the least loaded worker -- and only the NON-HIT suffix of the block table is moved
 (`prefix_hit_block_table`), so the prefix-hit rate is an outcome of the request mix, not a knob.
 
-    python benchmarks/ttft_sim.py --out profiles/r01_ttft_sim.json > profiles/r01_ttft_sim.md
+    python benchmarks/ttft_sim.py [--sweep fanout_n2.jsonl] [--cpu-bench bench_n1.json] [--pull-bench bench_n2.json] --out sim.json
 """
 import argparse
 import heapq
@@ -48,48 +50,46 @@ ap.add_argument("--prefill-tok-per-s", type=float, default=60000.0)
 ap.add_argument("--first-decode-ms", type=float, default=8.0)
 ap.add_argument("--seed", type=int, default=0)
 ap.add_argument("--out", default="")
+ap.add_argument("--sweep", default="", help="fanout_sweep.py jsonl of 1 -> 1 pushes to fit `ours` to")
+ap.add_argument("--cpu-bench", default="", help="bench.py result line with a cpu_baseline")
+ap.add_argument("--pull-bench", default="", help="bench.py --gpus 2 result line (pull direction)")
 a = ap.parse_args()
 
 
 def fit_ours():
     """latency_ms + bytes / BW from the measured 1 -> 1 pushes (least squares over the sweep's sizes)."""
     pts = []
-    path = os.path.join(ROOT, "profiles", "r01_fanout_n2.jsonl")
-    if os.path.exists(path):
-        for line in open(path):
+    if a.sweep:
+        for line in open(a.sweep):
             d = json.loads(line)
             if d["mode"] == "distinct" and d["max_ctas"] == 0 and d["cast"] == "none":
                 pts.append((d["blocks_moved"] * 2 * 1024 * 1024, d["ms"]))
     if len(pts) < 2:
-        return 0.02, 700.0, "fallback (no sweep file)"
+        return 0.02, 450.0, "fallback: assumed 20 us launch latency + H100 SXM data-sheet NVLink 4 rate (450 GB/s per direction), not measured"
     x = np.array([p[0] for p in pts], dtype=np.float64)
     y = np.array([p[1] for p in pts], dtype=np.float64)
     slope, icpt = np.polyfit(x, y, 1)
     return max(0.0, float(icpt)), 1e-6 / slope, f"fit over {len(pts)} measured 1->1 pushes"
 
 
-def _bench_line(name):
-    for line in open(os.path.join(ROOT, "profiles", name)):
+def _bench_line(path):
+    for line in open(path):
         if line.startswith("{"):
             return json.loads(line)
-    raise ValueError(name)
+    raise ValueError(path)
 
 
 def cpu_rate():
-    for name in ("r02_bench_n1.json", "r01_bench_n1_b.json"):
-        try:
-            return float(_bench_line(name)["cpu_baseline"]["value"]), f"profiles/{name} cpu_baseline"
-        except Exception:
-            continue
-    return 47.0, "fallback"
+    if a.cpu_bench:
+        return float(_bench_line(a.cpu_bench)["cpu_baseline"]["value"]), f"{a.cpu_bench} cpu_baseline"
+    return 47.0, "fallback: assumed 47 GB/s, not measured"
 
 
 def pull_rate():
-    """round 2: the decode GPU pulls (reads the prefill pool over NVLink) -- measured 1 -> 1 rate of the bench line"""
-    try:
-        return float(_bench_line("r02_bench_n2_pull.json")["value"]), "profiles/r02_bench_n2_pull.json"
-    except Exception:
-        return None, "no pull bench line"
+    """the decode GPU pulls (reads the prefill pool over NVLink) -- measured 1 -> 1 rate of the bench line"""
+    if a.pull_bench:
+        return float(_bench_line(a.pull_bench)["value"]), a.pull_bench
+    return None, "no pull bench line"
 
 
 LAT_MS, BW_GBS, ours_src = fit_ours()

@@ -1,4 +1,4 @@
-"""dynamo_b200 -- Blackwell-native (sm_100a) KV-block transfer path behind Dynamo's KVBM surface.
+"""dynamo_b200 -- Hopper-native (sm_90a) KV-block transfer path behind Dynamo's KVBM surface.
 
 Only what the prefill->decode KV hand-off needs:
   csrc/kernels   CUDA kernels + the C ABI of libkvbm_kernels.so (include/kvbm_kernels.h)

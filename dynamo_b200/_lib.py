@@ -22,7 +22,7 @@ def load(path: str) -> C.CDLL:
         if not os.path.exists(path):
             raise NativeLibraryMissing(
                 f"{path} is not built. Run `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a). dynamo_b200 has no CPU fallback for the KV transfer path.")
+                "(nvcc, sm_90a). dynamo_b200 has no CPU fallback for the KV transfer path.")
         lib = C.CDLL(path, mode=C.RTLD_GLOBAL)
         _cache[path] = lib
     return lib

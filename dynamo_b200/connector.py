@@ -1,4 +1,4 @@
-"""Worker side of Dynamo's KVBM connector, over the B200 transfer path (SURVEY.md §8 f1).
+"""Worker side of Dynamo's KVBM connector, over the H100 transfer path (SURVEY.md §8 f1).
 
 Mirrors the surface the vLLM / TRT-LLM model runner calls through pyo3
 (`PyKvConnectorWorker`, /root/reference/lib/bindings/kvbm/src/block_manager/vllm/connector/worker.rs:474-560;
@@ -404,7 +404,7 @@ class KvConnectorWorker:
                 enq = (cr.request_id, cr.uuid) in self._enqueued
                 if not enq and self._ready_flags is not None and req.from_pool == DEVICE and self.bound and \
                         any(op.uuid == cr.uuid and op.request_id == cr.request_id for op in self.offloading_operations):
-                    # B200 path: an offload announced for the iteration that is running can be launched NOW -- the copy is
+                    # this path: an offload announced for the iteration that is running can be launched NOW -- the copy is
                     # gated layer by layer on this iteration's ready flags, so it streams behind the forward pass instead
                     # of starting after the last layer.  (It still counts for the slot only once save_kv_layer enqueues it.)
                     self._enqueued[(cr.request_id, cr.uuid)] = self._epoch

@@ -143,7 +143,7 @@ CUmulticastObjectProp mc_prop(int num_devices, size_t size, bool shareable)
   return p;
 }
 
-// bound size: a multiple of the multicast granularity -- the RECOMMENDED one (512 MiB on B200) for pools that are
+// bound size: a multiple of the multicast granularity -- the RECOMMENDED one (queried from the driver) for pools that are
 // at least that large, the MINIMUM (2 MiB) for small ones
 int round_size(int num_devices, size_t bytes, bool shareable, size_t* rounded, size_t* va_align)
 {

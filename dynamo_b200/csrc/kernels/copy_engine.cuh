@@ -10,9 +10,9 @@
 //   * the CONSUMER warp waits for `full`, issues the bulk stores (or converts fp8<->bf16 / stores SIMT / multimem),
 //     hands the slot back through the `empty` mbarrier once the store has read it, and publishes per-layer and
 //     whole-transfer completion.  It never computes an address.
-// A CTA holds R such rings.  Why dynamic scheduling: SMs of a B200 do not move bytes at the same rate (two dies, L2
-// slice distance) -- with a static split the slowest ring finished 80-100 us after the fastest on a 170 us copy
-// (benchmarks/copylab.cu, profiles/r02_copylab_n1.jsonl); with tickets all rings finish within ~5 us.
+// A CTA holds R such rings.  Why dynamic scheduling: SMs do not move bytes at the same rate (distance to the L2
+// partition that holds an address, contention with other work on the GPU), so a static split waits for the slowest
+// ring; tickets let fast rings take over the tail (benchmarks/copylab.cu compares both, `sched` 0 vs 1/2).
 #pragma once
 #include "ptx.cuh"
 
@@ -263,8 +263,8 @@ __device__ __forceinline__ void warp_cast_simt(uint8_t* dst, const uint8_t* src,
 // ------------------------------------------------------------------------------------------
 // FAST = the plain hot path, known at compile time: one destination, TMA load + TMA store, no cache hints, no gating and
 // no per-layer flags.  A ring is ONE instruction stream per direction, so every instruction of the per-item chain costs
-// its full latency (~10 ns); folding the run-time generality away is worth 10 % on the HBM-bound copy
-// (profiles/r02_copylab_libsweep.jsonl vs r02_copylab_engine.jsonl).
+// its full latency; folding the run-time generality away shortens the chain that bounds the HBM-bound copy
+// (benchmarks/copylab --only libsweep against --only engine).
 template <int CAST, bool FAST, class Gen>
 __device__ __forceinline__ void ring_producer(const Gen& gen, uint32_t total, uint32_t my_ring, uint32_t nrings,
                                               const RingSmem& sm, int ndst_rt, const RingParams& rp, const StreamSync& ss)

@@ -1,4 +1,4 @@
-// libkvbm_kernels.so -- sm_100a KV-block transfer kernels behind the reference C ABI
+// libkvbm_kernels.so -- sm_90a KV-block transfer kernels behind the reference C ABI
 // (see include/kvbm_kernels.h for the contract and the reference lines each entry replaces).
 #include <cuda_runtime_api.h>
 
@@ -66,12 +66,11 @@ struct RingCfg {
   uint32_t out_tile;  // cast only
 };
 
-// Defaults measured on B200 (benchmarks/copylab.cu -> profiles/r02_copylab_*.jsonl).  One SM moves at most ~50 GB/s per
-// direction through the TMA however many rings it runs, so the HBM-bound copy wants (nearly) every SM: 132-148 CTAs copy
-// 512 MiB HBM->HBM in 0.170 ms (cudaMemcpy 0.173, reference K1 0.177-0.178); 74 CTAs sit at the per-SM limit and are
-// sensitive to every instruction of the per-item chain.  A whole 32 KiB region per bulk op halves that chain's share;
-// smaller regions get more rings per CTA instead (~192 KiB of slots per CTA either way).  16 CTAs saturate an NVLink
-// peer: callers that overlap the transfer with compute pass max_ctas.
+// Defaults.  One SM moves a bounded number of bytes per second through the TMA however many rings it runs, so the
+// HBM-bound copy wants every SM: one CTA per SM (132 on an H100 SXM).  A whole 32 KiB region per bulk op keeps the
+// per-item instruction chain short; smaller regions get more rings per CTA instead (~192 KiB of slots per CTA either
+// way, within the 227 KiB a block may opt into on sm_90).  Callers that overlap the transfer with compute and need
+// only NVLink peer bandwidth pass max_ctas.  benchmarks/copylab.cu sweeps these choices.
 constexpr int kDefaultStages = 6;
 constexpr uint32_t kDefaultTile = 32768;
 constexpr int kDefaultBatch = 8;
@@ -191,7 +190,7 @@ static void sched_release(int dev, int slot, cudaStream_t stream)
 // ------------------------------------------------------------------------------------------------
 // K1: pointer-pair copy (legacy ABI).  Hardware-scheduled SIMT: one CTA per (pair, 32 KiB chunk) -- or one warp per
 // pair when pairs are small -- 4 independent 16 B loads in flight per thread (8 and 4 are equal on HBM, 4 is a little
-// better when the source is pinned host memory: profiles/r02_k1_unroll_sweep.txt), the alignment ladder of the reference.
+// better when the source is pinned host memory), the alignment ladder of the reference.
 // The CTA scheduler is the dynamic load balancer here, so the ABI needs no workspace and the library no state.
 // ------------------------------------------------------------------------------------------------
 constexpr uint32_t kPairChunk = 32768;
@@ -1176,5 +1175,5 @@ kvbm_kernels_launch_count(void)
 extern "C" const char*
 kvbm_kernels_build_info(void)
 {
-  return "libkvbm_kernels sm_100a tma=cp.async.bulk cast=e4m3<->bf16";
+  return "libkvbm_kernels sm_90a tma=cp.async.bulk cast=e4m3<->bf16";
 }

@@ -4,7 +4,7 @@
 // `vectorised_copy(void** src, void** dst, size_t size, int num_pairs)`, launching it with
 // grid = min(1024, num_pairs), block = 256, 0 bytes of dynamic shared memory
 // (/root/reference/lib/llm/src/block_manager/block/transfer/cuda.rs:85-153, :521-548); the module can be
-// replaced at run time through DYN_FATBIN_PATH (cuda.rs:588-611).  This file builds that module for sm_100a.
+// replaced at run time through DYN_FATBIN_PATH (cuda.rs:588-611).  This file builds that module for sm_90a.
 // The fixed launch configuration gives no workspace for a tile scheduler, so the kernel is the SIMT engine of the
 // library's K1 (8 independent 16-byte loads in flight per thread, the reference's alignment ladder), pairs strided
 // over the grid; pairs larger than 32 KiB are additionally split over the warps' CTAs chunk by chunk.

@@ -19,7 +19,7 @@ Mirrors, relative to /root/reference/lib/bindings/kvbm/src/block_manager/vllm/:
   connector.rs:21-110                  SchedulerOutput / NewRequestData / CachedRequestData
 The transfer-engine half (slot.rs:1442-1820: allocate host blocks, send a `BlockTransferRequest` to the workers, register
 the blocks once the copy is done) is the small `HostPool` + `send` callback below; the bytes themselves move through
-`KvConnectorWorker.handle_block_transfer` -> `TransferManager` -> the B200 kernels.  Dynamo's block manager (pools with
+`KvConnectorWorker.handle_block_transfer` -> `TransferManager` -> the sm_90a kernels.  Dynamo's block manager (pools with
 reuse policies, disk tier, metrics, ZMQ) stays Dynamo's: this class is what makes the worker's protocol drivable end to end.
 """
 from __future__ import annotations

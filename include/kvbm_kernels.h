@@ -1,5 +1,5 @@
 /*
- * kvbm_kernels.h -- C ABI of libkvbm_kernels.so, the B200-native (sm_100a) replacement for
+ * kvbm_kernels.h -- C ABI of libkvbm_kernels.so, the H100-native (sm_90a) replacement for
  * Dynamo's lib/kvbm-kernels.
  *
  * Part 1 are the six symbols the reference exports and its Rust FFI binds
@@ -226,7 +226,7 @@ cudaError_t kvbm_kernels_stream_wait_event(cudaStream_t stream, void* event);
 
 /* Number of kernel launches issued by this library since load (bench accounting). */
 uint64_t kvbm_kernels_launch_count(void);
-/* "sm_100a" build tag + whether the TMA path is compiled in. */
+/* "sm_90a" build tag + whether the TMA path is compiled in. */
 const char* kvbm_kernels_build_info(void);
 
 #ifdef __cplusplus

@@ -4,10 +4,12 @@ Mirrors the reference's kernel tests:
   lib/kvbm-kernels/tests/memcpy_batch.rs       (no-ops, H2D+D2H roundtrips over all 3 modes, KAT patterns)
   lib/kvbm-kernels/tests/kernel_roundtrip.rs   (permute roundtrip x dtype x layout, poison fill, empty batch)
   lib/kvbm-kernels/src/tensor_kernels.rs:286-  (universal_roundtrip with +0.25 encoded values)
-and compares every result bit-for-bit with the CPU oracle, and with the reference's own kernels
-(oracle/_ref/libkvbm_kernels_ref.so, compiled unmodified) when that library is present.
+and compares every result bit-for-bit with the CPU oracle, and with the reference's own kernels: with the
+outputs they produced on an H100, stored under tests/golden (make_ref_outputs.py), and live when
+oracle/_ref/libkvbm_kernels_ref.so (compiled unmodified) is present.
 """
 import ctypes as C
+import hashlib
 import os
 
 import numpy as np
@@ -23,6 +25,7 @@ pytestmark = pytest.mark.gpu
 
 REF_SO = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref",
                       "libkvbm_kernels_ref.so")
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
 def ref_lib():
@@ -136,23 +139,35 @@ def test_vectorized_copy_one_huge_pair_is_split_over_the_chip():
     assert torch.equal(src, dst)
 
 
-def test_vectorized_copy_matches_reference_kernel_bit_for_bit():
-    R = ref_lib()
-    if R is None:
-        pytest.skip("oracle/_ref not built")
-    size, pairs = 32768, 512   # one (block,layer,outer) region of Llama-3-8B bf16 per pair
-    pool = torch.randint(0, 256, (pairs * 2, size), dtype=torch.uint8, device="cuda")
-    perm = torch.randperm(pairs * 2)[:pairs]
-    ours, theirs = dev_u8(pairs * size).view(pairs, size), dev_u8(pairs * size).view(pairs, size)
-    dperm = torch.randperm(pairs)
-    st = dev_ptr_table([pool[int(i)].data_ptr() for i in perm])
-    d1 = dev_ptr_table([ours[int(i)].data_ptr() for i in dperm])
-    d2 = dev_ptr_table([theirs[int(i)].data_ptr() for i in dperm])
-    assert K.vectorized_copy(st.data_ptr(), d1.data_ptr(), size, pairs, stream_ptr()) == 0
-    assert R.kvbm_kernels_launch_vectorized_copy(st.data_ptr(), d2.data_ptr(), size, pairs, stream_ptr()) == 0
+def k1_reference_case(launch):
+    """The seeded K1 case whose reference output is stored under tests/golden: 512 pairs of 32 KiB (one
+    (block,layer,outer) region of Llama-3-8B bf16 each) gathered from a 1024-region pool in random order and
+    scattered in another.  Returns the destination rows as a [pairs, size] uint8 array."""
+    size, pairs = 32768, 512
+    rng = np.random.default_rng(139)
+    pool = rng.integers(0, 256, (pairs * 2, size), dtype=np.uint8)
+    perm, dperm = rng.permutation(pairs * 2)[:pairs], rng.permutation(pairs)
+    d_pool = torch.from_numpy(pool).cuda()
+    out = dev_u8(pairs * size).view(pairs, size)
+    st = dev_ptr_table([d_pool[int(i)].data_ptr() for i in perm])
+    dt = dev_ptr_table([out[int(i)].data_ptr() for i in dperm])
+    assert launch(st.data_ptr(), dt.data_ptr(), size, pairs, stream_ptr()) == 0
     torch.cuda.synchronize()
-    assert torch.equal(ours, theirs)
-    assert torch.equal(ours[dperm], pool[perm])
+    got = out.cpu().numpy()
+    assert np.array_equal(got[dperm], pool[perm])
+    return got
+
+
+def row_sha256(rows):
+    return np.stack([np.frombuffer(hashlib.sha256(r.tobytes()).digest(), dtype=np.uint8) for r in rows])
+
+
+def test_vectorized_copy_matches_reference_kernel_bit_for_bit():
+    ours = k1_reference_case(K.vectorized_copy)
+    assert np.array_equal(row_sha256(ours), np.load(os.path.join(GOLDEN, "ref_k1_rows_sha256.npy")))
+    R = ref_lib()
+    if R is not None:
+        assert np.array_equal(ours, k1_reference_case(R.kvbm_kernels_launch_vectorized_copy))
 
 
 # ---------------------------------------------------------------- K2/K3 permute
@@ -202,30 +217,35 @@ def test_permute_llama70b_tp_reshard_shape(layout):
     _permute_case(1, layout, (8, 4, 2, 16, 128), 3)
 
 
-@pytest.mark.parametrize("layout", [kats.NHD, kats.HND])
-def test_permute_position_encoded_kat_and_reference_kernel(layout):
+def permute_position_encoded_chunks(L, layout):
+    """block_from_universal of the position-encoded F32 KAT through library L; returns the nl*no chunks as float32."""
     d = kats.PERMUTE_DIMS
     dims = (d["nh"], d["nl"], d["no"], d["nt"], d["hd"])
     uni = kats.position_encoded_universal(**d)
-    want = kats.make_blocks(uni, layout)
-    sp = stream_ptr()
     du = torch.from_numpy(uni.reshape(-1).view(np.uint8).copy()).cuda()
     ut = dev_ptr_table([du.data_ptr()])
-    outs = {}
-    for name, L in (("ours", K.lib()), ("ref", ref_lib())):
-        if L is None:
-            continue
-        chunks = [dev_u8(w.nbytes, fill=0xDE) for w in want]
-        bt = dev_ptr_table([t.data_ptr() for t in chunks])
-        rc = L.kvbm_kernels_launch_block_from_universal(ut.data_ptr(), bt.data_ptr(), 1, *dims, 2, layout, sp)
-        assert rc == 0
-        torch.cuda.synchronize()
-        outs[name] = [c.cpu().numpy().view(np.float32) for c in chunks]
-    for got, w in zip(outs["ours"], want):
-        assert np.array_equal(got, w)
-    if "ref" in outs:
-        for a, b in zip(outs["ours"], outs["ref"]):
-            assert np.array_equal(a, b)
+    chunks = [dev_u8(w.nbytes, fill=0xDE) for w in kats.make_blocks(uni, layout)]
+    bt = dev_ptr_table([t.data_ptr() for t in chunks])
+    assert L.kvbm_kernels_launch_block_from_universal(ut.data_ptr(), bt.data_ptr(), 1, *dims, 2, layout, stream_ptr()) == 0
+    torch.cuda.synchronize()
+    return np.stack([c.cpu().numpy().view(np.float32) for c in chunks])
+
+
+def permute_golden_path(layout):
+    return os.path.join(GOLDEN, "ref_block_from_universal_%s.npy" % ("nhd" if layout == kats.NHD else "hnd"))
+
+
+@pytest.mark.parametrize("layout", [kats.NHD, kats.HND])
+def test_permute_position_encoded_kat_and_reference_kernel(layout):
+    d = kats.PERMUTE_DIMS
+    want = kats.make_blocks(kats.position_encoded_universal(**d), layout)
+    ours = permute_position_encoded_chunks(K.lib(), layout)
+    for got, w in zip(ours, want):
+        assert np.array_equal(got, w.reshape(-1))
+    assert np.array_equal(ours, np.load(permute_golden_path(layout)))
+    R = ref_lib()
+    if R is not None:
+        assert np.array_equal(ours, permute_position_encoded_chunks(R, layout))
 
 
 def test_universal_roundtrip_quarter_offsets():
