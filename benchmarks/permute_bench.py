@@ -1,7 +1,8 @@
 """Layout-transforming hand-off, timed: kvbm_kernels_paged_permute (layouts + block tables, no pointer tables) against the flow the
 reference's K2 needs (host builds nb*nl*no chunk pointers + nb universal pointers, uploads them, launches
 kvbm_kernels_launch_universal_from_block -- tensor_kernels.rs:177-215) and against the plain paged copy of the same bytes.
-Llama-3-70B KV geometry by default.  Prints one JSON line; roofline = bytes read + written / measured HBM copy peak."""
+Llama-3-70B KV geometry by default.  Prints one JSON line; roofline = bytes read + written / the HBM peak bench.py uses
+(the measured copy peak, else the H100 data sheet's)."""
 import argparse
 import json
 import os
@@ -13,6 +14,7 @@ import numpy as np
 import torch
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
+import bench  # noqa: E402
 from dynamo_b200 import kernels as K  # noqa: E402
 
 p = argparse.ArgumentParser()
@@ -37,11 +39,7 @@ if a.peer >= 0:
     import ctypes
     rt = ctypes.CDLL("libcudart.so")
     rt.cudaDeviceEnablePeerAccess(a.peer, 0)
-peak = 6462.4
-try:
-    peak = float(json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "MEASURED_PEAKS.json")))["hbm_gbs"])
-except Exception:
-    pass
+peak, peak_src = bench.peaks()
 
 # engine pool: layer-separate, block-is-second-dim (vLLM), NHD inside a region; universal pool: fully contiguous
 op = [torch.randint(0, 256, (no * nb * region,), dtype=torch.uint8, device=sdev) for _ in range(nl)]
@@ -131,7 +129,8 @@ def wall(fn, iters=a.iters):
 
 
 res = {"geometry": {"blocks": n, "layers": nl, "outer": no, "page": nt, "heads": nh, "head_dim": hd, "elem": elem, "MiB_moved": moved / 2**20},
-       "peer": a.peer, "peer_side": a.peer_side if a.peer >= 0 else None, "paged_equals_legacy": same}
+       "peer": a.peer, "peer_side": a.peer_side if a.peer >= 0 else None, "paged_equals_legacy": same,
+       "hbm_peak_GBps": peak, "hbm_peak_source": peak_src}
 for name, fn in (("paged_permute_to_universal", paged), ("paged_permute_from_universal", paged_back), ("legacy_k2_kernel_only", legacy_kernel_only),
                  ("plain_paged_copy", plain_copy)):
     ms = timed(fn)

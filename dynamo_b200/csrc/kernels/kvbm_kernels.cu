@@ -9,7 +9,6 @@
 #include <atomic>
 #include <mutex>
 #include <cstdio>
-#include <cstdlib>
 #include <vector>
 
 namespace kvbm {
@@ -195,9 +194,10 @@ static void sched_release(int dev, int slot, cudaStream_t stream)
 // ------------------------------------------------------------------------------------------------
 constexpr uint32_t kPairChunk = 32768;
 constexpr uint32_t kPairSmall = 4096;
+constexpr int kPairThreads = 256;
+constexpr int kPairLoads = 4;
 
-template <int U>
-__global__ void __launch_bounds__(256)
+__global__ void __launch_bounds__(kPairThreads)
 kvbm_pair_copy_kernel(void* const* __restrict__ src_ptrs, void* const* __restrict__ dst_ptrs, size_t copy_size,
                       uint32_t chunks_per_pair, uint64_t num_pairs)
 {
@@ -205,7 +205,7 @@ kvbm_pair_copy_kernel(void* const* __restrict__ src_ptrs, void* const* __restric
   if (copy_size <= kPairSmall) {  // warp per pair
     const uint64_t pair = bid * (blockDim.x >> 5) + (threadIdx.x >> 5);
     if (pair >= num_pairs) return;
-    group_copy_simt<U>(static_cast<uint8_t*>(dst_ptrs[pair]), static_cast<const uint8_t*>(src_ptrs[pair]), copy_size, threadIdx.x & 31, 32);
+    group_copy_simt<kPairLoads>(static_cast<uint8_t*>(dst_ptrs[pair]), static_cast<const uint8_t*>(src_ptrs[pair]), copy_size, threadIdx.x & 31, 32);
     return;
   }
   const uint64_t pair = bid / chunks_per_pair;
@@ -214,8 +214,8 @@ kvbm_pair_copy_kernel(void* const* __restrict__ src_ptrs, void* const* __restric
   const size_t off = static_cast<size_t>(chunk) * kPairChunk;
   const size_t left = copy_size - off;
   // chunk boundaries are multiples of 32 KiB, so the alignment class of (src, dst) is the same for every chunk
-  group_copy_simt<U>(static_cast<uint8_t*>(dst_ptrs[pair]) + off, static_cast<const uint8_t*>(src_ptrs[pair]) + off,
-                     left < kPairChunk ? left : kPairChunk, threadIdx.x, blockDim.x);
+  group_copy_simt<kPairLoads>(static_cast<uint8_t*>(dst_ptrs[pair]) + off, static_cast<const uint8_t*>(src_ptrs[pair]) + off,
+                              left < kPairChunk ? left : kPairChunk, threadIdx.x, blockDim.x);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -354,9 +354,9 @@ kvbm_paged_copy_kernel(const __grid_constant__ PagedGen gen, const __grid_consta
 }
 
 // ------------------------------------------------------------------------------------------------
-// K2 / K3: block stacks <-> universal.  Index peel identical in meaning to the reference
-// (tensor_kernels.cu:150-228) but done per 16-byte vector when a head row allows it, and with
-// 32-bit arithmetic; one thread moves VEC bytes.
+// K2 / K3: block stacks <-> universal, generic path for rows the head-row walk below does not take (not a whole number of
+// 16-byte vectors, or past its bounds).  Index peel identical in meaning to the reference (tensor_kernels.cu:150-228) but
+// done per VEC-byte vector when a head row allows it, and with 32-bit arithmetic; one thread moves VEC bytes.
 // ------------------------------------------------------------------------------------------------
 template <int VEC, bool TO_UNIVERSAL>
 __global__ void __launch_bounds__(256)
@@ -401,76 +401,18 @@ kvbm_permute_kernel(void* const* universal_ptrs, void* const* block_ptrs, uint64
   }
 }
 
-// Fast path of K2 / K3 for head rows that are a power-of-two number of 16-byte vectors (hd*elem = 64 B ... 4 KiB: every
-// real KV geometry).  One CTA per (block, layer, outer) chunk -- the hardware CTA scheduler balances the SMs -- and one
-// warp per head: for a fixed head the universal side is ONE contiguous run of nt rows and the chunk side is nt rows at a
-// constant stride (NHD) or contiguous as well (HND), so a lane's addresses advance by shifts and adds: no division per
-// vector (the reference peels 5 div/mod per ELEMENT, tensor_kernels.cu:150-187) and 8 independent 16 B loads per lane
-// are in flight before the first store.
-template <bool TO_UNIVERSAL>
-__global__ void __launch_bounds__(256)
-kvbm_permute_rows_kernel(void* const* __restrict__ universal_ptrs, void* const* __restrict__ block_ptrs, uint32_t nh, uint32_t nl,
-                         uint32_t no, uint32_t nt, uint32_t log2_v /* 16 B vectors per head row */, uint32_t elem, int layout)
-{
-  const uint32_t chunk_id = blockIdx.x;  // (b * nl + nl_i) * no + no_i
-  const uint32_t b = chunk_id / (nl * no);
-  const uint32_t rem = chunk_id - b * (nl * no);
-  const uint32_t nl_i = rem / no, no_i = rem - nl_i * no;
-  uint8_t* chunk = static_cast<uint8_t*>(block_ptrs[chunk_id]);
-  uint8_t* uni = static_cast<uint8_t*>(universal_ptrs[b]);
-  const uint32_t V = 1u << log2_v;
-  const uint32_t row = V << 4;            // bytes per head row
-  const uint32_t run = nt << log2_v;      // 16 B vectors of one head on the universal side
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
-  const bool aligned = ((reinterpret_cast<uintptr_t>(chunk) | reinterpret_cast<uintptr_t>(uni)) & 15) == 0;
-  for (uint32_t nh_i = warp; nh_i < nh; nh_i += nwarps) {
-    uint8_t* u = uni + (static_cast<size_t>((nh_i * nl + nl_i) * no + no_i) * nt << log2_v << 4);
-    // chunk-side offset of vector v = (nt_i, c): NHD (nt_i*nh + nh_i)*row + 16c ; HND (nh_i*nt + nt_i)*row + 16c
-    const size_t c_base = layout == KVBM_BLOCK_LAYOUT_NHD ? static_cast<size_t>(nh_i) * row : static_cast<size_t>(nh_i) * nt * row;
-    const size_t c_stride = layout == KVBM_BLOCK_LAYOUT_NHD ? static_cast<size_t>(nh) * row : row;
-    auto chunk_off = [&](uint32_t v) { return c_base + static_cast<size_t>(v >> log2_v) * c_stride + ((v & (V - 1)) << 4); };
-    if (aligned) {
-      constexpr int U = 8;
-      uint32_t v = lane;
-      for (; v + (U - 1) * 32 < run; v += U * 32) {
-        uint4 x[U];
-#pragma unroll
-        for (int k = 0; k < U; ++k)
-          x[k] = ptx::ld_stream_v4(TO_UNIVERSAL ? chunk + chunk_off(v + k * 32) : u + (static_cast<size_t>(v + k * 32) << 4));
-#pragma unroll
-        for (int k = 0; k < U; ++k)
-          ptx::st_stream_v4(TO_UNIVERSAL ? u + (static_cast<size_t>(v + k * 32) << 4) : chunk + chunk_off(v + k * 32), x[k]);
-      }
-      for (; v < run; v += 32) {
-        const uint4 x = ptx::ld_stream_v4(TO_UNIVERSAL ? chunk + chunk_off(v) : u + (static_cast<size_t>(v) << 4));
-        ptx::st_stream_v4(TO_UNIVERSAL ? u + (static_cast<size_t>(v) << 4) : chunk + chunk_off(v), x);
-      }
-    } else {
-      // buffers only promise element alignment: same walk, one element at a time
-      const uint32_t per_vec = 16 / elem;
-      for (uint32_t e = lane; e < run * per_vec; e += 32) {
-        const uint32_t v = e / per_vec, within = (e - v * per_vec) * elem;
-        uint8_t* cp = chunk + chunk_off(v) + within;
-        uint8_t* up = u + (static_cast<size_t>(v) << 4) + within;
-        uint8_t* d = TO_UNIVERSAL ? up : cp;
-        const uint8_t* sp = TO_UNIVERSAL ? cp : up;
-        if (elem == 2) *reinterpret_cast<uint16_t*>(d) = *reinterpret_cast<const uint16_t*>(sp);
-        else if (elem == 4) *reinterpret_cast<uint32_t*>(d) = *reinterpret_cast<const uint32_t*>(sp);
-        else *reinterpret_cast<uint2*>(d) = *reinterpret_cast<const uint2*>(sp);
-      }
-    }
-  }
-}
-
 // ------------------------------------------------------------------------------------------------
-// Paged permute: the K2 / K3 walk with the addresses computed from the pools' layouts and block tables instead of
-// host-built pointer tables, and for any pair of KvBlockLayouts (kv_block_layout.rs:85-95).  For a fixed
-// (block, layer, outer, head) the nt rows of one head sit at  base + head * head_stride + t * tok_stride  on either side:
+// The head-row walk of the permuting kernels (K2 / K3 on pointer tables, and the paged transform).  For a fixed
+// (block, layer, outer, head) the nt rows of one head sit at  base + head * head_stride + t * tok_stride  on either side,
+// for every KvBlockLayout (kv_block_layout.rs:85-95):
 //   UniversalTP [nh,nl,no,nt,hd]  base = block + (l*no + o)*nt*row     head_stride = nl*no*nt*row  tok_stride = row
 //   UniversalPP [nl,nh,no,nt,hd]  base = block + l*nh*no*nt*row + o*nt*row   head_stride = no*nt*row   tok_stride = row
 //   OperationalHND [nl,no,nh,nt,hd]  base = region(l, o)               head_stride = nt*row        tok_stride = row
 //   OperationalNHD [nl,no,nt,nh,hd]  base = region(l, o)               head_stride = row           tok_stride = nh*row
-// One CTA per (block pair, layer, outer), one warp per head, 8 independent 16 B loads per lane before the first store.
+// K2 / K3's chunk [nt,nh,hd] / [nh,nt,hd] is an OperationalNHD / HND region and its universal block is UniversalTP.
+// One CTA per (block, layer, outer) unit -- the hardware CTA scheduler balances the SMs --, one warp per head, a few
+// integer ops per 16 B vector (the reference peels 5 div/mod per ELEMENT, tensor_kernels.cu:150-187) and 8 independent
+// 16 B loads per lane in flight before the first store.
 // ------------------------------------------------------------------------------------------------
 struct PermuteSide {
   const uint64_t* layer_base;
@@ -483,11 +425,155 @@ struct PermuteSide {
   int universal;
 };
 
+// The stride table above, for one side of a transform.  False for a format without one, or strides that are not whole
+// 16 B vectors.
+static bool fill_permute_side(const kvbm_permute_side& in, uint32_t nl, uint32_t no, uint32_t nh, uint32_t nt, uint32_t row, PermuteSide* out)
+{
+  const uint64_t head_run = static_cast<uint64_t>(nt) * row;
+  PermuteSide p{};
+  p.layer_base = in.layout.layer_base;
+  p.ids = in.block_ids;
+  p.block_stride = in.layout.block_stride;
+  switch (in.kv_layout) {
+    case KVBM_KV_UNIVERSAL_TP:
+      p.universal = 1;
+      p.layer_step = no * head_run;
+      p.outer_step = head_run;
+      p.head_stride = static_cast<uint64_t>(nl) * no * head_run;
+      p.tok_stride = row;
+      break;
+    case KVBM_KV_UNIVERSAL_PP:
+      p.universal = 1;
+      p.layer_step = static_cast<uint64_t>(nh) * no * head_run;
+      p.outer_step = head_run;
+      p.head_stride = no * head_run;
+      p.tok_stride = row;
+      break;
+    case KVBM_KV_OPERATIONAL_HND:
+      p.outer_step = in.layout.outer_stride;
+      p.head_stride = head_run;
+      p.tok_stride = row;
+      break;
+    case KVBM_KV_OPERATIONAL_NHD:
+      p.outer_step = in.layout.outer_stride;
+      p.head_stride = row;
+      p.tok_stride = static_cast<uint64_t>(nh) * row;
+      break;
+    default:
+      return false;
+  }
+  if ((p.block_stride | p.outer_step) & 15) return false;
+  *out = p;
+  return true;
+}
+
+// How vector v of one head's run of nt rows splits into (token t, 16 B column c), v = t * V + c with V vectors per row:
+// a shift and a mask when V is a power of two, else a multiply-high by ceil(2^32 / V) (head_dim 80, 96, 192, MLA's
+// 576 ...), exact for v < 2^32 / V, so the 8 loads of a lane stay independent.
+struct RowSplit {
+  uint32_t vpr;    // pow2: log2 of V, else V
+  uint32_t magic;  // !pow2: ceil(2^32 / V)
+  bool pow2;
+};
+
+// The walk takes rows of a whole number of 16 B vectors, 16 B ... 64 KiB, and with the multiply-high only while
+// nt * V < 2^32 / V.  False otherwise.
+static bool row_split(uint64_t row_bytes, uint64_t nt, RowSplit* out)
+{
+  if (row_bytes < 16 || row_bytes > 65536 || (row_bytes & 15)) return false;
+  const uint32_t V = static_cast<uint32_t>(row_bytes >> 4);
+  if ((V & (V - 1)) == 0) {
+    uint32_t log2_v = 0;
+    while ((1u << log2_v) < V) ++log2_v;
+    *out = {log2_v, 0u, true};
+    return true;
+  }
+  if (nt * V >= (1ull << 32) / V) return false;
+  *out = {V, static_cast<uint32_t>(((1ull << 32) + V - 1) / V), false};
+  return true;
+}
+
+template <bool POW2>
+__device__ __forceinline__ uint32_t row_run(const RowSplit& r, uint32_t nt)  // 16 B vectors of one head
+{
+  return POW2 ? nt << r.vpr : nt * r.vpr;
+}
+
+// Offset of vector v from its head's base.  32-bit: a head's rows lie within one region of nt * nh * row < 2^32 bytes.
+template <bool POW2>
+__device__ __forceinline__ uint32_t row_offset(const RowSplit& r, uint32_t v, uint32_t tok_stride)
+{
+  const uint32_t t = POW2 ? v >> r.vpr : __umulhi(v, r.magic);
+  const uint32_t c = POW2 ? v & ((1u << r.vpr) - 1) : v - t * r.vpr;
+  return t * tok_stride + (c << 4);
+}
+
+// One unit: every head of it, one warp per head.  sb / db: the unit's bases; both must be 16 B aligned.  The last batch of
+// a head is predicated rather than a serial tail: for head_dim 64 ... 96 in bf16 it is the whole head, and its loads stay
+// independent.
+template <bool POW2>
+__device__ __forceinline__ void walk_head_rows(const uint8_t* sb, uint64_t s_head, uint32_t s_tok, uint8_t* db, uint64_t d_head,
+                                               uint32_t d_tok, uint32_t nh, uint32_t nt, const RowSplit& r)
+{
+  constexpr int U = 8;
+  const uint32_t run = row_run<POW2>(r, nt);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
+  for (uint32_t h = warp; h < nh; h += nwarps) {
+    const uint8_t* sh = sb + h * s_head;
+    uint8_t* dh = db + h * d_head;
+    for (uint32_t v = lane; v < run; v += U * 32) {
+      uint4 x[U];
+#pragma unroll
+      for (int k = 0; k < U; ++k)
+        if (v + k * 32 < run) x[k] = ptx::ld_stream_v4(sh + row_offset<POW2>(r, v + k * 32, s_tok));
+#pragma unroll
+      for (int k = 0; k < U; ++k)
+        if (v + k * 32 < run) ptx::st_stream_v4(dh + row_offset<POW2>(r, v + k * 32, d_tok), x[k]);
+    }
+  }
+}
+
+// K2 / K3 on the reference's pointer tables.  S is the source side, D the destination; the universal side's base is
+// universal_ptrs[b] + l * layer_step + o * outer_step, the chunk side's is block_ptrs[unit].  The ABI only promises
+// element alignment for the tables, so a unit whose bases are not 16 B aligned takes the same walk one element at a time.
+template <bool POW2>
+__global__ void __launch_bounds__(256)
+kvbm_permute_table_kernel(void* const* __restrict__ universal_ptrs, void* const* __restrict__ block_ptrs, const __grid_constant__ PermuteSide S,
+                          const __grid_constant__ PermuteSide D, uint32_t nl, uint32_t no, uint32_t nh, uint32_t nt, RowSplit r, uint32_t elem)
+{
+  const uint32_t unit = blockIdx.x;  // (b * nl + l) * no + o
+  const uint32_t b = unit / (nl * no);
+  const uint32_t rem = unit - b * (nl * no);
+  const uint32_t l = rem / no, o = rem - l * no;
+  auto base_of = [&](const PermuteSide& X) {
+    return X.universal ? static_cast<uint8_t*>(universal_ptrs[b]) + l * X.layer_step + o * X.outer_step : static_cast<uint8_t*>(block_ptrs[unit]);
+  };
+  const uint8_t* sb = base_of(S);
+  uint8_t* db = base_of(D);
+  if (((reinterpret_cast<uintptr_t>(sb) | reinterpret_cast<uintptr_t>(db)) & 15) == 0) {
+    walk_head_rows<POW2>(sb, S.head_stride, S.tok_stride, db, D.head_stride, D.tok_stride, nh, nt, r);
+    return;
+  }
+  const uint32_t per_vec = 16 / elem, n = row_run<POW2>(r, nt) * per_vec;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
+  for (uint32_t h = warp; h < nh; h += nwarps) {
+    for (uint32_t e = lane; e < n; e += 32) {
+      const uint32_t v = e / per_vec, within = (e - v * per_vec) * elem;
+      const uint8_t* sp = sb + h * S.head_stride + row_offset<POW2>(r, v, S.tok_stride) + within;
+      uint8_t* dp = db + h * D.head_stride + row_offset<POW2>(r, v, D.tok_stride) + within;
+      if (elem == 2) *reinterpret_cast<uint16_t*>(dp) = *reinterpret_cast<const uint16_t*>(sp);
+      else if (elem == 4) *reinterpret_cast<uint32_t*>(dp) = *reinterpret_cast<const uint32_t*>(sp);
+      else *reinterpret_cast<uint2*>(dp) = *reinterpret_cast<const uint2*>(sp);
+    }
+  }
+}
+
+// Paged permute: the walk with the bases computed from the pools' layouts and block tables instead of host-built pointer
+// tables, for any pair of KvBlockLayouts.  One CTA per (block pair, layer, outer).
 template <bool POW2>
 __global__ void __launch_bounds__(256)
 kvbm_paged_permute_kernel(const __grid_constant__ PermuteSide S, const __grid_constant__ PermuteSide D, uint32_t layer_begin,
-                          uint32_t nlayers, uint32_t no, uint32_t nh, uint32_t nt, uint32_t vpr /* POW2: log2 of, else: 16 B vectors per row */,
-                          uint32_t magic /* !POW2: ceil(2^32 / vpr) */)
+                          uint32_t nlayers, uint32_t no, uint32_t nh, uint32_t nt, RowSplit r)
 {
   const uint32_t unit = blockIdx.x;  // (pair * nlayers + l) * no + o
   const uint32_t pair = unit / (nlayers * no);
@@ -497,55 +583,7 @@ kvbm_paged_permute_kernel(const __grid_constant__ PermuteSide S, const __grid_co
     return reinterpret_cast<uint8_t*>(static_cast<uintptr_t>(__ldg(X.layer_base + (X.universal ? 0 : l)))) +
            static_cast<uint64_t>(__ldg(X.ids + pair)) * X.block_stride + l * X.layer_step + o * X.outer_step;
   };
-  const uint8_t* sb = base_of(S);
-  uint8_t* db = base_of(D);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
-  constexpr int U = 8;
-  if (POW2) {
-    const uint32_t log2_v = vpr;
-    const uint32_t V = 1u << log2_v;
-    const uint32_t run = nt << log2_v;  // 16 B vectors of one head
-    for (uint32_t h = warp; h < nh; h += nwarps) {
-      const uint8_t* sh = sb + h * S.head_stride;
-      uint8_t* dh = db + h * D.head_stride;
-      auto off = [&](const PermuteSide& X, uint32_t v) { return static_cast<uint64_t>(v >> log2_v) * X.tok_stride + ((v & (V - 1)) << 4); };
-      uint32_t v = lane;
-      for (; v + (U - 1) * 32 < run; v += U * 32) {
-        uint4 x[U];
-#pragma unroll
-        for (int k = 0; k < U; ++k) x[k] = ptx::ld_stream_v4(sh + off(S, v + k * 32));
-#pragma unroll
-        for (int k = 0; k < U; ++k) ptx::st_stream_v4(dh + off(D, v + k * 32), x[k]);
-      }
-      for (; v < run; v += 32) ptx::st_stream_v4(dh + off(D, v), ptx::ld_stream_v4(sh + off(S, v)));
-    }
-  } else {
-    // rows of any whole number of 16 B vectors (head_dim 80, 96, 192, MLA's 576 ...): token = v / V by a multiply-high with
-    // ceil(2^32 / V) (exact for v < 2^32 / V; the host checks nt * V against it), so the 8 loads stay independent
-    const uint32_t V = vpr;
-    const uint32_t run = nt * V;
-    for (uint32_t h = warp; h < nh; h += nwarps) {
-      const uint8_t* sh = sb + h * S.head_stride;
-      uint8_t* dh = db + h * D.head_stride;
-      uint32_t v = lane;
-      for (; v + (U - 1) * 32 < run; v += U * 32) {
-        uint4 x[U];
-        uint64_t od[U];
-#pragma unroll
-        for (int k = 0; k < U; ++k) {
-          const uint32_t vk = v + k * 32, t = __umulhi(vk, magic), c = vk - t * V;
-          x[k] = ptx::ld_stream_v4(sh + static_cast<uint64_t>(t) * S.tok_stride + (c << 4));
-          od[k] = static_cast<uint64_t>(t) * D.tok_stride + (c << 4);
-        }
-#pragma unroll
-        for (int k = 0; k < U; ++k) ptx::st_stream_v4(dh + od[k], x[k]);
-      }
-      for (; v < run; v += 32) {
-        const uint32_t t = __umulhi(v, magic), c = v - t * V;
-        ptx::st_stream_v4(dh + static_cast<uint64_t>(t) * D.tok_stride + (c << 4), ptx::ld_stream_v4(sh + static_cast<uint64_t>(t) * S.tok_stride + (c << 4)));
-      }
-    }
-  }
+  walk_head_rows<POW2>(base_of(S), S.head_stride, S.tok_stride, base_of(D), D.head_stride, D.tok_stride, nh, nt, r);
 }
 
 __global__ void kvbm_signal_kernel(uint32_t* a, uint32_t va, uint32_t* b, uint32_t vb)
@@ -583,25 +621,36 @@ static cudaError_t launch_permute(void* const* universal_ptrs, void* const* bloc
   if (layout != KVBM_BLOCK_LAYOUT_NHD && layout != KVBM_BLOCK_LAYOUT_HND) return cudaErrorInvalidValue;
   if (total_per_block * elem >= (1ull << 32)) return cudaErrorInvalidValue;
 
-  // The vector must divide a head row AND every buffer must be aligned to it.  Chunk/universal
-  // buffers come from cudaMalloc / torch (>= 256 B aligned) in practice, but the ABI takes raw
-  // pointers, so only widen past the element size when the row allows it and keep 2/4/8-byte
-  // vectors naturally aligned with the element type.
   const size_t row = hd * elem;
   DeviceInfo di;
   cudaError_t e = device_info(&di);
   if (e != cudaSuccess) return e;
-  if (row >= 16 && row <= 4096 && (row & (row - 1)) == 0 && num_blocks * nl * no < (1ull << 31) && nh * nl * no * nt * row < (1ull << 40)) {
-    uint32_t log2_v = 0;
-    while ((16u << log2_v) < row) ++log2_v;
+  RowSplit r;
+  if (num_blocks * nl * no < (1ull << 31) && row_split(row, nt, &r)) {
+    // the walk's strides: UniversalTP on the universal side, the chunk's own layout as an operational region
+    kvbm_permute_side uni{}, chunk{};
+    uni.kv_layout = KVBM_KV_UNIVERSAL_TP;
+    chunk.kv_layout = layout == KVBM_BLOCK_LAYOUT_NHD ? KVBM_KV_OPERATIONAL_NHD : KVBM_KV_OPERATIONAL_HND;
+    PermuteSide U, C;
+    const uint32_t nl32 = static_cast<uint32_t>(nl), no32 = static_cast<uint32_t>(no), nh32 = static_cast<uint32_t>(nh),
+                   nt32 = static_cast<uint32_t>(nt);
+    fill_permute_side(uni, nl32, no32, nh32, nt32, static_cast<uint32_t>(row), &U);
+    fill_permute_side(chunk, nl32, no32, nh32, nt32, static_cast<uint32_t>(row), &C);
+    const PermuteSide& S = TO_UNIVERSAL ? C : U;
+    const PermuteSide& D = TO_UNIVERSAL ? U : C;
     const unsigned grid = static_cast<unsigned>(num_blocks * nl * no);
-    const int threads = static_cast<int>(std::min<size_t>(8, std::max<size_t>(1, nh))) * 32;
-    kvbm_permute_rows_kernel<TO_UNIVERSAL><<<grid, threads, 0, stream>>>(universal_ptrs, block_ptrs, static_cast<uint32_t>(nh),
-                                                                          static_cast<uint32_t>(nl), static_cast<uint32_t>(no),
-                                                                          static_cast<uint32_t>(nt), log2_v, static_cast<uint32_t>(elem), layout);
+    const int threads = static_cast<int>(std::min<size_t>(8, nh)) * 32;
+    if (r.pow2)
+      kvbm_permute_table_kernel<true><<<grid, threads, 0, stream>>>(universal_ptrs, block_ptrs, S, D, nl32, no32, nh32, nt32, r, static_cast<uint32_t>(elem));
+    else
+      kvbm_permute_table_kernel<false><<<grid, threads, 0, stream>>>(universal_ptrs, block_ptrs, S, D, nl32, no32, nh32, nt32, r, static_cast<uint32_t>(elem));
     g_launches.fetch_add(1, std::memory_order_relaxed);
     return cudaGetLastError();
   }
+  // The vector must divide a head row AND every buffer must be aligned to it.  Chunk/universal
+  // buffers come from cudaMalloc / torch (>= 256 B aligned) in practice, but the ABI takes raw
+  // pointers, so only widen past the element size when the row allows it and keep 2/4/8-byte
+  // vectors naturally aligned with the element type.
   int vec = static_cast<int>(elem);
   if (row % 16 == 0)
     vec = 16;
@@ -651,10 +700,7 @@ static cudaError_t preload_kernels()
   cudaError_t e;
 #define KVBM_PRELOAD(k) \
   if ((e = cudaFuncGetAttributes(&attr, k)) != cudaSuccess) return e;
-  KVBM_PRELOAD(kvbm_pair_copy_kernel<8>)
-  KVBM_PRELOAD(kvbm_pair_copy_kernel<4>)
-  KVBM_PRELOAD(kvbm_pair_copy_kernel<2>)
-  KVBM_PRELOAD(kvbm_pair_copy_kernel<1>)
+  KVBM_PRELOAD(kvbm_pair_copy_kernel)
   KVBM_PRELOAD((kvbm_paged_copy_kernel<KVBM_CAST_NONE, false>))
   KVBM_PRELOAD((kvbm_paged_copy_kernel<KVBM_CAST_FP8E4M3_TO_BF16, false>))
   KVBM_PRELOAD((kvbm_paged_copy_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false>))
@@ -666,8 +712,8 @@ static cudaError_t preload_kernels()
   KVBM_PRELOAD(kvbm_paged_permute_kernel<true>)
   KVBM_PRELOAD(kvbm_paged_permute_kernel<false>)
   KVBM_PRELOAD(kvbm_signal_kernel)
-  KVBM_PRELOAD((kvbm_permute_rows_kernel<true>))
-  KVBM_PRELOAD((kvbm_permute_rows_kernel<false>))
+  KVBM_PRELOAD(kvbm_permute_table_kernel<true>)
+  KVBM_PRELOAD(kvbm_permute_table_kernel<false>)
   KVBM_PRELOAD((kvbm_permute_kernel<16, true>))
   KVBM_PRELOAD((kvbm_permute_kernel<8, true>))
   KVBM_PRELOAD((kvbm_permute_kernel<4, true>))
@@ -731,7 +777,7 @@ kvbm_kernels_launch_vectorized_copy(void** src_ptrs, void** dst_ptrs, size_t cop
   uint64_t ctas;
   uint32_t chunks_per_pair = 1;
   if (copy_size_bytes <= kPairSmall) {
-    ctas = (pairs + 7) / 8;  // 8 warps per CTA, one pair each
+    ctas = (pairs + kPairThreads / 32 - 1) / (kPairThreads / 32);  // one warp per pair
   } else {
     const uint64_t cpp = (copy_size_bytes + kPairChunk - 1) / kPairChunk;
     if (cpp >= (1ull << 32)) return cudaErrorInvalidValue;
@@ -741,17 +787,8 @@ kvbm_kernels_launch_vectorized_copy(void** src_ptrs, void** dst_ptrs, size_t cop
   const uint64_t gx = std::min<uint64_t>(ctas, 1ull << 30);
   const uint64_t gy = (ctas + gx - 1) / gx;
   if (gy > 65535) return cudaErrorInvalidValue;
-  // tuning knobs for experiments (benchmarks/kvbench.py): loads in flight per thread and CTA width
-  static const int k1_unroll = [] { const char* e = std::getenv("KVBM_K1_UNROLL"); return e ? std::atoi(e) : 4; }();
-  static const int k1_threads = [] { const char* e = std::getenv("KVBM_K1_THREADS"); const int t = e ? std::atoi(e) : 256; return t >= 32 && t <= 256 && t % 32 == 0 ? t : 256; }();
-  if (copy_size_bytes <= kPairSmall) ctas = (pairs + (k1_threads / 32) - 1) / (k1_threads / 32);
-  const dim3 grid(static_cast<unsigned>(std::min<uint64_t>(ctas, 1ull << 30)), static_cast<unsigned>((ctas + std::min<uint64_t>(ctas, 1ull << 30) - 1) / std::min<uint64_t>(ctas, 1ull << 30)));
-  switch (k1_unroll) {
-    case 1: kvbm_pair_copy_kernel<1><<<grid, k1_threads, 0, stream>>>(src_ptrs, dst_ptrs, copy_size_bytes, chunks_per_pair, pairs); break;
-    case 2: kvbm_pair_copy_kernel<2><<<grid, k1_threads, 0, stream>>>(src_ptrs, dst_ptrs, copy_size_bytes, chunks_per_pair, pairs); break;
-    case 8: kvbm_pair_copy_kernel<8><<<grid, k1_threads, 0, stream>>>(src_ptrs, dst_ptrs, copy_size_bytes, chunks_per_pair, pairs); break;
-    default: kvbm_pair_copy_kernel<4><<<grid, k1_threads, 0, stream>>>(src_ptrs, dst_ptrs, copy_size_bytes, chunks_per_pair, pairs); break;
-  }
+  kvbm_pair_copy_kernel<<<dim3(static_cast<unsigned>(gx), static_cast<unsigned>(gy)), kPairThreads, 0, stream>>>(
+      src_ptrs, dst_ptrs, copy_size_bytes, chunks_per_pair, pairs);
   g_launches.fetch_add(1, std::memory_order_relaxed);
   return cudaGetLastError();  // :570
 }
@@ -819,46 +856,6 @@ kvbm_kernels_launch_block_from_universal(const void* const* universal_ptrs, void
                                num_blocks, nh, nl, no, nt, hd, dtype, layout, stream);
 }
 
-static bool fill_permute_side(const kvbm_permute_side& in, uint32_t nl, uint32_t no, uint32_t nh, uint32_t nt, uint32_t row, PermuteSide* out)
-{
-  const uint64_t head_run = static_cast<uint64_t>(nt) * row;
-  PermuteSide p{};
-  p.layer_base = in.layout.layer_base;
-  p.ids = in.block_ids;
-  p.block_stride = in.layout.block_stride;
-  switch (in.kv_layout) {
-    case KVBM_KV_UNIVERSAL_TP:
-      p.universal = 1;
-      p.layer_step = no * head_run;
-      p.outer_step = head_run;
-      p.head_stride = static_cast<uint64_t>(nl) * no * head_run;
-      p.tok_stride = row;
-      break;
-    case KVBM_KV_UNIVERSAL_PP:
-      p.universal = 1;
-      p.layer_step = static_cast<uint64_t>(nh) * no * head_run;
-      p.outer_step = head_run;
-      p.head_stride = no * head_run;
-      p.tok_stride = row;
-      break;
-    case KVBM_KV_OPERATIONAL_HND:
-      p.outer_step = in.layout.outer_stride;
-      p.head_stride = head_run;
-      p.tok_stride = row;
-      break;
-    case KVBM_KV_OPERATIONAL_NHD:
-      p.outer_step = in.layout.outer_stride;
-      p.head_stride = row;
-      p.tok_stride = static_cast<uint64_t>(nh) * row;
-      break;
-    default:
-      return false;
-  }
-  if ((p.block_stride | p.outer_step) & 15) return false;
-  *out = p;
-  return true;
-}
-
 // Host-only view of the stride table the permuting kernel walks with (no GPU needed): lets the CPU suite check the
 // address arithmetic of every KvBlockLayout against the oracle's dim_order definition, at sizes no GPU test allocates.
 extern "C" int
@@ -897,7 +894,8 @@ kvbm_kernels_paged_permute(const kvbm_permute_side* src, const kvbm_permute_side
   if (!src || !dst || !src->block_ids || !dst->block_ids || !src->layout.layer_base || !dst->layout.layer_base) return cudaErrorInvalidValue;
   const uint32_t nl = src->layout.num_layers, no = src->layout.outer_dim;
   if (nl == 0 || no == 0 || nl != dst->layout.num_layers || no != dst->layout.outer_dim || static_cast<uint32_t>(layer_end) > nl) return cudaErrorInvalidValue;
-  if (row_bytes < 16 || row_bytes > 65536 || (row_bytes & 15) || num_heads == 0 || page_size == 0) return cudaErrorInvalidValue;
+  RowSplit r;
+  if (num_heads == 0 || page_size == 0 || !row_split(row_bytes, page_size, &r)) return cudaErrorInvalidValue;
   const uint64_t region = static_cast<uint64_t>(page_size) * num_heads * row_bytes;
   if (region != src->layout.region_bytes || region != dst->layout.region_bytes) return cudaErrorInvalidValue;
   PermuteSide S, D;
@@ -909,16 +907,10 @@ kvbm_kernels_paged_permute(const kvbm_permute_side* src, const kvbm_permute_side
   const int threads = static_cast<int>(std::min<uint32_t>(8, num_heads)) * 32;
   const unsigned grid = static_cast<unsigned>(units);
   const uint32_t lb = static_cast<uint32_t>(layer_begin), nlay = static_cast<uint32_t>(layer_end - layer_begin);
-  if ((row_bytes & (row_bytes - 1)) == 0) {
-    uint32_t log2_v = 0;
-    while ((16u << log2_v) < row_bytes) ++log2_v;
-    kvbm_paged_permute_kernel<true><<<grid, threads, 0, stream>>>(S, D, lb, nlay, no, num_heads, page_size, log2_v, 0u);
-  } else {
-    const uint32_t V = row_bytes >> 4;
-    const uint64_t magic = ((1ull << 32) + V - 1) / V;
-    if (static_cast<uint64_t>(page_size) * V >= (1ull << 32) / V) return cudaErrorInvalidValue;  // exactness bound of the multiply-high division
-    kvbm_paged_permute_kernel<false><<<grid, threads, 0, stream>>>(S, D, lb, nlay, no, num_heads, page_size, V, static_cast<uint32_t>(magic));
-  }
+  if (r.pow2)
+    kvbm_paged_permute_kernel<true><<<grid, threads, 0, stream>>>(S, D, lb, nlay, no, num_heads, page_size, r);
+  else
+    kvbm_paged_permute_kernel<false><<<grid, threads, 0, stream>>>(S, D, lb, nlay, no, num_heads, page_size, r);
   g_launches.fetch_add(1, std::memory_order_relaxed);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;

@@ -180,7 +180,9 @@ def test_permute_empty_batch_noop_and_bad_dtype():
     assert K.universal_from_block(0, 0, 2, 1, 1, 1, 1, 1, 9, K.BlockLayout.NHD, sp) == K.CUDA_ERROR_INVALID_VALUE  # tensor_kernels.cu:327
 
 
-def _permute_case(dtype, layout, dims, nb, seed=11):
+def _permute_case(dtype, layout, dims, nb, seed=11, offset=0):
+    """offset: every chunk and universal buffer starts that many elements into its allocation (the ABI only promises
+    element alignment for the pointer tables)."""
     nh, nl, no, nt, hd = dims
     npd, elem = kats.DTYPES[dtype], kats.ELEM[dtype]
     rng = np.random.default_rng(seed)
@@ -188,8 +190,11 @@ def _permute_case(dtype, layout, dims, nb, seed=11):
             for _ in range(nb)]
     ref_chunks = [c for u in unis for c in kats.make_blocks(u, layout)]
     sp = stream_ptr()
-    d_chunks = [torch.from_numpy(c.view(np.uint8).copy()).cuda() for c in ref_chunks]
-    d_unis = [dev_u8(u.nbytes, fill=0xDE) for u in unis]
+    sh = offset * elem
+    d_chunks = [dev_u8(c.nbytes + sh, fill=0xDE)[sh:] for c in ref_chunks]
+    for t, c in zip(d_chunks, ref_chunks):
+        t.copy_(torch.from_numpy(c.view(np.uint8)))
+    d_unis = [dev_u8(u.nbytes + sh, fill=0xDE)[sh:] for u in unis]
     bt, ut = dev_ptr_table([t.data_ptr() for t in d_chunks]), dev_ptr_table([t.data_ptr() for t in d_unis])
     assert K.universal_from_block(ut.data_ptr(), bt.data_ptr(), nb, nh, nl, no, nt, hd, dtype, layout, sp) == 0
     torch.cuda.synchronize()
@@ -213,8 +218,11 @@ def test_permute_roundtrip_reference_dims(dtype, layout):
 
 @pytest.mark.parametrize("layout", [kats.NHD, kats.HND])
 def test_permute_llama70b_tp_reshard_shape(layout):
-    # SURVEY §8 a15: per block [8, nl, 2, 16, 128] bf16 (fewer layers to keep the test small) -> 16 B vector path
-    _permute_case(1, layout, (8, 4, 2, 16, 128), 3)
+    # SURVEY §8 a15: per block [8, nl, 2, 16, hd] bf16 (fewer layers to keep the test small).  Rows of a whole number of
+    # 16 B vectors (power of two or not: head_dim 80, 96, MLA's 576) take the head-row walk; offset 1 moves every buffer
+    # one element off 16 B alignment, which takes the same walk one element at a time.
+    for hd, offset in [(128, 0), (80, 0), (96, 0), (576, 0), (128, 1), (80, 1)]:
+        _permute_case(1, layout, (8, 4, 2, 16, hd), 3, offset=offset)
 
 
 def permute_position_encoded_chunks(L, layout):

@@ -117,29 +117,31 @@ def test_layer_ranges_signals_and_argument_checks():
 
 
 def test_agrees_with_the_legacy_k2_k3_symbols():
-    """The pointer-table kernels the reference exports (tensor_kernels.cu:306-360) and the paged form write the same bytes."""
-    nl, no, nt, nh, hd, elem = 5, 2, 16, 8, 128, 2
-    row = hd * elem
+    """The pointer-table kernels the reference exports (tensor_kernels.cu:306-360) and the paged form write the same bytes,
+    for rows that are a power-of-two number of 16 B vectors (hd 128) and rows that are not (hd 80)."""
+    nl, no, nt, nh, elem = 5, 2, 16, 8, 2
     nb = 6
-    src = _host("LWs", nb, nl, no, nt, nh, hd, elem)
-    randomize(src, 21)
-    S = DevicePool(src)
-    uni_a = torch.zeros(nb * nl * no * nt * nh * row, dtype=torch.uint8, device="cuda:0")
-    uni_b = torch.zeros_like(uni_a)
-    bs = nl * no * nt * nh * row
-    # legacy: host-built pointer tables
-    chunk_ptrs = torch.tensor([S.region_addr(b, l, o) for b in range(nb) for l in range(nl) for o in range(no)], dtype=torch.int64, device="cuda:0")
-    uni_ptrs = torch.tensor([uni_a.data_ptr() + b * bs for b in range(nb)], dtype=torch.int64, device="cuda:0")
-    K.check(K.universal_from_block(uni_ptrs.data_ptr(), chunk_ptrs.data_ptr(), nb, nh, nl, no, nt, hd, K.TensorDataType.BF16,
-                                   K.BlockLayout.NHD, stream_ptr()))
-    # paged: layouts + block tables only
-    lb = torch.tensor([uni_b.data_ptr() + l * no * nt * nh * row for l in range(nl)], dtype=torch.int64, device="cuda:0")
-    udesc = K.PagedLayout(lb.data_ptr(), bs, nt * nh * row, nt * nh * row, nl, no, nb)
-    ids = ids_dev(range(nb))
-    K.check(K.paged_permute(K.PermuteSide(S.desc, ids.data_ptr(), int(KV.OperationalNHD)), K.PermuteSide(udesc, ids.data_ptr(), int(KV.UniversalTP)),
-                            nb, 0, nl, nh, nt, row, stream=stream_ptr()))
-    torch.cuda.synchronize()
-    assert torch.equal(uni_a, uni_b) and bool(uni_a.any())
+    for hd in (128, 80):
+        row = hd * elem
+        src = _host("LWs", nb, nl, no, nt, nh, hd, elem)
+        randomize(src, 21)
+        S = DevicePool(src)
+        uni_a = torch.zeros(nb * nl * no * nt * nh * row, dtype=torch.uint8, device="cuda:0")
+        uni_b = torch.zeros_like(uni_a)
+        bs = nl * no * nt * nh * row
+        # legacy: host-built pointer tables
+        chunk_ptrs = torch.tensor([S.region_addr(b, l, o) for b in range(nb) for l in range(nl) for o in range(no)], dtype=torch.int64, device="cuda:0")
+        uni_ptrs = torch.tensor([uni_a.data_ptr() + b * bs for b in range(nb)], dtype=torch.int64, device="cuda:0")
+        K.check(K.universal_from_block(uni_ptrs.data_ptr(), chunk_ptrs.data_ptr(), nb, nh, nl, no, nt, hd, K.TensorDataType.BF16,
+                                       K.BlockLayout.NHD, stream_ptr()))
+        # paged: layouts + block tables only
+        lb = torch.tensor([uni_b.data_ptr() + l * no * nt * nh * row for l in range(nl)], dtype=torch.int64, device="cuda:0")
+        udesc = K.PagedLayout(lb.data_ptr(), bs, nt * nh * row, nt * nh * row, nl, no, nb)
+        ids = ids_dev(range(nb))
+        K.check(K.paged_permute(K.PermuteSide(S.desc, ids.data_ptr(), int(KV.OperationalNHD)), K.PermuteSide(udesc, ids.data_ptr(), int(KV.UniversalTP)),
+                                nb, 0, nl, nh, nt, row, stream=stream_ptr()))
+        torch.cuda.synchronize()
+        assert torch.equal(uni_a, uni_b) and bool(uni_a.any()), hd
 
 
 # ---------------------------------------------------------------------------------------------------------------------
