@@ -27,6 +27,8 @@ p.add_argument("--page", type=int, default=16)
 p.add_argument("--iters", type=int, default=20)
 p.add_argument("--peer", type=int, default=-1, help="put one pool on this GPU (the launch stays on GPU 0); -1 = same GPU")
 p.add_argument("--peer-side", choices=["dst", "src"], default="dst", help="dst: universal pool on the peer (push); src: engine pool on the peer (pull)")
+p.add_argument("--cast", choices=["none", "fp8-to-bf16", "bf16-to-fp8"], default="none",
+               help="time the transform with the fused cast against the paged copy's cast and the two-pass workaround instead")
 a = p.parse_args()
 nl, no, nt, nh, hd, elem = a.layers, 2, a.page, a.heads, a.head_dim, 2
 row, region = hd * elem, nt * nh * hd * elem
@@ -71,6 +73,75 @@ def timed(fn, iters=a.iters, warm=3):
         e1.synchronize()
         ts.append(e0.elapsed_time(e1))
     return statistics.median(ts)
+
+
+def pool_pair(e):
+    """An engine pool (as `op`) and a universal pool (as `uni`) of e-byte elements: (engine layers, universal tensor, engine
+    descriptor, universal descriptor, the layer-base tables the descriptors point to)."""
+    reg = nt * nh * hd * e
+    eng = [torch.randint(0, 256, (no * nb * reg,), dtype=torch.uint8, device=sdev) for _ in range(nl)]
+    un = torch.zeros(nb * nl * no * reg, dtype=torch.uint8, device=ddev)
+    torch.cuda.synchronize(sdev)
+    eb = torch.tensor([t.data_ptr() for t in eng], dtype=torch.int64, device=dev)
+    ub = torch.tensor([un.data_ptr() + l * no * reg for l in range(nl)], dtype=torch.int64, device=dev)
+    return eng, un, K.PagedLayout(eb.data_ptr(), reg, nb * reg, reg, nl, no, nb), K.PagedLayout(ub.data_ptr(), nl * no * reg, reg, reg, nl, no, nb), (eb, ub)
+
+
+def cast_bench():
+    """(a) the fused permute + cast, engine -> universal and back; (b) the paged copy's fused cast of the same bytes (the floor
+    for 3 bytes per element); (c) the cheapest two-pass workaround: the permute in fp8 through a staging pool plus the paged
+    copy's cast, ordered so that the permute moves the narrow dtype (5 bytes per element)."""
+    up = a.cast == "fp8-to-bf16"
+    mode = K.CastMode.FP8E4M3_TO_BF16 if up else K.CastMode.BF16_TO_FP8E4M3
+    _eng8, uni8, eng8_desc, uni8_desc, _bases = pool_pair(1)  # the tensors stay alive while the descriptors are used
+    # source / destination descriptors of the engine -> universal direction; the fp8 pool of the other side is the staging pool
+    es, us, ed, ud = (eng8_desc, uni8_desc, op_desc, uni_desc) if up else (op_desc, uni_desc, eng8_desc, uni8_desc)
+    out = uni if up else uni8
+    src_row = hd * (1 if up else 2)
+    side = lambda desc, ids, kv: K.PermuteSide(desc, ids.data_ptr(), kv)  # noqa: E731
+
+    def fused_to():
+        K.check(K.paged_permute_cast(side(es, sid_d, 4), side(ud, did_d, 1), n, 0, nl, nh, nt, src_row, mode, stream=sp))
+
+    def fused_from():
+        K.check(K.paged_permute_cast(side(us, did_d, 1), side(ed, sid_d, 4), n, 0, nl, nh, nt, src_row, mode, stream=sp))
+
+    def cast_copy():
+        K.check(K.paged_copy(es, [K.PagedDst(ud, sid_d.data_ptr(), did_d.data_ptr(), 0, 0)], n, 0, nl, int(mode), None, sp))
+
+    def two_pass():
+        if up:   # permute fp8 into the fp8 universal pool, then cast it into the bf16 one
+            K.check(K.paged_permute(side(eng8_desc, sid_d, 4), side(uni8_desc, did_d, 1), n, 0, nl, nh, nt, hd, stream=sp))
+            K.check(K.paged_copy(uni8_desc, [K.PagedDst(uni_desc, did_d.data_ptr(), did_d.data_ptr(), 0, 0)], n, 0, nl, int(mode), None, sp))
+        else:    # cast into the fp8 engine pool, then permute fp8 into the fp8 universal pool
+            K.check(K.paged_copy(op_desc, [K.PagedDst(eng8_desc, sid_d.data_ptr(), sid_d.data_ptr(), 0, 0)], n, 0, nl, int(mode), None, sp))
+            K.check(K.paged_permute(side(eng8_desc, sid_d, 4), side(uni8_desc, did_d, 1), n, 0, nl, nh, nt, hd, stream=sp))
+
+    fused_to()
+    torch.cuda.synchronize()
+    fused_out = out.clone()
+    out.zero_()
+    torch.cuda.synchronize(ddev)
+    two_pass()
+    torch.cuda.synchronize()
+    same = bool(torch.equal(fused_out, out))
+    elems = n * nl * no * nt * nh * hd
+    res = {"geometry": {"blocks": n, "layers": nl, "outer": no, "page": nt, "heads": nh, "head_dim": hd, "cast": a.cast,
+                        "MiB_fp8": elems / 2**20, "MiB_bf16": 2 * elems / 2**20},
+           "peer": a.peer, "peer_side": a.peer_side if a.peer >= 0 else None, "fused_equals_two_pass": same,
+           "hbm_peak_GBps": peak, "hbm_peak_source": peak_src}
+    for name, fn, per_elem in (("fused_permute_cast_to_universal", fused_to, 3), ("fused_permute_cast_from_universal", fused_from, 3),
+                               ("paged_copy_cast", cast_copy, 3), ("two_pass_fp8_permute_and_cast_copy", two_pass, 5)):
+        ms = timed(fn)
+        moved_rw = per_elem * elems
+        res[name] = {"ms": round(ms, 4), "bytes_read_plus_write": moved_rw, "GBps_read_plus_write": round(moved_rw / ms / 1e6, 1),
+                     "frac_of_hbm_peak": round(moved_rw / ms / 1e6 / peak, 3)}
+    print(json.dumps(res))
+
+
+if a.cast != "none":
+    cast_bench()
+    sys.exit(0)
 
 
 def paged():

@@ -612,8 +612,9 @@ static int launch_cuda(kvbm_transfer_manager* m, Layout* S, Layout* const* D, in
 }
 
 // The layout-transforming transfer: what select_transform_kernel's result would drive if the reference ran it inside
-// execute_transfer (it rejects the pair instead, transfer/mod.rs:128-147).  One kvbm_kernels_paged_permute launch:
-// block tables uploaded like launch_cuda's, no pointer tables, completion word written by a trailing signal kernel.
+// execute_transfer (it rejects the pair instead, transfer/mod.rs:128-147).  One kvbm_kernels_paged_permute_cast launch, with the
+// transfer's fp8 <-> bf16 cast fused in: block tables uploaded like launch_cuda's, no pointer tables, completion word written by a
+// trailing signal kernel.
 static int launch_transform(kvbm_transfer_manager* m, Layout* S, Layout* D, int src_kv, int dst_kv, const size_t* src_ids,
                             const size_t* dst_ids, size_t n, size_t lb, size_t le, const kvbm_transfer_options& o,
                             cudaStream_t stream, Slot** slot_out, uint64_t* seq_out)
@@ -631,11 +632,11 @@ static int launch_transform(kvbm_transfer_manager* m, Layout* S, Layout* D, int 
   kvbm_permute_side ps{descriptor(*S), sl->dev_ids, src_kv}, pd{descriptor(*D), sl->dev_ids + n, dst_kv};
   const size_t nh = S->cfg.num_heads;
   const size_t row = S->cfg.inner_dim / nh * S->cfg.dtype_width_bytes;
-  cudaError_t e = kvbm_kernels_paged_permute(&ps, &pd, static_cast<int>(n), static_cast<int>(lb), static_cast<int>(le),
-                                             static_cast<uint32_t>(nh), static_cast<uint32_t>(S->cfg.page_size),
-                                             static_cast<uint32_t>(row), o.done_flag, o.epoch, sl->host_flag,
-                                             static_cast<uint32_t>(seq), stream);
-  if (e != cudaSuccess) return fail_cuda(e, "kvbm_kernels_paged_permute");
+  cudaError_t e = kvbm_kernels_paged_permute_cast(&ps, &pd, static_cast<int>(n), static_cast<int>(lb), static_cast<int>(le),
+                                                  static_cast<uint32_t>(nh), static_cast<uint32_t>(S->cfg.page_size),
+                                                  static_cast<uint32_t>(row), o.cast_mode, o.done_flag, o.epoch, sl->host_flag,
+                                                  static_cast<uint32_t>(seq), stream);
+  if (e != cudaSuccess) return fail_cuda(e, "kvbm_kernels_paged_permute_cast");
   CU(cudaEventRecord(sl->ev, stream));
   sl->in_flight = true;
   m->bytes_moved += n * (le - lb) * S->cfg.outer_dim * D->region;
@@ -734,17 +735,25 @@ static int execute(kvbm_transfer_manager* m, kvbm_layout_handle src_h, int nd, c
       return fail(KVBM_ERR_UNSUPPORTED, std::string("Layout transformation not supported: src=") + kv_name(src_kv) + ", dst=" + kv_name(dst_kv));
     if (t != KVBM_TRANSFORM_NONE) {
       if (nd != 1) return fail(KVBM_ERR_UNSUPPORTED, "a layout-transforming transfer takes one destination");
-      if (o.cast_mode != KVBM_CAST_NONE) return fail(KVBM_ERR_UNSUPPORTED, "the fused cast and a layout transformation cannot be combined");
       if (o.layer_ready_flags || o.layer_done_flags || o.per_dst_done_flags || o.per_dst_layer_done_flags || o.multicast)
         return fail(KVBM_ERR_UNSUPPORTED, "layer streaming / multicast are not available on a layout-transforming transfer");
       const kvbm_layout_config &sc = S->cfg, &dc = D[d]->cfg;
       if (!sc.num_heads || !dc.num_heads) return fail(KVBM_ERR_CONFIG, "num_heads_required_for_kv_block_layout");  // config.rs:118-126
-      if (sc.num_heads != dc.num_heads || sc.page_size != dc.page_size || sc.inner_dim != dc.inner_dim || sc.dtype_width_bytes != dc.dtype_width_bytes)
+      // with the fused cast the dtype widths differ as check_compat requires (1 -> 2 or 2 -> 1)
+      if (sc.num_heads != dc.num_heads || sc.page_size != dc.page_size || sc.inner_dim != dc.inner_dim ||
+          (o.cast_mode == KVBM_CAST_NONE && sc.dtype_width_bytes != dc.dtype_width_bytes))
         return fail(KVBM_ERR_INCOMPATIBLE, "a layout transformation needs equal num_heads, page_size, inner_dim and dtype on both sides");
       if (sc.inner_dim % sc.num_heads) return fail(KVBM_ERR_CONFIG, "inner_dim_must_be_divisible_by_num_heads");
-      const size_t row = sc.inner_dim / sc.num_heads * sc.dtype_width_bytes;
-      if (row < 16 || row > 65536 || (row & 15))
-        return fail(KVBM_ERR_UNSUPPORTED, "layout transformation: head_dim * dtype width must be a multiple of 16 bytes in 16..65536, got " + std::to_string(row));
+      const size_t head_dim = sc.inner_dim / sc.num_heads;
+      if (o.cast_mode != KVBM_CAST_NONE) {  // the walk splits the fp8 row (head_dim bytes) into 16 B vectors
+        if (head_dim < 16 || head_dim > 65536 || (head_dim & 15))
+          return fail(KVBM_ERR_UNSUPPORTED, "layout transformation with the fused cast: head_dim must be a multiple of 16 in 16..65536 (the fp8 row in whole "
+                                            "16-byte vectors), got " + std::to_string(head_dim));
+      } else {
+        const size_t row = head_dim * sc.dtype_width_bytes;
+        if (row < 16 || row > 65536 || (row & 15))
+          return fail(KVBM_ERR_UNSUPPORTED, "layout transformation: head_dim * dtype width must be a multiple of 16 bytes in 16..65536, got " + std::to_string(row));
+      }
       const bool s_uni = src_kv == KVBM_KV_UNIVERSAL_TP || src_kv == KVBM_KV_UNIVERSAL_PP;
       const bool d_uni = dst_kv == KVBM_KV_UNIVERSAL_TP || dst_kv == KVBM_KV_UNIVERSAL_PP;
       if ((s_uni && !S->fully_contiguous) || (d_uni && !D[d]->fully_contiguous))

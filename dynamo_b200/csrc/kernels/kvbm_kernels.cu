@@ -499,36 +499,82 @@ __device__ __forceinline__ uint32_t row_run(const RowSplit& r, uint32_t nt)  // 
   return POW2 ? nt << r.vpr : nt * r.vpr;
 }
 
-// Offset of vector v from its head's base.  32-bit: a head's rows lie within one region of nt * nh * row < 2^32 bytes.
-template <bool POW2>
+// Offset of vector v from its head's base, for a side whose vector is 2^SHIFT bytes (16, or 32 for the bf16 side of a
+// cast).  32-bit: a head's rows lie within one region of nt * nh * row < 2^32 bytes.
+template <bool POW2, int SHIFT = 4>
 __device__ __forceinline__ uint32_t row_offset(const RowSplit& r, uint32_t v, uint32_t tok_stride)
 {
   const uint32_t t = POW2 ? v >> r.vpr : __umulhi(v, r.magic);
   const uint32_t c = POW2 ? v & ((1u << r.vpr) - 1) : v - t * r.vpr;
-  return t * tok_stride + (c << 4);
+  return t * tok_stride + (c << SHIFT);
+}
+
+// One vector of a cast walk: 16 e4m3 codes <-> 16 bf16, bit for bit the conversions of the paged copy's cast rings.
+// in[0 .. IN) are the 16 B loads of the source side, out[0 .. OUT) the 16 B stores of the destination side.
+__device__ __forceinline__ void cast_vector_up(const uint4 (&in)[1], uint4 (&out)[2])
+{
+  const uint32_t w[4] = {in[0].x, in[0].y, in[0].z, in[0].w};
+  uint32_t o[8];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    o[2 * k] = ptx::e4m3x2_to_bf16x2(static_cast<uint16_t>(w[k] & 0xffff));
+    o[2 * k + 1] = ptx::e4m3x2_to_bf16x2(static_cast<uint16_t>(w[k] >> 16));
+  }
+  out[0] = make_uint4(o[0], o[1], o[2], o[3]);
+  out[1] = make_uint4(o[4], o[5], o[6], o[7]);
+}
+__device__ __forceinline__ void cast_vector_down(const uint4 (&in)[2], uint4 (&out)[1])
+{
+  const uint32_t w[8] = {in[0].x, in[0].y, in[0].z, in[0].w, in[1].x, in[1].y, in[1].z, in[1].w};
+  uint32_t o[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+    o[k] = static_cast<uint32_t>(ptx::bf16x2_to_e4m3x2(w[2 * k])) | (static_cast<uint32_t>(ptx::bf16x2_to_e4m3x2(w[2 * k + 1])) << 16);
+  out[0] = make_uint4(o[0], o[1], o[2], o[3]);
 }
 
 // One unit: every head of it, one warp per head.  sb / db: the unit's bases; both must be 16 B aligned.  The last batch of
 // a head is predicated rather than a serial tail: for head_dim 64 ... 96 in bf16 it is the whole head, and its loads stay
-// independent.
-template <bool POW2>
+// independent.  With a cast (KVBM_CAST_*) the walk counts 16 B vectors of the fp8 side's row: one vector is 16 elements,
+// 16 B on the fp8 side and 32 B on the bf16 side, so fp8 -> bf16 turns one load into two stores and bf16 -> fp8 two loads
+// into one store.  Every lane keeps 8 independent 16 B loads in flight in all three forms.
+template <int CAST, bool POW2>
 __device__ __forceinline__ void walk_head_rows(const uint8_t* sb, uint64_t s_head, uint32_t s_tok, uint8_t* db, uint64_t d_head,
                                                uint32_t d_tok, uint32_t nh, uint32_t nt, const RowSplit& r)
 {
-  constexpr int U = 8;
+  constexpr int IN = CAST == KVBM_CAST_BF16_TO_FP8E4M3 ? 2 : 1;   // 16 B loads per vector
+  constexpr int OUT = CAST == KVBM_CAST_FP8E4M3_TO_BF16 ? 2 : 1;  // 16 B stores per vector
+  constexpr int U = 8 / IN;
   const uint32_t run = row_run<POW2>(r, nt);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
   for (uint32_t h = warp; h < nh; h += nwarps) {
     const uint8_t* sh = sb + h * s_head;
     uint8_t* dh = db + h * d_head;
     for (uint32_t v = lane; v < run; v += U * 32) {
-      uint4 x[U];
+      uint4 x[U][IN];
 #pragma unroll
       for (int k = 0; k < U; ++k)
-        if (v + k * 32 < run) x[k] = ptx::ld_stream_v4(sh + row_offset<POW2>(r, v + k * 32, s_tok));
+        if (v + k * 32 < run) {
+          const uint8_t* s = sh + row_offset<POW2, 3 + IN>(r, v + k * 32, s_tok);
+#pragma unroll
+          for (int i = 0; i < IN; ++i) x[k][i] = ptx::ld_stream_v4(s + 16 * i);
+        }
 #pragma unroll
       for (int k = 0; k < U; ++k)
-        if (v + k * 32 < run) ptx::st_stream_v4(dh + row_offset<POW2>(r, v + k * 32, d_tok), x[k]);
+        if (v + k * 32 < run) {
+          uint8_t* d = dh + row_offset<POW2, 3 + OUT>(r, v + k * 32, d_tok);
+          if constexpr (CAST == KVBM_CAST_NONE) {
+            ptx::st_stream_v4(d, x[k][0]);
+          } else {
+            uint4 y[OUT];
+            if constexpr (CAST == KVBM_CAST_FP8E4M3_TO_BF16)
+              cast_vector_up(x[k], y);
+            else
+              cast_vector_down(x[k], y);
+#pragma unroll
+            for (int i = 0; i < OUT; ++i) ptx::st_stream_v4(d + 16 * i, y[i]);
+          }
+        }
     }
   }
 }
@@ -551,7 +597,7 @@ kvbm_permute_table_kernel(void* const* __restrict__ universal_ptrs, void* const*
   const uint8_t* sb = base_of(S);
   uint8_t* db = base_of(D);
   if (((reinterpret_cast<uintptr_t>(sb) | reinterpret_cast<uintptr_t>(db)) & 15) == 0) {
-    walk_head_rows<POW2>(sb, S.head_stride, S.tok_stride, db, D.head_stride, D.tok_stride, nh, nt, r);
+    walk_head_rows<KVBM_CAST_NONE, POW2>(sb, S.head_stride, S.tok_stride, db, D.head_stride, D.tok_stride, nh, nt, r);
     return;
   }
   const uint32_t per_vec = 16 / elem, n = row_run<POW2>(r, nt) * per_vec;
@@ -569,8 +615,9 @@ kvbm_permute_table_kernel(void* const* __restrict__ universal_ptrs, void* const*
 }
 
 // Paged permute: the walk with the bases computed from the pools' layouts and block tables instead of host-built pointer
-// tables, for any pair of KvBlockLayouts.  One CTA per (block pair, layer, outer).
-template <bool POW2>
+// tables, for any pair of KvBlockLayouts, optionally casting (CAST: KVBM_CAST_*; each side's strides are for its own row).
+// One CTA per (block pair, layer, outer).
+template <int CAST, bool POW2>
 __global__ void __launch_bounds__(256)
 kvbm_paged_permute_kernel(const __grid_constant__ PermuteSide S, const __grid_constant__ PermuteSide D, uint32_t layer_begin,
                           uint32_t nlayers, uint32_t no, uint32_t nh, uint32_t nt, RowSplit r)
@@ -583,7 +630,7 @@ kvbm_paged_permute_kernel(const __grid_constant__ PermuteSide S, const __grid_co
     return reinterpret_cast<uint8_t*>(static_cast<uintptr_t>(__ldg(X.layer_base + (X.universal ? 0 : l)))) +
            static_cast<uint64_t>(__ldg(X.ids + pair)) * X.block_stride + l * X.layer_step + o * X.outer_step;
   };
-  walk_head_rows<POW2>(base_of(S), S.head_stride, S.tok_stride, base_of(D), D.head_stride, D.tok_stride, nh, nt, r);
+  walk_head_rows<CAST, POW2>(base_of(S), S.head_stride, S.tok_stride, base_of(D), D.head_stride, D.tok_stride, nh, nt, r);
 }
 
 __global__ void kvbm_signal_kernel(uint32_t* a, uint32_t va, uint32_t* b, uint32_t vb)
@@ -709,8 +756,12 @@ static cudaError_t preload_kernels()
   KVBM_PRELOAD((kvbm_paged_copy_kernel<KVBM_CAST_BF16_TO_FP8E4M3, true>))
   KVBM_PRELOAD(kvbm_set_flags_kernel)
   KVBM_PRELOAD(kvbm_wait_flag_kernel)
-  KVBM_PRELOAD(kvbm_paged_permute_kernel<true>)
-  KVBM_PRELOAD(kvbm_paged_permute_kernel<false>)
+  KVBM_PRELOAD((kvbm_paged_permute_kernel<KVBM_CAST_NONE, true>))
+  KVBM_PRELOAD((kvbm_paged_permute_kernel<KVBM_CAST_NONE, false>))
+  KVBM_PRELOAD((kvbm_paged_permute_kernel<KVBM_CAST_FP8E4M3_TO_BF16, true>))
+  KVBM_PRELOAD((kvbm_paged_permute_kernel<KVBM_CAST_FP8E4M3_TO_BF16, false>))
+  KVBM_PRELOAD((kvbm_paged_permute_kernel<KVBM_CAST_BF16_TO_FP8E4M3, true>))
+  KVBM_PRELOAD((kvbm_paged_permute_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false>))
   KVBM_PRELOAD(kvbm_signal_kernel)
   KVBM_PRELOAD(kvbm_permute_table_kernel<true>)
   KVBM_PRELOAD(kvbm_permute_table_kernel<false>)
@@ -882,7 +933,18 @@ kvbm_kernels_paged_permute(const kvbm_permute_side* src, const kvbm_permute_side
                            int layer_end, uint32_t num_heads, uint32_t page_size, uint32_t row_bytes, uint32_t* done_flag,
                            uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
 {
+  return kvbm_kernels_paged_permute_cast(src, dst, num_blocks, layer_begin, layer_end, num_heads, page_size, row_bytes, KVBM_CAST_NONE,
+                                         done_flag, epoch, completion_flag, completion_value, stream);
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_permute_cast(const kvbm_permute_side* src, const kvbm_permute_side* dst, int num_blocks, int layer_begin,
+                                int layer_end, uint32_t num_heads, uint32_t page_size, uint32_t src_row_bytes, int cast_mode,
+                                uint32_t* done_flag, uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value,
+                                cudaStream_t stream)
+{
   if (num_blocks < 0 || layer_begin < 0 || layer_end < layer_begin) return cudaErrorInvalidValue;
+  if (cast_mode < KVBM_CAST_NONE || cast_mode > KVBM_CAST_BF16_TO_FP8E4M3) return cudaErrorInvalidValue;
   const bool signal = done_flag || completion_flag;
   auto finish = [&]() -> cudaError_t {
     if (!signal) return cudaSuccess;
@@ -894,23 +956,37 @@ kvbm_kernels_paged_permute(const kvbm_permute_side* src, const kvbm_permute_side
   if (!src || !dst || !src->block_ids || !dst->block_ids || !src->layout.layer_base || !dst->layout.layer_base) return cudaErrorInvalidValue;
   const uint32_t nl = src->layout.num_layers, no = src->layout.outer_dim;
   if (nl == 0 || no == 0 || nl != dst->layout.num_layers || no != dst->layout.outer_dim || static_cast<uint32_t>(layer_end) > nl) return cudaErrorInvalidValue;
+  // The walk splits the fp8 side's row into 16 B vectors when casting (the bf16 side's vectors are 32 B), else the row.
+  if (cast_mode == KVBM_CAST_BF16_TO_FP8E4M3 && (src_row_bytes & 1)) return cudaErrorInvalidValue;
+  const uint64_t dst_row_bytes = cast_mode == KVBM_CAST_FP8E4M3_TO_BF16   ? 2ull * src_row_bytes
+                                 : cast_mode == KVBM_CAST_BF16_TO_FP8E4M3 ? src_row_bytes / 2
+                                                                          : src_row_bytes;
+  const uint64_t walk_row = cast_mode == KVBM_CAST_BF16_TO_FP8E4M3 ? dst_row_bytes : src_row_bytes;
   RowSplit r;
-  if (num_heads == 0 || page_size == 0 || !row_split(row_bytes, page_size, &r)) return cudaErrorInvalidValue;
-  const uint64_t region = static_cast<uint64_t>(page_size) * num_heads * row_bytes;
-  if (region != src->layout.region_bytes || region != dst->layout.region_bytes) return cudaErrorInvalidValue;
+  if (num_heads == 0 || page_size == 0 || !row_split(walk_row, page_size, &r)) return cudaErrorInvalidValue;
+  const uint64_t rows = static_cast<uint64_t>(page_size) * num_heads;
+  if (rows * src_row_bytes != src->layout.region_bytes || rows * dst_row_bytes != dst->layout.region_bytes) return cudaErrorInvalidValue;
   PermuteSide S, D;
-  if (!fill_permute_side(*src, nl, no, num_heads, page_size, row_bytes, &S) ||
-      !fill_permute_side(*dst, nl, no, num_heads, page_size, row_bytes, &D))
+  if (!fill_permute_side(*src, nl, no, num_heads, page_size, src_row_bytes, &S) ||
+      !fill_permute_side(*dst, nl, no, num_heads, page_size, static_cast<uint32_t>(dst_row_bytes), &D))
     return cudaErrorInvalidValue;
   const uint64_t units = static_cast<uint64_t>(num_blocks) * (layer_end - layer_begin) * no;
   if (units >= (1ull << 31)) return cudaErrorInvalidValue;
   const int threads = static_cast<int>(std::min<uint32_t>(8, num_heads)) * 32;
   const unsigned grid = static_cast<unsigned>(units);
   const uint32_t lb = static_cast<uint32_t>(layer_begin), nlay = static_cast<uint32_t>(layer_end - layer_begin);
-  if (r.pow2)
-    kvbm_paged_permute_kernel<true><<<grid, threads, 0, stream>>>(S, D, lb, nlay, no, num_heads, page_size, r);
-  else
-    kvbm_paged_permute_kernel<false><<<grid, threads, 0, stream>>>(S, D, lb, nlay, no, num_heads, page_size, r);
+  auto go = [&](auto kern) { kern<<<grid, threads, 0, stream>>>(S, D, lb, nlay, no, num_heads, page_size, r); };
+  switch (cast_mode) {
+    case KVBM_CAST_NONE:
+      r.pow2 ? go(kvbm_paged_permute_kernel<KVBM_CAST_NONE, true>) : go(kvbm_paged_permute_kernel<KVBM_CAST_NONE, false>);
+      break;
+    case KVBM_CAST_FP8E4M3_TO_BF16:
+      r.pow2 ? go(kvbm_paged_permute_kernel<KVBM_CAST_FP8E4M3_TO_BF16, true>) : go(kvbm_paged_permute_kernel<KVBM_CAST_FP8E4M3_TO_BF16, false>);
+      break;
+    default:
+      r.pow2 ? go(kvbm_paged_permute_kernel<KVBM_CAST_BF16_TO_FP8E4M3, true>) : go(kvbm_paged_permute_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false>);
+      break;
+  }
   g_launches.fetch_add(1, std::memory_order_relaxed);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;

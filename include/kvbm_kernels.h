@@ -205,6 +205,19 @@ cudaError_t kvbm_kernels_paged_permute(const kvbm_permute_side* src, const kvbm_
                                        uint32_t row_bytes, uint32_t* done_flag, uint32_t epoch, uint32_t* completion_flag,
                                        uint32_t completion_value, cudaStream_t stream);
 
+/* kvbm_kernels_paged_permute with the fp8 e4m3 <-> bf16 cast of kvbm_kernels_paged_copy_v2 fused in: the same walk, one launch,
+ * bits identical to the paged copy's cast (fp8 NaN codes -> 0x7fc0; bf16 -> fp8 round-to-nearest-even, saturating to +-448,
+ * NaN -> 0x7f with its sign).  src_row_bytes is the SOURCE row (head_dim * source element size); the destination row is twice
+ * it for KVBM_CAST_FP8E4M3_TO_BF16, half of it for KVBM_CAST_BF16_TO_FP8E4M3 (src_row_bytes must then be even) and equal for
+ * KVBM_CAST_NONE, which is exactly kvbm_kernels_paged_permute.  Each side's region_bytes must be page_size * num_heads * its
+ * own row.  With a cast the fp8 side's row must be a multiple of 16 in 16..65536 (head_dim a multiple of 16); the walk moves
+ * 16 e4m3 codes / 32 B of bf16 per vector.  An unknown cast_mode is cudaErrorInvalidValue; the zero-count early return (which
+ * still signals), the stride, index-range and grid rules and the signals are those of kvbm_kernels_paged_permute. */
+cudaError_t kvbm_kernels_paged_permute_cast(const kvbm_permute_side* src, const kvbm_permute_side* dst, int num_blocks,
+                                            int layer_begin, int layer_end, uint32_t num_heads, uint32_t page_size,
+                                            uint32_t src_row_bytes, int cast_mode, uint32_t* done_flag, uint32_t epoch,
+                                            uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream);
+
 /* Host-only (no GPU): the stride table kvbm_kernels_paged_permute walks with for one side.  out[0] = 1 when offsets count
  * from the block's first byte (universal formats) or 0 when they count from the (layer, outer) region's first byte; the
  * element (layer l, outer o, head h, token t) then sits at  [out[0] ? l * out[1] + o * out[2] : 0] + h * out[3] + t * out[4].
