@@ -29,6 +29,8 @@ p.add_argument("--peer", type=int, default=-1, help="put one pool on this GPU (t
 p.add_argument("--peer-side", choices=["dst", "src"], default="dst", help="dst: universal pool on the peer (push); src: engine pool on the peer (pull)")
 p.add_argument("--cast", choices=["none", "fp8-to-bf16", "bf16-to-fp8"], default="none",
                help="time the transform with the fused cast against the paged copy's cast and the two-pass workaround instead")
+p.add_argument("--reshard", default=None, metavar="SRC_TP:DST_TP",
+               help="time one decode rank's assembly of its heads from the source ranks' pools (TP re-shard) instead; --cast composes")
 a = p.parse_args()
 nl, no, nt, nh, hd, elem = a.layers, 2, a.page, a.heads, a.head_dim, 2
 row, region = hd * elem, nt * nh * hd * elem
@@ -139,6 +141,76 @@ def cast_bench():
     print(json.dumps(res))
 
 
+def reshard_bench():
+    """Decode rank 0 of a SRC_TP -> DST_TP re-shard: every launch of its plan (kvbm_kernels_paged_permute_heads, engine pools
+    OperationalNHD layer-separate on both sides, --cast fused in), per hand-off, median over three runs.  Compared with the plain
+    paged copy (its cast with --cast) of the same destination bytes and with the full-head permute (every head of a TP1 pool,
+    NHD -> NHD) per byte."""
+    from dynamo_b200.physical import tp_reshard_plan
+    from oracle import oracle as O
+    from tests.reshard_oracle import reshard_block
+    src_tp, dst_tp = (int(x) for x in a.reshard.split(":"))
+    mode = {"none": K.CastMode.NONE, "fp8-to-bf16": K.CastMode.FP8E4M3_TO_BF16, "bf16-to-fp8": K.CastMode.BF16_TO_FP8E4M3}[a.cast]
+    se, de = {"none": (2, 2), "fp8-to-bf16": (1, 2), "bf16-to-fp8": (2, 1)}[a.cast]
+    snh, dnh = max(1, nh // src_tp), max(1, nh // dst_tp)
+    plan = tp_reshard_plan(nh, src_tp, dst_tp, 0)
+
+    def engine(heads, e, device):
+        reg = nt * heads * hd * e
+        layers = [torch.randint(0, 256, (no * nb * reg,), dtype=torch.uint8, device=device) for _ in range(nl)]
+        base = torch.tensor([t.data_ptr() for t in layers], dtype=torch.int64, device=dev)
+        return layers, base, K.PagedLayout(base.data_ptr(), reg, nb * reg, reg, nl, no, nb)
+
+    srcs = {w.src_rank: engine(snh, se, sdev) for w in plan}
+    dst = engine(dnh, de, ddev)
+    side = lambda desc, ids: K.PermuteSide(desc, ids.data_ptr(), int(K.KvBlockLayout.OperationalNHD))  # noqa: E731
+
+    def assemble():
+        for w in plan:
+            K.check(K.paged_permute_heads(side(srcs[w.src_rank][2], sid_d), side(dst[2], did_d), n, 0, nl, snh, w.src_head_begin, dnh,
+                                          w.dst_head_begin, w.head_count, nt, hd * se, int(mode), stream=sp))
+
+    assemble()
+    torch.cuda.synchronize()
+    def block(pool, b):   # the [layer][outer] regions of block b of a block-is-second-dim pool
+        return np.concatenate([pool[0][l].view(no, nb, -1)[o, b].cpu().numpy() for l in range(nl) for o in range(no)])
+
+    same = sum(w.head_count for w in plan) == dnh   # the plan writes every destination head, so the old bytes do not matter
+    for i in (0, n - 1):   # sampled blocks against the oracle
+        want = np.zeros(nl * no * nt * dnh * hd * de, dtype=np.uint8)
+        for w in plan:
+            want = reshard_block(block(srcs[w.src_rank], int(sid[i])), want, O.KV_OPERATIONAL_NHD, O.KV_OPERATIONAL_NHD, nl, no, nt, snh,
+                                 dnh, hd * se, int(mode), w.src_head_begin, w.dst_head_begin, w.head_count)
+        same = same and bool(np.array_equal(block(dst, int(did[i])), want))
+    plain_src = engine(dnh, se, sdev)   # the same destination bytes as one paged copy (its cast with --cast)
+
+    def plain():
+        K.check(K.paged_copy(plain_src[2], [K.PagedDst(dst[2], sid_d.data_ptr(), did_d.data_ptr(), 0, 0)], n, 0, nl, int(mode), None, sp))
+
+    full_src, full_dst = engine(nh, se, sdev), engine(nh, de, ddev)
+
+    def full_permute():
+        K.check(K.paged_permute_heads(side(full_src[2], sid_d), side(full_dst[2], did_d), n, 0, nl, nh, 0, nh, 0, nh, nt, hd * se, int(mode),
+                                      stream=sp))
+
+    elems = n * nl * no * nt * dnh * hd
+    res = {"geometry": {"blocks": n, "layers": nl, "outer": no, "page": nt, "heads": nh, "head_dim": hd, "cast": a.cast,
+                        "src_tp": src_tp, "dst_tp": dst_tp, "src_heads_per_rank": snh, "dst_heads_per_rank": dnh},
+           "plan": [[w.src_rank, w.src_head_begin, w.dst_head_begin, w.head_count] for w in plan],
+           "window_widths": [w.head_count for w in plan], "launches": len(plan), "reshard_equals_oracle": same,
+           "peer": a.peer, "peer_side": a.peer_side if a.peer >= 0 else None, "hbm_peak_GBps": peak, "hbm_peak_source": peak_src}
+    for name, fn, count in (("reshard_assembly", assemble, elems), ("plain_paged_copy_same_bytes", plain, elems),
+                            ("full_head_permute_tp1", full_permute, n * nl * no * nt * nh * hd)):
+        ms = statistics.median([timed(fn) for _ in range(3)])
+        rw = count * (se + de)
+        res[name] = {"ms": round(ms, 4), "bytes_read_plus_write": rw, "GBps_read_plus_write": round(rw / ms / 1e6, 1),
+                     "frac_of_hbm_peak": round(rw / ms / 1e6 / peak, 3)}
+    print(json.dumps(res))
+
+
+if a.reshard:
+    reshard_bench()
+    sys.exit(0)
 if a.cast != "none":
     cast_bench()
     sys.exit(0)

@@ -529,7 +529,9 @@ static int acquire_slot(kvbm_transfer_manager* m, size_t ids_needed, size_t ws_n
   return KVBM_OK;
 }
 
-static int check_compat(const Layout& S, const Layout& D, int cast)
+// heads: a head-window transfer, whose regions differ when the head counts do; the head rows (head_dim elements) must match
+// instead.  Both configs then carry num_heads dividing inner_dim (checked by the caller).
+static int check_compat(const Layout& S, const Layout& D, int cast, bool heads = false)
 {
   if (S.cfg.num_layers != D.cfg.num_layers)  // executor/cuda.rs:52-58, memcpy.rs:49-55
     return fail(KVBM_ERR_INCOMPATIBLE, "Layouts have incompatible layer counts: src=" + std::to_string(S.cfg.num_layers) +
@@ -538,7 +540,11 @@ static int check_compat(const Layout& S, const Layout& D, int cast)
     return fail(KVBM_ERR_INCOMPATIBLE, "Layouts have incompatible outer dimensions: src=" + std::to_string(S.cfg.outer_dim) +
                                            ", dst=" + std::to_string(D.cfg.outer_dim));
   const size_t num = cast == KVBM_CAST_FP8E4M3_TO_BF16 ? 2 : 1, den = cast == KVBM_CAST_BF16_TO_FP8E4M3 ? 2 : 1;
-  if (S.region * num != D.region * den)
+  if (heads) {
+    const size_t s_row = S.cfg.inner_dim / S.cfg.num_heads * S.cfg.dtype_width_bytes, d_row = D.cfg.inner_dim / D.cfg.num_heads * D.cfg.dtype_width_bytes;
+    if (s_row * num != d_row * den)
+      return fail(KVBM_ERR_INCOMPATIBLE, "Head row size mismatch: src=" + std::to_string(s_row) + ", dst=" + std::to_string(d_row));
+  } else if (S.region * num != D.region * den)
     return fail(KVBM_ERR_INCOMPATIBLE, "Memory region size mismatch: src=" + std::to_string(S.region) + ", dst=" + std::to_string(D.region));
   if (cast == KVBM_CAST_FP8E4M3_TO_BF16 && (S.cfg.dtype_width_bytes != 1 || D.cfg.dtype_width_bytes != 2))
     return fail(KVBM_ERR_INCOMPATIBLE, "fp8->bf16 cast needs dtype widths 1 -> 2");
@@ -612,11 +618,11 @@ static int launch_cuda(kvbm_transfer_manager* m, Layout* S, Layout* const* D, in
 }
 
 // The layout-transforming transfer: what select_transform_kernel's result would drive if the reference ran it inside
-// execute_transfer (it rejects the pair instead, transfer/mod.rs:128-147).  One kvbm_kernels_paged_permute_cast launch, with the
-// transfer's fp8 <-> bf16 cast fused in: block tables uploaded like launch_cuda's, no pointer tables, completion word written by a
-// trailing signal kernel.
+// execute_transfer (it rejects the pair instead, transfer/mod.rs:128-147).  One kvbm_kernels_paged_permute_heads launch, with the
+// transfer's fp8 <-> bf16 cast fused in and, when `window`, only the options' head window moved: block tables uploaded like
+// launch_cuda's, no pointer tables, completion word written by a trailing signal kernel.
 static int launch_transform(kvbm_transfer_manager* m, Layout* S, Layout* D, int src_kv, int dst_kv, const size_t* src_ids,
-                            const size_t* dst_ids, size_t n, size_t lb, size_t le, const kvbm_transfer_options& o,
+                            const size_t* dst_ids, size_t n, size_t lb, size_t le, const kvbm_transfer_options& o, bool window,
                             cudaStream_t stream, Slot** slot_out, uint64_t* seq_out)
 {
   Slot* sl;
@@ -630,16 +636,18 @@ static int launch_transform(kvbm_transfer_manager* m, Layout* S, Layout* D, int 
   CU(cudaMemcpyAsync(sl->dev_ids, sl->pinned_ids, 2 * n * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
   m->h2d_bytes += 2 * n * sizeof(int32_t);
   kvbm_permute_side ps{descriptor(*S), sl->dev_ids, src_kv}, pd{descriptor(*D), sl->dev_ids + n, dst_kv};
-  const size_t nh = S->cfg.num_heads;
-  const size_t row = S->cfg.inner_dim / nh * S->cfg.dtype_width_bytes;
-  cudaError_t e = kvbm_kernels_paged_permute_cast(&ps, &pd, static_cast<int>(n), static_cast<int>(lb), static_cast<int>(le),
-                                                  static_cast<uint32_t>(nh), static_cast<uint32_t>(S->cfg.page_size),
-                                                  static_cast<uint32_t>(row), o.cast_mode, o.done_flag, o.epoch, sl->host_flag,
-                                                  static_cast<uint32_t>(seq), stream);
-  if (e != cudaSuccess) return fail_cuda(e, "kvbm_kernels_paged_permute_cast");
+  const size_t snh = S->cfg.num_heads, dnh = D->cfg.num_heads;
+  const size_t sb = window ? o.src_head_begin : 0, db = window ? o.dst_head_begin : 0, k = window ? o.head_count : snh;
+  const size_t row = S->cfg.inner_dim / snh * S->cfg.dtype_width_bytes;
+  cudaError_t e = kvbm_kernels_paged_permute_heads(&ps, &pd, static_cast<int>(n), static_cast<int>(lb), static_cast<int>(le),
+                                                   static_cast<uint32_t>(snh), static_cast<uint32_t>(sb), static_cast<uint32_t>(dnh),
+                                                   static_cast<uint32_t>(db), static_cast<uint32_t>(k), static_cast<uint32_t>(S->cfg.page_size),
+                                                   static_cast<uint32_t>(row), o.cast_mode, o.done_flag, o.epoch, sl->host_flag,
+                                                   static_cast<uint32_t>(seq), stream);
+  if (e != cudaSuccess) return fail_cuda(e, "kvbm_kernels_paged_permute_heads");
   CU(cudaEventRecord(sl->ev, stream));
   sl->in_flight = true;
-  m->bytes_moved += n * (le - lb) * S->cfg.outer_dim * D->region;
+  m->bytes_moved += n * (le - lb) * S->cfg.outer_dim * (D->region / dnh * k);
   *slot_out = sl;
   *seq_out = seq;
   return KVBM_OK;
@@ -708,11 +716,25 @@ static int execute(kvbm_transfer_manager* m, kvbm_layout_handle src_h, int nd, c
   if (!S) return fail(KVBM_ERR_HANDLE, "invalid source handle");
   if (S->unmapped) return fail(KVBM_ERR_UNSUPPORTED, "source layout is a descriptor of another process's host memory: not addressable from this process");
   std::vector<Layout*> D(nd);
+  bool window = false;
   for (int d = 0; d < nd; ++d) {
     D[d] = m->find(dst_h[d]);
     if (!D[d]) return fail(KVBM_ERR_HANDLE, "invalid destination handle");
     if (D[d]->unmapped) return fail(KVBM_ERR_UNSUPPORTED, "destination layout is a descriptor of another process's host memory: not addressable from this process");
-    int rc = check_compat(*S, *D[d], o.cast_mode);
+    if (o.head_count) {  // a head window (TP re-shard): both head counts known, the window inside both
+      if (nd != 1) return fail(KVBM_ERR_UNSUPPORTED, "a layout-transforming transfer takes one destination");
+      const kvbm_layout_config &sc = S->cfg, &dc = D[d]->cfg;
+      if (!sc.num_heads || !dc.num_heads) return fail(KVBM_ERR_CONFIG, "num_heads_required_for_kv_block_layout");  // config.rs:118-126
+      if (sc.inner_dim % sc.num_heads || dc.inner_dim % dc.num_heads) return fail(KVBM_ERR_CONFIG, "inner_dim_must_be_divisible_by_num_heads");
+      if (o.src_head_begin > sc.num_heads || o.head_count > sc.num_heads - o.src_head_begin || o.dst_head_begin > dc.num_heads ||
+          o.head_count > dc.num_heads - o.dst_head_begin)
+        return fail(KVBM_ERR_RANGE, "Head window src " + std::to_string(o.src_head_begin) + "+" + std::to_string(o.head_count) + " of " +
+                                        std::to_string(sc.num_heads) + " heads, dst " + std::to_string(o.dst_head_begin) + "+" +
+                                        std::to_string(o.head_count) + " of " + std::to_string(dc.num_heads) + " heads is out of range");
+      // a window over every head of both sides is the transfer without one
+      window = !(o.src_head_begin == 0 && o.dst_head_begin == 0 && o.head_count == sc.num_heads && o.head_count == dc.num_heads);
+    }
+    int rc = check_compat(*S, *D[d], o.cast_mode, window);
     if (rc) return rc;
     if (n && (!src_ids || !dst_ids || !src_ids[d] || !dst_ids[d])) return fail(KVBM_ERR, "null block id list");
     rc = validate_block_transfer(src_ids[d], n, dst_ids[d], n, S->cfg.num_blocks, D[d]->cfg.num_blocks, src_h == dst_h[d]);
@@ -731,17 +753,22 @@ static int execute(kvbm_transfer_manager* m, kvbm_layout_handle src_h, int nd, c
     if (t == KVBM_TRANSFORM_UNSUPPORTED && (src_kv == KVBM_KV_UNIVERSAL_TP || src_kv == KVBM_KV_UNIVERSAL_PP) &&
         (dst_kv == KVBM_KV_UNIVERSAL_TP || dst_kv == KVBM_KV_UNIVERSAL_PP))
       t = KVBM_TRANSFORM_UNIVERSAL_TO_UNIVERSAL;
-    if (t == KVBM_TRANSFORM_UNSUPPORTED)
+    // a head window walks heads by the formats' strides, so both formats must be named ones
+    if (t == KVBM_TRANSFORM_UNSUPPORTED || (window && (!kv_known(src_kv) || !kv_known(dst_kv))))
       return fail(KVBM_ERR_UNSUPPORTED, std::string("Layout transformation not supported: src=") + kv_name(src_kv) + ", dst=" + kv_name(dst_kv));
-    if (t != KVBM_TRANSFORM_NONE) {
+    if (t != KVBM_TRANSFORM_NONE || window) {  // a head window takes the permuting launch even between equal formats
       if (nd != 1) return fail(KVBM_ERR_UNSUPPORTED, "a layout-transforming transfer takes one destination");
       if (o.layer_ready_flags || o.layer_done_flags || o.per_dst_done_flags || o.per_dst_layer_done_flags || o.multicast)
         return fail(KVBM_ERR_UNSUPPORTED, "layer streaming / multicast are not available on a layout-transforming transfer");
       const kvbm_layout_config &sc = S->cfg, &dc = D[d]->cfg;
       if (!sc.num_heads || !dc.num_heads) return fail(KVBM_ERR_CONFIG, "num_heads_required_for_kv_block_layout");  // config.rs:118-126
       // with the fused cast the dtype widths differ as check_compat requires (1 -> 2 or 2 -> 1)
-      if (sc.num_heads != dc.num_heads || sc.page_size != dc.page_size || sc.inner_dim != dc.inner_dim ||
-          (o.cast_mode == KVBM_CAST_NONE && sc.dtype_width_bytes != dc.dtype_width_bytes))
+      if (window) {  // the head counts may differ; the heads themselves may not
+        if (sc.page_size != dc.page_size || sc.inner_dim / sc.num_heads != dc.inner_dim / dc.num_heads ||
+            (o.cast_mode == KVBM_CAST_NONE && sc.dtype_width_bytes != dc.dtype_width_bytes))
+          return fail(KVBM_ERR_INCOMPATIBLE, "a head-window transfer needs equal head_dim, page_size and dtype on both sides");
+      } else if (sc.num_heads != dc.num_heads || sc.page_size != dc.page_size || sc.inner_dim != dc.inner_dim ||
+                 (o.cast_mode == KVBM_CAST_NONE && sc.dtype_width_bytes != dc.dtype_width_bytes))
         return fail(KVBM_ERR_INCOMPATIBLE, "a layout transformation needs equal num_heads, page_size, inner_dim and dtype on both sides");
       if (sc.inner_dim % sc.num_heads) return fail(KVBM_ERR_CONFIG, "inner_dim_must_be_divisible_by_num_heads");
       const size_t head_dim = sc.inner_dim / sc.num_heads;
@@ -768,6 +795,7 @@ static int execute(kvbm_transfer_manager* m, kvbm_layout_handle src_h, int nd, c
     }
     transform = t;
   }
+  const bool permute = transform != KVBM_TRANSFORM_NONE || window;
   const int dst_kv0 = o.dst_kv_layout ? o.dst_kv_layout : D[0]->kv_block_layout;
   size_t lb = 0, le = S->cfg.num_layers;
   if (o.has_layer_range) {
@@ -799,7 +827,7 @@ static int execute(kvbm_transfer_manager* m, kvbm_layout_handle src_h, int nd, c
     if (nd != 1) return fail(KVBM_ERR_UNSUPPORTED, "two-hop transfers take one destination");
     if (o.use_caller_stream) return fail(KVBM_ERR_UNSUPPORTED, "Two-hop transfers don't support caller-provided streams");  // executor/mod.rs:441
     if (o.cast_mode != KVBM_CAST_NONE) return fail(KVBM_ERR_UNSUPPORTED, "the fused cast is not available on two-hop transfers");
-    if (transform != KVBM_TRANSFORM_NONE) return fail(KVBM_ERR_UNSUPPORTED, "a layout transformation is not available on two-hop transfers");
+    if (permute) return fail(KVBM_ERR_UNSUPPORTED, "a layout transformation is not available on two-hop transfers");
     if (!o.bounce_layout || !o.bounce_block_ids || o.num_bounce_blocks == 0)
       return fail(KVBM_ERR, "Two-hop transfers require a bounce buffer.");  // executor/mod.rs:514-519
     Layout* B = m->find(o.bounce_layout);
@@ -819,7 +847,7 @@ static int execute(kvbm_transfer_manager* m, kvbm_layout_handle src_h, int nd, c
 
   if (plan.first == KVBM_STRATEGY_MEMCPY) {
     if (o.cast_mode != KVBM_CAST_NONE) return fail(KVBM_ERR_UNSUPPORTED, "the fused cast exists only on the CUDA strategies");
-    if (transform != KVBM_TRANSFORM_NONE) return fail(KVBM_ERR_UNSUPPORTED, "layout transformations exist only on the CUDA strategies");
+    if (permute) return fail(KVBM_ERR_UNSUPPORTED, "layout transformations exist only on the CUDA strategies");
     if (o.use_caller_stream) return fail(KVBM_ERR_UNSUPPORTED, "cuda_stream option is not supported for Memcpy strategy");  // executor/mod.rs:272-276
     for (int d = 0; d < nd; ++d) {
       int rc = host_memcpy_transfer(*S, *D[d], src_ids[d], dst_ids[d], n, o.has_layer_range != 0, lb, le);
@@ -843,8 +871,8 @@ static int execute(kvbm_transfer_manager* m, kvbm_layout_handle src_h, int nd, c
     stream = m->h2d[m->rr_h2d++ % kStreams];
   Slot* sl;
   uint64_t seq;
-  int rc = transform != KVBM_TRANSFORM_NONE ? launch_transform(m, S, D[0], src_kv, dst_kv0, src_ids[0], dst_ids[0], n, lb, le, o, stream, &sl, &seq)
-                                            : launch_cuda(m, S, D.data(), nd, src_ids, dst_ids, n, replicate, lb, le, o, stream, nullptr, &sl, &seq);
+  int rc = permute ? launch_transform(m, S, D[0], src_kv, dst_kv0, src_ids[0], dst_ids[0], n, lb, le, o, window, stream, &sl, &seq)
+                   : launch_cuda(m, S, D.data(), nd, src_ids, dst_ids, n, replicate, lb, le, o, stream, nullptr, &sl, &seq);
   if (rc) return rc;
   // caller-provided stream: caller manages sync, completed() is returned (cuda.rs:139-141)
   if (out) *out = o.use_caller_stream ? 0 : seq;
@@ -1343,6 +1371,38 @@ extern "C" int kvbm_manager_kv_block_layout(kvbm_transfer_manager* m, kvbm_layou
 
 extern "C" int kvbm_select_transform_kernel(int src_kv_layout, int dst_kv_layout) { return select_transform_kernel(src_kv_layout, dst_kv_layout); }
 extern "C" int kvbm_kv_layout_requires_transform(int a, int b) { return kv_requires_transform(a, b) ? 1 : 0; }
+
+extern "C" int kvbm_tp_reshard_plan(size_t num_kv_heads, size_t src_tp, size_t dst_tp, size_t dst_rank, kvbm_head_window* out, size_t cap,
+                                    size_t* n_out)
+{
+  const size_t H = num_kv_heads;
+  if (!n_out) return fail(KVBM_ERR, "null argument");
+  *n_out = 0;
+  if (!H || !src_tp || !dst_tp) return fail(KVBM_ERR_CONFIG, "num_kv_heads, src_tp and dst_tp must be positive");
+  for (size_t tp : {src_tp, dst_tp})
+    if (H % tp && tp % H)
+      return fail(KVBM_ERR_CONFIG, std::to_string(H) + " KV heads cannot be sharded over TP " + std::to_string(tp) +
+                                       ": one of the two must divide the other");
+  if (dst_rank >= dst_tp) return fail(KVBM_ERR_RANGE, "dst_rank " + std::to_string(dst_rank) + " out of range for TP " + std::to_string(dst_tp));
+  // vLLM's ownership: rank r of tp holds heads [r*H/tp, r*H/tp + max(1, H/tp)); replicated over tp/H ranks when tp > H
+  const size_t d_first = dst_rank * H / dst_tp, d_count = std::max<size_t>(1, H / dst_tp);
+  const size_t s_per = std::max<size_t>(1, H / src_tp), replicas = src_tp > H ? src_tp / H : 1;
+  std::vector<kvbm_head_window> w;
+  for (size_t j = 0; j < d_count; ++j) {
+    const size_t g = d_first + j;  // global head
+    const size_t rank = replicas > 1 ? g * replicas + dst_rank % replicas : g / s_per;
+    const size_t local = g - rank * H / src_tp;
+    if (!w.empty() && w.back().src_rank == rank && w.back().src_head_begin + w.back().head_count == local)
+      ++w.back().head_count;
+    else
+      w.push_back({rank, local, j, 1});
+  }
+  *n_out = w.size();
+  if (!out) return KVBM_OK;
+  if (cap < w.size()) return fail(KVBM_ERR, "kvbm_tp_reshard_plan: " + std::to_string(w.size()) + " windows do not fit in " + std::to_string(cap));
+  std::copy(w.begin(), w.end(), out);
+  return KVBM_OK;
+}
 
 extern "C" int kvbm_manager_set_capabilities(kvbm_transfer_manager* m, const kvbm_transfer_capabilities* caps)
 {

@@ -533,21 +533,22 @@ __device__ __forceinline__ void cast_vector_down(const uint4 (&in)[2], uint4 (&o
   out[0] = make_uint4(o[0], o[1], o[2], o[3]);
 }
 
-// One unit: every head of it, one warp per head.  sb / db: the unit's bases; both must be 16 B aligned.  The last batch of
+// One unit: heads h0, h0 + hstep, ... < nh of it, one warp per head (h0 = the warp, hstep = the CTA's warps when a CTA
+// walks one unit).  sb / db: the unit's bases; both must be 16 B aligned.  The last batch of
 // a head is predicated rather than a serial tail: for head_dim 64 ... 96 in bf16 it is the whole head, and its loads stay
 // independent.  With a cast (KVBM_CAST_*) the walk counts 16 B vectors of the fp8 side's row: one vector is 16 elements,
 // 16 B on the fp8 side and 32 B on the bf16 side, so fp8 -> bf16 turns one load into two stores and bf16 -> fp8 two loads
 // into one store.  Every lane keeps 8 independent 16 B loads in flight in all three forms.
 template <int CAST, bool POW2>
 __device__ __forceinline__ void walk_head_rows(const uint8_t* sb, uint64_t s_head, uint32_t s_tok, uint8_t* db, uint64_t d_head,
-                                               uint32_t d_tok, uint32_t nh, uint32_t nt, const RowSplit& r)
+                                               uint32_t d_tok, uint32_t h0, uint32_t hstep, uint32_t nh, uint32_t nt, const RowSplit& r)
 {
   constexpr int IN = CAST == KVBM_CAST_BF16_TO_FP8E4M3 ? 2 : 1;   // 16 B loads per vector
   constexpr int OUT = CAST == KVBM_CAST_FP8E4M3_TO_BF16 ? 2 : 1;  // 16 B stores per vector
   constexpr int U = 8 / IN;
   const uint32_t run = row_run<POW2>(r, nt);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
-  for (uint32_t h = warp; h < nh; h += nwarps) {
+  const int lane = threadIdx.x & 31;
+  for (uint32_t h = h0; h < nh; h += hstep) {
     const uint8_t* sh = sb + h * s_head;
     uint8_t* dh = db + h * d_head;
     for (uint32_t v = lane; v < run; v += U * 32) {
@@ -597,7 +598,8 @@ kvbm_permute_table_kernel(void* const* __restrict__ universal_ptrs, void* const*
   const uint8_t* sb = base_of(S);
   uint8_t* db = base_of(D);
   if (((reinterpret_cast<uintptr_t>(sb) | reinterpret_cast<uintptr_t>(db)) & 15) == 0) {
-    walk_head_rows<KVBM_CAST_NONE, POW2>(sb, S.head_stride, S.tok_stride, db, D.head_stride, D.tok_stride, nh, nt, r);
+    walk_head_rows<KVBM_CAST_NONE, POW2>(sb, S.head_stride, S.tok_stride, db, D.head_stride, D.tok_stride, threadIdx.x >> 5, blockDim.x >> 5,
+                                         nh, nt, r);
     return;
   }
   const uint32_t per_vec = 16 / elem, n = row_run<POW2>(r, nt) * per_vec;
@@ -615,12 +617,15 @@ kvbm_permute_table_kernel(void* const* __restrict__ universal_ptrs, void* const*
 }
 
 // Paged permute: the walk with the bases computed from the pools' layouts and block tables instead of host-built pointer
-// tables, for any pair of KvBlockLayouts, optionally casting (CAST: KVBM_CAST_*; each side's strides are for its own row).
-// One CTA per (block pair, layer, outer).
+// tables, for any pair of KvBlockLayouts, optionally casting (CAST: KVBM_CAST_*; each side's strides are for its own row and
+// its own head count).  nh heads of every unit move: source heads from s_win / head_stride on, destination heads from
+// d_win / head_stride on (s_win, d_win: the head windows' byte offsets; 0 for every head of both sides).  One CTA per
+// (block pair, layer, outer), also for a window of one head: packing several units of a narrow window into one CTA measured
+// no faster (DESIGN §4.2b).
 template <int CAST, bool POW2>
 __global__ void __launch_bounds__(256)
 kvbm_paged_permute_kernel(const __grid_constant__ PermuteSide S, const __grid_constant__ PermuteSide D, uint32_t layer_begin,
-                          uint32_t nlayers, uint32_t no, uint32_t nh, uint32_t nt, RowSplit r)
+                          uint32_t nlayers, uint32_t no, uint32_t nh, uint32_t nt, RowSplit r, uint64_t s_win, uint64_t d_win)
 {
   const uint32_t unit = blockIdx.x;  // (pair * nlayers + l) * no + o
   const uint32_t pair = unit / (nlayers * no);
@@ -630,7 +635,8 @@ kvbm_paged_permute_kernel(const __grid_constant__ PermuteSide S, const __grid_co
     return reinterpret_cast<uint8_t*>(static_cast<uintptr_t>(__ldg(X.layer_base + (X.universal ? 0 : l)))) +
            static_cast<uint64_t>(__ldg(X.ids + pair)) * X.block_stride + l * X.layer_step + o * X.outer_step;
   };
-  walk_head_rows<CAST, POW2>(base_of(S), S.head_stride, S.tok_stride, base_of(D), D.head_stride, D.tok_stride, nh, nt, r);
+  walk_head_rows<CAST, POW2>(base_of(S) + s_win, S.head_stride, S.tok_stride, base_of(D) + d_win, D.head_stride, D.tok_stride,
+                             threadIdx.x >> 5, blockDim.x >> 5, nh, nt, r);
 }
 
 __global__ void kvbm_signal_kernel(uint32_t* a, uint32_t va, uint32_t* b, uint32_t vb)
@@ -943,6 +949,17 @@ kvbm_kernels_paged_permute_cast(const kvbm_permute_side* src, const kvbm_permute
                                 uint32_t* done_flag, uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value,
                                 cudaStream_t stream)
 {
+  return kvbm_kernels_paged_permute_heads(src, dst, num_blocks, layer_begin, layer_end, num_heads, 0, num_heads, 0, num_heads, page_size,
+                                          src_row_bytes, cast_mode, done_flag, epoch, completion_flag, completion_value, stream);
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_permute_heads(const kvbm_permute_side* src, const kvbm_permute_side* dst, int num_blocks, int layer_begin,
+                                 int layer_end, uint32_t src_num_heads, uint32_t src_head_begin, uint32_t dst_num_heads,
+                                 uint32_t dst_head_begin, uint32_t head_count, uint32_t page_size, uint32_t src_row_bytes, int cast_mode,
+                                 uint32_t* done_flag, uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value,
+                                 cudaStream_t stream)
+{
   if (num_blocks < 0 || layer_begin < 0 || layer_end < layer_begin) return cudaErrorInvalidValue;
   if (cast_mode < KVBM_CAST_NONE || cast_mode > KVBM_CAST_BF16_TO_FP8E4M3) return cudaErrorInvalidValue;
   const bool signal = done_flag || completion_flag;
@@ -963,19 +980,22 @@ kvbm_kernels_paged_permute_cast(const kvbm_permute_side* src, const kvbm_permute
                                                                           : src_row_bytes;
   const uint64_t walk_row = cast_mode == KVBM_CAST_BF16_TO_FP8E4M3 ? dst_row_bytes : src_row_bytes;
   RowSplit r;
-  if (num_heads == 0 || page_size == 0 || !row_split(walk_row, page_size, &r)) return cudaErrorInvalidValue;
-  const uint64_t rows = static_cast<uint64_t>(page_size) * num_heads;
-  if (rows * src_row_bytes != src->layout.region_bytes || rows * dst_row_bytes != dst->layout.region_bytes) return cudaErrorInvalidValue;
+  if (head_count == 0 || page_size == 0 || !row_split(walk_row, page_size, &r)) return cudaErrorInvalidValue;
+  if (static_cast<uint64_t>(src_head_begin) + head_count > src_num_heads || static_cast<uint64_t>(dst_head_begin) + head_count > dst_num_heads)
+    return cudaErrorInvalidValue;
+  const uint64_t s_rows = static_cast<uint64_t>(page_size) * src_num_heads, d_rows = static_cast<uint64_t>(page_size) * dst_num_heads;
+  if (s_rows * src_row_bytes != src->layout.region_bytes || d_rows * dst_row_bytes != dst->layout.region_bytes) return cudaErrorInvalidValue;
   PermuteSide S, D;
-  if (!fill_permute_side(*src, nl, no, num_heads, page_size, src_row_bytes, &S) ||
-      !fill_permute_side(*dst, nl, no, num_heads, page_size, static_cast<uint32_t>(dst_row_bytes), &D))
+  if (!fill_permute_side(*src, nl, no, src_num_heads, page_size, src_row_bytes, &S) ||
+      !fill_permute_side(*dst, nl, no, dst_num_heads, page_size, static_cast<uint32_t>(dst_row_bytes), &D))
     return cudaErrorInvalidValue;
   const uint64_t units = static_cast<uint64_t>(num_blocks) * (layer_end - layer_begin) * no;
   if (units >= (1ull << 31)) return cudaErrorInvalidValue;
-  const int threads = static_cast<int>(std::min<uint32_t>(8, num_heads)) * 32;
+  const int threads = static_cast<int>(std::min<uint32_t>(8, head_count)) * 32;
   const unsigned grid = static_cast<unsigned>(units);
   const uint32_t lb = static_cast<uint32_t>(layer_begin), nlay = static_cast<uint32_t>(layer_end - layer_begin);
-  auto go = [&](auto kern) { kern<<<grid, threads, 0, stream>>>(S, D, lb, nlay, no, num_heads, page_size, r); };
+  const uint64_t s_win = src_head_begin * S.head_stride, d_win = dst_head_begin * D.head_stride;  // the windows' first heads
+  auto go = [&](auto kern) { kern<<<grid, threads, 0, stream>>>(S, D, lb, nlay, no, head_count, page_size, r, s_win, d_win); };
   switch (cast_mode) {
     case KVBM_CAST_NONE:
       r.pow2 ? go(kvbm_paged_permute_kernel<KVBM_CAST_NONE, true>) : go(kvbm_paged_permute_kernel<KVBM_CAST_NONE, false>);

@@ -152,6 +152,10 @@ def lib() -> C.CDLL:
         L.kvbm_kernels_paged_permute_cast.argtypes = [C.POINTER(PermuteSide), C.POINTER(PermuteSide), i, i, i, C.c_uint32, C.c_uint32,
                                                       C.c_uint32, i, vp, C.c_uint32, vp, C.c_uint32, vp]
         L.kvbm_kernels_paged_permute_cast.restype = i
+        L.kvbm_kernels_paged_permute_heads.argtypes = [C.POINTER(PermuteSide), C.POINTER(PermuteSide), i, i, i, C.c_uint32, C.c_uint32,
+                                                       C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, i, vp, C.c_uint32, vp,
+                                                       C.c_uint32, vp]
+        L.kvbm_kernels_paged_permute_heads.restype = i
         L.kvbm_kernels_permute_strides.argtypes = [i, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64, C.c_uint64,
                                                    C.POINTER(C.c_uint64)]
         L.kvbm_kernels_permute_strides.restype = i
@@ -173,7 +177,7 @@ EXPORTED_SYMBOLS = [
     "kvbm_kernels_has_memcpy_batch_async", "kvbm_kernels_is_stub_build",
     "kvbm_kernels_paged_copy_v2", "kvbm_kernels_set_flags", "kvbm_kernels_wait_flag", "kvbm_kernels_stream_wait_event",
     "kvbm_kernels_launch_count", "kvbm_kernels_build_info", "kvbm_kernels_gate_would_spin", "kvbm_kernels_paged_permute",
-    "kvbm_kernels_permute_strides", "kvbm_kernels_paged_permute_cast",
+    "kvbm_kernels_permute_strides", "kvbm_kernels_paged_permute_cast", "kvbm_kernels_paged_permute_heads",
 ]
 
 GATE_AUTO, GATE_SPIN, GATE_STREAM_WAIT = 0, 1, 2
@@ -245,6 +249,18 @@ def paged_permute_cast(src: PermuteSide, dst: PermuteSide, num_blocks: int, laye
     return lib().kvbm_kernels_paged_permute_cast(C.byref(src), C.byref(dst), num_blocks, layer_begin, layer_end, num_heads, page_size,
                                                  src_row_bytes, int(cast_mode), done_flag or None, epoch, completion_flag or None,
                                                  completion_value, stream)
+
+
+def paged_permute_heads(src: PermuteSide, dst: PermuteSide, num_blocks: int, layer_begin: int, layer_end: int, src_num_heads: int,
+                        src_head_begin: int, dst_num_heads: int, dst_head_begin: int, head_count: int, page_size: int, src_row_bytes: int,
+                        cast_mode: int = 0, done_flag: int = 0, epoch: int = 0, completion_flag: int = 0, completion_value: int = 0,
+                        stream: int = 0) -> int:
+    """`paged_permute_cast` over a head window on each side (a TP re-shard): source heads [src_head_begin, +head_count) land as
+    destination heads [dst_head_begin, +head_count); each side has its own head count and every destination byte outside the
+    window keeps its value.  include/kvbm_kernels.h (kvbm_kernels_paged_permute_heads)."""
+    return lib().kvbm_kernels_paged_permute_heads(C.byref(src), C.byref(dst), num_blocks, layer_begin, layer_end, src_num_heads,
+                                                  src_head_begin, dst_num_heads, dst_head_begin, head_count, page_size, src_row_bytes,
+                                                  int(cast_mode), done_flag or None, epoch, completion_flag or None, completion_value, stream)
 
 
 def permute_strides(kv_layout: int, num_layers: int, outer_dim: int, num_heads: int, page_size: int, row_bytes: int,

@@ -17,8 +17,9 @@ from __future__ import annotations
 
 import ctypes as C
 import enum
+import dataclasses
 from dataclasses import dataclass
-from typing import List, Optional, Sequence
+from typing import List, Mapping, Optional, Sequence, Union
 
 from . import _lib, kernels
 
@@ -105,7 +106,14 @@ class _COptions(C.Structure):
         ("gate_mode", C.c_int),
         ("per_dst_done_flags", C.c_void_p),
         ("per_dst_layer_done_flags", C.c_void_p),
+        ("src_head_begin", C.c_size_t),
+        ("dst_head_begin", C.c_size_t),
+        ("head_count", C.c_size_t),
     ]
+
+
+class _CHeadWindow(C.Structure):
+    _fields_ = [(n, C.c_size_t) for n in ("src_rank", "src_head_begin", "dst_head_begin", "head_count")]
 
 
 @dataclass
@@ -155,6 +163,7 @@ class TransferOptions:
     gate_mode: int = 0                    # kernels.GATE_AUTO / GATE_SPIN / GATE_STREAM_WAIT
     per_dst_done_flags: Optional[Sequence[int]] = None        # fan-out: one done-flag address per destination (0 = none)
     per_dst_layer_done_flags: Optional[Sequence[int]] = None  # fan-out: one layer-done array address per destination
+    head_window: Optional[tuple] = None   # (src_head_begin, dst_head_begin, head_count): move only these heads (TP re-shard)
 
     @staticmethod
     def from_layer_range(layer_range: Optional[range]) -> "TransferOptions":
@@ -167,12 +176,13 @@ class TransferOptions:
             bl, ids = self.bounce_buffer
             self._bounce_keepalive = (C.c_size_t * max(1, len(ids)))(*[int(x) for x in ids])
             bids, nb = C.cast(self._bounce_keepalive, C.c_void_p), len(ids)
+        sb, db, k = self.head_window if self.head_window is not None else (0, 0, 0)
         return _COptions(int(lr is not None), lr.start if lr is not None else 0, lr.stop if lr is not None else 0,
                          self.cuda_stream or 0, int(self.cuda_stream is not None), int(self.cast_mode), self.max_ctas,
                          self.layer_ready_flags, self.layer_done_flags, self.epoch, self.gate_timeout_ms,
                          int(self.multicast), self.done_flag, int(bl), bids, nb, int(self.src_kv_layout),
                          int(self.dst_kv_layout), int(self.gate_mode), self._ptr_array("_pd", self.per_dst_done_flags),
-                         self._ptr_array("_pl", self.per_dst_layer_done_flags))
+                         self._ptr_array("_pl", self.per_dst_layer_done_flags), int(sb), int(db), int(k))
 
     def _ptr_array(self, keep: str, ptrs):
         if ptrs is None:
@@ -206,7 +216,7 @@ EXPORTED_SYMBOLS = [
     "kvbm_select_direct_strategy_remote", "kvbm_select_strategy", "kvbm_manager_select_strategy",
     "kvbm_mc_supported", "kvbm_mc_group_create", "kvbm_mc_group_export_fd", "kvbm_mc_group_import_fd",
     "kvbm_mc_group_size", "kvbm_mc_group_add_device", "kvbm_mc_group_bind_local", "kvbm_mc_group_bind_addr", "kvbm_mc_group_map",
-    "kvbm_mc_group_destroy",
+    "kvbm_mc_group_destroy", "kvbm_tp_reshard_plan",
 ]
 
 
@@ -253,6 +263,7 @@ def lib() -> C.CDLL:
         L.kvbm_manager_kv_block_layout.argtypes = [vp, u64]
         L.kvbm_select_transform_kernel.argtypes = [i, i]
         L.kvbm_kv_layout_requires_transform.argtypes = [i, i]
+        L.kvbm_tp_reshard_plan.argtypes = [sz, sz, sz, sz, P(_CHeadWindow), sz, P(sz)]
         L.kvbm_notification_is_complete.argtypes = [vp, u64]
         L.kvbm_notification_wait.argtypes = [vp, u64, C.c_int64]
         L.kvbm_manager_bytes_moved.argtypes = [vp]
@@ -364,6 +375,27 @@ def validate_block_transfer(src_ids: Sequence[int], dst_ids: Sequence[int], src_
     s, ns = _size_array(src_ids)
     d, nd = _size_array(dst_ids)
     _check(lib().kvbm_validate_block_transfer(s, ns, d, nd, src_num_blocks, dst_num_blocks, int(same_layout)))
+
+
+@dataclass(frozen=True)
+class HeadWindow:
+    """One entry of a TP re-shard plan: heads [src_head_begin, +head_count) of source rank src_rank's blocks are heads
+    [dst_head_begin, +head_count) of the decode rank's blocks (rank-local indices)."""
+    src_rank: int
+    src_head_begin: int
+    dst_head_begin: int
+    head_count: int
+
+
+def tp_reshard_plan(num_kv_heads: int, src_tp: int, dst_tp: int, dst_rank: int) -> List[HeadWindow]:
+    """Which source rank supplies which heads of decode rank `dst_rank` (kvbm_tp_reshard_plan, include/kvbm_physical.h): vLLM's
+    head ownership on both sides, replica dst_rank % replicas of a replicated source head, ascending destination heads, adjacent
+    heads of one source merged."""
+    n = C.c_size_t()
+    _check(lib().kvbm_tp_reshard_plan(num_kv_heads, src_tp, dst_tp, dst_rank, None, 0, C.byref(n)))
+    out = (_CHeadWindow * max(1, n.value))()
+    _check(lib().kvbm_tp_reshard_plan(num_kv_heads, src_tp, dst_tp, dst_rank, out, n.value, C.byref(n)))
+    return [HeadWindow(w.src_rank, w.src_head_begin, w.dst_head_begin, w.head_count) for w in out[:n.value]]
 
 
 class TransferCompleteNotification:
@@ -526,6 +558,25 @@ class TransferManager:
         if rc:
             _check(rc)
         return TransferCompleteNotification(self, tok.value)
+
+    def execute_reshard(self, sources: Mapping[int, tuple], dst: int, dst_block_ids: Sequence[int], plan: Sequence[HeadWindow],
+                        options: Union[None, TransferOptions, Sequence[TransferOptions]] = None) -> List[TransferCompleteNotification]:
+        """Assemble blocks of a decode rank from the source ranks' blocks, one `execute_transfer` with a head window per plan entry
+        (`tp_reshard_plan`).  `sources` maps a source rank to (layout handle, block ids); `dst_block_ids[i]` receives head
+        windows of each source's block i.  The windows of one destination block are byte-disjoint, so the transfers may run on
+        different manager streams at once.  `options` is applied to every entry, or is one TransferOptions per entry -- the way to
+        give each entry its own done_flag (there is no combined flag).  Returns one notification per entry."""
+        per = list(options) if isinstance(options, (list, tuple)) else [options] * len(plan)
+        if len(per) != len(plan):
+            raise ValueError(f"{len(per)} options for {len(plan)} plan entries")
+        if len(plan) > 1 and not isinstance(options, (list, tuple)) and options is not None and options.done_flag:
+            raise ValueError("one done_flag would be written by every entry of the plan: pass one TransferOptions per entry")
+        notes = []
+        for w, o in zip(plan, per):
+            h, ids = sources[w.src_rank]
+            o = dataclasses.replace(o or TransferOptions(), head_window=(w.src_head_begin, w.dst_head_begin, w.head_count))
+            notes.append(self.execute_transfer(h, ids, dst, dst_block_ids, o))
+        return notes
 
     def execute_fanout(self, src: int, dsts: Sequence[int], src_block_ids: Sequence[Sequence[int]],
                        dst_block_ids: Sequence[Sequence[int]], replicate: bool = False,

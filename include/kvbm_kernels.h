@@ -218,6 +218,21 @@ cudaError_t kvbm_kernels_paged_permute_cast(const kvbm_permute_side* src, const 
                                             uint32_t src_row_bytes, int cast_mode, uint32_t* done_flag, uint32_t epoch,
                                             uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream);
 
+/* kvbm_kernels_paged_permute_cast over a head window on each side (a tensor-parallel re-shard): head src_head_begin + j of
+ * source block src->block_ids[i] lands as head dst_head_begin + j of destination block dst->block_ids[i], for j < head_count,
+ * every layer of [layer_begin, layer_end), every outer index and token, re-ordered from the source format to the destination
+ * format and cast as cast_mode says.  Every destination byte outside the window keeps its value.  Each side has its own head
+ * count: its region_bytes must be page_size * its num_heads * its row, and its strides are those of its own head count.
+ * head_count == 0 or a window past either side's num_heads is cudaErrorInvalidValue; every other rule (rows, cast, strides,
+ * grid bounds, the zero-count early return that still signals) is kvbm_kernels_paged_permute_cast's, which is this call with
+ * the full window (begin 0, count num_heads on both sides). */
+cudaError_t kvbm_kernels_paged_permute_heads(const kvbm_permute_side* src, const kvbm_permute_side* dst, int num_blocks,
+                                             int layer_begin, int layer_end, uint32_t src_num_heads, uint32_t src_head_begin,
+                                             uint32_t dst_num_heads, uint32_t dst_head_begin, uint32_t head_count,
+                                             uint32_t page_size, uint32_t src_row_bytes, int cast_mode, uint32_t* done_flag,
+                                             uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value,
+                                             cudaStream_t stream);
+
 /* Host-only (no GPU): the stride table kvbm_kernels_paged_permute walks with for one side.  out[0] = 1 when offsets count
  * from the block's first byte (universal formats) or 0 when they count from the (layer, outer) region's first byte; the
  * element (layer l, outer o, head h, token t) then sits at  [out[0] ? l * out[1] + o * out[2] : 0] + h * out[3] + t * out[4].

@@ -122,6 +122,11 @@ typedef struct kvbm_transfer_options {
    * the one multicast write -- what a staged broadcast needs (disagg.StagedBroadcast). */
   uint32_t* const* per_dst_done_flags;
   uint32_t* const* per_dst_layer_done_flags;
+  /* head window (tensor-parallel re-shard): heads [src_head_begin, src_head_begin + head_count) of each source block land as
+   * heads [dst_head_begin, dst_head_begin + head_count) of its destination block; every other destination byte keeps its
+   * value.  head_count 0 = every head (no window).  The two layouts may have different num_heads; see
+   * kvbm_manager_execute_transfer for the rules. */
+  size_t src_head_begin, dst_head_begin, head_count;
 } kvbm_transfer_options;
 
 typedef struct kvbm_transfer_manager kvbm_transfer_manager;
@@ -149,6 +154,21 @@ int kvbm_select_strategy(int src_kind, int src_is_local, int dst_kind, int dst_i
 /* validate_block_transfer, debug flavour (validation.rs:168-225). */
 int kvbm_validate_block_transfer(const size_t* src_ids, size_t n_src, const size_t* dst_ids, size_t n_dst,
                                  size_t src_num_blocks, size_t dst_num_blocks, int same_layout);
+
+/* One entry of a tensor-parallel re-shard plan: heads [src_head_begin, src_head_begin + head_count) of source rank src_rank's
+ * blocks are heads [dst_head_begin, dst_head_begin + head_count) of the decode rank's blocks (rank-local head indices). */
+typedef struct kvbm_head_window {
+  size_t src_rank, src_head_begin, dst_head_begin, head_count;
+} kvbm_head_window;
+/* Which source rank supplies which heads of decode rank dst_rank when num_kv_heads KV heads are sharded over src_tp ranks on
+ * the source side and dst_tp on the destination side.  Ownership follows vLLM: with tp ranks and H heads, rank r holds heads
+ * [r*H/tp, r*H/tp + max(1, H/tp)); when tp > H each head is replicated over tp/H ranks and the plan reads replica
+ * dst_rank % (tp/H), so concurrent pulls of different decode ranks spread over the source GPUs.  Windows come out in ascending
+ * destination head order; adjacent heads from the same source rank are merged.  H % tp or tp % H must be 0 on both sides
+ * (else KVBM_ERR_CONFIG, as is a zero argument); dst_rank >= dst_tp is KVBM_ERR_RANGE.  *n_out receives the number of
+ * windows; out == NULL only counts, a cap below the count is KVBM_ERR.  Pure host logic. */
+int kvbm_tp_reshard_plan(size_t num_kv_heads, size_t src_tp, size_t dst_tp, size_t dst_rank, kvbm_head_window* out, size_t cap,
+                         size_t* n_out);
 
 /* ---- TransferManager ---- */
 /* cuda_device_id < 0: host-only manager (Memcpy strategy only; every CUDA strategy returns KVBM_ERR_CUDA). */
