@@ -14,7 +14,10 @@ WANT = {"paged_copy_kernelILi0": "paged_copy_cast0", "paged_copy_kernelILi1": "p
         "pair_copy_kernel": "pair_copy_k1", "permute_table_kernelILb1": "permute_table_pow2", "permute_table_kernelILb0": "permute_table_mulhi",
         "paged_permute_kernelILi0ELb1": "paged_permute_pow2", "paged_permute_kernelILi0ELb0": "paged_permute_mulhi",
         "paged_permute_kernelILi1ELb1": "paged_permute_fp8_to_bf16_pow2", "paged_permute_kernelILi1ELb0": "paged_permute_fp8_to_bf16_mulhi",
-        "paged_permute_kernelILi2ELb1": "paged_permute_bf16_to_fp8_pow2", "paged_permute_kernelILi2ELb0": "paged_permute_bf16_to_fp8_mulhi"}
+        "paged_permute_kernelILi2ELb1": "paged_permute_bf16_to_fp8_pow2", "paged_permute_kernelILi2ELb0": "paged_permute_bf16_to_fp8_mulhi",
+        "paged_gather_kernelILi0ELb1": "paged_gather_pow2", "paged_gather_kernelILi0ELb0": "paged_gather_mulhi",
+        "paged_gather_kernelILi1ELb1": "paged_gather_fp8_to_bf16_pow2", "paged_gather_kernelILi1ELb0": "paged_gather_fp8_to_bf16_mulhi",
+        "paged_gather_kernelILi2ELb1": "paged_gather_bf16_to_fp8_pow2", "paged_gather_kernelILi2ELb0": "paged_gather_bf16_to_fp8_mulhi"}
 KEYS = ["UBLKCP.S.G", "UBLKCP.G.S", "SYNCS.ARRIVE.TRANS64", "SYNCS.PHASECHK.TRANS64.TRYWAIT", "SYNCS.ARRIVE", "UTMACMDFLUSH", "FENCE.VIEW.ASYNC",
             "F2FP", "ATOMG", "LDG.E.NA.128", "STG.E.NA.128", "LDS.128", "STS.128", "NANOSLEEP", "SHFL"]
 

@@ -141,11 +141,20 @@ def cast_bench():
     print(json.dumps(res))
 
 
+def card():
+    """The name and power limit of GPU 0, read now: they belong beside every time this run prints."""
+    import subprocess
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True)
+    name, _, limit = q.stdout.strip().partition(", ") if q.returncode == 0 else (torch.cuda.get_device_name(0), "", "not read")
+    return {"name": name, "power_limit": limit}
+
+
 def reshard_bench():
     """Decode rank 0 of a SRC_TP -> DST_TP re-shard: every launch of its plan (kvbm_kernels_paged_permute_heads, engine pools
     OperationalNHD layer-separate on both sides, --cast fused in), per hand-off, median over three runs.  Compared with the plain
     paged copy (its cast with --cast) of the same destination bytes and with the full-head permute (every head of a TP1 pool,
-    NHD -> NHD) per byte."""
+    NHD -> NHD) per byte.  reshard_one_launch runs the same plan as one kvbm_kernels_paged_permute_gather launch on the same
+    pools and stream; one_launch_equals_per_entry compares the whole destination pool after either arm."""
     from dynamo_b200.physical import tp_reshard_plan
     from oracle import oracle as O
     from tests.reshard_oracle import reshard_block
@@ -182,6 +191,20 @@ def reshard_bench():
             want = reshard_block(block(srcs[w.src_rank], int(sid[i])), want, O.KV_OPERATIONAL_NHD, O.KV_OPERATIONAL_NHD, nl, no, nt, snh,
                                  dnh, hd * se, int(mode), w.src_head_begin, w.dst_head_begin, w.head_count)
         same = same and bool(np.array_equal(block(dst, int(did[i])), want))
+    gather_srcs = [K.PermuteSource(side(srcs[w.src_rank][2], sid_d), snh, w.src_head_begin, w.dst_head_begin, w.head_count) for w in plan]
+
+    def one_launch():   # the same plan as one kvbm_kernels_paged_permute_gather launch
+        K.check(K.paged_permute_gather(gather_srcs, side(dst[2], did_d), dnh, n, 0, nl, nt, hd * se, int(mode), stream=sp))
+
+    def dst_after(fn):   # the whole destination pool after fn, from the same pre-filled pool
+        for t in dst[0]:
+            t.fill_(0x5A)
+        torch.cuda.synchronize()
+        fn()
+        torch.cuda.synchronize()
+        return [t.clone() for t in dst[0]]
+
+    one_equal = all(torch.equal(x, y) for x, y in zip(dst_after(assemble), dst_after(one_launch)))
     plain_src = engine(dnh, se, sdev)   # the same destination bytes as one paged copy (its cast with --cast)
 
     def plain():
@@ -198,8 +221,10 @@ def reshard_bench():
                         "src_tp": src_tp, "dst_tp": dst_tp, "src_heads_per_rank": snh, "dst_heads_per_rank": dnh},
            "plan": [[w.src_rank, w.src_head_begin, w.dst_head_begin, w.head_count] for w in plan],
            "window_widths": [w.head_count for w in plan], "launches": len(plan), "reshard_equals_oracle": same,
-           "peer": a.peer, "peer_side": a.peer_side if a.peer >= 0 else None, "hbm_peak_GBps": peak, "hbm_peak_source": peak_src}
-    for name, fn, count in (("reshard_assembly", assemble, elems), ("plain_paged_copy_same_bytes", plain, elems),
+           "peer": a.peer, "peer_side": a.peer_side if a.peer >= 0 else None, "hbm_peak_GBps": peak, "hbm_peak_source": peak_src,
+           "one_launch_equals_per_entry": one_equal, "card": card()}
+    for name, fn, count in (("reshard_assembly", assemble, elems), ("reshard_one_launch", one_launch, elems),
+                            ("plain_paged_copy_same_bytes", plain, elems),
                             ("full_head_permute_tp1", full_permute, n * nl * no * nt * nh * hd)):
         ms = statistics.median([timed(fn) for _ in range(3)])
         rw = count * (se + de)

@@ -703,15 +703,28 @@ static int execute_two_hop(kvbm_transfer_manager* m, Layout* S, Layout* D, Layou
   return KVBM_OK;
 }
 
+// One entry of a gather, as execute() resolved it: the layouts, their formats, the layer range and the direct CUDA strategy.
+struct GatherEntry {
+  Layout *S, *D;
+  int src_kv, dst_kv;
+  size_t lb, le;
+  int strategy;
+};
+
+// `gather`: validate one windowed entry of a gather and fill *gather instead of running it.  The caller holds the manager
+// mutex; the entry always takes the permuting path (also for a window over every head of both sides) and every check and
+// rejection text is that of a windowed execute_transfer.  An empty entry (n == 0 or an empty layer range) leaves
+// gather->strategy at -1.
 static int execute(kvbm_transfer_manager* m, kvbm_layout_handle src_h, int nd, const kvbm_layout_handle* dst_h,
                    const size_t* const* src_ids, const size_t* const* dst_ids, size_t n, bool replicate,
-                   const kvbm_transfer_options* opts_in, kvbm_notification* out)
+                   const kvbm_transfer_options* opts_in, kvbm_notification* out, GatherEntry* gather = nullptr)
 {
   kvbm_transfer_options o{};
   if (opts_in) o = *opts_in;
   if (out) *out = 0;
   if (nd < 1 || nd > KVBM_MAX_DESTINATIONS) return fail(KVBM_ERR, "number of destinations must be in 1..=8");
-  std::lock_guard<std::mutex> lk(m->mu);
+  std::unique_lock<std::mutex> lk(m->mu, std::defer_lock);
+  if (!gather) lk.lock();
   Layout* S = m->find(src_h);
   if (!S) return fail(KVBM_ERR_HANDLE, "invalid source handle");
   if (S->unmapped) return fail(KVBM_ERR_UNSUPPORTED, "source layout is a descriptor of another process's host memory: not addressable from this process");
@@ -732,7 +745,7 @@ static int execute(kvbm_transfer_manager* m, kvbm_layout_handle src_h, int nd, c
                                         std::to_string(sc.num_heads) + " heads, dst " + std::to_string(o.dst_head_begin) + "+" +
                                         std::to_string(o.head_count) + " of " + std::to_string(dc.num_heads) + " heads is out of range");
       // a window over every head of both sides is the transfer without one
-      window = !(o.src_head_begin == 0 && o.dst_head_begin == 0 && o.head_count == sc.num_heads && o.head_count == dc.num_heads);
+      window = gather || !(o.src_head_begin == 0 && o.dst_head_begin == 0 && o.head_count == sc.num_heads && o.head_count == dc.num_heads);
     }
     int rc = check_compat(*S, *D[d], o.cast_mode, window);
     if (rc) return rc;
@@ -804,6 +817,7 @@ static int execute(kvbm_transfer_manager* m, kvbm_layout_handle src_h, int nd, c
     if (lb > le || le > S->cfg.num_layers)
       return fail(KVBM_ERR_RANGE, "Layer range " + std::to_string(lb) + ".." + std::to_string(le) + " exceeds num_layers " + std::to_string(S->cfg.num_layers));
   }
+  if (gather) *gather = GatherEntry{S, D[0], src_kv, dst_kv0, lb, le, -1};
   if (n == 0 || lb == le) return KVBM_OK;
 
   // select_strategy (strategy.rs:78-108): every layout handled here is local or peer-mapped
@@ -859,6 +873,10 @@ static int execute(kvbm_transfer_manager* m, kvbm_layout_handle src_h, int nd, c
   if (!cuda_strategy(plan.first))
     return fail(KVBM_ERR_UNSUPPORTED, "NIXL strategies are outside this library (the NVLink peer path replaces them)");
   if (m->device < 0) return fail(KVBM_ERR_CUDA, "this TransferManager was created without a CUDA device; CUDA strategies have no CPU fallback");
+  if (gather) {
+    gather->strategy = plan.first;
+    return KVBM_OK;
+  }
 
   DeviceGuard g(m->device);
   // stream: caller's, or round-robin from the pool (cuda.rs:82-90: D2H pool for D2H, H2D pool otherwise)
@@ -875,6 +893,90 @@ static int execute(kvbm_transfer_manager* m, kvbm_layout_handle src_h, int nd, c
                    : launch_cuda(m, S, D.data(), nd, src_ids, dst_ids, n, replicate, lb, le, o, stream, nullptr, &sl, &seq);
   if (rc) return rc;
   // caller-provided stream: caller manages sync, completed() is returned (cuda.rs:139-141)
+  if (out) *out = o.use_caller_stream ? 0 : seq;
+  return KVBM_OK;
+}
+
+// A TP re-shard's assembly as one hand-off: every window is validated as the windowed execute_transfer of its (source,
+// destination) pair, then one kvbm_kernels_paged_permute_gather launch moves all of them and one signal launch writes the
+// done flag and the completion word after the last byte landed.
+static int execute_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, const size_t* const* src_ids,
+                          kvbm_layout_handle dst_h, const size_t* dst_ids, size_t n, const kvbm_head_window* windows, size_t nw,
+                          const kvbm_transfer_options* opts_in, kvbm_notification* out)
+{
+  kvbm_transfer_options o{};
+  if (opts_in) o = *opts_in;
+  if (out) *out = 0;
+  if (num_srcs == 0 || !srcs || !windows || nw == 0) return fail(KVBM_ERR, "a gather needs at least one source and one window");
+  if (o.head_count) return fail(KVBM_ERR, "a gather takes its head windows from the windows argument: options.head_count must be 0");
+  if (nw > KVBM_GATHER_MAX_SOURCES)
+    return fail(KVBM_ERR_UNSUPPORTED, "a gather takes at most " + std::to_string(KVBM_GATHER_MAX_SOURCES) + " windows, got " + std::to_string(nw));
+  for (size_t j = 0; j < nw; ++j) {
+    if (windows[j].src_rank >= num_srcs)
+      return fail(KVBM_ERR_RANGE, "window " + std::to_string(j) + " names source " + std::to_string(windows[j].src_rank) + " of " +
+                                      std::to_string(num_srcs));
+    if (windows[j].head_count == 0) return fail(KVBM_ERR_RANGE, "window " + std::to_string(j) + " has no heads");
+    for (size_t t = 0; t < j; ++t)
+      if (windows[j].dst_head_begin < windows[t].dst_head_begin + windows[t].head_count &&
+          windows[t].dst_head_begin < windows[j].dst_head_begin + windows[j].head_count)
+        return fail(KVBM_ERR_OVERLAP, "windows " + std::to_string(t) + " and " + std::to_string(j) + " overlap in the destination");
+  }
+  if (n && (!src_ids || !dst_ids)) return fail(KVBM_ERR, "null block id list");
+  std::lock_guard<std::mutex> lk(m->mu);
+  std::vector<GatherEntry> e(nw);
+  for (size_t j = 0; j < nw; ++j) {
+    kvbm_transfer_options oj = o;
+    oj.src_head_begin = windows[j].src_head_begin;
+    oj.dst_head_begin = windows[j].dst_head_begin;
+    oj.head_count = windows[j].head_count;
+    const size_t* s = src_ids ? src_ids[windows[j].src_rank] : nullptr;
+    int rc = execute(m, srcs[windows[j].src_rank], 1, &dst_h, &s, &dst_ids, n, true, &oj, nullptr, &e[j]);
+    if (rc) return rc;
+    if (e[j].strategy != e[0].strategy) return fail(KVBM_ERR_UNSUPPORTED, "the sources of a gather need the same CUDA strategy");
+  }
+  if (e[0].strategy < 0) return KVBM_OK;  // nothing to move (no blocks or an empty layer range), as execute()
+
+  DeviceGuard g(m->device);
+  cudaStream_t stream;
+  if (o.use_caller_stream)
+    stream = o.cuda_stream;
+  else if (e[0].strategy == KVBM_STRATEGY_CUDA_ASYNC_D2H)
+    stream = m->d2h[m->rr_d2h++ % kStreams];
+  else
+    stream = m->h2d[m->rr_h2d++ % kStreams];
+  // one upload of every source's table and the destination's: source s at s * n, the destination at num_srcs * n
+  Slot* sl;
+  uint64_t seq;
+  int rc = acquire_slot(m, (num_srcs + 1) * n, 4, &sl, &seq);
+  if (rc) return rc;
+  for (size_t s = 0; s < num_srcs; ++s)
+    if (src_ids[s])
+      for (size_t i = 0; i < n; ++i) sl->pinned_ids[s * n + i] = static_cast<int32_t>(src_ids[s][i]);
+  for (size_t i = 0; i < n; ++i) sl->pinned_ids[num_srcs * n + i] = static_cast<int32_t>(dst_ids[i]);
+  CU(cudaMemcpyAsync(sl->dev_ids, sl->pinned_ids, (num_srcs + 1) * n * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
+  m->h2d_bytes += (num_srcs + 1) * n * sizeof(int32_t);
+  Layout* D = e[0].D;
+  kvbm_permute_side pd{descriptor(*D), sl->dev_ids + num_srcs * n, e[0].dst_kv};
+  kvbm_permute_source ks[KVBM_GATHER_MAX_SOURCES] = {};
+  size_t bytes = 0;
+  for (size_t j = 0; j < nw; ++j) {
+    const size_t r = windows[j].src_rank;
+    ks[j] = kvbm_permute_source{{descriptor(*e[j].S), sl->dev_ids + r * n, e[j].src_kv}, static_cast<uint32_t>(e[j].S->cfg.num_heads),
+                                static_cast<uint32_t>(windows[j].src_head_begin), static_cast<uint32_t>(windows[j].dst_head_begin),
+                                static_cast<uint32_t>(windows[j].head_count)};
+    bytes += D->region / D->cfg.num_heads * windows[j].head_count;
+  }
+  const Layout* S0 = e[0].S;
+  const size_t row = S0->cfg.inner_dim / S0->cfg.num_heads * S0->cfg.dtype_width_bytes;
+  cudaError_t ce = kvbm_kernels_paged_permute_gather(ks, static_cast<int>(nw), &pd, static_cast<uint32_t>(D->cfg.num_heads), static_cast<int>(n),
+                                                     static_cast<int>(e[0].lb), static_cast<int>(e[0].le), static_cast<uint32_t>(S0->cfg.page_size),
+                                                     static_cast<uint32_t>(row), o.cast_mode, o.done_flag, o.epoch, sl->host_flag,
+                                                     static_cast<uint32_t>(seq), stream);
+  if (ce != cudaSuccess) return fail_cuda(ce, "kvbm_kernels_paged_permute_gather");
+  CU(cudaEventRecord(sl->ev, stream));
+  sl->in_flight = true;
+  m->bytes_moved += n * (e[0].le - e[0].lb) * S0->cfg.outer_dim * bytes;
+  // caller-provided stream: caller manages sync, completed() is returned, as execute()
   if (out) *out = o.use_caller_stream ? 0 : seq;
   return KVBM_OK;
 }
@@ -1420,6 +1522,21 @@ extern "C" int kvbm_manager_execute_transfer(kvbm_transfer_manager* m, kvbm_layo
   const size_t* s[1] = {src_ids};
   const size_t* d[1] = {dst_ids};
   return execute(m, src, 1, &dst, s, d, n, true, opts, out);
+  } catch (const std::exception& e) {
+    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
+  } catch (...) {
+    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
+  }
+}
+
+extern "C" int kvbm_manager_execute_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs,
+                                           const size_t* const* src_ids, kvbm_layout_handle dst, const size_t* dst_ids, size_t n,
+                                           const kvbm_head_window* windows, size_t num_windows, const kvbm_transfer_options* opts,
+                                           kvbm_notification* out)
+{
+  try {
+  if (!m) return fail(KVBM_ERR, "null manager");
+  return execute_gather(m, num_srcs, srcs, src_ids, dst, dst_ids, n, windows, num_windows, opts, out);
   } catch (const std::exception& e) {
     return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
   } catch (...) {

@@ -639,6 +639,46 @@ kvbm_paged_permute_kernel(const __grid_constant__ PermuteSide S, const __grid_co
                              threadIdx.x >> 5, blockDim.x >> 5, nh, nt, r);
 }
 
+// The gather: several sources, each with its own pool, format, head count and head window, into one destination.  The
+// covered destination heads are numbered 0 .. covered-1 in source order; entry[j] names the source of covered head j,
+// which is head j - first of that source's window.  s_win / d_win: the window's first head on either side, in bytes.
+struct GatherSource {
+  PermuteSide S;
+  uint64_t s_win, d_win;
+  uint32_t first;
+};
+struct GatherParams {
+  PermuteSide D;
+  GatherSource src[KVBM_GATHER_MAX_SOURCES];
+  uint8_t entry[KVBM_GATHER_MAX_HEADS];
+  uint32_t covered;
+};
+
+// One CTA per destination (block, layer, outer) unit, as the paged permute, with one warp per covered destination head
+// (looping by the CTA's warps past 8): every source's window of the unit is written by the same CTA, so a destination row
+// that holds every head (OperationalNHD) is written whole by one CTA.  Each warp looks up its source and runs the same walk
+// over one head.
+template <int CAST, bool POW2>
+__global__ void __launch_bounds__(256)
+kvbm_paged_gather_kernel(const __grid_constant__ GatherParams P, uint32_t layer_begin, uint32_t nlayers, uint32_t no, uint32_t nt, RowSplit r)
+{
+  const uint32_t unit = blockIdx.x;  // (pair * nlayers + l) * no + o
+  const uint32_t pair = unit / (nlayers * no);
+  const uint32_t rem = unit - pair * (nlayers * no);
+  const uint32_t l = layer_begin + rem / no, o = rem % no;
+  auto base_of = [&](const PermuteSide& X) {
+    return reinterpret_cast<uint8_t*>(static_cast<uintptr_t>(__ldg(X.layer_base + (X.universal ? 0 : l)))) +
+           static_cast<uint64_t>(__ldg(X.ids + pair)) * X.block_stride + l * X.layer_step + o * X.outer_step;
+  };
+  uint8_t* db = base_of(P.D);
+  for (uint32_t j = threadIdx.x >> 5; j < P.covered; j += blockDim.x >> 5) {
+    const GatherSource& G = P.src[P.entry[j]];
+    const uint32_t h = j - G.first;  // head h of the window: walk heads h .. h of the window's bases
+    walk_head_rows<CAST, POW2>(base_of(G.S) + G.s_win, G.S.head_stride, G.S.tok_stride, db + G.d_win, P.D.head_stride, P.D.tok_stride,
+                               h, 1, h + 1, nt, r);
+  }
+}
+
 __global__ void kvbm_signal_kernel(uint32_t* a, uint32_t va, uint32_t* b, uint32_t vb)
 {
   __threadfence_system();
@@ -768,6 +808,12 @@ static cudaError_t preload_kernels()
   KVBM_PRELOAD((kvbm_paged_permute_kernel<KVBM_CAST_FP8E4M3_TO_BF16, false>))
   KVBM_PRELOAD((kvbm_paged_permute_kernel<KVBM_CAST_BF16_TO_FP8E4M3, true>))
   KVBM_PRELOAD((kvbm_paged_permute_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false>))
+  KVBM_PRELOAD((kvbm_paged_gather_kernel<KVBM_CAST_NONE, true>))
+  KVBM_PRELOAD((kvbm_paged_gather_kernel<KVBM_CAST_NONE, false>))
+  KVBM_PRELOAD((kvbm_paged_gather_kernel<KVBM_CAST_FP8E4M3_TO_BF16, true>))
+  KVBM_PRELOAD((kvbm_paged_gather_kernel<KVBM_CAST_FP8E4M3_TO_BF16, false>))
+  KVBM_PRELOAD((kvbm_paged_gather_kernel<KVBM_CAST_BF16_TO_FP8E4M3, true>))
+  KVBM_PRELOAD((kvbm_paged_gather_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false>))
   KVBM_PRELOAD(kvbm_signal_kernel)
   KVBM_PRELOAD(kvbm_permute_table_kernel<true>)
   KVBM_PRELOAD(kvbm_permute_table_kernel<false>)
@@ -1005,6 +1051,82 @@ kvbm_kernels_paged_permute_heads(const kvbm_permute_side* src, const kvbm_permut
       break;
     default:
       r.pow2 ? go(kvbm_paged_permute_kernel<KVBM_CAST_BF16_TO_FP8E4M3, true>) : go(kvbm_paged_permute_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false>);
+      break;
+  }
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  return finish();
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_permute_gather(const kvbm_permute_source* srcs, int num_srcs, const kvbm_permute_side* dst, uint32_t dst_num_heads,
+                                  int num_blocks, int layer_begin, int layer_end, uint32_t page_size, uint32_t src_row_bytes,
+                                  int cast_mode, uint32_t* done_flag, uint32_t epoch, uint32_t* completion_flag,
+                                  uint32_t completion_value, cudaStream_t stream)
+{
+  if (num_blocks < 0 || layer_begin < 0 || layer_end < layer_begin) return cudaErrorInvalidValue;
+  if (cast_mode < KVBM_CAST_NONE || cast_mode > KVBM_CAST_BF16_TO_FP8E4M3) return cudaErrorInvalidValue;
+  if (!srcs || num_srcs < 1 || num_srcs > KVBM_GATHER_MAX_SOURCES) return cudaErrorInvalidValue;
+  const bool signal = done_flag || completion_flag;
+  auto finish = [&]() -> cudaError_t {
+    if (!signal) return cudaSuccess;
+    kvbm_signal_kernel<<<1, 1, 0, stream>>>(done_flag, epoch, completion_flag, completion_value);
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    return cudaGetLastError();
+  };
+  if (num_blocks == 0 || layer_end == layer_begin) return finish();
+  if (!dst || !dst->block_ids || !dst->layout.layer_base) return cudaErrorInvalidValue;
+  const uint32_t nl = dst->layout.num_layers, no = dst->layout.outer_dim;
+  if (nl == 0 || no == 0 || static_cast<uint32_t>(layer_end) > nl) return cudaErrorInvalidValue;
+  // the row rules of kvbm_kernels_paged_permute_heads, shared by every source
+  if (cast_mode == KVBM_CAST_BF16_TO_FP8E4M3 && (src_row_bytes & 1)) return cudaErrorInvalidValue;
+  const uint64_t dst_row_bytes = cast_mode == KVBM_CAST_FP8E4M3_TO_BF16   ? 2ull * src_row_bytes
+                                 : cast_mode == KVBM_CAST_BF16_TO_FP8E4M3 ? src_row_bytes / 2
+                                                                          : src_row_bytes;
+  const uint64_t walk_row = cast_mode == KVBM_CAST_BF16_TO_FP8E4M3 ? dst_row_bytes : src_row_bytes;
+  RowSplit r;
+  if (page_size == 0 || !row_split(walk_row, page_size, &r)) return cudaErrorInvalidValue;
+  if (static_cast<uint64_t>(page_size) * dst_num_heads * dst_row_bytes != dst->layout.region_bytes) return cudaErrorInvalidValue;
+  GatherParams P{};
+  if (!fill_permute_side(*dst, nl, no, dst_num_heads, page_size, static_cast<uint32_t>(dst_row_bytes), &P.D)) return cudaErrorInvalidValue;
+  uint32_t covered = 0;
+  for (int s = 0; s < num_srcs; ++s) {
+    const kvbm_permute_source& X = srcs[s];
+    if (!X.side.block_ids || !X.side.layout.layer_base || X.side.layout.num_layers != nl || X.side.layout.outer_dim != no)
+      return cudaErrorInvalidValue;
+    if (X.head_count == 0 || static_cast<uint64_t>(X.src_head_begin) + X.head_count > X.num_heads ||
+        static_cast<uint64_t>(X.dst_head_begin) + X.head_count > dst_num_heads)
+      return cudaErrorInvalidValue;
+    for (int t = 0; t < s; ++t)  // two windows writing the same destination head would race
+      if (X.dst_head_begin < srcs[t].dst_head_begin + srcs[t].head_count && srcs[t].dst_head_begin < X.dst_head_begin + X.head_count)
+        return cudaErrorInvalidValue;
+    if (static_cast<uint64_t>(page_size) * X.num_heads * src_row_bytes != X.side.layout.region_bytes) return cudaErrorInvalidValue;
+    GatherSource& G = P.src[s];
+    if (!fill_permute_side(X.side, nl, no, X.num_heads, page_size, src_row_bytes, &G.S)) return cudaErrorInvalidValue;
+    if (covered + X.head_count > KVBM_GATHER_MAX_HEADS) return cudaErrorInvalidValue;
+    G.s_win = X.src_head_begin * G.S.head_stride;
+    G.d_win = X.dst_head_begin * P.D.head_stride;
+    G.first = covered;
+    for (uint32_t j = 0; j < X.head_count; ++j) P.entry[covered + j] = static_cast<uint8_t>(s);
+    covered += X.head_count;
+  }
+  P.covered = covered;
+  const uint64_t units = static_cast<uint64_t>(num_blocks) * (layer_end - layer_begin) * no;
+  if (units >= (1ull << 31)) return cudaErrorInvalidValue;
+  const int threads = static_cast<int>(std::min<uint32_t>(8, covered)) * 32;
+  const unsigned grid = static_cast<unsigned>(units);
+  const uint32_t lb = static_cast<uint32_t>(layer_begin), nlay = static_cast<uint32_t>(layer_end - layer_begin);
+  auto go = [&](auto kern) { kern<<<grid, threads, 0, stream>>>(P, lb, nlay, no, page_size, r); };
+  switch (cast_mode) {
+    case KVBM_CAST_NONE:
+      r.pow2 ? go(kvbm_paged_gather_kernel<KVBM_CAST_NONE, true>) : go(kvbm_paged_gather_kernel<KVBM_CAST_NONE, false>);
+      break;
+    case KVBM_CAST_FP8E4M3_TO_BF16:
+      r.pow2 ? go(kvbm_paged_gather_kernel<KVBM_CAST_FP8E4M3_TO_BF16, true>) : go(kvbm_paged_gather_kernel<KVBM_CAST_FP8E4M3_TO_BF16, false>);
+      break;
+    default:
+      r.pow2 ? go(kvbm_paged_gather_kernel<KVBM_CAST_BF16_TO_FP8E4M3, true>) : go(kvbm_paged_gather_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false>);
       break;
   }
   g_launches.fetch_add(1, std::memory_order_relaxed);

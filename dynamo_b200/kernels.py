@@ -98,6 +98,16 @@ class PermuteSide(C.Structure):
     _fields_ = [("layout", PagedLayout), ("block_ids", C.c_void_p), ("kv_layout", C.c_int)]
 
 
+class PermuteSource(C.Structure):
+    """struct kvbm_permute_source: one source of `paged_permute_gather` (a side, its head count and its head window)"""
+    _fields_ = [("side", PermuteSide), ("num_heads", C.c_uint32), ("src_head_begin", C.c_uint32), ("dst_head_begin", C.c_uint32),
+                ("head_count", C.c_uint32)]
+
+
+GATHER_MAX_SOURCES = 16      # KVBM_GATHER_MAX_SOURCES
+GATHER_MAX_HEADS = 256       # KVBM_GATHER_MAX_HEADS
+
+
 class PagedCopyOpts(C.Structure):
     """struct kvbm_paged_copy_opts"""
     _fields_ = [
@@ -156,6 +166,9 @@ def lib() -> C.CDLL:
                                                        C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, i, vp, C.c_uint32, vp,
                                                        C.c_uint32, vp]
         L.kvbm_kernels_paged_permute_heads.restype = i
+        L.kvbm_kernels_paged_permute_gather.argtypes = [C.POINTER(PermuteSource), i, C.POINTER(PermuteSide), C.c_uint32, i, i, i, C.c_uint32,
+                                                        C.c_uint32, i, vp, C.c_uint32, vp, C.c_uint32, vp]
+        L.kvbm_kernels_paged_permute_gather.restype = i
         L.kvbm_kernels_permute_strides.argtypes = [i, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64, C.c_uint64,
                                                    C.POINTER(C.c_uint64)]
         L.kvbm_kernels_permute_strides.restype = i
@@ -178,6 +191,7 @@ EXPORTED_SYMBOLS = [
     "kvbm_kernels_paged_copy_v2", "kvbm_kernels_set_flags", "kvbm_kernels_wait_flag", "kvbm_kernels_stream_wait_event",
     "kvbm_kernels_launch_count", "kvbm_kernels_build_info", "kvbm_kernels_gate_would_spin", "kvbm_kernels_paged_permute",
     "kvbm_kernels_permute_strides", "kvbm_kernels_paged_permute_cast", "kvbm_kernels_paged_permute_heads",
+    "kvbm_kernels_paged_permute_gather",
 ]
 
 GATE_AUTO, GATE_SPIN, GATE_STREAM_WAIT = 0, 1, 2
@@ -261,6 +275,18 @@ def paged_permute_heads(src: PermuteSide, dst: PermuteSide, num_blocks: int, lay
     return lib().kvbm_kernels_paged_permute_heads(C.byref(src), C.byref(dst), num_blocks, layer_begin, layer_end, src_num_heads,
                                                   src_head_begin, dst_num_heads, dst_head_begin, head_count, page_size, src_row_bytes,
                                                   int(cast_mode), done_flag or None, epoch, completion_flag or None, completion_value, stream)
+
+
+def paged_permute_gather(srcs: Sequence[PermuteSource], dst: PermuteSide, dst_num_heads: int, num_blocks: int, layer_begin: int,
+                         layer_end: int, page_size: int, src_row_bytes: int, cast_mode: int = 0, done_flag: int = 0, epoch: int = 0,
+                         completion_flag: int = 0, completion_value: int = 0, stream: int = 0) -> int:
+    """`paged_permute_heads` over several sources in ONE launch (a TP re-shard's assembly): each source's head window lands in
+    the destination, whose bytes outside the union of the windows keep their values; the flags are written once, after every
+    window.  include/kvbm_kernels.h (kvbm_kernels_paged_permute_gather)."""
+    arr = (PermuteSource * max(1, len(srcs)))(*srcs)
+    return lib().kvbm_kernels_paged_permute_gather(arr, len(srcs), C.byref(dst), dst_num_heads, num_blocks, layer_begin, layer_end, page_size,
+                                                   src_row_bytes, int(cast_mode), done_flag or None, epoch, completion_flag or None,
+                                                   completion_value, stream)
 
 
 def permute_strides(kv_layout: int, num_layers: int, outer_dim: int, num_heads: int, page_size: int, row_bytes: int,

@@ -216,7 +216,7 @@ EXPORTED_SYMBOLS = [
     "kvbm_select_direct_strategy_remote", "kvbm_select_strategy", "kvbm_manager_select_strategy",
     "kvbm_mc_supported", "kvbm_mc_group_create", "kvbm_mc_group_export_fd", "kvbm_mc_group_import_fd",
     "kvbm_mc_group_size", "kvbm_mc_group_add_device", "kvbm_mc_group_bind_local", "kvbm_mc_group_bind_addr", "kvbm_mc_group_map",
-    "kvbm_mc_group_destroy", "kvbm_tp_reshard_plan",
+    "kvbm_mc_group_destroy", "kvbm_tp_reshard_plan", "kvbm_manager_execute_gather",
 ]
 
 
@@ -264,6 +264,7 @@ def lib() -> C.CDLL:
         L.kvbm_select_transform_kernel.argtypes = [i, i]
         L.kvbm_kv_layout_requires_transform.argtypes = [i, i]
         L.kvbm_tp_reshard_plan.argtypes = [sz, sz, sz, sz, P(_CHeadWindow), sz, P(sz)]
+        L.kvbm_manager_execute_gather.argtypes = [vp, sz, P(u64), P(P(sz)), u64, vp, sz, P(_CHeadWindow), sz, P(_COptions), P(u64)]
         L.kvbm_notification_is_complete.argtypes = [vp, u64]
         L.kvbm_notification_wait.argtypes = [vp, u64, C.c_int64]
         L.kvbm_manager_bytes_moved.argtypes = [vp]
@@ -565,7 +566,8 @@ class TransferManager:
         (`tp_reshard_plan`).  `sources` maps a source rank to (layout handle, block ids); `dst_block_ids[i]` receives head
         windows of each source's block i.  The windows of one destination block are byte-disjoint, so the transfers may run on
         different manager streams at once.  `options` is applied to every entry, or is one TransferOptions per entry -- the way to
-        give each entry its own done_flag (there is no combined flag).  Returns one notification per entry."""
+        give each entry its own done_flag (there is no combined flag).  Returns one notification per entry.  `execute_gather`
+        runs the same plan as one launch with one notification and one done_flag."""
         per = list(options) if isinstance(options, (list, tuple)) else [options] * len(plan)
         if len(per) != len(plan):
             raise ValueError(f"{len(per)} options for {len(plan)} plan entries")
@@ -577,6 +579,30 @@ class TransferManager:
             o = dataclasses.replace(o or TransferOptions(), head_window=(w.src_head_begin, w.dst_head_begin, w.head_count))
             notes.append(self.execute_transfer(h, ids, dst, dst_block_ids, o))
         return notes
+
+    def execute_gather(self, sources: Mapping[int, tuple], dst: int, dst_block_ids: Sequence[int], plan: Sequence[HeadWindow],
+                       options: Optional[TransferOptions] = None) -> TransferCompleteNotification:
+        """`execute_reshard` as ONE hand-off (kvbm_manager_execute_gather): the same `sources` mapping (source rank -> (layout
+        handle, block ids)) and plan, at most 16 windows, moved by one permuting launch.  Returns one notification, and
+        `options.done_flag` is written once, after every window's bytes landed.  `options.head_window` must be None."""
+        ranks = sorted({w.src_rank for w in plan})
+        index = {r: i for i, r in enumerate(ranks)}
+        n = len(dst_block_ids)
+        if any(len(sources[r][1]) != n for r in ranks):
+            raise KvbmError(ErrorCode.LENGTH_MISMATCH, "Block ID lists have mismatched lengths")
+        hs = (C.c_uint64 * max(1, len(ranks)))(*[sources[r][0] for r in ranks])
+        s_arrays = [_size_array(sources[r][1])[0] for r in ranks]
+        d, _ = _size_array(dst_block_ids)
+        PP = C.POINTER(C.c_size_t)
+        as_ptr = lambda a: a._as_parameter_ if isinstance(a, _NpView) else C.cast(a, PP)  # noqa: E731
+        sp = (PP * max(1, len(ranks)))(*[as_ptr(a) for a in s_arrays])
+        ws = (_CHeadWindow * max(1, len(plan)))(*[_CHeadWindow(index[w.src_rank], w.src_head_begin, w.dst_head_begin, w.head_count)
+                                                  for w in plan])
+        tok = C.c_uint64()
+        o = (options or TransferOptions())._c()
+        _check(lib().kvbm_manager_execute_gather(self._h, len(ranks), hs, sp, dst, d.addr if type(d) is _NpView else d, n, ws, len(plan),
+                                                 C.byref(o), C.byref(tok)))
+        return TransferCompleteNotification(self, tok.value)
 
     def execute_fanout(self, src: int, dsts: Sequence[int], src_block_ids: Sequence[Sequence[int]],
                        dst_block_ids: Sequence[Sequence[int]], replicate: bool = False,

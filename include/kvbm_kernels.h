@@ -233,6 +233,33 @@ cudaError_t kvbm_kernels_paged_permute_heads(const kvbm_permute_side* src, const
                                              uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value,
                                              cudaStream_t stream);
 
+/* One source of kvbm_kernels_paged_permute_gather: a pool side with its own head count and one head window into the
+ * destination.  A pool may appear in several sources (with different windows). */
+typedef struct kvbm_permute_source {
+  kvbm_permute_side side;  /* side.block_ids: int32[num_blocks], block i lands in the destination's block_ids[i] */
+  uint32_t num_heads;      /* this source's heads per block (its region_bytes = page_size * num_heads * src_row_bytes) */
+  uint32_t src_head_begin, dst_head_begin, head_count;
+} kvbm_permute_source;
+
+#define KVBM_GATHER_MAX_SOURCES 16
+#define KVBM_GATHER_MAX_HEADS 256
+
+/* A gather (a decode rank assembling its re-sharded heads from several source ranks): for every source s, head
+ * src_head_begin + j of srcs[s].side.block_ids[i] lands as head dst_head_begin + j of dst->block_ids[i], for j < head_count,
+ * every layer of [layer_begin, layer_end), re-ordered and cast as kvbm_kernels_paged_permute_heads would -- but as ONE
+ * permuting launch over all sources, then one signal launch that writes done_flag / completion_flag once, after every
+ * source's bytes landed.  Every destination byte outside the union of the windows keeps its value.  All sources share
+ * page_size, src_row_bytes and cast_mode; each has its own format, pool and head count.  cudaErrorInvalidValue for:
+ * num_srcs outside 1..KVBM_GATHER_MAX_SOURCES, a null srcs / dst / table, head_count == 0 or a window past either side's
+ * heads, two windows overlapping in the destination, more than KVBM_GATHER_MAX_HEADS destination heads covered, a source
+ * whose num_layers / outer_dim differ from the destination's, and every rule of kvbm_kernels_paged_permute_heads (rows,
+ * cast, strides, grid bounds) applied to each (source, destination) pair.  The zero-count early return still signals. */
+cudaError_t kvbm_kernels_paged_permute_gather(const kvbm_permute_source* srcs, int num_srcs, const kvbm_permute_side* dst,
+                                              uint32_t dst_num_heads, int num_blocks, int layer_begin, int layer_end,
+                                              uint32_t page_size, uint32_t src_row_bytes, int cast_mode, uint32_t* done_flag,
+                                              uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value,
+                                              cudaStream_t stream);
+
 /* Host-only (no GPU): the stride table kvbm_kernels_paged_permute walks with for one side.  out[0] = 1 when offsets count
  * from the block's first byte (universal formats) or 0 when they count from the (layer, outer) region's first byte; the
  * element (layer l, outer o, head h, token t) then sits at  [out[0] ? l * out[1] + o * out[2] : 0] + h * out[3] + t * out[4].

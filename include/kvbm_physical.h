@@ -262,6 +262,22 @@ int kvbm_manager_execute_fanout(kvbm_transfer_manager* m, kvbm_layout_handle src
                                 const size_t* const* dst_ids, size_t n, int replicate,
                                 const kvbm_transfer_options* opts, kvbm_notification* out);
 
+/* N -> 1 in ONE launch: a decode rank assembles its blocks from several source pools (a TP re-shard plan,
+ * kvbm_tp_reshard_plan).  windows[j].src_rank indexes srcs / src_ids, so a plan can be passed as it is; a source may appear in
+ * several windows.  Heads [src_head_begin, +head_count) of block src_ids[src_rank][i] land as heads [dst_head_begin,
+ * +head_count) of block dst_ids[i]; every other destination byte keeps its value.  Each (source, destination) pair must pass
+ * what a windowed kvbm_manager_execute_transfer checks and is rejected with the same codes and texts (formats, head rows,
+ * casts, contiguity, alignment, block ids, layer range, layer streaming / multicast / fan-out flags, Two-hop and Memcpy
+ * strategies, both remote); all sources must select the same CUDA strategy.  Also: at most KVBM_GATHER_MAX_SOURCES (16)
+ * windows (KVBM_ERR_UNSUPPORTED), src_rank >= num_srcs or an empty window (KVBM_ERR_RANGE), windows overlapping in the
+ * destination (KVBM_ERR_OVERLAP), opts->head_count != 0 (KVBM_ERR).  One H2D upload of the (num_srcs + 1) * n ids, one
+ * kvbm_kernels_paged_permute_gather launch, one signal launch: opts->done_flag and the notification complete once, after
+ * every window's bytes landed.  bytes_moved counts each window's destination bytes. */
+int kvbm_manager_execute_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs,
+                                const size_t* const* src_ids, kvbm_layout_handle dst, const size_t* dst_ids, size_t n,
+                                const kvbm_head_window* windows, size_t num_windows, const kvbm_transfer_options* opts,
+                                kvbm_notification* out);
+
 /* Completion: the transfer's last warp writes a flag in pinned host memory (no cudaEventQuery polling). */
 int kvbm_notification_is_complete(kvbm_transfer_manager* m, kvbm_notification n);  /* 1 / 0 / <0 error */
 int kvbm_notification_wait(kvbm_transfer_manager* m, kvbm_notification n, int64_t timeout_us);
