@@ -10,7 +10,13 @@ import subprocess
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SO = os.path.join(ROOT, "dynamo_b200", "libkvbm_kernels.so")
-WANT = {"paged_copy_kernelILi0": "paged_copy_cast0", "paged_copy_kernelILi1": "paged_copy_fp8_to_bf16", "paged_copy_kernelILi2": "paged_copy_bf16_to_fp8",
+# the scaled instantiations (third template argument true) first: the unscaled keys are prefixes of their names
+WANT = {"paged_copy_kernelILi1ELb0ELb1": "paged_copy_fp8_to_bf16_scaled", "paged_copy_kernelILi2ELb0ELb1": "paged_copy_bf16_to_fp8_scaled",
+        "paged_permute_kernelILi1ELb1ELb1": "paged_permute_fp8_to_bf16_pow2_scaled", "paged_permute_kernelILi1ELb0ELb1": "paged_permute_fp8_to_bf16_mulhi_scaled",
+        "paged_permute_kernelILi2ELb1ELb1": "paged_permute_bf16_to_fp8_pow2_scaled", "paged_permute_kernelILi2ELb0ELb1": "paged_permute_bf16_to_fp8_mulhi_scaled",
+        "paged_gather_kernelILi1ELb1ELb1": "paged_gather_fp8_to_bf16_pow2_scaled", "paged_gather_kernelILi1ELb0ELb1": "paged_gather_fp8_to_bf16_mulhi_scaled",
+        "paged_gather_kernelILi2ELb1ELb1": "paged_gather_bf16_to_fp8_pow2_scaled", "paged_gather_kernelILi2ELb0ELb1": "paged_gather_bf16_to_fp8_mulhi_scaled",
+        "paged_copy_kernelILi0": "paged_copy_cast0", "paged_copy_kernelILi1": "paged_copy_fp8_to_bf16", "paged_copy_kernelILi2": "paged_copy_bf16_to_fp8",
         "pair_copy_kernel": "pair_copy_k1", "permute_table_kernelILb1": "permute_table_pow2", "permute_table_kernelILb0": "permute_table_mulhi",
         "paged_permute_kernelILi0ELb1": "paged_permute_pow2", "paged_permute_kernelILi0ELb0": "paged_permute_mulhi",
         "paged_permute_kernelILi1ELb1": "paged_permute_fp8_to_bf16_pow2", "paged_permute_kernelILi1ELb0": "paged_permute_fp8_to_bf16_mulhi",

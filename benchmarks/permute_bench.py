@@ -29,6 +29,8 @@ p.add_argument("--peer", type=int, default=-1, help="put one pool on this GPU (t
 p.add_argument("--peer-side", choices=["dst", "src"], default="dst", help="dst: universal pool on the peer (push); src: engine pool on the peer (pull)")
 p.add_argument("--cast", choices=["none", "fp8-to-bf16", "bf16-to-fp8"], default="none",
                help="time the transform with the fused cast against the paged copy's cast and the two-pass workaround instead")
+p.add_argument("--scaled", action="store_true",
+               help="with --cast: also time the same launches with per-(layer, K/V) fp8 KV-cache scales, alternating with the unscaled arms")
 p.add_argument("--reshard", default=None, metavar="SRC_TP:DST_TP",
                help="time one decode rank's assembly of its heads from the source ranks' pools (TP re-shard) instead; --cast composes")
 a = p.parse_args()
@@ -132,13 +134,69 @@ def cast_bench():
                         "MiB_fp8": elems / 2**20, "MiB_bf16": 2 * elems / 2**20},
            "peer": a.peer, "peer_side": a.peer_side if a.peer >= 0 else None, "fused_equals_two_pass": same,
            "hbm_peak_GBps": peak, "hbm_peak_source": peak_src}
-    for name, fn, per_elem in (("fused_permute_cast_to_universal", fused_to, 3), ("fused_permute_cast_from_universal", fused_from, 3),
-                               ("paged_copy_cast", cast_copy, 3), ("two_pass_fp8_permute_and_cast_copy", two_pass, 5)):
-        ms = timed(fn)
+    arms = [("fused_permute_cast_to_universal", fused_to, 3), ("fused_permute_cast_from_universal", fused_from, 3),
+            ("paged_copy_cast", cast_copy, 3), ("two_pass_fp8_permute_and_cast_copy", two_pass, 5)]
+    if a.scaled:
+        arms = scaled_arms(arms, res, mode, side, es, us, ed, ud, src_row, out, _eng8 if up else op)
+    for name, fn, per_elem in arms:
+        # --scaled: the median of three runs, the arms alternating so that scaled and unscaled see the same card state
+        ms = statistics.median(times[name]) if a.scaled else timed(fn)
         moved_rw = per_elem * elems
         res[name] = {"ms": round(ms, 4), "bytes_read_plus_write": moved_rw, "GBps_read_plus_write": round(moved_rw / ms / 1e6, 1),
                      "frac_of_hbm_peak": round(moved_rw / ms / 1e6 / peak, 3)}
     print(json.dumps(res))
+
+
+times = {}
+
+
+def scaled_arms(arms, res, mode, side, es, us, ed, ud, src_row, out, eng):
+    """The scaled twins of the fused permute + cast (both directions) and of the paged copy's cast, distinct scales per (layer,
+    K/V); checks two sampled blocks of each against tests/scaled_cast_oracle.py and times every arm three times, alternating."""
+    from tests.scaled_cast_oracle import cast_bytes_scaled, kv_layout_permute_cast_scaled
+    h = (np.random.default_rng(1).uniform(0.01, 4.0, nl * no) * (1 + np.arange(nl * no) * 1e-3)).astype(np.float32)
+    sc = torch.from_numpy(h).to(dev)
+
+    def fused_to_s():
+        K.check(K.paged_permute_heads(side(es, sid_d, 4), side(ud, did_d, 1), n, 0, nl, nh, 0, nh, 0, nh, nt, src_row, mode, stream=sp,
+                                      cast_scales=sc))
+
+    def fused_from_s():
+        K.check(K.paged_permute_heads(side(us, did_d, 1), side(ed, sid_d, 4), n, 0, nl, nh, 0, nh, 0, nh, nt, src_row, mode, stream=sp,
+                                      cast_scales=sc))
+
+    def cast_copy_s():
+        K.check(K.paged_copy(es, [K.PagedDst(ud, sid_d.data_ptr(), did_d.data_ptr(), 0, 0)], n, 0, nl, int(mode),
+                             K.PagedCopyOpts(cast_scales=sc.data_ptr()), sp))
+
+    src_block = lambda b: np.concatenate([eng[l].view(no, nb, -1)[o, b].cpu().numpy() for l in range(nl) for o in range(no)])  # noqa: E731
+    ok = True
+    for fn in (fused_to_s, cast_copy_s):
+        out.zero_()
+        torch.cuda.synchronize()
+        fn()
+        torch.cuda.synchronize()
+        for i in (0, n - 1):
+            blk = src_block(int(sid[i]))
+            got = out.view(nb, -1)[int(did[i])].cpu().numpy()
+            if fn is fused_to_s:
+                want = kv_layout_permute_cast_scaled(blk, 4, 1, nl, no, nt, nh, src_row, int(mode), h)
+            else:   # region (l, o) of the universal block, cast with its own scale
+                want = np.concatenate([cast_bytes_scaled(r, int(mode), float(h[k])) for k, r in enumerate(np.split(blk, nl * no))])
+            ok = ok and bool(np.array_equal(got, want))
+    res["scaled_equals_oracle"] = ok
+    res["card"] = card()
+    res["scales"] = "distinct per (layer, outer), uniform in [0.01, 4)"
+    named = {"fused_permute_cast_to_universal": fused_to_s, "fused_permute_cast_from_universal": fused_from_s, "paged_copy_cast": cast_copy_s}
+    out_arms = []
+    for name, fn, per in arms:
+        out_arms.append((name, fn, per))
+        if name in named:
+            out_arms.append((name + "_scaled", named[name], per))
+    for _ in range(3):
+        for name, fn, _per in out_arms:
+            times.setdefault(name, []).append(timed(fn))
+    return out_arms
 
 
 def card():

@@ -607,6 +607,7 @@ static int launch_cuda(kvbm_transfer_manager* m, Layout* S, Layout* const* D, in
   ko.multicast = o.multicast;
   ko.completion_flag = sl->host_flag;
   ko.completion_value = static_cast<uint32_t>(seq);
+  ko.cast_scales = o.cast_scales;
   cudaError_t e = kvbm_kernels_paged_copy_v2(&sdesc, dd, nd, static_cast<int>(n), static_cast<int>(lb), static_cast<int>(le), o.cast_mode, &ko, stream);
   if (e != cudaSuccess) return fail_cuda(e, "kvbm_kernels_paged_copy_v2");
   CU(cudaEventRecord(sl->ev, stream));
@@ -639,17 +640,32 @@ static int launch_transform(kvbm_transfer_manager* m, Layout* S, Layout* D, int 
   const size_t snh = S->cfg.num_heads, dnh = D->cfg.num_heads;
   const size_t sb = window ? o.src_head_begin : 0, db = window ? o.dst_head_begin : 0, k = window ? o.head_count : snh;
   const size_t row = S->cfg.inner_dim / snh * S->cfg.dtype_width_bytes;
-  cudaError_t e = kvbm_kernels_paged_permute_heads(&ps, &pd, static_cast<int>(n), static_cast<int>(lb), static_cast<int>(le),
-                                                   static_cast<uint32_t>(snh), static_cast<uint32_t>(sb), static_cast<uint32_t>(dnh),
-                                                   static_cast<uint32_t>(db), static_cast<uint32_t>(k), static_cast<uint32_t>(S->cfg.page_size),
-                                                   static_cast<uint32_t>(row), o.cast_mode, o.done_flag, o.epoch, sl->host_flag,
-                                                   static_cast<uint32_t>(seq), stream);
-  if (e != cudaSuccess) return fail_cuda(e, "kvbm_kernels_paged_permute_heads");
+  cudaError_t e = kvbm_kernels_paged_permute_heads_scaled(&ps, &pd, static_cast<int>(n), static_cast<int>(lb), static_cast<int>(le),
+                                                          static_cast<uint32_t>(snh), static_cast<uint32_t>(sb), static_cast<uint32_t>(dnh),
+                                                          static_cast<uint32_t>(db), static_cast<uint32_t>(k),
+                                                          static_cast<uint32_t>(S->cfg.page_size), static_cast<uint32_t>(row), o.cast_mode,
+                                                          o.cast_scales, o.done_flag, o.epoch, sl->host_flag, static_cast<uint32_t>(seq), stream);
+  if (e != cudaSuccess) return fail_cuda(e, "kvbm_kernels_paged_permute_heads_scaled");
   CU(cudaEventRecord(sl->ev, stream));
   sl->in_flight = true;
   m->bytes_moved += n * (le - lb) * S->cfg.outer_dim * (D->region / dnh * k);
   *slot_out = sl;
   *seq_out = seq;
+  return KVBM_OK;
+}
+
+// The cast kernels read the scales on the manager's device: its own device memory, or pinned host memory mapped into its address
+// space.  Anything else (pageable host memory, another GPU's memory) must not reach a kernel.
+static int check_cast_scales(kvbm_transfer_manager* m, const float* p)
+{
+  cudaPointerAttributes a{};
+  const cudaError_t e = cudaPointerGetAttributes(&a, p);
+  if (e != cudaSuccess) (void)cudaGetLastError();
+  const bool ok = e == cudaSuccess && ((a.type == cudaMemoryTypeDevice && a.device == m->device) ||
+                                       (a.type == cudaMemoryTypeHost && a.devicePointer == static_cast<const void*>(p)));
+  if (!ok)
+    return fail(KVBM_ERR, "cast_scales must be device memory of device " + std::to_string(m->device) +
+                              " or pinned host memory mapped into it (a pageable or another device's pointer cannot be read by the cast)");
   return KVBM_OK;
 }
 
@@ -817,6 +833,13 @@ static int execute(kvbm_transfer_manager* m, kvbm_layout_handle src_h, int nd, c
     if (lb > le || le > S->cfg.num_layers)
       return fail(KVBM_ERR_RANGE, "Layer range " + std::to_string(lb) + ".." + std::to_string(le) + " exceeds num_layers " + std::to_string(S->cfg.num_layers));
   }
+  if (o.cast_scales) {  // fp8 KV-cache scales: one per (layer, outer) of the pools, for the fp8 side of a cast
+    if (o.cast_mode == KVBM_CAST_NONE) return fail(KVBM_ERR, "cast_scales need a cast_mode: they scale the fp8 side of a cast");
+    const size_t need = S->cfg.num_layers * S->cfg.outer_dim;
+    if (o.num_cast_scales < need)
+      return fail(KVBM_ERR_RANGE, "cast_scales holds " + std::to_string(o.num_cast_scales) + " scales, the pools need num_layers * outer_dim = " +
+                                      std::to_string(need));
+  }
   if (gather) *gather = GatherEntry{S, D[0], src_kv, dst_kv0, lb, le, -1};
   if (n == 0 || lb == le) return KVBM_OK;
 
@@ -873,6 +896,10 @@ static int execute(kvbm_transfer_manager* m, kvbm_layout_handle src_h, int nd, c
   if (!cuda_strategy(plan.first))
     return fail(KVBM_ERR_UNSUPPORTED, "NIXL strategies are outside this library (the NVLink peer path replaces them)");
   if (m->device < 0) return fail(KVBM_ERR_CUDA, "this TransferManager was created without a CUDA device; CUDA strategies have no CPU fallback");
+  if (o.cast_scales) {
+    int rc = check_cast_scales(m, o.cast_scales);
+    if (rc) return rc;
+  }
   if (gather) {
     gather->strategy = plan.first;
     return KVBM_OK;
@@ -968,11 +995,11 @@ static int execute_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_
   }
   const Layout* S0 = e[0].S;
   const size_t row = S0->cfg.inner_dim / S0->cfg.num_heads * S0->cfg.dtype_width_bytes;
-  cudaError_t ce = kvbm_kernels_paged_permute_gather(ks, static_cast<int>(nw), &pd, static_cast<uint32_t>(D->cfg.num_heads), static_cast<int>(n),
-                                                     static_cast<int>(e[0].lb), static_cast<int>(e[0].le), static_cast<uint32_t>(S0->cfg.page_size),
-                                                     static_cast<uint32_t>(row), o.cast_mode, o.done_flag, o.epoch, sl->host_flag,
-                                                     static_cast<uint32_t>(seq), stream);
-  if (ce != cudaSuccess) return fail_cuda(ce, "kvbm_kernels_paged_permute_gather");
+  cudaError_t ce = kvbm_kernels_paged_permute_gather_scaled(ks, static_cast<int>(nw), &pd, static_cast<uint32_t>(D->cfg.num_heads),
+                                                            static_cast<int>(n), static_cast<int>(e[0].lb), static_cast<int>(e[0].le),
+                                                            static_cast<uint32_t>(S0->cfg.page_size), static_cast<uint32_t>(row), o.cast_mode,
+                                                            o.cast_scales, o.done_flag, o.epoch, sl->host_flag, static_cast<uint32_t>(seq), stream);
+  if (ce != cudaSuccess) return fail_cuda(ce, "kvbm_kernels_paged_permute_gather_scaled");
   CU(cudaEventRecord(sl->ev, stream));
   sl->in_flight = true;
   m->bytes_moved += n * (e[0].le - e[0].lb) * S0->cfg.outer_dim * bytes;

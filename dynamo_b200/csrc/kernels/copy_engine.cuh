@@ -125,6 +125,14 @@ struct RingParams {
                       // 2 = loads only (diagnostic), 3 = stores only (diagnostic)
 };
 
+// The scales of a scaled cast (SCALED rings): scales[layer * outer_dim + outer] is the dequantisation scale of the fp8 side.
+// The generator packs an item's outer index above its layer, Piece::layer = layer | outer << 16 (layer < 2^16, outer < 2^15),
+// and the consumer applies the item's scale to every element it converts.
+struct CastScales {
+  const float* scales;
+  uint32_t outer_dim;
+};
+
 // Per-slot control block the producer fills before it arms the slot's `full` barrier.
 struct SlotCtl {
   uint64_t src;
@@ -250,10 +258,10 @@ __device__ __forceinline__ void warp_copy_simt_mc(uint8_t* dst, const uint8_t* s
   }
 }
 
-template <bool UP>
-__device__ __forceinline__ void convert_smem(uint32_t in_smem, uint32_t out_smem, uint32_t src_bytes, int lane);
-template <bool UP>
-__device__ __forceinline__ void warp_cast_simt(uint8_t* dst, const uint8_t* src, uint32_t src_bytes, int lane);
+template <bool UP, bool SCALED>
+__device__ __forceinline__ void convert_smem(uint32_t in_smem, uint32_t out_smem, uint32_t src_bytes, int lane, const ptx::Scale& scale);
+template <bool UP, bool SCALED>
+__device__ __forceinline__ void warp_cast_simt(uint8_t* dst, const uint8_t* src, uint32_t src_bytes, int lane, const ptx::Scale& scale);
 
 // ------------------------------------------------------------------------------------------
 // Producer warp.  Gen::get(item, Piece&) is called by up to `batch` lanes at once (one item each).
@@ -265,7 +273,8 @@ __device__ __forceinline__ void warp_cast_simt(uint8_t* dst, const uint8_t* src,
 // no per-layer flags.  A ring is ONE instruction stream per direction, so every instruction of the per-item chain costs
 // its full latency; folding the run-time generality away shortens the chain that bounds the HBM-bound copy
 // (benchmarks/copylab --only libsweep against --only engine).
-template <int CAST, bool FAST, class Gen>
+// SCALED: Piece::layer carries the outer index above bit 16 (CastScales); gating looks at the layer bits only.
+template <int CAST, bool FAST, bool SCALED, class Gen>
 __device__ __forceinline__ void ring_producer(const Gen& gen, uint32_t total, uint32_t my_ring, uint32_t nrings,
                                               const RingSmem& sm, int ndst_rt, const RingParams& rp, const StreamSync& ss)
 {
@@ -323,7 +332,8 @@ __device__ __forceinline__ void ring_producer(const Gen& gen, uint32_t total, ui
     for (uint32_t i = 0; i < cnt; ++i) {
       const uint64_t src_i = __shfl_sync(0xffffffffu, reinterpret_cast<uint64_t>(p.src), i);
       const uint32_t meta_i = __shfl_sync(0xffffffffu, meta, i);
-      const int layer_i = FAST ? 0 : __shfl_sync(0xffffffffu, p.layer, i);
+      const int packed_i = FAST ? 0 : __shfl_sync(0xffffffffu, p.layer, i);
+      const int layer_i = SCALED ? (packed_i & 0xffff) : packed_i;
       uint64_t dst_i[kMaxDst];
 #pragma unroll
       for (int d = 0; d < kMaxDst; ++d)
@@ -342,7 +352,7 @@ __device__ __forceinline__ void ring_producer(const Gen& gen, uint32_t total, ui
 #pragma unroll
         for (int d = 0; d < kMaxDst; ++d)
           if (d < ndst) c.dst[d] = dst_i[d];
-        c.layer = static_cast<uint32_t>(layer_i);
+        c.layer = static_cast<uint32_t>(packed_i);
         c.bytes = meta_i;
         const uint32_t bytes_i = meta_i & ~kSlotTma;
         const bool load = (meta_i & kSlotTma) != 0 && variant != 3;
@@ -378,8 +388,9 @@ __device__ __forceinline__ void ring_producer(const Gen& gen, uint32_t total, ui
 // layer, it drains its stores and adds what it finished to the layer's counter -- so a receiver that releases
 // layer l+1 only after seeing layer l done can never dead-lock against a producer blocked on l+1's gate.
 // ------------------------------------------------------------------------------------------
-template <int CAST, bool FAST>
-__device__ __forceinline__ void ring_consumer(const RingSmem& sm, int ndst_rt, const RingParams& rp, const StreamSync& ss)
+template <int CAST, bool FAST, bool SCALED>
+__device__ __forceinline__ void ring_consumer(const RingSmem& sm, int ndst_rt, const RingParams& rp, const StreamSync& ss,
+                                              const CastScales& cs)
 {
   const int lane = threadIdx.x & 31;
   const int ndst = FAST ? 1 : ndst_rt;
@@ -438,7 +449,9 @@ __device__ __forceinline__ void ring_consumer(const RingSmem& sm, int ndst_rt, c
     const uint32_t meta_bytes = c.bytes;
     const uint32_t bytes = meta_bytes & ~kSlotTma;
     const bool tma = (meta_bytes & kSlotTma) != 0;
-    const int layer = static_cast<int>(meta_layer);
+    const int layer = SCALED ? static_cast<int>(meta_layer & 0xffffu) : static_cast<int>(meta_layer);
+    ptx::Scale scale{1.f, 1.f};
+    if constexpr (SCALED) scale = ptx::make_scale(__ldg(cs.scales + static_cast<uint32_t>(layer) * cs.outer_dim + (meta_layer >> 16)));
     const uint32_t in = sm.in0 + slot * rp.tile_in;
     if (want_layers && unpublished != 0 && layer != cur_layer) publish(q);
     cur_layer = layer;
@@ -453,7 +466,7 @@ __device__ __forceinline__ void ring_consumer(const RingSmem& sm, int ndst_rt, c
         else if (CAST == 0)
           warp_copy_simt(dst, src, bytes, lane);
         else
-          warp_cast_simt<CAST == 1>(dst, src, bytes, lane);
+          warp_cast_simt<CAST == 1, SCALED>(dst, src, bytes, lane, scale);
       }
       __syncwarp();
       if (lane == 0) {
@@ -497,14 +510,23 @@ __device__ __forceinline__ void ring_consumer(const RingSmem& sm, int ndst_rt, c
       const uint32_t ob = sm.out0 + (q & 1) * rp.tile_out;
       if (lane == 0) ptx::bulk_wait_read<1>();  // store q-2 (same out buffer) has been read out
       __syncwarp();
-      convert_smem<CAST == 1>(in, ob, bytes, lane);
+      convert_smem<CAST == 1, SCALED>(in, ob, bytes, lane, scale);
       ptx::fence_proxy_async_smem();
       __syncwarp();
       if (lane == 0) {
+        // SCALED rings take the destinations out of the slot's control block before handing the slot back: once it is back
+        // the producer may overwrite them, and with several destinations a store issued after the hand-back could read the
+        // next item's address (NOTES item 9)
+        uint64_t dst_addr[kMaxDst];
+        if constexpr (SCALED) {
+#pragma unroll
+          for (int d = 0; d < kMaxDst; ++d)
+            if (d < ndst) dst_addr[d] = c.dst[d];
+        }
         ptx::mbar_arrive(sm.empty0 + 8 * slot);  // the input slot is free as soon as it has been converted
 #pragma unroll
         for (int d = 0; d < kMaxDst; ++d)
-          if (d < ndst) ptx::bulk_s2g(reinterpret_cast<void*>(c.dst[d]), ob, dst_bytes);
+          if (d < ndst) ptx::bulk_s2g(reinterpret_cast<void*>(SCALED ? dst_addr[d] : c.dst[d]), ob, dst_bytes);
         ptx::bulk_commit();
       }
     }
@@ -544,9 +566,9 @@ __device__ __forceinline__ void ring_consumer(const RingSmem& sm, int ndst_rt, c
 // ------------------------------------------------------------------------------------------
 // Conversion helpers of the cast rings.
 // ------------------------------------------------------------------------------------------
-template <bool UP>
+template <bool UP, bool SCALED>
 __device__ __forceinline__ void convert_smem(uint32_t in_smem, uint32_t out_smem, uint32_t src_bytes,
-                                             int lane)
+                                             int lane, const ptx::Scale& scale)
 {
   if (UP) {
     // 16 fp8 in (16 B) -> 16 bf16 out (32 B) per lane-iteration
@@ -557,8 +579,13 @@ __device__ __forceinline__ void convert_smem(uint32_t in_smem, uint32_t out_smem
       uint32_t o[8];
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
-        o[2 * k] = ptx::e4m3x2_to_bf16x2(static_cast<uint16_t>(w[k] & 0xffff));
-        o[2 * k + 1] = ptx::e4m3x2_to_bf16x2(static_cast<uint16_t>(w[k] >> 16));
+        if constexpr (SCALED) {
+          o[2 * k] = ptx::e4m3x2_to_bf16x2_scaled(static_cast<uint16_t>(w[k] & 0xffff), scale);
+          o[2 * k + 1] = ptx::e4m3x2_to_bf16x2_scaled(static_cast<uint16_t>(w[k] >> 16), scale);
+        } else {
+          o[2 * k] = ptx::e4m3x2_to_bf16x2(static_cast<uint16_t>(w[k] & 0xffff));
+          o[2 * k + 1] = ptx::e4m3x2_to_bf16x2(static_cast<uint16_t>(w[k] >> 16));
+        }
       }
       asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(out_smem + 2 * off), "r"(o[0]), "r"(o[1]), "r"(o[2]), "r"(o[3]) : "memory");
       asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(out_smem + 2 * off + 16), "r"(o[4]), "r"(o[5]), "r"(o[6]), "r"(o[7]) : "memory");
@@ -572,35 +599,42 @@ __device__ __forceinline__ void convert_smem(uint32_t in_smem, uint32_t out_smem
       uint32_t w[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
       uint32_t o[4];
 #pragma unroll
-      for (int k = 0; k < 4; ++k)
-        o[k] = static_cast<uint32_t>(ptx::bf16x2_to_e4m3x2(w[2 * k])) |
-               (static_cast<uint32_t>(ptx::bf16x2_to_e4m3x2(w[2 * k + 1])) << 16);
+      for (int k = 0; k < 4; ++k) {
+        if constexpr (SCALED)
+          o[k] = static_cast<uint32_t>(ptx::bf16x2_to_e4m3x2_scaled(w[2 * k], scale)) |
+                 (static_cast<uint32_t>(ptx::bf16x2_to_e4m3x2_scaled(w[2 * k + 1], scale)) << 16);
+        else
+          o[k] = static_cast<uint32_t>(ptx::bf16x2_to_e4m3x2(w[2 * k])) |
+                 (static_cast<uint32_t>(ptx::bf16x2_to_e4m3x2(w[2 * k + 1])) << 16);
+      }
       asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(out_smem + off / 2), "r"(o[0]), "r"(o[1]), "r"(o[2]), "r"(o[3]) : "memory");
     }
   }
 }
 
 // SIMT conversion straight from global to global for pieces TMA cannot take (any alignment).
-template <bool UP>
+template <bool UP, bool SCALED>
 __device__ __forceinline__ void warp_cast_simt(uint8_t* dst, const uint8_t* src, uint32_t src_bytes,
-                                               int lane)
+                                               int lane, const ptx::Scale& scale)
 {
+  auto up = [&](uint16_t two) { return SCALED ? ptx::e4m3x2_to_bf16x2_scaled(two, scale) : ptx::e4m3x2_to_bf16x2(two); };
+  auto down = [&](uint32_t two) { return SCALED ? ptx::bf16x2_to_e4m3x2_scaled(two, scale) : ptx::bf16x2_to_e4m3x2(two); };
   if (UP) {
     uint16_t* d = reinterpret_cast<uint16_t*>(dst);
     const uint32_t pairs = src_bytes >> 1;
     for (uint32_t i = lane; i < pairs; i += 32) {
       uint16_t two = static_cast<uint16_t>(src[2 * i]) | (static_cast<uint16_t>(src[2 * i + 1]) << 8);
-      uint32_t r = ptx::e4m3x2_to_bf16x2(two);
+      uint32_t r = up(two);
       d[2 * i] = static_cast<uint16_t>(r & 0xffff);
       d[2 * i + 1] = static_cast<uint16_t>(r >> 16);
     }
     if ((src_bytes & 1) && lane == 0)
-      d[src_bytes - 1] = static_cast<uint16_t>(ptx::e4m3x2_to_bf16x2(src[src_bytes - 1]) & 0xffff);
+      d[src_bytes - 1] = static_cast<uint16_t>(up(src[src_bytes - 1]) & 0xffff);
   } else {
     const uint16_t* s = reinterpret_cast<const uint16_t*>(src);
     const uint32_t elems = src_bytes >> 1;
     for (uint32_t i = lane; i < elems; i += 32)
-      dst[i] = static_cast<uint8_t>(ptx::bf16x2_to_e4m3x2(s[i]) & 0xff);
+      dst[i] = static_cast<uint8_t>(down(s[i]) & 0xff);
   }
 }
 
@@ -612,9 +646,9 @@ __host__ __device__ constexpr uint32_t cta_smem_bytes(int R, int S, uint32_t til
   return static_cast<uint32_t>(R) * (ring_ctl_bytes() + static_cast<uint32_t>(S) * tile_in + 2u * tile_out);
 }
 
-template <int CAST, bool FAST, class Gen>
+template <int CAST, bool FAST, bool SCALED = false, class Gen>
 __device__ __forceinline__ void run_rings(uint8_t* smem, const Gen& gen, uint32_t total, int ndst, const RingParams& rp,
-                                          const StreamSync& ss)
+                                          const StreamSync& ss, const CastScales& cs = CastScales{})
 {
   const int warp = threadIdx.x >> 5;
   const int R = blockDim.x >> 6;
@@ -639,9 +673,9 @@ __device__ __forceinline__ void run_rings(uint8_t* smem, const Gen& gen, uint32_
   const uint32_t nrings = gridDim.x * R;
   const uint32_t my_ring = blockIdx.x * R + ring;
   if (producer)
-    ring_producer<CAST, FAST>(gen, total, my_ring, nrings, sm, ndst, rp, ss);
+    ring_producer<CAST, FAST, SCALED>(gen, total, my_ring, nrings, sm, ndst, rp, ss);
   else
-    ring_consumer<CAST, FAST>(sm, ndst, rp, ss);
+    ring_consumer<CAST, FAST, SCALED>(sm, ndst, rp, ss, cs);
 }
 
 }  // namespace kvbm

@@ -236,6 +236,8 @@ struct PagedArgs {
   uint32_t dst_num, dst_den;  // destination bytes = source bytes * dst_num / dst_den (cast)
 };
 
+// PACK_OUTER (a scaled cast): Piece::layer = layer | o << 16, so the consumer can find the (layer, outer) scale (CastScales).
+template <bool PACK_OUTER>
 struct PagedGen {
   PagedArgs a;
   // item order (layer-major so a layer completes early for streaming):
@@ -262,7 +264,7 @@ struct PagedGen {
     const uint64_t soff = static_cast<uint64_t>(t) * a.tile;
     const uint32_t left = a.src.region_bytes - static_cast<uint32_t>(soff);
     p.bytes = left < a.tile ? left : a.tile;
-    p.layer = static_cast<int>(layer);
+    p.layer = PACK_OUTER ? static_cast<int>(layer | (o << 16)) : static_cast<int>(layer);
     const uint64_t doff = soff * a.dst_num / a.dst_den;
     const int32_t sb = __ldg(a.src_ids[d] + blk);
     p.src = reinterpret_cast<const uint8_t*>(__ldg(a.src.layer_base + layer) + static_cast<uint64_t>(sb) * a.src.block_stride +
@@ -339,18 +341,19 @@ __device__ __forceinline__ StreamSync make_sync(const PagedSyncArgs& s, const Pa
   return ss;
 }
 
-template <int CAST, bool FAST>
+// SCALED: the cast applies scales[layer * outer + o] (kvbm_paged_copy_opts.cast_scales); only with a cast, never FAST.
+template <int CAST, bool FAST, bool SCALED = false>
 __global__ void __launch_bounds__(512, 1)
-kvbm_paged_copy_kernel(const __grid_constant__ PagedGen gen, const __grid_constant__ PagedSyncArgs sync,
+kvbm_paged_copy_kernel(const __grid_constant__ PagedGen<SCALED> gen, const __grid_constant__ PagedSyncArgs sync,
                        uint32_t total, int S, int P, int batch, int static_schedule, uint32_t out_tile, int allow_tma, int cache_hint,
-                       int variant)
+                       int variant, const float* scales)
 {
   extern __shared__ __align__(128) uint8_t smem[];
   const int R = blockDim.x >> 6;
   const int ring_ndst = gen.a.replicate ? gen.a.ndst : 1;
   const StreamSync ss = make_sync(sync, gen.a, total, R);
   RingParams rp{S, P, batch, gen.a.tile, out_tile, allow_tma != 0, static_schedule != 0, cache_hint, CAST == KVBM_CAST_NONE ? variant : 0};
-  run_rings<CAST, FAST>(smem, gen, total, ring_ndst, rp, ss);
+  run_rings<CAST, FAST, SCALED>(smem, gen, total, ring_ndst, rp, ss, CastScales{scales, gen.a.outer});
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -509,27 +512,40 @@ __device__ __forceinline__ uint32_t row_offset(const RowSplit& r, uint32_t v, ui
   return t * tok_stride + (c << SHIFT);
 }
 
-// One vector of a cast walk: 16 e4m3 codes <-> 16 bf16, bit for bit the conversions of the paged copy's cast rings.
-// in[0 .. IN) are the 16 B loads of the source side, out[0 .. OUT) the 16 B stores of the destination side.
-__device__ __forceinline__ void cast_vector_up(const uint4 (&in)[1], uint4 (&out)[2])
+// One vector of a cast walk: 16 e4m3 codes <-> 16 bf16, bit for bit the conversions of the paged copy's cast rings (SCALED:
+// its scaled conversions with the unit's scale).  in[0 .. IN) are the 16 B loads of the source side, out[0 .. OUT) the 16 B
+// stores of the destination side.
+template <bool SCALED>
+__device__ __forceinline__ void cast_vector_up(const uint4 (&in)[1], uint4 (&out)[2], const ptx::Scale& scale)
 {
   const uint32_t w[4] = {in[0].x, in[0].y, in[0].z, in[0].w};
   uint32_t o[8];
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
-    o[2 * k] = ptx::e4m3x2_to_bf16x2(static_cast<uint16_t>(w[k] & 0xffff));
-    o[2 * k + 1] = ptx::e4m3x2_to_bf16x2(static_cast<uint16_t>(w[k] >> 16));
+    if constexpr (SCALED) {
+      o[2 * k] = ptx::e4m3x2_to_bf16x2_scaled(static_cast<uint16_t>(w[k] & 0xffff), scale);
+      o[2 * k + 1] = ptx::e4m3x2_to_bf16x2_scaled(static_cast<uint16_t>(w[k] >> 16), scale);
+    } else {
+      o[2 * k] = ptx::e4m3x2_to_bf16x2(static_cast<uint16_t>(w[k] & 0xffff));
+      o[2 * k + 1] = ptx::e4m3x2_to_bf16x2(static_cast<uint16_t>(w[k] >> 16));
+    }
   }
   out[0] = make_uint4(o[0], o[1], o[2], o[3]);
   out[1] = make_uint4(o[4], o[5], o[6], o[7]);
 }
-__device__ __forceinline__ void cast_vector_down(const uint4 (&in)[2], uint4 (&out)[1])
+template <bool SCALED>
+__device__ __forceinline__ void cast_vector_down(const uint4 (&in)[2], uint4 (&out)[1], const ptx::Scale& scale)
 {
   const uint32_t w[8] = {in[0].x, in[0].y, in[0].z, in[0].w, in[1].x, in[1].y, in[1].z, in[1].w};
   uint32_t o[4];
 #pragma unroll
-  for (int k = 0; k < 4; ++k)
-    o[k] = static_cast<uint32_t>(ptx::bf16x2_to_e4m3x2(w[2 * k])) | (static_cast<uint32_t>(ptx::bf16x2_to_e4m3x2(w[2 * k + 1])) << 16);
+  for (int k = 0; k < 4; ++k) {
+    if constexpr (SCALED)
+      o[k] = static_cast<uint32_t>(ptx::bf16x2_to_e4m3x2_scaled(w[2 * k], scale)) |
+             (static_cast<uint32_t>(ptx::bf16x2_to_e4m3x2_scaled(w[2 * k + 1], scale)) << 16);
+    else
+      o[k] = static_cast<uint32_t>(ptx::bf16x2_to_e4m3x2(w[2 * k])) | (static_cast<uint32_t>(ptx::bf16x2_to_e4m3x2(w[2 * k + 1])) << 16);
+  }
   out[0] = make_uint4(o[0], o[1], o[2], o[3]);
 }
 
@@ -538,10 +554,12 @@ __device__ __forceinline__ void cast_vector_down(const uint4 (&in)[2], uint4 (&o
 // a head is predicated rather than a serial tail: for head_dim 64 ... 96 in bf16 it is the whole head, and its loads stay
 // independent.  With a cast (KVBM_CAST_*) the walk counts 16 B vectors of the fp8 side's row: one vector is 16 elements,
 // 16 B on the fp8 side and 32 B on the bf16 side, so fp8 -> bf16 turns one load into two stores and bf16 -> fp8 two loads
-// into one store.  Every lane keeps 8 independent 16 B loads in flight in all three forms.
-template <int CAST, bool POW2>
+// into one store.  Every lane keeps 8 independent 16 B loads in flight in all three forms.  SCALED: the cast applies `scale`,
+// the fp8 side's dequantisation scale of the unit (one (block, layer, outer), so one scale).
+template <int CAST, bool POW2, bool SCALED = false>
 __device__ __forceinline__ void walk_head_rows(const uint8_t* sb, uint64_t s_head, uint32_t s_tok, uint8_t* db, uint64_t d_head,
-                                               uint32_t d_tok, uint32_t h0, uint32_t hstep, uint32_t nh, uint32_t nt, const RowSplit& r)
+                                               uint32_t d_tok, uint32_t h0, uint32_t hstep, uint32_t nh, uint32_t nt, const RowSplit& r,
+                                               const ptx::Scale& scale = ptx::Scale{1.f, 1.f})
 {
   constexpr int IN = CAST == KVBM_CAST_BF16_TO_FP8E4M3 ? 2 : 1;   // 16 B loads per vector
   constexpr int OUT = CAST == KVBM_CAST_FP8E4M3_TO_BF16 ? 2 : 1;  // 16 B stores per vector
@@ -569,9 +587,9 @@ __device__ __forceinline__ void walk_head_rows(const uint8_t* sb, uint64_t s_hea
           } else {
             uint4 y[OUT];
             if constexpr (CAST == KVBM_CAST_FP8E4M3_TO_BF16)
-              cast_vector_up(x[k], y);
+              cast_vector_up<SCALED>(x[k], y, scale);
             else
-              cast_vector_down(x[k], y);
+              cast_vector_down<SCALED>(x[k], y, scale);
 #pragma unroll
             for (int i = 0; i < OUT; ++i) ptx::st_stream_v4(d + 16 * i, y[i]);
           }
@@ -621,11 +639,12 @@ kvbm_permute_table_kernel(void* const* __restrict__ universal_ptrs, void* const*
 // its own head count).  nh heads of every unit move: source heads from s_win / head_stride on, destination heads from
 // d_win / head_stride on (s_win, d_win: the head windows' byte offsets; 0 for every head of both sides).  One CTA per
 // (block pair, layer, outer), also for a window of one head: packing several units of a narrow window into one CTA measured
-// no faster (DESIGN §4.2b).
-template <int CAST, bool POW2>
+// no faster (DESIGN §4.2b).  SCALED: the cast applies scales[l * no + o], loaded once per CTA.
+template <int CAST, bool POW2, bool SCALED = false>
 __global__ void __launch_bounds__(256)
 kvbm_paged_permute_kernel(const __grid_constant__ PermuteSide S, const __grid_constant__ PermuteSide D, uint32_t layer_begin,
-                          uint32_t nlayers, uint32_t no, uint32_t nh, uint32_t nt, RowSplit r, uint64_t s_win, uint64_t d_win)
+                          uint32_t nlayers, uint32_t no, uint32_t nh, uint32_t nt, RowSplit r, uint64_t s_win, uint64_t d_win,
+                          const float* scales)
 {
   const uint32_t unit = blockIdx.x;  // (pair * nlayers + l) * no + o
   const uint32_t pair = unit / (nlayers * no);
@@ -635,8 +654,9 @@ kvbm_paged_permute_kernel(const __grid_constant__ PermuteSide S, const __grid_co
     return reinterpret_cast<uint8_t*>(static_cast<uintptr_t>(__ldg(X.layer_base + (X.universal ? 0 : l)))) +
            static_cast<uint64_t>(__ldg(X.ids + pair)) * X.block_stride + l * X.layer_step + o * X.outer_step;
   };
-  walk_head_rows<CAST, POW2>(base_of(S) + s_win, S.head_stride, S.tok_stride, base_of(D) + d_win, D.head_stride, D.tok_stride,
-                             threadIdx.x >> 5, blockDim.x >> 5, nh, nt, r);
+  const ptx::Scale scale = ptx::make_scale(SCALED ? __ldg(scales + l * no + o) : 1.f);
+  walk_head_rows<CAST, POW2, SCALED>(base_of(S) + s_win, S.head_stride, S.tok_stride, base_of(D) + d_win, D.head_stride, D.tok_stride,
+                                     threadIdx.x >> 5, blockDim.x >> 5, nh, nt, r, scale);
 }
 
 // The gather: several sources, each with its own pool, format, head count and head window, into one destination.  The
@@ -657,10 +677,11 @@ struct GatherParams {
 // One CTA per destination (block, layer, outer) unit, as the paged permute, with one warp per covered destination head
 // (looping by the CTA's warps past 8): every source's window of the unit is written by the same CTA, so a destination row
 // that holds every head (OperationalNHD) is written whole by one CTA.  Each warp looks up its source and runs the same walk
-// over one head.
-template <int CAST, bool POW2>
+// over one head.  SCALED: one scale array for every source, scales[l * no + o] loaded once per CTA.
+template <int CAST, bool POW2, bool SCALED = false>
 __global__ void __launch_bounds__(256)
-kvbm_paged_gather_kernel(const __grid_constant__ GatherParams P, uint32_t layer_begin, uint32_t nlayers, uint32_t no, uint32_t nt, RowSplit r)
+kvbm_paged_gather_kernel(const __grid_constant__ GatherParams P, uint32_t layer_begin, uint32_t nlayers, uint32_t no, uint32_t nt, RowSplit r,
+                         const float* scales)
 {
   const uint32_t unit = blockIdx.x;  // (pair * nlayers + l) * no + o
   const uint32_t pair = unit / (nlayers * no);
@@ -671,11 +692,12 @@ kvbm_paged_gather_kernel(const __grid_constant__ GatherParams P, uint32_t layer_
            static_cast<uint64_t>(__ldg(X.ids + pair)) * X.block_stride + l * X.layer_step + o * X.outer_step;
   };
   uint8_t* db = base_of(P.D);
+  const ptx::Scale scale = ptx::make_scale(SCALED ? __ldg(scales + l * no + o) : 1.f);
   for (uint32_t j = threadIdx.x >> 5; j < P.covered; j += blockDim.x >> 5) {
     const GatherSource& G = P.src[P.entry[j]];
     const uint32_t h = j - G.first;  // head h of the window: walk heads h .. h of the window's bases
-    walk_head_rows<CAST, POW2>(base_of(G.S) + G.s_win, G.S.head_stride, G.S.tok_stride, db + G.d_win, P.D.head_stride, P.D.tok_stride,
-                               h, 1, h + 1, nt, r);
+    walk_head_rows<CAST, POW2, SCALED>(base_of(G.S) + G.s_win, G.S.head_stride, G.S.tok_stride, db + G.d_win, P.D.head_stride,
+                                       P.D.tok_stride, h, 1, h + 1, nt, r, scale);
   }
 }
 
@@ -800,6 +822,8 @@ static cudaError_t preload_kernels()
   KVBM_PRELOAD((kvbm_paged_copy_kernel<KVBM_CAST_NONE, true>))
   KVBM_PRELOAD((kvbm_paged_copy_kernel<KVBM_CAST_FP8E4M3_TO_BF16, true>))
   KVBM_PRELOAD((kvbm_paged_copy_kernel<KVBM_CAST_BF16_TO_FP8E4M3, true>))
+  KVBM_PRELOAD((kvbm_paged_copy_kernel<KVBM_CAST_FP8E4M3_TO_BF16, false, true>))
+  KVBM_PRELOAD((kvbm_paged_copy_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false, true>))
   KVBM_PRELOAD(kvbm_set_flags_kernel)
   KVBM_PRELOAD(kvbm_wait_flag_kernel)
   KVBM_PRELOAD((kvbm_paged_permute_kernel<KVBM_CAST_NONE, true>))
@@ -808,12 +832,20 @@ static cudaError_t preload_kernels()
   KVBM_PRELOAD((kvbm_paged_permute_kernel<KVBM_CAST_FP8E4M3_TO_BF16, false>))
   KVBM_PRELOAD((kvbm_paged_permute_kernel<KVBM_CAST_BF16_TO_FP8E4M3, true>))
   KVBM_PRELOAD((kvbm_paged_permute_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false>))
+  KVBM_PRELOAD((kvbm_paged_permute_kernel<KVBM_CAST_FP8E4M3_TO_BF16, true, true>))
+  KVBM_PRELOAD((kvbm_paged_permute_kernel<KVBM_CAST_FP8E4M3_TO_BF16, false, true>))
+  KVBM_PRELOAD((kvbm_paged_permute_kernel<KVBM_CAST_BF16_TO_FP8E4M3, true, true>))
+  KVBM_PRELOAD((kvbm_paged_permute_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false, true>))
   KVBM_PRELOAD((kvbm_paged_gather_kernel<KVBM_CAST_NONE, true>))
   KVBM_PRELOAD((kvbm_paged_gather_kernel<KVBM_CAST_NONE, false>))
   KVBM_PRELOAD((kvbm_paged_gather_kernel<KVBM_CAST_FP8E4M3_TO_BF16, true>))
   KVBM_PRELOAD((kvbm_paged_gather_kernel<KVBM_CAST_FP8E4M3_TO_BF16, false>))
   KVBM_PRELOAD((kvbm_paged_gather_kernel<KVBM_CAST_BF16_TO_FP8E4M3, true>))
   KVBM_PRELOAD((kvbm_paged_gather_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false>))
+  KVBM_PRELOAD((kvbm_paged_gather_kernel<KVBM_CAST_FP8E4M3_TO_BF16, true, true>))
+  KVBM_PRELOAD((kvbm_paged_gather_kernel<KVBM_CAST_FP8E4M3_TO_BF16, false, true>))
+  KVBM_PRELOAD((kvbm_paged_gather_kernel<KVBM_CAST_BF16_TO_FP8E4M3, true, true>))
+  KVBM_PRELOAD((kvbm_paged_gather_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false, true>))
   KVBM_PRELOAD(kvbm_signal_kernel)
   KVBM_PRELOAD(kvbm_permute_table_kernel<true>)
   KVBM_PRELOAD(kvbm_permute_table_kernel<false>)
@@ -1006,8 +1038,21 @@ kvbm_kernels_paged_permute_heads(const kvbm_permute_side* src, const kvbm_permut
                                  uint32_t* done_flag, uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value,
                                  cudaStream_t stream)
 {
+  return kvbm_kernels_paged_permute_heads_scaled(src, dst, num_blocks, layer_begin, layer_end, src_num_heads, src_head_begin, dst_num_heads,
+                                                 dst_head_begin, head_count, page_size, src_row_bytes, cast_mode, nullptr, done_flag, epoch,
+                                                 completion_flag, completion_value, stream);
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_permute_heads_scaled(const kvbm_permute_side* src, const kvbm_permute_side* dst, int num_blocks, int layer_begin,
+                                        int layer_end, uint32_t src_num_heads, uint32_t src_head_begin, uint32_t dst_num_heads,
+                                        uint32_t dst_head_begin, uint32_t head_count, uint32_t page_size, uint32_t src_row_bytes,
+                                        int cast_mode, const float* cast_scales, uint32_t* done_flag, uint32_t epoch,
+                                        uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
+{
   if (num_blocks < 0 || layer_begin < 0 || layer_end < layer_begin) return cudaErrorInvalidValue;
   if (cast_mode < KVBM_CAST_NONE || cast_mode > KVBM_CAST_BF16_TO_FP8E4M3) return cudaErrorInvalidValue;
+  if (cast_scales && cast_mode == KVBM_CAST_NONE) return cudaErrorInvalidValue;  // scales belong to the fp8 side of a cast
   const bool signal = done_flag || completion_flag;
   auto finish = [&]() -> cudaError_t {
     if (!signal) return cudaSuccess;
@@ -1041,16 +1086,23 @@ kvbm_kernels_paged_permute_heads(const kvbm_permute_side* src, const kvbm_permut
   const unsigned grid = static_cast<unsigned>(units);
   const uint32_t lb = static_cast<uint32_t>(layer_begin), nlay = static_cast<uint32_t>(layer_end - layer_begin);
   const uint64_t s_win = src_head_begin * S.head_stride, d_win = dst_head_begin * D.head_stride;  // the windows' first heads
-  auto go = [&](auto kern) { kern<<<grid, threads, 0, stream>>>(S, D, lb, nlay, no, head_count, page_size, r, s_win, d_win); };
+  auto go = [&](auto kern) { kern<<<grid, threads, 0, stream>>>(S, D, lb, nlay, no, head_count, page_size, r, s_win, d_win, cast_scales); };
+  const bool sc = cast_scales != nullptr;
   switch (cast_mode) {
     case KVBM_CAST_NONE:
       r.pow2 ? go(kvbm_paged_permute_kernel<KVBM_CAST_NONE, true>) : go(kvbm_paged_permute_kernel<KVBM_CAST_NONE, false>);
       break;
     case KVBM_CAST_FP8E4M3_TO_BF16:
-      r.pow2 ? go(kvbm_paged_permute_kernel<KVBM_CAST_FP8E4M3_TO_BF16, true>) : go(kvbm_paged_permute_kernel<KVBM_CAST_FP8E4M3_TO_BF16, false>);
+      if (sc)
+        r.pow2 ? go(kvbm_paged_permute_kernel<KVBM_CAST_FP8E4M3_TO_BF16, true, true>) : go(kvbm_paged_permute_kernel<KVBM_CAST_FP8E4M3_TO_BF16, false, true>);
+      else
+        r.pow2 ? go(kvbm_paged_permute_kernel<KVBM_CAST_FP8E4M3_TO_BF16, true>) : go(kvbm_paged_permute_kernel<KVBM_CAST_FP8E4M3_TO_BF16, false>);
       break;
     default:
-      r.pow2 ? go(kvbm_paged_permute_kernel<KVBM_CAST_BF16_TO_FP8E4M3, true>) : go(kvbm_paged_permute_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false>);
+      if (sc)
+        r.pow2 ? go(kvbm_paged_permute_kernel<KVBM_CAST_BF16_TO_FP8E4M3, true, true>) : go(kvbm_paged_permute_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false, true>);
+      else
+        r.pow2 ? go(kvbm_paged_permute_kernel<KVBM_CAST_BF16_TO_FP8E4M3, true>) : go(kvbm_paged_permute_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false>);
       break;
   }
   g_launches.fetch_add(1, std::memory_order_relaxed);
@@ -1065,8 +1117,20 @@ kvbm_kernels_paged_permute_gather(const kvbm_permute_source* srcs, int num_srcs,
                                   int cast_mode, uint32_t* done_flag, uint32_t epoch, uint32_t* completion_flag,
                                   uint32_t completion_value, cudaStream_t stream)
 {
+  return kvbm_kernels_paged_permute_gather_scaled(srcs, num_srcs, dst, dst_num_heads, num_blocks, layer_begin, layer_end, page_size,
+                                                  src_row_bytes, cast_mode, nullptr, done_flag, epoch, completion_flag, completion_value,
+                                                  stream);
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_permute_gather_scaled(const kvbm_permute_source* srcs, int num_srcs, const kvbm_permute_side* dst,
+                                         uint32_t dst_num_heads, int num_blocks, int layer_begin, int layer_end, uint32_t page_size,
+                                         uint32_t src_row_bytes, int cast_mode, const float* cast_scales, uint32_t* done_flag,
+                                         uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
+{
   if (num_blocks < 0 || layer_begin < 0 || layer_end < layer_begin) return cudaErrorInvalidValue;
   if (cast_mode < KVBM_CAST_NONE || cast_mode > KVBM_CAST_BF16_TO_FP8E4M3) return cudaErrorInvalidValue;
+  if (cast_scales && cast_mode == KVBM_CAST_NONE) return cudaErrorInvalidValue;
   if (!srcs || num_srcs < 1 || num_srcs > KVBM_GATHER_MAX_SOURCES) return cudaErrorInvalidValue;
   const bool signal = done_flag || completion_flag;
   auto finish = [&]() -> cudaError_t {
@@ -1117,16 +1181,23 @@ kvbm_kernels_paged_permute_gather(const kvbm_permute_source* srcs, int num_srcs,
   const int threads = static_cast<int>(std::min<uint32_t>(8, covered)) * 32;
   const unsigned grid = static_cast<unsigned>(units);
   const uint32_t lb = static_cast<uint32_t>(layer_begin), nlay = static_cast<uint32_t>(layer_end - layer_begin);
-  auto go = [&](auto kern) { kern<<<grid, threads, 0, stream>>>(P, lb, nlay, no, page_size, r); };
+  auto go = [&](auto kern) { kern<<<grid, threads, 0, stream>>>(P, lb, nlay, no, page_size, r, cast_scales); };
+  const bool sc = cast_scales != nullptr;
   switch (cast_mode) {
     case KVBM_CAST_NONE:
       r.pow2 ? go(kvbm_paged_gather_kernel<KVBM_CAST_NONE, true>) : go(kvbm_paged_gather_kernel<KVBM_CAST_NONE, false>);
       break;
     case KVBM_CAST_FP8E4M3_TO_BF16:
-      r.pow2 ? go(kvbm_paged_gather_kernel<KVBM_CAST_FP8E4M3_TO_BF16, true>) : go(kvbm_paged_gather_kernel<KVBM_CAST_FP8E4M3_TO_BF16, false>);
+      if (sc)
+        r.pow2 ? go(kvbm_paged_gather_kernel<KVBM_CAST_FP8E4M3_TO_BF16, true, true>) : go(kvbm_paged_gather_kernel<KVBM_CAST_FP8E4M3_TO_BF16, false, true>);
+      else
+        r.pow2 ? go(kvbm_paged_gather_kernel<KVBM_CAST_FP8E4M3_TO_BF16, true>) : go(kvbm_paged_gather_kernel<KVBM_CAST_FP8E4M3_TO_BF16, false>);
       break;
     default:
-      r.pow2 ? go(kvbm_paged_gather_kernel<KVBM_CAST_BF16_TO_FP8E4M3, true>) : go(kvbm_paged_gather_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false>);
+      if (sc)
+        r.pow2 ? go(kvbm_paged_gather_kernel<KVBM_CAST_BF16_TO_FP8E4M3, true, true>) : go(kvbm_paged_gather_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false, true>);
+      else
+        r.pow2 ? go(kvbm_paged_gather_kernel<KVBM_CAST_BF16_TO_FP8E4M3, true>) : go(kvbm_paged_gather_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false>);
       break;
   }
   g_launches.fetch_add(1, std::memory_order_relaxed);
@@ -1181,7 +1252,11 @@ paged_copy_impl(const kvbm_paged_layout* src, const kvbm_paged_dst* dsts, int nu
     return cudaErrorInvalidValue;
   const int data_dsts = mc ? 1 : num_dsts;
 
-  PagedGen gen{};
+  // a scaled cast packs the outer index above the layer of every item (CastScales)
+  const float* scales = o.cast_scales;
+  if (scales && (src->num_layers > 65536 || src->outer_dim > 32768)) return cudaErrorInvalidValue;
+
+  PagedGen<false> gen{};
   PagedSyncArgs sync{};
   gen.a.src = *src;
   gen.a.ndst = data_dsts;
@@ -1249,11 +1324,11 @@ paged_copy_impl(const kvbm_paged_layout* src, const kvbm_paged_dst* dsts, int nu
     sync.ctl = sched_acquire(dev, stream, &pool_slot);
   }
 
-  auto launch = [&](auto kern) -> cudaError_t {
+  auto launch = [&](auto kern, const auto& g) -> cudaError_t {
     cudaError_t err = set_smem(kern, rc.smem);
     if (err == cudaSuccess) {
-      kern<<<grid, rc.rings * 64, rc.smem, stream>>>(gen, sync, total32, rc.stages, rc.pending, rc.batch, o.static_schedule,
-                                                     rc.out_tile, allow_tma, o.cache_hint, mc ? (o.multicast == 2 ? 0 : 4) : o.variant);
+      kern<<<grid, rc.rings * 64, rc.smem, stream>>>(g, sync, total32, rc.stages, rc.pending, rc.batch, o.static_schedule,
+                                                     rc.out_tile, allow_tma, o.cache_hint, mc ? (o.multicast == 2 ? 0 : 4) : o.variant, scales);
       g_launches.fetch_add(1, std::memory_order_relaxed);
       err = cudaGetLastError();
     }
@@ -1265,13 +1340,17 @@ paged_copy_impl(const kvbm_paged_layout* src, const kvbm_paged_dst* dsts, int nu
   for (int d = 0; d < num_dsts; ++d) any_layer_flags = any_layer_flags || dsts[d].layer_done_flags != nullptr;
   const bool fast = !mc && o.variant == 0 && o.cache_hint == 0 && allow_tma && !o.layer_ready_flags && !any_layer_flags &&
                     (gen.a.replicate ? data_dsts : 1) == 1;
+  // a scaled cast takes the general rings (its own instantiation), whatever `fast` says
+  const PagedGen<true> sgen{gen.a};
   switch (cast_mode) {
     case KVBM_CAST_NONE:
-      return fast ? launch(kvbm_paged_copy_kernel<KVBM_CAST_NONE, true>) : launch(kvbm_paged_copy_kernel<KVBM_CAST_NONE, false>);
+      return fast ? launch(kvbm_paged_copy_kernel<KVBM_CAST_NONE, true>, gen) : launch(kvbm_paged_copy_kernel<KVBM_CAST_NONE, false>, gen);
     case KVBM_CAST_FP8E4M3_TO_BF16:
-      return fast ? launch(kvbm_paged_copy_kernel<KVBM_CAST_FP8E4M3_TO_BF16, true>) : launch(kvbm_paged_copy_kernel<KVBM_CAST_FP8E4M3_TO_BF16, false>);
+      if (scales) return launch(kvbm_paged_copy_kernel<KVBM_CAST_FP8E4M3_TO_BF16, false, true>, sgen);
+      return fast ? launch(kvbm_paged_copy_kernel<KVBM_CAST_FP8E4M3_TO_BF16, true>, gen) : launch(kvbm_paged_copy_kernel<KVBM_CAST_FP8E4M3_TO_BF16, false>, gen);
     default:
-      return fast ? launch(kvbm_paged_copy_kernel<KVBM_CAST_BF16_TO_FP8E4M3, true>) : launch(kvbm_paged_copy_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false>);
+      if (scales) return launch(kvbm_paged_copy_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false, true>, sgen);
+      return fast ? launch(kvbm_paged_copy_kernel<KVBM_CAST_BF16_TO_FP8E4M3, true>, gen) : launch(kvbm_paged_copy_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false>, gen);
   }
 }
 
@@ -1307,6 +1386,7 @@ kvbm_kernels_paged_copy_v2(const kvbm_paged_layout* src, const kvbm_paged_dst* d
                            int layer_begin, int layer_end, int cast_mode, const kvbm_paged_copy_opts* opts,
                            cudaStream_t stream)
 {
+  if (opts && opts->cast_scales && cast_mode == KVBM_CAST_NONE) return cudaErrorInvalidValue;  // scales belong to a cast's fp8 side
   const bool gated = opts && opts->layer_ready_flags != nullptr;
   if (!gated || num_blocks == 0 || num_dsts == 0 || layer_end <= layer_begin || !dsts || num_dsts < 0 || num_dsts > KVBM_MAX_DESTINATIONS)
     return paged_copy_impl(src, dsts, num_dsts, num_blocks, layer_begin, layer_end, cast_mode, opts, stream);

@@ -128,6 +128,7 @@ class PagedCopyOpts(C.Structure):
         ("multicast", C.c_int),
         ("gate_mode", C.c_int),
         ("static_schedule", C.c_int),
+        ("cast_scales", C.c_void_p),      # device-accessible float[num_layers * outer_dim]: the fp8 side's scales, or None
     ]
 
 
@@ -166,9 +167,16 @@ def lib() -> C.CDLL:
                                                        C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, i, vp, C.c_uint32, vp,
                                                        C.c_uint32, vp]
         L.kvbm_kernels_paged_permute_heads.restype = i
+        L.kvbm_kernels_paged_permute_heads_scaled.argtypes = [C.POINTER(PermuteSide), C.POINTER(PermuteSide), i, i, i, C.c_uint32,
+                                                              C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, i, vp,
+                                                              vp, C.c_uint32, vp, C.c_uint32, vp]
+        L.kvbm_kernels_paged_permute_heads_scaled.restype = i
         L.kvbm_kernels_paged_permute_gather.argtypes = [C.POINTER(PermuteSource), i, C.POINTER(PermuteSide), C.c_uint32, i, i, i, C.c_uint32,
                                                         C.c_uint32, i, vp, C.c_uint32, vp, C.c_uint32, vp]
         L.kvbm_kernels_paged_permute_gather.restype = i
+        L.kvbm_kernels_paged_permute_gather_scaled.argtypes = [C.POINTER(PermuteSource), i, C.POINTER(PermuteSide), C.c_uint32, i, i, i,
+                                                               C.c_uint32, C.c_uint32, i, vp, vp, C.c_uint32, vp, C.c_uint32, vp]
+        L.kvbm_kernels_paged_permute_gather_scaled.restype = i
         L.kvbm_kernels_permute_strides.argtypes = [i, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64, C.c_uint64,
                                                    C.POINTER(C.c_uint64)]
         L.kvbm_kernels_permute_strides.restype = i
@@ -191,8 +199,24 @@ EXPORTED_SYMBOLS = [
     "kvbm_kernels_paged_copy_v2", "kvbm_kernels_set_flags", "kvbm_kernels_wait_flag", "kvbm_kernels_stream_wait_event",
     "kvbm_kernels_launch_count", "kvbm_kernels_build_info", "kvbm_kernels_gate_would_spin", "kvbm_kernels_paged_permute",
     "kvbm_kernels_permute_strides", "kvbm_kernels_paged_permute_cast", "kvbm_kernels_paged_permute_heads",
-    "kvbm_kernels_paged_permute_gather",
+    "kvbm_kernels_paged_permute_gather", "kvbm_kernels_paged_permute_heads_scaled", "kvbm_kernels_paged_permute_gather_scaled",
 ]
+
+
+def scales_ptr(cast_scales) -> Optional[int]:
+    """Address of a cast-scale array: None, an int address, or a contiguous float32 tensor / array (torch: data_ptr(), numpy:
+    ctypes.data).  The array must outlive the launch."""
+    if cast_scales is None or isinstance(cast_scales, int):
+        return cast_scales or None
+    if hasattr(cast_scales, "data_ptr"):
+        import torch
+        if cast_scales.dtype != torch.float32 or not cast_scales.is_contiguous():
+            raise ValueError("cast_scales must be a contiguous float32 tensor")
+        return cast_scales.data_ptr()
+    import numpy as np
+    if cast_scales.dtype != np.float32 or not cast_scales.flags["C_CONTIGUOUS"]:
+        raise ValueError("cast_scales must be a contiguous float32 array")
+    return cast_scales.ctypes.data
 
 GATE_AUTO, GATE_SPIN, GATE_STREAM_WAIT = 0, 1, 2
 
@@ -268,10 +292,17 @@ def paged_permute_cast(src: PermuteSide, dst: PermuteSide, num_blocks: int, laye
 def paged_permute_heads(src: PermuteSide, dst: PermuteSide, num_blocks: int, layer_begin: int, layer_end: int, src_num_heads: int,
                         src_head_begin: int, dst_num_heads: int, dst_head_begin: int, head_count: int, page_size: int, src_row_bytes: int,
                         cast_mode: int = 0, done_flag: int = 0, epoch: int = 0, completion_flag: int = 0, completion_value: int = 0,
-                        stream: int = 0) -> int:
+                        stream: int = 0, cast_scales=None) -> int:
     """`paged_permute_cast` over a head window on each side (a TP re-shard): source heads [src_head_begin, +head_count) land as
     destination heads [dst_head_begin, +head_count); each side has its own head count and every destination byte outside the
-    window keeps its value.  include/kvbm_kernels.h (kvbm_kernels_paged_permute_heads)."""
+    window keeps its value.  `cast_scales` (float32[num_layers * outer_dim] on the device, see `scales_ptr`): the fp8 side's
+    dequantisation scale per (layer, outer), applied by the cast.  include/kvbm_kernels.h (kvbm_kernels_paged_permute_heads,
+    kvbm_kernels_paged_permute_heads_scaled)."""
+    if cast_scales is not None:
+        return lib().kvbm_kernels_paged_permute_heads_scaled(C.byref(src), C.byref(dst), num_blocks, layer_begin, layer_end, src_num_heads,
+                                                             src_head_begin, dst_num_heads, dst_head_begin, head_count, page_size,
+                                                             src_row_bytes, int(cast_mode), scales_ptr(cast_scales), done_flag or None, epoch,
+                                                             completion_flag or None, completion_value, stream)
     return lib().kvbm_kernels_paged_permute_heads(C.byref(src), C.byref(dst), num_blocks, layer_begin, layer_end, src_num_heads,
                                                   src_head_begin, dst_num_heads, dst_head_begin, head_count, page_size, src_row_bytes,
                                                   int(cast_mode), done_flag or None, epoch, completion_flag or None, completion_value, stream)
@@ -279,11 +310,16 @@ def paged_permute_heads(src: PermuteSide, dst: PermuteSide, num_blocks: int, lay
 
 def paged_permute_gather(srcs: Sequence[PermuteSource], dst: PermuteSide, dst_num_heads: int, num_blocks: int, layer_begin: int,
                          layer_end: int, page_size: int, src_row_bytes: int, cast_mode: int = 0, done_flag: int = 0, epoch: int = 0,
-                         completion_flag: int = 0, completion_value: int = 0, stream: int = 0) -> int:
+                         completion_flag: int = 0, completion_value: int = 0, stream: int = 0, cast_scales=None) -> int:
     """`paged_permute_heads` over several sources in ONE launch (a TP re-shard's assembly): each source's head window lands in
     the destination, whose bytes outside the union of the windows keep their values; the flags are written once, after every
-    window.  include/kvbm_kernels.h (kvbm_kernels_paged_permute_gather)."""
+    window.  `cast_scales`: one scale array for every source, as `paged_permute_heads`.  include/kvbm_kernels.h
+    (kvbm_kernels_paged_permute_gather, kvbm_kernels_paged_permute_gather_scaled)."""
     arr = (PermuteSource * max(1, len(srcs)))(*srcs)
+    if cast_scales is not None:
+        return lib().kvbm_kernels_paged_permute_gather_scaled(arr, len(srcs), C.byref(dst), dst_num_heads, num_blocks, layer_begin, layer_end,
+                                                              page_size, src_row_bytes, int(cast_mode), scales_ptr(cast_scales),
+                                                              done_flag or None, epoch, completion_flag or None, completion_value, stream)
     return lib().kvbm_kernels_paged_permute_gather(arr, len(srcs), C.byref(dst), dst_num_heads, num_blocks, layer_begin, layer_end, page_size,
                                                    src_row_bytes, int(cast_mode), done_flag or None, epoch, completion_flag or None,
                                                    completion_value, stream)

@@ -109,6 +109,8 @@ class _COptions(C.Structure):
         ("src_head_begin", C.c_size_t),
         ("dst_head_begin", C.c_size_t),
         ("head_count", C.c_size_t),
+        ("cast_scales", C.c_void_p),
+        ("num_cast_scales", C.c_size_t),
     ]
 
 
@@ -164,6 +166,9 @@ class TransferOptions:
     per_dst_done_flags: Optional[Sequence[int]] = None        # fan-out: one done-flag address per destination (0 = none)
     per_dst_layer_done_flags: Optional[Sequence[int]] = None  # fan-out: one layer-done array address per destination
     head_window: Optional[tuple] = None   # (src_head_begin, dst_head_begin, head_count): move only these heads (TP re-shard)
+    # fp8 KV-cache scales: a contiguous float32 CUDA tensor of num_layers * outer_dim entries (entry l * outer_dim + o scales the
+    # fp8 side of layer l, outer index o), applied by the cast; kept alive by this object
+    cast_scales: Optional[object] = None
 
     @staticmethod
     def from_layer_range(layer_range: Optional[range]) -> "TransferOptions":
@@ -182,7 +187,16 @@ class TransferOptions:
                          self.layer_ready_flags, self.layer_done_flags, self.epoch, self.gate_timeout_ms,
                          int(self.multicast), self.done_flag, int(bl), bids, nb, int(self.src_kv_layout),
                          int(self.dst_kv_layout), int(self.gate_mode), self._ptr_array("_pd", self.per_dst_done_flags),
-                         self._ptr_array("_pl", self.per_dst_layer_done_flags), int(sb), int(db), int(k))
+                         self._ptr_array("_pl", self.per_dst_layer_done_flags), int(sb), int(db), int(k),
+                         kernels.scales_ptr(self.cast_scales), self._num_scales())
+
+    def _num_scales(self) -> int:
+        s = self.cast_scales
+        if s is None:
+            return 0
+        if isinstance(s, int):
+            raise TypeError("TransferOptions.cast_scales takes a float32 tensor (its numel is the scale count), not an address")
+        return int(s.numel()) if hasattr(s, "numel") else int(s.size)
 
     def _ptr_array(self, keep: str, ptrs):
         if ptrs is None:

@@ -158,6 +158,14 @@ typedef struct kvbm_paged_copy_opts {
                                      (2) force either behaviour.  gate_timeout_ms applies to the spinning form only. */
   int static_schedule;            /* diagnostics: 1 = split the tiles round-robin over the rings instead of the dynamic
                                      (ticket) tile scheduler */
+  const float* cast_scales;       /* nullable; device-accessible float[num_layers * outer_dim] (the source pool's): entry
+                                     l * outer_dim + o is the dequantisation scale of the FP8 side for layer l (absolute, whatever
+                                     the layer range) and outer index o -- an engine's fp8 KV cache stores x / s and reads fp8 * s.
+                                     fp8 -> bf16 writes bf16_rne(fp32_rn(fp8 * s)) (NaN codes -> 0x7fc0); bf16 -> fp8 writes
+                                     e4m3_satfinite_rne(fp32_rn(bf16 / s)) (NaN -> 0x7f | sign), every code equal to the one IEEE
+                                     division gives for 2^-60 <= |s| <= 2^60; zero, negative, non-finite or more extreme scales give
+                                     unspecified codes.  s = 1 gives the unscaled bits.  Needs a cast_mode (cudaErrorInvalidValue with KVBM_CAST_NONE),
+                                     num_layers <= 65536 and outer_dim <= 32768; runs the general (non-FAST) rings. */
 } kvbm_paged_copy_opts;
 
 /* Gather `num_blocks` non-contiguous blocks x layers [layer_begin, layer_end) x outer from `src`,
@@ -233,6 +241,17 @@ cudaError_t kvbm_kernels_paged_permute_heads(const kvbm_permute_side* src, const
                                              uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value,
                                              cudaStream_t stream);
 
+/* kvbm_kernels_paged_permute_heads with the fp8 side's per-(layer, outer) dequantisation scales applied by the cast: cast_scales
+ * (nullable) is a device-accessible float[num_layers * outer_dim] with the meaning, the formulas and the bits of
+ * kvbm_paged_copy_opts.cast_scales.  NULL is exactly kvbm_kernels_paged_permute_heads.  Scales with KVBM_CAST_NONE are
+ * cudaErrorInvalidValue, returned before any CUDA call. */
+cudaError_t kvbm_kernels_paged_permute_heads_scaled(const kvbm_permute_side* src, const kvbm_permute_side* dst, int num_blocks,
+                                                    int layer_begin, int layer_end, uint32_t src_num_heads, uint32_t src_head_begin,
+                                                    uint32_t dst_num_heads, uint32_t dst_head_begin, uint32_t head_count,
+                                                    uint32_t page_size, uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
+                                                    uint32_t* done_flag, uint32_t epoch, uint32_t* completion_flag,
+                                                    uint32_t completion_value, cudaStream_t stream);
+
 /* One source of kvbm_kernels_paged_permute_gather: a pool side with its own head count and one head window into the
  * destination.  A pool may appear in several sources (with different windows). */
 typedef struct kvbm_permute_source {
@@ -259,6 +278,14 @@ cudaError_t kvbm_kernels_paged_permute_gather(const kvbm_permute_source* srcs, i
                                               uint32_t page_size, uint32_t src_row_bytes, int cast_mode, uint32_t* done_flag,
                                               uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value,
                                               cudaStream_t stream);
+
+/* kvbm_kernels_paged_permute_gather with scales, as kvbm_kernels_paged_permute_heads_scaled: ONE cast_scales array for every
+ * source (per-tensor scales from a checkpoint are the same on every TP rank), indexed by the absolute layer and outer index. */
+cudaError_t kvbm_kernels_paged_permute_gather_scaled(const kvbm_permute_source* srcs, int num_srcs, const kvbm_permute_side* dst,
+                                                     uint32_t dst_num_heads, int num_blocks, int layer_begin, int layer_end,
+                                                     uint32_t page_size, uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
+                                                     uint32_t* done_flag, uint32_t epoch, uint32_t* completion_flag,
+                                                     uint32_t completion_value, cudaStream_t stream);
 
 /* Host-only (no GPU): the stride table kvbm_kernels_paged_permute walks with for one side.  out[0] = 1 when offsets count
  * from the block's first byte (universal formats) or 0 when they count from the (layer, outer) region's first byte; the

@@ -127,6 +127,13 @@ typedef struct kvbm_transfer_options {
    * value.  head_count 0 = every head (no window).  The two layouts may have different num_heads; see
    * kvbm_manager_execute_transfer for the rules. */
   size_t src_head_begin, dst_head_begin, head_count;
+  /* fp8 KV-cache scales: with a cast_mode, cast_scales[l * outer_dim + o] is the dequantisation scale of the FP8 side for layer
+   * l (absolute) and outer index o, applied by every cast launch (kvbm_paged_copy_opts.cast_scales has the formulas).  NULL =
+   * unscaled.  num_cast_scales must be at least num_layers * outer_dim (KVBM_ERR_RANGE); scales without a cast_mode and a pointer
+   * the manager's device cannot read (anything but its own device memory or pinned host memory mapped into it) are KVBM_ERR.
+   * All three are rejected before any launch.  A gather applies one array to every source. */
+  const float* cast_scales;
+  size_t num_cast_scales;
 } kvbm_transfer_options;
 
 typedef struct kvbm_transfer_manager kvbm_transfer_manager;
