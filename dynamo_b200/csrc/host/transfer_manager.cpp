@@ -618,38 +618,61 @@ static int launch_cuda(kvbm_transfer_manager* m, Layout* S, Layout* const* D, in
   return KVBM_OK;
 }
 
+// One entry of a gather, as execute() resolved it: the layouts, their formats, the layer range and the direct CUDA strategy.
+struct GatherEntry {
+  Layout *S, *D;
+  int src_kv, dst_kv;
+  size_t lb, le;
+  int strategy;
+};
+
 // The layout-transforming transfer: what select_transform_kernel's result would drive if the reference ran it inside
-// execute_transfer (it rejects the pair instead, transfer/mod.rs:128-147).  One kvbm_kernels_paged_permute_heads launch, with the
-// transfer's fp8 <-> bf16 cast fused in and, when `window`, only the options' head window moved: block tables uploaded like
-// launch_cuda's, no pointer tables, completion word written by a trailing signal kernel.
-static int launch_transform(kvbm_transfer_manager* m, Layout* S, Layout* D, int src_kv, int dst_kv, const size_t* src_ids,
-                            const size_t* dst_ids, size_t n, size_t lb, size_t le, const kvbm_transfer_options& o, bool window,
-                            cudaStream_t stream, Slot** slot_out, uint64_t* seq_out)
+// execute_transfer (it rejects the pair instead, transfer/mod.rs:128-147).  One permuting launch moves every head window w[j]
+// from source w[j].src_rank (resolved as e[j]) into e[0].D over e[0]'s layer range, with the transfer's fp8 <-> bf16 cast fused
+// in: kvbm_kernels_paged_permute_heads for one window (any head count), kvbm_kernels_paged_permute_gather for several.  Block
+// tables are uploaded like launch_cuda's, source s at s * n and the destination's at num_srcs * n, no pointer tables; the
+// completion word is written by a trailing signal kernel.
+static int launch_permute(kvbm_transfer_manager* m, const GatherEntry* e, const kvbm_head_window* w, size_t nw, size_t num_srcs,
+                          const size_t* const* src_ids, const size_t* dst_ids, size_t n, const kvbm_transfer_options& o,
+                          cudaStream_t stream, uint64_t* seq_out)
 {
   Slot* sl;
   uint64_t seq;
-  int rc = acquire_slot(m, 2 * n, 4, &sl, &seq);
+  int rc = acquire_slot(m, (num_srcs + 1) * n, 4, &sl, &seq);
   if (rc) return rc;
-  for (size_t i = 0; i < n; ++i) {
-    sl->pinned_ids[i] = static_cast<int32_t>(src_ids[i]);
-    sl->pinned_ids[n + i] = static_cast<int32_t>(dst_ids[i]);
+  for (size_t s = 0; s < num_srcs; ++s)
+    if (src_ids[s])
+      for (size_t i = 0; i < n; ++i) sl->pinned_ids[s * n + i] = static_cast<int32_t>(src_ids[s][i]);
+  for (size_t i = 0; i < n; ++i) sl->pinned_ids[num_srcs * n + i] = static_cast<int32_t>(dst_ids[i]);
+  CU(cudaMemcpyAsync(sl->dev_ids, sl->pinned_ids, (num_srcs + 1) * n * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
+  m->h2d_bytes += (num_srcs + 1) * n * sizeof(int32_t);
+  const Layout *S0 = e[0].S, *D = e[0].D;
+  kvbm_permute_side pd{descriptor(*D), sl->dev_ids + num_srcs * n, e[0].dst_kv};
+  kvbm_permute_source ks[KVBM_GATHER_MAX_SOURCES] = {};
+  size_t heads = 0;
+  for (size_t j = 0; j < nw; ++j) {
+    ks[j] = kvbm_permute_source{{descriptor(*e[j].S), sl->dev_ids + w[j].src_rank * n, e[j].src_kv}, static_cast<uint32_t>(e[j].S->cfg.num_heads),
+                                static_cast<uint32_t>(w[j].src_head_begin), static_cast<uint32_t>(w[j].dst_head_begin),
+                                static_cast<uint32_t>(w[j].head_count)};
+    heads += w[j].head_count;
   }
-  CU(cudaMemcpyAsync(sl->dev_ids, sl->pinned_ids, 2 * n * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
-  m->h2d_bytes += 2 * n * sizeof(int32_t);
-  kvbm_permute_side ps{descriptor(*S), sl->dev_ids, src_kv}, pd{descriptor(*D), sl->dev_ids + n, dst_kv};
-  const size_t snh = S->cfg.num_heads, dnh = D->cfg.num_heads;
-  const size_t sb = window ? o.src_head_begin : 0, db = window ? o.dst_head_begin : 0, k = window ? o.head_count : snh;
-  const size_t row = S->cfg.inner_dim / snh * S->cfg.dtype_width_bytes;
-  cudaError_t e = kvbm_kernels_paged_permute_heads_scaled(&ps, &pd, static_cast<int>(n), static_cast<int>(lb), static_cast<int>(le),
-                                                          static_cast<uint32_t>(snh), static_cast<uint32_t>(sb), static_cast<uint32_t>(dnh),
-                                                          static_cast<uint32_t>(db), static_cast<uint32_t>(k),
-                                                          static_cast<uint32_t>(S->cfg.page_size), static_cast<uint32_t>(row), o.cast_mode,
-                                                          o.cast_scales, o.done_flag, o.epoch, sl->host_flag, static_cast<uint32_t>(seq), stream);
-  if (e != cudaSuccess) return fail_cuda(e, "kvbm_kernels_paged_permute_heads_scaled");
+  const uint32_t dnh = static_cast<uint32_t>(D->cfg.num_heads), page = static_cast<uint32_t>(S0->cfg.page_size);
+  const uint32_t row = static_cast<uint32_t>(S0->cfg.inner_dim / S0->cfg.num_heads * S0->cfg.dtype_width_bytes);
+  const int nb = static_cast<int>(n), lb = static_cast<int>(e[0].lb), le = static_cast<int>(e[0].le);
+  if (nw == 1) {
+    const kvbm_permute_source& k = ks[0];
+    cudaError_t ce = kvbm_kernels_paged_permute_heads_scaled(&k.side, &pd, nb, lb, le, k.num_heads, k.src_head_begin, dnh, k.dst_head_begin,
+                                                             k.head_count, page, row, o.cast_mode, o.cast_scales, o.done_flag, o.epoch,
+                                                             sl->host_flag, static_cast<uint32_t>(seq), stream);
+    if (ce != cudaSuccess) return fail_cuda(ce, "kvbm_kernels_paged_permute_heads_scaled");
+  } else {
+    cudaError_t ce = kvbm_kernels_paged_permute_gather_scaled(ks, static_cast<int>(nw), &pd, dnh, nb, lb, le, page, row, o.cast_mode,
+                                                              o.cast_scales, o.done_flag, o.epoch, sl->host_flag, static_cast<uint32_t>(seq), stream);
+    if (ce != cudaSuccess) return fail_cuda(ce, "kvbm_kernels_paged_permute_gather_scaled");
+  }
   CU(cudaEventRecord(sl->ev, stream));
   sl->in_flight = true;
-  m->bytes_moved += n * (le - lb) * S->cfg.outer_dim * (D->region / dnh * k);
-  *slot_out = sl;
+  m->bytes_moved += n * (e[0].le - e[0].lb) * S0->cfg.outer_dim * (D->region / D->cfg.num_heads * heads);
   *seq_out = seq;
   return KVBM_OK;
 }
@@ -671,6 +694,13 @@ static int check_cast_scales(kvbm_transfer_manager* m, const float* p)
 
 static bool cuda_strategy(int s) { return s == KVBM_STRATEGY_CUDA_ASYNC_H2D || s == KVBM_STRATEGY_CUDA_ASYNC_D2H || s == KVBM_STRATEGY_CUDA_ASYNC_D2D; }
 
+// The stream of a CUDA strategy: the caller's, or round-robin from the pool (cuda.rs:82-90: D2H pool for D2H, H2D pool otherwise).
+static cudaStream_t pick_stream(kvbm_transfer_manager* m, int strategy, const kvbm_transfer_options& o)
+{
+  if (o.use_caller_stream) return o.cuda_stream;
+  return strategy == KVBM_STRATEGY_CUDA_ASYNC_D2H ? m->d2h[m->rr_d2h++ % kStreams] : m->h2d[m->rr_h2d++ % kStreams];
+}
+
 // execute_two_hop_transfer (executor/mod.rs:477-571) with handle_buffered_transfer's two bounce groups (:357-416): the
 // bounce blocks are split in two halves; chunk i goes src -> half (i & 1) -> dst.  The reference runs two tokio tasks
 // that each await their hops; here both hops are stream work ordered by events, so chunk i+1's first hop overlaps chunk
@@ -679,8 +709,7 @@ static int execute_two_hop(kvbm_transfer_manager* m, Layout* S, Layout* D, Layou
                            size_t n, const size_t* bounce_ids, size_t nb, size_t lb, size_t le, const kvbm_transfer_plan& plan,
                            const kvbm_transfer_options& o, kvbm_notification* out)
 {
-  auto pick = [&](int strategy) { return strategy == KVBM_STRATEGY_CUDA_ASYNC_D2H ? m->d2h[m->rr_d2h++ % kStreams] : m->h2d[m->rr_h2d++ % kStreams]; };
-  cudaStream_t s1 = pick(plan.first), s2 = pick(plan.second);
+  cudaStream_t s1 = pick_stream(m, plan.first, o), s2 = pick_stream(m, plan.second, o);  // never the caller's: execute() rejects it
   nb = std::min(nb, n);
   const size_t half = nb >= 2 ? nb / 2 : nb;
   const size_t group_begin[2] = {0, half};
@@ -718,14 +747,6 @@ static int execute_two_hop(kvbm_transfer_manager* m, Layout* S, Layout* D, Layou
   if (out) *out = last;
   return KVBM_OK;
 }
-
-// One entry of a gather, as execute() resolved it: the layouts, their formats, the layer range and the direct CUDA strategy.
-struct GatherEntry {
-  Layout *S, *D;
-  int src_kv, dst_kv;
-  size_t lb, le;
-  int strategy;
-};
 
 // `gather`: validate one windowed entry of a gather and fill *gather instead of running it.  The caller holds the manager
 // mutex; the entry always takes the permuting path (also for a window over every head of both sides) and every check and
@@ -906,18 +927,18 @@ static int execute(kvbm_transfer_manager* m, kvbm_layout_handle src_h, int nd, c
   }
 
   DeviceGuard g(m->device);
-  // stream: caller's, or round-robin from the pool (cuda.rs:82-90: D2H pool for D2H, H2D pool otherwise)
-  cudaStream_t stream;
-  if (o.use_caller_stream)
-    stream = o.cuda_stream;
-  else if (plan.first == KVBM_STRATEGY_CUDA_ASYNC_D2H)
-    stream = m->d2h[m->rr_d2h++ % kStreams];
-  else
-    stream = m->h2d[m->rr_h2d++ % kStreams];
-  Slot* sl;
+  const cudaStream_t stream = pick_stream(m, plan.first, o);
   uint64_t seq;
-  int rc = permute ? launch_transform(m, S, D[0], src_kv, dst_kv0, src_ids[0], dst_ids[0], n, lb, le, o, window, stream, &sl, &seq)
-                   : launch_cuda(m, S, D.data(), nd, src_ids, dst_ids, n, replicate, lb, le, o, stream, nullptr, &sl, &seq);
+  int rc;
+  if (permute) {  // a plain transform is the window over every head
+    const GatherEntry e{S, D[0], src_kv, dst_kv0, lb, le, plan.first};
+    const kvbm_head_window w = window ? kvbm_head_window{0, o.src_head_begin, o.dst_head_begin, o.head_count}
+                                      : kvbm_head_window{0, 0, 0, S->cfg.num_heads};
+    rc = launch_permute(m, &e, &w, 1, 1, src_ids, dst_ids[0], n, o, stream, &seq);
+  } else {
+    Slot* sl;
+    rc = launch_cuda(m, S, D.data(), nd, src_ids, dst_ids, n, replicate, lb, le, o, stream, nullptr, &sl, &seq);
+  }
   if (rc) return rc;
   // caller-provided stream: caller manages sync, completed() is returned (cuda.rs:139-141)
   if (out) *out = o.use_caller_stream ? 0 : seq;
@@ -964,45 +985,9 @@ static int execute_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_
   if (e[0].strategy < 0) return KVBM_OK;  // nothing to move (no blocks or an empty layer range), as execute()
 
   DeviceGuard g(m->device);
-  cudaStream_t stream;
-  if (o.use_caller_stream)
-    stream = o.cuda_stream;
-  else if (e[0].strategy == KVBM_STRATEGY_CUDA_ASYNC_D2H)
-    stream = m->d2h[m->rr_d2h++ % kStreams];
-  else
-    stream = m->h2d[m->rr_h2d++ % kStreams];
-  // one upload of every source's table and the destination's: source s at s * n, the destination at num_srcs * n
-  Slot* sl;
   uint64_t seq;
-  int rc = acquire_slot(m, (num_srcs + 1) * n, 4, &sl, &seq);
+  int rc = launch_permute(m, e.data(), windows, nw, num_srcs, src_ids, dst_ids, n, o, pick_stream(m, e[0].strategy, o), &seq);
   if (rc) return rc;
-  for (size_t s = 0; s < num_srcs; ++s)
-    if (src_ids[s])
-      for (size_t i = 0; i < n; ++i) sl->pinned_ids[s * n + i] = static_cast<int32_t>(src_ids[s][i]);
-  for (size_t i = 0; i < n; ++i) sl->pinned_ids[num_srcs * n + i] = static_cast<int32_t>(dst_ids[i]);
-  CU(cudaMemcpyAsync(sl->dev_ids, sl->pinned_ids, (num_srcs + 1) * n * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
-  m->h2d_bytes += (num_srcs + 1) * n * sizeof(int32_t);
-  Layout* D = e[0].D;
-  kvbm_permute_side pd{descriptor(*D), sl->dev_ids + num_srcs * n, e[0].dst_kv};
-  kvbm_permute_source ks[KVBM_GATHER_MAX_SOURCES] = {};
-  size_t bytes = 0;
-  for (size_t j = 0; j < nw; ++j) {
-    const size_t r = windows[j].src_rank;
-    ks[j] = kvbm_permute_source{{descriptor(*e[j].S), sl->dev_ids + r * n, e[j].src_kv}, static_cast<uint32_t>(e[j].S->cfg.num_heads),
-                                static_cast<uint32_t>(windows[j].src_head_begin), static_cast<uint32_t>(windows[j].dst_head_begin),
-                                static_cast<uint32_t>(windows[j].head_count)};
-    bytes += D->region / D->cfg.num_heads * windows[j].head_count;
-  }
-  const Layout* S0 = e[0].S;
-  const size_t row = S0->cfg.inner_dim / S0->cfg.num_heads * S0->cfg.dtype_width_bytes;
-  cudaError_t ce = kvbm_kernels_paged_permute_gather_scaled(ks, static_cast<int>(nw), &pd, static_cast<uint32_t>(D->cfg.num_heads),
-                                                            static_cast<int>(n), static_cast<int>(e[0].lb), static_cast<int>(e[0].le),
-                                                            static_cast<uint32_t>(S0->cfg.page_size), static_cast<uint32_t>(row), o.cast_mode,
-                                                            o.cast_scales, o.done_flag, o.epoch, sl->host_flag, static_cast<uint32_t>(seq), stream);
-  if (ce != cudaSuccess) return fail_cuda(ce, "kvbm_kernels_paged_permute_gather_scaled");
-  CU(cudaEventRecord(sl->ev, stream));
-  sl->in_flight = true;
-  m->bytes_moved += n * (e[0].le - e[0].lb) * S0->cfg.outer_dim * bytes;
   // caller-provided stream: caller manages sync, completed() is returned, as execute()
   if (out) *out = o.use_caller_stream ? 0 : seq;
   return KVBM_OK;

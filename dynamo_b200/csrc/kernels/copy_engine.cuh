@@ -225,11 +225,7 @@ __device__ __forceinline__ void warp_store_from_smem(uint8_t* dst, uint32_t src_
 {
   uint4* d = reinterpret_cast<uint4*>(dst);
   const uint32_t n = bytes >> 4;
-  for (uint32_t i = lane; i < n; i += 32) {
-    uint4 v;
-    asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(src_smem + i * 16));
-    ptx::st_stream_v4(d + i, v);
-  }
+  for (uint32_t i = lane; i < n; i += 32) ptx::st_stream_v4(d + i, ptx::ld_shared_v4(src_smem + i * 16));
 }
 
 // smem -> NVLink multicast address (variant 4): one store, the switch delivers it to every bound device
@@ -237,11 +233,7 @@ __device__ __forceinline__ void warp_store_from_smem_mc(uint8_t* dst, uint32_t s
 {
   uint4* d = reinterpret_cast<uint4*>(dst);
   const uint32_t n = bytes >> 4;
-  for (uint32_t i = lane; i < n; i += 32) {
-    uint4 v;
-    asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(src_smem + i * 16));
-    ptx::multimem_st_v4(d + i, v);
-  }
+  for (uint32_t i = lane; i < n; i += 32) ptx::multimem_st_v4(d + i, ptx::ld_shared_v4(src_smem + i * 16));
 }
 // global -> multicast for pieces the TMA load cannot take (the launcher guarantees 4-byte granularity)
 __device__ __forceinline__ void warp_copy_simt_mc(uint8_t* dst, const uint8_t* src, uint32_t bytes, int lane)
@@ -258,10 +250,76 @@ __device__ __forceinline__ void warp_copy_simt_mc(uint8_t* dst, const uint8_t* s
   }
 }
 
+// ------------------------------------------------------------------------------------------
+// The fp8 <-> bf16 conversion of the cast rings and of the head-row walk (kvbm_kernels.cu).
+// ------------------------------------------------------------------------------------------
+// One vector: 16 e4m3 codes <-> 16 bf16 (SCALED: with the fp8 side's `scale`).  in[] are the 16 B words of the source side,
+// out[] those of the destination side: one in and two out for fp8 -> bf16, two in and one out for bf16 -> fp8.
+template <bool SCALED>
+__device__ __forceinline__ void cast_vector(const uint4 (&in)[1], uint4 (&out)[2], const ptx::Scale& scale)
+{
+  const uint32_t w[4] = {in[0].x, in[0].y, in[0].z, in[0].w};
+  uint32_t o[8];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    o[2 * k] = ptx::cvt_up2<SCALED>(static_cast<uint16_t>(w[k] & 0xffff), scale);
+    o[2 * k + 1] = ptx::cvt_up2<SCALED>(static_cast<uint16_t>(w[k] >> 16), scale);
+  }
+  out[0] = make_uint4(o[0], o[1], o[2], o[3]);
+  out[1] = make_uint4(o[4], o[5], o[6], o[7]);
+}
+template <bool SCALED>
+__device__ __forceinline__ void cast_vector(const uint4 (&in)[2], uint4 (&out)[1], const ptx::Scale& scale)
+{
+  const uint32_t w[8] = {in[0].x, in[0].y, in[0].z, in[0].w, in[1].x, in[1].y, in[1].z, in[1].w};
+  uint32_t o[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+    o[k] = static_cast<uint32_t>(ptx::cvt_down2<SCALED>(w[2 * k], scale)) | (static_cast<uint32_t>(ptx::cvt_down2<SCALED>(w[2 * k + 1], scale)) << 16);
+  out[0] = make_uint4(o[0], o[1], o[2], o[3]);
+}
+
+// A cast ring's slot: the vectors of src_bytes in shared memory at in_smem, converted to out_smem.
 template <bool UP, bool SCALED>
-__device__ __forceinline__ void convert_smem(uint32_t in_smem, uint32_t out_smem, uint32_t src_bytes, int lane, const ptx::Scale& scale);
+__device__ __forceinline__ void convert_smem(uint32_t in_smem, uint32_t out_smem, uint32_t src_bytes, int lane, const ptx::Scale& scale)
+{
+  constexpr int IN = UP ? 1 : 2, OUT = UP ? 2 : 1;  // 16 B words per vector on either side
+  for (uint32_t off = lane * 16 * IN; off < src_bytes; off += 32 * 16 * IN) {
+    uint4 x[IN], y[OUT];
+    x[0] = ptx::ld_shared_v4(in_smem + off);
+    if constexpr (!UP) x[1] = ptx::ld_shared_v4(in_smem + off + 16);
+    cast_vector<SCALED>(x, y, scale);
+    if constexpr (UP) {
+      ptx::st_shared_v4(out_smem + 2 * off, y[0]);
+      ptx::st_shared_v4(out_smem + 2 * off + 16, y[1]);
+    } else {
+      ptx::st_shared_v4(out_smem + off / 2, y[0]);
+    }
+  }
+}
+
+// SIMT conversion straight from global to global for pieces TMA cannot take (any alignment).
 template <bool UP, bool SCALED>
-__device__ __forceinline__ void warp_cast_simt(uint8_t* dst, const uint8_t* src, uint32_t src_bytes, int lane, const ptx::Scale& scale);
+__device__ __forceinline__ void warp_cast_simt(uint8_t* dst, const uint8_t* src, uint32_t src_bytes, int lane, const ptx::Scale& scale)
+{
+  if (UP) {
+    uint16_t* d = reinterpret_cast<uint16_t*>(dst);
+    const uint32_t pairs = src_bytes >> 1;
+    for (uint32_t i = lane; i < pairs; i += 32) {
+      uint16_t two = static_cast<uint16_t>(src[2 * i]) | (static_cast<uint16_t>(src[2 * i + 1]) << 8);
+      uint32_t r = ptx::cvt_up2<SCALED>(two, scale);
+      d[2 * i] = static_cast<uint16_t>(r & 0xffff);
+      d[2 * i + 1] = static_cast<uint16_t>(r >> 16);
+    }
+    if ((src_bytes & 1) && lane == 0)
+      d[src_bytes - 1] = static_cast<uint16_t>(ptx::cvt_up2<SCALED>(src[src_bytes - 1], scale) & 0xffff);
+  } else {
+    const uint16_t* s = reinterpret_cast<const uint16_t*>(src);
+    const uint32_t elems = src_bytes >> 1;
+    for (uint32_t i = lane; i < elems; i += 32)
+      dst[i] = static_cast<uint8_t>(ptx::cvt_down2<SCALED>(s[i], scale) & 0xff);
+  }
+}
 
 // ------------------------------------------------------------------------------------------
 // Producer warp.  Gen::get(item, Piece&) is called by up to `batch` lanes at once (one item each).
@@ -560,81 +618,6 @@ __device__ __forceinline__ void ring_consumer(const RingSmem& sm, int ndst_rt, c
   if (lane == 0) {
     if (want_layers && unpublished != 0) arrive_layer(ss, cur_layer, unpublished);
     arrive_transfer(ss);
-  }
-}
-
-// ------------------------------------------------------------------------------------------
-// Conversion helpers of the cast rings.
-// ------------------------------------------------------------------------------------------
-template <bool UP, bool SCALED>
-__device__ __forceinline__ void convert_smem(uint32_t in_smem, uint32_t out_smem, uint32_t src_bytes,
-                                             int lane, const ptx::Scale& scale)
-{
-  if (UP) {
-    // 16 fp8 in (16 B) -> 16 bf16 out (32 B) per lane-iteration
-    for (uint32_t off = lane * 16; off < src_bytes; off += 32 * 16) {
-      uint4 v;
-      asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(in_smem + off));
-      uint32_t w[4] = {v.x, v.y, v.z, v.w};
-      uint32_t o[8];
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        if constexpr (SCALED) {
-          o[2 * k] = ptx::e4m3x2_to_bf16x2_scaled(static_cast<uint16_t>(w[k] & 0xffff), scale);
-          o[2 * k + 1] = ptx::e4m3x2_to_bf16x2_scaled(static_cast<uint16_t>(w[k] >> 16), scale);
-        } else {
-          o[2 * k] = ptx::e4m3x2_to_bf16x2(static_cast<uint16_t>(w[k] & 0xffff));
-          o[2 * k + 1] = ptx::e4m3x2_to_bf16x2(static_cast<uint16_t>(w[k] >> 16));
-        }
-      }
-      asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(out_smem + 2 * off), "r"(o[0]), "r"(o[1]), "r"(o[2]), "r"(o[3]) : "memory");
-      asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(out_smem + 2 * off + 16), "r"(o[4]), "r"(o[5]), "r"(o[6]), "r"(o[7]) : "memory");
-    }
-  } else {
-    // 16 bf16 in (32 B) -> 16 fp8 out (16 B)
-    for (uint32_t off = lane * 32; off < src_bytes; off += 32 * 32) {
-      uint4 a, b;
-      asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w) : "r"(in_smem + off));
-      asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w) : "r"(in_smem + off + 16));
-      uint32_t w[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-      uint32_t o[4];
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        if constexpr (SCALED)
-          o[k] = static_cast<uint32_t>(ptx::bf16x2_to_e4m3x2_scaled(w[2 * k], scale)) |
-                 (static_cast<uint32_t>(ptx::bf16x2_to_e4m3x2_scaled(w[2 * k + 1], scale)) << 16);
-        else
-          o[k] = static_cast<uint32_t>(ptx::bf16x2_to_e4m3x2(w[2 * k])) |
-                 (static_cast<uint32_t>(ptx::bf16x2_to_e4m3x2(w[2 * k + 1])) << 16);
-      }
-      asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(out_smem + off / 2), "r"(o[0]), "r"(o[1]), "r"(o[2]), "r"(o[3]) : "memory");
-    }
-  }
-}
-
-// SIMT conversion straight from global to global for pieces TMA cannot take (any alignment).
-template <bool UP, bool SCALED>
-__device__ __forceinline__ void warp_cast_simt(uint8_t* dst, const uint8_t* src, uint32_t src_bytes,
-                                               int lane, const ptx::Scale& scale)
-{
-  auto up = [&](uint16_t two) { return SCALED ? ptx::e4m3x2_to_bf16x2_scaled(two, scale) : ptx::e4m3x2_to_bf16x2(two); };
-  auto down = [&](uint32_t two) { return SCALED ? ptx::bf16x2_to_e4m3x2_scaled(two, scale) : ptx::bf16x2_to_e4m3x2(two); };
-  if (UP) {
-    uint16_t* d = reinterpret_cast<uint16_t*>(dst);
-    const uint32_t pairs = src_bytes >> 1;
-    for (uint32_t i = lane; i < pairs; i += 32) {
-      uint16_t two = static_cast<uint16_t>(src[2 * i]) | (static_cast<uint16_t>(src[2 * i + 1]) << 8);
-      uint32_t r = up(two);
-      d[2 * i] = static_cast<uint16_t>(r & 0xffff);
-      d[2 * i + 1] = static_cast<uint16_t>(r >> 16);
-    }
-    if ((src_bytes & 1) && lane == 0)
-      d[src_bytes - 1] = static_cast<uint16_t>(up(src[src_bytes - 1]) & 0xffff);
-  } else {
-    const uint16_t* s = reinterpret_cast<const uint16_t*>(src);
-    const uint32_t elems = src_bytes >> 1;
-    for (uint32_t i = lane; i < elems; i += 32)
-      dst[i] = static_cast<uint8_t>(down(s[i]) & 0xff);
   }
 }
 

@@ -8,6 +8,7 @@
 #include <algorithm>
 #include <atomic>
 #include <mutex>
+#include <type_traits>
 #include <cstdio>
 #include <vector>
 
@@ -512,43 +513,6 @@ __device__ __forceinline__ uint32_t row_offset(const RowSplit& r, uint32_t v, ui
   return t * tok_stride + (c << SHIFT);
 }
 
-// One vector of a cast walk: 16 e4m3 codes <-> 16 bf16, bit for bit the conversions of the paged copy's cast rings (SCALED:
-// its scaled conversions with the unit's scale).  in[0 .. IN) are the 16 B loads of the source side, out[0 .. OUT) the 16 B
-// stores of the destination side.
-template <bool SCALED>
-__device__ __forceinline__ void cast_vector_up(const uint4 (&in)[1], uint4 (&out)[2], const ptx::Scale& scale)
-{
-  const uint32_t w[4] = {in[0].x, in[0].y, in[0].z, in[0].w};
-  uint32_t o[8];
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    if constexpr (SCALED) {
-      o[2 * k] = ptx::e4m3x2_to_bf16x2_scaled(static_cast<uint16_t>(w[k] & 0xffff), scale);
-      o[2 * k + 1] = ptx::e4m3x2_to_bf16x2_scaled(static_cast<uint16_t>(w[k] >> 16), scale);
-    } else {
-      o[2 * k] = ptx::e4m3x2_to_bf16x2(static_cast<uint16_t>(w[k] & 0xffff));
-      o[2 * k + 1] = ptx::e4m3x2_to_bf16x2(static_cast<uint16_t>(w[k] >> 16));
-    }
-  }
-  out[0] = make_uint4(o[0], o[1], o[2], o[3]);
-  out[1] = make_uint4(o[4], o[5], o[6], o[7]);
-}
-template <bool SCALED>
-__device__ __forceinline__ void cast_vector_down(const uint4 (&in)[2], uint4 (&out)[1], const ptx::Scale& scale)
-{
-  const uint32_t w[8] = {in[0].x, in[0].y, in[0].z, in[0].w, in[1].x, in[1].y, in[1].z, in[1].w};
-  uint32_t o[4];
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    if constexpr (SCALED)
-      o[k] = static_cast<uint32_t>(ptx::bf16x2_to_e4m3x2_scaled(w[2 * k], scale)) |
-             (static_cast<uint32_t>(ptx::bf16x2_to_e4m3x2_scaled(w[2 * k + 1], scale)) << 16);
-    else
-      o[k] = static_cast<uint32_t>(ptx::bf16x2_to_e4m3x2(w[2 * k])) | (static_cast<uint32_t>(ptx::bf16x2_to_e4m3x2(w[2 * k + 1])) << 16);
-  }
-  out[0] = make_uint4(o[0], o[1], o[2], o[3]);
-}
-
 // One unit: heads h0, h0 + hstep, ... < nh of it, one warp per head (h0 = the warp, hstep = the CTA's warps when a CTA
 // walks one unit).  sb / db: the unit's bases; both must be 16 B aligned.  The last batch of
 // a head is predicated rather than a serial tail: for head_dim 64 ... 96 in bf16 it is the whole head, and its loads stay
@@ -586,10 +550,7 @@ __device__ __forceinline__ void walk_head_rows(const uint8_t* sb, uint64_t s_hea
             ptx::st_stream_v4(d, x[k][0]);
           } else {
             uint4 y[OUT];
-            if constexpr (CAST == KVBM_CAST_FP8E4M3_TO_BF16)
-              cast_vector_up<SCALED>(x[k], y, scale);
-            else
-              cast_vector_down<SCALED>(x[k], y, scale);
+            cast_vector<SCALED>(x[k], y, scale);  // bit for bit the paged copy's cast rings (copy_engine.cuh)
 #pragma unroll
             for (int i = 0; i < OUT; ++i) ptx::st_stream_v4(d + 16 * i, y[i]);
           }
@@ -698,6 +659,23 @@ kvbm_paged_gather_kernel(const __grid_constant__ GatherParams P, uint32_t layer_
     const uint32_t h = j - G.first;  // head h of the window: walk heads h .. h of the window's bases
     walk_head_rows<CAST, POW2, SCALED>(base_of(G.S) + G.s_win, G.S.head_stride, G.S.tok_stride, db + G.d_win, P.D.head_stride,
                                        P.D.tok_stride, h, 1, h + 1, nt, r, scale);
+  }
+}
+
+// The instantiation of the permuting kernels a launch takes for its cast mode, row split and scales: calls
+// f(integral_constant<int, CAST>, bool_constant<POW2>, bool_constant<SCALED>).  Scales without a cast take the unscaled
+// instantiation (the launch rejects them first), so no scaled kernel exists without a cast.  preload_kernels() passes every
+// run-time combination through here, so whatever a launch can pick is loaded up front.
+template <class F>
+static void with_walk_kernel(int cast_mode, bool pow2, bool scaled, F&& f)
+{
+  auto go = [&](auto cast, auto sc) { pow2 ? f(cast, std::true_type{}, sc) : f(cast, std::false_type{}, sc); };
+  using Up = std::integral_constant<int, KVBM_CAST_FP8E4M3_TO_BF16>;
+  using Down = std::integral_constant<int, KVBM_CAST_BF16_TO_FP8E4M3>;
+  switch (cast_mode) {
+    case KVBM_CAST_NONE: return go(std::integral_constant<int, KVBM_CAST_NONE>{}, std::false_type{});
+    case KVBM_CAST_FP8E4M3_TO_BF16: return scaled ? go(Up{}, std::true_type{}) : go(Up{}, std::false_type{});
+    default: return scaled ? go(Down{}, std::true_type{}) : go(Down{}, std::false_type{});
   }
 }
 
@@ -812,7 +790,7 @@ __global__ void kvbm_wait_flag_kernel(const uint32_t* flag, uint32_t value)
 static cudaError_t preload_kernels()
 {
   cudaFuncAttributes attr;
-  cudaError_t e;
+  cudaError_t e = cudaSuccess;
 #define KVBM_PRELOAD(k) \
   if ((e = cudaFuncGetAttributes(&attr, k)) != cudaSuccess) return e;
   KVBM_PRELOAD(kvbm_pair_copy_kernel)
@@ -826,26 +804,6 @@ static cudaError_t preload_kernels()
   KVBM_PRELOAD((kvbm_paged_copy_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false, true>))
   KVBM_PRELOAD(kvbm_set_flags_kernel)
   KVBM_PRELOAD(kvbm_wait_flag_kernel)
-  KVBM_PRELOAD((kvbm_paged_permute_kernel<KVBM_CAST_NONE, true>))
-  KVBM_PRELOAD((kvbm_paged_permute_kernel<KVBM_CAST_NONE, false>))
-  KVBM_PRELOAD((kvbm_paged_permute_kernel<KVBM_CAST_FP8E4M3_TO_BF16, true>))
-  KVBM_PRELOAD((kvbm_paged_permute_kernel<KVBM_CAST_FP8E4M3_TO_BF16, false>))
-  KVBM_PRELOAD((kvbm_paged_permute_kernel<KVBM_CAST_BF16_TO_FP8E4M3, true>))
-  KVBM_PRELOAD((kvbm_paged_permute_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false>))
-  KVBM_PRELOAD((kvbm_paged_permute_kernel<KVBM_CAST_FP8E4M3_TO_BF16, true, true>))
-  KVBM_PRELOAD((kvbm_paged_permute_kernel<KVBM_CAST_FP8E4M3_TO_BF16, false, true>))
-  KVBM_PRELOAD((kvbm_paged_permute_kernel<KVBM_CAST_BF16_TO_FP8E4M3, true, true>))
-  KVBM_PRELOAD((kvbm_paged_permute_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false, true>))
-  KVBM_PRELOAD((kvbm_paged_gather_kernel<KVBM_CAST_NONE, true>))
-  KVBM_PRELOAD((kvbm_paged_gather_kernel<KVBM_CAST_NONE, false>))
-  KVBM_PRELOAD((kvbm_paged_gather_kernel<KVBM_CAST_FP8E4M3_TO_BF16, true>))
-  KVBM_PRELOAD((kvbm_paged_gather_kernel<KVBM_CAST_FP8E4M3_TO_BF16, false>))
-  KVBM_PRELOAD((kvbm_paged_gather_kernel<KVBM_CAST_BF16_TO_FP8E4M3, true>))
-  KVBM_PRELOAD((kvbm_paged_gather_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false>))
-  KVBM_PRELOAD((kvbm_paged_gather_kernel<KVBM_CAST_FP8E4M3_TO_BF16, true, true>))
-  KVBM_PRELOAD((kvbm_paged_gather_kernel<KVBM_CAST_FP8E4M3_TO_BF16, false, true>))
-  KVBM_PRELOAD((kvbm_paged_gather_kernel<KVBM_CAST_BF16_TO_FP8E4M3, true, true>))
-  KVBM_PRELOAD((kvbm_paged_gather_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false, true>))
   KVBM_PRELOAD(kvbm_signal_kernel)
   KVBM_PRELOAD(kvbm_permute_table_kernel<true>)
   KVBM_PRELOAD(kvbm_permute_table_kernel<false>)
@@ -858,7 +816,15 @@ static cudaError_t preload_kernels()
   KVBM_PRELOAD((kvbm_permute_kernel<4, false>))
   KVBM_PRELOAD((kvbm_permute_kernel<2, false>))
 #undef KVBM_PRELOAD
-  return cudaSuccess;
+  // the paged permute and gather: every instantiation launch_paged_permute can select, through its own selection helper
+  for (int cast = KVBM_CAST_NONE; cast <= KVBM_CAST_BF16_TO_FP8E4M3; ++cast)
+    for (int pow2 = 0; pow2 < 2; ++pow2)
+      for (int scaled = 0; scaled < 2; ++scaled)
+        with_walk_kernel(cast, pow2, scaled, [&](auto c, auto p, auto sc) {
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_permute_kernel<c, p, sc>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_gather_kernel<c, p, sc>);
+        });
+  return e;
 }
 
 // Stream memory operations (cuStreamWriteValue32 / cuStreamWaitValue32) through the driver entry point:
@@ -888,6 +854,81 @@ template <class K>
 static cudaError_t set_smem(K kernel, uint32_t bytes)
 {
   return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
+}
+
+// Every permuting launch: a head transform is one source, a gather several.  Runs the checks of both entries once, signals
+// when there is nothing to move, and launches kvbm_paged_permute_kernel for one source (the faster of the two, DESIGN §4.2b) or
+// kvbm_paged_gather_kernel for several.  max_covered: how many destination heads the sources may cover together; at most
+// KVBM_GATHER_MAX_HEADS (the gather's head map) whenever num_srcs > 1.
+static cudaError_t launch_paged_permute(const kvbm_permute_source* srcs, int num_srcs, const kvbm_permute_side* dst, uint32_t dst_num_heads,
+                                        int num_blocks, int layer_begin, int layer_end, uint32_t page_size, uint32_t src_row_bytes,
+                                        int cast_mode, const float* cast_scales, uint32_t* done_flag, uint32_t epoch,
+                                        uint32_t* completion_flag, uint32_t completion_value, uint32_t max_covered, cudaStream_t stream)
+{
+  if (num_blocks < 0 || layer_begin < 0 || layer_end < layer_begin) return cudaErrorInvalidValue;
+  if (cast_mode < KVBM_CAST_NONE || cast_mode > KVBM_CAST_BF16_TO_FP8E4M3) return cudaErrorInvalidValue;
+  if (cast_scales && cast_mode == KVBM_CAST_NONE) return cudaErrorInvalidValue;  // scales belong to the fp8 side of a cast
+  if (!srcs || num_srcs < 1 || num_srcs > KVBM_GATHER_MAX_SOURCES) return cudaErrorInvalidValue;
+  auto finish = [&]() -> cudaError_t {
+    if (!done_flag && !completion_flag) return cudaSuccess;
+    kvbm_signal_kernel<<<1, 1, 0, stream>>>(done_flag, epoch, completion_flag, completion_value);
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    return cudaGetLastError();
+  };
+  if (num_blocks == 0 || layer_end == layer_begin) return finish();
+  if (!dst || !dst->block_ids || !dst->layout.layer_base) return cudaErrorInvalidValue;
+  const uint32_t nl = dst->layout.num_layers, no = dst->layout.outer_dim;
+  if (nl == 0 || no == 0 || static_cast<uint32_t>(layer_end) > nl) return cudaErrorInvalidValue;
+  // The walk splits the fp8 side's row into 16 B vectors when casting (the bf16 side's vectors are 32 B), else the row.
+  if (cast_mode == KVBM_CAST_BF16_TO_FP8E4M3 && (src_row_bytes & 1)) return cudaErrorInvalidValue;
+  const uint64_t dst_row_bytes = cast_mode == KVBM_CAST_FP8E4M3_TO_BF16   ? 2ull * src_row_bytes
+                                 : cast_mode == KVBM_CAST_BF16_TO_FP8E4M3 ? src_row_bytes / 2
+                                                                          : src_row_bytes;
+  const uint64_t walk_row = cast_mode == KVBM_CAST_BF16_TO_FP8E4M3 ? dst_row_bytes : src_row_bytes;
+  RowSplit r;
+  if (page_size == 0 || !row_split(walk_row, page_size, &r)) return cudaErrorInvalidValue;
+  if (static_cast<uint64_t>(page_size) * dst_num_heads * dst_row_bytes != dst->layout.region_bytes) return cudaErrorInvalidValue;
+  GatherParams P{};
+  if (!fill_permute_side(*dst, nl, no, dst_num_heads, page_size, static_cast<uint32_t>(dst_row_bytes), &P.D)) return cudaErrorInvalidValue;
+  uint32_t covered = 0;
+  for (int s = 0; s < num_srcs; ++s) {
+    const kvbm_permute_source& X = srcs[s];
+    if (!X.side.block_ids || !X.side.layout.layer_base || X.side.layout.num_layers != nl || X.side.layout.outer_dim != no)
+      return cudaErrorInvalidValue;
+    if (X.head_count == 0 || static_cast<uint64_t>(X.src_head_begin) + X.head_count > X.num_heads ||
+        static_cast<uint64_t>(X.dst_head_begin) + X.head_count > dst_num_heads)
+      return cudaErrorInvalidValue;
+    for (int t = 0; t < s; ++t)  // two windows writing the same destination head would race
+      if (X.dst_head_begin < srcs[t].dst_head_begin + srcs[t].head_count && srcs[t].dst_head_begin < X.dst_head_begin + X.head_count)
+        return cudaErrorInvalidValue;
+    if (static_cast<uint64_t>(page_size) * X.num_heads * src_row_bytes != X.side.layout.region_bytes) return cudaErrorInvalidValue;
+    GatherSource& G = P.src[s];
+    if (!fill_permute_side(X.side, nl, no, X.num_heads, page_size, src_row_bytes, &G.S)) return cudaErrorInvalidValue;
+    if (static_cast<uint64_t>(covered) + X.head_count > max_covered) return cudaErrorInvalidValue;
+    G.s_win = X.src_head_begin * G.S.head_stride;  // the windows' first heads
+    G.d_win = X.dst_head_begin * P.D.head_stride;
+    G.first = covered;
+    if (num_srcs > 1)
+      for (uint32_t j = 0; j < X.head_count; ++j) P.entry[covered + j] = static_cast<uint8_t>(s);
+    covered += X.head_count;
+  }
+  P.covered = covered;
+  const uint64_t units = static_cast<uint64_t>(num_blocks) * (layer_end - layer_begin) * no;
+  if (units >= (1ull << 31)) return cudaErrorInvalidValue;
+  const int threads = static_cast<int>(std::min<uint32_t>(8, covered)) * 32;
+  const unsigned grid = static_cast<unsigned>(units);
+  const uint32_t lb = static_cast<uint32_t>(layer_begin), nlay = static_cast<uint32_t>(layer_end - layer_begin);
+  with_walk_kernel(cast_mode, r.pow2, cast_scales != nullptr, [&](auto c, auto p, auto sc) {
+    const GatherSource& G = P.src[0];
+    if (num_srcs == 1)
+      kvbm_paged_permute_kernel<c, p, sc><<<grid, threads, 0, stream>>>(G.S, P.D, lb, nlay, no, covered, page_size, r, G.s_win, G.d_win, cast_scales);
+    else
+      kvbm_paged_gather_kernel<c, p, sc><<<grid, threads, 0, stream>>>(P, lb, nlay, no, page_size, r, cast_scales);
+  });
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  return finish();
 }
 
 }  // namespace kvbm
@@ -1050,65 +1091,9 @@ kvbm_kernels_paged_permute_heads_scaled(const kvbm_permute_side* src, const kvbm
                                         int cast_mode, const float* cast_scales, uint32_t* done_flag, uint32_t epoch,
                                         uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
 {
-  if (num_blocks < 0 || layer_begin < 0 || layer_end < layer_begin) return cudaErrorInvalidValue;
-  if (cast_mode < KVBM_CAST_NONE || cast_mode > KVBM_CAST_BF16_TO_FP8E4M3) return cudaErrorInvalidValue;
-  if (cast_scales && cast_mode == KVBM_CAST_NONE) return cudaErrorInvalidValue;  // scales belong to the fp8 side of a cast
-  const bool signal = done_flag || completion_flag;
-  auto finish = [&]() -> cudaError_t {
-    if (!signal) return cudaSuccess;
-    kvbm_signal_kernel<<<1, 1, 0, stream>>>(done_flag, epoch, completion_flag, completion_value);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    return cudaGetLastError();
-  };
-  if (num_blocks == 0 || layer_end == layer_begin) return finish();
-  if (!src || !dst || !src->block_ids || !dst->block_ids || !src->layout.layer_base || !dst->layout.layer_base) return cudaErrorInvalidValue;
-  const uint32_t nl = src->layout.num_layers, no = src->layout.outer_dim;
-  if (nl == 0 || no == 0 || nl != dst->layout.num_layers || no != dst->layout.outer_dim || static_cast<uint32_t>(layer_end) > nl) return cudaErrorInvalidValue;
-  // The walk splits the fp8 side's row into 16 B vectors when casting (the bf16 side's vectors are 32 B), else the row.
-  if (cast_mode == KVBM_CAST_BF16_TO_FP8E4M3 && (src_row_bytes & 1)) return cudaErrorInvalidValue;
-  const uint64_t dst_row_bytes = cast_mode == KVBM_CAST_FP8E4M3_TO_BF16   ? 2ull * src_row_bytes
-                                 : cast_mode == KVBM_CAST_BF16_TO_FP8E4M3 ? src_row_bytes / 2
-                                                                          : src_row_bytes;
-  const uint64_t walk_row = cast_mode == KVBM_CAST_BF16_TO_FP8E4M3 ? dst_row_bytes : src_row_bytes;
-  RowSplit r;
-  if (head_count == 0 || page_size == 0 || !row_split(walk_row, page_size, &r)) return cudaErrorInvalidValue;
-  if (static_cast<uint64_t>(src_head_begin) + head_count > src_num_heads || static_cast<uint64_t>(dst_head_begin) + head_count > dst_num_heads)
-    return cudaErrorInvalidValue;
-  const uint64_t s_rows = static_cast<uint64_t>(page_size) * src_num_heads, d_rows = static_cast<uint64_t>(page_size) * dst_num_heads;
-  if (s_rows * src_row_bytes != src->layout.region_bytes || d_rows * dst_row_bytes != dst->layout.region_bytes) return cudaErrorInvalidValue;
-  PermuteSide S, D;
-  if (!fill_permute_side(*src, nl, no, src_num_heads, page_size, src_row_bytes, &S) ||
-      !fill_permute_side(*dst, nl, no, dst_num_heads, page_size, static_cast<uint32_t>(dst_row_bytes), &D))
-    return cudaErrorInvalidValue;
-  const uint64_t units = static_cast<uint64_t>(num_blocks) * (layer_end - layer_begin) * no;
-  if (units >= (1ull << 31)) return cudaErrorInvalidValue;
-  const int threads = static_cast<int>(std::min<uint32_t>(8, head_count)) * 32;
-  const unsigned grid = static_cast<unsigned>(units);
-  const uint32_t lb = static_cast<uint32_t>(layer_begin), nlay = static_cast<uint32_t>(layer_end - layer_begin);
-  const uint64_t s_win = src_head_begin * S.head_stride, d_win = dst_head_begin * D.head_stride;  // the windows' first heads
-  auto go = [&](auto kern) { kern<<<grid, threads, 0, stream>>>(S, D, lb, nlay, no, head_count, page_size, r, s_win, d_win, cast_scales); };
-  const bool sc = cast_scales != nullptr;
-  switch (cast_mode) {
-    case KVBM_CAST_NONE:
-      r.pow2 ? go(kvbm_paged_permute_kernel<KVBM_CAST_NONE, true>) : go(kvbm_paged_permute_kernel<KVBM_CAST_NONE, false>);
-      break;
-    case KVBM_CAST_FP8E4M3_TO_BF16:
-      if (sc)
-        r.pow2 ? go(kvbm_paged_permute_kernel<KVBM_CAST_FP8E4M3_TO_BF16, true, true>) : go(kvbm_paged_permute_kernel<KVBM_CAST_FP8E4M3_TO_BF16, false, true>);
-      else
-        r.pow2 ? go(kvbm_paged_permute_kernel<KVBM_CAST_FP8E4M3_TO_BF16, true>) : go(kvbm_paged_permute_kernel<KVBM_CAST_FP8E4M3_TO_BF16, false>);
-      break;
-    default:
-      if (sc)
-        r.pow2 ? go(kvbm_paged_permute_kernel<KVBM_CAST_BF16_TO_FP8E4M3, true, true>) : go(kvbm_paged_permute_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false, true>);
-      else
-        r.pow2 ? go(kvbm_paged_permute_kernel<KVBM_CAST_BF16_TO_FP8E4M3, true>) : go(kvbm_paged_permute_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false>);
-      break;
-  }
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return e;
-  return finish();
+  const kvbm_permute_source one{src ? *src : kvbm_permute_side{}, src_num_heads, src_head_begin, dst_head_begin, head_count};
+  return launch_paged_permute(&one, 1, dst, dst_num_heads, num_blocks, layer_begin, layer_end, page_size, src_row_bytes, cast_mode,
+                              cast_scales, done_flag, epoch, completion_flag, completion_value, UINT32_MAX, stream);
 }
 
 extern "C" cudaError_t
@@ -1128,82 +1113,8 @@ kvbm_kernels_paged_permute_gather_scaled(const kvbm_permute_source* srcs, int nu
                                          uint32_t src_row_bytes, int cast_mode, const float* cast_scales, uint32_t* done_flag,
                                          uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
 {
-  if (num_blocks < 0 || layer_begin < 0 || layer_end < layer_begin) return cudaErrorInvalidValue;
-  if (cast_mode < KVBM_CAST_NONE || cast_mode > KVBM_CAST_BF16_TO_FP8E4M3) return cudaErrorInvalidValue;
-  if (cast_scales && cast_mode == KVBM_CAST_NONE) return cudaErrorInvalidValue;
-  if (!srcs || num_srcs < 1 || num_srcs > KVBM_GATHER_MAX_SOURCES) return cudaErrorInvalidValue;
-  const bool signal = done_flag || completion_flag;
-  auto finish = [&]() -> cudaError_t {
-    if (!signal) return cudaSuccess;
-    kvbm_signal_kernel<<<1, 1, 0, stream>>>(done_flag, epoch, completion_flag, completion_value);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    return cudaGetLastError();
-  };
-  if (num_blocks == 0 || layer_end == layer_begin) return finish();
-  if (!dst || !dst->block_ids || !dst->layout.layer_base) return cudaErrorInvalidValue;
-  const uint32_t nl = dst->layout.num_layers, no = dst->layout.outer_dim;
-  if (nl == 0 || no == 0 || static_cast<uint32_t>(layer_end) > nl) return cudaErrorInvalidValue;
-  // the row rules of kvbm_kernels_paged_permute_heads, shared by every source
-  if (cast_mode == KVBM_CAST_BF16_TO_FP8E4M3 && (src_row_bytes & 1)) return cudaErrorInvalidValue;
-  const uint64_t dst_row_bytes = cast_mode == KVBM_CAST_FP8E4M3_TO_BF16   ? 2ull * src_row_bytes
-                                 : cast_mode == KVBM_CAST_BF16_TO_FP8E4M3 ? src_row_bytes / 2
-                                                                          : src_row_bytes;
-  const uint64_t walk_row = cast_mode == KVBM_CAST_BF16_TO_FP8E4M3 ? dst_row_bytes : src_row_bytes;
-  RowSplit r;
-  if (page_size == 0 || !row_split(walk_row, page_size, &r)) return cudaErrorInvalidValue;
-  if (static_cast<uint64_t>(page_size) * dst_num_heads * dst_row_bytes != dst->layout.region_bytes) return cudaErrorInvalidValue;
-  GatherParams P{};
-  if (!fill_permute_side(*dst, nl, no, dst_num_heads, page_size, static_cast<uint32_t>(dst_row_bytes), &P.D)) return cudaErrorInvalidValue;
-  uint32_t covered = 0;
-  for (int s = 0; s < num_srcs; ++s) {
-    const kvbm_permute_source& X = srcs[s];
-    if (!X.side.block_ids || !X.side.layout.layer_base || X.side.layout.num_layers != nl || X.side.layout.outer_dim != no)
-      return cudaErrorInvalidValue;
-    if (X.head_count == 0 || static_cast<uint64_t>(X.src_head_begin) + X.head_count > X.num_heads ||
-        static_cast<uint64_t>(X.dst_head_begin) + X.head_count > dst_num_heads)
-      return cudaErrorInvalidValue;
-    for (int t = 0; t < s; ++t)  // two windows writing the same destination head would race
-      if (X.dst_head_begin < srcs[t].dst_head_begin + srcs[t].head_count && srcs[t].dst_head_begin < X.dst_head_begin + X.head_count)
-        return cudaErrorInvalidValue;
-    if (static_cast<uint64_t>(page_size) * X.num_heads * src_row_bytes != X.side.layout.region_bytes) return cudaErrorInvalidValue;
-    GatherSource& G = P.src[s];
-    if (!fill_permute_side(X.side, nl, no, X.num_heads, page_size, src_row_bytes, &G.S)) return cudaErrorInvalidValue;
-    if (covered + X.head_count > KVBM_GATHER_MAX_HEADS) return cudaErrorInvalidValue;
-    G.s_win = X.src_head_begin * G.S.head_stride;
-    G.d_win = X.dst_head_begin * P.D.head_stride;
-    G.first = covered;
-    for (uint32_t j = 0; j < X.head_count; ++j) P.entry[covered + j] = static_cast<uint8_t>(s);
-    covered += X.head_count;
-  }
-  P.covered = covered;
-  const uint64_t units = static_cast<uint64_t>(num_blocks) * (layer_end - layer_begin) * no;
-  if (units >= (1ull << 31)) return cudaErrorInvalidValue;
-  const int threads = static_cast<int>(std::min<uint32_t>(8, covered)) * 32;
-  const unsigned grid = static_cast<unsigned>(units);
-  const uint32_t lb = static_cast<uint32_t>(layer_begin), nlay = static_cast<uint32_t>(layer_end - layer_begin);
-  auto go = [&](auto kern) { kern<<<grid, threads, 0, stream>>>(P, lb, nlay, no, page_size, r, cast_scales); };
-  const bool sc = cast_scales != nullptr;
-  switch (cast_mode) {
-    case KVBM_CAST_NONE:
-      r.pow2 ? go(kvbm_paged_gather_kernel<KVBM_CAST_NONE, true>) : go(kvbm_paged_gather_kernel<KVBM_CAST_NONE, false>);
-      break;
-    case KVBM_CAST_FP8E4M3_TO_BF16:
-      if (sc)
-        r.pow2 ? go(kvbm_paged_gather_kernel<KVBM_CAST_FP8E4M3_TO_BF16, true, true>) : go(kvbm_paged_gather_kernel<KVBM_CAST_FP8E4M3_TO_BF16, false, true>);
-      else
-        r.pow2 ? go(kvbm_paged_gather_kernel<KVBM_CAST_FP8E4M3_TO_BF16, true>) : go(kvbm_paged_gather_kernel<KVBM_CAST_FP8E4M3_TO_BF16, false>);
-      break;
-    default:
-      if (sc)
-        r.pow2 ? go(kvbm_paged_gather_kernel<KVBM_CAST_BF16_TO_FP8E4M3, true, true>) : go(kvbm_paged_gather_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false, true>);
-      else
-        r.pow2 ? go(kvbm_paged_gather_kernel<KVBM_CAST_BF16_TO_FP8E4M3, true>) : go(kvbm_paged_gather_kernel<KVBM_CAST_BF16_TO_FP8E4M3, false>);
-      break;
-  }
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return e;
-  return finish();
+  return launch_paged_permute(srcs, num_srcs, dst, dst_num_heads, num_blocks, layer_begin, layer_end, page_size, src_row_bytes, cast_mode,
+                              cast_scales, done_flag, epoch, completion_flag, completion_value, KVBM_GATHER_MAX_HEADS, stream);
 }
 
 extern "C" bool
