@@ -572,19 +572,16 @@ __device__ __forceinline__ void ring_consumer(const RingSmem& sm, int ndst_rt, c
       ptx::fence_proxy_async_smem();
       __syncwarp();
       if (lane == 0) {
-        // SCALED rings take the destinations out of the slot's control block before handing the slot back: once it is back
-        // the producer may overwrite them, and with several destinations a store issued after the hand-back could read the
-        // next item's address (NOTES item 9)
+        // the destinations come out of the slot's control block before the slot is handed back: once it is back the producer
+        // may overwrite them with a later item's, and a store issued after the hand-back would go to that item's address
         uint64_t dst_addr[kMaxDst];
-        if constexpr (SCALED) {
 #pragma unroll
-          for (int d = 0; d < kMaxDst; ++d)
-            if (d < ndst) dst_addr[d] = c.dst[d];
-        }
+        for (int d = 0; d < kMaxDst; ++d)
+          if (d < ndst) dst_addr[d] = c.dst[d];
         ptx::mbar_arrive(sm.empty0 + 8 * slot);  // the input slot is free as soon as it has been converted
 #pragma unroll
         for (int d = 0; d < kMaxDst; ++d)
-          if (d < ndst) ptx::bulk_s2g(reinterpret_cast<void*>(SCALED ? dst_addr[d] : c.dst[d]), ob, dst_bytes);
+          if (d < ndst) ptx::bulk_s2g(reinterpret_cast<void*>(dst_addr[d]), ob, dst_bytes);
         ptx::bulk_commit();
       }
     }
