@@ -2,6 +2,7 @@
 #pragma once
 #include <cstddef>
 #include <cstdint>
+#include <exception>
 #include <string>
 #include <vector>
 
@@ -164,5 +165,19 @@ inline int make_layer_separate(const kvbm_layout_config& cfg, const uintptr_t* b
 
 // records the thread's last error message (kvbm_last_error) and returns `code`; defined in transfer_manager.cpp
 int set_last_error(int code, const std::string& msg);
+
+// Runs the body of a C ABI entry point: no exception may cross the C boundary, so one that escapes `body` becomes KVBM_ERR with
+// an "internal error" message.
+template <class F>
+int guarded(F&& body)
+{
+  try {
+    return body();
+  } catch (const std::exception& e) {
+    return set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
+  } catch (...) {
+    return set_last_error(KVBM_ERR, "internal error");
+  }
+}
 
 }  // namespace kvbm_host

@@ -23,6 +23,7 @@
 
 namespace {
 
+using kvbm_host::guarded;
 using kvbm_host::set_last_error;
 
 struct Driver {
@@ -187,7 +188,7 @@ extern "C" int kvbm_mc_supported(int device)
 
 extern "C" int kvbm_mc_group_create(int num_devices, size_t bytes_per_device, int shareable, kvbm_mc_group** out)
 {
-  try {
+  return guarded([&]() -> int {
   if (!out || num_devices < 1 || bytes_per_device == 0) return set_last_error(KVBM_ERR, "bad multicast group arguments");
   Driver& d = driver();
   if (!d.ok) return set_last_error(KVBM_ERR_CUDA, d.why);
@@ -211,16 +212,12 @@ extern "C" int kvbm_mc_group_create(int num_devices, size_t bytes_per_device, in
   }
   *out = g;
   return KVBM_OK;
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 
 extern "C" int kvbm_mc_group_export_fd(kvbm_mc_group* g, int* fd)
 {
-  try {
+  return guarded([&]() -> int {
   int rc = check_ready(g);
   if (rc) return rc;
   if (!fd) return set_last_error(KVBM_ERR, "null fd");
@@ -229,16 +226,12 @@ extern "C" int kvbm_mc_group_export_fd(kvbm_mc_group* g, int* fd)
   DRV(driver().MemExportToShareableHandle(&h, g->mc, CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR, 0));
   *fd = h;
   return KVBM_OK;
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 
 extern "C" int kvbm_mc_group_import_fd(int fd, int num_devices, size_t bytes_per_device, kvbm_mc_group** out)
 {
-  try {
+  return guarded([&]() -> int {
   if (!out || fd < 0 || num_devices < 1 || bytes_per_device == 0) return set_last_error(KVBM_ERR, "bad multicast import arguments");
   Driver& d = driver();
   if (!d.ok) return set_last_error(KVBM_ERR_CUDA, d.why);
@@ -261,18 +254,14 @@ extern "C" int kvbm_mc_group_import_fd(int fd, int num_devices, size_t bytes_per
   }
   *out = g;
   return KVBM_OK;
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 
 extern "C" size_t kvbm_mc_group_size(const kvbm_mc_group* g) { return g ? g->size : 0; }
 
 extern "C" int kvbm_mc_group_add_device(kvbm_mc_group* g, int device)
 {
-  try {
+  return guarded([&]() -> int {
   int rc = check_ready(g);
   if (rc) return rc;
   if ((rc = touch_device(device))) return rc;
@@ -280,16 +269,12 @@ extern "C" int kvbm_mc_group_add_device(kvbm_mc_group* g, int device)
   DRV(driver().DeviceGet(&dev, device));
   DRV(driver().MulticastAddDevice(g->mc, dev));
   return KVBM_OK;
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 
 extern "C" int kvbm_mc_group_bind_local(kvbm_mc_group* g, int device, void** unicast_ptr)
 {
-  try {
+  return guarded([&]() -> int {
   int rc = check_ready(g);
   if (rc) return rc;
   if (!unicast_ptr) return set_last_error(KVBM_ERR, "null out pointer");
@@ -341,11 +326,7 @@ extern "C" int kvbm_mc_group_bind_local(kvbm_mc_group* g, int device, void** uni
   g->members.push_back(mb);
   *unicast_ptr = reinterpret_cast<void*>(mb.va);
   return KVBM_OK;
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 
 // Bind memory the ENGINE already owns (a KV pool it allocated itself) instead of allocating a pool here: the range must be
@@ -353,7 +334,7 @@ extern "C" int kvbm_mc_group_bind_local(kvbm_mc_group* g, int device, void** uni
 // aligned to the multicast granularity.  The first kvbm_mc_group_size() bytes of `ptr` become this device's share.
 extern "C" int kvbm_mc_group_bind_addr(kvbm_mc_group* g, int device, void* ptr, size_t bytes)
 {
-  try {
+  return guarded([&]() -> int {
   int rc = check_ready(g);
   if (rc) return rc;
   if (!ptr || bytes < g->size) return set_last_error(KVBM_ERR, "bind_addr: the range must cover kvbm_mc_group_size() bytes");
@@ -368,16 +349,12 @@ extern "C" int kvbm_mc_group_bind_addr(kvbm_mc_group* g, int device, void* ptr, 
   mb.owned = false;
   g->members.push_back(mb);
   return KVBM_OK;
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 
 extern "C" int kvbm_mc_group_map(kvbm_mc_group* g, int device, void** multicast_ptr)
 {
-  try {
+  return guarded([&]() -> int {
   int rc = check_ready(g);
   if (rc) return rc;
   if (!multicast_ptr) return set_last_error(KVBM_ERR, "null out pointer");
@@ -403,11 +380,7 @@ extern "C" int kvbm_mc_group_map(kvbm_mc_group* g, int device, void** multicast_
   g->mappings.push_back(mp);
   *multicast_ptr = reinterpret_cast<void*>(mp.va);
   return KVBM_OK;
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 
 extern "C" void kvbm_mc_group_destroy(kvbm_mc_group* g)

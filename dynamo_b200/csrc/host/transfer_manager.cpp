@@ -529,6 +529,33 @@ static int acquire_slot(kvbm_transfer_manager* m, size_t ids_needed, size_t ws_n
   return KVBM_OK;
 }
 
+// The block tables of one launch on `stream`, optionally ordered after `wait_ev`: acquire a slot, narrow list k to int32 at
+// k * n of its pinned staging (a null list leaves its run unwritten) and upload all of them with one async copy (no host
+// sync; the reference blocks on pointers_transfered_event.synchronize(), cuda.rs:324).
+static int stage_ids(kvbm_transfer_manager* m, const size_t* const* lists, size_t num_lists, size_t n, size_t ws_needed,
+                     cudaStream_t stream, cudaEvent_t wait_ev, Slot** out, uint64_t* seq)
+{
+  int rc = acquire_slot(m, num_lists * n, ws_needed, out, seq);
+  if (rc) return rc;
+  Slot* sl = *out;
+  if (wait_ev) CU(cudaStreamWaitEvent(stream, wait_ev, 0));
+  for (size_t k = 0; k < num_lists; ++k)
+    if (lists[k])
+      for (size_t i = 0; i < n; ++i) sl->pinned_ids[k * n + i] = static_cast<int32_t>(lists[k][i]);
+  CU(cudaMemcpyAsync(sl->dev_ids, sl->pinned_ids, num_lists * n * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
+  m->h2d_bytes += num_lists * n * sizeof(int32_t);
+  return KVBM_OK;
+}
+
+// After the launch: the slot stays busy until its event, and the launch's payload is counted.
+static int finish_slot(kvbm_transfer_manager* m, Slot* sl, cudaStream_t stream, uint64_t bytes)
+{
+  CU(cudaEventRecord(sl->ev, stream));
+  sl->in_flight = true;
+  m->bytes_moved += bytes;
+  return KVBM_OK;
+}
+
 // heads: a head-window transfer, whose regions differ when the head counts do; the head rows (head_dim elements) must match
 // instead.  Both configs then carry num_heads dividing inner_dim (checked by the caller).
 static int check_compat(const Layout& S, const Layout& D, int cast, bool heads = false)
@@ -559,43 +586,29 @@ static int launch_cuda(kvbm_transfer_manager* m, Layout* S, Layout* const* D, in
                        const size_t* const* dst_ids, size_t n, bool replicate, size_t lb, size_t le,
                        const kvbm_transfer_options& o, cudaStream_t stream, cudaEvent_t wait_ev, Slot** slot_out, uint64_t* seq_out)
 {
-  // block tables: narrow to int32 into pinned staging, async upload on the transfer's stream (no host sync;
-  // the reference blocks on pointers_transfered_event.synchronize(), cuda.rs:324)
-  const size_t lists = replicate ? static_cast<size_t>(nd) + 1 : 2 * static_cast<size_t>(nd);
+  // block tables: replicate = [src, dst 0, dst 1, ...], otherwise [src 0, dst 0, src 1, dst 1, ...]
+  const size_t* lists[2 * KVBM_MAX_DESTINATIONS];
+  size_t k = 0;
+  if (replicate) lists[k++] = src_ids[0];
+  for (int d = 0; d < nd; ++d) {
+    if (!replicate) lists[k++] = src_ids[d];
+    lists[k++] = dst_ids[d];
+  }
   Slot* sl;
   uint64_t seq;
-  int rc = acquire_slot(m, lists * n, S->cfg.num_layers + 4, &sl, &seq);
+  int rc = stage_ids(m, lists, k, n, S->cfg.num_layers + 4, stream, wait_ev, &sl, &seq);
   if (rc) return rc;
-  if (wait_ev) CU(cudaStreamWaitEvent(stream, wait_ev, 0));
-  auto narrow = [&](const size_t* ids, int32_t* dstp) { for (size_t i = 0; i < n; ++i) dstp[i] = static_cast<int32_t>(ids[i]); };
-  std::vector<const int32_t*> dev_src(nd), dev_dst(nd);
-  size_t k = 0;
-  if (replicate) {
-    narrow(src_ids[0], sl->pinned_ids);
-    for (int d = 0; d < nd; ++d) dev_src[d] = sl->dev_ids;
-    k = 1;
-  }
-  for (int d = 0; d < nd; ++d) {
-    if (!replicate) {
-      narrow(src_ids[d], sl->pinned_ids + k * n);
-      dev_src[d] = sl->dev_ids + k * n;
-      ++k;
-    }
-    narrow(dst_ids[d], sl->pinned_ids + k * n);
-    dev_dst[d] = sl->dev_ids + k * n;
-    ++k;
-  }
-  CU(cudaMemcpyAsync(sl->dev_ids, sl->pinned_ids, k * n * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
-  m->h2d_bytes += k * n * sizeof(int32_t);
 
   kvbm_paged_layout sdesc = descriptor(*S);
   kvbm_paged_dst dd[KVBM_MAX_DESTINATIONS] = {};
+  uint64_t bytes = 0;
   for (int d = 0; d < nd; ++d) {
     dd[d].layout = descriptor(*D[d]);
-    dd[d].src_block_ids = dev_src[d];
-    dd[d].dst_block_ids = dev_dst[d];
+    dd[d].src_block_ids = sl->dev_ids + (replicate ? 0 : 2 * d) * n;
+    dd[d].dst_block_ids = sl->dev_ids + (replicate ? 1 + d : 2 * d + 1) * n;
     dd[d].done_flag = o.per_dst_done_flags ? o.per_dst_done_flags[d] : ((d == 0) ? o.done_flag : nullptr);
     dd[d].layer_done_flags = o.per_dst_layer_done_flags ? o.per_dst_layer_done_flags[d] : ((d == 0) ? o.layer_done_flags : nullptr);
+    bytes += n * (le - lb) * S->cfg.outer_dim * D[d]->region;
   }
   kvbm_paged_copy_opts ko{};
   ko.epoch = o.epoch;
@@ -610,51 +623,53 @@ static int launch_cuda(kvbm_transfer_manager* m, Layout* S, Layout* const* D, in
   ko.cast_scales = o.cast_scales;
   cudaError_t e = kvbm_kernels_paged_copy_v2(&sdesc, dd, nd, static_cast<int>(n), static_cast<int>(lb), static_cast<int>(le), o.cast_mode, &ko, stream);
   if (e != cudaSuccess) return fail_cuda(e, "kvbm_kernels_paged_copy_v2");
-  CU(cudaEventRecord(sl->ev, stream));
-  sl->in_flight = true;
-  for (int d = 0; d < nd; ++d) m->bytes_moved += n * (le - lb) * S->cfg.outer_dim * D[d]->region;
+  if ((rc = finish_slot(m, sl, stream, bytes))) return rc;
   *slot_out = sl;
   *seq_out = seq;
   return KVBM_OK;
 }
 
-// One entry of a gather, as execute() resolved it: the layouts, their formats, the layer range and the direct CUDA strategy.
-struct GatherEntry {
-  Layout *S, *D;
-  int src_kv, dst_kv;
-  size_t lb, le;
-  int strategy;
+// A request as resolve() validated it: its layouts and effective formats (the options override a layout's own), whether it
+// takes the permuting launch and with which head window (the whole source unless the request names one), the layer range, the
+// strategy plan and a two-hop plan's bounce layout.  `empty`: nothing to move (no blocks or an empty layer range); nothing
+// after the layer range is resolved then.
+struct Transfer {
+  Layout* S = nullptr;
+  Layout* D[KVBM_MAX_DESTINATIONS] = {};
+  Layout* B = nullptr;
+  int src_kv = KVBM_KV_UNKNOWN, dst_kv = KVBM_KV_UNKNOWN;  // dst_kv: of D[0]
+  bool permute = false;
+  kvbm_head_window window{};
+  size_t lb = 0, le = 0;
+  kvbm_transfer_plan plan{};
+  bool empty = false;
 };
 
 // The layout-transforming transfer: what select_transform_kernel's result would drive if the reference ran it inside
-// execute_transfer (it rejects the pair instead, transfer/mod.rs:128-147).  One permuting launch moves every head window w[j]
-// from source w[j].src_rank (resolved as e[j]) into e[0].D over e[0]'s layer range, with the transfer's fp8 <-> bf16 cast fused
-// in: kvbm_kernels_paged_permute_heads for one window (any head count), kvbm_kernels_paged_permute_gather for several.  Block
-// tables are uploaded like launch_cuda's, source s at s * n and the destination's at num_srcs * n, no pointer tables; the
-// completion word is written by a trailing signal kernel.
-static int launch_permute(kvbm_transfer_manager* m, const GatherEntry* e, const kvbm_head_window* w, size_t nw, size_t num_srcs,
-                          const size_t* const* src_ids, const size_t* dst_ids, size_t n, const kvbm_transfer_options& o,
-                          cudaStream_t stream, uint64_t* seq_out)
+// execute_transfer (it rejects the pair instead, transfer/mod.rs:128-147).  One permuting launch moves every entry's head window
+// from source e[j].window.src_rank into e[0].D over e[0]'s layer range, with the transfer's fp8 <-> bf16 cast fused in:
+// kvbm_kernels_paged_permute_heads for one window (any head count), kvbm_kernels_paged_permute_gather for several.  Block
+// tables: source s at s * n and the destination's at num_srcs * n, no pointer tables; the completion word is written by a
+// trailing signal kernel.
+static int launch_permute(kvbm_transfer_manager* m, const Transfer* e, size_t nw, size_t num_srcs, const size_t* const* src_ids,
+                          const size_t* dst_ids, size_t n, const kvbm_transfer_options& o, cudaStream_t stream, uint64_t* seq_out)
 {
+  std::vector<const size_t*> lists(src_ids, src_ids + num_srcs);
+  lists.push_back(dst_ids);
   Slot* sl;
   uint64_t seq;
-  int rc = acquire_slot(m, (num_srcs + 1) * n, 4, &sl, &seq);
+  int rc = stage_ids(m, lists.data(), lists.size(), n, 4, stream, nullptr, &sl, &seq);
   if (rc) return rc;
-  for (size_t s = 0; s < num_srcs; ++s)
-    if (src_ids[s])
-      for (size_t i = 0; i < n; ++i) sl->pinned_ids[s * n + i] = static_cast<int32_t>(src_ids[s][i]);
-  for (size_t i = 0; i < n; ++i) sl->pinned_ids[num_srcs * n + i] = static_cast<int32_t>(dst_ids[i]);
-  CU(cudaMemcpyAsync(sl->dev_ids, sl->pinned_ids, (num_srcs + 1) * n * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
-  m->h2d_bytes += (num_srcs + 1) * n * sizeof(int32_t);
-  const Layout *S0 = e[0].S, *D = e[0].D;
+  const Layout *S0 = e[0].S, *D = e[0].D[0];
   kvbm_permute_side pd{descriptor(*D), sl->dev_ids + num_srcs * n, e[0].dst_kv};
   kvbm_permute_source ks[KVBM_GATHER_MAX_SOURCES] = {};
   size_t heads = 0;
   for (size_t j = 0; j < nw; ++j) {
-    ks[j] = kvbm_permute_source{{descriptor(*e[j].S), sl->dev_ids + w[j].src_rank * n, e[j].src_kv}, static_cast<uint32_t>(e[j].S->cfg.num_heads),
-                                static_cast<uint32_t>(w[j].src_head_begin), static_cast<uint32_t>(w[j].dst_head_begin),
-                                static_cast<uint32_t>(w[j].head_count)};
-    heads += w[j].head_count;
+    const kvbm_head_window& w = e[j].window;
+    ks[j] = kvbm_permute_source{{descriptor(*e[j].S), sl->dev_ids + w.src_rank * n, e[j].src_kv}, static_cast<uint32_t>(e[j].S->cfg.num_heads),
+                                static_cast<uint32_t>(w.src_head_begin), static_cast<uint32_t>(w.dst_head_begin),
+                                static_cast<uint32_t>(w.head_count)};
+    heads += w.head_count;
   }
   const uint32_t dnh = static_cast<uint32_t>(D->cfg.num_heads), page = static_cast<uint32_t>(S0->cfg.page_size);
   const uint32_t row = static_cast<uint32_t>(S0->cfg.inner_dim / S0->cfg.num_heads * S0->cfg.dtype_width_bytes);
@@ -670,9 +685,7 @@ static int launch_permute(kvbm_transfer_manager* m, const GatherEntry* e, const 
                                                               o.cast_scales, o.done_flag, o.epoch, sl->host_flag, static_cast<uint32_t>(seq), stream);
     if (ce != cudaSuccess) return fail_cuda(ce, "kvbm_kernels_paged_permute_gather_scaled");
   }
-  CU(cudaEventRecord(sl->ev, stream));
-  sl->in_flight = true;
-  m->bytes_moved += n * (e[0].le - e[0].lb) * S0->cfg.outer_dim * (D->region / D->cfg.num_heads * heads);
+  if ((rc = finish_slot(m, sl, stream, n * (e[0].le - e[0].lb) * S0->cfg.outer_dim * (D->region / D->cfg.num_heads * heads)))) return rc;
   *seq_out = seq;
   return KVBM_OK;
 }
@@ -709,7 +722,7 @@ static int execute_two_hop(kvbm_transfer_manager* m, Layout* S, Layout* D, Layou
                            size_t n, const size_t* bounce_ids, size_t nb, size_t lb, size_t le, const kvbm_transfer_plan& plan,
                            const kvbm_transfer_options& o, kvbm_notification* out)
 {
-  cudaStream_t s1 = pick_stream(m, plan.first, o), s2 = pick_stream(m, plan.second, o);  // never the caller's: execute() rejects it
+  cudaStream_t s1 = pick_stream(m, plan.first, o), s2 = pick_stream(m, plan.second, o);  // never the caller's: resolve() rejects it
   nb = std::min(nb, n);
   const size_t half = nb >= 2 ? nb / 2 : nb;
   const size_t group_begin[2] = {0, half};
@@ -748,111 +761,173 @@ static int execute_two_hop(kvbm_transfer_manager* m, Layout* S, Layout* D, Layou
   return KVBM_OK;
 }
 
-// `gather`: validate one windowed entry of a gather and fill *gather instead of running it.  The caller holds the manager
-// mutex; the entry always takes the permuting path (also for a window over every head of both sides) and every check and
-// rejection text is that of a windowed execute_transfer.  An empty entry (n == 0 or an empty layer range) leaves
-// gather->strategy at -1.
-static int execute(kvbm_transfer_manager* m, kvbm_layout_handle src_h, int nd, const kvbm_layout_handle* dst_h,
-                   const size_t* const* src_ids, const size_t* const* dst_ids, size_t n, bool replicate,
-                   const kvbm_transfer_options* opts_in, kvbm_notification* out, GatherEntry* gather = nullptr)
+// Checks that both the head-window block and the permuting path of resolve() make.  Each runs from both places because a
+// request failing several checks reports the first one in the order the two blocks make them.
+static int need_one_destination(int nd)
 {
-  kvbm_transfer_options o{};
-  if (opts_in) o = *opts_in;
-  if (out) *out = 0;
+  return nd == 1 ? KVBM_OK : fail(KVBM_ERR_UNSUPPORTED, "a layout-transforming transfer takes one destination");
+}
+// LayoutConfig::validate_for_kv_block_layout (config.rs:118-126)
+static int need_num_heads(const kvbm_layout_config& c)
+{
+  return c.num_heads ? KVBM_OK : fail(KVBM_ERR_CONFIG, "num_heads_required_for_kv_block_layout");
+}
+static int need_divisible_heads(const kvbm_layout_config& c)
+{
+  return c.inner_dim % c.num_heads ? fail(KVBM_ERR_CONFIG, "inner_dim_must_be_divisible_by_num_heads") : KVBM_OK;
+}
+
+// A head window (TP re-shard): both head counts known, the window inside both.
+static int check_head_window(const Layout& S, const Layout& D, const kvbm_head_window& w, int nd)
+{
+  const kvbm_layout_config &sc = S.cfg, &dc = D.cfg;
+  int rc;
+  if ((rc = need_one_destination(nd)) || (rc = need_num_heads(sc)) || (rc = need_num_heads(dc)) || (rc = need_divisible_heads(sc)) ||
+      (rc = need_divisible_heads(dc)))
+    return rc;
+  if (w.src_head_begin > sc.num_heads || w.head_count > sc.num_heads - w.src_head_begin || w.dst_head_begin > dc.num_heads ||
+      w.head_count > dc.num_heads - w.dst_head_begin)
+    return fail(KVBM_ERR_RANGE, "Head window src " + std::to_string(w.src_head_begin) + "+" + std::to_string(w.head_count) + " of " +
+                                    std::to_string(sc.num_heads) + " heads, dst " + std::to_string(w.dst_head_begin) + "+" +
+                                    std::to_string(w.head_count) + " of " + std::to_string(dc.num_heads) + " heads is out of range");
+  return KVBM_OK;
+}
+
+// The permuting launch on one (source, destination) pair: one destination, no layer streaming or multicast, and the geometry
+// the head-row walk needs.  With the fused cast the dtype widths differ as check_compat requires (1 -> 2 or 2 -> 1).
+static int check_permute(const Layout& S, const Layout& D, int src_kv, int dst_kv, bool window, int nd, const kvbm_transfer_options& o)
+{
+  int rc;
+  if ((rc = need_one_destination(nd))) return rc;
+  if (o.layer_ready_flags || o.layer_done_flags || o.per_dst_done_flags || o.per_dst_layer_done_flags || o.multicast)
+    return fail(KVBM_ERR_UNSUPPORTED, "layer streaming / multicast are not available on a layout-transforming transfer");
+  const kvbm_layout_config &sc = S.cfg, &dc = D.cfg;
+  if ((rc = need_num_heads(sc)) || (rc = need_num_heads(dc))) return rc;
+  if (window) {  // the head counts may differ; the heads themselves may not
+    if (sc.page_size != dc.page_size || sc.inner_dim / sc.num_heads != dc.inner_dim / dc.num_heads ||
+        (o.cast_mode == KVBM_CAST_NONE && sc.dtype_width_bytes != dc.dtype_width_bytes))
+      return fail(KVBM_ERR_INCOMPATIBLE, "a head-window transfer needs equal head_dim, page_size and dtype on both sides");
+  } else if (sc.num_heads != dc.num_heads || sc.page_size != dc.page_size || sc.inner_dim != dc.inner_dim ||
+             (o.cast_mode == KVBM_CAST_NONE && sc.dtype_width_bytes != dc.dtype_width_bytes))
+    return fail(KVBM_ERR_INCOMPATIBLE, "a layout transformation needs equal num_heads, page_size, inner_dim and dtype on both sides");
+  if ((rc = need_divisible_heads(sc))) return rc;  // after the equality above, the source's inner_dim speaks for both
+  const size_t head_dim = sc.inner_dim / sc.num_heads;
+  if (o.cast_mode != KVBM_CAST_NONE) {  // the walk splits the fp8 row (head_dim bytes) into 16 B vectors
+    if (head_dim < 16 || head_dim > 65536 || (head_dim & 15))
+      return fail(KVBM_ERR_UNSUPPORTED, "layout transformation with the fused cast: head_dim must be a multiple of 16 in 16..65536 (the fp8 row in whole "
+                                        "16-byte vectors), got " + std::to_string(head_dim));
+  } else {
+    const size_t row = head_dim * sc.dtype_width_bytes;
+    if (row < 16 || row > 65536 || (row & 15))
+      return fail(KVBM_ERR_UNSUPPORTED, "layout transformation: head_dim * dtype width must be a multiple of 16 bytes in 16..65536, got " + std::to_string(row));
+  }
+  const bool s_uni = src_kv == KVBM_KV_UNIVERSAL_TP || src_kv == KVBM_KV_UNIVERSAL_PP;
+  const bool d_uni = dst_kv == KVBM_KV_UNIVERSAL_TP || dst_kv == KVBM_KV_UNIVERSAL_PP;
+  if ((s_uni && !S.fully_contiguous) || (d_uni && !D.fully_contiguous))
+    return fail(KVBM_ERR_INCOMPATIBLE, "a universal KV block layout needs a fully contiguous pool");
+  auto aligned16 = [](const Layout& L) {
+    if ((L.block_stride | L.outer_stride) & 15) return false;
+    for (uint64_t b : L.layer_base)
+      if (b & 15) return false;
+    return true;
+  };
+  if (!aligned16(S) || !aligned16(D)) return fail(KVBM_ERR_UNSUPPORTED, "layout transformation needs 16-byte aligned pools and strides");
+  return KVBM_OK;
+}
+
+// The rejections of the strategy t->plan names, in the order its path makes them, and a two-hop plan's bounce layout.  A
+// permuting transfer passes them only on a direct CUDA strategy.
+static int check_strategy(kvbm_transfer_manager* m, int nd, const kvbm_transfer_options& o, Transfer* t)
+{
+  const kvbm_transfer_plan& p = t->plan;
+  if (!p.two_hop && p.first == KVBM_STRATEGY_MEMCPY) {
+    if (o.cast_mode != KVBM_CAST_NONE) return fail(KVBM_ERR_UNSUPPORTED, "the fused cast exists only on the CUDA strategies");
+    if (t->permute) return fail(KVBM_ERR_UNSUPPORTED, "layout transformations exist only on the CUDA strategies");
+    if (o.use_caller_stream) return fail(KVBM_ERR_UNSUPPORTED, "cuda_stream option is not supported for Memcpy strategy");  // executor/mod.rs:272-276
+    return KVBM_OK;
+  }
+  if (p.two_hop ? !cuda_strategy(p.first) || !cuda_strategy(p.second) : !cuda_strategy(p.first))
+    return fail(KVBM_ERR_UNSUPPORTED, p.two_hop ? "two-hop plans with a NIXL (disk / remote agent) leg are outside this library"
+                                                : "NIXL strategies are outside this library (the NVLink peer path replaces them)");
+  if (m->device < 0) return fail(KVBM_ERR_CUDA, "this TransferManager was created without a CUDA device; CUDA strategies have no CPU fallback");
+  if (!p.two_hop) return o.cast_scales ? check_cast_scales(m, o.cast_scales) : KVBM_OK;
+  if (nd != 1) return fail(KVBM_ERR_UNSUPPORTED, "two-hop transfers take one destination");
+  if (o.use_caller_stream) return fail(KVBM_ERR_UNSUPPORTED, "Two-hop transfers don't support caller-provided streams");  // executor/mod.rs:441
+  if (o.cast_mode != KVBM_CAST_NONE) return fail(KVBM_ERR_UNSUPPORTED, "the fused cast is not available on two-hop transfers");
+  if (t->permute) return fail(KVBM_ERR_UNSUPPORTED, "a layout transformation is not available on two-hop transfers");
+  if (!o.bounce_layout || !o.bounce_block_ids || o.num_bounce_blocks == 0)
+    return fail(KVBM_ERR, "Two-hop transfers require a bounce buffer.");  // executor/mod.rs:514-519
+  Layout* B = t->B = m->find(o.bounce_layout);
+  if (!B) return fail(KVBM_ERR_HANDLE, "invalid bounce buffer handle");
+  if (B->storage != p.bounce_location) return fail(KVBM_ERR, "Bounce buffer layout does not match bounce location.");  // :521-527
+  int rc;
+  if ((rc = check_compat(*t->S, *B, KVBM_CAST_NONE)) || (rc = check_compat(*B, *t->D[0], KVBM_CAST_NONE))) return rc;
+  std::unordered_set<size_t> seen;
+  for (size_t i = 0; i < o.num_bounce_blocks; ++i) {
+    if (o.bounce_block_ids[i] >= B->cfg.num_blocks) return fail(KVBM_ERR_RANGE, "bounce block id out of range");
+    if (!seen.insert(o.bounce_block_ids[i]).second) return fail(KVBM_ERR_DUPLICATE_DST, "duplicate bounce block id");
+  }
+  return KVBM_OK;
+}
+
+// Validate one request and resolve it into *t; the caller holds m->mu.  `heads`: a head window that always takes the permuting
+// launch (a gather's).  Without it the options' window applies, and one over every head of both sides is the transfer without a
+// window.  A request that fails several checks reports the first in the order below.
+static int resolve(kvbm_transfer_manager* m, kvbm_layout_handle src_h, int nd, const kvbm_layout_handle* dst_h,
+                   const size_t* const* src_ids, const size_t* const* dst_ids, size_t n, const kvbm_transfer_options& o,
+                   const kvbm_head_window* heads, Transfer* t)
+{
   if (nd < 1 || nd > KVBM_MAX_DESTINATIONS) return fail(KVBM_ERR, "number of destinations must be in 1..=8");
-  std::unique_lock<std::mutex> lk(m->mu, std::defer_lock);
-  if (!gather) lk.lock();
-  Layout* S = m->find(src_h);
+  Layout* S = t->S = m->find(src_h);
   if (!S) return fail(KVBM_ERR_HANDLE, "invalid source handle");
   if (S->unmapped) return fail(KVBM_ERR_UNSUPPORTED, "source layout is a descriptor of another process's host memory: not addressable from this process");
-  std::vector<Layout*> D(nd);
+  const kvbm_head_window w = heads ? *heads : kvbm_head_window{0, o.src_head_begin, o.dst_head_begin, o.head_count};
   bool window = false;
   for (int d = 0; d < nd; ++d) {
-    D[d] = m->find(dst_h[d]);
-    if (!D[d]) return fail(KVBM_ERR_HANDLE, "invalid destination handle");
-    if (D[d]->unmapped) return fail(KVBM_ERR_UNSUPPORTED, "destination layout is a descriptor of another process's host memory: not addressable from this process");
-    if (o.head_count) {  // a head window (TP re-shard): both head counts known, the window inside both
-      if (nd != 1) return fail(KVBM_ERR_UNSUPPORTED, "a layout-transforming transfer takes one destination");
-      const kvbm_layout_config &sc = S->cfg, &dc = D[d]->cfg;
-      if (!sc.num_heads || !dc.num_heads) return fail(KVBM_ERR_CONFIG, "num_heads_required_for_kv_block_layout");  // config.rs:118-126
-      if (sc.inner_dim % sc.num_heads || dc.inner_dim % dc.num_heads) return fail(KVBM_ERR_CONFIG, "inner_dim_must_be_divisible_by_num_heads");
-      if (o.src_head_begin > sc.num_heads || o.head_count > sc.num_heads - o.src_head_begin || o.dst_head_begin > dc.num_heads ||
-          o.head_count > dc.num_heads - o.dst_head_begin)
-        return fail(KVBM_ERR_RANGE, "Head window src " + std::to_string(o.src_head_begin) + "+" + std::to_string(o.head_count) + " of " +
-                                        std::to_string(sc.num_heads) + " heads, dst " + std::to_string(o.dst_head_begin) + "+" +
-                                        std::to_string(o.head_count) + " of " + std::to_string(dc.num_heads) + " heads is out of range");
-      // a window over every head of both sides is the transfer without one
-      window = gather || !(o.src_head_begin == 0 && o.dst_head_begin == 0 && o.head_count == sc.num_heads && o.head_count == dc.num_heads);
+    Layout* D = t->D[d] = m->find(dst_h[d]);
+    if (!D) return fail(KVBM_ERR_HANDLE, "invalid destination handle");
+    if (D->unmapped) return fail(KVBM_ERR_UNSUPPORTED, "destination layout is a descriptor of another process's host memory: not addressable from this process");
+    int rc;
+    if (w.head_count) {
+      if ((rc = check_head_window(*S, *D, w, nd))) return rc;
+      window = heads || !(w.src_head_begin == 0 && w.dst_head_begin == 0 && w.head_count == S->cfg.num_heads && w.head_count == D->cfg.num_heads);
     }
-    int rc = check_compat(*S, *D[d], o.cast_mode, window);
-    if (rc) return rc;
+    if ((rc = check_compat(*S, *D, o.cast_mode, window))) return rc;
     if (n && (!src_ids || !dst_ids || !src_ids[d] || !dst_ids[d])) return fail(KVBM_ERR, "null block id list");
-    rc = validate_block_transfer(src_ids[d], n, dst_ids[d], n, S->cfg.num_blocks, D[d]->cfg.num_blocks, src_h == dst_h[d]);
-    if (rc) return rc;
+    if ((rc = validate_block_transfer(src_ids[d], n, dst_ids[d], n, S->cfg.num_blocks, D->cfg.num_blocks, src_h == dst_h[d]))) return rc;
   }
   for (int d = 0; d < nd; ++d)  // select_strategy, strategy.rs:86-90
-    if (S->remote && D[d]->remote) return fail(KVBM_ERR_UNSUPPORTED, "Both src and dst are remote - this is not supported.");
+    if (S->remote && t->D[d]->remote) return fail(KVBM_ERR_UNSUPPORTED, "Both src and dst are remote - this is not supported.");
   // effective_src_layout / effective_dst_layout (executor/mod.rs:103-119): the option overrides the layout's own format.
   // The reference rejects every pair that needs a transformation (validate_layout_compatibility, transfer/mod.rs:128-147);
   // here the pairs select_transform_kernel names -- plus UniversalTP <-> UniversalPP, its TODO -- run as ONE permuting launch.
-  const int src_kv = o.src_kv_layout ? o.src_kv_layout : S->kv_block_layout;
-  int transform = KVBM_TRANSFORM_NONE;
+  const int src_kv = t->src_kv = o.src_kv_layout ? o.src_kv_layout : S->kv_block_layout;
   for (int d = 0; d < nd; ++d) {
-    const int dst_kv = o.dst_kv_layout ? o.dst_kv_layout : D[d]->kv_block_layout;
-    int t = select_transform_kernel(src_kv, dst_kv);
-    if (t == KVBM_TRANSFORM_UNSUPPORTED && (src_kv == KVBM_KV_UNIVERSAL_TP || src_kv == KVBM_KV_UNIVERSAL_PP) &&
+    const int dst_kv = o.dst_kv_layout ? o.dst_kv_layout : t->D[d]->kv_block_layout;
+    int tk = select_transform_kernel(src_kv, dst_kv);
+    if (tk == KVBM_TRANSFORM_UNSUPPORTED && (src_kv == KVBM_KV_UNIVERSAL_TP || src_kv == KVBM_KV_UNIVERSAL_PP) &&
         (dst_kv == KVBM_KV_UNIVERSAL_TP || dst_kv == KVBM_KV_UNIVERSAL_PP))
-      t = KVBM_TRANSFORM_UNIVERSAL_TO_UNIVERSAL;
+      tk = KVBM_TRANSFORM_UNIVERSAL_TO_UNIVERSAL;
     // a head window walks heads by the formats' strides, so both formats must be named ones
-    if (t == KVBM_TRANSFORM_UNSUPPORTED || (window && (!kv_known(src_kv) || !kv_known(dst_kv))))
+    if (tk == KVBM_TRANSFORM_UNSUPPORTED || (window && (!kv_known(src_kv) || !kv_known(dst_kv))))
       return fail(KVBM_ERR_UNSUPPORTED, std::string("Layout transformation not supported: src=") + kv_name(src_kv) + ", dst=" + kv_name(dst_kv));
-    if (t != KVBM_TRANSFORM_NONE || window) {  // a head window takes the permuting launch even between equal formats
-      if (nd != 1) return fail(KVBM_ERR_UNSUPPORTED, "a layout-transforming transfer takes one destination");
-      if (o.layer_ready_flags || o.layer_done_flags || o.per_dst_done_flags || o.per_dst_layer_done_flags || o.multicast)
-        return fail(KVBM_ERR_UNSUPPORTED, "layer streaming / multicast are not available on a layout-transforming transfer");
-      const kvbm_layout_config &sc = S->cfg, &dc = D[d]->cfg;
-      if (!sc.num_heads || !dc.num_heads) return fail(KVBM_ERR_CONFIG, "num_heads_required_for_kv_block_layout");  // config.rs:118-126
-      // with the fused cast the dtype widths differ as check_compat requires (1 -> 2 or 2 -> 1)
-      if (window) {  // the head counts may differ; the heads themselves may not
-        if (sc.page_size != dc.page_size || sc.inner_dim / sc.num_heads != dc.inner_dim / dc.num_heads ||
-            (o.cast_mode == KVBM_CAST_NONE && sc.dtype_width_bytes != dc.dtype_width_bytes))
-          return fail(KVBM_ERR_INCOMPATIBLE, "a head-window transfer needs equal head_dim, page_size and dtype on both sides");
-      } else if (sc.num_heads != dc.num_heads || sc.page_size != dc.page_size || sc.inner_dim != dc.inner_dim ||
-                 (o.cast_mode == KVBM_CAST_NONE && sc.dtype_width_bytes != dc.dtype_width_bytes))
-        return fail(KVBM_ERR_INCOMPATIBLE, "a layout transformation needs equal num_heads, page_size, inner_dim and dtype on both sides");
-      if (sc.inner_dim % sc.num_heads) return fail(KVBM_ERR_CONFIG, "inner_dim_must_be_divisible_by_num_heads");
-      const size_t head_dim = sc.inner_dim / sc.num_heads;
-      if (o.cast_mode != KVBM_CAST_NONE) {  // the walk splits the fp8 row (head_dim bytes) into 16 B vectors
-        if (head_dim < 16 || head_dim > 65536 || (head_dim & 15))
-          return fail(KVBM_ERR_UNSUPPORTED, "layout transformation with the fused cast: head_dim must be a multiple of 16 in 16..65536 (the fp8 row in whole "
-                                            "16-byte vectors), got " + std::to_string(head_dim));
-      } else {
-        const size_t row = head_dim * sc.dtype_width_bytes;
-        if (row < 16 || row > 65536 || (row & 15))
-          return fail(KVBM_ERR_UNSUPPORTED, "layout transformation: head_dim * dtype width must be a multiple of 16 bytes in 16..65536, got " + std::to_string(row));
-      }
-      const bool s_uni = src_kv == KVBM_KV_UNIVERSAL_TP || src_kv == KVBM_KV_UNIVERSAL_PP;
-      const bool d_uni = dst_kv == KVBM_KV_UNIVERSAL_TP || dst_kv == KVBM_KV_UNIVERSAL_PP;
-      if ((s_uni && !S->fully_contiguous) || (d_uni && !D[d]->fully_contiguous))
-        return fail(KVBM_ERR_INCOMPATIBLE, "a universal KV block layout needs a fully contiguous pool");
-      auto aligned16 = [](const Layout& L) {
-        if ((L.block_stride | L.outer_stride) & 15) return false;
-        for (uint64_t b : L.layer_base)
-          if (b & 15) return false;
-        return true;
-      };
-      if (!aligned16(*S) || !aligned16(*D[d])) return fail(KVBM_ERR_UNSUPPORTED, "layout transformation needs 16-byte aligned pools and strides");
+    // a head window takes the permuting launch even between equal formats; more than one destination never gets past here
+    t->permute = tk != KVBM_TRANSFORM_NONE || window;
+    if (t->permute) {
+      int rc = check_permute(*S, *t->D[d], src_kv, dst_kv, window, nd, o);
+      if (rc) return rc;
     }
-    transform = t;
   }
-  const bool permute = transform != KVBM_TRANSFORM_NONE || window;
-  const int dst_kv0 = o.dst_kv_layout ? o.dst_kv_layout : D[0]->kv_block_layout;
-  size_t lb = 0, le = S->cfg.num_layers;
+  t->dst_kv = o.dst_kv_layout ? o.dst_kv_layout : t->D[0]->kv_block_layout;
+  t->window = window ? w : kvbm_head_window{0, 0, 0, S->cfg.num_heads};  // a plain transform is the window over every head
+  t->lb = 0;
+  t->le = S->cfg.num_layers;
   if (o.has_layer_range) {
-    lb = o.layer_begin;
-    le = o.layer_end;
-    if (lb > le || le > S->cfg.num_layers)
-      return fail(KVBM_ERR_RANGE, "Layer range " + std::to_string(lb) + ".." + std::to_string(le) + " exceeds num_layers " + std::to_string(S->cfg.num_layers));
+    t->lb = o.layer_begin;
+    t->le = o.layer_end;
+    if (t->lb > t->le || t->le > S->cfg.num_layers)
+      return fail(KVBM_ERR_RANGE, "Layer range " + std::to_string(t->lb) + ".." + std::to_string(t->le) + " exceeds num_layers " +
+                                      std::to_string(S->cfg.num_layers));
   }
   if (o.cast_scales) {  // fp8 KV-cache scales: one per (layer, outer) of the pools, for the fp8 side of a cast
     if (o.cast_mode == KVBM_CAST_NONE) return fail(KVBM_ERR, "cast_scales need a cast_mode: they scale the fp8 side of a cast");
@@ -861,84 +936,55 @@ static int execute(kvbm_transfer_manager* m, kvbm_layout_handle src_h, int nd, c
       return fail(KVBM_ERR_RANGE, "cast_scales holds " + std::to_string(o.num_cast_scales) + " scales, the pools need num_layers * outer_dim = " +
                                       std::to_string(need));
   }
-  if (gather) *gather = GatherEntry{S, D[0], src_kv, dst_kv0, lb, le, -1};
-  if (n == 0 || lb == le) return KVBM_OK;
+  t->empty = n == 0 || t->lb == t->le;
+  if (t->empty) return KVBM_OK;
 
   // select_strategy (strategy.rs:78-108): every layout handled here is local or peer-mapped
-  kvbm_transfer_plan plan{};
   for (int d = 0; d < nd; ++d) {
+    const Layout& D = *t->D[d];
     kvbm_transfer_plan p{};
-    int rc = select_direct_strategy(S->storage, D[d]->storage, &m->caps, &p);
+    int rc = select_direct_strategy(S->storage, D.storage, &m->caps, &p);
     if (rc) return rc;
     // strategy.rs:222-233,245-278: a device pool of ANOTHER GPU is "remote"; without GPU RDMA it is reached through
     // pinned host memory: TwoHop { CudaAsyncD2H, Pinned, CudaAsyncH2D }
     if (!p.two_hop && p.first == KVBM_STRATEGY_CUDA_ASYNC_D2D && !m->caps.allow_gpu_rdma &&
-        (S->device_id != D[d]->device_id || S->remote != D[d]->remote))
+        (S->device_id != D.device_id || S->remote != D.remote))
       p = kvbm_transfer_plan{1, KVBM_STRATEGY_CUDA_ASYNC_D2H, KVBM_STORAGE_PINNED, KVBM_STRATEGY_CUDA_ASYNC_H2D};
-    if (d && (p.first != plan.first || p.two_hop != plan.two_hop)) return fail(KVBM_ERR_UNSUPPORTED, "destinations need different strategies");
-    plan = p;
+    if (d && (p.first != t->plan.first || p.two_hop != t->plan.two_hop)) return fail(KVBM_ERR_UNSUPPORTED, "destinations need different strategies");
+    t->plan = p;
   }
-  if (plan.two_hop) {
-    if (!cuda_strategy(plan.first) || !cuda_strategy(plan.second))
-      return fail(KVBM_ERR_UNSUPPORTED, "two-hop plans with a NIXL (disk / remote agent) leg are outside this library");
-    if (m->device < 0) return fail(KVBM_ERR_CUDA, "this TransferManager was created without a CUDA device; CUDA strategies have no CPU fallback");
-    if (nd != 1) return fail(KVBM_ERR_UNSUPPORTED, "two-hop transfers take one destination");
-    if (o.use_caller_stream) return fail(KVBM_ERR_UNSUPPORTED, "Two-hop transfers don't support caller-provided streams");  // executor/mod.rs:441
-    if (o.cast_mode != KVBM_CAST_NONE) return fail(KVBM_ERR_UNSUPPORTED, "the fused cast is not available on two-hop transfers");
-    if (permute) return fail(KVBM_ERR_UNSUPPORTED, "a layout transformation is not available on two-hop transfers");
-    if (!o.bounce_layout || !o.bounce_block_ids || o.num_bounce_blocks == 0)
-      return fail(KVBM_ERR, "Two-hop transfers require a bounce buffer.");  // executor/mod.rs:514-519
-    Layout* B = m->find(o.bounce_layout);
-    if (!B) return fail(KVBM_ERR_HANDLE, "invalid bounce buffer handle");
-    if (B->storage != plan.bounce_location) return fail(KVBM_ERR, "Bounce buffer layout does not match bounce location.");  // :521-527
-    int rc = check_compat(*S, *B, KVBM_CAST_NONE);
-    if (rc) return rc;
-    if ((rc = check_compat(*B, *D[0], KVBM_CAST_NONE))) return rc;
-    std::unordered_set<size_t> seen;
-    for (size_t i = 0; i < o.num_bounce_blocks; ++i) {
-      if (o.bounce_block_ids[i] >= B->cfg.num_blocks) return fail(KVBM_ERR_RANGE, "bounce block id out of range");
-      if (!seen.insert(o.bounce_block_ids[i]).second) return fail(KVBM_ERR_DUPLICATE_DST, "duplicate bounce block id");
-    }
-    DeviceGuard g(m->device);
-    return execute_two_hop(m, S, D[0], B, src_ids[0], dst_ids[0], n, o.bounce_block_ids, o.num_bounce_blocks, lb, le, plan, o, out);
-  }
+  return check_strategy(m, nd, o, t);
+}
 
-  if (plan.first == KVBM_STRATEGY_MEMCPY) {
-    if (o.cast_mode != KVBM_CAST_NONE) return fail(KVBM_ERR_UNSUPPORTED, "the fused cast exists only on the CUDA strategies");
-    if (permute) return fail(KVBM_ERR_UNSUPPORTED, "layout transformations exist only on the CUDA strategies");
-    if (o.use_caller_stream) return fail(KVBM_ERR_UNSUPPORTED, "cuda_stream option is not supported for Memcpy strategy");  // executor/mod.rs:272-276
+// execute_transfer / execute_fanout: one of four paths after validation -- two-hop, Memcpy, the permuting launch or the paged copy.
+static int execute(kvbm_transfer_manager* m, kvbm_layout_handle src_h, int nd, const kvbm_layout_handle* dst_h,
+                   const size_t* const* src_ids, const size_t* const* dst_ids, size_t n, bool replicate,
+                   const kvbm_transfer_options* opts_in, kvbm_notification* out)
+{
+  kvbm_transfer_options o{};
+  if (opts_in) o = *opts_in;
+  if (out) *out = 0;
+  std::lock_guard<std::mutex> lk(m->mu);
+  Transfer t;
+  int rc = resolve(m, src_h, nd, dst_h, src_ids, dst_ids, n, o, nullptr, &t);
+  if (rc || t.empty) return rc;
+  if (t.plan.two_hop) {
+    DeviceGuard g(m->device);
+    return execute_two_hop(m, t.S, t.D[0], t.B, src_ids[0], dst_ids[0], n, o.bounce_block_ids, o.num_bounce_blocks, t.lb, t.le, t.plan, o, out);
+  }
+  if (t.plan.first == KVBM_STRATEGY_MEMCPY) {
     for (int d = 0; d < nd; ++d) {
-      int rc = host_memcpy_transfer(*S, *D[d], src_ids[d], dst_ids[d], n, o.has_layer_range != 0, lb, le);
-      if (rc) return rc;
-      m->bytes_moved += n * (le - lb) * S->cfg.outer_dim * D[d]->region;
+      if ((rc = host_memcpy_transfer(*t.S, *t.D[d], src_ids[d], dst_ids[d], n, o.has_layer_range != 0, t.lb, t.le))) return rc;
+      m->bytes_moved += n * (t.le - t.lb) * t.S->cfg.outer_dim * t.D[d]->region;
     }
     return KVBM_OK;  // synchronous: TransferCompleteNotification::completed() (memcpy.rs:91-92)
   }
-  if (!cuda_strategy(plan.first))
-    return fail(KVBM_ERR_UNSUPPORTED, "NIXL strategies are outside this library (the NVLink peer path replaces them)");
-  if (m->device < 0) return fail(KVBM_ERR_CUDA, "this TransferManager was created without a CUDA device; CUDA strategies have no CPU fallback");
-  if (o.cast_scales) {
-    int rc = check_cast_scales(m, o.cast_scales);
-    if (rc) return rc;
-  }
-  if (gather) {
-    gather->strategy = plan.first;
-    return KVBM_OK;
-  }
-
   DeviceGuard g(m->device);
-  const cudaStream_t stream = pick_stream(m, plan.first, o);
+  const cudaStream_t stream = pick_stream(m, t.plan.first, o);
   uint64_t seq;
-  int rc;
-  if (permute) {  // a plain transform is the window over every head
-    const GatherEntry e{S, D[0], src_kv, dst_kv0, lb, le, plan.first};
-    const kvbm_head_window w = window ? kvbm_head_window{0, o.src_head_begin, o.dst_head_begin, o.head_count}
-                                      : kvbm_head_window{0, 0, 0, S->cfg.num_heads};
-    rc = launch_permute(m, &e, &w, 1, 1, src_ids, dst_ids[0], n, o, stream, &seq);
-  } else {
-    Slot* sl;
-    rc = launch_cuda(m, S, D.data(), nd, src_ids, dst_ids, n, replicate, lb, le, o, stream, nullptr, &sl, &seq);
-  }
+  Slot* sl;
+  rc = t.permute ? launch_permute(m, &t, 1, 1, src_ids, dst_ids[0], n, o, stream, &seq)
+                 : launch_cuda(m, t.S, t.D, nd, src_ids, dst_ids, n, replicate, t.lb, t.le, o, stream, nullptr, &sl, &seq);
   if (rc) return rc;
   // caller-provided stream: caller manages sync, completed() is returned (cuda.rs:139-141)
   if (out) *out = o.use_caller_stream ? 0 : seq;
@@ -971,22 +1017,18 @@ static int execute_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_
   }
   if (n && (!src_ids || !dst_ids)) return fail(KVBM_ERR, "null block id list");
   std::lock_guard<std::mutex> lk(m->mu);
-  std::vector<GatherEntry> e(nw);
+  Transfer e[KVBM_GATHER_MAX_SOURCES];
   for (size_t j = 0; j < nw; ++j) {
-    kvbm_transfer_options oj = o;
-    oj.src_head_begin = windows[j].src_head_begin;
-    oj.dst_head_begin = windows[j].dst_head_begin;
-    oj.head_count = windows[j].head_count;
     const size_t* s = src_ids ? src_ids[windows[j].src_rank] : nullptr;
-    int rc = execute(m, srcs[windows[j].src_rank], 1, &dst_h, &s, &dst_ids, n, true, &oj, nullptr, &e[j]);
+    int rc = resolve(m, srcs[windows[j].src_rank], 1, &dst_h, &s, &dst_ids, n, o, &windows[j], &e[j]);
     if (rc) return rc;
-    if (e[j].strategy != e[0].strategy) return fail(KVBM_ERR_UNSUPPORTED, "the sources of a gather need the same CUDA strategy");
+    if (e[j].plan.first != e[0].plan.first) return fail(KVBM_ERR_UNSUPPORTED, "the sources of a gather need the same CUDA strategy");
   }
-  if (e[0].strategy < 0) return KVBM_OK;  // nothing to move (no blocks or an empty layer range), as execute()
+  if (e[0].empty) return KVBM_OK;  // nothing to move (no blocks or an empty layer range), as execute()
 
   DeviceGuard g(m->device);
   uint64_t seq;
-  int rc = launch_permute(m, e.data(), windows, nw, num_srcs, src_ids, dst_ids, n, o, pick_stream(m, e[0].strategy, o), &seq);
+  int rc = launch_permute(m, e, nw, num_srcs, src_ids, dst_ids, n, o, pick_stream(m, e[0].plan.first, o), &seq);
   if (rc) return rc;
   // caller-provided stream: caller manages sync, completed() is returned, as execute()
   if (out) *out = o.use_caller_stream ? 0 : seq;
@@ -1002,88 +1044,64 @@ extern "C" const char* kvbm_last_error(void) { return g_last_error.c_str(); }
 
 extern "C" int kvbm_layout_config_validate(const kvbm_layout_config* cfg)
 {
-  try {
+  return guarded([&]() -> int {
   if (!cfg) return fail(KVBM_ERR, "null config");
   std::string why;
   int rc = validate_config(*cfg, &why);
   return rc ? fail(rc, why) : KVBM_OK;
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 extern "C" size_t kvbm_layout_required_bytes(const kvbm_layout_config* cfg) { return cfg ? required_bytes(*cfg) : 0; }
 extern "C" size_t kvbm_layout_bytes_per_block(const kvbm_layout_config* cfg) { return cfg ? bytes_per_block(*cfg) : 0; }
 
 extern "C" int kvbm_select_direct_strategy(int src_kind, int dst_kind, const kvbm_transfer_capabilities* caps, kvbm_transfer_plan* out)
 {
-  try {
+  return guarded([&]() -> int {
   if (!out) return fail(KVBM_ERR, "null plan");
   return select_direct_strategy(src_kind, dst_kind, caps, out);
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 
 extern "C" int kvbm_select_direct_strategy_remote(int src_kind, int dst_kind, int dst_is_remote, const kvbm_transfer_capabilities* caps,
                                                   kvbm_transfer_plan* out)
 {
-  try {
+  return guarded([&]() -> int {
   if (!out) return fail(KVBM_ERR, "null plan");
   return select_direct_strategy(src_kind, dst_kind, caps, out, dst_is_remote != 0);
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 
 extern "C" int kvbm_select_strategy(int src_kind, int src_is_local, int dst_kind, int dst_is_local, const kvbm_transfer_capabilities* caps,
                                     kvbm_transfer_plan* out)
 {
-  try {
+  return guarded([&]() -> int {
   if (!out) return fail(KVBM_ERR, "null plan");
   return select_strategy(src_kind, src_is_local != 0, dst_kind, dst_is_local != 0, caps, out);
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 
 extern "C" int kvbm_manager_select_strategy(kvbm_transfer_manager* m, kvbm_layout_handle src, kvbm_layout_handle dst, kvbm_transfer_plan* out)
 {
-  try {
+  return guarded([&]() -> int {
   if (!m || !out) return fail(KVBM_ERR, "null argument");
   std::lock_guard<std::mutex> lk(m->mu);
   Layout *S = m->find(src), *D = m->find(dst);
   if (!S || !D) return fail(KVBM_ERR_HANDLE, "invalid layout handle");
   return select_strategy(S->storage, !S->remote, D->storage, !D->remote, &m->caps, out);
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 
 extern "C" int kvbm_validate_block_transfer(const size_t* src_ids, size_t n_src, const size_t* dst_ids, size_t n_dst,
                                             size_t src_num_blocks, size_t dst_num_blocks, int same_layout)
 {
-  try {
+  return guarded([&]() -> int {
   return validate_block_transfer(src_ids, n_src, dst_ids, n_dst, src_num_blocks, dst_num_blocks, same_layout != 0);
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 
 extern "C" int kvbm_manager_create(int cuda_device_id, uint64_t worker_id, kvbm_transfer_manager** out)
 {
-  try {
+  return guarded([&]() -> int {
   if (!out) return fail(KVBM_ERR, "null out");
   auto m = std::make_unique<kvbm_transfer_manager>();
   m->device = cuda_device_id;
@@ -1103,11 +1121,7 @@ extern "C" int kvbm_manager_create(int cuda_device_id, uint64_t worker_id, kvbm_
   }
   *out = m.release();
   return KVBM_OK;
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 
 extern "C" void kvbm_manager_destroy(kvbm_transfer_manager* m)
@@ -1156,25 +1170,21 @@ static int finish_register(kvbm_transfer_manager* m, Layout&& L, int storage_kin
 extern "C" int kvbm_manager_register_fully_contiguous(kvbm_transfer_manager* m, const kvbm_layout_config* cfg, void* base, size_t size,
                                                       int storage_kind, int device_id, kvbm_layout_handle* out)
 {
-  try {
+  return guarded([&]() -> int {
   if (!m || !cfg || !out) return fail(KVBM_ERR, "null argument");
   Layout L;
   std::string why;
   int rc = make_fully_contiguous(*cfg, reinterpret_cast<uintptr_t>(base), size, &L, &why);
   if (rc) return fail(rc, why);
   return finish_register(m, std::move(L), storage_kind, device_id, out);
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 
 extern "C" int kvbm_manager_register_layer_separate(kvbm_transfer_manager* m, const kvbm_layout_config* cfg, void* const* layer_bases,
                                                     const size_t* layer_sizes, int block_dim, int storage_kind, int device_id,
                                                     kvbm_layout_handle* out)
 {
-  try {
+  return guarded([&]() -> int {
   if (!m || !cfg || !out || !layer_bases || !layer_sizes) return fail(KVBM_ERR, "null argument");
   std::vector<uintptr_t> bases(cfg->num_layers);
   for (size_t i = 0; i < cfg->num_layers; ++i) bases[i] = reinterpret_cast<uintptr_t>(layer_bases[i]);
@@ -1183,16 +1193,12 @@ extern "C" int kvbm_manager_register_layer_separate(kvbm_transfer_manager* m, co
   int rc = make_layer_separate(*cfg, bases.data(), layer_sizes, cfg->num_layers, block_dim, &L, &why);
   if (rc) return fail(rc, why);
   return finish_register(m, std::move(L), storage_kind, device_id, out);
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 
 extern "C" int kvbm_manager_unregister(kvbm_transfer_manager* m, kvbm_layout_handle h)
 {
-  try {
+  return guarded([&]() -> int {
   if (!m) return fail(KVBM_ERR, "null manager");
   std::lock_guard<std::mutex> lk(m->mu);
   auto it = m->layouts.find(h);
@@ -1208,17 +1214,13 @@ extern "C" int kvbm_manager_unregister(kvbm_transfer_manager* m, kvbm_layout_han
   }
   m->layouts.erase(it);
   return KVBM_OK;
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 
 extern "C" int kvbm_layout_memory_region(kvbm_transfer_manager* m, kvbm_layout_handle h, size_t block, size_t layer, size_t outer,
                                          uintptr_t* addr, size_t* size)
 {
-  try {
+  return guarded([&]() -> int {
   if (!m || !addr) return fail(KVBM_ERR, "null argument");
   std::lock_guard<std::mutex> lk(m->mu);
   Layout* L = m->find(h);
@@ -1226,11 +1228,7 @@ extern "C" int kvbm_layout_memory_region(kvbm_transfer_manager* m, kvbm_layout_h
   std::string why;
   int rc = L->memory_region(block, layer, outer, addr, size, &why);
   return rc ? fail(rc, why) : KVBM_OK;
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 
 extern "C" int kvbm_layout_is_fully_contiguous(kvbm_transfer_manager* m, kvbm_layout_handle h)
@@ -1243,7 +1241,7 @@ extern "C" int kvbm_layout_is_fully_contiguous(kvbm_transfer_manager* m, kvbm_la
 
 extern "C" int kvbm_manager_enable_peer_access(kvbm_transfer_manager* m, int peer_device)
 {
-  try {
+  return guarded([&]() -> int {
   if (!m || m->device < 0) return fail(KVBM_ERR_CUDA, "manager has no CUDA device");
   if (peer_device == m->device) return KVBM_OK;
   DeviceGuard g(m->device);
@@ -1257,11 +1255,7 @@ extern "C" int kvbm_manager_enable_peer_access(kvbm_transfer_manager* m, int pee
   }
   if (e != cudaSuccess) return fail_cuda(e, "cudaDeviceEnablePeerAccess");
   return KVBM_OK;
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 
 // base address + size of the cudaMalloc allocation containing p (driver entry point, no -lcuda needed)
@@ -1287,7 +1281,7 @@ static int allocation_range(uintptr_t p, uintptr_t* base, size_t* size)
 
 extern "C" int kvbm_manager_export_metadata(kvbm_transfer_manager* m, kvbm_layout_handle h, void* buf, size_t cap, size_t* len)
 {
-  try {
+  return guarded([&]() -> int {
   if (!m || !len) return fail(KVBM_ERR, "null argument");
   std::lock_guard<std::mutex> lk(m->mu);
   Layout* L = m->find(h);
@@ -1335,11 +1329,7 @@ extern "C" int kvbm_manager_export_metadata(kvbm_transfer_manager* m, kvbm_layou
     p += sizeof(ba);
   }
   return KVBM_OK;
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 
 static int import_metadata_impl(kvbm_transfer_manager* m, const void* buf, size_t len, const void* const* local_bases, size_t num_local_bases,
@@ -1347,13 +1337,9 @@ static int import_metadata_impl(kvbm_transfer_manager* m, const void* buf, size_
 
 extern "C" int kvbm_manager_import_metadata(kvbm_transfer_manager* m, const void* buf, size_t len, kvbm_layout_handle* out)
 {
-  try {
+  return guarded([&]() -> int {
   return import_metadata_impl(m, buf, len, nullptr, 0, out);
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 
 // Host pools of another process that THIS process has mapped itself (POSIX / SysV shared memory, a hugetlbfs file, memory
@@ -1362,14 +1348,10 @@ extern "C" int kvbm_manager_import_metadata(kvbm_transfer_manager* m, const void
 extern "C" int kvbm_manager_import_metadata_mapped(kvbm_transfer_manager* m, const void* buf, size_t len, const void* const* local_bases,
                                                    size_t num_local_bases, kvbm_layout_handle* out)
 {
-  try {
+  return guarded([&]() -> int {
   if (!local_bases || num_local_bases == 0) return fail(KVBM_ERR, "local_bases: one address per allocation of the layout");
   return import_metadata_impl(m, buf, len, local_bases, num_local_bases, out);
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 
 static int import_metadata_impl(kvbm_transfer_manager* m, const void* buf, size_t len, const void* const* local_bases, size_t num_local_bases,
@@ -1452,7 +1434,7 @@ static int import_metadata_impl(kvbm_transfer_manager* m, const void* buf, size_
 // layer_separate.rs:91-101): the format of one block of a registered layout; Unknown until set.
 extern "C" int kvbm_manager_set_kv_block_layout(kvbm_transfer_manager* m, kvbm_layout_handle h, int kv_layout)
 {
-  try {
+  return guarded([&]() -> int {
   if (!m) return fail(KVBM_ERR, "null manager");
   if (kv_layout < KVBM_KV_UNKNOWN || kv_layout > KVBM_KV_OPERATIONAL_NHD) return fail(KVBM_ERR, "unknown KvBlockLayout");
   std::lock_guard<std::mutex> lk(m->mu);
@@ -1461,18 +1443,14 @@ extern "C" int kvbm_manager_set_kv_block_layout(kvbm_transfer_manager* m, kvbm_l
   if (kv_layout != KVBM_KV_UNKNOWN) {
     // LayoutConfig::validate_for_kv_block_layout (config.rs:114-140); the head dimension is inner_dim / num_heads, the
     // figure consistent with required_bytes (:64-71) and with the chunk size K2 / K3 take
-    if (!L->cfg.num_heads) return fail(KVBM_ERR_CONFIG, "num_heads_required_for_kv_block_layout");
-    if (L->cfg.inner_dim % L->cfg.num_heads) return fail(KVBM_ERR_CONFIG, "inner_dim_must_be_divisible_by_num_heads");
+    int rc;
+    if ((rc = need_num_heads(L->cfg)) || (rc = need_divisible_heads(L->cfg))) return rc;
     if ((kv_layout == KVBM_KV_UNIVERSAL_TP || kv_layout == KVBM_KV_UNIVERSAL_PP) && !L->fully_contiguous)
       return fail(KVBM_ERR_CONFIG, "universal KV block layouts exist only on fully contiguous layouts");  // layer_separate.rs:91-101
   }
   L->kv_block_layout = kv_layout;
   return KVBM_OK;
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 
 extern "C" int kvbm_manager_kv_block_layout(kvbm_transfer_manager* m, kvbm_layout_handle h)
@@ -1529,16 +1507,12 @@ extern "C" int kvbm_manager_set_capabilities(kvbm_transfer_manager* m, const kvb
 extern "C" int kvbm_manager_execute_transfer(kvbm_transfer_manager* m, kvbm_layout_handle src, const size_t* src_ids, kvbm_layout_handle dst,
                                              const size_t* dst_ids, size_t n, const kvbm_transfer_options* opts, kvbm_notification* out)
 {
-  try {
+  return guarded([&]() -> int {
   if (!m) return fail(KVBM_ERR, "null manager");
   const size_t* s[1] = {src_ids};
   const size_t* d[1] = {dst_ids};
   return execute(m, src, 1, &dst, s, d, n, true, opts, out);
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 
 extern "C" int kvbm_manager_execute_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs,
@@ -1546,21 +1520,17 @@ extern "C" int kvbm_manager_execute_gather(kvbm_transfer_manager* m, size_t num_
                                            const kvbm_head_window* windows, size_t num_windows, const kvbm_transfer_options* opts,
                                            kvbm_notification* out)
 {
-  try {
+  return guarded([&]() -> int {
   if (!m) return fail(KVBM_ERR, "null manager");
   return execute_gather(m, num_srcs, srcs, src_ids, dst, dst_ids, n, windows, num_windows, opts, out);
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 
 extern "C" int kvbm_manager_execute_fanout(kvbm_transfer_manager* m, kvbm_layout_handle src, int num_dsts, const kvbm_layout_handle* dsts,
                                            const size_t* const* src_ids, const size_t* const* dst_ids, size_t n, int replicate,
                                            const kvbm_transfer_options* opts, kvbm_notification* out)
 {
-  try {
+  return guarded([&]() -> int {
   if (!m || !dsts) return fail(KVBM_ERR, "null argument");
   bool rep = replicate != 0;
   if (!rep && src_ids) {
@@ -1569,11 +1539,7 @@ extern "C" int kvbm_manager_execute_fanout(kvbm_transfer_manager* m, kvbm_layout
       if (src_ids[d] != src_ids[0]) rep = false;
   }
   return execute(m, src, num_dsts, dsts, src_ids, dst_ids, n, rep, opts, out);
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 
 extern "C" int kvbm_notification_is_complete(kvbm_transfer_manager* m, kvbm_notification n)
@@ -1593,7 +1559,7 @@ extern "C" int kvbm_notification_is_complete(kvbm_transfer_manager* m, kvbm_noti
 
 extern "C" int kvbm_notification_wait(kvbm_transfer_manager* m, kvbm_notification n, int64_t timeout_us)
 {
-  try {
+  return guarded([&]() -> int {
   if (!m) return fail(KVBM_ERR, "null manager");
   const auto t0 = std::chrono::steady_clock::now();
   unsigned spins = 0;
@@ -1609,11 +1575,7 @@ extern "C" int kvbm_notification_wait(kvbm_transfer_manager* m, kvbm_notificatio
       sched_yield();
     }
   }
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 
 extern "C" uint64_t kvbm_manager_bytes_moved(kvbm_transfer_manager* m) { return m ? m->bytes_moved.load() : 0; }
@@ -1701,7 +1663,7 @@ static int copy_out(const void* data, size_t need, void* buf, size_t cap, size_t
 
 extern "C" int kvbm_layout_descriptor_json(kvbm_transfer_manager* m, kvbm_layout_handle h, char* buf, size_t cap, size_t* len)
 {
-  try {
+  return guarded([&]() -> int {
   if (!m || !len) return fail(KVBM_ERR, "null argument");
   std::string js;
   {
@@ -1711,16 +1673,12 @@ extern "C" int kvbm_layout_descriptor_json(kvbm_transfer_manager* m, kvbm_layout
     js = kvbm_wire::descriptor_to_json(to_wire(*L, agent_name_of(m->worker_id)));
   }
   return copy_out(js.data(), js.size(), buf, cap, len);
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 
 extern "C" int kvbm_manager_import_descriptor_json(kvbm_transfer_manager* m, const char* json, size_t len, kvbm_layout_handle* out)
 {
-  try {
+  return guarded([&]() -> int {
   if (!m || !json || !out) return fail(KVBM_ERR, "null argument");
   kvbm_wire::Descriptor d;
   std::string why;
@@ -1747,11 +1705,7 @@ extern "C" int kvbm_manager_import_descriptor_json(kvbm_transfer_manager* m, con
                       : d.location == kvbm_wire::kDisk   ? KVBM_STORAGE_DISK
                                                          : KVBM_STORAGE_SYSTEM;
   return finish_register(m, std::move(L), storage, d.location == kvbm_wire::kDevice ? static_cast<int>(d.location_arg) : 0, out);
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 
 // TransferManager::export_metadata (manager/mod.rs:112, registry :519-556): every local host / device layout, one blob.
@@ -1759,7 +1713,7 @@ extern "C" int kvbm_manager_import_descriptor_json(kvbm_transfer_manager* m, con
 // CUDA IPC handle per allocation, so the importing process can map the pools and reach them over NVLink.
 extern "C" int kvbm_manager_export_serialized_layout(kvbm_transfer_manager* m, void* buf, size_t cap, size_t* len)
 {
-  try {
+  return guarded([&]() -> int {
   if (!m || !len) return fail(KVBM_ERR, "null argument");
   std::vector<kvbm_layout_handle> handles;
   kvbm_wire::Bundle b;
@@ -1795,18 +1749,14 @@ extern "C" int kvbm_manager_export_serialized_layout(kvbm_transfer_manager* m, v
   b.nixl_metadata = std::move(t.out);
   const std::vector<uint8_t> bytes = kvbm_wire::encode_bundle(b);
   return copy_out(bytes.data(), bytes.size(), buf, cap, len);
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
 
 // TransferManager::import_metadata (manager/mod.rs:130, registry :572-633)
 extern "C" int kvbm_manager_import_serialized_layout(kvbm_transfer_manager* m, const void* buf, size_t len, kvbm_layout_handle* out, size_t cap,
                                                      size_t* n_out)
 {
-  try {
+  return guarded([&]() -> int {
   if (!m || !buf || !n_out) return fail(KVBM_ERR, "null argument");
   kvbm_wire::Bundle b;
   std::string why;
@@ -1866,9 +1816,5 @@ extern "C" int kvbm_manager_import_serialized_layout(kvbm_transfer_manager* m, c
   std::lock_guard<std::mutex> lk(m->mu);
   m->loaded_remotes.insert(key);
   return KVBM_OK;
-  } catch (const std::exception& e) {
-    return kvbm_host::set_last_error(KVBM_ERR, std::string("internal error: ") + e.what());
-  } catch (...) {
-    return kvbm_host::set_last_error(KVBM_ERR, "internal error");
-  }
+  });
 }
