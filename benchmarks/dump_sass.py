@@ -24,6 +24,13 @@ WANT = {"paged_copy_kernelILi1ELb0ELb1": "paged_copy_fp8_to_bf16_scaled", "paged
         "paged_gather_kernelILi0ELb1": "paged_gather_pow2", "paged_gather_kernelILi0ELb0": "paged_gather_mulhi",
         "paged_gather_kernelILi1ELb1": "paged_gather_fp8_to_bf16_pow2", "paged_gather_kernelILi1ELb0": "paged_gather_fp8_to_bf16_mulhi",
         "paged_gather_kernelILi2ELb1": "paged_gather_bf16_to_fp8_pow2", "paged_gather_kernelILi2ELb0": "paged_gather_bf16_to_fp8_mulhi"}
+# the re-paging kernel: <cast, row pow2, scaled, small page pow2>, every instantiation named in full (no prefix clashes)
+for _c, _cn in ((0, ""), (1, "_fp8_to_bf16"), (2, "_bf16_to_fp8")):
+    for _sc in ((0, 1) if _c else (0,)):
+        for _r in (1, 0):
+            for _p in (1, 0):
+                WANT[f"paged_repage_kernelILi{_c}ELb{_r}ELb{_sc}ELb{_p}E"] = (
+                    f"paged_repage{_cn}_row_{'pow2' if _r else 'mulhi'}_page_{'pow2' if _p else 'mulhi'}{'_scaled' if _sc else ''}")
 KEYS = ["UBLKCP.S.G", "UBLKCP.G.S", "SYNCS.ARRIVE.TRANS64", "SYNCS.PHASECHK.TRANS64.TRYWAIT", "SYNCS.ARRIVE", "UTMACMDFLUSH", "FENCE.VIEW.ASYNC",
             "F2FP", "ATOMG", "LDG.E.NA.128", "STG.E.NA.128", "LDS.128", "STS.128", "NANOSLEEP", "SHFL"]
 

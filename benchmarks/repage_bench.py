@@ -1,0 +1,192 @@
+"""Re-paging hand-off, timed: kvbm_kernels_paged_repage moving a 4k-token sequence between block tables of different page sizes,
+against (a) the paged permute of the same bytes with equal pages (the rate to approach) and (b) what a caller has to do without
+it: K1 (kvbm_kernels_launch_vectorized_copy) over host-built pointer tables of min(Ps, Pd)-token runs, timed as the whole host
+flow (build the tables, upload them, launch, wait).  K1 cannot cast, so it runs only without --cast.
+
+Llama-3-8B KV geometry (32 layers, K/V, 8 heads x 128, bf16) on vLLM-style layer-separate NHD pools with random block tables,
+plus MLA (one outer index, one 576-wide head).  One JSON line per arm with the card's name and power limit; sample destination
+blocks of every arm are compared with tests/repage_oracle.py."""
+import argparse
+import json
+import os
+import statistics
+import subprocess
+import sys
+import time
+
+import numpy as np
+import torch
+
+ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
+sys.path.insert(0, ROOT)
+from dynamo_b200 import kernels as K  # noqa: E402
+from tests.repage_oracle import repage, table_slice  # noqa: E402
+
+p = argparse.ArgumentParser()
+p.add_argument("--tokens", type=int, default=4096)
+p.add_argument("--iters", type=int, default=20)
+p.add_argument("--cast", choices=["none", "fp8-to-bf16"], default="none")
+p.add_argument("--only", default=None, help="comma-separated config names to run")
+a = p.parse_args()
+CAST = K.CastMode.FP8E4M3_TO_BF16 if a.cast == "fp8-to-bf16" else K.CastMode.NONE
+SE, DE = (1, 2) if CAST else (2, 2)
+NHD = int(K.KvBlockLayout.OperationalNHD)
+dev = torch.device("cuda:0")
+torch.cuda.set_device(0)
+stream = torch.cuda.current_stream()
+sp = int(stream.cuda_stream)
+
+# name: (src page, dst page, token_begin, token_end, outer, heads, head_dim)
+T = a.tokens
+CONFIGS = {"16to64": (16, 64, 0, T, 2, 8, 128), "64to16": (64, 16, 0, T, 2, 8, 128), "16to16_partial": (16, 16, 0, T - 5, 2, 8, 128),
+           "1to16": (1, 16, 0, T, 2, 8, 128), "16to1": (16, 1, 0, T, 2, 8, 128), "mla_16to64": (16, 64, 0, T, 1, 1, 576)}
+NL = 32
+
+
+def card():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True)
+    name, _, limit = q.stdout.strip().partition(", ") if q.returncode == 0 else (torch.cuda.get_device_name(0), "", "not read")
+    return {"name": name, "power_limit": limit}
+
+
+class Pool:
+    """A vLLM-style layer-separate pool (block is the second dimension), NHD regions of `page` tokens."""
+
+    def __init__(self, nb, page, no, nh, hd, elem, seed):
+        self.nb, self.page, self.no, self.region = nb, page, no, page * nh * hd * elem
+        g = torch.Generator(device=dev).manual_seed(seed)
+        self.layers = [torch.randint(0, 256, (no * nb * self.region,), dtype=torch.uint8, device=dev, generator=g) for _ in range(NL)]
+        self.base = torch.tensor([t.data_ptr() for t in self.layers], dtype=torch.int64, device=dev)
+        self.desc = K.PagedLayout(self.base.data_ptr(), self.region, nb * self.region, self.region, NL, no, nb)
+
+    def block(self, b):
+        return np.concatenate([self.layers[l][o * self.nb * self.region + b * self.region:][:self.region].cpu().numpy()
+                               for l in range(NL) for o in range(self.no)])
+
+
+def timed(fn, iters=a.iters, warm=3):
+    for _ in range(warm):
+        fn()
+    torch.cuda.synchronize()
+    ts = []
+    for _ in range(iters):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(stream)
+        fn()
+        e1.record(stream)
+        e1.synchronize()
+        ts.append(e0.elapsed_time(e1))
+    return statistics.median(ts)
+
+
+def wall(fn, iters=a.iters, warm=3):
+    for _ in range(warm):
+        fn()
+        torch.cuda.synchronize()
+    ts = []
+    for _ in range(iters):
+        t0 = time.perf_counter()
+        fn()
+        torch.cuda.synchronize()
+        ts.append((time.perf_counter() - t0) * 1e3)
+    return statistics.median(ts)
+
+
+def run(name, ps, pd, tb, te, no, nh, hd):
+    rng = np.random.default_rng(0)
+    ns, nd = -(-te // ps), -(-te // pd)
+    src, dst = Pool(ns + 8, ps, no, nh, hd, SE, 1), Pool(nd + 8, pd, no, nh, hd, DE, 2)
+    stab, dtab = rng.permutation(ns + 8)[:ns].tolist(), rng.permutation(nd + 8)[:nd].tolist()
+    sids, dids = table_slice(stab, tb, te, ps), table_slice(dtab, tb, te, pd)
+    si, di = torch.tensor(sids, dtype=torch.int32, device=dev), torch.tensor(dids, dtype=torch.int32, device=dev)
+    s_row = hd * SE
+    moved = (te - tb) * NL * no * nh * hd * (SE + DE)          # bytes read + written
+    # sample destination blocks: the first, one in the middle, the last; their bytes before any arm ran
+    sample = sorted({0, len(dids) // 2, len(dids) - 1})
+    before = {j: dst.block(dids[j]) for j in sample}
+
+    def expected(j):
+        lo, hi = max(tb, (tb // pd + j) * pd), min(te, (tb // pd + j + 1) * pd)
+        s = table_slice(stab, lo, hi, ps)
+        return repage([src.block(b) for b in s], [before[j]], NHD, NHD, NL, no, nh, ps, pd, s_row, lo, hi, int(CAST))[0]
+
+    def check(arm):
+        torch.cuda.synchronize()
+        for j in sample:
+            assert np.array_equal(dst.block(dids[j]), expected(j)), (name, arm, j)
+            for l in range(NL):           # restore the sample so the next arm starts from the same bytes
+                for o in range(no):
+                    off = (l * no + o) * dst.region
+                    dst.layers[l][o * dst.nb * dst.region + dids[j] * dst.region:][:dst.region].copy_(
+                        torch.from_numpy(before[j][off:off + dst.region]))
+
+    out = []
+    info = card()
+
+    def emit(arm, ms, **kw):
+        r = {"config": name, "arm": arm, "src_page": ps, "dst_page": pd, "tokens": te - tb, "layers": NL, "outer": no, "heads": nh,
+             "head_dim": hd, "cast": a.cast, "ms": round(ms, 4), "GBps": round(moved / ms / 1e6, 1), "card": info}
+        r.update(kw)
+        print(json.dumps(r), flush=True)
+        out.append(r)
+
+    S = K.PermuteSide(src.desc, si.data_ptr(), NHD)
+    D = K.PermuteSide(dst.desc, di.data_ptr(), NHD)
+    fn = lambda: K.check(K.paged_repage(S, ps, D, pd, tb, te, 0, NL, nh, s_row, int(CAST), stream=sp), "paged_repage")  # noqa: E731
+    ms = timed(fn)
+    check("repage")
+    emit("repage", ms)
+
+    # the same bytes with equal pages: the paged permute of the big page's blocks (NHD -> NHD, fused cast as asked)
+    big = max(ps, pd)
+    nbig = -(-(te - tb) // big)
+    eq_src, eq_dst = Pool(nbig + 8, big, no, nh, hd, SE, 3), Pool(nbig + 8, big, no, nh, hd, DE, 4)
+    es = torch.tensor(rng.permutation(nbig + 8)[:nbig].tolist(), dtype=torch.int32, device=dev)
+    ed = torch.tensor(rng.permutation(nbig + 8)[:nbig].tolist(), dtype=torch.int32, device=dev)
+    ES, ED = K.PermuteSide(eq_src.desc, es.data_ptr(), NHD), K.PermuteSide(eq_dst.desc, ed.data_ptr(), NHD)
+    ms_eq = timed(lambda: K.check(K.paged_permute_cast(ES, ED, nbig, 0, NL, nh, big, s_row, int(CAST), stream=sp), "paged_permute_cast"))
+    torch.cuda.synchronize()
+    b0 = int(es[0].item()), int(ed[0].item())
+    want = repage([eq_src.block(b0[0])], [eq_dst.block(b0[1])], NHD, NHD, NL, no, nh, big, big, s_row, 0, big, int(CAST))[0]
+    assert np.array_equal(eq_dst.block(b0[1]), want), (name, "same_page")
+    emit("same_page_permute", ms_eq, page=big, blocks=nbig)
+    del eq_src, eq_dst
+
+    if CAST == K.CastMode.NONE:
+        # K1 over host-built pointer tables of min(Ps, Pd)-token runs: NHD keeps a run of tokens contiguous inside a region
+        run_t = min(ps, pd)
+        runs = [(t, min(t + run_t - (t % run_t), te)) for t in range(tb, te, run_t)] if tb % run_t == 0 else None
+        assert runs is not None
+        full = [r for r in runs if r[1] - r[0] == run_t]
+        tok_b = nh * hd * SE
+        stab_a, dtab_a = np.array(stab, dtype=np.int64), np.array(dtab, dtype=np.int64)
+        s_lay = np.array([t.data_ptr() for t in src.layers], dtype=np.int64)
+        d_lay = np.array([t.data_ptr() for t in dst.layers], dtype=np.int64)
+        t0s = np.array([r[0] for r in full], dtype=np.int64)
+
+        def k1_flow():
+            # (layer, outer, run) -> the run's address on each side
+            s_blk, s_slot = stab_a[t0s // ps], t0s % ps
+            d_blk, d_slot = dtab_a[t0s // pd], t0s % pd
+            lo = np.arange(NL * no, dtype=np.int64)
+            l_idx, o_idx = lo // no, lo % no
+            sp_tab = (s_lay[l_idx][:, None] + (o_idx * src.nb * src.region)[:, None] + (s_blk * src.region + s_slot * tok_b)[None, :]).reshape(-1)
+            dp_tab = (d_lay[l_idx][:, None] + (o_idx * dst.nb * dst.region)[:, None] + (d_blk * dst.region + d_slot * tok_b)[None, :]).reshape(-1)
+            tab = torch.from_numpy(np.concatenate([sp_tab, dp_tab])).pin_memory().to(dev, non_blocking=True)
+            n = sp_tab.size
+            K.check(K.vectorized_copy(tab.data_ptr(), tab.data_ptr() + 8 * n, run_t * tok_b, n, sp), "vectorized_copy")
+
+        if len(full) == len(runs):
+            ms_k1 = wall(k1_flow)
+            check("k1")
+            ms_rp_wall = wall(fn)
+            emit("k1_pointer_tables", ms_k1, run_tokens=run_t, pairs=NL * no * len(full), timed_as="host flow (tables, upload, launch, wait)")
+            emit("repage_host_flow", ms_rp_wall, timed_as="host flow (launch, wait)")
+    return out
+
+
+for name, cfg in CONFIGS.items():
+    if a.only and name not in a.only.split(","):
+        continue
+    run(name, *cfg)
+    torch.cuda.empty_cache()

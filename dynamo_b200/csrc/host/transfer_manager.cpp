@@ -101,13 +101,10 @@ static bool validate_fast(const size_t* src_ids, const size_t* dst_ids, size_t n
   return ok;
 }
 
-static int validate_block_transfer(const size_t* src_ids, size_t n_src, const size_t* dst_ids, size_t n_dst,
-                                   size_t src_blocks, size_t dst_blocks, bool same_layout)
+// The id checks of validate_block_transfer in its order, for lists of any lengths (a re-paging transfer's two lists differ).
+static int check_block_ids(const size_t* src_ids, size_t n_src, const size_t* dst_ids, size_t n_dst, size_t src_blocks,
+                           size_t dst_blocks, bool same_layout)
 {
-  if (n_src != n_dst)  // validation.rs:177-183
-    return fail(KVBM_ERR_LENGTH_MISMATCH, "Block ID lists have mismatched lengths: src=" + std::to_string(n_src) +
-                                              ", dst=" + std::to_string(n_dst) + ", bounce=None");
-  if (n_src == 0 || validate_fast(src_ids, dst_ids, n_src, src_blocks, dst_blocks, same_layout)) return KVBM_OK;
   std::unordered_set<size_t> seen;
   seen.reserve(n_dst * 2);
   for (size_t i = 0; i < n_dst; ++i)  // validate_dst_unique, validation.rs:55-70
@@ -118,13 +115,23 @@ static int validate_block_transfer(const size_t* src_ids, size_t n_src, const si
       if (seen.count(src_ids[i]))
         return fail(KVBM_ERR_OVERLAP, "Source and destination blocks overlap (same layout): overlapping = [" + std::to_string(src_ids[i]) + "]");
   }
-  for (size_t i = 0; i < n_src; ++i) {  // validate_block_ids_in_range, validation.rs:139-158
-    if (src_ids[i] >= src_blocks)
+  for (size_t i = 0; i < std::max(n_src, n_dst); ++i) {  // validate_block_ids_in_range, validation.rs:139-158
+    if (i < n_src && src_ids[i] >= src_blocks)
       return fail(KVBM_ERR_RANGE, "Block ID " + std::to_string(src_ids[i]) + " out of range for source (max=" + std::to_string(src_blocks) + ")");
-    if (dst_ids[i] >= dst_blocks)
+    if (i < n_dst && dst_ids[i] >= dst_blocks)
       return fail(KVBM_ERR_RANGE, "Block ID " + std::to_string(dst_ids[i]) + " out of range for destination (max=" + std::to_string(dst_blocks) + ")");
   }
   return KVBM_OK;
+}
+
+static int validate_block_transfer(const size_t* src_ids, size_t n_src, const size_t* dst_ids, size_t n_dst,
+                                   size_t src_blocks, size_t dst_blocks, bool same_layout)
+{
+  if (n_src != n_dst)  // validation.rs:177-183
+    return fail(KVBM_ERR_LENGTH_MISMATCH, "Block ID lists have mismatched lengths: src=" + std::to_string(n_src) +
+                                              ", dst=" + std::to_string(n_dst) + ", bounce=None");
+  if (n_src == 0 || validate_fast(src_ids, dst_ids, n_src, src_blocks, dst_blocks, same_layout)) return KVBM_OK;
+  return check_block_ids(src_ids, n_src, dst_ids, n_dst, src_blocks, dst_blocks, same_layout);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -529,22 +536,39 @@ static int acquire_slot(kvbm_transfer_manager* m, size_t ids_needed, size_t ws_n
   return KVBM_OK;
 }
 
-// The block tables of one launch on `stream`, optionally ordered after `wait_ev`: acquire a slot, narrow list k to int32 at
-// k * n of its pinned staging (a null list leaves its run unwritten) and upload all of them with one async copy (no host
-// sync; the reference blocks on pointers_transfered_event.synchronize(), cuda.rs:324).
-static int stage_ids(kvbm_transfer_manager* m, const size_t* const* lists, size_t num_lists, size_t n, size_t ws_needed,
+// The block tables of one launch on `stream`, optionally ordered after `wait_ev`: acquire a slot, narrow list k (lens[k] ids) to
+// int32 right after list k - 1 in its pinned staging (a null list leaves its run unwritten) and upload all of them with one async
+// copy (no host sync; the reference blocks on pointers_transfered_event.synchronize(), cuda.rs:324).
+static int stage_ids(kvbm_transfer_manager* m, const size_t* const* lists, const size_t* lens, size_t num_lists, size_t ws_needed,
                      cudaStream_t stream, cudaEvent_t wait_ev, Slot** out, uint64_t* seq)
 {
-  int rc = acquire_slot(m, num_lists * n, ws_needed, out, seq);
+  size_t total = 0;
+  for (size_t k = 0; k < num_lists; ++k) total += lens[k];
+  int rc = acquire_slot(m, total, ws_needed, out, seq);
   if (rc) return rc;
   Slot* sl = *out;
   if (wait_ev) CU(cudaStreamWaitEvent(stream, wait_ev, 0));
-  for (size_t k = 0; k < num_lists; ++k)
+  for (size_t k = 0, at = 0; k < num_lists; at += lens[k++])
     if (lists[k])
-      for (size_t i = 0; i < n; ++i) sl->pinned_ids[k * n + i] = static_cast<int32_t>(lists[k][i]);
-  CU(cudaMemcpyAsync(sl->dev_ids, sl->pinned_ids, num_lists * n * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
-  m->h2d_bytes += num_lists * n * sizeof(int32_t);
+      for (size_t i = 0; i < lens[k]; ++i) sl->pinned_ids[at + i] = static_cast<int32_t>(lists[k][i]);
+  CU(cudaMemcpyAsync(sl->dev_ids, sl->pinned_ids, total * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
+  m->h2d_bytes += total * sizeof(int32_t);
   return KVBM_OK;
+}
+
+// Lists of n ids each: list k at k * n.  A fan-out's lists fit on the stack; a gather may name any number of sources.
+static int stage_ids(kvbm_transfer_manager* m, const size_t* const* lists, size_t num_lists, size_t n, size_t ws_needed,
+                     cudaStream_t stream, cudaEvent_t wait_ev, Slot** out, uint64_t* seq)
+{
+  size_t stack[2 * KVBM_MAX_DESTINATIONS + 1];
+  std::vector<size_t> heap;
+  size_t* lens = stack;
+  if (num_lists > sizeof(stack) / sizeof(stack[0])) {
+    heap.resize(num_lists);
+    lens = heap.data();
+  }
+  for (size_t k = 0; k < num_lists; ++k) lens[k] = n;
+  return stage_ids(m, lists, lens, num_lists, ws_needed, stream, wait_ev, out, seq);
 }
 
 // After the launch: the slot stays busy until its event, and the launch's payload is counted.
@@ -793,6 +817,8 @@ static int check_head_window(const Layout& S, const Layout& D, const kvbm_head_w
   return KVBM_OK;
 }
 
+static int check_walk(const Layout& S, const Layout& D, int src_kv, int dst_kv, int cast_mode);
+
 // The permuting launch on one (source, destination) pair: one destination, no layer streaming or multicast, and the geometry
 // the head-row walk needs.  With the fused cast the dtype widths differ as check_compat requires (1 -> 2 or 2 -> 1).
 static int check_permute(const Layout& S, const Layout& D, int src_kv, int dst_kv, bool window, int nd, const kvbm_transfer_options& o)
@@ -811,8 +837,16 @@ static int check_permute(const Layout& S, const Layout& D, int src_kv, int dst_k
              (o.cast_mode == KVBM_CAST_NONE && sc.dtype_width_bytes != dc.dtype_width_bytes))
     return fail(KVBM_ERR_INCOMPATIBLE, "a layout transformation needs equal num_heads, page_size, inner_dim and dtype on both sides");
   if ((rc = need_divisible_heads(sc))) return rc;  // after the equality above, the source's inner_dim speaks for both
+  return check_walk(S, D, src_kv, dst_kv, o.cast_mode);
+}
+
+// What the head-row walk needs of a (source, destination) pair whose head_dim and dtypes check_compat accepted: whole 16-byte
+// rows (the fp8 row with a cast), a fully contiguous pool under a universal format, 16-byte aligned pools and strides.
+static int check_walk(const Layout& S, const Layout& D, int src_kv, int dst_kv, int cast_mode)
+{
+  const kvbm_layout_config& sc = S.cfg;
   const size_t head_dim = sc.inner_dim / sc.num_heads;
-  if (o.cast_mode != KVBM_CAST_NONE) {  // the walk splits the fp8 row (head_dim bytes) into 16 B vectors
+  if (cast_mode != KVBM_CAST_NONE) {  // the walk splits the fp8 row (head_dim bytes) into 16 B vectors
     if (head_dim < 16 || head_dim > 65536 || (head_dim & 15))
       return fail(KVBM_ERR_UNSUPPORTED, "layout transformation with the fused cast: head_dim must be a multiple of 16 in 16..65536 (the fp8 row in whole "
                                         "16-byte vectors), got " + std::to_string(head_dim));
@@ -835,6 +869,12 @@ static int check_permute(const Layout& S, const Layout& D, int src_kv, int dst_k
   return KVBM_OK;
 }
 
+static int need_cuda_device(const kvbm_transfer_manager* m)
+{
+  return m->device < 0 ? fail(KVBM_ERR_CUDA, "this TransferManager was created without a CUDA device; CUDA strategies have no CPU fallback")
+                       : KVBM_OK;
+}
+
 // The rejections of the strategy t->plan names, in the order its path makes them, and a two-hop plan's bounce layout.  A
 // permuting transfer passes them only on a direct CUDA strategy.
 static int check_strategy(kvbm_transfer_manager* m, int nd, const kvbm_transfer_options& o, Transfer* t)
@@ -849,7 +889,7 @@ static int check_strategy(kvbm_transfer_manager* m, int nd, const kvbm_transfer_
   if (p.two_hop ? !cuda_strategy(p.first) || !cuda_strategy(p.second) : !cuda_strategy(p.first))
     return fail(KVBM_ERR_UNSUPPORTED, p.two_hop ? "two-hop plans with a NIXL (disk / remote agent) leg are outside this library"
                                                 : "NIXL strategies are outside this library (the NVLink peer path replaces them)");
-  if (m->device < 0) return fail(KVBM_ERR_CUDA, "this TransferManager was created without a CUDA device; CUDA strategies have no CPU fallback");
+  if (int rc = need_cuda_device(m)) return rc;
   if (!p.two_hop) return o.cast_scales ? check_cast_scales(m, o.cast_scales) : KVBM_OK;
   if (nd != 1) return fail(KVBM_ERR_UNSUPPORTED, "two-hop transfers take one destination");
   if (o.use_caller_stream) return fail(KVBM_ERR_UNSUPPORTED, "Two-hop transfers don't support caller-provided streams");  // executor/mod.rs:441
@@ -1031,6 +1071,98 @@ static int execute_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_
   int rc = launch_permute(m, e, nw, num_srcs, src_ids, dst_ids, n, o, pick_stream(m, e[0].plan.first, o), &seq);
   if (rc) return rc;
   // caller-provided stream: caller manages sync, completed() is returned, as execute()
+  if (out) *out = o.use_caller_stream ? 0 : seq;
+  return KVBM_OK;
+}
+
+// Blocks a token range [tb, te) touches on a side with pages of `page` tokens: table[tb / page .. ceil(te / page)).
+static size_t repage_blocks(size_t tb, size_t te, size_t page) { return tb == te ? 0 : (te + page - 1) / page - tb / page; }
+
+// Re-paging hand-off: tokens [tb, te) of one sequence from the source's block table to the destination's, each side with its own
+// page size, as one kvbm_kernels_paged_repage launch.  Validated on its own (execute() and resolve() assume one page size and
+// equal id counts), in the order below; a request that fails several checks reports the first.
+static int execute_repage(kvbm_transfer_manager* m, kvbm_layout_handle src_h, const size_t* src_ids, size_t n_src, kvbm_layout_handle dst_h,
+                          const size_t* dst_ids, size_t n_dst, size_t tb, size_t te, const kvbm_transfer_options* opts_in, kvbm_notification* out)
+{
+  kvbm_transfer_options o{};
+  if (opts_in) o = *opts_in;
+  if (out) *out = 0;
+  std::lock_guard<std::mutex> lk(m->mu);
+  Layout* S = m->find(src_h);
+  if (!S) return fail(KVBM_ERR_HANDLE, "invalid source handle");
+  Layout* D = m->find(dst_h);
+  if (!D) return fail(KVBM_ERR_HANDLE, "invalid destination handle");
+  if (S->unmapped || D->unmapped)
+    return fail(KVBM_ERR_UNSUPPORTED, "a re-paging transfer needs both layouts addressable from this process (one is a descriptor of another process's host memory)");
+  if (S->remote && D->remote) return fail(KVBM_ERR_UNSUPPORTED, "Both src and dst are remote - this is not supported.");
+  if (o.head_count || o.layer_ready_flags || o.layer_done_flags || o.per_dst_done_flags || o.per_dst_layer_done_flags || o.multicast ||
+      o.bounce_layout || o.bounce_block_ids || o.num_bounce_blocks)
+    return fail(KVBM_ERR_UNSUPPORTED, "a re-paging transfer takes no head window, layer streaming, per-destination flags, multicast or bounce buffer");
+  const int src_kv = o.src_kv_layout ? o.src_kv_layout : S->kv_block_layout;
+  const int dst_kv = o.dst_kv_layout ? o.dst_kv_layout : D->kv_block_layout;
+  if (src_kv < KVBM_KV_UNIVERSAL_TP || src_kv > KVBM_KV_OPERATIONAL_NHD || dst_kv < KVBM_KV_UNIVERSAL_TP || dst_kv > KVBM_KV_OPERATIONAL_NHD)
+    return fail(KVBM_ERR_UNSUPPORTED, std::string("re-paging needs named KV block layouts on both sides (the format decides where a token lives): src=") +
+                                          kv_name(src_kv) + ", dst=" + kv_name(dst_kv));
+  int rc;
+  if ((rc = need_num_heads(S->cfg)) || (rc = need_num_heads(D->cfg)) || (rc = need_divisible_heads(S->cfg)) || (rc = need_divisible_heads(D->cfg)))
+    return rc;
+  if ((rc = check_compat(*S, *D, o.cast_mode, true))) return rc;
+  const size_t ps = S->cfg.page_size, pd = D->cfg.page_size;
+  if (S->cfg.num_heads != D->cfg.num_heads || (o.cast_mode == KVBM_CAST_NONE && S->cfg.dtype_width_bytes != D->cfg.dtype_width_bytes))
+    return fail(KVBM_ERR_INCOMPATIBLE, "a re-paging transfer needs equal num_heads, head_dim and dtype on both sides");
+  if (ps % pd && pd % ps)
+    return fail(KVBM_ERR_INCOMPATIBLE, "re-paging needs one page size to divide the other: src=" + std::to_string(ps) + ", dst=" + std::to_string(pd));
+  if ((rc = check_walk(*S, *D, src_kv, dst_kv, o.cast_mode))) return rc;
+  if (tb > te || te > (size_t{1} << 31))
+    return fail(KVBM_ERR_RANGE, "Token range " + std::to_string(tb) + ".." + std::to_string(te) + " is reversed or reaches past 2^31 tokens");
+  size_t lb = 0, le = S->cfg.num_layers;
+  if (o.has_layer_range) {
+    lb = o.layer_begin;
+    le = o.layer_end;
+    if (lb > le || le > S->cfg.num_layers)
+      return fail(KVBM_ERR_RANGE, "Layer range " + std::to_string(lb) + ".." + std::to_string(le) + " exceeds num_layers " +
+                                      std::to_string(S->cfg.num_layers));
+  }
+  if (o.cast_scales) {
+    if (o.cast_mode == KVBM_CAST_NONE) return fail(KVBM_ERR, "cast_scales need a cast_mode: they scale the fp8 side of a cast");
+    const size_t need = S->cfg.num_layers * S->cfg.outer_dim;
+    if (o.num_cast_scales < need)
+      return fail(KVBM_ERR_RANGE, "cast_scales holds " + std::to_string(o.num_cast_scales) + " scales, the pools need num_layers * outer_dim = " +
+                                      std::to_string(need));
+  }
+  const size_t want_src = repage_blocks(tb, te, ps), want_dst = repage_blocks(tb, te, pd);
+  if (n_src != want_src || n_dst != want_dst)
+    return fail(KVBM_ERR_LENGTH_MISMATCH, "tokens " + std::to_string(tb) + ".." + std::to_string(te) + " span " + std::to_string(want_src) +
+                                              " source and " + std::to_string(want_dst) + " destination blocks, got src=" + std::to_string(n_src) +
+                                              ", dst=" + std::to_string(n_dst));
+  if ((n_src && !src_ids) || (n_dst && !dst_ids)) return fail(KVBM_ERR, "null block id list");
+  if ((rc = check_block_ids(src_ids, n_src, dst_ids, n_dst, S->cfg.num_blocks, D->cfg.num_blocks, src_h == dst_h))) return rc;
+  if (tb == te || lb == le) return KVBM_OK;  // nothing to move, as execute()
+  kvbm_transfer_plan p{};
+  if ((rc = select_direct_strategy(S->storage, D->storage, &m->caps, &p))) return rc;
+  const bool two_hop = p.two_hop || (p.first == KVBM_STRATEGY_CUDA_ASYNC_D2D && !m->caps.allow_gpu_rdma &&
+                                     (S->device_id != D->device_id || S->remote != D->remote));
+  if (two_hop || !cuda_strategy(p.first))
+    return fail(KVBM_ERR_UNSUPPORTED, "re-paging runs on a direct CUDA strategy only (not Memcpy, two-hop or NIXL plans)");
+  if ((rc = need_cuda_device(m))) return rc;
+  if (o.cast_scales && (rc = check_cast_scales(m, o.cast_scales))) return rc;
+
+  DeviceGuard g(m->device);
+  const cudaStream_t stream = pick_stream(m, p.first, o);
+  const size_t* lists[2] = {src_ids, dst_ids};
+  const size_t lens[2] = {n_src, n_dst};
+  Slot* sl;
+  uint64_t seq;
+  if ((rc = stage_ids(m, lists, lens, 2, 4, stream, nullptr, &sl, &seq))) return rc;
+  const kvbm_permute_side ks{descriptor(*S), sl->dev_ids, src_kv}, kd{descriptor(*D), sl->dev_ids + n_src, dst_kv};
+  const size_t nh = S->cfg.num_heads, row = S->cfg.inner_dim / nh * S->cfg.dtype_width_bytes;
+  cudaError_t ce = kvbm_kernels_paged_repage(&ks, static_cast<uint32_t>(ps), &kd, static_cast<uint32_t>(pd), static_cast<uint32_t>(tb),
+                                             static_cast<uint32_t>(te), static_cast<int>(lb), static_cast<int>(le), static_cast<uint32_t>(nh),
+                                             static_cast<uint32_t>(row), o.cast_mode, o.cast_scales, o.done_flag, o.epoch, sl->host_flag,
+                                             static_cast<uint32_t>(seq), stream);
+  if (ce != cudaSuccess) return fail_cuda(ce, "kvbm_kernels_paged_repage");
+  const size_t d_row = D->cfg.inner_dim / D->cfg.num_heads * D->cfg.dtype_width_bytes;
+  if ((rc = finish_slot(m, sl, stream, (te - tb) * (le - lb) * S->cfg.outer_dim * nh * d_row))) return rc;
   if (out) *out = o.use_caller_stream ? 0 : seq;
   return KVBM_OK;
 }
@@ -1523,6 +1655,16 @@ extern "C" int kvbm_manager_execute_gather(kvbm_transfer_manager* m, size_t num_
   return guarded([&]() -> int {
   if (!m) return fail(KVBM_ERR, "null manager");
   return execute_gather(m, num_srcs, srcs, src_ids, dst, dst_ids, n, windows, num_windows, opts, out);
+  });
+}
+
+extern "C" int kvbm_manager_execute_repage(kvbm_transfer_manager* m, kvbm_layout_handle src, const size_t* src_ids, size_t n_src,
+                                           kvbm_layout_handle dst, const size_t* dst_ids, size_t n_dst, size_t token_begin, size_t token_end,
+                                           const kvbm_transfer_options* opts, kvbm_notification* out)
+{
+  return guarded([&]() -> int {
+  if (!m) return fail(KVBM_ERR, "null manager");
+  return execute_repage(m, src, src_ids, n_src, dst, dst_ids, n_dst, token_begin, token_end, opts, out);
   });
 }
 

@@ -662,6 +662,91 @@ kvbm_paged_gather_kernel(const __grid_constant__ GatherParams P, uint32_t layer_
   }
 }
 
+// Re-paging: a token range [token_begin, token_end) of one sequence between two block tables whose page sizes differ (one divides
+// the other).  Sequence token p sits in slot p % P of block ids[p / P - first] on each side, P being that side's page.  `big` is
+// the side with the larger page (the source on a tie), `small` the other; each side's strides are those of its own page.  One
+// CTA per (big block, layer, outer) unit, clipped to the token range, one warp per head.  Within a head the lane's vector v is
+// (token t of the unit, 16 B column c) by the row split; the token's slot in the big block is q = q0 + t, its small block and
+// slot come from q by the page split (a shift and a mask, or a multiply-high exact for q < 2^32 / small_page).  The walk runs
+// over all the unit's tokens, so one-token pages still keep 8 independent 16 B loads per lane in flight.
+struct RepageParams {
+  PermuteSide big, small;
+  RowSplit page;          // q -> (small block, slot): log2 / magic of the small page
+  uint32_t small_page;
+  uint32_t big_page;
+  uint32_t ratio;         // big_page / small_page
+  uint32_t big_first;     // token_begin / big_page: the big side's ids start at this block of the sequence
+  uint32_t small_first;   // token_begin / small_page
+  uint32_t token_begin, token_end;
+  uint32_t layer_begin, nlayers, no, nh;
+  uint32_t src_small;     // 1: the source is the small side
+};
+
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__global__ void __launch_bounds__(256)
+kvbm_paged_repage_kernel(const __grid_constant__ RepageParams P, RowSplit r, const float* scales)
+{
+  constexpr int IN = CAST == KVBM_CAST_BF16_TO_FP8E4M3 ? 2 : 1;   // 16 B loads per vector
+  constexpr int OUT = CAST == KVBM_CAST_FP8E4M3_TO_BF16 ? 2 : 1;  // 16 B stores per vector
+  constexpr int U = 8 / IN;
+  const uint32_t unit = blockIdx.x;  // (big block j * nlayers + l) * no + o
+  const uint32_t j = unit / (P.nlayers * P.no);
+  const uint32_t rem = unit - j * (P.nlayers * P.no);
+  const uint32_t l = P.layer_begin + rem / P.no, o = rem % P.no;
+  const uint32_t first = (P.big_first + j) * P.big_page;  // sequence position of the big block's slot 0
+  const uint32_t t0 = max(P.token_begin, first), t1 = min(P.token_end, first + P.big_page);
+  const uint32_t q0 = t0 - first;
+  // small block b of this unit is entry small_k + b of the small table; small_k wraps below 0 in the unit whose first small
+  // blocks lie before the range, and small_k + b (b >= those blocks) wraps back: index in uint32, never offset the pointer by it
+  const uint32_t small_k = (P.big_first + j) * P.ratio - P.small_first;
+  const uint8_t* big_base = reinterpret_cast<uint8_t*>(static_cast<uintptr_t>(__ldg(P.big.layer_base + (P.big.universal ? 0 : l)))) +
+                            static_cast<uint64_t>(__ldg(P.big.ids + j)) * P.big.block_stride + l * P.big.layer_step + o * P.big.outer_step;
+  const uint8_t* small_base = reinterpret_cast<uint8_t*>(static_cast<uintptr_t>(__ldg(P.small.layer_base + (P.small.universal ? 0 : l)))) +
+                              l * P.small.layer_step + o * P.small.outer_step;
+  const ptx::Scale scale = ptx::make_scale(SCALED ? __ldg(scales + l * P.no + o) : 1.f);
+  // column shifts of either side: the source's vector is 16 * IN bytes, the destination's 16 * OUT
+  const uint32_t big_shift = P.src_small ? 3 + OUT : 3 + IN, small_shift = P.src_small ? 3 + IN : 3 + OUT;
+  const uint32_t big_tok = static_cast<uint32_t>(P.big.tok_stride), small_tok = static_cast<uint32_t>(P.small.tok_stride);
+  const uint32_t run = row_run<POW2>(r, t1 - t0);
+  const int lane = threadIdx.x & 31;
+  for (uint32_t h = threadIdx.x >> 5; h < P.nh; h += blockDim.x >> 5) {
+    const uint8_t* bh = big_base + h * P.big.head_stride;
+    const uint8_t* sh = small_base + h * P.small.head_stride;
+    for (uint32_t v = lane; v < run; v += U * 32) {
+      uint4 x[U][IN];
+      uint8_t* dp[U];
+#pragma unroll
+      for (int k = 0; k < U; ++k)
+        if (v + k * 32 < run) {
+          const uint32_t vv = v + k * 32;
+          const uint32_t t = POW2 ? vv >> r.vpr : __umulhi(vv, r.magic);
+          const uint32_t c = POW2 ? vv & ((1u << r.vpr) - 1) : vv - t * r.vpr;
+          const uint32_t q = q0 + t;
+          const uint32_t b = PPOW2 ? q >> P.page.vpr : __umulhi(q, P.page.magic);
+          const uint32_t slot = PPOW2 ? q & (P.small_page - 1) : q - b * P.small_page;
+          const uint8_t* big_p = bh + q * big_tok + (c << big_shift);
+          const uint8_t* small_p = sh + static_cast<uint64_t>(__ldg(P.small.ids + (small_k + b))) * P.small.block_stride + slot * small_tok + (c << small_shift);
+          const uint8_t* s = P.src_small ? small_p : big_p;
+          dp[k] = const_cast<uint8_t*>(P.src_small ? big_p : small_p);
+#pragma unroll
+          for (int i = 0; i < IN; ++i) x[k][i] = ptx::ld_stream_v4(s + 16 * i);
+        }
+#pragma unroll
+      for (int k = 0; k < U; ++k)
+        if (v + k * 32 < run) {
+          if constexpr (CAST == KVBM_CAST_NONE) {
+            ptx::st_stream_v4(dp[k], x[k][0]);
+          } else {
+            uint4 y[OUT];
+            cast_vector<SCALED>(x[k], y, scale);  // bit for bit the paged permute's cast
+#pragma unroll
+            for (int i = 0; i < OUT; ++i) ptx::st_stream_v4(dp[k] + 16 * i, y[i]);
+          }
+        }
+    }
+  }
+}
+
 // The instantiation of the permuting kernels a launch takes for its cast mode, row split and scales: calls
 // f(integral_constant<int, CAST>, bool_constant<POW2>, bool_constant<SCALED>).  Scales without a cast take the unscaled
 // instantiation (the launch rejects them first), so no scaled kernel exists without a cast.  preload_kernels() passes every
@@ -823,6 +908,8 @@ static cudaError_t preload_kernels()
         with_walk_kernel(cast, pow2, scaled, [&](auto c, auto p, auto sc) {
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_permute_kernel<c, p, sc>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_gather_kernel<c, p, sc>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_kernel<c, p, sc, true>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_kernel<c, p, sc, false>);
         });
   return e;
 }
@@ -924,6 +1011,87 @@ static cudaError_t launch_paged_permute(const kvbm_permute_source* srcs, int num
       kvbm_paged_permute_kernel<c, p, sc><<<grid, threads, 0, stream>>>(G.S, P.D, lb, nlay, no, covered, page_size, r, G.s_win, G.d_win, cast_scales);
     else
       kvbm_paged_gather_kernel<c, p, sc><<<grid, threads, 0, stream>>>(P, lb, nlay, no, page_size, r, cast_scales);
+  });
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  return finish();
+}
+
+// kvbm_kernels_paged_repage: every check before any CUDA call, the signal on an empty range, then one re-paging launch and the
+// signal launch, as launch_paged_permute.
+static cudaError_t launch_paged_repage(const kvbm_permute_side* src, uint32_t src_page, const kvbm_permute_side* dst, uint32_t dst_page,
+                                       uint32_t token_begin, uint32_t token_end, int layer_begin, int layer_end, uint32_t nh,
+                                       uint32_t src_row_bytes, int cast_mode, const float* cast_scales, uint32_t* done_flag, uint32_t epoch,
+                                       uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
+{
+  if (layer_begin < 0 || layer_end < layer_begin || token_end < token_begin) return cudaErrorInvalidValue;
+  if (cast_mode < KVBM_CAST_NONE || cast_mode > KVBM_CAST_BF16_TO_FP8E4M3) return cudaErrorInvalidValue;
+  if (cast_scales && cast_mode == KVBM_CAST_NONE) return cudaErrorInvalidValue;
+  auto finish = [&]() -> cudaError_t {
+    if (!done_flag && !completion_flag) return cudaSuccess;
+    kvbm_signal_kernel<<<1, 1, 0, stream>>>(done_flag, epoch, completion_flag, completion_value);
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    return cudaGetLastError();
+  };
+  if (token_end == token_begin || layer_end == layer_begin) return finish();
+  if (!src || !dst || !src->block_ids || !dst->block_ids || !src->layout.layer_base || !dst->layout.layer_base) return cudaErrorInvalidValue;
+  const uint32_t nl = dst->layout.num_layers, no = dst->layout.outer_dim;
+  if (nl == 0 || no == 0 || nh == 0 || src->layout.num_layers != nl || src->layout.outer_dim != no || static_cast<uint32_t>(layer_end) > nl)
+    return cudaErrorInvalidValue;
+  if (src_page == 0 || dst_page == 0) return cudaErrorInvalidValue;
+  const bool src_small = src_page < dst_page;
+  const uint32_t big_page = src_small ? dst_page : src_page, small_page = src_small ? src_page : dst_page;
+  if (big_page % small_page) return cudaErrorInvalidValue;
+  // slot arithmetic in 32 bits: every big block of the range ends below 2^32, and the page split is exact for q < big_page
+  const uint64_t big_end = (static_cast<uint64_t>(token_end) + big_page - 1) / big_page * big_page;
+  if (big_end >= (1ull << 32) || static_cast<uint64_t>(big_page) * small_page >= (1ull << 32)) return cudaErrorInvalidValue;
+  if (cast_mode == KVBM_CAST_BF16_TO_FP8E4M3 && (src_row_bytes & 1)) return cudaErrorInvalidValue;
+  const uint64_t dst_row_bytes = cast_mode == KVBM_CAST_FP8E4M3_TO_BF16   ? 2ull * src_row_bytes
+                                 : cast_mode == KVBM_CAST_BF16_TO_FP8E4M3 ? src_row_bytes / 2
+                                                                          : src_row_bytes;
+  const uint64_t walk_row = cast_mode == KVBM_CAST_BF16_TO_FP8E4M3 ? dst_row_bytes : src_row_bytes;
+  RowSplit r;
+  if (!row_split(walk_row, big_page, &r)) return cudaErrorInvalidValue;
+  if (static_cast<uint64_t>(src_page) * nh * src_row_bytes != src->layout.region_bytes ||
+      static_cast<uint64_t>(dst_page) * nh * dst_row_bytes != dst->layout.region_bytes)
+    return cudaErrorInvalidValue;
+  PermuteSide S, D;
+  if (!fill_permute_side(*src, nl, no, nh, src_page, src_row_bytes, &S) ||
+      !fill_permute_side(*dst, nl, no, nh, dst_page, static_cast<uint32_t>(dst_row_bytes), &D))
+    return cudaErrorInvalidValue;
+  RepageParams P{};
+  P.big = src_small ? D : S;
+  P.small = src_small ? S : D;
+  P.small_page = small_page;
+  P.big_page = big_page;
+  P.ratio = big_page / small_page;
+  P.big_first = token_begin / big_page;
+  P.small_first = token_begin / small_page;
+  P.token_begin = token_begin;
+  P.token_end = token_end;
+  P.layer_begin = static_cast<uint32_t>(layer_begin);
+  P.nlayers = static_cast<uint32_t>(layer_end - layer_begin);
+  P.no = no;
+  P.nh = nh;
+  P.src_small = src_small ? 1 : 0;
+  // the small page's split, in RowSplit's form: log2 of the page, or the page and ceil(2^32 / page)
+  const bool page_pow2 = (small_page & (small_page - 1)) == 0;
+  if (page_pow2) {
+    while ((1u << P.page.vpr) < small_page) ++P.page.vpr;
+    P.page.pow2 = true;
+  } else {
+    P.page = {small_page, static_cast<uint32_t>(((1ull << 32) + small_page - 1) / small_page), false};
+  }
+  const uint64_t units = (static_cast<uint64_t>(big_end / big_page) - P.big_first) * P.nlayers * no;
+  if (units >= (1ull << 31)) return cudaErrorInvalidValue;
+  const int threads = static_cast<int>(std::min<uint32_t>(8, nh)) * 32;
+  const unsigned grid = static_cast<unsigned>(units);
+  with_walk_kernel(cast_mode, r.pow2, cast_scales != nullptr, [&](auto c, auto p, auto sc) {
+    if (page_pow2)
+      kvbm_paged_repage_kernel<c, p, sc, true><<<grid, threads, 0, stream>>>(P, r, cast_scales);
+    else
+      kvbm_paged_repage_kernel<c, p, sc, false><<<grid, threads, 0, stream>>>(P, r, cast_scales);
   });
   g_launches.fetch_add(1, std::memory_order_relaxed);
   cudaError_t e = cudaGetLastError();
@@ -1115,6 +1283,16 @@ kvbm_kernels_paged_permute_gather_scaled(const kvbm_permute_source* srcs, int nu
 {
   return launch_paged_permute(srcs, num_srcs, dst, dst_num_heads, num_blocks, layer_begin, layer_end, page_size, src_row_bytes, cast_mode,
                               cast_scales, done_flag, epoch, completion_flag, completion_value, KVBM_GATHER_MAX_HEADS, stream);
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_repage(const kvbm_permute_side* src, uint32_t src_page_size, const kvbm_permute_side* dst, uint32_t dst_page_size,
+                          uint32_t token_begin, uint32_t token_end, int layer_begin, int layer_end, uint32_t num_heads,
+                          uint32_t src_row_bytes, int cast_mode, const float* cast_scales, uint32_t* done_flag, uint32_t epoch,
+                          uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
+{
+  return launch_paged_repage(src, src_page_size, dst, dst_page_size, token_begin, token_end, layer_begin, layer_end, num_heads,
+                             src_row_bytes, cast_mode, cast_scales, done_flag, epoch, completion_flag, completion_value, stream);
 }
 
 extern "C" bool

@@ -177,6 +177,9 @@ def lib() -> C.CDLL:
         L.kvbm_kernels_paged_permute_gather_scaled.argtypes = [C.POINTER(PermuteSource), i, C.POINTER(PermuteSide), C.c_uint32, i, i, i,
                                                                C.c_uint32, C.c_uint32, i, vp, vp, C.c_uint32, vp, C.c_uint32, vp]
         L.kvbm_kernels_paged_permute_gather_scaled.restype = i
+        L.kvbm_kernels_paged_repage.argtypes = [C.POINTER(PermuteSide), C.c_uint32, C.POINTER(PermuteSide), C.c_uint32, C.c_uint32,
+                                                C.c_uint32, i, i, C.c_uint32, C.c_uint32, i, vp, vp, C.c_uint32, vp, C.c_uint32, vp]
+        L.kvbm_kernels_paged_repage.restype = i
         L.kvbm_kernels_permute_strides.argtypes = [i, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64, C.c_uint64,
                                                    C.POINTER(C.c_uint64)]
         L.kvbm_kernels_permute_strides.restype = i
@@ -200,6 +203,7 @@ EXPORTED_SYMBOLS = [
     "kvbm_kernels_launch_count", "kvbm_kernels_build_info", "kvbm_kernels_gate_would_spin", "kvbm_kernels_paged_permute",
     "kvbm_kernels_permute_strides", "kvbm_kernels_paged_permute_cast", "kvbm_kernels_paged_permute_heads",
     "kvbm_kernels_paged_permute_gather", "kvbm_kernels_paged_permute_heads_scaled", "kvbm_kernels_paged_permute_gather_scaled",
+    "kvbm_kernels_paged_repage",
 ]
 
 
@@ -323,6 +327,18 @@ def paged_permute_gather(srcs: Sequence[PermuteSource], dst: PermuteSide, dst_nu
     return lib().kvbm_kernels_paged_permute_gather(arr, len(srcs), C.byref(dst), dst_num_heads, num_blocks, layer_begin, layer_end, page_size,
                                                    src_row_bytes, int(cast_mode), done_flag or None, epoch, completion_flag or None,
                                                    completion_value, stream)
+
+
+def paged_repage(src: PermuteSide, src_page_size: int, dst: PermuteSide, dst_page_size: int, token_begin: int, token_end: int,
+                 layer_begin: int, layer_end: int, num_heads: int, src_row_bytes: int, cast_mode: int = 0, cast_scales=None,
+                 done_flag: int = 0, epoch: int = 0, completion_flag: int = 0, completion_value: int = 0, stream: int = 0) -> int:
+    """Tokens [token_begin, token_end) of one sequence between two block tables with different page sizes (one divides the other):
+    src.block_ids = src_table[token_begin // Ps .. ceil(token_end / Ps)), dst.block_ids likewise for Pd; re-ordered between the
+    formats and cast as `paged_permute_heads` would; every other destination byte keeps its value.  include/kvbm_kernels.h
+    (kvbm_kernels_paged_repage)."""
+    return lib().kvbm_kernels_paged_repage(C.byref(src), src_page_size, C.byref(dst), dst_page_size, token_begin, token_end, layer_begin,
+                                           layer_end, num_heads, src_row_bytes, int(cast_mode), scales_ptr(cast_scales), done_flag or None,
+                                           epoch, completion_flag or None, completion_value, stream)
 
 
 def permute_strides(kv_layout: int, num_layers: int, outer_dim: int, num_heads: int, page_size: int, row_bytes: int,

@@ -230,7 +230,7 @@ EXPORTED_SYMBOLS = [
     "kvbm_select_direct_strategy_remote", "kvbm_select_strategy", "kvbm_manager_select_strategy",
     "kvbm_mc_supported", "kvbm_mc_group_create", "kvbm_mc_group_export_fd", "kvbm_mc_group_import_fd",
     "kvbm_mc_group_size", "kvbm_mc_group_add_device", "kvbm_mc_group_bind_local", "kvbm_mc_group_bind_addr", "kvbm_mc_group_map",
-    "kvbm_mc_group_destroy", "kvbm_tp_reshard_plan", "kvbm_manager_execute_gather",
+    "kvbm_mc_group_destroy", "kvbm_tp_reshard_plan", "kvbm_manager_execute_gather", "kvbm_manager_execute_repage",
 ]
 
 
@@ -279,6 +279,7 @@ def lib() -> C.CDLL:
         L.kvbm_kv_layout_requires_transform.argtypes = [i, i]
         L.kvbm_tp_reshard_plan.argtypes = [sz, sz, sz, sz, P(_CHeadWindow), sz, P(sz)]
         L.kvbm_manager_execute_gather.argtypes = [vp, sz, P(u64), P(P(sz)), u64, vp, sz, P(_CHeadWindow), sz, P(_COptions), P(u64)]
+        L.kvbm_manager_execute_repage.argtypes = [vp, u64, vp, sz, u64, vp, sz, sz, sz, P(_COptions), P(u64)]
         L.kvbm_notification_is_complete.argtypes = [vp, u64]
         L.kvbm_notification_wait.argtypes = [vp, u64, C.c_int64]
         L.kvbm_manager_bytes_moved.argtypes = [vp]
@@ -616,6 +617,25 @@ class TransferManager:
         o = (options or TransferOptions())._c()
         _check(lib().kvbm_manager_execute_gather(self._h, len(ranks), hs, sp, dst, d.addr if type(d) is _NpView else d, n, ws, len(plan),
                                                  C.byref(o), C.byref(tok)))
+        return TransferCompleteNotification(self, tok.value)
+
+    def execute_repage(self, src: int, src_block_ids: Sequence[int], dst: int, dst_block_ids: Sequence[int], tokens: range,
+                       options: Optional[TransferOptions] = None) -> TransferCompleteNotification:
+        """Move tokens `tokens` (a step-1 range of sequence positions) between two layouts with different page sizes (one divides
+        the other), re-ordering formats and casting as `execute_transfer` would (kvbm_manager_execute_repage).  `src_block_ids` is
+        the source table's entries tokens.start // Ps .. ceil(tokens.stop / Ps), `dst_block_ids` the destination's for Pd; every
+        destination byte outside the range keeps its value, so a prefix the decode side already holds, or a partial last block,
+        is left alone.  Options: layer_range, cast_mode, cast_scales, src_kv_layout / dst_kv_layout, done_flag / epoch and
+        cuda_stream; the others are rejected."""
+        if tokens.step != 1:
+            raise ValueError("tokens must be a range with step 1")
+        s, ns = _size_array(src_block_ids)
+        d, nd = _size_array(dst_block_ids)
+        tok = C.c_uint64()
+        o = (options or TransferOptions())._c()
+        _check(lib().kvbm_manager_execute_repage(self._h, src, s.addr if type(s) is _NpView else s, ns, dst,
+                                                 d.addr if type(d) is _NpView else d, nd, tokens.start, tokens.stop, C.byref(o),
+                                                 C.byref(tok)))
         return TransferCompleteNotification(self, tok.value)
 
     def execute_fanout(self, src: int, dsts: Sequence[int], src_block_ids: Sequence[Sequence[int]],

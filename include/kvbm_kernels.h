@@ -287,6 +287,24 @@ cudaError_t kvbm_kernels_paged_permute_gather_scaled(const kvbm_permute_source* 
                                                      uint32_t* done_flag, uint32_t epoch, uint32_t* completion_flag,
                                                      uint32_t completion_value, cudaStream_t stream);
 
+/* Re-paging: tokens [token_begin, token_end) of one sequence between two block tables with different page sizes (a prefill
+ * engine's pages to a decode engine's), re-ordered from src->kv_layout to dst->kv_layout and cast as cast_mode says (bits
+ * identical to kvbm_kernels_paged_permute_heads_scaled; cast_scales as there, indexed by the absolute layer and outer index).
+ * Sequence token p sits in slot p % P of block table[p / P] on a side whose page is P, so src->block_ids holds
+ * src_table[token_begin / Ps .. ceil(token_end / Ps)) and dst->block_ids dst_table[token_begin / Pd .. ceil(token_end / Pd)).
+ * Every layer of [layer_begin, layer_end), outer index and head of each token in the range moves; every other destination byte
+ * keeps its value, including the slots of the first and last destination blocks outside the range.  One page size must
+ * divide the other (equal sizes are a token-range copy); both must be non-zero.  Each side's region_bytes must be its page *
+ * num_heads * its row, both sides share num_layers and outer_dim, both formats must be named (KVBM_KV_* 1..4), the row, cast
+ * and stride rules are kvbm_kernels_paged_permute_cast's, and the range's last block of the larger page must end below 2^32
+ * tokens.  Anything else is cudaErrorInvalidValue, returned before any CUDA call.  An empty token or layer range moves nothing
+ * and still signals; done_flag / completion_flag are written as kvbm_kernels_paged_permute_cast writes them. */
+cudaError_t kvbm_kernels_paged_repage(const kvbm_permute_side* src, uint32_t src_page_size, const kvbm_permute_side* dst,
+                                      uint32_t dst_page_size, uint32_t token_begin, uint32_t token_end, int layer_begin,
+                                      int layer_end, uint32_t num_heads, uint32_t src_row_bytes, int cast_mode,
+                                      const float* cast_scales, uint32_t* done_flag, uint32_t epoch, uint32_t* completion_flag,
+                                      uint32_t completion_value, cudaStream_t stream);
+
 /* Host-only (no GPU): the stride table kvbm_kernels_paged_permute walks with for one side.  out[0] = 1 when offsets count
  * from the block's first byte (universal formats) or 0 when they count from the (layer, outer) region's first byte; the
  * element (layer l, outer o, head h, token t) then sits at  [out[0] ? l * out[1] + o * out[2] : 0] + h * out[3] + t * out[4].

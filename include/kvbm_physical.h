@@ -285,6 +285,28 @@ int kvbm_manager_execute_gather(kvbm_transfer_manager* m, size_t num_srcs, const
                                 const kvbm_head_window* windows, size_t num_windows, const kvbm_transfer_options* opts,
                                 kvbm_notification* out);
 
+/* Re-paging hand-off between engines with different page sizes, over any token range: tokens [token_begin, token_end) of one
+ * sequence move from src's block table to dst's, each layout with its own page_size (one must divide the other; equal sizes are
+ * a token-range copy).  Token p sits in slot p % P of block table[p / P] on a side of page P, so src_ids holds
+ * src_table[token_begin / Ps .. ceil(token_end / Ps)) (n_src ids) and dst_ids dst_table[token_begin / Pd .. ceil(token_end / Pd))
+ * (n_dst ids).  Every layer of the options' layer range, outer index and head of those tokens is re-ordered between the two
+ * formats and cast as opts->cast_mode / cast_scales say; every other destination byte keeps its value, including the slots
+ * of the first and last destination blocks outside the range.  Honoured options: the layer range, cast_mode, cast_scales /
+ * num_cast_scales, src_kv_layout / dst_kv_layout, done_flag / epoch and the caller stream.  Errors, first one wins:
+ * KVBM_ERR_HANDLE unknown handle; KVBM_ERR_UNSUPPORTED an unmapped host descriptor, both sides remote, a head window, layer
+ * streaming / per-destination flags / multicast / a bounce buffer in the options, or a format that is not named (1..4);
+ * KVBM_ERR_CONFIG num_heads missing or not dividing inner_dim; KVBM_ERR_INCOMPATIBLE layer count, outer dim, head row, cast
+ * dtype, num_heads or dtype mismatch, pages that do not divide, and the permuting path's row, contiguity and alignment rules
+ * (KVBM_ERR_UNSUPPORTED for rows and alignment, as execute_transfer); KVBM_ERR_RANGE token_begin > token_end or token_end
+ * past 2^31, a layer range past num_layers, too few cast scales; KVBM_ERR_LENGTH_MISMATCH n_src / n_dst other than the counts
+ * the range implies; KVBM_ERR_DUPLICATE_DST / KVBM_ERR_OVERLAP / KVBM_ERR_RANGE for ids as kvbm_validate_block_transfer;
+ * an empty token or layer range then returns KVBM_OK with nothing launched; KVBM_ERR_UNSUPPORTED a strategy other than a
+ * direct CUDA one (Memcpy, two-hop, NIXL); KVBM_ERR_CUDA a host-only manager.  One upload of both id lists, one
+ * kvbm_kernels_paged_repage launch; bytes_moved counts tokens * layers * outer_dim * num_heads * the destination row. */
+int kvbm_manager_execute_repage(kvbm_transfer_manager* m, kvbm_layout_handle src, const size_t* src_ids, size_t n_src,
+                                kvbm_layout_handle dst, const size_t* dst_ids, size_t n_dst, size_t token_begin, size_t token_end,
+                                const kvbm_transfer_options* opts, kvbm_notification* out);
+
 /* Completion: the transfer's last warp writes a flag in pinned host memory (no cudaEventQuery polling). */
 int kvbm_notification_is_complete(kvbm_transfer_manager* m, kvbm_notification n);  /* 1 / 0 / <0 error */
 int kvbm_notification_wait(kvbm_transfer_manager* m, kvbm_notification n, int64_t timeout_us);
