@@ -5,7 +5,15 @@ flow (build the tables, upload them, launch, wait).  K1 cannot cast, so it runs 
 
 Llama-3-8B KV geometry (32 layers, K/V, 8 heads x 128, bf16) on vLLM-style layer-separate NHD pools with random block tables,
 plus MLA (one outer index, one 576-wide head).  One JSON line per arm with the card's name and power limit; sample destination
-blocks of every arm are compared with tests/repage_oracle.py."""
+blocks of every arm are compared with tests/repage_oracle.py.
+
+--reshard S:D times kvbm_kernels_paged_repage_gather instead: decode rank 0 of TP D (page Pd) assembling its heads from the ranks
+of TP S (page Ps) that hold them, over the whole sequence, in one launch.  Its arms, alternated within each of the --iters rounds
+and timed with CUDA events (median): the one launch; the two-pass workaround without it (kvbm_kernels_paged_repage per source
+into a staging pool with page Pd and the source's heads, then kvbm_kernels_paged_permute_gather out of the staging pools), timed
+whole; and the same-page gather of the same bytes from sources that already have page Pd (the rate to approach).  The pages
+default to 8:1 -> 1:16, 4:2 -> 64:16, 2:8 -> 16:64; --pages Ps:Pd overrides them.  Sample destination blocks of every arm are
+compared with tests/repage_gather_oracle.py."""
 import argparse
 import json
 import os
@@ -21,12 +29,16 @@ ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
 sys.path.insert(0, ROOT)
 from dynamo_b200 import kernels as K  # noqa: E402
 from tests.repage_oracle import repage, table_slice  # noqa: E402
+from tests.repage_gather_oracle import repage_gather  # noqa: E402
+from tests.reshard_oracle import reshard_plan  # noqa: E402
 
 p = argparse.ArgumentParser()
 p.add_argument("--tokens", type=int, default=4096)
 p.add_argument("--iters", type=int, default=20)
 p.add_argument("--cast", choices=["none", "fp8-to-bf16"], default="none")
 p.add_argument("--only", default=None, help="comma-separated config names to run")
+p.add_argument("--reshard", default=None, help="S:D -- time the re-paging gather from TP S to rank 0 of TP D")
+p.add_argument("--pages", default=None, help="Ps:Pd for --reshard (default: 8:1 1:16, 4:2 64:16, 2:8 16:64)")
 a = p.parse_args()
 CAST = K.CastMode.FP8E4M3_TO_BF16 if a.cast == "fp8-to-bf16" else K.CastMode.NONE
 SE, DE = (1, 2) if CAST else (2, 2)
@@ -185,8 +197,110 @@ def run(name, ps, pd, tb, te, no, nh, hd):
     return out
 
 
-for name, cfg in CONFIGS.items():
-    if a.only and name not in a.only.split(","):
-        continue
-    run(name, *cfg)
-    torch.cuda.empty_cache()
+def run_reshard(src_tp, dst_tp, ps, pd, H=8, hd=128, no=2):
+    """Decode rank 0 of TP dst_tp (page pd) from the TP src_tp ranks (page ps) that hold its heads: one launch, the two-pass
+    workaround and the same-page gather, alternated."""
+    name = f"tp{src_tp}_p{ps}_to_tp{dst_tp}_p{pd}"
+    plan = reshard_plan(H, src_tp, dst_tp, 0)             # (src_rank, src_head_begin, dst_head_begin, head_count)
+    ranks = sorted({w[0] for w in plan})
+    index = {r: i for i, r in enumerate(ranks)}
+    snh, dnh = max(1, H // src_tp), max(1, H // dst_tp)
+    covered = sum(w[3] for w in plan)
+    tb, te = 0, a.tokens
+    ns, nd = -(-te // ps), -(-te // pd)
+    rng = np.random.default_rng(0)
+    src = {r: Pool(ns + 8, ps, no, snh, hd, SE, 10 + r) for r in ranks}
+    stab = {r: rng.permutation(ns + 8)[:ns].tolist() for r in ranks}
+    dst = Pool(nd + 8, pd, no, dnh, hd, DE, 2)
+    dtab = rng.permutation(nd + 8)[:nd].tolist()
+    si = {r: torch.tensor(stab[r], dtype=torch.int32, device=dev) for r in ranks}
+    di = torch.tensor(dtab, dtype=torch.int32, device=dev)
+    s_row = hd * SE
+    moved = (te - tb) * NL * no * covered * hd * (SE + DE)    # bytes read + written
+    D = K.PermuteSide(dst.desc, di.data_ptr(), NHD)
+    srcs = [K.PermuteSource(K.PermuteSide(src[r].desc, si[r].data_ptr(), NHD), snh, sb, db, k) for r, sb, db, k in plan]
+
+    def one():
+        K.check(K.paged_repage_gather(srcs, ps, D, dnh, pd, tb, te, 0, NL, s_row, int(CAST), stream=sp), "paged_repage_gather")
+
+    # the workaround: each source re-paged into a staging pool of page pd with its own heads (the cast in this pass), then the
+    # gather out of the staging pools; staging block i is destination block i
+    stage = {r: Pool(nd, pd, no, snh, hd, DE, 20 + r) for r in ranks}
+    ident = torch.arange(nd, dtype=torch.int32, device=dev)
+    st_src = {r: K.PermuteSide(stage[r].desc, ident.data_ptr(), NHD) for r in ranks}
+    st_gather = [K.PermuteSource(st_src[r], snh, sb, db, k) for r, sb, db, k in plan]
+
+    def two_pass():
+        for r in ranks:
+            K.check(K.paged_repage(K.PermuteSide(src[r].desc, si[r].data_ptr(), NHD), ps, st_src[r], pd, tb, te, 0, NL, snh, s_row, int(CAST),
+                                   stream=sp), "paged_repage")
+        K.check(K.paged_permute_gather(st_gather, D, dnh, nd, 0, NL, pd, hd * DE, stream=sp), "paged_permute_gather")
+
+    # the same bytes with equal pages: sources that already have page pd
+    eq = {r: Pool(nd + 8, pd, no, snh, hd, SE, 30 + r) for r in ranks}
+    etab = {r: rng.permutation(nd + 8)[:nd].tolist() for r in ranks}
+    ei = {r: torch.tensor(etab[r], dtype=torch.int32, device=dev) for r in ranks}
+    eq_dst = Pool(nd + 8, pd, no, dnh, hd, DE, 5)
+    edi = torch.tensor(rng.permutation(nd + 8)[:nd].tolist(), dtype=torch.int32, device=dev)
+    ED = K.PermuteSide(eq_dst.desc, edi.data_ptr(), NHD)
+    eq_srcs = [K.PermuteSource(K.PermuteSide(eq[r].desc, ei[r].data_ptr(), NHD), snh, sb, db, k) for r, sb, db, k in plan]
+
+    def same_page():
+        K.check(K.paged_permute_gather(eq_srcs, ED, dnh, nd, 0, NL, pd, s_row, int(CAST), stream=sp), "paged_permute_gather")
+
+    sample = sorted({0, nd // 2, nd - 1})
+    windows = [(index[r], sb, db, k) for r, sb, db, k in plan]
+
+    def host_blocks(pool, ids):    # one download per layer, then the blocks' regions in (layer, outer) order
+        h = [t.cpu().numpy() for t in pool.layers]
+        return [np.concatenate([h[l][o * pool.nb * pool.region + b * pool.region:][:pool.region] for l in range(NL) for o in range(pool.no)])
+                for b in ids]
+
+    def check(arm, pool, tables, page, d_pool, d_ids):
+        torch.cuda.synchronize()
+        for j in sample:            # every covered head of every token is overwritten: the old bytes do not show through
+            lo, hi = j * pd, (j + 1) * pd
+            sources = [(host_blocks(pool[r], table_slice(tables[r], lo, hi, page)), NHD, snh) for r in ranks]
+            got = host_blocks(d_pool, [d_ids[j]])
+            want = repage_gather(sources, windows, got, NHD, dnh, NL, no, page, pd, s_row, lo, hi, int(CAST))[0]
+            assert np.array_equal(got[0], want), (name, arm, j)
+
+    arms = {"repage_gather": one, "two_pass": two_pass, "same_page_gather": same_page}
+    for fn in arms.values():
+        for _ in range(3):
+            fn()
+    check("repage_gather", src, stab, ps, dst, dtab)
+    two_pass()
+    check("two_pass", src, stab, ps, dst, dtab)
+    check("same_page_gather", eq, etab, pd, eq_dst, edi.tolist())
+    times = {k: [] for k in arms}
+    for _ in range(a.iters):           # the arms alternate within every round
+        for k, fn in arms.items():
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record(stream)
+            fn()
+            e1.record(stream)
+            e1.synchronize()
+            times[k].append(e0.elapsed_time(e1))
+    info = card()
+    ref = statistics.median(times["same_page_gather"])
+    for k in arms:
+        ms = statistics.median(times[k])
+        print(json.dumps({"config": name, "arm": k, "src_tp": src_tp, "dst_tp": dst_tp, "src_page": ps, "dst_page": pd, "sources": len(ranks),
+                          "tokens": te - tb, "layers": NL, "outer": no, "covered_heads": covered, "head_dim": hd, "cast": a.cast,
+                          "ms": round(ms, 4), "GBps": round(moved / ms / 1e6, 1), "vs_same_page": round(ref / ms, 3),
+                          "timed_as": "all launches of the arm, CUDA events, median of %d alternated rounds" % a.iters, "card": info}),
+              flush=True)
+
+
+if a.reshard:
+    s_tp, d_tp = (int(x) for x in a.reshard.split(":"))
+    default_pages = {(8, 1): (1, 16), (4, 2): (64, 16), (2, 8): (16, 64)}
+    pages = tuple(int(x) for x in a.pages.split(":")) if a.pages else default_pages[(s_tp, d_tp)]
+    run_reshard(s_tp, d_tp, *pages)
+else:
+    for name, cfg in CONFIGS.items():
+        if a.only and name not in a.only.split(","):
+            continue
+        run(name, *cfg)
+        torch.cuda.empty_cache()

@@ -1031,16 +1031,11 @@ static int execute(kvbm_transfer_manager* m, kvbm_layout_handle src_h, int nd, c
   return KVBM_OK;
 }
 
-// A TP re-shard's assembly as one hand-off: every window is validated as the windowed execute_transfer of its (source,
-// destination) pair, then one kvbm_kernels_paged_permute_gather launch moves all of them and one signal launch writes the
-// done flag and the completion word after the last byte landed.
-static int execute_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, const size_t* const* src_ids,
-                          kvbm_layout_handle dst_h, const size_t* dst_ids, size_t n, const kvbm_head_window* windows, size_t nw,
-                          const kvbm_transfer_options* opts_in, kvbm_notification* out)
+// The windows of a gather, before any layout is looked up: at least one source and one window, none in the options, at most
+// KVBM_GATHER_MAX_SOURCES, each naming a source, with heads, on destination heads no other window writes.
+static int check_gather_windows(size_t num_srcs, const kvbm_layout_handle* srcs, const kvbm_head_window* windows, size_t nw,
+                                const kvbm_transfer_options& o)
 {
-  kvbm_transfer_options o{};
-  if (opts_in) o = *opts_in;
-  if (out) *out = 0;
   if (num_srcs == 0 || !srcs || !windows || nw == 0) return fail(KVBM_ERR, "a gather needs at least one source and one window");
   if (o.head_count) return fail(KVBM_ERR, "a gather takes its head windows from the windows argument: options.head_count must be 0");
   if (nw > KVBM_GATHER_MAX_SOURCES)
@@ -1055,6 +1050,20 @@ static int execute_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_
           windows[t].dst_head_begin < windows[j].dst_head_begin + windows[j].head_count)
         return fail(KVBM_ERR_OVERLAP, "windows " + std::to_string(t) + " and " + std::to_string(j) + " overlap in the destination");
   }
+  return KVBM_OK;
+}
+
+// A TP re-shard's assembly as one hand-off: every window is validated as the windowed execute_transfer of its (source,
+// destination) pair, then one kvbm_kernels_paged_permute_gather launch moves all of them and one signal launch writes the
+// done flag and the completion word after the last byte landed.
+static int execute_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, const size_t* const* src_ids,
+                          kvbm_layout_handle dst_h, const size_t* dst_ids, size_t n, const kvbm_head_window* windows, size_t nw,
+                          const kvbm_transfer_options* opts_in, kvbm_notification* out)
+{
+  kvbm_transfer_options o{};
+  if (opts_in) o = *opts_in;
+  if (out) *out = 0;
+  if (int rc = check_gather_windows(num_srcs, srcs, windows, nw, o)) return rc;
   if (n && (!src_ids || !dst_ids)) return fail(KVBM_ERR, "null block id list");
   std::lock_guard<std::mutex> lk(m->mu);
   Transfer e[KVBM_GATHER_MAX_SOURCES];
@@ -1078,6 +1087,83 @@ static int execute_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_
 // Blocks a token range [tb, te) touches on a side with pages of `page` tokens: table[tb / page .. ceil(te / page)).
 static size_t repage_blocks(size_t tb, size_t te, size_t page) { return tb == te ? 0 : (te + page - 1) / page - tb / page; }
 
+// The checks of one re-paging (source, destination) pair, in execute_repage's order: both layouts addressable and not both remote,
+// the options re-paging takes, named formats (the options override a layout's own; filled into *src_kv / *dst_kv), head counts
+// known and dividing inner_dim, check_compat's head row and cast dtypes, equal num_heads (unless `windows`: a gather's head
+// windows pick the heads, so the counts may differ) and dtypes, pages that divide and the walk's rules.
+static int check_repage_pair(const Layout& S, const Layout& D, const kvbm_transfer_options& o, bool windows, int* src_kv, int* dst_kv)
+{
+  if (S.unmapped || D.unmapped)
+    return fail(KVBM_ERR_UNSUPPORTED, "a re-paging transfer needs both layouts addressable from this process (one is a descriptor of another process's host memory)");
+  if (S.remote && D.remote) return fail(KVBM_ERR_UNSUPPORTED, "Both src and dst are remote - this is not supported.");
+  if (o.head_count || o.layer_ready_flags || o.layer_done_flags || o.per_dst_done_flags || o.per_dst_layer_done_flags || o.multicast ||
+      o.bounce_layout || o.bounce_block_ids || o.num_bounce_blocks)
+    return fail(KVBM_ERR_UNSUPPORTED, "a re-paging transfer takes no head window, layer streaming, per-destination flags, multicast or bounce buffer");
+  const int skv = *src_kv = o.src_kv_layout ? o.src_kv_layout : S.kv_block_layout;
+  const int dkv = *dst_kv = o.dst_kv_layout ? o.dst_kv_layout : D.kv_block_layout;
+  if (skv < KVBM_KV_UNIVERSAL_TP || skv > KVBM_KV_OPERATIONAL_NHD || dkv < KVBM_KV_UNIVERSAL_TP || dkv > KVBM_KV_OPERATIONAL_NHD)
+    return fail(KVBM_ERR_UNSUPPORTED, std::string("re-paging needs named KV block layouts on both sides (the format decides where a token lives): src=") +
+                                          kv_name(skv) + ", dst=" + kv_name(dkv));
+  int rc;
+  if ((rc = need_num_heads(S.cfg)) || (rc = need_num_heads(D.cfg)) || (rc = need_divisible_heads(S.cfg)) || (rc = need_divisible_heads(D.cfg)))
+    return rc;
+  if ((rc = check_compat(S, D, o.cast_mode, true))) return rc;
+  const size_t ps = S.cfg.page_size, pd = D.cfg.page_size;
+  if ((!windows && S.cfg.num_heads != D.cfg.num_heads) || (o.cast_mode == KVBM_CAST_NONE && S.cfg.dtype_width_bytes != D.cfg.dtype_width_bytes))
+    return fail(KVBM_ERR_INCOMPATIBLE, "a re-paging transfer needs equal num_heads, head_dim and dtype on both sides");
+  if (ps % pd && pd % ps)
+    return fail(KVBM_ERR_INCOMPATIBLE, "re-paging needs one page size to divide the other: src=" + std::to_string(ps) + ", dst=" + std::to_string(pd));
+  return check_walk(S, D, skv, dkv, o.cast_mode);
+}
+
+// The ranges of a re-paging request against its source: the token range within 2^31 tokens, the options' layer range (filled
+// into *lb / *le) and enough cast scales.
+static int check_repage_ranges(const Layout& S, size_t tb, size_t te, const kvbm_transfer_options& o, size_t* lb, size_t* le)
+{
+  if (tb > te || te > (size_t{1} << 31))
+    return fail(KVBM_ERR_RANGE, "Token range " + std::to_string(tb) + ".." + std::to_string(te) + " is reversed or reaches past 2^31 tokens");
+  *lb = 0;
+  *le = S.cfg.num_layers;
+  if (o.has_layer_range) {
+    *lb = o.layer_begin;
+    *le = o.layer_end;
+    if (*lb > *le || *le > S.cfg.num_layers)
+      return fail(KVBM_ERR_RANGE, "Layer range " + std::to_string(*lb) + ".." + std::to_string(*le) + " exceeds num_layers " +
+                                      std::to_string(S.cfg.num_layers));
+  }
+  if (o.cast_scales) {
+    if (o.cast_mode == KVBM_CAST_NONE) return fail(KVBM_ERR, "cast_scales need a cast_mode: they scale the fp8 side of a cast");
+    const size_t need = S.cfg.num_layers * S.cfg.outer_dim;
+    if (o.num_cast_scales < need)
+      return fail(KVBM_ERR_RANGE, "cast_scales holds " + std::to_string(o.num_cast_scales) + " scales, the pools need num_layers * outer_dim = " +
+                                      std::to_string(need));
+  }
+  return KVBM_OK;
+}
+
+// The id counts a token range implies on either side of a re-paging request.
+static int check_repage_counts(size_t tb, size_t te, size_t ps, size_t pd, size_t n_src, size_t n_dst)
+{
+  const size_t want_src = repage_blocks(tb, te, ps), want_dst = repage_blocks(tb, te, pd);
+  if (n_src != want_src || n_dst != want_dst)
+    return fail(KVBM_ERR_LENGTH_MISMATCH, "tokens " + std::to_string(tb) + ".." + std::to_string(te) + " span " + std::to_string(want_src) +
+                                              " source and " + std::to_string(want_dst) + " destination blocks, got src=" + std::to_string(n_src) +
+                                              ", dst=" + std::to_string(n_dst));
+  return KVBM_OK;
+}
+
+// The strategy of a re-paging pair: a direct CUDA one, as select_direct_strategy and resolve()'s peer rule give it.
+static int repage_strategy(kvbm_transfer_manager* m, const Layout& S, const Layout& D, kvbm_transfer_plan* p)
+{
+  *p = kvbm_transfer_plan{};
+  if (int rc = select_direct_strategy(S.storage, D.storage, &m->caps, p)) return rc;
+  const bool two_hop = p->two_hop || (p->first == KVBM_STRATEGY_CUDA_ASYNC_D2D && !m->caps.allow_gpu_rdma &&
+                                      (S.device_id != D.device_id || S.remote != D.remote));
+  if (two_hop || !cuda_strategy(p->first))
+    return fail(KVBM_ERR_UNSUPPORTED, "re-paging runs on a direct CUDA strategy only (not Memcpy, two-hop or NIXL plans)");
+  return KVBM_OK;
+}
+
 // Re-paging hand-off: tokens [tb, te) of one sequence from the source's block table to the destination's, each side with its own
 // page size, as one kvbm_kernels_paged_repage launch.  Validated on its own (execute() and resolve() assume one page size and
 // equal id counts), in the order below; a request that fails several checks reports the first.
@@ -1092,58 +1178,17 @@ static int execute_repage(kvbm_transfer_manager* m, kvbm_layout_handle src_h, co
   if (!S) return fail(KVBM_ERR_HANDLE, "invalid source handle");
   Layout* D = m->find(dst_h);
   if (!D) return fail(KVBM_ERR_HANDLE, "invalid destination handle");
-  if (S->unmapped || D->unmapped)
-    return fail(KVBM_ERR_UNSUPPORTED, "a re-paging transfer needs both layouts addressable from this process (one is a descriptor of another process's host memory)");
-  if (S->remote && D->remote) return fail(KVBM_ERR_UNSUPPORTED, "Both src and dst are remote - this is not supported.");
-  if (o.head_count || o.layer_ready_flags || o.layer_done_flags || o.per_dst_done_flags || o.per_dst_layer_done_flags || o.multicast ||
-      o.bounce_layout || o.bounce_block_ids || o.num_bounce_blocks)
-    return fail(KVBM_ERR_UNSUPPORTED, "a re-paging transfer takes no head window, layer streaming, per-destination flags, multicast or bounce buffer");
-  const int src_kv = o.src_kv_layout ? o.src_kv_layout : S->kv_block_layout;
-  const int dst_kv = o.dst_kv_layout ? o.dst_kv_layout : D->kv_block_layout;
-  if (src_kv < KVBM_KV_UNIVERSAL_TP || src_kv > KVBM_KV_OPERATIONAL_NHD || dst_kv < KVBM_KV_UNIVERSAL_TP || dst_kv > KVBM_KV_OPERATIONAL_NHD)
-    return fail(KVBM_ERR_UNSUPPORTED, std::string("re-paging needs named KV block layouts on both sides (the format decides where a token lives): src=") +
-                                          kv_name(src_kv) + ", dst=" + kv_name(dst_kv));
-  int rc;
-  if ((rc = need_num_heads(S->cfg)) || (rc = need_num_heads(D->cfg)) || (rc = need_divisible_heads(S->cfg)) || (rc = need_divisible_heads(D->cfg)))
-    return rc;
-  if ((rc = check_compat(*S, *D, o.cast_mode, true))) return rc;
+  int src_kv, dst_kv, rc;
+  size_t lb, le;
+  if ((rc = check_repage_pair(*S, *D, o, false, &src_kv, &dst_kv))) return rc;
+  if ((rc = check_repage_ranges(*S, tb, te, o, &lb, &le))) return rc;
   const size_t ps = S->cfg.page_size, pd = D->cfg.page_size;
-  if (S->cfg.num_heads != D->cfg.num_heads || (o.cast_mode == KVBM_CAST_NONE && S->cfg.dtype_width_bytes != D->cfg.dtype_width_bytes))
-    return fail(KVBM_ERR_INCOMPATIBLE, "a re-paging transfer needs equal num_heads, head_dim and dtype on both sides");
-  if (ps % pd && pd % ps)
-    return fail(KVBM_ERR_INCOMPATIBLE, "re-paging needs one page size to divide the other: src=" + std::to_string(ps) + ", dst=" + std::to_string(pd));
-  if ((rc = check_walk(*S, *D, src_kv, dst_kv, o.cast_mode))) return rc;
-  if (tb > te || te > (size_t{1} << 31))
-    return fail(KVBM_ERR_RANGE, "Token range " + std::to_string(tb) + ".." + std::to_string(te) + " is reversed or reaches past 2^31 tokens");
-  size_t lb = 0, le = S->cfg.num_layers;
-  if (o.has_layer_range) {
-    lb = o.layer_begin;
-    le = o.layer_end;
-    if (lb > le || le > S->cfg.num_layers)
-      return fail(KVBM_ERR_RANGE, "Layer range " + std::to_string(lb) + ".." + std::to_string(le) + " exceeds num_layers " +
-                                      std::to_string(S->cfg.num_layers));
-  }
-  if (o.cast_scales) {
-    if (o.cast_mode == KVBM_CAST_NONE) return fail(KVBM_ERR, "cast_scales need a cast_mode: they scale the fp8 side of a cast");
-    const size_t need = S->cfg.num_layers * S->cfg.outer_dim;
-    if (o.num_cast_scales < need)
-      return fail(KVBM_ERR_RANGE, "cast_scales holds " + std::to_string(o.num_cast_scales) + " scales, the pools need num_layers * outer_dim = " +
-                                      std::to_string(need));
-  }
-  const size_t want_src = repage_blocks(tb, te, ps), want_dst = repage_blocks(tb, te, pd);
-  if (n_src != want_src || n_dst != want_dst)
-    return fail(KVBM_ERR_LENGTH_MISMATCH, "tokens " + std::to_string(tb) + ".." + std::to_string(te) + " span " + std::to_string(want_src) +
-                                              " source and " + std::to_string(want_dst) + " destination blocks, got src=" + std::to_string(n_src) +
-                                              ", dst=" + std::to_string(n_dst));
+  if ((rc = check_repage_counts(tb, te, ps, pd, n_src, n_dst))) return rc;
   if ((n_src && !src_ids) || (n_dst && !dst_ids)) return fail(KVBM_ERR, "null block id list");
   if ((rc = check_block_ids(src_ids, n_src, dst_ids, n_dst, S->cfg.num_blocks, D->cfg.num_blocks, src_h == dst_h))) return rc;
   if (tb == te || lb == le) return KVBM_OK;  // nothing to move, as execute()
-  kvbm_transfer_plan p{};
-  if ((rc = select_direct_strategy(S->storage, D->storage, &m->caps, &p))) return rc;
-  const bool two_hop = p.two_hop || (p.first == KVBM_STRATEGY_CUDA_ASYNC_D2D && !m->caps.allow_gpu_rdma &&
-                                     (S->device_id != D->device_id || S->remote != D->remote));
-  if (two_hop || !cuda_strategy(p.first))
-    return fail(KVBM_ERR_UNSUPPORTED, "re-paging runs on a direct CUDA strategy only (not Memcpy, two-hop or NIXL plans)");
+  kvbm_transfer_plan p;
+  if ((rc = repage_strategy(m, *S, *D, &p))) return rc;
   if ((rc = need_cuda_device(m))) return rc;
   if (o.cast_scales && (rc = check_cast_scales(m, o.cast_scales))) return rc;
 
@@ -1163,6 +1208,83 @@ static int execute_repage(kvbm_transfer_manager* m, kvbm_layout_handle src_h, co
   if (ce != cudaSuccess) return fail_cuda(ce, "kvbm_kernels_paged_repage");
   const size_t d_row = D->cfg.inner_dim / D->cfg.num_heads * D->cfg.dtype_width_bytes;
   if ((rc = finish_slot(m, sl, stream, (te - tb) * (le - lb) * S->cfg.outer_dim * nh * d_row))) return rc;
+  if (out) *out = o.use_caller_stream ? 0 : seq;
+  return KVBM_OK;
+}
+
+// A TP re-shard's assembly across engines with different page sizes: execute_gather's windows over execute_repage's token range.
+// The windows are checked as execute_gather checks them; the source of every window is then checked against the destination as
+// execute_repage checks its pair (the head counts may differ), with its head window and with one page size for every source.
+// One upload of every source's ids and the destination's, one kvbm_kernels_paged_repage_gather launch and one notification.
+static int execute_repage_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, const size_t* const* src_ids,
+                                 size_t n_src, kvbm_layout_handle dst_h, const size_t* dst_ids, size_t n_dst, size_t tb, size_t te,
+                                 const kvbm_head_window* windows, size_t nw, const kvbm_transfer_options* opts_in, kvbm_notification* out)
+{
+  kvbm_transfer_options o{};
+  if (opts_in) o = *opts_in;
+  if (out) *out = 0;
+  if (int rc = check_gather_windows(num_srcs, srcs, windows, nw, o)) return rc;
+  std::lock_guard<std::mutex> lk(m->mu);
+  Layout* D = m->find(dst_h);
+  if (!D) return fail(KVBM_ERR_HANDLE, "invalid destination handle");
+  Layout* S[KVBM_GATHER_MAX_SOURCES];
+  int src_kv[KVBM_GATHER_MAX_SOURCES], dst_kv = KVBM_KV_UNKNOWN, rc;
+  size_t heads = 0;
+  for (size_t j = 0; j < nw; ++j) {
+    const kvbm_head_window& w = windows[j];
+    if (!(S[j] = m->find(srcs[w.src_rank]))) return fail(KVBM_ERR_HANDLE, "invalid source handle");
+    if ((rc = check_repage_pair(*S[j], *D, o, true, &src_kv[j], &dst_kv)) || (rc = check_head_window(*S[j], *D, w, 1))) return rc;
+    if (S[j]->cfg.page_size != S[0]->cfg.page_size)
+      return fail(KVBM_ERR_INCOMPATIBLE, "the sources of a re-paging gather need one page size: source " + std::to_string(windows[0].src_rank) +
+                                             " has " + std::to_string(S[0]->cfg.page_size) + ", source " + std::to_string(w.src_rank) +
+                                             " has " + std::to_string(S[j]->cfg.page_size));
+    heads += w.head_count;
+  }
+  size_t lb, le;
+  if ((rc = check_repage_ranges(*S[0], tb, te, o, &lb, &le))) return rc;
+  const size_t ps = S[0]->cfg.page_size, pd = D->cfg.page_size;
+  if ((rc = check_repage_counts(tb, te, ps, pd, n_src, n_dst))) return rc;
+  if ((n_src && !src_ids) || (n_dst && !dst_ids)) return fail(KVBM_ERR, "null block id list");
+  for (size_t j = 0; j < nw; ++j) {
+    const size_t* s = n_src ? src_ids[windows[j].src_rank] : nullptr;
+    if (n_src && !s) return fail(KVBM_ERR, "null block id list");
+    if ((rc = check_block_ids(s, n_src, dst_ids, n_dst, S[j]->cfg.num_blocks, D->cfg.num_blocks, srcs[windows[j].src_rank] == dst_h))) return rc;
+  }
+  if (tb == te || lb == le) return KVBM_OK;  // nothing to move, as execute_repage
+  kvbm_transfer_plan p, p0{};
+  for (size_t j = 0; j < nw; ++j) {
+    if ((rc = repage_strategy(m, *S[j], *D, &p))) return rc;
+    if (j && p.first != p0.first) return fail(KVBM_ERR_UNSUPPORTED, "the sources of a gather need the same CUDA strategy");
+    p0 = p;
+  }
+  if ((rc = need_cuda_device(m))) return rc;
+  if (o.cast_scales && (rc = check_cast_scales(m, o.cast_scales))) return rc;
+
+  DeviceGuard g(m->device);
+  const cudaStream_t stream = pick_stream(m, p0.first, o);
+  std::vector<const size_t*> lists(src_ids, src_ids + num_srcs);
+  lists.push_back(dst_ids);
+  std::vector<size_t> lens(num_srcs, n_src);
+  lens.push_back(n_dst);
+  Slot* sl;
+  uint64_t seq;
+  if ((rc = stage_ids(m, lists.data(), lens.data(), lists.size(), 4, stream, nullptr, &sl, &seq))) return rc;
+  const kvbm_permute_side kd{descriptor(*D), sl->dev_ids + num_srcs * n_src, dst_kv};
+  kvbm_permute_source ks[KVBM_GATHER_MAX_SOURCES] = {};
+  for (size_t j = 0; j < nw; ++j) {
+    const kvbm_head_window& w = windows[j];
+    ks[j] = kvbm_permute_source{{descriptor(*S[j]), sl->dev_ids + w.src_rank * n_src, src_kv[j]}, static_cast<uint32_t>(S[j]->cfg.num_heads),
+                                static_cast<uint32_t>(w.src_head_begin), static_cast<uint32_t>(w.dst_head_begin),
+                                static_cast<uint32_t>(w.head_count)};
+  }
+  const size_t row = S[0]->cfg.inner_dim / S[0]->cfg.num_heads * S[0]->cfg.dtype_width_bytes;
+  cudaError_t ce = kvbm_kernels_paged_repage_gather(ks, static_cast<int>(nw), static_cast<uint32_t>(ps), &kd, static_cast<uint32_t>(D->cfg.num_heads),
+                                                    static_cast<uint32_t>(pd), static_cast<uint32_t>(tb), static_cast<uint32_t>(te),
+                                                    static_cast<int>(lb), static_cast<int>(le), static_cast<uint32_t>(row), o.cast_mode,
+                                                    o.cast_scales, o.done_flag, o.epoch, sl->host_flag, static_cast<uint32_t>(seq), stream);
+  if (ce != cudaSuccess) return fail_cuda(ce, "kvbm_kernels_paged_repage_gather");
+  const size_t d_row = D->cfg.inner_dim / D->cfg.num_heads * D->cfg.dtype_width_bytes;
+  if ((rc = finish_slot(m, sl, stream, (te - tb) * (le - lb) * D->cfg.outer_dim * heads * d_row))) return rc;
   if (out) *out = o.use_caller_stream ? 0 : seq;
   return KVBM_OK;
 }
@@ -1665,6 +1787,17 @@ extern "C" int kvbm_manager_execute_repage(kvbm_transfer_manager* m, kvbm_layout
   return guarded([&]() -> int {
   if (!m) return fail(KVBM_ERR, "null manager");
   return execute_repage(m, src, src_ids, n_src, dst, dst_ids, n_dst, token_begin, token_end, opts, out);
+  });
+}
+
+extern "C" int kvbm_manager_execute_repage_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs,
+                                                  const size_t* const* src_ids, size_t n_src, kvbm_layout_handle dst, const size_t* dst_ids,
+                                                  size_t n_dst, size_t token_begin, size_t token_end, const kvbm_head_window* windows,
+                                                  size_t num_windows, const kvbm_transfer_options* opts, kvbm_notification* out)
+{
+  return guarded([&]() -> int {
+  if (!m) return fail(KVBM_ERR, "null manager");
+  return execute_repage_gather(m, num_srcs, srcs, src_ids, n_src, dst, dst_ids, n_dst, token_begin, token_end, windows, num_windows, opts, out);
   });
 }
 

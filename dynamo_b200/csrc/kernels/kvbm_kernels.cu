@@ -669,8 +669,7 @@ kvbm_paged_gather_kernel(const __grid_constant__ GatherParams P, uint32_t layer_
 // (token t of the unit, 16 B column c) by the row split; the token's slot in the big block is q = q0 + t, its small block and
 // slot come from q by the page split (a shift and a mask, or a multiply-high exact for q < 2^32 / small_page).  The walk runs
 // over all the unit's tokens, so one-token pages still keep 8 independent 16 B loads per lane in flight.
-struct RepageParams {
-  PermuteSide big, small;
+struct RepageGeom {
   RowSplit page;          // q -> (small block, slot): log2 / magic of the small page
   uint32_t small_page;
   uint32_t big_page;
@@ -681,6 +680,59 @@ struct RepageParams {
   uint32_t layer_begin, nlayers, no, nh;
   uint32_t src_small;     // 1: the source is the small side
 };
+struct RepageParams {
+  PermuteSide big, small;
+  RepageGeom g;
+};
+
+// One head of a re-paging unit: its run of `run` 16 B vectors from slot q0 of the big block on.  bh: the head's rows in the
+// big block; sh: its rows in the small side's (layer, outer) region, before the block offset.  Small block b of the unit is
+// entry small_k + b of small_ids; small_k wraps below 0 in the unit whose first small blocks lie before the range, and
+// small_k + b (b >= those blocks) wraps back: index in uint32, never offset the pointer by it.  kvbm_paged_repage_kernel keeps
+// its own copy of this loop: calling the helper from it changes the register allocation of all 20 of its instantiations.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__device__ __forceinline__ void repage_head_rows(const uint8_t* bh, uint32_t big_tok, uint32_t big_shift, const uint8_t* sh,
+                                                 const int32_t* small_ids, uint32_t small_k, uint64_t small_block_stride,
+                                                 uint32_t small_tok, uint32_t small_shift, const RepageGeom& G, uint32_t q0,
+                                                 uint32_t run, const RowSplit& r, const ptx::Scale& scale)
+{
+  constexpr int IN = CAST == KVBM_CAST_BF16_TO_FP8E4M3 ? 2 : 1;   // 16 B loads per vector
+  constexpr int OUT = CAST == KVBM_CAST_FP8E4M3_TO_BF16 ? 2 : 1;  // 16 B stores per vector
+  constexpr int U = 8 / IN;
+  const int lane = threadIdx.x & 31;
+  for (uint32_t v = lane; v < run; v += U * 32) {
+    uint4 x[U][IN];
+    uint8_t* dp[U];
+#pragma unroll
+    for (int k = 0; k < U; ++k)
+      if (v + k * 32 < run) {
+        const uint32_t vv = v + k * 32;
+        const uint32_t t = POW2 ? vv >> r.vpr : __umulhi(vv, r.magic);
+        const uint32_t c = POW2 ? vv & ((1u << r.vpr) - 1) : vv - t * r.vpr;
+        const uint32_t q = q0 + t;
+        const uint32_t b = PPOW2 ? q >> G.page.vpr : __umulhi(q, G.page.magic);
+        const uint32_t slot = PPOW2 ? q & (G.small_page - 1) : q - b * G.small_page;
+        const uint8_t* big_p = bh + q * big_tok + (c << big_shift);
+        const uint8_t* small_p = sh + static_cast<uint64_t>(__ldg(small_ids + (small_k + b))) * small_block_stride + slot * small_tok + (c << small_shift);
+        const uint8_t* s = G.src_small ? small_p : big_p;
+        dp[k] = const_cast<uint8_t*>(G.src_small ? big_p : small_p);
+#pragma unroll
+        for (int i = 0; i < IN; ++i) x[k][i] = ptx::ld_stream_v4(s + 16 * i);
+      }
+#pragma unroll
+    for (int k = 0; k < U; ++k)
+      if (v + k * 32 < run) {
+        if constexpr (CAST == KVBM_CAST_NONE) {
+          ptx::st_stream_v4(dp[k], x[k][0]);
+        } else {
+          uint4 y[OUT];
+          cast_vector<SCALED>(x[k], y, scale);  // bit for bit the paged permute's cast
+#pragma unroll
+          for (int i = 0; i < OUT; ++i) ptx::st_stream_v4(dp[k] + 16 * i, y[i]);
+        }
+      }
+  }
+}
 
 template <int CAST, bool POW2, bool SCALED, bool PPOW2>
 __global__ void __launch_bounds__(256)
@@ -690,26 +742,26 @@ kvbm_paged_repage_kernel(const __grid_constant__ RepageParams P, RowSplit r, con
   constexpr int OUT = CAST == KVBM_CAST_FP8E4M3_TO_BF16 ? 2 : 1;  // 16 B stores per vector
   constexpr int U = 8 / IN;
   const uint32_t unit = blockIdx.x;  // (big block j * nlayers + l) * no + o
-  const uint32_t j = unit / (P.nlayers * P.no);
-  const uint32_t rem = unit - j * (P.nlayers * P.no);
-  const uint32_t l = P.layer_begin + rem / P.no, o = rem % P.no;
-  const uint32_t first = (P.big_first + j) * P.big_page;  // sequence position of the big block's slot 0
-  const uint32_t t0 = max(P.token_begin, first), t1 = min(P.token_end, first + P.big_page);
+  const uint32_t j = unit / (P.g.nlayers * P.g.no);
+  const uint32_t rem = unit - j * (P.g.nlayers * P.g.no);
+  const uint32_t l = P.g.layer_begin + rem / P.g.no, o = rem % P.g.no;
+  const uint32_t first = (P.g.big_first + j) * P.g.big_page;  // sequence position of the big block's slot 0
+  const uint32_t t0 = max(P.g.token_begin, first), t1 = min(P.g.token_end, first + P.g.big_page);
   const uint32_t q0 = t0 - first;
   // small block b of this unit is entry small_k + b of the small table; small_k wraps below 0 in the unit whose first small
   // blocks lie before the range, and small_k + b (b >= those blocks) wraps back: index in uint32, never offset the pointer by it
-  const uint32_t small_k = (P.big_first + j) * P.ratio - P.small_first;
+  const uint32_t small_k = (P.g.big_first + j) * P.g.ratio - P.g.small_first;
   const uint8_t* big_base = reinterpret_cast<uint8_t*>(static_cast<uintptr_t>(__ldg(P.big.layer_base + (P.big.universal ? 0 : l)))) +
                             static_cast<uint64_t>(__ldg(P.big.ids + j)) * P.big.block_stride + l * P.big.layer_step + o * P.big.outer_step;
   const uint8_t* small_base = reinterpret_cast<uint8_t*>(static_cast<uintptr_t>(__ldg(P.small.layer_base + (P.small.universal ? 0 : l)))) +
                               l * P.small.layer_step + o * P.small.outer_step;
-  const ptx::Scale scale = ptx::make_scale(SCALED ? __ldg(scales + l * P.no + o) : 1.f);
+  const ptx::Scale scale = ptx::make_scale(SCALED ? __ldg(scales + l * P.g.no + o) : 1.f);
   // column shifts of either side: the source's vector is 16 * IN bytes, the destination's 16 * OUT
-  const uint32_t big_shift = P.src_small ? 3 + OUT : 3 + IN, small_shift = P.src_small ? 3 + IN : 3 + OUT;
+  const uint32_t big_shift = P.g.src_small ? 3 + OUT : 3 + IN, small_shift = P.g.src_small ? 3 + IN : 3 + OUT;
   const uint32_t big_tok = static_cast<uint32_t>(P.big.tok_stride), small_tok = static_cast<uint32_t>(P.small.tok_stride);
   const uint32_t run = row_run<POW2>(r, t1 - t0);
   const int lane = threadIdx.x & 31;
-  for (uint32_t h = threadIdx.x >> 5; h < P.nh; h += blockDim.x >> 5) {
+  for (uint32_t h = threadIdx.x >> 5; h < P.g.nh; h += blockDim.x >> 5) {
     const uint8_t* bh = big_base + h * P.big.head_stride;
     const uint8_t* sh = small_base + h * P.small.head_stride;
     for (uint32_t v = lane; v < run; v += U * 32) {
@@ -722,12 +774,12 @@ kvbm_paged_repage_kernel(const __grid_constant__ RepageParams P, RowSplit r, con
           const uint32_t t = POW2 ? vv >> r.vpr : __umulhi(vv, r.magic);
           const uint32_t c = POW2 ? vv & ((1u << r.vpr) - 1) : vv - t * r.vpr;
           const uint32_t q = q0 + t;
-          const uint32_t b = PPOW2 ? q >> P.page.vpr : __umulhi(q, P.page.magic);
-          const uint32_t slot = PPOW2 ? q & (P.small_page - 1) : q - b * P.small_page;
+          const uint32_t b = PPOW2 ? q >> P.g.page.vpr : __umulhi(q, P.g.page.magic);
+          const uint32_t slot = PPOW2 ? q & (P.g.small_page - 1) : q - b * P.g.small_page;
           const uint8_t* big_p = bh + q * big_tok + (c << big_shift);
           const uint8_t* small_p = sh + static_cast<uint64_t>(__ldg(P.small.ids + (small_k + b))) * P.small.block_stride + slot * small_tok + (c << small_shift);
-          const uint8_t* s = P.src_small ? small_p : big_p;
-          dp[k] = const_cast<uint8_t*>(P.src_small ? big_p : small_p);
+          const uint8_t* s = P.g.src_small ? small_p : big_p;
+          dp[k] = const_cast<uint8_t*>(P.g.src_small ? big_p : small_p);
 #pragma unroll
           for (int i = 0; i < IN; ++i) x[k][i] = ptx::ld_stream_v4(s + 16 * i);
         }
@@ -744,6 +796,57 @@ kvbm_paged_repage_kernel(const __grid_constant__ RepageParams P, RowSplit r, con
           }
         }
     }
+  }
+}
+
+// Re-paging and the gather in one launch: several sources with one page size Ps (a prefill TP group), each with its own pool,
+// format, head count and head window, into one destination of page Pd, over a token range.  The unit is the re-paging one: one
+// CTA per (block of the larger-page side, layer, outer), clipped to the range; the warps are the gather's: one per covered
+// destination head, looping by the CTA's warps past 8, each finding its source through the head map.  All sources share Ps and
+// the range, so big block j names the same sequence positions in every source: when the sources have the larger page each warp
+// reads block j of its own table; when the destination has it, a unit is one destination block and one CTA writes whole rows
+// of an OperationalNHD destination.  The small side's block comes per 16 B vector from the warp's own source table or the
+// destination's.  geo.nh: the covered heads.  SCALED: one scale array for every source, scales[l * no + o].
+struct RepageGatherParams {
+  GatherParams g;
+  RepageGeom geo;
+};
+
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__global__ void __launch_bounds__(256)
+kvbm_paged_repage_gather_kernel(const __grid_constant__ RepageGatherParams P, RowSplit r, const float* scales)
+{
+  constexpr int IN = CAST == KVBM_CAST_BF16_TO_FP8E4M3 ? 2 : 1;
+  constexpr int OUT = CAST == KVBM_CAST_FP8E4M3_TO_BF16 ? 2 : 1;
+  const RepageGeom& G = P.geo;
+  const PermuteSide& D = P.g.D;
+  const uint32_t unit = blockIdx.x;  // (big block j * nlayers + l) * no + o
+  const uint32_t j = unit / (G.nlayers * G.no);
+  const uint32_t rem = unit - j * (G.nlayers * G.no);
+  const uint32_t l = G.layer_begin + rem / G.no, o = rem % G.no;
+  const uint32_t first = (G.big_first + j) * G.big_page;
+  const uint32_t t0 = max(G.token_begin, first), t1 = min(G.token_end, first + G.big_page);
+  const uint32_t q0 = t0 - first;
+  const uint32_t small_k = (G.big_first + j) * G.ratio - G.small_first;
+  auto region = [&](const PermuteSide& X) {  // the (layer, outer) region of a side, before the block offset
+    return reinterpret_cast<const uint8_t*>(static_cast<uintptr_t>(__ldg(X.layer_base + (X.universal ? 0 : l)))) + l * X.layer_step +
+           o * X.outer_step;
+  };
+  const uint8_t* d_region = region(D);
+  const ptx::Scale scale = ptx::make_scale(SCALED ? __ldg(scales + l * G.no + o) : 1.f);
+  const uint32_t big_shift = G.src_small ? 3 + OUT : 3 + IN, small_shift = G.src_small ? 3 + IN : 3 + OUT;
+  const uint32_t run = row_run<POW2>(r, t1 - t0);
+  for (uint32_t k = threadIdx.x >> 5; k < P.g.covered; k += blockDim.x >> 5) {
+    const GatherSource& S = P.g.src[P.g.entry[k]];
+    const uint32_t h = k - S.first;  // head h of the window
+    const uint8_t* sh = region(S.S) + S.s_win + h * S.S.head_stride;
+    const uint8_t* dh = d_region + S.d_win + h * D.head_stride;
+    const bool ss = G.src_small;
+    const PermuteSide& B = ss ? D : S.S;
+    const PermuteSide& Sm = ss ? S.S : D;
+    const uint8_t* bh = (ss ? dh : sh) + static_cast<uint64_t>(__ldg(B.ids + j)) * B.block_stride;
+    repage_head_rows<CAST, POW2, SCALED, PPOW2>(bh, static_cast<uint32_t>(B.tok_stride), big_shift, ss ? sh : dh, Sm.ids, small_k,
+                                                Sm.block_stride, static_cast<uint32_t>(Sm.tok_stride), small_shift, G, q0, run, r, scale);
   }
 }
 
@@ -910,6 +1013,8 @@ static cudaError_t preload_kernels()
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_gather_kernel<c, p, sc>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_kernel<c, p, sc, true>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_kernel<c, p, sc, false>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_gather_kernel<c, p, sc, true>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_gather_kernel<c, p, sc, false>);
         });
   return e;
 }
@@ -943,6 +1048,67 @@ static cudaError_t set_smem(K kernel, uint32_t bytes)
   return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
 }
 
+// The launch checks every permuting and re-paging entry shares.  Before the empty-range signal: a cast mode the walk knows, and
+// scales only with a cast (they belong to the fp8 side of it).
+static bool cast_args_ok(int cast_mode, const float* cast_scales)
+{
+  if (cast_mode < KVBM_CAST_NONE || cast_mode > KVBM_CAST_BF16_TO_FP8E4M3) return false;
+  return !(cast_scales && cast_mode == KVBM_CAST_NONE);
+}
+
+// The signal launch after the work (or instead of it on an empty range): done_flag / completion_flag written once.
+static cudaError_t signal_launch(uint32_t* done_flag, uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
+{
+  if (!done_flag && !completion_flag) return cudaSuccess;
+  kvbm_signal_kernel<<<1, 1, 0, stream>>>(done_flag, epoch, completion_flag, completion_value);
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  return cudaGetLastError();
+}
+
+// The walk splits the fp8 side's row into 16 B vectors when casting (the bf16 side's vectors are 32 B), else the row; an odd
+// bf16 row has no fp8 row.  Fills the destination's row and the row the walk counts vectors of.
+static bool cast_rows(uint32_t src_row_bytes, int cast_mode, uint64_t* dst_row_bytes, uint64_t* walk_row)
+{
+  if (cast_mode == KVBM_CAST_BF16_TO_FP8E4M3 && (src_row_bytes & 1)) return false;
+  *dst_row_bytes = cast_mode == KVBM_CAST_FP8E4M3_TO_BF16   ? 2ull * src_row_bytes
+                   : cast_mode == KVBM_CAST_BF16_TO_FP8E4M3 ? src_row_bytes / 2
+                                                            : src_row_bytes;
+  *walk_row = cast_mode == KVBM_CAST_BF16_TO_FP8E4M3 ? *dst_row_bytes : src_row_bytes;
+  return true;
+}
+
+// The sources of a gather into P->D (dst_num_heads heads): each source's layers and outer dims those of the destination, its
+// window inside both sides' heads and on destination heads no other window writes (two would race), its region page * its
+// heads * row, its strides, and at most max_covered covered heads in all.  Fills P->src, P->covered and, with several sources,
+// the head map P->entry.
+static bool fill_gather_sources(const kvbm_permute_source* srcs, int num_srcs, uint32_t dst_num_heads, uint32_t nl, uint32_t no,
+                                uint32_t page_size, uint32_t src_row_bytes, uint32_t max_covered, GatherParams* P)
+{
+  uint32_t covered = 0;
+  for (int s = 0; s < num_srcs; ++s) {
+    const kvbm_permute_source& X = srcs[s];
+    if (!X.side.block_ids || !X.side.layout.layer_base || X.side.layout.num_layers != nl || X.side.layout.outer_dim != no) return false;
+    if (X.head_count == 0 || static_cast<uint64_t>(X.src_head_begin) + X.head_count > X.num_heads ||
+        static_cast<uint64_t>(X.dst_head_begin) + X.head_count > dst_num_heads)
+      return false;
+    for (int t = 0; t < s; ++t)
+      if (X.dst_head_begin < srcs[t].dst_head_begin + srcs[t].head_count && srcs[t].dst_head_begin < X.dst_head_begin + X.head_count)
+        return false;
+    if (static_cast<uint64_t>(page_size) * X.num_heads * src_row_bytes != X.side.layout.region_bytes) return false;
+    GatherSource& G = P->src[s];
+    if (!fill_permute_side(X.side, nl, no, X.num_heads, page_size, src_row_bytes, &G.S)) return false;
+    if (static_cast<uint64_t>(covered) + X.head_count > max_covered) return false;
+    G.s_win = X.src_head_begin * G.S.head_stride;  // the windows' first heads
+    G.d_win = X.dst_head_begin * P->D.head_stride;
+    G.first = covered;
+    if (num_srcs > 1)
+      for (uint32_t j = 0; j < X.head_count; ++j) P->entry[covered + j] = static_cast<uint8_t>(s);
+    covered += X.head_count;
+  }
+  P->covered = covered;
+  return true;
+}
+
 // Every permuting launch: a head transform is one source, a gather several.  Runs the checks of both entries once, signals
 // when there is nothing to move, and launches kvbm_paged_permute_kernel for one source (the faster of the two, DESIGN §4.2b) or
 // kvbm_paged_gather_kernel for several.  max_covered: how many destination heads the sources may cover together; at most
@@ -953,53 +1119,21 @@ static cudaError_t launch_paged_permute(const kvbm_permute_source* srcs, int num
                                         uint32_t* completion_flag, uint32_t completion_value, uint32_t max_covered, cudaStream_t stream)
 {
   if (num_blocks < 0 || layer_begin < 0 || layer_end < layer_begin) return cudaErrorInvalidValue;
-  if (cast_mode < KVBM_CAST_NONE || cast_mode > KVBM_CAST_BF16_TO_FP8E4M3) return cudaErrorInvalidValue;
-  if (cast_scales && cast_mode == KVBM_CAST_NONE) return cudaErrorInvalidValue;  // scales belong to the fp8 side of a cast
+  if (!cast_args_ok(cast_mode, cast_scales)) return cudaErrorInvalidValue;
   if (!srcs || num_srcs < 1 || num_srcs > KVBM_GATHER_MAX_SOURCES) return cudaErrorInvalidValue;
-  auto finish = [&]() -> cudaError_t {
-    if (!done_flag && !completion_flag) return cudaSuccess;
-    kvbm_signal_kernel<<<1, 1, 0, stream>>>(done_flag, epoch, completion_flag, completion_value);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    return cudaGetLastError();
-  };
-  if (num_blocks == 0 || layer_end == layer_begin) return finish();
+  if (num_blocks == 0 || layer_end == layer_begin) return signal_launch(done_flag, epoch, completion_flag, completion_value, stream);
   if (!dst || !dst->block_ids || !dst->layout.layer_base) return cudaErrorInvalidValue;
   const uint32_t nl = dst->layout.num_layers, no = dst->layout.outer_dim;
   if (nl == 0 || no == 0 || static_cast<uint32_t>(layer_end) > nl) return cudaErrorInvalidValue;
-  // The walk splits the fp8 side's row into 16 B vectors when casting (the bf16 side's vectors are 32 B), else the row.
-  if (cast_mode == KVBM_CAST_BF16_TO_FP8E4M3 && (src_row_bytes & 1)) return cudaErrorInvalidValue;
-  const uint64_t dst_row_bytes = cast_mode == KVBM_CAST_FP8E4M3_TO_BF16   ? 2ull * src_row_bytes
-                                 : cast_mode == KVBM_CAST_BF16_TO_FP8E4M3 ? src_row_bytes / 2
-                                                                          : src_row_bytes;
-  const uint64_t walk_row = cast_mode == KVBM_CAST_BF16_TO_FP8E4M3 ? dst_row_bytes : src_row_bytes;
+  uint64_t dst_row_bytes, walk_row;
+  if (!cast_rows(src_row_bytes, cast_mode, &dst_row_bytes, &walk_row)) return cudaErrorInvalidValue;
   RowSplit r;
   if (page_size == 0 || !row_split(walk_row, page_size, &r)) return cudaErrorInvalidValue;
   if (static_cast<uint64_t>(page_size) * dst_num_heads * dst_row_bytes != dst->layout.region_bytes) return cudaErrorInvalidValue;
   GatherParams P{};
   if (!fill_permute_side(*dst, nl, no, dst_num_heads, page_size, static_cast<uint32_t>(dst_row_bytes), &P.D)) return cudaErrorInvalidValue;
-  uint32_t covered = 0;
-  for (int s = 0; s < num_srcs; ++s) {
-    const kvbm_permute_source& X = srcs[s];
-    if (!X.side.block_ids || !X.side.layout.layer_base || X.side.layout.num_layers != nl || X.side.layout.outer_dim != no)
-      return cudaErrorInvalidValue;
-    if (X.head_count == 0 || static_cast<uint64_t>(X.src_head_begin) + X.head_count > X.num_heads ||
-        static_cast<uint64_t>(X.dst_head_begin) + X.head_count > dst_num_heads)
-      return cudaErrorInvalidValue;
-    for (int t = 0; t < s; ++t)  // two windows writing the same destination head would race
-      if (X.dst_head_begin < srcs[t].dst_head_begin + srcs[t].head_count && srcs[t].dst_head_begin < X.dst_head_begin + X.head_count)
-        return cudaErrorInvalidValue;
-    if (static_cast<uint64_t>(page_size) * X.num_heads * src_row_bytes != X.side.layout.region_bytes) return cudaErrorInvalidValue;
-    GatherSource& G = P.src[s];
-    if (!fill_permute_side(X.side, nl, no, X.num_heads, page_size, src_row_bytes, &G.S)) return cudaErrorInvalidValue;
-    if (static_cast<uint64_t>(covered) + X.head_count > max_covered) return cudaErrorInvalidValue;
-    G.s_win = X.src_head_begin * G.S.head_stride;  // the windows' first heads
-    G.d_win = X.dst_head_begin * P.D.head_stride;
-    G.first = covered;
-    if (num_srcs > 1)
-      for (uint32_t j = 0; j < X.head_count; ++j) P.entry[covered + j] = static_cast<uint8_t>(s);
-    covered += X.head_count;
-  }
-  P.covered = covered;
+  if (!fill_gather_sources(srcs, num_srcs, dst_num_heads, nl, no, page_size, src_row_bytes, max_covered, &P)) return cudaErrorInvalidValue;
+  const uint32_t covered = P.covered;
   const uint64_t units = static_cast<uint64_t>(num_blocks) * (layer_end - layer_begin) * no;
   if (units >= (1ull << 31)) return cudaErrorInvalidValue;
   const int threads = static_cast<int>(std::min<uint32_t>(8, covered)) * 32;
@@ -1015,7 +1149,49 @@ static cudaError_t launch_paged_permute(const kvbm_permute_source* srcs, int num
   g_launches.fetch_add(1, std::memory_order_relaxed);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
-  return finish();
+  return signal_launch(done_flag, epoch, completion_flag, completion_value, stream);
+}
+
+// The geometry every re-paging launch shares, and its checks: non-zero pages, one dividing the other, slot arithmetic in 32 bits
+// (every block of the larger page in the range ends below 2^32, and the page split is exact for q < big_page), the cast's rows
+// and the row split of the larger page, and fewer than 2^31 units.  Fills everything of *G but nh, the walk's row split, the
+// destination's row, the unit count and whether the small page is a power of two.
+static bool repage_geometry(uint32_t src_page, uint32_t dst_page, uint32_t token_begin, uint32_t token_end, int layer_begin, int layer_end,
+                            uint32_t no, uint32_t src_row_bytes, int cast_mode, RepageGeom* G, RowSplit* r, uint64_t* dst_row_bytes,
+                            uint64_t* units, bool* page_pow2)
+{
+  if (src_page == 0 || dst_page == 0) return false;
+  const bool src_small = src_page < dst_page;
+  const uint32_t big_page = src_small ? dst_page : src_page, small_page = src_small ? src_page : dst_page;
+  if (big_page % small_page) return false;
+  const uint64_t big_end = (static_cast<uint64_t>(token_end) + big_page - 1) / big_page * big_page;
+  if (big_end >= (1ull << 32) || static_cast<uint64_t>(big_page) * small_page >= (1ull << 32)) return false;
+  uint64_t walk_row;
+  if (!cast_rows(src_row_bytes, cast_mode, dst_row_bytes, &walk_row) || !row_split(walk_row, big_page, r)) return false;
+  RepageGeom g{};
+  g.small_page = small_page;
+  g.big_page = big_page;
+  g.ratio = big_page / small_page;
+  g.big_first = token_begin / big_page;
+  g.small_first = token_begin / small_page;
+  g.token_begin = token_begin;
+  g.token_end = token_end;
+  g.layer_begin = static_cast<uint32_t>(layer_begin);
+  g.nlayers = static_cast<uint32_t>(layer_end - layer_begin);
+  g.no = no;
+  g.src_small = src_small ? 1 : 0;
+  // the small page's split, in RowSplit's form: log2 of the page, or the page and ceil(2^32 / page)
+  *page_pow2 = (small_page & (small_page - 1)) == 0;
+  if (*page_pow2) {
+    while ((1u << g.page.vpr) < small_page) ++g.page.vpr;
+    g.page.pow2 = true;
+  } else {
+    g.page = {small_page, static_cast<uint32_t>(((1ull << 32) + small_page - 1) / small_page), false};
+  }
+  *units = (static_cast<uint64_t>(big_end / big_page) - g.big_first) * g.nlayers * no;
+  if (*units >= (1ull << 31)) return false;
+  *G = g;
+  return true;
 }
 
 // kvbm_kernels_paged_repage: every check before any CUDA call, the signal on an empty range, then one re-paging launch and the
@@ -1026,33 +1202,19 @@ static cudaError_t launch_paged_repage(const kvbm_permute_side* src, uint32_t sr
                                        uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
 {
   if (layer_begin < 0 || layer_end < layer_begin || token_end < token_begin) return cudaErrorInvalidValue;
-  if (cast_mode < KVBM_CAST_NONE || cast_mode > KVBM_CAST_BF16_TO_FP8E4M3) return cudaErrorInvalidValue;
-  if (cast_scales && cast_mode == KVBM_CAST_NONE) return cudaErrorInvalidValue;
-  auto finish = [&]() -> cudaError_t {
-    if (!done_flag && !completion_flag) return cudaSuccess;
-    kvbm_signal_kernel<<<1, 1, 0, stream>>>(done_flag, epoch, completion_flag, completion_value);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    return cudaGetLastError();
-  };
-  if (token_end == token_begin || layer_end == layer_begin) return finish();
+  if (!cast_args_ok(cast_mode, cast_scales)) return cudaErrorInvalidValue;
+  if (token_end == token_begin || layer_end == layer_begin) return signal_launch(done_flag, epoch, completion_flag, completion_value, stream);
   if (!src || !dst || !src->block_ids || !dst->block_ids || !src->layout.layer_base || !dst->layout.layer_base) return cudaErrorInvalidValue;
   const uint32_t nl = dst->layout.num_layers, no = dst->layout.outer_dim;
   if (nl == 0 || no == 0 || nh == 0 || src->layout.num_layers != nl || src->layout.outer_dim != no || static_cast<uint32_t>(layer_end) > nl)
     return cudaErrorInvalidValue;
-  if (src_page == 0 || dst_page == 0) return cudaErrorInvalidValue;
-  const bool src_small = src_page < dst_page;
-  const uint32_t big_page = src_small ? dst_page : src_page, small_page = src_small ? src_page : dst_page;
-  if (big_page % small_page) return cudaErrorInvalidValue;
-  // slot arithmetic in 32 bits: every big block of the range ends below 2^32, and the page split is exact for q < big_page
-  const uint64_t big_end = (static_cast<uint64_t>(token_end) + big_page - 1) / big_page * big_page;
-  if (big_end >= (1ull << 32) || static_cast<uint64_t>(big_page) * small_page >= (1ull << 32)) return cudaErrorInvalidValue;
-  if (cast_mode == KVBM_CAST_BF16_TO_FP8E4M3 && (src_row_bytes & 1)) return cudaErrorInvalidValue;
-  const uint64_t dst_row_bytes = cast_mode == KVBM_CAST_FP8E4M3_TO_BF16   ? 2ull * src_row_bytes
-                                 : cast_mode == KVBM_CAST_BF16_TO_FP8E4M3 ? src_row_bytes / 2
-                                                                          : src_row_bytes;
-  const uint64_t walk_row = cast_mode == KVBM_CAST_BF16_TO_FP8E4M3 ? dst_row_bytes : src_row_bytes;
+  RepageParams P{};
   RowSplit r;
-  if (!row_split(walk_row, big_page, &r)) return cudaErrorInvalidValue;
+  uint64_t dst_row_bytes, units;
+  bool page_pow2;
+  if (!repage_geometry(src_page, dst_page, token_begin, token_end, layer_begin, layer_end, no, src_row_bytes, cast_mode, &P.g, &r,
+                       &dst_row_bytes, &units, &page_pow2))
+    return cudaErrorInvalidValue;
   if (static_cast<uint64_t>(src_page) * nh * src_row_bytes != src->layout.region_bytes ||
       static_cast<uint64_t>(dst_page) * nh * dst_row_bytes != dst->layout.region_bytes)
     return cudaErrorInvalidValue;
@@ -1060,31 +1222,9 @@ static cudaError_t launch_paged_repage(const kvbm_permute_side* src, uint32_t sr
   if (!fill_permute_side(*src, nl, no, nh, src_page, src_row_bytes, &S) ||
       !fill_permute_side(*dst, nl, no, nh, dst_page, static_cast<uint32_t>(dst_row_bytes), &D))
     return cudaErrorInvalidValue;
-  RepageParams P{};
-  P.big = src_small ? D : S;
-  P.small = src_small ? S : D;
-  P.small_page = small_page;
-  P.big_page = big_page;
-  P.ratio = big_page / small_page;
-  P.big_first = token_begin / big_page;
-  P.small_first = token_begin / small_page;
-  P.token_begin = token_begin;
-  P.token_end = token_end;
-  P.layer_begin = static_cast<uint32_t>(layer_begin);
-  P.nlayers = static_cast<uint32_t>(layer_end - layer_begin);
-  P.no = no;
-  P.nh = nh;
-  P.src_small = src_small ? 1 : 0;
-  // the small page's split, in RowSplit's form: log2 of the page, or the page and ceil(2^32 / page)
-  const bool page_pow2 = (small_page & (small_page - 1)) == 0;
-  if (page_pow2) {
-    while ((1u << P.page.vpr) < small_page) ++P.page.vpr;
-    P.page.pow2 = true;
-  } else {
-    P.page = {small_page, static_cast<uint32_t>(((1ull << 32) + small_page - 1) / small_page), false};
-  }
-  const uint64_t units = (static_cast<uint64_t>(big_end / big_page) - P.big_first) * P.nlayers * no;
-  if (units >= (1ull << 31)) return cudaErrorInvalidValue;
+  P.big = P.g.src_small ? D : S;
+  P.small = P.g.src_small ? S : D;
+  P.g.nh = nh;
   const int threads = static_cast<int>(std::min<uint32_t>(8, nh)) * 32;
   const unsigned grid = static_cast<unsigned>(units);
   with_walk_kernel(cast_mode, r.pow2, cast_scales != nullptr, [&](auto c, auto p, auto sc) {
@@ -1096,7 +1236,48 @@ static cudaError_t launch_paged_repage(const kvbm_permute_side* src, uint32_t sr
   g_launches.fetch_add(1, std::memory_order_relaxed);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
-  return finish();
+  return signal_launch(done_flag, epoch, completion_flag, completion_value, stream);
+}
+
+// kvbm_kernels_paged_repage_gather: the checks of launch_paged_permute's sources and of launch_paged_repage's pages, each side's
+// region at its own page and head count, all before any CUDA call; the signal on an empty range; then one launch and the signal.
+static cudaError_t launch_paged_repage_gather(const kvbm_permute_source* srcs, int num_srcs, uint32_t src_page, const kvbm_permute_side* dst,
+                                              uint32_t dst_num_heads, uint32_t dst_page, uint32_t token_begin, uint32_t token_end,
+                                              int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
+                                              uint32_t* done_flag, uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value,
+                                              cudaStream_t stream)
+{
+  if (layer_begin < 0 || layer_end < layer_begin || token_end < token_begin) return cudaErrorInvalidValue;
+  if (!cast_args_ok(cast_mode, cast_scales)) return cudaErrorInvalidValue;
+  if (!srcs || num_srcs < 1 || num_srcs > KVBM_GATHER_MAX_SOURCES) return cudaErrorInvalidValue;
+  if (token_end == token_begin || layer_end == layer_begin) return signal_launch(done_flag, epoch, completion_flag, completion_value, stream);
+  if (!dst || !dst->block_ids || !dst->layout.layer_base) return cudaErrorInvalidValue;
+  const uint32_t nl = dst->layout.num_layers, no = dst->layout.outer_dim;
+  if (nl == 0 || no == 0 || static_cast<uint32_t>(layer_end) > nl) return cudaErrorInvalidValue;
+  RepageGatherParams P{};
+  RowSplit r;
+  uint64_t dst_row_bytes, units;
+  bool page_pow2;
+  if (!repage_geometry(src_page, dst_page, token_begin, token_end, layer_begin, layer_end, no, src_row_bytes, cast_mode, &P.geo, &r,
+                       &dst_row_bytes, &units, &page_pow2))
+    return cudaErrorInvalidValue;
+  if (static_cast<uint64_t>(dst_page) * dst_num_heads * dst_row_bytes != dst->layout.region_bytes) return cudaErrorInvalidValue;
+  if (!fill_permute_side(*dst, nl, no, dst_num_heads, dst_page, static_cast<uint32_t>(dst_row_bytes), &P.g.D)) return cudaErrorInvalidValue;
+  if (!fill_gather_sources(srcs, num_srcs, dst_num_heads, nl, no, src_page, src_row_bytes, KVBM_GATHER_MAX_HEADS, &P.g))
+    return cudaErrorInvalidValue;
+  P.geo.nh = P.g.covered;
+  const int threads = static_cast<int>(std::min<uint32_t>(8, P.g.covered)) * 32;
+  const unsigned grid = static_cast<unsigned>(units);
+  with_walk_kernel(cast_mode, r.pow2, cast_scales != nullptr, [&](auto c, auto p, auto sc) {
+    if (page_pow2)
+      kvbm_paged_repage_gather_kernel<c, p, sc, true><<<grid, threads, 0, stream>>>(P, r, cast_scales);
+    else
+      kvbm_paged_repage_gather_kernel<c, p, sc, false><<<grid, threads, 0, stream>>>(P, r, cast_scales);
+  });
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  return signal_launch(done_flag, epoch, completion_flag, completion_value, stream);
 }
 
 }  // namespace kvbm
@@ -1293,6 +1474,17 @@ kvbm_kernels_paged_repage(const kvbm_permute_side* src, uint32_t src_page_size, 
 {
   return launch_paged_repage(src, src_page_size, dst, dst_page_size, token_begin, token_end, layer_begin, layer_end, num_heads,
                              src_row_bytes, cast_mode, cast_scales, done_flag, epoch, completion_flag, completion_value, stream);
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_repage_gather(const kvbm_permute_source* srcs, int num_srcs, uint32_t src_page_size, const kvbm_permute_side* dst,
+                                 uint32_t dst_num_heads, uint32_t dst_page_size, uint32_t token_begin, uint32_t token_end, int layer_begin,
+                                 int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales, uint32_t* done_flag,
+                                 uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
+{
+  return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, token_begin, token_end, layer_begin,
+                                    layer_end, src_row_bytes, cast_mode, cast_scales, done_flag, epoch, completion_flag, completion_value,
+                                    stream);
 }
 
 extern "C" bool

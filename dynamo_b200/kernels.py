@@ -180,6 +180,10 @@ def lib() -> C.CDLL:
         L.kvbm_kernels_paged_repage.argtypes = [C.POINTER(PermuteSide), C.c_uint32, C.POINTER(PermuteSide), C.c_uint32, C.c_uint32,
                                                 C.c_uint32, i, i, C.c_uint32, C.c_uint32, i, vp, vp, C.c_uint32, vp, C.c_uint32, vp]
         L.kvbm_kernels_paged_repage.restype = i
+        L.kvbm_kernels_paged_repage_gather.argtypes = [C.POINTER(PermuteSource), i, C.c_uint32, C.POINTER(PermuteSide), C.c_uint32,
+                                                       C.c_uint32, C.c_uint32, C.c_uint32, i, i, C.c_uint32, i, vp, vp, C.c_uint32, vp,
+                                                       C.c_uint32, vp]
+        L.kvbm_kernels_paged_repage_gather.restype = i
         L.kvbm_kernels_permute_strides.argtypes = [i, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64, C.c_uint64,
                                                    C.POINTER(C.c_uint64)]
         L.kvbm_kernels_permute_strides.restype = i
@@ -203,7 +207,7 @@ EXPORTED_SYMBOLS = [
     "kvbm_kernels_launch_count", "kvbm_kernels_build_info", "kvbm_kernels_gate_would_spin", "kvbm_kernels_paged_permute",
     "kvbm_kernels_permute_strides", "kvbm_kernels_paged_permute_cast", "kvbm_kernels_paged_permute_heads",
     "kvbm_kernels_paged_permute_gather", "kvbm_kernels_paged_permute_heads_scaled", "kvbm_kernels_paged_permute_gather_scaled",
-    "kvbm_kernels_paged_repage",
+    "kvbm_kernels_paged_repage", "kvbm_kernels_paged_repage_gather",
 ]
 
 
@@ -339,6 +343,20 @@ def paged_repage(src: PermuteSide, src_page_size: int, dst: PermuteSide, dst_pag
     return lib().kvbm_kernels_paged_repage(C.byref(src), src_page_size, C.byref(dst), dst_page_size, token_begin, token_end, layer_begin,
                                            layer_end, num_heads, src_row_bytes, int(cast_mode), scales_ptr(cast_scales), done_flag or None,
                                            epoch, completion_flag or None, completion_value, stream)
+
+
+def paged_repage_gather(srcs: Sequence[PermuteSource], src_page_size: int, dst: PermuteSide, dst_num_heads: int, dst_page_size: int,
+                        token_begin: int, token_end: int, layer_begin: int, layer_end: int, src_row_bytes: int, cast_mode: int = 0,
+                        cast_scales=None, done_flag: int = 0, epoch: int = 0, completion_flag: int = 0, completion_value: int = 0,
+                        stream: int = 0) -> int:
+    """`paged_permute_gather`'s head windows over `paged_repage`'s token range, in ONE launch: every source shares the page size
+    src_page_size (its block_ids = its table[token_begin // Ps .. ceil(token_end / Ps))), the destination has its own
+    (dst.block_ids likewise for Pd); every destination byte outside the windows' heads and the range keeps its value, and the
+    flags are written once.  include/kvbm_kernels.h (kvbm_kernels_paged_repage_gather)."""
+    arr = (PermuteSource * max(1, len(srcs)))(*srcs)
+    return lib().kvbm_kernels_paged_repage_gather(arr, len(srcs), src_page_size, C.byref(dst), dst_num_heads, dst_page_size, token_begin,
+                                                  token_end, layer_begin, layer_end, src_row_bytes, int(cast_mode), scales_ptr(cast_scales),
+                                                  done_flag or None, epoch, completion_flag or None, completion_value, stream)
 
 
 def permute_strides(kv_layout: int, num_layers: int, outer_dim: int, num_heads: int, page_size: int, row_bytes: int,

@@ -231,6 +231,7 @@ EXPORTED_SYMBOLS = [
     "kvbm_mc_supported", "kvbm_mc_group_create", "kvbm_mc_group_export_fd", "kvbm_mc_group_import_fd",
     "kvbm_mc_group_size", "kvbm_mc_group_add_device", "kvbm_mc_group_bind_local", "kvbm_mc_group_bind_addr", "kvbm_mc_group_map",
     "kvbm_mc_group_destroy", "kvbm_tp_reshard_plan", "kvbm_manager_execute_gather", "kvbm_manager_execute_repage",
+    "kvbm_manager_execute_repage_gather",
 ]
 
 
@@ -280,6 +281,8 @@ def lib() -> C.CDLL:
         L.kvbm_tp_reshard_plan.argtypes = [sz, sz, sz, sz, P(_CHeadWindow), sz, P(sz)]
         L.kvbm_manager_execute_gather.argtypes = [vp, sz, P(u64), P(P(sz)), u64, vp, sz, P(_CHeadWindow), sz, P(_COptions), P(u64)]
         L.kvbm_manager_execute_repage.argtypes = [vp, u64, vp, sz, u64, vp, sz, sz, sz, P(_COptions), P(u64)]
+        L.kvbm_manager_execute_repage_gather.argtypes = [vp, sz, P(u64), P(P(sz)), sz, u64, vp, sz, sz, sz, P(_CHeadWindow), sz,
+                                                         P(_COptions), P(u64)]
         L.kvbm_notification_is_complete.argtypes = [vp, u64]
         L.kvbm_notification_wait.argtypes = [vp, u64, C.c_int64]
         L.kvbm_manager_bytes_moved.argtypes = [vp]
@@ -636,6 +639,33 @@ class TransferManager:
         _check(lib().kvbm_manager_execute_repage(self._h, src, s.addr if type(s) is _NpView else s, ns, dst,
                                                  d.addr if type(d) is _NpView else d, nd, tokens.start, tokens.stop, C.byref(o),
                                                  C.byref(tok)))
+        return TransferCompleteNotification(self, tok.value)
+
+    def execute_repage_gather(self, sources: Mapping[int, tuple], dst: int, dst_block_ids: Sequence[int], plan: Sequence[HeadWindow],
+                              tokens: range, options: Optional[TransferOptions] = None) -> TransferCompleteNotification:
+        """`execute_gather` across engines with different page sizes, as ONE hand-off (kvbm_manager_execute_repage_gather): the
+        same `sources` mapping (source rank -> (layout handle, block ids)) and plan, over `execute_repage`'s `tokens` range.  Every
+        source has one page size Ps and its ids are its table's entries tokens.start // Ps .. ceil(tokens.stop / Ps);
+        `dst_block_ids` are the destination's for its own page.  Options: those of `execute_repage`."""
+        if tokens.step != 1:
+            raise ValueError("tokens must be a range with step 1")
+        ranks = sorted({w.src_rank for w in plan})
+        index = {r: i for i, r in enumerate(ranks)}
+        n_src = len(sources[ranks[0]][1]) if ranks else 0
+        if any(len(sources[r][1]) != n_src for r in ranks):
+            raise KvbmError(ErrorCode.LENGTH_MISMATCH, "the sources' block id lists have different lengths")
+        hs = (C.c_uint64 * max(1, len(ranks)))(*[sources[r][0] for r in ranks])
+        s_arrays = [_size_array(sources[r][1])[0] for r in ranks]
+        d, n_dst = _size_array(dst_block_ids)
+        PP = C.POINTER(C.c_size_t)
+        as_ptr = lambda a: a._as_parameter_ if isinstance(a, _NpView) else C.cast(a, PP)  # noqa: E731
+        sp = (PP * max(1, len(ranks)))(*[as_ptr(a) for a in s_arrays])
+        ws = (_CHeadWindow * max(1, len(plan)))(*[_CHeadWindow(index[w.src_rank], w.src_head_begin, w.dst_head_begin, w.head_count)
+                                                  for w in plan])
+        tok = C.c_uint64()
+        o = (options or TransferOptions())._c()
+        _check(lib().kvbm_manager_execute_repage_gather(self._h, len(ranks), hs, sp, n_src, dst, d.addr if type(d) is _NpView else d, n_dst,
+                                                        tokens.start, tokens.stop, ws, len(plan), C.byref(o), C.byref(tok)))
         return TransferCompleteNotification(self, tok.value)
 
     def execute_fanout(self, src: int, dsts: Sequence[int], src_block_ids: Sequence[Sequence[int]],

@@ -305,6 +305,26 @@ cudaError_t kvbm_kernels_paged_repage(const kvbm_permute_side* src, uint32_t src
                                       const float* cast_scales, uint32_t* done_flag, uint32_t epoch, uint32_t* completion_flag,
                                       uint32_t completion_value, cudaStream_t stream);
 
+/* Re-paging and the gather in one launch (a decode rank assembling its re-sharded heads from source ranks whose engine has another
+ * page size): for every source s, head src_head_begin + j of srcs[s] lands as head dst_head_begin + j of the destination, for
+ * j < head_count, at every token of [token_begin, token_end), every layer of [layer_begin, layer_end) and every outer index,
+ * re-ordered and cast as kvbm_kernels_paged_permute_heads_scaled would, with the same bits.  Tokens sit as in
+ * kvbm_kernels_paged_repage: srcs[s].side.block_ids holds that source's table[token_begin / Ps .. ceil(token_end / Ps)),
+ * dst->block_ids the destination's table[token_begin / Pd .. ceil(token_end / Pd)).  All sources share src_page_size (Ps),
+ * src_row_bytes and cast_mode; each has its own pool, format and num_heads (its region_bytes = Ps * num_heads * src_row_bytes);
+ * the destination's region_bytes is Pd * dst_num_heads * its row.  cast_scales (nullable): one array for every source, indexed
+ * by the absolute layer and outer index.  Every other destination byte keeps its value: heads outside the union of the windows,
+ * and the slots of the first and last destination blocks outside the range.  cudaErrorInvalidValue, returned before any CUDA
+ * call, for every rule of kvbm_kernels_paged_permute_gather's sources and windows and of kvbm_kernels_paged_repage's pages,
+ * ranges, rows and strides.  One launch, then one signal launch that writes done_flag / completion_flag once; an empty token or
+ * layer range launches nothing and still signals. */
+cudaError_t kvbm_kernels_paged_repage_gather(const kvbm_permute_source* srcs, int num_srcs, uint32_t src_page_size,
+                                             const kvbm_permute_side* dst, uint32_t dst_num_heads, uint32_t dst_page_size,
+                                             uint32_t token_begin, uint32_t token_end, int layer_begin, int layer_end,
+                                             uint32_t src_row_bytes, int cast_mode, const float* cast_scales, uint32_t* done_flag,
+                                             uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value,
+                                             cudaStream_t stream);
+
 /* Host-only (no GPU): the stride table kvbm_kernels_paged_permute walks with for one side.  out[0] = 1 when offsets count
  * from the block's first byte (universal formats) or 0 when they count from the (layer, outer) region's first byte; the
  * element (layer l, outer o, head h, token t) then sits at  [out[0] ? l * out[1] + o * out[2] : 0] + h * out[3] + t * out[4].

@@ -307,6 +307,29 @@ int kvbm_manager_execute_repage(kvbm_transfer_manager* m, kvbm_layout_handle src
                                 kvbm_layout_handle dst, const size_t* dst_ids, size_t n_dst, size_t token_begin, size_t token_end,
                                 const kvbm_transfer_options* opts, kvbm_notification* out);
 
+/* A TP re-shard's assembly across engines with different page sizes (prefill pages of Ps tokens at one TP degree, decode pages
+ * of Pd at another), as ONE hand-off: kvbm_manager_execute_gather's windows over kvbm_manager_execute_repage's token range.  For
+ * window w, head w.src_head_begin + j of source w.src_rank lands as destination head w.dst_head_begin + j (j < w.head_count), at
+ * every token of [token_begin, token_end), every layer of the options' layer range and every outer index, re-ordered and cast as
+ * execute_repage would.  src_ids[s] holds source s's table[token_begin / Ps .. ceil(token_end / Ps)) (n_src ids each), dst_ids
+ * the destination's table[token_begin / Pd .. ceil(token_end / Pd)) (n_dst ids).  Every other destination byte keeps its value:
+ * heads no window covers, and the slots of the first and last destination blocks outside the range.  windows are
+ * kvbm_head_windows, so a kvbm_tp_reshard_plan passes as it is.  Honoured options: execute_repage's (src_kv_layout applies to
+ * every source).  Errors, first one wins: execute_gather's window checks (KVBM_ERR no source or window, or options.head_count;
+ * KVBM_ERR_UNSUPPORTED more than KVBM_GATHER_MAX_SOURCES windows; KVBM_ERR_RANGE a window naming no source or with no heads;
+ * KVBM_ERR_OVERLAP two windows on one destination head); KVBM_ERR_HANDLE; then for each window's source, execute_repage's checks
+ * of its pair with the destination (num_heads may differ), the window inside both sides' heads (KVBM_ERR_RANGE) and
+ * KVBM_ERR_INCOMPATIBLE a page size other than the first source's; execute_repage's token range, layer range, cast scales and
+ * id counts (KVBM_ERR_LENGTH_MISMATCH n_src / n_dst other than the range implies for Ps / Pd); the ids of each window's source
+ * against the destination's, as execute_repage; an empty token or layer range then returns KVBM_OK with nothing launched;
+ * KVBM_ERR_UNSUPPORTED a strategy other than a direct CUDA one, or sources with different ones; KVBM_ERR_CUDA a host-only
+ * manager.  One upload of num_srcs * n_src + n_dst ids, one kvbm_kernels_paged_repage_gather launch, one notification;
+ * bytes_moved counts tokens * layers * outer_dim * covered heads * the destination row. */
+int kvbm_manager_execute_repage_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs,
+                                       const size_t* const* src_ids, size_t n_src, kvbm_layout_handle dst, const size_t* dst_ids,
+                                       size_t n_dst, size_t token_begin, size_t token_end, const kvbm_head_window* windows,
+                                       size_t num_windows, const kvbm_transfer_options* opts, kvbm_notification* out);
+
 /* Completion: the transfer's last warp writes a flag in pinned host memory (no cudaEventQuery polling). */
 int kvbm_notification_is_complete(kvbm_transfer_manager* m, kvbm_notification n);  /* 1 / 0 / <0 error */
 int kvbm_notification_wait(kvbm_transfer_manager* m, kvbm_notification n, int64_t timeout_us);
