@@ -755,10 +755,7 @@ static int execute_two_hop(kvbm_transfer_manager* m, Layout* S, Layout* D, Layou
   cudaEvent_t hop2_done[2] = {nullptr, nullptr};
   kvbm_transfer_options o1 = o, o2 = o;
   o1.done_flag = nullptr;        // completion signals belong to the hop that lands the bytes at the destination
-  o1.layer_done_flags = nullptr;
-  o1.per_dst_done_flags = nullptr;
-  o1.per_dst_layer_done_flags = nullptr;
-  o2.layer_ready_flags = nullptr;  // ... and gating to the hop that reads the source
+  o1.per_dst_done_flags = nullptr;  // (layer streaming is rejected by check_strategy)
   uint64_t last = 0;
   size_t pos = 0;
   for (int c = 0; pos < n; ++c) {
@@ -774,7 +771,10 @@ static int execute_two_hop(kvbm_transfer_manager* m, Layout* S, Layout* D, Layou
     if (rc) return rc;
     Layout* Dp = D;
     kvbm_transfer_options o2c = o2;
-    if (pos + cnt < n) o2c.done_flag = nullptr;  // only the last chunk announces the whole transfer
+    if (pos + cnt < n) {  // only the last chunk announces the whole transfer
+      o2c.done_flag = nullptr;
+      o2c.per_dst_done_flags = nullptr;
+    }
     rc = launch_cuda(m, B, &Dp, 1, &bids, &dp, cnt, true, lb, le, o2c, s2, a->ev, &b, &sb);
     if (rc) return rc;
     hop2_done[g] = b->ev;
@@ -895,6 +895,9 @@ static int check_strategy(kvbm_transfer_manager* m, int nd, const kvbm_transfer_
   if (o.use_caller_stream) return fail(KVBM_ERR_UNSUPPORTED, "Two-hop transfers don't support caller-provided streams");  // executor/mod.rs:441
   if (o.cast_mode != KVBM_CAST_NONE) return fail(KVBM_ERR_UNSUPPORTED, "the fused cast is not available on two-hop transfers");
   if (t->permute) return fail(KVBM_ERR_UNSUPPORTED, "a layout transformation is not available on two-hop transfers");
+  // each chunk's first hop would be a whole gated launch and its second hop would announce layers other chunks have not landed
+  if (o.layer_ready_flags || o.layer_done_flags || o.per_dst_layer_done_flags)
+    return fail(KVBM_ERR_UNSUPPORTED, "layer streaming is not available on two-hop transfers");
   if (!o.bounce_layout || !o.bounce_block_ids || o.num_bounce_blocks == 0)
     return fail(KVBM_ERR, "Two-hop transfers require a bounce buffer.");  // executor/mod.rs:514-519
   Layout* B = t->B = m->find(o.bounce_layout);

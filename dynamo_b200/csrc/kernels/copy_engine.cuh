@@ -93,7 +93,7 @@ __device__ __forceinline__ bool piece_tma_ok(const Piece& p)
 // `ctl` is three zeroed words the launch owns: [0] rings finished, [1] abort, [2] scheduler tickets.  They are left
 // zeroed by the last ring to finish, so the same words serve the next launch.
 struct StreamSync {
-  const uint32_t* layer_ready;  // wait until layer_ready[l] >= epoch before reading layer l
+  const uint32_t* layer_ready;  // wait until layer_ready[l] reaches epoch (epoch_reached) before reading layer l
   uint32_t* layer_counters;     // [num_layers] zeroed: items of layer l that have landed
   uint32_t* ctl;                // see above; null = static tile schedule, no completion signals
   uint32_t* done_flag[kMaxDst];
@@ -153,6 +153,10 @@ struct RingSmem {
   uint32_t out0;  // 2 * tile_out (cast only)
 };
 
+// A ready flag has reached the epoch when (int32_t)(flag - epoch) >= 0: the cyclic order of CU_STREAM_WAIT_VALUE_GEQ, so the
+// spinning gate and the stream-wait gate agree, also across the 32-bit wrap (include/kvbm_kernels.h, kvbm_paged_copy_opts.epoch).
+__device__ __forceinline__ bool epoch_reached(uint32_t flag, uint32_t epoch) { return static_cast<int32_t>(flag - epoch) >= 0; }
+
 // Flag polls are relaxed loads; one acquire fence follows a successful probe (an ld.acquire.sys per poll would
 // invalidate L1 every time and, measured, slowed the co-resident compute kernel).
 // Returns false when the flag was not released within gate_timeout_ns or another ring already gave up: a spinning
@@ -164,7 +168,7 @@ __device__ __forceinline__ bool wait_layer_ready(const StreamSync& ss, int layer
   if (lane == 0) {
     const uint64_t t0 = ptx::globaltimer_ns();
     uint32_t polls = 0;
-    while (ptx::ld_relaxed_sys(ss.layer_ready + layer) < ss.epoch) {
+    while (!epoch_reached(ptx::ld_relaxed_sys(ss.layer_ready + layer), ss.epoch)) {
       __nanosleep(128);
       if ((++polls & 255u) == 0) {
         if (ptx::ld_relaxed_sys(ss.ctl + 1) != 0) {

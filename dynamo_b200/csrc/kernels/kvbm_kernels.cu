@@ -970,9 +970,10 @@ __global__ void kvbm_set_flags_kernel(uint32_t* flags, int first, int count, uin
     ptx::st_release_sys(flags + first + i, value);
   }
 }
+// The fallback of kvbm_kernels_wait_flag when stream memops are missing: the same cyclic order as CU_STREAM_WAIT_VALUE_GEQ.
 __global__ void kvbm_wait_flag_kernel(const uint32_t* flag, uint32_t value)
 {
-  while (ptx::ld_acquire_sys(flag) < value) __nanosleep(100);
+  while (!epoch_reached(ptx::ld_acquire_sys(flag), value)) __nanosleep(100);
 }
 
 static cudaError_t preload_kernels()
@@ -1685,7 +1686,8 @@ kvbm_kernels_paged_copy_v2(const kvbm_paged_layout* src, const kvbm_paged_dst* d
   kvbm_paged_dst dd[KVBM_MAX_DESTINATIONS];
   for (int l = layer_begin; l < layer_end; ++l) {
     const bool last = l + 1 == layer_end;
-    // CU_STREAM_WAIT_VALUE_GEQ: the stream front-end polls the word, no SM is occupied
+    // CU_STREAM_WAIT_VALUE_GEQ: the stream front-end polls the word, no SM is occupied; (int32)(flag - epoch) >= 0, the order
+    // the spinning gate uses too (epoch_reached)
     if (g_wait32(stream, reinterpret_cast<unsigned long long>(opts->layer_ready_flags + l), opts->epoch, 0) != 0) return cudaErrorUnknown;
     for (int d = 0; d < num_dsts; ++d) {
       dd[d] = dsts[d];

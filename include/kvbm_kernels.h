@@ -121,8 +121,11 @@ enum {
 };
 
 typedef struct kvbm_paged_copy_opts {
-  uint32_t epoch;                 /* value written to done flags / compared with ready flags (>=) */
-  const uint32_t* layer_ready_flags; /* nullable; [num_layers]; layer l is read only after flag >= epoch */
+  uint32_t epoch;                 /* value written to done flags; a ready flag has reached it iff (int32_t)(flag - epoch) >= 0,
+                                     the cyclic order of CU_STREAM_WAIT_VALUE_GEQ, in both gate modes.  Epochs may wrap past
+                                     0xFFFFFFFF; a flag must never lag its epoch by 2^31 or more (zeroed flags and epochs counting
+                                     up from 1 satisfy that).  kvbm_kernels_wait_flag uses the same order. */
+  const uint32_t* layer_ready_flags; /* nullable; [num_layers]; layer l is read only after flag l has reached epoch */
   uint32_t* sync_workspace;       /* device u32[KVBM_SYNC_WORKSPACE_WORDS(num_layers)], zeroed (left zeroed by every launch):
                                      per-layer landed-item counters, then the launch's control words (rings finished, abort,
                                      tile-scheduler tickets).  Required iff any flag or gating is used; without it the
@@ -336,7 +339,8 @@ int kvbm_kernels_permute_strides(int kv_layout, uint32_t num_layers, uint32_t ou
  * cuModuleGetLoadingMode), 0 when it would gate on the stream instead. */
 int kvbm_kernels_gate_would_spin(void);
 
-/* Small helpers so hosts without a CUDA binding (ctypes, cgo, JNI) can drive the flags. */
+/* Small helpers so hosts without a CUDA binding (ctypes, cgo, JNI) can drive the flags.  wait_flag holds the stream until
+ * (int32_t)(*flag - value) >= 0, the epoch order of kvbm_paged_copy_opts.epoch. */
 cudaError_t kvbm_kernels_set_flags(uint32_t* flags, int first, int count, uint32_t value,
                                    cudaStream_t stream);
 cudaError_t kvbm_kernels_wait_flag(const uint32_t* flag, uint32_t value, cudaStream_t stream);
