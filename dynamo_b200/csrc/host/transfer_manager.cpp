@@ -301,6 +301,9 @@ struct kvbm_transfer_manager {
   // CUDA IPC mappings opened by import_metadata, keyed by the 64-byte handle: an allocation shared by several
   // imported layouts (e.g. two tensors in one allocator segment) is mapped once; closed when the manager dies.
   std::unordered_map<std::string, void*> ipc_cache;
+  // other devices whose memory this manager's device may touch: peer access enabled through kvbm_manager_enable_peer_access,
+  // or the devices of IPC mappings opened with lazy peer access
+  std::set<int> peers;
   // (agent name, worker id) of every SerializedLayout imported so far (manager/mod.rs:572-584 refuses a second load)
   std::set<std::pair<std::string, uint64_t>> loaded_remotes;
   // TransferCapabilities (transfer/strategy.rs:245-278).  allow_gpu_rdma = peers may be written directly over NVLink
@@ -669,22 +672,44 @@ struct Transfer {
   bool empty = false;
 };
 
+// The gate of a streamed launch: window j reads source ranks[j], so it waits for that source's flags; the options' epoch, gate
+// mode, timeout, CTA cap and done flag; the slot's workspace and completion word.
+static kvbm_permute_stream layer_stream(const kvbm_layer_stream& ls, const size_t* ranks, size_t nw, const kvbm_transfer_options& o,
+                                        const Slot& sl, uint64_t seq)
+{
+  kvbm_permute_stream st{};
+  for (size_t j = 0; j < nw; ++j) st.layer_ready_flags[j] = ls.src_layer_ready_flags[ranks[j]];
+  st.layer_done_flags = ls.layer_done_flags;
+  st.done_flag = o.done_flag;
+  st.epoch = o.epoch;
+  st.sync_workspace = sl.dev_ws;
+  st.completion_flag = sl.host_flag;
+  st.completion_value = static_cast<uint32_t>(seq);
+  st.gate_mode = o.gate_mode;
+  st.gate_timeout_ms = o.gate_timeout_ms;
+  st.max_ctas = o.max_ctas;
+  return st;
+}
+
 // The layout-transforming transfer: what select_transform_kernel's result would drive if the reference ran it inside
 // execute_transfer (it rejects the pair instead, transfer/mod.rs:128-147).  One permuting launch moves every entry's head window
 // from source e[j].window.src_rank into e[0].D over e[0]'s layer range, with the transfer's fp8 <-> bf16 cast fused in:
 // kvbm_kernels_paged_permute_heads for one window (any head count), kvbm_kernels_paged_permute_gather for several.  Block
 // tables: source s at s * n and the destination's at num_srcs * n, no pointer tables; the completion word is written by a
 // trailing signal kernel.
+// ls: a streamed gather (execute_gather_streamed), one kvbm_kernels_paged_permute_gather_streamed launch gated on every window's
+// source flags, with the slot's workspace staged for the destination's layers.
 static int launch_permute(kvbm_transfer_manager* m, const Transfer* e, size_t nw, size_t num_srcs, const size_t* const* src_ids,
-                          const size_t* dst_ids, size_t n, const kvbm_transfer_options& o, cudaStream_t stream, uint64_t* seq_out)
+                          const size_t* dst_ids, size_t n, const kvbm_transfer_options& o, cudaStream_t stream, uint64_t* seq_out,
+                          const kvbm_layer_stream* ls = nullptr)
 {
   std::vector<const size_t*> lists(src_ids, src_ids + num_srcs);
   lists.push_back(dst_ids);
   Slot* sl;
   uint64_t seq;
-  int rc = stage_ids(m, lists.data(), lists.size(), n, 4, stream, nullptr, &sl, &seq);
-  if (rc) return rc;
   const Layout *S0 = e[0].S, *D = e[0].D[0];
+  int rc = stage_ids(m, lists.data(), lists.size(), n, ls ? D->cfg.num_layers + 4 : 4, stream, nullptr, &sl, &seq);
+  if (rc) return rc;
   kvbm_permute_side pd{descriptor(*D), sl->dev_ids + num_srcs * n, e[0].dst_kv};
   kvbm_permute_source ks[KVBM_GATHER_MAX_SOURCES] = {};
   size_t heads = 0;
@@ -698,7 +723,14 @@ static int launch_permute(kvbm_transfer_manager* m, const Transfer* e, size_t nw
   const uint32_t dnh = static_cast<uint32_t>(D->cfg.num_heads), page = static_cast<uint32_t>(S0->cfg.page_size);
   const uint32_t row = static_cast<uint32_t>(S0->cfg.inner_dim / S0->cfg.num_heads * S0->cfg.dtype_width_bytes);
   const int nb = static_cast<int>(n), lb = static_cast<int>(e[0].lb), le = static_cast<int>(e[0].le);
-  if (nw == 1) {
+  if (ls) {
+    size_t ranks[KVBM_GATHER_MAX_SOURCES];
+    for (size_t j = 0; j < nw; ++j) ranks[j] = e[j].window.src_rank;
+    const kvbm_permute_stream st = layer_stream(*ls, ranks, nw, o, *sl, seq);
+    cudaError_t ce = kvbm_kernels_paged_permute_gather_streamed(ks, static_cast<int>(nw), &pd, dnh, nb, lb, le, page, row, o.cast_mode,
+                                                                o.cast_scales, &st, stream);
+    if (ce != cudaSuccess) return fail_cuda(ce, "kvbm_kernels_paged_permute_gather_streamed");
+  } else if (nw == 1) {
     const kvbm_permute_source& k = ks[0];
     cudaError_t ce = kvbm_kernels_paged_permute_heads_scaled(&k.side, &pd, nb, lb, le, k.num_heads, k.src_head_begin, dnh, k.dst_head_begin,
                                                              k.head_count, page, row, o.cast_mode, o.cast_scales, o.done_flag, o.epoch,
@@ -726,6 +758,45 @@ static int check_cast_scales(kvbm_transfer_manager* m, const float* p)
   if (!ok)
     return fail(KVBM_ERR, "cast_scales must be device memory of device " + std::to_string(m->device) +
                               " or pinned host memory mapped into it (a pageable or another device's pointer cannot be read by the cast)");
+  return KVBM_OK;
+}
+
+// The shape of a streamed request's flags, before anything else is checked: one ready-flag array per source, none null.
+static int check_layer_stream_shape(const kvbm_layer_stream* ls, size_t num_srcs)
+{
+  if (!ls || !ls->src_layer_ready_flags) return fail(KVBM_ERR, "a streamed transfer needs a kvbm_layer_stream with ready flags");
+  if (ls->num_srcs != num_srcs)
+    return fail(KVBM_ERR_LENGTH_MISMATCH, "the layer stream names " + std::to_string(ls->num_srcs) + " sources' ready flags, the request has " +
+                                              std::to_string(num_srcs) + " sources");
+  for (size_t s = 0; s < num_srcs; ++s)
+    if (!ls->src_layer_ready_flags[s]) return fail(KVBM_ERR, "source " + std::to_string(s) + " has no layer ready flags");
+  return KVBM_OK;
+}
+
+// The flags of a streamed request are polled and written by the kernels on the manager's device: its own device memory, memory of
+// a device it has peer access to (enabled through kvbm_manager_enable_peer_access, or by an IPC mapping this manager opened) or
+// pinned host memory mapped into its address space.  Anything else (pageable host memory, a device without enabled peer access)
+// must not reach a kernel.
+static int check_layer_stream_flags(kvbm_transfer_manager* m, const kvbm_layer_stream& ls, const size_t* ranks, size_t nw)
+{
+  auto reachable = [&](const void* p) {
+    cudaPointerAttributes a{};
+    const cudaError_t e = cudaPointerGetAttributes(&a, p);
+    if (e != cudaSuccess) {
+      (void)cudaGetLastError();
+      return false;
+    }
+    if (a.type == cudaMemoryTypeHost) return a.devicePointer == p;
+    if (a.type != cudaMemoryTypeDevice) return false;
+    return a.device == m->device || m->peers.count(a.device) != 0;
+  };
+  for (size_t j = 0; j < nw; ++j)
+    if (!reachable(ls.src_layer_ready_flags[ranks[j]]))
+      return fail(KVBM_ERR, "the layer ready flags of source " + std::to_string(ranks[j]) + " are not reachable from device " +
+                                std::to_string(m->device) + " (its own memory, a device it has peer access to, or mapped pinned host memory)");
+  if (ls.layer_done_flags && !reachable(ls.layer_done_flags))
+    return fail(KVBM_ERR, "the layer done flags are not reachable from device " + std::to_string(m->device) +
+                              " (its own memory, a device it has peer access to, or mapped pinned host memory)");
   return KVBM_OK;
 }
 
@@ -1059,9 +1130,10 @@ static int check_gather_windows(size_t num_srcs, const kvbm_layout_handle* srcs,
 // A TP re-shard's assembly as one hand-off: every window is validated as the windowed execute_transfer of its (source,
 // destination) pair, then one kvbm_kernels_paged_permute_gather launch moves all of them and one signal launch writes the
 // done flag and the completion word after the last byte landed.
+// ls: the streamed gather, checked as above and then for its flags, launched gated on them.
 static int execute_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, const size_t* const* src_ids,
                           kvbm_layout_handle dst_h, const size_t* dst_ids, size_t n, const kvbm_head_window* windows, size_t nw,
-                          const kvbm_transfer_options* opts_in, kvbm_notification* out)
+                          const kvbm_transfer_options* opts_in, kvbm_notification* out, const kvbm_layer_stream* ls = nullptr)
 {
   kvbm_transfer_options o{};
   if (opts_in) o = *opts_in;
@@ -1077,10 +1149,15 @@ static int execute_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_
     if (e[j].plan.first != e[0].plan.first) return fail(KVBM_ERR_UNSUPPORTED, "the sources of a gather need the same CUDA strategy");
   }
   if (e[0].empty) return KVBM_OK;  // nothing to move (no blocks or an empty layer range), as execute()
+  if (ls) {
+    size_t ranks[KVBM_GATHER_MAX_SOURCES];
+    for (size_t j = 0; j < nw; ++j) ranks[j] = windows[j].src_rank;
+    if (int rc = check_layer_stream_flags(m, *ls, ranks, nw)) return rc;
+  }
 
   DeviceGuard g(m->device);
   uint64_t seq;
-  int rc = launch_permute(m, e, nw, num_srcs, src_ids, dst_ids, n, o, pick_stream(m, e[0].plan.first, o), &seq);
+  int rc = launch_permute(m, e, nw, num_srcs, src_ids, dst_ids, n, o, pick_stream(m, e[0].plan.first, o), &seq, ls);
   if (rc) return rc;
   // caller-provided stream: caller manages sync, completed() is returned, as execute()
   if (out) *out = o.use_caller_stream ? 0 : seq;
@@ -1221,7 +1298,8 @@ static int execute_repage(kvbm_transfer_manager* m, kvbm_layout_handle src_h, co
 // One upload of every source's ids and the destination's, one kvbm_kernels_paged_repage_gather launch and one notification.
 static int execute_repage_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, const size_t* const* src_ids,
                                  size_t n_src, kvbm_layout_handle dst_h, const size_t* dst_ids, size_t n_dst, size_t tb, size_t te,
-                                 const kvbm_head_window* windows, size_t nw, const kvbm_transfer_options* opts_in, kvbm_notification* out)
+                                 const kvbm_head_window* windows, size_t nw, const kvbm_transfer_options* opts_in, kvbm_notification* out,
+                                 const kvbm_layer_stream* ls = nullptr)
 {
   kvbm_transfer_options o{};
   if (opts_in) o = *opts_in;
@@ -1262,6 +1340,9 @@ static int execute_repage_gather(kvbm_transfer_manager* m, size_t num_srcs, cons
   }
   if ((rc = need_cuda_device(m))) return rc;
   if (o.cast_scales && (rc = check_cast_scales(m, o.cast_scales))) return rc;
+  size_t ranks[KVBM_GATHER_MAX_SOURCES];
+  for (size_t j = 0; j < nw; ++j) ranks[j] = windows[j].src_rank;
+  if (ls && (rc = check_layer_stream_flags(m, *ls, ranks, nw))) return rc;
 
   DeviceGuard g(m->device);
   const cudaStream_t stream = pick_stream(m, p0.first, o);
@@ -1271,7 +1352,7 @@ static int execute_repage_gather(kvbm_transfer_manager* m, size_t num_srcs, cons
   lens.push_back(n_dst);
   Slot* sl;
   uint64_t seq;
-  if ((rc = stage_ids(m, lists.data(), lens.data(), lists.size(), 4, stream, nullptr, &sl, &seq))) return rc;
+  if ((rc = stage_ids(m, lists.data(), lens.data(), lists.size(), ls ? D->cfg.num_layers + 4 : 4, stream, nullptr, &sl, &seq))) return rc;
   const kvbm_permute_side kd{descriptor(*D), sl->dev_ids + num_srcs * n_src, dst_kv};
   kvbm_permute_source ks[KVBM_GATHER_MAX_SOURCES] = {};
   for (size_t j = 0; j < nw; ++j) {
@@ -1281,11 +1362,21 @@ static int execute_repage_gather(kvbm_transfer_manager* m, size_t num_srcs, cons
                                 static_cast<uint32_t>(w.head_count)};
   }
   const size_t row = S[0]->cfg.inner_dim / S[0]->cfg.num_heads * S[0]->cfg.dtype_width_bytes;
-  cudaError_t ce = kvbm_kernels_paged_repage_gather(ks, static_cast<int>(nw), static_cast<uint32_t>(ps), &kd, static_cast<uint32_t>(D->cfg.num_heads),
-                                                    static_cast<uint32_t>(pd), static_cast<uint32_t>(tb), static_cast<uint32_t>(te),
-                                                    static_cast<int>(lb), static_cast<int>(le), static_cast<uint32_t>(row), o.cast_mode,
-                                                    o.cast_scales, o.done_flag, o.epoch, sl->host_flag, static_cast<uint32_t>(seq), stream);
-  if (ce != cudaSuccess) return fail_cuda(ce, "kvbm_kernels_paged_repage_gather");
+  if (ls) {
+    const kvbm_permute_stream st = layer_stream(*ls, ranks, nw, o, *sl, seq);
+    cudaError_t ce = kvbm_kernels_paged_repage_gather_streamed(ks, static_cast<int>(nw), static_cast<uint32_t>(ps), &kd,
+                                                               static_cast<uint32_t>(D->cfg.num_heads), static_cast<uint32_t>(pd),
+                                                               static_cast<uint32_t>(tb), static_cast<uint32_t>(te), static_cast<int>(lb),
+                                                               static_cast<int>(le), static_cast<uint32_t>(row), o.cast_mode, o.cast_scales, &st,
+                                                               stream);
+    if (ce != cudaSuccess) return fail_cuda(ce, "kvbm_kernels_paged_repage_gather_streamed");
+  } else {
+    cudaError_t ce = kvbm_kernels_paged_repage_gather(ks, static_cast<int>(nw), static_cast<uint32_t>(ps), &kd, static_cast<uint32_t>(D->cfg.num_heads),
+                                                      static_cast<uint32_t>(pd), static_cast<uint32_t>(tb), static_cast<uint32_t>(te),
+                                                      static_cast<int>(lb), static_cast<int>(le), static_cast<uint32_t>(row), o.cast_mode,
+                                                      o.cast_scales, o.done_flag, o.epoch, sl->host_flag, static_cast<uint32_t>(seq), stream);
+    if (ce != cudaSuccess) return fail_cuda(ce, "kvbm_kernels_paged_repage_gather");
+  }
   const size_t d_row = D->cfg.inner_dim / D->cfg.num_heads * D->cfg.dtype_width_bytes;
   if ((rc = finish_slot(m, sl, stream, (te - tb) * (le - lb) * D->cfg.outer_dim * heads * d_row))) return rc;
   if (out) *out = o.use_caller_stream ? 0 : seq;
@@ -1508,9 +1599,11 @@ extern "C" int kvbm_manager_enable_peer_access(kvbm_transfer_manager* m, int pee
   cudaError_t e = cudaDeviceEnablePeerAccess(peer_device, 0);
   if (e == cudaErrorPeerAccessAlreadyEnabled) {
     (void)cudaGetLastError();
-    return KVBM_OK;
+    e = cudaSuccess;
   }
   if (e != cudaSuccess) return fail_cuda(e, "cudaDeviceEnablePeerAccess");
+  std::lock_guard<std::mutex> lk(m->mu);
+  m->peers.insert(peer_device);
   return KVBM_OK;
   });
 }
@@ -1670,8 +1763,12 @@ static int import_metadata_impl(kvbm_transfer_manager* m, const void* buf, size_
       if (!mapped) {
         cudaError_t e = cudaIpcOpenMemHandle(&mapped, ih, cudaIpcMemLazyEnablePeerAccess);
         if (e != cudaSuccess) return fail_cuda(e, "cudaIpcOpenMemHandle");
+        cudaPointerAttributes pa{};
+        const bool attr_ok = cudaPointerGetAttributes(&pa, mapped) == cudaSuccess;
+        if (!attr_ok) (void)cudaGetLastError();
         std::lock_guard<std::mutex> lk(m->mu);
         m->ipc_cache[key] = mapped;
+        if (attr_ok && pa.type == cudaMemoryTypeDevice && pa.device != m->device) m->peers.insert(pa.device);
       }
       bases[i] = reinterpret_cast<uintptr_t>(mapped) + ba.offset_in_ipc;
     }
@@ -1801,6 +1898,34 @@ extern "C" int kvbm_manager_execute_repage_gather(kvbm_transfer_manager* m, size
   return guarded([&]() -> int {
   if (!m) return fail(KVBM_ERR, "null manager");
   return execute_repage_gather(m, num_srcs, srcs, src_ids, n_src, dst, dst_ids, n_dst, token_begin, token_end, windows, num_windows, opts, out);
+  });
+}
+
+extern "C" int kvbm_manager_execute_gather_streamed(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs,
+                                                    const size_t* const* src_ids, kvbm_layout_handle dst, const size_t* dst_ids, size_t n,
+                                                    const kvbm_head_window* windows, size_t num_windows, const kvbm_layer_stream* ls,
+                                                    const kvbm_transfer_options* opts, kvbm_notification* out)
+{
+  return guarded([&]() -> int {
+  if (!m) return fail(KVBM_ERR, "null manager");
+  if (out) *out = 0;
+  if (int rc = check_layer_stream_shape(ls, num_srcs)) return rc;
+  return execute_gather(m, num_srcs, srcs, src_ids, dst, dst_ids, n, windows, num_windows, opts, out, ls);
+  });
+}
+
+extern "C" int kvbm_manager_execute_repage_gather_streamed(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs,
+                                                           const size_t* const* src_ids, size_t n_src, kvbm_layout_handle dst,
+                                                           const size_t* dst_ids, size_t n_dst, size_t token_begin, size_t token_end,
+                                                           const kvbm_head_window* windows, size_t num_windows, const kvbm_layer_stream* ls,
+                                                           const kvbm_transfer_options* opts, kvbm_notification* out)
+{
+  return guarded([&]() -> int {
+  if (!m) return fail(KVBM_ERR, "null manager");
+  if (out) *out = 0;
+  if (int rc = check_layer_stream_shape(ls, num_srcs)) return rc;
+  return execute_repage_gather(m, num_srcs, srcs, src_ids, n_src, dst, dst_ids, n_dst, token_begin, token_end, windows, num_windows, opts, out,
+                               ls);
   });
 }
 

@@ -12,6 +12,8 @@
 #include <cstdio>
 #include <vector>
 
+static bool eager_module_loading();
+
 namespace kvbm {
 
 // ------------------------------------------------------------------------------------------------
@@ -850,6 +852,160 @@ kvbm_paged_repage_gather_kernel(const __grid_constant__ RepageGatherParams P, Ro
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// Layer streaming of the permuting and re-paging gathers (kvbm_permute_stream, spinning form).  The ungated kernels are one
+// CTA per unit in block-major order, scheduled by the hardware: gating them would fill the GPU with spinners that starve the
+// producer.  The gated kernels are a persistent grid instead: each CTA claims a batch of `batch` consecutive units per ticket
+// from the ticket word ctl[2] in LAYER-major order, waits once per layer it enters for that layer's flag of every source (warp
+// 0, wait_layer_ready's relaxed polls, acquire fence, timeout and abort word), walks each unit with the ungated kernel's
+// per-head loop, and publishes what it moved of a layer -- every thread fences its stores, one barrier, one arrive_layer with
+// the count -- when the batch ends and before it enters another layer.  So a CTA publishes every unit before it can wait on a
+// later layer: a receiver that releases layer l + 1 only after seeing layer l done cannot dead-lock against it.  The warps of a
+// CTA run on into the batch's next unit without waiting for each other.  The last CTA to finish runs arrive_transfer
+// (re-zeroes the workspace, done / completion flags, or 0xFFFFFFFF on abort).
+// ------------------------------------------------------------------------------------------------
+struct GateArgs {
+  StreamSync ss;  // ndst 1: the destination's layer_done / done flags; items = units; total_rings = CTAs
+  const uint32_t* ready[KVBM_GATHER_MAX_SOURCES];
+  int num_ready;
+};
+
+// Every source's ready flag of layer l, waited for by warp 0; the verdict goes to the whole CTA.  False: the transfer aborted.
+__device__ __forceinline__ bool gate_layer(const GateArgs& A, uint32_t l, uint32_t* s_ok)
+{
+  if (threadIdx.x < 32) {
+    bool ok = true;
+    for (int s = 0; s < A.num_ready && ok; ++s) {
+      StreamSync w = A.ss;
+      w.layer_ready = A.ready[s];
+      ok = wait_layer_ready(w, static_cast<int>(l), threadIdx.x);
+    }
+    if (threadIdx.x == 0) *s_ok = ok ? 1u : 0u;
+  }
+  __syncthreads();
+  return *s_ok != 0;
+}
+
+// `count` units of layer l are done: their stores are visible at gpu scope before thread 0 counts them (arrive_layer's acq_rel
+// atomic; the CTA that completes a layer adds the system-scope fence before the flag).  The barrier also ends every thread's
+// reads of the shared claim word.
+__device__ __forceinline__ void publish_units(const GateArgs& A, uint32_t l, uint32_t count)
+{
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0 && A.ss.want_layers && count != 0) arrive_layer(A.ss, static_cast<int>(l), count);
+}
+
+// The claim / gate / publish loop of both gated kernels over units [0, total): layer_of(u) is unit u's absolute layer,
+// walk(u, l) moves it.
+template <class LayerOf, class Walk>
+__device__ __forceinline__ void gated_units(const GateArgs& A, uint32_t total, uint32_t batch, LayerOf layer_of, Walk walk)
+{
+  __shared__ uint32_t s_ticket, s_ok;
+  uint32_t entered = UINT32_MAX;
+  for (;;) {
+    if (threadIdx.x == 0) s_ticket = atomicAdd(A.ss.ctl + 2, 1u);
+    __syncthreads();
+    const uint64_t first = static_cast<uint64_t>(s_ticket) * batch;
+    if (first >= total) break;
+    const uint32_t last = static_cast<uint32_t>(min(first + batch, static_cast<uint64_t>(total)));
+    uint32_t pending = 0;
+    bool aborted = false;
+    for (uint32_t u = static_cast<uint32_t>(first); u < last; ++u) {
+      const uint32_t l = layer_of(u);
+      if (l != entered) {
+        if (pending != 0) publish_units(A, entered, pending);
+        pending = 0;
+        if (!gate_layer(A, l, &s_ok)) {
+          aborted = true;
+          break;
+        }
+        entered = l;
+      }
+      walk(u, l);
+      ++pending;
+    }
+    if (aborted) break;
+    publish_units(A, entered, pending);
+  }
+  if (threadIdx.x == 0) arrive_transfer(A.ss);
+}
+
+// kvbm_paged_gather_kernel's unit walk behind the gate; unit = (l * num_blocks + pair) * no + o over the layer range.
+template <int CAST, bool POW2, bool SCALED>
+__global__ void __launch_bounds__(256, 1)
+kvbm_gated_gather_kernel(const __grid_constant__ GatherParams P, const __grid_constant__ GateArgs A, uint32_t num_blocks, uint32_t layer_begin,
+                         uint32_t nlayers, uint32_t no, uint32_t nt, RowSplit r, const float* scales, uint32_t batch)
+{
+  const uint32_t per_layer = num_blocks * no;
+  gated_units(A, per_layer * nlayers, batch, [&](uint32_t u) { return layer_begin + u / per_layer; }, [&](uint32_t u, uint32_t l) {
+    const uint32_t rem = u - (l - layer_begin) * per_layer;
+    const uint32_t pair = rem / no, o = rem - pair * no;
+    auto base_of = [&](const PermuteSide& X) {
+      return reinterpret_cast<uint8_t*>(static_cast<uintptr_t>(__ldg(X.layer_base + (X.universal ? 0 : l)))) +
+             static_cast<uint64_t>(__ldg(X.ids + pair)) * X.block_stride + l * X.layer_step + o * X.outer_step;
+    };
+    uint8_t* db = base_of(P.D);
+    const ptx::Scale scale = ptx::make_scale(SCALED ? __ldg(scales + l * no + o) : 1.f);
+    for (uint32_t j = threadIdx.x >> 5; j < P.covered; j += blockDim.x >> 5) {
+      const GatherSource& G = P.src[P.entry[j]];
+      const uint32_t h = j - G.first;
+      walk_head_rows<CAST, POW2, SCALED>(base_of(G.S) + G.s_win, G.S.head_stride, G.S.tok_stride, db + G.d_win, P.D.head_stride,
+                                         P.D.tok_stride, h, 1, h + 1, nt, r, scale);
+    }
+  });
+}
+
+// kvbm_paged_repage_gather_kernel's unit walk behind the gate; unit = (l * num_big + j) * no + o over the layer range.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__global__ void __launch_bounds__(256)
+kvbm_gated_repage_gather_kernel(const __grid_constant__ RepageGatherParams P, const __grid_constant__ GateArgs A, uint32_t num_big, RowSplit r,
+                                const float* scales, uint32_t batch)
+{
+  constexpr int IN = CAST == KVBM_CAST_BF16_TO_FP8E4M3 ? 2 : 1;
+  constexpr int OUT = CAST == KVBM_CAST_FP8E4M3_TO_BF16 ? 2 : 1;
+  const RepageGeom& G = P.geo;
+  const PermuteSide& D = P.g.D;
+  const uint32_t per_layer = num_big * G.no;
+  gated_units(A, per_layer * G.nlayers, batch, [&](uint32_t u) { return G.layer_begin + u / per_layer; }, [&](uint32_t u, uint32_t l) {
+    const uint32_t rem = u - (l - G.layer_begin) * per_layer;
+    const uint32_t j = rem / G.no, o = rem - j * G.no;
+    const uint32_t first = (G.big_first + j) * G.big_page;
+    const uint32_t t0 = max(G.token_begin, first), t1 = min(G.token_end, first + G.big_page);
+    const uint32_t q0 = t0 - first;
+    const uint32_t small_k = (G.big_first + j) * G.ratio - G.small_first;
+    auto region = [&](const PermuteSide& X) {
+      return reinterpret_cast<const uint8_t*>(static_cast<uintptr_t>(__ldg(X.layer_base + (X.universal ? 0 : l)))) + l * X.layer_step +
+             o * X.outer_step;
+    };
+    const uint8_t* d_region = region(D);
+    const ptx::Scale scale = ptx::make_scale(SCALED ? __ldg(scales + l * G.no + o) : 1.f);
+    const uint32_t run = row_run<POW2>(r, t1 - t0);
+    const uint32_t big_shift = G.src_small ? 3 + OUT : 3 + IN, small_shift = G.src_small ? 3 + IN : 3 + OUT;
+    for (uint32_t k = threadIdx.x >> 5; k < P.g.covered; k += blockDim.x >> 5) {
+      const GatherSource& S = P.g.src[P.g.entry[k]];
+      const uint32_t h = k - S.first;
+      const uint8_t* sh = region(S.S) + S.s_win + h * S.S.head_stride;
+      const uint8_t* dh = d_region + S.d_win + h * D.head_stride;
+      const bool ss = G.src_small;
+      const PermuteSide& B = ss ? D : S.S;
+      const PermuteSide& Sm = ss ? S.S : D;
+      const uint8_t* bh = (ss ? dh : sh) + static_cast<uint64_t>(__ldg(B.ids + j)) * B.block_stride;
+      repage_head_rows<CAST, POW2, SCALED, PPOW2>(bh, static_cast<uint32_t>(B.tok_stride), big_shift, ss ? sh : dh, Sm.ids, small_k,
+                                                  Sm.block_stride, static_cast<uint32_t>(Sm.tok_stride), small_shift, G, q0, run, r, scale);
+    }
+  });
+}
+
+// The stream-wait form's signal after layer l: its layer-done flag, and after the last layer the done and completion flags.
+__global__ void kvbm_layer_signal_kernel(uint32_t* layer_done, uint32_t* done, uint32_t epoch, uint32_t* completion, uint32_t completion_value)
+{
+  __threadfence_system();
+  if (layer_done) ptx::st_release_sys(layer_done, epoch);
+  if (done) ptx::st_release_sys(done, epoch);
+  if (completion) ptx::st_release_sys(completion, completion_value);
+}
+
 // The instantiation of the permuting kernels a launch takes for its cast mode, row split and scales: calls
 // f(integral_constant<int, CAST>, bool_constant<POW2>, bool_constant<SCALED>).  Scales without a cast take the unscaled
 // instantiation (the launch rejects them first), so no scaled kernel exists without a cast.  preload_kernels() passes every
@@ -1016,7 +1172,11 @@ static cudaError_t preload_kernels()
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_kernel<c, p, sc, false>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_gather_kernel<c, p, sc, true>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_gather_kernel<c, p, sc, false>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_gather_kernel<c, p, sc>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_gather_kernel<c, p, sc, true>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_gather_kernel<c, p, sc, false>);
         });
+  if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_layer_signal_kernel);
   return e;
 }
 
@@ -1110,14 +1270,115 @@ static bool fill_gather_sources(const kvbm_permute_source* srcs, int num_srcs, u
   return true;
 }
 
+// The gate's own argument rules (kvbm_permute_stream), checked before anything else of a streamed entry: a descriptor, a known
+// gate mode, a workspace when the caller asks for the spinning form, and a ready-flag array for every used source.
+static bool stream_args_ok(const kvbm_permute_stream* st, int num_srcs)
+{
+  if (!st || st->gate_mode < KVBM_GATE_AUTO || st->gate_mode > KVBM_GATE_STREAM_WAIT) return false;
+  if (st->gate_mode == KVBM_GATE_SPIN && !st->sync_workspace) return false;
+  for (int s = 0; s < num_srcs && s < KVBM_GATHER_MAX_SOURCES; ++s)
+    if (!st->layer_ready_flags[s]) return false;
+  return true;
+}
+
+// The form of a streamed launch, after every argument check: 1 spinning, 2 stream-wait (kvbm_paged_copy_v2's rule for gate_mode),
+// 0 with *err set when neither can run.  Loads every kernel of the library first (device_info), as the paged copy's gate does.
+static int gate_form(const kvbm_permute_stream& st, cudaError_t* err)
+{
+  DeviceInfo di;
+  if ((*err = device_info(&di)) != cudaSuccess) return 0;
+  bool spin = st.gate_mode == KVBM_GATE_SPIN || (st.gate_mode == KVBM_GATE_AUTO && eager_module_loading());
+  if (!spin && !stream_memops()) {
+    if (st.gate_mode != KVBM_GATE_AUTO) {
+      *err = cudaErrorNotSupported;
+      return 0;
+    }
+    spin = true;
+  }
+  if (spin && !st.sync_workspace) {  // AUTO chose the spinning form, whose abort word and counters live in the workspace
+    *err = cudaErrorInvalidValue;
+    return 0;
+  }
+  return spin ? 1 : 2;
+}
+
+// The spinning form's default grid: half the SMs.  A spinning CTA holds its SM for the whole prefill, and an SM that already runs
+// a CTA of one kernel does not always take a CTA of another (a shared-memory carveout of its own, for one): with a spinning CTA
+// on every SM of an H100 a producer's one-thread layer kernel never started and the gate timed out.  Half the SMs leaves the
+// engine at least as many SMs as the transfer holds, wherever the CTAs are placed.
+static int gate_default_ctas(const DeviceInfo& di) { return std::max(1, di.sm_count / 2); }
+
+// The spinning form's grid (max_ctas, 0 = gate_default_ctas, never more CTAs than units), its batch (units per ticket: about
+// half a CTA's share of a layer, 1 .. 8) and its StreamSync: the workspace's [nl] layer counters and 3 control words, the units
+// of one layer per layer, the destination's flags as the one flag destination.
+static cudaError_t gate_args(const kvbm_permute_stream& st, int num_srcs, uint32_t nl, int layer_begin, int layer_end, uint64_t units,
+                             GateArgs* A, unsigned* grid, uint32_t* batch)
+{
+  DeviceInfo di;
+  cudaError_t e = device_info(&di);
+  if (e != cudaSuccess) return e;
+  const int cap = st.max_ctas > 0 ? st.max_ctas : gate_default_ctas(di);
+  *grid = static_cast<unsigned>(std::min<uint64_t>(units, static_cast<uint64_t>(cap)));
+  const uint64_t per_layer = units / static_cast<uint64_t>(layer_end - layer_begin);
+  *batch = static_cast<uint32_t>(std::min<uint64_t>(8, std::max<uint64_t>(1, (per_layer + 2ull * *grid - 1) / (2ull * *grid))));
+  *A = GateArgs{};
+  StreamSync& ss = A->ss;
+  ss.gate = true;
+  ss.layer_counters = st.sync_workspace;
+  ss.ctl = st.sync_workspace + nl;
+  ss.done_flag[0] = st.done_flag;
+  ss.layer_done[0] = st.layer_done_flags;
+  ss.completion_flag = st.completion_flag;
+  ss.completion_value = st.completion_value;
+  ss.epoch = st.epoch;
+  ss.total_rings = *grid;
+  ss.items_per_layer = static_cast<uint32_t>(units / static_cast<uint64_t>(layer_end - layer_begin));
+  ss.ndst = 1;
+  ss.layer_begin = layer_begin;
+  ss.layer_end = layer_end;
+  ss.gate_timeout_ns = static_cast<uint64_t>(st.gate_timeout_ms > 0 ? st.gate_timeout_ms : 10000) * 1000000ull;
+  ss.want_layers = st.layer_done_flags != nullptr;
+  ss.want_done = st.done_flag != nullptr || st.completion_flag != nullptr;
+  for (int s = 0; s < num_srcs; ++s) A->ready[s] = st.layer_ready_flags[s];
+  A->num_ready = num_srcs;
+  return cudaSuccess;
+}
+
+// The stream-wait form: per layer, the stream waits for every source's flag (cuStreamWaitValue32, GEQ: the cyclic order of
+// epoch_reached), launch_layer(l) moves the layer unsignalled, and one signal launch writes its layer-done flag, plus the done
+// and completion flags after the last layer.  Nothing resident spins.
+template <class F>
+static cudaError_t stream_wait_layers(const kvbm_permute_stream& st, int num_srcs, int layer_begin, int layer_end, cudaStream_t stream,
+                                      F&& launch_layer)
+{
+  for (int l = layer_begin; l < layer_end; ++l) {
+    for (int s = 0; s < num_srcs; ++s)
+      if (g_wait32(stream, reinterpret_cast<unsigned long long>(st.layer_ready_flags[s] + l), st.epoch, 0) != 0) return cudaErrorUnknown;
+    cudaError_t e = launch_layer(l);
+    if (e != cudaSuccess) return e;
+    const bool last = l + 1 == layer_end;
+    uint32_t* done = last ? st.done_flag : nullptr;
+    uint32_t* completion = last ? st.completion_flag : nullptr;
+    uint32_t* layer_done = st.layer_done_flags ? st.layer_done_flags + l : nullptr;
+    if (layer_done || done || completion) {
+      kvbm_layer_signal_kernel<<<1, 1, 0, stream>>>(layer_done, done, st.epoch, completion, st.completion_value);
+      g_launches.fetch_add(1, std::memory_order_relaxed);
+      if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    }
+  }
+  return cudaSuccess;
+}
+
 // Every permuting launch: a head transform is one source, a gather several.  Runs the checks of both entries once, signals
 // when there is nothing to move, and launches kvbm_paged_permute_kernel for one source (the faster of the two, DESIGN §4.2b) or
 // kvbm_paged_gather_kernel for several.  max_covered: how many destination heads the sources may cover together; at most
-// KVBM_GATHER_MAX_HEADS (the gather's head map) whenever num_srcs > 1.
+// KVBM_GATHER_MAX_HEADS (the gather's head map) whenever num_srcs > 1.  st: a streamed launch (its flags are the ones passed),
+// which takes the gated gather kernel, or per layer this launch unstreamed.
 static cudaError_t launch_paged_permute(const kvbm_permute_source* srcs, int num_srcs, const kvbm_permute_side* dst, uint32_t dst_num_heads,
                                         int num_blocks, int layer_begin, int layer_end, uint32_t page_size, uint32_t src_row_bytes,
                                         int cast_mode, const float* cast_scales, uint32_t* done_flag, uint32_t epoch,
-                                        uint32_t* completion_flag, uint32_t completion_value, uint32_t max_covered, cudaStream_t stream)
+                                        uint32_t* completion_flag, uint32_t completion_value, uint32_t max_covered, cudaStream_t stream,
+                                        const kvbm_permute_stream* st = nullptr)
 {
   if (num_blocks < 0 || layer_begin < 0 || layer_end < layer_begin) return cudaErrorInvalidValue;
   if (!cast_args_ok(cast_mode, cast_scales)) return cudaErrorInvalidValue;
@@ -1140,6 +1401,26 @@ static cudaError_t launch_paged_permute(const kvbm_permute_source* srcs, int num
   const int threads = static_cast<int>(std::min<uint32_t>(8, covered)) * 32;
   const unsigned grid = static_cast<unsigned>(units);
   const uint32_t lb = static_cast<uint32_t>(layer_begin), nlay = static_cast<uint32_t>(layer_end - layer_begin);
+  if (st) {
+    cudaError_t e;
+    const int form = gate_form(*st, &e);
+    if (form == 0) return e;
+    if (form == 2)
+      return stream_wait_layers(*st, num_srcs, layer_begin, layer_end, stream, [&](int l) {
+        return launch_paged_permute(srcs, num_srcs, dst, dst_num_heads, num_blocks, l, l + 1, page_size, src_row_bytes, cast_mode, cast_scales,
+                                    nullptr, 0, nullptr, 0, max_covered, stream);
+      });
+    GateArgs A;
+    unsigned ctas;
+    uint32_t batch;
+    if ((e = gate_args(*st, num_srcs, nl, layer_begin, layer_end, units, &A, &ctas, &batch)) != cudaSuccess) return e;
+    with_walk_kernel(cast_mode, r.pow2, cast_scales != nullptr, [&](auto c, auto p, auto sc) {
+      kvbm_gated_gather_kernel<c, p, sc><<<ctas, threads, 0, stream>>>(P, A, static_cast<uint32_t>(num_blocks), lb, nlay, no, page_size, r,
+                                                                       cast_scales, batch);
+    });
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    return cudaGetLastError();
+  }
   with_walk_kernel(cast_mode, r.pow2, cast_scales != nullptr, [&](auto c, auto p, auto sc) {
     const GatherSource& G = P.src[0];
     if (num_srcs == 1)
@@ -1242,11 +1523,12 @@ static cudaError_t launch_paged_repage(const kvbm_permute_side* src, uint32_t sr
 
 // kvbm_kernels_paged_repage_gather: the checks of launch_paged_permute's sources and of launch_paged_repage's pages, each side's
 // region at its own page and head count, all before any CUDA call; the signal on an empty range; then one launch and the signal.
+// st: a streamed launch, as launch_paged_permute's.
 static cudaError_t launch_paged_repage_gather(const kvbm_permute_source* srcs, int num_srcs, uint32_t src_page, const kvbm_permute_side* dst,
                                               uint32_t dst_num_heads, uint32_t dst_page, uint32_t token_begin, uint32_t token_end,
                                               int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
                                               uint32_t* done_flag, uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value,
-                                              cudaStream_t stream)
+                                              cudaStream_t stream, const kvbm_permute_stream* st = nullptr)
 {
   if (layer_begin < 0 || layer_end < layer_begin || token_end < token_begin) return cudaErrorInvalidValue;
   if (!cast_args_ok(cast_mode, cast_scales)) return cudaErrorInvalidValue;
@@ -1269,6 +1551,29 @@ static cudaError_t launch_paged_repage_gather(const kvbm_permute_source* srcs, i
   P.geo.nh = P.g.covered;
   const int threads = static_cast<int>(std::min<uint32_t>(8, P.g.covered)) * 32;
   const unsigned grid = static_cast<unsigned>(units);
+  if (st) {
+    cudaError_t e;
+    const int form = gate_form(*st, &e);
+    if (form == 0) return e;
+    if (form == 2)
+      return stream_wait_layers(*st, num_srcs, layer_begin, layer_end, stream, [&](int l) {
+        return launch_paged_repage_gather(srcs, num_srcs, src_page, dst, dst_num_heads, dst_page, token_begin, token_end, l, l + 1,
+                                          src_row_bytes, cast_mode, cast_scales, nullptr, 0, nullptr, 0, stream);
+      });
+    GateArgs A;
+    unsigned ctas;
+    uint32_t batch;
+    if ((e = gate_args(*st, num_srcs, nl, layer_begin, layer_end, units, &A, &ctas, &batch)) != cudaSuccess) return e;
+    const uint32_t num_big = static_cast<uint32_t>(units / (static_cast<uint64_t>(P.geo.nlayers) * no));
+    with_walk_kernel(cast_mode, r.pow2, cast_scales != nullptr, [&](auto c, auto p, auto sc) {
+      if (page_pow2)
+        kvbm_gated_repage_gather_kernel<c, p, sc, true><<<ctas, threads, 0, stream>>>(P, A, num_big, r, cast_scales, batch);
+      else
+        kvbm_gated_repage_gather_kernel<c, p, sc, false><<<ctas, threads, 0, stream>>>(P, A, num_big, r, cast_scales, batch);
+    });
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    return cudaGetLastError();
+  }
   with_walk_kernel(cast_mode, r.pow2, cast_scales != nullptr, [&](auto c, auto p, auto sc) {
     if (page_pow2)
       kvbm_paged_repage_gather_kernel<c, p, sc, true><<<grid, threads, 0, stream>>>(P, r, cast_scales);
@@ -1486,6 +1791,29 @@ kvbm_kernels_paged_repage_gather(const kvbm_permute_source* srcs, int num_srcs, 
   return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, token_begin, token_end, layer_begin,
                                     layer_end, src_row_bytes, cast_mode, cast_scales, done_flag, epoch, completion_flag, completion_value,
                                     stream);
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_permute_gather_streamed(const kvbm_permute_source* srcs, int num_srcs, const kvbm_permute_side* dst, uint32_t dst_num_heads,
+                                           int num_blocks, int layer_begin, int layer_end, uint32_t page_size, uint32_t src_row_bytes,
+                                           int cast_mode, const float* cast_scales, const kvbm_permute_stream* st, cudaStream_t stream)
+{
+  if (!stream_args_ok(st, num_srcs)) return cudaErrorInvalidValue;
+  return launch_paged_permute(srcs, num_srcs, dst, dst_num_heads, num_blocks, layer_begin, layer_end, page_size, src_row_bytes, cast_mode,
+                              cast_scales, st->done_flag, st->epoch, st->completion_flag, st->completion_value, KVBM_GATHER_MAX_HEADS, stream,
+                              st);
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_repage_gather_streamed(const kvbm_permute_source* srcs, int num_srcs, uint32_t src_page_size, const kvbm_permute_side* dst,
+                                          uint32_t dst_num_heads, uint32_t dst_page_size, uint32_t token_begin, uint32_t token_end,
+                                          int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
+                                          const kvbm_permute_stream* st, cudaStream_t stream)
+{
+  if (!stream_args_ok(st, num_srcs)) return cudaErrorInvalidValue;
+  return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, token_begin, token_end, layer_begin,
+                                    layer_end, src_row_bytes, cast_mode, cast_scales, st->done_flag, st->epoch, st->completion_flag,
+                                    st->completion_value, stream, st);
 }
 
 extern "C" bool

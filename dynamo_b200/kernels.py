@@ -108,6 +108,22 @@ GATHER_MAX_SOURCES = 16      # KVBM_GATHER_MAX_SOURCES
 GATHER_MAX_HEADS = 256       # KVBM_GATHER_MAX_HEADS
 
 
+class PermuteStream(C.Structure):
+    """struct kvbm_permute_stream: the gate of `paged_permute_gather_streamed` / `paged_repage_gather_streamed`"""
+    _fields_ = [
+        ("layer_ready_flags", C.c_void_p * GATHER_MAX_SOURCES),  # per source (srcs[] index): its [num_layers] ready flags
+        ("layer_done_flags", C.c_void_p),
+        ("done_flag", C.c_void_p),
+        ("epoch", C.c_uint32),
+        ("sync_workspace", C.c_void_p),   # u32[sync_workspace_words(num_layers)], zeroed (spinning form)
+        ("completion_flag", C.c_void_p),
+        ("completion_value", C.c_uint32),
+        ("gate_mode", C.c_int),
+        ("gate_timeout_ms", C.c_int),
+        ("max_ctas", C.c_int),
+    ]
+
+
 class PagedCopyOpts(C.Structure):
     """struct kvbm_paged_copy_opts"""
     _fields_ = [
@@ -184,6 +200,13 @@ def lib() -> C.CDLL:
                                                        C.c_uint32, C.c_uint32, C.c_uint32, i, i, C.c_uint32, i, vp, vp, C.c_uint32, vp,
                                                        C.c_uint32, vp]
         L.kvbm_kernels_paged_repage_gather.restype = i
+        L.kvbm_kernels_paged_permute_gather_streamed.argtypes = [C.POINTER(PermuteSource), i, C.POINTER(PermuteSide), C.c_uint32, i, i, i,
+                                                                 C.c_uint32, C.c_uint32, i, vp, C.POINTER(PermuteStream), vp]
+        L.kvbm_kernels_paged_permute_gather_streamed.restype = i
+        L.kvbm_kernels_paged_repage_gather_streamed.argtypes = [C.POINTER(PermuteSource), i, C.c_uint32, C.POINTER(PermuteSide), C.c_uint32,
+                                                                C.c_uint32, C.c_uint32, C.c_uint32, i, i, C.c_uint32, i, vp,
+                                                                C.POINTER(PermuteStream), vp]
+        L.kvbm_kernels_paged_repage_gather_streamed.restype = i
         L.kvbm_kernels_permute_strides.argtypes = [i, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64, C.c_uint64,
                                                    C.POINTER(C.c_uint64)]
         L.kvbm_kernels_permute_strides.restype = i
@@ -207,7 +230,8 @@ EXPORTED_SYMBOLS = [
     "kvbm_kernels_launch_count", "kvbm_kernels_build_info", "kvbm_kernels_gate_would_spin", "kvbm_kernels_paged_permute",
     "kvbm_kernels_permute_strides", "kvbm_kernels_paged_permute_cast", "kvbm_kernels_paged_permute_heads",
     "kvbm_kernels_paged_permute_gather", "kvbm_kernels_paged_permute_heads_scaled", "kvbm_kernels_paged_permute_gather_scaled",
-    "kvbm_kernels_paged_repage", "kvbm_kernels_paged_repage_gather",
+    "kvbm_kernels_paged_repage", "kvbm_kernels_paged_repage_gather", "kvbm_kernels_paged_permute_gather_streamed",
+    "kvbm_kernels_paged_repage_gather_streamed",
 ]
 
 
@@ -357,6 +381,29 @@ def paged_repage_gather(srcs: Sequence[PermuteSource], src_page_size: int, dst: 
     return lib().kvbm_kernels_paged_repage_gather(arr, len(srcs), src_page_size, C.byref(dst), dst_num_heads, dst_page_size, token_begin,
                                                   token_end, layer_begin, layer_end, src_row_bytes, int(cast_mode), scales_ptr(cast_scales),
                                                   done_flag or None, epoch, completion_flag or None, completion_value, stream)
+
+
+def paged_permute_gather_streamed(srcs: Sequence[PermuteSource], dst: PermuteSide, dst_num_heads: int, num_blocks: int, layer_begin: int,
+                                  layer_end: int, page_size: int, src_row_bytes: int, cast_mode: int, cast_scales,
+                                  st: Optional[PermuteStream], stream: int = 0) -> int:
+    """`paged_permute_gather` streamed layer by layer behind `st`'s ready flags (one array per source); the flags of `st` replace the
+    done / completion arguments.  One source with a full window is a format change, one with a partial window a re-shard.
+    include/kvbm_kernels.h (kvbm_kernels_paged_permute_gather_streamed)."""
+    arr = (PermuteSource * max(1, len(srcs)))(*srcs)
+    return lib().kvbm_kernels_paged_permute_gather_streamed(arr, len(srcs), C.byref(dst), dst_num_heads, num_blocks, layer_begin, layer_end,
+                                                            page_size, src_row_bytes, int(cast_mode), scales_ptr(cast_scales),
+                                                            C.byref(st) if st is not None else None, stream)
+
+
+def paged_repage_gather_streamed(srcs: Sequence[PermuteSource], src_page_size: int, dst: PermuteSide, dst_num_heads: int,
+                                 dst_page_size: int, token_begin: int, token_end: int, layer_begin: int, layer_end: int, src_row_bytes: int,
+                                 cast_mode: int, cast_scales, st: Optional[PermuteStream], stream: int = 0) -> int:
+    """`paged_repage_gather` streamed as `paged_permute_gather_streamed`; one full-window source is `paged_repage`.
+    include/kvbm_kernels.h (kvbm_kernels_paged_repage_gather_streamed)."""
+    arr = (PermuteSource * max(1, len(srcs)))(*srcs)
+    return lib().kvbm_kernels_paged_repage_gather_streamed(arr, len(srcs), src_page_size, C.byref(dst), dst_num_heads, dst_page_size,
+                                                           token_begin, token_end, layer_begin, layer_end, src_row_bytes, int(cast_mode),
+                                                           scales_ptr(cast_scales), C.byref(st) if st is not None else None, stream)
 
 
 def permute_strides(kv_layout: int, num_layers: int, outer_dim: int, num_heads: int, page_size: int, row_bytes: int,

@@ -118,6 +118,11 @@ class _CHeadWindow(C.Structure):
     _fields_ = [(n, C.c_size_t) for n in ("src_rank", "src_head_begin", "dst_head_begin", "head_count")]
 
 
+class _CLayerStream(C.Structure):
+    """struct kvbm_layer_stream"""
+    _fields_ = [("src_layer_ready_flags", C.c_void_p), ("num_srcs", C.c_size_t), ("layer_done_flags", C.c_void_p)]
+
+
 @dataclass
 class LayoutConfig:
     num_blocks: int
@@ -231,7 +236,7 @@ EXPORTED_SYMBOLS = [
     "kvbm_mc_supported", "kvbm_mc_group_create", "kvbm_mc_group_export_fd", "kvbm_mc_group_import_fd",
     "kvbm_mc_group_size", "kvbm_mc_group_add_device", "kvbm_mc_group_bind_local", "kvbm_mc_group_bind_addr", "kvbm_mc_group_map",
     "kvbm_mc_group_destroy", "kvbm_tp_reshard_plan", "kvbm_manager_execute_gather", "kvbm_manager_execute_repage",
-    "kvbm_manager_execute_repage_gather",
+    "kvbm_manager_execute_repage_gather", "kvbm_manager_execute_gather_streamed", "kvbm_manager_execute_repage_gather_streamed",
 ]
 
 
@@ -283,6 +288,10 @@ def lib() -> C.CDLL:
         L.kvbm_manager_execute_repage.argtypes = [vp, u64, vp, sz, u64, vp, sz, sz, sz, P(_COptions), P(u64)]
         L.kvbm_manager_execute_repage_gather.argtypes = [vp, sz, P(u64), P(P(sz)), sz, u64, vp, sz, sz, sz, P(_CHeadWindow), sz,
                                                          P(_COptions), P(u64)]
+        L.kvbm_manager_execute_gather_streamed.argtypes = [vp, sz, P(u64), P(P(sz)), u64, vp, sz, P(_CHeadWindow), sz, P(_CLayerStream),
+                                                           P(_COptions), P(u64)]
+        L.kvbm_manager_execute_repage_gather_streamed.argtypes = [vp, sz, P(u64), P(P(sz)), sz, u64, vp, sz, sz, sz, P(_CHeadWindow), sz,
+                                                                  P(_CLayerStream), P(_COptions), P(u64)]
         L.kvbm_notification_is_complete.argtypes = [vp, u64]
         L.kvbm_notification_wait.argtypes = [vp, u64, C.c_int64]
         L.kvbm_manager_bytes_moved.argtypes = [vp]
@@ -598,28 +607,64 @@ class TransferManager:
             notes.append(self.execute_transfer(h, ids, dst, dst_block_ids, o))
         return notes
 
+    @staticmethod
+    def _gather_args(sources: Mapping[int, tuple], ranks: Sequence[int], dst_block_ids: Sequence[int], plan: Sequence[HeadWindow]):
+        """The C arguments of a gather: the plan's source ranks in `ranks` order (the C sources), their handles and id lists, the
+        destination's ids and count, the windows with src_rank as an index into `ranks`.  The id arrays are returned so that they
+        outlive the call."""
+        index = {r: i for i, r in enumerate(ranks)}
+        hs = (C.c_uint64 * max(1, len(ranks)))(*[sources[r][0] for r in ranks])
+        s_arrays = [_size_array(sources[r][1])[0] for r in ranks]
+        d, nd = _size_array(dst_block_ids)
+        PP = C.POINTER(C.c_size_t)
+        as_ptr = lambda a: a._as_parameter_ if isinstance(a, _NpView) else C.cast(a, PP)  # noqa: E731
+        sp = (PP * max(1, len(ranks)))(*[as_ptr(a) for a in s_arrays])
+        ws = (_CHeadWindow * max(1, len(plan)))(*[_CHeadWindow(index[w.src_rank], w.src_head_begin, w.dst_head_begin, w.head_count)
+                                                  for w in plan])
+        return hs, s_arrays, sp, d.addr if type(d) is _NpView else d, nd, ws
+
+    @staticmethod
+    def _layer_stream(ranks: Sequence[int], ready_flags: Mapping[int, int], layer_done_flags: int) -> "_CLayerStream":
+        """struct kvbm_layer_stream for the plan's source ranks; a rank missing from `ready_flags` passes NULL (rejected)."""
+        flags = (C.c_void_p * max(1, len(ranks)))(*[int(ready_flags.get(r, 0)) or None for r in ranks])
+        ls = _CLayerStream(C.cast(flags, C.c_void_p), len(ranks), layer_done_flags or None)
+        ls._keep = flags
+        return ls
+
     def execute_gather(self, sources: Mapping[int, tuple], dst: int, dst_block_ids: Sequence[int], plan: Sequence[HeadWindow],
                        options: Optional[TransferOptions] = None) -> TransferCompleteNotification:
         """`execute_reshard` as ONE hand-off (kvbm_manager_execute_gather): the same `sources` mapping (source rank -> (layout
         handle, block ids)) and plan, at most 16 windows, moved by one permuting launch.  Returns one notification, and
         `options.done_flag` is written once, after every window's bytes landed.  `options.head_window` must be None."""
         ranks = sorted({w.src_rank for w in plan})
-        index = {r: i for i, r in enumerate(ranks)}
         n = len(dst_block_ids)
         if any(len(sources[r][1]) != n for r in ranks):
             raise KvbmError(ErrorCode.LENGTH_MISMATCH, "Block ID lists have mismatched lengths")
-        hs = (C.c_uint64 * max(1, len(ranks)))(*[sources[r][0] for r in ranks])
-        s_arrays = [_size_array(sources[r][1])[0] for r in ranks]
-        d, _ = _size_array(dst_block_ids)
-        PP = C.POINTER(C.c_size_t)
-        as_ptr = lambda a: a._as_parameter_ if isinstance(a, _NpView) else C.cast(a, PP)  # noqa: E731
-        sp = (PP * max(1, len(ranks)))(*[as_ptr(a) for a in s_arrays])
-        ws = (_CHeadWindow * max(1, len(plan)))(*[_CHeadWindow(index[w.src_rank], w.src_head_begin, w.dst_head_begin, w.head_count)
-                                                  for w in plan])
+        hs, _keep, sp, d, n, ws = self._gather_args(sources, ranks, dst_block_ids, plan)
         tok = C.c_uint64()
         o = (options or TransferOptions())._c()
-        _check(lib().kvbm_manager_execute_gather(self._h, len(ranks), hs, sp, dst, d.addr if type(d) is _NpView else d, n, ws, len(plan),
-                                                 C.byref(o), C.byref(tok)))
+        _check(lib().kvbm_manager_execute_gather(self._h, len(ranks), hs, sp, dst, d, n, ws, len(plan), C.byref(o), C.byref(tok)))
+        return TransferCompleteNotification(self, tok.value)
+
+    def execute_gather_streamed(self, sources: Mapping[int, tuple], dst: int, dst_block_ids: Sequence[int], plan: Sequence[HeadWindow],
+                                ready_flags: Mapping[int, int], options: Optional[TransferOptions] = None,
+                                layer_done_flags: int = 0) -> TransferCompleteNotification:
+        """`execute_gather` streamed layer by layer (kvbm_manager_execute_gather_streamed): `ready_flags` maps a source rank to
+        the address of its [num_layers] u32 ready flags, and layer l of that source is read only after its flag l has reached
+        `options.epoch`; `layer_done_flags` (an address on the destination, or 0) gets entry l = epoch once layer l of every
+        window landed.  A one-window plan streams a plain format change (a window over every head of both sides) or a single
+        re-shard window.  Options: those of `execute_gather`, plus epoch, gate_mode, gate_timeout_ms, max_ctas and done_flag; the
+        options' own layer flags stay rejected.  The bytes and bytes_moved are `execute_gather`'s."""
+        ranks = sorted({w.src_rank for w in plan})
+        n = len(dst_block_ids)
+        if any(len(sources[r][1]) != n for r in ranks):
+            raise KvbmError(ErrorCode.LENGTH_MISMATCH, "Block ID lists have mismatched lengths")
+        hs, _keep, sp, d, n, ws = self._gather_args(sources, ranks, dst_block_ids, plan)
+        ls = self._layer_stream(ranks, ready_flags, layer_done_flags)
+        tok = C.c_uint64()
+        o = (options or TransferOptions())._c()
+        _check(lib().kvbm_manager_execute_gather_streamed(self._h, len(ranks), hs, sp, dst, d, n, ws, len(plan), C.byref(ls), C.byref(o),
+                                                          C.byref(tok)))
         return TransferCompleteNotification(self, tok.value)
 
     def execute_repage(self, src: int, src_block_ids: Sequence[int], dst: int, dst_block_ids: Sequence[int], tokens: range,
@@ -650,22 +695,33 @@ class TransferManager:
         if tokens.step != 1:
             raise ValueError("tokens must be a range with step 1")
         ranks = sorted({w.src_rank for w in plan})
-        index = {r: i for i, r in enumerate(ranks)}
         n_src = len(sources[ranks[0]][1]) if ranks else 0
         if any(len(sources[r][1]) != n_src for r in ranks):
             raise KvbmError(ErrorCode.LENGTH_MISMATCH, "the sources' block id lists have different lengths")
-        hs = (C.c_uint64 * max(1, len(ranks)))(*[sources[r][0] for r in ranks])
-        s_arrays = [_size_array(sources[r][1])[0] for r in ranks]
-        d, n_dst = _size_array(dst_block_ids)
-        PP = C.POINTER(C.c_size_t)
-        as_ptr = lambda a: a._as_parameter_ if isinstance(a, _NpView) else C.cast(a, PP)  # noqa: E731
-        sp = (PP * max(1, len(ranks)))(*[as_ptr(a) for a in s_arrays])
-        ws = (_CHeadWindow * max(1, len(plan)))(*[_CHeadWindow(index[w.src_rank], w.src_head_begin, w.dst_head_begin, w.head_count)
-                                                  for w in plan])
+        hs, _keep, sp, d, n_dst, ws = self._gather_args(sources, ranks, dst_block_ids, plan)
         tok = C.c_uint64()
         o = (options or TransferOptions())._c()
-        _check(lib().kvbm_manager_execute_repage_gather(self._h, len(ranks), hs, sp, n_src, dst, d.addr if type(d) is _NpView else d, n_dst,
-                                                        tokens.start, tokens.stop, ws, len(plan), C.byref(o), C.byref(tok)))
+        _check(lib().kvbm_manager_execute_repage_gather(self._h, len(ranks), hs, sp, n_src, dst, d, n_dst, tokens.start, tokens.stop, ws,
+                                                        len(plan), C.byref(o), C.byref(tok)))
+        return TransferCompleteNotification(self, tok.value)
+
+    def execute_repage_gather_streamed(self, sources: Mapping[int, tuple], dst: int, dst_block_ids: Sequence[int],
+                                       plan: Sequence[HeadWindow], tokens: range, ready_flags: Mapping[int, int],
+                                       options: Optional[TransferOptions] = None, layer_done_flags: int = 0) -> TransferCompleteNotification:
+        """`execute_repage_gather` streamed layer by layer (kvbm_manager_execute_repage_gather_streamed), with the flags of
+        `execute_gather_streamed`.  A one-window plan over every head of both sides streams a plain re-page."""
+        if tokens.step != 1:
+            raise ValueError("tokens must be a range with step 1")
+        ranks = sorted({w.src_rank for w in plan})
+        n_src = len(sources[ranks[0]][1]) if ranks else 0
+        if any(len(sources[r][1]) != n_src for r in ranks):
+            raise KvbmError(ErrorCode.LENGTH_MISMATCH, "the sources' block id lists have different lengths")
+        hs, _keep, sp, d, n_dst, ws = self._gather_args(sources, ranks, dst_block_ids, plan)
+        ls = self._layer_stream(ranks, ready_flags, layer_done_flags)
+        tok = C.c_uint64()
+        o = (options or TransferOptions())._c()
+        _check(lib().kvbm_manager_execute_repage_gather_streamed(self._h, len(ranks), hs, sp, n_src, dst, d, n_dst, tokens.start,
+                                                                 tokens.stop, ws, len(plan), C.byref(ls), C.byref(o), C.byref(tok)))
         return TransferCompleteNotification(self, tok.value)
 
     def execute_fanout(self, src: int, dsts: Sequence[int], src_block_ids: Sequence[Sequence[int]],

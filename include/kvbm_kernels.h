@@ -328,6 +328,62 @@ cudaError_t kvbm_kernels_paged_repage_gather(const kvbm_permute_source* srcs, in
                                              uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value,
                                              cudaStream_t stream);
 
+/* ---- layer streaming of the layout-transforming hand-offs ------------------------------------------------------------------
+ * The gate of kvbm_kernels_paged_permute_gather_streamed / kvbm_kernels_paged_repage_gather_streamed.  Layer l of source s
+ * (srcs[] index) is read only after layer_ready_flags[s][l] has reached `epoch` (the cyclic order of kvbm_paged_copy_opts.epoch).
+ * One CTA writes every window of a destination unit, so a unit at layer l waits for flag l of EVERY source.
+ *
+ * Two forms, chosen by gate_mode with kvbm_paged_copy_opts.gate_mode's rule (KVBM_GATE_AUTO spins only under eager module
+ * loading, and falls back to spinning when stream memory operations are missing; KVBM_GATE_STREAM_WAIT without them is
+ * cudaErrorNotSupported):
+ *  - spinning: ONE launch of a persistent grid of max_ctas CTAs (0 = half the SMs) that claims batches of (block, layer,
+ *    outer) units in layer-major order from the workspace's ticket word, waits once per layer it enters (gate_timeout_ms, 0 = 10 s: a longer
+ *    wait aborts the transfer: done_flag is not written and completion_flag becomes 0xFFFFFFFF), publishes each finished unit
+ *    before it waits on a later layer, and writes the done flags itself -- no trailing signal launch.  Needs sync_workspace.
+ *  - stream-wait: per layer, cuStreamWaitValue32 (GEQ) on each source's flag, the unstreamed launch over [l, l + 1) and a
+ *    one-thread signal launch; nothing resident spins.  max_ctas, gate_timeout_ms and sync_workspace do not apply.  The wait has
+ *    no timeout, and it holds the device's hardware queue that `stream` maps to, not just `stream`: when the process uses more
+ *    streams than the device has queues (CUDA_DEVICE_MAX_CONNECTIONS, 8 by default), a producer stream that shares the queue
+ *    and releases the flags later never runs.  Release the flags from another process or device, from a stream created before
+ *    the others share queues, or raise CUDA_DEVICE_MAX_CONNECTIONS.
+ * Either way layer_done_flags[l] is written (epoch, system scope) once every byte of layer l landed, and done_flag (epoch) /
+ * completion_flag (completion_value) after the last byte.  The destination bytes are those of the unstreamed entry. */
+typedef struct kvbm_permute_stream {
+  const uint32_t* layer_ready_flags[KVBM_GATHER_MAX_SOURCES]; /* per source (srcs[] index), [num_layers] each; non-null for s < num_srcs */
+  uint32_t* layer_done_flags; /* nullable, [num_layers], the destination's: entry l = epoch once layer l landed */
+  uint32_t* done_flag;        /* nullable */
+  uint32_t epoch;
+  uint32_t* sync_workspace;   /* device u32[KVBM_SYNC_WORKSPACE_WORDS(num_layers)], zeroed, left zeroed (spinning form) */
+  uint32_t* completion_flag;  /* nullable */
+  uint32_t completion_value;
+  int gate_mode;              /* KVBM_GATE_AUTO / SPIN / STREAM_WAIT */
+  int gate_timeout_ms;        /* spinning form only; 0 = 10 s */
+  int max_ctas;               /* spinning form only: persistent grid size, 0 = half the SMs.  A spinning CTA holds its SM for the
+                                 whole prefill, and an SM running one may not take another kernel's CTA (with a spinning CTA on
+                                 every SM of an H100 a producer's layer kernel never started): values near the SM count can
+                                 starve a producer on the same GPU until the gate times out */
+} kvbm_permute_stream;
+
+/* kvbm_kernels_paged_permute_gather_scaled, streamed layer by layer behind `st`'s ready flags.  One source with a full window is a
+ * format change (with or without a cast), one source with a partial window a re-shard, several sources a gather; the destination
+ * bytes equal the unstreamed call's bit for bit.  Every argument rule of kvbm_kernels_paged_permute_gather_scaled applies (its
+ * KVBM_GATHER_MAX_HEADS covered heads also to one source).  cudaErrorInvalidValue, before any CUDA call, also for a null `st`, a
+ * null ready-flag array of a used source, a gate_mode out of range and the spinning form without sync_workspace (KVBM_GATE_SPIN
+ * before any CUDA call; KVBM_GATE_AUTO once it has chosen that form).  An empty block or layer range waits for nothing and writes
+ * done_flag and completion_flag at once, as the unstreamed entry does; it writes no layer_done_flags. */
+cudaError_t kvbm_kernels_paged_permute_gather_streamed(const kvbm_permute_source* srcs, int num_srcs, const kvbm_permute_side* dst,
+                                                       uint32_t dst_num_heads, int num_blocks, int layer_begin, int layer_end,
+                                                       uint32_t page_size, uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
+                                                       const kvbm_permute_stream* st, cudaStream_t stream);
+
+/* kvbm_kernels_paged_repage_gather, streamed as kvbm_kernels_paged_permute_gather_streamed is.  One source with a full window is
+ * kvbm_kernels_paged_repage.  Its argument rules are kvbm_kernels_paged_repage_gather's plus the gate's above. */
+cudaError_t kvbm_kernels_paged_repage_gather_streamed(const kvbm_permute_source* srcs, int num_srcs, uint32_t src_page_size,
+                                                      const kvbm_permute_side* dst, uint32_t dst_num_heads, uint32_t dst_page_size,
+                                                      uint32_t token_begin, uint32_t token_end, int layer_begin, int layer_end,
+                                                      uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
+                                                      const kvbm_permute_stream* st, cudaStream_t stream);
+
 /* Host-only (no GPU): the stride table kvbm_kernels_paged_permute walks with for one side.  out[0] = 1 when offsets count
  * from the block's first byte (universal formats) or 0 when they count from the (layer, outer) region's first byte; the
  * element (layer l, outer o, head h, token t) then sits at  [out[0] ? l * out[1] + o * out[2] : 0] + h * out[3] + t * out[4].

@@ -330,6 +330,39 @@ int kvbm_manager_execute_repage_gather(kvbm_transfer_manager* m, size_t num_srcs
                                        size_t n_dst, size_t token_begin, size_t token_end, const kvbm_head_window* windows,
                                        size_t num_windows, const kvbm_transfer_options* opts, kvbm_notification* out);
 
+/* Layer streaming of a gather or re-paging gather: the per-layer flags, the only way to pass them to these transfers. */
+typedef struct kvbm_layer_stream {
+  const uint32_t* const* src_layer_ready_flags; /* [num_srcs], indexed like srcs: source s's [num_layers] ready flags; layer l of
+                                                   source s is read once flag l has reached opts->epoch (kvbm_paged_copy_opts.epoch's
+                                                   cyclic order) */
+  size_t num_srcs;
+  uint32_t* layer_done_flags;                   /* nullable, [num_layers], on the destination: entry l = epoch once layer l landed */
+} kvbm_layer_stream;
+
+/* kvbm_manager_execute_gather, streamed layer by layer: every window's layer l is read only after its source's ready flag l has
+ * reached opts->epoch, and layer_done_flags[l] is written once every window's layer l landed.  A one-window plan streams a plain
+ * format change (a window over every head of both sides) or a single re-shard window.  Validation is execute_gather's, with its
+ * codes and texts (the options' own layer_ready_flags / layer_done_flags / per_dst_* / multicast stay rejected); before it,
+ * KVBM_ERR for a NULL ls, a NULL flag table or a NULL entry, and KVBM_ERR_LENGTH_MISMATCH for ls->num_srcs != num_srcs; after
+ * it, KVBM_ERR for a flag array the manager's device cannot reach: allowed are its own memory, memory of a device whose peer
+ * access was enabled through kvbm_manager_enable_peer_access or by an IPC mapping this manager opened, and mapped pinned host
+ * memory.  Honoured on top of execute_gather's options: epoch, gate_mode,
+ * gate_timeout_ms, max_ctas and done_flag (see kvbm_permute_stream for the two gate forms).  The notification completes as a
+ * gated execute_transfer's, with KVBM_ERR_TIMEOUT after the spinning form gave up on a flag.  The destination bytes and
+ * bytes_moved equal execute_gather's.  At most KVBM_GATHER_MAX_HEADS covered heads, also with one window. */
+int kvbm_manager_execute_gather_streamed(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs,
+                                         const size_t* const* src_ids, kvbm_layout_handle dst, const size_t* dst_ids, size_t n,
+                                         const kvbm_head_window* windows, size_t num_windows, const kvbm_layer_stream* ls,
+                                         const kvbm_transfer_options* opts, kvbm_notification* out);
+
+/* kvbm_manager_execute_repage_gather, streamed as kvbm_manager_execute_gather_streamed is; one window over every head of both
+ * sides streams a plain re-page.  Validation is execute_repage_gather's, with the same additions. */
+int kvbm_manager_execute_repage_gather_streamed(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs,
+                                                const size_t* const* src_ids, size_t n_src, kvbm_layout_handle dst, const size_t* dst_ids,
+                                                size_t n_dst, size_t token_begin, size_t token_end, const kvbm_head_window* windows,
+                                                size_t num_windows, const kvbm_layer_stream* ls, const kvbm_transfer_options* opts,
+                                                kvbm_notification* out);
+
 /* Completion: the transfer's last warp writes a flag in pinned host memory (no cudaEventQuery polling). */
 int kvbm_notification_is_complete(kvbm_transfer_manager* m, kvbm_notification n);  /* 1 / 0 / <0 error */
 int kvbm_notification_wait(kvbm_transfer_manager* m, kvbm_notification n, int64_t timeout_us);
