@@ -597,6 +597,21 @@ kvbm_permute_table_kernel(void* const* __restrict__ universal_ptrs, void* const*
   }
 }
 
+// The (layer l, outer o) region of a side of a paged transform, before any block offset.
+__device__ __forceinline__ uint8_t* side_region(const PermuteSide& X, uint32_t l, uint32_t o)
+{
+  return reinterpret_cast<uint8_t*>(static_cast<uintptr_t>(__ldg(X.layer_base + (X.universal ? 0 : l)))) + l * X.layer_step +
+         o * X.outer_step;
+}
+
+// The same region in block ids[i] of the side's table.  The sum is written out in this order rather than as side_region() plus
+// the block offset: the other order costs the paged permute up to 15 more registers (53 -> 68 uncast).
+__device__ __forceinline__ uint8_t* side_block(const PermuteSide& X, uint32_t i, uint32_t l, uint32_t o)
+{
+  return reinterpret_cast<uint8_t*>(static_cast<uintptr_t>(__ldg(X.layer_base + (X.universal ? 0 : l)))) +
+         static_cast<uint64_t>(__ldg(X.ids + i)) * X.block_stride + l * X.layer_step + o * X.outer_step;
+}
+
 // Paged permute: the walk with the bases computed from the pools' layouts and block tables instead of host-built pointer
 // tables, for any pair of KvBlockLayouts, optionally casting (CAST: KVBM_CAST_*; each side's strides are for its own row and
 // its own head count).  nh heads of every unit move: source heads from s_win / head_stride on, destination heads from
@@ -613,13 +628,9 @@ kvbm_paged_permute_kernel(const __grid_constant__ PermuteSide S, const __grid_co
   const uint32_t pair = unit / (nlayers * no);
   const uint32_t rem = unit - pair * (nlayers * no);
   const uint32_t l = layer_begin + rem / no, o = rem % no;
-  auto base_of = [&](const PermuteSide& X) {
-    return reinterpret_cast<uint8_t*>(static_cast<uintptr_t>(__ldg(X.layer_base + (X.universal ? 0 : l)))) +
-           static_cast<uint64_t>(__ldg(X.ids + pair)) * X.block_stride + l * X.layer_step + o * X.outer_step;
-  };
   const ptx::Scale scale = ptx::make_scale(SCALED ? __ldg(scales + l * no + o) : 1.f);
-  walk_head_rows<CAST, POW2, SCALED>(base_of(S) + s_win, S.head_stride, S.tok_stride, base_of(D) + d_win, D.head_stride, D.tok_stride,
-                                     threadIdx.x >> 5, blockDim.x >> 5, nh, nt, r, scale);
+  walk_head_rows<CAST, POW2, SCALED>(side_block(S, pair, l, o) + s_win, S.head_stride, S.tok_stride, side_block(D, pair, l, o) + d_win,
+                                     D.head_stride, D.tok_stride, threadIdx.x >> 5, blockDim.x >> 5, nh, nt, r, scale);
 }
 
 // The gather: several sources, each with its own pool, format, head count and head window, into one destination.  The
@@ -637,10 +648,25 @@ struct GatherParams {
   uint32_t covered;
 };
 
-// One CTA per destination (block, layer, outer) unit, as the paged permute, with one warp per covered destination head
-// (looping by the CTA's warps past 8): every source's window of the unit is written by the same CTA, so a destination row
+// One destination (block, layer, outer) unit of the gather, block `pair` of the tables, with one warp per covered destination
+// head (looping by the CTA's warps past 8): every source's window of the unit is written by the same CTA, so a destination row
 // that holds every head (OperationalNHD) is written whole by one CTA.  Each warp looks up its source and runs the same walk
-// over one head.  SCALED: one scale array for every source, scales[l * no + o] loaded once per CTA.
+// over one head.  SCALED: one scale array for every source, scales[l * no + o] loaded once per unit.
+template <int CAST, bool POW2, bool SCALED>
+__device__ __forceinline__ void gather_unit(const GatherParams& P, uint32_t pair, uint32_t l, uint32_t o, uint32_t no, uint32_t nt,
+                                            const RowSplit& r, const float* scales)
+{
+  uint8_t* db = side_block(P.D, pair, l, o);
+  const ptx::Scale scale = ptx::make_scale(SCALED ? __ldg(scales + l * no + o) : 1.f);
+  for (uint32_t j = threadIdx.x >> 5; j < P.covered; j += blockDim.x >> 5) {
+    const GatherSource& G = P.src[P.entry[j]];
+    const uint32_t h = j - G.first;  // head h of the window: walk heads h .. h of the window's bases
+    walk_head_rows<CAST, POW2, SCALED>(side_block(G.S, pair, l, o) + G.s_win, G.S.head_stride, G.S.tok_stride, db + G.d_win,
+                                       P.D.head_stride, P.D.tok_stride, h, 1, h + 1, nt, r, scale);
+  }
+}
+
+// One CTA per destination unit, as the paged permute.
 template <int CAST, bool POW2, bool SCALED = false>
 __global__ void __launch_bounds__(256)
 kvbm_paged_gather_kernel(const __grid_constant__ GatherParams P, uint32_t layer_begin, uint32_t nlayers, uint32_t no, uint32_t nt, RowSplit r,
@@ -649,19 +675,7 @@ kvbm_paged_gather_kernel(const __grid_constant__ GatherParams P, uint32_t layer_
   const uint32_t unit = blockIdx.x;  // (pair * nlayers + l) * no + o
   const uint32_t pair = unit / (nlayers * no);
   const uint32_t rem = unit - pair * (nlayers * no);
-  const uint32_t l = layer_begin + rem / no, o = rem % no;
-  auto base_of = [&](const PermuteSide& X) {
-    return reinterpret_cast<uint8_t*>(static_cast<uintptr_t>(__ldg(X.layer_base + (X.universal ? 0 : l)))) +
-           static_cast<uint64_t>(__ldg(X.ids + pair)) * X.block_stride + l * X.layer_step + o * X.outer_step;
-  };
-  uint8_t* db = base_of(P.D);
-  const ptx::Scale scale = ptx::make_scale(SCALED ? __ldg(scales + l * no + o) : 1.f);
-  for (uint32_t j = threadIdx.x >> 5; j < P.covered; j += blockDim.x >> 5) {
-    const GatherSource& G = P.src[P.entry[j]];
-    const uint32_t h = j - G.first;  // head h of the window: walk heads h .. h of the window's bases
-    walk_head_rows<CAST, POW2, SCALED>(base_of(G.S) + G.s_win, G.S.head_stride, G.S.tok_stride, db + G.d_win, P.D.head_stride,
-                                       P.D.tok_stride, h, 1, h + 1, nt, r, scale);
-  }
+  gather_unit<CAST, POW2, SCALED>(P, pair, layer_begin + rem / no, rem % no, no, nt, r, scales);
 }
 
 // Re-paging: a token range [token_begin, token_end) of one sequence between two block tables whose page sizes differ (one divides
@@ -687,11 +701,23 @@ struct RepageParams {
   RepageGeom g;
 };
 
+// Big block j of the range (entry j of the big side's table), clipped to the token range: the slot q0 of its first token in
+// the range, its token count, and small_k, the small table's entry of its first small block.  small_k wraps below 0 in the
+// unit whose first small blocks lie before the range, and small_k + b (b >= those blocks) wraps back: index in uint32, never
+// offset the pointer by it.
+struct RepageUnit {
+  uint32_t q0, tokens, small_k;
+};
+__device__ __forceinline__ RepageUnit repage_unit(const RepageGeom& G, uint32_t j)
+{
+  const uint32_t first = (G.big_first + j) * G.big_page;  // sequence position of the big block's slot 0
+  const uint32_t t0 = max(G.token_begin, first), t1 = min(G.token_end, first + G.big_page);
+  return {t0 - first, t1 - t0, (G.big_first + j) * G.ratio - G.small_first};
+}
+
 // One head of a re-paging unit: its run of `run` 16 B vectors from slot q0 of the big block on.  bh: the head's rows in the
 // big block; sh: its rows in the small side's (layer, outer) region, before the block offset.  Small block b of the unit is
-// entry small_k + b of small_ids; small_k wraps below 0 in the unit whose first small blocks lie before the range, and
-// small_k + b (b >= those blocks) wraps back: index in uint32, never offset the pointer by it.  kvbm_paged_repage_kernel keeps
-// its own copy of this loop: calling the helper from it changes the register allocation of all 20 of its instantiations.
+// entry small_k + b of small_ids (RepageUnit).  Every re-paging kernel runs its heads through this loop.
 template <int CAST, bool POW2, bool SCALED, bool PPOW2>
 __device__ __forceinline__ void repage_head_rows(const uint8_t* bh, uint32_t big_tok, uint32_t big_shift, const uint8_t* sh,
                                                  const int32_t* small_ids, uint32_t small_k, uint64_t small_block_stride,
@@ -740,65 +766,23 @@ template <int CAST, bool POW2, bool SCALED, bool PPOW2>
 __global__ void __launch_bounds__(256)
 kvbm_paged_repage_kernel(const __grid_constant__ RepageParams P, RowSplit r, const float* scales)
 {
-  constexpr int IN = CAST == KVBM_CAST_BF16_TO_FP8E4M3 ? 2 : 1;   // 16 B loads per vector
-  constexpr int OUT = CAST == KVBM_CAST_FP8E4M3_TO_BF16 ? 2 : 1;  // 16 B stores per vector
-  constexpr int U = 8 / IN;
+  constexpr int IN = CAST == KVBM_CAST_BF16_TO_FP8E4M3 ? 2 : 1;
+  constexpr int OUT = CAST == KVBM_CAST_FP8E4M3_TO_BF16 ? 2 : 1;
   const uint32_t unit = blockIdx.x;  // (big block j * nlayers + l) * no + o
   const uint32_t j = unit / (P.g.nlayers * P.g.no);
   const uint32_t rem = unit - j * (P.g.nlayers * P.g.no);
   const uint32_t l = P.g.layer_begin + rem / P.g.no, o = rem % P.g.no;
-  const uint32_t first = (P.g.big_first + j) * P.g.big_page;  // sequence position of the big block's slot 0
-  const uint32_t t0 = max(P.g.token_begin, first), t1 = min(P.g.token_end, first + P.g.big_page);
-  const uint32_t q0 = t0 - first;
-  // small block b of this unit is entry small_k + b of the small table; small_k wraps below 0 in the unit whose first small
-  // blocks lie before the range, and small_k + b (b >= those blocks) wraps back: index in uint32, never offset the pointer by it
-  const uint32_t small_k = (P.g.big_first + j) * P.g.ratio - P.g.small_first;
-  const uint8_t* big_base = reinterpret_cast<uint8_t*>(static_cast<uintptr_t>(__ldg(P.big.layer_base + (P.big.universal ? 0 : l)))) +
-                            static_cast<uint64_t>(__ldg(P.big.ids + j)) * P.big.block_stride + l * P.big.layer_step + o * P.big.outer_step;
-  const uint8_t* small_base = reinterpret_cast<uint8_t*>(static_cast<uintptr_t>(__ldg(P.small.layer_base + (P.small.universal ? 0 : l)))) +
-                              l * P.small.layer_step + o * P.small.outer_step;
+  const RepageUnit u = repage_unit(P.g, j);
+  const uint8_t* big_base = side_block(P.big, j, l, o);
+  const uint8_t* small_base = side_region(P.small, l, o);
   const ptx::Scale scale = ptx::make_scale(SCALED ? __ldg(scales + l * P.g.no + o) : 1.f);
   // column shifts of either side: the source's vector is 16 * IN bytes, the destination's 16 * OUT
   const uint32_t big_shift = P.g.src_small ? 3 + OUT : 3 + IN, small_shift = P.g.src_small ? 3 + IN : 3 + OUT;
-  const uint32_t big_tok = static_cast<uint32_t>(P.big.tok_stride), small_tok = static_cast<uint32_t>(P.small.tok_stride);
-  const uint32_t run = row_run<POW2>(r, t1 - t0);
-  const int lane = threadIdx.x & 31;
-  for (uint32_t h = threadIdx.x >> 5; h < P.g.nh; h += blockDim.x >> 5) {
-    const uint8_t* bh = big_base + h * P.big.head_stride;
-    const uint8_t* sh = small_base + h * P.small.head_stride;
-    for (uint32_t v = lane; v < run; v += U * 32) {
-      uint4 x[U][IN];
-      uint8_t* dp[U];
-#pragma unroll
-      for (int k = 0; k < U; ++k)
-        if (v + k * 32 < run) {
-          const uint32_t vv = v + k * 32;
-          const uint32_t t = POW2 ? vv >> r.vpr : __umulhi(vv, r.magic);
-          const uint32_t c = POW2 ? vv & ((1u << r.vpr) - 1) : vv - t * r.vpr;
-          const uint32_t q = q0 + t;
-          const uint32_t b = PPOW2 ? q >> P.g.page.vpr : __umulhi(q, P.g.page.magic);
-          const uint32_t slot = PPOW2 ? q & (P.g.small_page - 1) : q - b * P.g.small_page;
-          const uint8_t* big_p = bh + q * big_tok + (c << big_shift);
-          const uint8_t* small_p = sh + static_cast<uint64_t>(__ldg(P.small.ids + (small_k + b))) * P.small.block_stride + slot * small_tok + (c << small_shift);
-          const uint8_t* s = P.g.src_small ? small_p : big_p;
-          dp[k] = const_cast<uint8_t*>(P.g.src_small ? big_p : small_p);
-#pragma unroll
-          for (int i = 0; i < IN; ++i) x[k][i] = ptx::ld_stream_v4(s + 16 * i);
-        }
-#pragma unroll
-      for (int k = 0; k < U; ++k)
-        if (v + k * 32 < run) {
-          if constexpr (CAST == KVBM_CAST_NONE) {
-            ptx::st_stream_v4(dp[k], x[k][0]);
-          } else {
-            uint4 y[OUT];
-            cast_vector<SCALED>(x[k], y, scale);  // bit for bit the paged permute's cast
-#pragma unroll
-            for (int i = 0; i < OUT; ++i) ptx::st_stream_v4(dp[k] + 16 * i, y[i]);
-          }
-        }
-    }
-  }
+  const uint32_t run = row_run<POW2>(r, u.tokens);
+  for (uint32_t h = threadIdx.x >> 5; h < P.g.nh; h += blockDim.x >> 5)
+    repage_head_rows<CAST, POW2, SCALED, PPOW2>(big_base + h * P.big.head_stride, static_cast<uint32_t>(P.big.tok_stride), big_shift,
+                                                small_base + h * P.small.head_stride, P.small.ids, u.small_k, P.small.block_stride,
+                                                static_cast<uint32_t>(P.small.tok_stride), small_shift, P.g, u.q0, run, r, scale);
 }
 
 // Re-paging and the gather in one launch: several sources with one page size Ps (a prefill TP group), each with its own pool,
@@ -814,42 +798,43 @@ struct RepageGatherParams {
   RepageGeom geo;
 };
 
+// Unit (big block j, layer l, outer o) of the re-paging gather.
 template <int CAST, bool POW2, bool SCALED, bool PPOW2>
-__global__ void __launch_bounds__(256)
-kvbm_paged_repage_gather_kernel(const __grid_constant__ RepageGatherParams P, RowSplit r, const float* scales)
+__device__ __forceinline__ void repage_gather_unit(const RepageGatherParams& P, uint32_t j, uint32_t l, uint32_t o, const RowSplit& r,
+                                                   const float* scales)
 {
   constexpr int IN = CAST == KVBM_CAST_BF16_TO_FP8E4M3 ? 2 : 1;
   constexpr int OUT = CAST == KVBM_CAST_FP8E4M3_TO_BF16 ? 2 : 1;
   const RepageGeom& G = P.geo;
   const PermuteSide& D = P.g.D;
-  const uint32_t unit = blockIdx.x;  // (big block j * nlayers + l) * no + o
-  const uint32_t j = unit / (G.nlayers * G.no);
-  const uint32_t rem = unit - j * (G.nlayers * G.no);
-  const uint32_t l = G.layer_begin + rem / G.no, o = rem % G.no;
-  const uint32_t first = (G.big_first + j) * G.big_page;
-  const uint32_t t0 = max(G.token_begin, first), t1 = min(G.token_end, first + G.big_page);
-  const uint32_t q0 = t0 - first;
-  const uint32_t small_k = (G.big_first + j) * G.ratio - G.small_first;
-  auto region = [&](const PermuteSide& X) {  // the (layer, outer) region of a side, before the block offset
-    return reinterpret_cast<const uint8_t*>(static_cast<uintptr_t>(__ldg(X.layer_base + (X.universal ? 0 : l)))) + l * X.layer_step +
-           o * X.outer_step;
-  };
-  const uint8_t* d_region = region(D);
+  const RepageUnit u = repage_unit(G, j);
+  const uint8_t* d_region = side_region(D, l, o);
   const ptx::Scale scale = ptx::make_scale(SCALED ? __ldg(scales + l * G.no + o) : 1.f);
   const uint32_t big_shift = G.src_small ? 3 + OUT : 3 + IN, small_shift = G.src_small ? 3 + IN : 3 + OUT;
-  const uint32_t run = row_run<POW2>(r, t1 - t0);
+  const uint32_t run = row_run<POW2>(r, u.tokens);
   for (uint32_t k = threadIdx.x >> 5; k < P.g.covered; k += blockDim.x >> 5) {
     const GatherSource& S = P.g.src[P.g.entry[k]];
     const uint32_t h = k - S.first;  // head h of the window
-    const uint8_t* sh = region(S.S) + S.s_win + h * S.S.head_stride;
+    const uint8_t* sh = side_region(S.S, l, o) + S.s_win + h * S.S.head_stride;
     const uint8_t* dh = d_region + S.d_win + h * D.head_stride;
     const bool ss = G.src_small;
     const PermuteSide& B = ss ? D : S.S;
     const PermuteSide& Sm = ss ? S.S : D;
     const uint8_t* bh = (ss ? dh : sh) + static_cast<uint64_t>(__ldg(B.ids + j)) * B.block_stride;
-    repage_head_rows<CAST, POW2, SCALED, PPOW2>(bh, static_cast<uint32_t>(B.tok_stride), big_shift, ss ? sh : dh, Sm.ids, small_k,
-                                                Sm.block_stride, static_cast<uint32_t>(Sm.tok_stride), small_shift, G, q0, run, r, scale);
+    repage_head_rows<CAST, POW2, SCALED, PPOW2>(bh, static_cast<uint32_t>(B.tok_stride), big_shift, ss ? sh : dh, Sm.ids, u.small_k,
+                                                Sm.block_stride, static_cast<uint32_t>(Sm.tok_stride), small_shift, G, u.q0, run, r, scale);
   }
+}
+
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__global__ void __launch_bounds__(256)
+kvbm_paged_repage_gather_kernel(const __grid_constant__ RepageGatherParams P, RowSplit r, const float* scales)
+{
+  const RepageGeom& G = P.geo;
+  const uint32_t unit = blockIdx.x;  // (big block j * nlayers + l) * no + o
+  const uint32_t j = unit / (G.nlayers * G.no);
+  const uint32_t rem = unit - j * (G.nlayers * G.no);
+  repage_gather_unit<CAST, POW2, SCALED, PPOW2>(P, j, G.layer_begin + rem / G.no, rem % G.no, r, scales);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -858,7 +843,7 @@ kvbm_paged_repage_gather_kernel(const __grid_constant__ RepageGatherParams P, Ro
 // producer.  The gated kernels are a persistent grid instead: each CTA claims a batch of `batch` consecutive units per ticket
 // from the ticket word ctl[2] in LAYER-major order, waits once per layer it enters for that layer's flag of every source (warp
 // 0, wait_layer_ready's relaxed polls, acquire fence, timeout and abort word), walks each unit with the ungated kernel's
-// per-head loop, and publishes what it moved of a layer -- every thread fences its stores, one barrier, one arrive_layer with
+// unit body (gather_unit / repage_gather_unit), and publishes what it moved of a layer -- every thread fences its stores, one barrier, one arrive_layer with
 // the count -- when the batch ends and before it enters another layer.  So a CTA publishes every unit before it can wait on a
 // later layer: a receiver that releases layer l + 1 only after seeing layer l done cannot dead-lock against it.  The warps of a
 // CTA run on into the batch's next unit without waiting for each other.  The last CTA to finish runs arrive_transfer
@@ -940,19 +925,8 @@ kvbm_gated_gather_kernel(const __grid_constant__ GatherParams P, const __grid_co
   const uint32_t per_layer = num_blocks * no;
   gated_units(A, per_layer * nlayers, batch, [&](uint32_t u) { return layer_begin + u / per_layer; }, [&](uint32_t u, uint32_t l) {
     const uint32_t rem = u - (l - layer_begin) * per_layer;
-    const uint32_t pair = rem / no, o = rem - pair * no;
-    auto base_of = [&](const PermuteSide& X) {
-      return reinterpret_cast<uint8_t*>(static_cast<uintptr_t>(__ldg(X.layer_base + (X.universal ? 0 : l)))) +
-             static_cast<uint64_t>(__ldg(X.ids + pair)) * X.block_stride + l * X.layer_step + o * X.outer_step;
-    };
-    uint8_t* db = base_of(P.D);
-    const ptx::Scale scale = ptx::make_scale(SCALED ? __ldg(scales + l * no + o) : 1.f);
-    for (uint32_t j = threadIdx.x >> 5; j < P.covered; j += blockDim.x >> 5) {
-      const GatherSource& G = P.src[P.entry[j]];
-      const uint32_t h = j - G.first;
-      walk_head_rows<CAST, POW2, SCALED>(base_of(G.S) + G.s_win, G.S.head_stride, G.S.tok_stride, db + G.d_win, P.D.head_stride,
-                                         P.D.tok_stride, h, 1, h + 1, nt, r, scale);
-    }
+    const uint32_t pair = rem / no;
+    gather_unit<CAST, POW2, SCALED>(P, pair, l, rem - pair * no, no, nt, r, scales);
   });
 }
 
@@ -962,38 +936,12 @@ __global__ void __launch_bounds__(256)
 kvbm_gated_repage_gather_kernel(const __grid_constant__ RepageGatherParams P, const __grid_constant__ GateArgs A, uint32_t num_big, RowSplit r,
                                 const float* scales, uint32_t batch)
 {
-  constexpr int IN = CAST == KVBM_CAST_BF16_TO_FP8E4M3 ? 2 : 1;
-  constexpr int OUT = CAST == KVBM_CAST_FP8E4M3_TO_BF16 ? 2 : 1;
   const RepageGeom& G = P.geo;
-  const PermuteSide& D = P.g.D;
   const uint32_t per_layer = num_big * G.no;
   gated_units(A, per_layer * G.nlayers, batch, [&](uint32_t u) { return G.layer_begin + u / per_layer; }, [&](uint32_t u, uint32_t l) {
     const uint32_t rem = u - (l - G.layer_begin) * per_layer;
-    const uint32_t j = rem / G.no, o = rem - j * G.no;
-    const uint32_t first = (G.big_first + j) * G.big_page;
-    const uint32_t t0 = max(G.token_begin, first), t1 = min(G.token_end, first + G.big_page);
-    const uint32_t q0 = t0 - first;
-    const uint32_t small_k = (G.big_first + j) * G.ratio - G.small_first;
-    auto region = [&](const PermuteSide& X) {
-      return reinterpret_cast<const uint8_t*>(static_cast<uintptr_t>(__ldg(X.layer_base + (X.universal ? 0 : l)))) + l * X.layer_step +
-             o * X.outer_step;
-    };
-    const uint8_t* d_region = region(D);
-    const ptx::Scale scale = ptx::make_scale(SCALED ? __ldg(scales + l * G.no + o) : 1.f);
-    const uint32_t run = row_run<POW2>(r, t1 - t0);
-    const uint32_t big_shift = G.src_small ? 3 + OUT : 3 + IN, small_shift = G.src_small ? 3 + IN : 3 + OUT;
-    for (uint32_t k = threadIdx.x >> 5; k < P.g.covered; k += blockDim.x >> 5) {
-      const GatherSource& S = P.g.src[P.g.entry[k]];
-      const uint32_t h = k - S.first;
-      const uint8_t* sh = region(S.S) + S.s_win + h * S.S.head_stride;
-      const uint8_t* dh = d_region + S.d_win + h * D.head_stride;
-      const bool ss = G.src_small;
-      const PermuteSide& B = ss ? D : S.S;
-      const PermuteSide& Sm = ss ? S.S : D;
-      const uint8_t* bh = (ss ? dh : sh) + static_cast<uint64_t>(__ldg(B.ids + j)) * B.block_stride;
-      repage_head_rows<CAST, POW2, SCALED, PPOW2>(bh, static_cast<uint32_t>(B.tok_stride), big_shift, ss ? sh : dh, Sm.ids, small_k,
-                                                  Sm.block_stride, static_cast<uint32_t>(Sm.tok_stride), small_shift, G, q0, run, r, scale);
-    }
+    const uint32_t j = rem / G.no;
+    repage_gather_unit<CAST, POW2, SCALED, PPOW2>(P, j, l, rem - j * G.no, r, scales);
   });
 }
 
@@ -1226,6 +1174,15 @@ static cudaError_t signal_launch(uint32_t* done_flag, uint32_t epoch, uint32_t* 
   return cudaGetLastError();
 }
 
+// The end of a transform's launch: count it, and return its launch error or, on success, the signal launch's.
+static cudaError_t launched(cudaStream_t stream, uint32_t* done_flag = nullptr, uint32_t epoch = 0, uint32_t* completion_flag = nullptr,
+                            uint32_t completion_value = 0)
+{
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  const cudaError_t e = cudaGetLastError();
+  return e != cudaSuccess ? e : signal_launch(done_flag, epoch, completion_flag, completion_value, stream);
+}
+
 // The walk splits the fp8 side's row into 16 B vectors when casting (the bf16 side's vectors are 32 B), else the row; an odd
 // bf16 row has no fp8 row.  Fills the destination's row and the row the walk counts vectors of.
 static bool cast_rows(uint32_t src_row_bytes, int cast_mode, uint64_t* dst_row_bytes, uint64_t* walk_row)
@@ -1344,26 +1301,37 @@ static cudaError_t gate_args(const kvbm_permute_stream& st, int num_srcs, uint32
   return cudaSuccess;
 }
 
-// The stream-wait form: per layer, the stream waits for every source's flag (cuStreamWaitValue32, GEQ: the cyclic order of
-// epoch_reached), launch_layer(l) moves the layer unsignalled, and one signal launch writes its layer-done flag, plus the done
-// and completion flags after the last layer.  Nothing resident spins.
-template <class F>
-static cudaError_t stream_wait_layers(const kvbm_permute_stream& st, int num_srcs, int layer_begin, int layer_end, cudaStream_t stream,
-                                      F&& launch_layer)
+// A streamed launch of `units` units over layers [layer_begin, layer_end) of an nl-layer destination, after every argument check.
+// The spinning form: launch_gated(A, ctas, batch) launches the gated kernel, which writes every flag itself.  The stream-wait
+// form: per layer, the stream waits for every source's flag (cuStreamWaitValue32, GEQ: the cyclic order of epoch_reached),
+// launch_layer(l) moves the layer unsignalled, and one signal launch writes its layer-done flag, plus the done and completion
+// flags after the last layer.  Nothing resident spins.
+template <class Layer, class Gated>
+static cudaError_t launch_streamed(const kvbm_permute_stream& st, int num_srcs, uint32_t nl, int layer_begin, int layer_end, uint64_t units,
+                                   cudaStream_t stream, Layer&& launch_layer, Gated&& launch_gated)
 {
+  cudaError_t e;
+  const int form = gate_form(st, &e);
+  if (form == 0) return e;
+  if (form == 1) {
+    GateArgs A;
+    unsigned ctas;
+    uint32_t batch;
+    if ((e = gate_args(st, num_srcs, nl, layer_begin, layer_end, units, &A, &ctas, &batch)) != cudaSuccess) return e;
+    launch_gated(A, ctas, batch);
+    return launched(stream);
+  }
   for (int l = layer_begin; l < layer_end; ++l) {
     for (int s = 0; s < num_srcs; ++s)
       if (g_wait32(stream, reinterpret_cast<unsigned long long>(st.layer_ready_flags[s] + l), st.epoch, 0) != 0) return cudaErrorUnknown;
-    cudaError_t e = launch_layer(l);
-    if (e != cudaSuccess) return e;
+    if ((e = launch_layer(l)) != cudaSuccess) return e;
     const bool last = l + 1 == layer_end;
     uint32_t* done = last ? st.done_flag : nullptr;
     uint32_t* completion = last ? st.completion_flag : nullptr;
     uint32_t* layer_done = st.layer_done_flags ? st.layer_done_flags + l : nullptr;
     if (layer_done || done || completion) {
       kvbm_layer_signal_kernel<<<1, 1, 0, stream>>>(layer_done, done, st.epoch, completion, st.completion_value);
-      g_launches.fetch_add(1, std::memory_order_relaxed);
-      if ((e = cudaGetLastError()) != cudaSuccess) return e;
+      if ((e = launched(stream)) != cudaSuccess) return e;
     }
   }
   return cudaSuccess;
@@ -1401,26 +1369,19 @@ static cudaError_t launch_paged_permute(const kvbm_permute_source* srcs, int num
   const int threads = static_cast<int>(std::min<uint32_t>(8, covered)) * 32;
   const unsigned grid = static_cast<unsigned>(units);
   const uint32_t lb = static_cast<uint32_t>(layer_begin), nlay = static_cast<uint32_t>(layer_end - layer_begin);
-  if (st) {
-    cudaError_t e;
-    const int form = gate_form(*st, &e);
-    if (form == 0) return e;
-    if (form == 2)
-      return stream_wait_layers(*st, num_srcs, layer_begin, layer_end, stream, [&](int l) {
-        return launch_paged_permute(srcs, num_srcs, dst, dst_num_heads, num_blocks, l, l + 1, page_size, src_row_bytes, cast_mode, cast_scales,
-                                    nullptr, 0, nullptr, 0, max_covered, stream);
-      });
-    GateArgs A;
-    unsigned ctas;
-    uint32_t batch;
-    if ((e = gate_args(*st, num_srcs, nl, layer_begin, layer_end, units, &A, &ctas, &batch)) != cudaSuccess) return e;
-    with_walk_kernel(cast_mode, r.pow2, cast_scales != nullptr, [&](auto c, auto p, auto sc) {
-      kvbm_gated_gather_kernel<c, p, sc><<<ctas, threads, 0, stream>>>(P, A, static_cast<uint32_t>(num_blocks), lb, nlay, no, page_size, r,
-                                                                       cast_scales, batch);
-    });
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    return cudaGetLastError();
-  }
+  if (st)
+    return launch_streamed(
+        *st, num_srcs, nl, layer_begin, layer_end, units, stream,
+        [&](int l) {
+          return launch_paged_permute(srcs, num_srcs, dst, dst_num_heads, num_blocks, l, l + 1, page_size, src_row_bytes, cast_mode,
+                                      cast_scales, nullptr, 0, nullptr, 0, max_covered, stream);
+        },
+        [&](const GateArgs& A, unsigned ctas, uint32_t batch) {
+          with_walk_kernel(cast_mode, r.pow2, cast_scales != nullptr, [&](auto c, auto p, auto sc) {
+            kvbm_gated_gather_kernel<c, p, sc><<<ctas, threads, 0, stream>>>(P, A, static_cast<uint32_t>(num_blocks), lb, nlay, no, page_size,
+                                                                             r, cast_scales, batch);
+          });
+        });
   with_walk_kernel(cast_mode, r.pow2, cast_scales != nullptr, [&](auto c, auto p, auto sc) {
     const GatherSource& G = P.src[0];
     if (num_srcs == 1)
@@ -1428,10 +1389,7 @@ static cudaError_t launch_paged_permute(const kvbm_permute_source* srcs, int num
     else
       kvbm_paged_gather_kernel<c, p, sc><<<grid, threads, 0, stream>>>(P, lb, nlay, no, page_size, r, cast_scales);
   });
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return e;
-  return signal_launch(done_flag, epoch, completion_flag, completion_value, stream);
+  return launched(stream, done_flag, epoch, completion_flag, completion_value);
 }
 
 // The geometry every re-paging launch shares, and its checks: non-zero pages, one dividing the other, slot arithmetic in 32 bits
@@ -1476,59 +1434,16 @@ static bool repage_geometry(uint32_t src_page, uint32_t dst_page, uint32_t token
   return true;
 }
 
-// kvbm_kernels_paged_repage: every check before any CUDA call, the signal on an empty range, then one re-paging launch and the
-// signal launch, as launch_paged_permute.
-static cudaError_t launch_paged_repage(const kvbm_permute_side* src, uint32_t src_page, const kvbm_permute_side* dst, uint32_t dst_page,
-                                       uint32_t token_begin, uint32_t token_end, int layer_begin, int layer_end, uint32_t nh,
-                                       uint32_t src_row_bytes, int cast_mode, const float* cast_scales, uint32_t* done_flag, uint32_t epoch,
-                                       uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
-{
-  if (layer_begin < 0 || layer_end < layer_begin || token_end < token_begin) return cudaErrorInvalidValue;
-  if (!cast_args_ok(cast_mode, cast_scales)) return cudaErrorInvalidValue;
-  if (token_end == token_begin || layer_end == layer_begin) return signal_launch(done_flag, epoch, completion_flag, completion_value, stream);
-  if (!src || !dst || !src->block_ids || !dst->block_ids || !src->layout.layer_base || !dst->layout.layer_base) return cudaErrorInvalidValue;
-  const uint32_t nl = dst->layout.num_layers, no = dst->layout.outer_dim;
-  if (nl == 0 || no == 0 || nh == 0 || src->layout.num_layers != nl || src->layout.outer_dim != no || static_cast<uint32_t>(layer_end) > nl)
-    return cudaErrorInvalidValue;
-  RepageParams P{};
-  RowSplit r;
-  uint64_t dst_row_bytes, units;
-  bool page_pow2;
-  if (!repage_geometry(src_page, dst_page, token_begin, token_end, layer_begin, layer_end, no, src_row_bytes, cast_mode, &P.g, &r,
-                       &dst_row_bytes, &units, &page_pow2))
-    return cudaErrorInvalidValue;
-  if (static_cast<uint64_t>(src_page) * nh * src_row_bytes != src->layout.region_bytes ||
-      static_cast<uint64_t>(dst_page) * nh * dst_row_bytes != dst->layout.region_bytes)
-    return cudaErrorInvalidValue;
-  PermuteSide S, D;
-  if (!fill_permute_side(*src, nl, no, nh, src_page, src_row_bytes, &S) ||
-      !fill_permute_side(*dst, nl, no, nh, dst_page, static_cast<uint32_t>(dst_row_bytes), &D))
-    return cudaErrorInvalidValue;
-  P.big = P.g.src_small ? D : S;
-  P.small = P.g.src_small ? S : D;
-  P.g.nh = nh;
-  const int threads = static_cast<int>(std::min<uint32_t>(8, nh)) * 32;
-  const unsigned grid = static_cast<unsigned>(units);
-  with_walk_kernel(cast_mode, r.pow2, cast_scales != nullptr, [&](auto c, auto p, auto sc) {
-    if (page_pow2)
-      kvbm_paged_repage_kernel<c, p, sc, true><<<grid, threads, 0, stream>>>(P, r, cast_scales);
-    else
-      kvbm_paged_repage_kernel<c, p, sc, false><<<grid, threads, 0, stream>>>(P, r, cast_scales);
-  });
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return e;
-  return signal_launch(done_flag, epoch, completion_flag, completion_value, stream);
-}
-
-// kvbm_kernels_paged_repage_gather: the checks of launch_paged_permute's sources and of launch_paged_repage's pages, each side's
-// region at its own page and head count, all before any CUDA call; the signal on an empty range; then one launch and the signal.
-// st: a streamed launch, as launch_paged_permute's.
+// Every re-paging launch: a plain re-page is one source whose window covers every head of both sides, a re-paging gather one
+// or more windows.  Runs the checks of launch_paged_permute's sources and of repage_geometry's pages, each side's region at its
+// own page and head count, all before any CUDA call; signals when there is nothing to move; then launches
+// kvbm_paged_repage_kernel for a plain re-page, else kvbm_paged_repage_gather_kernel, and the signal.  max_covered and st: as
+// launch_paged_permute's (st takes the gated re-paging gather kernel, or per layer this launch unstreamed).
 static cudaError_t launch_paged_repage_gather(const kvbm_permute_source* srcs, int num_srcs, uint32_t src_page, const kvbm_permute_side* dst,
                                               uint32_t dst_num_heads, uint32_t dst_page, uint32_t token_begin, uint32_t token_end,
                                               int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
                                               uint32_t* done_flag, uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value,
-                                              cudaStream_t stream, const kvbm_permute_stream* st = nullptr)
+                                              uint32_t max_covered, cudaStream_t stream, const kvbm_permute_stream* st = nullptr)
 {
   if (layer_begin < 0 || layer_end < layer_begin || token_end < token_begin) return cudaErrorInvalidValue;
   if (!cast_args_ok(cast_mode, cast_scales)) return cudaErrorInvalidValue;
@@ -1546,44 +1461,43 @@ static cudaError_t launch_paged_repage_gather(const kvbm_permute_source* srcs, i
     return cudaErrorInvalidValue;
   if (static_cast<uint64_t>(dst_page) * dst_num_heads * dst_row_bytes != dst->layout.region_bytes) return cudaErrorInvalidValue;
   if (!fill_permute_side(*dst, nl, no, dst_num_heads, dst_page, static_cast<uint32_t>(dst_row_bytes), &P.g.D)) return cudaErrorInvalidValue;
-  if (!fill_gather_sources(srcs, num_srcs, dst_num_heads, nl, no, src_page, src_row_bytes, KVBM_GATHER_MAX_HEADS, &P.g))
-    return cudaErrorInvalidValue;
+  if (!fill_gather_sources(srcs, num_srcs, dst_num_heads, nl, no, src_page, src_row_bytes, max_covered, &P.g)) return cudaErrorInvalidValue;
   P.geo.nh = P.g.covered;
   const int threads = static_cast<int>(std::min<uint32_t>(8, P.g.covered)) * 32;
   const unsigned grid = static_cast<unsigned>(units);
-  if (st) {
-    cudaError_t e;
-    const int form = gate_form(*st, &e);
-    if (form == 0) return e;
-    if (form == 2)
-      return stream_wait_layers(*st, num_srcs, layer_begin, layer_end, stream, [&](int l) {
-        return launch_paged_repage_gather(srcs, num_srcs, src_page, dst, dst_num_heads, dst_page, token_begin, token_end, l, l + 1,
-                                          src_row_bytes, cast_mode, cast_scales, nullptr, 0, nullptr, 0, stream);
-      });
-    GateArgs A;
-    unsigned ctas;
-    uint32_t batch;
-    if ((e = gate_args(*st, num_srcs, nl, layer_begin, layer_end, units, &A, &ctas, &batch)) != cudaSuccess) return e;
-    const uint32_t num_big = static_cast<uint32_t>(units / (static_cast<uint64_t>(P.geo.nlayers) * no));
-    with_walk_kernel(cast_mode, r.pow2, cast_scales != nullptr, [&](auto c, auto p, auto sc) {
-      if (page_pow2)
-        kvbm_gated_repage_gather_kernel<c, p, sc, true><<<ctas, threads, 0, stream>>>(P, A, num_big, r, cast_scales, batch);
-      else
-        kvbm_gated_repage_gather_kernel<c, p, sc, false><<<ctas, threads, 0, stream>>>(P, A, num_big, r, cast_scales, batch);
-    });
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    return cudaGetLastError();
-  }
+  if (st)
+    return launch_streamed(
+        *st, num_srcs, nl, layer_begin, layer_end, units, stream,
+        [&](int l) {
+          return launch_paged_repage_gather(srcs, num_srcs, src_page, dst, dst_num_heads, dst_page, token_begin, token_end, l, l + 1,
+                                            src_row_bytes, cast_mode, cast_scales, nullptr, 0, nullptr, 0, max_covered, stream);
+        },
+        [&](const GateArgs& A, unsigned ctas, uint32_t batch) {
+          const uint32_t num_big = static_cast<uint32_t>(units / (static_cast<uint64_t>(P.geo.nlayers) * no));
+          with_walk_kernel(cast_mode, r.pow2, cast_scales != nullptr, [&](auto c, auto p, auto sc) {
+            if (page_pow2)
+              kvbm_gated_repage_gather_kernel<c, p, sc, true><<<ctas, threads, 0, stream>>>(P, A, num_big, r, cast_scales, batch);
+            else
+              kvbm_gated_repage_gather_kernel<c, p, sc, false><<<ctas, threads, 0, stream>>>(P, A, num_big, r, cast_scales, batch);
+          });
+        });
+  // a window over every head of both sides (the checks above make both its starts 0)
+  const bool plain = num_srcs == 1 && srcs[0].head_count == srcs[0].num_heads && srcs[0].head_count == dst_num_heads;
+  RepageParams R{};
+  R.big = P.geo.src_small ? P.g.D : P.g.src[0].S;
+  R.small = P.geo.src_small ? P.g.src[0].S : P.g.D;
+  R.g = P.geo;
   with_walk_kernel(cast_mode, r.pow2, cast_scales != nullptr, [&](auto c, auto p, auto sc) {
-    if (page_pow2)
+    if (plain && page_pow2)
+      kvbm_paged_repage_kernel<c, p, sc, true><<<grid, threads, 0, stream>>>(R, r, cast_scales);
+    else if (plain)
+      kvbm_paged_repage_kernel<c, p, sc, false><<<grid, threads, 0, stream>>>(R, r, cast_scales);
+    else if (page_pow2)
       kvbm_paged_repage_gather_kernel<c, p, sc, true><<<grid, threads, 0, stream>>>(P, r, cast_scales);
     else
       kvbm_paged_repage_gather_kernel<c, p, sc, false><<<grid, threads, 0, stream>>>(P, r, cast_scales);
   });
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return e;
-  return signal_launch(done_flag, epoch, completion_flag, completion_value, stream);
+  return launched(stream, done_flag, epoch, completion_flag, completion_value);
 }
 
 }  // namespace kvbm
@@ -1778,8 +1692,10 @@ kvbm_kernels_paged_repage(const kvbm_permute_side* src, uint32_t src_page_size, 
                           uint32_t src_row_bytes, int cast_mode, const float* cast_scales, uint32_t* done_flag, uint32_t epoch,
                           uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
 {
-  return launch_paged_repage(src, src_page_size, dst, dst_page_size, token_begin, token_end, layer_begin, layer_end, num_heads,
-                             src_row_bytes, cast_mode, cast_scales, done_flag, epoch, completion_flag, completion_value, stream);
+  const kvbm_permute_source one{src ? *src : kvbm_permute_side{}, num_heads, 0, 0, num_heads};
+  return launch_paged_repage_gather(&one, 1, src_page_size, dst, num_heads, dst_page_size, token_begin, token_end, layer_begin, layer_end,
+                                    src_row_bytes, cast_mode, cast_scales, done_flag, epoch, completion_flag, completion_value, UINT32_MAX,
+                                    stream);
 }
 
 extern "C" cudaError_t
@@ -1790,7 +1706,7 @@ kvbm_kernels_paged_repage_gather(const kvbm_permute_source* srcs, int num_srcs, 
 {
   return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, token_begin, token_end, layer_begin,
                                     layer_end, src_row_bytes, cast_mode, cast_scales, done_flag, epoch, completion_flag, completion_value,
-                                    stream);
+                                    KVBM_GATHER_MAX_HEADS, stream);
 }
 
 extern "C" cudaError_t
@@ -1813,7 +1729,7 @@ kvbm_kernels_paged_repage_gather_streamed(const kvbm_permute_source* srcs, int n
   if (!stream_args_ok(st, num_srcs)) return cudaErrorInvalidValue;
   return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, token_begin, token_end, layer_begin,
                                     layer_end, src_row_bytes, cast_mode, cast_scales, st->done_flag, st->epoch, st->completion_flag,
-                                    st->completion_value, stream, st);
+                                    st->completion_value, KVBM_GATHER_MAX_HEADS, stream, st);
 }
 
 extern "C" bool

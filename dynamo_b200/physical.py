@@ -623,6 +623,24 @@ class TransferManager:
                                                   for w in plan])
         return hs, s_arrays, sp, d.addr if type(d) is _NpView else d, nd, ws
 
+    def _gather_call(self, sources: Mapping[int, tuple], dst_block_ids: Sequence[int], plan: Sequence[HeadWindow]):
+        """`execute_gather`'s source ranks, after its id-count check, and `_gather_args`."""
+        ranks = sorted({w.src_rank for w in plan})
+        n = len(dst_block_ids)
+        if any(len(sources[r][1]) != n for r in ranks):
+            raise KvbmError(ErrorCode.LENGTH_MISMATCH, "Block ID lists have mismatched lengths")
+        return ranks, self._gather_args(sources, ranks, dst_block_ids, plan)
+
+    def _repage_gather_call(self, sources: Mapping[int, tuple], dst_block_ids: Sequence[int], plan: Sequence[HeadWindow], tokens: range):
+        """`execute_repage_gather`'s source ranks and source id count, after its range and id-count checks, and `_gather_args`."""
+        if tokens.step != 1:
+            raise ValueError("tokens must be a range with step 1")
+        ranks = sorted({w.src_rank for w in plan})
+        n_src = len(sources[ranks[0]][1]) if ranks else 0
+        if any(len(sources[r][1]) != n_src for r in ranks):
+            raise KvbmError(ErrorCode.LENGTH_MISMATCH, "the sources' block id lists have different lengths")
+        return ranks, n_src, self._gather_args(sources, ranks, dst_block_ids, plan)
+
     @staticmethod
     def _layer_stream(ranks: Sequence[int], ready_flags: Mapping[int, int], layer_done_flags: int) -> "_CLayerStream":
         """struct kvbm_layer_stream for the plan's source ranks; a rank missing from `ready_flags` passes NULL (rejected)."""
@@ -636,11 +654,7 @@ class TransferManager:
         """`execute_reshard` as ONE hand-off (kvbm_manager_execute_gather): the same `sources` mapping (source rank -> (layout
         handle, block ids)) and plan, at most 16 windows, moved by one permuting launch.  Returns one notification, and
         `options.done_flag` is written once, after every window's bytes landed.  `options.head_window` must be None."""
-        ranks = sorted({w.src_rank for w in plan})
-        n = len(dst_block_ids)
-        if any(len(sources[r][1]) != n for r in ranks):
-            raise KvbmError(ErrorCode.LENGTH_MISMATCH, "Block ID lists have mismatched lengths")
-        hs, _keep, sp, d, n, ws = self._gather_args(sources, ranks, dst_block_ids, plan)
+        ranks, (hs, _keep, sp, d, n, ws) = self._gather_call(sources, dst_block_ids, plan)
         tok = C.c_uint64()
         o = (options or TransferOptions())._c()
         _check(lib().kvbm_manager_execute_gather(self._h, len(ranks), hs, sp, dst, d, n, ws, len(plan), C.byref(o), C.byref(tok)))
@@ -655,11 +669,7 @@ class TransferManager:
         window landed.  A one-window plan streams a plain format change (a window over every head of both sides) or a single
         re-shard window.  Options: those of `execute_gather`, plus epoch, gate_mode, gate_timeout_ms, max_ctas and done_flag; the
         options' own layer flags stay rejected.  The bytes and bytes_moved are `execute_gather`'s."""
-        ranks = sorted({w.src_rank for w in plan})
-        n = len(dst_block_ids)
-        if any(len(sources[r][1]) != n for r in ranks):
-            raise KvbmError(ErrorCode.LENGTH_MISMATCH, "Block ID lists have mismatched lengths")
-        hs, _keep, sp, d, n, ws = self._gather_args(sources, ranks, dst_block_ids, plan)
+        ranks, (hs, _keep, sp, d, n, ws) = self._gather_call(sources, dst_block_ids, plan)
         ls = self._layer_stream(ranks, ready_flags, layer_done_flags)
         tok = C.c_uint64()
         o = (options or TransferOptions())._c()
@@ -692,13 +702,7 @@ class TransferManager:
         same `sources` mapping (source rank -> (layout handle, block ids)) and plan, over `execute_repage`'s `tokens` range.  Every
         source has one page size Ps and its ids are its table's entries tokens.start // Ps .. ceil(tokens.stop / Ps);
         `dst_block_ids` are the destination's for its own page.  Options: those of `execute_repage`."""
-        if tokens.step != 1:
-            raise ValueError("tokens must be a range with step 1")
-        ranks = sorted({w.src_rank for w in plan})
-        n_src = len(sources[ranks[0]][1]) if ranks else 0
-        if any(len(sources[r][1]) != n_src for r in ranks):
-            raise KvbmError(ErrorCode.LENGTH_MISMATCH, "the sources' block id lists have different lengths")
-        hs, _keep, sp, d, n_dst, ws = self._gather_args(sources, ranks, dst_block_ids, plan)
+        ranks, n_src, (hs, _keep, sp, d, n_dst, ws) = self._repage_gather_call(sources, dst_block_ids, plan, tokens)
         tok = C.c_uint64()
         o = (options or TransferOptions())._c()
         _check(lib().kvbm_manager_execute_repage_gather(self._h, len(ranks), hs, sp, n_src, dst, d, n_dst, tokens.start, tokens.stop, ws,
@@ -710,13 +714,7 @@ class TransferManager:
                                        options: Optional[TransferOptions] = None, layer_done_flags: int = 0) -> TransferCompleteNotification:
         """`execute_repage_gather` streamed layer by layer (kvbm_manager_execute_repage_gather_streamed), with the flags of
         `execute_gather_streamed`.  A one-window plan over every head of both sides streams a plain re-page."""
-        if tokens.step != 1:
-            raise ValueError("tokens must be a range with step 1")
-        ranks = sorted({w.src_rank for w in plan})
-        n_src = len(sources[ranks[0]][1]) if ranks else 0
-        if any(len(sources[r][1]) != n_src for r in ranks):
-            raise KvbmError(ErrorCode.LENGTH_MISMATCH, "the sources' block id lists have different lengths")
-        hs, _keep, sp, d, n_dst, ws = self._gather_args(sources, ranks, dst_block_ids, plan)
+        ranks, n_src, (hs, _keep, sp, d, n_dst, ws) = self._repage_gather_call(sources, dst_block_ids, plan, tokens)
         ls = self._layer_stream(ranks, ready_flags, layer_done_flags)
         tok = C.c_uint64()
         o = (options or TransferOptions())._c()

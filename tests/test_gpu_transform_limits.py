@@ -144,6 +144,17 @@ def test_repage_warps_loop_over_heads_past_eight(nh, ps, pd, cast, scaled):
 
 
 @pytest.mark.parametrize("ps,pd", [(16, 64), (64, 16)], ids=str)
+def test_repage_takes_more_than_256_heads(ps, pd):
+    """kvbm_kernels_paged_repage has no head limit: 300 heads of a 16 B row, 37 or 38 per warp.  The same full window through
+    kvbm_kernels_paged_repage_gather is past the gather's 256 heads."""
+    nh = 300
+    c = _Range(ps, pd, 5, 2 * max(ps, pd) - 3, (2, 2, 8), CM.NONE, [nh], nh, [KV.OperationalNHD], KV.OperationalHND, nh + ps)
+    _rejected(lambda: c.launch("repage_gather"))
+    assert c.launch("repage") == 0
+    c.check()
+
+
+@pytest.mark.parametrize("ps,pd", [(16, 64), (64, 16)], ids=str)
 def test_repage_gather_covers_more_than_eight_heads(ps, pd):
     """TP4 -> TP1 on 32 KV heads: four 8-head windows, 32 covered heads over 8 warps."""
     windows = _windows(tp_reshard_plan(32, 4, 1, 0))

@@ -157,6 +157,13 @@ def test_repage_gather_argument_checks_before_any_cuda_call():
     assert _rg(two, tb=2**32 - 70, te=2**32 - 1) == INVAL
 
 
+def test_repage_gather_caps_one_full_window_at_256_heads():
+    """One window over every head of both sides runs the plain re-page's kernel, which kvbm_kernels_paged_repage launches with
+    no head limit; through the gather entry it still covers at most 256 heads."""
+    nh = K.GATHER_MAX_HEADS + 1
+    assert _rg([_src(nh=nh, k=nh, region=16 * nh * ROW)], dnh=nh, dst=_side(64, nh)) == INVAL
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # kvbm_manager_execute_repage_gather on a host-only manager: every rejection, then the missing device
 # ---------------------------------------------------------------------------------------------------------------------
