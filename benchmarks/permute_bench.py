@@ -33,6 +33,9 @@ p.add_argument("--scaled", action="store_true",
                help="with --cast: also time the same launches with per-(layer, K/V) fp8 KV-cache scales, alternating with the unscaled arms")
 p.add_argument("--reshard", default=None, metavar="SRC_TP:DST_TP",
                help="time one decode rank's assembly of its heads from the source ranks' pools (TP re-shard) instead; --cast composes")
+p.add_argument("--pp", default=None, metavar="SRC_PP:SRC_TP:DST_TP",
+               help="time decode rank 0's assembly of its layers and heads from a PP x TP prefill group (one pool per source rank, "
+                    "holding its stage's layers) instead; --cast composes")
 a = p.parse_args()
 nl, no, nt, nh, hd, elem = a.layers, 2, a.page, a.heads, a.head_dim, 2
 row, region = hd * elem, nt * nh * hd * elem
@@ -291,6 +294,116 @@ def reshard_bench():
     print(json.dumps(res))
 
 
+def pp_bench():
+    """Decode rank 0 (PP1) of a SRC_PP x SRC_TP -> DST_TP re-shard, engine pools OperationalNHD layer-separate on both sides, each
+    source pool holding only its stage's nl / SRC_PP layers.  Arms, alternated within each of five rounds (median of --iters per
+    arm and round): (1) stage_gather_one_launch, kvbm_kernels_paged_stage_gather over the plan; (2) per_stage_gathers, one
+    kvbm_kernels_paged_permute_gather per stage over that stage's layer range, its sources described by nl-entry layer_base
+    tables whose entries in the stage's range point at the pool's layers (the workaround without the staged gather, open to
+    operational formats only); (3) gather_from_full_layer_sources, the same bytes gathered from sources that hold every layer
+    (the ceiling); (4) plain_paged_copy_same_bytes.  stage_equals_per_stage compares the whole destination pool after arms 1
+    and 2.  gate_overhead: the streamed form with every flag already released, both gate modes, against arm 1."""
+    from dynamo_b200.physical import tp_pp_reshard_plan, tp_reshard_plan
+    src_pp, src_tp, dst_tp = (int(x) for x in a.pp.split(":"))
+    mode = {"none": K.CastMode.NONE, "fp8-to-bf16": K.CastMode.FP8E4M3_TO_BF16, "bf16-to-fp8": K.CastMode.BF16_TO_FP8E4M3}[a.cast]
+    se, de = {"none": (2, 2), "fp8-to-bf16": (1, 2), "bf16-to-fp8": (2, 1)}[a.cast]
+    snh, dnh, snl = max(1, nh // src_tp), max(1, nh // dst_tp), nl // src_pp
+    plan = tp_pp_reshard_plan(nh, nl, src_tp, src_pp, dst_tp, 1, 0)
+    keep = []
+
+    def engine(heads, e, layers, table=None):
+        reg = nt * heads * hd * e
+        ts = [torch.randint(0, 256, (no * nb * reg,), dtype=torch.uint8, device=dev) for _ in range(layers)]
+        ptrs = table(ts) if table else [t.data_ptr() for t in ts]
+        base = torch.tensor(ptrs, dtype=torch.int64, device=dev)
+        keep.append(base)
+        return ts, K.PagedLayout(base.data_ptr(), reg, nb * reg, reg, len(ptrs), no, nb)
+
+    side = lambda desc, ids: K.PermuteSide(desc, ids.data_ptr(), int(K.KvBlockLayout.OperationalNHD))  # noqa: E731
+    srcs = {w.src_rank: engine(snh, se, snl) for w in plan}
+    dst = engine(dnh, de, nl)
+    row = hd * se
+    staged = [K.StageSource(K.PermuteSource(side(srcs[w.src_rank][1], sid_d), snh, w.src_head_begin, w.dst_head_begin, w.head_count),
+                            w.src_layer_begin, w.dst_layer_begin, w.layer_count) for w in plan]
+
+    def stage_one():
+        K.check(K.paged_stage_gather(staged, side(dst[1], did_d), dnh, n, 0, nl, nt, row, int(mode), stream=sp))
+
+    # arm 2: per stage, each source seen through an nl-entry layer_base table shifted to the stage's destination layers
+    stages = sorted({(w.dst_layer_begin, w.layer_count) for w in plan})
+    per_stage = []
+    for d0, c in stages:
+        ws = [w for w in plan if w.dst_layer_begin == d0]
+        shifted = {}
+        for w in ws:
+            ts = srcs[w.src_rank][0]
+            ptrs = [ts[min(max(l - d0 + w.src_layer_begin, 0), snl - 1)].data_ptr() for l in range(nl)]
+            base = torch.tensor(ptrs, dtype=torch.int64, device=dev)
+            keep.append(base)
+            shifted[w.src_rank] = K.PagedLayout(base.data_ptr(), nt * snh * hd * se, nb * nt * snh * hd * se, nt * snh * hd * se, nl, no, nb)
+        per_stage.append((d0, d0 + c, [K.PermuteSource(side(shifted[w.src_rank], sid_d), snh, w.src_head_begin, w.dst_head_begin, w.head_count)
+                                       for w in ws]))
+
+    def stage_each():
+        for lb, le, ps in per_stage:
+            K.check(K.paged_permute_gather(ps, side(dst[1], did_d), dnh, n, lb, le, nt, row, int(mode), stream=sp))
+
+    tp_plan = tp_reshard_plan(nh, src_tp, dst_tp, 0)
+    full = {w.src_rank: engine(snh, se, nl) for w in tp_plan}
+    full_srcs = [K.PermuteSource(side(full[w.src_rank][1], sid_d), snh, w.src_head_begin, w.dst_head_begin, w.head_count) for w in tp_plan]
+
+    def ceiling():
+        K.check(K.paged_permute_gather(full_srcs, side(dst[1], did_d), dnh, n, 0, nl, nt, row, int(mode), stream=sp))
+
+    plain_src = engine(dnh, se, nl)
+
+    def plain():
+        K.check(K.paged_copy(plain_src[1], [K.PagedDst(dst[1], sid_d.data_ptr(), did_d.data_ptr(), 0, 0)], n, 0, nl, int(mode), None, sp))
+
+    def dst_after(fn):
+        for t in dst[0]:
+            t.fill_(0x5A)
+        torch.cuda.synchronize()
+        fn()
+        torch.cuda.synchronize()
+        return [t.clone() for t in dst[0]]
+
+    same = all(torch.equal(x, y) for x, y in zip(dst_after(stage_one), dst_after(stage_each)))
+    flags = {r: torch.ones(snl, dtype=torch.int32, device=dev) for r in srcs}
+    ws_words = torch.zeros(K.sync_workspace_words(nl), dtype=torch.int32, device=dev)
+
+    def streamed(gate):
+        st = K.PermuteStream()
+        for j, w in enumerate(plan):
+            st.layer_ready_flags[j] = flags[w.src_rank].data_ptr()
+        st.epoch, st.sync_workspace, st.gate_mode = 1, ws_words.data_ptr(), gate
+        return lambda: K.check(K.paged_stage_gather_streamed(staged, side(dst[1], did_d), dnh, n, 0, nl, nt, row, int(mode), None, st, sp))
+
+    arms = [("stage_gather_one_launch", stage_one), ("per_stage_gathers", stage_each), ("gather_from_full_layer_sources", ceiling),
+            ("plain_paged_copy_same_bytes", plain), ("streamed_spin_flags_released", streamed(K.GATE_SPIN)),
+            ("streamed_stream_wait_flags_released", streamed(K.GATE_STREAM_WAIT))]
+    rounds = {name: [] for name, _ in arms}
+    for _ in range(5):
+        for name, fn in arms:
+            rounds[name].append(timed(fn))
+    elems = n * nl * no * nt * dnh * hd
+    rw = elems * (se + de)
+    res = {"geometry": {"blocks": n, "layers": nl, "outer": no, "page": nt, "heads": nh, "head_dim": hd, "cast": a.cast, "src_pp": src_pp,
+                        "src_tp": src_tp, "dst_tp": dst_tp, "layers_per_source": snl},
+           "plan": [[w.src_rank, w.src_layer_begin, w.dst_layer_begin, w.layer_count, w.src_head_begin, w.dst_head_begin, w.head_count]
+                    for w in plan],
+           "stage_equals_per_stage": same, "hbm_peak_GBps": peak, "hbm_peak_source": peak_src, "card": card(),
+           "bytes_read_plus_write": rw}
+    for name, _ in arms:
+        ms = statistics.median(rounds[name])
+        res[name] = {"ms": round(ms, 4), "ms_min": round(min(rounds[name]), 4), "ms_max": round(max(rounds[name]), 4),
+                     "GBps_read_plus_write": round(rw / ms / 1e6, 1), "frac_of_hbm_peak": round(rw / ms / 1e6 / peak, 3)}
+    print(json.dumps(res))
+
+
+if a.pp:
+    pp_bench()
+    sys.exit(0)
 if a.reshard:
     reshard_bench()
     sys.exit(0)

@@ -584,10 +584,11 @@ static int finish_slot(kvbm_transfer_manager* m, Slot* sl, cudaStream_t stream, 
 }
 
 // heads: a head-window transfer, whose regions differ when the head counts do; the head rows (head_dim elements) must match
-// instead.  Both configs then carry num_heads dividing inner_dim (checked by the caller).
-static int check_compat(const Layout& S, const Layout& D, int cast, bool heads = false)
+// instead.  Both configs then carry num_heads dividing inner_dim (checked by the caller).  staged: a staged gather's pair, whose
+// layer windows map layers between pools of different layer counts.
+static int check_compat(const Layout& S, const Layout& D, int cast, bool heads = false, bool staged = false)
 {
-  if (S.cfg.num_layers != D.cfg.num_layers)  // executor/cuda.rs:52-58, memcpy.rs:49-55
+  if (!staged && S.cfg.num_layers != D.cfg.num_layers)  // executor/cuda.rs:52-58, memcpy.rs:49-55
     return fail(KVBM_ERR_INCOMPATIBLE, "Layouts have incompatible layer counts: src=" + std::to_string(S.cfg.num_layers) +
                                            ", dst=" + std::to_string(D.cfg.num_layers));
   if (S.cfg.outer_dim != D.cfg.outer_dim)  // cuda.rs:60-66
@@ -699,9 +700,11 @@ static kvbm_permute_stream layer_stream(const kvbm_layer_stream& ls, const size_
 // trailing signal kernel.
 // ls: a streamed gather (execute_gather_streamed), one kvbm_kernels_paged_permute_gather_streamed launch gated on every window's
 // source flags, with the slot's workspace staged for the destination's layers.
+// layers: a staged gather (execute_stage_gather), window j with the layer window of layers[j], one kvbm_kernels_paged_stage_gather
+// launch (or its streamed form with ls); each window's bytes count over its layers inside the layer range.
 static int launch_permute(kvbm_transfer_manager* m, const Transfer* e, size_t nw, size_t num_srcs, const size_t* const* src_ids,
                           const size_t* dst_ids, size_t n, const kvbm_transfer_options& o, cudaStream_t stream, uint64_t* seq_out,
-                          const kvbm_layer_stream* ls = nullptr)
+                          const kvbm_layer_stream* ls = nullptr, const kvbm_shard_window* layers = nullptr)
 {
   std::vector<const size_t*> lists(src_ids, src_ids + num_srcs);
   lists.push_back(dst_ids);
@@ -723,6 +726,33 @@ static int launch_permute(kvbm_transfer_manager* m, const Transfer* e, size_t nw
   const uint32_t dnh = static_cast<uint32_t>(D->cfg.num_heads), page = static_cast<uint32_t>(S0->cfg.page_size);
   const uint32_t row = static_cast<uint32_t>(S0->cfg.inner_dim / S0->cfg.num_heads * S0->cfg.dtype_width_bytes);
   const int nb = static_cast<int>(n), lb = static_cast<int>(e[0].lb), le = static_cast<int>(e[0].le);
+  if (layers) {
+    kvbm_stage_source ss[KVBM_GATHER_MAX_SOURCES] = {};
+    uint64_t bytes = 0;
+    for (size_t j = 0; j < nw; ++j) {
+      const kvbm_shard_window& w = layers[j];
+      ss[j] = kvbm_stage_source{ks[j], static_cast<uint32_t>(w.src_layer_begin), static_cast<uint32_t>(w.dst_layer_begin),
+                                static_cast<uint32_t>(w.layer_count)};
+      const size_t from = std::max(e[0].lb, w.dst_layer_begin), to = std::min(e[0].le, w.dst_layer_begin + w.layer_count);
+      if (to > from) bytes += n * (to - from) * S0->cfg.outer_dim * (D->region / D->cfg.num_heads * w.head_count);
+    }
+    cudaError_t ce;
+    if (ls) {
+      size_t ranks[KVBM_GATHER_MAX_SOURCES];
+      for (size_t j = 0; j < nw; ++j) ranks[j] = e[j].window.src_rank;
+      const kvbm_permute_stream st = layer_stream(*ls, ranks, nw, o, *sl, seq);
+      ce = kvbm_kernels_paged_stage_gather_streamed(ss, static_cast<int>(nw), &pd, dnh, nb, lb, le, page, row, o.cast_mode, o.cast_scales, &st,
+                                                    stream);
+      if (ce != cudaSuccess) return fail_cuda(ce, "kvbm_kernels_paged_stage_gather_streamed");
+    } else {
+      ce = kvbm_kernels_paged_stage_gather(ss, static_cast<int>(nw), &pd, dnh, nb, lb, le, page, row, o.cast_mode, o.cast_scales, o.done_flag,
+                                           o.epoch, sl->host_flag, static_cast<uint32_t>(seq), stream);
+      if (ce != cudaSuccess) return fail_cuda(ce, "kvbm_kernels_paged_stage_gather");
+    }
+    if ((rc = finish_slot(m, sl, stream, bytes))) return rc;
+    *seq_out = seq;
+    return KVBM_OK;
+  }
   if (ls) {
     size_t ranks[KVBM_GATHER_MAX_SOURCES];
     for (size_t j = 0; j < nw; ++j) ranks[j] = e[j].window.src_rank;
@@ -986,10 +1016,11 @@ static int check_strategy(kvbm_transfer_manager* m, int nd, const kvbm_transfer_
 
 // Validate one request and resolve it into *t; the caller holds m->mu.  `heads`: a head window that always takes the permuting
 // launch (a gather's).  Without it the options' window applies, and one over every head of both sides is the transfer without a
-// window.  A request that fails several checks reports the first in the order below.
+// window.  A request that fails several checks reports the first in the order below.  staged: a staged gather's window, whose
+// source may have other layers than the destination; the layer range and the cast scales are then the destination's.
 static int resolve(kvbm_transfer_manager* m, kvbm_layout_handle src_h, int nd, const kvbm_layout_handle* dst_h,
                    const size_t* const* src_ids, const size_t* const* dst_ids, size_t n, const kvbm_transfer_options& o,
-                   const kvbm_head_window* heads, Transfer* t)
+                   const kvbm_head_window* heads, Transfer* t, bool staged = false)
 {
   if (nd < 1 || nd > KVBM_MAX_DESTINATIONS) return fail(KVBM_ERR, "number of destinations must be in 1..=8");
   Layout* S = t->S = m->find(src_h);
@@ -1006,7 +1037,7 @@ static int resolve(kvbm_transfer_manager* m, kvbm_layout_handle src_h, int nd, c
       if ((rc = check_head_window(*S, *D, w, nd))) return rc;
       window = heads || !(w.src_head_begin == 0 && w.dst_head_begin == 0 && w.head_count == S->cfg.num_heads && w.head_count == D->cfg.num_heads);
     }
-    if ((rc = check_compat(*S, *D, o.cast_mode, window))) return rc;
+    if ((rc = check_compat(*S, *D, o.cast_mode, window, staged))) return rc;
     if (n && (!src_ids || !dst_ids || !src_ids[d] || !dst_ids[d])) return fail(KVBM_ERR, "null block id list");
     if ((rc = validate_block_transfer(src_ids[d], n, dst_ids[d], n, S->cfg.num_blocks, D->cfg.num_blocks, src_h == dst_h[d]))) return rc;
   }
@@ -1034,18 +1065,19 @@ static int resolve(kvbm_transfer_manager* m, kvbm_layout_handle src_h, int nd, c
   }
   t->dst_kv = o.dst_kv_layout ? o.dst_kv_layout : t->D[0]->kv_block_layout;
   t->window = window ? w : kvbm_head_window{0, 0, 0, S->cfg.num_heads};  // a plain transform is the window over every head
+  const size_t nl = staged ? t->D[0]->cfg.num_layers : S->cfg.num_layers;
   t->lb = 0;
-  t->le = S->cfg.num_layers;
+  t->le = nl;
   if (o.has_layer_range) {
     t->lb = o.layer_begin;
     t->le = o.layer_end;
-    if (t->lb > t->le || t->le > S->cfg.num_layers)
+    if (t->lb > t->le || t->le > nl)
       return fail(KVBM_ERR_RANGE, "Layer range " + std::to_string(t->lb) + ".." + std::to_string(t->le) + " exceeds num_layers " +
-                                      std::to_string(S->cfg.num_layers));
+                                      std::to_string(nl));
   }
   if (o.cast_scales) {  // fp8 KV-cache scales: one per (layer, outer) of the pools, for the fp8 side of a cast
     if (o.cast_mode == KVBM_CAST_NONE) return fail(KVBM_ERR, "cast_scales need a cast_mode: they scale the fp8 side of a cast");
-    const size_t need = S->cfg.num_layers * S->cfg.outer_dim;
+    const size_t need = nl * S->cfg.outer_dim;
     if (o.num_cast_scales < need)
       return fail(KVBM_ERR_RANGE, "cast_scales holds " + std::to_string(o.num_cast_scales) + " scales, the pools need num_layers * outer_dim = " +
                                       std::to_string(need));
@@ -1106,9 +1138,11 @@ static int execute(kvbm_transfer_manager* m, kvbm_layout_handle src_h, int nd, c
 }
 
 // The windows of a gather, before any layout is looked up: at least one source and one window, none in the options, at most
-// KVBM_GATHER_MAX_SOURCES, each naming a source, with heads, on destination heads no other window writes.
+// KVBM_GATHER_MAX_SOURCES, each naming a source, with heads, on destination heads no other window writes.  layers: a staged
+// gather's windows (windows[j] is layers[j]'s head window), each with layers, whose layer windows are equal (one stage) or
+// disjoint in the destination; only the windows of one stage may not share a destination head.
 static int check_gather_windows(size_t num_srcs, const kvbm_layout_handle* srcs, const kvbm_head_window* windows, size_t nw,
-                                const kvbm_transfer_options& o)
+                                const kvbm_transfer_options& o, const kvbm_shard_window* layers = nullptr)
 {
   if (num_srcs == 0 || !srcs || !windows || nw == 0) return fail(KVBM_ERR, "a gather needs at least one source and one window");
   if (o.head_count) return fail(KVBM_ERR, "a gather takes its head windows from the windows argument: options.head_count must be 0");
@@ -1119,10 +1153,21 @@ static int check_gather_windows(size_t num_srcs, const kvbm_layout_handle* srcs,
       return fail(KVBM_ERR_RANGE, "window " + std::to_string(j) + " names source " + std::to_string(windows[j].src_rank) + " of " +
                                       std::to_string(num_srcs));
     if (windows[j].head_count == 0) return fail(KVBM_ERR_RANGE, "window " + std::to_string(j) + " has no heads");
-    for (size_t t = 0; t < j; ++t)
+    if (layers && layers[j].layer_count == 0) return fail(KVBM_ERR_RANGE, "window " + std::to_string(j) + " has no layers");
+    for (size_t t = 0; t < j; ++t) {
+      if (layers) {
+        const kvbm_shard_window &a = layers[t], &b = layers[j];
+        if (a.dst_layer_begin != b.dst_layer_begin || a.layer_count != b.layer_count) {
+          if (b.dst_layer_begin < a.dst_layer_begin + a.layer_count && a.dst_layer_begin < b.dst_layer_begin + b.layer_count)
+            return fail(KVBM_ERR_OVERLAP, "windows " + std::to_string(t) + " and " + std::to_string(j) +
+                                              " have layer windows that partly overlap in the destination");
+          continue;  // different stages may share destination heads
+        }
+      }
       if (windows[j].dst_head_begin < windows[t].dst_head_begin + windows[t].head_count &&
           windows[t].dst_head_begin < windows[j].dst_head_begin + windows[j].head_count)
         return fail(KVBM_ERR_OVERLAP, "windows " + std::to_string(t) + " and " + std::to_string(j) + " overlap in the destination");
+    }
   }
   return KVBM_OK;
 }
@@ -1160,6 +1205,67 @@ static int execute_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_
   int rc = launch_permute(m, e, nw, num_srcs, src_ids, dst_ids, n, o, pick_stream(m, e[0].plan.first, o), &seq, ls);
   if (rc) return rc;
   // caller-provided stream: caller manages sync, completed() is returned, as execute()
+  if (out) *out = o.use_caller_stream ? 0 : seq;
+  return KVBM_OK;
+}
+
+// A PP x TP re-shard's assembly as one hand-off: execute_gather with a layer window per window.  The windows are checked as
+// execute_gather checks them, with head overlaps only within a stage and partly overlapping layer windows rejected; then each
+// layer window inside its source's and the destination's layers, and every destination layer of the range inside some window
+// (KVBM_ERR_RANGE); then each (source, destination) pair as execute_gather's but for the equal layer counts, the options' layer
+// range being the destination's.  One upload, one kvbm_kernels_paged_stage_gather launch, one notification.
+static int execute_stage_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, const size_t* const* src_ids,
+                                kvbm_layout_handle dst_h, const size_t* dst_ids, size_t n, const kvbm_shard_window* sw, size_t nw,
+                                const kvbm_layer_stream* ls, const kvbm_transfer_options* opts_in, kvbm_notification* out)
+{
+  kvbm_transfer_options o{};
+  if (opts_in) o = *opts_in;
+  if (out) *out = 0;
+  std::vector<kvbm_head_window> hw(sw ? nw : 0);
+  for (size_t j = 0; j < hw.size(); ++j) hw[j] = kvbm_head_window{sw[j].src_rank, sw[j].src_head_begin, sw[j].dst_head_begin, sw[j].head_count};
+  if (int rc = check_gather_windows(num_srcs, srcs, sw ? hw.data() : nullptr, nw, o, sw)) return rc;
+  if (n && (!src_ids || !dst_ids)) return fail(KVBM_ERR, "null block id list");
+  std::lock_guard<std::mutex> lk(m->mu);
+  const Layout* D = m->find(dst_h);
+  if (!D) return fail(KVBM_ERR_HANDLE, "invalid destination handle");
+  const size_t dnl = D->cfg.num_layers;
+  for (size_t j = 0; j < nw; ++j) {
+    const Layout* S = m->find(srcs[sw[j].src_rank]);
+    if (!S) return fail(KVBM_ERR_HANDLE, "invalid source handle");
+    const size_t snl = S->cfg.num_layers;
+    if (sw[j].src_layer_begin > snl || sw[j].layer_count > snl - sw[j].src_layer_begin)
+      return fail(KVBM_ERR_RANGE, "window " + std::to_string(j) + "'s source layers " + std::to_string(sw[j].src_layer_begin) + ".." +
+                                      std::to_string(sw[j].src_layer_begin + sw[j].layer_count) + " exceed the source's num_layers " +
+                                      std::to_string(snl));
+    if (sw[j].dst_layer_begin > dnl || sw[j].layer_count > dnl - sw[j].dst_layer_begin)
+      return fail(KVBM_ERR_RANGE, "window " + std::to_string(j) + "'s destination layers " + std::to_string(sw[j].dst_layer_begin) + ".." +
+                                      std::to_string(sw[j].dst_layer_begin + sw[j].layer_count) + " exceed the destination's num_layers " +
+                                      std::to_string(dnl));
+  }
+  const size_t lb = o.has_layer_range ? o.layer_begin : 0, le = o.has_layer_range ? std::min(o.layer_end, dnl) : dnl;
+  for (size_t l = lb; l < le; ++l) {  // a range past the destination's layers is resolve()'s to reject
+    bool in = false;
+    for (size_t j = 0; j < nw && !in; ++j) in = l >= sw[j].dst_layer_begin && l - sw[j].dst_layer_begin < sw[j].layer_count;
+    if (!in) return fail(KVBM_ERR_RANGE, "destination layer " + std::to_string(l) + " of the layer range is in no window's layers");
+  }
+  Transfer e[KVBM_GATHER_MAX_SOURCES];
+  for (size_t j = 0; j < nw; ++j) {
+    const size_t* s = src_ids ? src_ids[sw[j].src_rank] : nullptr;
+    int rc = resolve(m, srcs[sw[j].src_rank], 1, &dst_h, &s, &dst_ids, n, o, &hw[j], &e[j], true);
+    if (rc) return rc;
+    if (e[j].plan.first != e[0].plan.first) return fail(KVBM_ERR_UNSUPPORTED, "the sources of a gather need the same CUDA strategy");
+  }
+  if (e[0].empty) return KVBM_OK;  // nothing to move (no blocks or an empty layer range), as execute()
+  if (ls) {
+    size_t ranks[KVBM_GATHER_MAX_SOURCES];
+    for (size_t j = 0; j < nw; ++j) ranks[j] = sw[j].src_rank;
+    if (int rc = check_layer_stream_flags(m, *ls, ranks, nw)) return rc;
+  }
+
+  DeviceGuard g(m->device);
+  uint64_t seq;
+  int rc = launch_permute(m, e, nw, num_srcs, src_ids, dst_ids, n, o, pick_stream(m, e[0].plan.first, o), &seq, ls, sw);
+  if (rc) return rc;
   if (out) *out = o.use_caller_stream ? 0 : seq;
   return KVBM_OK;
 }
@@ -1818,12 +1924,9 @@ extern "C" int kvbm_manager_kv_block_layout(kvbm_transfer_manager* m, kvbm_layou
 extern "C" int kvbm_select_transform_kernel(int src_kv_layout, int dst_kv_layout) { return select_transform_kernel(src_kv_layout, dst_kv_layout); }
 extern "C" int kvbm_kv_layout_requires_transform(int a, int b) { return kv_requires_transform(a, b) ? 1 : 0; }
 
-extern "C" int kvbm_tp_reshard_plan(size_t num_kv_heads, size_t src_tp, size_t dst_tp, size_t dst_rank, kvbm_head_window* out, size_t cap,
-                                    size_t* n_out)
+// kvbm_tp_reshard_plan's windows, after its checks, into *out.
+static int tp_head_windows(size_t H, size_t src_tp, size_t dst_tp, size_t dst_rank, std::vector<kvbm_head_window>* out)
 {
-  const size_t H = num_kv_heads;
-  if (!n_out) return fail(KVBM_ERR, "null argument");
-  *n_out = 0;
   if (!H || !src_tp || !dst_tp) return fail(KVBM_ERR_CONFIG, "num_kv_heads, src_tp and dst_tp must be positive");
   for (size_t tp : {src_tp, dst_tp})
     if (H % tp && tp % H)
@@ -1833,7 +1936,8 @@ extern "C" int kvbm_tp_reshard_plan(size_t num_kv_heads, size_t src_tp, size_t d
   // vLLM's ownership: rank r of tp holds heads [r*H/tp, r*H/tp + max(1, H/tp)); replicated over tp/H ranks when tp > H
   const size_t d_first = dst_rank * H / dst_tp, d_count = std::max<size_t>(1, H / dst_tp);
   const size_t s_per = std::max<size_t>(1, H / src_tp), replicas = src_tp > H ? src_tp / H : 1;
-  std::vector<kvbm_head_window> w;
+  std::vector<kvbm_head_window>& w = *out;
+  w.clear();
   for (size_t j = 0; j < d_count; ++j) {
     const size_t g = d_first + j;  // global head
     const size_t rank = replicas > 1 ? g * replicas + dst_rank % replicas : g / s_per;
@@ -1843,11 +1947,75 @@ extern "C" int kvbm_tp_reshard_plan(size_t num_kv_heads, size_t src_tp, size_t d
     else
       w.push_back({rank, local, j, 1});
   }
+  return KVBM_OK;
+}
+
+extern "C" int kvbm_tp_reshard_plan(size_t num_kv_heads, size_t src_tp, size_t dst_tp, size_t dst_rank, kvbm_head_window* out, size_t cap,
+                                    size_t* n_out)
+{
+  if (!n_out) return fail(KVBM_ERR, "null argument");
+  *n_out = 0;
+  std::vector<kvbm_head_window> w;
+  if (int rc = tp_head_windows(num_kv_heads, src_tp, dst_tp, dst_rank, &w)) return rc;
   *n_out = w.size();
   if (!out) return KVBM_OK;
   if (cap < w.size()) return fail(KVBM_ERR, "kvbm_tp_reshard_plan: " + std::to_string(w.size()) + " windows do not fit in " + std::to_string(cap));
   std::copy(w.begin(), w.end(), out);
   return KVBM_OK;
+}
+
+// The first layer of every stage of a pipeline of pp stages over L layers, and L at the end ([pp + 1] bounds): the partition's
+// running sums, or an even split.  The library does not guess an engine's remainder policy, so an uneven L needs a partition.
+static int stage_bounds(const char* side, size_t L, size_t pp, const size_t* parts, std::vector<size_t>* out)
+{
+  std::vector<size_t>& b = *out;
+  b.assign(1, 0);
+  if (!parts && L % pp)
+    return fail(KVBM_ERR_CONFIG, std::string(side) + ": " + std::to_string(L) + " layers do not split evenly over PP " + std::to_string(pp) +
+                                     "; pass the engine's stage layer counts");
+  for (size_t p = 0; p < pp; ++p) {
+    const size_t c = parts ? parts[p] : L / pp;
+    if (c == 0) return fail(KVBM_ERR_CONFIG, std::string(side) + ": stage " + std::to_string(p) + " has no layers");
+    b.push_back(b.back() + c);
+  }
+  if (b.back() != L)
+    return fail(KVBM_ERR_CONFIG, std::string(side) + ": the stage layer counts sum to " + std::to_string(b.back()) + ", not num_layers " +
+                                     std::to_string(L));
+  return KVBM_OK;
+}
+
+extern "C" int kvbm_tp_pp_reshard_plan(size_t num_kv_heads, size_t num_layers, size_t src_tp, size_t src_pp, const size_t* src_stage_layers,
+                                       size_t dst_tp, size_t dst_pp, const size_t* dst_stage_layers, size_t dst_rank, kvbm_shard_window* out,
+                                       size_t cap, size_t* n_out)
+{
+  return guarded([&]() -> int {
+  if (!n_out) return fail(KVBM_ERR, "null argument");
+  *n_out = 0;
+  if (!num_kv_heads || !num_layers || !src_tp || !src_pp || !dst_tp || !dst_pp)
+    return fail(KVBM_ERR_CONFIG, "num_kv_heads, num_layers and every TP and PP degree must be positive");
+  std::vector<size_t> sb, db;
+  int rc;
+  if ((rc = stage_bounds("source", num_layers, src_pp, src_stage_layers, &sb)) || (rc = stage_bounds("destination", num_layers, dst_pp, dst_stage_layers, &db)))
+    return rc;
+  if (dst_rank >= dst_pp * dst_tp)
+    return fail(KVBM_ERR_RANGE, "dst_rank " + std::to_string(dst_rank) + " out of range for PP " + std::to_string(dst_pp) + " x TP " +
+                                    std::to_string(dst_tp));
+  std::vector<kvbm_head_window> heads;
+  if ((rc = tp_head_windows(num_kv_heads, src_tp, dst_tp, dst_rank % dst_tp, &heads))) return rc;
+  const size_t stage = dst_rank / dst_tp, d0 = db[stage], d1 = db[stage + 1];
+  std::vector<kvbm_shard_window> w;
+  for (size_t p = 0; p < src_pp; ++p) {
+    const size_t lo = std::max(d0, sb[p]), hi = std::min(d1, sb[p + 1]);
+    if (lo >= hi) continue;
+    for (const kvbm_head_window& h : heads)
+      w.push_back({p * src_tp + h.src_rank, lo - sb[p], lo - d0, hi - lo, h.src_head_begin, h.dst_head_begin, h.head_count});
+  }
+  *n_out = w.size();
+  if (!out) return KVBM_OK;
+  if (cap < w.size()) return fail(KVBM_ERR, "kvbm_tp_pp_reshard_plan: " + std::to_string(w.size()) + " windows do not fit in " + std::to_string(cap));
+  std::copy(w.begin(), w.end(), out);
+  return KVBM_OK;
+  });
 }
 
 extern "C" int kvbm_manager_set_capabilities(kvbm_transfer_manager* m, const kvbm_transfer_capabilities* caps)
@@ -1911,6 +2079,20 @@ extern "C" int kvbm_manager_execute_gather_streamed(kvbm_transfer_manager* m, si
   if (out) *out = 0;
   if (int rc = check_layer_stream_shape(ls, num_srcs)) return rc;
   return execute_gather(m, num_srcs, srcs, src_ids, dst, dst_ids, n, windows, num_windows, opts, out, ls);
+  });
+}
+
+extern "C" int kvbm_manager_execute_stage_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs,
+                                                 const size_t* const* src_ids, kvbm_layout_handle dst, const size_t* dst_ids, size_t n,
+                                                 const kvbm_shard_window* windows, size_t num_windows, const kvbm_layer_stream* ls,
+                                                 const kvbm_transfer_options* opts, kvbm_notification* out)
+{
+  return guarded([&]() -> int {
+  if (!m) return fail(KVBM_ERR, "null manager");
+  if (out) *out = 0;
+  if (ls)
+    if (int rc = check_layer_stream_shape(ls, num_srcs)) return rc;
+  return execute_stage_gather(m, num_srcs, srcs, src_ids, dst, dst_ids, n, windows, num_windows, ls, opts, out);
   });
 }
 

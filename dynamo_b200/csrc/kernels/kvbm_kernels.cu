@@ -881,10 +881,10 @@ __device__ __forceinline__ void publish_units(const GateArgs& A, uint32_t l, uin
   if (threadIdx.x == 0 && A.ss.want_layers && count != 0) arrive_layer(A.ss, static_cast<int>(l), count);
 }
 
-// The claim / gate / publish loop of both gated kernels over units [0, total): layer_of(u) is unit u's absolute layer,
-// walk(u, l) moves it.
-template <class LayerOf, class Walk>
-__device__ __forceinline__ void gated_units(const GateArgs& A, uint32_t total, uint32_t batch, LayerOf layer_of, Walk walk)
+// The claim / gate / publish loop of every gated kernel over units [0, total): layer_of(u) is unit u's absolute layer,
+// walk(u, l) moves it, gate(l, s_ok) waits for layer l's sources as gate_layer does.
+template <class LayerOf, class Walk, class Gate>
+__device__ __forceinline__ void gated_units(const GateArgs& A, uint32_t total, uint32_t batch, LayerOf layer_of, Walk walk, Gate gate)
 {
   __shared__ uint32_t s_ticket, s_ok;
   uint32_t entered = UINT32_MAX;
@@ -901,7 +901,7 @@ __device__ __forceinline__ void gated_units(const GateArgs& A, uint32_t total, u
       if (l != entered) {
         if (pending != 0) publish_units(A, entered, pending);
         pending = 0;
-        if (!gate_layer(A, l, &s_ok)) {
+        if (!gate(l, &s_ok)) {
           aborted = true;
           break;
         }
@@ -914,6 +914,13 @@ __device__ __forceinline__ void gated_units(const GateArgs& A, uint32_t total, u
     publish_units(A, entered, pending);
   }
   if (threadIdx.x == 0) arrive_transfer(A.ss);
+}
+
+// The loop gated on every source's flag of the unit's layer.
+template <class LayerOf, class Walk>
+__device__ __forceinline__ void gated_units(const GateArgs& A, uint32_t total, uint32_t batch, LayerOf layer_of, Walk walk)
+{
+  gated_units(A, total, batch, layer_of, walk, [&](uint32_t l, uint32_t* s_ok) { return gate_layer(A, l, s_ok); });
 }
 
 // kvbm_paged_gather_kernel's unit walk behind the gate; unit = (l * num_blocks + pair) * no + o over the layer range.
@@ -943,6 +950,97 @@ kvbm_gated_repage_gather_kernel(const __grid_constant__ RepageGatherParams P, co
     const uint32_t j = rem / G.no;
     repage_gather_unit<CAST, POW2, SCALED, PPOW2>(P, j, l, rem - j * G.no, r, scales);
   });
+}
+
+// ------------------------------------------------------------------------------------------------
+// The staged gather (DESIGN §4.2e): a pipeline-parallel re-shard.  Each source also has a layer window, source layers
+// [src_begin, src_begin + count) -> destination layers [dst_begin, dst_begin + count); sources with one destination window form a
+// stage.  Stage k covers destination layers [begin, end) and map entries first .. first + count - 1 of the gather's one head
+// map (stage by stage), `sources` is the mask of its sources, and shift[s] is source s's layer minus the destination's.  The
+// stages ascend and tile the launch's layer range.
+// ------------------------------------------------------------------------------------------------
+struct GatherStage {
+  uint32_t begin, end, first, count, sources;
+};
+struct StageGatherParams {
+  GatherParams g;
+  GatherStage stage[KVBM_GATHER_MAX_SOURCES];
+  uint32_t shift[KVBM_GATHER_MAX_SOURCES];
+};
+
+// The stage of destination layer l (one of the launch's range): the first stage that ends past it.
+__host__ __device__ __forceinline__ const GatherStage& stage_of(const StageGatherParams& P, uint32_t l)
+{
+  uint32_t k = 0;
+  while (l >= P.stage[k].end) ++k;
+  return P.stage[k];
+}
+
+// gather_unit over the stage of layer l only: its warps walk that stage's map entries, each reading its source at the source's
+// own layer l + shift.  SCALED: scales[l * no + o], by the destination layer.
+template <int CAST, bool POW2, bool SCALED>
+__device__ __forceinline__ void stage_gather_unit(const StageGatherParams& P, uint32_t pair, uint32_t l, uint32_t o, uint32_t no, uint32_t nt,
+                                                  const RowSplit& r, const float* scales)
+{
+  const GatherStage& T = stage_of(P, l);
+  uint8_t* db = side_block(P.g.D, pair, l, o);
+  const ptx::Scale scale = ptx::make_scale(SCALED ? __ldg(scales + l * no + o) : 1.f);
+  const uint32_t end = T.first + T.count;
+  for (uint32_t j = T.first + (threadIdx.x >> 5); j < end; j += blockDim.x >> 5) {
+    const uint32_t s = P.g.entry[j];
+    const GatherSource& G = P.g.src[s];
+    const uint32_t h = j - G.first;
+    walk_head_rows<CAST, POW2, SCALED>(side_block(G.S, pair, l + P.shift[s], o) + G.s_win, G.S.head_stride, G.S.tok_stride, db + G.d_win,
+                                       P.g.D.head_stride, P.g.D.tok_stride, h, 1, h + 1, nt, r, scale);
+  }
+}
+
+// One CTA per destination unit, as the gather.
+template <int CAST, bool POW2, bool SCALED = false>
+__global__ void __launch_bounds__(256)
+kvbm_paged_stage_gather_kernel(const __grid_constant__ StageGatherParams P, uint32_t layer_begin, uint32_t nlayers, uint32_t no, uint32_t nt,
+                               RowSplit r, const float* scales)
+{
+  const uint32_t unit = blockIdx.x;  // (pair * nlayers + l) * no + o
+  const uint32_t pair = unit / (nlayers * no);
+  const uint32_t rem = unit - pair * (nlayers * no);
+  stage_gather_unit<CAST, POW2, SCALED>(P, pair, layer_begin + rem / no, rem % no, no, nt, r, scales);
+}
+
+// gate_layer for the staged gather: the ready flags of only the sources of layer l's stage, each at its own layer l + shift.
+__device__ __forceinline__ bool gate_stage_layer(const GateArgs& A, const StageGatherParams& P, uint32_t l, uint32_t* s_ok)
+{
+  if (threadIdx.x < 32) {
+    const uint32_t mask = stage_of(P, l).sources;
+    bool ok = true;
+    for (int s = 0; s < A.num_ready && ok; ++s)
+      if ((mask >> s) & 1u) {
+        StreamSync w = A.ss;
+        w.layer_ready = A.ready[s];
+        ok = wait_layer_ready(w, static_cast<int>(l + P.shift[s]), threadIdx.x);
+      }
+    if (threadIdx.x == 0) *s_ok = ok ? 1u : 0u;
+  }
+  __syncthreads();
+  return *s_ok != 0;
+}
+
+// kvbm_paged_stage_gather_kernel's unit walk behind the stage gate; unit = (l * num_blocks + pair) * no + o over the layer range,
+// so a batch that crosses a stage boundary gates on the next stage's sources when it enters that layer.
+template <int CAST, bool POW2, bool SCALED>
+__global__ void __launch_bounds__(256, 1)
+kvbm_gated_stage_gather_kernel(const __grid_constant__ StageGatherParams P, const __grid_constant__ GateArgs A, uint32_t num_blocks,
+                               uint32_t layer_begin, uint32_t nlayers, uint32_t no, uint32_t nt, RowSplit r, const float* scales, uint32_t batch)
+{
+  const uint32_t per_layer = num_blocks * no;
+  gated_units(
+      A, per_layer * nlayers, batch, [&](uint32_t u) { return layer_begin + u / per_layer; },
+      [&](uint32_t u, uint32_t l) {
+        const uint32_t rem = u - (l - layer_begin) * per_layer;
+        const uint32_t pair = rem / no;
+        stage_gather_unit<CAST, POW2, SCALED>(P, pair, l, rem - pair * no, no, nt, r, scales);
+      },
+      [&](uint32_t l, uint32_t* s_ok) { return gate_stage_layer(A, P, l, s_ok); });
 }
 
 // The stream-wait form's signal after layer l: its layer-done flag, and after the last layer the done and completion flags.
@@ -1123,6 +1221,8 @@ static cudaError_t preload_kernels()
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_gather_kernel<c, p, sc>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_gather_kernel<c, p, sc, true>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_gather_kernel<c, p, sc, false>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_stage_gather_kernel<c, p, sc>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_stage_gather_kernel<c, p, sc>);
         });
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_layer_signal_kernel);
   return e;
@@ -1199,31 +1299,112 @@ static bool cast_rows(uint32_t src_row_bytes, int cast_mode, uint64_t* dst_row_b
 // window inside both sides' heads and on destination heads no other window writes (two would race), its region page * its
 // heads * row, its strides, and at most max_covered covered heads in all.  Fills P->src, P->covered and, with several sources,
 // the head map P->entry.
+// One source of a gather into a destination of dst_num_heads heads, outer_dim no and strides D: its table, its outer dims, its
+// window inside both sides' heads, its region page * its heads * row and its strides over its own src_nl layers.  Fills *G but
+// G->first.
+static bool fill_gather_source(const kvbm_permute_source& X, uint32_t src_nl, uint32_t dst_num_heads, uint32_t no, uint32_t page_size,
+                               uint32_t src_row_bytes, const PermuteSide& D, GatherSource* G)
+{
+  if (!X.side.block_ids || !X.side.layout.layer_base || X.side.layout.outer_dim != no) return false;
+  if (X.head_count == 0 || static_cast<uint64_t>(X.src_head_begin) + X.head_count > X.num_heads ||
+      static_cast<uint64_t>(X.dst_head_begin) + X.head_count > dst_num_heads)
+    return false;
+  if (static_cast<uint64_t>(page_size) * X.num_heads * src_row_bytes != X.side.layout.region_bytes) return false;
+  if (!fill_permute_side(X.side, src_nl, no, X.num_heads, page_size, src_row_bytes, &G->S)) return false;
+  G->s_win = X.src_head_begin * G->S.head_stride;  // the windows' first heads
+  G->d_win = X.dst_head_begin * D.head_stride;
+  return true;
+}
+
+static bool heads_overlap(const kvbm_permute_source& a, const kvbm_permute_source& b)
+{
+  return a.dst_head_begin < b.dst_head_begin + b.head_count && b.dst_head_begin < a.dst_head_begin + a.head_count;
+}
+
 static bool fill_gather_sources(const kvbm_permute_source* srcs, int num_srcs, uint32_t dst_num_heads, uint32_t nl, uint32_t no,
                                 uint32_t page_size, uint32_t src_row_bytes, uint32_t max_covered, GatherParams* P)
 {
   uint32_t covered = 0;
   for (int s = 0; s < num_srcs; ++s) {
     const kvbm_permute_source& X = srcs[s];
-    if (!X.side.block_ids || !X.side.layout.layer_base || X.side.layout.num_layers != nl || X.side.layout.outer_dim != no) return false;
-    if (X.head_count == 0 || static_cast<uint64_t>(X.src_head_begin) + X.head_count > X.num_heads ||
-        static_cast<uint64_t>(X.dst_head_begin) + X.head_count > dst_num_heads)
-      return false;
+    if (X.side.layout.num_layers != nl) return false;
     for (int t = 0; t < s; ++t)
-      if (X.dst_head_begin < srcs[t].dst_head_begin + srcs[t].head_count && srcs[t].dst_head_begin < X.dst_head_begin + X.head_count)
-        return false;
-    if (static_cast<uint64_t>(page_size) * X.num_heads * src_row_bytes != X.side.layout.region_bytes) return false;
+      if (heads_overlap(X, srcs[t])) return false;
     GatherSource& G = P->src[s];
-    if (!fill_permute_side(X.side, nl, no, X.num_heads, page_size, src_row_bytes, &G.S)) return false;
+    if (!fill_gather_source(X, nl, dst_num_heads, no, page_size, src_row_bytes, P->D, &G)) return false;
     if (static_cast<uint64_t>(covered) + X.head_count > max_covered) return false;
-    G.s_win = X.src_head_begin * G.S.head_stride;  // the windows' first heads
-    G.d_win = X.dst_head_begin * P->D.head_stride;
     G.first = covered;
     if (num_srcs > 1)
       for (uint32_t j = 0; j < X.head_count; ++j) P->entry[covered + j] = static_cast<uint8_t>(s);
     covered += X.head_count;
   }
   P->covered = covered;
+  return true;
+}
+
+// The sources of a staged gather into P->g.D (nl layers, dst_num_heads heads) over destination layers [lb, le): each layer window
+// non-empty and inside its source's own layers and the destination's; two windows equal (one stage) or disjoint in the
+// destination; the stages covering every layer of [lb, le); within a stage, windows on destination heads no other window of the
+// stage writes; every rule of fill_gather_source; at most KVBM_GATHER_MAX_HEADS covered heads over all stages.  Fills P->g's
+// sources and one head map, stage by stage in ascending destination layers, P->stage and P->shift; *widest: the most heads of
+// one stage.
+static bool fill_stage_sources(const kvbm_stage_source* srcs, int num_srcs, uint32_t dst_num_heads, uint32_t nl, uint32_t no, int lb, int le,
+                               uint32_t page_size, uint32_t src_row_bytes, StageGatherParams* P, uint32_t* widest)
+{
+  int stage_of_src[KVBM_GATHER_MAX_SOURCES];
+  int num_stages = 0;
+  GatherStage* T = P->stage;
+  for (int s = 0; s < num_srcs; ++s) {
+    const kvbm_stage_source& X = srcs[s];
+    const uint64_t src_end = static_cast<uint64_t>(X.src_layer_begin) + X.layer_count, dst_end = static_cast<uint64_t>(X.dst_layer_begin) + X.layer_count;
+    if (X.layer_count == 0 || src_end > X.src.side.layout.num_layers || dst_end > nl) return false;
+    int k = 0;
+    while (k < num_stages && !(T[k].begin == X.dst_layer_begin && T[k].end == dst_end)) {
+      if (X.dst_layer_begin < T[k].end && T[k].begin < dst_end) return false;  // a partial overlap
+      ++k;
+    }
+    if (k == num_stages) T[num_stages++] = GatherStage{X.dst_layer_begin, static_cast<uint32_t>(dst_end), 0, 0, 0};
+    stage_of_src[s] = k;
+    for (int t = 0; t < s; ++t)
+      if (stage_of_src[t] == k && heads_overlap(X.src, srcs[t].src)) return false;
+    T[k].sources |= 1u << s;
+    P->shift[s] = X.src_layer_begin - X.dst_layer_begin;
+  }
+  // ascending destination layers (insertion sort of at most 16), then the range must be tiled
+  int order[KVBM_GATHER_MAX_SOURCES];
+  for (int k = 0; k < num_stages; ++k) {
+    int at = k;
+    while (at > 0 && T[order[at - 1]].begin > T[k].begin) {
+      order[at] = order[at - 1];
+      --at;
+    }
+    order[at] = k;
+  }
+  uint32_t reached = static_cast<uint32_t>(lb);
+  for (int i = 0; i < num_stages; ++i)
+    if (T[order[i]].begin <= reached && T[order[i]].end > reached) reached = T[order[i]].end;
+  if (reached < static_cast<uint32_t>(le)) return false;
+  GatherStage sorted[KVBM_GATHER_MAX_SOURCES] = {};
+  uint32_t covered = 0;
+  *widest = 0;
+  for (int i = 0; i < num_stages; ++i) {
+    GatherStage& S = sorted[i] = T[order[i]];
+    S.first = covered;
+    for (int s = 0; s < num_srcs; ++s) {
+      if (!((S.sources >> s) & 1u)) continue;
+      const kvbm_permute_source& X = srcs[s].src;
+      GatherSource& G = P->g.src[s];
+      if (!fill_gather_source(X, X.side.layout.num_layers, dst_num_heads, no, page_size, src_row_bytes, P->g.D, &G)) return false;
+      if (static_cast<uint64_t>(covered) + X.head_count > KVBM_GATHER_MAX_HEADS) return false;
+      G.first = covered;
+      for (uint32_t j = 0; j < X.head_count; ++j) P->g.entry[covered + j] = static_cast<uint8_t>(s);
+      covered += X.head_count;
+    }
+    S.count = covered - S.first;
+    *widest = std::max(*widest, S.count);
+  }
+  std::copy(sorted, sorted + KVBM_GATHER_MAX_SOURCES, T);
+  P->g.covered = covered;
   return true;
 }
 
@@ -1305,10 +1486,11 @@ static cudaError_t gate_args(const kvbm_permute_stream& st, int num_srcs, uint32
 // The spinning form: launch_gated(A, ctas, batch) launches the gated kernel, which writes every flag itself.  The stream-wait
 // form: per layer, the stream waits for every source's flag (cuStreamWaitValue32, GEQ: the cyclic order of epoch_reached),
 // launch_layer(l) moves the layer unsignalled, and one signal launch writes its layer-done flag, plus the done and completion
-// flags after the last layer.  Nothing resident spins.
+// flags after the last layer.  Nothing resident spins.  staged: a staged gather's stages, whose stream-wait form waits per layer
+// for only the flags of that layer's stage, each source's at its own layer.
 template <class Layer, class Gated>
 static cudaError_t launch_streamed(const kvbm_permute_stream& st, int num_srcs, uint32_t nl, int layer_begin, int layer_end, uint64_t units,
-                                   cudaStream_t stream, Layer&& launch_layer, Gated&& launch_gated)
+                                   cudaStream_t stream, Layer&& launch_layer, Gated&& launch_gated, const StageGatherParams* staged = nullptr)
 {
   cudaError_t e;
   const int form = gate_form(st, &e);
@@ -1322,8 +1504,12 @@ static cudaError_t launch_streamed(const kvbm_permute_stream& st, int num_srcs, 
     return launched(stream);
   }
   for (int l = layer_begin; l < layer_end; ++l) {
-    for (int s = 0; s < num_srcs; ++s)
-      if (g_wait32(stream, reinterpret_cast<unsigned long long>(st.layer_ready_flags[s] + l), st.epoch, 0) != 0) return cudaErrorUnknown;
+    const uint32_t mask = staged ? stage_of(*staged, static_cast<uint32_t>(l)).sources : ~0u;
+    for (int s = 0; s < num_srcs; ++s) {
+      if (!((mask >> s) & 1u)) continue;
+      const uint32_t* flag = st.layer_ready_flags[s] + (staged ? static_cast<uint32_t>(l) + staged->shift[s] : static_cast<uint32_t>(l));
+      if (g_wait32(stream, reinterpret_cast<unsigned long long>(flag), st.epoch, 0) != 0) return cudaErrorUnknown;
+    }
     if ((e = launch_layer(l)) != cudaSuccess) return e;
     const bool last = l + 1 == layer_end;
     uint32_t* done = last ? st.done_flag : nullptr;
@@ -1341,12 +1527,13 @@ static cudaError_t launch_streamed(const kvbm_permute_stream& st, int num_srcs, 
 // when there is nothing to move, and launches kvbm_paged_permute_kernel for one source (the faster of the two, DESIGN §4.2b) or
 // kvbm_paged_gather_kernel for several.  max_covered: how many destination heads the sources may cover together; at most
 // KVBM_GATHER_MAX_HEADS (the gather's head map) whenever num_srcs > 1.  st: a streamed launch (its flags are the ones passed),
-// which takes the gated gather kernel, or per layer this launch unstreamed.
+// which takes the gated gather kernel, or per layer this launch unstreamed.  staged: the same sources with layer windows
+// (srcs[s] is staged[s].src), a staged gather checked by fill_stage_sources, which takes the stage gather kernels.
 static cudaError_t launch_paged_permute(const kvbm_permute_source* srcs, int num_srcs, const kvbm_permute_side* dst, uint32_t dst_num_heads,
                                         int num_blocks, int layer_begin, int layer_end, uint32_t page_size, uint32_t src_row_bytes,
                                         int cast_mode, const float* cast_scales, uint32_t* done_flag, uint32_t epoch,
                                         uint32_t* completion_flag, uint32_t completion_value, uint32_t max_covered, cudaStream_t stream,
-                                        const kvbm_permute_stream* st = nullptr)
+                                        const kvbm_permute_stream* st = nullptr, const kvbm_stage_source* staged = nullptr)
 {
   if (num_blocks < 0 || layer_begin < 0 || layer_end < layer_begin) return cudaErrorInvalidValue;
   if (!cast_args_ok(cast_mode, cast_scales)) return cudaErrorInvalidValue;
@@ -1360,13 +1547,17 @@ static cudaError_t launch_paged_permute(const kvbm_permute_source* srcs, int num
   RowSplit r;
   if (page_size == 0 || !row_split(walk_row, page_size, &r)) return cudaErrorInvalidValue;
   if (static_cast<uint64_t>(page_size) * dst_num_heads * dst_row_bytes != dst->layout.region_bytes) return cudaErrorInvalidValue;
-  GatherParams P{};
+  StageGatherParams SP{};
+  GatherParams& P = SP.g;
   if (!fill_permute_side(*dst, nl, no, dst_num_heads, page_size, static_cast<uint32_t>(dst_row_bytes), &P.D)) return cudaErrorInvalidValue;
-  if (!fill_gather_sources(srcs, num_srcs, dst_num_heads, nl, no, page_size, src_row_bytes, max_covered, &P)) return cudaErrorInvalidValue;
+  uint32_t widest = 0;
+  if (staged ? !fill_stage_sources(staged, num_srcs, dst_num_heads, nl, no, layer_begin, layer_end, page_size, src_row_bytes, &SP, &widest)
+             : !fill_gather_sources(srcs, num_srcs, dst_num_heads, nl, no, page_size, src_row_bytes, max_covered, &P))
+    return cudaErrorInvalidValue;
   const uint32_t covered = P.covered;
   const uint64_t units = static_cast<uint64_t>(num_blocks) * (layer_end - layer_begin) * no;
   if (units >= (1ull << 31)) return cudaErrorInvalidValue;
-  const int threads = static_cast<int>(std::min<uint32_t>(8, covered)) * 32;
+  const int threads = static_cast<int>(std::min<uint32_t>(8, staged ? widest : covered)) * 32;
   const unsigned grid = static_cast<unsigned>(units);
   const uint32_t lb = static_cast<uint32_t>(layer_begin), nlay = static_cast<uint32_t>(layer_end - layer_begin);
   if (st)
@@ -1374,17 +1565,24 @@ static cudaError_t launch_paged_permute(const kvbm_permute_source* srcs, int num
         *st, num_srcs, nl, layer_begin, layer_end, units, stream,
         [&](int l) {
           return launch_paged_permute(srcs, num_srcs, dst, dst_num_heads, num_blocks, l, l + 1, page_size, src_row_bytes, cast_mode,
-                                      cast_scales, nullptr, 0, nullptr, 0, max_covered, stream);
+                                      cast_scales, nullptr, 0, nullptr, 0, max_covered, stream, nullptr, staged);
         },
         [&](const GateArgs& A, unsigned ctas, uint32_t batch) {
           with_walk_kernel(cast_mode, r.pow2, cast_scales != nullptr, [&](auto c, auto p, auto sc) {
-            kvbm_gated_gather_kernel<c, p, sc><<<ctas, threads, 0, stream>>>(P, A, static_cast<uint32_t>(num_blocks), lb, nlay, no, page_size,
-                                                                             r, cast_scales, batch);
+            if (staged)
+              kvbm_gated_stage_gather_kernel<c, p, sc><<<ctas, threads, 0, stream>>>(SP, A, static_cast<uint32_t>(num_blocks), lb, nlay, no,
+                                                                                     page_size, r, cast_scales, batch);
+            else
+              kvbm_gated_gather_kernel<c, p, sc><<<ctas, threads, 0, stream>>>(P, A, static_cast<uint32_t>(num_blocks), lb, nlay, no, page_size,
+                                                                               r, cast_scales, batch);
           });
-        });
+        },
+        staged ? &SP : nullptr);
   with_walk_kernel(cast_mode, r.pow2, cast_scales != nullptr, [&](auto c, auto p, auto sc) {
     const GatherSource& G = P.src[0];
-    if (num_srcs == 1)
+    if (staged)
+      kvbm_paged_stage_gather_kernel<c, p, sc><<<grid, threads, 0, stream>>>(SP, lb, nlay, no, page_size, r, cast_scales);
+    else if (num_srcs == 1)
       kvbm_paged_permute_kernel<c, p, sc><<<grid, threads, 0, stream>>>(G.S, P.D, lb, nlay, no, covered, page_size, r, G.s_win, G.d_win, cast_scales);
     else
       kvbm_paged_gather_kernel<c, p, sc><<<grid, threads, 0, stream>>>(P, lb, nlay, no, page_size, r, cast_scales);
@@ -1718,6 +1916,48 @@ kvbm_kernels_paged_permute_gather_streamed(const kvbm_permute_source* srcs, int 
   return launch_paged_permute(srcs, num_srcs, dst, dst_num_heads, num_blocks, layer_begin, layer_end, page_size, src_row_bytes, cast_mode,
                               cast_scales, st->done_flag, st->epoch, st->completion_flag, st->completion_value, KVBM_GATHER_MAX_HEADS, stream,
                               st);
+}
+
+// The staged gather's entries: the gather's launch path with layer windows, or with none when every window is the identity over
+// the destination's layers (a PP1 plan), which is then exactly kvbm_kernels_paged_permute_gather_scaled / _streamed.
+static cudaError_t launch_stage_gather(const kvbm_stage_source* srcs, int num_srcs, const kvbm_permute_side* dst, uint32_t dst_num_heads,
+                                       int num_blocks, int layer_begin, int layer_end, uint32_t page_size, uint32_t src_row_bytes,
+                                       int cast_mode, const float* cast_scales, uint32_t* done_flag, uint32_t epoch,
+                                       uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream,
+                                       const kvbm_permute_stream* st = nullptr)
+{
+  if (!srcs || num_srcs < 1 || num_srcs > KVBM_GATHER_MAX_SOURCES) return cudaErrorInvalidValue;
+  kvbm_permute_source plain[KVBM_GATHER_MAX_SOURCES];
+  bool identity = dst != nullptr;
+  for (int s = 0; s < num_srcs; ++s) {
+    const kvbm_stage_source& X = srcs[s];
+    plain[s] = X.src;
+    identity = identity && X.src_layer_begin == 0 && X.dst_layer_begin == 0 && X.layer_count == dst->layout.num_layers &&
+               X.src.side.layout.num_layers == dst->layout.num_layers;
+  }
+  return launch_paged_permute(plain, num_srcs, dst, dst_num_heads, num_blocks, layer_begin, layer_end, page_size, src_row_bytes, cast_mode,
+                              cast_scales, done_flag, epoch, completion_flag, completion_value, KVBM_GATHER_MAX_HEADS, stream, st,
+                              identity ? nullptr : srcs);
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_stage_gather(const kvbm_stage_source* srcs, int num_srcs, const kvbm_permute_side* dst, uint32_t dst_num_heads,
+                                int num_blocks, int layer_begin, int layer_end, uint32_t page_size, uint32_t src_row_bytes, int cast_mode,
+                                const float* cast_scales, uint32_t* done_flag, uint32_t epoch, uint32_t* completion_flag,
+                                uint32_t completion_value, cudaStream_t stream)
+{
+  return launch_stage_gather(srcs, num_srcs, dst, dst_num_heads, num_blocks, layer_begin, layer_end, page_size, src_row_bytes, cast_mode,
+                             cast_scales, done_flag, epoch, completion_flag, completion_value, stream);
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_stage_gather_streamed(const kvbm_stage_source* srcs, int num_srcs, const kvbm_permute_side* dst, uint32_t dst_num_heads,
+                                         int num_blocks, int layer_begin, int layer_end, uint32_t page_size, uint32_t src_row_bytes,
+                                         int cast_mode, const float* cast_scales, const kvbm_permute_stream* st, cudaStream_t stream)
+{
+  if (!stream_args_ok(st, num_srcs)) return cudaErrorInvalidValue;
+  return launch_stage_gather(srcs, num_srcs, dst, dst_num_heads, num_blocks, layer_begin, layer_end, page_size, src_row_bytes, cast_mode,
+                             cast_scales, st->done_flag, st->epoch, st->completion_flag, st->completion_value, stream, st);
 }
 
 extern "C" cudaError_t

@@ -104,6 +104,12 @@ class PermuteSource(C.Structure):
                 ("head_count", C.c_uint32)]
 
 
+class StageSource(C.Structure):
+    """struct kvbm_stage_source: one source of `paged_stage_gather` (a gather source whose side has the pool's own num_layers,
+    and its layer window: source layers [src_layer_begin, +layer_count) land as destination layers [dst_layer_begin, +layer_count))"""
+    _fields_ = [("src", PermuteSource), ("src_layer_begin", C.c_uint32), ("dst_layer_begin", C.c_uint32), ("layer_count", C.c_uint32)]
+
+
 GATHER_MAX_SOURCES = 16      # KVBM_GATHER_MAX_SOURCES
 GATHER_MAX_HEADS = 256       # KVBM_GATHER_MAX_HEADS
 
@@ -207,6 +213,12 @@ def lib() -> C.CDLL:
                                                                 C.c_uint32, C.c_uint32, C.c_uint32, i, i, C.c_uint32, i, vp,
                                                                 C.POINTER(PermuteStream), vp]
         L.kvbm_kernels_paged_repage_gather_streamed.restype = i
+        L.kvbm_kernels_paged_stage_gather.argtypes = [C.POINTER(StageSource), i, C.POINTER(PermuteSide), C.c_uint32, i, i, i, C.c_uint32,
+                                                      C.c_uint32, i, vp, vp, C.c_uint32, vp, C.c_uint32, vp]
+        L.kvbm_kernels_paged_stage_gather.restype = i
+        L.kvbm_kernels_paged_stage_gather_streamed.argtypes = [C.POINTER(StageSource), i, C.POINTER(PermuteSide), C.c_uint32, i, i, i,
+                                                               C.c_uint32, C.c_uint32, i, vp, C.POINTER(PermuteStream), vp]
+        L.kvbm_kernels_paged_stage_gather_streamed.restype = i
         L.kvbm_kernels_permute_strides.argtypes = [i, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64, C.c_uint64,
                                                    C.POINTER(C.c_uint64)]
         L.kvbm_kernels_permute_strides.restype = i
@@ -231,7 +243,7 @@ EXPORTED_SYMBOLS = [
     "kvbm_kernels_permute_strides", "kvbm_kernels_paged_permute_cast", "kvbm_kernels_paged_permute_heads",
     "kvbm_kernels_paged_permute_gather", "kvbm_kernels_paged_permute_heads_scaled", "kvbm_kernels_paged_permute_gather_scaled",
     "kvbm_kernels_paged_repage", "kvbm_kernels_paged_repage_gather", "kvbm_kernels_paged_permute_gather_streamed",
-    "kvbm_kernels_paged_repage_gather_streamed",
+    "kvbm_kernels_paged_repage_gather_streamed", "kvbm_kernels_paged_stage_gather", "kvbm_kernels_paged_stage_gather_streamed",
 ]
 
 
@@ -404,6 +416,30 @@ def paged_repage_gather_streamed(srcs: Sequence[PermuteSource], src_page_size: i
     return lib().kvbm_kernels_paged_repage_gather_streamed(arr, len(srcs), src_page_size, C.byref(dst), dst_num_heads, dst_page_size,
                                                            token_begin, token_end, layer_begin, layer_end, src_row_bytes, int(cast_mode),
                                                            scales_ptr(cast_scales), C.byref(st) if st is not None else None, stream)
+
+
+def paged_stage_gather(srcs: Sequence[StageSource], dst: PermuteSide, dst_num_heads: int, num_blocks: int, layer_begin: int,
+                       layer_end: int, page_size: int, src_row_bytes: int, cast_mode: int = 0, cast_scales=None, done_flag: int = 0,
+                       epoch: int = 0, completion_flag: int = 0, completion_value: int = 0, stream: int = 0) -> int:
+    """`paged_permute_gather` with a layer window per source, in ONE launch (a decode rank assembling its layers and heads from a
+    PP x TP prefill group): sources with equal destination layer windows form a stage, and every destination layer of
+    [layer_begin, layer_end) takes the head windows of its stage, each read at the source's own layer.  `cast_scales` is indexed
+    by the destination layer.  include/kvbm_kernels.h (kvbm_kernels_paged_stage_gather)."""
+    arr = (StageSource * max(1, len(srcs)))(*srcs)
+    return lib().kvbm_kernels_paged_stage_gather(arr, len(srcs), C.byref(dst), dst_num_heads, num_blocks, layer_begin, layer_end, page_size,
+                                                 src_row_bytes, int(cast_mode), scales_ptr(cast_scales), done_flag or None, epoch,
+                                                 completion_flag or None, completion_value, stream)
+
+
+def paged_stage_gather_streamed(srcs: Sequence[StageSource], dst: PermuteSide, dst_num_heads: int, num_blocks: int, layer_begin: int,
+                                layer_end: int, page_size: int, src_row_bytes: int, cast_mode: int, cast_scales,
+                                st: Optional[PermuteStream], stream: int = 0) -> int:
+    """`paged_stage_gather` streamed layer by layer: `st.layer_ready_flags[s]` is source s's array over its own layers, and a
+    destination layer waits only for the sources of its stage.  include/kvbm_kernels.h (kvbm_kernels_paged_stage_gather_streamed)."""
+    arr = (StageSource * max(1, len(srcs)))(*srcs)
+    return lib().kvbm_kernels_paged_stage_gather_streamed(arr, len(srcs), C.byref(dst), dst_num_heads, num_blocks, layer_begin, layer_end,
+                                                          page_size, src_row_bytes, int(cast_mode), scales_ptr(cast_scales),
+                                                          C.byref(st) if st is not None else None, stream)
 
 
 def permute_strides(kv_layout: int, num_layers: int, outer_dim: int, num_heads: int, page_size: int, row_bytes: int,

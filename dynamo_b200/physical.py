@@ -118,6 +118,11 @@ class _CHeadWindow(C.Structure):
     _fields_ = [(n, C.c_size_t) for n in ("src_rank", "src_head_begin", "dst_head_begin", "head_count")]
 
 
+class _CShardWindow(C.Structure):
+    _fields_ = [(n, C.c_size_t) for n in ("src_rank", "src_layer_begin", "dst_layer_begin", "layer_count", "src_head_begin",
+                                          "dst_head_begin", "head_count")]
+
+
 class _CLayerStream(C.Structure):
     """struct kvbm_layer_stream"""
     _fields_ = [("src_layer_ready_flags", C.c_void_p), ("num_srcs", C.c_size_t), ("layer_done_flags", C.c_void_p)]
@@ -237,6 +242,7 @@ EXPORTED_SYMBOLS = [
     "kvbm_mc_group_size", "kvbm_mc_group_add_device", "kvbm_mc_group_bind_local", "kvbm_mc_group_bind_addr", "kvbm_mc_group_map",
     "kvbm_mc_group_destroy", "kvbm_tp_reshard_plan", "kvbm_manager_execute_gather", "kvbm_manager_execute_repage",
     "kvbm_manager_execute_repage_gather", "kvbm_manager_execute_gather_streamed", "kvbm_manager_execute_repage_gather_streamed",
+    "kvbm_tp_pp_reshard_plan", "kvbm_manager_execute_stage_gather",
 ]
 
 
@@ -292,6 +298,9 @@ def lib() -> C.CDLL:
                                                            P(_COptions), P(u64)]
         L.kvbm_manager_execute_repage_gather_streamed.argtypes = [vp, sz, P(u64), P(P(sz)), sz, u64, vp, sz, sz, sz, P(_CHeadWindow), sz,
                                                                   P(_CLayerStream), P(_COptions), P(u64)]
+        L.kvbm_tp_pp_reshard_plan.argtypes = [sz, sz, sz, sz, P(sz), sz, sz, P(sz), sz, P(_CShardWindow), sz, P(sz)]
+        L.kvbm_manager_execute_stage_gather.argtypes = [vp, sz, P(u64), P(P(sz)), u64, vp, sz, P(_CShardWindow), sz, P(_CLayerStream),
+                                                        P(_COptions), P(u64)]
         L.kvbm_notification_is_complete.argtypes = [vp, u64]
         L.kvbm_notification_wait.argtypes = [vp, u64, C.c_int64]
         L.kvbm_manager_bytes_moved.argtypes = [vp]
@@ -424,6 +433,42 @@ def tp_reshard_plan(num_kv_heads: int, src_tp: int, dst_tp: int, dst_rank: int) 
     out = (_CHeadWindow * max(1, n.value))()
     _check(lib().kvbm_tp_reshard_plan(num_kv_heads, src_tp, dst_tp, dst_rank, out, n.value, C.byref(n)))
     return [HeadWindow(w.src_rank, w.src_head_begin, w.dst_head_begin, w.head_count) for w in out[:n.value]]
+
+
+@dataclass(frozen=True)
+class ShardWindow:
+    """One entry of a PP x TP re-shard plan: heads [src_head_begin, +head_count) of layers [src_layer_begin, +layer_count) of
+    source rank src_rank's blocks are heads [dst_head_begin, +head_count) of layers [dst_layer_begin, +layer_count) of the decode
+    rank's blocks.  Layers are stage-local on each side (a pool's layer 0 is its stage's first layer), heads rank-local."""
+    src_rank: int
+    src_layer_begin: int
+    dst_layer_begin: int
+    layer_count: int
+    src_head_begin: int
+    dst_head_begin: int
+    head_count: int
+
+
+def tp_pp_reshard_plan(num_kv_heads: int, num_layers: int, src_tp: int, src_pp: int, dst_tp: int, dst_pp: int, dst_rank: int,
+                       src_stage_layers: Optional[Sequence[int]] = None,
+                       dst_stage_layers: Optional[Sequence[int]] = None) -> List[ShardWindow]:
+    """Which source rank supplies which layers and heads of decode rank `dst_rank` (kvbm_tp_pp_reshard_plan,
+    include/kvbm_physical.h): ranks are pp_rank * tp + tp_rank on both sides; `*_stage_layers` are each stage's layer counts
+    (None: an even split, which needs num_layers % pp == 0); for each source stage that shares layers with the decode rank's
+    stage, `tp_reshard_plan`'s head windows over the shared layers, in ascending destination layer, then head order."""
+    def parts(v):
+        return None if v is None else (C.c_size_t * max(1, len(v)))(*[int(x) for x in v])
+    sp, dp = parts(src_stage_layers), parts(dst_stage_layers)
+    for v, pp in ((src_stage_layers, src_pp), (dst_stage_layers, dst_pp)):
+        if v is not None and len(v) != pp:
+            raise ValueError(f"{len(v)} stage layer counts for PP {pp}")
+    n = C.c_size_t()
+    args = (num_kv_heads, num_layers, src_tp, src_pp, sp, dst_tp, dst_pp, dp, dst_rank)
+    _check(lib().kvbm_tp_pp_reshard_plan(*args, None, 0, C.byref(n)))
+    out = (_CShardWindow * max(1, n.value))()
+    _check(lib().kvbm_tp_pp_reshard_plan(*args, out, n.value, C.byref(n)))
+    return [ShardWindow(w.src_rank, w.src_layer_begin, w.dst_layer_begin, w.layer_count, w.src_head_begin, w.dst_head_begin, w.head_count)
+            for w in out[:n.value]]
 
 
 class TransferCompleteNotification:
@@ -675,6 +720,25 @@ class TransferManager:
         o = (options or TransferOptions())._c()
         _check(lib().kvbm_manager_execute_gather_streamed(self._h, len(ranks), hs, sp, dst, d, n, ws, len(plan), C.byref(ls), C.byref(o),
                                                           C.byref(tok)))
+        return TransferCompleteNotification(self, tok.value)
+
+    def execute_stage_gather(self, sources: Mapping[int, tuple], dst: int, dst_block_ids: Sequence[int], plan: Sequence[ShardWindow],
+                             options: Optional[TransferOptions] = None, ready_flags: Optional[Mapping[int, int]] = None,
+                             layer_done_flags: int = 0) -> TransferCompleteNotification:
+        """A PP x TP re-shard's assembly as ONE hand-off (kvbm_manager_execute_stage_gather): `execute_gather` with a layer window
+        per plan entry (`tp_pp_reshard_plan`), each source pool holding only its stage's layers.  `sources` maps a source rank to
+        (layout handle, block ids), as `execute_gather`.  The options' layer range and cast scales count destination layers.
+        `ready_flags` (None: not streamed) maps a source rank to the address of the u32 ready flags over ITS OWN layers, as
+        `execute_gather_streamed`; a destination layer waits only for its stage's sources.  `layer_done_flags`: the destination's."""
+        ranks, (hs, _keep, sp, d, n, _ws) = self._gather_call(sources, dst_block_ids, plan)
+        index = {r: i for i, r in enumerate(ranks)}
+        ws = (_CShardWindow * max(1, len(plan)))(*[_CShardWindow(index[w.src_rank], w.src_layer_begin, w.dst_layer_begin, w.layer_count,
+                                                                 w.src_head_begin, w.dst_head_begin, w.head_count) for w in plan])
+        ls = self._layer_stream(ranks, ready_flags, layer_done_flags) if ready_flags is not None else None
+        tok = C.c_uint64()
+        o = (options or TransferOptions())._c()
+        _check(lib().kvbm_manager_execute_stage_gather(self._h, len(ranks), hs, sp, dst, d, n, ws, len(plan),
+                                                       C.byref(ls) if ls is not None else None, C.byref(o), C.byref(tok)))
         return TransferCompleteNotification(self, tok.value)
 
     def execute_repage(self, src: int, src_block_ids: Sequence[int], dst: int, dst_block_ids: Sequence[int], tokens: range,

@@ -384,6 +384,44 @@ cudaError_t kvbm_kernels_paged_repage_gather_streamed(const kvbm_permute_source*
                                                       uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
                                                       const kvbm_permute_stream* st, cudaStream_t stream);
 
+/* ---- the staged gather: a pipeline-parallel re-shard ------------------------------------------------------------------------
+ * One source of kvbm_kernels_paged_stage_gather: a gather source (its side with the source pool's OWN layout.num_layers, head
+ * count and head window) plus a layer window: source layers [src_layer_begin, src_layer_begin + layer_count) land as destination
+ * layers [dst_layer_begin, dst_layer_begin + layer_count).  A prefill engine with pipeline parallelism has one pool per stage,
+ * holding only that stage's layers; its layer 0 is the stage's first layer. */
+typedef struct kvbm_stage_source {
+  kvbm_permute_source src;
+  uint32_t src_layer_begin, dst_layer_begin, layer_count;
+} kvbm_stage_source;
+
+/* kvbm_kernels_paged_permute_gather_scaled with a layer window per source (a decode rank assembling its layers and heads from a
+ * PP x TP prefill group) in ONE launch, then one signal launch.  Sources whose layer windows are equal in the destination form a
+ * stage; for every destination layer l of [layer_begin, layer_end) and every source s of l's stage, head src_head_begin + j of
+ * srcs[s] at source layer l - dst_layer_begin + src_layer_begin lands as head dst_head_begin + j at destination layer l,
+ * re-ordered and cast as kvbm_kernels_paged_permute_heads_scaled would, with the same bits.  Every other destination byte keeps
+ * its value.  cast_scales (nullable): one float[dst num_layers * outer_dim] array indexed by the DESTINATION layer and outer index.
+ * cudaErrorInvalidValue, before any CUDA call, for: num_srcs outside 1..KVBM_GATHER_MAX_SOURCES; layer_count == 0 or a window past
+ * its source's num_layers or the destination's; two layer windows that overlap in the destination without being equal; a
+ * destination layer of [layer_begin, layer_end) that no stage covers (stages may extend past the range); two head windows of one
+ * stage that overlap in the destination (those of different stages may); more than KVBM_GATHER_MAX_HEADS covered heads counted
+ * over all stages; and every other rule of kvbm_kernels_paged_permute_gather_scaled but the equal layer counts (outer_dim,
+ * page_size, rows, cast, strides are shared by all sources).  An empty block or layer range moves nothing and still signals.
+ * When every window is the identity over a source whose num_layers is the destination's, this is
+ * kvbm_kernels_paged_permute_gather_scaled. */
+cudaError_t kvbm_kernels_paged_stage_gather(const kvbm_stage_source* srcs, int num_srcs, const kvbm_permute_side* dst,
+                                            uint32_t dst_num_heads, int num_blocks, int layer_begin, int layer_end, uint32_t page_size,
+                                            uint32_t src_row_bytes, int cast_mode, const float* cast_scales, uint32_t* done_flag,
+                                            uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream);
+
+/* kvbm_kernels_paged_stage_gather streamed as kvbm_kernels_paged_permute_gather_streamed is, with these flag conventions:
+ * st->layer_ready_flags[s] is source s's array over ITS OWN layers ([srcs[s].src.side.layout.num_layers]), and a unit of
+ * destination layer l waits only for the sources of l's stage, each at its own layer; layer_done_flags and sync_workspace are the
+ * destination's ([dst num_layers]).  The argument rules are kvbm_kernels_paged_stage_gather's plus the gate's. */
+cudaError_t kvbm_kernels_paged_stage_gather_streamed(const kvbm_stage_source* srcs, int num_srcs, const kvbm_permute_side* dst,
+                                                     uint32_t dst_num_heads, int num_blocks, int layer_begin, int layer_end,
+                                                     uint32_t page_size, uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
+                                                     const kvbm_permute_stream* st, cudaStream_t stream);
+
 /* Host-only (no GPU): the stride table kvbm_kernels_paged_permute walks with for one side.  out[0] = 1 when offsets count
  * from the block's first byte (universal formats) or 0 when they count from the (layer, outer) region's first byte; the
  * element (layer l, outer o, head h, token t) then sits at  [out[0] ? l * out[1] + o * out[2] : 0] + h * out[3] + t * out[4].

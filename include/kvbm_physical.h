@@ -177,6 +177,27 @@ typedef struct kvbm_head_window {
 int kvbm_tp_reshard_plan(size_t num_kv_heads, size_t src_tp, size_t dst_tp, size_t dst_rank, kvbm_head_window* out, size_t cap,
                          size_t* n_out);
 
+/* One entry of a pipeline- and tensor-parallel re-shard plan: heads [src_head_begin, +head_count) of layers [src_layer_begin,
+ * +layer_count) of source rank src_rank's blocks are heads [dst_head_begin, +head_count) of layers [dst_layer_begin,
+ * +layer_count) of the decode rank's blocks.  Layers are stage-local on each side (layer 0 of a pool is the first layer of its
+ * pipeline stage), heads rank-local. */
+typedef struct kvbm_shard_window {
+  size_t src_rank, src_layer_begin, dst_layer_begin, layer_count, src_head_begin, dst_head_begin, head_count;
+} kvbm_shard_window;
+/* Which source rank supplies which layers and heads of decode rank dst_rank when num_layers layers of num_kv_heads KV heads are
+ * split over src_pp pipeline stages of src_tp ranks on the source side and dst_pp x dst_tp on the destination side.  Ranks are
+ * numbered pp_rank * tp + tp_rank on both sides.  src_stage_layers / dst_stage_layers: each stage's layer count ([pp] entries,
+ * ascending stages); NULL splits evenly, which needs num_layers % pp == 0.  For each source stage that shares layers with the
+ * decode rank's stage, the plan holds kvbm_tp_reshard_plan's head windows of that pair of TP degrees (its ownership and replica
+ * rule, for tp rank dst_rank % dst_tp) over the shared layers, in ascending destination layer, then destination head order.
+ * With src_pp = dst_pp = 1 it is kvbm_tp_reshard_plan's plan over every layer.  Errors: KVBM_ERR a null n_out or a cap below the
+ * count (out == NULL only counts); KVBM_ERR_CONFIG a zero argument, num_layers % pp != 0 with a NULL partition, a partition with
+ * a zero stage or that does not sum to num_layers, and kvbm_tp_reshard_plan's head rule; KVBM_ERR_RANGE dst_rank >= dst_pp *
+ * dst_tp.  Pure host logic. */
+int kvbm_tp_pp_reshard_plan(size_t num_kv_heads, size_t num_layers, size_t src_tp, size_t src_pp, const size_t* src_stage_layers,
+                            size_t dst_tp, size_t dst_pp, const size_t* dst_stage_layers, size_t dst_rank, kvbm_shard_window* out,
+                            size_t cap, size_t* n_out);
+
 /* ---- TransferManager ---- */
 /* cuda_device_id < 0: host-only manager (Memcpy strategy only; every CUDA strategy returns KVBM_ERR_CUDA). */
 int kvbm_manager_create(int cuda_device_id, uint64_t worker_id, kvbm_transfer_manager** out);
@@ -354,6 +375,26 @@ int kvbm_manager_execute_gather_streamed(kvbm_transfer_manager* m, size_t num_sr
                                          const size_t* const* src_ids, kvbm_layout_handle dst, const size_t* dst_ids, size_t n,
                                          const kvbm_head_window* windows, size_t num_windows, const kvbm_layer_stream* ls,
                                          const kvbm_transfer_options* opts, kvbm_notification* out);
+
+/* A PP x TP re-shard's assembly as ONE hand-off: kvbm_manager_execute_gather with a layer window per window (a
+ * kvbm_tp_pp_reshard_plan passes as it is; windows[j].src_rank indexes srcs / src_ids).  Heads [src_head_begin, +head_count) of
+ * layers [src_layer_begin, +layer_count) of block src_ids[src_rank][i] land as heads [dst_head_begin, +head_count) of layers
+ * [dst_layer_begin, +layer_count) of block dst_ids[i]; every other destination byte keeps its value.  Windows with equal
+ * destination layer windows form a stage.  The options' layer range counts destination layers, and so do cast_scales
+ * ([dst num_layers * outer_dim]).  ls (nullable): streamed as kvbm_manager_execute_gather_streamed, ls->src_layer_ready_flags[s]
+ * being source s's array over its own layers and layer_done_flags the destination's.  Errors, first one wins: with ls, its shape
+ * as kvbm_manager_execute_gather_streamed; execute_gather's window checks, except that only windows of one stage may not
+ * share a destination head, plus KVBM_ERR_RANGE a window without layers and KVBM_ERR_OVERLAP two layer windows that partly
+ * overlap in the destination; KVBM_ERR_HANDLE an unknown handle; KVBM_ERR_RANGE a layer window past its source's or the
+ * destination's num_layers, or a destination layer of the range that no window covers; each (source, destination) pair's checks
+ * of execute_gather with the same codes and texts, except the equal layer counts; an empty block or layer range then returns
+ * KVBM_OK with nothing launched; with ls,
+ * its flags' reachability.  One upload, one kvbm_kernels_paged_stage_gather launch, one notification; bytes_moved counts each
+ * window's destination bytes over its layers inside the range. */
+int kvbm_manager_execute_stage_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs,
+                                      const size_t* const* src_ids, kvbm_layout_handle dst, const size_t* dst_ids, size_t n,
+                                      const kvbm_shard_window* windows, size_t num_windows, const kvbm_layer_stream* ls,
+                                      const kvbm_transfer_options* opts, kvbm_notification* out);
 
 /* kvbm_manager_execute_repage_gather, streamed as kvbm_manager_execute_gather_streamed is; one window over every head of both
  * sides streams a plain re-page.  Validation is execute_repage_gather's, with the same additions. */
