@@ -657,10 +657,10 @@ static int launch_cuda(kvbm_transfer_manager* m, Layout* S, Layout* const* D, in
   return KVBM_OK;
 }
 
-// A request as resolve() validated it: its layouts and effective formats (the options override a layout's own), whether it
-// takes the permuting launch and with which head window (the whole source unless the request names one), the layer range, the
-// strategy plan and a two-hop plan's bounce layout.  `empty`: nothing to move (no blocks or an empty layer range); nothing
-// after the layer range is resolved then.
+// A request as resolve() (or the re-paging checks) validated it: its layouts and effective formats (the options override a
+// layout's own), whether it takes the permuting launch and with which head window (the whole source unless the request names
+// one), the layer range, the strategy plan and a two-hop plan's bounce layout.  `empty`: nothing to move (no blocks or an empty
+// layer range); nothing after the layer range is resolved then.
 struct Transfer {
   Layout* S = nullptr;
   Layout* D[KVBM_MAX_DESTINATIONS] = {};
@@ -673,13 +673,13 @@ struct Transfer {
   bool empty = false;
 };
 
-// The gate of a streamed launch: window j reads source ranks[j], so it waits for that source's flags; the options' epoch, gate
-// mode, timeout, CTA cap and done flag; the slot's workspace and completion word.
-static kvbm_permute_stream layer_stream(const kvbm_layer_stream& ls, const size_t* ranks, size_t nw, const kvbm_transfer_options& o,
+// The gate of a streamed launch: window j reads source e[j].window.src_rank, so it waits for that source's flags; the options'
+// epoch, gate mode, timeout, CTA cap and done flag; the slot's workspace and completion word.
+static kvbm_permute_stream layer_stream(const kvbm_layer_stream& ls, const Transfer* e, size_t nw, const kvbm_transfer_options& o,
                                         const Slot& sl, uint64_t seq)
 {
   kvbm_permute_stream st{};
-  for (size_t j = 0; j < nw; ++j) st.layer_ready_flags[j] = ls.src_layer_ready_flags[ranks[j]];
+  for (size_t j = 0; j < nw; ++j) st.layer_ready_flags[j] = ls.src_layer_ready_flags[e[j].window.src_rank];
   st.layer_done_flags = ls.layer_done_flags;
   st.done_flag = o.done_flag;
   st.epoch = o.epoch;
@@ -692,100 +692,133 @@ static kvbm_permute_stream layer_stream(const kvbm_layer_stream& ls, const size_
   return st;
 }
 
-// The layout-transforming transfer: what select_transform_kernel's result would drive if the reference ran it inside
-// execute_transfer (it rejects the pair instead, transfer/mod.rs:128-147).  One permuting launch moves every entry's head window
-// from source e[j].window.src_rank into e[0].D over e[0]'s layer range, with the transfer's fp8 <-> bf16 cast fused in:
-// kvbm_kernels_paged_permute_heads for one window (any head count), kvbm_kernels_paged_permute_gather for several.  Block
-// tables: source s at s * n and the destination's at num_srcs * n, no pointer tables; the completion word is written by a
-// trailing signal kernel.
-// ls: a streamed gather (execute_gather_streamed), one kvbm_kernels_paged_permute_gather_streamed launch gated on every window's
-// source flags, with the slot's workspace staged for the destination's layers.
-// layers: a staged gather (execute_stage_gather), window j with the layer window of layers[j], one kvbm_kernels_paged_stage_gather
-// launch (or its streamed form with ls); each window's bytes count over its layers inside the layer range.
-static int launch_permute(kvbm_transfer_manager* m, const Transfer* e, size_t nw, size_t num_srcs, const size_t* const* src_ids,
-                          const size_t* dst_ids, size_t n, const kvbm_transfer_options& o, cudaStream_t stream, uint64_t* seq_out,
-                          const kvbm_layer_stream* ls = nullptr, const kvbm_shard_window* layers = nullptr)
+static int checked(cudaError_t e, const char* what) { return e == cudaSuccess ? KVBM_OK : fail_cuda(e, what); }
+
+// The launch every layout-transforming hand-off ends with, on `stream`.  One slot takes the block tables [source 0 ..
+// num_srcs - 1 (n_src ids each), destination (n_dst ids)] and, with ls, a workspace over the destination's layers.  Window j
+// becomes the kvbm_permute_source of e[j]'s source and head window, reading table e[j].window.src_rank; the destination's side
+// is e[0]'s; with ls, the gate.  `launch(sources, destination, gate or null, slot, seq)` makes the kernel call and returns its
+// code.  Then the slot counts `bytes`, *seq_out gets the launch's sequence number and *out the notification: 0 on a caller
+// stream, whose caller manages sync.
+template <class Launch>
+static int launch_transform(kvbm_transfer_manager* m, const Transfer* e, size_t nw, size_t num_srcs, const size_t* const* src_ids,
+                            size_t n_src, const size_t* dst_ids, size_t n_dst, const kvbm_layer_stream* ls, const kvbm_transfer_options& o,
+                            cudaStream_t stream, uint64_t bytes, uint64_t* seq_out, kvbm_notification* out, Launch&& launch)
 {
-  std::vector<const size_t*> lists(src_ids, src_ids + num_srcs);
-  lists.push_back(dst_ids);
+  // the tables' pointers and lengths fit on the stack for every request that names only the sources its windows read; a
+  // gather may pass any number of sources
+  const size_t k = num_srcs + 1;
+  const size_t* stack_lists[KVBM_GATHER_MAX_SOURCES + 1];
+  size_t stack_lens[KVBM_GATHER_MAX_SOURCES + 1];
+  std::vector<const size_t*> heap_lists;
+  std::vector<size_t> heap_lens;
+  const size_t** lists = stack_lists;
+  size_t* lens = stack_lens;
+  if (k > KVBM_GATHER_MAX_SOURCES + 1) {
+    heap_lists.resize(k);
+    heap_lens.resize(k);
+    lists = heap_lists.data();
+    lens = heap_lens.data();
+  }
+  std::copy(src_ids, src_ids + num_srcs, lists);
+  std::fill(lens, lens + num_srcs, n_src);
+  lists[num_srcs] = dst_ids;
+  lens[num_srcs] = n_dst;
+  const Layout& D = *e[0].D[0];
   Slot* sl;
   uint64_t seq;
-  const Layout *S0 = e[0].S, *D = e[0].D[0];
-  int rc = stage_ids(m, lists.data(), lists.size(), n, ls ? D->cfg.num_layers + 4 : 4, stream, nullptr, &sl, &seq);
+  int rc = stage_ids(m, lists, lens, k, ls ? D.cfg.num_layers + 4 : 4, stream, nullptr, &sl, &seq);
   if (rc) return rc;
-  kvbm_permute_side pd{descriptor(*D), sl->dev_ids + num_srcs * n, e[0].dst_kv};
+  const kvbm_permute_side kd{descriptor(D), sl->dev_ids + num_srcs * n_src, e[0].dst_kv};
   kvbm_permute_source ks[KVBM_GATHER_MAX_SOURCES] = {};
-  size_t heads = 0;
   for (size_t j = 0; j < nw; ++j) {
     const kvbm_head_window& w = e[j].window;
-    ks[j] = kvbm_permute_source{{descriptor(*e[j].S), sl->dev_ids + w.src_rank * n, e[j].src_kv}, static_cast<uint32_t>(e[j].S->cfg.num_heads),
+    ks[j] = kvbm_permute_source{{descriptor(*e[j].S), sl->dev_ids + w.src_rank * n_src, e[j].src_kv}, static_cast<uint32_t>(e[j].S->cfg.num_heads),
                                 static_cast<uint32_t>(w.src_head_begin), static_cast<uint32_t>(w.dst_head_begin),
                                 static_cast<uint32_t>(w.head_count)};
-    heads += w.head_count;
   }
-  const uint32_t dnh = static_cast<uint32_t>(D->cfg.num_heads), page = static_cast<uint32_t>(S0->cfg.page_size);
-  const uint32_t row = static_cast<uint32_t>(S0->cfg.inner_dim / S0->cfg.num_heads * S0->cfg.dtype_width_bytes);
-  const int nb = static_cast<int>(n), lb = static_cast<int>(e[0].lb), le = static_cast<int>(e[0].le);
-  if (layers) {
-    kvbm_stage_source ss[KVBM_GATHER_MAX_SOURCES] = {};
-    uint64_t bytes = 0;
-    for (size_t j = 0; j < nw; ++j) {
-      const kvbm_shard_window& w = layers[j];
-      ss[j] = kvbm_stage_source{ks[j], static_cast<uint32_t>(w.src_layer_begin), static_cast<uint32_t>(w.dst_layer_begin),
-                                static_cast<uint32_t>(w.layer_count)};
-      const size_t from = std::max(e[0].lb, w.dst_layer_begin), to = std::min(e[0].le, w.dst_layer_begin + w.layer_count);
-      if (to > from) bytes += n * (to - from) * S0->cfg.outer_dim * (D->region / D->cfg.num_heads * w.head_count);
-    }
-    cudaError_t ce;
-    if (ls) {
-      size_t ranks[KVBM_GATHER_MAX_SOURCES];
-      for (size_t j = 0; j < nw; ++j) ranks[j] = e[j].window.src_rank;
-      const kvbm_permute_stream st = layer_stream(*ls, ranks, nw, o, *sl, seq);
-      ce = kvbm_kernels_paged_stage_gather_streamed(ss, static_cast<int>(nw), &pd, dnh, nb, lb, le, page, row, o.cast_mode, o.cast_scales, &st,
-                                                    stream);
-      if (ce != cudaSuccess) return fail_cuda(ce, "kvbm_kernels_paged_stage_gather_streamed");
-    } else {
-      ce = kvbm_kernels_paged_stage_gather(ss, static_cast<int>(nw), &pd, dnh, nb, lb, le, page, row, o.cast_mode, o.cast_scales, o.done_flag,
-                                           o.epoch, sl->host_flag, static_cast<uint32_t>(seq), stream);
-      if (ce != cudaSuccess) return fail_cuda(ce, "kvbm_kernels_paged_stage_gather");
-    }
-    if ((rc = finish_slot(m, sl, stream, bytes))) return rc;
-    *seq_out = seq;
-    return KVBM_OK;
-  }
-  if (ls) {
-    size_t ranks[KVBM_GATHER_MAX_SOURCES];
-    for (size_t j = 0; j < nw; ++j) ranks[j] = e[j].window.src_rank;
-    const kvbm_permute_stream st = layer_stream(*ls, ranks, nw, o, *sl, seq);
-    cudaError_t ce = kvbm_kernels_paged_permute_gather_streamed(ks, static_cast<int>(nw), &pd, dnh, nb, lb, le, page, row, o.cast_mode,
-                                                                o.cast_scales, &st, stream);
-    if (ce != cudaSuccess) return fail_cuda(ce, "kvbm_kernels_paged_permute_gather_streamed");
-  } else if (nw == 1) {
-    const kvbm_permute_source& k = ks[0];
-    cudaError_t ce = kvbm_kernels_paged_permute_heads_scaled(&k.side, &pd, nb, lb, le, k.num_heads, k.src_head_begin, dnh, k.dst_head_begin,
-                                                             k.head_count, page, row, o.cast_mode, o.cast_scales, o.done_flag, o.epoch,
-                                                             sl->host_flag, static_cast<uint32_t>(seq), stream);
-    if (ce != cudaSuccess) return fail_cuda(ce, "kvbm_kernels_paged_permute_heads_scaled");
-  } else {
-    cudaError_t ce = kvbm_kernels_paged_permute_gather_scaled(ks, static_cast<int>(nw), &pd, dnh, nb, lb, le, page, row, o.cast_mode,
-                                                              o.cast_scales, o.done_flag, o.epoch, sl->host_flag, static_cast<uint32_t>(seq), stream);
-    if (ce != cudaSuccess) return fail_cuda(ce, "kvbm_kernels_paged_permute_gather_scaled");
-  }
-  if ((rc = finish_slot(m, sl, stream, n * (e[0].le - e[0].lb) * S0->cfg.outer_dim * (D->region / D->cfg.num_heads * heads)))) return rc;
-  *seq_out = seq;
+  kvbm_permute_stream st{};
+  if (ls) st = layer_stream(*ls, e, nw, o, *sl, seq);
+  if ((rc = launch(ks, kd, ls ? &st : nullptr, *sl, seq))) return rc;
+  if ((rc = finish_slot(m, sl, stream, bytes))) return rc;
+  if (seq_out) *seq_out = seq;
+  if (out) *out = o.use_caller_stream ? 0 : seq;
   return KVBM_OK;
 }
 
-// The cast kernels read the scales on the manager's device: its own device memory, or pinned host memory mapped into its address
-// space.  Anything else (pageable host memory, another GPU's memory) must not reach a kernel.
-static int check_cast_scales(kvbm_transfer_manager* m, const float* p)
+// The layout-transforming transfer: what select_transform_kernel's result would drive if the reference ran it inside
+// execute_transfer (it rejects the pair instead, transfer/mod.rs:128-147).  One permuting launch moves every entry's head window
+// from source e[j].window.src_rank into e[0].D over e[0]'s layer range, with the transfer's fp8 <-> bf16 cast fused in:
+// kvbm_kernels_paged_permute_heads for one window (any head count), kvbm_kernels_paged_permute_gather for several, and
+// kvbm_kernels_paged_permute_gather_streamed with ls (gated on every window's source flags).  Every source list and the
+// destination's hold n ids; the completion word is written by a trailing signal kernel.
+// layers: a staged gather, window j with the layer window of layers[j], one kvbm_kernels_paged_stage_gather launch (or its
+// streamed form with ls); each window's bytes count over its layers inside the layer range.
+// *seq_out: the launch's sequence number; *out: the notification, as launch_transform sets them (either may be null).
+static int launch_permute(kvbm_transfer_manager* m, const Transfer* e, size_t nw, size_t num_srcs, const size_t* const* src_ids,
+                          const size_t* dst_ids, size_t n, const kvbm_transfer_options& o, cudaStream_t stream, uint64_t* seq_out,
+                          kvbm_notification* out = nullptr, const kvbm_layer_stream* ls = nullptr, const kvbm_shard_window* layers = nullptr)
+{
+  const Layout *S0 = e[0].S, *D = e[0].D[0];
+  uint64_t bytes = 0;
+  for (size_t j = 0; j < nw; ++j) {
+    size_t from = e[0].lb, to = e[0].le;
+    if (layers) {
+      from = std::max(from, layers[j].dst_layer_begin);
+      to = std::min(to, layers[j].dst_layer_begin + layers[j].layer_count);
+    }
+    if (to > from) bytes += n * (to - from) * S0->cfg.outer_dim * (D->region / D->cfg.num_heads * e[j].window.head_count);
+  }
+  const uint32_t dnh = static_cast<uint32_t>(D->cfg.num_heads), page = static_cast<uint32_t>(S0->cfg.page_size);
+  const uint32_t row = static_cast<uint32_t>(S0->cfg.inner_dim / S0->cfg.num_heads * S0->cfg.dtype_width_bytes);
+  const int nb = static_cast<int>(n), lb = static_cast<int>(e[0].lb), le = static_cast<int>(e[0].le), k = static_cast<int>(nw);
+  auto launch = [&](const kvbm_permute_source* ks, const kvbm_permute_side& kd, const kvbm_permute_stream* st, const Slot& sl, uint64_t seq) {
+    const uint32_t value = static_cast<uint32_t>(seq);
+    if (layers) {
+      kvbm_stage_source ss[KVBM_GATHER_MAX_SOURCES] = {};
+      for (size_t j = 0; j < nw; ++j)
+        ss[j] = kvbm_stage_source{ks[j], static_cast<uint32_t>(layers[j].src_layer_begin), static_cast<uint32_t>(layers[j].dst_layer_begin),
+                                  static_cast<uint32_t>(layers[j].layer_count)};
+      if (st)
+        return checked(kvbm_kernels_paged_stage_gather_streamed(ss, k, &kd, dnh, nb, lb, le, page, row, o.cast_mode, o.cast_scales, st, stream),
+                       "kvbm_kernels_paged_stage_gather_streamed");
+      return checked(kvbm_kernels_paged_stage_gather(ss, k, &kd, dnh, nb, lb, le, page, row, o.cast_mode, o.cast_scales, o.done_flag, o.epoch,
+                                                     sl.host_flag, value, stream),
+                     "kvbm_kernels_paged_stage_gather");
+    }
+    if (st)
+      return checked(kvbm_kernels_paged_permute_gather_streamed(ks, k, &kd, dnh, nb, lb, le, page, row, o.cast_mode, o.cast_scales, st, stream),
+                     "kvbm_kernels_paged_permute_gather_streamed");
+    if (nw == 1)
+      return checked(kvbm_kernels_paged_permute_heads_scaled(&ks[0].side, &kd, nb, lb, le, ks[0].num_heads, ks[0].src_head_begin, dnh,
+                                                             ks[0].dst_head_begin, ks[0].head_count, page, row, o.cast_mode, o.cast_scales,
+                                                             o.done_flag, o.epoch, sl.host_flag, value, stream),
+                     "kvbm_kernels_paged_permute_heads_scaled");
+    return checked(kvbm_kernels_paged_permute_gather_scaled(ks, k, &kd, dnh, nb, lb, le, page, row, o.cast_mode, o.cast_scales, o.done_flag,
+                                                            o.epoch, sl.host_flag, value, stream),
+                   "kvbm_kernels_paged_permute_gather_scaled");
+  };
+  return launch_transform(m, e, nw, num_srcs, src_ids, n, dst_ids, n, ls, o, stream, bytes, seq_out, out, launch);
+}
+
+// Whether kernels on the manager's device can use p: its own device memory, pinned host memory mapped into its address space,
+// or, with `peers`, memory of a device it has peer access to (enabled through kvbm_manager_enable_peer_access, or by an IPC
+// mapping this manager opened).  Pageable host memory and any other device's memory cannot be.
+static bool reachable(const kvbm_transfer_manager* m, const void* p, bool peers)
 {
   cudaPointerAttributes a{};
-  const cudaError_t e = cudaPointerGetAttributes(&a, p);
-  if (e != cudaSuccess) (void)cudaGetLastError();
-  const bool ok = e == cudaSuccess && ((a.type == cudaMemoryTypeDevice && a.device == m->device) ||
-                                       (a.type == cudaMemoryTypeHost && a.devicePointer == static_cast<const void*>(p)));
-  if (!ok)
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+    (void)cudaGetLastError();
+    return false;
+  }
+  if (a.type == cudaMemoryTypeHost) return a.devicePointer == p;
+  return a.type == cudaMemoryTypeDevice && (a.device == m->device || (peers && m->peers.count(a.device) != 0));
+}
+
+// The cast kernels read the scales on the manager's device, never through a peer.
+static int check_cast_scales(kvbm_transfer_manager* m, const float* p)
+{
+  if (!reachable(m, p, false))
     return fail(KVBM_ERR, "cast_scales must be device memory of device " + std::to_string(m->device) +
                               " or pinned host memory mapped into it (a pageable or another device's pointer cannot be read by the cast)");
   return KVBM_OK;
@@ -803,28 +836,17 @@ static int check_layer_stream_shape(const kvbm_layer_stream* ls, size_t num_srcs
   return KVBM_OK;
 }
 
-// The flags of a streamed request are polled and written by the kernels on the manager's device: its own device memory, memory of
-// a device it has peer access to (enabled through kvbm_manager_enable_peer_access, or by an IPC mapping this manager opened) or
-// pinned host memory mapped into its address space.  Anything else (pageable host memory, a device without enabled peer access)
-// must not reach a kernel.
-static int check_layer_stream_flags(kvbm_transfer_manager* m, const kvbm_layer_stream& ls, const size_t* ranks, size_t nw)
+// The flags of a streamed request are polled and written by the kernels on the manager's device, which may reach them through
+// a peer: the ready flags of every window's source (e[j].window.src_rank) and the layer done flags.
+static int check_layer_stream_flags(kvbm_transfer_manager* m, const kvbm_layer_stream& ls, const Transfer* e, size_t nw)
 {
-  auto reachable = [&](const void* p) {
-    cudaPointerAttributes a{};
-    const cudaError_t e = cudaPointerGetAttributes(&a, p);
-    if (e != cudaSuccess) {
-      (void)cudaGetLastError();
-      return false;
-    }
-    if (a.type == cudaMemoryTypeHost) return a.devicePointer == p;
-    if (a.type != cudaMemoryTypeDevice) return false;
-    return a.device == m->device || m->peers.count(a.device) != 0;
-  };
-  for (size_t j = 0; j < nw; ++j)
-    if (!reachable(ls.src_layer_ready_flags[ranks[j]]))
-      return fail(KVBM_ERR, "the layer ready flags of source " + std::to_string(ranks[j]) + " are not reachable from device " +
+  for (size_t j = 0; j < nw; ++j) {
+    const size_t r = e[j].window.src_rank;
+    if (!reachable(m, ls.src_layer_ready_flags[r], true))
+      return fail(KVBM_ERR, "the layer ready flags of source " + std::to_string(r) + " are not reachable from device " +
                                 std::to_string(m->device) + " (its own memory, a device it has peer access to, or mapped pinned host memory)");
-  if (ls.layer_done_flags && !reachable(ls.layer_done_flags))
+  }
+  if (ls.layer_done_flags && !reachable(m, ls.layer_done_flags, true))
     return fail(KVBM_ERR, "the layer done flags are not reachable from device " + std::to_string(m->device) +
                               " (its own memory, a device it has peer access to, or mapped pinned host memory)");
   return KVBM_OK;
@@ -1014,6 +1036,30 @@ static int check_strategy(kvbm_transfer_manager* m, int nd, const kvbm_transfer_
   return KVBM_OK;
 }
 
+// The options' layer range over the layers of `c` (filled into *lb / *le) and enough fp8 KV-cache scales: one per (layer, outer)
+// of those layers, for the fp8 side of a cast.  `c` is the pool whose layers the range counts: the destination's for a staged
+// gather, the source's otherwise.
+static int check_layer_range(const kvbm_layout_config& c, const kvbm_transfer_options& o, size_t* lb, size_t* le)
+{
+  *lb = 0;
+  *le = c.num_layers;
+  if (o.has_layer_range) {
+    *lb = o.layer_begin;
+    *le = o.layer_end;
+    if (*lb > *le || *le > c.num_layers)
+      return fail(KVBM_ERR_RANGE, "Layer range " + std::to_string(*lb) + ".." + std::to_string(*le) + " exceeds num_layers " +
+                                      std::to_string(c.num_layers));
+  }
+  if (o.cast_scales) {
+    if (o.cast_mode == KVBM_CAST_NONE) return fail(KVBM_ERR, "cast_scales need a cast_mode: they scale the fp8 side of a cast");
+    const size_t need = c.num_layers * c.outer_dim;
+    if (o.num_cast_scales < need)
+      return fail(KVBM_ERR_RANGE, "cast_scales holds " + std::to_string(o.num_cast_scales) + " scales, the pools need num_layers * outer_dim = " +
+                                      std::to_string(need));
+  }
+  return KVBM_OK;
+}
+
 // Validate one request and resolve it into *t; the caller holds m->mu.  `heads`: a head window that always takes the permuting
 // launch (a gather's).  Without it the options' window applies, and one over every head of both sides is the transfer without a
 // window.  A request that fails several checks reports the first in the order below.  staged: a staged gather's window, whose
@@ -1065,23 +1111,7 @@ static int resolve(kvbm_transfer_manager* m, kvbm_layout_handle src_h, int nd, c
   }
   t->dst_kv = o.dst_kv_layout ? o.dst_kv_layout : t->D[0]->kv_block_layout;
   t->window = window ? w : kvbm_head_window{0, 0, 0, S->cfg.num_heads};  // a plain transform is the window over every head
-  const size_t nl = staged ? t->D[0]->cfg.num_layers : S->cfg.num_layers;
-  t->lb = 0;
-  t->le = nl;
-  if (o.has_layer_range) {
-    t->lb = o.layer_begin;
-    t->le = o.layer_end;
-    if (t->lb > t->le || t->le > nl)
-      return fail(KVBM_ERR_RANGE, "Layer range " + std::to_string(t->lb) + ".." + std::to_string(t->le) + " exceeds num_layers " +
-                                      std::to_string(nl));
-  }
-  if (o.cast_scales) {  // fp8 KV-cache scales: one per (layer, outer) of the pools, for the fp8 side of a cast
-    if (o.cast_mode == KVBM_CAST_NONE) return fail(KVBM_ERR, "cast_scales need a cast_mode: they scale the fp8 side of a cast");
-    const size_t need = nl * S->cfg.outer_dim;
-    if (o.num_cast_scales < need)
-      return fail(KVBM_ERR_RANGE, "cast_scales holds " + std::to_string(o.num_cast_scales) + " scales, the pools need num_layers * outer_dim = " +
-                                      std::to_string(need));
-  }
+  if (int rc = check_layer_range(staged ? t->D[0]->cfg : S->cfg, o, &t->lb, &t->le)) return rc;
   t->empty = n == 0 || t->lb == t->le;
   if (t->empty) return KVBM_OK;
 
@@ -1172,60 +1202,12 @@ static int check_gather_windows(size_t num_srcs, const kvbm_layout_handle* srcs,
   return KVBM_OK;
 }
 
-// A TP re-shard's assembly as one hand-off: every window is validated as the windowed execute_transfer of its (source,
-// destination) pair, then one kvbm_kernels_paged_permute_gather launch moves all of them and one signal launch writes the
-// done flag and the completion word after the last byte landed.
-// ls: the streamed gather, checked as above and then for its flags, launched gated on them.
-static int execute_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, const size_t* const* src_ids,
-                          kvbm_layout_handle dst_h, const size_t* dst_ids, size_t n, const kvbm_head_window* windows, size_t nw,
-                          const kvbm_transfer_options* opts_in, kvbm_notification* out, const kvbm_layer_stream* ls = nullptr)
+// What a staged gather checks of its layer windows once the windows passed check_gather_windows, under the manager's lock:
+// the destination's handle, each layer window inside its source's and the destination's layers, and every destination layer of
+// the options' range inside some window (KVBM_ERR_RANGE).
+static int check_stage_layers(kvbm_transfer_manager* m, const kvbm_layout_handle* srcs, kvbm_layout_handle dst_h, const kvbm_shard_window* sw,
+                              size_t nw, const kvbm_transfer_options& o)
 {
-  kvbm_transfer_options o{};
-  if (opts_in) o = *opts_in;
-  if (out) *out = 0;
-  if (int rc = check_gather_windows(num_srcs, srcs, windows, nw, o)) return rc;
-  if (n && (!src_ids || !dst_ids)) return fail(KVBM_ERR, "null block id list");
-  std::lock_guard<std::mutex> lk(m->mu);
-  Transfer e[KVBM_GATHER_MAX_SOURCES];
-  for (size_t j = 0; j < nw; ++j) {
-    const size_t* s = src_ids ? src_ids[windows[j].src_rank] : nullptr;
-    int rc = resolve(m, srcs[windows[j].src_rank], 1, &dst_h, &s, &dst_ids, n, o, &windows[j], &e[j]);
-    if (rc) return rc;
-    if (e[j].plan.first != e[0].plan.first) return fail(KVBM_ERR_UNSUPPORTED, "the sources of a gather need the same CUDA strategy");
-  }
-  if (e[0].empty) return KVBM_OK;  // nothing to move (no blocks or an empty layer range), as execute()
-  if (ls) {
-    size_t ranks[KVBM_GATHER_MAX_SOURCES];
-    for (size_t j = 0; j < nw; ++j) ranks[j] = windows[j].src_rank;
-    if (int rc = check_layer_stream_flags(m, *ls, ranks, nw)) return rc;
-  }
-
-  DeviceGuard g(m->device);
-  uint64_t seq;
-  int rc = launch_permute(m, e, nw, num_srcs, src_ids, dst_ids, n, o, pick_stream(m, e[0].plan.first, o), &seq, ls);
-  if (rc) return rc;
-  // caller-provided stream: caller manages sync, completed() is returned, as execute()
-  if (out) *out = o.use_caller_stream ? 0 : seq;
-  return KVBM_OK;
-}
-
-// A PP x TP re-shard's assembly as one hand-off: execute_gather with a layer window per window.  The windows are checked as
-// execute_gather checks them, with head overlaps only within a stage and partly overlapping layer windows rejected; then each
-// layer window inside its source's and the destination's layers, and every destination layer of the range inside some window
-// (KVBM_ERR_RANGE); then each (source, destination) pair as execute_gather's but for the equal layer counts, the options' layer
-// range being the destination's.  One upload, one kvbm_kernels_paged_stage_gather launch, one notification.
-static int execute_stage_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, const size_t* const* src_ids,
-                                kvbm_layout_handle dst_h, const size_t* dst_ids, size_t n, const kvbm_shard_window* sw, size_t nw,
-                                const kvbm_layer_stream* ls, const kvbm_transfer_options* opts_in, kvbm_notification* out)
-{
-  kvbm_transfer_options o{};
-  if (opts_in) o = *opts_in;
-  if (out) *out = 0;
-  std::vector<kvbm_head_window> hw(sw ? nw : 0);
-  for (size_t j = 0; j < hw.size(); ++j) hw[j] = kvbm_head_window{sw[j].src_rank, sw[j].src_head_begin, sw[j].dst_head_begin, sw[j].head_count};
-  if (int rc = check_gather_windows(num_srcs, srcs, sw ? hw.data() : nullptr, nw, o, sw)) return rc;
-  if (n && (!src_ids || !dst_ids)) return fail(KVBM_ERR, "null block id list");
-  std::lock_guard<std::mutex> lk(m->mu);
   const Layout* D = m->find(dst_h);
   if (!D) return fail(KVBM_ERR_HANDLE, "invalid destination handle");
   const size_t dnl = D->cfg.num_layers;
@@ -1248,32 +1230,48 @@ static int execute_stage_gather(kvbm_transfer_manager* m, size_t num_srcs, const
     for (size_t j = 0; j < nw && !in; ++j) in = l >= sw[j].dst_layer_begin && l - sw[j].dst_layer_begin < sw[j].layer_count;
     if (!in) return fail(KVBM_ERR_RANGE, "destination layer " + std::to_string(l) + " of the layer range is in no window's layers");
   }
+  return KVBM_OK;
+}
+
+// A TP re-shard's assembly as one hand-off: every window is validated as the windowed execute_transfer of its (source,
+// destination) pair, then one permuting launch moves all of them and one signal launch writes the done flag and the
+// completion word after the last byte landed.
+// ls: the streamed gather, checked as above and then for its flags, launched gated on them.
+// layers: a PP x TP re-shard's assembly (the staged gather), windows[j] being the head window of layers[j].  The windows are
+// checked with head overlaps only within a stage and partly overlapping layer windows rejected; then check_stage_layers; then
+// each pair as above but for the equal layer counts, the options' layer range being the destination's.
+static int execute_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, const size_t* const* src_ids,
+                          kvbm_layout_handle dst_h, const size_t* dst_ids, size_t n, const kvbm_head_window* windows, size_t nw,
+                          const kvbm_transfer_options* opts_in, kvbm_notification* out, const kvbm_layer_stream* ls = nullptr,
+                          const kvbm_shard_window* layers = nullptr)
+{
+  kvbm_transfer_options o{};
+  if (opts_in) o = *opts_in;
+  if (out) *out = 0;
+  if (int rc = check_gather_windows(num_srcs, srcs, windows, nw, o, layers)) return rc;
+  if (n && (!src_ids || !dst_ids)) return fail(KVBM_ERR, "null block id list");
+  std::lock_guard<std::mutex> lk(m->mu);
+  if (layers)
+    if (int rc = check_stage_layers(m, srcs, dst_h, layers, nw, o)) return rc;
   Transfer e[KVBM_GATHER_MAX_SOURCES];
   for (size_t j = 0; j < nw; ++j) {
-    const size_t* s = src_ids ? src_ids[sw[j].src_rank] : nullptr;
-    int rc = resolve(m, srcs[sw[j].src_rank], 1, &dst_h, &s, &dst_ids, n, o, &hw[j], &e[j], true);
+    const size_t* s = src_ids ? src_ids[windows[j].src_rank] : nullptr;
+    int rc = resolve(m, srcs[windows[j].src_rank], 1, &dst_h, &s, &dst_ids, n, o, &windows[j], &e[j], layers != nullptr);
     if (rc) return rc;
     if (e[j].plan.first != e[0].plan.first) return fail(KVBM_ERR_UNSUPPORTED, "the sources of a gather need the same CUDA strategy");
   }
   if (e[0].empty) return KVBM_OK;  // nothing to move (no blocks or an empty layer range), as execute()
-  if (ls) {
-    size_t ranks[KVBM_GATHER_MAX_SOURCES];
-    for (size_t j = 0; j < nw; ++j) ranks[j] = sw[j].src_rank;
-    if (int rc = check_layer_stream_flags(m, *ls, ranks, nw)) return rc;
-  }
+  if (ls)
+    if (int rc = check_layer_stream_flags(m, *ls, e, nw)) return rc;
 
   DeviceGuard g(m->device);
-  uint64_t seq;
-  int rc = launch_permute(m, e, nw, num_srcs, src_ids, dst_ids, n, o, pick_stream(m, e[0].plan.first, o), &seq, ls, sw);
-  if (rc) return rc;
-  if (out) *out = o.use_caller_stream ? 0 : seq;
-  return KVBM_OK;
+  return launch_permute(m, e, nw, num_srcs, src_ids, dst_ids, n, o, pick_stream(m, e[0].plan.first, o), nullptr, out, ls, layers);
 }
 
 // Blocks a token range [tb, te) touches on a side with pages of `page` tokens: table[tb / page .. ceil(te / page)).
 static size_t repage_blocks(size_t tb, size_t te, size_t page) { return tb == te ? 0 : (te + page - 1) / page - tb / page; }
 
-// The checks of one re-paging (source, destination) pair, in execute_repage's order: both layouts addressable and not both remote,
+// The checks of one re-paging (source, destination) pair, in this order: both layouts addressable and not both remote,
 // the options re-paging takes, named formats (the options override a layout's own; filled into *src_kv / *dst_kv), head counts
 // known and dividing inner_dim, check_compat's head row and cast dtypes, equal num_heads (unless `windows`: a gather's head
 // windows pick the heads, so the counts may differ) and dtypes, pages that divide and the walk's rules.
@@ -1302,31 +1300,6 @@ static int check_repage_pair(const Layout& S, const Layout& D, const kvbm_transf
   return check_walk(S, D, skv, dkv, o.cast_mode);
 }
 
-// The ranges of a re-paging request against its source: the token range within 2^31 tokens, the options' layer range (filled
-// into *lb / *le) and enough cast scales.
-static int check_repage_ranges(const Layout& S, size_t tb, size_t te, const kvbm_transfer_options& o, size_t* lb, size_t* le)
-{
-  if (tb > te || te > (size_t{1} << 31))
-    return fail(KVBM_ERR_RANGE, "Token range " + std::to_string(tb) + ".." + std::to_string(te) + " is reversed or reaches past 2^31 tokens");
-  *lb = 0;
-  *le = S.cfg.num_layers;
-  if (o.has_layer_range) {
-    *lb = o.layer_begin;
-    *le = o.layer_end;
-    if (*lb > *le || *le > S.cfg.num_layers)
-      return fail(KVBM_ERR_RANGE, "Layer range " + std::to_string(*lb) + ".." + std::to_string(*le) + " exceeds num_layers " +
-                                      std::to_string(S.cfg.num_layers));
-  }
-  if (o.cast_scales) {
-    if (o.cast_mode == KVBM_CAST_NONE) return fail(KVBM_ERR, "cast_scales need a cast_mode: they scale the fp8 side of a cast");
-    const size_t need = S.cfg.num_layers * S.cfg.outer_dim;
-    if (o.num_cast_scales < need)
-      return fail(KVBM_ERR_RANGE, "cast_scales holds " + std::to_string(o.num_cast_scales) + " scales, the pools need num_layers * outer_dim = " +
-                                      std::to_string(need));
-  }
-  return KVBM_OK;
-}
-
 // The id counts a token range implies on either side of a re-paging request.
 static int check_repage_counts(size_t tb, size_t te, size_t ps, size_t pd, size_t n_src, size_t n_dst)
 {
@@ -1350,143 +1323,92 @@ static int repage_strategy(kvbm_transfer_manager* m, const Layout& S, const Layo
   return KVBM_OK;
 }
 
-// Re-paging hand-off: tokens [tb, te) of one sequence from the source's block table to the destination's, each side with its own
-// page size, as one kvbm_kernels_paged_repage launch.  Validated on its own (execute() and resolve() assume one page size and
-// equal id counts), in the order below; a request that fails several checks reports the first.
-static int execute_repage(kvbm_transfer_manager* m, kvbm_layout_handle src_h, const size_t* src_ids, size_t n_src, kvbm_layout_handle dst_h,
-                          const size_t* dst_ids, size_t n_dst, size_t tb, size_t te, const kvbm_transfer_options* opts_in, kvbm_notification* out)
-{
-  kvbm_transfer_options o{};
-  if (opts_in) o = *opts_in;
-  if (out) *out = 0;
-  std::lock_guard<std::mutex> lk(m->mu);
-  Layout* S = m->find(src_h);
-  if (!S) return fail(KVBM_ERR_HANDLE, "invalid source handle");
-  Layout* D = m->find(dst_h);
-  if (!D) return fail(KVBM_ERR_HANDLE, "invalid destination handle");
-  int src_kv, dst_kv, rc;
-  size_t lb, le;
-  if ((rc = check_repage_pair(*S, *D, o, false, &src_kv, &dst_kv))) return rc;
-  if ((rc = check_repage_ranges(*S, tb, te, o, &lb, &le))) return rc;
-  const size_t ps = S->cfg.page_size, pd = D->cfg.page_size;
-  if ((rc = check_repage_counts(tb, te, ps, pd, n_src, n_dst))) return rc;
-  if ((n_src && !src_ids) || (n_dst && !dst_ids)) return fail(KVBM_ERR, "null block id list");
-  if ((rc = check_block_ids(src_ids, n_src, dst_ids, n_dst, S->cfg.num_blocks, D->cfg.num_blocks, src_h == dst_h))) return rc;
-  if (tb == te || lb == le) return KVBM_OK;  // nothing to move, as execute()
-  kvbm_transfer_plan p;
-  if ((rc = repage_strategy(m, *S, *D, &p))) return rc;
-  if ((rc = need_cuda_device(m))) return rc;
-  if (o.cast_scales && (rc = check_cast_scales(m, o.cast_scales))) return rc;
-
-  DeviceGuard g(m->device);
-  const cudaStream_t stream = pick_stream(m, p.first, o);
-  const size_t* lists[2] = {src_ids, dst_ids};
-  const size_t lens[2] = {n_src, n_dst};
-  Slot* sl;
-  uint64_t seq;
-  if ((rc = stage_ids(m, lists, lens, 2, 4, stream, nullptr, &sl, &seq))) return rc;
-  const kvbm_permute_side ks{descriptor(*S), sl->dev_ids, src_kv}, kd{descriptor(*D), sl->dev_ids + n_src, dst_kv};
-  const size_t nh = S->cfg.num_heads, row = S->cfg.inner_dim / nh * S->cfg.dtype_width_bytes;
-  cudaError_t ce = kvbm_kernels_paged_repage(&ks, static_cast<uint32_t>(ps), &kd, static_cast<uint32_t>(pd), static_cast<uint32_t>(tb),
-                                             static_cast<uint32_t>(te), static_cast<int>(lb), static_cast<int>(le), static_cast<uint32_t>(nh),
-                                             static_cast<uint32_t>(row), o.cast_mode, o.cast_scales, o.done_flag, o.epoch, sl->host_flag,
-                                             static_cast<uint32_t>(seq), stream);
-  if (ce != cudaSuccess) return fail_cuda(ce, "kvbm_kernels_paged_repage");
-  const size_t d_row = D->cfg.inner_dim / D->cfg.num_heads * D->cfg.dtype_width_bytes;
-  if ((rc = finish_slot(m, sl, stream, (te - tb) * (le - lb) * S->cfg.outer_dim * nh * d_row))) return rc;
-  if (out) *out = o.use_caller_stream ? 0 : seq;
-  return KVBM_OK;
-}
-
-// A TP re-shard's assembly across engines with different page sizes: execute_gather's windows over execute_repage's token range.
-// The windows are checked as execute_gather checks them; the source of every window is then checked against the destination as
-// execute_repage checks its pair (the head counts may differ), with its head window and with one page size for every source.
-// One upload of every source's ids and the destination's, one kvbm_kernels_paged_repage_gather launch and one notification.
+// Re-paging hand-off: tokens [tb, te) of one sequence from the sources' block tables to the destination's, each side with its
+// own page size, as one launch with one notification.  Validated on its own (resolve() assumes one page size and equal id
+// counts), in the order below; a request that fails several checks reports the first.
+// gather: a TP re-shard's assembly across engines with different page sizes (kvbm_manager_execute_repage_gather and its
+// streamed form), execute_gather's windows over the token range.  The windows are checked as execute_gather checks them and
+// the destination's handle is looked up first; every window's source is then checked against the destination as a pair
+// whose head counts may differ, with its head window and with one page size for every source.  Launched through
+// kvbm_kernels_paged_repage_gather, or its streamed form with ls.
+// Otherwise the plain re-page (kvbm_manager_execute_repage): source 0 over every head of both sides, `windows` unused.  Its
+// source's handle is looked up first, its options fail the pair's checks, its head counts must be equal, and it is launched
+// through kvbm_kernels_paged_repage, which has no head limit.
 static int execute_repage_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, const size_t* const* src_ids,
                                  size_t n_src, kvbm_layout_handle dst_h, const size_t* dst_ids, size_t n_dst, size_t tb, size_t te,
                                  const kvbm_head_window* windows, size_t nw, const kvbm_transfer_options* opts_in, kvbm_notification* out,
-                                 const kvbm_layer_stream* ls = nullptr)
+                                 const kvbm_layer_stream* ls = nullptr, bool gather = true)
 {
   kvbm_transfer_options o{};
   if (opts_in) o = *opts_in;
   if (out) *out = 0;
-  if (int rc = check_gather_windows(num_srcs, srcs, windows, nw, o)) return rc;
+  int rc;
+  if (gather && (rc = check_gather_windows(num_srcs, srcs, windows, nw, o))) return rc;
   std::lock_guard<std::mutex> lk(m->mu);
-  Layout* D = m->find(dst_h);
-  if (!D) return fail(KVBM_ERR_HANDLE, "invalid destination handle");
-  Layout* S[KVBM_GATHER_MAX_SOURCES];
-  int src_kv[KVBM_GATHER_MAX_SOURCES], dst_kv = KVBM_KV_UNKNOWN, rc;
+  Layout* D = nullptr;
+  auto find_dst = [&] { return (D = m->find(dst_h)) ? KVBM_OK : fail(KVBM_ERR_HANDLE, "invalid destination handle"); };
+  if (gather && (rc = find_dst())) return rc;  // the plain re-page looks its destination up after its source, in the loop
+  Transfer e[KVBM_GATHER_MAX_SOURCES];
   size_t heads = 0;
   for (size_t j = 0; j < nw; ++j) {
-    const kvbm_head_window& w = windows[j];
-    if (!(S[j] = m->find(srcs[w.src_rank]))) return fail(KVBM_ERR_HANDLE, "invalid source handle");
-    if ((rc = check_repage_pair(*S[j], *D, o, true, &src_kv[j], &dst_kv)) || (rc = check_head_window(*S[j], *D, w, 1))) return rc;
-    if (S[j]->cfg.page_size != S[0]->cfg.page_size)
-      return fail(KVBM_ERR_INCOMPATIBLE, "the sources of a re-paging gather need one page size: source " + std::to_string(windows[0].src_rank) +
-                                             " has " + std::to_string(S[0]->cfg.page_size) + ", source " + std::to_string(w.src_rank) +
-                                             " has " + std::to_string(S[j]->cfg.page_size));
+    Layout* S = e[j].S = m->find(srcs[gather ? windows[j].src_rank : 0]);
+    if (!S) return fail(KVBM_ERR_HANDLE, "invalid source handle");
+    if (!D && (rc = find_dst())) return rc;
+    const kvbm_head_window& w = e[j].window = gather ? windows[j] : kvbm_head_window{0, 0, 0, S->cfg.num_heads};
+    e[j].D[0] = D;
+    if ((rc = check_repage_pair(*S, *D, o, gather, &e[j].src_kv, &e[j].dst_kv)) || (rc = check_head_window(*S, *D, w, 1))) return rc;
+    if (S->cfg.page_size != e[0].S->cfg.page_size)
+      return fail(KVBM_ERR_INCOMPATIBLE, "the sources of a re-paging gather need one page size: source " + std::to_string(e[0].window.src_rank) +
+                                             " has " + std::to_string(e[0].S->cfg.page_size) + ", source " + std::to_string(w.src_rank) +
+                                             " has " + std::to_string(S->cfg.page_size));
     heads += w.head_count;
   }
+  const Layout& S0 = *e[0].S;
+  if (tb > te || te > (size_t{1} << 31))
+    return fail(KVBM_ERR_RANGE, "Token range " + std::to_string(tb) + ".." + std::to_string(te) + " is reversed or reaches past 2^31 tokens");
   size_t lb, le;
-  if ((rc = check_repage_ranges(*S[0], tb, te, o, &lb, &le))) return rc;
-  const size_t ps = S[0]->cfg.page_size, pd = D->cfg.page_size;
+  if ((rc = check_layer_range(S0.cfg, o, &lb, &le))) return rc;
+  const size_t ps = S0.cfg.page_size, pd = D->cfg.page_size;
   if ((rc = check_repage_counts(tb, te, ps, pd, n_src, n_dst))) return rc;
   if ((n_src && !src_ids) || (n_dst && !dst_ids)) return fail(KVBM_ERR, "null block id list");
   for (size_t j = 0; j < nw; ++j) {
-    const size_t* s = n_src ? src_ids[windows[j].src_rank] : nullptr;
+    const size_t r = e[j].window.src_rank;
+    const size_t* s = n_src ? src_ids[r] : nullptr;
     if (n_src && !s) return fail(KVBM_ERR, "null block id list");
-    if ((rc = check_block_ids(s, n_src, dst_ids, n_dst, S[j]->cfg.num_blocks, D->cfg.num_blocks, srcs[windows[j].src_rank] == dst_h))) return rc;
+    if ((rc = check_block_ids(s, n_src, dst_ids, n_dst, e[j].S->cfg.num_blocks, D->cfg.num_blocks, srcs[r] == dst_h))) return rc;
   }
-  if (tb == te || lb == le) return KVBM_OK;  // nothing to move, as execute_repage
-  kvbm_transfer_plan p, p0{};
+  if (tb == te || lb == le) return KVBM_OK;  // nothing to move, as execute()
   for (size_t j = 0; j < nw; ++j) {
-    if ((rc = repage_strategy(m, *S[j], *D, &p))) return rc;
-    if (j && p.first != p0.first) return fail(KVBM_ERR_UNSUPPORTED, "the sources of a gather need the same CUDA strategy");
-    p0 = p;
+    if ((rc = repage_strategy(m, *e[j].S, *D, &e[j].plan))) return rc;
+    if (e[j].plan.first != e[0].plan.first) return fail(KVBM_ERR_UNSUPPORTED, "the sources of a gather need the same CUDA strategy");
   }
   if ((rc = need_cuda_device(m))) return rc;
   if (o.cast_scales && (rc = check_cast_scales(m, o.cast_scales))) return rc;
-  size_t ranks[KVBM_GATHER_MAX_SOURCES];
-  for (size_t j = 0; j < nw; ++j) ranks[j] = windows[j].src_rank;
-  if (ls && (rc = check_layer_stream_flags(m, *ls, ranks, nw))) return rc;
+  if (ls && (rc = check_layer_stream_flags(m, *ls, e, nw))) return rc;
 
   DeviceGuard g(m->device);
-  const cudaStream_t stream = pick_stream(m, p0.first, o);
-  std::vector<const size_t*> lists(src_ids, src_ids + num_srcs);
-  lists.push_back(dst_ids);
-  std::vector<size_t> lens(num_srcs, n_src);
-  lens.push_back(n_dst);
-  Slot* sl;
-  uint64_t seq;
-  if ((rc = stage_ids(m, lists.data(), lens.data(), lists.size(), ls ? D->cfg.num_layers + 4 : 4, stream, nullptr, &sl, &seq))) return rc;
-  const kvbm_permute_side kd{descriptor(*D), sl->dev_ids + num_srcs * n_src, dst_kv};
-  kvbm_permute_source ks[KVBM_GATHER_MAX_SOURCES] = {};
-  for (size_t j = 0; j < nw; ++j) {
-    const kvbm_head_window& w = windows[j];
-    ks[j] = kvbm_permute_source{{descriptor(*S[j]), sl->dev_ids + w.src_rank * n_src, src_kv[j]}, static_cast<uint32_t>(S[j]->cfg.num_heads),
-                                static_cast<uint32_t>(w.src_head_begin), static_cast<uint32_t>(w.dst_head_begin),
-                                static_cast<uint32_t>(w.head_count)};
-  }
-  const size_t row = S[0]->cfg.inner_dim / S[0]->cfg.num_heads * S[0]->cfg.dtype_width_bytes;
-  if (ls) {
-    const kvbm_permute_stream st = layer_stream(*ls, ranks, nw, o, *sl, seq);
-    cudaError_t ce = kvbm_kernels_paged_repage_gather_streamed(ks, static_cast<int>(nw), static_cast<uint32_t>(ps), &kd,
-                                                               static_cast<uint32_t>(D->cfg.num_heads), static_cast<uint32_t>(pd),
-                                                               static_cast<uint32_t>(tb), static_cast<uint32_t>(te), static_cast<int>(lb),
-                                                               static_cast<int>(le), static_cast<uint32_t>(row), o.cast_mode, o.cast_scales, &st,
-                                                               stream);
-    if (ce != cudaSuccess) return fail_cuda(ce, "kvbm_kernels_paged_repage_gather_streamed");
-  } else {
-    cudaError_t ce = kvbm_kernels_paged_repage_gather(ks, static_cast<int>(nw), static_cast<uint32_t>(ps), &kd, static_cast<uint32_t>(D->cfg.num_heads),
-                                                      static_cast<uint32_t>(pd), static_cast<uint32_t>(tb), static_cast<uint32_t>(te),
-                                                      static_cast<int>(lb), static_cast<int>(le), static_cast<uint32_t>(row), o.cast_mode,
-                                                      o.cast_scales, o.done_flag, o.epoch, sl->host_flag, static_cast<uint32_t>(seq), stream);
-    if (ce != cudaSuccess) return fail_cuda(ce, "kvbm_kernels_paged_repage_gather");
-  }
+  const cudaStream_t stream = pick_stream(m, e[0].plan.first, o);
   const size_t d_row = D->cfg.inner_dim / D->cfg.num_heads * D->cfg.dtype_width_bytes;
-  if ((rc = finish_slot(m, sl, stream, (te - tb) * (le - lb) * D->cfg.outer_dim * heads * d_row))) return rc;
-  if (out) *out = o.use_caller_stream ? 0 : seq;
-  return KVBM_OK;
+  const uint32_t row = static_cast<uint32_t>(S0.cfg.inner_dim / S0.cfg.num_heads * S0.cfg.dtype_width_bytes);
+  const uint32_t ups = static_cast<uint32_t>(ps), upd = static_cast<uint32_t>(pd), dnh = static_cast<uint32_t>(D->cfg.num_heads);
+  const uint32_t utb = static_cast<uint32_t>(tb), ute = static_cast<uint32_t>(te);
+  const int ilb = static_cast<int>(lb), ile = static_cast<int>(le), k = static_cast<int>(nw);
+  auto launch = [&](const kvbm_permute_source* ks, const kvbm_permute_side& kd, const kvbm_permute_stream* st, const Slot& sl, uint64_t seq) {
+    const uint32_t value = static_cast<uint32_t>(seq);
+    if (st)
+      return checked(kvbm_kernels_paged_repage_gather_streamed(ks, k, ups, &kd, dnh, upd, utb, ute, ilb, ile, row, o.cast_mode, o.cast_scales,
+                                                               st, stream),
+                     "kvbm_kernels_paged_repage_gather_streamed");
+    if (gather)
+      return checked(kvbm_kernels_paged_repage_gather(ks, k, ups, &kd, dnh, upd, utb, ute, ilb, ile, row, o.cast_mode, o.cast_scales,
+                                                      o.done_flag, o.epoch, sl.host_flag, value, stream),
+                     "kvbm_kernels_paged_repage_gather");
+    return checked(kvbm_kernels_paged_repage(&ks[0].side, ups, &kd, upd, utb, ute, ilb, ile, ks[0].num_heads, row, o.cast_mode, o.cast_scales,
+                                             o.done_flag, o.epoch, sl.host_flag, value, stream),
+                   "kvbm_kernels_paged_repage");
+  };
+  return launch_transform(m, e, nw, num_srcs, src_ids, n_src, dst_ids, n_dst, ls, o, stream, (te - tb) * (le - lb) * D->cfg.outer_dim * heads * d_row,
+                          nullptr, out, launch);
 }
 
 }  // namespace kvbm_host
@@ -2054,7 +1976,8 @@ extern "C" int kvbm_manager_execute_repage(kvbm_transfer_manager* m, kvbm_layout
 {
   return guarded([&]() -> int {
   if (!m) return fail(KVBM_ERR, "null manager");
-  return execute_repage(m, src, src_ids, n_src, dst, dst_ids, n_dst, token_begin, token_end, opts, out);
+  return execute_repage_gather(m, 1, &src, &src_ids, n_src, dst, dst_ids, n_dst, token_begin, token_end, /*windows=*/nullptr, 1, opts, out,
+                               /*ls=*/nullptr, /*gather=*/false);
   });
 }
 
@@ -2092,7 +2015,10 @@ extern "C" int kvbm_manager_execute_stage_gather(kvbm_transfer_manager* m, size_
   if (out) *out = 0;
   if (ls)
     if (int rc = check_layer_stream_shape(ls, num_srcs)) return rc;
-  return execute_stage_gather(m, num_srcs, srcs, src_ids, dst, dst_ids, n, windows, num_windows, ls, opts, out);
+  std::vector<kvbm_head_window> hw(windows ? num_windows : 0);
+  for (size_t j = 0; j < hw.size(); ++j)
+    hw[j] = kvbm_head_window{windows[j].src_rank, windows[j].src_head_begin, windows[j].dst_head_begin, windows[j].head_count};
+  return execute_gather(m, num_srcs, srcs, src_ids, dst, dst_ids, n, windows ? hw.data() : nullptr, num_windows, opts, out, ls, windows);
   });
 }
 
