@@ -13,7 +13,12 @@ and timed with CUDA events (median): the one launch; the two-pass workaround wit
 into a staging pool with page Pd and the source's heads, then kvbm_kernels_paged_permute_gather out of the staging pools), timed
 whole; and the same-page gather of the same bytes from sources that already have page Pd (the rate to approach).  The pages
 default to 8:1 -> 1:16, 4:2 -> 64:16, 2:8 -> 16:64; --pages Ps:Pd overrides them.  Sample destination blocks of every arm are
-compared with tests/repage_gather_oracle.py."""
+compared with tests/repage_gather_oracle.py.
+
+--pp SRC_PP:SRC_TP:DST_TP times kvbm_kernels_paged_stage_repage_gather on a 4k-token Llama-3-70B sequence (80 layers, 8 KV heads
+x 128): decode rank 0 of TP DST_TP (page Pd) from a SRC_PP x SRC_TP prefill group (page Ps, each source pool holding only its
+stage's layers), against the two-pass workaround, the re-paging gather from sources that hold every layer and the same-page
+staged gather (run_pp).  --pages Ps:Pd, default 16:64."""
 import argparse
 import json
 import os
@@ -38,7 +43,9 @@ p.add_argument("--iters", type=int, default=20)
 p.add_argument("--cast", choices=["none", "fp8-to-bf16"], default="none")
 p.add_argument("--only", default=None, help="comma-separated config names to run")
 p.add_argument("--reshard", default=None, help="S:D -- time the re-paging gather from TP S to rank 0 of TP D")
-p.add_argument("--pages", default=None, help="Ps:Pd for --reshard (default: 8:1 1:16, 4:2 64:16, 2:8 16:64)")
+p.add_argument("--pages", default=None, help="Ps:Pd for --reshard (default: 8:1 1:16, 4:2 64:16, 2:8 16:64) or --pp (default 16:64)")
+p.add_argument("--pp", default=None, metavar="SRC_PP:SRC_TP:DST_TP",
+               help="time kvbm_kernels_paged_stage_repage_gather: decode rank 0 of TP DST_TP from a SRC_PP x SRC_TP prefill group")
 a = p.parse_args()
 CAST = K.CastMode.FP8E4M3_TO_BF16 if a.cast == "fp8-to-bf16" else K.CastMode.NONE
 SE, DE = (1, 2) if CAST else (2, 2)
@@ -64,16 +71,16 @@ def card():
 class Pool:
     """A vLLM-style layer-separate pool (block is the second dimension), NHD regions of `page` tokens."""
 
-    def __init__(self, nb, page, no, nh, hd, elem, seed):
-        self.nb, self.page, self.no, self.region = nb, page, no, page * nh * hd * elem
+    def __init__(self, nb, page, no, nh, hd, elem, seed, nl=None):
+        self.nb, self.page, self.no, self.region, self.nl = nb, page, no, page * nh * hd * elem, nl or NL
         g = torch.Generator(device=dev).manual_seed(seed)
-        self.layers = [torch.randint(0, 256, (no * nb * self.region,), dtype=torch.uint8, device=dev, generator=g) for _ in range(NL)]
+        self.layers = [torch.randint(0, 256, (no * nb * self.region,), dtype=torch.uint8, device=dev, generator=g) for _ in range(self.nl)]
         self.base = torch.tensor([t.data_ptr() for t in self.layers], dtype=torch.int64, device=dev)
-        self.desc = K.PagedLayout(self.base.data_ptr(), self.region, nb * self.region, self.region, NL, no, nb)
+        self.desc = K.PagedLayout(self.base.data_ptr(), self.region, nb * self.region, self.region, self.nl, no, nb)
 
     def block(self, b):
         return np.concatenate([self.layers[l][o * self.nb * self.region + b * self.region:][:self.region].cpu().numpy()
-                               for l in range(NL) for o in range(self.no)])
+                               for l in range(self.nl) for o in range(self.no)])
 
 
 def timed(fn, iters=a.iters, warm=3):
@@ -293,7 +300,124 @@ def run_reshard(src_tp, dst_tp, ps, pd, H=8, hd=128, no=2):
               flush=True)
 
 
-if a.reshard:
+def run_pp(src_pp, src_tp, dst_tp, ps, pd, H=8, hd=128, no=2, nl=80):
+    """Decode rank 0 (PP1, TP dst_tp, page pd) of a Llama-3-70B sequence (80 layers, 8 KV heads x 128) from a src_pp x src_tp
+    prefill group (page ps), every source pool holding only its stage's layers.  Arms, alternated within each of 5 rounds of
+    --iters launches (CUDA events): the one launch; the two-pass workaround (the staged gather at ps into a staging pool that
+    holds every decode layer, then kvbm_kernels_paged_repage out of it); the re-paging gather of the same bytes from sources that
+    hold every layer (the ceiling); the staged gather from sources that already have page pd.  Median of the round medians, with
+    their range.  Sample destination blocks of every arm are compared with tests/stage_repage_oracle.py."""
+    from dynamo_b200.physical import tp_pp_reshard_plan, tp_reshard_plan
+    from tests.stage_repage_oracle import stage_repage_gather
+    name = f"pp{src_pp}tp{src_tp}_p{ps}_to_tp{dst_tp}_p{pd}"
+    plan = tp_pp_reshard_plan(H, nl, src_tp, src_pp, dst_tp, 1, 0)
+    ranks = sorted({w.src_rank for w in plan})
+    snh, dnh, snl = max(1, H // src_tp), max(1, H // dst_tp), nl // src_pp
+    tb, te = 0, a.tokens
+    ns, nd = -(-te // ps), -(-te // pd)
+    rng = np.random.default_rng(0)
+    s_row, d_row = hd * SE, hd * DE
+    moved = (te - tb) * nl * no * dnh * hd * (SE + DE)    # bytes read + written: every head of every decode layer
+
+    def side(pool, ids):
+        return K.PermuteSide(pool.desc, ids.data_ptr(), NHD)
+
+    def tables(n_ids):
+        tab = {r: rng.permutation(n_ids + 8)[:n_ids].tolist() for r in ranks}
+        return tab, {r: torch.tensor(tab[r], dtype=torch.int32, device=dev) for r in ranks}
+
+    src = {r: Pool(ns + 8, ps, no, snh, hd, SE, 10 + r, nl=snl) for r in ranks}
+    stab, si = tables(ns)
+    dst = Pool(nd + 8, pd, no, dnh, hd, DE, 2, nl=nl)
+    dtab = rng.permutation(nd + 8)[:nd].tolist()
+    di = torch.tensor(dtab, dtype=torch.int32, device=dev)
+    D = side(dst, di)
+    staged = [K.StageSource(K.PermuteSource(side(src[w.src_rank], si[w.src_rank]), snh, w.src_head_begin, w.dst_head_begin, w.head_count),
+                            w.src_layer_begin, w.dst_layer_begin, w.layer_count) for w in plan]
+
+    def one():
+        K.check(K.paged_stage_repage_gather(staged, ps, D, dnh, pd, tb, te, 0, nl, s_row, int(CAST), stream=sp), "paged_stage_repage_gather")
+
+    # the workaround: the staged gather (with the cast) into a staging pool of page ps over every decode layer, staging block i
+    # holding tokens [i * ps, (i + 1) * ps), then the plain re-page of the staging pool into the destination
+    staging = Pool(ns, ps, no, dnh, hd, DE, 3, nl=nl)
+    ident = torch.arange(ns, dtype=torch.int32, device=dev)
+    st_d = side(staging, ident)
+
+    def two_pass():
+        K.check(K.paged_stage_gather(staged, st_d, dnh, ns, 0, nl, ps, s_row, int(CAST), stream=sp), "paged_stage_gather")
+        K.check(K.paged_repage(st_d, ps, D, pd, tb, te, 0, nl, dnh, d_row, 0, stream=sp), "paged_repage")
+
+    # the ceiling: the same bytes re-page-gathered from TP sources that hold every layer
+    tp_plan = tp_reshard_plan(H, src_tp, dst_tp, 0)
+    full = {w.src_rank: Pool(ns + 8, ps, no, snh, hd, SE, 40 + w.src_rank, nl=nl) for w in tp_plan}
+    ftab = {r: rng.permutation(ns + 8)[:ns].tolist() for r in full}
+    fi = {r: torch.tensor(ftab[r], dtype=torch.int32, device=dev) for r in full}
+    full_srcs = [K.PermuteSource(side(full[w.src_rank], fi[w.src_rank]), snh, w.src_head_begin, w.dst_head_begin, w.head_count) for w in tp_plan]
+
+    def ceiling():
+        K.check(K.paged_repage_gather(full_srcs, ps, D, dnh, pd, tb, te, 0, nl, s_row, int(CAST), stream=sp), "paged_repage_gather")
+
+    # the staged gather of the same bytes from sources that already have page pd, into a destination of its own
+    eq = {r: Pool(nd + 8, pd, no, snh, hd, SE, 30 + r, nl=snl) for r in ranks}
+    etab, ei = tables(nd)
+    eq_dst = Pool(nd + 8, pd, no, dnh, hd, DE, 5, nl=nl)
+    edtab = rng.permutation(nd + 8)[:nd].tolist()
+    edi = torch.tensor(edtab, dtype=torch.int32, device=dev)
+    eq_staged = [K.StageSource(K.PermuteSource(side(eq[w.src_rank], ei[w.src_rank]), snh, w.src_head_begin, w.dst_head_begin, w.head_count),
+                               w.src_layer_begin, w.dst_layer_begin, w.layer_count) for w in plan]
+
+    def same_page():
+        K.check(K.paged_stage_gather(eq_staged, side(eq_dst, edi), dnh, nd, 0, nl, pd, s_row, int(CAST), stream=sp), "paged_stage_gather")
+
+    sample = sorted({0, nd // 2, nd - 1})
+
+    def check(arm, pools, tabs, page, d_pool, d_ids, windows):
+        torch.cuda.synchronize()
+        for j in sample:            # every head of every token is overwritten: the old bytes do not show through
+            lo, hi = j * pd, min((j + 1) * pd, te)
+            order = sorted(pools)
+            sources = [([pools[r].block(b) for b in table_slice(tabs[r], lo, hi, page)], NHD, snh, pools[r].nl) for r in order]
+            got = d_pool.block(d_ids[j])
+            win = [(order.index(w[0]),) + tuple(w[1:]) for w in windows]
+            want = stage_repage_gather(sources, win, [got], NHD, dnh, nl, no, page, pd, s_row, lo, hi, int(CAST))[0]
+            assert np.array_equal(got, want), (name, arm, j)
+
+    stage_windows = [(w.src_rank, w.src_layer_begin, w.dst_layer_begin, w.layer_count, w.src_head_begin, w.dst_head_begin, w.head_count)
+                     for w in plan]
+    full_windows = [(w.src_rank, 0, 0, nl, w.src_head_begin, w.dst_head_begin, w.head_count) for w in tp_plan]
+    arms = {"stage_repage_one_launch": one, "two_pass_stage_gather_then_repage": two_pass, "repage_gather_from_full_layer_sources": ceiling,
+            "same_page_stage_gather": same_page}
+    for k, fn in arms.items():
+        for t in (eq_dst if k == "same_page_stage_gather" else dst).layers:   # the arm alone decides the bytes it is checked on
+            t.fill_(0x5A)
+        for _ in range(3):
+            fn()
+        if k == "same_page_stage_gather":
+            check(k, eq, etab, pd, eq_dst, edtab, stage_windows)
+        elif k == "repage_gather_from_full_layer_sources":
+            check(k, full, ftab, ps, dst, dtab, full_windows)
+        else:
+            check(k, src, stab, ps, dst, dtab, stage_windows)
+    rounds = {k: [] for k in arms}
+    for _ in range(5):                 # the arms alternate within every round
+        for k, fn in arms.items():
+            rounds[k].append(timed(fn))
+    info = card()
+    for k in arms:
+        ms = statistics.median(rounds[k])
+        print(json.dumps({"config": name, "arm": k, "src_pp": src_pp, "src_tp": src_tp, "dst_tp": dst_tp, "src_page": ps, "dst_page": pd,
+                          "sources": len(ranks), "tokens": te - tb, "layers": nl, "outer": no, "heads": dnh, "head_dim": hd, "cast": a.cast,
+                          "ms": round(ms, 4), "ms_range": [round(min(rounds[k]), 4), round(max(rounds[k]), 4)],
+                          "GBps": round(moved / ms / 1e6, 1),
+                          "timed_as": "CUDA events, median of 5 alternated rounds of median-of-%d launches" % a.iters, "card": info}),
+              flush=True)
+
+
+if a.pp:
+    s_pp, s_tp, d_tp = (int(x) for x in a.pp.split(":"))
+    run_pp(s_pp, s_tp, d_tp, *(tuple(int(x) for x in a.pages.split(":")) if a.pages else (16, 64)))
+elif a.reshard:
     s_tp, d_tp = (int(x) for x in a.reshard.split(":"))
     default_pages = {(8, 1): (1, 16), (4, 2): (64, 16), (2, 8): (16, 64)}
     pages = tuple(int(x) for x in a.pages.split(":")) if a.pages else default_pages[(s_tp, d_tp)]

@@ -1274,8 +1274,10 @@ static size_t repage_blocks(size_t tb, size_t te, size_t page) { return tb == te
 // The checks of one re-paging (source, destination) pair, in this order: both layouts addressable and not both remote,
 // the options re-paging takes, named formats (the options override a layout's own; filled into *src_kv / *dst_kv), head counts
 // known and dividing inner_dim, check_compat's head row and cast dtypes, equal num_heads (unless `windows`: a gather's head
-// windows pick the heads, so the counts may differ) and dtypes, pages that divide and the walk's rules.
-static int check_repage_pair(const Layout& S, const Layout& D, const kvbm_transfer_options& o, bool windows, int* src_kv, int* dst_kv)
+// windows pick the heads, so the counts may differ) and dtypes, pages that divide and the walk's rules.  staged: a staged
+// re-paging gather's pair, whose layer counts may differ (check_compat's staged).
+static int check_repage_pair(const Layout& S, const Layout& D, const kvbm_transfer_options& o, bool windows, int* src_kv, int* dst_kv,
+                             bool staged = false)
 {
   if (S.unmapped || D.unmapped)
     return fail(KVBM_ERR_UNSUPPORTED, "a re-paging transfer needs both layouts addressable from this process (one is a descriptor of another process's host memory)");
@@ -1291,7 +1293,7 @@ static int check_repage_pair(const Layout& S, const Layout& D, const kvbm_transf
   int rc;
   if ((rc = need_num_heads(S.cfg)) || (rc = need_num_heads(D.cfg)) || (rc = need_divisible_heads(S.cfg)) || (rc = need_divisible_heads(D.cfg)))
     return rc;
-  if ((rc = check_compat(S, D, o.cast_mode, true))) return rc;
+  if ((rc = check_compat(S, D, o.cast_mode, true, staged))) return rc;
   const size_t ps = S.cfg.page_size, pd = D.cfg.page_size;
   if ((!windows && S.cfg.num_heads != D.cfg.num_heads) || (o.cast_mode == KVBM_CAST_NONE && S.cfg.dtype_width_bytes != D.cfg.dtype_width_bytes))
     return fail(KVBM_ERR_INCOMPATIBLE, "a re-paging transfer needs equal num_heads, head_dim and dtype on both sides");
@@ -1331,43 +1333,48 @@ static int repage_strategy(kvbm_transfer_manager* m, const Layout& S, const Layo
 // the destination's handle is looked up first; every window's source is then checked against the destination as a pair
 // whose head counts may differ, with its head window and with one page size for every source.  Launched through
 // kvbm_kernels_paged_repage_gather, or its streamed form with ls.
+// layers: a staged re-paging gather, a PP x TP re-shard's assembly across engines with different page sizes
+// (kvbm_manager_execute_stage_repage_gather), windows[j] being the head window of layers[j].  The windows are checked as
+// execute_gather checks a staged gather's, then check_stage_layers, then each pair as above but for the equal layer counts;
+// the options' layer range and the cast scales are the destination's.  Launched through kvbm_kernels_paged_stage_repage_gather,
+// or its streamed form with ls; each window's bytes count over its layers inside the layer range.
 // Otherwise the plain re-page (kvbm_manager_execute_repage): source 0 over every head of both sides, `windows` unused.  Its
 // source's handle is looked up first, its options fail the pair's checks, its head counts must be equal, and it is launched
 // through kvbm_kernels_paged_repage, which has no head limit.
 static int execute_repage_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, const size_t* const* src_ids,
                                  size_t n_src, kvbm_layout_handle dst_h, const size_t* dst_ids, size_t n_dst, size_t tb, size_t te,
                                  const kvbm_head_window* windows, size_t nw, const kvbm_transfer_options* opts_in, kvbm_notification* out,
-                                 const kvbm_layer_stream* ls = nullptr, bool gather = true)
+                                 const kvbm_layer_stream* ls = nullptr, bool gather = true, const kvbm_shard_window* layers = nullptr)
 {
   kvbm_transfer_options o{};
   if (opts_in) o = *opts_in;
   if (out) *out = 0;
   int rc;
-  if (gather && (rc = check_gather_windows(num_srcs, srcs, windows, nw, o))) return rc;
+  if (gather && (rc = check_gather_windows(num_srcs, srcs, windows, nw, o, layers))) return rc;
   std::lock_guard<std::mutex> lk(m->mu);
+  if (layers && (rc = check_stage_layers(m, srcs, dst_h, layers, nw, o))) return rc;
   Layout* D = nullptr;
   auto find_dst = [&] { return (D = m->find(dst_h)) ? KVBM_OK : fail(KVBM_ERR_HANDLE, "invalid destination handle"); };
   if (gather && (rc = find_dst())) return rc;  // the plain re-page looks its destination up after its source, in the loop
   Transfer e[KVBM_GATHER_MAX_SOURCES];
-  size_t heads = 0;
   for (size_t j = 0; j < nw; ++j) {
     Layout* S = e[j].S = m->find(srcs[gather ? windows[j].src_rank : 0]);
     if (!S) return fail(KVBM_ERR_HANDLE, "invalid source handle");
     if (!D && (rc = find_dst())) return rc;
     const kvbm_head_window& w = e[j].window = gather ? windows[j] : kvbm_head_window{0, 0, 0, S->cfg.num_heads};
     e[j].D[0] = D;
-    if ((rc = check_repage_pair(*S, *D, o, gather, &e[j].src_kv, &e[j].dst_kv)) || (rc = check_head_window(*S, *D, w, 1))) return rc;
+    if ((rc = check_repage_pair(*S, *D, o, gather, &e[j].src_kv, &e[j].dst_kv, layers != nullptr)) || (rc = check_head_window(*S, *D, w, 1)))
+      return rc;
     if (S->cfg.page_size != e[0].S->cfg.page_size)
       return fail(KVBM_ERR_INCOMPATIBLE, "the sources of a re-paging gather need one page size: source " + std::to_string(e[0].window.src_rank) +
                                              " has " + std::to_string(e[0].S->cfg.page_size) + ", source " + std::to_string(w.src_rank) +
                                              " has " + std::to_string(S->cfg.page_size));
-    heads += w.head_count;
   }
   const Layout& S0 = *e[0].S;
   if (tb > te || te > (size_t{1} << 31))
     return fail(KVBM_ERR_RANGE, "Token range " + std::to_string(tb) + ".." + std::to_string(te) + " is reversed or reaches past 2^31 tokens");
   size_t lb, le;
-  if ((rc = check_layer_range(S0.cfg, o, &lb, &le))) return rc;
+  if ((rc = check_layer_range(layers ? D->cfg : S0.cfg, o, &lb, &le))) return rc;
   const size_t ps = S0.cfg.page_size, pd = D->cfg.page_size;
   if ((rc = check_repage_counts(tb, te, ps, pd, n_src, n_dst))) return rc;
   if ((n_src && !src_ids) || (n_dst && !dst_ids)) return fail(KVBM_ERR, "null block id list");
@@ -1393,8 +1400,30 @@ static int execute_repage_gather(kvbm_transfer_manager* m, size_t num_srcs, cons
   const uint32_t ups = static_cast<uint32_t>(ps), upd = static_cast<uint32_t>(pd), dnh = static_cast<uint32_t>(D->cfg.num_heads);
   const uint32_t utb = static_cast<uint32_t>(tb), ute = static_cast<uint32_t>(te);
   const int ilb = static_cast<int>(lb), ile = static_cast<int>(le), k = static_cast<int>(nw);
+  uint64_t bytes = 0;
+  for (size_t j = 0; j < nw; ++j) {
+    size_t from = lb, to = le;
+    if (layers) {
+      from = std::max(from, layers[j].dst_layer_begin);
+      to = std::min(to, layers[j].dst_layer_begin + layers[j].layer_count);
+    }
+    if (to > from) bytes += (te - tb) * (to - from) * D->cfg.outer_dim * e[j].window.head_count * d_row;
+  }
   auto launch = [&](const kvbm_permute_source* ks, const kvbm_permute_side& kd, const kvbm_permute_stream* st, const Slot& sl, uint64_t seq) {
     const uint32_t value = static_cast<uint32_t>(seq);
+    if (layers) {
+      kvbm_stage_source ss[KVBM_GATHER_MAX_SOURCES] = {};
+      for (size_t j = 0; j < nw; ++j)
+        ss[j] = kvbm_stage_source{ks[j], static_cast<uint32_t>(layers[j].src_layer_begin), static_cast<uint32_t>(layers[j].dst_layer_begin),
+                                  static_cast<uint32_t>(layers[j].layer_count)};
+      if (st)
+        return checked(kvbm_kernels_paged_stage_repage_gather_streamed(ss, k, ups, &kd, dnh, upd, utb, ute, ilb, ile, row, o.cast_mode,
+                                                                       o.cast_scales, st, stream),
+                       "kvbm_kernels_paged_stage_repage_gather_streamed");
+      return checked(kvbm_kernels_paged_stage_repage_gather(ss, k, ups, &kd, dnh, upd, utb, ute, ilb, ile, row, o.cast_mode, o.cast_scales,
+                                                            o.done_flag, o.epoch, sl.host_flag, value, stream),
+                     "kvbm_kernels_paged_stage_repage_gather");
+    }
     if (st)
       return checked(kvbm_kernels_paged_repage_gather_streamed(ks, k, ups, &kd, dnh, upd, utb, ute, ilb, ile, row, o.cast_mode, o.cast_scales,
                                                                st, stream),
@@ -1407,8 +1436,7 @@ static int execute_repage_gather(kvbm_transfer_manager* m, size_t num_srcs, cons
                                              o.done_flag, o.epoch, sl.host_flag, value, stream),
                    "kvbm_kernels_paged_repage");
   };
-  return launch_transform(m, e, nw, num_srcs, src_ids, n_src, dst_ids, n_dst, ls, o, stream, (te - tb) * (le - lb) * D->cfg.outer_dim * heads * d_row,
-                          nullptr, out, launch);
+  return launch_transform(m, e, nw, num_srcs, src_ids, n_src, dst_ids, n_dst, ls, o, stream, bytes, nullptr, out, launch);
 }
 
 }  // namespace kvbm_host
@@ -2019,6 +2047,25 @@ extern "C" int kvbm_manager_execute_stage_gather(kvbm_transfer_manager* m, size_
   for (size_t j = 0; j < hw.size(); ++j)
     hw[j] = kvbm_head_window{windows[j].src_rank, windows[j].src_head_begin, windows[j].dst_head_begin, windows[j].head_count};
   return execute_gather(m, num_srcs, srcs, src_ids, dst, dst_ids, n, windows ? hw.data() : nullptr, num_windows, opts, out, ls, windows);
+  });
+}
+
+extern "C" int kvbm_manager_execute_stage_repage_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs,
+                                                        const size_t* const* src_ids, size_t n_src, kvbm_layout_handle dst,
+                                                        const size_t* dst_ids, size_t n_dst, size_t token_begin, size_t token_end,
+                                                        const kvbm_shard_window* windows, size_t num_windows, const kvbm_layer_stream* ls,
+                                                        const kvbm_transfer_options* opts, kvbm_notification* out)
+{
+  return guarded([&]() -> int {
+  if (!m) return fail(KVBM_ERR, "null manager");
+  if (out) *out = 0;
+  if (ls)
+    if (int rc = check_layer_stream_shape(ls, num_srcs)) return rc;
+  std::vector<kvbm_head_window> hw(windows ? num_windows : 0);
+  for (size_t j = 0; j < hw.size(); ++j)
+    hw[j] = kvbm_head_window{windows[j].src_rank, windows[j].src_head_begin, windows[j].dst_head_begin, windows[j].head_count};
+  return execute_repage_gather(m, num_srcs, srcs, src_ids, n_src, dst, dst_ids, n_dst, token_begin, token_end, windows ? hw.data() : nullptr,
+                               num_windows, opts, out, ls, /*gather=*/true, windows);
   });
 }
 

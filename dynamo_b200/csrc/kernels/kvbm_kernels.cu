@@ -798,24 +798,25 @@ struct RepageGatherParams {
   RepageGeom geo;
 };
 
-// Unit (big block j, layer l, outer o) of the re-paging gather.
-template <int CAST, bool POW2, bool SCALED, bool PPOW2>
-__device__ __forceinline__ void repage_gather_unit(const RepageGatherParams& P, uint32_t j, uint32_t l, uint32_t o, const RowSplit& r,
-                                                   const float* scales)
+// Unit (big block j, destination layer l, outer o) of the re-paging gather over map entries [first, end) of g's head map: the
+// warp of entry k reads its source s at the source's own layer l + shift(s).  SCALED: scales[l * no + o], by the destination layer.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2, class Shift>
+__device__ __forceinline__ void repage_gather_heads(const GatherParams& g, const RepageGeom& G, uint32_t first, uint32_t end, Shift shift,
+                                                    uint32_t j, uint32_t l, uint32_t o, const RowSplit& r, const float* scales)
 {
   constexpr int IN = CAST == KVBM_CAST_BF16_TO_FP8E4M3 ? 2 : 1;
   constexpr int OUT = CAST == KVBM_CAST_FP8E4M3_TO_BF16 ? 2 : 1;
-  const RepageGeom& G = P.geo;
-  const PermuteSide& D = P.g.D;
+  const PermuteSide& D = g.D;
   const RepageUnit u = repage_unit(G, j);
   const uint8_t* d_region = side_region(D, l, o);
   const ptx::Scale scale = ptx::make_scale(SCALED ? __ldg(scales + l * G.no + o) : 1.f);
   const uint32_t big_shift = G.src_small ? 3 + OUT : 3 + IN, small_shift = G.src_small ? 3 + IN : 3 + OUT;
   const uint32_t run = row_run<POW2>(r, u.tokens);
-  for (uint32_t k = threadIdx.x >> 5; k < P.g.covered; k += blockDim.x >> 5) {
-    const GatherSource& S = P.g.src[P.g.entry[k]];
+  for (uint32_t k = first + (threadIdx.x >> 5); k < end; k += blockDim.x >> 5) {
+    const uint32_t s = g.entry[k];
+    const GatherSource& S = g.src[s];
     const uint32_t h = k - S.first;  // head h of the window
-    const uint8_t* sh = side_region(S.S, l, o) + S.s_win + h * S.S.head_stride;
+    const uint8_t* sh = side_region(S.S, l + shift(s), o) + S.s_win + h * S.S.head_stride;
     const uint8_t* dh = d_region + S.d_win + h * D.head_stride;
     const bool ss = G.src_small;
     const PermuteSide& B = ss ? D : S.S;
@@ -824,6 +825,14 @@ __device__ __forceinline__ void repage_gather_unit(const RepageGatherParams& P, 
     repage_head_rows<CAST, POW2, SCALED, PPOW2>(bh, static_cast<uint32_t>(B.tok_stride), big_shift, ss ? sh : dh, Sm.ids, u.small_k,
                                                 Sm.block_stride, static_cast<uint32_t>(Sm.tok_stride), small_shift, G, u.q0, run, r, scale);
   }
+}
+
+// Unit (big block j, layer l, outer o) of the re-paging gather: every covered head, every source at layer l.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__device__ __forceinline__ void repage_gather_unit(const RepageGatherParams& P, uint32_t j, uint32_t l, uint32_t o, const RowSplit& r,
+                                                   const float* scales)
+{
+  repage_gather_heads<CAST, POW2, SCALED, PPOW2>(P.g, P.geo, 0, P.g.covered, [](uint32_t) { return 0u; }, j, l, o, r, scales);
 }
 
 template <int CAST, bool POW2, bool SCALED, bool PPOW2>
@@ -1043,6 +1052,54 @@ kvbm_gated_stage_gather_kernel(const __grid_constant__ StageGatherParams P, cons
       [&](uint32_t l, uint32_t* s_ok) { return gate_stage_layer(A, P, l, s_ok); });
 }
 
+// The staged re-paging gather (DESIGN §4.2e): the staged gather's stages and layer windows with the re-paging gather's unit, one
+// CTA per (big block j, layer, outer) clipped to the token range.  All sources share Ps, so big block j names the same sequence
+// positions in every source of every stage.
+struct StageRepageParams {
+  StageGatherParams s;
+  RepageGeom geo;
+};
+
+// Unit (big block j, destination layer l, outer o): the warps walk the map entries of l's stage only.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__device__ __forceinline__ void stage_repage_unit(const StageRepageParams& P, uint32_t j, uint32_t l, uint32_t o, const RowSplit& r,
+                                                  const float* scales)
+{
+  const GatherStage& T = stage_of(P.s, l);
+  repage_gather_heads<CAST, POW2, SCALED, PPOW2>(P.s.g, P.geo, T.first, T.first + T.count, [&](uint32_t s) { return P.s.shift[s]; }, j, l,
+                                                 o, r, scales);
+}
+
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__global__ void __launch_bounds__(256)
+kvbm_paged_stage_repage_gather_kernel(const __grid_constant__ StageRepageParams P, RowSplit r, const float* scales)
+{
+  const RepageGeom& G = P.geo;
+  const uint32_t unit = blockIdx.x;  // (big block j * nlayers + l) * no + o
+  const uint32_t j = unit / (G.nlayers * G.no);
+  const uint32_t rem = unit - j * (G.nlayers * G.no);
+  stage_repage_unit<CAST, POW2, SCALED, PPOW2>(P, j, G.layer_begin + rem / G.no, rem % G.no, r, scales);
+}
+
+// kvbm_paged_stage_repage_gather_kernel's unit walk behind the stage gate; unit = (l * num_big + j) * no + o over the layer range,
+// so a batch that crosses a stage boundary gates on the next stage's sources when it enters that layer.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__global__ void __launch_bounds__(256)
+kvbm_gated_stage_repage_gather_kernel(const __grid_constant__ StageRepageParams P, const __grid_constant__ GateArgs A, uint32_t num_big,
+                                      RowSplit r, const float* scales, uint32_t batch)
+{
+  const RepageGeom& G = P.geo;
+  const uint32_t per_layer = num_big * G.no;
+  gated_units(
+      A, per_layer * G.nlayers, batch, [&](uint32_t u) { return G.layer_begin + u / per_layer; },
+      [&](uint32_t u, uint32_t l) {
+        const uint32_t rem = u - (l - G.layer_begin) * per_layer;
+        const uint32_t j = rem / G.no;
+        stage_repage_unit<CAST, POW2, SCALED, PPOW2>(P, j, l, rem - j * G.no, r, scales);
+      },
+      [&](uint32_t l, uint32_t* s_ok) { return gate_stage_layer(A, P.s, l, s_ok); });
+}
+
 // The stream-wait form's signal after layer l: its layer-done flag, and after the last layer the done and completion flags.
 __global__ void kvbm_layer_signal_kernel(uint32_t* layer_done, uint32_t* done, uint32_t epoch, uint32_t* completion, uint32_t completion_value)
 {
@@ -1223,6 +1280,10 @@ static cudaError_t preload_kernels()
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_gather_kernel<c, p, sc, false>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_stage_gather_kernel<c, p, sc>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_stage_gather_kernel<c, p, sc>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_stage_repage_gather_kernel<c, p, sc, true>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_stage_repage_gather_kernel<c, p, sc, false>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_stage_repage_gather_kernel<c, p, sc, true>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_stage_repage_gather_kernel<c, p, sc, false>);
         });
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_layer_signal_kernel);
   return e;
@@ -1636,12 +1697,14 @@ static bool repage_geometry(uint32_t src_page, uint32_t dst_page, uint32_t token
 // or more windows.  Runs the checks of launch_paged_permute's sources and of repage_geometry's pages, each side's region at its
 // own page and head count, all before any CUDA call; signals when there is nothing to move; then launches
 // kvbm_paged_repage_kernel for a plain re-page, else kvbm_paged_repage_gather_kernel, and the signal.  max_covered and st: as
-// launch_paged_permute's (st takes the gated re-paging gather kernel, or per layer this launch unstreamed).
+// launch_paged_permute's (st takes the gated re-paging gather kernel, or per layer this launch unstreamed).  staged: as
+// launch_paged_permute's, checked by fill_stage_sources at the source page, which takes the stage re-paging gather kernels.
 static cudaError_t launch_paged_repage_gather(const kvbm_permute_source* srcs, int num_srcs, uint32_t src_page, const kvbm_permute_side* dst,
                                               uint32_t dst_num_heads, uint32_t dst_page, uint32_t token_begin, uint32_t token_end,
                                               int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
                                               uint32_t* done_flag, uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value,
-                                              uint32_t max_covered, cudaStream_t stream, const kvbm_permute_stream* st = nullptr)
+                                              uint32_t max_covered, cudaStream_t stream, const kvbm_permute_stream* st = nullptr,
+                                              const kvbm_stage_source* staged = nullptr)
 {
   if (layer_begin < 0 || layer_end < layer_begin || token_end < token_begin) return cudaErrorInvalidValue;
   if (!cast_args_ok(cast_mode, cast_scales)) return cudaErrorInvalidValue;
@@ -1651,42 +1714,58 @@ static cudaError_t launch_paged_repage_gather(const kvbm_permute_source* srcs, i
   const uint32_t nl = dst->layout.num_layers, no = dst->layout.outer_dim;
   if (nl == 0 || no == 0 || static_cast<uint32_t>(layer_end) > nl) return cudaErrorInvalidValue;
   RepageGatherParams P{};
+  StageRepageParams SP{};
+  GatherParams& g = staged ? SP.s.g : P.g;
+  RepageGeom& geo = staged ? SP.geo : P.geo;
   RowSplit r;
   uint64_t dst_row_bytes, units;
   bool page_pow2;
-  if (!repage_geometry(src_page, dst_page, token_begin, token_end, layer_begin, layer_end, no, src_row_bytes, cast_mode, &P.geo, &r,
+  if (!repage_geometry(src_page, dst_page, token_begin, token_end, layer_begin, layer_end, no, src_row_bytes, cast_mode, &geo, &r,
                        &dst_row_bytes, &units, &page_pow2))
     return cudaErrorInvalidValue;
   if (static_cast<uint64_t>(dst_page) * dst_num_heads * dst_row_bytes != dst->layout.region_bytes) return cudaErrorInvalidValue;
-  if (!fill_permute_side(*dst, nl, no, dst_num_heads, dst_page, static_cast<uint32_t>(dst_row_bytes), &P.g.D)) return cudaErrorInvalidValue;
-  if (!fill_gather_sources(srcs, num_srcs, dst_num_heads, nl, no, src_page, src_row_bytes, max_covered, &P.g)) return cudaErrorInvalidValue;
-  P.geo.nh = P.g.covered;
-  const int threads = static_cast<int>(std::min<uint32_t>(8, P.g.covered)) * 32;
+  if (!fill_permute_side(*dst, nl, no, dst_num_heads, dst_page, static_cast<uint32_t>(dst_row_bytes), &g.D)) return cudaErrorInvalidValue;
+  uint32_t widest = 0;
+  if (staged ? !fill_stage_sources(staged, num_srcs, dst_num_heads, nl, no, layer_begin, layer_end, src_page, src_row_bytes, &SP.s, &widest)
+             : !fill_gather_sources(srcs, num_srcs, dst_num_heads, nl, no, src_page, src_row_bytes, max_covered, &P.g))
+    return cudaErrorInvalidValue;
+  geo.nh = g.covered;
+  const int threads = static_cast<int>(std::min<uint32_t>(8, staged ? widest : g.covered)) * 32;
   const unsigned grid = static_cast<unsigned>(units);
   if (st)
     return launch_streamed(
         *st, num_srcs, nl, layer_begin, layer_end, units, stream,
         [&](int l) {
           return launch_paged_repage_gather(srcs, num_srcs, src_page, dst, dst_num_heads, dst_page, token_begin, token_end, l, l + 1,
-                                            src_row_bytes, cast_mode, cast_scales, nullptr, 0, nullptr, 0, max_covered, stream);
+                                            src_row_bytes, cast_mode, cast_scales, nullptr, 0, nullptr, 0, max_covered, stream, nullptr,
+                                            staged);
         },
         [&](const GateArgs& A, unsigned ctas, uint32_t batch) {
-          const uint32_t num_big = static_cast<uint32_t>(units / (static_cast<uint64_t>(P.geo.nlayers) * no));
+          const uint32_t num_big = static_cast<uint32_t>(units / (static_cast<uint64_t>(geo.nlayers) * no));
           with_walk_kernel(cast_mode, r.pow2, cast_scales != nullptr, [&](auto c, auto p, auto sc) {
-            if (page_pow2)
+            if (staged && page_pow2)
+              kvbm_gated_stage_repage_gather_kernel<c, p, sc, true><<<ctas, threads, 0, stream>>>(SP, A, num_big, r, cast_scales, batch);
+            else if (staged)
+              kvbm_gated_stage_repage_gather_kernel<c, p, sc, false><<<ctas, threads, 0, stream>>>(SP, A, num_big, r, cast_scales, batch);
+            else if (page_pow2)
               kvbm_gated_repage_gather_kernel<c, p, sc, true><<<ctas, threads, 0, stream>>>(P, A, num_big, r, cast_scales, batch);
             else
               kvbm_gated_repage_gather_kernel<c, p, sc, false><<<ctas, threads, 0, stream>>>(P, A, num_big, r, cast_scales, batch);
           });
-        });
+        },
+        staged ? &SP.s : nullptr);
   // a window over every head of both sides (the checks above make both its starts 0)
-  const bool plain = num_srcs == 1 && srcs[0].head_count == srcs[0].num_heads && srcs[0].head_count == dst_num_heads;
+  const bool plain = !staged && num_srcs == 1 && srcs[0].head_count == srcs[0].num_heads && srcs[0].head_count == dst_num_heads;
   RepageParams R{};
   R.big = P.geo.src_small ? P.g.D : P.g.src[0].S;
   R.small = P.geo.src_small ? P.g.src[0].S : P.g.D;
   R.g = P.geo;
   with_walk_kernel(cast_mode, r.pow2, cast_scales != nullptr, [&](auto c, auto p, auto sc) {
-    if (plain && page_pow2)
+    if (staged && page_pow2)
+      kvbm_paged_stage_repage_gather_kernel<c, p, sc, true><<<grid, threads, 0, stream>>>(SP, r, cast_scales);
+    else if (staged)
+      kvbm_paged_stage_repage_gather_kernel<c, p, sc, false><<<grid, threads, 0, stream>>>(SP, r, cast_scales);
+    else if (plain && page_pow2)
       kvbm_paged_repage_kernel<c, p, sc, true><<<grid, threads, 0, stream>>>(R, r, cast_scales);
     else if (plain)
       kvbm_paged_repage_kernel<c, p, sc, false><<<grid, threads, 0, stream>>>(R, r, cast_scales);
@@ -1918,8 +1997,24 @@ kvbm_kernels_paged_permute_gather_streamed(const kvbm_permute_source* srcs, int 
                               st);
 }
 
-// The staged gather's entries: the gather's launch path with layer windows, or with none when every window is the identity over
-// the destination's layers (a PP1 plan), which is then exactly kvbm_kernels_paged_permute_gather_scaled / _streamed.
+// A staged entry's num_srcs (1 .. KVBM_GATHER_MAX_SOURCES) sources as plain gather sources (plain[s] = srcs[s].src), and the
+// layer windows to launch with: none when every window is the identity over a source whose num_layers is the destination's (a
+// PP1 plan), which then launches exactly what the unstaged entry launches.
+static const kvbm_stage_source* split_stages(const kvbm_stage_source* srcs, int num_srcs, const kvbm_permute_side* dst,
+                                             kvbm_permute_source* plain)
+{
+  bool identity = dst != nullptr;
+  for (int s = 0; s < num_srcs; ++s) {
+    const kvbm_stage_source& X = srcs[s];
+    plain[s] = X.src;
+    identity = identity && X.src_layer_begin == 0 && X.dst_layer_begin == 0 && X.layer_count == dst->layout.num_layers &&
+               X.src.side.layout.num_layers == dst->layout.num_layers;
+  }
+  return identity ? nullptr : srcs;
+}
+
+// The staged gather's entries: the gather's launch path with layer windows, or with none for a PP1 plan, which is then exactly
+// kvbm_kernels_paged_permute_gather_scaled / _streamed.
 static cudaError_t launch_stage_gather(const kvbm_stage_source* srcs, int num_srcs, const kvbm_permute_side* dst, uint32_t dst_num_heads,
                                        int num_blocks, int layer_begin, int layer_end, uint32_t page_size, uint32_t src_row_bytes,
                                        int cast_mode, const float* cast_scales, uint32_t* done_flag, uint32_t epoch,
@@ -1928,16 +2023,50 @@ static cudaError_t launch_stage_gather(const kvbm_stage_source* srcs, int num_sr
 {
   if (!srcs || num_srcs < 1 || num_srcs > KVBM_GATHER_MAX_SOURCES) return cudaErrorInvalidValue;
   kvbm_permute_source plain[KVBM_GATHER_MAX_SOURCES];
-  bool identity = dst != nullptr;
-  for (int s = 0; s < num_srcs; ++s) {
-    const kvbm_stage_source& X = srcs[s];
-    plain[s] = X.src;
-    identity = identity && X.src_layer_begin == 0 && X.dst_layer_begin == 0 && X.layer_count == dst->layout.num_layers &&
-               X.src.side.layout.num_layers == dst->layout.num_layers;
-  }
+  const kvbm_stage_source* staged = split_stages(srcs, num_srcs, dst, plain);
   return launch_paged_permute(plain, num_srcs, dst, dst_num_heads, num_blocks, layer_begin, layer_end, page_size, src_row_bytes, cast_mode,
-                              cast_scales, done_flag, epoch, completion_flag, completion_value, KVBM_GATHER_MAX_HEADS, stream, st,
-                              identity ? nullptr : srcs);
+                              cast_scales, done_flag, epoch, completion_flag, completion_value, KVBM_GATHER_MAX_HEADS, stream, st, staged);
+}
+
+// The staged re-paging gather's entries: the re-paging gather's launch path with layer windows, or with none for a PP1 plan, which
+// is then exactly kvbm_kernels_paged_repage_gather / _streamed.
+static cudaError_t launch_stage_repage_gather(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page, const kvbm_permute_side* dst,
+                                              uint32_t dst_num_heads, uint32_t dst_page, uint32_t token_begin, uint32_t token_end,
+                                              int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
+                                              uint32_t* done_flag, uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value,
+                                              cudaStream_t stream, const kvbm_permute_stream* st = nullptr)
+{
+  if (!srcs || num_srcs < 1 || num_srcs > KVBM_GATHER_MAX_SOURCES) return cudaErrorInvalidValue;
+  kvbm_permute_source plain[KVBM_GATHER_MAX_SOURCES];
+  const kvbm_stage_source* staged = split_stages(srcs, num_srcs, dst, plain);
+  return launch_paged_repage_gather(plain, num_srcs, src_page, dst, dst_num_heads, dst_page, token_begin, token_end, layer_begin, layer_end,
+                                    src_row_bytes, cast_mode, cast_scales, done_flag, epoch, completion_flag, completion_value,
+                                    KVBM_GATHER_MAX_HEADS, stream, st, staged);
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_stage_repage_gather(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page_size, const kvbm_permute_side* dst,
+                                       uint32_t dst_num_heads, uint32_t dst_page_size, uint32_t token_begin, uint32_t token_end,
+                                       int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
+                                       uint32_t* done_flag, uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value,
+                                       cudaStream_t stream)
+{
+  return launch_stage_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, token_begin, token_end, layer_begin,
+                                    layer_end, src_row_bytes, cast_mode, cast_scales, done_flag, epoch, completion_flag, completion_value,
+                                    stream);
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_stage_repage_gather_streamed(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page_size,
+                                                const kvbm_permute_side* dst, uint32_t dst_num_heads, uint32_t dst_page_size,
+                                                uint32_t token_begin, uint32_t token_end, int layer_begin, int layer_end,
+                                                uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
+                                                const kvbm_permute_stream* st, cudaStream_t stream)
+{
+  if (!stream_args_ok(st, num_srcs)) return cudaErrorInvalidValue;
+  return launch_stage_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, token_begin, token_end, layer_begin,
+                                    layer_end, src_row_bytes, cast_mode, cast_scales, st->done_flag, st->epoch, st->completion_flag,
+                                    st->completion_value, stream, st);
 }
 
 extern "C" cudaError_t

@@ -219,6 +219,14 @@ def lib() -> C.CDLL:
         L.kvbm_kernels_paged_stage_gather_streamed.argtypes = [C.POINTER(StageSource), i, C.POINTER(PermuteSide), C.c_uint32, i, i, i,
                                                                C.c_uint32, C.c_uint32, i, vp, C.POINTER(PermuteStream), vp]
         L.kvbm_kernels_paged_stage_gather_streamed.restype = i
+        L.kvbm_kernels_paged_stage_repage_gather.argtypes = [C.POINTER(StageSource), i, C.c_uint32, C.POINTER(PermuteSide), C.c_uint32,
+                                                             C.c_uint32, C.c_uint32, C.c_uint32, i, i, C.c_uint32, i, vp, vp, C.c_uint32,
+                                                             vp, C.c_uint32, vp]
+        L.kvbm_kernels_paged_stage_repage_gather.restype = i
+        L.kvbm_kernels_paged_stage_repage_gather_streamed.argtypes = [C.POINTER(StageSource), i, C.c_uint32, C.POINTER(PermuteSide),
+                                                                      C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, i, i, C.c_uint32, i,
+                                                                      vp, C.POINTER(PermuteStream), vp]
+        L.kvbm_kernels_paged_stage_repage_gather_streamed.restype = i
         L.kvbm_kernels_permute_strides.argtypes = [i, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64, C.c_uint64,
                                                    C.POINTER(C.c_uint64)]
         L.kvbm_kernels_permute_strides.restype = i
@@ -244,6 +252,7 @@ EXPORTED_SYMBOLS = [
     "kvbm_kernels_paged_permute_gather", "kvbm_kernels_paged_permute_heads_scaled", "kvbm_kernels_paged_permute_gather_scaled",
     "kvbm_kernels_paged_repage", "kvbm_kernels_paged_repage_gather", "kvbm_kernels_paged_permute_gather_streamed",
     "kvbm_kernels_paged_repage_gather_streamed", "kvbm_kernels_paged_stage_gather", "kvbm_kernels_paged_stage_gather_streamed",
+    "kvbm_kernels_paged_stage_repage_gather", "kvbm_kernels_paged_stage_repage_gather_streamed",
 ]
 
 
@@ -440,6 +449,34 @@ def paged_stage_gather_streamed(srcs: Sequence[StageSource], dst: PermuteSide, d
     return lib().kvbm_kernels_paged_stage_gather_streamed(arr, len(srcs), C.byref(dst), dst_num_heads, num_blocks, layer_begin, layer_end,
                                                           page_size, src_row_bytes, int(cast_mode), scales_ptr(cast_scales),
                                                           C.byref(st) if st is not None else None, stream)
+
+
+def paged_stage_repage_gather(srcs: Sequence[StageSource], src_page_size: int, dst: PermuteSide, dst_num_heads: int, dst_page_size: int,
+                              token_begin: int, token_end: int, layer_begin: int, layer_end: int, src_row_bytes: int, cast_mode: int = 0,
+                              cast_scales=None, done_flag: int = 0, epoch: int = 0, completion_flag: int = 0, completion_value: int = 0,
+                              stream: int = 0) -> int:
+    """`paged_stage_gather`'s layer windows over `paged_repage_gather`'s token range, in ONE launch (a decode rank assembling its
+    layers and heads from a PP x TP prefill group with another page size): every source shares src_page_size and its block_ids
+    are its table[token_begin // Ps .. ceil(token_end / Ps)); `cast_scales` is indexed by the destination layer.
+    include/kvbm_kernels.h (kvbm_kernels_paged_stage_repage_gather)."""
+    arr = (StageSource * max(1, len(srcs)))(*srcs)
+    return lib().kvbm_kernels_paged_stage_repage_gather(arr, len(srcs), src_page_size, C.byref(dst), dst_num_heads, dst_page_size,
+                                                        token_begin, token_end, layer_begin, layer_end, src_row_bytes, int(cast_mode),
+                                                        scales_ptr(cast_scales), done_flag or None, epoch, completion_flag or None,
+                                                        completion_value, stream)
+
+
+def paged_stage_repage_gather_streamed(srcs: Sequence[StageSource], src_page_size: int, dst: PermuteSide, dst_num_heads: int,
+                                       dst_page_size: int, token_begin: int, token_end: int, layer_begin: int, layer_end: int,
+                                       src_row_bytes: int, cast_mode: int, cast_scales, st: Optional[PermuteStream],
+                                       stream: int = 0) -> int:
+    """`paged_stage_repage_gather` streamed with `paged_stage_gather_streamed`'s flags: `st.layer_ready_flags[s]` runs over source
+    s's own layers.  include/kvbm_kernels.h (kvbm_kernels_paged_stage_repage_gather_streamed)."""
+    arr = (StageSource * max(1, len(srcs)))(*srcs)
+    return lib().kvbm_kernels_paged_stage_repage_gather_streamed(arr, len(srcs), src_page_size, C.byref(dst), dst_num_heads, dst_page_size,
+                                                                 token_begin, token_end, layer_begin, layer_end, src_row_bytes,
+                                                                 int(cast_mode), scales_ptr(cast_scales),
+                                                                 C.byref(st) if st is not None else None, stream)
 
 
 def permute_strides(kv_layout: int, num_layers: int, outer_dim: int, num_heads: int, page_size: int, row_bytes: int,

@@ -242,7 +242,7 @@ EXPORTED_SYMBOLS = [
     "kvbm_mc_group_size", "kvbm_mc_group_add_device", "kvbm_mc_group_bind_local", "kvbm_mc_group_bind_addr", "kvbm_mc_group_map",
     "kvbm_mc_group_destroy", "kvbm_tp_reshard_plan", "kvbm_manager_execute_gather", "kvbm_manager_execute_repage",
     "kvbm_manager_execute_repage_gather", "kvbm_manager_execute_gather_streamed", "kvbm_manager_execute_repage_gather_streamed",
-    "kvbm_tp_pp_reshard_plan", "kvbm_manager_execute_stage_gather",
+    "kvbm_tp_pp_reshard_plan", "kvbm_manager_execute_stage_gather", "kvbm_manager_execute_stage_repage_gather",
 ]
 
 
@@ -301,6 +301,8 @@ def lib() -> C.CDLL:
         L.kvbm_tp_pp_reshard_plan.argtypes = [sz, sz, sz, sz, P(sz), sz, sz, P(sz), sz, P(_CShardWindow), sz, P(sz)]
         L.kvbm_manager_execute_stage_gather.argtypes = [vp, sz, P(u64), P(P(sz)), u64, vp, sz, P(_CShardWindow), sz, P(_CLayerStream),
                                                         P(_COptions), P(u64)]
+        L.kvbm_manager_execute_stage_repage_gather.argtypes = [vp, sz, P(u64), P(P(sz)), sz, u64, vp, sz, sz, sz, P(_CShardWindow), sz,
+                                                               P(_CLayerStream), P(_COptions), P(u64)]
         L.kvbm_notification_is_complete.argtypes = [vp, u64]
         L.kvbm_notification_wait.argtypes = [vp, u64, C.c_int64]
         L.kvbm_manager_bytes_moved.argtypes = [vp]
@@ -687,6 +689,13 @@ class TransferManager:
         return ranks, n_src, self._gather_args(sources, ranks, dst_block_ids, plan)
 
     @staticmethod
+    def _shard_windows(ranks: Sequence[int], plan: Sequence[ShardWindow]):
+        """The C windows of a staged plan, with src_rank as an index into `ranks`."""
+        index = {r: i for i, r in enumerate(ranks)}
+        return (_CShardWindow * max(1, len(plan)))(*[_CShardWindow(index[w.src_rank], w.src_layer_begin, w.dst_layer_begin, w.layer_count,
+                                                                   w.src_head_begin, w.dst_head_begin, w.head_count) for w in plan])
+
+    @staticmethod
     def _layer_stream(ranks: Sequence[int], ready_flags: Mapping[int, int], layer_done_flags: int) -> "_CLayerStream":
         """struct kvbm_layer_stream for the plan's source ranks; a rank missing from `ready_flags` passes NULL (rejected)."""
         flags = (C.c_void_p * max(1, len(ranks)))(*[int(ready_flags.get(r, 0)) or None for r in ranks])
@@ -731,9 +740,7 @@ class TransferManager:
         `ready_flags` (None: not streamed) maps a source rank to the address of the u32 ready flags over ITS OWN layers, as
         `execute_gather_streamed`; a destination layer waits only for its stage's sources.  `layer_done_flags`: the destination's."""
         ranks, (hs, _keep, sp, d, n, _ws) = self._gather_call(sources, dst_block_ids, plan)
-        index = {r: i for i, r in enumerate(ranks)}
-        ws = (_CShardWindow * max(1, len(plan)))(*[_CShardWindow(index[w.src_rank], w.src_layer_begin, w.dst_layer_begin, w.layer_count,
-                                                                 w.src_head_begin, w.dst_head_begin, w.head_count) for w in plan])
+        ws = self._shard_windows(ranks, plan)
         ls = self._layer_stream(ranks, ready_flags, layer_done_flags) if ready_flags is not None else None
         tok = C.c_uint64()
         o = (options or TransferOptions())._c()
@@ -784,6 +791,24 @@ class TransferManager:
         o = (options or TransferOptions())._c()
         _check(lib().kvbm_manager_execute_repage_gather_streamed(self._h, len(ranks), hs, sp, n_src, dst, d, n_dst, tokens.start,
                                                                  tokens.stop, ws, len(plan), C.byref(ls), C.byref(o), C.byref(tok)))
+        return TransferCompleteNotification(self, tok.value)
+
+    def execute_stage_repage_gather(self, sources: Mapping[int, tuple], dst: int, dst_block_ids: Sequence[int], plan: Sequence[ShardWindow],
+                                    tokens: range, options: Optional[TransferOptions] = None, ready_flags: Optional[Mapping[int, int]] = None,
+                                    layer_done_flags: int = 0) -> TransferCompleteNotification:
+        """A PP x TP re-shard's assembly across engines with different page sizes, as ONE hand-off
+        (kvbm_manager_execute_stage_repage_gather): `execute_stage_gather`'s plan (`tp_pp_reshard_plan`) over `execute_repage_gather`'s
+        `tokens` range.  Every source has one page size Ps and its ids are its table's entries tokens.start // Ps ..
+        ceil(tokens.stop / Ps); `dst_block_ids` are the destination's for its own page.  The options' layer range and cast scales
+        count destination layers.  `ready_flags` / `layer_done_flags`: as `execute_stage_gather`'s (None: not streamed)."""
+        ranks, n_src, (hs, _keep, sp, d, n_dst, _ws) = self._repage_gather_call(sources, dst_block_ids, plan, tokens)
+        ws = self._shard_windows(ranks, plan)
+        ls = self._layer_stream(ranks, ready_flags, layer_done_flags) if ready_flags is not None else None
+        tok = C.c_uint64()
+        o = (options or TransferOptions())._c()
+        _check(lib().kvbm_manager_execute_stage_repage_gather(self._h, len(ranks), hs, sp, n_src, dst, d, n_dst, tokens.start, tokens.stop,
+                                                              ws, len(plan), C.byref(ls) if ls is not None else None, C.byref(o),
+                                                              C.byref(tok)))
         return TransferCompleteNotification(self, tok.value)
 
     def execute_fanout(self, src: int, dsts: Sequence[int], src_block_ids: Sequence[Sequence[int]],

@@ -422,6 +422,37 @@ cudaError_t kvbm_kernels_paged_stage_gather_streamed(const kvbm_stage_source* sr
                                                      uint32_t page_size, uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
                                                      const kvbm_permute_stream* st, cudaStream_t stream);
 
+/* kvbm_kernels_paged_stage_gather with kvbm_kernels_paged_repage_gather's token range (a decode rank assembling its layers and heads
+ * from a PP x TP prefill group whose engine has another page size) in ONE launch, then one signal launch.  For every destination
+ * layer l of [layer_begin, layer_end) and every source s of l's stage, head src_head_begin + j of srcs[s] at source layer
+ * l - dst_layer_begin + src_layer_begin lands as head dst_head_begin + j at destination layer l, at every token of
+ * [token_begin, token_end) and every outer index, re-ordered and cast as kvbm_kernels_paged_repage_gather would, with the same bits.
+ * Tokens sit as in kvbm_kernels_paged_repage: srcs[s].src.side.block_ids holds source s's table[token_begin / Ps ..
+ * ceil(token_end / Ps)), dst->block_ids the destination's table for Pd.  All sources share src_page_size (Ps), src_row_bytes and
+ * cast_mode; each has its own pool, format, num_heads and num_layers.  cast_scales (nullable): one float[dst num_layers *
+ * outer_dim] array indexed by the DESTINATION layer and outer index.  Every other destination byte keeps its value: heads outside
+ * the windows of a layer's stage, and the slots of the first and last destination blocks outside the range.
+ * cudaErrorInvalidValue, before any CUDA call, for every rule of kvbm_kernels_paged_stage_gather's sources, stages and windows
+ * and of kvbm_kernels_paged_repage's pages, ranges, rows and strides.  An empty token or layer range moves nothing and still
+ * signals.  When every window is the identity over a source whose num_layers is the destination's, this is
+ * kvbm_kernels_paged_repage_gather. */
+cudaError_t kvbm_kernels_paged_stage_repage_gather(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page_size,
+                                                   const kvbm_permute_side* dst, uint32_t dst_num_heads, uint32_t dst_page_size,
+                                                   uint32_t token_begin, uint32_t token_end, int layer_begin, int layer_end,
+                                                   uint32_t src_row_bytes, int cast_mode, const float* cast_scales, uint32_t* done_flag,
+                                                   uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value,
+                                                   cudaStream_t stream);
+
+/* kvbm_kernels_paged_stage_repage_gather streamed with kvbm_kernels_paged_stage_gather_streamed's flag conventions:
+ * st->layer_ready_flags[s] runs over source s's OWN layers, a unit of destination layer l waits only for the sources of l's stage,
+ * each at its own layer, and layer_done_flags and sync_workspace are the destination's.  The argument rules are
+ * kvbm_kernels_paged_stage_repage_gather's plus the gate's. */
+cudaError_t kvbm_kernels_paged_stage_repage_gather_streamed(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page_size,
+                                                            const kvbm_permute_side* dst, uint32_t dst_num_heads, uint32_t dst_page_size,
+                                                            uint32_t token_begin, uint32_t token_end, int layer_begin, int layer_end,
+                                                            uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
+                                                            const kvbm_permute_stream* st, cudaStream_t stream);
+
 /* Host-only (no GPU): the stride table kvbm_kernels_paged_permute walks with for one side.  out[0] = 1 when offsets count
  * from the block's first byte (universal formats) or 0 when they count from the (layer, outer) region's first byte; the
  * element (layer l, outer o, head h, token t) then sits at  [out[0] ? l * out[1] + o * out[2] : 0] + h * out[3] + t * out[4].

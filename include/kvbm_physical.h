@@ -404,6 +404,26 @@ int kvbm_manager_execute_repage_gather_streamed(kvbm_transfer_manager* m, size_t
                                                 size_t num_windows, const kvbm_layer_stream* ls, const kvbm_transfer_options* opts,
                                                 kvbm_notification* out);
 
+/* A PP x TP re-shard's assembly across engines with different page sizes as ONE hand-off: kvbm_manager_execute_stage_gather's
+ * layer windows over kvbm_manager_execute_repage_gather's token range (a kvbm_tp_pp_reshard_plan passes as it is).  Heads
+ * [src_head_begin, +head_count) of layers [src_layer_begin, +layer_count) of source src_rank land as heads [dst_head_begin,
+ * +head_count) of layers [dst_layer_begin, +layer_count) of the destination, at every token of [token_begin, token_end), with the
+ * ids of kvbm_manager_execute_repage_gather (src_ids[s]: source s's table for Ps, n_src ids each; dst_ids: the destination's for
+ * Pd).  Every other destination byte keeps its value.  All sources share one page size; each may have its own num_layers.  The
+ * options' layer range counts destination layers, and so do cast_scales ([dst num_layers * outer_dim]).  ls (nullable): streamed
+ * as kvbm_manager_execute_stage_gather.  Errors, first one wins: with ls, its shape as kvbm_manager_execute_gather_streamed;
+ * kvbm_manager_execute_stage_gather's window checks; its KVBM_ERR_HANDLE and layer-window checks; each window's pair checks of
+ * kvbm_manager_execute_repage_gather except the equal layer counts, then its one page size; its token range; the layer range
+ * and cast scales against the destination; then the id counts, block ids, strategy, device, cast scales and, with ls, flag
+ * reachability as kvbm_manager_execute_repage_gather (an empty token or layer range returns KVBM_OK with nothing launched).  One
+ * upload, one kvbm_kernels_paged_stage_repage_gather launch (its streamed form with ls), one notification; bytes_moved counts
+ * each window's destination bytes over its layers inside the range. */
+int kvbm_manager_execute_stage_repage_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs,
+                                             const size_t* const* src_ids, size_t n_src, kvbm_layout_handle dst, const size_t* dst_ids,
+                                             size_t n_dst, size_t token_begin, size_t token_end, const kvbm_shard_window* windows,
+                                             size_t num_windows, const kvbm_layer_stream* ls, const kvbm_transfer_options* opts,
+                                             kvbm_notification* out);
+
 /* Completion: the transfer's last warp writes a flag in pinned host memory (no cudaEventQuery polling). */
 int kvbm_notification_is_complete(kvbm_transfer_manager* m, kvbm_notification n);  /* 1 / 0 / <0 error */
 int kvbm_notification_wait(kvbm_transfer_manager* m, kvbm_notification n, int64_t timeout_us);
