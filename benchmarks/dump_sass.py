@@ -37,15 +37,8 @@ for _c, _cn in ((0, ""), (1, "_fp8_to_bf16"), (2, "_bf16_to_fp8")):
                 # the layer-streamed (gated, persistent) re-paging gather
                 WANT[f"gated_repage_gather_kernelILi{_c}ELb{_r}ELb{_sc}ELb{_p}E"] = (
                     f"gated_repage_gather{_cn}_row_{'pow2' if _r else 'mulhi'}_page_{'pow2' if _p else 'mulhi'}{'_scaled' if _sc else ''}")
-                # the staged re-paging gather (PP x TP re-shard across page sizes) and its layer-streamed form
-                for _f in ("paged_stage_repage_gather", "gated_stage_repage_gather"):
-                    WANT[f"{_f}_kernelILi{_c}ELb{_r}ELb{_sc}ELb{_p}E"] = (
-                        f"{_f}{_cn}_row_{'pow2' if _r else 'mulhi'}_page_{'pow2' if _p else 'mulhi'}{'_scaled' if _sc else ''}")
             # the layer-streamed (gated, persistent) gather: <cast, row pow2, scaled>
             WANT[f"gated_gather_kernelILi{_c}ELb{_r}ELb{_sc}E"] = f"gated_gather{_cn}_{'pow2' if _r else 'mulhi'}{'_scaled' if _sc else ''}"
-            # the staged gather (PP x TP re-shard) and its layer-streamed form: <cast, row pow2, scaled>
-            for _f in ("paged_stage_gather", "gated_stage_gather"):
-                WANT[f"{_f}_kernelILi{_c}ELb{_r}ELb{_sc}E"] = f"{_f}{_cn}_{'pow2' if _r else 'mulhi'}{'_scaled' if _sc else ''}"
 WANT["layer_signal_kernel"] = "layer_signal"
 KEYS = ["UBLKCP.S.G", "UBLKCP.G.S", "SYNCS.ARRIVE.TRANS64", "SYNCS.PHASECHK.TRANS64.TRYWAIT", "SYNCS.ARRIVE", "UTMACMDFLUSH", "FENCE.VIEW.ASYNC",
             "F2FP", "ATOMG", "LDG.E.NA.128", "STG.E.NA.128", "LDS.128", "STS.128", "NANOSLEEP", "SHFL"]

@@ -633,35 +633,56 @@ kvbm_paged_permute_kernel(const __grid_constant__ PermuteSide S, const __grid_co
                                      D.head_stride, D.tok_stride, threadIdx.x >> 5, blockDim.x >> 5, nh, nt, r, scale);
 }
 
-// The gather: several sources, each with its own pool, format, head count and head window, into one destination.  The
-// covered destination heads are numbered 0 .. covered-1 in source order; entry[j] names the source of covered head j,
-// which is head j - first of that source's window.  s_win / d_win: the window's first head on either side, in bytes.
+// The gather: several sources, each with its own pool, format, head count, head window and layer window, into one destination.
+// The covered destination heads are numbered 0 .. covered-1; entry[j] names the source of covered head j, which is head
+// j - first of that source's window.  s_win / d_win: the window's first head on either side, in bytes.  A layer window maps
+// source layers [src_begin, src_begin + count) to destination layers [dst_begin, dst_begin + count); sources with one
+// destination window form a stage (DESIGN §4.2e).  Stage k covers destination layers [begin, end) and map entries first ..
+// first + count - 1 (the map runs stage by stage, in source order within a stage), `sources` is the mask of its sources, and
+// shift[s] is source s's layer minus the destination's.  The stages ascend and tile the launch's layer range: a gather without
+// layer windows (a PP1 plan) is one stage over every layer, every shift 0.
 struct GatherSource {
   PermuteSide S;
   uint64_t s_win, d_win;
   uint32_t first;
+};
+struct GatherStage {
+  uint32_t begin, end, first, count, sources;
 };
 struct GatherParams {
   PermuteSide D;
   GatherSource src[KVBM_GATHER_MAX_SOURCES];
   uint8_t entry[KVBM_GATHER_MAX_HEADS];
   uint32_t covered;
+  alignas(8) GatherStage stage[KVBM_GATHER_MAX_SOURCES];  // the measured layout: 4 B earlier reschedules the re-paging gathers
+  uint32_t shift[KVBM_GATHER_MAX_SOURCES];
 };
 
+// The stage of destination layer l (one of the launch's range): the first stage that ends past it.
+__host__ __device__ __forceinline__ const GatherStage& stage_of(const GatherParams& P, uint32_t l)
+{
+  uint32_t k = 0;
+  while (l >= P.stage[k].end) ++k;
+  return P.stage[k];
+}
+
 // One destination (block, layer, outer) unit of the gather, block `pair` of the tables, with one warp per covered destination
-// head (looping by the CTA's warps past 8): every source's window of the unit is written by the same CTA, so a destination row
-// that holds every head (OperationalNHD) is written whole by one CTA.  Each warp looks up its source and runs the same walk
-// over one head.  SCALED: one scale array for every source, scales[l * no + o] loaded once per unit.
+// head of layer l's stage T (looping by the CTA's warps past 8): every source's window of the unit is written by the same CTA, so
+// a destination row that holds every head (OperationalNHD) is written whole by one CTA.  Each warp looks up its source and runs
+// the same walk over one head, reading the source at its own layer l + shift.  SCALED: one scale array for every source,
+// scales[l * no + o] by the destination layer, loaded once per unit.
 template <int CAST, bool POW2, bool SCALED>
-__device__ __forceinline__ void gather_unit(const GatherParams& P, uint32_t pair, uint32_t l, uint32_t o, uint32_t no, uint32_t nt,
-                                            const RowSplit& r, const float* scales)
+__device__ __forceinline__ void gather_unit(const GatherParams& P, const GatherStage& T, uint32_t pair, uint32_t l, uint32_t o, uint32_t no,
+                                            uint32_t nt, const RowSplit& r, const float* scales)
 {
   uint8_t* db = side_block(P.D, pair, l, o);
   const ptx::Scale scale = ptx::make_scale(SCALED ? __ldg(scales + l * no + o) : 1.f);
-  for (uint32_t j = threadIdx.x >> 5; j < P.covered; j += blockDim.x >> 5) {
-    const GatherSource& G = P.src[P.entry[j]];
+  const uint32_t end = T.first + T.count;
+  for (uint32_t j = T.first + (threadIdx.x >> 5); j < end; j += blockDim.x >> 5) {
+    const uint32_t s = P.entry[j];
+    const GatherSource& G = P.src[s];
     const uint32_t h = j - G.first;  // head h of the window: walk heads h .. h of the window's bases
-    walk_head_rows<CAST, POW2, SCALED>(side_block(G.S, pair, l, o) + G.s_win, G.S.head_stride, G.S.tok_stride, db + G.d_win,
+    walk_head_rows<CAST, POW2, SCALED>(side_block(G.S, pair, l + P.shift[s], o) + G.s_win, G.S.head_stride, G.S.tok_stride, db + G.d_win,
                                        P.D.head_stride, P.D.tok_stride, h, 1, h + 1, nt, r, scale);
   }
 }
@@ -675,7 +696,8 @@ kvbm_paged_gather_kernel(const __grid_constant__ GatherParams P, uint32_t layer_
   const uint32_t unit = blockIdx.x;  // (pair * nlayers + l) * no + o
   const uint32_t pair = unit / (nlayers * no);
   const uint32_t rem = unit - pair * (nlayers * no);
-  gather_unit<CAST, POW2, SCALED>(P, pair, layer_begin + rem / no, rem % no, no, nt, r, scales);
+  const uint32_t l = layer_begin + rem / no;
+  gather_unit<CAST, POW2, SCALED>(P, stage_of(P, l), pair, l, rem % no, no, nt, r, scales);
 }
 
 // Re-paging: a token range [token_begin, token_end) of one sequence between two block tables whose page sizes differ (one divides
@@ -785,27 +807,30 @@ kvbm_paged_repage_kernel(const __grid_constant__ RepageParams P, RowSplit r, con
                                                 static_cast<uint32_t>(P.small.tok_stride), small_shift, P.g, u.q0, run, r, scale);
 }
 
-// Re-paging and the gather in one launch: several sources with one page size Ps (a prefill TP group), each with its own pool,
-// format, head count and head window, into one destination of page Pd, over a token range.  The unit is the re-paging one: one
-// CTA per (block of the larger-page side, layer, outer), clipped to the range; the warps are the gather's: one per covered
-// destination head, looping by the CTA's warps past 8, each finding its source through the head map.  All sources share Ps and
-// the range, so big block j names the same sequence positions in every source: when the sources have the larger page each warp
-// reads block j of its own table; when the destination has it, a unit is one destination block and one CTA writes whole rows
-// of an OperationalNHD destination.  The small side's block comes per 16 B vector from the warp's own source table or the
-// destination's.  geo.nh: the covered heads.  SCALED: one scale array for every source, scales[l * no + o].
+// Re-paging and the gather in one launch: several sources with one page size Ps (a prefill TP or PP x TP group), each with its
+// own pool, format, head count, head window and layer window, into one destination of page Pd, over a token range.  The unit is
+// the re-paging one: one CTA per (block of the larger-page side, layer, outer), clipped to the range; the warps are the
+// gather's: one per covered destination head of the layer's stage, looping by the CTA's warps past 8, each finding its source
+// through the head map and reading it at its own layer.  All sources share Ps and the range, so big block j names the same
+// sequence positions in every source: when the sources have the larger page each warp reads block j of its own table; when the
+// destination has it, a unit is one destination block and one CTA writes whole rows of an OperationalNHD destination.  The
+// small side's block comes per 16 B vector from the warp's own source table or the destination's.  geo.nh: the covered heads.
 struct RepageGatherParams {
   GatherParams g;
   RepageGeom geo;
 };
 
-// Unit (big block j, destination layer l, outer o) of the re-paging gather over map entries [first, end) of g's head map: the
-// warp of entry k reads its source s at the source's own layer l + shift(s).  SCALED: scales[l * no + o], by the destination layer.
-template <int CAST, bool POW2, bool SCALED, bool PPOW2, class Shift>
-__device__ __forceinline__ void repage_gather_heads(const GatherParams& g, const RepageGeom& G, uint32_t first, uint32_t end, Shift shift,
-                                                    uint32_t j, uint32_t l, uint32_t o, const RowSplit& r, const float* scales)
+// Unit (big block j, destination layer l, outer o) of the re-paging gather: the warp of map entry k of l's stage T reads its source
+// s at the source's own layer l + shift[s].  SCALED: one scale array for every source, scales[l * no + o] by the destination layer.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__device__ __forceinline__ void repage_gather_unit(const RepageGatherParams& P, const GatherStage& T, uint32_t j, uint32_t l, uint32_t o,
+                                                   const RowSplit& r, const float* scales)
 {
   constexpr int IN = CAST == KVBM_CAST_BF16_TO_FP8E4M3 ? 2 : 1;
   constexpr int OUT = CAST == KVBM_CAST_FP8E4M3_TO_BF16 ? 2 : 1;
+  const GatherParams& g = P.g;
+  const RepageGeom& G = P.geo;
+  const uint32_t first = T.first, end = T.first + T.count;
   const PermuteSide& D = g.D;
   const RepageUnit u = repage_unit(G, j);
   const uint8_t* d_region = side_region(D, l, o);
@@ -816,7 +841,7 @@ __device__ __forceinline__ void repage_gather_heads(const GatherParams& g, const
     const uint32_t s = g.entry[k];
     const GatherSource& S = g.src[s];
     const uint32_t h = k - S.first;  // head h of the window
-    const uint8_t* sh = side_region(S.S, l + shift(s), o) + S.s_win + h * S.S.head_stride;
+    const uint8_t* sh = side_region(S.S, l + g.shift[s], o) + S.s_win + h * S.S.head_stride;
     const uint8_t* dh = d_region + S.d_win + h * D.head_stride;
     const bool ss = G.src_small;
     const PermuteSide& B = ss ? D : S.S;
@@ -827,36 +852,32 @@ __device__ __forceinline__ void repage_gather_heads(const GatherParams& g, const
   }
 }
 
-// Unit (big block j, layer l, outer o) of the re-paging gather: every covered head, every source at layer l.
+// Three CTAs per SM (at most 80 registers): the stage lookup otherwise takes the scaled fp8 -> bf16 walk with a power-of-two
+// row and page to 86 registers, and to two CTAs per SM.
 template <int CAST, bool POW2, bool SCALED, bool PPOW2>
-__device__ __forceinline__ void repage_gather_unit(const RepageGatherParams& P, uint32_t j, uint32_t l, uint32_t o, const RowSplit& r,
-                                                   const float* scales)
-{
-  repage_gather_heads<CAST, POW2, SCALED, PPOW2>(P.g, P.geo, 0, P.g.covered, [](uint32_t) { return 0u; }, j, l, o, r, scales);
-}
-
-template <int CAST, bool POW2, bool SCALED, bool PPOW2>
-__global__ void __launch_bounds__(256)
+__global__ void __launch_bounds__(256, 3)
 kvbm_paged_repage_gather_kernel(const __grid_constant__ RepageGatherParams P, RowSplit r, const float* scales)
 {
   const RepageGeom& G = P.geo;
   const uint32_t unit = blockIdx.x;  // (big block j * nlayers + l) * no + o
   const uint32_t j = unit / (G.nlayers * G.no);
   const uint32_t rem = unit - j * (G.nlayers * G.no);
-  repage_gather_unit<CAST, POW2, SCALED, PPOW2>(P, j, G.layer_begin + rem / G.no, rem % G.no, r, scales);
+  const uint32_t l = G.layer_begin + rem / G.no;
+  repage_gather_unit<CAST, POW2, SCALED, PPOW2>(P, stage_of(P.g, l), j, l, rem % G.no, r, scales);
 }
 
 // ------------------------------------------------------------------------------------------------
 // Layer streaming of the permuting and re-paging gathers (kvbm_permute_stream, spinning form).  The ungated kernels are one
 // CTA per unit in block-major order, scheduled by the hardware: gating them would fill the GPU with spinners that starve the
 // producer.  The gated kernels are a persistent grid instead: each CTA claims a batch of `batch` consecutive units per ticket
-// from the ticket word ctl[2] in LAYER-major order, waits once per layer it enters for that layer's flag of every source (warp
+// from the ticket word ctl[2] in LAYER-major order, waits once per layer it enters for the flags of that layer's stage (warp
 // 0, wait_layer_ready's relaxed polls, acquire fence, timeout and abort word), walks each unit with the ungated kernel's
 // unit body (gather_unit / repage_gather_unit), and publishes what it moved of a layer -- every thread fences its stores, one barrier, one arrive_layer with
 // the count -- when the batch ends and before it enters another layer.  So a CTA publishes every unit before it can wait on a
-// later layer: a receiver that releases layer l + 1 only after seeing layer l done cannot dead-lock against it.  The warps of a
-// CTA run on into the batch's next unit without waiting for each other.  The last CTA to finish runs arrive_transfer
-// (re-zeroes the workspace, done / completion flags, or 0xFFFFFFFF on abort).
+// later layer: a receiver that releases layer l + 1 only after seeing layer l done cannot dead-lock against it, and a batch that
+// crosses a stage boundary gates on the next stage's sources when it enters that layer.  The warps of a CTA run on into the
+// batch's next unit without waiting for each other.  The last CTA to finish runs arrive_transfer (re-zeroes the workspace, done
+// / completion flags, or 0xFFFFFFFF on abort).
 // ------------------------------------------------------------------------------------------------
 struct GateArgs {
   StreamSync ss;  // ndst 1: the destination's layer_done / done flags; items = units; total_rings = CTAs
@@ -864,16 +885,18 @@ struct GateArgs {
   int num_ready;
 };
 
-// Every source's ready flag of layer l, waited for by warp 0; the verdict goes to the whole CTA.  False: the transfer aborted.
-__device__ __forceinline__ bool gate_layer(const GateArgs& A, uint32_t l, uint32_t* s_ok)
+// The ready flags of the sources of layer l's stage T, each at its own layer l + shift, waited for by warp 0; the verdict goes
+// to the whole CTA.  False: the transfer aborted.
+__device__ __forceinline__ bool gate_layer(const GateArgs& A, const GatherParams& P, const GatherStage& T, uint32_t l, uint32_t* s_ok)
 {
   if (threadIdx.x < 32) {
     bool ok = true;
-    for (int s = 0; s < A.num_ready && ok; ++s) {
-      StreamSync w = A.ss;
-      w.layer_ready = A.ready[s];
-      ok = wait_layer_ready(w, static_cast<int>(l), threadIdx.x);
-    }
+    for (int s = 0; s < A.num_ready && ok; ++s)
+      if ((T.sources >> s) & 1u) {
+        StreamSync w = A.ss;
+        w.layer_ready = A.ready[s];
+        ok = wait_layer_ready(w, static_cast<int>(l + P.shift[s]), threadIdx.x);
+      }
     if (threadIdx.x == 0) *s_ok = ok ? 1u : 0u;
   }
   __syncthreads();
@@ -890,13 +913,14 @@ __device__ __forceinline__ void publish_units(const GateArgs& A, uint32_t l, uin
   if (threadIdx.x == 0 && A.ss.want_layers && count != 0) arrive_layer(A.ss, static_cast<int>(l), count);
 }
 
-// The claim / gate / publish loop of every gated kernel over units [0, total): layer_of(u) is unit u's absolute layer,
-// walk(u, l) moves it, gate(l, s_ok) waits for layer l's sources as gate_layer does.
-template <class LayerOf, class Walk, class Gate>
-__device__ __forceinline__ void gated_units(const GateArgs& A, uint32_t total, uint32_t batch, LayerOf layer_of, Walk walk, Gate gate)
+// The claim / gate / publish loop of every gated kernel over units [0, total) of the gather P: layer_of(u) is unit u's absolute
+// layer, walk(u, l, T) moves it with T its layer's stage, looked up once per layer the CTA enters.
+template <class LayerOf, class Walk>
+__device__ __forceinline__ void gated_units(const GateArgs& A, const GatherParams& P, uint32_t total, uint32_t batch, LayerOf layer_of, Walk walk)
 {
   __shared__ uint32_t s_ticket, s_ok;
   uint32_t entered = UINT32_MAX;
+  GatherStage T{};
   for (;;) {
     if (threadIdx.x == 0) s_ticket = atomicAdd(A.ss.ctl + 2, 1u);
     __syncthreads();
@@ -910,26 +934,20 @@ __device__ __forceinline__ void gated_units(const GateArgs& A, uint32_t total, u
       if (l != entered) {
         if (pending != 0) publish_units(A, entered, pending);
         pending = 0;
-        if (!gate(l, &s_ok)) {
+        T = stage_of(P, l);
+        if (!gate_layer(A, P, T, l, &s_ok)) {
           aborted = true;
           break;
         }
         entered = l;
       }
-      walk(u, l);
+      walk(u, l, T);
       ++pending;
     }
     if (aborted) break;
     publish_units(A, entered, pending);
   }
   if (threadIdx.x == 0) arrive_transfer(A.ss);
-}
-
-// The loop gated on every source's flag of the unit's layer.
-template <class LayerOf, class Walk>
-__device__ __forceinline__ void gated_units(const GateArgs& A, uint32_t total, uint32_t batch, LayerOf layer_of, Walk walk)
-{
-  gated_units(A, total, batch, layer_of, walk, [&](uint32_t l, uint32_t* s_ok) { return gate_layer(A, l, s_ok); });
 }
 
 // kvbm_paged_gather_kernel's unit walk behind the gate; unit = (l * num_blocks + pair) * no + o over the layer range.
@@ -939,10 +957,10 @@ kvbm_gated_gather_kernel(const __grid_constant__ GatherParams P, const __grid_co
                          uint32_t nlayers, uint32_t no, uint32_t nt, RowSplit r, const float* scales, uint32_t batch)
 {
   const uint32_t per_layer = num_blocks * no;
-  gated_units(A, per_layer * nlayers, batch, [&](uint32_t u) { return layer_begin + u / per_layer; }, [&](uint32_t u, uint32_t l) {
+  gated_units(A, P, per_layer * nlayers, batch, [&](uint32_t u) { return layer_begin + u / per_layer; }, [&](uint32_t u, uint32_t l, const GatherStage& T) {
     const uint32_t rem = u - (l - layer_begin) * per_layer;
     const uint32_t pair = rem / no;
-    gather_unit<CAST, POW2, SCALED>(P, pair, l, rem - pair * no, no, nt, r, scales);
+    gather_unit<CAST, POW2, SCALED>(P, T, pair, l, rem - pair * no, no, nt, r, scales);
   });
 }
 
@@ -954,150 +972,11 @@ kvbm_gated_repage_gather_kernel(const __grid_constant__ RepageGatherParams P, co
 {
   const RepageGeom& G = P.geo;
   const uint32_t per_layer = num_big * G.no;
-  gated_units(A, per_layer * G.nlayers, batch, [&](uint32_t u) { return G.layer_begin + u / per_layer; }, [&](uint32_t u, uint32_t l) {
+  gated_units(A, P.g, per_layer * G.nlayers, batch, [&](uint32_t u) { return G.layer_begin + u / per_layer; }, [&](uint32_t u, uint32_t l, const GatherStage& T) {
     const uint32_t rem = u - (l - G.layer_begin) * per_layer;
     const uint32_t j = rem / G.no;
-    repage_gather_unit<CAST, POW2, SCALED, PPOW2>(P, j, l, rem - j * G.no, r, scales);
+    repage_gather_unit<CAST, POW2, SCALED, PPOW2>(P, T, j, l, rem - j * G.no, r, scales);
   });
-}
-
-// ------------------------------------------------------------------------------------------------
-// The staged gather (DESIGN §4.2e): a pipeline-parallel re-shard.  Each source also has a layer window, source layers
-// [src_begin, src_begin + count) -> destination layers [dst_begin, dst_begin + count); sources with one destination window form a
-// stage.  Stage k covers destination layers [begin, end) and map entries first .. first + count - 1 of the gather's one head
-// map (stage by stage), `sources` is the mask of its sources, and shift[s] is source s's layer minus the destination's.  The
-// stages ascend and tile the launch's layer range.
-// ------------------------------------------------------------------------------------------------
-struct GatherStage {
-  uint32_t begin, end, first, count, sources;
-};
-struct StageGatherParams {
-  GatherParams g;
-  GatherStage stage[KVBM_GATHER_MAX_SOURCES];
-  uint32_t shift[KVBM_GATHER_MAX_SOURCES];
-};
-
-// The stage of destination layer l (one of the launch's range): the first stage that ends past it.
-__host__ __device__ __forceinline__ const GatherStage& stage_of(const StageGatherParams& P, uint32_t l)
-{
-  uint32_t k = 0;
-  while (l >= P.stage[k].end) ++k;
-  return P.stage[k];
-}
-
-// gather_unit over the stage of layer l only: its warps walk that stage's map entries, each reading its source at the source's
-// own layer l + shift.  SCALED: scales[l * no + o], by the destination layer.
-template <int CAST, bool POW2, bool SCALED>
-__device__ __forceinline__ void stage_gather_unit(const StageGatherParams& P, uint32_t pair, uint32_t l, uint32_t o, uint32_t no, uint32_t nt,
-                                                  const RowSplit& r, const float* scales)
-{
-  const GatherStage& T = stage_of(P, l);
-  uint8_t* db = side_block(P.g.D, pair, l, o);
-  const ptx::Scale scale = ptx::make_scale(SCALED ? __ldg(scales + l * no + o) : 1.f);
-  const uint32_t end = T.first + T.count;
-  for (uint32_t j = T.first + (threadIdx.x >> 5); j < end; j += blockDim.x >> 5) {
-    const uint32_t s = P.g.entry[j];
-    const GatherSource& G = P.g.src[s];
-    const uint32_t h = j - G.first;
-    walk_head_rows<CAST, POW2, SCALED>(side_block(G.S, pair, l + P.shift[s], o) + G.s_win, G.S.head_stride, G.S.tok_stride, db + G.d_win,
-                                       P.g.D.head_stride, P.g.D.tok_stride, h, 1, h + 1, nt, r, scale);
-  }
-}
-
-// One CTA per destination unit, as the gather.
-template <int CAST, bool POW2, bool SCALED = false>
-__global__ void __launch_bounds__(256)
-kvbm_paged_stage_gather_kernel(const __grid_constant__ StageGatherParams P, uint32_t layer_begin, uint32_t nlayers, uint32_t no, uint32_t nt,
-                               RowSplit r, const float* scales)
-{
-  const uint32_t unit = blockIdx.x;  // (pair * nlayers + l) * no + o
-  const uint32_t pair = unit / (nlayers * no);
-  const uint32_t rem = unit - pair * (nlayers * no);
-  stage_gather_unit<CAST, POW2, SCALED>(P, pair, layer_begin + rem / no, rem % no, no, nt, r, scales);
-}
-
-// gate_layer for the staged gather: the ready flags of only the sources of layer l's stage, each at its own layer l + shift.
-__device__ __forceinline__ bool gate_stage_layer(const GateArgs& A, const StageGatherParams& P, uint32_t l, uint32_t* s_ok)
-{
-  if (threadIdx.x < 32) {
-    const uint32_t mask = stage_of(P, l).sources;
-    bool ok = true;
-    for (int s = 0; s < A.num_ready && ok; ++s)
-      if ((mask >> s) & 1u) {
-        StreamSync w = A.ss;
-        w.layer_ready = A.ready[s];
-        ok = wait_layer_ready(w, static_cast<int>(l + P.shift[s]), threadIdx.x);
-      }
-    if (threadIdx.x == 0) *s_ok = ok ? 1u : 0u;
-  }
-  __syncthreads();
-  return *s_ok != 0;
-}
-
-// kvbm_paged_stage_gather_kernel's unit walk behind the stage gate; unit = (l * num_blocks + pair) * no + o over the layer range,
-// so a batch that crosses a stage boundary gates on the next stage's sources when it enters that layer.
-template <int CAST, bool POW2, bool SCALED>
-__global__ void __launch_bounds__(256, 1)
-kvbm_gated_stage_gather_kernel(const __grid_constant__ StageGatherParams P, const __grid_constant__ GateArgs A, uint32_t num_blocks,
-                               uint32_t layer_begin, uint32_t nlayers, uint32_t no, uint32_t nt, RowSplit r, const float* scales, uint32_t batch)
-{
-  const uint32_t per_layer = num_blocks * no;
-  gated_units(
-      A, per_layer * nlayers, batch, [&](uint32_t u) { return layer_begin + u / per_layer; },
-      [&](uint32_t u, uint32_t l) {
-        const uint32_t rem = u - (l - layer_begin) * per_layer;
-        const uint32_t pair = rem / no;
-        stage_gather_unit<CAST, POW2, SCALED>(P, pair, l, rem - pair * no, no, nt, r, scales);
-      },
-      [&](uint32_t l, uint32_t* s_ok) { return gate_stage_layer(A, P, l, s_ok); });
-}
-
-// The staged re-paging gather (DESIGN §4.2e): the staged gather's stages and layer windows with the re-paging gather's unit, one
-// CTA per (big block j, layer, outer) clipped to the token range.  All sources share Ps, so big block j names the same sequence
-// positions in every source of every stage.
-struct StageRepageParams {
-  StageGatherParams s;
-  RepageGeom geo;
-};
-
-// Unit (big block j, destination layer l, outer o): the warps walk the map entries of l's stage only.
-template <int CAST, bool POW2, bool SCALED, bool PPOW2>
-__device__ __forceinline__ void stage_repage_unit(const StageRepageParams& P, uint32_t j, uint32_t l, uint32_t o, const RowSplit& r,
-                                                  const float* scales)
-{
-  const GatherStage& T = stage_of(P.s, l);
-  repage_gather_heads<CAST, POW2, SCALED, PPOW2>(P.s.g, P.geo, T.first, T.first + T.count, [&](uint32_t s) { return P.s.shift[s]; }, j, l,
-                                                 o, r, scales);
-}
-
-template <int CAST, bool POW2, bool SCALED, bool PPOW2>
-__global__ void __launch_bounds__(256)
-kvbm_paged_stage_repage_gather_kernel(const __grid_constant__ StageRepageParams P, RowSplit r, const float* scales)
-{
-  const RepageGeom& G = P.geo;
-  const uint32_t unit = blockIdx.x;  // (big block j * nlayers + l) * no + o
-  const uint32_t j = unit / (G.nlayers * G.no);
-  const uint32_t rem = unit - j * (G.nlayers * G.no);
-  stage_repage_unit<CAST, POW2, SCALED, PPOW2>(P, j, G.layer_begin + rem / G.no, rem % G.no, r, scales);
-}
-
-// kvbm_paged_stage_repage_gather_kernel's unit walk behind the stage gate; unit = (l * num_big + j) * no + o over the layer range,
-// so a batch that crosses a stage boundary gates on the next stage's sources when it enters that layer.
-template <int CAST, bool POW2, bool SCALED, bool PPOW2>
-__global__ void __launch_bounds__(256)
-kvbm_gated_stage_repage_gather_kernel(const __grid_constant__ StageRepageParams P, const __grid_constant__ GateArgs A, uint32_t num_big,
-                                      RowSplit r, const float* scales, uint32_t batch)
-{
-  const RepageGeom& G = P.geo;
-  const uint32_t per_layer = num_big * G.no;
-  gated_units(
-      A, per_layer * G.nlayers, batch, [&](uint32_t u) { return G.layer_begin + u / per_layer; },
-      [&](uint32_t u, uint32_t l) {
-        const uint32_t rem = u - (l - G.layer_begin) * per_layer;
-        const uint32_t j = rem / G.no;
-        stage_repage_unit<CAST, POW2, SCALED, PPOW2>(P, j, l, rem - j * G.no, r, scales);
-      },
-      [&](uint32_t l, uint32_t* s_ok) { return gate_stage_layer(A, P.s, l, s_ok); });
 }
 
 // The stream-wait form's signal after layer l: its layer-done flag, and after the last layer the done and completion flags.
@@ -1278,12 +1157,6 @@ static cudaError_t preload_kernels()
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_gather_kernel<c, p, sc>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_gather_kernel<c, p, sc, true>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_gather_kernel<c, p, sc, false>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_stage_gather_kernel<c, p, sc>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_stage_gather_kernel<c, p, sc>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_stage_repage_gather_kernel<c, p, sc, true>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_stage_repage_gather_kernel<c, p, sc, false>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_stage_repage_gather_kernel<c, p, sc, true>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_stage_repage_gather_kernel<c, p, sc, false>);
         });
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_layer_signal_kernel);
   return e;
@@ -1356,10 +1229,6 @@ static bool cast_rows(uint32_t src_row_bytes, int cast_mode, uint64_t* dst_row_b
   return true;
 }
 
-// The sources of a gather into P->D (dst_num_heads heads): each source's layers and outer dims those of the destination, its
-// window inside both sides' heads and on destination heads no other window writes (two would race), its region page * its
-// heads * row, its strides, and at most max_covered covered heads in all.  Fills P->src, P->covered and, with several sources,
-// the head map P->entry.
 // One source of a gather into a destination of dst_num_heads heads, outer_dim no and strides D: its table, its outer dims, its
 // window inside both sides' heads, its region page * its heads * row and its strides over its own src_nl layers.  Fills *G but
 // G->first.
@@ -1382,35 +1251,14 @@ static bool heads_overlap(const kvbm_permute_source& a, const kvbm_permute_sourc
   return a.dst_head_begin < b.dst_head_begin + b.head_count && b.dst_head_begin < a.dst_head_begin + a.head_count;
 }
 
-static bool fill_gather_sources(const kvbm_permute_source* srcs, int num_srcs, uint32_t dst_num_heads, uint32_t nl, uint32_t no,
-                                uint32_t page_size, uint32_t src_row_bytes, uint32_t max_covered, GatherParams* P)
-{
-  uint32_t covered = 0;
-  for (int s = 0; s < num_srcs; ++s) {
-    const kvbm_permute_source& X = srcs[s];
-    if (X.side.layout.num_layers != nl) return false;
-    for (int t = 0; t < s; ++t)
-      if (heads_overlap(X, srcs[t])) return false;
-    GatherSource& G = P->src[s];
-    if (!fill_gather_source(X, nl, dst_num_heads, no, page_size, src_row_bytes, P->D, &G)) return false;
-    if (static_cast<uint64_t>(covered) + X.head_count > max_covered) return false;
-    G.first = covered;
-    if (num_srcs > 1)
-      for (uint32_t j = 0; j < X.head_count; ++j) P->entry[covered + j] = static_cast<uint8_t>(s);
-    covered += X.head_count;
-  }
-  P->covered = covered;
-  return true;
-}
-
-// The sources of a staged gather into P->g.D (nl layers, dst_num_heads heads) over destination layers [lb, le): each layer window
+// The sources of a gather into P->D (nl layers, dst_num_heads heads) over destination layers [lb, le): each layer window
 // non-empty and inside its source's own layers and the destination's; two windows equal (one stage) or disjoint in the
 // destination; the stages covering every layer of [lb, le); within a stage, windows on destination heads no other window of the
-// stage writes; every rule of fill_gather_source; at most KVBM_GATHER_MAX_HEADS covered heads over all stages.  Fills P->g's
-// sources and one head map, stage by stage in ascending destination layers, P->stage and P->shift; *widest: the most heads of
-// one stage.
+// stage writes (two would race); every rule of fill_gather_source; at most max_covered covered heads over all stages.  Fills
+// P->src, P->covered, P->stage and P->shift, and with several sources the head map P->entry, stage by stage in ascending
+// destination layers; *widest: the most heads of one stage.
 static bool fill_stage_sources(const kvbm_stage_source* srcs, int num_srcs, uint32_t dst_num_heads, uint32_t nl, uint32_t no, int lb, int le,
-                               uint32_t page_size, uint32_t src_row_bytes, StageGatherParams* P, uint32_t* widest)
+                               uint32_t page_size, uint32_t src_row_bytes, uint32_t max_covered, GatherParams* P, uint32_t* widest)
 {
   int stage_of_src[KVBM_GATHER_MAX_SOURCES];
   int num_stages = 0;
@@ -1454,18 +1302,19 @@ static bool fill_stage_sources(const kvbm_stage_source* srcs, int num_srcs, uint
     for (int s = 0; s < num_srcs; ++s) {
       if (!((S.sources >> s) & 1u)) continue;
       const kvbm_permute_source& X = srcs[s].src;
-      GatherSource& G = P->g.src[s];
-      if (!fill_gather_source(X, X.side.layout.num_layers, dst_num_heads, no, page_size, src_row_bytes, P->g.D, &G)) return false;
-      if (static_cast<uint64_t>(covered) + X.head_count > KVBM_GATHER_MAX_HEADS) return false;
+      GatherSource& G = P->src[s];
+      if (!fill_gather_source(X, X.side.layout.num_layers, dst_num_heads, no, page_size, src_row_bytes, P->D, &G)) return false;
+      if (static_cast<uint64_t>(covered) + X.head_count > max_covered) return false;
       G.first = covered;
-      for (uint32_t j = 0; j < X.head_count; ++j) P->g.entry[covered + j] = static_cast<uint8_t>(s);
+      if (num_srcs > 1)
+        for (uint32_t j = 0; j < X.head_count; ++j) P->entry[covered + j] = static_cast<uint8_t>(s);
       covered += X.head_count;
     }
     S.count = covered - S.first;
     *widest = std::max(*widest, S.count);
   }
   std::copy(sorted, sorted + KVBM_GATHER_MAX_SOURCES, T);
-  P->g.covered = covered;
+  P->covered = covered;
   return true;
 }
 
@@ -1545,13 +1394,12 @@ static cudaError_t gate_args(const kvbm_permute_stream& st, int num_srcs, uint32
 
 // A streamed launch of `units` units over layers [layer_begin, layer_end) of an nl-layer destination, after every argument check.
 // The spinning form: launch_gated(A, ctas, batch) launches the gated kernel, which writes every flag itself.  The stream-wait
-// form: per layer, the stream waits for every source's flag (cuStreamWaitValue32, GEQ: the cyclic order of epoch_reached),
-// launch_layer(l) moves the layer unsignalled, and one signal launch writes its layer-done flag, plus the done and completion
-// flags after the last layer.  Nothing resident spins.  staged: a staged gather's stages, whose stream-wait form waits per layer
-// for only the flags of that layer's stage, each source's at its own layer.
+// form: per layer l, the stream waits for the flag of every source of l's stage in P at the source's own layer
+// (cuStreamWaitValue32, GEQ: the cyclic order of epoch_reached), launch_layer(l) moves the layer unsignalled, and one signal
+// launch writes its layer-done flag, plus the done and completion flags after the last layer.  Nothing resident spins.
 template <class Layer, class Gated>
-static cudaError_t launch_streamed(const kvbm_permute_stream& st, int num_srcs, uint32_t nl, int layer_begin, int layer_end, uint64_t units,
-                                   cudaStream_t stream, Layer&& launch_layer, Gated&& launch_gated, const StageGatherParams* staged = nullptr)
+static cudaError_t launch_streamed(const kvbm_permute_stream& st, const GatherParams& P, int num_srcs, uint32_t nl, int layer_begin,
+                                   int layer_end, uint64_t units, cudaStream_t stream, Layer&& launch_layer, Gated&& launch_gated)
 {
   cudaError_t e;
   const int form = gate_form(st, &e);
@@ -1565,10 +1413,10 @@ static cudaError_t launch_streamed(const kvbm_permute_stream& st, int num_srcs, 
     return launched(stream);
   }
   for (int l = layer_begin; l < layer_end; ++l) {
-    const uint32_t mask = staged ? stage_of(*staged, static_cast<uint32_t>(l)).sources : ~0u;
+    const uint32_t mask = stage_of(P, static_cast<uint32_t>(l)).sources;
     for (int s = 0; s < num_srcs; ++s) {
       if (!((mask >> s) & 1u)) continue;
-      const uint32_t* flag = st.layer_ready_flags[s] + (staged ? static_cast<uint32_t>(l) + staged->shift[s] : static_cast<uint32_t>(l));
+      const uint32_t* flag = st.layer_ready_flags[s] + (static_cast<uint32_t>(l) + P.shift[s]);
       if (g_wait32(stream, reinterpret_cast<unsigned long long>(flag), st.epoch, 0) != 0) return cudaErrorUnknown;
     }
     if ((e = launch_layer(l)) != cudaSuccess) return e;
@@ -1584,17 +1432,33 @@ static cudaError_t launch_streamed(const kvbm_permute_stream& st, int num_srcs, 
   return cudaSuccess;
 }
 
-// Every permuting launch: a head transform is one source, a gather several.  Runs the checks of both entries once, signals
-// when there is nothing to move, and launches kvbm_paged_permute_kernel for one source (the faster of the two, DESIGN §4.2b) or
-// kvbm_paged_gather_kernel for several.  max_covered: how many destination heads the sources may cover together; at most
-// KVBM_GATHER_MAX_HEADS (the gather's head map) whenever num_srcs > 1.  st: a streamed launch (its flags are the ones passed),
-// which takes the gated gather kernel, or per layer this launch unstreamed.  staged: the same sources with layer windows
-// (srcs[s] is staged[s].src), a staged gather checked by fill_stage_sources, which takes the stage gather kernels.
-static cudaError_t launch_paged_permute(const kvbm_permute_source* srcs, int num_srcs, const kvbm_permute_side* dst, uint32_t dst_num_heads,
+// A source that moves its own layers, all nl of the destination's: its layer window is the identity over them (a PP1 plan).
+static bool whole_layers(const kvbm_stage_source& X, uint32_t nl)
+{
+  return X.src_layer_begin == 0 && X.dst_layer_begin == 0 && X.layer_count == nl && X.src.side.layout.num_layers == nl;
+}
+
+// The sources of an entry without layer windows in out[]: one stage over every layer of dst, every shift 0.  The gather's rule
+// that each source has the destination's num_layers stays: a source without gets an empty window, which fill_stage_sources
+// rejects.  A null srcs or a num_srcs outside 1 .. KVBM_GATHER_MAX_SOURCES gives null, which the launch rejects.
+static const kvbm_stage_source* one_stage(const kvbm_permute_source* srcs, int num_srcs, const kvbm_permute_side* dst, kvbm_stage_source* out)
+{
+  if (!srcs || num_srcs < 1 || num_srcs > KVBM_GATHER_MAX_SOURCES) return nullptr;
+  const uint32_t nl = dst ? dst->layout.num_layers : 0;
+  for (int s = 0; s < num_srcs; ++s) out[s] = kvbm_stage_source{srcs[s], 0, 0, srcs[s].side.layout.num_layers == nl ? nl : 0};
+  return out;
+}
+
+// Every permuting launch: a head transform is one source, a gather several, each with a layer window.  Runs the checks of every
+// entry once, signals when there is nothing to move, and launches kvbm_paged_permute_kernel for one source over its whole layers
+// (the faster of the two, DESIGN §4.2b) or else kvbm_paged_gather_kernel.  max_covered: how many destination heads the sources
+// may cover together; at most KVBM_GATHER_MAX_HEADS (the gather's head map) unless the launch is the permute kernel's.  st: a
+// streamed launch (its flags are the ones passed), which takes the gated gather kernel, or per layer this launch unstreamed.
+static cudaError_t launch_paged_permute(const kvbm_stage_source* srcs, int num_srcs, const kvbm_permute_side* dst, uint32_t dst_num_heads,
                                         int num_blocks, int layer_begin, int layer_end, uint32_t page_size, uint32_t src_row_bytes,
                                         int cast_mode, const float* cast_scales, uint32_t* done_flag, uint32_t epoch,
                                         uint32_t* completion_flag, uint32_t completion_value, uint32_t max_covered, cudaStream_t stream,
-                                        const kvbm_permute_stream* st = nullptr, const kvbm_stage_source* staged = nullptr)
+                                        const kvbm_permute_stream* st = nullptr)
 {
   if (num_blocks < 0 || layer_begin < 0 || layer_end < layer_begin) return cudaErrorInvalidValue;
   if (!cast_args_ok(cast_mode, cast_scales)) return cudaErrorInvalidValue;
@@ -1608,43 +1472,34 @@ static cudaError_t launch_paged_permute(const kvbm_permute_source* srcs, int num
   RowSplit r;
   if (page_size == 0 || !row_split(walk_row, page_size, &r)) return cudaErrorInvalidValue;
   if (static_cast<uint64_t>(page_size) * dst_num_heads * dst_row_bytes != dst->layout.region_bytes) return cudaErrorInvalidValue;
-  StageGatherParams SP{};
-  GatherParams& P = SP.g;
+  GatherParams P{};
   if (!fill_permute_side(*dst, nl, no, dst_num_heads, page_size, static_cast<uint32_t>(dst_row_bytes), &P.D)) return cudaErrorInvalidValue;
-  uint32_t widest = 0;
-  if (staged ? !fill_stage_sources(staged, num_srcs, dst_num_heads, nl, no, layer_begin, layer_end, page_size, src_row_bytes, &SP, &widest)
-             : !fill_gather_sources(srcs, num_srcs, dst_num_heads, nl, no, page_size, src_row_bytes, max_covered, &P))
+  uint32_t widest;
+  if (!fill_stage_sources(srcs, num_srcs, dst_num_heads, nl, no, layer_begin, layer_end, page_size, src_row_bytes, max_covered, &P, &widest))
     return cudaErrorInvalidValue;
-  const uint32_t covered = P.covered;
   const uint64_t units = static_cast<uint64_t>(num_blocks) * (layer_end - layer_begin) * no;
   if (units >= (1ull << 31)) return cudaErrorInvalidValue;
-  const int threads = static_cast<int>(std::min<uint32_t>(8, staged ? widest : covered)) * 32;
+  const int threads = static_cast<int>(std::min<uint32_t>(8, widest)) * 32;
   const unsigned grid = static_cast<unsigned>(units);
   const uint32_t lb = static_cast<uint32_t>(layer_begin), nlay = static_cast<uint32_t>(layer_end - layer_begin);
   if (st)
     return launch_streamed(
-        *st, num_srcs, nl, layer_begin, layer_end, units, stream,
+        *st, P, num_srcs, nl, layer_begin, layer_end, units, stream,
         [&](int l) {
           return launch_paged_permute(srcs, num_srcs, dst, dst_num_heads, num_blocks, l, l + 1, page_size, src_row_bytes, cast_mode,
-                                      cast_scales, nullptr, 0, nullptr, 0, max_covered, stream, nullptr, staged);
+                                      cast_scales, nullptr, 0, nullptr, 0, max_covered, stream);
         },
         [&](const GateArgs& A, unsigned ctas, uint32_t batch) {
           with_walk_kernel(cast_mode, r.pow2, cast_scales != nullptr, [&](auto c, auto p, auto sc) {
-            if (staged)
-              kvbm_gated_stage_gather_kernel<c, p, sc><<<ctas, threads, 0, stream>>>(SP, A, static_cast<uint32_t>(num_blocks), lb, nlay, no,
-                                                                                     page_size, r, cast_scales, batch);
-            else
-              kvbm_gated_gather_kernel<c, p, sc><<<ctas, threads, 0, stream>>>(P, A, static_cast<uint32_t>(num_blocks), lb, nlay, no, page_size,
-                                                                               r, cast_scales, batch);
+            kvbm_gated_gather_kernel<c, p, sc><<<ctas, threads, 0, stream>>>(P, A, static_cast<uint32_t>(num_blocks), lb, nlay, no, page_size,
+                                                                             r, cast_scales, batch);
           });
-        },
-        staged ? &SP : nullptr);
+        });
   with_walk_kernel(cast_mode, r.pow2, cast_scales != nullptr, [&](auto c, auto p, auto sc) {
     const GatherSource& G = P.src[0];
-    if (staged)
-      kvbm_paged_stage_gather_kernel<c, p, sc><<<grid, threads, 0, stream>>>(SP, lb, nlay, no, page_size, r, cast_scales);
-    else if (num_srcs == 1)
-      kvbm_paged_permute_kernel<c, p, sc><<<grid, threads, 0, stream>>>(G.S, P.D, lb, nlay, no, covered, page_size, r, G.s_win, G.d_win, cast_scales);
+    if (num_srcs == 1 && whole_layers(srcs[0], nl))
+      kvbm_paged_permute_kernel<c, p, sc><<<grid, threads, 0, stream>>>(G.S, P.D, lb, nlay, no, P.covered, page_size, r, G.s_win, G.d_win,
+                                                                        cast_scales);
     else
       kvbm_paged_gather_kernel<c, p, sc><<<grid, threads, 0, stream>>>(P, lb, nlay, no, page_size, r, cast_scales);
   });
@@ -1693,18 +1548,16 @@ static bool repage_geometry(uint32_t src_page, uint32_t dst_page, uint32_t token
   return true;
 }
 
-// Every re-paging launch: a plain re-page is one source whose window covers every head of both sides, a re-paging gather one
-// or more windows.  Runs the checks of launch_paged_permute's sources and of repage_geometry's pages, each side's region at its
-// own page and head count, all before any CUDA call; signals when there is nothing to move; then launches
+// Every re-paging launch: a plain re-page is one source whose window covers every head and every layer of both sides, a
+// re-paging gather one or more windows.  Runs the checks of launch_paged_permute's sources and of repage_geometry's pages, each
+// side's region at its own page and head count, all before any CUDA call; signals when there is nothing to move; then launches
 // kvbm_paged_repage_kernel for a plain re-page, else kvbm_paged_repage_gather_kernel, and the signal.  max_covered and st: as
-// launch_paged_permute's (st takes the gated re-paging gather kernel, or per layer this launch unstreamed).  staged: as
-// launch_paged_permute's, checked by fill_stage_sources at the source page, which takes the stage re-paging gather kernels.
-static cudaError_t launch_paged_repage_gather(const kvbm_permute_source* srcs, int num_srcs, uint32_t src_page, const kvbm_permute_side* dst,
+// launch_paged_permute's (st takes the gated re-paging gather kernel, or per layer this launch unstreamed).
+static cudaError_t launch_paged_repage_gather(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page, const kvbm_permute_side* dst,
                                               uint32_t dst_num_heads, uint32_t dst_page, uint32_t token_begin, uint32_t token_end,
                                               int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
                                               uint32_t* done_flag, uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value,
-                                              uint32_t max_covered, cudaStream_t stream, const kvbm_permute_stream* st = nullptr,
-                                              const kvbm_stage_source* staged = nullptr)
+                                              uint32_t max_covered, cudaStream_t stream, const kvbm_permute_stream* st = nullptr)
 {
   if (layer_begin < 0 || layer_end < layer_begin || token_end < token_begin) return cudaErrorInvalidValue;
   if (!cast_args_ok(cast_mode, cast_scales)) return cudaErrorInvalidValue;
@@ -1714,58 +1567,45 @@ static cudaError_t launch_paged_repage_gather(const kvbm_permute_source* srcs, i
   const uint32_t nl = dst->layout.num_layers, no = dst->layout.outer_dim;
   if (nl == 0 || no == 0 || static_cast<uint32_t>(layer_end) > nl) return cudaErrorInvalidValue;
   RepageGatherParams P{};
-  StageRepageParams SP{};
-  GatherParams& g = staged ? SP.s.g : P.g;
-  RepageGeom& geo = staged ? SP.geo : P.geo;
   RowSplit r;
   uint64_t dst_row_bytes, units;
   bool page_pow2;
-  if (!repage_geometry(src_page, dst_page, token_begin, token_end, layer_begin, layer_end, no, src_row_bytes, cast_mode, &geo, &r,
+  if (!repage_geometry(src_page, dst_page, token_begin, token_end, layer_begin, layer_end, no, src_row_bytes, cast_mode, &P.geo, &r,
                        &dst_row_bytes, &units, &page_pow2))
     return cudaErrorInvalidValue;
   if (static_cast<uint64_t>(dst_page) * dst_num_heads * dst_row_bytes != dst->layout.region_bytes) return cudaErrorInvalidValue;
-  if (!fill_permute_side(*dst, nl, no, dst_num_heads, dst_page, static_cast<uint32_t>(dst_row_bytes), &g.D)) return cudaErrorInvalidValue;
-  uint32_t widest = 0;
-  if (staged ? !fill_stage_sources(staged, num_srcs, dst_num_heads, nl, no, layer_begin, layer_end, src_page, src_row_bytes, &SP.s, &widest)
-             : !fill_gather_sources(srcs, num_srcs, dst_num_heads, nl, no, src_page, src_row_bytes, max_covered, &P.g))
+  if (!fill_permute_side(*dst, nl, no, dst_num_heads, dst_page, static_cast<uint32_t>(dst_row_bytes), &P.g.D)) return cudaErrorInvalidValue;
+  uint32_t widest;
+  if (!fill_stage_sources(srcs, num_srcs, dst_num_heads, nl, no, layer_begin, layer_end, src_page, src_row_bytes, max_covered, &P.g, &widest))
     return cudaErrorInvalidValue;
-  geo.nh = g.covered;
-  const int threads = static_cast<int>(std::min<uint32_t>(8, staged ? widest : g.covered)) * 32;
+  P.geo.nh = P.g.covered;
+  const int threads = static_cast<int>(std::min<uint32_t>(8, widest)) * 32;
   const unsigned grid = static_cast<unsigned>(units);
   if (st)
     return launch_streamed(
-        *st, num_srcs, nl, layer_begin, layer_end, units, stream,
+        *st, P.g, num_srcs, nl, layer_begin, layer_end, units, stream,
         [&](int l) {
           return launch_paged_repage_gather(srcs, num_srcs, src_page, dst, dst_num_heads, dst_page, token_begin, token_end, l, l + 1,
-                                            src_row_bytes, cast_mode, cast_scales, nullptr, 0, nullptr, 0, max_covered, stream, nullptr,
-                                            staged);
+                                            src_row_bytes, cast_mode, cast_scales, nullptr, 0, nullptr, 0, max_covered, stream);
         },
         [&](const GateArgs& A, unsigned ctas, uint32_t batch) {
-          const uint32_t num_big = static_cast<uint32_t>(units / (static_cast<uint64_t>(geo.nlayers) * no));
+          const uint32_t num_big = static_cast<uint32_t>(units / (static_cast<uint64_t>(P.geo.nlayers) * no));
           with_walk_kernel(cast_mode, r.pow2, cast_scales != nullptr, [&](auto c, auto p, auto sc) {
-            if (staged && page_pow2)
-              kvbm_gated_stage_repage_gather_kernel<c, p, sc, true><<<ctas, threads, 0, stream>>>(SP, A, num_big, r, cast_scales, batch);
-            else if (staged)
-              kvbm_gated_stage_repage_gather_kernel<c, p, sc, false><<<ctas, threads, 0, stream>>>(SP, A, num_big, r, cast_scales, batch);
-            else if (page_pow2)
+            if (page_pow2)
               kvbm_gated_repage_gather_kernel<c, p, sc, true><<<ctas, threads, 0, stream>>>(P, A, num_big, r, cast_scales, batch);
             else
               kvbm_gated_repage_gather_kernel<c, p, sc, false><<<ctas, threads, 0, stream>>>(P, A, num_big, r, cast_scales, batch);
           });
-        },
-        staged ? &SP.s : nullptr);
-  // a window over every head of both sides (the checks above make both its starts 0)
-  const bool plain = !staged && num_srcs == 1 && srcs[0].head_count == srcs[0].num_heads && srcs[0].head_count == dst_num_heads;
+        });
+  // a window over every layer and every head of both sides (the checks above make its starts 0)
+  const kvbm_permute_source& X = srcs[0].src;
+  const bool plain = num_srcs == 1 && whole_layers(srcs[0], nl) && X.head_count == X.num_heads && X.head_count == dst_num_heads;
   RepageParams R{};
   R.big = P.geo.src_small ? P.g.D : P.g.src[0].S;
   R.small = P.geo.src_small ? P.g.src[0].S : P.g.D;
   R.g = P.geo;
   with_walk_kernel(cast_mode, r.pow2, cast_scales != nullptr, [&](auto c, auto p, auto sc) {
-    if (staged && page_pow2)
-      kvbm_paged_stage_repage_gather_kernel<c, p, sc, true><<<grid, threads, 0, stream>>>(SP, r, cast_scales);
-    else if (staged)
-      kvbm_paged_stage_repage_gather_kernel<c, p, sc, false><<<grid, threads, 0, stream>>>(SP, r, cast_scales);
-    else if (plain && page_pow2)
+    if (plain && page_pow2)
       kvbm_paged_repage_kernel<c, p, sc, true><<<grid, threads, 0, stream>>>(R, r, cast_scales);
     else if (plain)
       kvbm_paged_repage_kernel<c, p, sc, false><<<grid, threads, 0, stream>>>(R, r, cast_scales);
@@ -1938,8 +1778,9 @@ kvbm_kernels_paged_permute_heads_scaled(const kvbm_permute_side* src, const kvbm
                                         uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
 {
   const kvbm_permute_source one{src ? *src : kvbm_permute_side{}, src_num_heads, src_head_begin, dst_head_begin, head_count};
-  return launch_paged_permute(&one, 1, dst, dst_num_heads, num_blocks, layer_begin, layer_end, page_size, src_row_bytes, cast_mode,
-                              cast_scales, done_flag, epoch, completion_flag, completion_value, UINT32_MAX, stream);
+  kvbm_stage_source staged[1];
+  return launch_paged_permute(one_stage(&one, 1, dst, staged), 1, dst, dst_num_heads, num_blocks, layer_begin, layer_end, page_size,
+                              src_row_bytes, cast_mode, cast_scales, done_flag, epoch, completion_flag, completion_value, UINT32_MAX, stream);
 }
 
 extern "C" cudaError_t
@@ -1959,8 +1800,10 @@ kvbm_kernels_paged_permute_gather_scaled(const kvbm_permute_source* srcs, int nu
                                          uint32_t src_row_bytes, int cast_mode, const float* cast_scales, uint32_t* done_flag,
                                          uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
 {
-  return launch_paged_permute(srcs, num_srcs, dst, dst_num_heads, num_blocks, layer_begin, layer_end, page_size, src_row_bytes, cast_mode,
-                              cast_scales, done_flag, epoch, completion_flag, completion_value, KVBM_GATHER_MAX_HEADS, stream);
+  kvbm_stage_source staged[KVBM_GATHER_MAX_SOURCES];
+  return launch_paged_permute(one_stage(srcs, num_srcs, dst, staged), num_srcs, dst, dst_num_heads, num_blocks, layer_begin, layer_end,
+                              page_size, src_row_bytes, cast_mode, cast_scales, done_flag, epoch, completion_flag, completion_value,
+                              KVBM_GATHER_MAX_HEADS, stream);
 }
 
 extern "C" cudaError_t
@@ -1970,9 +1813,10 @@ kvbm_kernels_paged_repage(const kvbm_permute_side* src, uint32_t src_page_size, 
                           uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
 {
   const kvbm_permute_source one{src ? *src : kvbm_permute_side{}, num_heads, 0, 0, num_heads};
-  return launch_paged_repage_gather(&one, 1, src_page_size, dst, num_heads, dst_page_size, token_begin, token_end, layer_begin, layer_end,
-                                    src_row_bytes, cast_mode, cast_scales, done_flag, epoch, completion_flag, completion_value, UINT32_MAX,
-                                    stream);
+  kvbm_stage_source staged[1];
+  return launch_paged_repage_gather(one_stage(&one, 1, dst, staged), 1, src_page_size, dst, num_heads, dst_page_size, token_begin, token_end,
+                                    layer_begin, layer_end, src_row_bytes, cast_mode, cast_scales, done_flag, epoch, completion_flag,
+                                    completion_value, UINT32_MAX, stream);
 }
 
 extern "C" cudaError_t
@@ -1981,9 +1825,10 @@ kvbm_kernels_paged_repage_gather(const kvbm_permute_source* srcs, int num_srcs, 
                                  int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales, uint32_t* done_flag,
                                  uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
 {
-  return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, token_begin, token_end, layer_begin,
-                                    layer_end, src_row_bytes, cast_mode, cast_scales, done_flag, epoch, completion_flag, completion_value,
-                                    KVBM_GATHER_MAX_HEADS, stream);
+  kvbm_stage_source staged[KVBM_GATHER_MAX_SOURCES];
+  return launch_paged_repage_gather(one_stage(srcs, num_srcs, dst, staged), num_srcs, src_page_size, dst, dst_num_heads, dst_page_size,
+                                    token_begin, token_end, layer_begin, layer_end, src_row_bytes, cast_mode, cast_scales, done_flag, epoch,
+                                    completion_flag, completion_value, KVBM_GATHER_MAX_HEADS, stream);
 }
 
 extern "C" cudaError_t
@@ -1992,56 +1837,10 @@ kvbm_kernels_paged_permute_gather_streamed(const kvbm_permute_source* srcs, int 
                                            int cast_mode, const float* cast_scales, const kvbm_permute_stream* st, cudaStream_t stream)
 {
   if (!stream_args_ok(st, num_srcs)) return cudaErrorInvalidValue;
-  return launch_paged_permute(srcs, num_srcs, dst, dst_num_heads, num_blocks, layer_begin, layer_end, page_size, src_row_bytes, cast_mode,
-                              cast_scales, st->done_flag, st->epoch, st->completion_flag, st->completion_value, KVBM_GATHER_MAX_HEADS, stream,
-                              st);
-}
-
-// A staged entry's num_srcs (1 .. KVBM_GATHER_MAX_SOURCES) sources as plain gather sources (plain[s] = srcs[s].src), and the
-// layer windows to launch with: none when every window is the identity over a source whose num_layers is the destination's (a
-// PP1 plan), which then launches exactly what the unstaged entry launches.
-static const kvbm_stage_source* split_stages(const kvbm_stage_source* srcs, int num_srcs, const kvbm_permute_side* dst,
-                                             kvbm_permute_source* plain)
-{
-  bool identity = dst != nullptr;
-  for (int s = 0; s < num_srcs; ++s) {
-    const kvbm_stage_source& X = srcs[s];
-    plain[s] = X.src;
-    identity = identity && X.src_layer_begin == 0 && X.dst_layer_begin == 0 && X.layer_count == dst->layout.num_layers &&
-               X.src.side.layout.num_layers == dst->layout.num_layers;
-  }
-  return identity ? nullptr : srcs;
-}
-
-// The staged gather's entries: the gather's launch path with layer windows, or with none for a PP1 plan, which is then exactly
-// kvbm_kernels_paged_permute_gather_scaled / _streamed.
-static cudaError_t launch_stage_gather(const kvbm_stage_source* srcs, int num_srcs, const kvbm_permute_side* dst, uint32_t dst_num_heads,
-                                       int num_blocks, int layer_begin, int layer_end, uint32_t page_size, uint32_t src_row_bytes,
-                                       int cast_mode, const float* cast_scales, uint32_t* done_flag, uint32_t epoch,
-                                       uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream,
-                                       const kvbm_permute_stream* st = nullptr)
-{
-  if (!srcs || num_srcs < 1 || num_srcs > KVBM_GATHER_MAX_SOURCES) return cudaErrorInvalidValue;
-  kvbm_permute_source plain[KVBM_GATHER_MAX_SOURCES];
-  const kvbm_stage_source* staged = split_stages(srcs, num_srcs, dst, plain);
-  return launch_paged_permute(plain, num_srcs, dst, dst_num_heads, num_blocks, layer_begin, layer_end, page_size, src_row_bytes, cast_mode,
-                              cast_scales, done_flag, epoch, completion_flag, completion_value, KVBM_GATHER_MAX_HEADS, stream, st, staged);
-}
-
-// The staged re-paging gather's entries: the re-paging gather's launch path with layer windows, or with none for a PP1 plan, which
-// is then exactly kvbm_kernels_paged_repage_gather / _streamed.
-static cudaError_t launch_stage_repage_gather(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page, const kvbm_permute_side* dst,
-                                              uint32_t dst_num_heads, uint32_t dst_page, uint32_t token_begin, uint32_t token_end,
-                                              int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
-                                              uint32_t* done_flag, uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value,
-                                              cudaStream_t stream, const kvbm_permute_stream* st = nullptr)
-{
-  if (!srcs || num_srcs < 1 || num_srcs > KVBM_GATHER_MAX_SOURCES) return cudaErrorInvalidValue;
-  kvbm_permute_source plain[KVBM_GATHER_MAX_SOURCES];
-  const kvbm_stage_source* staged = split_stages(srcs, num_srcs, dst, plain);
-  return launch_paged_repage_gather(plain, num_srcs, src_page, dst, dst_num_heads, dst_page, token_begin, token_end, layer_begin, layer_end,
-                                    src_row_bytes, cast_mode, cast_scales, done_flag, epoch, completion_flag, completion_value,
-                                    KVBM_GATHER_MAX_HEADS, stream, st, staged);
+  kvbm_stage_source staged[KVBM_GATHER_MAX_SOURCES];
+  return launch_paged_permute(one_stage(srcs, num_srcs, dst, staged), num_srcs, dst, dst_num_heads, num_blocks, layer_begin, layer_end,
+                              page_size, src_row_bytes, cast_mode, cast_scales, st->done_flag, st->epoch, st->completion_flag,
+                              st->completion_value, KVBM_GATHER_MAX_HEADS, stream, st);
 }
 
 extern "C" cudaError_t
@@ -2051,9 +1850,9 @@ kvbm_kernels_paged_stage_repage_gather(const kvbm_stage_source* srcs, int num_sr
                                        uint32_t* done_flag, uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value,
                                        cudaStream_t stream)
 {
-  return launch_stage_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, token_begin, token_end, layer_begin,
+  return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, token_begin, token_end, layer_begin,
                                     layer_end, src_row_bytes, cast_mode, cast_scales, done_flag, epoch, completion_flag, completion_value,
-                                    stream);
+                                    KVBM_GATHER_MAX_HEADS, stream);
 }
 
 extern "C" cudaError_t
@@ -2064,9 +1863,9 @@ kvbm_kernels_paged_stage_repage_gather_streamed(const kvbm_stage_source* srcs, i
                                                 const kvbm_permute_stream* st, cudaStream_t stream)
 {
   if (!stream_args_ok(st, num_srcs)) return cudaErrorInvalidValue;
-  return launch_stage_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, token_begin, token_end, layer_begin,
+  return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, token_begin, token_end, layer_begin,
                                     layer_end, src_row_bytes, cast_mode, cast_scales, st->done_flag, st->epoch, st->completion_flag,
-                                    st->completion_value, stream, st);
+                                    st->completion_value, KVBM_GATHER_MAX_HEADS, stream, st);
 }
 
 extern "C" cudaError_t
@@ -2075,8 +1874,8 @@ kvbm_kernels_paged_stage_gather(const kvbm_stage_source* srcs, int num_srcs, con
                                 const float* cast_scales, uint32_t* done_flag, uint32_t epoch, uint32_t* completion_flag,
                                 uint32_t completion_value, cudaStream_t stream)
 {
-  return launch_stage_gather(srcs, num_srcs, dst, dst_num_heads, num_blocks, layer_begin, layer_end, page_size, src_row_bytes, cast_mode,
-                             cast_scales, done_flag, epoch, completion_flag, completion_value, stream);
+  return launch_paged_permute(srcs, num_srcs, dst, dst_num_heads, num_blocks, layer_begin, layer_end, page_size, src_row_bytes, cast_mode,
+                              cast_scales, done_flag, epoch, completion_flag, completion_value, KVBM_GATHER_MAX_HEADS, stream);
 }
 
 extern "C" cudaError_t
@@ -2085,8 +1884,9 @@ kvbm_kernels_paged_stage_gather_streamed(const kvbm_stage_source* srcs, int num_
                                          int cast_mode, const float* cast_scales, const kvbm_permute_stream* st, cudaStream_t stream)
 {
   if (!stream_args_ok(st, num_srcs)) return cudaErrorInvalidValue;
-  return launch_stage_gather(srcs, num_srcs, dst, dst_num_heads, num_blocks, layer_begin, layer_end, page_size, src_row_bytes, cast_mode,
-                             cast_scales, st->done_flag, st->epoch, st->completion_flag, st->completion_value, stream, st);
+  return launch_paged_permute(srcs, num_srcs, dst, dst_num_heads, num_blocks, layer_begin, layer_end, page_size, src_row_bytes, cast_mode,
+                              cast_scales, st->done_flag, st->epoch, st->completion_flag, st->completion_value, KVBM_GATHER_MAX_HEADS, stream,
+                              st);
 }
 
 extern "C" cudaError_t
@@ -2096,9 +1896,10 @@ kvbm_kernels_paged_repage_gather_streamed(const kvbm_permute_source* srcs, int n
                                           const kvbm_permute_stream* st, cudaStream_t stream)
 {
   if (!stream_args_ok(st, num_srcs)) return cudaErrorInvalidValue;
-  return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, token_begin, token_end, layer_begin,
-                                    layer_end, src_row_bytes, cast_mode, cast_scales, st->done_flag, st->epoch, st->completion_flag,
-                                    st->completion_value, KVBM_GATHER_MAX_HEADS, stream, st);
+  kvbm_stage_source staged[KVBM_GATHER_MAX_SOURCES];
+  return launch_paged_repage_gather(one_stage(srcs, num_srcs, dst, staged), num_srcs, src_page_size, dst, dst_num_heads, dst_page_size,
+                                    token_begin, token_end, layer_begin, layer_end, src_row_bytes, cast_mode, cast_scales, st->done_flag,
+                                    st->epoch, st->completion_flag, st->completion_value, KVBM_GATHER_MAX_HEADS, stream, st);
 }
 
 extern "C" bool

@@ -4,10 +4,7 @@ window covers included).  Source pools hold only their stage's layers, so their 
 The streamed cases follow tests/test_gpu_transform_stream.py's discipline: poisoned sources, the launch first, per-layer writes
 and flag releases on one producer stream after it, the checker's state read once the launch finished, every flag released in
 a `finally`."""
-import os
 import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -27,8 +24,6 @@ ELEMS = {CM.NONE: (2, 2), CM.FP8E4M3_TO_BF16: (1, 2), CM.BF16_TO_FP8E4M3: (2, 1)
 GATES = [K.GATE_SPIN, K.GATE_STREAM_WAIT]
 GATE_IDS = ["spin", "stream_wait"]
 GUARD = 8                       # u32 words after every source's ready flags
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SO = os.path.join(ROOT, "dynamo_b200", "libkvbm_kernels.so")
 
 
 class StageRig:
@@ -226,19 +221,8 @@ WALKS = {(c, p, s) for c in (0, 1, 2) for p in (True, False) for s in ((False,) 
 EXPECTED = {(f, w) for f in ("paged", "gated") for w in WALKS}
 
 
-def test_the_expected_stage_set_is_what_the_library_contains():
-    assert len(EXPECTED) == 20
-    tool = shutil.which("cuobjdump") or next((p for p in ("/usr/local/cuda/bin/cuobjdump",) if os.path.exists(p)), None)
-    if not tool or not os.path.exists(SO):
-        pytest.skip("needs the built libkvbm_kernels.so and cuobjdump")
-    names = subprocess.run([tool, "-sass", SO], capture_output=True, text=True, check=True).stdout
-    found = {(m.group(1), (int(m.group(2)), m.group(3) == "1", m.group(4) == "1"))
-             for m in re.finditer(r"kvbm_(paged|gated)_stage_gather_kernelILi(\d)ELb(\d)ELb(\d)E", names)}
-    assert found == EXPECTED
-
-
 @pytest.mark.gpu
-def test_every_stage_instantiation_is_reached():
+def test_staged_plans_reach_every_gather_instantiation():
     from torch.profiler import ProfilerActivity, profile
     rigs = []
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
@@ -261,7 +245,7 @@ def test_every_stage_instantiation_is_reached():
     names = {e.name for e in prof.events()}
     found = set()
     for n in names:
-        for m in re.finditer(r"kvbm_(paged|gated)_stage_gather_kernel<([^<>]*)>", n):
+        for m in re.finditer(r"kvbm_(paged|gated)_gather_kernel<([^<>]*)>", n):
             c, p, s = (a.strip().replace("(int)", "") for a in m.group(2).split(","))
             found.add((m.group(1), (int(c), p == "true", s == "true")))
     assert found == EXPECTED, sorted(names)[:20]

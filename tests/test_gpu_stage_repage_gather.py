@@ -212,7 +212,7 @@ WALKS = {(c, p, s) for c in (0, 1, 2) for p in (True, False) for s in ((False,) 
 EXPECTED = {(f, w + (pp,)) for f in ("paged", "gated") for w in WALKS for pp in (True, False)}
 
 
-def test_every_stage_repage_instantiation_is_reached():
+def test_staged_plans_reach_every_repage_gather_instantiation():
     from torch.profiler import ProfilerActivity, profile
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         for c, p, s in sorted(WALKS):
@@ -232,7 +232,7 @@ def test_every_stage_repage_instantiation_is_reached():
                     r.check()
     found = set()
     for e in prof.events():
-        for m in re.finditer(r"kvbm_(paged|gated)_stage_repage_gather_kernel<([^<>]*)>", e.name):
+        for m in re.finditer(r"kvbm_(paged|gated)_repage_gather_kernel<([^<>]*)>", e.name):
             c, p, s, pp = (a.strip().replace("(int)", "") for a in m.group(2).split(","))
             found.add((m.group(1), (int(c), p == "true", s == "true", pp == "true")))
     assert found == EXPECTED

@@ -85,15 +85,18 @@ def _describe(s):
 
 def test_the_expected_set_is_what_the_library_contains():
     """The 100 instantiations the profiler test expects are exactly those compiled into libkvbm_kernels.so (cuobjdump, as
-    benchmarks/dump_sass.py reads them)."""
+    benchmarks/dump_sass.py reads them), and no kernel of the library is a staged twin of one of them."""
     assert len(EXPECTED) == 100
     so = os.path.join(ROOT, "dynamo_b200", "libkvbm_kernels.so")
     tool = shutil.which("cuobjdump") or next((p for p in ("/usr/local/cuda/bin/cuobjdump",) if os.path.exists(p)), None)
     if not os.path.exists(so) or tool is None:
         pytest.skip("needs the built libkvbm_kernels.so and cuobjdump")
     txt = subprocess.run([tool, "-sass", so], capture_output=True, text=True, check=True).stdout
-    found = _mangled(re.findall(r"Function : (\S+)", txt))
+    functions = re.findall(r"Function : (\S+)", txt)
+    found = _mangled(functions)
     assert found == EXPECTED, f"in the library only: {_describe(found - EXPECTED)}; expected only: {_describe(EXPECTED - found)}"
+    # the staged gathers are these gathers with a stage table: no second family of them
+    assert not [n for n in functions if "_stage_" in n]
 
 
 # ---------------------------------------------------------------------------------------------------------------------

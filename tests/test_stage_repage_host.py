@@ -2,10 +2,6 @@
 symbols, the oracle against the re-paging gather's and the staged gather's oracles, the kernel entry's argument checks that
 return before any CUDA call, the instantiations in the built library, and the manager's rejections on a host-only manager with
 the first rejection pinned for requests that fail two checks."""
-import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -18,8 +14,6 @@ from tests.repage_gather_oracle import repage_gather
 from tests.stage_oracle import stage_block
 from tests.stage_repage_oracle import stage_repage_gather
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SO = os.path.join(ROOT, "dynamo_b200", "libkvbm_kernels.so")
 KV = K.KvBlockLayout
 INVAL = K.CUDA_ERROR_INVALID_VALUE
 KINDS = [KV.UniversalTP, KV.UniversalPP, KV.OperationalHND, KV.OperationalNHD]
@@ -137,24 +131,6 @@ def test_stage_repage_argument_checks_before_any_cuda_call():
     st.sync_workspace = 0x4000
     st.layer_ready_flags[3] = 0                      # a used source without ready flags
     assert stream(st) == INVAL
-
-
-# ---------------------------------------------------------------------------------------------------------------------
-# the instantiations in the built library
-# ---------------------------------------------------------------------------------------------------------------------
-WALKS = {(c, p, s) for c in (0, 1, 2) for p in (True, False) for s in ((False,) if c == 0 else (False, True))}
-EXPECTED = {(f, w + (pp,)) for f in ("paged", "gated") for w in WALKS for pp in (True, False)}
-
-
-def test_the_expected_stage_repage_set_is_what_the_library_contains():
-    assert len(EXPECTED) == 40
-    tool = shutil.which("cuobjdump") or next((p for p in ("/usr/local/cuda/bin/cuobjdump",) if os.path.exists(p)), None)
-    if not tool or not os.path.exists(SO):
-        pytest.skip("needs the built libkvbm_kernels.so and cuobjdump")
-    names = subprocess.run([tool, "-sass", SO], capture_output=True, text=True, check=True).stdout
-    found = {(m.group(1), (int(m.group(2)), m.group(3) == "1", m.group(4) == "1", m.group(5) == "1"))
-             for m in re.finditer(r"kvbm_(paged|gated)_stage_repage_gather_kernelILi(\d)ELb(\d)ELb(\d)ELb(\d)E", names)}
-    assert found == EXPECTED
 
 
 # ---------------------------------------------------------------------------------------------------------------------
