@@ -542,20 +542,26 @@ static int acquire_slot(kvbm_transfer_manager* m, size_t ids_needed, size_t ws_n
 // The block tables of one launch on `stream`, optionally ordered after `wait_ev`: acquire a slot, narrow list k (lens[k] ids) to
 // int32 right after list k - 1 in its pinned staging (a null list leaves its run unwritten) and upload all of them with one async
 // copy (no host sync; the reference blocks on pointers_transfered_event.synchronize(), cuda.rs:324).
+// units (a batch's unit table, num_units 16 B records) travels in the same copy, behind the ids at units_at(total ids).
+static size_t units_at(size_t total_ids) { return (total_ids + 3) & ~size_t{3}; }  // in int32 entries: 16 B aligned in the slot
+
 static int stage_ids(kvbm_transfer_manager* m, const size_t* const* lists, const size_t* lens, size_t num_lists, size_t ws_needed,
-                     cudaStream_t stream, cudaEvent_t wait_ev, Slot** out, uint64_t* seq)
+                     cudaStream_t stream, cudaEvent_t wait_ev, Slot** out, uint64_t* seq, const kvbm_repage_unit* units = nullptr,
+                     size_t num_units = 0)
 {
   size_t total = 0;
   for (size_t k = 0; k < num_lists; ++k) total += lens[k];
-  int rc = acquire_slot(m, total, ws_needed, out, seq);
+  const size_t words = num_units ? units_at(total) + num_units * (sizeof(kvbm_repage_unit) / sizeof(int32_t)) : total;
+  int rc = acquire_slot(m, words, ws_needed, out, seq);
   if (rc) return rc;
   Slot* sl = *out;
   if (wait_ev) CU(cudaStreamWaitEvent(stream, wait_ev, 0));
   for (size_t k = 0, at = 0; k < num_lists; at += lens[k++])
     if (lists[k])
       for (size_t i = 0; i < lens[k]; ++i) sl->pinned_ids[at + i] = static_cast<int32_t>(lists[k][i]);
-  CU(cudaMemcpyAsync(sl->dev_ids, sl->pinned_ids, total * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
-  m->h2d_bytes += total * sizeof(int32_t);
+  if (num_units) std::memcpy(sl->pinned_ids + units_at(total), units, num_units * sizeof(kvbm_repage_unit));
+  CU(cudaMemcpyAsync(sl->dev_ids, sl->pinned_ids, words * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
+  m->h2d_bytes += words * sizeof(int32_t);
   return KVBM_OK;
 }
 
@@ -699,11 +705,12 @@ static int checked(cudaError_t e, const char* what) { return e == cudaSuccess ? 
 // becomes the kvbm_permute_source of e[j]'s source and head window, reading table e[j].window.src_rank; the destination's side
 // is e[0]'s; with ls, the gate.  `launch(sources, destination, gate or null, slot, seq)` makes the kernel call and returns its
 // code.  Then the slot counts `bytes`, *seq_out gets the launch's sequence number and *out the notification: 0 on a caller
-// stream, whose caller manages sync.
+// stream, whose caller manages sync.  units: a batch's unit table, staged behind the tables at units_at(every id) of the slot.
 template <class Launch>
 static int launch_transform(kvbm_transfer_manager* m, const Transfer* e, size_t nw, size_t num_srcs, const size_t* const* src_ids,
                             size_t n_src, const size_t* dst_ids, size_t n_dst, const kvbm_layer_stream* ls, const kvbm_transfer_options& o,
-                            cudaStream_t stream, uint64_t bytes, uint64_t* seq_out, kvbm_notification* out, Launch&& launch)
+                            cudaStream_t stream, uint64_t bytes, uint64_t* seq_out, kvbm_notification* out, Launch&& launch,
+                            const kvbm_repage_unit* units = nullptr, size_t num_units = 0)
 {
   // the tables' pointers and lengths fit on the stack for every request that names only the sources its windows read; a
   // gather may pass any number of sources
@@ -727,7 +734,7 @@ static int launch_transform(kvbm_transfer_manager* m, const Transfer* e, size_t 
   const Layout& D = *e[0].D[0];
   Slot* sl;
   uint64_t seq;
-  int rc = stage_ids(m, lists, lens, k, ls ? D.cfg.num_layers + 4 : 4, stream, nullptr, &sl, &seq);
+  int rc = stage_ids(m, lists, lens, k, ls ? D.cfg.num_layers + 4 : 4, stream, nullptr, &sl, &seq, units, num_units);
   if (rc) return rc;
   const kvbm_permute_side kd{descriptor(D), sl->dev_ids + num_srcs * n_src, e[0].dst_kv};
   kvbm_permute_source ks[KVBM_GATHER_MAX_SOURCES] = {};
@@ -1341,22 +1348,27 @@ static int repage_strategy(kvbm_transfer_manager* m, const Layout& S, const Layo
 // Otherwise the plain re-page (kvbm_manager_execute_repage): source 0 over every head of both sides, `windows` unused.  Its
 // source's handle is looked up first, its options fail the pair's checks, its head counts must be equal, and it is launched
 // through kvbm_kernels_paged_repage, which has no head limit.
-static int execute_repage_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, const size_t* const* src_ids,
-                                 size_t n_src, kvbm_layout_handle dst_h, const size_t* dst_ids, size_t n_dst, size_t tb, size_t te,
-                                 const kvbm_head_window* windows, size_t nw, const kvbm_transfer_options* opts_in, kvbm_notification* out,
-                                 const kvbm_layer_stream* ls = nullptr, bool gather = true, const kvbm_shard_window* layers = nullptr)
-{
-  kvbm_transfer_options o{};
-  if (opts_in) o = *opts_in;
-  if (out) *out = 0;
-  int rc;
-  if (gather && (rc = check_gather_windows(num_srcs, srcs, windows, nw, o, layers))) return rc;
-  std::lock_guard<std::mutex> lk(m->mu);
-  if (layers && (rc = check_stage_layers(m, srcs, dst_h, layers, nw, o))) return rc;
+// A re-paging request as check_repage_request validated it: every window's Transfer, the destination, the layer range and
+// whether there is nothing to move.
+struct RepageRequest {
+  Transfer e[KVBM_GATHER_MAX_SOURCES];
   Layout* D = nullptr;
+  size_t lb = 0, le = 0;
+  bool empty = false;
+};
+
+// Every check of a re-paging request after check_gather_windows, under the manager's lock, in the order above.
+static int check_repage_request(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, const size_t* const* src_ids,
+                                size_t n_src, kvbm_layout_handle dst_h, const size_t* dst_ids, size_t n_dst, size_t tb, size_t te,
+                                const kvbm_head_window* windows, size_t nw, const kvbm_transfer_options& o, const kvbm_layer_stream* ls,
+                                bool gather, const kvbm_shard_window* layers, RepageRequest* R)
+{
+  int rc;
+  if (layers && (rc = check_stage_layers(m, srcs, dst_h, layers, nw, o))) return rc;
+  Layout*& D = R->D = nullptr;
+  Transfer* e = R->e;
   auto find_dst = [&] { return (D = m->find(dst_h)) ? KVBM_OK : fail(KVBM_ERR_HANDLE, "invalid destination handle"); };
   if (gather && (rc = find_dst())) return rc;  // the plain re-page looks its destination up after its source, in the loop
-  Transfer e[KVBM_GATHER_MAX_SOURCES];
   for (size_t j = 0; j < nw; ++j) {
     Layout* S = e[j].S = m->find(srcs[gather ? windows[j].src_rank : 0]);
     if (!S) return fail(KVBM_ERR_HANDLE, "invalid source handle");
@@ -1373,10 +1385,8 @@ static int execute_repage_gather(kvbm_transfer_manager* m, size_t num_srcs, cons
   const Layout& S0 = *e[0].S;
   if (tb > te || te > (size_t{1} << 31))
     return fail(KVBM_ERR_RANGE, "Token range " + std::to_string(tb) + ".." + std::to_string(te) + " is reversed or reaches past 2^31 tokens");
-  size_t lb, le;
-  if ((rc = check_layer_range(layers ? D->cfg : S0.cfg, o, &lb, &le))) return rc;
-  const size_t ps = S0.cfg.page_size, pd = D->cfg.page_size;
-  if ((rc = check_repage_counts(tb, te, ps, pd, n_src, n_dst))) return rc;
+  if ((rc = check_layer_range(layers ? D->cfg : S0.cfg, o, &R->lb, &R->le))) return rc;
+  if ((rc = check_repage_counts(tb, te, S0.cfg.page_size, D->cfg.page_size, n_src, n_dst))) return rc;
   if ((n_src && !src_ids) || (n_dst && !dst_ids)) return fail(KVBM_ERR, "null block id list");
   for (size_t j = 0; j < nw; ++j) {
     const size_t r = e[j].window.src_rank;
@@ -1384,7 +1394,8 @@ static int execute_repage_gather(kvbm_transfer_manager* m, size_t num_srcs, cons
     if (n_src && !s) return fail(KVBM_ERR, "null block id list");
     if ((rc = check_block_ids(s, n_src, dst_ids, n_dst, e[j].S->cfg.num_blocks, D->cfg.num_blocks, srcs[r] == dst_h))) return rc;
   }
-  if (tb == te || lb == le) return KVBM_OK;  // nothing to move, as execute()
+  R->empty = tb == te || R->lb == R->le;
+  if (R->empty) return KVBM_OK;  // nothing to move, as execute()
   for (size_t j = 0; j < nw; ++j) {
     if ((rc = repage_strategy(m, *e[j].S, *D, &e[j].plan))) return rc;
     if (e[j].plan.first != e[0].plan.first) return fail(KVBM_ERR_UNSUPPORTED, "the sources of a gather need the same CUDA strategy");
@@ -1392,30 +1403,64 @@ static int execute_repage_gather(kvbm_transfer_manager* m, size_t num_srcs, cons
   if ((rc = need_cuda_device(m))) return rc;
   if (o.cast_scales && (rc = check_cast_scales(m, o.cast_scales))) return rc;
   if (ls && (rc = check_layer_stream_flags(m, *ls, e, nw))) return rc;
+  return KVBM_OK;
+}
 
-  DeviceGuard g(m->device);
-  const cudaStream_t stream = pick_stream(m, e[0].plan.first, o);
-  const size_t d_row = D->cfg.inner_dim / D->cfg.num_heads * D->cfg.dtype_width_bytes;
-  const uint32_t row = static_cast<uint32_t>(S0.cfg.inner_dim / S0.cfg.num_heads * S0.cfg.dtype_width_bytes);
-  const uint32_t ups = static_cast<uint32_t>(ps), upd = static_cast<uint32_t>(pd), dnh = static_cast<uint32_t>(D->cfg.num_heads);
-  const uint32_t utb = static_cast<uint32_t>(tb), ute = static_cast<uint32_t>(te);
-  const int ilb = static_cast<int>(lb), ile = static_cast<int>(le), k = static_cast<int>(nw);
+// What a validated request moves over tokens [tb, te): each window's destination bytes over its layers inside the layer range.
+static uint64_t repage_bytes(const RepageRequest& R, size_t nw, const kvbm_shard_window* layers, size_t tb, size_t te)
+{
+  const Layout& D = *R.D;
+  const size_t d_row = D.cfg.inner_dim / D.cfg.num_heads * D.cfg.dtype_width_bytes;
   uint64_t bytes = 0;
   for (size_t j = 0; j < nw; ++j) {
-    size_t from = lb, to = le;
+    size_t from = R.lb, to = R.le;
     if (layers) {
       from = std::max(from, layers[j].dst_layer_begin);
       to = std::min(to, layers[j].dst_layer_begin + layers[j].layer_count);
     }
-    if (to > from) bytes += (te - tb) * (to - from) * D->cfg.outer_dim * e[j].window.head_count * d_row;
+    if (to > from) bytes += (te - tb) * (to - from) * D.cfg.outer_dim * R.e[j].window.head_count * d_row;
   }
+  return bytes;
+}
+
+// The kernel sources of a staged plan: window j's gather source with its layer window.
+static void stage_sources(const kvbm_permute_source* ks, const kvbm_shard_window* layers, size_t nw, kvbm_stage_source* ss)
+{
+  for (size_t j = 0; j < nw; ++j)
+    ss[j] = kvbm_stage_source{ks[j], static_cast<uint32_t>(layers[j].src_layer_begin), static_cast<uint32_t>(layers[j].dst_layer_begin),
+                              static_cast<uint32_t>(layers[j].layer_count)};
+}
+
+static int execute_repage_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, const size_t* const* src_ids,
+                                 size_t n_src, kvbm_layout_handle dst_h, const size_t* dst_ids, size_t n_dst, size_t tb, size_t te,
+                                 const kvbm_head_window* windows, size_t nw, const kvbm_transfer_options* opts_in, kvbm_notification* out,
+                                 const kvbm_layer_stream* ls = nullptr, bool gather = true, const kvbm_shard_window* layers = nullptr)
+{
+  kvbm_transfer_options o{};
+  if (opts_in) o = *opts_in;
+  if (out) *out = 0;
+  int rc;
+  if (gather && (rc = check_gather_windows(num_srcs, srcs, windows, nw, o, layers))) return rc;
+  std::lock_guard<std::mutex> lk(m->mu);
+  RepageRequest R;
+  if ((rc = check_repage_request(m, num_srcs, srcs, src_ids, n_src, dst_h, dst_ids, n_dst, tb, te, windows, nw, o, ls, gather, layers, &R)))
+    return rc;
+  if (R.empty) return KVBM_OK;
+  const Transfer* e = R.e;
+  const Layout &S0 = *e[0].S, *D = R.D;
+
+  DeviceGuard g(m->device);
+  const cudaStream_t stream = pick_stream(m, e[0].plan.first, o);
+  const uint32_t row = static_cast<uint32_t>(S0.cfg.inner_dim / S0.cfg.num_heads * S0.cfg.dtype_width_bytes);
+  const uint32_t ups = static_cast<uint32_t>(S0.cfg.page_size), upd = static_cast<uint32_t>(D->cfg.page_size);
+  const uint32_t dnh = static_cast<uint32_t>(D->cfg.num_heads);
+  const uint32_t utb = static_cast<uint32_t>(tb), ute = static_cast<uint32_t>(te);
+  const int ilb = static_cast<int>(R.lb), ile = static_cast<int>(R.le), k = static_cast<int>(nw);
   auto launch = [&](const kvbm_permute_source* ks, const kvbm_permute_side& kd, const kvbm_permute_stream* st, const Slot& sl, uint64_t seq) {
     const uint32_t value = static_cast<uint32_t>(seq);
     if (layers) {
       kvbm_stage_source ss[KVBM_GATHER_MAX_SOURCES] = {};
-      for (size_t j = 0; j < nw; ++j)
-        ss[j] = kvbm_stage_source{ks[j], static_cast<uint32_t>(layers[j].src_layer_begin), static_cast<uint32_t>(layers[j].dst_layer_begin),
-                                  static_cast<uint32_t>(layers[j].layer_count)};
+      stage_sources(ks, layers, nw, ss);
       if (st)
         return checked(kvbm_kernels_paged_stage_repage_gather_streamed(ss, k, ups, &kd, dnh, upd, utb, ute, ilb, ile, row, o.cast_mode,
                                                                        o.cast_scales, st, stream),
@@ -1436,7 +1481,86 @@ static int execute_repage_gather(kvbm_transfer_manager* m, size_t num_srcs, cons
                                              o.done_flag, o.epoch, sl.host_flag, value, stream),
                    "kvbm_kernels_paged_repage");
   };
-  return launch_transform(m, e, nw, num_srcs, src_ids, n_src, dst_ids, n_dst, ls, o, stream, bytes, nullptr, out, launch);
+  return launch_transform(m, e, nw, num_srcs, src_ids, n_src, dst_ids, n_dst, ls, o, stream, repage_bytes(R, nw, layers, tb, te), nullptr, out,
+                          launch);
+}
+
+// A batch of sequences as one hand-off (kvbm_manager_execute_repage_batch): every sequence passes check_repage_request as the
+// staged re-paging gather it would be alone; then the concatenated tables are checked for a destination block named twice; then
+// one slot takes every table and the unit table in one copy, and one batch launch moves every sequence.
+static int execute_repage_batch(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, kvbm_layout_handle dst_h,
+                                const kvbm_repage_batch_seq* seqs, size_t num_seqs, const kvbm_head_window* windows,
+                                const kvbm_shard_window* layers, size_t nw, const kvbm_layer_stream* ls, const kvbm_transfer_options* opts_in,
+                                kvbm_notification* out)
+{
+  kvbm_transfer_options o{};
+  if (opts_in) o = *opts_in;
+  if (out) *out = 0;
+  int rc;
+  if ((rc = check_gather_windows(num_srcs, srcs, windows, nw, o, layers))) return rc;
+  if (num_seqs && !seqs) return fail(KVBM_ERR, "null sequence list");
+  std::lock_guard<std::mutex> lk(m->mu);
+  RepageRequest R, Ri;
+  bool any = false;
+  uint64_t bytes = 0;
+  std::vector<kvbm_repage_seq> ranges;
+  std::vector<std::vector<size_t>> cat(num_srcs + 1);  // each source's concatenated table, then the destination's
+  std::vector<bool> read(num_srcs, false);             // the sources some window reads: the others' tables may be null
+  for (size_t j = 0; j < nw; ++j) read[windows[j].src_rank] = true;
+  for (size_t i = 0; i < num_seqs; ++i) {
+    const kvbm_repage_batch_seq& q = seqs[i];
+    if ((rc = check_repage_request(m, num_srcs, srcs, q.src_ids, q.n_src, dst_h, q.dst_ids, q.n_dst, q.token_begin, q.token_end, windows, nw, o,
+                                   ls, true, layers, &Ri)))
+      return rc;
+    if (Ri.empty) continue;
+    R = Ri;
+    any = true;
+    bytes += repage_bytes(R, nw, layers, q.token_begin, q.token_end);
+    ranges.push_back(kvbm_repage_seq{static_cast<uint32_t>(q.token_begin), static_cast<uint32_t>(q.token_end)});
+    for (size_t r = 0; r < num_srcs; ++r)
+      if (read[r]) cat[r].insert(cat[r].end(), q.src_ids[r], q.src_ids[r] + q.n_src);
+    cat[num_srcs].insert(cat[num_srcs].end(), q.dst_ids, q.dst_ids + q.n_dst);
+  }
+  if (!any) return KVBM_OK;  // no sequences, only empty ranges or an empty layer range: nothing to move
+  const Transfer* e = R.e;
+  const Layout &S0 = *e[0].S, *D = R.D;
+  const std::vector<size_t>& cd = cat[num_srcs];
+  for (size_t j = 0; j < nw; ++j) {  // the destination's uniqueness once; a source in the destination's layout also against it
+    const size_t r = windows[j].src_rank;
+    const bool same = srcs[r] == dst_h;
+    if ((j == 0 || same) &&
+        (rc = check_block_ids(cat[r].data(), cat[r].size(), cd.data(), cd.size(), e[j].S->cfg.num_blocks, D->cfg.num_blocks, same)))
+      return rc;
+  }
+  const uint32_t ups = static_cast<uint32_t>(S0.cfg.page_size), upd = static_cast<uint32_t>(D->cfg.page_size);
+  size_t num_units = 0, n_src = 0, n_dst = 0;
+  if (kvbm_kernels_repage_batch_units(ranges.data(), ranges.size(), ups, upd, nullptr, 0, &num_units, &n_src, &n_dst))
+    return fail(KVBM_ERR, "the batch's token ranges and page sizes have no unit table");
+  std::vector<kvbm_repage_unit> units(num_units);
+  kvbm_kernels_repage_batch_units(ranges.data(), ranges.size(), ups, upd, units.data(), units.size(), &num_units, &n_src, &n_dst);
+  std::vector<const size_t*> lists(num_srcs);
+  for (size_t r = 0; r < num_srcs; ++r) lists[r] = read[r] ? cat[r].data() : nullptr;
+
+  DeviceGuard g(m->device);
+  const cudaStream_t stream = pick_stream(m, e[0].plan.first, o);
+  const uint32_t row = static_cast<uint32_t>(S0.cfg.inner_dim / S0.cfg.num_heads * S0.cfg.dtype_width_bytes);
+  const uint32_t dnh = static_cast<uint32_t>(D->cfg.num_heads);
+  const int ilb = static_cast<int>(R.lb), ile = static_cast<int>(R.le), k = static_cast<int>(nw);
+  auto launch = [&](const kvbm_permute_source* ks, const kvbm_permute_side& kd, const kvbm_permute_stream* st, const Slot& sl, uint64_t seq) {
+    const auto* du = reinterpret_cast<const kvbm_repage_unit*>(sl.dev_ids + units_at(num_srcs * n_src + n_dst));
+    kvbm_stage_source ss[KVBM_GATHER_MAX_SOURCES] = {};
+    stage_sources(ks, layers, nw, ss);
+    if (st)
+      return checked(kvbm_kernels_paged_stage_repage_gather_batch_streamed(ss, k, ups, &kd, dnh, upd, ranges.data(), ranges.size(), du, num_units,
+                                                                           ilb, ile, row, o.cast_mode, o.cast_scales, st, stream),
+                     "kvbm_kernels_paged_stage_repage_gather_batch_streamed");
+    return checked(kvbm_kernels_paged_stage_repage_gather_batch(ss, k, ups, &kd, dnh, upd, ranges.data(), ranges.size(), du, num_units, ilb, ile,
+                                                                row, o.cast_mode, o.cast_scales, o.done_flag, o.epoch, sl.host_flag,
+                                                                static_cast<uint32_t>(seq), stream),
+                   "kvbm_kernels_paged_stage_repage_gather_batch");
+  };
+  return launch_transform(m, e, nw, num_srcs, lists.data(), n_src, cd.data(), n_dst, ls, o, stream, bytes, nullptr, out, launch, units.data(),
+                          num_units);
 }
 
 }  // namespace kvbm_host
@@ -2066,6 +2190,23 @@ extern "C" int kvbm_manager_execute_stage_repage_gather(kvbm_transfer_manager* m
     hw[j] = kvbm_head_window{windows[j].src_rank, windows[j].src_head_begin, windows[j].dst_head_begin, windows[j].head_count};
   return execute_repage_gather(m, num_srcs, srcs, src_ids, n_src, dst, dst_ids, n_dst, token_begin, token_end, windows ? hw.data() : nullptr,
                                num_windows, opts, out, ls, /*gather=*/true, windows);
+  });
+}
+
+extern "C" int kvbm_manager_execute_repage_batch(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs,
+                                                 kvbm_layout_handle dst, const kvbm_repage_batch_seq* seqs, size_t num_seqs,
+                                                 const kvbm_shard_window* windows, size_t num_windows, const kvbm_layer_stream* ls,
+                                                 const kvbm_transfer_options* opts, kvbm_notification* out)
+{
+  return guarded([&]() -> int {
+  if (!m) return fail(KVBM_ERR, "null manager");
+  if (out) *out = 0;
+  if (ls)
+    if (int rc = check_layer_stream_shape(ls, num_srcs)) return rc;
+  std::vector<kvbm_head_window> hw(windows ? num_windows : 0);
+  for (size_t j = 0; j < hw.size(); ++j)
+    hw[j] = kvbm_head_window{windows[j].src_rank, windows[j].src_head_begin, windows[j].dst_head_begin, windows[j].head_count};
+  return execute_repage_batch(m, num_srcs, srcs, dst, seqs, num_seqs, windows ? hw.data() : nullptr, windows, num_windows, ls, opts, out);
   });
 }
 

@@ -737,6 +737,15 @@ __device__ __forceinline__ RepageUnit repage_unit(const RepageGeom& G, uint32_t 
   return {t0 - first, t1 - t0, (G.big_first + j) * G.ratio - G.small_first};
 }
 
+// A batch of sequences (kvbm_repage_unit): the same three words of big block j, loaded from the batch's unit table, whose
+// small_k indexes the concatenated small table.  One 16 B load where a search over per-sequence prefix sums would be log2(n)
+// dependent loads at the head of a CTA that lives a few microseconds.
+__device__ __forceinline__ RepageUnit batch_unit(const kvbm_repage_unit* units, uint32_t j)
+{
+  const uint4 w = __ldg(reinterpret_cast<const uint4*>(units) + j);
+  return {w.x, w.y, w.z};
+}
+
 // One head of a re-paging unit: its run of `run` 16 B vectors from slot q0 of the big block on.  bh: the head's rows in the
 // big block; sh: its rows in the small side's (layer, outer) region, before the block offset.  Small block b of the unit is
 // entry small_k + b of small_ids (RepageUnit).  Every re-paging kernel runs its heads through this loop.
@@ -822,9 +831,10 @@ struct RepageGatherParams {
 
 // Unit (big block j, destination layer l, outer o) of the re-paging gather: the warp of map entry k of l's stage T reads its source
 // s at the source's own layer l + shift[s].  SCALED: one scale array for every source, scales[l * no + o] by the destination layer.
-template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+// TABLE: a batch of sequences, whose unit comes from `units` (batch_unit) instead of the launch's one token range.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2, bool TABLE = false>
 __device__ __forceinline__ void repage_gather_unit(const RepageGatherParams& P, const GatherStage& T, uint32_t j, uint32_t l, uint32_t o,
-                                                   const RowSplit& r, const float* scales)
+                                                   const RowSplit& r, const float* scales, const kvbm_repage_unit* units = nullptr)
 {
   constexpr int IN = CAST == KVBM_CAST_BF16_TO_FP8E4M3 ? 2 : 1;
   constexpr int OUT = CAST == KVBM_CAST_FP8E4M3_TO_BF16 ? 2 : 1;
@@ -832,7 +842,11 @@ __device__ __forceinline__ void repage_gather_unit(const RepageGatherParams& P, 
   const RepageGeom& G = P.geo;
   const uint32_t first = T.first, end = T.first + T.count;
   const PermuteSide& D = g.D;
-  const RepageUnit u = repage_unit(G, j);
+  RepageUnit u;
+  if constexpr (TABLE)
+    u = batch_unit(units, j);
+  else
+    u = repage_unit(G, j);
   const uint8_t* d_region = side_region(D, l, o);
   const ptx::Scale scale = ptx::make_scale(SCALED ? __ldg(scales + l * G.no + o) : 1.f);
   const uint32_t big_shift = G.src_small ? 3 + OUT : 3 + IN, small_shift = G.src_small ? 3 + IN : 3 + OUT;
@@ -864,6 +878,20 @@ kvbm_paged_repage_gather_kernel(const __grid_constant__ RepageGatherParams P, Ro
   const uint32_t rem = unit - j * (G.nlayers * G.no);
   const uint32_t l = G.layer_begin + rem / G.no;
   repage_gather_unit<CAST, POW2, SCALED, PPOW2>(P, stage_of(P.g, l), j, l, rem % G.no, r, scales);
+}
+
+// kvbm_paged_repage_gather_kernel over a batch of sequences: big block j is entry j of the concatenated big table and record j
+// of `units`; geo's token range and first blocks are unused.  The same bound: three CTAs per SM.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__global__ void __launch_bounds__(256, 3)
+kvbm_paged_batch_repage_gather_kernel(const __grid_constant__ RepageGatherParams P, const kvbm_repage_unit* units, RowSplit r, const float* scales)
+{
+  const RepageGeom& G = P.geo;
+  const uint32_t unit = blockIdx.x;  // (big block j * nlayers + l) * no + o
+  const uint32_t j = unit / (G.nlayers * G.no);
+  const uint32_t rem = unit - j * (G.nlayers * G.no);
+  const uint32_t l = G.layer_begin + rem / G.no;
+  repage_gather_unit<CAST, POW2, SCALED, PPOW2, true>(P, stage_of(P.g, l), j, l, rem % G.no, r, scales, units);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -976,6 +1004,22 @@ kvbm_gated_repage_gather_kernel(const __grid_constant__ RepageGatherParams P, co
     const uint32_t rem = u - (l - G.layer_begin) * per_layer;
     const uint32_t j = rem / G.no;
     repage_gather_unit<CAST, POW2, SCALED, PPOW2>(P, T, j, l, rem - j * G.no, r, scales);
+  });
+}
+
+// kvbm_gated_repage_gather_kernel over a batch of sequences (num_big: the length of `units`): layer l is done once it landed for
+// every sequence.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__global__ void __launch_bounds__(256)
+kvbm_gated_batch_repage_gather_kernel(const __grid_constant__ RepageGatherParams P, const __grid_constant__ GateArgs A,
+                                      const kvbm_repage_unit* units, uint32_t num_big, RowSplit r, const float* scales, uint32_t batch)
+{
+  const RepageGeom& G = P.geo;
+  const uint32_t per_layer = num_big * G.no;
+  gated_units(A, P.g, per_layer * G.nlayers, batch, [&](uint32_t u) { return G.layer_begin + u / per_layer; }, [&](uint32_t u, uint32_t l, const GatherStage& T) {
+    const uint32_t rem = u - (l - G.layer_begin) * per_layer;
+    const uint32_t j = rem / G.no;
+    repage_gather_unit<CAST, POW2, SCALED, PPOW2, true>(P, T, j, l, rem - j * G.no, r, scales, units);
   });
 }
 
@@ -1157,6 +1201,10 @@ static cudaError_t preload_kernels()
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_gather_kernel<c, p, sc>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_gather_kernel<c, p, sc, true>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_gather_kernel<c, p, sc, false>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_batch_repage_gather_kernel<c, p, sc, true>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_batch_repage_gather_kernel<c, p, sc, false>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_batch_repage_gather_kernel<c, p, sc, true>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_batch_repage_gather_kernel<c, p, sc, false>);
         });
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_layer_signal_kernel);
   return e;
@@ -1506,30 +1554,23 @@ static cudaError_t launch_paged_permute(const kvbm_stage_source* srcs, int num_s
   return launched(stream, done_flag, epoch, completion_flag, completion_value);
 }
 
-// The geometry every re-paging launch shares, and its checks: non-zero pages, one dividing the other, slot arithmetic in 32 bits
-// (every block of the larger page in the range ends below 2^32, and the page split is exact for q < big_page), the cast's rows
-// and the row split of the larger page, and fewer than 2^31 units.  Fills everything of *G but nh, the walk's row split, the
-// destination's row, the unit count and whether the small page is a power of two.
-static bool repage_geometry(uint32_t src_page, uint32_t dst_page, uint32_t token_begin, uint32_t token_end, int layer_begin, int layer_end,
-                            uint32_t no, uint32_t src_row_bytes, int cast_mode, RepageGeom* G, RowSplit* r, uint64_t* dst_row_bytes,
-                            uint64_t* units, bool* page_pow2)
+// What every re-paging launch derives from its two pages, and their checks: non-zero pages, one dividing the other, the page
+// split exact for q < big_page, the cast's rows and the row split of the larger page.  Fills everything of *G but the token
+// range's fields and nh, the walk's row split, the destination's row and whether the small page is a power of two.
+static bool repage_pages(uint32_t src_page, uint32_t dst_page, int layer_begin, int layer_end, uint32_t no, uint32_t src_row_bytes,
+                         int cast_mode, RepageGeom* G, RowSplit* r, uint64_t* dst_row_bytes, bool* page_pow2)
 {
   if (src_page == 0 || dst_page == 0) return false;
   const bool src_small = src_page < dst_page;
   const uint32_t big_page = src_small ? dst_page : src_page, small_page = src_small ? src_page : dst_page;
   if (big_page % small_page) return false;
-  const uint64_t big_end = (static_cast<uint64_t>(token_end) + big_page - 1) / big_page * big_page;
-  if (big_end >= (1ull << 32) || static_cast<uint64_t>(big_page) * small_page >= (1ull << 32)) return false;
+  if (static_cast<uint64_t>(big_page) * small_page >= (1ull << 32)) return false;
   uint64_t walk_row;
   if (!cast_rows(src_row_bytes, cast_mode, dst_row_bytes, &walk_row) || !row_split(walk_row, big_page, r)) return false;
   RepageGeom g{};
   g.small_page = small_page;
   g.big_page = big_page;
   g.ratio = big_page / small_page;
-  g.big_first = token_begin / big_page;
-  g.small_first = token_begin / small_page;
-  g.token_begin = token_begin;
-  g.token_end = token_end;
   g.layer_begin = static_cast<uint32_t>(layer_begin);
   g.nlayers = static_cast<uint32_t>(layer_end - layer_begin);
   g.no = no;
@@ -1542,27 +1583,64 @@ static bool repage_geometry(uint32_t src_page, uint32_t dst_page, uint32_t token
   } else {
     g.page = {small_page, static_cast<uint32_t>(((1ull << 32) + small_page - 1) / small_page), false};
   }
-  *units = (static_cast<uint64_t>(big_end / big_page) - g.big_first) * g.nlayers * no;
+  *G = g;
+  return true;
+}
+
+// repage_pages plus one token range: slot arithmetic in 32 bits (every block of the larger page in the range ends below 2^32)
+// and fewer than 2^31 units.  Fills the range's fields of *G and the unit count.
+static bool repage_geometry(uint32_t src_page, uint32_t dst_page, uint32_t token_begin, uint32_t token_end, int layer_begin, int layer_end,
+                            uint32_t no, uint32_t src_row_bytes, int cast_mode, RepageGeom* G, RowSplit* r, uint64_t* dst_row_bytes,
+                            uint64_t* units, bool* page_pow2)
+{
+  RepageGeom g;
+  if (!repage_pages(src_page, dst_page, layer_begin, layer_end, no, src_row_bytes, cast_mode, &g, r, dst_row_bytes, page_pow2)) return false;
+  const uint64_t big_end = (static_cast<uint64_t>(token_end) + g.big_page - 1) / g.big_page * g.big_page;
+  if (big_end >= (1ull << 32)) return false;
+  g.big_first = token_begin / g.big_page;
+  g.small_first = token_begin / g.small_page;
+  g.token_begin = token_begin;
+  g.token_end = token_end;
+  *units = (static_cast<uint64_t>(big_end / g.big_page) - g.big_first) * g.nlayers * no;
   if (*units >= (1ull << 31)) return false;
   *G = g;
   return true;
 }
+
+// A batch of sequences of a re-paging launch: the caller's ranges (host) and unit table (device-accessible).
+struct RepageBatch {
+  const kvbm_repage_seq* seqs;
+  size_t num_seqs;
+  const kvbm_repage_unit* units;
+  size_t num_units;
+};
 
 // Every re-paging launch: a plain re-page is one source whose window covers every head and every layer of both sides, a
 // re-paging gather one or more windows.  Runs the checks of launch_paged_permute's sources and of repage_geometry's pages, each
 // side's region at its own page and head count, all before any CUDA call; signals when there is nothing to move; then launches
 // kvbm_paged_repage_kernel for a plain re-page, else kvbm_paged_repage_gather_kernel, and the signal.  max_covered and st: as
 // launch_paged_permute's (st takes the gated re-paging gather kernel, or per layer this launch unstreamed).
+// B: a batch of sequences in place of the one token range (token_begin / token_end unused).  Its ranges and pages are checked
+// through kvbm_kernels_repage_batch_units, whose unit count must be the caller's; it always takes the batch gather kernels.
 static cudaError_t launch_paged_repage_gather(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page, const kvbm_permute_side* dst,
                                               uint32_t dst_num_heads, uint32_t dst_page, uint32_t token_begin, uint32_t token_end,
                                               int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
                                               uint32_t* done_flag, uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value,
-                                              uint32_t max_covered, cudaStream_t stream, const kvbm_permute_stream* st = nullptr)
+                                              uint32_t max_covered, cudaStream_t stream, const kvbm_permute_stream* st = nullptr,
+                                              const RepageBatch* B = nullptr)
 {
-  if (layer_begin < 0 || layer_end < layer_begin || token_end < token_begin) return cudaErrorInvalidValue;
+  if (layer_begin < 0 || layer_end < layer_begin || (!B && token_end < token_begin)) return cudaErrorInvalidValue;
   if (!cast_args_ok(cast_mode, cast_scales)) return cudaErrorInvalidValue;
   if (!srcs || num_srcs < 1 || num_srcs > KVBM_GATHER_MAX_SOURCES) return cudaErrorInvalidValue;
-  if (token_end == token_begin || layer_end == layer_begin) return signal_launch(done_flag, epoch, completion_flag, completion_value, stream);
+  size_t num_big = 0;
+  if (B) {
+    size_t src_ids, dst_ids;
+    if (kvbm_kernels_repage_batch_units(B->seqs, B->num_seqs, src_page, dst_page, nullptr, 0, &num_big, &src_ids, &dst_ids) != 0)
+      return cudaErrorInvalidValue;
+    if (num_big != B->num_units || (num_big != 0 && !B->units)) return cudaErrorInvalidValue;
+  }
+  if ((B ? num_big == 0 : token_end == token_begin) || layer_end == layer_begin)
+    return signal_launch(done_flag, epoch, completion_flag, completion_value, stream);
   if (!dst || !dst->block_ids || !dst->layout.layer_base) return cudaErrorInvalidValue;
   const uint32_t nl = dst->layout.num_layers, no = dst->layout.outer_dim;
   if (nl == 0 || no == 0 || static_cast<uint32_t>(layer_end) > nl) return cudaErrorInvalidValue;
@@ -1570,9 +1648,15 @@ static cudaError_t launch_paged_repage_gather(const kvbm_stage_source* srcs, int
   RowSplit r;
   uint64_t dst_row_bytes, units;
   bool page_pow2;
-  if (!repage_geometry(src_page, dst_page, token_begin, token_end, layer_begin, layer_end, no, src_row_bytes, cast_mode, &P.geo, &r,
-                       &dst_row_bytes, &units, &page_pow2))
+  if (B) {
+    if (!repage_pages(src_page, dst_page, layer_begin, layer_end, no, src_row_bytes, cast_mode, &P.geo, &r, &dst_row_bytes, &page_pow2))
+      return cudaErrorInvalidValue;
+    if (num_big >= (1ull << 31) || (units = static_cast<uint64_t>(num_big) * P.geo.nlayers) >= (1ull << 31) || (units *= no) >= (1ull << 31))
+      return cudaErrorInvalidValue;
+  } else if (!repage_geometry(src_page, dst_page, token_begin, token_end, layer_begin, layer_end, no, src_row_bytes, cast_mode, &P.geo, &r,
+                              &dst_row_bytes, &units, &page_pow2)) {
     return cudaErrorInvalidValue;
+  }
   if (static_cast<uint64_t>(dst_page) * dst_num_heads * dst_row_bytes != dst->layout.region_bytes) return cudaErrorInvalidValue;
   if (!fill_permute_side(*dst, nl, no, dst_num_heads, dst_page, static_cast<uint32_t>(dst_row_bytes), &P.g.D)) return cudaErrorInvalidValue;
   uint32_t widest;
@@ -1586,26 +1670,34 @@ static cudaError_t launch_paged_repage_gather(const kvbm_stage_source* srcs, int
         *st, P.g, num_srcs, nl, layer_begin, layer_end, units, stream,
         [&](int l) {
           return launch_paged_repage_gather(srcs, num_srcs, src_page, dst, dst_num_heads, dst_page, token_begin, token_end, l, l + 1,
-                                            src_row_bytes, cast_mode, cast_scales, nullptr, 0, nullptr, 0, max_covered, stream);
+                                            src_row_bytes, cast_mode, cast_scales, nullptr, 0, nullptr, 0, max_covered, stream, nullptr, B);
         },
         [&](const GateArgs& A, unsigned ctas, uint32_t batch) {
-          const uint32_t num_big = static_cast<uint32_t>(units / (static_cast<uint64_t>(P.geo.nlayers) * no));
+          const uint32_t nb = static_cast<uint32_t>(units / (static_cast<uint64_t>(P.geo.nlayers) * no));
           with_walk_kernel(cast_mode, r.pow2, cast_scales != nullptr, [&](auto c, auto p, auto sc) {
-            if (page_pow2)
-              kvbm_gated_repage_gather_kernel<c, p, sc, true><<<ctas, threads, 0, stream>>>(P, A, num_big, r, cast_scales, batch);
+            if (B && page_pow2)
+              kvbm_gated_batch_repage_gather_kernel<c, p, sc, true><<<ctas, threads, 0, stream>>>(P, A, B->units, nb, r, cast_scales, batch);
+            else if (B)
+              kvbm_gated_batch_repage_gather_kernel<c, p, sc, false><<<ctas, threads, 0, stream>>>(P, A, B->units, nb, r, cast_scales, batch);
+            else if (page_pow2)
+              kvbm_gated_repage_gather_kernel<c, p, sc, true><<<ctas, threads, 0, stream>>>(P, A, nb, r, cast_scales, batch);
             else
-              kvbm_gated_repage_gather_kernel<c, p, sc, false><<<ctas, threads, 0, stream>>>(P, A, num_big, r, cast_scales, batch);
+              kvbm_gated_repage_gather_kernel<c, p, sc, false><<<ctas, threads, 0, stream>>>(P, A, nb, r, cast_scales, batch);
           });
         });
   // a window over every layer and every head of both sides (the checks above make its starts 0)
   const kvbm_permute_source& X = srcs[0].src;
-  const bool plain = num_srcs == 1 && whole_layers(srcs[0], nl) && X.head_count == X.num_heads && X.head_count == dst_num_heads;
+  const bool plain = !B && num_srcs == 1 && whole_layers(srcs[0], nl) && X.head_count == X.num_heads && X.head_count == dst_num_heads;
   RepageParams R{};
   R.big = P.geo.src_small ? P.g.D : P.g.src[0].S;
   R.small = P.geo.src_small ? P.g.src[0].S : P.g.D;
   R.g = P.geo;
   with_walk_kernel(cast_mode, r.pow2, cast_scales != nullptr, [&](auto c, auto p, auto sc) {
-    if (plain && page_pow2)
+    if (B && page_pow2)
+      kvbm_paged_batch_repage_gather_kernel<c, p, sc, true><<<grid, threads, 0, stream>>>(P, B->units, r, cast_scales);
+    else if (B)
+      kvbm_paged_batch_repage_gather_kernel<c, p, sc, false><<<grid, threads, 0, stream>>>(P, B->units, r, cast_scales);
+    else if (plain && page_pow2)
       kvbm_paged_repage_kernel<c, p, sc, true><<<grid, threads, 0, stream>>>(R, r, cast_scales);
     else if (plain)
       kvbm_paged_repage_kernel<c, p, sc, false><<<grid, threads, 0, stream>>>(R, r, cast_scales);
@@ -1866,6 +1958,69 @@ kvbm_kernels_paged_stage_repage_gather_streamed(const kvbm_stage_source* srcs, i
   return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, token_begin, token_end, layer_begin,
                                     layer_end, src_row_bytes, cast_mode, cast_scales, st->done_flag, st->epoch, st->completion_flag,
                                     st->completion_value, KVBM_GATHER_MAX_HEADS, stream, st);
+}
+
+extern "C" int
+kvbm_kernels_repage_batch_units(const kvbm_repage_seq* seqs, size_t num_seqs, uint32_t src_page_size, uint32_t dst_page_size,
+                                kvbm_repage_unit* out, size_t cap, size_t* num_units, size_t* src_ids, size_t* dst_ids)
+{
+  if ((num_seqs && !seqs) || (cap && !out) || !num_units || !src_ids || !dst_ids) return 1;
+  if (src_page_size == 0 || dst_page_size == 0) return 1;
+  const bool src_small = src_page_size < dst_page_size;
+  const uint64_t big = src_small ? dst_page_size : src_page_size, small = src_small ? src_page_size : dst_page_size;
+  if (big % small || big * small >= (1ull << 32)) return 1;
+  for (size_t i = 0; i < num_seqs; ++i) {
+    if (seqs[i].token_end < seqs[i].token_begin) return 1;
+    if (seqs[i].token_end != seqs[i].token_begin && (seqs[i].token_end + big - 1) / big * big >= (1ull << 32)) return 1;
+  }
+  const uint64_t ratio = big / small;
+  size_t nb = 0, ns = 0;
+  for (size_t i = 0; i < num_seqs; ++i) {
+    const uint64_t tb = seqs[i].token_begin, te = seqs[i].token_end;
+    if (tb == te) continue;
+    const uint64_t big_first = tb / big, big_end = (te + big - 1) / big, small_first = tb / small, small_end = (te + small - 1) / small;
+    uint64_t j = big_first;
+    for (; j < big_end && nb < cap; ++j, ++nb) {
+      const uint64_t first = j * big, t0 = std::max(tb, first), t1 = std::min(te, first + big);
+      // the concatenated small table's entry of the block's first small block: below 0 (wrapping) when it lies before the range
+      out[nb] = kvbm_repage_unit{static_cast<uint32_t>(t0 - first), static_cast<uint32_t>(t1 - t0),
+                                 static_cast<uint32_t>(ns + j * ratio - small_first), static_cast<uint32_t>(i)};
+    }
+    nb += static_cast<size_t>(big_end - j);  // past the capacity: counted, not written
+    ns += static_cast<size_t>(small_end - small_first);
+  }
+  *num_units = nb;
+  *src_ids = src_small ? ns : nb;
+  *dst_ids = src_small ? nb : ns;
+  return 0;
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_stage_repage_gather_batch(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page_size, const kvbm_permute_side* dst,
+                                             uint32_t dst_num_heads, uint32_t dst_page_size, const kvbm_repage_seq* seqs, size_t num_seqs,
+                                             const kvbm_repage_unit* units, size_t num_units, int layer_begin, int layer_end,
+                                             uint32_t src_row_bytes, int cast_mode, const float* cast_scales, uint32_t* done_flag,
+                                             uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
+{
+  const RepageBatch B{seqs, num_seqs, units, num_units};
+  return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, 0, 0, layer_begin, layer_end,
+                                    src_row_bytes, cast_mode, cast_scales, done_flag, epoch, completion_flag, completion_value,
+                                    KVBM_GATHER_MAX_HEADS, stream, nullptr, &B);
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_stage_repage_gather_batch_streamed(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page_size,
+                                                      const kvbm_permute_side* dst, uint32_t dst_num_heads, uint32_t dst_page_size,
+                                                      const kvbm_repage_seq* seqs, size_t num_seqs, const kvbm_repage_unit* units,
+                                                      size_t num_units, int layer_begin, int layer_end, uint32_t src_row_bytes,
+                                                      int cast_mode, const float* cast_scales, const kvbm_permute_stream* st,
+                                                      cudaStream_t stream)
+{
+  if (!stream_args_ok(st, num_srcs)) return cudaErrorInvalidValue;
+  const RepageBatch B{seqs, num_seqs, units, num_units};
+  return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, 0, 0, layer_begin, layer_end,
+                                    src_row_bytes, cast_mode, cast_scales, st->done_flag, st->epoch, st->completion_flag,
+                                    st->completion_value, KVBM_GATHER_MAX_HEADS, stream, st, &B);
 }
 
 extern "C" cudaError_t

@@ -13,7 +13,7 @@ from __future__ import annotations
 
 import ctypes as C
 import enum
-from typing import Optional, Sequence
+from typing import Optional, Sequence, Tuple
 
 from . import _lib
 
@@ -108,6 +108,16 @@ class StageSource(C.Structure):
     """struct kvbm_stage_source: one source of `paged_stage_gather` (a gather source whose side has the pool's own num_layers,
     and its layer window: source layers [src_layer_begin, +layer_count) land as destination layers [dst_layer_begin, +layer_count))"""
     _fields_ = [("src", PermuteSource), ("src_layer_begin", C.c_uint32), ("dst_layer_begin", C.c_uint32), ("layer_count", C.c_uint32)]
+
+
+class RepageSeq(C.Structure):
+    """struct kvbm_repage_seq: one sequence's token range in a batch (host memory)"""
+    _fields_ = [("token_begin", C.c_uint32), ("token_end", C.c_uint32)]
+
+
+class RepageUnit(C.Structure):
+    """struct kvbm_repage_unit: one block of the larger-page side of a batch, 16 B (`repage_batch_units` writes them)"""
+    _fields_ = [("q0", C.c_uint32), ("tokens", C.c_uint32), ("small_k", C.c_uint32), ("seq", C.c_uint32)]
 
 
 GATHER_MAX_SOURCES = 16      # KVBM_GATHER_MAX_SOURCES
@@ -227,6 +237,16 @@ def lib() -> C.CDLL:
                                                                       C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, i, i, C.c_uint32, i,
                                                                       vp, C.POINTER(PermuteStream), vp]
         L.kvbm_kernels_paged_stage_repage_gather_streamed.restype = i
+        L.kvbm_kernels_repage_batch_units.argtypes = [vp, sz, C.c_uint32, C.c_uint32, vp, sz, C.POINTER(sz), C.POINTER(sz), C.POINTER(sz)]
+        L.kvbm_kernels_repage_batch_units.restype = i
+        L.kvbm_kernels_paged_stage_repage_gather_batch.argtypes = [C.POINTER(StageSource), i, C.c_uint32, C.POINTER(PermuteSide), C.c_uint32,
+                                                                   C.c_uint32, vp, sz, vp, sz, i, i, C.c_uint32, i, vp, vp, C.c_uint32, vp,
+                                                                   C.c_uint32, vp]
+        L.kvbm_kernels_paged_stage_repage_gather_batch.restype = i
+        L.kvbm_kernels_paged_stage_repage_gather_batch_streamed.argtypes = [C.POINTER(StageSource), i, C.c_uint32, C.POINTER(PermuteSide),
+                                                                            C.c_uint32, C.c_uint32, vp, sz, vp, sz, i, i, C.c_uint32, i, vp,
+                                                                            C.POINTER(PermuteStream), vp]
+        L.kvbm_kernels_paged_stage_repage_gather_batch_streamed.restype = i
         L.kvbm_kernels_permute_strides.argtypes = [i, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64, C.c_uint64,
                                                    C.POINTER(C.c_uint64)]
         L.kvbm_kernels_permute_strides.restype = i
@@ -253,6 +273,8 @@ EXPORTED_SYMBOLS = [
     "kvbm_kernels_paged_repage", "kvbm_kernels_paged_repage_gather", "kvbm_kernels_paged_permute_gather_streamed",
     "kvbm_kernels_paged_repage_gather_streamed", "kvbm_kernels_paged_stage_gather", "kvbm_kernels_paged_stage_gather_streamed",
     "kvbm_kernels_paged_stage_repage_gather", "kvbm_kernels_paged_stage_repage_gather_streamed",
+    "kvbm_kernels_repage_batch_units", "kvbm_kernels_paged_stage_repage_gather_batch",
+    "kvbm_kernels_paged_stage_repage_gather_batch_streamed",
 ]
 
 
@@ -477,6 +499,56 @@ def paged_stage_repage_gather_streamed(srcs: Sequence[StageSource], src_page_siz
                                                                  token_begin, token_end, layer_begin, layer_end, src_row_bytes,
                                                                  int(cast_mode), scales_ptr(cast_scales),
                                                                  C.byref(st) if st is not None else None, stream)
+
+
+def _repage_seqs(seqs: Sequence[Tuple[int, int]]):
+    return (RepageSeq * max(1, len(seqs)))(*[RepageSeq(int(b), int(e)) for b, e in seqs])
+
+
+def repage_batch_units(seqs: Sequence[Tuple[int, int]], src_page_size: int, dst_page_size: int):
+    """Host-only: the unit table of a batch of (token_begin, token_end) ranges as a numpy uint32 array [num_units, 4] (q0, tokens,
+    small_k, seq) and the lengths of each source's and the destination's concatenated block table; None when the pages or a range
+    break a rule.  include/kvbm_kernels.h (kvbm_kernels_repage_batch_units)."""
+    import numpy as np
+    arr = _repage_seqs(seqs)
+    n, ns, nd = C.c_size_t(), C.c_size_t(), C.c_size_t()
+    call = lib().kvbm_kernels_repage_batch_units
+    if call(C.cast(arr, C.c_void_p), len(seqs), src_page_size, dst_page_size, None, 0, C.byref(n), C.byref(ns), C.byref(nd)):
+        return None
+    out = np.zeros((n.value, 4), dtype=np.uint32)
+    if call(C.cast(arr, C.c_void_p), len(seqs), src_page_size, dst_page_size, out.ctypes.data, n.value, C.byref(n), C.byref(ns), C.byref(nd)):
+        return None
+    return out, ns.value, nd.value
+
+
+def paged_stage_repage_gather_batch(srcs: Sequence[StageSource], src_page_size: int, dst: PermuteSide, dst_num_heads: int,
+                                    dst_page_size: int, seqs: Sequence[Tuple[int, int]], units: int, num_units: int, layer_begin: int,
+                                    layer_end: int, src_row_bytes: int, cast_mode: int = 0, cast_scales=None, done_flag: int = 0,
+                                    epoch: int = 0, completion_flag: int = 0, completion_value: int = 0, stream: int = 0) -> int:
+    """`paged_stage_repage_gather` over a batch of sequences in ONE launch with one signal: `seqs` are the (token_begin, token_end)
+    ranges, every side's block_ids the concatenation of the per-sequence tables, `units` the device address of the table
+    `repage_batch_units` made for the same ranges and pages.  Two sequences must not share a destination block.
+    include/kvbm_kernels.h (kvbm_kernels_paged_stage_repage_gather_batch)."""
+    arr = (StageSource * max(1, len(srcs)))(*srcs)
+    return lib().kvbm_kernels_paged_stage_repage_gather_batch(arr, len(srcs), src_page_size, C.byref(dst), dst_num_heads, dst_page_size,
+                                                              C.cast(_repage_seqs(seqs), C.c_void_p), len(seqs), units or None, num_units,
+                                                              layer_begin, layer_end, src_row_bytes, int(cast_mode),
+                                                              scales_ptr(cast_scales), done_flag or None, epoch, completion_flag or None,
+                                                              completion_value, stream)
+
+
+def paged_stage_repage_gather_batch_streamed(srcs: Sequence[StageSource], src_page_size: int, dst: PermuteSide, dst_num_heads: int,
+                                             dst_page_size: int, seqs: Sequence[Tuple[int, int]], units: int, num_units: int,
+                                             layer_begin: int, layer_end: int, src_row_bytes: int, cast_mode: int, cast_scales,
+                                             st: Optional[PermuteStream], stream: int = 0) -> int:
+    """`paged_stage_repage_gather_batch` streamed with `paged_stage_repage_gather_streamed`'s flags: one ready flag per (source,
+    layer) covers the batch.  include/kvbm_kernels.h (kvbm_kernels_paged_stage_repage_gather_batch_streamed)."""
+    arr = (StageSource * max(1, len(srcs)))(*srcs)
+    return lib().kvbm_kernels_paged_stage_repage_gather_batch_streamed(arr, len(srcs), src_page_size, C.byref(dst), dst_num_heads,
+                                                                       dst_page_size, C.cast(_repage_seqs(seqs), C.c_void_p), len(seqs),
+                                                                       units or None, num_units, layer_begin, layer_end, src_row_bytes,
+                                                                       int(cast_mode), scales_ptr(cast_scales),
+                                                                       C.byref(st) if st is not None else None, stream)
 
 
 def permute_strides(kv_layout: int, num_layers: int, outer_dim: int, num_heads: int, page_size: int, row_bytes: int,

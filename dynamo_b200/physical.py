@@ -123,6 +123,12 @@ class _CShardWindow(C.Structure):
                                           "dst_head_begin", "head_count")]
 
 
+class _CRepageBatchSeq(C.Structure):
+    """struct kvbm_repage_batch_seq"""
+    _fields_ = [("token_begin", C.c_size_t), ("token_end", C.c_size_t), ("src_ids", C.c_void_p), ("n_src", C.c_size_t),
+                ("dst_ids", C.c_void_p), ("n_dst", C.c_size_t)]
+
+
 class _CLayerStream(C.Structure):
     """struct kvbm_layer_stream"""
     _fields_ = [("src_layer_ready_flags", C.c_void_p), ("num_srcs", C.c_size_t), ("layer_done_flags", C.c_void_p)]
@@ -243,6 +249,7 @@ EXPORTED_SYMBOLS = [
     "kvbm_mc_group_destroy", "kvbm_tp_reshard_plan", "kvbm_manager_execute_gather", "kvbm_manager_execute_repage",
     "kvbm_manager_execute_repage_gather", "kvbm_manager_execute_gather_streamed", "kvbm_manager_execute_repage_gather_streamed",
     "kvbm_tp_pp_reshard_plan", "kvbm_manager_execute_stage_gather", "kvbm_manager_execute_stage_repage_gather",
+    "kvbm_manager_execute_repage_batch",
 ]
 
 
@@ -303,6 +310,8 @@ def lib() -> C.CDLL:
                                                         P(_COptions), P(u64)]
         L.kvbm_manager_execute_stage_repage_gather.argtypes = [vp, sz, P(u64), P(P(sz)), sz, u64, vp, sz, sz, sz, P(_CShardWindow), sz,
                                                                P(_CLayerStream), P(_COptions), P(u64)]
+        L.kvbm_manager_execute_repage_batch.argtypes = [vp, sz, P(u64), u64, P(_CRepageBatchSeq), sz, P(_CShardWindow), sz, P(_CLayerStream),
+                                                        P(_COptions), P(u64)]
         L.kvbm_notification_is_complete.argtypes = [vp, u64]
         L.kvbm_notification_wait.argtypes = [vp, u64, C.c_int64]
         L.kvbm_manager_bytes_moved.argtypes = [vp]
@@ -809,6 +818,45 @@ class TransferManager:
         _check(lib().kvbm_manager_execute_stage_repage_gather(self._h, len(ranks), hs, sp, n_src, dst, d, n_dst, tokens.start, tokens.stop,
                                                               ws, len(plan), C.byref(ls) if ls is not None else None, C.byref(o),
                                                               C.byref(tok)))
+        return TransferCompleteNotification(self, tok.value)
+
+    def execute_repage_batch(self, sources: Mapping[int, int], dst: int, seqs: Sequence[tuple], plan: Sequence, options: Optional[TransferOptions] = None,
+                             ready_flags: Optional[Mapping[int, int]] = None, layer_done_flags: int = 0,
+                             num_layers: Optional[int] = None) -> TransferCompleteNotification:
+        """A batch of sequences as ONE hand-off (kvbm_manager_execute_repage_batch): what a continuous-batching decode step admits at
+        once, each sequence with its own prefix-cache hit, length and block tables.  `sources` maps a source rank to its layout
+        handle; `seqs` is a list of (tokens, {src_rank: src_block_ids}, dst_block_ids), each what `execute_stage_repage_gather`
+        takes for one request; `plan` is a ShardWindow list, or a HeadWindow list (a PP1 plan) with `num_layers` the destination's
+        layer count.  One staged copy of every table, one launch, one notification, `options.done_flag` written once; with
+        `ready_flags`, `layer_done_flags[l]` is written once layer l of every sequence landed.  Two sequences may share source
+        blocks; a destination block may appear once in the whole batch.  The first rejected sequence raises what
+        `execute_stage_repage_gather` would raise for it."""
+        if plan and isinstance(plan[0], HeadWindow):
+            if num_layers is None:
+                raise ValueError("a HeadWindow plan needs num_layers, the destination's layer count")
+            plan = [ShardWindow(w.src_rank, 0, 0, num_layers, w.src_head_begin, w.dst_head_begin, w.head_count) for w in plan]
+        ranks = sorted({w.src_rank for w in plan})
+        hs = (C.c_uint64 * max(1, len(ranks)))(*[sources[r] for r in ranks])
+        ws = self._shard_windows(ranks, plan)
+        PP = C.POINTER(C.c_size_t)
+        keep, cs = [], (_CRepageBatchSeq * max(1, len(seqs)))()
+        for c, (tokens, src_ids, dst_ids) in zip(cs, seqs):
+            if tokens.step != 1:
+                raise ValueError("tokens must be a range with step 1")
+            n_src = len(src_ids[ranks[0]]) if ranks else 0
+            if any(len(src_ids[r]) != n_src for r in ranks):
+                raise KvbmError(ErrorCode.LENGTH_MISMATCH, "the sources' block id lists have different lengths")
+            arrays = [_size_array(src_ids[r])[0] for r in ranks]
+            d, n_dst = _size_array(dst_ids)
+            sp = (C.c_void_p * max(1, len(ranks)))(*[a.addr if type(a) is _NpView else C.addressof(a) for a in arrays])
+            keep += [arrays, d, sp]
+            c.token_begin, c.token_end, c.src_ids, c.n_src = tokens.start, tokens.stop, C.addressof(sp), n_src
+            c.dst_ids, c.n_dst = (d.addr if type(d) is _NpView else C.addressof(d)), n_dst
+        ls = self._layer_stream(ranks, ready_flags, layer_done_flags) if ready_flags is not None else None
+        tok = C.c_uint64()
+        o = (options or TransferOptions())._c()
+        _check(lib().kvbm_manager_execute_repage_batch(self._h, len(ranks), hs, dst, cs, len(seqs), ws, len(plan),
+                                                       C.byref(ls) if ls is not None else None, C.byref(o), C.byref(tok)))
         return TransferCompleteNotification(self, tok.value)
 
     def execute_fanout(self, src: int, dsts: Sequence[int], src_block_ids: Sequence[Sequence[int]],

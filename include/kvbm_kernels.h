@@ -453,6 +453,66 @@ cudaError_t kvbm_kernels_paged_stage_repage_gather_streamed(const kvbm_stage_sou
                                                             uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
                                                             const kvbm_permute_stream* st, cudaStream_t stream);
 
+/* ---- a batch of sequences in one re-paging launch ---------------------------------------------------------------------------
+ * A decode step admits many requests, each with its own prefix-cache hit (its own token_begin, often inside a block), length
+ * and block tables.  A batch moves them in ONE launch with one signal.  Sequence i is the range [token_begin, token_end) that
+ * kvbm_kernels_paged_stage_repage_gather takes, and every side's block table is the concatenation, in batch order, of the tables
+ * the single entry would take: sequence i contributes its table[token_begin / P .. ceil(token_end / P)) for the side's page P
+ * (nothing when its range is empty).  All sources share Ps, so every source's concatenated table has the same per-sequence
+ * offsets. */
+typedef struct kvbm_repage_seq {
+  uint32_t token_begin, token_end;
+} kvbm_repage_seq;
+
+/* One block of the larger-page side (the source's on a tie), in batch order; record j belongs to entry j of that side's
+ * concatenated table.  q0: the slot of the block's first token inside the sequence's range; tokens: how many of its tokens lie in
+ * the range; small_k: the entry of the smaller-page side's concatenated table that holds the block's first small block -- when
+ * those first small blocks lie before the range it wraps below 0 in uint32 and small_k + b wraps back for every small block b the
+ * range touches; seq: the sequence the block belongs to (not read by the kernels). */
+typedef struct kvbm_repage_unit {
+  uint32_t q0, tokens, small_k, seq;
+} kvbm_repage_unit;
+
+/* Host-only (no GPU): the unit table of a batch and the lengths of its concatenated tables.  Writes min(*num_units, cap) records
+ * to out (out may be NULL when cap is 0: a sizing call) and always the three counts: *num_units records, *src_ids / *dst_ids
+ * entries in each source's / the destination's concatenated table.  Returns non-zero, writing nothing, for a null seqs with
+ * num_seqs > 0, a page of 0, pages of which neither divides the other, big_page * small_page >= 2^32, a reversed range, or a
+ * sequence whose last block of the larger page ends at or past 2^32 tokens. */
+int kvbm_kernels_repage_batch_units(const kvbm_repage_seq* seqs, size_t num_seqs, uint32_t src_page_size, uint32_t dst_page_size,
+                                    kvbm_repage_unit* out, size_t cap, size_t* num_units, size_t* src_ids, size_t* dst_ids);
+
+/* kvbm_kernels_paged_stage_repage_gather over a batch: sources, stages, head windows, layer range, formats, cast and scales are
+ * the launch's, as there; the token ranges are `seqs` (host memory) and the tables are concatenated as above.  `units` is
+ * device-accessible memory holding what kvbm_kernels_repage_batch_units produced for the same seqs and pages; like the block
+ * ids it is the caller's memory, read by the kernel and not on the host, and must stay valid until the launch has run.
+ * cudaErrorInvalidValue, before any CUDA call, for: every rule of kvbm_kernels_paged_stage_repage_gather's sources, stages,
+ * windows, pages, rows, cast and strides; a null seqs with num_seqs > 0; any rule of kvbm_kernels_repage_batch_units; a
+ * num_units other than the helper's count; a null units with num_units > 0; num_units * layers * outer_dim of 2^31 or more.
+ * Two sequences may share SOURCE blocks (a shared prefix).  Two sequences must not share a DESTINATION block: the entry cannot
+ * read device ids, so this is the caller's rule.  A batch always runs the gather kernels, also for one full-window source.
+ * One signal for the batch: done_flag / completion_flag are written once, after every sequence's bytes landed; per-sequence
+ * completion words are not provided.  num_seqs == 0, only empty ranges, or an empty layer range move nothing and still
+ * signal.  A batch of one sequence writes exactly the bytes of kvbm_kernels_paged_stage_repage_gather with that range, and a
+ * batch of n the bytes of n such launches in any order. */
+cudaError_t kvbm_kernels_paged_stage_repage_gather_batch(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page_size,
+                                                         const kvbm_permute_side* dst, uint32_t dst_num_heads, uint32_t dst_page_size,
+                                                         const kvbm_repage_seq* seqs, size_t num_seqs, const kvbm_repage_unit* units,
+                                                         size_t num_units, int layer_begin, int layer_end, uint32_t src_row_bytes,
+                                                         int cast_mode, const float* cast_scales, uint32_t* done_flag, uint32_t epoch,
+                                                         uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream);
+
+/* The batch streamed with kvbm_kernels_paged_stage_repage_gather_streamed's flag conventions.  A prefill batch computes layer l
+ * for all its sequences together, so one ready flag per (source, layer) covers the batch, and layer_done_flags[l] is written once
+ * layer l of EVERY sequence landed.  The argument rules are the batch's plus the gate's; a batch that moves nothing waits for
+ * nothing, writes done_flag / completion_flag at once and no layer_done_flags. */
+cudaError_t kvbm_kernels_paged_stage_repage_gather_batch_streamed(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page_size,
+                                                                  const kvbm_permute_side* dst, uint32_t dst_num_heads,
+                                                                  uint32_t dst_page_size, const kvbm_repage_seq* seqs, size_t num_seqs,
+                                                                  const kvbm_repage_unit* units, size_t num_units, int layer_begin,
+                                                                  int layer_end, uint32_t src_row_bytes, int cast_mode,
+                                                                  const float* cast_scales, const kvbm_permute_stream* st,
+                                                                  cudaStream_t stream);
+
 /* Host-only (no GPU): the stride table kvbm_kernels_paged_permute walks with for one side.  out[0] = 1 when offsets count
  * from the block's first byte (universal formats) or 0 when they count from the (layer, outer) region's first byte; the
  * element (layer l, outer o, head h, token t) then sits at  [out[0] ? l * out[1] + o * out[2] : 0] + h * out[3] + t * out[4].

@@ -424,6 +424,33 @@ int kvbm_manager_execute_stage_repage_gather(kvbm_transfer_manager* m, size_t nu
                                              size_t num_windows, const kvbm_layer_stream* ls, const kvbm_transfer_options* opts,
                                              kvbm_notification* out);
 
+/* One sequence of kvbm_manager_execute_repage_batch: the arguments kvbm_manager_execute_stage_repage_gather takes per request. */
+typedef struct kvbm_repage_batch_seq {
+  size_t token_begin, token_end;
+  const size_t* const* src_ids; /* [num_srcs] lists of n_src ids: source s's table[token_begin / Ps .. ceil(token_end / Ps)) */
+  size_t n_src;
+  const size_t* dst_ids;        /* the destination's table[token_begin / Pd .. ceil(token_end / Pd)) */
+  size_t n_dst;
+} kvbm_repage_batch_seq;
+
+/* A batch of sequences as ONE hand-off (what a continuous-batching decode step admits, or a prefill batch finishes, at once):
+ * kvbm_manager_execute_stage_repage_gather for every sequence of seqs[], each with its own token range and block tables, under
+ * one plan, one set of options and, with ls, one set of layer flags -- one staged copy of every table and the batch's unit
+ * table, one kvbm_kernels_paged_stage_repage_gather_batch launch (its streamed form with ls), one notification, and
+ * options.done_flag written once, after every sequence's bytes landed.  A plan without layer windows (PP1) is windows whose
+ * layer window is the identity over every layer.  With ls, layer_done_flags[l] is written once layer l of every sequence
+ * landed.  Two sequences may share source blocks (a shared prefix); a destination block may appear once in the whole batch.
+ * Errors: with ls, its shape; then, sequence by sequence in batch order, every check of
+ * kvbm_manager_execute_stage_repage_gather with its code and text, so the first rejected sequence returns what the single call
+ * would have returned for it (a batch without sequences still has its windows checked); then the concatenated destination ids
+ * unique (KVBM_ERR_DUPLICATE_DST) and, where a source is the destination's layout, disjoint from its concatenated source ids
+ * (KVBM_ERR_OVERLAP).  A batch whose sequences or layer range are all empty returns KVBM_OK with nothing launched.  bytes_moved
+ * counts the sum of what the single calls would.  Per-sequence completion words are not provided. */
+int kvbm_manager_execute_repage_batch(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, kvbm_layout_handle dst,
+                                      const kvbm_repage_batch_seq* seqs, size_t num_seqs, const kvbm_shard_window* windows,
+                                      size_t num_windows, const kvbm_layer_stream* ls, const kvbm_transfer_options* opts,
+                                      kvbm_notification* out);
+
 /* Completion: the transfer's last warp writes a flag in pinned host memory (no cudaEventQuery polling). */
 int kvbm_notification_is_complete(kvbm_transfer_manager* m, kvbm_notification n);  /* 1 / 0 / <0 error */
 int kvbm_notification_wait(kvbm_transfer_manager* m, kvbm_notification n, int64_t timeout_us);
