@@ -753,57 +753,66 @@ static int launch_transform(kvbm_transfer_manager* m, const Transfer* e, size_t 
   return KVBM_OK;
 }
 
+// What a layout-transforming launch moves: `units` (blocks or tokens) x each window's layers inside [lb, le) (layers[j]'s layer
+// window, or every layer) x the outer dimension x its heads x `head_bytes`, a destination head's bytes per unit.
+static uint64_t transform_bytes(const Transfer* e, size_t nw, const kvbm_shard_window* layers, size_t lb, size_t le, uint64_t units,
+                                uint64_t head_bytes)
+{
+  uint64_t bytes = 0;
+  for (size_t j = 0; j < nw; ++j) {
+    size_t from = lb, to = le;
+    if (layers) {
+      from = std::max(from, layers[j].dst_layer_begin);
+      to = std::min(to, layers[j].dst_layer_begin + layers[j].layer_count);
+    }
+    if (to > from) bytes += units * (to - from) * e[0].D[0]->cfg.outer_dim * e[j].window.head_count * head_bytes;
+  }
+  return bytes;
+}
+
+// The kernel sources of a launch: window j's gather source with the layer window of layers[j], or without layers the identity
+// window over the destination's nl layers (an unstaged request, whose sources check_compat gave the destination's layer count).
+static void stage_sources(const kvbm_permute_source* ks, const kvbm_shard_window* layers, size_t nw, size_t nl, kvbm_stage_source* ss)
+{
+  for (size_t j = 0; j < nw; ++j)
+    ss[j] = layers ? kvbm_stage_source{ks[j], static_cast<uint32_t>(layers[j].src_layer_begin), static_cast<uint32_t>(layers[j].dst_layer_begin),
+                                       static_cast<uint32_t>(layers[j].layer_count)}
+                   : kvbm_stage_source{ks[j], 0, 0, static_cast<uint32_t>(nl)};
+}
+
 // The layout-transforming transfer: what select_transform_kernel's result would drive if the reference ran it inside
 // execute_transfer (it rejects the pair instead, transfer/mod.rs:128-147).  One permuting launch moves every entry's head window
 // from source e[j].window.src_rank into e[0].D over e[0]'s layer range, with the transfer's fp8 <-> bf16 cast fused in:
-// kvbm_kernels_paged_permute_heads for one window (any head count), kvbm_kernels_paged_permute_gather for several, and
-// kvbm_kernels_paged_permute_gather_streamed with ls (gated on every window's source flags).  Every source list and the
-// destination's hold n ids; the completion word is written by a trailing signal kernel.
-// layers: a staged gather, window j with the layer window of layers[j], one kvbm_kernels_paged_stage_gather launch (or its
-// streamed form with ls); each window's bytes count over its layers inside the layer range.
+// kvbm_kernels_paged_permute_heads_scaled for one unstaged, unstreamed window (any head count), else
+// kvbm_kernels_paged_stage_gather, or its streamed form with ls (gated on every window's source flags).  Every source list and
+// the destination's hold n ids; the completion word is written by a trailing signal kernel.
+// layers: a staged gather, window j with the layer window of layers[j]; without, every window is one stage over the
+// destination's layers.  Each window's bytes count over its layers inside the layer range.
 // *seq_out: the launch's sequence number; *out: the notification, as launch_transform sets them (either may be null).
 static int launch_permute(kvbm_transfer_manager* m, const Transfer* e, size_t nw, size_t num_srcs, const size_t* const* src_ids,
                           const size_t* dst_ids, size_t n, const kvbm_transfer_options& o, cudaStream_t stream, uint64_t* seq_out,
                           kvbm_notification* out = nullptr, const kvbm_layer_stream* ls = nullptr, const kvbm_shard_window* layers = nullptr)
 {
   const Layout *S0 = e[0].S, *D = e[0].D[0];
-  uint64_t bytes = 0;
-  for (size_t j = 0; j < nw; ++j) {
-    size_t from = e[0].lb, to = e[0].le;
-    if (layers) {
-      from = std::max(from, layers[j].dst_layer_begin);
-      to = std::min(to, layers[j].dst_layer_begin + layers[j].layer_count);
-    }
-    if (to > from) bytes += n * (to - from) * S0->cfg.outer_dim * (D->region / D->cfg.num_heads * e[j].window.head_count);
-  }
+  const uint64_t bytes = transform_bytes(e, nw, layers, e[0].lb, e[0].le, n, D->region / D->cfg.num_heads);
   const uint32_t dnh = static_cast<uint32_t>(D->cfg.num_heads), page = static_cast<uint32_t>(S0->cfg.page_size);
   const uint32_t row = static_cast<uint32_t>(S0->cfg.inner_dim / S0->cfg.num_heads * S0->cfg.dtype_width_bytes);
   const int nb = static_cast<int>(n), lb = static_cast<int>(e[0].lb), le = static_cast<int>(e[0].le), k = static_cast<int>(nw);
   auto launch = [&](const kvbm_permute_source* ks, const kvbm_permute_side& kd, const kvbm_permute_stream* st, const Slot& sl, uint64_t seq) {
     const uint32_t value = static_cast<uint32_t>(seq);
-    if (layers) {
-      kvbm_stage_source ss[KVBM_GATHER_MAX_SOURCES] = {};
-      for (size_t j = 0; j < nw; ++j)
-        ss[j] = kvbm_stage_source{ks[j], static_cast<uint32_t>(layers[j].src_layer_begin), static_cast<uint32_t>(layers[j].dst_layer_begin),
-                                  static_cast<uint32_t>(layers[j].layer_count)};
-      if (st)
-        return checked(kvbm_kernels_paged_stage_gather_streamed(ss, k, &kd, dnh, nb, lb, le, page, row, o.cast_mode, o.cast_scales, st, stream),
-                       "kvbm_kernels_paged_stage_gather_streamed");
-      return checked(kvbm_kernels_paged_stage_gather(ss, k, &kd, dnh, nb, lb, le, page, row, o.cast_mode, o.cast_scales, o.done_flag, o.epoch,
-                                                     sl.host_flag, value, stream),
-                     "kvbm_kernels_paged_stage_gather");
-    }
-    if (st)
-      return checked(kvbm_kernels_paged_permute_gather_streamed(ks, k, &kd, dnh, nb, lb, le, page, row, o.cast_mode, o.cast_scales, st, stream),
-                     "kvbm_kernels_paged_permute_gather_streamed");
-    if (nw == 1)
+    if (nw == 1 && !layers && !st)
       return checked(kvbm_kernels_paged_permute_heads_scaled(&ks[0].side, &kd, nb, lb, le, ks[0].num_heads, ks[0].src_head_begin, dnh,
                                                              ks[0].dst_head_begin, ks[0].head_count, page, row, o.cast_mode, o.cast_scales,
                                                              o.done_flag, o.epoch, sl.host_flag, value, stream),
                      "kvbm_kernels_paged_permute_heads_scaled");
-    return checked(kvbm_kernels_paged_permute_gather_scaled(ks, k, &kd, dnh, nb, lb, le, page, row, o.cast_mode, o.cast_scales, o.done_flag,
-                                                            o.epoch, sl.host_flag, value, stream),
-                   "kvbm_kernels_paged_permute_gather_scaled");
+    kvbm_stage_source ss[KVBM_GATHER_MAX_SOURCES] = {};
+    stage_sources(ks, layers, nw, D->cfg.num_layers, ss);
+    if (st)
+      return checked(kvbm_kernels_paged_stage_gather_streamed(ss, k, &kd, dnh, nb, lb, le, page, row, o.cast_mode, o.cast_scales, st, stream),
+                     "kvbm_kernels_paged_stage_gather_streamed");
+    return checked(kvbm_kernels_paged_stage_gather(ss, k, &kd, dnh, nb, lb, le, page, row, o.cast_mode, o.cast_scales, o.done_flag, o.epoch,
+                                                   sl.host_flag, value, stream),
+                   "kvbm_kernels_paged_stage_gather");
   };
   return launch_transform(m, e, nw, num_srcs, src_ids, n, dst_ids, n, ls, o, stream, bytes, seq_out, out, launch);
 }
@@ -1338,13 +1347,13 @@ static int repage_strategy(kvbm_transfer_manager* m, const Layout& S, const Layo
 // gather: a TP re-shard's assembly across engines with different page sizes (kvbm_manager_execute_repage_gather and its
 // streamed form), execute_gather's windows over the token range.  The windows are checked as execute_gather checks them and
 // the destination's handle is looked up first; every window's source is then checked against the destination as a pair
-// whose head counts may differ, with its head window and with one page size for every source.  Launched through
-// kvbm_kernels_paged_repage_gather, or its streamed form with ls.
+// whose head counts may differ, with its head window and with one page size for every source.  Launched as one stage over the
+// destination's layers through kvbm_kernels_paged_stage_repage_gather, or its streamed form with ls.
 // layers: a staged re-paging gather, a PP x TP re-shard's assembly across engines with different page sizes
 // (kvbm_manager_execute_stage_repage_gather), windows[j] being the head window of layers[j].  The windows are checked as
 // execute_gather checks a staged gather's, then check_stage_layers, then each pair as above but for the equal layer counts;
-// the options' layer range and the cast scales are the destination's.  Launched through kvbm_kernels_paged_stage_repage_gather,
-// or its streamed form with ls; each window's bytes count over its layers inside the layer range.
+// the options' layer range and the cast scales are the destination's.  Launched through the same entries with its layer
+// windows; each window's bytes count over its layers inside the layer range.
 // Otherwise the plain re-page (kvbm_manager_execute_repage): source 0 over every head of both sides, `windows` unused.  Its
 // source's handle is looked up first, its options fail the pair's checks, its head counts must be equal, and it is launched
 // through kvbm_kernels_paged_repage, which has no head limit.
@@ -1406,161 +1415,115 @@ static int check_repage_request(kvbm_transfer_manager* m, size_t num_srcs, const
   return KVBM_OK;
 }
 
-// What a validated request moves over tokens [tb, te): each window's destination bytes over its layers inside the layer range.
-static uint64_t repage_bytes(const RepageRequest& R, size_t nw, const kvbm_shard_window* layers, size_t tb, size_t te)
-{
-  const Layout& D = *R.D;
-  const size_t d_row = D.cfg.inner_dim / D.cfg.num_heads * D.cfg.dtype_width_bytes;
-  uint64_t bytes = 0;
-  for (size_t j = 0; j < nw; ++j) {
-    size_t from = R.lb, to = R.le;
-    if (layers) {
-      from = std::max(from, layers[j].dst_layer_begin);
-      to = std::min(to, layers[j].dst_layer_begin + layers[j].layer_count);
-    }
-    if (to > from) bytes += (te - tb) * (to - from) * D.cfg.outer_dim * R.e[j].window.head_count * d_row;
-  }
-  return bytes;
-}
-
-// The kernel sources of a staged plan: window j's gather source with its layer window.
-static void stage_sources(const kvbm_permute_source* ks, const kvbm_shard_window* layers, size_t nw, kvbm_stage_source* ss)
-{
-  for (size_t j = 0; j < nw; ++j)
-    ss[j] = kvbm_stage_source{ks[j], static_cast<uint32_t>(layers[j].src_layer_begin), static_cast<uint32_t>(layers[j].dst_layer_begin),
-                              static_cast<uint32_t>(layers[j].layer_count)};
-}
-
-static int execute_repage_gather(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, const size_t* const* src_ids,
-                                 size_t n_src, kvbm_layout_handle dst_h, const size_t* dst_ids, size_t n_dst, size_t tb, size_t te,
-                                 const kvbm_head_window* windows, size_t nw, const kvbm_transfer_options* opts_in, kvbm_notification* out,
-                                 const kvbm_layer_stream* ls = nullptr, bool gather = true, const kvbm_shard_window* layers = nullptr)
+// A re-paging request over a list of sequences, each the token range and tables of one check_repage_request: the single entries
+// pass their one range as one sequence, kvbm_manager_execute_repage_batch its list (`batch`).  Every sequence is checked in
+// turn and the first rejected one returns its code and text; an empty one moves nothing.  Then a batch's concatenated tables
+// are checked for a destination block named twice, and one slot takes every table (and a batch's unit table) in one copy, and
+// one launch moves every sequence: through the _batch kernel entries for a batch, else the single range's.
+static int execute_repage(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, kvbm_layout_handle dst_h,
+                          const kvbm_repage_batch_seq* seqs, size_t num_seqs, const kvbm_head_window* windows, size_t nw,
+                          const kvbm_transfer_options* opts_in, kvbm_notification* out, const kvbm_layer_stream* ls = nullptr,
+                          bool gather = true, const kvbm_shard_window* layers = nullptr, bool batch = false)
 {
   kvbm_transfer_options o{};
   if (opts_in) o = *opts_in;
   if (out) *out = 0;
   int rc;
   if (gather && (rc = check_gather_windows(num_srcs, srcs, windows, nw, o, layers))) return rc;
+  if (batch && num_seqs && !seqs) return fail(KVBM_ERR, "null sequence list");
   std::lock_guard<std::mutex> lk(m->mu);
+  // every sequence resolves the same windows, destination and layer range: only `empty` (and the strategy, set for a
+  // sequence that is not empty) is the last sequence's own
   RepageRequest R;
-  if ((rc = check_repage_request(m, num_srcs, srcs, src_ids, n_src, dst_h, dst_ids, n_dst, tb, te, windows, nw, o, ls, gather, layers, &R)))
-    return rc;
-  if (R.empty) return KVBM_OK;
-  const Transfer* e = R.e;
-  const Layout &S0 = *e[0].S, *D = R.D;
-
-  DeviceGuard g(m->device);
-  const cudaStream_t stream = pick_stream(m, e[0].plan.first, o);
-  const uint32_t row = static_cast<uint32_t>(S0.cfg.inner_dim / S0.cfg.num_heads * S0.cfg.dtype_width_bytes);
-  const uint32_t ups = static_cast<uint32_t>(S0.cfg.page_size), upd = static_cast<uint32_t>(D->cfg.page_size);
-  const uint32_t dnh = static_cast<uint32_t>(D->cfg.num_heads);
-  const uint32_t utb = static_cast<uint32_t>(tb), ute = static_cast<uint32_t>(te);
-  const int ilb = static_cast<int>(R.lb), ile = static_cast<int>(R.le), k = static_cast<int>(nw);
-  auto launch = [&](const kvbm_permute_source* ks, const kvbm_permute_side& kd, const kvbm_permute_stream* st, const Slot& sl, uint64_t seq) {
-    const uint32_t value = static_cast<uint32_t>(seq);
-    if (layers) {
-      kvbm_stage_source ss[KVBM_GATHER_MAX_SOURCES] = {};
-      stage_sources(ks, layers, nw, ss);
-      if (st)
-        return checked(kvbm_kernels_paged_stage_repage_gather_streamed(ss, k, ups, &kd, dnh, upd, utb, ute, ilb, ile, row, o.cast_mode,
-                                                                       o.cast_scales, st, stream),
-                       "kvbm_kernels_paged_stage_repage_gather_streamed");
-      return checked(kvbm_kernels_paged_stage_repage_gather(ss, k, ups, &kd, dnh, upd, utb, ute, ilb, ile, row, o.cast_mode, o.cast_scales,
-                                                            o.done_flag, o.epoch, sl.host_flag, value, stream),
-                     "kvbm_kernels_paged_stage_repage_gather");
-    }
-    if (st)
-      return checked(kvbm_kernels_paged_repage_gather_streamed(ks, k, ups, &kd, dnh, upd, utb, ute, ilb, ile, row, o.cast_mode, o.cast_scales,
-                                                               st, stream),
-                     "kvbm_kernels_paged_repage_gather_streamed");
-    if (gather)
-      return checked(kvbm_kernels_paged_repage_gather(ks, k, ups, &kd, dnh, upd, utb, ute, ilb, ile, row, o.cast_mode, o.cast_scales,
-                                                      o.done_flag, o.epoch, sl.host_flag, value, stream),
-                     "kvbm_kernels_paged_repage_gather");
-    return checked(kvbm_kernels_paged_repage(&ks[0].side, ups, &kd, upd, utb, ute, ilb, ile, ks[0].num_heads, row, o.cast_mode, o.cast_scales,
-                                             o.done_flag, o.epoch, sl.host_flag, value, stream),
-                   "kvbm_kernels_paged_repage");
-  };
-  return launch_transform(m, e, nw, num_srcs, src_ids, n_src, dst_ids, n_dst, ls, o, stream, repage_bytes(R, nw, layers, tb, te), nullptr, out,
-                          launch);
-}
-
-// A batch of sequences as one hand-off (kvbm_manager_execute_repage_batch): every sequence passes check_repage_request as the
-// staged re-paging gather it would be alone; then the concatenated tables are checked for a destination block named twice; then
-// one slot takes every table and the unit table in one copy, and one batch launch moves every sequence.
-static int execute_repage_batch(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, kvbm_layout_handle dst_h,
-                                const kvbm_repage_batch_seq* seqs, size_t num_seqs, const kvbm_head_window* windows,
-                                const kvbm_shard_window* layers, size_t nw, const kvbm_layer_stream* ls, const kvbm_transfer_options* opts_in,
-                                kvbm_notification* out)
-{
-  kvbm_transfer_options o{};
-  if (opts_in) o = *opts_in;
-  if (out) *out = 0;
-  int rc;
-  if ((rc = check_gather_windows(num_srcs, srcs, windows, nw, o, layers))) return rc;
-  if (num_seqs && !seqs) return fail(KVBM_ERR, "null sequence list");
-  std::lock_guard<std::mutex> lk(m->mu);
-  RepageRequest R, Ri;
   bool any = false;
   uint64_t bytes = 0;
-  std::vector<kvbm_repage_seq> ranges;
-  std::vector<std::vector<size_t>> cat(num_srcs + 1);  // each source's concatenated table, then the destination's
-  std::vector<bool> read(num_srcs, false);             // the sources some window reads: the others' tables may be null
-  for (size_t j = 0; j < nw; ++j) read[windows[j].src_rank] = true;
   for (size_t i = 0; i < num_seqs; ++i) {
     const kvbm_repage_batch_seq& q = seqs[i];
     if ((rc = check_repage_request(m, num_srcs, srcs, q.src_ids, q.n_src, dst_h, q.dst_ids, q.n_dst, q.token_begin, q.token_end, windows, nw, o,
-                                   ls, true, layers, &Ri)))
+                                   ls, gather, layers, &R)))
       return rc;
-    if (Ri.empty) continue;
-    R = Ri;
+    if (R.empty) continue;
     any = true;
-    bytes += repage_bytes(R, nw, layers, q.token_begin, q.token_end);
-    ranges.push_back(kvbm_repage_seq{static_cast<uint32_t>(q.token_begin), static_cast<uint32_t>(q.token_end)});
-    for (size_t r = 0; r < num_srcs; ++r)
-      if (read[r]) cat[r].insert(cat[r].end(), q.src_ids[r], q.src_ids[r] + q.n_src);
-    cat[num_srcs].insert(cat[num_srcs].end(), q.dst_ids, q.dst_ids + q.n_dst);
+    const Layout& D = *R.D;
+    bytes += transform_bytes(R.e, nw, layers, R.lb, R.le, q.token_end - q.token_begin, D.cfg.inner_dim / D.cfg.num_heads * D.cfg.dtype_width_bytes);
   }
   if (!any) return KVBM_OK;  // no sequences, only empty ranges or an empty layer range: nothing to move
   const Transfer* e = R.e;
   const Layout &S0 = *e[0].S, *D = R.D;
-  const std::vector<size_t>& cd = cat[num_srcs];
-  for (size_t j = 0; j < nw; ++j) {  // the destination's uniqueness once; a source in the destination's layout also against it
-    const size_t r = windows[j].src_rank;
-    const bool same = srcs[r] == dst_h;
-    if ((j == 0 || same) &&
-        (rc = check_block_ids(cat[r].data(), cat[r].size(), cd.data(), cd.size(), e[j].S->cfg.num_blocks, D->cfg.num_blocks, same)))
-      return rc;
-  }
   const uint32_t ups = static_cast<uint32_t>(S0.cfg.page_size), upd = static_cast<uint32_t>(D->cfg.page_size);
-  size_t num_units = 0, n_src = 0, n_dst = 0;
-  if (kvbm_kernels_repage_batch_units(ranges.data(), ranges.size(), ups, upd, nullptr, 0, &num_units, &n_src, &n_dst))
-    return fail(KVBM_ERR, "the batch's token ranges and page sizes have no unit table");
-  std::vector<kvbm_repage_unit> units(num_units);
-  kvbm_kernels_repage_batch_units(ranges.data(), ranges.size(), ups, upd, units.data(), units.size(), &num_units, &n_src, &n_dst);
-  std::vector<const size_t*> lists(num_srcs);
-  for (size_t r = 0; r < num_srcs; ++r) lists[r] = read[r] ? cat[r].data() : nullptr;
+  const size_t* const* src_ids = seqs[0].src_ids;
+  const size_t* dst_ids = seqs[0].dst_ids;
+  size_t n_src = seqs[0].n_src, n_dst = seqs[0].n_dst;
+  std::vector<kvbm_repage_seq> ranges;
+  std::vector<kvbm_repage_unit> units;
+  std::vector<std::vector<size_t>> cat;  // a batch's: each source's concatenated table, then the destination's
+  std::vector<const size_t*> lists;
+  if (batch) {
+    cat.resize(num_srcs + 1);
+    std::vector<bool> read(num_srcs, false);  // the sources some window reads: the others' tables may be null
+    for (size_t j = 0; j < nw; ++j) read[windows[j].src_rank] = true;
+    for (size_t i = 0; i < num_seqs; ++i) {
+      const kvbm_repage_batch_seq& q = seqs[i];
+      if (q.token_begin == q.token_end) continue;
+      ranges.push_back(kvbm_repage_seq{static_cast<uint32_t>(q.token_begin), static_cast<uint32_t>(q.token_end)});
+      for (size_t r = 0; r < num_srcs; ++r)
+        if (read[r]) cat[r].insert(cat[r].end(), q.src_ids[r], q.src_ids[r] + q.n_src);
+      cat[num_srcs].insert(cat[num_srcs].end(), q.dst_ids, q.dst_ids + q.n_dst);
+    }
+    const std::vector<size_t>& cd = cat[num_srcs];
+    for (size_t j = 0; j < nw; ++j) {  // the destination's uniqueness once; a source in the destination's layout also against it
+      const size_t r = windows[j].src_rank;
+      const bool same = srcs[r] == dst_h;
+      if ((j == 0 || same) &&
+          (rc = check_block_ids(cat[r].data(), cat[r].size(), cd.data(), cd.size(), e[j].S->cfg.num_blocks, D->cfg.num_blocks, same)))
+        return rc;
+    }
+    size_t num_units = 0;
+    if (kvbm_kernels_repage_batch_units(ranges.data(), ranges.size(), ups, upd, nullptr, 0, &num_units, &n_src, &n_dst))
+      return fail(KVBM_ERR, "the batch's token ranges and page sizes have no unit table");
+    units.resize(num_units);
+    kvbm_kernels_repage_batch_units(ranges.data(), ranges.size(), ups, upd, units.data(), units.size(), &num_units, &n_src, &n_dst);
+    lists.resize(num_srcs);
+    for (size_t r = 0; r < num_srcs; ++r) lists[r] = read[r] ? cat[r].data() : nullptr;
+    src_ids = lists.data();
+    dst_ids = cd.data();
+  }
 
   DeviceGuard g(m->device);
   const cudaStream_t stream = pick_stream(m, e[0].plan.first, o);
   const uint32_t row = static_cast<uint32_t>(S0.cfg.inner_dim / S0.cfg.num_heads * S0.cfg.dtype_width_bytes);
   const uint32_t dnh = static_cast<uint32_t>(D->cfg.num_heads);
+  const uint32_t utb = static_cast<uint32_t>(seqs[0].token_begin), ute = static_cast<uint32_t>(seqs[0].token_end);
   const int ilb = static_cast<int>(R.lb), ile = static_cast<int>(R.le), k = static_cast<int>(nw);
   auto launch = [&](const kvbm_permute_source* ks, const kvbm_permute_side& kd, const kvbm_permute_stream* st, const Slot& sl, uint64_t seq) {
-    const auto* du = reinterpret_cast<const kvbm_repage_unit*>(sl.dev_ids + units_at(num_srcs * n_src + n_dst));
+    const uint32_t value = static_cast<uint32_t>(seq);
+    if (!gather)
+      return checked(kvbm_kernels_paged_repage(&ks[0].side, ups, &kd, upd, utb, ute, ilb, ile, ks[0].num_heads, row, o.cast_mode, o.cast_scales,
+                                               o.done_flag, o.epoch, sl.host_flag, value, stream),
+                     "kvbm_kernels_paged_repage");
     kvbm_stage_source ss[KVBM_GATHER_MAX_SOURCES] = {};
-    stage_sources(ks, layers, nw, ss);
+    stage_sources(ks, layers, nw, D->cfg.num_layers, ss);
+    if (batch) {
+      const auto* du = reinterpret_cast<const kvbm_repage_unit*>(sl.dev_ids + units_at(num_srcs * n_src + n_dst));
+      if (st)
+        return checked(kvbm_kernels_paged_stage_repage_gather_batch_streamed(ss, k, ups, &kd, dnh, upd, ranges.data(), ranges.size(), du,
+                                                                             units.size(), ilb, ile, row, o.cast_mode, o.cast_scales, st, stream),
+                       "kvbm_kernels_paged_stage_repage_gather_batch_streamed");
+      return checked(kvbm_kernels_paged_stage_repage_gather_batch(ss, k, ups, &kd, dnh, upd, ranges.data(), ranges.size(), du, units.size(), ilb,
+                                                                  ile, row, o.cast_mode, o.cast_scales, o.done_flag, o.epoch, sl.host_flag, value,
+                                                                  stream),
+                     "kvbm_kernels_paged_stage_repage_gather_batch");
+    }
     if (st)
-      return checked(kvbm_kernels_paged_stage_repage_gather_batch_streamed(ss, k, ups, &kd, dnh, upd, ranges.data(), ranges.size(), du, num_units,
-                                                                           ilb, ile, row, o.cast_mode, o.cast_scales, st, stream),
-                     "kvbm_kernels_paged_stage_repage_gather_batch_streamed");
-    return checked(kvbm_kernels_paged_stage_repage_gather_batch(ss, k, ups, &kd, dnh, upd, ranges.data(), ranges.size(), du, num_units, ilb, ile,
-                                                                row, o.cast_mode, o.cast_scales, o.done_flag, o.epoch, sl.host_flag,
-                                                                static_cast<uint32_t>(seq), stream),
-                   "kvbm_kernels_paged_stage_repage_gather_batch");
+      return checked(kvbm_kernels_paged_stage_repage_gather_streamed(ss, k, ups, &kd, dnh, upd, utb, ute, ilb, ile, row, o.cast_mode,
+                                                                     o.cast_scales, st, stream),
+                     "kvbm_kernels_paged_stage_repage_gather_streamed");
+    return checked(kvbm_kernels_paged_stage_repage_gather(ss, k, ups, &kd, dnh, upd, utb, ute, ilb, ile, row, o.cast_mode, o.cast_scales,
+                                                          o.done_flag, o.epoch, sl.host_flag, value, stream),
+                   "kvbm_kernels_paged_stage_repage_gather");
   };
-  return launch_transform(m, e, nw, num_srcs, lists.data(), n_src, cd.data(), n_dst, ls, o, stream, bytes, nullptr, out, launch, units.data(),
-                          num_units);
+  return launch_transform(m, e, nw, num_srcs, src_ids, n_src, dst_ids, n_dst, ls, o, stream, bytes, nullptr, out, launch, units.data(),
+                          units.size());
 }
 
 }  // namespace kvbm_host
@@ -2128,8 +2091,8 @@ extern "C" int kvbm_manager_execute_repage(kvbm_transfer_manager* m, kvbm_layout
 {
   return guarded([&]() -> int {
   if (!m) return fail(KVBM_ERR, "null manager");
-  return execute_repage_gather(m, 1, &src, &src_ids, n_src, dst, dst_ids, n_dst, token_begin, token_end, /*windows=*/nullptr, 1, opts, out,
-                               /*ls=*/nullptr, /*gather=*/false);
+  const kvbm_repage_batch_seq q{token_begin, token_end, &src_ids, n_src, dst_ids, n_dst};
+  return execute_repage(m, 1, &src, dst, &q, 1, /*windows=*/nullptr, 1, opts, out, /*ls=*/nullptr, /*gather=*/false);
   });
 }
 
@@ -2140,8 +2103,28 @@ extern "C" int kvbm_manager_execute_repage_gather(kvbm_transfer_manager* m, size
 {
   return guarded([&]() -> int {
   if (!m) return fail(KVBM_ERR, "null manager");
-  return execute_repage_gather(m, num_srcs, srcs, src_ids, n_src, dst, dst_ids, n_dst, token_begin, token_end, windows, num_windows, opts, out);
+  const kvbm_repage_batch_seq q{token_begin, token_end, src_ids, n_src, dst_ids, n_dst};
+  return execute_repage(m, num_srcs, srcs, dst, &q, 1, windows, num_windows, opts, out);
   });
+}
+
+// The start of every entry that may stream: a null manager, then the layer stream's shape when there is one or `streamed`
+// requires it.
+static int stream_entry(kvbm_transfer_manager* m, const kvbm_layer_stream* ls, size_t num_srcs, bool streamed, kvbm_notification* out)
+{
+  if (!m) return fail(KVBM_ERR, "null manager");
+  if (out) *out = 0;
+  return ls || streamed ? check_layer_stream_shape(ls, num_srcs) : KVBM_OK;
+}
+
+// The head windows of a staged plan's windows, in hw[], or null without windows.  Only the first KVBM_GATHER_MAX_SOURCES are
+// copied: check_gather_windows rejects more windows than that before it reads any.
+static const kvbm_head_window* head_windows(const kvbm_shard_window* windows, size_t nw, kvbm_head_window* hw)
+{
+  if (!windows) return nullptr;
+  for (size_t j = 0; j < std::min<size_t>(nw, KVBM_GATHER_MAX_SOURCES); ++j)
+    hw[j] = kvbm_head_window{windows[j].src_rank, windows[j].src_head_begin, windows[j].dst_head_begin, windows[j].head_count};
+  return hw;
 }
 
 extern "C" int kvbm_manager_execute_gather_streamed(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs,
@@ -2150,9 +2133,7 @@ extern "C" int kvbm_manager_execute_gather_streamed(kvbm_transfer_manager* m, si
                                                     const kvbm_transfer_options* opts, kvbm_notification* out)
 {
   return guarded([&]() -> int {
-  if (!m) return fail(KVBM_ERR, "null manager");
-  if (out) *out = 0;
-  if (int rc = check_layer_stream_shape(ls, num_srcs)) return rc;
+  if (int rc = stream_entry(m, ls, num_srcs, true, out)) return rc;
   return execute_gather(m, num_srcs, srcs, src_ids, dst, dst_ids, n, windows, num_windows, opts, out, ls);
   });
 }
@@ -2163,14 +2144,9 @@ extern "C" int kvbm_manager_execute_stage_gather(kvbm_transfer_manager* m, size_
                                                  const kvbm_transfer_options* opts, kvbm_notification* out)
 {
   return guarded([&]() -> int {
-  if (!m) return fail(KVBM_ERR, "null manager");
-  if (out) *out = 0;
-  if (ls)
-    if (int rc = check_layer_stream_shape(ls, num_srcs)) return rc;
-  std::vector<kvbm_head_window> hw(windows ? num_windows : 0);
-  for (size_t j = 0; j < hw.size(); ++j)
-    hw[j] = kvbm_head_window{windows[j].src_rank, windows[j].src_head_begin, windows[j].dst_head_begin, windows[j].head_count};
-  return execute_gather(m, num_srcs, srcs, src_ids, dst, dst_ids, n, windows ? hw.data() : nullptr, num_windows, opts, out, ls, windows);
+  if (int rc = stream_entry(m, ls, num_srcs, false, out)) return rc;
+  kvbm_head_window hw[KVBM_GATHER_MAX_SOURCES];
+  return execute_gather(m, num_srcs, srcs, src_ids, dst, dst_ids, n, head_windows(windows, num_windows, hw), num_windows, opts, out, ls, windows);
   });
 }
 
@@ -2181,15 +2157,11 @@ extern "C" int kvbm_manager_execute_stage_repage_gather(kvbm_transfer_manager* m
                                                         const kvbm_transfer_options* opts, kvbm_notification* out)
 {
   return guarded([&]() -> int {
-  if (!m) return fail(KVBM_ERR, "null manager");
-  if (out) *out = 0;
-  if (ls)
-    if (int rc = check_layer_stream_shape(ls, num_srcs)) return rc;
-  std::vector<kvbm_head_window> hw(windows ? num_windows : 0);
-  for (size_t j = 0; j < hw.size(); ++j)
-    hw[j] = kvbm_head_window{windows[j].src_rank, windows[j].src_head_begin, windows[j].dst_head_begin, windows[j].head_count};
-  return execute_repage_gather(m, num_srcs, srcs, src_ids, n_src, dst, dst_ids, n_dst, token_begin, token_end, windows ? hw.data() : nullptr,
-                               num_windows, opts, out, ls, /*gather=*/true, windows);
+  if (int rc = stream_entry(m, ls, num_srcs, false, out)) return rc;
+  kvbm_head_window hw[KVBM_GATHER_MAX_SOURCES];
+  const kvbm_repage_batch_seq q{token_begin, token_end, src_ids, n_src, dst_ids, n_dst};
+  return execute_repage(m, num_srcs, srcs, dst, &q, 1, head_windows(windows, num_windows, hw), num_windows, opts, out, ls, /*gather=*/true,
+                        windows);
   });
 }
 
@@ -2199,14 +2171,10 @@ extern "C" int kvbm_manager_execute_repage_batch(kvbm_transfer_manager* m, size_
                                                  const kvbm_transfer_options* opts, kvbm_notification* out)
 {
   return guarded([&]() -> int {
-  if (!m) return fail(KVBM_ERR, "null manager");
-  if (out) *out = 0;
-  if (ls)
-    if (int rc = check_layer_stream_shape(ls, num_srcs)) return rc;
-  std::vector<kvbm_head_window> hw(windows ? num_windows : 0);
-  for (size_t j = 0; j < hw.size(); ++j)
-    hw[j] = kvbm_head_window{windows[j].src_rank, windows[j].src_head_begin, windows[j].dst_head_begin, windows[j].head_count};
-  return execute_repage_batch(m, num_srcs, srcs, dst, seqs, num_seqs, windows ? hw.data() : nullptr, windows, num_windows, ls, opts, out);
+  if (int rc = stream_entry(m, ls, num_srcs, false, out)) return rc;
+  kvbm_head_window hw[KVBM_GATHER_MAX_SOURCES];
+  return execute_repage(m, num_srcs, srcs, dst, seqs, num_seqs, head_windows(windows, num_windows, hw), num_windows, opts, out, ls,
+                        /*gather=*/true, windows, /*batch=*/true);
   });
 }
 
@@ -2217,11 +2185,9 @@ extern "C" int kvbm_manager_execute_repage_gather_streamed(kvbm_transfer_manager
                                                            const kvbm_transfer_options* opts, kvbm_notification* out)
 {
   return guarded([&]() -> int {
-  if (!m) return fail(KVBM_ERR, "null manager");
-  if (out) *out = 0;
-  if (int rc = check_layer_stream_shape(ls, num_srcs)) return rc;
-  return execute_repage_gather(m, num_srcs, srcs, src_ids, n_src, dst, dst_ids, n_dst, token_begin, token_end, windows, num_windows, opts, out,
-                               ls);
+  if (int rc = stream_entry(m, ls, num_srcs, true, out)) return rc;
+  const kvbm_repage_batch_seq q{token_begin, token_end, src_ids, n_src, dst_ids, n_dst};
+  return execute_repage(m, num_srcs, srcs, dst, &q, 1, windows, num_windows, opts, out, ls);
   });
 }
 

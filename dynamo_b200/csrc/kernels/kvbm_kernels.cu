@@ -1049,6 +1049,16 @@ static void with_walk_kernel(int cast_mode, bool pow2, bool scaled, F&& f)
   }
 }
 
+// with_walk_kernel for the re-paging kernels, whose last template argument is the small page's split: calls
+// f(cast, row pow2, scaled, bool_constant<PAGE_POW2>).
+template <class F>
+static void with_repage_kernel(int cast_mode, bool pow2, bool scaled, bool page_pow2, F&& f)
+{
+  with_walk_kernel(cast_mode, pow2, scaled, [&](auto c, auto p, auto sc) {
+    page_pow2 ? f(c, p, sc, std::true_type{}) : f(c, p, sc, std::false_type{});
+  });
+}
+
 __global__ void kvbm_signal_kernel(uint32_t* a, uint32_t va, uint32_t* b, uint32_t vb)
 {
   __threadfence_system();
@@ -1674,15 +1684,11 @@ static cudaError_t launch_paged_repage_gather(const kvbm_stage_source* srcs, int
         },
         [&](const GateArgs& A, unsigned ctas, uint32_t batch) {
           const uint32_t nb = static_cast<uint32_t>(units / (static_cast<uint64_t>(P.geo.nlayers) * no));
-          with_walk_kernel(cast_mode, r.pow2, cast_scales != nullptr, [&](auto c, auto p, auto sc) {
-            if (B && page_pow2)
-              kvbm_gated_batch_repage_gather_kernel<c, p, sc, true><<<ctas, threads, 0, stream>>>(P, A, B->units, nb, r, cast_scales, batch);
-            else if (B)
-              kvbm_gated_batch_repage_gather_kernel<c, p, sc, false><<<ctas, threads, 0, stream>>>(P, A, B->units, nb, r, cast_scales, batch);
-            else if (page_pow2)
-              kvbm_gated_repage_gather_kernel<c, p, sc, true><<<ctas, threads, 0, stream>>>(P, A, nb, r, cast_scales, batch);
+          with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, page_pow2, [&](auto c, auto p, auto sc, auto pp) {
+            if (B)
+              kvbm_gated_batch_repage_gather_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, A, B->units, nb, r, cast_scales, batch);
             else
-              kvbm_gated_repage_gather_kernel<c, p, sc, false><<<ctas, threads, 0, stream>>>(P, A, nb, r, cast_scales, batch);
+              kvbm_gated_repage_gather_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, A, nb, r, cast_scales, batch);
           });
         });
   // a window over every layer and every head of both sides (the checks above make its starts 0)
@@ -1692,19 +1698,13 @@ static cudaError_t launch_paged_repage_gather(const kvbm_stage_source* srcs, int
   R.big = P.geo.src_small ? P.g.D : P.g.src[0].S;
   R.small = P.geo.src_small ? P.g.src[0].S : P.g.D;
   R.g = P.geo;
-  with_walk_kernel(cast_mode, r.pow2, cast_scales != nullptr, [&](auto c, auto p, auto sc) {
-    if (B && page_pow2)
-      kvbm_paged_batch_repage_gather_kernel<c, p, sc, true><<<grid, threads, 0, stream>>>(P, B->units, r, cast_scales);
-    else if (B)
-      kvbm_paged_batch_repage_gather_kernel<c, p, sc, false><<<grid, threads, 0, stream>>>(P, B->units, r, cast_scales);
-    else if (plain && page_pow2)
-      kvbm_paged_repage_kernel<c, p, sc, true><<<grid, threads, 0, stream>>>(R, r, cast_scales);
+  with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, page_pow2, [&](auto c, auto p, auto sc, auto pp) {
+    if (B)
+      kvbm_paged_batch_repage_gather_kernel<c, p, sc, pp><<<grid, threads, 0, stream>>>(P, B->units, r, cast_scales);
     else if (plain)
-      kvbm_paged_repage_kernel<c, p, sc, false><<<grid, threads, 0, stream>>>(R, r, cast_scales);
-    else if (page_pow2)
-      kvbm_paged_repage_gather_kernel<c, p, sc, true><<<grid, threads, 0, stream>>>(P, r, cast_scales);
+      kvbm_paged_repage_kernel<c, p, sc, pp><<<grid, threads, 0, stream>>>(R, r, cast_scales);
     else
-      kvbm_paged_repage_gather_kernel<c, p, sc, false><<<grid, threads, 0, stream>>>(P, r, cast_scales);
+      kvbm_paged_repage_gather_kernel<c, p, sc, pp><<<grid, threads, 0, stream>>>(P, r, cast_scales);
   });
   return launched(stream, done_flag, epoch, completion_flag, completion_value);
 }
