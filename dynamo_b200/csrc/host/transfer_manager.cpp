@@ -1526,6 +1526,154 @@ static int execute_repage(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_
                           units.size());
 }
 
+// The windows of a scatter, before any layout is looked up: at least one destination and one window, none in the options, at most
+// KVBM_GATHER_MAX_SOURCES, each naming a destination, with heads and layers; source layer windows equal (one stage) or disjoint;
+// the windows of one destination on disjoint (layer, head) rectangles of it; no destination handle listed twice.
+static int check_scatter_windows(size_t num_dsts, const kvbm_layout_handle* dsts, const kvbm_scatter_window* w, size_t nw,
+                                 const kvbm_transfer_options& o)
+{
+  if (num_dsts == 0 || !dsts || !w || nw == 0) return fail(KVBM_ERR, "a scatter needs at least one destination and one window");
+  if (o.head_count) return fail(KVBM_ERR, "a scatter takes its head windows from the windows argument: options.head_count must be 0");
+  if (nw > KVBM_GATHER_MAX_SOURCES)
+    return fail(KVBM_ERR_UNSUPPORTED, "a scatter takes at most " + std::to_string(KVBM_GATHER_MAX_SOURCES) + " windows, got " + std::to_string(nw));
+  auto meet = [](size_t a, size_t na, size_t b, size_t nb) { return a < b + nb && b < a + na; };
+  for (size_t j = 0; j < nw; ++j) {
+    if (w[j].dst_rank >= num_dsts)
+      return fail(KVBM_ERR_RANGE, "window " + std::to_string(j) + " names destination " + std::to_string(w[j].dst_rank) + " of " +
+                                      std::to_string(num_dsts));
+    if (w[j].head_count == 0) return fail(KVBM_ERR_RANGE, "window " + std::to_string(j) + " has no heads");
+    if (w[j].layer_count == 0) return fail(KVBM_ERR_RANGE, "window " + std::to_string(j) + " has no layers");
+    for (size_t t = 0; t < j; ++t) {
+      const bool same = w[t].src_layer_begin == w[j].src_layer_begin && w[t].layer_count == w[j].layer_count;
+      if (!same && meet(w[t].src_layer_begin, w[t].layer_count, w[j].src_layer_begin, w[j].layer_count))
+        return fail(KVBM_ERR_OVERLAP, "windows " + std::to_string(t) + " and " + std::to_string(j) + " have source layer windows that partly overlap");
+      if (w[t].dst_rank == w[j].dst_rank && meet(w[t].dst_layer_begin, w[t].layer_count, w[j].dst_layer_begin, w[j].layer_count) &&
+          meet(w[t].dst_head_begin, w[t].head_count, w[j].dst_head_begin, w[j].head_count))
+        return fail(KVBM_ERR_OVERLAP, "windows " + std::to_string(t) + " and " + std::to_string(j) + " overlap in destination " +
+                                          std::to_string(w[j].dst_rank));
+    }
+  }
+  for (size_t d = 0; d < num_dsts; ++d)
+    for (size_t e = 0; e < d; ++e)
+      if (dsts[d] == dsts[e]) return fail(KVBM_ERR_OVERLAP, "destinations " + std::to_string(e) + " and " + std::to_string(d) + " are one layout");
+  return KVBM_OK;
+}
+
+// One prefill rank's KV into every decode rank that needs it (kvbm_manager_execute_repage_scatter), validated in the order its
+// header gives, then one staged copy of [source ids (n_src), destination 0 .. num_dsts - 1 ids (n_dst each)], one
+// kvbm_kernels_paged_repage_scatter launch whose signal writes the per-destination done flags and the completion word, and the
+// options' done flag after it.
+static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle src_h, const size_t* src_ids, size_t n_src, size_t num_dsts,
+                                  const kvbm_layout_handle* dsts, const size_t* const* dst_ids, size_t n_dst, size_t tb, size_t te,
+                                  const kvbm_scatter_window* w, size_t nw, const kvbm_transfer_options* opts_in, kvbm_notification* out)
+{
+  kvbm_transfer_options o{};
+  if (opts_in) o = *opts_in;
+  if (out) *out = 0;
+  int rc;
+  if ((rc = check_scatter_windows(num_dsts, dsts, w, nw, o))) return rc;
+  std::lock_guard<std::mutex> lk(m->mu);
+  Layout* S = m->find(src_h);
+  if (!S) return fail(KVBM_ERR_HANDLE, "invalid source handle");
+  std::vector<Layout*> D(num_dsts);
+  for (size_t d = 0; d < num_dsts; ++d)
+    if (!(D[d] = m->find(dsts[d]))) return fail(KVBM_ERR_HANDLE, "invalid destination handle");
+  const size_t snl = S->cfg.num_layers;
+  for (size_t j = 0; j < nw; ++j) {
+    const size_t dnl = D[w[j].dst_rank]->cfg.num_layers;
+    if (w[j].src_layer_begin > snl || w[j].layer_count > snl - w[j].src_layer_begin)
+      return fail(KVBM_ERR_RANGE, "window " + std::to_string(j) + "'s source layers " + std::to_string(w[j].src_layer_begin) + ".." +
+                                      std::to_string(w[j].src_layer_begin + w[j].layer_count) + " exceed the source's num_layers " +
+                                      std::to_string(snl));
+    if (w[j].dst_layer_begin > dnl || w[j].layer_count > dnl - w[j].dst_layer_begin)
+      return fail(KVBM_ERR_RANGE, "window " + std::to_string(j) + "'s destination layers " + std::to_string(w[j].dst_layer_begin) + ".." +
+                                      std::to_string(w[j].dst_layer_begin + w[j].layer_count) + " exceed the destination's num_layers " +
+                                      std::to_string(dnl));
+  }
+  {
+    const size_t lb = o.has_layer_range ? o.layer_begin : 0, le = o.has_layer_range ? std::min(o.layer_end, snl) : snl;
+    for (size_t l = lb; l < le; ++l) {  // a range past the source's layers is check_layer_range's to reject
+      bool in = false;
+      for (size_t j = 0; j < nw && !in; ++j) in = l >= w[j].src_layer_begin && l - w[j].src_layer_begin < w[j].layer_count;
+      if (!in) return fail(KVBM_ERR_RANGE, "source layer " + std::to_string(l) + " of the layer range is in no window's layers");
+    }
+  }
+  // the pair checks take the per-destination done flags, which a scatter honours, as absent
+  kvbm_transfer_options op = o;
+  op.per_dst_done_flags = nullptr;
+  Transfer e[KVBM_GATHER_MAX_SOURCES];
+  for (size_t j = 0; j < nw; ++j) {
+    Layout& Dj = *D[w[j].dst_rank];
+    e[j].S = S;
+    e[j].D[0] = &Dj;
+    e[j].window = kvbm_head_window{0, w[j].src_head_begin, w[j].dst_head_begin, w[j].head_count};
+    if ((rc = check_repage_pair(*S, Dj, op, true, &e[j].src_kv, &e[j].dst_kv, true)) || (rc = check_head_window(*S, Dj, e[j].window, 1))) return rc;
+    if (Dj.cfg.page_size != D[w[0].dst_rank]->cfg.page_size)
+      return fail(KVBM_ERR_INCOMPATIBLE, "the destinations of a scatter need one page size: destination " + std::to_string(w[0].dst_rank) +
+                                             " has " + std::to_string(D[w[0].dst_rank]->cfg.page_size) + ", destination " +
+                                             std::to_string(w[j].dst_rank) + " has " + std::to_string(Dj.cfg.page_size));
+  }
+  const size_t ps = S->cfg.page_size, pd = D[w[0].dst_rank]->cfg.page_size;
+  if (tb > te || te > (size_t{1} << 31))
+    return fail(KVBM_ERR_RANGE, "Token range " + std::to_string(tb) + ".." + std::to_string(te) + " is reversed or reaches past 2^31 tokens");
+  size_t lb, le;
+  if ((rc = check_layer_range(S->cfg, o, &lb, &le))) return rc;
+  if ((rc = check_repage_counts(tb, te, ps, pd, n_src, n_dst))) return rc;
+  if ((n_src && !src_ids) || (n_dst && !dst_ids)) return fail(KVBM_ERR, "null block id list");
+  for (size_t j = 0; j < nw; ++j) {
+    const size_t d = w[j].dst_rank;
+    if (n_dst && !dst_ids[d]) return fail(KVBM_ERR, "null block id list");
+    if ((rc = check_block_ids(src_ids, n_src, n_dst ? dst_ids[d] : nullptr, n_dst, S->cfg.num_blocks, D[d]->cfg.num_blocks, src_h == dsts[d])))
+      return rc;
+  }
+  if (tb == te || lb == le) return KVBM_OK;  // nothing to move, as execute()
+  for (size_t j = 0; j < nw; ++j) {
+    if ((rc = repage_strategy(m, *S, *e[j].D[0], &e[j].plan))) return rc;
+    if (e[j].plan.first != e[0].plan.first) return fail(KVBM_ERR_UNSUPPORTED, "the destinations of a scatter need the same CUDA strategy");
+  }
+  if ((rc = need_cuda_device(m))) return rc;
+  if (o.cast_scales && (rc = check_cast_scales(m, o.cast_scales))) return rc;
+
+  // what lands: each window's destination bytes over its layers inside the range
+  uint64_t bytes = 0;
+  for (size_t j = 0; j < nw; ++j) {
+    const Layout& Dj = *e[j].D[0];
+    const size_t from = std::max(lb, w[j].src_layer_begin), to = std::min(le, w[j].src_layer_begin + w[j].layer_count);
+    if (to > from) bytes += (te - tb) * (to - from) * Dj.cfg.outer_dim * w[j].head_count * (Dj.cfg.inner_dim / Dj.cfg.num_heads * Dj.cfg.dtype_width_bytes);
+  }
+  DeviceGuard g(m->device);
+  const cudaStream_t stream = pick_stream(m, e[0].plan.first, o);
+  std::vector<const size_t*> lists(num_dsts + 1);
+  std::vector<size_t> lens(num_dsts + 1, n_dst);
+  lists[0] = src_ids;
+  lens[0] = n_src;
+  for (size_t d = 0; d < num_dsts; ++d) lists[1 + d] = n_dst ? dst_ids[d] : nullptr;
+  Slot* sl;
+  uint64_t seq;
+  if ((rc = stage_ids(m, lists.data(), lens.data(), num_dsts + 1, 4, stream, nullptr, &sl, &seq))) return rc;
+  const kvbm_permute_side ks{descriptor(*S), sl->dev_ids, e[0].src_kv};
+  kvbm_scatter_target kt[KVBM_GATHER_MAX_SOURCES] = {};
+  for (size_t j = 0; j < nw; ++j) {
+    const size_t d = w[j].dst_rank;
+    kt[j] = kvbm_scatter_target{{descriptor(*D[d]), sl->dev_ids + n_src + d * n_dst, e[j].dst_kv}, static_cast<uint32_t>(D[d]->cfg.num_heads),
+                                static_cast<uint32_t>(w[j].src_head_begin), static_cast<uint32_t>(w[j].dst_head_begin),
+                                static_cast<uint32_t>(w[j].head_count), static_cast<uint32_t>(w[j].src_layer_begin),
+                                static_cast<uint32_t>(w[j].dst_layer_begin), static_cast<uint32_t>(w[j].layer_count),
+                                o.per_dst_done_flags ? o.per_dst_done_flags[d] : nullptr};
+  }
+  const uint32_t row = static_cast<uint32_t>(S->cfg.inner_dim / S->cfg.num_heads * S->cfg.dtype_width_bytes);
+  if ((rc = checked(kvbm_kernels_paged_repage_scatter(&ks, static_cast<uint32_t>(S->cfg.num_heads), static_cast<uint32_t>(ps), kt,
+                                                      static_cast<int>(nw), static_cast<uint32_t>(pd), static_cast<uint32_t>(tb),
+                                                      static_cast<uint32_t>(te), static_cast<int>(lb), static_cast<int>(le), row, o.cast_mode,
+                                                      o.cast_scales, o.epoch, sl->host_flag, static_cast<uint32_t>(seq), stream),
+                    "kvbm_kernels_paged_repage_scatter")))
+    return rc;
+  if (o.done_flag && (rc = checked(kvbm_kernels_set_flags(o.done_flag, 0, 1, o.epoch, stream), "kvbm_kernels_set_flags"))) return rc;
+  if ((rc = finish_slot(m, sl, stream, bytes))) return rc;
+  if (out) *out = o.use_caller_stream ? 0 : seq;
+  return KVBM_OK;
+}
+
 }  // namespace kvbm_host
 
 // =====================================================================================================
@@ -2021,6 +2169,35 @@ static int stage_bounds(const char* side, size_t L, size_t pp, const size_t* par
   return KVBM_OK;
 }
 
+// kvbm_tp_pp_reshard_plan's windows of decode rank dst_rank, after the checks every rank shares (the caller's), into *w.
+static int tp_pp_windows(size_t num_kv_heads, size_t src_tp, size_t src_pp, const std::vector<size_t>& sb, size_t dst_tp,
+                         const std::vector<size_t>& db, size_t dst_rank, std::vector<kvbm_shard_window>* w)
+{
+  std::vector<kvbm_head_window> heads;
+  if (int rc = tp_head_windows(num_kv_heads, src_tp, dst_tp, dst_rank % dst_tp, &heads)) return rc;
+  const size_t stage = dst_rank / dst_tp, d0 = db[stage], d1 = db[stage + 1];
+  w->clear();
+  for (size_t p = 0; p < src_pp; ++p) {
+    const size_t lo = std::max(d0, sb[p]), hi = std::min(d1, sb[p + 1]);
+    if (lo >= hi) continue;
+    for (const kvbm_head_window& h : heads)
+      w->push_back({p * src_tp + h.src_rank, lo - sb[p], lo - d0, hi - lo, h.src_head_begin, h.dst_head_begin, h.head_count});
+  }
+  return KVBM_OK;
+}
+
+// The checks both PP x TP plans make before they name a rank: positive arguments and each side's stage bounds.
+static int tp_pp_bounds(size_t num_kv_heads, size_t num_layers, size_t src_tp, size_t src_pp, const size_t* src_stage_layers, size_t dst_tp,
+                        size_t dst_pp, const size_t* dst_stage_layers, std::vector<size_t>* sb, std::vector<size_t>* db)
+{
+  if (!num_kv_heads || !num_layers || !src_tp || !src_pp || !dst_tp || !dst_pp)
+    return fail(KVBM_ERR_CONFIG, "num_kv_heads, num_layers and every TP and PP degree must be positive");
+  int rc;
+  if ((rc = stage_bounds("source", num_layers, src_pp, src_stage_layers, sb)) || (rc = stage_bounds("destination", num_layers, dst_pp, dst_stage_layers, db)))
+    return rc;
+  return KVBM_OK;
+}
+
 extern "C" int kvbm_tp_pp_reshard_plan(size_t num_kv_heads, size_t num_layers, size_t src_tp, size_t src_pp, const size_t* src_stage_layers,
                                        size_t dst_tp, size_t dst_pp, const size_t* dst_stage_layers, size_t dst_rank, kvbm_shard_window* out,
                                        size_t cap, size_t* n_out)
@@ -2028,28 +2205,47 @@ extern "C" int kvbm_tp_pp_reshard_plan(size_t num_kv_heads, size_t num_layers, s
   return guarded([&]() -> int {
   if (!n_out) return fail(KVBM_ERR, "null argument");
   *n_out = 0;
-  if (!num_kv_heads || !num_layers || !src_tp || !src_pp || !dst_tp || !dst_pp)
-    return fail(KVBM_ERR_CONFIG, "num_kv_heads, num_layers and every TP and PP degree must be positive");
   std::vector<size_t> sb, db;
   int rc;
-  if ((rc = stage_bounds("source", num_layers, src_pp, src_stage_layers, &sb)) || (rc = stage_bounds("destination", num_layers, dst_pp, dst_stage_layers, &db)))
-    return rc;
+  if ((rc = tp_pp_bounds(num_kv_heads, num_layers, src_tp, src_pp, src_stage_layers, dst_tp, dst_pp, dst_stage_layers, &sb, &db))) return rc;
   if (dst_rank >= dst_pp * dst_tp)
     return fail(KVBM_ERR_RANGE, "dst_rank " + std::to_string(dst_rank) + " out of range for PP " + std::to_string(dst_pp) + " x TP " +
                                     std::to_string(dst_tp));
-  std::vector<kvbm_head_window> heads;
-  if ((rc = tp_head_windows(num_kv_heads, src_tp, dst_tp, dst_rank % dst_tp, &heads))) return rc;
-  const size_t stage = dst_rank / dst_tp, d0 = db[stage], d1 = db[stage + 1];
   std::vector<kvbm_shard_window> w;
-  for (size_t p = 0; p < src_pp; ++p) {
-    const size_t lo = std::max(d0, sb[p]), hi = std::min(d1, sb[p + 1]);
-    if (lo >= hi) continue;
-    for (const kvbm_head_window& h : heads)
-      w.push_back({p * src_tp + h.src_rank, lo - sb[p], lo - d0, hi - lo, h.src_head_begin, h.dst_head_begin, h.head_count});
-  }
+  if ((rc = tp_pp_windows(num_kv_heads, src_tp, src_pp, sb, dst_tp, db, dst_rank, &w))) return rc;
   *n_out = w.size();
   if (!out) return KVBM_OK;
   if (cap < w.size()) return fail(KVBM_ERR, "kvbm_tp_pp_reshard_plan: " + std::to_string(w.size()) + " windows do not fit in " + std::to_string(cap));
+  std::copy(w.begin(), w.end(), out);
+  return KVBM_OK;
+  });
+}
+
+extern "C" int kvbm_tp_pp_scatter_plan(size_t num_kv_heads, size_t num_layers, size_t src_tp, size_t src_pp, const size_t* src_stage_layers,
+                                       size_t dst_tp, size_t dst_pp, const size_t* dst_stage_layers, size_t src_rank, kvbm_scatter_window* out,
+                                       size_t cap, size_t* n_out)
+{
+  return guarded([&]() -> int {
+  if (!n_out) return fail(KVBM_ERR, "null argument");
+  *n_out = 0;
+  std::vector<size_t> sb, db;
+  int rc;
+  if ((rc = tp_pp_bounds(num_kv_heads, num_layers, src_tp, src_pp, src_stage_layers, dst_tp, dst_pp, dst_stage_layers, &sb, &db))) return rc;
+  if (src_rank >= src_pp * src_tp)
+    return fail(KVBM_ERR_RANGE, "src_rank " + std::to_string(src_rank) + " out of range for PP " + std::to_string(src_pp) + " x TP " +
+                                    std::to_string(src_tp));
+  // the inverse of the gather plans: every decode rank's windows that read src_rank, in ascending decode rank
+  std::vector<kvbm_scatter_window> w;
+  std::vector<kvbm_shard_window> g;
+  for (size_t d = 0; d < dst_pp * dst_tp; ++d) {
+    if ((rc = tp_pp_windows(num_kv_heads, src_tp, src_pp, sb, dst_tp, db, d, &g))) return rc;
+    for (const kvbm_shard_window& x : g)
+      if (x.src_rank == src_rank)
+        w.push_back({d, x.src_layer_begin, x.dst_layer_begin, x.layer_count, x.src_head_begin, x.dst_head_begin, x.head_count});
+  }
+  *n_out = w.size();
+  if (!out) return KVBM_OK;
+  if (cap < w.size()) return fail(KVBM_ERR, "kvbm_tp_pp_scatter_plan: " + std::to_string(w.size()) + " windows do not fit in " + std::to_string(cap));
   std::copy(w.begin(), w.end(), out);
   return KVBM_OK;
   });
@@ -2105,6 +2301,17 @@ extern "C" int kvbm_manager_execute_repage_gather(kvbm_transfer_manager* m, size
   if (!m) return fail(KVBM_ERR, "null manager");
   const kvbm_repage_batch_seq q{token_begin, token_end, src_ids, n_src, dst_ids, n_dst};
   return execute_repage(m, num_srcs, srcs, dst, &q, 1, windows, num_windows, opts, out);
+  });
+}
+
+extern "C" int kvbm_manager_execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle src, const size_t* src_ids, size_t n_src,
+                                                   size_t num_dsts, const kvbm_layout_handle* dsts, const size_t* const* dst_ids, size_t n_dst,
+                                                   size_t token_begin, size_t token_end, const kvbm_scatter_window* windows,
+                                                   size_t num_windows, const kvbm_transfer_options* opts, kvbm_notification* out)
+{
+  return guarded([&]() -> int {
+  if (!m) return fail(KVBM_ERR, "null manager");
+  return execute_repage_scatter(m, src, src_ids, n_src, num_dsts, dsts, dst_ids, n_dst, token_begin, token_end, windows, num_windows, opts, out);
   });
 }
 

@@ -658,8 +658,10 @@ struct GatherParams {
   uint32_t shift[KVBM_GATHER_MAX_SOURCES];
 };
 
-// The stage of destination layer l (one of the launch's range): the first stage that ends past it.
-__host__ __device__ __forceinline__ const GatherStage& stage_of(const GatherParams& P, uint32_t l)
+// The stage of destination layer l (one of the launch's range): the first stage that ends past it.  The scatter's params
+// (ScatterParams) number their stages by source layer.
+template <class Params>
+__host__ __device__ __forceinline__ const GatherStage& stage_of(const Params& P, uint32_t l)
 {
   uint32_t k = 0;
   while (l >= P.stage[k].end) ++k;
@@ -746,9 +748,53 @@ __device__ __forceinline__ RepageUnit batch_unit(const kvbm_repage_unit* units, 
   return {w.x, w.y, w.z};
 }
 
+// Where 16 B vector vv of a re-paging head's run sits: its 16 B column c, its token's slot q in the big block, and the small
+// block (entry small_k + b of the small table) and slot that hold the same token.
+struct RepageAt {
+  uint32_t c, q, b, slot;
+};
+template <bool POW2, bool PPOW2>
+__device__ __forceinline__ RepageAt repage_at(const RepageGeom& G, const RowSplit& r, uint32_t q0, uint32_t vv)
+{
+  const uint32_t t = POW2 ? vv >> r.vpr : __umulhi(vv, r.magic);
+  const uint32_t c = POW2 ? vv & ((1u << r.vpr) - 1) : vv - t * r.vpr;
+  const uint32_t q = q0 + t;
+  const uint32_t b = PPOW2 ? q >> G.page.vpr : __umulhi(q, G.page.magic);
+  const uint32_t slot = PPOW2 ? q & (G.small_page - 1) : q - b * G.small_page;
+  return {c, q, b, slot};
+}
+
+// The vector's address on the big side (bh: the head's rows in the big block) and on the small side (sh: the head's rows in the
+// small side's (layer, outer) region, before the block offset; small block b is entry small_k + b of small_ids, RepageUnit).
+__device__ __forceinline__ const uint8_t* repage_big(const uint8_t* bh, uint32_t big_tok, uint32_t big_shift, const RepageAt& a)
+{
+  return bh + a.q * big_tok + (a.c << big_shift);
+}
+__device__ __forceinline__ const uint8_t* repage_small(const uint8_t* sh, const int32_t* small_ids, uint32_t small_k,
+                                                       uint64_t small_block_stride, uint32_t small_tok, uint32_t small_shift, const RepageAt& a)
+{
+  return sh + static_cast<uint64_t>(__ldg(small_ids + (small_k + a.b))) * small_block_stride + a.slot * small_tok + (a.c << small_shift);
+}
+
+// The load half of a re-paging walk: the IN 16 B loads of one vector.  The store half: the OUT 16 B stores of one vector as the
+// destination holds it -- the loaded vector itself without a cast, else cast_vector's result (bit for bit the paged permute's
+// cast), which a scatter computes once and stores to every destination of the vector.
+template <int IN>
+__device__ __forceinline__ void load_vector(const uint8_t* s, uint4 (&x)[IN])
+{
+#pragma unroll
+  for (int i = 0; i < IN; ++i) x[i] = ptx::ld_stream_v4(s + 16 * i);
+}
+template <int OUT>
+__device__ __forceinline__ void store_vector(const uint8_t* d, const uint4 (&y)[OUT])
+{
+#pragma unroll
+  for (int i = 0; i < OUT; ++i) ptx::st_stream_v4(const_cast<uint8_t*>(d) + 16 * i, y[i]);
+}
+
 // One head of a re-paging unit: its run of `run` 16 B vectors from slot q0 of the big block on.  bh: the head's rows in the
 // big block; sh: its rows in the small side's (layer, outer) region, before the block offset.  Small block b of the unit is
-// entry small_k + b of small_ids (RepageUnit).  Every re-paging kernel runs its heads through this loop.
+// entry small_k + b of small_ids (RepageUnit).  Every re-paging kernel but the scatter runs its heads through this loop.
 template <int CAST, bool POW2, bool SCALED, bool PPOW2>
 __device__ __forceinline__ void repage_head_rows(const uint8_t* bh, uint32_t big_tok, uint32_t big_shift, const uint8_t* sh,
                                                  const int32_t* small_ids, uint32_t small_k, uint64_t small_block_stride,
@@ -765,29 +811,22 @@ __device__ __forceinline__ void repage_head_rows(const uint8_t* bh, uint32_t big
 #pragma unroll
     for (int k = 0; k < U; ++k)
       if (v + k * 32 < run) {
-        const uint32_t vv = v + k * 32;
-        const uint32_t t = POW2 ? vv >> r.vpr : __umulhi(vv, r.magic);
-        const uint32_t c = POW2 ? vv & ((1u << r.vpr) - 1) : vv - t * r.vpr;
-        const uint32_t q = q0 + t;
-        const uint32_t b = PPOW2 ? q >> G.page.vpr : __umulhi(q, G.page.magic);
-        const uint32_t slot = PPOW2 ? q & (G.small_page - 1) : q - b * G.small_page;
-        const uint8_t* big_p = bh + q * big_tok + (c << big_shift);
-        const uint8_t* small_p = sh + static_cast<uint64_t>(__ldg(small_ids + (small_k + b))) * small_block_stride + slot * small_tok + (c << small_shift);
+        const RepageAt a = repage_at<POW2, PPOW2>(G, r, q0, v + k * 32);
+        const uint8_t* big_p = repage_big(bh, big_tok, big_shift, a);
+        const uint8_t* small_p = repage_small(sh, small_ids, small_k, small_block_stride, small_tok, small_shift, a);
         const uint8_t* s = G.src_small ? small_p : big_p;
         dp[k] = const_cast<uint8_t*>(G.src_small ? big_p : small_p);
-#pragma unroll
-        for (int i = 0; i < IN; ++i) x[k][i] = ptx::ld_stream_v4(s + 16 * i);
+        load_vector(s, x[k]);
       }
 #pragma unroll
     for (int k = 0; k < U; ++k)
       if (v + k * 32 < run) {
         if constexpr (CAST == KVBM_CAST_NONE) {
-          ptx::st_stream_v4(dp[k], x[k][0]);
+          store_vector(dp[k], x[k]);
         } else {
           uint4 y[OUT];
-          cast_vector<SCALED>(x[k], y, scale);  // bit for bit the paged permute's cast
-#pragma unroll
-          for (int i = 0; i < OUT; ++i) ptx::st_stream_v4(dp[k] + 16 * i, y[i]);
+          cast_vector<SCALED>(x[k], y, scale);
+          store_vector(dp[k], y);
         }
       }
   }
@@ -892,6 +931,111 @@ kvbm_paged_batch_repage_gather_kernel(const __grid_constant__ RepageGatherParams
   const uint32_t rem = unit - j * (G.nlayers * G.no);
   const uint32_t l = G.layer_begin + rem / G.no;
   repage_gather_unit<CAST, POW2, SCALED, PPOW2, true>(P, stage_of(P.g, l), j, l, rem % G.no, r, scales, units);
+}
+
+// The re-paging scatter, the gather's mirror image: ONE source pool of page Ps (a prefill rank) into up to
+// KVBM_GATHER_MAX_SOURCES targets of page Pd, each a destination pool's side with its own format, table and head count, one head
+// window and one layer window; a pool may appear in several targets.  Targets with one source layer window form a stage; the
+// stages ascend in source layers and tile the launch's (source) layer range.  The covered source heads of every stage are numbered
+// entry 0 .. entries-1, stage by stage in ascending head order: head[k] is entry k's source head, and pairs pair_first[k] ..
+// pair_first[k + 1] - 1 its (target, destination head) pairs, pair_tgt[p] naming the target, whose destination head is the source
+// head plus head_delta and whose destination layer the source layer plus shift (both modulo 2^32).
+struct ScatterTarget {
+  PermuteSide D;
+  uint32_t shift, head_delta;
+};
+struct ScatterParams {
+  PermuteSide S;
+  ScatterTarget tgt[KVBM_GATHER_MAX_SOURCES];
+  RepageGeom geo;
+  GatherStage stage[KVBM_GATHER_MAX_SOURCES];  // begin / end: source layers; first / count: entries
+  uint32_t head[KVBM_GATHER_MAX_HEADS];
+  uint16_t pair_first[KVBM_GATHER_MAX_HEADS + 1];
+  uint8_t pair_tgt[KVBM_GATHER_MAX_HEADS];
+};
+
+// One covered source head (entry k) of a scatter unit (big block j, source layer l, outer o): the re-paging walk's load half reads
+// each 16 B vector ONCE and casts it once, and its store half writes it to every (target, destination head) pair of the entry,
+// each at its own layer.  With Ps >= Pd block j is the source's and each target finds the vector's small block in its own table;
+// with Ps < Pd block j is entry j of every target's table (they share Pd and the range).
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__device__ __forceinline__ void scatter_head_rows(const ScatterParams& P, uint32_t k, uint32_t j, uint32_t l, uint32_t o, const RepageUnit& u,
+                                                  uint32_t run, const RowSplit& r, const ptx::Scale& scale)
+{
+  constexpr int IN = CAST == KVBM_CAST_BF16_TO_FP8E4M3 ? 2 : 1;
+  constexpr int OUT = CAST == KVBM_CAST_FP8E4M3_TO_BF16 ? 2 : 1;
+  constexpr int U = 8 / IN;
+  const RepageGeom& G = P.geo;
+  const PermuteSide& S = P.S;
+  const bool ss = G.src_small;
+  const uint32_t big_shift = ss ? 3 + OUT : 3 + IN, small_shift = ss ? 3 + IN : 3 + OUT;
+  const uint32_t h = P.head[k], p0 = P.pair_first[k], p1 = P.pair_first[k + 1];
+  const uint8_t* sh = (ss ? side_region(S, l, o) : side_block(S, j, l, o)) + h * S.head_stride;
+  const int lane = threadIdx.x & 31;
+  for (uint32_t v = lane; v < run; v += U * 32) {
+    uint4 x[U][IN];
+#pragma unroll
+    for (int i = 0; i < U; ++i)
+      if (v + i * 32 < run) {
+        const RepageAt a = repage_at<POW2, PPOW2>(G, r, u.q0, v + i * 32);
+        load_vector(ss ? repage_small(sh, S.ids, u.small_k, S.block_stride, static_cast<uint32_t>(S.tok_stride), small_shift, a)
+                       : repage_big(sh, static_cast<uint32_t>(S.tok_stride), big_shift, a),
+                    x[i]);
+      }
+#pragma unroll
+    for (int i = 0; i < U; ++i)
+      if (v + i * 32 < run) {
+        const RepageAt a = repage_at<POW2, PPOW2>(G, r, u.q0, v + i * 32);
+        uint4 y[OUT];
+        if constexpr (CAST == KVBM_CAST_NONE)
+          y[0] = x[i][0];
+        else
+          cast_vector<SCALED>(x[i], y, scale);
+#pragma unroll 1
+        for (uint32_t p = p0; p < p1; ++p) {
+          const ScatterTarget& T = P.tgt[P.pair_tgt[p]];
+          const PermuteSide& D = T.D;
+          const uint32_t dl = l + T.shift;
+          const uint8_t* dh = (ss ? side_block(D, j, dl, o) : side_region(D, dl, o)) + (h + T.head_delta) * D.head_stride;
+          store_vector(ss ? repage_big(dh, static_cast<uint32_t>(D.tok_stride), big_shift, a)
+                          : repage_small(dh, D.ids, u.small_k, D.block_stride, static_cast<uint32_t>(D.tok_stride), small_shift, a),
+                       y);
+        }
+      }
+  }
+}
+
+// One CTA per (big block j, source layer l, outer o) unit, clipped to the range, as the re-paging gather; one warp per covered
+// source head of l's stage, looping by the CTA's warps past 8.  SCALED: the SOURCE's scales[l * no + o], loaded once per unit.
+// The re-paging gathers' bound: three CTAs per SM.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__global__ void __launch_bounds__(256, 3)
+kvbm_paged_repage_scatter_kernel(const __grid_constant__ ScatterParams P, RowSplit r, const float* scales)
+{
+  const RepageGeom& G = P.geo;
+  const uint32_t unit = blockIdx.x;  // (big block j * nlayers + l) * no + o
+  const uint32_t j = unit / (G.nlayers * G.no);
+  const uint32_t rem = unit - j * (G.nlayers * G.no);
+  const uint32_t l = G.layer_begin + rem / G.no, o = rem % G.no;
+  const GatherStage& T = stage_of(P, l);
+  const RepageUnit u = repage_unit(G, j);
+  const ptx::Scale scale = ptx::make_scale(SCALED ? __ldg(scales + l * G.no + o) : 1.f);
+  const uint32_t run = row_run<POW2>(r, u.tokens);
+  const uint32_t end = T.first + T.count;
+  for (uint32_t k = T.first + (threadIdx.x >> 5); k < end; k += blockDim.x >> 5)
+    scatter_head_rows<CAST, POW2, SCALED, PPOW2>(P, k, j, l, o, u, run, r, scale);
+}
+
+// The scatter's signal after its launch: every target's done flag (epoch) and the completion word, system scope.
+struct ScatterFlags {
+  uint32_t* done[KVBM_GATHER_MAX_SOURCES];
+};
+__global__ void kvbm_scatter_signal_kernel(const ScatterFlags F, int n, uint32_t epoch, uint32_t* completion, uint32_t completion_value)
+{
+  __threadfence_system();
+  for (int t = 0; t < n; ++t)
+    if (F.done[t]) ptx::st_release_sys(F.done[t], epoch);
+  if (completion) ptx::st_release_sys(completion, completion_value);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1215,8 +1359,11 @@ static cudaError_t preload_kernels()
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_batch_repage_gather_kernel<c, p, sc, false>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_batch_repage_gather_kernel<c, p, sc, true>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_batch_repage_gather_kernel<c, p, sc, false>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_scatter_kernel<c, p, sc, true>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_scatter_kernel<c, p, sc, false>);
         });
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_layer_signal_kernel);
+  if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_scatter_signal_kernel);
   return e;
 }
 
@@ -1709,6 +1856,151 @@ static cudaError_t launch_paged_repage_gather(const kvbm_stage_source* srcs, int
   return launched(stream, done_flag, epoch, completion_flag, completion_value);
 }
 
+// The scatter's signal launch: every target's done flag and the completion word, none when all are null.
+static cudaError_t scatter_signal(const kvbm_scatter_target* targets, int num_targets, uint32_t epoch, uint32_t* completion_flag,
+                                  uint32_t completion_value, cudaStream_t stream)
+{
+  ScatterFlags F{};
+  bool any = completion_flag != nullptr;
+  for (int t = 0; t < num_targets; ++t) any |= (F.done[t] = targets[t].done_flag) != nullptr;
+  if (!any) return cudaSuccess;
+  kvbm_scatter_signal_kernel<<<1, 1, 0, stream>>>(F, num_targets, epoch, completion_flag, completion_value);
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  return cudaGetLastError();
+}
+
+static bool spans_overlap(uint64_t a, uint64_t na, uint64_t b, uint64_t nb) { return a < b + nb && b < a + na; }
+
+// The targets of a scatter from a source of src_nh heads and src_nl layers over source layers [lb, le), into P->tgt, P->stage and
+// the entry / pair tables: each target's side (region Pd * its heads * dst_row, the source's outer_dim, its strides over its own
+// layers), a non-empty head window and layer window inside both sides, stages whose source layer windows are equal or disjoint
+// and tile [lb, le), at most KVBM_GATHER_MAX_HEADS pairs, and no two targets on one pool and table whose destination (layer,
+// head) rectangles overlap.  *widest: the most entries of one stage.
+static bool fill_scatter_targets(const kvbm_scatter_target* tg, int n, uint32_t src_nh, uint32_t src_nl, uint32_t no, int lb, int le,
+                                 uint32_t dst_page, uint64_t dst_row, ScatterParams* P, uint32_t* widest)
+{
+  int stage_of_tgt[KVBM_GATHER_MAX_SOURCES];
+  int num_stages = 0;
+  GatherStage* T = P->stage;
+  uint32_t pairs = 0;
+  for (int t = 0; t < n; ++t) {
+    const kvbm_scatter_target& X = tg[t];
+    const kvbm_paged_layout& L = X.side.layout;
+    if (!X.side.block_ids || !L.layer_base || L.outer_dim != no) return false;
+    if (static_cast<uint64_t>(dst_page) * X.num_heads * dst_row != L.region_bytes) return false;
+    if (!fill_permute_side(X.side, L.num_layers, no, X.num_heads, dst_page, static_cast<uint32_t>(dst_row), &P->tgt[t].D)) return false;
+    if (X.head_count == 0 || static_cast<uint64_t>(X.src_head_begin) + X.head_count > src_nh ||
+        static_cast<uint64_t>(X.dst_head_begin) + X.head_count > X.num_heads)
+      return false;
+    const uint64_t src_end = static_cast<uint64_t>(X.src_layer_begin) + X.layer_count;
+    if (X.layer_count == 0 || src_end > src_nl || static_cast<uint64_t>(X.dst_layer_begin) + X.layer_count > L.num_layers) return false;
+    if ((pairs += X.head_count) > KVBM_GATHER_MAX_HEADS) return false;
+    int k = 0;
+    while (k < num_stages && !(T[k].begin == X.src_layer_begin && T[k].end == src_end)) {
+      if (X.src_layer_begin < T[k].end && T[k].begin < src_end) return false;  // a partial overlap
+      ++k;
+    }
+    if (k == num_stages) T[num_stages++] = GatherStage{X.src_layer_begin, static_cast<uint32_t>(src_end), 0, 0, 0};
+    stage_of_tgt[t] = k;
+    for (int u = 0; u < t; ++u) {
+      const kvbm_scatter_target& Y = tg[u];
+      if (Y.side.layout.layer_base == L.layer_base && Y.side.block_ids == X.side.block_ids &&
+          spans_overlap(X.dst_layer_begin, X.layer_count, Y.dst_layer_begin, Y.layer_count) &&
+          spans_overlap(X.dst_head_begin, X.head_count, Y.dst_head_begin, Y.head_count))
+        return false;
+    }
+    P->tgt[t].shift = X.dst_layer_begin - X.src_layer_begin;
+    P->tgt[t].head_delta = X.dst_head_begin - X.src_head_begin;
+  }
+  // ascending source layers (insertion sort of at most 16), then the range must be tiled
+  int order[KVBM_GATHER_MAX_SOURCES];
+  for (int k = 0; k < num_stages; ++k) {
+    int at = k;
+    while (at > 0 && T[order[at - 1]].begin > T[k].begin) {
+      order[at] = order[at - 1];
+      --at;
+    }
+    order[at] = k;
+  }
+  uint32_t reached = static_cast<uint32_t>(lb);
+  for (int i = 0; i < num_stages; ++i)
+    if (T[order[i]].begin <= reached && T[order[i]].end > reached) reached = T[order[i]].end;
+  if (reached < static_cast<uint32_t>(le)) return false;
+  // per stage: its (source head, target) pairs in ascending head, then target order, one entry per head
+  GatherStage sorted[KVBM_GATHER_MAX_SOURCES] = {};
+  uint32_t entries = 0, p = 0;
+  *widest = 0;
+  for (int i = 0; i < num_stages; ++i) {
+    GatherStage& S = sorted[i] = T[order[i]];
+    S.first = entries;
+    uint32_t hs[KVBM_GATHER_MAX_HEADS];
+    uint8_t ts[KVBM_GATHER_MAX_HEADS];
+    uint32_t m = 0;
+    for (int t = 0; t < n; ++t) {
+      if (stage_of_tgt[t] != order[i]) continue;
+      for (uint32_t h = tg[t].src_head_begin; h < tg[t].src_head_begin + tg[t].head_count; ++h) {
+        uint32_t at = m++;
+        while (at > 0 && hs[at - 1] > h) {  // stable: a head's pairs stay in target order
+          hs[at] = hs[at - 1];
+          ts[at] = ts[at - 1];
+          --at;
+        }
+        hs[at] = h;
+        ts[at] = static_cast<uint8_t>(t);
+      }
+    }
+    for (uint32_t a = 0; a < m; ++a, ++p) {
+      if (a == 0 || hs[a] != hs[a - 1]) {
+        P->head[entries] = hs[a];
+        P->pair_first[entries++] = static_cast<uint16_t>(p);
+      }
+      P->pair_tgt[p] = ts[a];
+    }
+    S.count = entries - S.first;
+    *widest = std::max(*widest, S.count);
+  }
+  P->pair_first[entries] = static_cast<uint16_t>(p);
+  std::copy(sorted, sorted + KVBM_GATHER_MAX_SOURCES, T);
+  return true;
+}
+
+// The scatter: every check before any CUDA call (the empty-range signal after the cast, range and target-count rules, as the
+// re-paging gather), then one kvbm_paged_repage_scatter_kernel launch and the signal.
+static cudaError_t launch_paged_repage_scatter(const kvbm_permute_side* src, uint32_t src_num_heads, uint32_t src_page,
+                                               const kvbm_scatter_target* targets, int num_targets, uint32_t dst_page, uint32_t token_begin,
+                                               uint32_t token_end, int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode,
+                                               const float* cast_scales, uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value,
+                                               cudaStream_t stream)
+{
+  if (layer_begin < 0 || layer_end < layer_begin || token_end < token_begin) return cudaErrorInvalidValue;
+  if (!cast_args_ok(cast_mode, cast_scales)) return cudaErrorInvalidValue;
+  if (!targets || num_targets < 1 || num_targets > KVBM_GATHER_MAX_SOURCES) return cudaErrorInvalidValue;
+  if (token_end == token_begin || layer_end == layer_begin)
+    return scatter_signal(targets, num_targets, epoch, completion_flag, completion_value, stream);
+  if (!src || !src->block_ids || !src->layout.layer_base) return cudaErrorInvalidValue;
+  const uint32_t nl = src->layout.num_layers, no = src->layout.outer_dim;
+  if (nl == 0 || no == 0 || static_cast<uint32_t>(layer_end) > nl) return cudaErrorInvalidValue;
+  ScatterParams P{};
+  RowSplit r;
+  uint64_t dst_row_bytes, units;
+  bool page_pow2;
+  if (!repage_geometry(src_page, dst_page, token_begin, token_end, layer_begin, layer_end, no, src_row_bytes, cast_mode, &P.geo, &r,
+                       &dst_row_bytes, &units, &page_pow2))
+    return cudaErrorInvalidValue;
+  if (static_cast<uint64_t>(src_page) * src_num_heads * src_row_bytes != src->layout.region_bytes) return cudaErrorInvalidValue;
+  if (!fill_permute_side(*src, nl, no, src_num_heads, src_page, src_row_bytes, &P.S)) return cudaErrorInvalidValue;
+  uint32_t widest;
+  if (!fill_scatter_targets(targets, num_targets, src_num_heads, nl, no, layer_begin, layer_end, dst_page, dst_row_bytes, &P, &widest))
+    return cudaErrorInvalidValue;
+  const int threads = static_cast<int>(std::min<uint32_t>(8, widest)) * 32;
+  with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, page_pow2, [&](auto c, auto p, auto sc, auto pp) {
+    kvbm_paged_repage_scatter_kernel<c, p, sc, pp><<<static_cast<unsigned>(units), threads, 0, stream>>>(P, r, cast_scales);
+  });
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  const cudaError_t e = cudaGetLastError();
+  return e != cudaSuccess ? e : scatter_signal(targets, num_targets, epoch, completion_flag, completion_value, stream);
+}
+
 }  // namespace kvbm
 
 using namespace kvbm;
@@ -2021,6 +2313,16 @@ kvbm_kernels_paged_stage_repage_gather_batch_streamed(const kvbm_stage_source* s
   return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, 0, 0, layer_begin, layer_end,
                                     src_row_bytes, cast_mode, cast_scales, st->done_flag, st->epoch, st->completion_flag,
                                     st->completion_value, KVBM_GATHER_MAX_HEADS, stream, st, &B);
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_repage_scatter(const kvbm_permute_side* src, uint32_t src_num_heads, uint32_t src_page_size, const kvbm_scatter_target* targets,
+                                  int num_targets, uint32_t dst_page_size, uint32_t token_begin, uint32_t token_end, int layer_begin,
+                                  int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales, uint32_t epoch,
+                                  uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
+{
+  return launch_paged_repage_scatter(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, token_begin, token_end, layer_begin,
+                                     layer_end, src_row_bytes, cast_mode, cast_scales, epoch, completion_flag, completion_value, stream);
 }
 
 extern "C" cudaError_t

@@ -120,6 +120,14 @@ class RepageUnit(C.Structure):
     _fields_ = [("q0", C.c_uint32), ("tokens", C.c_uint32), ("small_k", C.c_uint32), ("seq", C.c_uint32)]
 
 
+class ScatterTarget(C.Structure):
+    """struct kvbm_scatter_target: one target of `paged_repage_scatter` (a destination side, its head count, one head window, one
+    layer window and its nullable done flag)"""
+    _fields_ = [("side", PermuteSide), ("num_heads", C.c_uint32), ("src_head_begin", C.c_uint32), ("dst_head_begin", C.c_uint32),
+                ("head_count", C.c_uint32), ("src_layer_begin", C.c_uint32), ("dst_layer_begin", C.c_uint32), ("layer_count", C.c_uint32),
+                ("done_flag", C.c_void_p)]
+
+
 GATHER_MAX_SOURCES = 16      # KVBM_GATHER_MAX_SOURCES
 GATHER_MAX_HEADS = 256       # KVBM_GATHER_MAX_HEADS
 
@@ -247,6 +255,10 @@ def lib() -> C.CDLL:
                                                                             C.c_uint32, C.c_uint32, vp, sz, vp, sz, i, i, C.c_uint32, i, vp,
                                                                             C.POINTER(PermuteStream), vp]
         L.kvbm_kernels_paged_stage_repage_gather_batch_streamed.restype = i
+        L.kvbm_kernels_paged_repage_scatter.argtypes = [C.POINTER(PermuteSide), C.c_uint32, C.c_uint32, C.POINTER(ScatterTarget), i,
+                                                        C.c_uint32, C.c_uint32, C.c_uint32, i, i, C.c_uint32, i, vp, C.c_uint32, vp,
+                                                        C.c_uint32, vp]
+        L.kvbm_kernels_paged_repage_scatter.restype = i
         L.kvbm_kernels_permute_strides.argtypes = [i, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64, C.c_uint64,
                                                    C.POINTER(C.c_uint64)]
         L.kvbm_kernels_permute_strides.restype = i
@@ -274,7 +286,7 @@ EXPORTED_SYMBOLS = [
     "kvbm_kernels_paged_repage_gather_streamed", "kvbm_kernels_paged_stage_gather", "kvbm_kernels_paged_stage_gather_streamed",
     "kvbm_kernels_paged_stage_repage_gather", "kvbm_kernels_paged_stage_repage_gather_streamed",
     "kvbm_kernels_repage_batch_units", "kvbm_kernels_paged_stage_repage_gather_batch",
-    "kvbm_kernels_paged_stage_repage_gather_batch_streamed",
+    "kvbm_kernels_paged_stage_repage_gather_batch_streamed", "kvbm_kernels_paged_repage_scatter",
 ]
 
 
@@ -549,6 +561,19 @@ def paged_stage_repage_gather_batch_streamed(srcs: Sequence[StageSource], src_pa
                                                                        units or None, num_units, layer_begin, layer_end, src_row_bytes,
                                                                        int(cast_mode), scales_ptr(cast_scales),
                                                                        C.byref(st) if st is not None else None, stream)
+
+
+def paged_repage_scatter(src: PermuteSide, src_num_heads: int, src_page_size: int, targets: Sequence[ScatterTarget], dst_page_size: int,
+                         token_begin: int, token_end: int, layer_begin: int, layer_end: int, src_row_bytes: int, cast_mode: int = 0,
+                         cast_scales=None, epoch: int = 0, completion_flag: int = 0, completion_value: int = 0, stream: int = 0) -> int:
+    """One source (its block_ids = its table[token_begin // Ps .. ceil(token_end / Ps))) into every target in ONE launch: each
+    target's head window of the source's layer window lands in its destination at its own heads and layers, every source vector
+    read once and cast once; the layer range and `cast_scales` count SOURCE layers.  Then every target's done flag (epoch) and the
+    completion word are written once.  include/kvbm_kernels.h (kvbm_kernels_paged_repage_scatter)."""
+    arr = (ScatterTarget * max(1, len(targets)))(*targets)
+    return lib().kvbm_kernels_paged_repage_scatter(C.byref(src), src_num_heads, src_page_size, arr, len(targets), dst_page_size, token_begin,
+                                                   token_end, layer_begin, layer_end, src_row_bytes, int(cast_mode), scales_ptr(cast_scales),
+                                                   epoch, completion_flag or None, completion_value, stream)
 
 
 def permute_strides(kv_layout: int, num_layers: int, outer_dim: int, num_heads: int, page_size: int, row_bytes: int,

@@ -123,6 +123,11 @@ class _CShardWindow(C.Structure):
                                           "dst_head_begin", "head_count")]
 
 
+class _CScatterWindow(C.Structure):
+    _fields_ = [(n, C.c_size_t) for n in ("dst_rank", "src_layer_begin", "dst_layer_begin", "layer_count", "src_head_begin", "dst_head_begin",
+                                          "head_count")]
+
+
 class _CRepageBatchSeq(C.Structure):
     """struct kvbm_repage_batch_seq"""
     _fields_ = [("token_begin", C.c_size_t), ("token_end", C.c_size_t), ("src_ids", C.c_void_p), ("n_src", C.c_size_t),
@@ -249,7 +254,7 @@ EXPORTED_SYMBOLS = [
     "kvbm_mc_group_destroy", "kvbm_tp_reshard_plan", "kvbm_manager_execute_gather", "kvbm_manager_execute_repage",
     "kvbm_manager_execute_repage_gather", "kvbm_manager_execute_gather_streamed", "kvbm_manager_execute_repage_gather_streamed",
     "kvbm_tp_pp_reshard_plan", "kvbm_manager_execute_stage_gather", "kvbm_manager_execute_stage_repage_gather",
-    "kvbm_manager_execute_repage_batch",
+    "kvbm_manager_execute_repage_batch", "kvbm_tp_pp_scatter_plan", "kvbm_manager_execute_repage_scatter",
 ]
 
 
@@ -312,6 +317,9 @@ def lib() -> C.CDLL:
                                                                P(_CLayerStream), P(_COptions), P(u64)]
         L.kvbm_manager_execute_repage_batch.argtypes = [vp, sz, P(u64), u64, P(_CRepageBatchSeq), sz, P(_CShardWindow), sz, P(_CLayerStream),
                                                         P(_COptions), P(u64)]
+        L.kvbm_tp_pp_scatter_plan.argtypes = [sz, sz, sz, sz, P(sz), sz, sz, P(sz), sz, P(_CScatterWindow), sz, P(sz)]
+        L.kvbm_manager_execute_repage_scatter.argtypes = [vp, u64, vp, sz, sz, P(u64), P(P(sz)), sz, sz, sz, P(_CScatterWindow), sz,
+                                                          P(_COptions), P(u64)]
         L.kvbm_notification_is_complete.argtypes = [vp, u64]
         L.kvbm_notification_wait.argtypes = [vp, u64, C.c_int64]
         L.kvbm_manager_bytes_moved.argtypes = [vp]
@@ -479,6 +487,41 @@ def tp_pp_reshard_plan(num_kv_heads: int, num_layers: int, src_tp: int, src_pp: 
     out = (_CShardWindow * max(1, n.value))()
     _check(lib().kvbm_tp_pp_reshard_plan(*args, out, n.value, C.byref(n)))
     return [ShardWindow(w.src_rank, w.src_layer_begin, w.dst_layer_begin, w.layer_count, w.src_head_begin, w.dst_head_begin, w.head_count)
+            for w in out[:n.value]]
+
+
+@dataclass(frozen=True)
+class ScatterWindow:
+    """One entry of a scatter plan: heads [src_head_begin, +head_count) of layers [src_layer_begin, +layer_count) of the prefill
+    rank's blocks are heads [dst_head_begin, +head_count) of layers [dst_layer_begin, +layer_count) of decode rank dst_rank's blocks
+    (stage-local layers, rank-local heads)."""
+    dst_rank: int
+    src_layer_begin: int
+    dst_layer_begin: int
+    layer_count: int
+    src_head_begin: int
+    dst_head_begin: int
+    head_count: int
+
+
+def tp_pp_scatter_plan(num_kv_heads: int, num_layers: int, src_tp: int, src_pp: int, dst_tp: int, dst_pp: int, src_rank: int,
+                       src_stage_layers: Optional[Sequence[int]] = None,
+                       dst_stage_layers: Optional[Sequence[int]] = None) -> List[ScatterWindow]:
+    """Which layers and heads of prefill rank `src_rank` go to which decode rank (kvbm_tp_pp_scatter_plan, include/kvbm_physical.h):
+    the windows of `tp_pp_reshard_plan` over every decode rank that read `src_rank`, tagged with their decode rank, in ascending
+    (dst_rank, destination layer, destination head) order, so the push and pull plans of one group move the same bytes."""
+    def parts(v):
+        return None if v is None else (C.c_size_t * max(1, len(v)))(*[int(x) for x in v])
+    sp, dp = parts(src_stage_layers), parts(dst_stage_layers)
+    for v, pp in ((src_stage_layers, src_pp), (dst_stage_layers, dst_pp)):
+        if v is not None and len(v) != pp:
+            raise ValueError(f"{len(v)} stage layer counts for PP {pp}")
+    n = C.c_size_t()
+    args = (num_kv_heads, num_layers, src_tp, src_pp, sp, dst_tp, dst_pp, dp, src_rank)
+    _check(lib().kvbm_tp_pp_scatter_plan(*args, None, 0, C.byref(n)))
+    out = (_CScatterWindow * max(1, n.value))()
+    _check(lib().kvbm_tp_pp_scatter_plan(*args, out, n.value, C.byref(n)))
+    return [ScatterWindow(w.dst_rank, w.src_layer_begin, w.dst_layer_begin, w.layer_count, w.src_head_begin, w.dst_head_begin, w.head_count)
             for w in out[:n.value]]
 
 
@@ -857,6 +900,36 @@ class TransferManager:
         o = (options or TransferOptions())._c()
         _check(lib().kvbm_manager_execute_repage_batch(self._h, len(ranks), hs, dst, cs, len(seqs), ws, len(plan),
                                                        C.byref(ls) if ls is not None else None, C.byref(o), C.byref(tok)))
+        return TransferCompleteNotification(self, tok.value)
+
+    def execute_repage_scatter(self, src: int, src_block_ids: Sequence[int], dsts: Sequence[int], dst_block_ids: Sequence[Sequence[int]],
+                               plan: Sequence[ScatterWindow], tokens: range,
+                               options: Optional[TransferOptions] = None) -> TransferCompleteNotification:
+        """One prefill rank's KV to every decode rank that needs it, as ONE hand-off (kvbm_manager_execute_repage_scatter): heads and
+        layers of `src` land in `dsts[w.dst_rank]` as each plan entry says (`tp_pp_scatter_plan` passes as it is), over `tokens`.
+        `src_block_ids` is the source table's entries tokens.start // Ps .. ceil(tokens.stop / Ps), `dst_block_ids[d]` destination
+        d's for its page Pd (one Pd for every destination).  Each source vector is read once and cast once, however many windows
+        take it.  The options' layer range and cast scales count SOURCE layers; `options.per_dst_done_flags` is indexed like
+        `dsts`; `options.done_flag` and the notification complete once, after every destination landed."""
+        if tokens.step != 1:
+            raise ValueError("tokens must be a range with step 1")
+        if len(dst_block_ids) != len(dsts):
+            raise ValueError(f"{len(dst_block_ids)} destination id lists for {len(dsts)} destinations")
+        s, ns = _size_array(src_block_ids)
+        n_dst = len(dst_block_ids[0]) if dsts else 0
+        if any(len(x) != n_dst for x in dst_block_ids):
+            raise KvbmError(ErrorCode.LENGTH_MISMATCH, "the destinations' block id lists have different lengths")
+        hs = (C.c_uint64 * max(1, len(dsts)))(*dsts)
+        d_arrays = [_size_array(x)[0] for x in dst_block_ids]
+        PP = C.POINTER(C.c_size_t)
+        as_ptr = lambda a: a._as_parameter_ if isinstance(a, _NpView) else C.cast(a, PP)  # noqa: E731
+        dp = (PP * max(1, len(dsts)))(*[as_ptr(a) for a in d_arrays])
+        ws = (_CScatterWindow * max(1, len(plan)))(*[_CScatterWindow(w.dst_rank, w.src_layer_begin, w.dst_layer_begin, w.layer_count,
+                                                                     w.src_head_begin, w.dst_head_begin, w.head_count) for w in plan])
+        tok = C.c_uint64()
+        o = (options or TransferOptions())._c()
+        _check(lib().kvbm_manager_execute_repage_scatter(self._h, src, s.addr if type(s) is _NpView else s, ns, len(dsts), hs, dp, n_dst,
+                                                         tokens.start, tokens.stop, ws, len(plan), C.byref(o), C.byref(tok)))
         return TransferCompleteNotification(self, tok.value)
 
     def execute_fanout(self, src: int, dsts: Sequence[int], src_block_ids: Sequence[Sequence[int]],

@@ -513,6 +513,43 @@ cudaError_t kvbm_kernels_paged_stage_repage_gather_batch_streamed(const kvbm_sta
                                                                   const float* cast_scales, const kvbm_permute_stream* st,
                                                                   cudaStream_t stream);
 
+/* ---- the re-paging scatter: one prefill rank's KV to every decode rank that needs it ------------------------------------------
+ * The mirror image of kvbm_kernels_paged_stage_repage_gather: ONE source pool writes into up to KVBM_GATHER_MAX_SOURCES targets.
+ * A target is one destination pool's side plus one head window (source heads [src_head_begin, +head_count) land as destination
+ * heads [dst_head_begin, +head_count)) and one layer window (source layers [src_layer_begin, +layer_count) land as destination
+ * layers [dst_layer_begin, +layer_count)); a pool may appear in several targets.  Targets with equal source layer windows form a
+ * stage.  side.block_ids holds the target's table[token_begin / Pd .. ceil(token_end / Pd)); side.layout.num_layers is the pool's
+ * own.  done_flag (nullable) receives epoch with system scope once the launch's bytes landed; targets of one pool may share it. */
+typedef struct kvbm_scatter_target {
+  kvbm_permute_side side;   /* destination pool, format, table for Pd over the range */
+  uint32_t num_heads;       /* this destination's heads per block (its region_bytes = Pd * num_heads * its row) */
+  uint32_t src_head_begin, dst_head_begin, head_count;
+  uint32_t src_layer_begin, dst_layer_begin, layer_count;
+  uint32_t* done_flag;      /* nullable */
+} kvbm_scatter_target;
+
+/* One source (src: its pool, format and table[token_begin / Ps .. ceil(token_end / Ps)), src_num_heads heads per block, page Ps)
+ * into num_targets targets of one page Pd, in ONE launch, then one signal launch that writes every target's done_flag and
+ * completion_flag (completion_value).  Each 16 B source vector is loaded once and cast once, then stored to every target of its
+ * layer's stage that covers its head: replicated heads (dst_tp > num_kv_heads, MLA's one latent head) are read once.  The
+ * destination bytes equal those of num_targets separate kvbm_kernels_paged_stage_repage_gather launches, bit for bit: launch t has
+ * the source as its one stage source with target t's windows, over the destination image of source layers [layer_begin,
+ * layer_end) under t's layer window, with cast_scales re-indexed to destination layers.  Every other destination byte keeps its
+ * value.  The token range, the cast and src_row_bytes are shared; layer_begin / layer_end count SOURCE layers, and cast_scales
+ * (nullable) is the SOURCE's float[src num_layers * outer_dim], indexed by the source layer and outer index.
+ * cudaErrorInvalidValue, before any CUDA call, for: every page, range, row, stride and cast rule of
+ * kvbm_kernels_paged_stage_repage_gather; num_targets outside 1..KVBM_GATHER_MAX_SOURCES; an empty head or layer window, or one
+ * past the source's or its destination's heads or layers; two stages whose source layer windows overlap without being equal; a
+ * source layer of [layer_begin, layer_end) that no stage covers; more than KVBM_GATHER_MAX_HEADS (target, head) pairs over all
+ * stages; two targets with the same side.layout.layer_base and side.block_ids pointers whose destination (layer, head) rectangles
+ * overlap.  The entry cannot read device ids, so for targets that share a pool through different tables, keeping their
+ * destination blocks disjoint is the caller's rule.  An empty token or layer range moves nothing and still signals. */
+cudaError_t kvbm_kernels_paged_repage_scatter(const kvbm_permute_side* src, uint32_t src_num_heads, uint32_t src_page_size,
+                                              const kvbm_scatter_target* targets, int num_targets, uint32_t dst_page_size,
+                                              uint32_t token_begin, uint32_t token_end, int layer_begin, int layer_end,
+                                              uint32_t src_row_bytes, int cast_mode, const float* cast_scales, uint32_t epoch,
+                                              uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream);
+
 /* Host-only (no GPU): the stride table kvbm_kernels_paged_permute walks with for one side.  out[0] = 1 when offsets count
  * from the block's first byte (universal formats) or 0 when they count from the (layer, outer) region's first byte; the
  * element (layer l, outer o, head h, token t) then sits at  [out[0] ? l * out[1] + o * out[2] : 0] + h * out[3] + t * out[4].

@@ -198,6 +198,22 @@ int kvbm_tp_pp_reshard_plan(size_t num_kv_heads, size_t num_layers, size_t src_t
                             size_t dst_tp, size_t dst_pp, const size_t* dst_stage_layers, size_t dst_rank, kvbm_shard_window* out,
                             size_t cap, size_t* n_out);
 
+/* One entry of a scatter plan: heads [src_head_begin, +head_count) of layers [src_layer_begin, +layer_count) of the prefill rank's
+ * blocks are heads [dst_head_begin, +head_count) of layers [dst_layer_begin, +layer_count) of decode rank dst_rank's blocks
+ * (stage-local layers, rank-local heads, as kvbm_shard_window). */
+typedef struct kvbm_scatter_window {
+  size_t dst_rank, src_layer_begin, dst_layer_begin, layer_count, src_head_begin, dst_head_begin, head_count;
+} kvbm_scatter_window;
+/* The push side of kvbm_tp_pp_reshard_plan: which layers and heads of prefill rank src_rank go to which decode rank.  Defined as
+ * the inverse of the gather plans: exactly the windows with that src_rank of kvbm_tp_pp_reshard_plan over every decode rank, each
+ * tagged with its decode rank, in ascending (dst_rank, destination layer, destination head) order.  Replicated heads follow the
+ * gather plan's replica rule (replica dst_rank % replicas), so the push and pull plans of one group move the same bytes.  The
+ * arguments, errors and count / cap convention are kvbm_tp_pp_reshard_plan's, with KVBM_ERR_RANGE for src_rank >= src_pp * src_tp
+ * in place of its dst_rank rule.  Pure host logic. */
+int kvbm_tp_pp_scatter_plan(size_t num_kv_heads, size_t num_layers, size_t src_tp, size_t src_pp, const size_t* src_stage_layers,
+                            size_t dst_tp, size_t dst_pp, const size_t* dst_stage_layers, size_t src_rank, kvbm_scatter_window* out,
+                            size_t cap, size_t* n_out);
+
 /* ---- TransferManager ---- */
 /* cuda_device_id < 0: host-only manager (Memcpy strategy only; every CUDA strategy returns KVBM_ERR_CUDA). */
 int kvbm_manager_create(int cuda_device_id, uint64_t worker_id, kvbm_transfer_manager** out);
@@ -450,6 +466,31 @@ int kvbm_manager_execute_repage_batch(kvbm_transfer_manager* m, size_t num_srcs,
                                       const kvbm_repage_batch_seq* seqs, size_t num_seqs, const kvbm_shard_window* windows,
                                       size_t num_windows, const kvbm_layer_stream* ls, const kvbm_transfer_options* opts,
                                       kvbm_notification* out);
+
+/* One prefill rank's KV to every decode rank that needs it, as ONE hand-off: the mirror image of
+ * kvbm_manager_execute_stage_repage_gather.  For window w, heads [src_head_begin, +head_count) of source layers [src_layer_begin,
+ * +layer_count) land as heads [dst_head_begin, +head_count) of layers [dst_layer_begin, +layer_count) of dsts[w.dst_rank], at every
+ * token of [token_begin, token_end); a kvbm_tp_pp_scatter_plan passes as it is.  src_ids holds the source's table[token_begin / Ps
+ * .. ceil(token_end / Ps)) (n_src ids), dst_ids[d] destination d's table[token_begin / Pd .. ceil(token_end / Pd)) (n_dst ids
+ * each); every destination has the same page Pd.  Every other destination byte keeps its value.  Each source vector is read once
+ * and cast once, however many windows take it (replicated heads, MLA's latent head).  The options' layer range and cast_scales
+ * count SOURCE layers ([src num_layers * outer_dim]).  Honoured options: execute_repage's, plus per_dst_done_flags (indexed like
+ * dsts); done_flag and the notification complete once, after every destination landed.  Errors, first one wins: KVBM_ERR no
+ * destination or window, or options.head_count; KVBM_ERR_UNSUPPORTED more than KVBM_GATHER_MAX_SOURCES windows; KVBM_ERR_RANGE a
+ * window naming no destination, with no heads or no layers; KVBM_ERR_OVERLAP two windows whose source layer windows partly
+ * overlap, two windows of one destination whose destination (layer, head) rectangles intersect, or one handle listed twice in
+ * dsts; KVBM_ERR_HANDLE an unknown handle; KVBM_ERR_RANGE a layer window past the source's or its destination's num_layers, or a
+ * source layer of the range that no window covers; each (source, destination) pair's checks of
+ * kvbm_manager_execute_stage_repage_gather with its codes and texts (layer streaming and multicast in the options are
+ * KVBM_ERR_UNSUPPORTED there); KVBM_ERR_INCOMPATIBLE destinations with different page sizes; then the token range, the layer range
+ * and cast scales against the source, the id counts, the block ids of each pair, strategy, device and cast-scale reachability as
+ * there (an empty token or layer range returns KVBM_OK with nothing launched).  One staged copy of every id list, one
+ * kvbm_kernels_paged_repage_scatter launch, one notification; bytes_moved counts each window's destination bytes over its layers
+ * inside the range. */
+int kvbm_manager_execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle src, const size_t* src_ids, size_t n_src,
+                                        size_t num_dsts, const kvbm_layout_handle* dsts, const size_t* const* dst_ids, size_t n_dst,
+                                        size_t token_begin, size_t token_end, const kvbm_scatter_window* windows, size_t num_windows,
+                                        const kvbm_transfer_options* opts, kvbm_notification* out);
 
 /* Completion: the transfer's last warp writes a flag in pinned host memory (no cudaEventQuery polling). */
 int kvbm_notification_is_complete(kvbm_transfer_manager* m, kvbm_notification n);  /* 1 / 0 / <0 error */
