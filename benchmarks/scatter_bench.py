@@ -36,7 +36,7 @@ p.add_argument("--iters", type=int, default=10, help="launches per arm per round
 p.add_argument("--rounds", type=int, default=5)
 p.add_argument("--only", default=None, help="comma-separated case names")
 p.add_argument("--tokens", type=int, default=4096)
-a = p.parse_args()
+a = p.parse_args(None if __name__ == "__main__" else [])   # imported: the defaults
 if not torch.cuda.is_available():
     sys.exit("scatter_bench.py needs a GPU")
 dev = torch.device("cuda:0")
@@ -188,4 +188,5 @@ def main():
         print(f"| {name} | {s['targets']} | {s['pairs']} | {s['bytes'] / 2**20:.0f} | {cell(s)} | {cell(g['singles'])} | {cell(g.get('fanout'))} |")
 
 
-main()
+if __name__ == "__main__":
+    main()

@@ -38,7 +38,7 @@ p.add_argument("--cast", choices=["none", "fp8-to-bf16"], default="none")
 p.add_argument("--only", default=None, help="comma-separated shapes: tp8_tp1, tp4_tp2, repage")
 p.add_argument("--mode", choices=["gate", "tail", "both"], default="both")
 p.add_argument("--layer-us", type=float, default=100.0, help="busy time of one emulated prefill layer (tail mode)")
-a = p.parse_args()
+a = p.parse_args(None if __name__ == "__main__" else [])   # imported: the defaults
 CAST = K.CastMode.FP8E4M3_TO_BF16 if a.cast == "fp8-to-bf16" else K.CastMode.NONE
 SE, DE = (1, 2) if CAST else (2, 2)
 NHD, UTP = int(K.KvBlockLayout.OperationalNHD), int(K.KvBlockLayout.UniversalTP)
@@ -52,6 +52,21 @@ def card():
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True)
     name, _, limit = q.stdout.strip().partition(", ") if q.returncode == 0 else (torch.cuda.get_device_name(0), "", "not read")
     return name, limit
+
+
+def layer_cycles(us):
+    """Clock cycles of a busy kernel that runs `us` microseconds on device 0."""
+    props = torch.cuda.get_device_properties(0)
+    return int(us * props.clock_rate / 1e3) if hasattr(props, "clock_rate") else int(us * 1980)
+
+
+def emulate_prefill(prod, flags, nl, epoch, cycles):
+    """The prefill on stream `prod`: per layer l a busy kernel of `cycles`, then entry l of every ready-flag array in `flags`."""
+    with torch.cuda.stream(prod):
+        for l in range(nl):
+            torch.cuda._sleep(cycles)
+            for f in flags:
+                K.check(K.set_flags(f, l, 1, epoch, int(prod.cuda_stream)), "set_flags")
 
 
 class Pool:
@@ -167,8 +182,7 @@ def run_shape(name, nl, ranks, snh, ps, pd):
 
     if a.mode in ("tail", "both"):
         prod = torch.cuda.Stream()
-        cycles = int(a.layer_us * torch.cuda.get_device_properties(0).clock_rate / 1e3) if hasattr(torch.cuda.get_device_properties(0), "clock_rate") \
-            else int(a.layer_us * 1980)
+        cycles = layer_cycles(a.layer_us)
         with torch.cuda.stream(prod):   # the producer's kernels load before anything spins
             torch.cuda._sleep(100)
             K.check(K.set_flags(ready[0].data_ptr(), 0, 1, epoch[0], int(prod.cuda_stream)), "set_flags")
@@ -183,12 +197,8 @@ def run_shape(name, nl, ranks, snh, ps, pd):
                 end = torch.cuda.Event(enable_timing=True)
                 if arm[1] is not None:
                     go(arm)                        # enqueued before the prefill starts
-                with torch.cuda.stream(prod):
-                    for l in range(nl):
-                        torch.cuda._sleep(cycles)
-                        for r in range(ranks):
-                            K.check(K.set_flags(ready[r].data_ptr(), l, 1, epoch[0], int(prod.cuda_stream)), "set_flags")
-                    last.record(prod)
+                emulate_prefill(prod, [ready[r].data_ptr() for r in range(ranks)], nl, epoch[0], cycles)
+                last.record(prod)
                 if arm[1] is None:
                     stream.wait_event(last)
                     go(arm)
@@ -205,8 +215,9 @@ def run_shape(name, nl, ranks, snh, ps, pd):
                               "power_limit": limit}), flush=True)
 
 
-for nm, shape in SHAPES.items():
-    if a.only and nm not in a.only.split(","):
-        continue
-    run_shape(nm, *shape)
-    torch.cuda.empty_cache()
+if __name__ == "__main__":
+    for nm, shape in SHAPES.items():
+        if a.only and nm not in a.only.split(","):
+            continue
+        run_shape(nm, *shape)
+        torch.cuda.empty_cache()

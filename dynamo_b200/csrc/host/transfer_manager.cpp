@@ -1562,10 +1562,13 @@ static int check_scatter_windows(size_t num_dsts, const kvbm_layout_handle* dsts
 // One prefill rank's KV into every decode rank that needs it (kvbm_manager_execute_repage_scatter), validated in the order its
 // header gives, then one staged copy of [source ids (n_src), destination 0 .. num_dsts - 1 ids (n_dst each)], one
 // kvbm_kernels_paged_repage_scatter launch whose signal writes the per-destination done flags and the completion word, and the
-// options' done flag after it.
+// options' done flag after it.  ls: the streamed scatter (its shape checked by the caller), checked after every other rule for
+// its flags' reachability; the slot also holds the gate's workspace over the source's layers, and the one launch
+// (kvbm_kernels_paged_repage_scatter_streamed) writes every flag, the options' done flag included.
 static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle src_h, const size_t* src_ids, size_t n_src, size_t num_dsts,
                                   const kvbm_layout_handle* dsts, const size_t* const* dst_ids, size_t n_dst, size_t tb, size_t te,
-                                  const kvbm_scatter_window* w, size_t nw, const kvbm_transfer_options* opts_in, kvbm_notification* out)
+                                  const kvbm_scatter_window* w, size_t nw, const kvbm_transfer_options* opts_in, kvbm_notification* out,
+                                  const kvbm_layer_stream* ls = nullptr)
 {
   kvbm_transfer_options o{};
   if (opts_in) o = *opts_in;
@@ -1633,6 +1636,7 @@ static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle s
   }
   if ((rc = need_cuda_device(m))) return rc;
   if (o.cast_scales && (rc = check_cast_scales(m, o.cast_scales))) return rc;
+  if (ls && (rc = check_layer_stream_flags(m, *ls, e, 1))) return rc;
 
   // what lands: each window's destination bytes over its layers inside the range
   uint64_t bytes = 0;
@@ -1650,7 +1654,7 @@ static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle s
   for (size_t d = 0; d < num_dsts; ++d) lists[1 + d] = n_dst ? dst_ids[d] : nullptr;
   Slot* sl;
   uint64_t seq;
-  if ((rc = stage_ids(m, lists.data(), lens.data(), num_dsts + 1, 4, stream, nullptr, &sl, &seq))) return rc;
+  if ((rc = stage_ids(m, lists.data(), lens.data(), num_dsts + 1, ls ? snl + 4 : 4, stream, nullptr, &sl, &seq))) return rc;
   const kvbm_permute_side ks{descriptor(*S), sl->dev_ids, e[0].src_kv};
   kvbm_scatter_target kt[KVBM_GATHER_MAX_SOURCES] = {};
   for (size_t j = 0; j < nw; ++j) {
@@ -1662,13 +1666,21 @@ static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle s
                                 o.per_dst_done_flags ? o.per_dst_done_flags[d] : nullptr};
   }
   const uint32_t row = static_cast<uint32_t>(S->cfg.inner_dim / S->cfg.num_heads * S->cfg.dtype_width_bytes);
-  if ((rc = checked(kvbm_kernels_paged_repage_scatter(&ks, static_cast<uint32_t>(S->cfg.num_heads), static_cast<uint32_t>(ps), kt,
-                                                      static_cast<int>(nw), static_cast<uint32_t>(pd), static_cast<uint32_t>(tb),
-                                                      static_cast<uint32_t>(te), static_cast<int>(lb), static_cast<int>(le), row, o.cast_mode,
-                                                      o.cast_scales, o.epoch, sl->host_flag, static_cast<uint32_t>(seq), stream),
-                    "kvbm_kernels_paged_repage_scatter")))
-    return rc;
-  if (o.done_flag && (rc = checked(kvbm_kernels_set_flags(o.done_flag, 0, 1, o.epoch, stream), "kvbm_kernels_set_flags"))) return rc;
+  const uint32_t snh = static_cast<uint32_t>(S->cfg.num_heads), ups = static_cast<uint32_t>(ps), upd = static_cast<uint32_t>(pd);
+  const uint32_t utb = static_cast<uint32_t>(tb), ute = static_cast<uint32_t>(te);
+  const int k = static_cast<int>(nw), ilb = static_cast<int>(lb), ile = static_cast<int>(le);
+  if (ls) {
+    const kvbm_permute_stream st = layer_stream(*ls, e, 1, o, *sl, seq);
+    rc = checked(kvbm_kernels_paged_repage_scatter_streamed(&ks, snh, ups, kt, k, upd, utb, ute, ilb, ile, row, o.cast_mode, o.cast_scales, &st,
+                                                            stream),
+                 "kvbm_kernels_paged_repage_scatter_streamed");
+  } else {
+    rc = checked(kvbm_kernels_paged_repage_scatter(&ks, snh, ups, kt, k, upd, utb, ute, ilb, ile, row, o.cast_mode, o.cast_scales, o.epoch,
+                                                   sl->host_flag, static_cast<uint32_t>(seq), stream),
+                 "kvbm_kernels_paged_repage_scatter");
+    if (!rc && o.done_flag) rc = checked(kvbm_kernels_set_flags(o.done_flag, 0, 1, o.epoch, stream), "kvbm_kernels_set_flags");
+  }
+  if (rc) return rc;
   if ((rc = finish_slot(m, sl, stream, bytes))) return rc;
   if (out) *out = o.use_caller_stream ? 0 : seq;
   return KVBM_OK;
@@ -2322,6 +2334,19 @@ static int stream_entry(kvbm_transfer_manager* m, const kvbm_layer_stream* ls, s
   if (!m) return fail(KVBM_ERR, "null manager");
   if (out) *out = 0;
   return ls || streamed ? check_layer_stream_shape(ls, num_srcs) : KVBM_OK;
+}
+
+extern "C" int kvbm_manager_execute_repage_scatter_streamed(kvbm_transfer_manager* m, kvbm_layout_handle src, const size_t* src_ids,
+                                                            size_t n_src, size_t num_dsts, const kvbm_layout_handle* dsts,
+                                                            const size_t* const* dst_ids, size_t n_dst, size_t token_begin, size_t token_end,
+                                                            const kvbm_scatter_window* windows, size_t num_windows, const kvbm_layer_stream* ls,
+                                                            const kvbm_transfer_options* opts, kvbm_notification* out)
+{
+  return guarded([&]() -> int {
+  if (int rc = stream_entry(m, ls, 1, true, out)) return rc;
+  return execute_repage_scatter(m, src, src_ids, n_src, num_dsts, dsts, dst_ids, n_dst, token_begin, token_end, windows, num_windows, opts, out,
+                                ls);
+  });
 }
 
 // The head windows of a staged plan's windows, in hw[], or null without windows.  Only the first KVBM_GATHER_MAX_SOURCES are

@@ -201,9 +201,16 @@ __device__ __forceinline__ void arrive_layer(const StreamSync& ss, int layer, ui
   }
 }
 
+// No done flags besides the StreamSync's own.
+struct NoMoreFlags {
+  __device__ __forceinline__ void operator()() const {}
+};
+
 // This ring is finished (its stores have landed).  The last ring to get here re-zeroes the control words and
-// publishes the whole-transfer signals.
-__device__ __forceinline__ void arrive_transfer(const StreamSync& ss)
+// publishes the whole-transfer signals.  more_done(): done flags the StreamSync has no room for, written with its own done
+// flags (not after an abort) and before the completion word.
+template <class MoreDone = NoMoreFlags>
+__device__ __forceinline__ void arrive_transfer(const StreamSync& ss, const MoreDone& more_done = MoreDone{})
 {
   if (ss.ctl == nullptr) return;
   const uint32_t old = ptx::atom_add_acq_rel_gpu(ss.ctl, 1u);
@@ -219,6 +226,7 @@ __device__ __forceinline__ void arrive_transfer(const StreamSync& ss)
 #pragma unroll
     for (int d = 0; d < kMaxDst; ++d)
       if (d < ss.ndst && ss.done_flag[d] != nullptr) ptx::st_relaxed_sys(ss.done_flag[d], ss.epoch);
+    more_done();
   }
   // 0xFFFFFFFF = "this transfer gave up waiting for a layer": destinations are NOT told it completed
   if (ss.completion_flag != nullptr) ptx::st_relaxed_sys(ss.completion_flag, aborted ? 0xFFFFFFFFu : ss.completion_value);

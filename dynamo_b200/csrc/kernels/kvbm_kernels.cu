@@ -954,6 +954,10 @@ struct ScatterParams {
   uint8_t pair_tgt[KVBM_GATHER_MAX_HEADS];
 };
 
+// The layer of source s that a unit of launch layer l reads: a gather's source at its own shift, the scatter's one source at l.
+__host__ __device__ __forceinline__ uint32_t source_layer(const GatherParams& P, int s, uint32_t l) { return l + P.shift[s]; }
+__host__ __device__ __forceinline__ uint32_t source_layer(const ScatterParams&, int, uint32_t l) { return l; }
+
 // One covered source head (entry k) of a scatter unit (big block j, source layer l, outer o): the re-paging walk's load half reads
 // each 16 B vector ONCE and casts it once, and its store half writes it to every (target, destination head) pair of the entry,
 // each at its own layer.  With Ps >= Pd block j is the source's and each target finds the vector's small block in its own table;
@@ -1005,9 +1009,22 @@ __device__ __forceinline__ void scatter_head_rows(const ScatterParams& P, uint32
   }
 }
 
-// One CTA per (big block j, source layer l, outer o) unit, clipped to the range, as the re-paging gather; one warp per covered
-// source head of l's stage, looping by the CTA's warps past 8.  SCALED: the SOURCE's scales[l * no + o], loaded once per unit.
-// The re-paging gathers' bound: three CTAs per SM.
+// One (big block j, source layer l, outer o) unit of the scatter, clipped to the range, with l's stage T: one warp per covered
+// source head of T, looping by the CTA's warps past 8.  SCALED: the SOURCE's scales[l * no + o], loaded once per unit.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__device__ __forceinline__ void scatter_unit(const ScatterParams& P, const GatherStage& T, uint32_t j, uint32_t l, uint32_t o, const RowSplit& r,
+                                             const float* scales)
+{
+  const RepageGeom& G = P.geo;
+  const RepageUnit u = repage_unit(G, j);
+  const ptx::Scale scale = ptx::make_scale(SCALED ? __ldg(scales + l * G.no + o) : 1.f);
+  const uint32_t run = row_run<POW2>(r, u.tokens);
+  const uint32_t end = T.first + T.count;
+  for (uint32_t k = T.first + (threadIdx.x >> 5); k < end; k += blockDim.x >> 5)
+    scatter_head_rows<CAST, POW2, SCALED, PPOW2>(P, k, j, l, o, u, run, r, scale);
+}
+
+// One CTA per unit, as the re-paging gather.  The re-paging gathers' bound: three CTAs per SM.
 template <int CAST, bool POW2, bool SCALED, bool PPOW2>
 __global__ void __launch_bounds__(256, 3)
 kvbm_paged_repage_scatter_kernel(const __grid_constant__ ScatterParams P, RowSplit r, const float* scales)
@@ -1017,13 +1034,7 @@ kvbm_paged_repage_scatter_kernel(const __grid_constant__ ScatterParams P, RowSpl
   const uint32_t j = unit / (G.nlayers * G.no);
   const uint32_t rem = unit - j * (G.nlayers * G.no);
   const uint32_t l = G.layer_begin + rem / G.no, o = rem % G.no;
-  const GatherStage& T = stage_of(P, l);
-  const RepageUnit u = repage_unit(G, j);
-  const ptx::Scale scale = ptx::make_scale(SCALED ? __ldg(scales + l * G.no + o) : 1.f);
-  const uint32_t run = row_run<POW2>(r, u.tokens);
-  const uint32_t end = T.first + T.count;
-  for (uint32_t k = T.first + (threadIdx.x >> 5); k < end; k += blockDim.x >> 5)
-    scatter_head_rows<CAST, POW2, SCALED, PPOW2>(P, k, j, l, o, u, run, r, scale);
+  scatter_unit<CAST, POW2, SCALED, PPOW2>(P, stage_of(P, l), j, l, o, r, scales);
 }
 
 // The scatter's signal after its launch: every target's done flag (epoch) and the completion word, system scope.
@@ -1057,9 +1068,10 @@ struct GateArgs {
   int num_ready;
 };
 
-// The ready flags of the sources of layer l's stage T, each at its own layer l + shift, waited for by warp 0; the verdict goes
-// to the whole CTA.  False: the transfer aborted.
-__device__ __forceinline__ bool gate_layer(const GateArgs& A, const GatherParams& P, const GatherStage& T, uint32_t l, uint32_t* s_ok)
+// The ready flags of the sources of layer l's stage T, each at its own layer (source_layer), waited for by warp 0; the verdict
+// goes to the whole CTA.  False: the transfer aborted.
+template <class Params>
+__device__ __forceinline__ bool gate_layer(const GateArgs& A, const Params& P, const GatherStage& T, uint32_t l, uint32_t* s_ok)
 {
   if (threadIdx.x < 32) {
     bool ok = true;
@@ -1067,7 +1079,7 @@ __device__ __forceinline__ bool gate_layer(const GateArgs& A, const GatherParams
       if ((T.sources >> s) & 1u) {
         StreamSync w = A.ss;
         w.layer_ready = A.ready[s];
-        ok = wait_layer_ready(w, static_cast<int>(l + P.shift[s]), threadIdx.x);
+        ok = wait_layer_ready(w, static_cast<int>(source_layer(P, s, l)), threadIdx.x);
       }
     if (threadIdx.x == 0) *s_ok = ok ? 1u : 0u;
   }
@@ -1085,10 +1097,12 @@ __device__ __forceinline__ void publish_units(const GateArgs& A, uint32_t l, uin
   if (threadIdx.x == 0 && A.ss.want_layers && count != 0) arrive_layer(A.ss, static_cast<int>(l), count);
 }
 
-// The claim / gate / publish loop of every gated kernel over units [0, total) of the gather P: layer_of(u) is unit u's absolute
-// layer, walk(u, l, T) moves it with T its layer's stage, looked up once per layer the CTA enters.
-template <class LayerOf, class Walk>
-__device__ __forceinline__ void gated_units(const GateArgs& A, const GatherParams& P, uint32_t total, uint32_t batch, LayerOf layer_of, Walk walk)
+// The claim / gate / publish loop of every gated kernel over units [0, total) of the gather or scatter P: layer_of(u) is unit u's
+// absolute layer, walk(u, l, T) moves it with T its layer's stage, looked up once per layer the CTA enters.  more_done: the
+// last CTA's done flags besides A.ss's own (arrive_transfer).
+template <class Params, class LayerOf, class Walk, class MoreDone = NoMoreFlags>
+__device__ __forceinline__ void gated_units(const GateArgs& A, const Params& P, uint32_t total, uint32_t batch, LayerOf layer_of, Walk walk,
+                                            MoreDone more_done = MoreDone{})
 {
   __shared__ uint32_t s_ticket, s_ok;
   uint32_t entered = UINT32_MAX;
@@ -1119,7 +1133,7 @@ __device__ __forceinline__ void gated_units(const GateArgs& A, const GatherParam
     if (aborted) break;
     publish_units(A, entered, pending);
   }
-  if (threadIdx.x == 0) arrive_transfer(A.ss);
+  if (threadIdx.x == 0) arrive_transfer(A.ss, more_done);
 }
 
 // kvbm_paged_gather_kernel's unit walk behind the gate; unit = (l * num_blocks + pair) * no + o over the layer range.
@@ -1165,6 +1179,29 @@ kvbm_gated_batch_repage_gather_kernel(const __grid_constant__ RepageGatherParams
     const uint32_t j = rem / G.no;
     repage_gather_unit<CAST, POW2, SCALED, PPOW2, true>(P, T, j, l, rem - j * G.no, r, scales, units);
   });
+}
+
+// kvbm_paged_repage_scatter_kernel's unit walk behind the one source's gate; unit = (l * num_big + j) * no + o over the source
+// layer range, so layer_done[l] counts source layer l in every target.  A.ss holds the stream's own done flag; the last CTA
+// writes the num_flags target done flags of F with it, before the completion word.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__global__ void __launch_bounds__(256, 1)
+kvbm_gated_repage_push_kernel(const __grid_constant__ ScatterParams P, const __grid_constant__ GateArgs A, const __grid_constant__ ScatterFlags F,
+                              int num_flags, uint32_t num_big, RowSplit r, const float* scales, uint32_t batch)
+{
+  const RepageGeom& G = P.geo;
+  const uint32_t per_layer = num_big * G.no;
+  gated_units(
+      A, P, per_layer * G.nlayers, batch, [&](uint32_t u) { return G.layer_begin + u / per_layer; },
+      [&](uint32_t u, uint32_t l, const GatherStage& T) {
+        const uint32_t rem = u - (l - G.layer_begin) * per_layer;
+        const uint32_t j = rem / G.no;
+        scatter_unit<CAST, POW2, SCALED, PPOW2>(P, T, j, l, rem - j * G.no, r, scales);
+      },
+      [&]() {
+        for (int t = 0; t < num_flags; ++t)
+          if (F.done[t]) ptx::st_relaxed_sys(F.done[t], A.ss.epoch);
+      });
 }
 
 // The stream-wait form's signal after layer l: its layer-done flag, and after the last layer the done and completion flags.
@@ -1361,6 +1398,8 @@ static cudaError_t preload_kernels()
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_batch_repage_gather_kernel<c, p, sc, false>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_scatter_kernel<c, p, sc, true>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_scatter_kernel<c, p, sc, false>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_push_kernel<c, p, sc, true>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_push_kernel<c, p, sc, false>);
         });
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_layer_signal_kernel);
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_scatter_signal_kernel);
@@ -1597,13 +1636,14 @@ static cudaError_t gate_args(const kvbm_permute_stream& st, int num_srcs, uint32
   return cudaSuccess;
 }
 
-// A streamed launch of `units` units over layers [layer_begin, layer_end) of an nl-layer destination, after every argument check.
-// The spinning form: launch_gated(A, ctas, batch) launches the gated kernel, which writes every flag itself.  The stream-wait
-// form: per layer l, the stream waits for the flag of every source of l's stage in P at the source's own layer
-// (cuStreamWaitValue32, GEQ: the cyclic order of epoch_reached), launch_layer(l) moves the layer unsignalled, and one signal
-// launch writes its layer-done flag, plus the done and completion flags after the last layer.  Nothing resident spins.
-template <class Layer, class Gated>
-static cudaError_t launch_streamed(const kvbm_permute_stream& st, const GatherParams& P, int num_srcs, uint32_t nl, int layer_begin,
+// A streamed launch of `units` units over layers [layer_begin, layer_end) of an nl-layer launch (a gather's destination, the
+// scatter's source), after every argument check.  The spinning form: launch_gated(A, ctas, batch) launches the gated kernel,
+// which writes every flag itself.  The stream-wait form: per layer l, the stream waits for the flag of every source of l's stage
+// in P (a gather's or a scatter's) at the source's own layer (cuStreamWaitValue32, GEQ: the cyclic order of epoch_reached),
+// launch_layer(l) moves the layer (unsignalled, but for a scatter's target flags after its last layer), and one signal launch
+// writes its layer-done flag, plus the done and completion flags after the last layer.  Nothing resident spins.
+template <class Params, class Layer, class Gated>
+static cudaError_t launch_streamed(const kvbm_permute_stream& st, const Params& P, int num_srcs, uint32_t nl, int layer_begin,
                                    int layer_end, uint64_t units, cudaStream_t stream, Layer&& launch_layer, Gated&& launch_gated)
 {
   cudaError_t e;
@@ -1621,7 +1661,7 @@ static cudaError_t launch_streamed(const kvbm_permute_stream& st, const GatherPa
     const uint32_t mask = stage_of(P, static_cast<uint32_t>(l)).sources;
     for (int s = 0; s < num_srcs; ++s) {
       if (!((mask >> s) & 1u)) continue;
-      const uint32_t* flag = st.layer_ready_flags[s] + (static_cast<uint32_t>(l) + P.shift[s]);
+      const uint32_t* flag = st.layer_ready_flags[s] + source_layer(P, s, static_cast<uint32_t>(l));
       if (g_wait32(stream, reinterpret_cast<unsigned long long>(flag), st.epoch, 0) != 0) return cudaErrorUnknown;
     }
     if ((e = launch_layer(l)) != cudaSuccess) return e;
@@ -1856,17 +1896,29 @@ static cudaError_t launch_paged_repage_gather(const kvbm_stage_source* srcs, int
   return launched(stream, done_flag, epoch, completion_flag, completion_value);
 }
 
-// The scatter's signal launch: every target's done flag and the completion word, none when all are null.
-static cudaError_t scatter_signal(const kvbm_scatter_target* targets, int num_targets, uint32_t epoch, uint32_t* completion_flag,
-                                  uint32_t completion_value, cudaStream_t stream)
+// The scatter's target done flags; *any: whether one is set.
+static ScatterFlags scatter_flags(const kvbm_scatter_target* targets, int num_targets, bool* any)
 {
   ScatterFlags F{};
-  bool any = completion_flag != nullptr;
-  for (int t = 0; t < num_targets; ++t) any |= (F.done[t] = targets[t].done_flag) != nullptr;
-  if (!any) return cudaSuccess;
-  kvbm_scatter_signal_kernel<<<1, 1, 0, stream>>>(F, num_targets, epoch, completion_flag, completion_value);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  return cudaGetLastError();
+  *any = false;
+  for (int t = 0; t < num_targets; ++t) *any |= (F.done[t] = targets[t].done_flag) != nullptr;
+  return F;
+}
+
+// The scatter's signal launch: every target's done flag and the completion word, none when all are null.  done_flag (a streamed
+// launch's own, nullable) goes with the completion word in a second launch, so that the completion word comes last.
+static cudaError_t scatter_signal(const kvbm_scatter_target* targets, int num_targets, uint32_t* done_flag, uint32_t epoch,
+                                  uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
+{
+  bool any;
+  const ScatterFlags F = scatter_flags(targets, num_targets, &any);
+  uint32_t* last = done_flag ? nullptr : completion_flag;
+  if (any || last) {
+    kvbm_scatter_signal_kernel<<<1, 1, 0, stream>>>(F, num_targets, epoch, last, completion_value);
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    if (const cudaError_t e = cudaGetLastError(); e != cudaSuccess) return e;
+  }
+  return done_flag ? signal_launch(done_flag, epoch, completion_flag, completion_value, stream) : cudaSuccess;
 }
 
 static bool spans_overlap(uint64_t a, uint64_t na, uint64_t b, uint64_t nb) { return a < b + nb && b < a + na; }
@@ -1900,7 +1952,7 @@ static bool fill_scatter_targets(const kvbm_scatter_target* tg, int n, uint32_t 
       if (X.src_layer_begin < T[k].end && T[k].begin < src_end) return false;  // a partial overlap
       ++k;
     }
-    if (k == num_stages) T[num_stages++] = GatherStage{X.src_layer_begin, static_cast<uint32_t>(src_end), 0, 0, 0};
+    if (k == num_stages) T[num_stages++] = GatherStage{X.src_layer_begin, static_cast<uint32_t>(src_end), 0, 0, 1};  // the one source
     stage_of_tgt[t] = k;
     for (int u = 0; u < t; ++u) {
       const kvbm_scatter_target& Y = tg[u];
@@ -1965,18 +2017,20 @@ static bool fill_scatter_targets(const kvbm_scatter_target* tg, int n, uint32_t 
 }
 
 // The scatter: every check before any CUDA call (the empty-range signal after the cast, range and target-count rules, as the
-// re-paging gather), then one kvbm_paged_repage_scatter_kernel launch and the signal.
+// re-paging gather), then one kvbm_paged_repage_scatter_kernel launch and the signal.  st: a streamed launch (its flags are the
+// ones passed, and its done flag is written with the targets'), which takes the gated push kernel, or per source layer this
+// launch unstreamed.
 static cudaError_t launch_paged_repage_scatter(const kvbm_permute_side* src, uint32_t src_num_heads, uint32_t src_page,
                                                const kvbm_scatter_target* targets, int num_targets, uint32_t dst_page, uint32_t token_begin,
                                                uint32_t token_end, int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode,
                                                const float* cast_scales, uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value,
-                                               cudaStream_t stream)
+                                               cudaStream_t stream, const kvbm_permute_stream* st = nullptr)
 {
   if (layer_begin < 0 || layer_end < layer_begin || token_end < token_begin) return cudaErrorInvalidValue;
   if (!cast_args_ok(cast_mode, cast_scales)) return cudaErrorInvalidValue;
   if (!targets || num_targets < 1 || num_targets > KVBM_GATHER_MAX_SOURCES) return cudaErrorInvalidValue;
   if (token_end == token_begin || layer_end == layer_begin)
-    return scatter_signal(targets, num_targets, epoch, completion_flag, completion_value, stream);
+    return scatter_signal(targets, num_targets, st ? st->done_flag : nullptr, epoch, completion_flag, completion_value, stream);
   if (!src || !src->block_ids || !src->layout.layer_base) return cudaErrorInvalidValue;
   const uint32_t nl = src->layout.num_layers, no = src->layout.outer_dim;
   if (nl == 0 || no == 0 || static_cast<uint32_t>(layer_end) > nl) return cudaErrorInvalidValue;
@@ -1993,12 +2047,35 @@ static cudaError_t launch_paged_repage_scatter(const kvbm_permute_side* src, uin
   if (!fill_scatter_targets(targets, num_targets, src_num_heads, nl, no, layer_begin, layer_end, dst_page, dst_row_bytes, &P, &widest))
     return cudaErrorInvalidValue;
   const int threads = static_cast<int>(std::min<uint32_t>(8, widest)) * 32;
+  if (st) {
+    // the stream-wait form writes the targets' done flags after the last layer only
+    kvbm_scatter_target quiet[KVBM_GATHER_MAX_SOURCES];
+    std::copy(targets, targets + num_targets, quiet);
+    for (int t = 0; t < num_targets; ++t) quiet[t].done_flag = nullptr;
+    return launch_streamed(
+        *st, P, 1, nl, layer_begin, layer_end, units, stream,
+        [&](int l) {
+          return launch_paged_repage_scatter(src, src_num_heads, src_page, l + 1 == layer_end ? targets : quiet, num_targets, dst_page,
+                                             token_begin, token_end, l, l + 1, src_row_bytes, cast_mode, cast_scales, epoch, nullptr, 0,
+                                             stream);
+        },
+        [&](const GateArgs& A, unsigned ctas, uint32_t batch) {
+          GateArgs B = A;
+          bool any;
+          const ScatterFlags F = scatter_flags(targets, num_targets, &any);
+          B.ss.want_done |= any;
+          const uint32_t nb = static_cast<uint32_t>(units / (static_cast<uint64_t>(P.geo.nlayers) * no));
+          with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, page_pow2, [&](auto c, auto p, auto sc, auto pp) {
+            kvbm_gated_repage_push_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, B, F, num_targets, nb, r, cast_scales, batch);
+          });
+        });
+  }
   with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, page_pow2, [&](auto c, auto p, auto sc, auto pp) {
     kvbm_paged_repage_scatter_kernel<c, p, sc, pp><<<static_cast<unsigned>(units), threads, 0, stream>>>(P, r, cast_scales);
   });
   g_launches.fetch_add(1, std::memory_order_relaxed);
   const cudaError_t e = cudaGetLastError();
-  return e != cudaSuccess ? e : scatter_signal(targets, num_targets, epoch, completion_flag, completion_value, stream);
+  return e != cudaSuccess ? e : scatter_signal(targets, num_targets, nullptr, epoch, completion_flag, completion_value, stream);
 }
 
 }  // namespace kvbm
@@ -2323,6 +2400,18 @@ kvbm_kernels_paged_repage_scatter(const kvbm_permute_side* src, uint32_t src_num
 {
   return launch_paged_repage_scatter(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, token_begin, token_end, layer_begin,
                                      layer_end, src_row_bytes, cast_mode, cast_scales, epoch, completion_flag, completion_value, stream);
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_repage_scatter_streamed(const kvbm_permute_side* src, uint32_t src_num_heads, uint32_t src_page_size,
+                                           const kvbm_scatter_target* targets, int num_targets, uint32_t dst_page_size, uint32_t token_begin,
+                                           uint32_t token_end, int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode,
+                                           const float* cast_scales, const kvbm_permute_stream* st, cudaStream_t stream)
+{
+  if (!stream_args_ok(st, 1)) return cudaErrorInvalidValue;
+  return launch_paged_repage_scatter(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, token_begin, token_end, layer_begin,
+                                     layer_end, src_row_bytes, cast_mode, cast_scales, st->epoch, st->completion_flag, st->completion_value,
+                                     stream, st);
 }
 
 extern "C" cudaError_t

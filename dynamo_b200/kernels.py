@@ -259,6 +259,10 @@ def lib() -> C.CDLL:
                                                         C.c_uint32, C.c_uint32, C.c_uint32, i, i, C.c_uint32, i, vp, C.c_uint32, vp,
                                                         C.c_uint32, vp]
         L.kvbm_kernels_paged_repage_scatter.restype = i
+        L.kvbm_kernels_paged_repage_scatter_streamed.argtypes = [C.POINTER(PermuteSide), C.c_uint32, C.c_uint32, C.POINTER(ScatterTarget),
+                                                                 i, C.c_uint32, C.c_uint32, C.c_uint32, i, i, C.c_uint32, i, vp,
+                                                                 C.POINTER(PermuteStream), vp]
+        L.kvbm_kernels_paged_repage_scatter_streamed.restype = i
         L.kvbm_kernels_permute_strides.argtypes = [i, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64, C.c_uint64,
                                                    C.POINTER(C.c_uint64)]
         L.kvbm_kernels_permute_strides.restype = i
@@ -287,6 +291,7 @@ EXPORTED_SYMBOLS = [
     "kvbm_kernels_paged_stage_repage_gather", "kvbm_kernels_paged_stage_repage_gather_streamed",
     "kvbm_kernels_repage_batch_units", "kvbm_kernels_paged_stage_repage_gather_batch",
     "kvbm_kernels_paged_stage_repage_gather_batch_streamed", "kvbm_kernels_paged_repage_scatter",
+    "kvbm_kernels_paged_repage_scatter_streamed",
 ]
 
 
@@ -574,6 +579,19 @@ def paged_repage_scatter(src: PermuteSide, src_num_heads: int, src_page_size: in
     return lib().kvbm_kernels_paged_repage_scatter(C.byref(src), src_num_heads, src_page_size, arr, len(targets), dst_page_size, token_begin,
                                                    token_end, layer_begin, layer_end, src_row_bytes, int(cast_mode), scales_ptr(cast_scales),
                                                    epoch, completion_flag or None, completion_value, stream)
+
+
+def paged_repage_scatter_streamed(src: PermuteSide, src_num_heads: int, src_page_size: int, targets: Sequence[ScatterTarget],
+                                  dst_page_size: int, token_begin: int, token_end: int, layer_begin: int, layer_end: int,
+                                  src_row_bytes: int, cast_mode: int, cast_scales, st: Optional[PermuteStream], stream: int = 0) -> int:
+    """`paged_repage_scatter` streamed layer by layer behind the source's ready flags: `st.layer_ready_flags[0]` is the source's
+    [num_layers] array, and source layer l is read only once its flag reaches `st.epoch`.  `st.layer_done_flags` and
+    `st.sync_workspace` count source layers; `st.epoch` is also what every target's done flag receives.  The bytes are the
+    unstreamed call's.  include/kvbm_kernels.h (kvbm_kernels_paged_repage_scatter_streamed)."""
+    arr = (ScatterTarget * max(1, len(targets)))(*targets)
+    return lib().kvbm_kernels_paged_repage_scatter_streamed(C.byref(src), src_num_heads, src_page_size, arr, len(targets), dst_page_size,
+                                                            token_begin, token_end, layer_begin, layer_end, src_row_bytes, int(cast_mode),
+                                                            scales_ptr(cast_scales), C.byref(st) if st is not None else None, stream)
 
 
 def permute_strides(kv_layout: int, num_layers: int, outer_dim: int, num_heads: int, page_size: int, row_bytes: int,

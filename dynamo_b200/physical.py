@@ -255,6 +255,7 @@ EXPORTED_SYMBOLS = [
     "kvbm_manager_execute_repage_gather", "kvbm_manager_execute_gather_streamed", "kvbm_manager_execute_repage_gather_streamed",
     "kvbm_tp_pp_reshard_plan", "kvbm_manager_execute_stage_gather", "kvbm_manager_execute_stage_repage_gather",
     "kvbm_manager_execute_repage_batch", "kvbm_tp_pp_scatter_plan", "kvbm_manager_execute_repage_scatter",
+    "kvbm_manager_execute_repage_scatter_streamed",
 ]
 
 
@@ -320,6 +321,8 @@ def lib() -> C.CDLL:
         L.kvbm_tp_pp_scatter_plan.argtypes = [sz, sz, sz, sz, P(sz), sz, sz, P(sz), sz, P(_CScatterWindow), sz, P(sz)]
         L.kvbm_manager_execute_repage_scatter.argtypes = [vp, u64, vp, sz, sz, P(u64), P(P(sz)), sz, sz, sz, P(_CScatterWindow), sz,
                                                           P(_COptions), P(u64)]
+        L.kvbm_manager_execute_repage_scatter_streamed.argtypes = [vp, u64, vp, sz, sz, P(u64), P(P(sz)), sz, sz, sz, P(_CScatterWindow),
+                                                                   sz, P(_CLayerStream), P(_COptions), P(u64)]
         L.kvbm_notification_is_complete.argtypes = [vp, u64]
         L.kvbm_notification_wait.argtypes = [vp, u64, C.c_int64]
         L.kvbm_manager_bytes_moved.argtypes = [vp]
@@ -911,6 +914,32 @@ class TransferManager:
         d's for its page Pd (one Pd for every destination).  Each source vector is read once and cast once, however many windows
         take it.  The options' layer range and cast scales count SOURCE layers; `options.per_dst_done_flags` is indexed like
         `dsts`; `options.done_flag` and the notification complete once, after every destination landed."""
+        args = self._scatter_args(src, src_block_ids, dsts, dst_block_ids, plan, tokens)
+        tok = C.c_uint64()
+        o = (options or TransferOptions())._c()
+        _check(lib().kvbm_manager_execute_repage_scatter(self._h, *args, C.byref(o), C.byref(tok)))
+        return TransferCompleteNotification(self, tok.value)
+
+    def execute_repage_scatter_streamed(self, src: int, src_block_ids: Sequence[int], dsts: Sequence[int],
+                                        dst_block_ids: Sequence[Sequence[int]], plan: Sequence[ScatterWindow], tokens: range, ready_flags: int,
+                                        options: Optional[TransferOptions] = None, layer_done_flags: int = 0) -> TransferCompleteNotification:
+        """`execute_repage_scatter` streamed layer by layer (kvbm_manager_execute_repage_scatter_streamed): `ready_flags` is the
+        address of the source's [num_layers] u32 ready flags, and source layer l is read only after flag l has reached
+        `options.epoch`, so the push overlaps the prefill's forward pass; `layer_done_flags` (an address, or 0) gets entry l =
+        epoch once source layer l landed in every destination.  Options: those of `execute_repage_scatter`, plus epoch, gate_mode,
+        gate_timeout_ms and max_ctas; `per_dst_done_flags` and `done_flag` are written after the last byte, never after a gate
+        timeout.  The bytes and bytes_moved are `execute_repage_scatter`'s."""
+        args = self._scatter_args(src, src_block_ids, dsts, dst_block_ids, plan, tokens)
+        ls = self._layer_stream([0], {0: ready_flags}, layer_done_flags)
+        tok = C.c_uint64()
+        o = (options or TransferOptions())._c()
+        _check(lib().kvbm_manager_execute_repage_scatter_streamed(self._h, *args, C.byref(ls), C.byref(o), C.byref(tok)))
+        return TransferCompleteNotification(self, tok.value)
+
+    @staticmethod
+    def _scatter_args(src: int, src_block_ids: Sequence[int], dsts: Sequence[int], dst_block_ids: Sequence[Sequence[int]],
+                      plan: Sequence[ScatterWindow], tokens: range) -> tuple:
+        """The C arguments of a scatter from `src` through the window count; the arrays they point to stay alive with the tuple."""
         if tokens.step != 1:
             raise ValueError("tokens must be a range with step 1")
         if len(dst_block_ids) != len(dsts):
@@ -924,13 +953,10 @@ class TransferManager:
         PP = C.POINTER(C.c_size_t)
         as_ptr = lambda a: a._as_parameter_ if isinstance(a, _NpView) else C.cast(a, PP)  # noqa: E731
         dp = (PP * max(1, len(dsts)))(*[as_ptr(a) for a in d_arrays])
+        dp._keep = d_arrays
         ws = (_CScatterWindow * max(1, len(plan)))(*[_CScatterWindow(w.dst_rank, w.src_layer_begin, w.dst_layer_begin, w.layer_count,
                                                                      w.src_head_begin, w.dst_head_begin, w.head_count) for w in plan])
-        tok = C.c_uint64()
-        o = (options or TransferOptions())._c()
-        _check(lib().kvbm_manager_execute_repage_scatter(self._h, src, s.addr if type(s) is _NpView else s, ns, len(dsts), hs, dp, n_dst,
-                                                         tokens.start, tokens.stop, ws, len(plan), C.byref(o), C.byref(tok)))
-        return TransferCompleteNotification(self, tok.value)
+        return (src, s.addr if type(s) is _NpView else s, ns, len(dsts), hs, dp, n_dst, tokens.start, tokens.stop, ws, len(plan))
 
     def execute_fanout(self, src: int, dsts: Sequence[int], src_block_ids: Sequence[Sequence[int]],
                        dst_block_ids: Sequence[Sequence[int]], replicate: bool = False,

@@ -550,6 +550,26 @@ cudaError_t kvbm_kernels_paged_repage_scatter(const kvbm_permute_side* src, uint
                                               uint32_t src_row_bytes, int cast_mode, const float* cast_scales, uint32_t epoch,
                                               uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream);
 
+/* kvbm_kernels_paged_repage_scatter streamed layer by layer behind the source's ready flags, as
+ * kvbm_kernels_paged_permute_gather_streamed is: a prefill rank pushes each layer to every target while its forward pass is still
+ * computing later ones.  The bytes are the unstreamed call's, bit for bit; only the time at which each layer is read changes.
+ * Flag conventions, all in SOURCE layers: st->layer_ready_flags[0] is the source's [src num_layers] array (the other entries are
+ * not read), and source layer l is read only once its flag reached st->epoch; layer_done_flags[l] (nullable, [src num_layers]) is
+ * written once source layer l landed in every target that takes it; sync_workspace is u32[KVBM_SYNC_WORKSPACE_WORDS(src
+ * num_layers)].  After the last byte, every target's done_flag and st->done_flag receive st->epoch, then completion_flag
+ * receives completion_value: the completion word always comes last.  The spinning form is one persistent grid that claims (source
+ * layer, big block, outer) units in layer-major order and waits once per source layer it enters; its last CTA writes every flag.
+ * After a gate timeout no done flag is written (neither st->done_flag nor any target's) and completion_flag becomes 0xFFFFFFFF.
+ * The stream-wait form waits on the stream once per source layer and launches the unstreamed scatter over that layer; the target
+ * done flags are written after the last layer only.  The argument rules are kvbm_kernels_paged_repage_scatter's plus the gate's
+ * with one source, all checked before any CUDA call.  An empty token or layer range waits for nothing and writes the done flags
+ * and the completion word at once; it writes no layer_done_flags. */
+cudaError_t kvbm_kernels_paged_repage_scatter_streamed(const kvbm_permute_side* src, uint32_t src_num_heads, uint32_t src_page_size,
+                                                       const kvbm_scatter_target* targets, int num_targets, uint32_t dst_page_size,
+                                                       uint32_t token_begin, uint32_t token_end, int layer_begin, int layer_end,
+                                                       uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
+                                                       const kvbm_permute_stream* st, cudaStream_t stream);
+
 /* Host-only (no GPU): the stride table kvbm_kernels_paged_permute walks with for one side.  out[0] = 1 when offsets count
  * from the block's first byte (universal formats) or 0 when they count from the (layer, outer) region's first byte; the
  * element (layer l, outer o, head h, token t) then sits at  [out[0] ? l * out[1] + o * out[2] : 0] + h * out[3] + t * out[4].

@@ -492,6 +492,24 @@ int kvbm_manager_execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_ha
                                         size_t token_begin, size_t token_end, const kvbm_scatter_window* windows, size_t num_windows,
                                         const kvbm_transfer_options* opts, kvbm_notification* out);
 
+/* kvbm_manager_execute_repage_scatter streamed layer by layer: a prefill rank pushes each source layer to every destination as soon
+ * as its ready flag reached opts->epoch, while its forward pass computes later layers.  ls names the ONE source's flags:
+ * ls->src_layer_ready_flags[0] is its [src num_layers] array, and layer_done_flags (nullable, [src num_layers]) gets entry l =
+ * epoch once source layer l landed in every destination that takes it.  Errors, first one wins: KVBM_ERR for a NULL ls, a NULL
+ * flag table or a NULL entry, and KVBM_ERR_LENGTH_MISMATCH for ls->num_srcs != 1; then every check of
+ * kvbm_manager_execute_repage_scatter, in its order, with its codes and texts (the options' own layer flags and multicast stay
+ * rejected); then KVBM_ERR for a flag array the manager's device cannot reach, as kvbm_manager_execute_gather_streamed.  Honoured
+ * on top of execute_repage_scatter's options: epoch, gate_mode, gate_timeout_ms and max_ctas (see kvbm_permute_stream);
+ * per_dst_done_flags and done_flag are written once, after the last byte, and not after a gate timeout.  The notification
+ * completes as a gated transfer's, with KVBM_ERR_TIMEOUT after the spinning form gave up on a flag.  One staged copy of every id
+ * list and the gate's workspace, one kvbm_kernels_paged_repage_scatter_streamed launch; the destination bytes and bytes_moved
+ * equal execute_repage_scatter's. */
+int kvbm_manager_execute_repage_scatter_streamed(kvbm_transfer_manager* m, kvbm_layout_handle src, const size_t* src_ids, size_t n_src,
+                                                 size_t num_dsts, const kvbm_layout_handle* dsts, const size_t* const* dst_ids,
+                                                 size_t n_dst, size_t token_begin, size_t token_end, const kvbm_scatter_window* windows,
+                                                 size_t num_windows, const kvbm_layer_stream* ls, const kvbm_transfer_options* opts,
+                                                 kvbm_notification* out);
+
 /* Completion: the transfer's last warp writes a flag in pinned host memory (no cudaEventQuery polling). */
 int kvbm_notification_is_complete(kvbm_transfer_manager* m, kvbm_notification n);  /* 1 / 0 / <0 error */
 int kvbm_notification_wait(kvbm_transfer_manager* m, kvbm_notification n, int64_t timeout_us);
