@@ -2542,7 +2542,8 @@ paged_copy_impl(const kvbm_paged_layout* src, const kvbm_paged_dst* dsts, int nu
   gen.a.n_layers = static_cast<uint32_t>(layer_end - layer_begin);
   gen.a.outer = src->outer_dim;
   gen.a.tile = rc.tile;
-  gen.a.tiles_per_region = (src->region_bytes + rc.tile - 1) / rc.tile;
+  // in 64 bits: a region within one tile of 4 GiB would wrap to 0 tiles in 32
+  gen.a.tiles_per_region = static_cast<uint32_t>((static_cast<uint64_t>(src->region_bytes) + rc.tile - 1) / rc.tile);
   gen.a.dst_num = num;
   gen.a.dst_den = den;
   const uint64_t fan = gen.a.replicate ? 1 : static_cast<uint64_t>(data_dsts);
