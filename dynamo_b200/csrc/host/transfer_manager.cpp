@@ -1559,26 +1559,26 @@ static int check_scatter_windows(size_t num_dsts, const kvbm_layout_handle* dsts
   return KVBM_OK;
 }
 
-// One prefill rank's KV into every decode rank that needs it (kvbm_manager_execute_repage_scatter), validated in the order its
-// header gives, then one staged copy of [source ids (n_src), destination 0 .. num_dsts - 1 ids (n_dst each)], one
-// kvbm_kernels_paged_repage_scatter launch whose signal writes the per-destination done flags and the completion word, and the
-// options' done flag after it.  ls: the streamed scatter (its shape checked by the caller), checked after every other rule for
-// its flags' reachability; the slot also holds the gate's workspace over the source's layers, and the one launch
-// (kvbm_kernels_paged_repage_scatter_streamed) writes every flag, the options' done flag included.
-static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle src_h, const size_t* src_ids, size_t n_src, size_t num_dsts,
-                                  const kvbm_layout_handle* dsts, const size_t* const* dst_ids, size_t n_dst, size_t tb, size_t te,
-                                  const kvbm_scatter_window* w, size_t nw, const kvbm_transfer_options* opts_in, kvbm_notification* out,
-                                  const kvbm_layer_stream* ls = nullptr)
+// A scatter request as check_scatter_request validated it: the source, the destinations, every window's Transfer, the layer range
+// and whether there is nothing to move.
+struct ScatterRequest {
+  Layout* S = nullptr;
+  std::vector<Layout*> D;
+  Transfer e[KVBM_GATHER_MAX_SOURCES];
+  size_t lb = 0, le = 0;
+  bool empty = false;
+};
+
+// Every check of one sequence of a scatter after check_scatter_windows, under the manager's lock, in the order its header gives.
+static int check_scatter_request(kvbm_transfer_manager* m, kvbm_layout_handle src_h, const kvbm_scatter_batch_seq& q, size_t num_dsts,
+                                 const kvbm_layout_handle* dsts, const kvbm_scatter_window* w, size_t nw, const kvbm_transfer_options& o,
+                                 const kvbm_layer_stream* ls, ScatterRequest* R)
 {
-  kvbm_transfer_options o{};
-  if (opts_in) o = *opts_in;
-  if (out) *out = 0;
   int rc;
-  if ((rc = check_scatter_windows(num_dsts, dsts, w, nw, o))) return rc;
-  std::lock_guard<std::mutex> lk(m->mu);
-  Layout* S = m->find(src_h);
+  Layout* S = R->S = m->find(src_h);
   if (!S) return fail(KVBM_ERR_HANDLE, "invalid source handle");
-  std::vector<Layout*> D(num_dsts);
+  std::vector<Layout*>& D = R->D;
+  D.assign(num_dsts, nullptr);
   for (size_t d = 0; d < num_dsts; ++d)
     if (!(D[d] = m->find(dsts[d]))) return fail(KVBM_ERR_HANDLE, "invalid destination handle");
   const size_t snl = S->cfg.num_layers;
@@ -1604,7 +1604,7 @@ static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle s
   // the pair checks take the per-destination done flags, which a scatter honours, as absent
   kvbm_transfer_options op = o;
   op.per_dst_done_flags = nullptr;
-  Transfer e[KVBM_GATHER_MAX_SOURCES];
+  Transfer* e = R->e;
   for (size_t j = 0; j < nw; ++j) {
     Layout& Dj = *D[w[j].dst_rank];
     e[j].S = S;
@@ -1616,20 +1616,21 @@ static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle s
                                              " has " + std::to_string(D[w[0].dst_rank]->cfg.page_size) + ", destination " +
                                              std::to_string(w[j].dst_rank) + " has " + std::to_string(Dj.cfg.page_size));
   }
-  const size_t ps = S->cfg.page_size, pd = D[w[0].dst_rank]->cfg.page_size;
+  const size_t ps = S->cfg.page_size, pd = D[w[0].dst_rank]->cfg.page_size, tb = q.token_begin, te = q.token_end;
   if (tb > te || te > (size_t{1} << 31))
     return fail(KVBM_ERR_RANGE, "Token range " + std::to_string(tb) + ".." + std::to_string(te) + " is reversed or reaches past 2^31 tokens");
-  size_t lb, le;
-  if ((rc = check_layer_range(S->cfg, o, &lb, &le))) return rc;
-  if ((rc = check_repage_counts(tb, te, ps, pd, n_src, n_dst))) return rc;
-  if ((n_src && !src_ids) || (n_dst && !dst_ids)) return fail(KVBM_ERR, "null block id list");
+  if ((rc = check_layer_range(S->cfg, o, &R->lb, &R->le))) return rc;
+  if ((rc = check_repage_counts(tb, te, ps, pd, q.n_src, q.n_dst))) return rc;
+  if ((q.n_src && !q.src_ids) || (q.n_dst && !q.dst_ids)) return fail(KVBM_ERR, "null block id list");
   for (size_t j = 0; j < nw; ++j) {
     const size_t d = w[j].dst_rank;
-    if (n_dst && !dst_ids[d]) return fail(KVBM_ERR, "null block id list");
-    if ((rc = check_block_ids(src_ids, n_src, n_dst ? dst_ids[d] : nullptr, n_dst, S->cfg.num_blocks, D[d]->cfg.num_blocks, src_h == dsts[d])))
+    if (q.n_dst && !q.dst_ids[d]) return fail(KVBM_ERR, "null block id list");
+    if ((rc = check_block_ids(q.src_ids, q.n_src, q.n_dst ? q.dst_ids[d] : nullptr, q.n_dst, S->cfg.num_blocks, D[d]->cfg.num_blocks,
+                              src_h == dsts[d])))
       return rc;
   }
-  if (tb == te || lb == le) return KVBM_OK;  // nothing to move, as execute()
+  R->empty = tb == te || R->lb == R->le;
+  if (R->empty) return KVBM_OK;  // nothing to move, as execute()
   for (size_t j = 0; j < nw; ++j) {
     if ((rc = repage_strategy(m, *S, *e[j].D[0], &e[j].plan))) return rc;
     if (e[j].plan.first != e[0].plan.first) return fail(KVBM_ERR_UNSUPPORTED, "the destinations of a scatter need the same CUDA strategy");
@@ -1637,14 +1638,87 @@ static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle s
   if ((rc = need_cuda_device(m))) return rc;
   if (o.cast_scales && (rc = check_cast_scales(m, o.cast_scales))) return rc;
   if (ls && (rc = check_layer_stream_flags(m, *ls, e, 1))) return rc;
+  return KVBM_OK;
+}
 
-  // what lands: each window's destination bytes over its layers inside the range
+// One prefill rank's KV into every decode rank that needs it over a list of sequences, each the token range and tables of one
+// check_scatter_request: kvbm_manager_execute_repage_scatter and its streamed form pass their one range as one sequence,
+// kvbm_manager_execute_repage_scatter_batch its list (`batch`).  Every sequence is checked in turn and the first rejected one
+// returns its code and text; an empty one moves nothing.  Then a batch's concatenated tables are checked per destination for a
+// block named twice, and one staged copy takes [source ids, destination 0 .. num_dsts - 1 ids (the same count each)] (and a
+// batch's unit table), then one launch whose signal writes the per-destination done flags and the completion word, and the
+// options' done flag after it.  ls: the streamed scatter (its shape checked by the caller); the slot also holds the gate's
+// workspace over the source's layers, and the one streamed launch writes every flag, the options' done flag included.
+static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle src_h, size_t num_dsts, const kvbm_layout_handle* dsts,
+                                  const kvbm_scatter_batch_seq* seqs, size_t num_seqs, const kvbm_scatter_window* w, size_t nw,
+                                  const kvbm_transfer_options* opts_in, kvbm_notification* out, const kvbm_layer_stream* ls = nullptr,
+                                  bool batch = false)
+{
+  kvbm_transfer_options o{};
+  if (opts_in) o = *opts_in;
+  if (out) *out = 0;
+  int rc;
+  if ((rc = check_scatter_windows(num_dsts, dsts, w, nw, o))) return rc;
+  if (batch && num_seqs && !seqs) return fail(KVBM_ERR, "null sequence list");
+  std::lock_guard<std::mutex> lk(m->mu);
+  // every sequence resolves the same source, destinations, windows and layer range: only `empty` is the last sequence's own
+  ScatterRequest R;
+  bool any = false;
   uint64_t bytes = 0;
-  for (size_t j = 0; j < nw; ++j) {
-    const Layout& Dj = *e[j].D[0];
-    const size_t from = std::max(lb, w[j].src_layer_begin), to = std::min(le, w[j].src_layer_begin + w[j].layer_count);
-    if (to > from) bytes += (te - tb) * (to - from) * Dj.cfg.outer_dim * w[j].head_count * (Dj.cfg.inner_dim / Dj.cfg.num_heads * Dj.cfg.dtype_width_bytes);
+  for (size_t i = 0; i < num_seqs; ++i) {
+    const kvbm_scatter_batch_seq& q = seqs[i];
+    if ((rc = check_scatter_request(m, src_h, q, num_dsts, dsts, w, nw, o, ls, &R))) return rc;
+    if (R.empty) continue;
+    any = true;
+    // what lands: each window's destination bytes over its layers inside the range
+    for (size_t j = 0; j < nw; ++j) {
+      const Layout& Dj = *R.e[j].D[0];
+      const size_t from = std::max(R.lb, w[j].src_layer_begin), to = std::min(R.le, w[j].src_layer_begin + w[j].layer_count);
+      if (to > from)
+        bytes += (q.token_end - q.token_begin) * (to - from) * Dj.cfg.outer_dim * w[j].head_count *
+                 (Dj.cfg.inner_dim / Dj.cfg.num_heads * Dj.cfg.dtype_width_bytes);
+    }
   }
+  if (!any) return KVBM_OK;  // no sequences, only empty ranges or an empty layer range: nothing to move
+  const Transfer* e = R.e;
+  const Layout* S = R.S;
+  const std::vector<Layout*>& D = R.D;
+  const size_t snl = S->cfg.num_layers;
+  const uint32_t ups = static_cast<uint32_t>(S->cfg.page_size), upd = static_cast<uint32_t>(D[w[0].dst_rank]->cfg.page_size);
+  const size_t* src_ids = seqs[0].src_ids;
+  const size_t* const* dst_ids = seqs[0].dst_ids;
+  size_t n_src = seqs[0].n_src, n_dst = seqs[0].n_dst;
+  std::vector<kvbm_repage_seq> ranges;
+  std::vector<kvbm_repage_unit> units;
+  std::vector<std::vector<size_t>> cat;  // a batch's: the source's concatenated table, then each destination's
+  std::vector<const size_t*> cat_dst;
+  if (batch) {
+    std::vector<bool> named(num_dsts, false);  // the destinations some window writes: the others' tables may be null
+    for (size_t j = 0; j < nw; ++j) named[w[j].dst_rank] = true;
+    cat.resize(1 + num_dsts);
+    for (size_t i = 0; i < num_seqs; ++i) {
+      const kvbm_scatter_batch_seq& q = seqs[i];
+      if (q.token_begin == q.token_end) continue;
+      ranges.push_back(kvbm_repage_seq{static_cast<uint32_t>(q.token_begin), static_cast<uint32_t>(q.token_end)});
+      cat[0].insert(cat[0].end(), q.src_ids, q.src_ids + q.n_src);
+      for (size_t d = 0; d < num_dsts; ++d)
+        if (named[d]) cat[1 + d].insert(cat[1 + d].end(), q.dst_ids[d], q.dst_ids[d] + q.n_dst);
+    }
+    for (size_t d = 0; d < num_dsts; ++d)
+      if (named[d] && (rc = check_block_ids(cat[0].data(), cat[0].size(), cat[1 + d].data(), cat[1 + d].size(), S->cfg.num_blocks,
+                                            D[d]->cfg.num_blocks, src_h == dsts[d])))
+        return rc;
+    size_t num_units = 0;
+    if (kvbm_kernels_repage_batch_units(ranges.data(), ranges.size(), ups, upd, nullptr, 0, &num_units, &n_src, &n_dst))
+      return fail(KVBM_ERR, "the batch's token ranges and page sizes have no unit table");
+    units.resize(num_units);
+    kvbm_kernels_repage_batch_units(ranges.data(), ranges.size(), ups, upd, units.data(), units.size(), &num_units, &n_src, &n_dst);
+    src_ids = cat[0].data();
+    cat_dst.resize(num_dsts);
+    for (size_t d = 0; d < num_dsts; ++d) cat_dst[d] = named[d] ? cat[1 + d].data() : nullptr;
+    dst_ids = cat_dst.data();
+  }
+
   DeviceGuard g(m->device);
   const cudaStream_t stream = pick_stream(m, e[0].plan.first, o);
   std::vector<const size_t*> lists(num_dsts + 1);
@@ -1654,7 +1728,8 @@ static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle s
   for (size_t d = 0; d < num_dsts; ++d) lists[1 + d] = n_dst ? dst_ids[d] : nullptr;
   Slot* sl;
   uint64_t seq;
-  if ((rc = stage_ids(m, lists.data(), lens.data(), num_dsts + 1, ls ? snl + 4 : 4, stream, nullptr, &sl, &seq))) return rc;
+  if ((rc = stage_ids(m, lists.data(), lens.data(), num_dsts + 1, ls ? snl + 4 : 4, stream, nullptr, &sl, &seq, units.data(), units.size())))
+    return rc;
   const kvbm_permute_side ks{descriptor(*S), sl->dev_ids, e[0].src_kv};
   kvbm_scatter_target kt[KVBM_GATHER_MAX_SOURCES] = {};
   for (size_t j = 0; j < nw; ++j) {
@@ -1666,18 +1741,30 @@ static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle s
                                 o.per_dst_done_flags ? o.per_dst_done_flags[d] : nullptr};
   }
   const uint32_t row = static_cast<uint32_t>(S->cfg.inner_dim / S->cfg.num_heads * S->cfg.dtype_width_bytes);
-  const uint32_t snh = static_cast<uint32_t>(S->cfg.num_heads), ups = static_cast<uint32_t>(ps), upd = static_cast<uint32_t>(pd);
-  const uint32_t utb = static_cast<uint32_t>(tb), ute = static_cast<uint32_t>(te);
-  const int k = static_cast<int>(nw), ilb = static_cast<int>(lb), ile = static_cast<int>(le);
+  const uint32_t snh = static_cast<uint32_t>(S->cfg.num_heads);
+  const uint32_t utb = static_cast<uint32_t>(seqs[0].token_begin), ute = static_cast<uint32_t>(seqs[0].token_end);
+  const int k = static_cast<int>(nw), ilb = static_cast<int>(R.lb), ile = static_cast<int>(R.le);
+  const auto* du = reinterpret_cast<const kvbm_repage_unit*>(sl->dev_ids + units_at(n_src + num_dsts * n_dst));
   if (ls) {
     const kvbm_permute_stream st = layer_stream(*ls, e, 1, o, *sl, seq);
-    rc = checked(kvbm_kernels_paged_repage_scatter_streamed(&ks, snh, ups, kt, k, upd, utb, ute, ilb, ile, row, o.cast_mode, o.cast_scales, &st,
-                                                            stream),
-                 "kvbm_kernels_paged_repage_scatter_streamed");
+    if (batch)
+      rc = checked(kvbm_kernels_paged_repage_scatter_batch_streamed(&ks, snh, ups, kt, k, upd, ranges.data(), ranges.size(), du, units.size(),
+                                                                    ilb, ile, row, o.cast_mode, o.cast_scales, &st, stream),
+                   "kvbm_kernels_paged_repage_scatter_batch_streamed");
+    else
+      rc = checked(kvbm_kernels_paged_repage_scatter_streamed(&ks, snh, ups, kt, k, upd, utb, ute, ilb, ile, row, o.cast_mode, o.cast_scales,
+                                                              &st, stream),
+                   "kvbm_kernels_paged_repage_scatter_streamed");
   } else {
-    rc = checked(kvbm_kernels_paged_repage_scatter(&ks, snh, ups, kt, k, upd, utb, ute, ilb, ile, row, o.cast_mode, o.cast_scales, o.epoch,
-                                                   sl->host_flag, static_cast<uint32_t>(seq), stream),
-                 "kvbm_kernels_paged_repage_scatter");
+    if (batch)
+      rc = checked(kvbm_kernels_paged_repage_scatter_batch(&ks, snh, ups, kt, k, upd, ranges.data(), ranges.size(), du, units.size(), ilb, ile,
+                                                           row, o.cast_mode, o.cast_scales, o.epoch, sl->host_flag, static_cast<uint32_t>(seq),
+                                                           stream),
+                   "kvbm_kernels_paged_repage_scatter_batch");
+    else
+      rc = checked(kvbm_kernels_paged_repage_scatter(&ks, snh, ups, kt, k, upd, utb, ute, ilb, ile, row, o.cast_mode, o.cast_scales, o.epoch,
+                                                     sl->host_flag, static_cast<uint32_t>(seq), stream),
+                   "kvbm_kernels_paged_repage_scatter");
     if (!rc && o.done_flag) rc = checked(kvbm_kernels_set_flags(o.done_flag, 0, 1, o.epoch, stream), "kvbm_kernels_set_flags");
   }
   if (rc) return rc;
@@ -2323,7 +2410,8 @@ extern "C" int kvbm_manager_execute_repage_scatter(kvbm_transfer_manager* m, kvb
 {
   return guarded([&]() -> int {
   if (!m) return fail(KVBM_ERR, "null manager");
-  return execute_repage_scatter(m, src, src_ids, n_src, num_dsts, dsts, dst_ids, n_dst, token_begin, token_end, windows, num_windows, opts, out);
+  const kvbm_scatter_batch_seq q{token_begin, token_end, src_ids, n_src, dst_ids, n_dst};
+  return execute_repage_scatter(m, src, num_dsts, dsts, &q, 1, windows, num_windows, opts, out);
   });
 }
 
@@ -2344,8 +2432,19 @@ extern "C" int kvbm_manager_execute_repage_scatter_streamed(kvbm_transfer_manage
 {
   return guarded([&]() -> int {
   if (int rc = stream_entry(m, ls, 1, true, out)) return rc;
-  return execute_repage_scatter(m, src, src_ids, n_src, num_dsts, dsts, dst_ids, n_dst, token_begin, token_end, windows, num_windows, opts, out,
-                                ls);
+  const kvbm_scatter_batch_seq q{token_begin, token_end, src_ids, n_src, dst_ids, n_dst};
+  return execute_repage_scatter(m, src, num_dsts, dsts, &q, 1, windows, num_windows, opts, out, ls);
+  });
+}
+
+extern "C" int kvbm_manager_execute_repage_scatter_batch(kvbm_transfer_manager* m, kvbm_layout_handle src, size_t num_dsts,
+                                                         const kvbm_layout_handle* dsts, const kvbm_scatter_batch_seq* seqs, size_t num_seqs,
+                                                         const kvbm_scatter_window* windows, size_t num_windows, const kvbm_layer_stream* ls,
+                                                         const kvbm_transfer_options* opts, kvbm_notification* out)
+{
+  return guarded([&]() -> int {
+  if (int rc = stream_entry(m, ls, 1, false, out)) return rc;
+  return execute_repage_scatter(m, src, num_dsts, dsts, seqs, num_seqs, windows, num_windows, opts, out, ls, /*batch=*/true);
   });
 }
 

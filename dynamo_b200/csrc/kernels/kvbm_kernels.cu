@@ -1011,12 +1011,17 @@ __device__ __forceinline__ void scatter_head_rows(const ScatterParams& P, uint32
 
 // One (big block j, source layer l, outer o) unit of the scatter, clipped to the range, with l's stage T: one warp per covered
 // source head of T, looping by the CTA's warps past 8.  SCALED: the SOURCE's scales[l * no + o], loaded once per unit.
-template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+// TABLE: a batch of sequences, whose unit comes from `units` (batch_unit) instead of the launch's one token range.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2, bool TABLE = false>
 __device__ __forceinline__ void scatter_unit(const ScatterParams& P, const GatherStage& T, uint32_t j, uint32_t l, uint32_t o, const RowSplit& r,
-                                             const float* scales)
+                                             const float* scales, const kvbm_repage_unit* units = nullptr)
 {
   const RepageGeom& G = P.geo;
-  const RepageUnit u = repage_unit(G, j);
+  RepageUnit u;
+  if constexpr (TABLE)
+    u = batch_unit(units, j);
+  else
+    u = repage_unit(G, j);
   const ptx::Scale scale = ptx::make_scale(SCALED ? __ldg(scales + l * G.no + o) : 1.f);
   const uint32_t run = row_run<POW2>(r, u.tokens);
   const uint32_t end = T.first + T.count;
@@ -1035,6 +1040,21 @@ kvbm_paged_repage_scatter_kernel(const __grid_constant__ ScatterParams P, RowSpl
   const uint32_t rem = unit - j * (G.nlayers * G.no);
   const uint32_t l = G.layer_begin + rem / G.no, o = rem % G.no;
   scatter_unit<CAST, POW2, SCALED, PPOW2>(P, stage_of(P, l), j, l, o, r, scales);
+}
+
+// kvbm_paged_repage_scatter_kernel over a batch of sequences: big block j is entry j of the concatenated big table (the source's,
+// or every target's: they share Pd and the batch) and record j of `units`; geo's token range and first blocks are unused.  The
+// same bound: three CTAs per SM.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__global__ void __launch_bounds__(256, 3)
+kvbm_paged_repage_push_seqs_kernel(const __grid_constant__ ScatterParams P, const kvbm_repage_unit* units, RowSplit r, const float* scales)
+{
+  const RepageGeom& G = P.geo;
+  const uint32_t unit = blockIdx.x;  // (big block j * nlayers + l) * no + o
+  const uint32_t j = unit / (G.nlayers * G.no);
+  const uint32_t rem = unit - j * (G.nlayers * G.no);
+  const uint32_t l = G.layer_begin + rem / G.no, o = rem % G.no;
+  scatter_unit<CAST, POW2, SCALED, PPOW2, true>(P, stage_of(P, l), j, l, o, r, scales, units);
 }
 
 // The scatter's signal after its launch: every target's done flag (epoch) and the completion word, system scope.
@@ -1197,6 +1217,28 @@ kvbm_gated_repage_push_kernel(const __grid_constant__ ScatterParams P, const __g
         const uint32_t rem = u - (l - G.layer_begin) * per_layer;
         const uint32_t j = rem / G.no;
         scatter_unit<CAST, POW2, SCALED, PPOW2>(P, T, j, l, rem - j * G.no, r, scales);
+      },
+      [&]() {
+        for (int t = 0; t < num_flags; ++t)
+          if (F.done[t]) ptx::st_relaxed_sys(F.done[t], A.ss.epoch);
+      });
+}
+
+// kvbm_gated_repage_push_kernel over a batch of sequences (num_big: the length of `units`): source layer l is done once it landed
+// in every target for every sequence.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__global__ void __launch_bounds__(256, 1)
+kvbm_gated_repage_push_seqs_kernel(const __grid_constant__ ScatterParams P, const __grid_constant__ GateArgs A, const __grid_constant__ ScatterFlags F,
+                                   int num_flags, const kvbm_repage_unit* units, uint32_t num_big, RowSplit r, const float* scales, uint32_t batch)
+{
+  const RepageGeom& G = P.geo;
+  const uint32_t per_layer = num_big * G.no;
+  gated_units(
+      A, P, per_layer * G.nlayers, batch, [&](uint32_t u) { return G.layer_begin + u / per_layer; },
+      [&](uint32_t u, uint32_t l, const GatherStage& T) {
+        const uint32_t rem = u - (l - G.layer_begin) * per_layer;
+        const uint32_t j = rem / G.no;
+        scatter_unit<CAST, POW2, SCALED, PPOW2, true>(P, T, j, l, rem - j * G.no, r, scales, units);
       },
       [&]() {
         for (int t = 0; t < num_flags; ++t)
@@ -1400,6 +1442,10 @@ static cudaError_t preload_kernels()
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_scatter_kernel<c, p, sc, false>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_push_kernel<c, p, sc, true>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_push_kernel<c, p, sc, false>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_push_seqs_kernel<c, p, sc, true>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_push_seqs_kernel<c, p, sc, false>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_push_seqs_kernel<c, p, sc, true>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_push_seqs_kernel<c, p, sc, false>);
         });
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_layer_signal_kernel);
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_scatter_signal_kernel);
@@ -2019,17 +2065,25 @@ static bool fill_scatter_targets(const kvbm_scatter_target* tg, int n, uint32_t 
 // The scatter: every check before any CUDA call (the empty-range signal after the cast, range and target-count rules, as the
 // re-paging gather), then one kvbm_paged_repage_scatter_kernel launch and the signal.  st: a streamed launch (its flags are the
 // ones passed, and its done flag is written with the targets'), which takes the gated push kernel, or per source layer this
-// launch unstreamed.
+// launch unstreamed.  B: a batch of sequences in place of the one token range (token_begin / token_end unused), checked as
+// launch_paged_repage_gather checks it; it always takes the push_seqs kernels.
 static cudaError_t launch_paged_repage_scatter(const kvbm_permute_side* src, uint32_t src_num_heads, uint32_t src_page,
                                                const kvbm_scatter_target* targets, int num_targets, uint32_t dst_page, uint32_t token_begin,
                                                uint32_t token_end, int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode,
                                                const float* cast_scales, uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value,
-                                               cudaStream_t stream, const kvbm_permute_stream* st = nullptr)
+                                               cudaStream_t stream, const kvbm_permute_stream* st = nullptr, const RepageBatch* B = nullptr)
 {
-  if (layer_begin < 0 || layer_end < layer_begin || token_end < token_begin) return cudaErrorInvalidValue;
+  if (layer_begin < 0 || layer_end < layer_begin || (!B && token_end < token_begin)) return cudaErrorInvalidValue;
   if (!cast_args_ok(cast_mode, cast_scales)) return cudaErrorInvalidValue;
   if (!targets || num_targets < 1 || num_targets > KVBM_GATHER_MAX_SOURCES) return cudaErrorInvalidValue;
-  if (token_end == token_begin || layer_end == layer_begin)
+  size_t num_big = 0;
+  if (B) {
+    size_t src_ids, dst_ids;
+    if (kvbm_kernels_repage_batch_units(B->seqs, B->num_seqs, src_page, dst_page, nullptr, 0, &num_big, &src_ids, &dst_ids) != 0)
+      return cudaErrorInvalidValue;
+    if (num_big != B->num_units || (num_big != 0 && !B->units)) return cudaErrorInvalidValue;
+  }
+  if ((B ? num_big == 0 : token_end == token_begin) || layer_end == layer_begin)
     return scatter_signal(targets, num_targets, st ? st->done_flag : nullptr, epoch, completion_flag, completion_value, stream);
   if (!src || !src->block_ids || !src->layout.layer_base) return cudaErrorInvalidValue;
   const uint32_t nl = src->layout.num_layers, no = src->layout.outer_dim;
@@ -2038,9 +2092,15 @@ static cudaError_t launch_paged_repage_scatter(const kvbm_permute_side* src, uin
   RowSplit r;
   uint64_t dst_row_bytes, units;
   bool page_pow2;
-  if (!repage_geometry(src_page, dst_page, token_begin, token_end, layer_begin, layer_end, no, src_row_bytes, cast_mode, &P.geo, &r,
-                       &dst_row_bytes, &units, &page_pow2))
+  if (B) {
+    if (!repage_pages(src_page, dst_page, layer_begin, layer_end, no, src_row_bytes, cast_mode, &P.geo, &r, &dst_row_bytes, &page_pow2))
+      return cudaErrorInvalidValue;
+    if (num_big >= (1ull << 31) || (units = static_cast<uint64_t>(num_big) * P.geo.nlayers) >= (1ull << 31) || (units *= no) >= (1ull << 31))
+      return cudaErrorInvalidValue;
+  } else if (!repage_geometry(src_page, dst_page, token_begin, token_end, layer_begin, layer_end, no, src_row_bytes, cast_mode, &P.geo, &r,
+                              &dst_row_bytes, &units, &page_pow2)) {
     return cudaErrorInvalidValue;
+  }
   if (static_cast<uint64_t>(src_page) * src_num_heads * src_row_bytes != src->layout.region_bytes) return cudaErrorInvalidValue;
   if (!fill_permute_side(*src, nl, no, src_num_heads, src_page, src_row_bytes, &P.S)) return cudaErrorInvalidValue;
   uint32_t widest;
@@ -2057,21 +2117,28 @@ static cudaError_t launch_paged_repage_scatter(const kvbm_permute_side* src, uin
         [&](int l) {
           return launch_paged_repage_scatter(src, src_num_heads, src_page, l + 1 == layer_end ? targets : quiet, num_targets, dst_page,
                                              token_begin, token_end, l, l + 1, src_row_bytes, cast_mode, cast_scales, epoch, nullptr, 0,
-                                             stream);
+                                             stream, nullptr, B);
         },
         [&](const GateArgs& A, unsigned ctas, uint32_t batch) {
-          GateArgs B = A;
+          GateArgs Ag = A;
           bool any;
           const ScatterFlags F = scatter_flags(targets, num_targets, &any);
-          B.ss.want_done |= any;
+          Ag.ss.want_done |= any;
           const uint32_t nb = static_cast<uint32_t>(units / (static_cast<uint64_t>(P.geo.nlayers) * no));
           with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, page_pow2, [&](auto c, auto p, auto sc, auto pp) {
-            kvbm_gated_repage_push_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, B, F, num_targets, nb, r, cast_scales, batch);
+            if (B)
+              kvbm_gated_repage_push_seqs_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, Ag, F, num_targets, B->units, nb, r, cast_scales,
+                                                                                            batch);
+            else
+              kvbm_gated_repage_push_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, Ag, F, num_targets, nb, r, cast_scales, batch);
           });
         });
   }
   with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, page_pow2, [&](auto c, auto p, auto sc, auto pp) {
-    kvbm_paged_repage_scatter_kernel<c, p, sc, pp><<<static_cast<unsigned>(units), threads, 0, stream>>>(P, r, cast_scales);
+    if (B)
+      kvbm_paged_repage_push_seqs_kernel<c, p, sc, pp><<<static_cast<unsigned>(units), threads, 0, stream>>>(P, B->units, r, cast_scales);
+    else
+      kvbm_paged_repage_scatter_kernel<c, p, sc, pp><<<static_cast<unsigned>(units), threads, 0, stream>>>(P, r, cast_scales);
   });
   g_launches.fetch_add(1, std::memory_order_relaxed);
   const cudaError_t e = cudaGetLastError();
@@ -2412,6 +2479,32 @@ kvbm_kernels_paged_repage_scatter_streamed(const kvbm_permute_side* src, uint32_
   return launch_paged_repage_scatter(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, token_begin, token_end, layer_begin,
                                      layer_end, src_row_bytes, cast_mode, cast_scales, st->epoch, st->completion_flag, st->completion_value,
                                      stream, st);
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_repage_scatter_batch(const kvbm_permute_side* src, uint32_t src_num_heads, uint32_t src_page_size,
+                                        const kvbm_scatter_target* targets, int num_targets, uint32_t dst_page_size, const kvbm_repage_seq* seqs,
+                                        size_t num_seqs, const kvbm_repage_unit* units, size_t num_units, int layer_begin, int layer_end,
+                                        uint32_t src_row_bytes, int cast_mode, const float* cast_scales, uint32_t epoch,
+                                        uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
+{
+  const RepageBatch B{seqs, num_seqs, units, num_units};
+  return launch_paged_repage_scatter(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, 0, 0, layer_begin, layer_end,
+                                     src_row_bytes, cast_mode, cast_scales, epoch, completion_flag, completion_value, stream, nullptr, &B);
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_repage_scatter_batch_streamed(const kvbm_permute_side* src, uint32_t src_num_heads, uint32_t src_page_size,
+                                                 const kvbm_scatter_target* targets, int num_targets, uint32_t dst_page_size,
+                                                 const kvbm_repage_seq* seqs, size_t num_seqs, const kvbm_repage_unit* units, size_t num_units,
+                                                 int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
+                                                 const kvbm_permute_stream* st, cudaStream_t stream)
+{
+  if (!stream_args_ok(st, 1)) return cudaErrorInvalidValue;
+  const RepageBatch B{seqs, num_seqs, units, num_units};
+  return launch_paged_repage_scatter(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, 0, 0, layer_begin, layer_end,
+                                     src_row_bytes, cast_mode, cast_scales, st->epoch, st->completion_flag, st->completion_value, stream, st,
+                                     &B);
 }
 
 extern "C" cudaError_t

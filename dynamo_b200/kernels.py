@@ -263,6 +263,14 @@ def lib() -> C.CDLL:
                                                                  i, C.c_uint32, C.c_uint32, C.c_uint32, i, i, C.c_uint32, i, vp,
                                                                  C.POINTER(PermuteStream), vp]
         L.kvbm_kernels_paged_repage_scatter_streamed.restype = i
+        L.kvbm_kernels_paged_repage_scatter_batch.argtypes = [C.POINTER(PermuteSide), C.c_uint32, C.c_uint32, C.POINTER(ScatterTarget), i,
+                                                              C.c_uint32, vp, sz, vp, sz, i, i, C.c_uint32, i, vp, C.c_uint32, vp, C.c_uint32,
+                                                              vp]
+        L.kvbm_kernels_paged_repage_scatter_batch.restype = i
+        L.kvbm_kernels_paged_repage_scatter_batch_streamed.argtypes = [C.POINTER(PermuteSide), C.c_uint32, C.c_uint32,
+                                                                       C.POINTER(ScatterTarget), i, C.c_uint32, vp, sz, vp, sz, i, i,
+                                                                       C.c_uint32, i, vp, C.POINTER(PermuteStream), vp]
+        L.kvbm_kernels_paged_repage_scatter_batch_streamed.restype = i
         L.kvbm_kernels_permute_strides.argtypes = [i, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64, C.c_uint64,
                                                    C.POINTER(C.c_uint64)]
         L.kvbm_kernels_permute_strides.restype = i
@@ -291,7 +299,8 @@ EXPORTED_SYMBOLS = [
     "kvbm_kernels_paged_stage_repage_gather", "kvbm_kernels_paged_stage_repage_gather_streamed",
     "kvbm_kernels_repage_batch_units", "kvbm_kernels_paged_stage_repage_gather_batch",
     "kvbm_kernels_paged_stage_repage_gather_batch_streamed", "kvbm_kernels_paged_repage_scatter",
-    "kvbm_kernels_paged_repage_scatter_streamed",
+    "kvbm_kernels_paged_repage_scatter_streamed", "kvbm_kernels_paged_repage_scatter_batch",
+    "kvbm_kernels_paged_repage_scatter_batch_streamed",
 ]
 
 
@@ -592,6 +601,36 @@ def paged_repage_scatter_streamed(src: PermuteSide, src_num_heads: int, src_page
     return lib().kvbm_kernels_paged_repage_scatter_streamed(C.byref(src), src_num_heads, src_page_size, arr, len(targets), dst_page_size,
                                                             token_begin, token_end, layer_begin, layer_end, src_row_bytes, int(cast_mode),
                                                             scales_ptr(cast_scales), C.byref(st) if st is not None else None, stream)
+
+
+def paged_repage_scatter_batch(src: PermuteSide, src_num_heads: int, src_page_size: int, targets: Sequence[ScatterTarget],
+                               dst_page_size: int, seqs: Sequence[Tuple[int, int]], units: int, num_units: int, layer_begin: int,
+                               layer_end: int, src_row_bytes: int, cast_mode: int = 0, cast_scales=None, epoch: int = 0,
+                               completion_flag: int = 0, completion_value: int = 0, stream: int = 0) -> int:
+    """`paged_repage_scatter` over a batch of sequences in ONE launch with one signal: `seqs` are the (token_begin, token_end)
+    ranges, the source's and every target's block_ids the concatenation of the per-sequence tables, `units` the device address of
+    the table `repage_batch_units` made for the same ranges and pages (Ps, Pd).  Two sequences must not share a destination block
+    of one target pool.  include/kvbm_kernels.h (kvbm_kernels_paged_repage_scatter_batch)."""
+    arr = (ScatterTarget * max(1, len(targets)))(*targets)
+    return lib().kvbm_kernels_paged_repage_scatter_batch(C.byref(src), src_num_heads, src_page_size, arr, len(targets), dst_page_size,
+                                                         C.cast(_repage_seqs(seqs), C.c_void_p), len(seqs), units or None, num_units,
+                                                         layer_begin, layer_end, src_row_bytes, int(cast_mode), scales_ptr(cast_scales),
+                                                         epoch, completion_flag or None, completion_value, stream)
+
+
+def paged_repage_scatter_batch_streamed(src: PermuteSide, src_num_heads: int, src_page_size: int, targets: Sequence[ScatterTarget],
+                                        dst_page_size: int, seqs: Sequence[Tuple[int, int]], units: int, num_units: int,
+                                        layer_begin: int, layer_end: int, src_row_bytes: int, cast_mode: int, cast_scales,
+                                        st: Optional[PermuteStream], stream: int = 0) -> int:
+    """`paged_repage_scatter_batch` streamed with `paged_repage_scatter_streamed`'s flags: one ready flag per source layer covers
+    the batch, and layer_done_flags[l] is written once source layer l of every sequence landed in every target.
+    include/kvbm_kernels.h (kvbm_kernels_paged_repage_scatter_batch_streamed)."""
+    arr = (ScatterTarget * max(1, len(targets)))(*targets)
+    return lib().kvbm_kernels_paged_repage_scatter_batch_streamed(C.byref(src), src_num_heads, src_page_size, arr, len(targets),
+                                                                  dst_page_size, C.cast(_repage_seqs(seqs), C.c_void_p), len(seqs),
+                                                                  units or None, num_units, layer_begin, layer_end, src_row_bytes,
+                                                                  int(cast_mode), scales_ptr(cast_scales),
+                                                                  C.byref(st) if st is not None else None, stream)
 
 
 def permute_strides(kv_layout: int, num_layers: int, outer_dim: int, num_heads: int, page_size: int, row_bytes: int,

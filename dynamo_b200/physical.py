@@ -134,6 +134,12 @@ class _CRepageBatchSeq(C.Structure):
                 ("dst_ids", C.c_void_p), ("n_dst", C.c_size_t)]
 
 
+class _CScatterBatchSeq(C.Structure):
+    """struct kvbm_scatter_batch_seq"""
+    _fields_ = [("token_begin", C.c_size_t), ("token_end", C.c_size_t), ("src_ids", C.c_void_p), ("n_src", C.c_size_t),
+                ("dst_ids", C.c_void_p), ("n_dst", C.c_size_t)]
+
+
 class _CLayerStream(C.Structure):
     """struct kvbm_layer_stream"""
     _fields_ = [("src_layer_ready_flags", C.c_void_p), ("num_srcs", C.c_size_t), ("layer_done_flags", C.c_void_p)]
@@ -255,7 +261,7 @@ EXPORTED_SYMBOLS = [
     "kvbm_manager_execute_repage_gather", "kvbm_manager_execute_gather_streamed", "kvbm_manager_execute_repage_gather_streamed",
     "kvbm_tp_pp_reshard_plan", "kvbm_manager_execute_stage_gather", "kvbm_manager_execute_stage_repage_gather",
     "kvbm_manager_execute_repage_batch", "kvbm_tp_pp_scatter_plan", "kvbm_manager_execute_repage_scatter",
-    "kvbm_manager_execute_repage_scatter_streamed",
+    "kvbm_manager_execute_repage_scatter_streamed", "kvbm_manager_execute_repage_scatter_batch",
 ]
 
 
@@ -323,6 +329,8 @@ def lib() -> C.CDLL:
                                                           P(_COptions), P(u64)]
         L.kvbm_manager_execute_repage_scatter_streamed.argtypes = [vp, u64, vp, sz, sz, P(u64), P(P(sz)), sz, sz, sz, P(_CScatterWindow),
                                                                    sz, P(_CLayerStream), P(_COptions), P(u64)]
+        L.kvbm_manager_execute_repage_scatter_batch.argtypes = [vp, u64, sz, P(u64), P(_CScatterBatchSeq), sz, P(_CScatterWindow), sz,
+                                                                P(_CLayerStream), P(_COptions), P(u64)]
         L.kvbm_notification_is_complete.argtypes = [vp, u64]
         L.kvbm_notification_wait.argtypes = [vp, u64, C.c_int64]
         L.kvbm_manager_bytes_moved.argtypes = [vp]
@@ -934,6 +942,34 @@ class TransferManager:
         tok = C.c_uint64()
         o = (options or TransferOptions())._c()
         _check(lib().kvbm_manager_execute_repage_scatter_streamed(self._h, *args, C.byref(ls), C.byref(o), C.byref(tok)))
+        return TransferCompleteNotification(self, tok.value)
+
+    def execute_repage_scatter_batch(self, src: int, dsts: Sequence[int], seqs: Sequence[tuple], plan: Sequence[ScatterWindow],
+                                     options: Optional[TransferOptions] = None, ready_flags: Optional[int] = None,
+                                     layer_done_flags: int = 0) -> TransferCompleteNotification:
+        """A prefill batch's sequences pushed to every decode rank that needs them, as ONE hand-off
+        (kvbm_manager_execute_repage_scatter_batch): `seqs` is a list of (tokens, src_block_ids, [dst_block_ids per destination]),
+        each what `execute_repage_scatter` takes for one request, under one `plan` (`tp_pp_scatter_plan` passes as it is).  One
+        staged copy of every table, one launch, one notification; `options.per_dst_done_flags` and `options.done_flag` are written
+        once, after every sequence landed.  With `ready_flags` (the address of the source's [num_layers] u32 ready flags) it streams
+        as `execute_repage_scatter_streamed` does, and `layer_done_flags[l]` is written once source layer l of every sequence
+        landed.  Two sequences may share source blocks; a destination block may appear once per destination in the whole batch.
+        The first rejected sequence raises what `execute_repage_scatter` would raise for it."""
+        keep, cs, ws = [], (_CScatterBatchSeq * max(1, len(seqs)))(), None
+        for c, (tokens, src_ids, dst_ids) in zip(cs, seqs):
+            args = self._scatter_args(src, src_ids, dsts, dst_ids, plan, tokens)
+            _, s, ns, _, _, dp, n_dst, tb, te, ws, _ = args
+            keep.append(args)
+            c.token_begin, c.token_end, c.src_ids, c.n_src = tb, te, s if isinstance(s, int) else C.addressof(s), ns
+            c.dst_ids, c.n_dst = C.addressof(dp), n_dst
+        if ws is None:
+            ws = self._scatter_args(src, [], dsts, [[]] * len(dsts), plan, range(0, 0))[9]
+        hs = (C.c_uint64 * max(1, len(dsts)))(*dsts)
+        ls = self._layer_stream([0], {0: ready_flags}, layer_done_flags) if ready_flags is not None else None
+        tok = C.c_uint64()
+        o = (options or TransferOptions())._c()
+        _check(lib().kvbm_manager_execute_repage_scatter_batch(self._h, src, len(dsts), hs, cs, len(seqs), ws, len(plan),
+                                                               C.byref(ls) if ls is not None else None, C.byref(o), C.byref(tok)))
         return TransferCompleteNotification(self, tok.value)
 
     @staticmethod

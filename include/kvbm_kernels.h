@@ -570,6 +570,43 @@ cudaError_t kvbm_kernels_paged_repage_scatter_streamed(const kvbm_permute_side* 
                                                        uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
                                                        const kvbm_permute_stream* st, cudaStream_t stream);
 
+/* kvbm_kernels_paged_repage_scatter over a batch of sequences: what a continuous-batching prefill step finishes at once, each
+ * sequence with its own prefix-cache hit (token_begin, often inside a block), length and block tables, pushed to every target in
+ * ONE launch.  Source, targets, windows, pages, layer range, formats, cast and scales are the launch's, as there; the token ranges
+ * are `seqs` (host memory).  Concatenated tables: src->block_ids and every target's side.block_ids are concatenations in batch
+ * order, sequence i contributing its table[token_begin / P .. ceil(token_end / P)) for that side's page P (nothing when its range
+ * is empty).  Every target has Pd, so every target's concatenated table has the same per-sequence offsets, and the unit table of
+ * kvbm_kernels_repage_batch_units(seqs, Ps, Pd) serves every target: `units` is device-accessible memory holding what it
+ * produced, the caller's memory, read by the kernel and not on the host, valid until the launch has run.
+ * Equivalence: a batch of one sequence writes exactly the bytes of kvbm_kernels_paged_repage_scatter with that range, and a batch
+ * of n the bytes of n such launches in any order.  Two sequences may share SOURCE blocks (a shared prefix).  Within one target
+ * pool, two sequences must not share a DESTINATION block: the entry cannot read device ids, so this is the caller's rule.
+ * One signal for the batch: every target's done_flag and completion_flag are written once, after every sequence landed.
+ * num_seqs == 0, only empty ranges, or an empty layer range move nothing and still signal.  cudaErrorInvalidValue, before any
+ * CUDA call, for: every rule of kvbm_kernels_paged_repage_scatter but the token range's; any rule of
+ * kvbm_kernels_repage_batch_units (a null seqs with num_seqs > 0 among them); a num_units other than the helper's count; a null
+ * units with num_units > 0; num_units * layers * outer_dim of 2^31 or more. */
+cudaError_t kvbm_kernels_paged_repage_scatter_batch(const kvbm_permute_side* src, uint32_t src_num_heads, uint32_t src_page_size,
+                                                    const kvbm_scatter_target* targets, int num_targets, uint32_t dst_page_size,
+                                                    const kvbm_repage_seq* seqs, size_t num_seqs, const kvbm_repage_unit* units,
+                                                    size_t num_units, int layer_begin, int layer_end, uint32_t src_row_bytes,
+                                                    int cast_mode, const float* cast_scales, uint32_t epoch, uint32_t* completion_flag,
+                                                    uint32_t completion_value, cudaStream_t stream);
+
+/* The batch streamed with kvbm_kernels_paged_repage_scatter_streamed's flag conventions.  A prefill batch computes layer l for
+ * all its sequences together, so one ready flag per source layer covers the whole batch, and layer_done_flags[l] is written once
+ * source layer l of EVERY sequence landed in every target that takes it.  After a gate timeout no done flag is written (neither
+ * st->done_flag nor any target's) and completion_flag becomes 0xFFFFFFFF.  The stream-wait form launches the batch once per
+ * source layer and writes the target done flags after the last layer only.  The argument rules are the batch's plus the gate's
+ * with one source; a batch that moves nothing waits for nothing, writes the done flags and the completion word at once and no
+ * layer_done_flags. */
+cudaError_t kvbm_kernels_paged_repage_scatter_batch_streamed(const kvbm_permute_side* src, uint32_t src_num_heads, uint32_t src_page_size,
+                                                             const kvbm_scatter_target* targets, int num_targets, uint32_t dst_page_size,
+                                                             const kvbm_repage_seq* seqs, size_t num_seqs, const kvbm_repage_unit* units,
+                                                             size_t num_units, int layer_begin, int layer_end, uint32_t src_row_bytes,
+                                                             int cast_mode, const float* cast_scales, const kvbm_permute_stream* st,
+                                                             cudaStream_t stream);
+
 /* Host-only (no GPU): the stride table kvbm_kernels_paged_permute walks with for one side.  out[0] = 1 when offsets count
  * from the block's first byte (universal formats) or 0 when they count from the (layer, outer) region's first byte; the
  * element (layer l, outer o, head h, token t) then sits at  [out[0] ? l * out[1] + o * out[2] : 0] + h * out[3] + t * out[4].

@@ -510,6 +510,35 @@ int kvbm_manager_execute_repage_scatter_streamed(kvbm_transfer_manager* m, kvbm_
                                                  size_t num_windows, const kvbm_layer_stream* ls, const kvbm_transfer_options* opts,
                                                  kvbm_notification* out);
 
+/* One sequence of kvbm_manager_execute_repage_scatter_batch: the arguments kvbm_manager_execute_repage_scatter takes per request. */
+typedef struct kvbm_scatter_batch_seq {
+  size_t token_begin, token_end;
+  const size_t* src_ids;        /* the source's table[token_begin / Ps .. ceil(token_end / Ps)) */
+  size_t n_src;
+  const size_t* const* dst_ids; /* [num_dsts] lists of n_dst ids: destination d's table[token_begin / Pd .. ceil(token_end / Pd)) */
+  size_t n_dst;
+} kvbm_scatter_batch_seq;
+
+/* A prefill batch's sequences pushed to every decode rank that needs them, as ONE hand-off: kvbm_manager_execute_repage_scatter
+ * for every sequence of seqs[], each with its own token range and block tables, under one plan (a kvbm_tp_pp_scatter_plan passes as
+ * it is), one set of destinations and one set of options -- one staged copy of the source's and every destination's concatenated
+ * tables, the batch's unit table and, with ls, the gate's workspace; one kvbm_kernels_paged_repage_scatter_batch launch (its
+ * streamed form with ls); one notification.  ls (nullable) streams it as kvbm_manager_execute_repage_scatter_streamed does, with
+ * ls->num_srcs == 1: one ready flag per source layer covers the whole batch, and layer_done_flags[l] is written once source layer l
+ * of every sequence landed in every destination that takes it.  per_dst_done_flags and done_flag are written once, after every
+ * sequence landed (never after a gate timeout).  Two sequences may share source blocks (a shared prefix); a destination block may
+ * appear once per destination in the whole batch.  Errors, first one wins: with ls, its shape (as the streamed scatter); then,
+ * sequence by sequence in batch order, every check of kvbm_manager_execute_repage_scatter (and, with ls, of its streamed form) with
+ * its code and text, so the first rejected sequence returns what the single call would have returned for it (a batch without
+ * sequences still has its windows checked); then, for each destination, its concatenated ids unique (KVBM_ERR_DUPLICATE_DST) and,
+ * where the source is that destination's layout, disjoint from the concatenated source ids (KVBM_ERR_OVERLAP).  A batch whose
+ * sequences or layer range are all empty returns KVBM_OK with nothing launched.  bytes_moved counts the sum of what the single
+ * calls would.  Per-sequence completion words are not provided. */
+int kvbm_manager_execute_repage_scatter_batch(kvbm_transfer_manager* m, kvbm_layout_handle src, size_t num_dsts, const kvbm_layout_handle* dsts,
+                                              const kvbm_scatter_batch_seq* seqs, size_t num_seqs, const kvbm_scatter_window* windows,
+                                              size_t num_windows, const kvbm_layer_stream* ls, const kvbm_transfer_options* opts,
+                                              kvbm_notification* out);
+
 /* Completion: the transfer's last warp writes a flag in pinned host memory (no cudaEventQuery polling). */
 int kvbm_notification_is_complete(kvbm_transfer_manager* m, kvbm_notification n);  /* 1 / 0 / <0 error */
 int kvbm_notification_wait(kvbm_transfer_manager* m, kvbm_notification n, int64_t timeout_us);
