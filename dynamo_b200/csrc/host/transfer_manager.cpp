@@ -1218,6 +1218,34 @@ static int check_gather_windows(size_t num_srcs, const kvbm_layout_handle* srcs,
   return KVBM_OK;
 }
 
+// Layer window j (a kvbm_shard_window or kvbm_scatter_window) inside the source's snl layers and the destination's dnl.
+template <class Window>
+static int check_window_layers(const Window& w, size_t j, size_t snl, size_t dnl)
+{
+  if (w.src_layer_begin > snl || w.layer_count > snl - w.src_layer_begin)
+    return fail(KVBM_ERR_RANGE, "window " + std::to_string(j) + "'s source layers " + std::to_string(w.src_layer_begin) + ".." +
+                                    std::to_string(w.src_layer_begin + w.layer_count) + " exceed the source's num_layers " + std::to_string(snl));
+  if (w.dst_layer_begin > dnl || w.layer_count > dnl - w.dst_layer_begin)
+    return fail(KVBM_ERR_RANGE, "window " + std::to_string(j) + "'s destination layers " + std::to_string(w.dst_layer_begin) + ".." +
+                                    std::to_string(w.dst_layer_begin + w.layer_count) + " exceed the destination's num_layers " +
+                                    std::to_string(dnl));
+  return KVBM_OK;
+}
+
+// Every layer of the options' range over `side`'s nl layers (the side `begin` counts) in some window; a range past them is
+// rejected by the range's own check.
+template <class Window>
+static int check_layers_covered(const Window* w, size_t nw, size_t Window::*begin, size_t nl, const kvbm_transfer_options& o, const char* side)
+{
+  const size_t lb = o.has_layer_range ? o.layer_begin : 0, le = o.has_layer_range ? std::min(o.layer_end, nl) : nl;
+  for (size_t l = lb; l < le; ++l) {
+    bool in = false;
+    for (size_t j = 0; j < nw && !in; ++j) in = l >= w[j].*begin && l - w[j].*begin < w[j].layer_count;
+    if (!in) return fail(KVBM_ERR_RANGE, std::string(side) + " layer " + std::to_string(l) + " of the layer range is in no window's layers");
+  }
+  return KVBM_OK;
+}
+
 // What a staged gather checks of its layer windows once the windows passed check_gather_windows, under the manager's lock:
 // the destination's handle, each layer window inside its source's and the destination's layers, and every destination layer of
 // the options' range inside some window (KVBM_ERR_RANGE).
@@ -1230,23 +1258,9 @@ static int check_stage_layers(kvbm_transfer_manager* m, const kvbm_layout_handle
   for (size_t j = 0; j < nw; ++j) {
     const Layout* S = m->find(srcs[sw[j].src_rank]);
     if (!S) return fail(KVBM_ERR_HANDLE, "invalid source handle");
-    const size_t snl = S->cfg.num_layers;
-    if (sw[j].src_layer_begin > snl || sw[j].layer_count > snl - sw[j].src_layer_begin)
-      return fail(KVBM_ERR_RANGE, "window " + std::to_string(j) + "'s source layers " + std::to_string(sw[j].src_layer_begin) + ".." +
-                                      std::to_string(sw[j].src_layer_begin + sw[j].layer_count) + " exceed the source's num_layers " +
-                                      std::to_string(snl));
-    if (sw[j].dst_layer_begin > dnl || sw[j].layer_count > dnl - sw[j].dst_layer_begin)
-      return fail(KVBM_ERR_RANGE, "window " + std::to_string(j) + "'s destination layers " + std::to_string(sw[j].dst_layer_begin) + ".." +
-                                      std::to_string(sw[j].dst_layer_begin + sw[j].layer_count) + " exceed the destination's num_layers " +
-                                      std::to_string(dnl));
+    if (int rc = check_window_layers(sw[j], j, S->cfg.num_layers, dnl)) return rc;
   }
-  const size_t lb = o.has_layer_range ? o.layer_begin : 0, le = o.has_layer_range ? std::min(o.layer_end, dnl) : dnl;
-  for (size_t l = lb; l < le; ++l) {  // a range past the destination's layers is resolve()'s to reject
-    bool in = false;
-    for (size_t j = 0; j < nw && !in; ++j) in = l >= sw[j].dst_layer_begin && l - sw[j].dst_layer_begin < sw[j].layer_count;
-    if (!in) return fail(KVBM_ERR_RANGE, "destination layer " + std::to_string(l) + " of the layer range is in no window's layers");
-  }
-  return KVBM_OK;
+  return check_layers_covered(sw, nw, &kvbm_shard_window::dst_layer_begin, dnl, o, "destination");
 }
 
 // A TP re-shard's assembly as one hand-off: every window is validated as the windowed execute_transfer of its (source,
@@ -1341,6 +1355,35 @@ static int repage_strategy(kvbm_transfer_manager* m, const Layout& S, const Layo
   return KVBM_OK;
 }
 
+// A re-paging request's checks after its pairs', in order: the token range, the layer range over `c`'s layers (*lb / *le), the
+// id counts the range implies and non-null id lists.  The per-window lists follow, the caller's own.
+static int check_repage_range(size_t tb, size_t te, const kvbm_layout_config& c, const kvbm_transfer_options& o, size_t ps, size_t pd, size_t n_src,
+                              const void* src_ids, size_t n_dst, const void* dst_ids, size_t* lb, size_t* le)
+{
+  if (tb > te || te > (size_t{1} << 31))
+    return fail(KVBM_ERR_RANGE, "Token range " + std::to_string(tb) + ".." + std::to_string(te) + " is reversed or reaches past 2^31 tokens");
+  int rc;
+  if ((rc = check_layer_range(c, o, lb, le)) || (rc = check_repage_counts(tb, te, ps, pd, n_src, n_dst))) return rc;
+  if ((n_src && !src_ids) || (n_dst && !dst_ids)) return fail(KVBM_ERR, "null block id list");
+  return KVBM_OK;
+}
+
+// The last checks of a request with something to move, in order: each window's direct CUDA strategy (e[j].S to e[j].D[0]) and
+// one for all of them (else `mixed`, the error text), a CUDA device, the cast scales and, with ls, the flags of e[0 .. n_flagged).
+static int check_repage_launch(kvbm_transfer_manager* m, Transfer* e, size_t nw, const kvbm_transfer_options& o, const kvbm_layer_stream* ls,
+                               size_t n_flagged, const char* mixed)
+{
+  int rc;
+  for (size_t j = 0; j < nw; ++j) {
+    if ((rc = repage_strategy(m, *e[j].S, *e[j].D[0], &e[j].plan))) return rc;
+    if (e[j].plan.first != e[0].plan.first) return fail(KVBM_ERR_UNSUPPORTED, mixed);
+  }
+  if ((rc = need_cuda_device(m))) return rc;
+  if (o.cast_scales && (rc = check_cast_scales(m, o.cast_scales))) return rc;
+  if (ls && (rc = check_layer_stream_flags(m, *ls, e, n_flagged))) return rc;
+  return KVBM_OK;
+}
+
 // Re-paging hand-off: tokens [tb, te) of one sequence from the sources' block tables to the destination's, each side with its
 // own page size, as one launch with one notification.  Validated on its own (resolve() assumes one page size and equal id
 // counts), in the order below; a request that fails several checks reports the first.
@@ -1392,26 +1435,49 @@ static int check_repage_request(kvbm_transfer_manager* m, size_t num_srcs, const
                                              " has " + std::to_string(S->cfg.page_size));
   }
   const Layout& S0 = *e[0].S;
-  if (tb > te || te > (size_t{1} << 31))
-    return fail(KVBM_ERR_RANGE, "Token range " + std::to_string(tb) + ".." + std::to_string(te) + " is reversed or reaches past 2^31 tokens");
-  if ((rc = check_layer_range(layers ? D->cfg : S0.cfg, o, &R->lb, &R->le))) return rc;
-  if ((rc = check_repage_counts(tb, te, S0.cfg.page_size, D->cfg.page_size, n_src, n_dst))) return rc;
-  if ((n_src && !src_ids) || (n_dst && !dst_ids)) return fail(KVBM_ERR, "null block id list");
+  if ((rc = check_repage_range(tb, te, layers ? D->cfg : S0.cfg, o, S0.cfg.page_size, D->cfg.page_size, n_src, src_ids, n_dst, dst_ids, &R->lb,
+                               &R->le)))
+    return rc;
   for (size_t j = 0; j < nw; ++j) {
     const size_t r = e[j].window.src_rank;
     const size_t* s = n_src ? src_ids[r] : nullptr;
     if (n_src && !s) return fail(KVBM_ERR, "null block id list");
     if ((rc = check_block_ids(s, n_src, dst_ids, n_dst, e[j].S->cfg.num_blocks, D->cfg.num_blocks, srcs[r] == dst_h))) return rc;
   }
-  R->empty = tb == te || R->lb == R->le;
-  if (R->empty) return KVBM_OK;  // nothing to move, as execute()
-  for (size_t j = 0; j < nw; ++j) {
-    if ((rc = repage_strategy(m, *e[j].S, *D, &e[j].plan))) return rc;
-    if (e[j].plan.first != e[0].plan.first) return fail(KVBM_ERR_UNSUPPORTED, "the sources of a gather need the same CUDA strategy");
+  if ((R->empty = tb == te || R->lb == R->le)) return KVBM_OK;  // nothing to move, as execute()
+  return check_repage_launch(m, e, nw, o, ls, nw, "the sources of a gather need the same CUDA strategy");
+}
+
+// What a re-paging batch stages in its one copy: its non-empty sequences' ranges and each id list's tables, concatenated in batch
+// order, and the unit table.  lists[k]: list k's table, null for a list no window uses.
+struct BatchTables {
+  std::vector<kvbm_repage_seq> ranges;
+  std::vector<kvbm_repage_unit> units;
+  std::vector<std::vector<size_t>> cat;
+  std::vector<const size_t*> lists;
+};
+
+// List k of sequence q is ids(q, k): q.n_src ids for k < num_src_lists, else q.n_dst.  check(t->cat), the caller's duplicate-id
+// checks, runs before the unit table.  *n_src / *n_dst: each concatenated source and destination table's length.
+template <class Seq, class Ids, class Check>
+static int batch_tables(const Seq* seqs, size_t num_seqs, const std::vector<bool>& used, size_t num_src_lists, uint32_t ps, uint32_t pd,
+                        Ids ids, Check check, BatchTables* t, size_t* n_src, size_t* n_dst)
+{
+  t->cat.resize(used.size());
+  for (size_t i = 0; i < num_seqs; ++i) {
+    const Seq& q = seqs[i];
+    if (q.token_begin == q.token_end) continue;
+    t->ranges.push_back(kvbm_repage_seq{static_cast<uint32_t>(q.token_begin), static_cast<uint32_t>(q.token_end)});
+    for (size_t k = 0; k < used.size(); ++k)
+      if (used[k]) t->cat[k].insert(t->cat[k].end(), ids(q, k), ids(q, k) + (k < num_src_lists ? q.n_src : q.n_dst));
   }
-  if ((rc = need_cuda_device(m))) return rc;
-  if (o.cast_scales && (rc = check_cast_scales(m, o.cast_scales))) return rc;
-  if (ls && (rc = check_layer_stream_flags(m, *ls, e, nw))) return rc;
+  if (int rc = check(t->cat)) return rc;
+  size_t num_units = 0;
+  if (kvbm_kernels_repage_batch_units(t->ranges.data(), t->ranges.size(), ps, pd, nullptr, 0, &num_units, n_src, n_dst))
+    return fail(KVBM_ERR, "the batch's token ranges and page sizes have no unit table");
+  t->units.resize(num_units);
+  kvbm_kernels_repage_batch_units(t->ranges.data(), t->ranges.size(), ps, pd, t->units.data(), t->units.size(), &num_units, n_src, n_dst);
+  for (size_t k = 0; k < used.size(); ++k) t->lists.push_back(used[k] ? t->cat[k].data() : nullptr);
   return KVBM_OK;
 }
 
@@ -1454,39 +1520,26 @@ static int execute_repage(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_
   const size_t* const* src_ids = seqs[0].src_ids;
   const size_t* dst_ids = seqs[0].dst_ids;
   size_t n_src = seqs[0].n_src, n_dst = seqs[0].n_dst;
-  std::vector<kvbm_repage_seq> ranges;
-  std::vector<kvbm_repage_unit> units;
-  std::vector<std::vector<size_t>> cat;  // a batch's: each source's concatenated table, then the destination's
-  std::vector<const size_t*> lists;
+  BatchTables bt;
   if (batch) {
-    cat.resize(num_srcs + 1);
-    std::vector<bool> read(num_srcs, false);  // the sources some window reads: the others' tables may be null
-    for (size_t j = 0; j < nw; ++j) read[windows[j].src_rank] = true;
-    for (size_t i = 0; i < num_seqs; ++i) {
-      const kvbm_repage_batch_seq& q = seqs[i];
-      if (q.token_begin == q.token_end) continue;
-      ranges.push_back(kvbm_repage_seq{static_cast<uint32_t>(q.token_begin), static_cast<uint32_t>(q.token_end)});
-      for (size_t r = 0; r < num_srcs; ++r)
-        if (read[r]) cat[r].insert(cat[r].end(), q.src_ids[r], q.src_ids[r] + q.n_src);
-      cat[num_srcs].insert(cat[num_srcs].end(), q.dst_ids, q.dst_ids + q.n_dst);
-    }
-    const std::vector<size_t>& cd = cat[num_srcs];
-    for (size_t j = 0; j < nw; ++j) {  // the destination's uniqueness once; a source in the destination's layout also against it
-      const size_t r = windows[j].src_rank;
-      const bool same = srcs[r] == dst_h;
-      if ((j == 0 || same) &&
-          (rc = check_block_ids(cat[r].data(), cat[r].size(), cd.data(), cd.size(), e[j].S->cfg.num_blocks, D->cfg.num_blocks, same)))
-        return rc;
-    }
-    size_t num_units = 0;
-    if (kvbm_kernels_repage_batch_units(ranges.data(), ranges.size(), ups, upd, nullptr, 0, &num_units, &n_src, &n_dst))
-      return fail(KVBM_ERR, "the batch's token ranges and page sizes have no unit table");
-    units.resize(num_units);
-    kvbm_kernels_repage_batch_units(ranges.data(), ranges.size(), ups, upd, units.data(), units.size(), &num_units, &n_src, &n_dst);
-    lists.resize(num_srcs);
-    for (size_t r = 0; r < num_srcs; ++r) lists[r] = read[r] ? cat[r].data() : nullptr;
-    src_ids = lists.data();
-    dst_ids = cd.data();
+    std::vector<bool> used(num_srcs + 1, false);  // the sources some window reads (the others' tables may be null), the destination
+    for (size_t j = 0; j < nw; ++j) used[windows[j].src_rank] = true;
+    used[num_srcs] = true;
+    auto ids = [&](const kvbm_repage_batch_seq& q, size_t k) { return k < num_srcs ? q.src_ids[k] : q.dst_ids; };
+    auto unique = [&](const std::vector<std::vector<size_t>>& cat) -> int {
+      const std::vector<size_t>& cd = cat[num_srcs];
+      for (size_t j = 0; j < nw; ++j) {  // the destination's uniqueness once; a source in the destination's layout also against it
+        const size_t r = windows[j].src_rank;
+        const bool same = srcs[r] == dst_h;
+        if (j == 0 || same)
+          if (int rc = check_block_ids(cat[r].data(), cat[r].size(), cd.data(), cd.size(), e[j].S->cfg.num_blocks, D->cfg.num_blocks, same))
+            return rc;
+      }
+      return KVBM_OK;
+    };
+    if ((rc = batch_tables(seqs, num_seqs, used, num_srcs, ups, upd, ids, unique, &bt, &n_src, &n_dst))) return rc;
+    src_ids = bt.lists.data();
+    dst_ids = bt.lists[num_srcs];
   }
 
   DeviceGuard g(m->device);
@@ -1506,10 +1559,10 @@ static int execute_repage(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_
     if (batch) {
       const auto* du = reinterpret_cast<const kvbm_repage_unit*>(sl.dev_ids + units_at(num_srcs * n_src + n_dst));
       if (st)
-        return checked(kvbm_kernels_paged_stage_repage_gather_batch_streamed(ss, k, ups, &kd, dnh, upd, ranges.data(), ranges.size(), du,
-                                                                             units.size(), ilb, ile, row, o.cast_mode, o.cast_scales, st, stream),
+        return checked(kvbm_kernels_paged_stage_repage_gather_batch_streamed(ss, k, ups, &kd, dnh, upd, bt.ranges.data(), bt.ranges.size(), du,
+                                                                             bt.units.size(), ilb, ile, row, o.cast_mode, o.cast_scales, st, stream),
                        "kvbm_kernels_paged_stage_repage_gather_batch_streamed");
-      return checked(kvbm_kernels_paged_stage_repage_gather_batch(ss, k, ups, &kd, dnh, upd, ranges.data(), ranges.size(), du, units.size(), ilb,
+      return checked(kvbm_kernels_paged_stage_repage_gather_batch(ss, k, ups, &kd, dnh, upd, bt.ranges.data(), bt.ranges.size(), du, bt.units.size(), ilb,
                                                                   ile, row, o.cast_mode, o.cast_scales, o.done_flag, o.epoch, sl.host_flag, value,
                                                                   stream),
                      "kvbm_kernels_paged_stage_repage_gather_batch");
@@ -1522,8 +1575,8 @@ static int execute_repage(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_
                                                           o.done_flag, o.epoch, sl.host_flag, value, stream),
                    "kvbm_kernels_paged_stage_repage_gather");
   };
-  return launch_transform(m, e, nw, num_srcs, src_ids, n_src, dst_ids, n_dst, ls, o, stream, bytes, nullptr, out, launch, units.data(),
-                          units.size());
+  return launch_transform(m, e, nw, num_srcs, src_ids, n_src, dst_ids, n_dst, ls, o, stream, bytes, nullptr, out, launch, bt.units.data(),
+                          bt.units.size());
 }
 
 // The windows of a scatter, before any layout is looked up: at least one destination and one window, none in the options, at most
@@ -1581,26 +1634,9 @@ static int check_scatter_request(kvbm_transfer_manager* m, kvbm_layout_handle sr
   D.assign(num_dsts, nullptr);
   for (size_t d = 0; d < num_dsts; ++d)
     if (!(D[d] = m->find(dsts[d]))) return fail(KVBM_ERR_HANDLE, "invalid destination handle");
-  const size_t snl = S->cfg.num_layers;
-  for (size_t j = 0; j < nw; ++j) {
-    const size_t dnl = D[w[j].dst_rank]->cfg.num_layers;
-    if (w[j].src_layer_begin > snl || w[j].layer_count > snl - w[j].src_layer_begin)
-      return fail(KVBM_ERR_RANGE, "window " + std::to_string(j) + "'s source layers " + std::to_string(w[j].src_layer_begin) + ".." +
-                                      std::to_string(w[j].src_layer_begin + w[j].layer_count) + " exceed the source's num_layers " +
-                                      std::to_string(snl));
-    if (w[j].dst_layer_begin > dnl || w[j].layer_count > dnl - w[j].dst_layer_begin)
-      return fail(KVBM_ERR_RANGE, "window " + std::to_string(j) + "'s destination layers " + std::to_string(w[j].dst_layer_begin) + ".." +
-                                      std::to_string(w[j].dst_layer_begin + w[j].layer_count) + " exceed the destination's num_layers " +
-                                      std::to_string(dnl));
-  }
-  {
-    const size_t lb = o.has_layer_range ? o.layer_begin : 0, le = o.has_layer_range ? std::min(o.layer_end, snl) : snl;
-    for (size_t l = lb; l < le; ++l) {  // a range past the source's layers is check_layer_range's to reject
-      bool in = false;
-      for (size_t j = 0; j < nw && !in; ++j) in = l >= w[j].src_layer_begin && l - w[j].src_layer_begin < w[j].layer_count;
-      if (!in) return fail(KVBM_ERR_RANGE, "source layer " + std::to_string(l) + " of the layer range is in no window's layers");
-    }
-  }
+  for (size_t j = 0; j < nw; ++j)
+    if ((rc = check_window_layers(w[j], j, S->cfg.num_layers, D[w[j].dst_rank]->cfg.num_layers))) return rc;
+  if ((rc = check_layers_covered(w, nw, &kvbm_scatter_window::src_layer_begin, S->cfg.num_layers, o, "source"))) return rc;
   // the pair checks take the per-destination done flags, which a scatter honours, as absent
   kvbm_transfer_options op = o;
   op.per_dst_done_flags = nullptr;
@@ -1616,12 +1652,10 @@ static int check_scatter_request(kvbm_transfer_manager* m, kvbm_layout_handle sr
                                              " has " + std::to_string(D[w[0].dst_rank]->cfg.page_size) + ", destination " +
                                              std::to_string(w[j].dst_rank) + " has " + std::to_string(Dj.cfg.page_size));
   }
-  const size_t ps = S->cfg.page_size, pd = D[w[0].dst_rank]->cfg.page_size, tb = q.token_begin, te = q.token_end;
-  if (tb > te || te > (size_t{1} << 31))
-    return fail(KVBM_ERR_RANGE, "Token range " + std::to_string(tb) + ".." + std::to_string(te) + " is reversed or reaches past 2^31 tokens");
-  if ((rc = check_layer_range(S->cfg, o, &R->lb, &R->le))) return rc;
-  if ((rc = check_repage_counts(tb, te, ps, pd, q.n_src, q.n_dst))) return rc;
-  if ((q.n_src && !q.src_ids) || (q.n_dst && !q.dst_ids)) return fail(KVBM_ERR, "null block id list");
+  const size_t tb = q.token_begin, te = q.token_end;
+  if ((rc = check_repage_range(tb, te, S->cfg, o, S->cfg.page_size, D[w[0].dst_rank]->cfg.page_size, q.n_src, q.src_ids, q.n_dst, q.dst_ids,
+                               &R->lb, &R->le)))
+    return rc;
   for (size_t j = 0; j < nw; ++j) {
     const size_t d = w[j].dst_rank;
     if (q.n_dst && !q.dst_ids[d]) return fail(KVBM_ERR, "null block id list");
@@ -1629,16 +1663,8 @@ static int check_scatter_request(kvbm_transfer_manager* m, kvbm_layout_handle sr
                               src_h == dsts[d])))
       return rc;
   }
-  R->empty = tb == te || R->lb == R->le;
-  if (R->empty) return KVBM_OK;  // nothing to move, as execute()
-  for (size_t j = 0; j < nw; ++j) {
-    if ((rc = repage_strategy(m, *S, *e[j].D[0], &e[j].plan))) return rc;
-    if (e[j].plan.first != e[0].plan.first) return fail(KVBM_ERR_UNSUPPORTED, "the destinations of a scatter need the same CUDA strategy");
-  }
-  if ((rc = need_cuda_device(m))) return rc;
-  if (o.cast_scales && (rc = check_cast_scales(m, o.cast_scales))) return rc;
-  if (ls && (rc = check_layer_stream_flags(m, *ls, e, 1))) return rc;
-  return KVBM_OK;
+  if ((R->empty = tb == te || R->lb == R->le)) return KVBM_OK;  // nothing to move, as execute()
+  return check_repage_launch(m, e, nw, o, ls, 1, "the destinations of a scatter need the same CUDA strategy");
 }
 
 // One prefill rank's KV into every decode rank that needs it over a list of sequences, each the token range and tables of one
@@ -1688,35 +1714,23 @@ static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle s
   const size_t* src_ids = seqs[0].src_ids;
   const size_t* const* dst_ids = seqs[0].dst_ids;
   size_t n_src = seqs[0].n_src, n_dst = seqs[0].n_dst;
-  std::vector<kvbm_repage_seq> ranges;
-  std::vector<kvbm_repage_unit> units;
-  std::vector<std::vector<size_t>> cat;  // a batch's: the source's concatenated table, then each destination's
-  std::vector<const size_t*> cat_dst;
+  BatchTables bt;
   if (batch) {
-    std::vector<bool> named(num_dsts, false);  // the destinations some window writes: the others' tables may be null
-    for (size_t j = 0; j < nw; ++j) named[w[j].dst_rank] = true;
-    cat.resize(1 + num_dsts);
-    for (size_t i = 0; i < num_seqs; ++i) {
-      const kvbm_scatter_batch_seq& q = seqs[i];
-      if (q.token_begin == q.token_end) continue;
-      ranges.push_back(kvbm_repage_seq{static_cast<uint32_t>(q.token_begin), static_cast<uint32_t>(q.token_end)});
-      cat[0].insert(cat[0].end(), q.src_ids, q.src_ids + q.n_src);
+    std::vector<bool> used(1 + num_dsts, false);  // the source, the destinations some window writes (the others' tables may be null)
+    used[0] = true;
+    for (size_t j = 0; j < nw; ++j) used[1 + w[j].dst_rank] = true;
+    auto ids = [](const kvbm_scatter_batch_seq& q, size_t k) { return k ? q.dst_ids[k - 1] : q.src_ids; };
+    auto unique = [&](const std::vector<std::vector<size_t>>& cat) -> int {
       for (size_t d = 0; d < num_dsts; ++d)
-        if (named[d]) cat[1 + d].insert(cat[1 + d].end(), q.dst_ids[d], q.dst_ids[d] + q.n_dst);
-    }
-    for (size_t d = 0; d < num_dsts; ++d)
-      if (named[d] && (rc = check_block_ids(cat[0].data(), cat[0].size(), cat[1 + d].data(), cat[1 + d].size(), S->cfg.num_blocks,
-                                            D[d]->cfg.num_blocks, src_h == dsts[d])))
-        return rc;
-    size_t num_units = 0;
-    if (kvbm_kernels_repage_batch_units(ranges.data(), ranges.size(), ups, upd, nullptr, 0, &num_units, &n_src, &n_dst))
-      return fail(KVBM_ERR, "the batch's token ranges and page sizes have no unit table");
-    units.resize(num_units);
-    kvbm_kernels_repage_batch_units(ranges.data(), ranges.size(), ups, upd, units.data(), units.size(), &num_units, &n_src, &n_dst);
-    src_ids = cat[0].data();
-    cat_dst.resize(num_dsts);
-    for (size_t d = 0; d < num_dsts; ++d) cat_dst[d] = named[d] ? cat[1 + d].data() : nullptr;
-    dst_ids = cat_dst.data();
+        if (used[1 + d])
+          if (int rc = check_block_ids(cat[0].data(), cat[0].size(), cat[1 + d].data(), cat[1 + d].size(), S->cfg.num_blocks,
+                                       D[d]->cfg.num_blocks, src_h == dsts[d]))
+            return rc;
+      return KVBM_OK;
+    };
+    if ((rc = batch_tables(seqs, num_seqs, used, 1, ups, upd, ids, unique, &bt, &n_src, &n_dst))) return rc;
+    src_ids = bt.lists[0];
+    dst_ids = bt.lists.data() + 1;
   }
 
   DeviceGuard g(m->device);
@@ -1728,7 +1742,7 @@ static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle s
   for (size_t d = 0; d < num_dsts; ++d) lists[1 + d] = n_dst ? dst_ids[d] : nullptr;
   Slot* sl;
   uint64_t seq;
-  if ((rc = stage_ids(m, lists.data(), lens.data(), num_dsts + 1, ls ? snl + 4 : 4, stream, nullptr, &sl, &seq, units.data(), units.size())))
+  if ((rc = stage_ids(m, lists.data(), lens.data(), num_dsts + 1, ls ? snl + 4 : 4, stream, nullptr, &sl, &seq, bt.units.data(), bt.units.size())))
     return rc;
   const kvbm_permute_side ks{descriptor(*S), sl->dev_ids, e[0].src_kv};
   kvbm_scatter_target kt[KVBM_GATHER_MAX_SOURCES] = {};
@@ -1748,7 +1762,7 @@ static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle s
   if (ls) {
     const kvbm_permute_stream st = layer_stream(*ls, e, 1, o, *sl, seq);
     if (batch)
-      rc = checked(kvbm_kernels_paged_repage_scatter_batch_streamed(&ks, snh, ups, kt, k, upd, ranges.data(), ranges.size(), du, units.size(),
+      rc = checked(kvbm_kernels_paged_repage_scatter_batch_streamed(&ks, snh, ups, kt, k, upd, bt.ranges.data(), bt.ranges.size(), du, bt.units.size(),
                                                                     ilb, ile, row, o.cast_mode, o.cast_scales, &st, stream),
                    "kvbm_kernels_paged_repage_scatter_batch_streamed");
     else
@@ -1757,7 +1771,7 @@ static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle s
                    "kvbm_kernels_paged_repage_scatter_streamed");
   } else {
     if (batch)
-      rc = checked(kvbm_kernels_paged_repage_scatter_batch(&ks, snh, ups, kt, k, upd, ranges.data(), ranges.size(), du, units.size(), ilb, ile,
+      rc = checked(kvbm_kernels_paged_repage_scatter_batch(&ks, snh, ups, kt, k, upd, bt.ranges.data(), bt.ranges.size(), du, bt.units.size(), ilb, ile,
                                                            row, o.cast_mode, o.cast_scales, o.epoch, sl->host_flag, static_cast<uint32_t>(seq),
                                                            stream),
                    "kvbm_kernels_paged_repage_scatter_batch");

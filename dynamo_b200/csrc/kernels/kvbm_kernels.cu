@@ -748,6 +748,20 @@ __device__ __forceinline__ RepageUnit batch_unit(const kvbm_repage_unit* units, 
   return {w.x, w.y, w.z};
 }
 
+// The unit of a one-CTA-per-unit re-paging kernel, blockIdx.x = (big block j * nlayers + l - layer_begin) * no + o.  The caller
+// takes o = rem % no itself: the gathers after their stage lookup, the scatters before it.  Moving it changes how ptxas
+// schedules the division.
+struct RepageCta {
+  uint32_t j, l, rem;
+};
+__device__ __forceinline__ RepageCta repage_cta(const RepageGeom& G)
+{
+  const uint32_t unit = blockIdx.x;
+  const uint32_t j = unit / (G.nlayers * G.no);
+  const uint32_t rem = unit - j * (G.nlayers * G.no);
+  return {j, G.layer_begin + rem / G.no, rem};
+}
+
 // Where 16 B vector vv of a re-paging head's run sits: its 16 B column c, its token's slot q in the big block, and the small
 // block (entry small_k + b of the small table) and slot that hold the same token.
 struct RepageAt {
@@ -838,10 +852,8 @@ kvbm_paged_repage_kernel(const __grid_constant__ RepageParams P, RowSplit r, con
 {
   constexpr int IN = CAST == KVBM_CAST_BF16_TO_FP8E4M3 ? 2 : 1;
   constexpr int OUT = CAST == KVBM_CAST_FP8E4M3_TO_BF16 ? 2 : 1;
-  const uint32_t unit = blockIdx.x;  // (big block j * nlayers + l) * no + o
-  const uint32_t j = unit / (P.g.nlayers * P.g.no);
-  const uint32_t rem = unit - j * (P.g.nlayers * P.g.no);
-  const uint32_t l = P.g.layer_begin + rem / P.g.no, o = rem % P.g.no;
+  const auto [j, l, rem] = repage_cta(P.g);
+  const uint32_t o = rem % P.g.no;
   const RepageUnit u = repage_unit(P.g, j);
   const uint8_t* big_base = side_block(P.big, j, l, o);
   const uint8_t* small_base = side_region(P.small, l, o);
@@ -911,12 +923,8 @@ template <int CAST, bool POW2, bool SCALED, bool PPOW2>
 __global__ void __launch_bounds__(256, 3)
 kvbm_paged_repage_gather_kernel(const __grid_constant__ RepageGatherParams P, RowSplit r, const float* scales)
 {
-  const RepageGeom& G = P.geo;
-  const uint32_t unit = blockIdx.x;  // (big block j * nlayers + l) * no + o
-  const uint32_t j = unit / (G.nlayers * G.no);
-  const uint32_t rem = unit - j * (G.nlayers * G.no);
-  const uint32_t l = G.layer_begin + rem / G.no;
-  repage_gather_unit<CAST, POW2, SCALED, PPOW2>(P, stage_of(P.g, l), j, l, rem % G.no, r, scales);
+  const auto [j, l, rem] = repage_cta(P.geo);
+  repage_gather_unit<CAST, POW2, SCALED, PPOW2>(P, stage_of(P.g, l), j, l, rem % P.geo.no, r, scales);
 }
 
 // kvbm_paged_repage_gather_kernel over a batch of sequences: big block j is entry j of the concatenated big table and record j
@@ -925,12 +933,8 @@ template <int CAST, bool POW2, bool SCALED, bool PPOW2>
 __global__ void __launch_bounds__(256, 3)
 kvbm_paged_batch_repage_gather_kernel(const __grid_constant__ RepageGatherParams P, const kvbm_repage_unit* units, RowSplit r, const float* scales)
 {
-  const RepageGeom& G = P.geo;
-  const uint32_t unit = blockIdx.x;  // (big block j * nlayers + l) * no + o
-  const uint32_t j = unit / (G.nlayers * G.no);
-  const uint32_t rem = unit - j * (G.nlayers * G.no);
-  const uint32_t l = G.layer_begin + rem / G.no;
-  repage_gather_unit<CAST, POW2, SCALED, PPOW2, true>(P, stage_of(P.g, l), j, l, rem % G.no, r, scales, units);
+  const auto [j, l, rem] = repage_cta(P.geo);
+  repage_gather_unit<CAST, POW2, SCALED, PPOW2, true>(P, stage_of(P.g, l), j, l, rem % P.geo.no, r, scales, units);
 }
 
 // The re-paging scatter, the gather's mirror image: ONE source pool of page Ps (a prefill rank) into up to
@@ -1034,11 +1038,8 @@ template <int CAST, bool POW2, bool SCALED, bool PPOW2>
 __global__ void __launch_bounds__(256, 3)
 kvbm_paged_repage_scatter_kernel(const __grid_constant__ ScatterParams P, RowSplit r, const float* scales)
 {
-  const RepageGeom& G = P.geo;
-  const uint32_t unit = blockIdx.x;  // (big block j * nlayers + l) * no + o
-  const uint32_t j = unit / (G.nlayers * G.no);
-  const uint32_t rem = unit - j * (G.nlayers * G.no);
-  const uint32_t l = G.layer_begin + rem / G.no, o = rem % G.no;
+  const auto [j, l, rem] = repage_cta(P.geo);
+  const uint32_t o = rem % P.geo.no;
   scatter_unit<CAST, POW2, SCALED, PPOW2>(P, stage_of(P, l), j, l, o, r, scales);
 }
 
@@ -1049,11 +1050,8 @@ template <int CAST, bool POW2, bool SCALED, bool PPOW2>
 __global__ void __launch_bounds__(256, 3)
 kvbm_paged_repage_push_seqs_kernel(const __grid_constant__ ScatterParams P, const kvbm_repage_unit* units, RowSplit r, const float* scales)
 {
-  const RepageGeom& G = P.geo;
-  const uint32_t unit = blockIdx.x;  // (big block j * nlayers + l) * no + o
-  const uint32_t j = unit / (G.nlayers * G.no);
-  const uint32_t rem = unit - j * (G.nlayers * G.no);
-  const uint32_t l = G.layer_begin + rem / G.no, o = rem % G.no;
+  const auto [j, l, rem] = repage_cta(P.geo);
+  const uint32_t o = rem % P.geo.no;
   scatter_unit<CAST, POW2, SCALED, PPOW2, true>(P, stage_of(P, l), j, l, o, r, scales, units);
 }
 
@@ -1170,18 +1168,31 @@ kvbm_gated_gather_kernel(const __grid_constant__ GatherParams P, const __grid_co
   });
 }
 
+// gated_units over the units (l * num_big + j) * no + o of a re-paging launch's layer range G: unit(T, j, l, o) moves unit (big
+// block j, layer l, outer o), T being l's stage in P.
+template <class Params, class Unit, class MoreDone = NoMoreFlags>
+__device__ __forceinline__ void gated_repage_units(const GateArgs& A, const Params& P, const RepageGeom& G, uint32_t num_big, uint32_t batch,
+                                                   Unit unit, MoreDone more_done = MoreDone{})
+{
+  const uint32_t per_layer = num_big * G.no;
+  gated_units(
+      A, P, per_layer * G.nlayers, batch, [&](uint32_t u) { return G.layer_begin + u / per_layer; },
+      [&, unit](uint32_t u, uint32_t l, const GatherStage& T) {  // `unit` by value: by reference, ptxas schedules the loop differently
+        const uint32_t rem = u - (l - G.layer_begin) * per_layer;
+        const uint32_t j = rem / G.no;
+        unit(T, j, l, rem - j * G.no);
+      },
+      more_done);
+}
+
 // kvbm_paged_repage_gather_kernel's unit walk behind the gate; unit = (l * num_big + j) * no + o over the layer range.
 template <int CAST, bool POW2, bool SCALED, bool PPOW2>
 __global__ void __launch_bounds__(256)
 kvbm_gated_repage_gather_kernel(const __grid_constant__ RepageGatherParams P, const __grid_constant__ GateArgs A, uint32_t num_big, RowSplit r,
                                 const float* scales, uint32_t batch)
 {
-  const RepageGeom& G = P.geo;
-  const uint32_t per_layer = num_big * G.no;
-  gated_units(A, P.g, per_layer * G.nlayers, batch, [&](uint32_t u) { return G.layer_begin + u / per_layer; }, [&](uint32_t u, uint32_t l, const GatherStage& T) {
-    const uint32_t rem = u - (l - G.layer_begin) * per_layer;
-    const uint32_t j = rem / G.no;
-    repage_gather_unit<CAST, POW2, SCALED, PPOW2>(P, T, j, l, rem - j * G.no, r, scales);
+  gated_repage_units(A, P.g, P.geo, num_big, batch, [&](const GatherStage& T, uint32_t j, uint32_t l, uint32_t o) {
+    repage_gather_unit<CAST, POW2, SCALED, PPOW2>(P, T, j, l, o, r, scales);
   });
 }
 
@@ -1192,36 +1203,31 @@ __global__ void __launch_bounds__(256)
 kvbm_gated_batch_repage_gather_kernel(const __grid_constant__ RepageGatherParams P, const __grid_constant__ GateArgs A,
                                       const kvbm_repage_unit* units, uint32_t num_big, RowSplit r, const float* scales, uint32_t batch)
 {
-  const RepageGeom& G = P.geo;
-  const uint32_t per_layer = num_big * G.no;
-  gated_units(A, P.g, per_layer * G.nlayers, batch, [&](uint32_t u) { return G.layer_begin + u / per_layer; }, [&](uint32_t u, uint32_t l, const GatherStage& T) {
-    const uint32_t rem = u - (l - G.layer_begin) * per_layer;
-    const uint32_t j = rem / G.no;
-    repage_gather_unit<CAST, POW2, SCALED, PPOW2, true>(P, T, j, l, rem - j * G.no, r, scales, units);
+  gated_repage_units(A, P.g, P.geo, num_big, batch, [&](const GatherStage& T, uint32_t j, uint32_t l, uint32_t o) {
+    repage_gather_unit<CAST, POW2, SCALED, PPOW2, true>(P, T, j, l, o, r, scales, units);
   });
 }
 
+// The push kernels' hook in arrive_transfer: the num_flags target done flags of F, with A.ss's own and before the completion word.
+__device__ __forceinline__ auto target_done(const ScatterFlags& F, const int& num_flags, const GateArgs& A)
+{
+  return [&] {
+    for (int t = 0; t < num_flags; ++t)
+      if (F.done[t]) ptx::st_relaxed_sys(F.done[t], A.ss.epoch);
+  };
+}
+
 // kvbm_paged_repage_scatter_kernel's unit walk behind the one source's gate; unit = (l * num_big + j) * no + o over the source
-// layer range, so layer_done[l] counts source layer l in every target.  A.ss holds the stream's own done flag; the last CTA
-// writes the num_flags target done flags of F with it, before the completion word.
+// layer range, so layer_done[l] counts source layer l in every target.
 template <int CAST, bool POW2, bool SCALED, bool PPOW2>
 __global__ void __launch_bounds__(256, 1)
 kvbm_gated_repage_push_kernel(const __grid_constant__ ScatterParams P, const __grid_constant__ GateArgs A, const __grid_constant__ ScatterFlags F,
                               int num_flags, uint32_t num_big, RowSplit r, const float* scales, uint32_t batch)
 {
-  const RepageGeom& G = P.geo;
-  const uint32_t per_layer = num_big * G.no;
-  gated_units(
-      A, P, per_layer * G.nlayers, batch, [&](uint32_t u) { return G.layer_begin + u / per_layer; },
-      [&](uint32_t u, uint32_t l, const GatherStage& T) {
-        const uint32_t rem = u - (l - G.layer_begin) * per_layer;
-        const uint32_t j = rem / G.no;
-        scatter_unit<CAST, POW2, SCALED, PPOW2>(P, T, j, l, rem - j * G.no, r, scales);
-      },
-      [&]() {
-        for (int t = 0; t < num_flags; ++t)
-          if (F.done[t]) ptx::st_relaxed_sys(F.done[t], A.ss.epoch);
-      });
+  gated_repage_units(
+      A, P, P.geo, num_big, batch,
+      [&](const GatherStage& T, uint32_t j, uint32_t l, uint32_t o) { scatter_unit<CAST, POW2, SCALED, PPOW2>(P, T, j, l, o, r, scales); },
+      target_done(F, num_flags, A));
 }
 
 // kvbm_gated_repage_push_kernel over a batch of sequences (num_big: the length of `units`): source layer l is done once it landed
@@ -1231,19 +1237,10 @@ __global__ void __launch_bounds__(256, 1)
 kvbm_gated_repage_push_seqs_kernel(const __grid_constant__ ScatterParams P, const __grid_constant__ GateArgs A, const __grid_constant__ ScatterFlags F,
                                    int num_flags, const kvbm_repage_unit* units, uint32_t num_big, RowSplit r, const float* scales, uint32_t batch)
 {
-  const RepageGeom& G = P.geo;
-  const uint32_t per_layer = num_big * G.no;
-  gated_units(
-      A, P, per_layer * G.nlayers, batch, [&](uint32_t u) { return G.layer_begin + u / per_layer; },
-      [&](uint32_t u, uint32_t l, const GatherStage& T) {
-        const uint32_t rem = u - (l - G.layer_begin) * per_layer;
-        const uint32_t j = rem / G.no;
-        scatter_unit<CAST, POW2, SCALED, PPOW2, true>(P, T, j, l, rem - j * G.no, r, scales, units);
-      },
-      [&]() {
-        for (int t = 0; t < num_flags; ++t)
-          if (F.done[t]) ptx::st_relaxed_sys(F.done[t], A.ss.epoch);
-      });
+  gated_repage_units(
+      A, P, P.geo, num_big, batch,
+      [&](const GatherStage& T, uint32_t j, uint32_t l, uint32_t o) { scatter_unit<CAST, POW2, SCALED, PPOW2, true>(P, T, j, l, o, r, scales, units); },
+      target_done(F, num_flags, A));
 }
 
 // The stream-wait form's signal after layer l: its layer-done flag, and after the last layer the done and completion flags.
@@ -1541,6 +1538,36 @@ static bool heads_overlap(const kvbm_permute_source& a, const kvbm_permute_sourc
   return a.dst_head_begin < b.dst_head_begin + b.head_count && b.dst_head_begin < a.dst_head_begin + a.head_count;
 }
 
+// The stage of layer window [begin, end) (a gather's destination layers, the scatter's source layers) among T[0 .. *num_stages):
+// an equal window's, else a new one without sources; -1 when the window partly overlaps a stage.
+static int window_stage(GatherStage* T, int* num_stages, uint32_t begin, uint32_t end)
+{
+  int k = 0;
+  while (k < *num_stages && !(T[k].begin == begin && T[k].end == end)) {
+    if (begin < T[k].end && T[k].begin < end) return -1;  // a partial overlap
+    ++k;
+  }
+  if (k == *num_stages) T[(*num_stages)++] = GatherStage{begin, end, 0, 0, 0};
+  return k;
+}
+
+// order[i]: the i-th of window_stage's stages in ascending layers (an insertion sort of at most 16); whether they tile [lb, le).
+static bool order_stages(const GatherStage* T, int num_stages, int lb, int le, int* order)
+{
+  for (int k = 0; k < num_stages; ++k) {
+    int at = k;
+    while (at > 0 && T[order[at - 1]].begin > T[k].begin) {
+      order[at] = order[at - 1];
+      --at;
+    }
+    order[at] = k;
+  }
+  uint32_t reached = static_cast<uint32_t>(lb);
+  for (int i = 0; i < num_stages; ++i)
+    if (T[order[i]].begin <= reached && T[order[i]].end > reached) reached = T[order[i]].end;
+  return reached >= static_cast<uint32_t>(le);
+}
+
 // The sources of a gather into P->D (nl layers, dst_num_heads heads) over destination layers [lb, le): each layer window
 // non-empty and inside its source's own layers and the destination's; two windows equal (one stage) or disjoint in the
 // destination; the stages covering every layer of [lb, le); within a stage, windows on destination heads no other window of the
@@ -1557,32 +1584,15 @@ static bool fill_stage_sources(const kvbm_stage_source* srcs, int num_srcs, uint
     const kvbm_stage_source& X = srcs[s];
     const uint64_t src_end = static_cast<uint64_t>(X.src_layer_begin) + X.layer_count, dst_end = static_cast<uint64_t>(X.dst_layer_begin) + X.layer_count;
     if (X.layer_count == 0 || src_end > X.src.side.layout.num_layers || dst_end > nl) return false;
-    int k = 0;
-    while (k < num_stages && !(T[k].begin == X.dst_layer_begin && T[k].end == dst_end)) {
-      if (X.dst_layer_begin < T[k].end && T[k].begin < dst_end) return false;  // a partial overlap
-      ++k;
-    }
-    if (k == num_stages) T[num_stages++] = GatherStage{X.dst_layer_begin, static_cast<uint32_t>(dst_end), 0, 0, 0};
-    stage_of_src[s] = k;
+    const int k = stage_of_src[s] = window_stage(T, &num_stages, X.dst_layer_begin, static_cast<uint32_t>(dst_end));
+    if (k < 0) return false;
     for (int t = 0; t < s; ++t)
       if (stage_of_src[t] == k && heads_overlap(X.src, srcs[t].src)) return false;
     T[k].sources |= 1u << s;
     P->shift[s] = X.src_layer_begin - X.dst_layer_begin;
   }
-  // ascending destination layers (insertion sort of at most 16), then the range must be tiled
   int order[KVBM_GATHER_MAX_SOURCES];
-  for (int k = 0; k < num_stages; ++k) {
-    int at = k;
-    while (at > 0 && T[order[at - 1]].begin > T[k].begin) {
-      order[at] = order[at - 1];
-      --at;
-    }
-    order[at] = k;
-  }
-  uint32_t reached = static_cast<uint32_t>(lb);
-  for (int i = 0; i < num_stages; ++i)
-    if (T[order[i]].begin <= reached && T[order[i]].end > reached) reached = T[order[i]].end;
-  if (reached < static_cast<uint32_t>(le)) return false;
+  if (!order_stages(T, num_stages, lb, le, order)) return false;
   GatherStage sorted[KVBM_GATHER_MAX_SOURCES] = {};
   uint32_t covered = 0;
   *widest = 0;
@@ -1830,26 +1840,6 @@ static bool repage_pages(uint32_t src_page, uint32_t dst_page, int layer_begin, 
   return true;
 }
 
-// repage_pages plus one token range: slot arithmetic in 32 bits (every block of the larger page in the range ends below 2^32)
-// and fewer than 2^31 units.  Fills the range's fields of *G and the unit count.
-static bool repage_geometry(uint32_t src_page, uint32_t dst_page, uint32_t token_begin, uint32_t token_end, int layer_begin, int layer_end,
-                            uint32_t no, uint32_t src_row_bytes, int cast_mode, RepageGeom* G, RowSplit* r, uint64_t* dst_row_bytes,
-                            uint64_t* units, bool* page_pow2)
-{
-  RepageGeom g;
-  if (!repage_pages(src_page, dst_page, layer_begin, layer_end, no, src_row_bytes, cast_mode, &g, r, dst_row_bytes, page_pow2)) return false;
-  const uint64_t big_end = (static_cast<uint64_t>(token_end) + g.big_page - 1) / g.big_page * g.big_page;
-  if (big_end >= (1ull << 32)) return false;
-  g.big_first = token_begin / g.big_page;
-  g.small_first = token_begin / g.small_page;
-  g.token_begin = token_begin;
-  g.token_end = token_end;
-  *units = (static_cast<uint64_t>(big_end / g.big_page) - g.big_first) * g.nlayers * no;
-  if (*units >= (1ull << 31)) return false;
-  *G = g;
-  return true;
-}
-
 // A batch of sequences of a re-paging launch: the caller's ranges (host) and unit table (device-accessible).
 struct RepageBatch {
   const kvbm_repage_seq* seqs;
@@ -1858,13 +1848,63 @@ struct RepageBatch {
   size_t num_units;
 };
 
+// What repage_launch derives: repage_pages' results with the token range's fields, the units to launch (0: nothing to move), the
+// big blocks per (layer, outer), and the layers and outer dim of the pool whose layers the launch counts.
+struct RepageLaunch {
+  RepageGeom geo;
+  RowSplit r;
+  uint64_t dst_row_bytes, units;
+  uint32_t num_big, nl, no;
+  bool page_pow2;
+};
+
+// Every re-paging launch's first checks, before any CUDA call: ranges not reversed, cast_args_ok, and B checked by
+// kvbm_kernels_repage_batch_units with the caller's unit count.  An empty range or batch then leaves L->units 0 (the caller
+// signals).  Else `side` (a gather's destination, the scatter's source) needs a table, a base, a non-zero outer dim and the layer
+// range; the pages repage_pages' rules; a single range slots in 32 bits (its last block of the larger page ends below 2^32); the
+// launch fewer than 2^31 units.  False: rejected.
+static bool repage_launch(const kvbm_permute_side* side, uint32_t src_page, uint32_t dst_page, uint32_t token_begin, uint32_t token_end,
+                          int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales, const RepageBatch* B,
+                          RepageLaunch* L)
+{
+  if (layer_begin < 0 || layer_end < layer_begin || (!B && token_end < token_begin)) return false;
+  if (!cast_args_ok(cast_mode, cast_scales)) return false;
+  size_t num_big = 0;
+  if (B) {
+    size_t src_ids, dst_ids;
+    if (kvbm_kernels_repage_batch_units(B->seqs, B->num_seqs, src_page, dst_page, nullptr, 0, &num_big, &src_ids, &dst_ids) != 0) return false;
+    if (num_big != B->num_units || (num_big != 0 && !B->units)) return false;
+  }
+  L->units = 0;
+  if ((B ? num_big == 0 : token_end == token_begin) || layer_end == layer_begin) return true;
+  if (!side || !side->block_ids || !side->layout.layer_base) return false;
+  const uint32_t nl = L->nl = side->layout.num_layers, no = L->no = side->layout.outer_dim;
+  if (nl == 0 || no == 0 || static_cast<uint32_t>(layer_end) > nl) return false;
+  RepageGeom& g = L->geo;
+  if (!repage_pages(src_page, dst_page, layer_begin, layer_end, no, src_row_bytes, cast_mode, &g, &L->r, &L->dst_row_bytes, &L->page_pow2))
+    return false;
+  if (!B) {
+    const uint64_t big_end = (static_cast<uint64_t>(token_end) + g.big_page - 1) / g.big_page * g.big_page;
+    if (big_end >= (1ull << 32)) return false;
+    g.big_first = token_begin / g.big_page;
+    g.small_first = token_begin / g.small_page;
+    g.token_begin = token_begin;
+    g.token_end = token_end;
+    num_big = static_cast<size_t>(big_end / g.big_page) - g.big_first;
+  }
+  if (num_big >= (1ull << 31) || (L->units = static_cast<uint64_t>(num_big) * g.nlayers) >= (1ull << 31) || (L->units *= no) >= (1ull << 31))
+    return false;
+  L->num_big = static_cast<uint32_t>(num_big);
+  return true;
+}
+
 // Every re-paging launch: a plain re-page is one source whose window covers every head and every layer of both sides, a
-// re-paging gather one or more windows.  Runs the checks of launch_paged_permute's sources and of repage_geometry's pages, each
-// side's region at its own page and head count, all before any CUDA call; signals when there is nothing to move; then launches
-// kvbm_paged_repage_kernel for a plain re-page, else kvbm_paged_repage_gather_kernel, and the signal.  max_covered and st: as
-// launch_paged_permute's (st takes the gated re-paging gather kernel, or per layer this launch unstreamed).
-// B: a batch of sequences in place of the one token range (token_begin / token_end unused).  Its ranges and pages are checked
-// through kvbm_kernels_repage_batch_units, whose unit count must be the caller's; it always takes the batch gather kernels.
+// re-paging gather one or more windows.  Runs repage_launch's checks with the destination as the launch's side, and those of
+// launch_paged_permute's sources, each side's region at its own page and head count, all before any CUDA call; signals when
+// there is nothing to move; then launches kvbm_paged_repage_kernel for a plain re-page, else kvbm_paged_repage_gather_kernel,
+// and the signal.  max_covered and st: as launch_paged_permute's (st takes the gated re-paging gather kernel, or per layer this
+// launch unstreamed).  B: a batch of sequences in place of the one token range (token_begin / token_end unused), which always
+// takes the batch gather kernels.
 static cudaError_t launch_paged_repage_gather(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page, const kvbm_permute_side* dst,
                                               uint32_t dst_num_heads, uint32_t dst_page, uint32_t token_begin, uint32_t token_end,
                                               int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
@@ -1872,56 +1912,36 @@ static cudaError_t launch_paged_repage_gather(const kvbm_stage_source* srcs, int
                                               uint32_t max_covered, cudaStream_t stream, const kvbm_permute_stream* st = nullptr,
                                               const RepageBatch* B = nullptr)
 {
-  if (layer_begin < 0 || layer_end < layer_begin || (!B && token_end < token_begin)) return cudaErrorInvalidValue;
-  if (!cast_args_ok(cast_mode, cast_scales)) return cudaErrorInvalidValue;
-  if (!srcs || num_srcs < 1 || num_srcs > KVBM_GATHER_MAX_SOURCES) return cudaErrorInvalidValue;
-  size_t num_big = 0;
-  if (B) {
-    size_t src_ids, dst_ids;
-    if (kvbm_kernels_repage_batch_units(B->seqs, B->num_seqs, src_page, dst_page, nullptr, 0, &num_big, &src_ids, &dst_ids) != 0)
-      return cudaErrorInvalidValue;
-    if (num_big != B->num_units || (num_big != 0 && !B->units)) return cudaErrorInvalidValue;
-  }
-  if ((B ? num_big == 0 : token_end == token_begin) || layer_end == layer_begin)
-    return signal_launch(done_flag, epoch, completion_flag, completion_value, stream);
-  if (!dst || !dst->block_ids || !dst->layout.layer_base) return cudaErrorInvalidValue;
-  const uint32_t nl = dst->layout.num_layers, no = dst->layout.outer_dim;
-  if (nl == 0 || no == 0 || static_cast<uint32_t>(layer_end) > nl) return cudaErrorInvalidValue;
-  RepageGatherParams P{};
-  RowSplit r;
-  uint64_t dst_row_bytes, units;
-  bool page_pow2;
-  if (B) {
-    if (!repage_pages(src_page, dst_page, layer_begin, layer_end, no, src_row_bytes, cast_mode, &P.geo, &r, &dst_row_bytes, &page_pow2))
-      return cudaErrorInvalidValue;
-    if (num_big >= (1ull << 31) || (units = static_cast<uint64_t>(num_big) * P.geo.nlayers) >= (1ull << 31) || (units *= no) >= (1ull << 31))
-      return cudaErrorInvalidValue;
-  } else if (!repage_geometry(src_page, dst_page, token_begin, token_end, layer_begin, layer_end, no, src_row_bytes, cast_mode, &P.geo, &r,
-                              &dst_row_bytes, &units, &page_pow2)) {
+  RepageLaunch L;
+  if (!srcs || num_srcs < 1 || num_srcs > KVBM_GATHER_MAX_SOURCES ||
+      !repage_launch(dst, src_page, dst_page, token_begin, token_end, layer_begin, layer_end, src_row_bytes, cast_mode, cast_scales, B, &L))
     return cudaErrorInvalidValue;
-  }
-  if (static_cast<uint64_t>(dst_page) * dst_num_heads * dst_row_bytes != dst->layout.region_bytes) return cudaErrorInvalidValue;
-  if (!fill_permute_side(*dst, nl, no, dst_num_heads, dst_page, static_cast<uint32_t>(dst_row_bytes), &P.g.D)) return cudaErrorInvalidValue;
+  if (L.units == 0) return signal_launch(done_flag, epoch, completion_flag, completion_value, stream);
+  const uint32_t nl = L.nl, no = L.no;
+  const RowSplit& r = L.r;
+  RepageGatherParams P{};
+  P.geo = L.geo;
+  if (static_cast<uint64_t>(dst_page) * dst_num_heads * L.dst_row_bytes != dst->layout.region_bytes) return cudaErrorInvalidValue;
+  if (!fill_permute_side(*dst, nl, no, dst_num_heads, dst_page, static_cast<uint32_t>(L.dst_row_bytes), &P.g.D)) return cudaErrorInvalidValue;
   uint32_t widest;
   if (!fill_stage_sources(srcs, num_srcs, dst_num_heads, nl, no, layer_begin, layer_end, src_page, src_row_bytes, max_covered, &P.g, &widest))
     return cudaErrorInvalidValue;
   P.geo.nh = P.g.covered;
   const int threads = static_cast<int>(std::min<uint32_t>(8, widest)) * 32;
-  const unsigned grid = static_cast<unsigned>(units);
+  const unsigned grid = static_cast<unsigned>(L.units);
   if (st)
     return launch_streamed(
-        *st, P.g, num_srcs, nl, layer_begin, layer_end, units, stream,
+        *st, P.g, num_srcs, nl, layer_begin, layer_end, L.units, stream,
         [&](int l) {
           return launch_paged_repage_gather(srcs, num_srcs, src_page, dst, dst_num_heads, dst_page, token_begin, token_end, l, l + 1,
                                             src_row_bytes, cast_mode, cast_scales, nullptr, 0, nullptr, 0, max_covered, stream, nullptr, B);
         },
         [&](const GateArgs& A, unsigned ctas, uint32_t batch) {
-          const uint32_t nb = static_cast<uint32_t>(units / (static_cast<uint64_t>(P.geo.nlayers) * no));
-          with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, page_pow2, [&](auto c, auto p, auto sc, auto pp) {
+          with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, L.page_pow2, [&](auto c, auto p, auto sc, auto pp) {
             if (B)
-              kvbm_gated_batch_repage_gather_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, A, B->units, nb, r, cast_scales, batch);
+              kvbm_gated_batch_repage_gather_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, A, B->units, L.num_big, r, cast_scales, batch);
             else
-              kvbm_gated_repage_gather_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, A, nb, r, cast_scales, batch);
+              kvbm_gated_repage_gather_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, A, L.num_big, r, cast_scales, batch);
           });
         });
   // a window over every layer and every head of both sides (the checks above make its starts 0)
@@ -1931,7 +1951,7 @@ static cudaError_t launch_paged_repage_gather(const kvbm_stage_source* srcs, int
   R.big = P.geo.src_small ? P.g.D : P.g.src[0].S;
   R.small = P.geo.src_small ? P.g.src[0].S : P.g.D;
   R.g = P.geo;
-  with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, page_pow2, [&](auto c, auto p, auto sc, auto pp) {
+  with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, L.page_pow2, [&](auto c, auto p, auto sc, auto pp) {
     if (B)
       kvbm_paged_batch_repage_gather_kernel<c, p, sc, pp><<<grid, threads, 0, stream>>>(P, B->units, r, cast_scales);
     else if (plain)
@@ -1993,13 +2013,9 @@ static bool fill_scatter_targets(const kvbm_scatter_target* tg, int n, uint32_t 
     const uint64_t src_end = static_cast<uint64_t>(X.src_layer_begin) + X.layer_count;
     if (X.layer_count == 0 || src_end > src_nl || static_cast<uint64_t>(X.dst_layer_begin) + X.layer_count > L.num_layers) return false;
     if ((pairs += X.head_count) > KVBM_GATHER_MAX_HEADS) return false;
-    int k = 0;
-    while (k < num_stages && !(T[k].begin == X.src_layer_begin && T[k].end == src_end)) {
-      if (X.src_layer_begin < T[k].end && T[k].begin < src_end) return false;  // a partial overlap
-      ++k;
-    }
-    if (k == num_stages) T[num_stages++] = GatherStage{X.src_layer_begin, static_cast<uint32_t>(src_end), 0, 0, 1};  // the one source
-    stage_of_tgt[t] = k;
+    const int k = stage_of_tgt[t] = window_stage(T, &num_stages, X.src_layer_begin, static_cast<uint32_t>(src_end));
+    if (k < 0) return false;
+    T[k].sources = 1;  // the one source
     for (int u = 0; u < t; ++u) {
       const kvbm_scatter_target& Y = tg[u];
       if (Y.side.layout.layer_base == L.layer_base && Y.side.block_ids == X.side.block_ids &&
@@ -2010,20 +2026,8 @@ static bool fill_scatter_targets(const kvbm_scatter_target* tg, int n, uint32_t 
     P->tgt[t].shift = X.dst_layer_begin - X.src_layer_begin;
     P->tgt[t].head_delta = X.dst_head_begin - X.src_head_begin;
   }
-  // ascending source layers (insertion sort of at most 16), then the range must be tiled
   int order[KVBM_GATHER_MAX_SOURCES];
-  for (int k = 0; k < num_stages; ++k) {
-    int at = k;
-    while (at > 0 && T[order[at - 1]].begin > T[k].begin) {
-      order[at] = order[at - 1];
-      --at;
-    }
-    order[at] = k;
-  }
-  uint32_t reached = static_cast<uint32_t>(lb);
-  for (int i = 0; i < num_stages; ++i)
-    if (T[order[i]].begin <= reached && T[order[i]].end > reached) reached = T[order[i]].end;
-  if (reached < static_cast<uint32_t>(le)) return false;
+  if (!order_stages(T, num_stages, lb, le, order)) return false;
   // per stage: its (source head, target) pairs in ascending head, then target order, one entry per head
   GatherStage sorted[KVBM_GATHER_MAX_SOURCES] = {};
   uint32_t entries = 0, p = 0;
@@ -2062,49 +2066,30 @@ static bool fill_scatter_targets(const kvbm_scatter_target* tg, int n, uint32_t 
   return true;
 }
 
-// The scatter: every check before any CUDA call (the empty-range signal after the cast, range and target-count rules, as the
-// re-paging gather), then one kvbm_paged_repage_scatter_kernel launch and the signal.  st: a streamed launch (its flags are the
-// ones passed, and its done flag is written with the targets'), which takes the gated push kernel, or per source layer this
-// launch unstreamed.  B: a batch of sequences in place of the one token range (token_begin / token_end unused), checked as
-// launch_paged_repage_gather checks it; it always takes the push_seqs kernels.
+// The scatter: every check before any CUDA call (repage_launch's with the source as the launch's side, and the target-count rule
+// before them), then one kvbm_paged_repage_scatter_kernel launch and the signal.  st: a streamed launch (its flags are the ones
+// passed, and its done flag is written with the targets'), which takes the gated push kernel, or per source layer this launch
+// unstreamed.  B: a batch of sequences in place of the one token range (token_begin / token_end unused), which always takes the
+// push_seqs kernels.
 static cudaError_t launch_paged_repage_scatter(const kvbm_permute_side* src, uint32_t src_num_heads, uint32_t src_page,
                                                const kvbm_scatter_target* targets, int num_targets, uint32_t dst_page, uint32_t token_begin,
                                                uint32_t token_end, int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode,
                                                const float* cast_scales, uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value,
                                                cudaStream_t stream, const kvbm_permute_stream* st = nullptr, const RepageBatch* B = nullptr)
 {
-  if (layer_begin < 0 || layer_end < layer_begin || (!B && token_end < token_begin)) return cudaErrorInvalidValue;
-  if (!cast_args_ok(cast_mode, cast_scales)) return cudaErrorInvalidValue;
-  if (!targets || num_targets < 1 || num_targets > KVBM_GATHER_MAX_SOURCES) return cudaErrorInvalidValue;
-  size_t num_big = 0;
-  if (B) {
-    size_t src_ids, dst_ids;
-    if (kvbm_kernels_repage_batch_units(B->seqs, B->num_seqs, src_page, dst_page, nullptr, 0, &num_big, &src_ids, &dst_ids) != 0)
-      return cudaErrorInvalidValue;
-    if (num_big != B->num_units || (num_big != 0 && !B->units)) return cudaErrorInvalidValue;
-  }
-  if ((B ? num_big == 0 : token_end == token_begin) || layer_end == layer_begin)
-    return scatter_signal(targets, num_targets, st ? st->done_flag : nullptr, epoch, completion_flag, completion_value, stream);
-  if (!src || !src->block_ids || !src->layout.layer_base) return cudaErrorInvalidValue;
-  const uint32_t nl = src->layout.num_layers, no = src->layout.outer_dim;
-  if (nl == 0 || no == 0 || static_cast<uint32_t>(layer_end) > nl) return cudaErrorInvalidValue;
-  ScatterParams P{};
-  RowSplit r;
-  uint64_t dst_row_bytes, units;
-  bool page_pow2;
-  if (B) {
-    if (!repage_pages(src_page, dst_page, layer_begin, layer_end, no, src_row_bytes, cast_mode, &P.geo, &r, &dst_row_bytes, &page_pow2))
-      return cudaErrorInvalidValue;
-    if (num_big >= (1ull << 31) || (units = static_cast<uint64_t>(num_big) * P.geo.nlayers) >= (1ull << 31) || (units *= no) >= (1ull << 31))
-      return cudaErrorInvalidValue;
-  } else if (!repage_geometry(src_page, dst_page, token_begin, token_end, layer_begin, layer_end, no, src_row_bytes, cast_mode, &P.geo, &r,
-                              &dst_row_bytes, &units, &page_pow2)) {
+  RepageLaunch L;
+  if (!targets || num_targets < 1 || num_targets > KVBM_GATHER_MAX_SOURCES ||
+      !repage_launch(src, src_page, dst_page, token_begin, token_end, layer_begin, layer_end, src_row_bytes, cast_mode, cast_scales, B, &L))
     return cudaErrorInvalidValue;
-  }
+  if (L.units == 0) return scatter_signal(targets, num_targets, st ? st->done_flag : nullptr, epoch, completion_flag, completion_value, stream);
+  const uint32_t nl = L.nl, no = L.no;
+  const RowSplit& r = L.r;
+  ScatterParams P{};
+  P.geo = L.geo;
   if (static_cast<uint64_t>(src_page) * src_num_heads * src_row_bytes != src->layout.region_bytes) return cudaErrorInvalidValue;
   if (!fill_permute_side(*src, nl, no, src_num_heads, src_page, src_row_bytes, &P.S)) return cudaErrorInvalidValue;
   uint32_t widest;
-  if (!fill_scatter_targets(targets, num_targets, src_num_heads, nl, no, layer_begin, layer_end, dst_page, dst_row_bytes, &P, &widest))
+  if (!fill_scatter_targets(targets, num_targets, src_num_heads, nl, no, layer_begin, layer_end, dst_page, L.dst_row_bytes, &P, &widest))
     return cudaErrorInvalidValue;
   const int threads = static_cast<int>(std::min<uint32_t>(8, widest)) * 32;
   if (st) {
@@ -2113,7 +2098,7 @@ static cudaError_t launch_paged_repage_scatter(const kvbm_permute_side* src, uin
     std::copy(targets, targets + num_targets, quiet);
     for (int t = 0; t < num_targets; ++t) quiet[t].done_flag = nullptr;
     return launch_streamed(
-        *st, P, 1, nl, layer_begin, layer_end, units, stream,
+        *st, P, 1, nl, layer_begin, layer_end, L.units, stream,
         [&](int l) {
           return launch_paged_repage_scatter(src, src_num_heads, src_page, l + 1 == layer_end ? targets : quiet, num_targets, dst_page,
                                              token_begin, token_end, l, l + 1, src_row_bytes, cast_mode, cast_scales, epoch, nullptr, 0,
@@ -2124,21 +2109,20 @@ static cudaError_t launch_paged_repage_scatter(const kvbm_permute_side* src, uin
           bool any;
           const ScatterFlags F = scatter_flags(targets, num_targets, &any);
           Ag.ss.want_done |= any;
-          const uint32_t nb = static_cast<uint32_t>(units / (static_cast<uint64_t>(P.geo.nlayers) * no));
-          with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, page_pow2, [&](auto c, auto p, auto sc, auto pp) {
+          with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, L.page_pow2, [&](auto c, auto p, auto sc, auto pp) {
             if (B)
-              kvbm_gated_repage_push_seqs_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, Ag, F, num_targets, B->units, nb, r, cast_scales,
-                                                                                            batch);
+              kvbm_gated_repage_push_seqs_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, Ag, F, num_targets, B->units, L.num_big, r,
+                                                                                            cast_scales, batch);
             else
-              kvbm_gated_repage_push_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, Ag, F, num_targets, nb, r, cast_scales, batch);
+              kvbm_gated_repage_push_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, Ag, F, num_targets, L.num_big, r, cast_scales, batch);
           });
         });
   }
-  with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, page_pow2, [&](auto c, auto p, auto sc, auto pp) {
+  with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, L.page_pow2, [&](auto c, auto p, auto sc, auto pp) {
     if (B)
-      kvbm_paged_repage_push_seqs_kernel<c, p, sc, pp><<<static_cast<unsigned>(units), threads, 0, stream>>>(P, B->units, r, cast_scales);
+      kvbm_paged_repage_push_seqs_kernel<c, p, sc, pp><<<static_cast<unsigned>(L.units), threads, 0, stream>>>(P, B->units, r, cast_scales);
     else
-      kvbm_paged_repage_scatter_kernel<c, p, sc, pp><<<static_cast<unsigned>(units), threads, 0, stream>>>(P, r, cast_scales);
+      kvbm_paged_repage_scatter_kernel<c, p, sc, pp><<<static_cast<unsigned>(L.units), threads, 0, stream>>>(P, r, cast_scales);
   });
   g_launches.fetch_add(1, std::memory_order_relaxed);
   const cudaError_t e = cudaGetLastError();
