@@ -1622,10 +1622,14 @@ struct ScatterRequest {
   bool empty = false;
 };
 
+// Whether a routed scatter's sequence with destination mask *mask goes to destination d; every destination without a mask.
+static bool routed_to(const uint32_t* mask, size_t d) { return !mask || (d < 32 && ((*mask >> d) & 1u)); }
+
 // Every check of one sequence of a scatter after check_scatter_windows, under the manager's lock, in the order its header gives.
+// mask: a routed sequence's destinations, whose id lists alone are read and checked.
 static int check_scatter_request(kvbm_transfer_manager* m, kvbm_layout_handle src_h, const kvbm_scatter_batch_seq& q, size_t num_dsts,
                                  const kvbm_layout_handle* dsts, const kvbm_scatter_window* w, size_t nw, const kvbm_transfer_options& o,
-                                 const kvbm_layer_stream* ls, ScatterRequest* R)
+                                 const kvbm_layer_stream* ls, ScatterRequest* R, const uint32_t* mask = nullptr)
 {
   int rc;
   Layout* S = R->S = m->find(src_h);
@@ -1658,6 +1662,7 @@ static int check_scatter_request(kvbm_transfer_manager* m, kvbm_layout_handle sr
     return rc;
   for (size_t j = 0; j < nw; ++j) {
     const size_t d = w[j].dst_rank;
+    if (!routed_to(mask, d)) continue;
     if (q.n_dst && !q.dst_ids[d]) return fail(KVBM_ERR, "null block id list");
     if ((rc = check_block_ids(q.src_ids, q.n_src, q.n_dst ? q.dst_ids[d] : nullptr, q.n_dst, S->cfg.num_blocks, D[d]->cfg.num_blocks,
                               src_h == dsts[d])))
@@ -1675,10 +1680,14 @@ static int check_scatter_request(kvbm_transfer_manager* m, kvbm_layout_handle sr
 // batch's unit table), then one launch whose signal writes the per-destination done flags and the completion word, and the
 // options' done flag after it.  ls: the streamed scatter (its shape checked by the caller); the slot also holds the gate's
 // workspace over the source's layers, and the one streamed launch writes every flag, the options' done flag included.
+// masks: a routed batch (kvbm_manager_execute_repage_scatter_routed), sequence i going to the destinations of masks[i] only: the
+// routing checks run after the windows', each sequence's routed id lists alone are checked, the uniqueness per destination runs
+// over its routed sequences, unrouted positions of the staged tables are padded with block 0, and the unit table carries each
+// sequence's window mask for the routed kernel entries.
 static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle src_h, size_t num_dsts, const kvbm_layout_handle* dsts,
                                   const kvbm_scatter_batch_seq* seqs, size_t num_seqs, const kvbm_scatter_window* w, size_t nw,
                                   const kvbm_transfer_options* opts_in, kvbm_notification* out, const kvbm_layer_stream* ls = nullptr,
-                                  bool batch = false)
+                                  bool batch = false, const uint32_t* masks = nullptr)
 {
   kvbm_transfer_options o{};
   if (opts_in) o = *opts_in;
@@ -1686,6 +1695,19 @@ static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle s
   int rc;
   if ((rc = check_scatter_windows(num_dsts, dsts, w, nw, o))) return rc;
   if (batch && num_seqs && !seqs) return fail(KVBM_ERR, "null sequence list");
+  if (masks) {
+    if (num_dsts > 32)
+      return fail(KVBM_ERR_UNSUPPORTED, "a routed scatter takes at most 32 destinations, got " + std::to_string(num_dsts));
+    uint32_t written = 0;
+    for (size_t j = 0; j < nw; ++j) written |= 1u << w[j].dst_rank;
+    for (size_t i = 0; i < num_seqs; ++i) {
+      const std::string at = "sequence " + std::to_string(i);
+      if (masks[i] == 0) return fail(KVBM_ERR_RANGE, at + " is routed to no destination");
+      if (num_dsts < 32 && (masks[i] >> num_dsts) != 0)
+        return fail(KVBM_ERR_RANGE, at + " is routed past the " + std::to_string(num_dsts) + " destinations");
+      if (masks[i] & ~written) return fail(KVBM_ERR_RANGE, at + " is routed to a destination no window writes");
+    }
+  }
   std::lock_guard<std::mutex> lk(m->mu);
   // every sequence resolves the same source, destinations, windows and layer range: only `empty` is the last sequence's own
   ScatterRequest R;
@@ -1693,11 +1715,13 @@ static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle s
   uint64_t bytes = 0;
   for (size_t i = 0; i < num_seqs; ++i) {
     const kvbm_scatter_batch_seq& q = seqs[i];
-    if ((rc = check_scatter_request(m, src_h, q, num_dsts, dsts, w, nw, o, ls, &R))) return rc;
+    const uint32_t* mask = masks ? masks + i : nullptr;
+    if ((rc = check_scatter_request(m, src_h, q, num_dsts, dsts, w, nw, o, ls, &R, mask))) return rc;
     if (R.empty) continue;
     any = true;
-    // what lands: each window's destination bytes over its layers inside the range
+    // what lands: each routed window's destination bytes over its layers inside the range
     for (size_t j = 0; j < nw; ++j) {
+      if (!routed_to(mask, w[j].dst_rank)) continue;
       const Layout& Dj = *R.e[j].D[0];
       const size_t from = std::max(R.lb, w[j].src_layer_begin), to = std::min(R.le, w[j].src_layer_begin + w[j].layer_count);
       if (to > from)
@@ -1715,22 +1739,46 @@ static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle s
   const size_t* const* dst_ids = seqs[0].dst_ids;
   size_t n_src = seqs[0].n_src, n_dst = seqs[0].n_dst;
   BatchTables bt;
+  std::vector<kvbm_route_seq> routes;
   if (batch) {
     std::vector<bool> used(1 + num_dsts, false);  // the source, the destinations some window writes (the others' tables may be null)
     used[0] = true;
     for (size_t j = 0; j < nw; ++j) used[1 + w[j].dst_rank] = true;
-    auto ids = [](const kvbm_scatter_batch_seq& q, size_t k) { return k ? q.dst_ids[k - 1] : q.src_ids; };
+    std::vector<size_t> pad;  // a routed batch's unrouted positions: block 0, never read
+    for (size_t i = 0; masks && i < num_seqs; ++i) pad.resize(std::max(pad.size(), seqs[i].n_dst), 0);
+    auto ids = [&](const kvbm_scatter_batch_seq& q, size_t k) {
+      return !k ? q.src_ids : routed_to(masks ? masks + (&q - seqs) : nullptr, k - 1) ? q.dst_ids[k - 1] : pad.data();
+    };
     auto unique = [&](const std::vector<std::vector<size_t>>& cat) -> int {
-      for (size_t d = 0; d < num_dsts; ++d)
-        if (used[1 + d])
-          if (int rc = check_block_ids(cat[0].data(), cat[0].size(), cat[1 + d].data(), cat[1 + d].size(), S->cfg.num_blocks,
-                                       D[d]->cfg.num_blocks, src_h == dsts[d]))
-            return rc;
+      std::vector<size_t> routed;
+      for (size_t d = 0; d < num_dsts; ++d) {
+        if (!used[1 + d]) continue;
+        const std::vector<size_t>* cd = &cat[1 + d];
+        if (masks) {  // the ids of the sequences routed to d only
+          routed.clear();
+          for (size_t i = 0; i < num_seqs; ++i)
+            if (seqs[i].token_begin != seqs[i].token_end && routed_to(masks + i, d))
+              routed.insert(routed.end(), seqs[i].dst_ids[d], seqs[i].dst_ids[d] + seqs[i].n_dst);
+          cd = &routed;
+        }
+        if (int rc = check_block_ids(cat[0].data(), cat[0].size(), cd->data(), cd->size(), S->cfg.num_blocks, D[d]->cfg.num_blocks,
+                                     src_h == dsts[d]))
+          return rc;
+      }
       return KVBM_OK;
     };
     if ((rc = batch_tables(seqs, num_seqs, used, 1, ups, upd, ids, unique, &bt, &n_src, &n_dst))) return rc;
     src_ids = bt.lists[0];
     dst_ids = bt.lists.data() + 1;
+    if (masks) {  // each non-empty sequence's range with its window mask, which replaces the unit's sequence index
+      for (size_t i = 0; i < num_seqs; ++i) {
+        if (seqs[i].token_begin == seqs[i].token_end) continue;
+        uint32_t targets = 0;
+        for (size_t j = 0; j < nw; ++j) targets |= static_cast<uint32_t>(routed_to(masks + i, w[j].dst_rank)) << j;
+        routes.push_back(kvbm_route_seq{static_cast<uint32_t>(seqs[i].token_begin), static_cast<uint32_t>(seqs[i].token_end), targets});
+      }
+      for (kvbm_repage_unit& u : bt.units) u.seq = routes[u.seq].targets;
+    }
   }
 
   DeviceGuard g(m->device);
@@ -1759,9 +1807,14 @@ static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle s
   const uint32_t utb = static_cast<uint32_t>(seqs[0].token_begin), ute = static_cast<uint32_t>(seqs[0].token_end);
   const int k = static_cast<int>(nw), ilb = static_cast<int>(R.lb), ile = static_cast<int>(R.le);
   const auto* du = reinterpret_cast<const kvbm_repage_unit*>(sl->dev_ids + units_at(n_src + num_dsts * n_dst));
+  const auto* dr = reinterpret_cast<const kvbm_route_unit*>(du);
   if (ls) {
     const kvbm_permute_stream st = layer_stream(*ls, e, 1, o, *sl, seq);
-    if (batch)
+    if (masks)
+      rc = checked(kvbm_kernels_paged_repage_scatter_routed_streamed(&ks, snh, ups, kt, k, upd, routes.data(), routes.size(), dr, bt.units.size(),
+                                                                     ilb, ile, row, o.cast_mode, o.cast_scales, &st, stream),
+                   "kvbm_kernels_paged_repage_scatter_routed_streamed");
+    else if (batch)
       rc = checked(kvbm_kernels_paged_repage_scatter_batch_streamed(&ks, snh, ups, kt, k, upd, bt.ranges.data(), bt.ranges.size(), du, bt.units.size(),
                                                                     ilb, ile, row, o.cast_mode, o.cast_scales, &st, stream),
                    "kvbm_kernels_paged_repage_scatter_batch_streamed");
@@ -1770,7 +1823,12 @@ static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle s
                                                               &st, stream),
                    "kvbm_kernels_paged_repage_scatter_streamed");
   } else {
-    if (batch)
+    if (masks)
+      rc = checked(kvbm_kernels_paged_repage_scatter_routed(&ks, snh, ups, kt, k, upd, routes.data(), routes.size(), dr, bt.units.size(), ilb, ile,
+                                                            row, o.cast_mode, o.cast_scales, o.epoch, sl->host_flag, static_cast<uint32_t>(seq),
+                                                            stream),
+                   "kvbm_kernels_paged_repage_scatter_routed");
+    else if (batch)
       rc = checked(kvbm_kernels_paged_repage_scatter_batch(&ks, snh, ups, kt, k, upd, bt.ranges.data(), bt.ranges.size(), du, bt.units.size(), ilb, ile,
                                                            row, o.cast_mode, o.cast_scales, o.epoch, sl->host_flag, static_cast<uint32_t>(seq),
                                                            stream),
@@ -2459,6 +2517,25 @@ extern "C" int kvbm_manager_execute_repage_scatter_batch(kvbm_transfer_manager* 
   return guarded([&]() -> int {
   if (int rc = stream_entry(m, ls, 1, false, out)) return rc;
   return execute_repage_scatter(m, src, num_dsts, dsts, seqs, num_seqs, windows, num_windows, opts, out, ls, /*batch=*/true);
+  });
+}
+
+extern "C" int kvbm_manager_execute_repage_scatter_routed(kvbm_transfer_manager* m, kvbm_layout_handle src, size_t num_dsts,
+                                                          const kvbm_layout_handle* dsts, const kvbm_scatter_route_seq* seqs, size_t num_seqs,
+                                                          const kvbm_scatter_window* windows, size_t num_windows, const kvbm_layer_stream* ls,
+                                                          const kvbm_transfer_options* opts, kvbm_notification* out)
+{
+  return guarded([&]() -> int {
+  if (int rc = stream_entry(m, ls, 1, false, out)) return rc;
+  std::vector<kvbm_scatter_batch_seq> qs(seqs ? num_seqs : 0);
+  std::vector<uint32_t> masks(std::max<size_t>(1, qs.size()));  // never empty: a null masks is an unrouted call
+  for (size_t i = 0; i < qs.size(); ++i) {
+    const kvbm_scatter_route_seq& s = seqs[i];
+    qs[i] = kvbm_scatter_batch_seq{s.token_begin, s.token_end, s.src_ids, s.n_src, s.dst_ids, s.n_dst};
+    masks[i] = s.dst_mask;
+  }
+  return execute_repage_scatter(m, src, num_dsts, dsts, seqs ? qs.data() : nullptr, num_seqs, windows, num_windows, opts, out, ls,
+                                /*batch=*/true, masks.data());
   });
 }
 

@@ -966,9 +966,11 @@ __host__ __device__ __forceinline__ uint32_t source_layer(const ScatterParams&, 
 // each 16 B vector ONCE and casts it once, and its store half writes it to every (target, destination head) pair of the entry,
 // each at its own layer.  With Ps >= Pd block j is the source's and each target finds the vector's small block in its own table;
 // with Ps < Pd block j is entry j of every target's table (they share Pd and the range).
-template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+// ROUTE: only the pairs whose target's bit is set in `mask` (the unit's sequence's targets) are stored, and an entry with no such
+// pair loads nothing.  Only pair_tgt[p] < num_targets selects a bit, so bits at or above the launch's target count are never read.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2, bool ROUTE = false>
 __device__ __forceinline__ void scatter_head_rows(const ScatterParams& P, uint32_t k, uint32_t j, uint32_t l, uint32_t o, const RepageUnit& u,
-                                                  uint32_t run, const RowSplit& r, const ptx::Scale& scale)
+                                                  uint32_t run, const RowSplit& r, const ptx::Scale& scale, uint32_t mask = 0)
 {
   constexpr int IN = CAST == KVBM_CAST_BF16_TO_FP8E4M3 ? 2 : 1;
   constexpr int OUT = CAST == KVBM_CAST_FP8E4M3_TO_BF16 ? 2 : 1;
@@ -978,6 +980,11 @@ __device__ __forceinline__ void scatter_head_rows(const ScatterParams& P, uint32
   const bool ss = G.src_small;
   const uint32_t big_shift = ss ? 3 + OUT : 3 + IN, small_shift = ss ? 3 + IN : 3 + OUT;
   const uint32_t h = P.head[k], p0 = P.pair_first[k], p1 = P.pair_first[k + 1];
+  if constexpr (ROUTE) {
+    uint32_t routed = 0;
+    for (uint32_t p = p0; p < p1; ++p) routed |= (mask >> P.pair_tgt[p]) & 1u;
+    if (!routed) return;
+  }
   const uint8_t* sh = (ss ? side_region(S, l, o) : side_block(S, j, l, o)) + h * S.head_stride;
   const int lane = threadIdx.x & 31;
   for (uint32_t v = lane; v < run; v += U * 32) {
@@ -1001,6 +1008,8 @@ __device__ __forceinline__ void scatter_head_rows(const ScatterParams& P, uint32
           cast_vector<SCALED>(x[i], y, scale);
 #pragma unroll 1
         for (uint32_t p = p0; p < p1; ++p) {
+          if constexpr (ROUTE)
+            if (!((mask >> P.pair_tgt[p]) & 1u)) continue;
           const ScatterTarget& T = P.tgt[P.pair_tgt[p]];
           const PermuteSide& D = T.D;
           const uint32_t dl = l + T.shift;
@@ -1015,22 +1024,30 @@ __device__ __forceinline__ void scatter_head_rows(const ScatterParams& P, uint32
 
 // One (big block j, source layer l, outer o) unit of the scatter, clipped to the range, with l's stage T: one warp per covered
 // source head of T, looping by the CTA's warps past 8.  SCALED: the SOURCE's scales[l * no + o], loaded once per unit.
-// TABLE: a batch of sequences, whose unit comes from `units` (batch_unit) instead of the launch's one token range.
-template <int CAST, bool POW2, bool SCALED, bool PPOW2, bool TABLE = false>
+// TABLE: a batch of sequences, whose unit comes from `units` (batch_unit) instead of the launch's one token range.  ROUTE: a
+// routed batch, whose unit and target mask come from record j of `routes` in the same 16 B load (scatter_head_rows' ROUTE).
+template <int CAST, bool POW2, bool SCALED, bool PPOW2, bool TABLE = false, bool ROUTE = false>
 __device__ __forceinline__ void scatter_unit(const ScatterParams& P, const GatherStage& T, uint32_t j, uint32_t l, uint32_t o, const RowSplit& r,
-                                             const float* scales, const kvbm_repage_unit* units = nullptr)
+                                             const float* scales, const kvbm_repage_unit* units = nullptr,
+                                             const kvbm_route_unit* routes = nullptr)
 {
   const RepageGeom& G = P.geo;
   RepageUnit u;
-  if constexpr (TABLE)
+  uint32_t mask = 0;
+  if constexpr (ROUTE) {
+    const uint4 w = __ldg(reinterpret_cast<const uint4*>(routes) + j);
+    u = {w.x, w.y, w.z};
+    mask = w.w;
+  } else if constexpr (TABLE) {
     u = batch_unit(units, j);
-  else
+  } else {
     u = repage_unit(G, j);
+  }
   const ptx::Scale scale = ptx::make_scale(SCALED ? __ldg(scales + l * G.no + o) : 1.f);
   const uint32_t run = row_run<POW2>(r, u.tokens);
   const uint32_t end = T.first + T.count;
   for (uint32_t k = T.first + (threadIdx.x >> 5); k < end; k += blockDim.x >> 5)
-    scatter_head_rows<CAST, POW2, SCALED, PPOW2>(P, k, j, l, o, u, run, r, scale);
+    scatter_head_rows<CAST, POW2, SCALED, PPOW2, ROUTE>(P, k, j, l, o, u, run, r, scale, mask);
 }
 
 // One CTA per unit, as the re-paging gather.  The re-paging gathers' bound: three CTAs per SM.
@@ -1053,6 +1070,17 @@ kvbm_paged_repage_push_seqs_kernel(const __grid_constant__ ScatterParams P, cons
   const auto [j, l, rem] = repage_cta(P.geo);
   const uint32_t o = rem % P.geo.no;
   scatter_unit<CAST, POW2, SCALED, PPOW2, true>(P, stage_of(P, l), j, l, o, r, scales, units);
+}
+
+// kvbm_paged_repage_push_seqs_kernel over a routed batch: record j of `routes` also names the targets big block j goes to, and
+// only those are written.  The same bound: three CTAs per SM.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__global__ void __launch_bounds__(256, 3)
+kvbm_paged_repage_route_kernel(const __grid_constant__ ScatterParams P, const kvbm_route_unit* routes, RowSplit r, const float* scales)
+{
+  const auto [j, l, rem] = repage_cta(P.geo);
+  const uint32_t o = rem % P.geo.no;
+  scatter_unit<CAST, POW2, SCALED, PPOW2, true, true>(P, stage_of(P, l), j, l, o, r, scales, nullptr, routes);
 }
 
 // The scatter's signal after its launch: every target's done flag (epoch) and the completion word, system scope.
@@ -1240,6 +1268,21 @@ kvbm_gated_repage_push_seqs_kernel(const __grid_constant__ ScatterParams P, cons
   gated_repage_units(
       A, P, P.geo, num_big, batch,
       [&](const GatherStage& T, uint32_t j, uint32_t l, uint32_t o) { scatter_unit<CAST, POW2, SCALED, PPOW2, true>(P, T, j, l, o, r, scales, units); },
+      target_done(F, num_flags, A));
+}
+
+// kvbm_gated_repage_push_seqs_kernel over a routed batch (num_big: the length of `routes`): every unit of source layer l counts,
+// written or not, so layer l is done once it landed in every target each sequence is routed to.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__global__ void __launch_bounds__(256, 1)
+kvbm_gated_repage_route_kernel(const __grid_constant__ ScatterParams P, const __grid_constant__ GateArgs A, const __grid_constant__ ScatterFlags F,
+                               int num_flags, const kvbm_route_unit* routes, uint32_t num_big, RowSplit r, const float* scales, uint32_t batch)
+{
+  gated_repage_units(
+      A, P, P.geo, num_big, batch,
+      [&](const GatherStage& T, uint32_t j, uint32_t l, uint32_t o) {
+        scatter_unit<CAST, POW2, SCALED, PPOW2, true, true>(P, T, j, l, o, r, scales, nullptr, routes);
+      },
       target_done(F, num_flags, A));
 }
 
@@ -1443,6 +1486,10 @@ static cudaError_t preload_kernels()
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_push_seqs_kernel<c, p, sc, false>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_push_seqs_kernel<c, p, sc, true>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_push_seqs_kernel<c, p, sc, false>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_route_kernel<c, p, sc, true>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_route_kernel<c, p, sc, false>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_route_kernel<c, p, sc, true>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_route_kernel<c, p, sc, false>);
         });
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_layer_signal_kernel);
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_scatter_signal_kernel);
@@ -1840,12 +1887,16 @@ static bool repage_pages(uint32_t src_page, uint32_t dst_page, int layer_begin, 
   return true;
 }
 
-// A batch of sequences of a re-paging launch: the caller's ranges (host) and unit table (device-accessible).
+// A batch of sequences of a re-paging launch: the caller's ranges (host) and unit table (device-accessible).  route: a routed
+// scatter's batch, whose ranges and target masks are route_seqs and whose unit table is route_units (seqs and units unused).
 struct RepageBatch {
   const kvbm_repage_seq* seqs;
   size_t num_seqs;
   const kvbm_repage_unit* units;
   size_t num_units;
+  bool route = false;
+  const kvbm_route_seq* route_seqs = nullptr;
+  const kvbm_route_unit* route_units = nullptr;
 };
 
 // What repage_launch derives: repage_pages' results with the token range's fields, the units to launch (0: nothing to move), the
@@ -1859,7 +1910,8 @@ struct RepageLaunch {
 };
 
 // Every re-paging launch's first checks, before any CUDA call: ranges not reversed, cast_args_ok, and B checked by
-// kvbm_kernels_repage_batch_units with the caller's unit count.  An empty range or batch then leaves L->units 0 (the caller
+// kvbm_kernels_repage_batch_units (a routed batch: kvbm_kernels_repage_route_units) with the caller's unit count.  An empty range
+// or batch then leaves L->units 0 (the caller
 // signals).  Else `side` (a gather's destination, the scatter's source) needs a table, a base, a non-zero outer dim and the layer
 // range; the pages repage_pages' rules; a single range slots in 32 bits (its last block of the larger page ends below 2^32); the
 // launch fewer than 2^31 units.  False: rejected.
@@ -1872,8 +1924,11 @@ static bool repage_launch(const kvbm_permute_side* side, uint32_t src_page, uint
   size_t num_big = 0;
   if (B) {
     size_t src_ids, dst_ids;
-    if (kvbm_kernels_repage_batch_units(B->seqs, B->num_seqs, src_page, dst_page, nullptr, 0, &num_big, &src_ids, &dst_ids) != 0) return false;
-    if (num_big != B->num_units || (num_big != 0 && !B->units)) return false;
+    if ((B->route ? kvbm_kernels_repage_route_units(B->route_seqs, B->num_seqs, src_page, dst_page, nullptr, 0, &num_big, &src_ids, &dst_ids)
+                  : kvbm_kernels_repage_batch_units(B->seqs, B->num_seqs, src_page, dst_page, nullptr, 0, &num_big, &src_ids, &dst_ids)) != 0)
+      return false;
+    const void* table = B->route ? static_cast<const void*>(B->route_units) : B->units;
+    if (num_big != B->num_units || (num_big != 0 && !table)) return false;
   }
   L->units = 0;
   if ((B ? num_big == 0 : token_end == token_begin) || layer_end == layer_begin) return true;
@@ -2070,7 +2125,7 @@ static bool fill_scatter_targets(const kvbm_scatter_target* tg, int n, uint32_t 
 // before them), then one kvbm_paged_repage_scatter_kernel launch and the signal.  st: a streamed launch (its flags are the ones
 // passed, and its done flag is written with the targets'), which takes the gated push kernel, or per source layer this launch
 // unstreamed.  B: a batch of sequences in place of the one token range (token_begin / token_end unused), which always takes the
-// push_seqs kernels.
+// push_seqs kernels, or the route kernels for a routed batch, whose every target mask must be non-zero and below bit num_targets.
 static cudaError_t launch_paged_repage_scatter(const kvbm_permute_side* src, uint32_t src_num_heads, uint32_t src_page,
                                                const kvbm_scatter_target* targets, int num_targets, uint32_t dst_page, uint32_t token_begin,
                                                uint32_t token_end, int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode,
@@ -2078,8 +2133,11 @@ static cudaError_t launch_paged_repage_scatter(const kvbm_permute_side* src, uin
                                                cudaStream_t stream, const kvbm_permute_stream* st = nullptr, const RepageBatch* B = nullptr)
 {
   RepageLaunch L;
-  if (!targets || num_targets < 1 || num_targets > KVBM_GATHER_MAX_SOURCES ||
-      !repage_launch(src, src_page, dst_page, token_begin, token_end, layer_begin, layer_end, src_row_bytes, cast_mode, cast_scales, B, &L))
+  if (!targets || num_targets < 1 || num_targets > KVBM_GATHER_MAX_SOURCES) return cudaErrorInvalidValue;
+  if (B && B->route && B->route_seqs)
+    for (size_t i = 0; i < B->num_seqs; ++i)
+      if (B->route_seqs[i].targets == 0 || (B->route_seqs[i].targets >> num_targets) != 0) return cudaErrorInvalidValue;
+  if (!repage_launch(src, src_page, dst_page, token_begin, token_end, layer_begin, layer_end, src_row_bytes, cast_mode, cast_scales, B, &L))
     return cudaErrorInvalidValue;
   if (L.units == 0) return scatter_signal(targets, num_targets, st ? st->done_flag : nullptr, epoch, completion_flag, completion_value, stream);
   const uint32_t nl = L.nl, no = L.no;
@@ -2110,7 +2168,10 @@ static cudaError_t launch_paged_repage_scatter(const kvbm_permute_side* src, uin
           const ScatterFlags F = scatter_flags(targets, num_targets, &any);
           Ag.ss.want_done |= any;
           with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, L.page_pow2, [&](auto c, auto p, auto sc, auto pp) {
-            if (B)
+            if (B && B->route)
+              kvbm_gated_repage_route_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, Ag, F, num_targets, B->route_units, L.num_big, r,
+                                                                                        cast_scales, batch);
+            else if (B)
               kvbm_gated_repage_push_seqs_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, Ag, F, num_targets, B->units, L.num_big, r,
                                                                                             cast_scales, batch);
             else
@@ -2119,7 +2180,9 @@ static cudaError_t launch_paged_repage_scatter(const kvbm_permute_side* src, uin
         });
   }
   with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, L.page_pow2, [&](auto c, auto p, auto sc, auto pp) {
-    if (B)
+    if (B && B->route)
+      kvbm_paged_repage_route_kernel<c, p, sc, pp><<<static_cast<unsigned>(L.units), threads, 0, stream>>>(P, B->route_units, r, cast_scales);
+    else if (B)
       kvbm_paged_repage_push_seqs_kernel<c, p, sc, pp><<<static_cast<unsigned>(L.units), threads, 0, stream>>>(P, B->units, r, cast_scales);
     else
       kvbm_paged_repage_scatter_kernel<c, p, sc, pp><<<static_cast<unsigned>(L.units), threads, 0, stream>>>(P, r, cast_scales);
@@ -2380,9 +2443,10 @@ kvbm_kernels_paged_stage_repage_gather_streamed(const kvbm_stage_source* srcs, i
                                     st->completion_value, KVBM_GATHER_MAX_HEADS, stream, st);
 }
 
-extern "C" int
-kvbm_kernels_repage_batch_units(const kvbm_repage_seq* seqs, size_t num_seqs, uint32_t src_page_size, uint32_t dst_page_size,
-                                kvbm_repage_unit* out, size_t cap, size_t* num_units, size_t* src_ids, size_t* dst_ids)
+// kvbm_kernels_repage_batch_units over ranges of either sequence type; the fourth word of each unit is last(i) of its sequence i.
+template <class Seq, class Unit, class Last>
+static int batch_units(const Seq* seqs, size_t num_seqs, uint32_t src_page_size, uint32_t dst_page_size, Unit* out, size_t cap,
+                       size_t* num_units, size_t* src_ids, size_t* dst_ids, Last last)
 {
   if ((num_seqs && !seqs) || (cap && !out) || !num_units || !src_ids || !dst_ids) return 1;
   if (src_page_size == 0 || dst_page_size == 0) return 1;
@@ -2403,8 +2467,8 @@ kvbm_kernels_repage_batch_units(const kvbm_repage_seq* seqs, size_t num_seqs, ui
     for (; j < big_end && nb < cap; ++j, ++nb) {
       const uint64_t first = j * big, t0 = std::max(tb, first), t1 = std::min(te, first + big);
       // the concatenated small table's entry of the block's first small block: below 0 (wrapping) when it lies before the range
-      out[nb] = kvbm_repage_unit{static_cast<uint32_t>(t0 - first), static_cast<uint32_t>(t1 - t0),
-                                 static_cast<uint32_t>(ns + j * ratio - small_first), static_cast<uint32_t>(i)};
+      out[nb] = Unit{static_cast<uint32_t>(t0 - first), static_cast<uint32_t>(t1 - t0), static_cast<uint32_t>(ns + j * ratio - small_first),
+                     last(i)};
     }
     nb += static_cast<size_t>(big_end - j);  // past the capacity: counted, not written
     ns += static_cast<size_t>(small_end - small_first);
@@ -2413,6 +2477,22 @@ kvbm_kernels_repage_batch_units(const kvbm_repage_seq* seqs, size_t num_seqs, ui
   *src_ids = src_small ? ns : nb;
   *dst_ids = src_small ? nb : ns;
   return 0;
+}
+
+extern "C" int
+kvbm_kernels_repage_batch_units(const kvbm_repage_seq* seqs, size_t num_seqs, uint32_t src_page_size, uint32_t dst_page_size,
+                                kvbm_repage_unit* out, size_t cap, size_t* num_units, size_t* src_ids, size_t* dst_ids)
+{
+  return batch_units(seqs, num_seqs, src_page_size, dst_page_size, out, cap, num_units, src_ids, dst_ids,
+                     [](size_t i) { return static_cast<uint32_t>(i); });
+}
+
+extern "C" int
+kvbm_kernels_repage_route_units(const kvbm_route_seq* seqs, size_t num_seqs, uint32_t src_page_size, uint32_t dst_page_size,
+                                kvbm_route_unit* out, size_t cap, size_t* num_units, size_t* src_ids, size_t* dst_ids)
+{
+  return batch_units(seqs, num_seqs, src_page_size, dst_page_size, out, cap, num_units, src_ids, dst_ids,
+                     [seqs](size_t i) { return seqs[i].targets; });
 }
 
 extern "C" cudaError_t
@@ -2486,6 +2566,32 @@ kvbm_kernels_paged_repage_scatter_batch_streamed(const kvbm_permute_side* src, u
 {
   if (!stream_args_ok(st, 1)) return cudaErrorInvalidValue;
   const RepageBatch B{seqs, num_seqs, units, num_units};
+  return launch_paged_repage_scatter(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, 0, 0, layer_begin, layer_end,
+                                     src_row_bytes, cast_mode, cast_scales, st->epoch, st->completion_flag, st->completion_value, stream, st,
+                                     &B);
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_repage_scatter_routed(const kvbm_permute_side* src, uint32_t src_num_heads, uint32_t src_page_size,
+                                         const kvbm_scatter_target* targets, int num_targets, uint32_t dst_page_size, const kvbm_route_seq* seqs,
+                                         size_t num_seqs, const kvbm_route_unit* units, size_t num_units, int layer_begin, int layer_end,
+                                         uint32_t src_row_bytes, int cast_mode, const float* cast_scales, uint32_t epoch,
+                                         uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
+{
+  const RepageBatch B{nullptr, num_seqs, nullptr, num_units, true, seqs, units};
+  return launch_paged_repage_scatter(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, 0, 0, layer_begin, layer_end,
+                                     src_row_bytes, cast_mode, cast_scales, epoch, completion_flag, completion_value, stream, nullptr, &B);
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_repage_scatter_routed_streamed(const kvbm_permute_side* src, uint32_t src_num_heads, uint32_t src_page_size,
+                                                  const kvbm_scatter_target* targets, int num_targets, uint32_t dst_page_size,
+                                                  const kvbm_route_seq* seqs, size_t num_seqs, const kvbm_route_unit* units, size_t num_units,
+                                                  int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
+                                                  const kvbm_permute_stream* st, cudaStream_t stream)
+{
+  if (!stream_args_ok(st, 1)) return cudaErrorInvalidValue;
+  const RepageBatch B{nullptr, num_seqs, nullptr, num_units, true, seqs, units};
   return launch_paged_repage_scatter(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, 0, 0, layer_begin, layer_end,
                                      src_row_bytes, cast_mode, cast_scales, st->epoch, st->completion_flag, st->completion_value, stream, st,
                                      &B);

@@ -120,6 +120,16 @@ class RepageUnit(C.Structure):
     _fields_ = [("q0", C.c_uint32), ("tokens", C.c_uint32), ("small_k", C.c_uint32), ("seq", C.c_uint32)]
 
 
+class RouteSeq(C.Structure):
+    """struct kvbm_route_seq: one sequence of a routed scatter, its token range and its targets (bit t: target t; host memory)"""
+    _fields_ = [("token_begin", C.c_uint32), ("token_end", C.c_uint32), ("targets", C.c_uint32)]
+
+
+class RouteUnit(C.Structure):
+    """struct kvbm_route_unit: RepageUnit with the sequence's targets in place of seq, 16 B (`repage_route_units` writes them)"""
+    _fields_ = [("q0", C.c_uint32), ("tokens", C.c_uint32), ("small_k", C.c_uint32), ("targets", C.c_uint32)]
+
+
 class ScatterTarget(C.Structure):
     """struct kvbm_scatter_target: one target of `paged_repage_scatter` (a destination side, its head count, one head window, one
     layer window and its nullable done flag)"""
@@ -271,6 +281,12 @@ def lib() -> C.CDLL:
                                                                        C.POINTER(ScatterTarget), i, C.c_uint32, vp, sz, vp, sz, i, i,
                                                                        C.c_uint32, i, vp, C.POINTER(PermuteStream), vp]
         L.kvbm_kernels_paged_repage_scatter_batch_streamed.restype = i
+        L.kvbm_kernels_repage_route_units.argtypes = [vp, sz, C.c_uint32, C.c_uint32, vp, sz, C.POINTER(sz), C.POINTER(sz), C.POINTER(sz)]
+        L.kvbm_kernels_repage_route_units.restype = i
+        L.kvbm_kernels_paged_repage_scatter_routed.argtypes = L.kvbm_kernels_paged_repage_scatter_batch.argtypes
+        L.kvbm_kernels_paged_repage_scatter_routed.restype = i
+        L.kvbm_kernels_paged_repage_scatter_routed_streamed.argtypes = L.kvbm_kernels_paged_repage_scatter_batch_streamed.argtypes
+        L.kvbm_kernels_paged_repage_scatter_routed_streamed.restype = i
         L.kvbm_kernels_permute_strides.argtypes = [i, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64, C.c_uint64,
                                                    C.POINTER(C.c_uint64)]
         L.kvbm_kernels_permute_strides.restype = i
@@ -300,7 +316,8 @@ EXPORTED_SYMBOLS = [
     "kvbm_kernels_repage_batch_units", "kvbm_kernels_paged_stage_repage_gather_batch",
     "kvbm_kernels_paged_stage_repage_gather_batch_streamed", "kvbm_kernels_paged_repage_scatter",
     "kvbm_kernels_paged_repage_scatter_streamed", "kvbm_kernels_paged_repage_scatter_batch",
-    "kvbm_kernels_paged_repage_scatter_batch_streamed",
+    "kvbm_kernels_paged_repage_scatter_batch_streamed", "kvbm_kernels_repage_route_units", "kvbm_kernels_paged_repage_scatter_routed",
+    "kvbm_kernels_paged_repage_scatter_routed_streamed",
 ]
 
 
@@ -631,6 +648,56 @@ def paged_repage_scatter_batch_streamed(src: PermuteSide, src_num_heads: int, sr
                                                                   units or None, num_units, layer_begin, layer_end, src_row_bytes,
                                                                   int(cast_mode), scales_ptr(cast_scales),
                                                                   C.byref(st) if st is not None else None, stream)
+
+
+def _route_seqs(seqs: Sequence[Tuple[int, int, int]]):
+    return (RouteSeq * max(1, len(seqs)))(*[RouteSeq(int(b), int(e), int(t)) for b, e, t in seqs])
+
+
+def repage_route_units(seqs: Sequence[Tuple[int, int, int]], src_page_size: int, dst_page_size: int):
+    """Host-only: `repage_batch_units` over the (token_begin, token_end, targets) of a routed batch, each record's fourth word its
+    sequence's targets: a numpy uint32 array [num_units, 4] (q0, tokens, small_k, targets) and the two table lengths, or None.
+    include/kvbm_kernels.h (kvbm_kernels_repage_route_units)."""
+    import numpy as np
+    arr = _route_seqs(seqs)
+    n, ns, nd = C.c_size_t(), C.c_size_t(), C.c_size_t()
+    call = lib().kvbm_kernels_repage_route_units
+    if call(C.cast(arr, C.c_void_p), len(seqs), src_page_size, dst_page_size, None, 0, C.byref(n), C.byref(ns), C.byref(nd)):
+        return None
+    out = np.zeros((n.value, 4), dtype=np.uint32)
+    if call(C.cast(arr, C.c_void_p), len(seqs), src_page_size, dst_page_size, out.ctypes.data, n.value, C.byref(n), C.byref(ns), C.byref(nd)):
+        return None
+    return out, ns.value, nd.value
+
+
+def paged_repage_scatter_routed(src: PermuteSide, src_num_heads: int, src_page_size: int, targets: Sequence[ScatterTarget],
+                                dst_page_size: int, seqs: Sequence[Tuple[int, int, int]], units: int, num_units: int, layer_begin: int,
+                                layer_end: int, src_row_bytes: int, cast_mode: int = 0, cast_scales=None, epoch: int = 0,
+                                completion_flag: int = 0, completion_value: int = 0, stream: int = 0) -> int:
+    """`paged_repage_scatter_batch` with a target mask per sequence, in ONE launch with one signal: `seqs` are (token_begin,
+    token_end, targets), bit t of targets naming targets[t]; every target's block_ids has the batch layout (the positions of
+    sequences not routed to it are never read); `units` is the device address of the table `repage_route_units` made for the same
+    sequences and pages.  include/kvbm_kernels.h (kvbm_kernels_paged_repage_scatter_routed)."""
+    arr = (ScatterTarget * max(1, len(targets)))(*targets)
+    return lib().kvbm_kernels_paged_repage_scatter_routed(C.byref(src), src_num_heads, src_page_size, arr, len(targets), dst_page_size,
+                                                          C.cast(_route_seqs(seqs), C.c_void_p), len(seqs), units or None, num_units,
+                                                          layer_begin, layer_end, src_row_bytes, int(cast_mode), scales_ptr(cast_scales),
+                                                          epoch, completion_flag or None, completion_value, stream)
+
+
+def paged_repage_scatter_routed_streamed(src: PermuteSide, src_num_heads: int, src_page_size: int, targets: Sequence[ScatterTarget],
+                                         dst_page_size: int, seqs: Sequence[Tuple[int, int, int]], units: int, num_units: int,
+                                         layer_begin: int, layer_end: int, src_row_bytes: int, cast_mode: int, cast_scales,
+                                         st: Optional[PermuteStream], stream: int = 0) -> int:
+    """`paged_repage_scatter_routed` streamed with `paged_repage_scatter_batch_streamed`'s flags: layer_done_flags[l] is written
+    once source layer l of every sequence landed in every target it is routed to.
+    include/kvbm_kernels.h (kvbm_kernels_paged_repage_scatter_routed_streamed)."""
+    arr = (ScatterTarget * max(1, len(targets)))(*targets)
+    return lib().kvbm_kernels_paged_repage_scatter_routed_streamed(C.byref(src), src_num_heads, src_page_size, arr, len(targets),
+                                                                   dst_page_size, C.cast(_route_seqs(seqs), C.c_void_p), len(seqs),
+                                                                   units or None, num_units, layer_begin, layer_end, src_row_bytes,
+                                                                   int(cast_mode), scales_ptr(cast_scales),
+                                                                   C.byref(st) if st is not None else None, stream)
 
 
 def permute_strides(kv_layout: int, num_layers: int, outer_dim: int, num_heads: int, page_size: int, row_bytes: int,

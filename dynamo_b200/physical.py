@@ -140,6 +140,12 @@ class _CScatterBatchSeq(C.Structure):
                 ("dst_ids", C.c_void_p), ("n_dst", C.c_size_t)]
 
 
+class _CScatterRouteSeq(C.Structure):
+    """struct kvbm_scatter_route_seq"""
+    _fields_ = [("token_begin", C.c_size_t), ("token_end", C.c_size_t), ("src_ids", C.c_void_p), ("n_src", C.c_size_t),
+                ("dst_ids", C.c_void_p), ("n_dst", C.c_size_t), ("dst_mask", C.c_uint32)]
+
+
 class _CLayerStream(C.Structure):
     """struct kvbm_layer_stream"""
     _fields_ = [("src_layer_ready_flags", C.c_void_p), ("num_srcs", C.c_size_t), ("layer_done_flags", C.c_void_p)]
@@ -262,6 +268,7 @@ EXPORTED_SYMBOLS = [
     "kvbm_tp_pp_reshard_plan", "kvbm_manager_execute_stage_gather", "kvbm_manager_execute_stage_repage_gather",
     "kvbm_manager_execute_repage_batch", "kvbm_tp_pp_scatter_plan", "kvbm_manager_execute_repage_scatter",
     "kvbm_manager_execute_repage_scatter_streamed", "kvbm_manager_execute_repage_scatter_batch",
+    "kvbm_manager_execute_repage_scatter_routed",
 ]
 
 
@@ -331,6 +338,8 @@ def lib() -> C.CDLL:
                                                                    sz, P(_CLayerStream), P(_COptions), P(u64)]
         L.kvbm_manager_execute_repage_scatter_batch.argtypes = [vp, u64, sz, P(u64), P(_CScatterBatchSeq), sz, P(_CScatterWindow), sz,
                                                                 P(_CLayerStream), P(_COptions), P(u64)]
+        L.kvbm_manager_execute_repage_scatter_routed.argtypes = [vp, u64, sz, P(u64), P(_CScatterRouteSeq), sz, P(_CScatterWindow), sz,
+                                                                 P(_CLayerStream), P(_COptions), P(u64)]
         L.kvbm_notification_is_complete.argtypes = [vp, u64]
         L.kvbm_notification_wait.argtypes = [vp, u64, C.c_int64]
         L.kvbm_manager_bytes_moved.argtypes = [vp]
@@ -534,6 +543,15 @@ def tp_pp_scatter_plan(num_kv_heads: int, num_layers: int, src_tp: int, src_pp: 
     _check(lib().kvbm_tp_pp_scatter_plan(*args, out, n.value, C.byref(n)))
     return [ScatterWindow(w.dst_rank, w.src_layer_begin, w.dst_layer_begin, w.layer_count, w.src_head_begin, w.dst_head_begin, w.head_count)
             for w in out[:n.value]]
+
+
+def tile_scatter_plan(plan: Sequence[ScatterWindow], num_workers: int, ranks_per_worker: int) -> List[ScatterWindow]:
+    """One decode group's scatter plan (`tp_pp_scatter_plan`) repeated over `num_workers` identical decode workers of
+    `ranks_per_worker` ranks each: worker w's copy of a window names destination rank dst_rank + w * ranks_per_worker, so the
+    destinations are worker-major and a routed sequence for worker w sets bits w * ranks_per_worker .. +ranks_per_worker - 1."""
+    if num_workers < 1 or any(w.dst_rank >= ranks_per_worker for w in plan):
+        raise ValueError(f"a plan for {ranks_per_worker} ranks per worker cannot be tiled {num_workers} times")
+    return [dataclasses.replace(w, dst_rank=w.dst_rank + k * ranks_per_worker) for k in range(num_workers) for w in plan]
 
 
 class TransferCompleteNotification:
@@ -970,6 +988,45 @@ class TransferManager:
         o = (options or TransferOptions())._c()
         _check(lib().kvbm_manager_execute_repage_scatter_batch(self._h, src, len(dsts), hs, cs, len(seqs), ws, len(plan),
                                                                C.byref(ls) if ls is not None else None, C.byref(o), C.byref(tok)))
+        return TransferCompleteNotification(self, tok.value)
+
+    def execute_repage_scatter_routed(self, src: int, dsts: Sequence[int], seqs: Sequence[tuple], plan: Sequence[ScatterWindow],
+                                      options: Optional[TransferOptions] = None, ready_flags: Optional[int] = None,
+                                      layer_done_flags: int = 0) -> TransferCompleteNotification:
+        """A prefill batch whose sequences go to different decode workers, as ONE hand-off (kvbm_manager_execute_repage_scatter_routed):
+        `seqs` is a list of (tokens, src_block_ids, {dst_index: dst_block_ids}), the dict's keys being the destinations (indices
+        into `dsts`) the sequence goes to, under one `plan` (`tile_scatter_plan` over identical workers).  Each sequence lands in
+        its own destinations only; every other destination byte keeps its value.  One staged copy, one launch, one notification;
+        `options.per_dst_done_flags` and `options.done_flag` are written once, after every sequence landed.  With `ready_flags` it
+        streams as `execute_repage_scatter_batch` does.  A destination block may appear once per destination among the sequences
+        routed to it."""
+        keep, cs = [], (_CScatterRouteSeq * max(1, len(seqs)))()
+        for c, (tokens, src_ids, routed) in zip(cs, seqs):
+            if tokens.step != 1:
+                raise ValueError("tokens must be a range with step 1")
+            n_dst = len(next(iter(routed.values()))) if routed else 0
+            if any(len(x) != n_dst for x in routed.values()):
+                raise KvbmError(ErrorCode.LENGTH_MISMATCH, "the destinations' block id lists have different lengths")
+            s, ns = _size_array(src_ids)
+            arrays = {d: _size_array(x)[0] for d, x in routed.items() if 0 <= d < len(dsts)}
+            PP = C.POINTER(C.c_size_t)
+            as_ptr = lambda a: a._as_parameter_ if isinstance(a, _NpView) else C.cast(a, PP)  # noqa: E731
+            dp = (PP * max(1, len(dsts)))(*[as_ptr(arrays[d]) if d in arrays else None for d in range(len(dsts))])
+            keep.append((s, arrays, dp))
+            if any(not 0 <= d < 32 for d in routed):
+                raise ValueError(f"destination indices {sorted(routed)} do not fit a 32-bit mask")
+            c.token_begin, c.token_end, c.n_src, c.n_dst = tokens.start, tokens.stop, ns, n_dst
+            c.dst_mask = sum(1 << d for d in routed)
+            c.src_ids = s.addr if type(s) is _NpView else C.addressof(s)
+            c.dst_ids = C.addressof(dp)
+        ws = (_CScatterWindow * max(1, len(plan)))(*[_CScatterWindow(w.dst_rank, w.src_layer_begin, w.dst_layer_begin, w.layer_count,
+                                                                     w.src_head_begin, w.dst_head_begin, w.head_count) for w in plan])
+        hs = (C.c_uint64 * max(1, len(dsts)))(*dsts)
+        ls = self._layer_stream([0], {0: ready_flags}, layer_done_flags) if ready_flags is not None else None
+        tok = C.c_uint64()
+        o = (options or TransferOptions())._c()
+        _check(lib().kvbm_manager_execute_repage_scatter_routed(self._h, src, len(dsts), hs, cs, len(seqs), ws, len(plan),
+                                                                C.byref(ls) if ls is not None else None, C.byref(o), C.byref(tok)))
         return TransferCompleteNotification(self, tok.value)
 
     @staticmethod

@@ -468,7 +468,8 @@ typedef struct kvbm_repage_seq {
  * concatenated table.  q0: the slot of the block's first token inside the sequence's range; tokens: how many of its tokens lie in
  * the range; small_k: the entry of the smaller-page side's concatenated table that holds the block's first small block -- when
  * those first small blocks lie before the range it wraps below 0 in uint32 and small_k + b wraps back for every small block b the
- * range touches; seq: the sequence the block belongs to (not read by the kernels). */
+ * range touches; seq: the sequence the block belongs to (not read by the kernels).  The routed scatter entries take
+ * kvbm_route_unit instead: the same record with the sequence's target mask, which the kernels read, in place of seq. */
 typedef struct kvbm_repage_unit {
   uint32_t q0, tokens, small_k, seq;
 } kvbm_repage_unit;
@@ -606,6 +607,53 @@ cudaError_t kvbm_kernels_paged_repage_scatter_batch_streamed(const kvbm_permute_
                                                              size_t num_units, int layer_begin, int layer_end, uint32_t src_row_bytes,
                                                              int cast_mode, const float* cast_scales, const kvbm_permute_stream* st,
                                                              cudaStream_t stream);
+
+/* ---- the routed scatter: each sequence of a prefill batch to its own decode workers -------------------------------------------
+ * A prefill batch mixes requests of several decode workers, so each sequence names the subset of the launch's targets it goes to:
+ * targets, bit t = targets[t].  Host memory, as kvbm_repage_seq. */
+typedef struct kvbm_route_seq {
+  uint32_t token_begin, token_end, targets;
+} kvbm_route_seq;
+
+/* kvbm_repage_unit with the sequence's target mask in place of seq: a CTA loads its unit and its mask in one 16 B load. */
+typedef struct kvbm_route_unit {
+  uint32_t q0, tokens, small_k, targets;
+} kvbm_route_unit;
+
+/* Host-only (no GPU): kvbm_kernels_repage_batch_units over the ranges of seqs, with the same rules, counts and records, except
+ * that each record's fourth word is its sequence's targets. */
+int kvbm_kernels_repage_route_units(const kvbm_route_seq* seqs, size_t num_seqs, uint32_t src_page_size, uint32_t dst_page_size,
+                                    kvbm_route_unit* out, size_t cap, size_t* num_units, size_t* src_ids, size_t* dst_ids);
+
+/* kvbm_kernels_paged_repage_scatter_batch with a target mask per sequence, in ONE launch with one signal: for each sequence i, the
+ * bytes of kvbm_kernels_paged_repage_scatter over i's range with only the targets whose bit is set in seqs[i].targets.  Every
+ * other destination byte keeps its value, including the blocks of a target's table at the positions of sequences not routed to
+ * it.  With every mask all num_targets bits, the bytes of kvbm_kernels_paged_repage_scatter_batch on the same inputs.
+ * Tables: every target's concatenated table has the batch layout, sequence i contributing its table[token_begin / Pd ..
+ * ceil(token_end / Pd)) whether or not it is routed to that target; entries of sequences not routed to a target are never read
+ * and may hold any value, so one unit table, kvbm_kernels_repage_route_units(seqs, Ps, Pd), serves every target.  Only bits below
+ * num_targets are ever consulted, on the host and in the kernel.  Within one target pool, two sequences routed to it must not
+ * share a destination block.  Everything else is the batch scatter's: casts and scales, layer and head windows, shared source
+ * blocks, the done flags and the completion word written once after every sequence landed.  cudaErrorInvalidValue, before any
+ * CUDA call, for: every rule of kvbm_kernels_paged_repage_scatter_batch (with kvbm_kernels_repage_route_units for the unit
+ * count), and a sequence whose targets is 0 or has a bit at or above num_targets. */
+cudaError_t kvbm_kernels_paged_repage_scatter_routed(const kvbm_permute_side* src, uint32_t src_num_heads, uint32_t src_page_size,
+                                                     const kvbm_scatter_target* targets, int num_targets, uint32_t dst_page_size,
+                                                     const kvbm_route_seq* seqs, size_t num_seqs, const kvbm_route_unit* units,
+                                                     size_t num_units, int layer_begin, int layer_end, uint32_t src_row_bytes,
+                                                     int cast_mode, const float* cast_scales, uint32_t epoch, uint32_t* completion_flag,
+                                                     uint32_t completion_value, cudaStream_t stream);
+
+/* The routed scatter streamed with kvbm_kernels_paged_repage_scatter_batch_streamed's flag conventions: one ready flag per source
+ * layer covers the batch, and layer_done_flags[l] is written once source layer l of every sequence landed in every target it is
+ * routed to.  After a gate timeout no done flag is written and completion_flag becomes 0xFFFFFFFF.  The argument rules are the
+ * routed scatter's plus the gate's with one source. */
+cudaError_t kvbm_kernels_paged_repage_scatter_routed_streamed(const kvbm_permute_side* src, uint32_t src_num_heads, uint32_t src_page_size,
+                                                              const kvbm_scatter_target* targets, int num_targets, uint32_t dst_page_size,
+                                                              const kvbm_route_seq* seqs, size_t num_seqs, const kvbm_route_unit* units,
+                                                              size_t num_units, int layer_begin, int layer_end, uint32_t src_row_bytes,
+                                                              int cast_mode, const float* cast_scales, const kvbm_permute_stream* st,
+                                                              cudaStream_t stream);
 
 /* Host-only (no GPU): the stride table kvbm_kernels_paged_permute walks with for one side.  out[0] = 1 when offsets count
  * from the block's first byte (universal formats) or 0 when they count from the (layer, outer) region's first byte; the

@@ -539,6 +539,33 @@ int kvbm_manager_execute_repage_scatter_batch(kvbm_transfer_manager* m, kvbm_lay
                                               size_t num_windows, const kvbm_layer_stream* ls, const kvbm_transfer_options* opts,
                                               kvbm_notification* out);
 
+/* One sequence of kvbm_manager_execute_repage_scatter_routed: a kvbm_scatter_batch_seq plus the destinations it goes to. */
+typedef struct kvbm_scatter_route_seq {
+  size_t token_begin, token_end;
+  const size_t* src_ids;        /* the source's table[token_begin / Ps .. ceil(token_end / Ps)) */
+  size_t n_src;
+  const size_t* const* dst_ids; /* [num_dsts]; dst_ids[d] (n_dst ids) read only for d in dst_mask, the others may be NULL */
+  size_t n_dst;
+  uint32_t dst_mask;            /* bit d: this sequence goes to dsts[d] */
+} kvbm_scatter_route_seq;
+
+/* A prefill batch whose sequences belong to different decode workers, as ONE hand-off: kvbm_manager_execute_repage_scatter_batch
+ * where sequence i lands only in the destinations of seqs[i].dst_mask (every window whose dst_rank bit is set), through
+ * kvbm_kernels_paged_repage_scatter_routed, or its streamed form with ls.  Under one plan that tiles one decode group's windows over
+ * several identical workers, each sequence reaches its own worker's ranks and no others.  Every other destination byte keeps its
+ * value.  Errors, first one wins: with ls, its shape; the batch's window checks and a null sequence list; num_dsts > 32
+ * (KVBM_ERR_UNSUPPORTED); then sequence by sequence the routing: a dst_mask of 0, a bit at or above num_dsts, or a bit naming a
+ * destination no window writes (KVBM_ERR_RANGE); then sequence by sequence every check of kvbm_manager_execute_repage_scatter
+ * with its code and text, the per-destination id lists read and checked for routed destinations only; last, for each destination,
+ * the ids of the sequences routed to it unique (KVBM_ERR_DUPLICATE_DST) and, where the source is that destination's layout,
+ * disjoint from every source id (KVBM_ERR_OVERLAP).  A destination block may thus appear in two sequences routed to different
+ * destinations.  bytes_moved counts the routed windows' bytes only.  per_dst_done_flags and done_flag are written once, after the
+ * last byte, never after a gate timeout. */
+int kvbm_manager_execute_repage_scatter_routed(kvbm_transfer_manager* m, kvbm_layout_handle src, size_t num_dsts, const kvbm_layout_handle* dsts,
+                                               const kvbm_scatter_route_seq* seqs, size_t num_seqs, const kvbm_scatter_window* windows,
+                                               size_t num_windows, const kvbm_layer_stream* ls, const kvbm_transfer_options* opts,
+                                               kvbm_notification* out);
+
 /* Completion: the transfer's last warp writes a flag in pinned host memory (no cudaEventQuery polling). */
 int kvbm_notification_is_complete(kvbm_transfer_manager* m, kvbm_notification n);  /* 1 / 0 / <0 error */
 int kvbm_notification_wait(kvbm_transfer_manager* m, kvbm_notification n, int64_t timeout_us);
