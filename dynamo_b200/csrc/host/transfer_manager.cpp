@@ -1186,9 +1186,10 @@ static int execute(kvbm_transfer_manager* m, kvbm_layout_handle src_h, int nd, c
 // The windows of a gather, before any layout is looked up: at least one source and one window, none in the options, at most
 // KVBM_GATHER_MAX_SOURCES, each naming a source, with heads, on destination heads no other window writes.  layers: a staged
 // gather's windows (windows[j] is layers[j]'s head window), each with layers, whose layer windows are equal (one stage) or
-// disjoint in the destination; only the windows of one stage may not share a destination head.
+// disjoint in the destination; only the windows of one stage may not share a destination head.  shared_heads: a routed gather,
+// whose windows of one stage may share destination heads (its routing checks reject a sequence routed to two of them).
 static int check_gather_windows(size_t num_srcs, const kvbm_layout_handle* srcs, const kvbm_head_window* windows, size_t nw,
-                                const kvbm_transfer_options& o, const kvbm_shard_window* layers = nullptr)
+                                const kvbm_transfer_options& o, const kvbm_shard_window* layers = nullptr, bool shared_heads = false)
 {
   if (num_srcs == 0 || !srcs || !windows || nw == 0) return fail(KVBM_ERR, "a gather needs at least one source and one window");
   if (o.head_count) return fail(KVBM_ERR, "a gather takes its head windows from the windows argument: options.head_count must be 0");
@@ -1210,6 +1211,7 @@ static int check_gather_windows(size_t num_srcs, const kvbm_layout_handle* srcs,
           continue;  // different stages may share destination heads
         }
       }
+      if (shared_heads) continue;
       if (windows[j].dst_head_begin < windows[t].dst_head_begin + windows[t].head_count &&
           windows[t].dst_head_begin < windows[j].dst_head_begin + windows[j].head_count)
         return fail(KVBM_ERR_OVERLAP, "windows " + std::to_string(t) + " and " + std::to_string(j) + " overlap in the destination");
@@ -1409,11 +1411,15 @@ struct RepageRequest {
   bool empty = false;
 };
 
-// Every check of a re-paging request after check_gather_windows, under the manager's lock, in the order above.
+// Whether a routed gather's sequence with source mask *mask reads source r; every source without a mask.
+static bool reads_source(const uint32_t* mask, size_t r) { return !mask || (r < 32 && ((*mask >> r) & 1u)); }
+
+// Every check of a re-paging request after check_gather_windows, under the manager's lock, in the order above.  mask: a routed
+// sequence's sources, whose id lists alone are read and checked.
 static int check_repage_request(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, const size_t* const* src_ids,
                                 size_t n_src, kvbm_layout_handle dst_h, const size_t* dst_ids, size_t n_dst, size_t tb, size_t te,
                                 const kvbm_head_window* windows, size_t nw, const kvbm_transfer_options& o, const kvbm_layer_stream* ls,
-                                bool gather, const kvbm_shard_window* layers, RepageRequest* R)
+                                bool gather, const kvbm_shard_window* layers, RepageRequest* R, const uint32_t* mask = nullptr)
 {
   int rc;
   if (layers && (rc = check_stage_layers(m, srcs, dst_h, layers, nw, o))) return rc;
@@ -1440,6 +1446,7 @@ static int check_repage_request(kvbm_transfer_manager* m, size_t num_srcs, const
     return rc;
   for (size_t j = 0; j < nw; ++j) {
     const size_t r = e[j].window.src_rank;
+    if (!reads_source(mask, r)) continue;
     const size_t* s = n_src ? src_ids[r] : nullptr;
     if (n_src && !s) return fail(KVBM_ERR, "null block id list");
     if ((rc = check_block_ids(s, n_src, dst_ids, n_dst, e[j].S->cfg.num_blocks, D->cfg.num_blocks, srcs[r] == dst_h))) return rc;
@@ -1486,18 +1493,58 @@ static int batch_tables(const Seq* seqs, size_t num_seqs, const std::vector<bool
 // turn and the first rejected one returns its code and text; an empty one moves nothing.  Then a batch's concatenated tables
 // are checked for a destination block named twice, and one slot takes every table (and a batch's unit table) in one copy, and
 // one launch moves every sequence: through the _batch kernel entries for a batch, else the single range's.
+// masks: a routed batch (kvbm_manager_execute_repage_batch_routed), sequence i read from the sources of masks[i] only: the
+// windows of a stage may share destination heads, the routing checks run after the null sequence list, each sequence's routed id
+// lists alone are checked, the destination's ids are checked against the ids of the sequences routed to a source in its
+// layout, unrouted positions of the staged tables are padded with block 0, and the unit table carries each sequence's window
+// mask for the routed kernel entries.
 static int execute_repage(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, kvbm_layout_handle dst_h,
                           const kvbm_repage_batch_seq* seqs, size_t num_seqs, const kvbm_head_window* windows, size_t nw,
                           const kvbm_transfer_options* opts_in, kvbm_notification* out, const kvbm_layer_stream* ls = nullptr,
-                          bool gather = true, const kvbm_shard_window* layers = nullptr, bool batch = false)
+                          bool gather = true, const kvbm_shard_window* layers = nullptr, bool batch = false, const uint32_t* masks = nullptr)
 {
   kvbm_transfer_options o{};
   if (opts_in) o = *opts_in;
   if (out) *out = 0;
   int rc;
-  if (gather && (rc = check_gather_windows(num_srcs, srcs, windows, nw, o, layers))) return rc;
+  if (gather && (rc = check_gather_windows(num_srcs, srcs, windows, nw, o, layers, masks != nullptr))) return rc;
   if (batch && num_seqs && !seqs) return fail(KVBM_ERR, "null sequence list");
+  // a routed sequence's windows: bit j for each window whose source it reads
+  auto window_mask = [&](size_t i) {
+    uint32_t w = 0;
+    for (size_t j = 0; j < nw; ++j) w |= static_cast<uint32_t>(reads_source(masks + i, windows[j].src_rank)) << j;
+    return w;
+  };
+  if (masks && num_srcs > 32)
+    return fail(KVBM_ERR_UNSUPPORTED, "a routed gather takes at most 32 sources, got " + std::to_string(num_srcs));
   std::lock_guard<std::mutex> lk(m->mu);
+  if (masks) {
+    uint32_t read = 0;
+    for (size_t j = 0; j < nw; ++j) read |= 1u << windows[j].src_rank;
+    const Layout* Dl = m->find(dst_h);  // an invalid handle is the request checks' to report
+    for (size_t i = 0; i < num_seqs; ++i) {
+      const std::string at = "sequence " + std::to_string(i);
+      if (masks[i] == 0) return fail(KVBM_ERR_RANGE, at + " is routed to no source");
+      if (num_srcs < 32 && (masks[i] >> num_srcs) != 0)
+        return fail(KVBM_ERR_RANGE, at + " is routed past the " + std::to_string(num_srcs) + " sources");
+      if (masks[i] & ~read) return fail(KVBM_ERR_RANGE, at + " is routed to a source no window reads");
+      const uint32_t wm = window_mask(i);
+      std::vector<kvbm_shard_window> routed;
+      for (size_t j = 0; j < nw; ++j) {
+        if (!((wm >> j) & 1u)) continue;
+        for (size_t t = 0; t < j; ++t) {
+          const kvbm_shard_window &a = layers[t], &b = layers[j];
+          if (((wm >> t) & 1u) && a.dst_layer_begin == b.dst_layer_begin && a.layer_count == b.layer_count &&
+              b.dst_head_begin < a.dst_head_begin + a.head_count && a.dst_head_begin < b.dst_head_begin + b.head_count)
+            return fail(KVBM_ERR_OVERLAP, "windows " + std::to_string(t) + " and " + std::to_string(j) + " overlap in the destination");
+        }
+        routed.push_back(layers[j]);
+      }
+      if (Dl && (rc = check_layers_covered(routed.data(), routed.size(), &kvbm_shard_window::dst_layer_begin, Dl->cfg.num_layers, o,
+                                           "destination")))
+        return rc;
+    }
+  }
   // every sequence resolves the same windows, destination and layer range: only `empty` (and the strategy, set for a
   // sequence that is not empty) is the last sequence's own
   RepageRequest R;
@@ -1505,13 +1552,20 @@ static int execute_repage(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_
   uint64_t bytes = 0;
   for (size_t i = 0; i < num_seqs; ++i) {
     const kvbm_repage_batch_seq& q = seqs[i];
+    const uint32_t* mask = masks ? masks + i : nullptr;
     if ((rc = check_repage_request(m, num_srcs, srcs, q.src_ids, q.n_src, dst_h, q.dst_ids, q.n_dst, q.token_begin, q.token_end, windows, nw, o,
-                                   ls, gather, layers, &R)))
+                                   ls, gather, layers, &R, mask)))
       return rc;
     if (R.empty) continue;
     any = true;
     const Layout& D = *R.D;
-    bytes += transform_bytes(R.e, nw, layers, R.lb, R.le, q.token_end - q.token_begin, D.cfg.inner_dim / D.cfg.num_heads * D.cfg.dtype_width_bytes);
+    const uint64_t head_bytes = D.cfg.inner_dim / D.cfg.num_heads * D.cfg.dtype_width_bytes;
+    if (!mask) {
+      bytes += transform_bytes(R.e, nw, layers, R.lb, R.le, q.token_end - q.token_begin, head_bytes);
+      continue;
+    }
+    for (size_t j = 0; j < nw; ++j)  // the routed windows only
+      if (reads_source(mask, windows[j].src_rank)) bytes += transform_bytes(R.e + j, 1, layers + j, R.lb, R.le, q.token_end - q.token_begin, head_bytes);
   }
   if (!any) return KVBM_OK;  // no sequences, only empty ranges or an empty layer range: nothing to move
   const Transfer* e = R.e;
@@ -1521,25 +1575,45 @@ static int execute_repage(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_
   const size_t* dst_ids = seqs[0].dst_ids;
   size_t n_src = seqs[0].n_src, n_dst = seqs[0].n_dst;
   BatchTables bt;
+  std::vector<kvbm_route_seq> routes;
   if (batch) {
     std::vector<bool> used(num_srcs + 1, false);  // the sources some window reads (the others' tables may be null), the destination
     for (size_t j = 0; j < nw; ++j) used[windows[j].src_rank] = true;
     used[num_srcs] = true;
-    auto ids = [&](const kvbm_repage_batch_seq& q, size_t k) { return k < num_srcs ? q.src_ids[k] : q.dst_ids; };
+    std::vector<size_t> pad;  // a routed batch's unrouted positions: block 0, never read
+    for (size_t i = 0; masks && i < num_seqs; ++i) pad.resize(std::max(pad.size(), seqs[i].n_src), 0);
+    auto ids = [&](const kvbm_repage_batch_seq& q, size_t k) {
+      return k == num_srcs ? q.dst_ids : reads_source(masks ? masks + (&q - seqs) : nullptr, k) ? q.src_ids[k] : pad.data();
+    };
     auto unique = [&](const std::vector<std::vector<size_t>>& cat) -> int {
       const std::vector<size_t>& cd = cat[num_srcs];
+      std::vector<size_t> routed;
       for (size_t j = 0; j < nw; ++j) {  // the destination's uniqueness once; a source in the destination's layout also against it
         const size_t r = windows[j].src_rank;
         const bool same = srcs[r] == dst_h;
-        if (j == 0 || same)
-          if (int rc = check_block_ids(cat[r].data(), cat[r].size(), cd.data(), cd.size(), e[j].S->cfg.num_blocks, D->cfg.num_blocks, same))
-            return rc;
+        if (!(j == 0 || same)) continue;
+        const std::vector<size_t>* cs = &cat[r];
+        if (masks) {  // the ids of the sequences routed to r only
+          routed.clear();
+          for (size_t i = 0; i < num_seqs; ++i)
+            if (seqs[i].token_begin != seqs[i].token_end && reads_source(masks + i, r))
+              routed.insert(routed.end(), seqs[i].src_ids[r], seqs[i].src_ids[r] + seqs[i].n_src);
+          cs = &routed;
+        }
+        if (int rc = check_block_ids(cs->data(), cs->size(), cd.data(), cd.size(), e[j].S->cfg.num_blocks, D->cfg.num_blocks, same))
+          return rc;
       }
       return KVBM_OK;
     };
     if ((rc = batch_tables(seqs, num_seqs, used, num_srcs, ups, upd, ids, unique, &bt, &n_src, &n_dst))) return rc;
     src_ids = bt.lists.data();
     dst_ids = bt.lists[num_srcs];
+    if (masks) {  // each non-empty sequence's range with its window mask, which replaces the unit's sequence index
+      for (size_t i = 0; i < num_seqs; ++i)
+        if (seqs[i].token_begin != seqs[i].token_end)
+          routes.push_back(kvbm_route_seq{static_cast<uint32_t>(seqs[i].token_begin), static_cast<uint32_t>(seqs[i].token_end), window_mask(i)});
+      for (kvbm_repage_unit& u : bt.units) u.seq = routes[u.seq].targets;
+    }
   }
 
   DeviceGuard g(m->device);
@@ -1558,6 +1632,17 @@ static int execute_repage(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_
     stage_sources(ks, layers, nw, D->cfg.num_layers, ss);
     if (batch) {
       const auto* du = reinterpret_cast<const kvbm_repage_unit*>(sl.dev_ids + units_at(num_srcs * n_src + n_dst));
+      const auto* dr = reinterpret_cast<const kvbm_route_unit*>(du);
+      if (masks && st)
+        return checked(kvbm_kernels_paged_stage_repage_gather_routed_streamed(ss, k, ups, &kd, dnh, upd, routes.data(), routes.size(), dr,
+                                                                              bt.units.size(), ilb, ile, row, o.cast_mode, o.cast_scales, st,
+                                                                              stream),
+                       "kvbm_kernels_paged_stage_repage_gather_routed_streamed");
+      if (masks)
+        return checked(kvbm_kernels_paged_stage_repage_gather_routed(ss, k, ups, &kd, dnh, upd, routes.data(), routes.size(), dr, bt.units.size(),
+                                                                     ilb, ile, row, o.cast_mode, o.cast_scales, o.done_flag, o.epoch, sl.host_flag,
+                                                                     value, stream),
+                       "kvbm_kernels_paged_stage_repage_gather_routed");
       if (st)
         return checked(kvbm_kernels_paged_stage_repage_gather_batch_streamed(ss, k, ups, &kd, dnh, upd, bt.ranges.data(), bt.ranges.size(), du,
                                                                              bt.units.size(), ilb, ile, row, o.cast_mode, o.cast_scales, st, stream),
@@ -2597,6 +2682,26 @@ extern "C" int kvbm_manager_execute_repage_batch(kvbm_transfer_manager* m, size_
   kvbm_head_window hw[KVBM_GATHER_MAX_SOURCES];
   return execute_repage(m, num_srcs, srcs, dst, seqs, num_seqs, head_windows(windows, num_windows, hw), num_windows, opts, out, ls,
                         /*gather=*/true, windows, /*batch=*/true);
+  });
+}
+
+extern "C" int kvbm_manager_execute_repage_batch_routed(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs,
+                                                        kvbm_layout_handle dst, const kvbm_repage_route_seq* seqs, size_t num_seqs,
+                                                        const kvbm_shard_window* windows, size_t num_windows, const kvbm_layer_stream* ls,
+                                                        const kvbm_transfer_options* opts, kvbm_notification* out)
+{
+  return guarded([&]() -> int {
+  if (int rc = stream_entry(m, ls, num_srcs, false, out)) return rc;
+  kvbm_head_window hw[KVBM_GATHER_MAX_SOURCES];
+  std::vector<kvbm_repage_batch_seq> qs(seqs ? num_seqs : 0);
+  std::vector<uint32_t> masks(std::max<size_t>(1, qs.size()));  // never empty: a null masks is an unrouted call
+  for (size_t i = 0; i < qs.size(); ++i) {
+    const kvbm_repage_route_seq& s = seqs[i];
+    qs[i] = kvbm_repage_batch_seq{s.token_begin, s.token_end, s.src_ids, s.n_src, s.dst_ids, s.n_dst};
+    masks[i] = s.src_mask;
+  }
+  return execute_repage(m, num_srcs, srcs, dst, seqs ? qs.data() : nullptr, num_seqs, head_windows(windows, num_windows, hw), num_windows,
+                        opts, out, ls, /*gather=*/true, windows, /*batch=*/true, masks.data());
   });
 }
 

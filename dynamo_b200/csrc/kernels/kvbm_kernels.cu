@@ -883,9 +883,13 @@ struct RepageGatherParams {
 // Unit (big block j, destination layer l, outer o) of the re-paging gather: the warp of map entry k of l's stage T reads its source
 // s at the source's own layer l + shift[s].  SCALED: one scale array for every source, scales[l * no + o] by the destination layer.
 // TABLE: a batch of sequences, whose unit comes from `units` (batch_unit) instead of the launch's one token range.
-template <int CAST, bool POW2, bool SCALED, bool PPOW2, bool TABLE = false>
+// ROUTE: a routed batch, whose unit and source mask come from record j of `routes` in one 16 B load.  The warps walk only the
+// entries of the stage's sources in the mask, numbered densely (route_entry), so no warp idles on an unrouted window; heads[s]
+// is source s's entry count.  Only the stage's sources are consulted, so mask bits at or above the launch's sources never are.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2, bool TABLE = false, bool ROUTE = false>
 __device__ __forceinline__ void repage_gather_unit(const RepageGatherParams& P, const GatherStage& T, uint32_t j, uint32_t l, uint32_t o,
-                                                   const RowSplit& r, const float* scales, const kvbm_repage_unit* units = nullptr)
+                                                   const RowSplit& r, const float* scales, const kvbm_repage_unit* units = nullptr,
+                                                   const kvbm_route_unit* routes = nullptr, const uint16_t* heads = nullptr)
 {
   constexpr int IN = CAST == KVBM_CAST_BF16_TO_FP8E4M3 ? 2 : 1;
   constexpr int OUT = CAST == KVBM_CAST_FP8E4M3_TO_BF16 ? 2 : 1;
@@ -894,16 +898,22 @@ __device__ __forceinline__ void repage_gather_unit(const RepageGatherParams& P, 
   const uint32_t first = T.first, end = T.first + T.count;
   const PermuteSide& D = g.D;
   RepageUnit u;
-  if constexpr (TABLE)
+  uint32_t mask = 0;
+  if constexpr (ROUTE) {
+    const uint4 w = __ldg(reinterpret_cast<const uint4*>(routes) + j);
+    u = {w.x, w.y, w.z};
+    mask = w.w;
+  } else if constexpr (TABLE) {
     u = batch_unit(units, j);
-  else
+  } else {
     u = repage_unit(G, j);
+  }
   const uint8_t* d_region = side_region(D, l, o);
   const ptx::Scale scale = ptx::make_scale(SCALED ? __ldg(scales + l * G.no + o) : 1.f);
   const uint32_t big_shift = G.src_small ? 3 + OUT : 3 + IN, small_shift = G.src_small ? 3 + IN : 3 + OUT;
   const uint32_t run = row_run<POW2>(r, u.tokens);
-  for (uint32_t k = first + (threadIdx.x >> 5); k < end; k += blockDim.x >> 5) {
-    const uint32_t s = g.entry[k];
+  // map entry k of source s (head h = k - first of its window)
+  auto head = [&](uint32_t k, uint32_t s) {
     const GatherSource& S = g.src[s];
     const uint32_t h = k - S.first;  // head h of the window
     const uint8_t* sh = side_region(S.S, l + g.shift[s], o) + S.s_win + h * S.S.head_stride;
@@ -914,6 +924,18 @@ __device__ __forceinline__ void repage_gather_unit(const RepageGatherParams& P, 
     const uint8_t* bh = (ss ? dh : sh) + static_cast<uint64_t>(__ldg(B.ids + j)) * B.block_stride;
     repage_head_rows<CAST, POW2, SCALED, PPOW2>(bh, static_cast<uint32_t>(B.tok_stride), big_shift, ss ? sh : dh, Sm.ids, u.small_k,
                                                 Sm.block_stride, static_cast<uint32_t>(Sm.tok_stride), small_shift, G, u.q0, run, r, scale);
+  };
+  if constexpr (ROUTE) {
+    // routed entry i of the unit: the stage's map runs source by source in source order, so skip whole sources up to it
+    const uint32_t warps = blockDim.x >> 5;
+    uint32_t i = threadIdx.x >> 5;
+    for (uint32_t rest = T.sources & mask; rest != 0; rest &= rest - 1) {
+      const uint32_t s = __ffs(rest) - 1, n = heads[s], at = g.src[s].first;
+      for (; i < n; i += warps) head(at + i, s);
+      i -= n;
+    }
+  } else {
+    for (uint32_t k = first + (threadIdx.x >> 5); k < end; k += blockDim.x >> 5) head(k, g.entry[k]);
   }
 }
 
@@ -935,6 +957,22 @@ kvbm_paged_batch_repage_gather_kernel(const __grid_constant__ RepageGatherParams
 {
   const auto [j, l, rem] = repage_cta(P.geo);
   repage_gather_unit<CAST, POW2, SCALED, PPOW2, true>(P, stage_of(P.g, l), j, l, rem % P.geo.no, r, scales, units);
+}
+
+// Each source's entry count in the head map (its window's heads), which a routed unit needs to skip unrouted sources.
+struct SourceHeads {
+  uint16_t n[KVBM_GATHER_MAX_SOURCES];
+};
+
+// kvbm_paged_batch_repage_gather_kernel over a routed batch: record j of `routes` also names the sources big block j reads, and
+// only their entries are walked.  The same bound: three CTAs per SM.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__global__ void __launch_bounds__(256, 3)
+kvbm_paged_repage_fanin_kernel(const __grid_constant__ RepageGatherParams P, const __grid_constant__ SourceHeads H, const kvbm_route_unit* routes,
+                               RowSplit r, const float* scales)
+{
+  const auto [j, l, rem] = repage_cta(P.geo);
+  repage_gather_unit<CAST, POW2, SCALED, PPOW2, true, true>(P, stage_of(P.g, l), j, l, rem % P.geo.no, r, scales, nullptr, routes, H.n);
 }
 
 // The re-paging scatter, the gather's mirror image: ONE source pool of page Ps (a prefill rank) into up to
@@ -1236,6 +1274,18 @@ kvbm_gated_batch_repage_gather_kernel(const __grid_constant__ RepageGatherParams
   });
 }
 
+// kvbm_gated_batch_repage_gather_kernel over a routed batch (num_big: the length of `routes`).  Each stage's sources are the
+// routed ones only (the launch ANDs the union of the batch's masks in), so a source no sequence reads is never waited on.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__global__ void __launch_bounds__(256, 1)
+kvbm_gated_repage_fanin_kernel(const __grid_constant__ RepageGatherParams P, const __grid_constant__ GateArgs A, const __grid_constant__ SourceHeads H,
+                               const kvbm_route_unit* routes, uint32_t num_big, RowSplit r, const float* scales, uint32_t batch)
+{
+  gated_repage_units(A, P.g, P.geo, num_big, batch, [&](const GatherStage& T, uint32_t j, uint32_t l, uint32_t o) {
+    repage_gather_unit<CAST, POW2, SCALED, PPOW2, true, true>(P, T, j, l, o, r, scales, nullptr, routes, H.n);
+  });
+}
+
 // The push kernels' hook in arrive_transfer: the num_flags target done flags of F, with A.ss's own and before the completion word.
 __device__ __forceinline__ auto target_done(const ScatterFlags& F, const int& num_flags, const GateArgs& A)
 {
@@ -1490,6 +1540,10 @@ static cudaError_t preload_kernels()
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_route_kernel<c, p, sc, false>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_route_kernel<c, p, sc, true>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_route_kernel<c, p, sc, false>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_fanin_kernel<c, p, sc, true>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_fanin_kernel<c, p, sc, false>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_fanin_kernel<c, p, sc, true>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_fanin_kernel<c, p, sc, false>);
         });
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_layer_signal_kernel);
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_scatter_signal_kernel);
@@ -1620,13 +1674,21 @@ static bool order_stages(const GatherStage* T, int num_stages, int lb, int le, i
 // destination; the stages covering every layer of [lb, le); within a stage, windows on destination heads no other window of the
 // stage writes (two would race); every rule of fill_gather_source; at most max_covered covered heads over all stages.  Fills
 // P->src, P->covered, P->stage and P->shift, and with several sources the head map P->entry, stage by stage in ascending
-// destination layers; *widest: the most heads of one stage.
+// destination layers; *widest: the most heads of one stage.  masks: a routed gather's distinct source masks, under which two
+// windows of a stage may share destination heads unless one mask holds both.
 static bool fill_stage_sources(const kvbm_stage_source* srcs, int num_srcs, uint32_t dst_num_heads, uint32_t nl, uint32_t no, int lb, int le,
-                               uint32_t page_size, uint32_t src_row_bytes, uint32_t max_covered, GatherParams* P, uint32_t* widest)
+                               uint32_t page_size, uint32_t src_row_bytes, uint32_t max_covered, GatherParams* P, uint32_t* widest,
+                               const std::vector<uint32_t>* masks = nullptr)
 {
   int stage_of_src[KVBM_GATHER_MAX_SOURCES];
   int num_stages = 0;
   GatherStage* T = P->stage;
+  auto routed_together = [&](int s, int t) {
+    if (!masks) return true;
+    for (uint32_t m : *masks)
+      if (((m >> s) & 1u) && ((m >> t) & 1u)) return true;
+    return false;
+  };
   for (int s = 0; s < num_srcs; ++s) {
     const kvbm_stage_source& X = srcs[s];
     const uint64_t src_end = static_cast<uint64_t>(X.src_layer_begin) + X.layer_count, dst_end = static_cast<uint64_t>(X.dst_layer_begin) + X.layer_count;
@@ -1634,7 +1696,7 @@ static bool fill_stage_sources(const kvbm_stage_source* srcs, int num_srcs, uint
     const int k = stage_of_src[s] = window_stage(T, &num_stages, X.dst_layer_begin, static_cast<uint32_t>(dst_end));
     if (k < 0) return false;
     for (int t = 0; t < s; ++t)
-      if (stage_of_src[t] == k && heads_overlap(X.src, srcs[t].src)) return false;
+      if (stage_of_src[t] == k && heads_overlap(X.src, srcs[t].src) && routed_together(s, t)) return false;
     T[k].sources |= 1u << s;
     P->shift[s] = X.src_layer_begin - X.dst_layer_begin;
   }
@@ -1666,13 +1728,14 @@ static bool fill_stage_sources(const kvbm_stage_source* srcs, int num_srcs, uint
 }
 
 // The gate's own argument rules (kvbm_permute_stream), checked before anything else of a streamed entry: a descriptor, a known
-// gate mode, a workspace when the caller asks for the spinning form, and a ready-flag array for every used source.
-static bool stream_args_ok(const kvbm_permute_stream* st, int num_srcs)
+// gate mode, a workspace when the caller asks for the spinning form, and a ready-flag array for every used source (a routed
+// gather's: every source of `used`).
+static bool stream_args_ok(const kvbm_permute_stream* st, int num_srcs, uint32_t used = ~0u)
 {
   if (!st || st->gate_mode < KVBM_GATE_AUTO || st->gate_mode > KVBM_GATE_STREAM_WAIT) return false;
   if (st->gate_mode == KVBM_GATE_SPIN && !st->sync_workspace) return false;
   for (int s = 0; s < num_srcs && s < KVBM_GATHER_MAX_SOURCES; ++s)
-    if (!st->layer_ready_flags[s]) return false;
+    if (((used >> s) & 1u) && !st->layer_ready_flags[s]) return false;
   return true;
 }
 
@@ -1888,7 +1951,8 @@ static bool repage_pages(uint32_t src_page, uint32_t dst_page, int layer_begin, 
 }
 
 // A batch of sequences of a re-paging launch: the caller's ranges (host) and unit table (device-accessible).  route: a routed
-// scatter's batch, whose ranges and target masks are route_seqs and whose unit table is route_units (seqs and units unused).
+// batch, whose ranges and masks (a scatter's targets, a gather's sources) are route_seqs and whose unit table is route_units
+// (seqs and units unused).
 struct RepageBatch {
   const kvbm_repage_seq* seqs;
   size_t num_seqs;
@@ -1959,7 +2023,10 @@ static bool repage_launch(const kvbm_permute_side* side, uint32_t src_page, uint
 // there is nothing to move; then launches kvbm_paged_repage_kernel for a plain re-page, else kvbm_paged_repage_gather_kernel,
 // and the signal.  max_covered and st: as launch_paged_permute's (st takes the gated re-paging gather kernel, or per layer this
 // launch unstreamed).  B: a batch of sequences in place of the one token range (token_begin / token_end unused), which always
-// takes the batch gather kernels.
+// takes the batch gather kernels, or the fan-in kernels for a routed batch: bit s of a sequence's mask names srcs[s], every mask
+// must be non-zero and below bit num_srcs, and two windows of a stage may then share destination heads unless one mask holds both.
+// Each stage's sources are ANDed with the union of the masks, so both gate forms wait on routed sources only, and a CTA has as
+// many warps as the most routed entries of one stage under one mask (up to 8).
 static cudaError_t launch_paged_repage_gather(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page, const kvbm_permute_side* dst,
                                               uint32_t dst_num_heads, uint32_t dst_page, uint32_t token_begin, uint32_t token_end,
                                               int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
@@ -1968,8 +2035,18 @@ static cudaError_t launch_paged_repage_gather(const kvbm_stage_source* srcs, int
                                               const RepageBatch* B = nullptr)
 {
   RepageLaunch L;
-  if (!srcs || num_srcs < 1 || num_srcs > KVBM_GATHER_MAX_SOURCES ||
-      !repage_launch(dst, src_page, dst_page, token_begin, token_end, layer_begin, layer_end, src_row_bytes, cast_mode, cast_scales, B, &L))
+  if (!srcs || num_srcs < 1 || num_srcs > KVBM_GATHER_MAX_SOURCES) return cudaErrorInvalidValue;
+  const bool route = B && B->route;
+  std::vector<uint32_t> masks;  // a routed batch's distinct source masks
+  uint32_t routed = 0;          // and their union
+  if (route && B->route_seqs)
+    for (size_t i = 0; i < B->num_seqs; ++i) {
+      const uint32_t m = B->route_seqs[i].targets;
+      if (m == 0 || (m >> num_srcs) != 0) return cudaErrorInvalidValue;
+      if (std::find(masks.begin(), masks.end(), m) == masks.end()) masks.push_back(m);
+      routed |= m;
+    }
+  if (!repage_launch(dst, src_page, dst_page, token_begin, token_end, layer_begin, layer_end, src_row_bytes, cast_mode, cast_scales, B, &L))
     return cudaErrorInvalidValue;
   if (L.units == 0) return signal_launch(done_flag, epoch, completion_flag, completion_value, stream);
   const uint32_t nl = L.nl, no = L.no;
@@ -1979,9 +2056,24 @@ static cudaError_t launch_paged_repage_gather(const kvbm_stage_source* srcs, int
   if (static_cast<uint64_t>(dst_page) * dst_num_heads * L.dst_row_bytes != dst->layout.region_bytes) return cudaErrorInvalidValue;
   if (!fill_permute_side(*dst, nl, no, dst_num_heads, dst_page, static_cast<uint32_t>(L.dst_row_bytes), &P.g.D)) return cudaErrorInvalidValue;
   uint32_t widest;
-  if (!fill_stage_sources(srcs, num_srcs, dst_num_heads, nl, no, layer_begin, layer_end, src_page, src_row_bytes, max_covered, &P.g, &widest))
+  if (!fill_stage_sources(srcs, num_srcs, dst_num_heads, nl, no, layer_begin, layer_end, src_page, src_row_bytes, max_covered, &P.g, &widest,
+                          route ? &masks : nullptr))
     return cudaErrorInvalidValue;
   P.geo.nh = P.g.covered;
+  SourceHeads H{};
+  if (route) {
+    for (int s = 0; s < num_srcs; ++s) H.n[s] = static_cast<uint16_t>(srcs[s].src.head_count);
+    widest = 0;
+    for (GatherStage& T : P.g.stage) {
+      T.sources &= routed;
+      for (uint32_t m : masks) {
+        uint32_t n = 0;
+        for (int s = 0; s < num_srcs; ++s)
+          if ((T.sources & m) >> s & 1u) n += H.n[s];
+        widest = std::max(widest, n);
+      }
+    }
+  }
   const int threads = static_cast<int>(std::min<uint32_t>(8, widest)) * 32;
   const unsigned grid = static_cast<unsigned>(L.units);
   if (st)
@@ -1993,7 +2085,9 @@ static cudaError_t launch_paged_repage_gather(const kvbm_stage_source* srcs, int
         },
         [&](const GateArgs& A, unsigned ctas, uint32_t batch) {
           with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, L.page_pow2, [&](auto c, auto p, auto sc, auto pp) {
-            if (B)
+            if (route)
+              kvbm_gated_repage_fanin_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, A, H, B->route_units, L.num_big, r, cast_scales, batch);
+            else if (B)
               kvbm_gated_batch_repage_gather_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, A, B->units, L.num_big, r, cast_scales, batch);
             else
               kvbm_gated_repage_gather_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, A, L.num_big, r, cast_scales, batch);
@@ -2007,7 +2101,9 @@ static cudaError_t launch_paged_repage_gather(const kvbm_stage_source* srcs, int
   R.small = P.geo.src_small ? P.g.src[0].S : P.g.D;
   R.g = P.geo;
   with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, L.page_pow2, [&](auto c, auto p, auto sc, auto pp) {
-    if (B)
+    if (route)
+      kvbm_paged_repage_fanin_kernel<c, p, sc, pp><<<grid, threads, 0, stream>>>(P, H, B->route_units, r, cast_scales);
+    else if (B)
       kvbm_paged_batch_repage_gather_kernel<c, p, sc, pp><<<grid, threads, 0, stream>>>(P, B->units, r, cast_scales);
     else if (plain)
       kvbm_paged_repage_kernel<c, p, sc, pp><<<grid, threads, 0, stream>>>(R, r, cast_scales);
@@ -2518,6 +2614,36 @@ kvbm_kernels_paged_stage_repage_gather_batch_streamed(const kvbm_stage_source* s
 {
   if (!stream_args_ok(st, num_srcs)) return cudaErrorInvalidValue;
   const RepageBatch B{seqs, num_seqs, units, num_units};
+  return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, 0, 0, layer_begin, layer_end,
+                                    src_row_bytes, cast_mode, cast_scales, st->done_flag, st->epoch, st->completion_flag,
+                                    st->completion_value, KVBM_GATHER_MAX_HEADS, stream, st, &B);
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_stage_repage_gather_routed(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page_size, const kvbm_permute_side* dst,
+                                              uint32_t dst_num_heads, uint32_t dst_page_size, const kvbm_route_seq* seqs, size_t num_seqs,
+                                              const kvbm_route_unit* units, size_t num_units, int layer_begin, int layer_end,
+                                              uint32_t src_row_bytes, int cast_mode, const float* cast_scales, uint32_t* done_flag,
+                                              uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
+{
+  const RepageBatch B{nullptr, num_seqs, nullptr, num_units, true, seqs, units};
+  return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, 0, 0, layer_begin, layer_end,
+                                    src_row_bytes, cast_mode, cast_scales, done_flag, epoch, completion_flag, completion_value,
+                                    KVBM_GATHER_MAX_HEADS, stream, nullptr, &B);
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_stage_repage_gather_routed_streamed(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page_size,
+                                                       const kvbm_permute_side* dst, uint32_t dst_num_heads, uint32_t dst_page_size,
+                                                       const kvbm_route_seq* seqs, size_t num_seqs, const kvbm_route_unit* units,
+                                                       size_t num_units, int layer_begin, int layer_end, uint32_t src_row_bytes,
+                                                       int cast_mode, const float* cast_scales, const kvbm_permute_stream* st,
+                                                       cudaStream_t stream)
+{
+  uint32_t used = 0;  // the sources some sequence is routed to: only they need ready flags
+  for (size_t i = 0; seqs && i < num_seqs; ++i) used |= seqs[i].targets;
+  if (!stream_args_ok(st, num_srcs, used)) return cudaErrorInvalidValue;
+  const RepageBatch B{nullptr, num_seqs, nullptr, num_units, true, seqs, units};
   return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, 0, 0, layer_begin, layer_end,
                                     src_row_bytes, cast_mode, cast_scales, st->done_flag, st->epoch, st->completion_flag,
                                     st->completion_value, KVBM_GATHER_MAX_HEADS, stream, st, &B);

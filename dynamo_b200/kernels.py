@@ -287,6 +287,10 @@ def lib() -> C.CDLL:
         L.kvbm_kernels_paged_repage_scatter_routed.restype = i
         L.kvbm_kernels_paged_repage_scatter_routed_streamed.argtypes = L.kvbm_kernels_paged_repage_scatter_batch_streamed.argtypes
         L.kvbm_kernels_paged_repage_scatter_routed_streamed.restype = i
+        L.kvbm_kernels_paged_stage_repage_gather_routed.argtypes = L.kvbm_kernels_paged_stage_repage_gather_batch.argtypes
+        L.kvbm_kernels_paged_stage_repage_gather_routed.restype = i
+        L.kvbm_kernels_paged_stage_repage_gather_routed_streamed.argtypes = L.kvbm_kernels_paged_stage_repage_gather_batch_streamed.argtypes
+        L.kvbm_kernels_paged_stage_repage_gather_routed_streamed.restype = i
         L.kvbm_kernels_permute_strides.argtypes = [i, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64, C.c_uint64,
                                                    C.POINTER(C.c_uint64)]
         L.kvbm_kernels_permute_strides.restype = i
@@ -317,7 +321,8 @@ EXPORTED_SYMBOLS = [
     "kvbm_kernels_paged_stage_repage_gather_batch_streamed", "kvbm_kernels_paged_repage_scatter",
     "kvbm_kernels_paged_repage_scatter_streamed", "kvbm_kernels_paged_repage_scatter_batch",
     "kvbm_kernels_paged_repage_scatter_batch_streamed", "kvbm_kernels_repage_route_units", "kvbm_kernels_paged_repage_scatter_routed",
-    "kvbm_kernels_paged_repage_scatter_routed_streamed",
+    "kvbm_kernels_paged_repage_scatter_routed_streamed", "kvbm_kernels_paged_stage_repage_gather_routed",
+    "kvbm_kernels_paged_stage_repage_gather_routed_streamed",
 ]
 
 
@@ -698,6 +703,38 @@ def paged_repage_scatter_routed_streamed(src: PermuteSide, src_num_heads: int, s
                                                                    units or None, num_units, layer_begin, layer_end, src_row_bytes,
                                                                    int(cast_mode), scales_ptr(cast_scales),
                                                                    C.byref(st) if st is not None else None, stream)
+
+
+def paged_stage_repage_gather_routed(srcs: Sequence[StageSource], src_page_size: int, dst: PermuteSide, dst_num_heads: int,
+                                     dst_page_size: int, seqs: Sequence[Tuple[int, int, int]], units: int, num_units: int, layer_begin: int,
+                                     layer_end: int, src_row_bytes: int, cast_mode: int = 0, cast_scales=None, done_flag: int = 0,
+                                     epoch: int = 0, completion_flag: int = 0, completion_value: int = 0, stream: int = 0) -> int:
+    """`paged_stage_repage_gather_batch` with a source mask per sequence, in ONE launch with one signal: `seqs` are (token_begin,
+    token_end, sources), bit s of sources naming srcs[s]; every source's block_ids has the batch layout (the positions of sequences
+    not routed to it are never read); `units` is the device address of the table `repage_route_units` made for the same sequences
+    and pages.  Two windows of a stage may share destination heads when no mask holds both.
+    include/kvbm_kernels.h (kvbm_kernels_paged_stage_repage_gather_routed)."""
+    arr = (StageSource * max(1, len(srcs)))(*srcs)
+    return lib().kvbm_kernels_paged_stage_repage_gather_routed(arr, len(srcs), src_page_size, C.byref(dst), dst_num_heads, dst_page_size,
+                                                               C.cast(_route_seqs(seqs), C.c_void_p), len(seqs), units or None, num_units,
+                                                               layer_begin, layer_end, src_row_bytes, int(cast_mode),
+                                                               scales_ptr(cast_scales), done_flag or None, epoch, completion_flag or None,
+                                                               completion_value, stream)
+
+
+def paged_stage_repage_gather_routed_streamed(srcs: Sequence[StageSource], src_page_size: int, dst: PermuteSide, dst_num_heads: int,
+                                              dst_page_size: int, seqs: Sequence[Tuple[int, int, int]], units: int, num_units: int,
+                                              layer_begin: int, layer_end: int, src_row_bytes: int, cast_mode: int, cast_scales,
+                                              st: Optional[PermuteStream], stream: int = 0) -> int:
+    """`paged_stage_repage_gather_routed` streamed with `paged_stage_repage_gather_batch_streamed`'s flags; only the sources some
+    sequence is routed to are waited on, and the others' ready flags may be 0.
+    include/kvbm_kernels.h (kvbm_kernels_paged_stage_repage_gather_routed_streamed)."""
+    arr = (StageSource * max(1, len(srcs)))(*srcs)
+    return lib().kvbm_kernels_paged_stage_repage_gather_routed_streamed(arr, len(srcs), src_page_size, C.byref(dst), dst_num_heads,
+                                                                        dst_page_size, C.cast(_route_seqs(seqs), C.c_void_p), len(seqs),
+                                                                        units or None, num_units, layer_begin, layer_end, src_row_bytes,
+                                                                        int(cast_mode), scales_ptr(cast_scales),
+                                                                        C.byref(st) if st is not None else None, stream)
 
 
 def permute_strides(kv_layout: int, num_layers: int, outer_dim: int, num_heads: int, page_size: int, row_bytes: int,

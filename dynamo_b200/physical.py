@@ -134,6 +134,12 @@ class _CRepageBatchSeq(C.Structure):
                 ("dst_ids", C.c_void_p), ("n_dst", C.c_size_t)]
 
 
+class _CRepageRouteSeq(C.Structure):
+    """struct kvbm_repage_route_seq"""
+    _fields_ = [("token_begin", C.c_size_t), ("token_end", C.c_size_t), ("src_ids", C.c_void_p), ("n_src", C.c_size_t),
+                ("dst_ids", C.c_void_p), ("n_dst", C.c_size_t), ("src_mask", C.c_uint32)]
+
+
 class _CScatterBatchSeq(C.Structure):
     """struct kvbm_scatter_batch_seq"""
     _fields_ = [("token_begin", C.c_size_t), ("token_end", C.c_size_t), ("src_ids", C.c_void_p), ("n_src", C.c_size_t),
@@ -268,7 +274,7 @@ EXPORTED_SYMBOLS = [
     "kvbm_tp_pp_reshard_plan", "kvbm_manager_execute_stage_gather", "kvbm_manager_execute_stage_repage_gather",
     "kvbm_manager_execute_repage_batch", "kvbm_tp_pp_scatter_plan", "kvbm_manager_execute_repage_scatter",
     "kvbm_manager_execute_repage_scatter_streamed", "kvbm_manager_execute_repage_scatter_batch",
-    "kvbm_manager_execute_repage_scatter_routed",
+    "kvbm_manager_execute_repage_scatter_routed", "kvbm_manager_execute_repage_batch_routed",
 ]
 
 
@@ -331,6 +337,8 @@ def lib() -> C.CDLL:
                                                                P(_CLayerStream), P(_COptions), P(u64)]
         L.kvbm_manager_execute_repage_batch.argtypes = [vp, sz, P(u64), u64, P(_CRepageBatchSeq), sz, P(_CShardWindow), sz, P(_CLayerStream),
                                                         P(_COptions), P(u64)]
+        L.kvbm_manager_execute_repage_batch_routed.argtypes = [vp, sz, P(u64), u64, P(_CRepageRouteSeq), sz, P(_CShardWindow), sz,
+                                                               P(_CLayerStream), P(_COptions), P(u64)]
         L.kvbm_tp_pp_scatter_plan.argtypes = [sz, sz, sz, sz, P(sz), sz, sz, P(sz), sz, P(_CScatterWindow), sz, P(sz)]
         L.kvbm_manager_execute_repage_scatter.argtypes = [vp, u64, vp, sz, sz, P(u64), P(P(sz)), sz, sz, sz, P(_CScatterWindow), sz,
                                                           P(_COptions), P(u64)]
@@ -552,6 +560,17 @@ def tile_scatter_plan(plan: Sequence[ScatterWindow], num_workers: int, ranks_per
     if num_workers < 1 or any(w.dst_rank >= ranks_per_worker for w in plan):
         raise ValueError(f"a plan for {ranks_per_worker} ranks per worker cannot be tiled {num_workers} times")
     return [dataclasses.replace(w, dst_rank=w.dst_rank + k * ranks_per_worker) for k in range(num_workers) for w in plan]
+
+
+def tile_reshard_plan(plan: Sequence[ShardWindow], num_workers: int, ranks_per_worker: int) -> List[ShardWindow]:
+    """One prefill group's re-shard plan (`tp_pp_reshard_plan`) repeated over `num_workers` identical prefill workers of
+    `ranks_per_worker` ranks each, the mirror of `tile_scatter_plan`: worker w's copy of a window reads source rank src_rank +
+    w * ranks_per_worker, so the sources are worker-major and a routed sequence served by worker w sets bits w * ranks_per_worker
+    .. +ranks_per_worker - 1.  The copies of two workers write the same destination heads, which a routed gather allows as long
+    as no sequence is routed to both."""
+    if num_workers < 1 or any(w.src_rank >= ranks_per_worker for w in plan):
+        raise ValueError(f"a plan for {ranks_per_worker} ranks per worker cannot be tiled {num_workers} times")
+    return [dataclasses.replace(w, src_rank=w.src_rank + k * ranks_per_worker) for k in range(num_workers) for w in plan]
 
 
 class TransferCompleteNotification:
@@ -929,6 +948,48 @@ class TransferManager:
         o = (options or TransferOptions())._c()
         _check(lib().kvbm_manager_execute_repage_batch(self._h, len(ranks), hs, dst, cs, len(seqs), ws, len(plan),
                                                        C.byref(ls) if ls is not None else None, C.byref(o), C.byref(tok)))
+        return TransferCompleteNotification(self, tok.value)
+
+    def execute_repage_batch_routed(self, sources: Mapping[int, int], dst: int, seqs: Sequence[tuple], plan: Sequence[ShardWindow],
+                                    options: Optional[TransferOptions] = None, ready_flags: Optional[Mapping[int, int]] = None,
+                                    layer_done_flags: int = 0, num_layers: Optional[int] = None) -> TransferCompleteNotification:
+        """A decode step's new sequences, each served by its own prefill worker, as ONE hand-off
+        (kvbm_manager_execute_repage_batch_routed): `execute_repage_batch` where `seqs` is a list of (tokens, {src_rank:
+        src_block_ids}, dst_block_ids), the dict's keys being the source ranks the sequence is read from, under one `plan`
+        (`tile_reshard_plan` over identical prefill workers, or a HeadWindow list with `num_layers`).  Each sequence is read through
+        its own sources' windows only; windows of one stage may write the same destination heads as long as no sequence is routed
+        to two of them.  One staged copy, one launch, one notification; with `ready_flags` (source rank -> flags) it streams as
+        `execute_repage_batch` does, and only the sources some sequence names are waited on."""
+        if plan and isinstance(plan[0], HeadWindow):
+            if num_layers is None:
+                raise ValueError("a HeadWindow plan needs num_layers, the destination's layer count")
+            plan = [ShardWindow(w.src_rank, 0, 0, num_layers, w.src_head_begin, w.dst_head_begin, w.head_count) for w in plan]
+        ranks = sorted({w.src_rank for w in plan})
+        index = {r: i for i, r in enumerate(ranks)}
+        hs = (C.c_uint64 * max(1, len(ranks)))(*[sources[r] for r in ranks])
+        ws = self._shard_windows(ranks, plan)
+        keep, cs = [], (_CRepageRouteSeq * max(1, len(seqs)))()
+        for c, (tokens, src_ids, dst_ids) in zip(cs, seqs):
+            if tokens.step != 1:
+                raise ValueError("tokens must be a range with step 1")
+            n_src = len(next(iter(src_ids.values()))) if src_ids else 0
+            if any(len(x) != n_src for x in src_ids.values()):
+                raise KvbmError(ErrorCode.LENGTH_MISMATCH, "the sources' block id lists have different lengths")
+            if any(r not in index for r in src_ids):
+                raise ValueError(f"source ranks {sorted(set(src_ids) - set(index))} are read by no window of the plan")
+            arrays = {index[r]: _size_array(x)[0] for r, x in src_ids.items()}
+            d, n_dst = _size_array(dst_ids)
+            sp = (C.c_void_p * max(1, len(ranks)))(*[(a.addr if type(a) is _NpView else C.addressof(a)) if (a := arrays.get(i)) is not None
+                                                     else None for i in range(len(ranks))])
+            keep += [arrays, d, sp]
+            c.token_begin, c.token_end, c.src_ids, c.n_src = tokens.start, tokens.stop, C.addressof(sp), n_src
+            c.dst_ids, c.n_dst = (d.addr if type(d) is _NpView else C.addressof(d)), n_dst
+            c.src_mask = sum(1 << i for i in arrays)
+        ls = self._layer_stream(ranks, ready_flags, layer_done_flags) if ready_flags is not None else None
+        tok = C.c_uint64()
+        o = (options or TransferOptions())._c()
+        _check(lib().kvbm_manager_execute_repage_batch_routed(self._h, len(ranks), hs, dst, cs, len(seqs), ws, len(plan),
+                                                              C.byref(ls) if ls is not None else None, C.byref(o), C.byref(tok)))
         return TransferCompleteNotification(self, tok.value)
 
     def execute_repage_scatter(self, src: int, src_block_ids: Sequence[int], dsts: Sequence[int], dst_block_ids: Sequence[Sequence[int]],

@@ -655,6 +655,42 @@ cudaError_t kvbm_kernels_paged_repage_scatter_routed_streamed(const kvbm_permute
                                                               int cast_mode, const float* cast_scales, const kvbm_permute_stream* st,
                                                               cudaStream_t stream);
 
+/* ---- the routed gather: each sequence of a decode step from the prefill workers that served it -------------------------------
+ * The pull-side counterpart of the routed scatter, with the same kvbm_route_seq / kvbm_route_unit and
+ * kvbm_kernels_repage_route_units: on the gather, bit s of a sequence's `targets` names srcs[s] (one kvbm_stage_source, one
+ * window), the sources the sequence is read from.
+ * kvbm_kernels_paged_stage_repage_gather_batch with a source mask per sequence, in ONE launch with one signal: for each sequence
+ * i, the bytes of kvbm_kernels_paged_stage_repage_gather over i's range with only the windows whose bit is set in
+ * seqs[i].targets.  Every other destination byte keeps its value (a layer none of i's windows covers included).  Tables: every
+ * source's concatenated table has the batch layout, sequence i contributing its table whether or not it is routed to that
+ * source; positions of sequences not routed to a source are never read and may hold any value, so one unit table,
+ * kvbm_kernels_repage_route_units(seqs, Ps, Pd), serves every source.  A source no sequence is routed to is never read or
+ * waited on.  One rule differs from the batch gather: two head windows of one stage may share destination heads when no
+ * sequence's mask holds both (two prefill workers' windows write the same decode heads, for different sequences); the 256-head
+ * limit counts every window's heads, shared or not.  Everything else is the batch gather's: stages, layer windows, casts and
+ * scales, shared source blocks, no destination block in two sequences, and the done / completion flags written once after every
+ * sequence landed.  cudaErrorInvalidValue, before any CUDA call, for: every rule of kvbm_kernels_paged_stage_repage_gather_batch
+ * but the shared heads (with kvbm_kernels_repage_route_units for the unit count), a sequence whose mask is 0 or has a bit at or
+ * above num_srcs, and a mask holding two windows of one stage that share a destination head. */
+cudaError_t kvbm_kernels_paged_stage_repage_gather_routed(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page_size,
+                                                          const kvbm_permute_side* dst, uint32_t dst_num_heads, uint32_t dst_page_size,
+                                                          const kvbm_route_seq* seqs, size_t num_seqs, const kvbm_route_unit* units,
+                                                          size_t num_units, int layer_begin, int layer_end, uint32_t src_row_bytes,
+                                                          int cast_mode, const float* cast_scales, uint32_t* done_flag, uint32_t epoch,
+                                                          uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream);
+
+/* The routed gather streamed with kvbm_kernels_paged_stage_repage_gather_batch_streamed's flag conventions: one ready flag per
+ * (source, layer) covers the batch, and layer_done_flags[l] is written once layer l of every sequence landed.  Only the sources
+ * some sequence is routed to are waited on and need st->layer_ready_flags[s]; the others may be NULL.  The argument rules are
+ * the routed gather's plus the gate's. */
+cudaError_t kvbm_kernels_paged_stage_repage_gather_routed_streamed(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page_size,
+                                                                   const kvbm_permute_side* dst, uint32_t dst_num_heads,
+                                                                   uint32_t dst_page_size, const kvbm_route_seq* seqs, size_t num_seqs,
+                                                                   const kvbm_route_unit* units, size_t num_units, int layer_begin,
+                                                                   int layer_end, uint32_t src_row_bytes, int cast_mode,
+                                                                   const float* cast_scales, const kvbm_permute_stream* st,
+                                                                   cudaStream_t stream);
+
 /* Host-only (no GPU): the stride table kvbm_kernels_paged_permute walks with for one side.  out[0] = 1 when offsets count
  * from the block's first byte (universal formats) or 0 when they count from the (layer, outer) region's first byte; the
  * element (layer l, outer o, head h, token t) then sits at  [out[0] ? l * out[1] + o * out[2] : 0] + h * out[3] + t * out[4].

@@ -467,6 +467,36 @@ int kvbm_manager_execute_repage_batch(kvbm_transfer_manager* m, size_t num_srcs,
                                       size_t num_windows, const kvbm_layer_stream* ls, const kvbm_transfer_options* opts,
                                       kvbm_notification* out);
 
+/* One sequence of kvbm_manager_execute_repage_batch_routed: a kvbm_repage_batch_seq plus the sources it is read from. */
+typedef struct kvbm_repage_route_seq {
+  size_t token_begin, token_end;
+  const size_t* const* src_ids; /* [num_srcs]; src_ids[r] (n_src ids) read only for r in src_mask, the others may be NULL */
+  size_t n_src;
+  const size_t* dst_ids;        /* the destination's table[token_begin / Pd .. ceil(token_end / Pd)) */
+  size_t n_dst;
+  uint32_t src_mask;            /* bit r: this sequence is read from srcs[r] (every window whose src_rank bit is set) */
+} kvbm_repage_route_seq;
+
+/* A decode step's new sequences, each served by its own prefill worker, as ONE hand-off: kvbm_manager_execute_repage_batch where
+ * sequence i is read only through the windows whose source is in seqs[i].src_mask, through
+ * kvbm_kernels_paged_stage_repage_gather_routed, or its streamed form with ls.  Under one plan that tiles one prefill group's
+ * windows over several identical workers (tile_reshard_plan in Python), the windows of two workers write the same destination
+ * heads; that is allowed as long as no sequence is routed to both.  Every other destination byte keeps its value.  Errors, first
+ * one wins: with ls, its shape (ls->num_srcs == num_srcs, every entry non-null); the batch's window checks except that two windows
+ * of one stage may share destination heads; a null sequence list; num_srcs > 32 (KVBM_ERR_UNSUPPORTED); then sequence by sequence
+ * the routing: a src_mask of 0, a bit at or above num_srcs, or a bit naming a source no window reads (KVBM_ERR_RANGE), two routed
+ * windows of one stage sharing a destination head (KVBM_ERR_OVERLAP), a destination layer of the range no routed window covers
+ * (KVBM_ERR_RANGE); then sequence by sequence every check of kvbm_manager_execute_stage_repage_gather with its code and text, the
+ * source id lists read and checked for routed sources only; last, the destination ids unique over the whole batch
+ * (KVBM_ERR_DUPLICATE_DST) and, where a source is the destination's layout, disjoint from the ids of the sequences routed to it
+ * (KVBM_ERR_OVERLAP).  Unrouted positions of the staged source tables hold block 0 and are never read.  bytes_moved counts the
+ * routed windows' bytes only.  With ls, layer_done_flags[l] is written once layer l of every sequence landed, and only the
+ * sources some sequence is routed to are waited on. */
+int kvbm_manager_execute_repage_batch_routed(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, kvbm_layout_handle dst,
+                                             const kvbm_repage_route_seq* seqs, size_t num_seqs, const kvbm_shard_window* windows,
+                                             size_t num_windows, const kvbm_layer_stream* ls, const kvbm_transfer_options* opts,
+                                             kvbm_notification* out);
+
 /* One prefill rank's KV to every decode rank that needs it, as ONE hand-off: the mirror image of
  * kvbm_manager_execute_stage_repage_gather.  For window w, heads [src_head_begin, +head_count) of source layers [src_layer_begin,
  * +layer_count) land as heads [dst_head_begin, +head_count) of layers [dst_layer_begin, +layer_count) of dsts[w.dst_rank], at every
