@@ -1307,9 +1307,10 @@ static size_t repage_blocks(size_t tb, size_t te, size_t page) { return tb == te
 // the options re-paging takes, named formats (the options override a layout's own; filled into *src_kv / *dst_kv), head counts
 // known and dividing inner_dim, check_compat's head row and cast dtypes, equal num_heads (unless `windows`: a gather's head
 // windows pick the heads, so the counts may differ) and dtypes, pages that divide and the walk's rules.  staged: a staged
-// re-paging gather's pair, whose layer counts may differ (check_compat's staged).
+// re-paging gather's pair, whose layer counts may differ (check_compat's staged).  anypage: kvbm_manager_execute_repage_anypage's
+// pair, whose pages need not divide but must keep the page split exact (KVBM_ERR_UNSUPPORTED).
 static int check_repage_pair(const Layout& S, const Layout& D, const kvbm_transfer_options& o, bool windows, int* src_kv, int* dst_kv,
-                             bool staged = false)
+                             bool staged = false, bool anypage = false)
 {
   if (S.unmapped || D.unmapped)
     return fail(KVBM_ERR_UNSUPPORTED, "a re-paging transfer needs both layouts addressable from this process (one is a descriptor of another process's host memory)");
@@ -1329,8 +1330,16 @@ static int check_repage_pair(const Layout& S, const Layout& D, const kvbm_transf
   const size_t ps = S.cfg.page_size, pd = D.cfg.page_size;
   if ((!windows && S.cfg.num_heads != D.cfg.num_heads) || (o.cast_mode == KVBM_CAST_NONE && S.cfg.dtype_width_bytes != D.cfg.dtype_width_bytes))
     return fail(KVBM_ERR_INCOMPATIBLE, "a re-paging transfer needs equal num_heads, head_dim and dtype on both sides");
-  if (ps % pd && pd % ps)
+  if (anypage) {
+    // include/kvbm_kernels.h's exactness bound, (big + small - gcd) * small < 2^32, as the unit helper applies it to an empty batch
+    size_t nu, ns, nd;
+    if (ps > UINT32_MAX || pd > UINT32_MAX ||
+        kvbm_kernels_repage_anypage_units(nullptr, 0, static_cast<uint32_t>(ps), static_cast<uint32_t>(pd), nullptr, 0, &nu, &ns, &nd))
+      return fail(KVBM_ERR_UNSUPPORTED, "page sizes src=" + std::to_string(ps) + ", dst=" + std::to_string(pd) +
+                                            " are past the re-paging walk's exactness bound (big + small - gcd) * small < 2^32");
+  } else if (ps % pd && pd % ps) {
     return fail(KVBM_ERR_INCOMPATIBLE, "re-paging needs one page size to divide the other: src=" + std::to_string(ps) + ", dst=" + std::to_string(pd));
+  }
   return check_walk(S, D, skv, dkv, o.cast_mode);
 }
 
@@ -1415,11 +1424,12 @@ struct RepageRequest {
 static bool reads_source(const uint32_t* mask, size_t r) { return !mask || (r < 32 && ((*mask >> r) & 1u)); }
 
 // Every check of a re-paging request after check_gather_windows, under the manager's lock, in the order above.  mask: a routed
-// sequence's sources, whose id lists alone are read and checked.
+// sequence's sources, whose id lists alone are read and checked.  anypage: check_repage_pair's.
 static int check_repage_request(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, const size_t* const* src_ids,
                                 size_t n_src, kvbm_layout_handle dst_h, const size_t* dst_ids, size_t n_dst, size_t tb, size_t te,
                                 const kvbm_head_window* windows, size_t nw, const kvbm_transfer_options& o, const kvbm_layer_stream* ls,
-                                bool gather, const kvbm_shard_window* layers, RepageRequest* R, const uint32_t* mask = nullptr)
+                                bool gather, const kvbm_shard_window* layers, RepageRequest* R, const uint32_t* mask = nullptr,
+                                bool anypage = false)
 {
   int rc;
   if (layers && (rc = check_stage_layers(m, srcs, dst_h, layers, nw, o))) return rc;
@@ -1433,7 +1443,8 @@ static int check_repage_request(kvbm_transfer_manager* m, size_t num_srcs, const
     if (!D && (rc = find_dst())) return rc;
     const kvbm_head_window& w = e[j].window = gather ? windows[j] : kvbm_head_window{0, 0, 0, S->cfg.num_heads};
     e[j].D[0] = D;
-    if ((rc = check_repage_pair(*S, *D, o, gather, &e[j].src_kv, &e[j].dst_kv, layers != nullptr)) || (rc = check_head_window(*S, *D, w, 1)))
+    if ((rc = check_repage_pair(*S, *D, o, gather, &e[j].src_kv, &e[j].dst_kv, layers != nullptr, anypage)) ||
+        (rc = check_head_window(*S, *D, w, 1)))
       return rc;
     if (S->cfg.page_size != e[0].S->cfg.page_size)
       return fail(KVBM_ERR_INCOMPATIBLE, "the sources of a re-paging gather need one page size: source " + std::to_string(e[0].window.src_rank) +
@@ -1465,10 +1476,11 @@ struct BatchTables {
 };
 
 // List k of sequence q is ids(q, k): q.n_src ids for k < num_src_lists, else q.n_dst.  check(t->cat), the caller's duplicate-id
-// checks, runs before the unit table.  *n_src / *n_dst: each concatenated source and destination table's length.
+// checks, runs before the unit table.  *n_src / *n_dst: each concatenated source and destination table's length.  anypage: the
+// unit table is kvbm_kernels_repage_anypage_units' (the same 16 B records, the phase in the fourth word).
 template <class Seq, class Ids, class Check>
 static int batch_tables(const Seq* seqs, size_t num_seqs, const std::vector<bool>& used, size_t num_src_lists, uint32_t ps, uint32_t pd,
-                        Ids ids, Check check, BatchTables* t, size_t* n_src, size_t* n_dst)
+                        Ids ids, Check check, BatchTables* t, size_t* n_src, size_t* n_dst, bool anypage = false)
 {
   t->cat.resize(used.size());
   for (size_t i = 0; i < num_seqs; ++i) {
@@ -1479,11 +1491,16 @@ static int batch_tables(const Seq* seqs, size_t num_seqs, const std::vector<bool
       if (used[k]) t->cat[k].insert(t->cat[k].end(), ids(q, k), ids(q, k) + (k < num_src_lists ? q.n_src : q.n_dst));
   }
   if (int rc = check(t->cat)) return rc;
+  static_assert(sizeof(kvbm_repage_anypage_unit) == sizeof(kvbm_repage_unit), "one staged record layout");
+  auto units = [&](kvbm_repage_unit* out, size_t cap, size_t* num_units) {
+    return anypage ? kvbm_kernels_repage_anypage_units(t->ranges.data(), t->ranges.size(), ps, pd, reinterpret_cast<kvbm_repage_anypage_unit*>(out),
+                                                       cap, num_units, n_src, n_dst)
+                   : kvbm_kernels_repage_batch_units(t->ranges.data(), t->ranges.size(), ps, pd, out, cap, num_units, n_src, n_dst);
+  };
   size_t num_units = 0;
-  if (kvbm_kernels_repage_batch_units(t->ranges.data(), t->ranges.size(), ps, pd, nullptr, 0, &num_units, n_src, n_dst))
-    return fail(KVBM_ERR, "the batch's token ranges and page sizes have no unit table");
+  if (units(nullptr, 0, &num_units)) return fail(KVBM_ERR, "the batch's token ranges and page sizes have no unit table");
   t->units.resize(num_units);
-  kvbm_kernels_repage_batch_units(t->ranges.data(), t->ranges.size(), ps, pd, t->units.data(), t->units.size(), &num_units, n_src, n_dst);
+  units(t->units.data(), t->units.size(), &num_units);
   for (size_t k = 0; k < used.size(); ++k) t->lists.push_back(used[k] ? t->cat[k].data() : nullptr);
   return KVBM_OK;
 }
@@ -1498,10 +1515,13 @@ static int batch_tables(const Seq* seqs, size_t num_seqs, const std::vector<bool
 // lists alone are checked, the destination's ids are checked against the ids of the sequences routed to a source in its
 // layout, unrouted positions of the staged tables are padded with block 0, and the unit table carries each sequence's window
 // mask for the routed kernel entries.
+// anypage: a batch whose pages need not divide (kvbm_manager_execute_repage_anypage): check_repage_pair's anypage rule, the unit
+// table of kvbm_kernels_repage_anypage_units, and the anypage kernel entries.
 static int execute_repage(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, kvbm_layout_handle dst_h,
                           const kvbm_repage_batch_seq* seqs, size_t num_seqs, const kvbm_head_window* windows, size_t nw,
                           const kvbm_transfer_options* opts_in, kvbm_notification* out, const kvbm_layer_stream* ls = nullptr,
-                          bool gather = true, const kvbm_shard_window* layers = nullptr, bool batch = false, const uint32_t* masks = nullptr)
+                          bool gather = true, const kvbm_shard_window* layers = nullptr, bool batch = false, const uint32_t* masks = nullptr,
+                          bool anypage = false)
 {
   kvbm_transfer_options o{};
   if (opts_in) o = *opts_in;
@@ -1554,7 +1574,7 @@ static int execute_repage(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_
     const kvbm_repage_batch_seq& q = seqs[i];
     const uint32_t* mask = masks ? masks + i : nullptr;
     if ((rc = check_repage_request(m, num_srcs, srcs, q.src_ids, q.n_src, dst_h, q.dst_ids, q.n_dst, q.token_begin, q.token_end, windows, nw, o,
-                                   ls, gather, layers, &R, mask)))
+                                   ls, gather, layers, &R, mask, anypage)))
       return rc;
     if (R.empty) continue;
     any = true;
@@ -1605,7 +1625,7 @@ static int execute_repage(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_
       }
       return KVBM_OK;
     };
-    if ((rc = batch_tables(seqs, num_seqs, used, num_srcs, ups, upd, ids, unique, &bt, &n_src, &n_dst))) return rc;
+    if ((rc = batch_tables(seqs, num_seqs, used, num_srcs, ups, upd, ids, unique, &bt, &n_src, &n_dst, anypage))) return rc;
     src_ids = bt.lists.data();
     dst_ids = bt.lists[num_srcs];
     if (masks) {  // each non-empty sequence's range with its window mask, which replaces the unit's sequence index
@@ -1633,6 +1653,17 @@ static int execute_repage(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_
     if (batch) {
       const auto* du = reinterpret_cast<const kvbm_repage_unit*>(sl.dev_ids + units_at(num_srcs * n_src + n_dst));
       const auto* dr = reinterpret_cast<const kvbm_route_unit*>(du);
+      const auto* da = reinterpret_cast<const kvbm_repage_anypage_unit*>(du);
+      if (anypage && st)
+        return checked(kvbm_kernels_paged_stage_repage_gather_anypage_streamed(ss, k, ups, &kd, dnh, upd, bt.ranges.data(), bt.ranges.size(), da,
+                                                                               bt.units.size(), ilb, ile, row, o.cast_mode, o.cast_scales, st,
+                                                                               stream),
+                       "kvbm_kernels_paged_stage_repage_gather_anypage_streamed");
+      if (anypage)
+        return checked(kvbm_kernels_paged_stage_repage_gather_anypage(ss, k, ups, &kd, dnh, upd, bt.ranges.data(), bt.ranges.size(), da,
+                                                                      bt.units.size(), ilb, ile, row, o.cast_mode, o.cast_scales, o.done_flag,
+                                                                      o.epoch, sl.host_flag, value, stream),
+                       "kvbm_kernels_paged_stage_repage_gather_anypage");
       if (masks && st)
         return checked(kvbm_kernels_paged_stage_repage_gather_routed_streamed(ss, k, ups, &kd, dnh, upd, routes.data(), routes.size(), dr,
                                                                               bt.units.size(), ilb, ile, row, o.cast_mode, o.cast_scales, st,
@@ -2682,6 +2713,19 @@ extern "C" int kvbm_manager_execute_repage_batch(kvbm_transfer_manager* m, size_
   kvbm_head_window hw[KVBM_GATHER_MAX_SOURCES];
   return execute_repage(m, num_srcs, srcs, dst, seqs, num_seqs, head_windows(windows, num_windows, hw), num_windows, opts, out, ls,
                         /*gather=*/true, windows, /*batch=*/true);
+  });
+}
+
+extern "C" int kvbm_manager_execute_repage_anypage(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs,
+                                                   kvbm_layout_handle dst, const kvbm_repage_batch_seq* seqs, size_t num_seqs,
+                                                   const kvbm_shard_window* windows, size_t num_windows, const kvbm_layer_stream* ls,
+                                                   const kvbm_transfer_options* opts, kvbm_notification* out)
+{
+  return guarded([&]() -> int {
+  if (int rc = stream_entry(m, ls, num_srcs, false, out)) return rc;
+  kvbm_head_window hw[KVBM_GATHER_MAX_SOURCES];
+  return execute_repage(m, num_srcs, srcs, dst, seqs, num_seqs, head_windows(windows, num_windows, hw), num_windows, opts, out, ls,
+                        /*gather=*/true, windows, /*batch=*/true, /*masks=*/nullptr, /*anypage=*/true);
   });
 }
 

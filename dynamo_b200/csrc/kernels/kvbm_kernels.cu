@@ -8,6 +8,7 @@
 #include <algorithm>
 #include <atomic>
 #include <mutex>
+#include <numeric>
 #include <type_traits>
 #include <cstdio>
 #include <vector>
@@ -748,6 +749,18 @@ __device__ __forceinline__ RepageUnit batch_unit(const kvbm_repage_unit* units, 
   return {w.x, w.y, w.z};
 }
 
+// A batch whose pages need not divide (kvbm_repage_anypage_unit): batch_unit's three words and the unit's phase, the slot of
+// small block small_k that holds the big block's slot 0, in the same 16 B load.
+struct RepageAnyUnit {
+  RepageUnit u;
+  uint32_t phase;
+};
+__device__ __forceinline__ RepageAnyUnit anypage_unit(const kvbm_repage_anypage_unit* units, uint32_t j)
+{
+  const uint4 w = __ldg(reinterpret_cast<const uint4*>(units) + j);
+  return {{w.x, w.y, w.z}, w.w};
+}
+
 // The unit of a one-CTA-per-unit re-paging kernel, blockIdx.x = (big block j * nlayers + l - layer_begin) * no + o.  The caller
 // takes o = rem % no itself: the gathers after their stage lookup, the scatters before it.  Moving it changes how ptxas
 // schedules the division.
@@ -763,18 +776,22 @@ __device__ __forceinline__ RepageCta repage_cta(const RepageGeom& G)
 }
 
 // Where 16 B vector vv of a re-paging head's run sits: its 16 B column c, its token's slot q in the big block, and the small
-// block (entry small_k + b of the small table) and slot that hold the same token.
+// block (entry small_k + b of the small table) and slot that hold the same token.  PHASE: pages that need not divide (DESIGN
+// §4.2k), where the big block's slot 0 sits at slot `phase` of small block small_k, so the small side splits phase + q; the big
+// side's address still takes q.  phase + q < big_page + small_page - gcd, which keeps the multiply-high exact under
+// repage_pages' bound.  Without PHASE the small side splits q itself.
 struct RepageAt {
   uint32_t c, q, b, slot;
 };
-template <bool POW2, bool PPOW2>
-__device__ __forceinline__ RepageAt repage_at(const RepageGeom& G, const RowSplit& r, uint32_t q0, uint32_t vv)
+template <bool POW2, bool PPOW2, bool PHASE = false>
+__device__ __forceinline__ RepageAt repage_at(const RepageGeom& G, const RowSplit& r, uint32_t q0, uint32_t vv, uint32_t phase = 0)
 {
   const uint32_t t = POW2 ? vv >> r.vpr : __umulhi(vv, r.magic);
   const uint32_t c = POW2 ? vv & ((1u << r.vpr) - 1) : vv - t * r.vpr;
   const uint32_t q = q0 + t;
-  const uint32_t b = PPOW2 ? q >> G.page.vpr : __umulhi(q, G.page.magic);
-  const uint32_t slot = PPOW2 ? q & (G.small_page - 1) : q - b * G.small_page;
+  const uint32_t qs = PHASE ? phase + q : q;
+  const uint32_t b = PPOW2 ? qs >> G.page.vpr : __umulhi(qs, G.page.magic);
+  const uint32_t slot = PPOW2 ? qs & (G.small_page - 1) : qs - b * G.small_page;
   return {c, q, b, slot};
 }
 
@@ -808,12 +825,13 @@ __device__ __forceinline__ void store_vector(const uint8_t* d, const uint4 (&y)[
 
 // One head of a re-paging unit: its run of `run` 16 B vectors from slot q0 of the big block on.  bh: the head's rows in the
 // big block; sh: its rows in the small side's (layer, outer) region, before the block offset.  Small block b of the unit is
-// entry small_k + b of small_ids (RepageUnit).  Every re-paging kernel but the scatter runs its heads through this loop.
-template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+// entry small_k + b of small_ids (RepageUnit).  Every re-paging kernel but the scatter runs its heads through this loop.  PHASE /
+// phase: repage_at's, the unit's phase when pages need not divide.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2, bool PHASE = false>
 __device__ __forceinline__ void repage_head_rows(const uint8_t* bh, uint32_t big_tok, uint32_t big_shift, const uint8_t* sh,
                                                  const int32_t* small_ids, uint32_t small_k, uint64_t small_block_stride,
                                                  uint32_t small_tok, uint32_t small_shift, const RepageGeom& G, uint32_t q0,
-                                                 uint32_t run, const RowSplit& r, const ptx::Scale& scale)
+                                                 uint32_t run, const RowSplit& r, const ptx::Scale& scale, uint32_t phase = 0)
 {
   constexpr int IN = CAST == KVBM_CAST_BF16_TO_FP8E4M3 ? 2 : 1;   // 16 B loads per vector
   constexpr int OUT = CAST == KVBM_CAST_FP8E4M3_TO_BF16 ? 2 : 1;  // 16 B stores per vector
@@ -825,7 +843,7 @@ __device__ __forceinline__ void repage_head_rows(const uint8_t* bh, uint32_t big
 #pragma unroll
     for (int k = 0; k < U; ++k)
       if (v + k * 32 < run) {
-        const RepageAt a = repage_at<POW2, PPOW2>(G, r, q0, v + k * 32);
+        const RepageAt a = repage_at<POW2, PPOW2, PHASE>(G, r, q0, v + k * 32, phase);
         const uint8_t* big_p = repage_big(bh, big_tok, big_shift, a);
         const uint8_t* small_p = repage_small(sh, small_ids, small_k, small_block_stride, small_tok, small_shift, a);
         const uint8_t* s = G.src_small ? small_p : big_p;
@@ -886,10 +904,12 @@ struct RepageGatherParams {
 // ROUTE: a routed batch, whose unit and source mask come from record j of `routes` in one 16 B load.  The warps walk only the
 // entries of the stage's sources in the mask, numbered densely (route_entry), so no warp idles on an unrouted window; heads[s]
 // is source s's entry count.  Only the stage's sources are consulted, so mask bits at or above the launch's sources never are.
-template <int CAST, bool POW2, bool SCALED, bool PPOW2, bool TABLE = false, bool ROUTE = false>
+// ANY: a batch whose pages need not divide, whose unit and phase come from record j of `any` (anypage_unit).
+template <int CAST, bool POW2, bool SCALED, bool PPOW2, bool TABLE = false, bool ROUTE = false, bool ANY = false>
 __device__ __forceinline__ void repage_gather_unit(const RepageGatherParams& P, const GatherStage& T, uint32_t j, uint32_t l, uint32_t o,
                                                    const RowSplit& r, const float* scales, const kvbm_repage_unit* units = nullptr,
-                                                   const kvbm_route_unit* routes = nullptr, const uint16_t* heads = nullptr)
+                                                   const kvbm_route_unit* routes = nullptr, const uint16_t* heads = nullptr,
+                                                   const kvbm_repage_anypage_unit* any = nullptr)
 {
   constexpr int IN = CAST == KVBM_CAST_BF16_TO_FP8E4M3 ? 2 : 1;
   constexpr int OUT = CAST == KVBM_CAST_FP8E4M3_TO_BF16 ? 2 : 1;
@@ -898,8 +918,12 @@ __device__ __forceinline__ void repage_gather_unit(const RepageGatherParams& P, 
   const uint32_t first = T.first, end = T.first + T.count;
   const PermuteSide& D = g.D;
   RepageUnit u;
-  uint32_t mask = 0;
-  if constexpr (ROUTE) {
+  uint32_t mask = 0, phase = 0;
+  if constexpr (ANY) {
+    const RepageAnyUnit a = anypage_unit(any, j);
+    u = a.u;
+    phase = a.phase;
+  } else if constexpr (ROUTE) {
     const uint4 w = __ldg(reinterpret_cast<const uint4*>(routes) + j);
     u = {w.x, w.y, w.z};
     mask = w.w;
@@ -922,8 +946,9 @@ __device__ __forceinline__ void repage_gather_unit(const RepageGatherParams& P, 
     const PermuteSide& B = ss ? D : S.S;
     const PermuteSide& Sm = ss ? S.S : D;
     const uint8_t* bh = (ss ? dh : sh) + static_cast<uint64_t>(__ldg(B.ids + j)) * B.block_stride;
-    repage_head_rows<CAST, POW2, SCALED, PPOW2>(bh, static_cast<uint32_t>(B.tok_stride), big_shift, ss ? sh : dh, Sm.ids, u.small_k,
-                                                Sm.block_stride, static_cast<uint32_t>(Sm.tok_stride), small_shift, G, u.q0, run, r, scale);
+    repage_head_rows<CAST, POW2, SCALED, PPOW2, ANY>(bh, static_cast<uint32_t>(B.tok_stride), big_shift, ss ? sh : dh, Sm.ids, u.small_k,
+                                                     Sm.block_stride, static_cast<uint32_t>(Sm.tok_stride), small_shift, G, u.q0, run, r,
+                                                     scale, phase);
   };
   if constexpr (ROUTE) {
     // routed entry i of the unit: the stage's map runs source by source in source order, so skip whole sources up to it
@@ -973,6 +998,18 @@ kvbm_paged_repage_fanin_kernel(const __grid_constant__ RepageGatherParams P, con
 {
   const auto [j, l, rem] = repage_cta(P.geo);
   repage_gather_unit<CAST, POW2, SCALED, PPOW2, true, true>(P, stage_of(P.g, l), j, l, rem % P.geo.no, r, scales, nullptr, routes, H.n);
+}
+
+// kvbm_paged_batch_repage_gather_kernel over a batch whose pages need not divide: record j of `units` also carries big block j's
+// phase (DESIGN §4.2k).  The same bound: three CTAs per SM.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__global__ void __launch_bounds__(256, 3)
+kvbm_paged_repage_anypage_kernel(const __grid_constant__ RepageGatherParams P, const kvbm_repage_anypage_unit* units, RowSplit r,
+                                 const float* scales)
+{
+  const auto [j, l, rem] = repage_cta(P.geo);
+  repage_gather_unit<CAST, POW2, SCALED, PPOW2, false, false, true>(P, stage_of(P.g, l), j, l, rem % P.geo.no, r, scales, nullptr, nullptr,
+                                                                    nullptr, units);
 }
 
 // The re-paging scatter, the gather's mirror image: ONE source pool of page Ps (a prefill rank) into up to
@@ -1286,6 +1323,17 @@ kvbm_gated_repage_fanin_kernel(const __grid_constant__ RepageGatherParams P, con
   });
 }
 
+// kvbm_gated_batch_repage_gather_kernel over a batch whose pages need not divide (num_big: the length of `units`).
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__global__ void __launch_bounds__(256)
+kvbm_gated_repage_anypage_kernel(const __grid_constant__ RepageGatherParams P, const __grid_constant__ GateArgs A,
+                                 const kvbm_repage_anypage_unit* units, uint32_t num_big, RowSplit r, const float* scales, uint32_t batch)
+{
+  gated_repage_units(A, P.g, P.geo, num_big, batch, [&](const GatherStage& T, uint32_t j, uint32_t l, uint32_t o) {
+    repage_gather_unit<CAST, POW2, SCALED, PPOW2, false, false, true>(P, T, j, l, o, r, scales, nullptr, nullptr, nullptr, units);
+  });
+}
+
 // The push kernels' hook in arrive_transfer: the num_flags target done flags of F, with A.ss's own and before the completion word.
 __device__ __forceinline__ auto target_done(const ScatterFlags& F, const int& num_flags, const GateArgs& A)
 {
@@ -1544,6 +1592,10 @@ static cudaError_t preload_kernels()
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_fanin_kernel<c, p, sc, false>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_fanin_kernel<c, p, sc, true>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_fanin_kernel<c, p, sc, false>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_anypage_kernel<c, p, sc, true>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_anypage_kernel<c, p, sc, false>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_anypage_kernel<c, p, sc, true>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_anypage_kernel<c, p, sc, false>);
         });
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_layer_signal_kernel);
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_scatter_signal_kernel);
@@ -1917,17 +1969,28 @@ static cudaError_t launch_paged_permute(const kvbm_stage_source* srcs, int num_s
   return launched(stream, done_flag, epoch, completion_flag, completion_value);
 }
 
-// What every re-paging launch derives from its two pages, and their checks: non-zero pages, one dividing the other, the page
-// split exact for q < big_page, the cast's rows and the row split of the larger page.  Fills everything of *G but the token
-// range's fields and nh, the walk's row split, the destination's row and whether the small page is a power of two.
+// The page split's exactness bound (big_page + small_page - gcd) * small_page < 2^32.  The small side splits phase + q with
+// q < big_page and phase a multiple of the gcd below small_page (0 when the pages divide), so phase + q < big + small - gcd.  The
+// multiply-high with m = ceil(2^32 / small) = (2^32 + e) / small, e < small, is exact for every x with x * e < 2^32, which the
+// bound gives.  When small_page divides big_page it reads big_page * small_page < 2^32.  A small page of 2^16 or more fails it
+// (the factor big + small - gcd is at least big >= small), which keeps the 64-bit product from wrapping.
+static bool repage_exact(uint64_t big_page, uint64_t small_page)
+{
+  return small_page < (1u << 16) && (big_page + small_page - std::gcd(big_page, small_page)) * small_page < (1ull << 32);
+}
+
+// What every re-paging launch derives from its two pages, and their checks: non-zero pages, one dividing the other unless
+// `any` (kvbm_kernels_paged_stage_repage_gather_anypage), repage_exact, the cast's rows and the row split of the larger page.
+// Fills everything of *G but the token range's fields and nh, the walk's row split, the destination's row and whether the small
+// page is a power of two.
 static bool repage_pages(uint32_t src_page, uint32_t dst_page, int layer_begin, int layer_end, uint32_t no, uint32_t src_row_bytes,
-                         int cast_mode, RepageGeom* G, RowSplit* r, uint64_t* dst_row_bytes, bool* page_pow2)
+                         int cast_mode, RepageGeom* G, RowSplit* r, uint64_t* dst_row_bytes, bool* page_pow2, bool any = false)
 {
   if (src_page == 0 || dst_page == 0) return false;
   const bool src_small = src_page < dst_page;
   const uint32_t big_page = src_small ? dst_page : src_page, small_page = src_small ? src_page : dst_page;
-  if (big_page % small_page) return false;
-  if (static_cast<uint64_t>(big_page) * small_page >= (1ull << 32)) return false;
+  if (!any && big_page % small_page) return false;
+  if (!repage_exact(big_page, small_page)) return false;
   uint64_t walk_row;
   if (!cast_rows(src_row_bytes, cast_mode, dst_row_bytes, &walk_row) || !row_split(walk_row, big_page, r)) return false;
   RepageGeom g{};
@@ -1952,7 +2015,7 @@ static bool repage_pages(uint32_t src_page, uint32_t dst_page, int layer_begin, 
 
 // A batch of sequences of a re-paging launch: the caller's ranges (host) and unit table (device-accessible).  route: a routed
 // batch, whose ranges and masks (a scatter's targets, a gather's sources) are route_seqs and whose unit table is route_units
-// (seqs and units unused).
+// (seqs and units unused).  any_units: a batch whose pages need not divide, whose unit table is this one (units unused).
 struct RepageBatch {
   const kvbm_repage_seq* seqs;
   size_t num_seqs;
@@ -1961,6 +2024,8 @@ struct RepageBatch {
   bool route = false;
   const kvbm_route_seq* route_seqs = nullptr;
   const kvbm_route_unit* route_units = nullptr;
+  bool any = false;
+  const kvbm_repage_anypage_unit* any_units = nullptr;
 };
 
 // What repage_launch derives: repage_pages' results with the token range's fields, the units to launch (0: nothing to move), the
@@ -1974,7 +2039,8 @@ struct RepageLaunch {
 };
 
 // Every re-paging launch's first checks, before any CUDA call: ranges not reversed, cast_args_ok, and B checked by
-// kvbm_kernels_repage_batch_units (a routed batch: kvbm_kernels_repage_route_units) with the caller's unit count.  An empty range
+// kvbm_kernels_repage_batch_units (a routed batch: kvbm_kernels_repage_route_units; one whose pages need not divide:
+// kvbm_kernels_repage_anypage_units, and repage_pages without the divisibility rule) with the caller's unit count.  An empty range
 // or batch then leaves L->units 0 (the caller
 // signals).  Else `side` (a gather's destination, the scatter's source) needs a table, a base, a non-zero outer dim and the layer
 // range; the pages repage_pages' rules; a single range slots in 32 bits (its last block of the larger page ends below 2^32); the
@@ -1989,9 +2055,10 @@ static bool repage_launch(const kvbm_permute_side* side, uint32_t src_page, uint
   if (B) {
     size_t src_ids, dst_ids;
     if ((B->route ? kvbm_kernels_repage_route_units(B->route_seqs, B->num_seqs, src_page, dst_page, nullptr, 0, &num_big, &src_ids, &dst_ids)
+         : B->any ? kvbm_kernels_repage_anypage_units(B->seqs, B->num_seqs, src_page, dst_page, nullptr, 0, &num_big, &src_ids, &dst_ids)
                   : kvbm_kernels_repage_batch_units(B->seqs, B->num_seqs, src_page, dst_page, nullptr, 0, &num_big, &src_ids, &dst_ids)) != 0)
       return false;
-    const void* table = B->route ? static_cast<const void*>(B->route_units) : B->units;
+    const void* table = B->route ? static_cast<const void*>(B->route_units) : B->any ? static_cast<const void*>(B->any_units) : B->units;
     if (num_big != B->num_units || (num_big != 0 && !table)) return false;
   }
   L->units = 0;
@@ -2000,7 +2067,8 @@ static bool repage_launch(const kvbm_permute_side* side, uint32_t src_page, uint
   const uint32_t nl = L->nl = side->layout.num_layers, no = L->no = side->layout.outer_dim;
   if (nl == 0 || no == 0 || static_cast<uint32_t>(layer_end) > nl) return false;
   RepageGeom& g = L->geo;
-  if (!repage_pages(src_page, dst_page, layer_begin, layer_end, no, src_row_bytes, cast_mode, &g, &L->r, &L->dst_row_bytes, &L->page_pow2))
+  if (!repage_pages(src_page, dst_page, layer_begin, layer_end, no, src_row_bytes, cast_mode, &g, &L->r, &L->dst_row_bytes, &L->page_pow2,
+                    B && B->any))
     return false;
   if (!B) {
     const uint64_t big_end = (static_cast<uint64_t>(token_end) + g.big_page - 1) / g.big_page * g.big_page;
@@ -2026,7 +2094,8 @@ static bool repage_launch(const kvbm_permute_side* side, uint32_t src_page, uint
 // takes the batch gather kernels, or the fan-in kernels for a routed batch: bit s of a sequence's mask names srcs[s], every mask
 // must be non-zero and below bit num_srcs, and two windows of a stage may then share destination heads unless one mask holds both.
 // Each stage's sources are ANDed with the union of the masks, so both gate forms wait on routed sources only, and a CTA has as
-// many warps as the most routed entries of one stage under one mask (up to 8).
+// many warps as the most routed entries of one stage under one mask (up to 8).  A batch whose pages need not divide (B->any)
+// takes the anypage kernels.
 static cudaError_t launch_paged_repage_gather(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page, const kvbm_permute_side* dst,
                                               uint32_t dst_num_heads, uint32_t dst_page, uint32_t token_begin, uint32_t token_end,
                                               int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
@@ -2087,6 +2156,8 @@ static cudaError_t launch_paged_repage_gather(const kvbm_stage_source* srcs, int
           with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, L.page_pow2, [&](auto c, auto p, auto sc, auto pp) {
             if (route)
               kvbm_gated_repage_fanin_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, A, H, B->route_units, L.num_big, r, cast_scales, batch);
+            else if (B && B->any)
+              kvbm_gated_repage_anypage_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, A, B->any_units, L.num_big, r, cast_scales, batch);
             else if (B)
               kvbm_gated_batch_repage_gather_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, A, B->units, L.num_big, r, cast_scales, batch);
             else
@@ -2103,6 +2174,8 @@ static cudaError_t launch_paged_repage_gather(const kvbm_stage_source* srcs, int
   with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, L.page_pow2, [&](auto c, auto p, auto sc, auto pp) {
     if (route)
       kvbm_paged_repage_fanin_kernel<c, p, sc, pp><<<grid, threads, 0, stream>>>(P, H, B->route_units, r, cast_scales);
+    else if (B && B->any)
+      kvbm_paged_repage_anypage_kernel<c, p, sc, pp><<<grid, threads, 0, stream>>>(P, B->any_units, r, cast_scales);
     else if (B)
       kvbm_paged_batch_repage_gather_kernel<c, p, sc, pp><<<grid, threads, 0, stream>>>(P, B->units, r, cast_scales);
     else if (plain)
@@ -2539,21 +2612,21 @@ kvbm_kernels_paged_stage_repage_gather_streamed(const kvbm_stage_source* srcs, i
                                     st->completion_value, KVBM_GATHER_MAX_HEADS, stream, st);
 }
 
-// kvbm_kernels_repage_batch_units over ranges of either sequence type; the fourth word of each unit is last(i) of its sequence i.
+// kvbm_kernels_repage_batch_units over ranges of either sequence type; the fourth word of each unit is last(i, phase) of its
+// sequence i and the block's phase (0 unless `any`).  any: pages that need not divide (kvbm_kernels_repage_anypage_units).
 template <class Seq, class Unit, class Last>
 static int batch_units(const Seq* seqs, size_t num_seqs, uint32_t src_page_size, uint32_t dst_page_size, Unit* out, size_t cap,
-                       size_t* num_units, size_t* src_ids, size_t* dst_ids, Last last)
+                       size_t* num_units, size_t* src_ids, size_t* dst_ids, Last last, bool any = false)
 {
   if ((num_seqs && !seqs) || (cap && !out) || !num_units || !src_ids || !dst_ids) return 1;
   if (src_page_size == 0 || dst_page_size == 0) return 1;
   const bool src_small = src_page_size < dst_page_size;
   const uint64_t big = src_small ? dst_page_size : src_page_size, small = src_small ? src_page_size : dst_page_size;
-  if (big % small || big * small >= (1ull << 32)) return 1;
+  if ((!any && big % small) || !repage_exact(big, small)) return 1;
   for (size_t i = 0; i < num_seqs; ++i) {
     if (seqs[i].token_end < seqs[i].token_begin) return 1;
     if (seqs[i].token_end != seqs[i].token_begin && (seqs[i].token_end + big - 1) / big * big >= (1ull << 32)) return 1;
   }
-  const uint64_t ratio = big / small;
   size_t nb = 0, ns = 0;
   for (size_t i = 0; i < num_seqs; ++i) {
     const uint64_t tb = seqs[i].token_begin, te = seqs[i].token_end;
@@ -2562,9 +2635,10 @@ static int batch_units(const Seq* seqs, size_t num_seqs, uint32_t src_page_size,
     uint64_t j = big_first;
     for (; j < big_end && nb < cap; ++j, ++nb) {
       const uint64_t first = j * big, t0 = std::max(tb, first), t1 = std::min(te, first + big);
-      // the concatenated small table's entry of the block's first small block: below 0 (wrapping) when it lies before the range
-      out[nb] = Unit{static_cast<uint32_t>(t0 - first), static_cast<uint32_t>(t1 - t0), static_cast<uint32_t>(ns + j * ratio - small_first),
-                     last(i)};
+      // the concatenated small table's entry of the small block that holds the block's slot 0 (j * ratio with dividing pages): below
+      // 0 (wrapping) when it lies before the range; the phase is that slot 0's slot in it
+      out[nb] = Unit{static_cast<uint32_t>(t0 - first), static_cast<uint32_t>(t1 - t0), static_cast<uint32_t>(ns + first / small - small_first),
+                     last(i, static_cast<uint32_t>(first % small))};
     }
     nb += static_cast<size_t>(big_end - j);  // past the capacity: counted, not written
     ns += static_cast<size_t>(small_end - small_first);
@@ -2580,7 +2654,7 @@ kvbm_kernels_repage_batch_units(const kvbm_repage_seq* seqs, size_t num_seqs, ui
                                 kvbm_repage_unit* out, size_t cap, size_t* num_units, size_t* src_ids, size_t* dst_ids)
 {
   return batch_units(seqs, num_seqs, src_page_size, dst_page_size, out, cap, num_units, src_ids, dst_ids,
-                     [](size_t i) { return static_cast<uint32_t>(i); });
+                     [](size_t i, uint32_t) { return static_cast<uint32_t>(i); });
 }
 
 extern "C" int
@@ -2588,7 +2662,43 @@ kvbm_kernels_repage_route_units(const kvbm_route_seq* seqs, size_t num_seqs, uin
                                 kvbm_route_unit* out, size_t cap, size_t* num_units, size_t* src_ids, size_t* dst_ids)
 {
   return batch_units(seqs, num_seqs, src_page_size, dst_page_size, out, cap, num_units, src_ids, dst_ids,
-                     [seqs](size_t i) { return seqs[i].targets; });
+                     [seqs](size_t i, uint32_t) { return seqs[i].targets; });
+}
+
+extern "C" int
+kvbm_kernels_repage_anypage_units(const kvbm_repage_seq* seqs, size_t num_seqs, uint32_t src_page_size, uint32_t dst_page_size,
+                                  kvbm_repage_anypage_unit* out, size_t cap, size_t* num_units, size_t* src_ids, size_t* dst_ids)
+{
+  return batch_units(seqs, num_seqs, src_page_size, dst_page_size, out, cap, num_units, src_ids, dst_ids,
+                     [](size_t, uint32_t phase) { return phase; }, /*any=*/true);
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_stage_repage_gather_anypage(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page_size, const kvbm_permute_side* dst,
+                                               uint32_t dst_num_heads, uint32_t dst_page_size, const kvbm_repage_seq* seqs, size_t num_seqs,
+                                               const kvbm_repage_anypage_unit* units, size_t num_units, int layer_begin, int layer_end,
+                                               uint32_t src_row_bytes, int cast_mode, const float* cast_scales, uint32_t* done_flag,
+                                               uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
+{
+  const RepageBatch B{seqs, num_seqs, nullptr, num_units, false, nullptr, nullptr, true, units};
+  return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, 0, 0, layer_begin, layer_end,
+                                    src_row_bytes, cast_mode, cast_scales, done_flag, epoch, completion_flag, completion_value,
+                                    KVBM_GATHER_MAX_HEADS, stream, nullptr, &B);
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_stage_repage_gather_anypage_streamed(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page_size,
+                                                        const kvbm_permute_side* dst, uint32_t dst_num_heads, uint32_t dst_page_size,
+                                                        const kvbm_repage_seq* seqs, size_t num_seqs, const kvbm_repage_anypage_unit* units,
+                                                        size_t num_units, int layer_begin, int layer_end, uint32_t src_row_bytes,
+                                                        int cast_mode, const float* cast_scales, const kvbm_permute_stream* st,
+                                                        cudaStream_t stream)
+{
+  if (!stream_args_ok(st, num_srcs)) return cudaErrorInvalidValue;
+  const RepageBatch B{seqs, num_seqs, nullptr, num_units, false, nullptr, nullptr, true, units};
+  return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, 0, 0, layer_begin, layer_end,
+                                    src_row_bytes, cast_mode, cast_scales, st->done_flag, st->epoch, st->completion_flag,
+                                    st->completion_value, KVBM_GATHER_MAX_HEADS, stream, st, &B);
 }
 
 extern "C" cudaError_t

@@ -130,6 +130,11 @@ class RouteUnit(C.Structure):
     _fields_ = [("q0", C.c_uint32), ("tokens", C.c_uint32), ("small_k", C.c_uint32), ("targets", C.c_uint32)]
 
 
+class RepageAnypageUnit(C.Structure):
+    """struct kvbm_repage_anypage_unit: RepageUnit with the block's phase in place of seq, 16 B (`repage_anypage_units` writes them)"""
+    _fields_ = [("q0", C.c_uint32), ("tokens", C.c_uint32), ("small_k", C.c_uint32), ("phase", C.c_uint32)]
+
+
 class ScatterTarget(C.Structure):
     """struct kvbm_scatter_target: one target of `paged_repage_scatter` (a destination side, its head count, one head window, one
     layer window and its nullable done flag)"""
@@ -291,6 +296,12 @@ def lib() -> C.CDLL:
         L.kvbm_kernels_paged_stage_repage_gather_routed.restype = i
         L.kvbm_kernels_paged_stage_repage_gather_routed_streamed.argtypes = L.kvbm_kernels_paged_stage_repage_gather_batch_streamed.argtypes
         L.kvbm_kernels_paged_stage_repage_gather_routed_streamed.restype = i
+        L.kvbm_kernels_repage_anypage_units.argtypes = L.kvbm_kernels_repage_batch_units.argtypes
+        L.kvbm_kernels_repage_anypage_units.restype = i
+        L.kvbm_kernels_paged_stage_repage_gather_anypage.argtypes = L.kvbm_kernels_paged_stage_repage_gather_batch.argtypes
+        L.kvbm_kernels_paged_stage_repage_gather_anypage.restype = i
+        L.kvbm_kernels_paged_stage_repage_gather_anypage_streamed.argtypes = L.kvbm_kernels_paged_stage_repage_gather_batch_streamed.argtypes
+        L.kvbm_kernels_paged_stage_repage_gather_anypage_streamed.restype = i
         L.kvbm_kernels_permute_strides.argtypes = [i, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64, C.c_uint64,
                                                    C.POINTER(C.c_uint64)]
         L.kvbm_kernels_permute_strides.restype = i
@@ -322,7 +333,8 @@ EXPORTED_SYMBOLS = [
     "kvbm_kernels_paged_repage_scatter_streamed", "kvbm_kernels_paged_repage_scatter_batch",
     "kvbm_kernels_paged_repage_scatter_batch_streamed", "kvbm_kernels_repage_route_units", "kvbm_kernels_paged_repage_scatter_routed",
     "kvbm_kernels_paged_repage_scatter_routed_streamed", "kvbm_kernels_paged_stage_repage_gather_routed",
-    "kvbm_kernels_paged_stage_repage_gather_routed_streamed",
+    "kvbm_kernels_paged_stage_repage_gather_routed_streamed", "kvbm_kernels_repage_anypage_units",
+    "kvbm_kernels_paged_stage_repage_gather_anypage", "kvbm_kernels_paged_stage_repage_gather_anypage_streamed",
 ]
 
 
@@ -553,20 +565,23 @@ def _repage_seqs(seqs: Sequence[Tuple[int, int]]):
     return (RepageSeq * max(1, len(seqs)))(*[RepageSeq(int(b), int(e)) for b, e in seqs])
 
 
+def _unit_table(call, arr, num_seqs: int, src_page_size: int, dst_page_size: int):
+    """A unit helper's sizing call, then its table as a numpy uint32 array [num_units, 4] with the two table lengths, or None."""
+    import numpy as np
+    n, ns, nd = C.c_size_t(), C.c_size_t(), C.c_size_t()
+    if call(C.cast(arr, C.c_void_p), num_seqs, src_page_size, dst_page_size, None, 0, C.byref(n), C.byref(ns), C.byref(nd)):
+        return None
+    out = np.zeros((n.value, 4), dtype=np.uint32)
+    if call(C.cast(arr, C.c_void_p), num_seqs, src_page_size, dst_page_size, out.ctypes.data, n.value, C.byref(n), C.byref(ns), C.byref(nd)):
+        return None
+    return out, ns.value, nd.value
+
+
 def repage_batch_units(seqs: Sequence[Tuple[int, int]], src_page_size: int, dst_page_size: int):
     """Host-only: the unit table of a batch of (token_begin, token_end) ranges as a numpy uint32 array [num_units, 4] (q0, tokens,
     small_k, seq) and the lengths of each source's and the destination's concatenated block table; None when the pages or a range
     break a rule.  include/kvbm_kernels.h (kvbm_kernels_repage_batch_units)."""
-    import numpy as np
-    arr = _repage_seqs(seqs)
-    n, ns, nd = C.c_size_t(), C.c_size_t(), C.c_size_t()
-    call = lib().kvbm_kernels_repage_batch_units
-    if call(C.cast(arr, C.c_void_p), len(seqs), src_page_size, dst_page_size, None, 0, C.byref(n), C.byref(ns), C.byref(nd)):
-        return None
-    out = np.zeros((n.value, 4), dtype=np.uint32)
-    if call(C.cast(arr, C.c_void_p), len(seqs), src_page_size, dst_page_size, out.ctypes.data, n.value, C.byref(n), C.byref(ns), C.byref(nd)):
-        return None
-    return out, ns.value, nd.value
+    return _unit_table(lib().kvbm_kernels_repage_batch_units, _repage_seqs(seqs), len(seqs), src_page_size, dst_page_size)
 
 
 def paged_stage_repage_gather_batch(srcs: Sequence[StageSource], src_page_size: int, dst: PermuteSide, dst_num_heads: int,
@@ -597,6 +612,43 @@ def paged_stage_repage_gather_batch_streamed(srcs: Sequence[StageSource], src_pa
                                                                        units or None, num_units, layer_begin, layer_end, src_row_bytes,
                                                                        int(cast_mode), scales_ptr(cast_scales),
                                                                        C.byref(st) if st is not None else None, stream)
+
+
+def repage_anypage_units(seqs: Sequence[Tuple[int, int]], src_page_size: int, dst_page_size: int):
+    """Host-only: `repage_batch_units` for any two non-zero pages, each record's fourth word its big block's phase (the slot of
+    small block small_k that holds the big block's slot 0): a numpy uint32 array [num_units, 4] (q0, tokens, small_k, phase) and
+    the two table lengths, or None when the pages pass the exactness bound or a range breaks a rule.
+    include/kvbm_kernels.h (kvbm_kernels_repage_anypage_units)."""
+    return _unit_table(lib().kvbm_kernels_repage_anypage_units, _repage_seqs(seqs), len(seqs), src_page_size, dst_page_size)
+
+
+def paged_stage_repage_gather_anypage(srcs: Sequence[StageSource], src_page_size: int, dst: PermuteSide, dst_num_heads: int,
+                                      dst_page_size: int, seqs: Sequence[Tuple[int, int]], units: int, num_units: int, layer_begin: int,
+                                      layer_end: int, src_row_bytes: int, cast_mode: int = 0, cast_scales=None, done_flag: int = 0,
+                                      epoch: int = 0, completion_flag: int = 0, completion_value: int = 0, stream: int = 0) -> int:
+    """`paged_stage_repage_gather_batch` for any two non-zero pages, dividing or not: `units` is the device address of the table
+    `repage_anypage_units` made for the same ranges and pages.  With dividing pages it writes the batch's bytes.
+    include/kvbm_kernels.h (kvbm_kernels_paged_stage_repage_gather_anypage)."""
+    arr = (StageSource * max(1, len(srcs)))(*srcs)
+    return lib().kvbm_kernels_paged_stage_repage_gather_anypage(arr, len(srcs), src_page_size, C.byref(dst), dst_num_heads, dst_page_size,
+                                                                C.cast(_repage_seqs(seqs), C.c_void_p), len(seqs), units or None, num_units,
+                                                                layer_begin, layer_end, src_row_bytes, int(cast_mode),
+                                                                scales_ptr(cast_scales), done_flag or None, epoch, completion_flag or None,
+                                                                completion_value, stream)
+
+
+def paged_stage_repage_gather_anypage_streamed(srcs: Sequence[StageSource], src_page_size: int, dst: PermuteSide, dst_num_heads: int,
+                                               dst_page_size: int, seqs: Sequence[Tuple[int, int]], units: int, num_units: int,
+                                               layer_begin: int, layer_end: int, src_row_bytes: int, cast_mode: int, cast_scales,
+                                               st: Optional[PermuteStream], stream: int = 0) -> int:
+    """`paged_stage_repage_gather_anypage` streamed with `paged_stage_repage_gather_batch_streamed`'s flags and gate forms.
+    include/kvbm_kernels.h (kvbm_kernels_paged_stage_repage_gather_anypage_streamed)."""
+    arr = (StageSource * max(1, len(srcs)))(*srcs)
+    return lib().kvbm_kernels_paged_stage_repage_gather_anypage_streamed(arr, len(srcs), src_page_size, C.byref(dst), dst_num_heads,
+                                                                         dst_page_size, C.cast(_repage_seqs(seqs), C.c_void_p), len(seqs),
+                                                                         units or None, num_units, layer_begin, layer_end, src_row_bytes,
+                                                                         int(cast_mode), scales_ptr(cast_scales),
+                                                                         C.byref(st) if st is not None else None, stream)
 
 
 def paged_repage_scatter(src: PermuteSide, src_num_heads: int, src_page_size: int, targets: Sequence[ScatterTarget], dst_page_size: int,
@@ -663,16 +715,7 @@ def repage_route_units(seqs: Sequence[Tuple[int, int, int]], src_page_size: int,
     """Host-only: `repage_batch_units` over the (token_begin, token_end, targets) of a routed batch, each record's fourth word its
     sequence's targets: a numpy uint32 array [num_units, 4] (q0, tokens, small_k, targets) and the two table lengths, or None.
     include/kvbm_kernels.h (kvbm_kernels_repage_route_units)."""
-    import numpy as np
-    arr = _route_seqs(seqs)
-    n, ns, nd = C.c_size_t(), C.c_size_t(), C.c_size_t()
-    call = lib().kvbm_kernels_repage_route_units
-    if call(C.cast(arr, C.c_void_p), len(seqs), src_page_size, dst_page_size, None, 0, C.byref(n), C.byref(ns), C.byref(nd)):
-        return None
-    out = np.zeros((n.value, 4), dtype=np.uint32)
-    if call(C.cast(arr, C.c_void_p), len(seqs), src_page_size, dst_page_size, out.ctypes.data, n.value, C.byref(n), C.byref(ns), C.byref(nd)):
-        return None
-    return out, ns.value, nd.value
+    return _unit_table(lib().kvbm_kernels_repage_route_units, _route_seqs(seqs), len(seqs), src_page_size, dst_page_size)
 
 
 def paged_repage_scatter_routed(src: PermuteSide, src_num_heads: int, src_page_size: int, targets: Sequence[ScatterTarget],

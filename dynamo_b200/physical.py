@@ -274,7 +274,7 @@ EXPORTED_SYMBOLS = [
     "kvbm_tp_pp_reshard_plan", "kvbm_manager_execute_stage_gather", "kvbm_manager_execute_stage_repage_gather",
     "kvbm_manager_execute_repage_batch", "kvbm_tp_pp_scatter_plan", "kvbm_manager_execute_repage_scatter",
     "kvbm_manager_execute_repage_scatter_streamed", "kvbm_manager_execute_repage_scatter_batch",
-    "kvbm_manager_execute_repage_scatter_routed", "kvbm_manager_execute_repage_batch_routed",
+    "kvbm_manager_execute_repage_scatter_routed", "kvbm_manager_execute_repage_batch_routed", "kvbm_manager_execute_repage_anypage",
 ]
 
 
@@ -337,6 +337,7 @@ def lib() -> C.CDLL:
                                                                P(_CLayerStream), P(_COptions), P(u64)]
         L.kvbm_manager_execute_repage_batch.argtypes = [vp, sz, P(u64), u64, P(_CRepageBatchSeq), sz, P(_CShardWindow), sz, P(_CLayerStream),
                                                         P(_COptions), P(u64)]
+        L.kvbm_manager_execute_repage_anypage.argtypes = L.kvbm_manager_execute_repage_batch.argtypes
         L.kvbm_manager_execute_repage_batch_routed.argtypes = [vp, sz, P(u64), u64, P(_CRepageRouteSeq), sz, P(_CShardWindow), sz,
                                                                P(_CLayerStream), P(_COptions), P(u64)]
         L.kvbm_tp_pp_scatter_plan.argtypes = [sz, sz, sz, sz, P(sz), sz, sz, P(sz), sz, P(_CScatterWindow), sz, P(sz)]
@@ -922,6 +923,21 @@ class TransferManager:
         `ready_flags`, `layer_done_flags[l]` is written once layer l of every sequence landed.  Two sequences may share source
         blocks; a destination block may appear once in the whole batch.  The first rejected sequence raises what
         `execute_stage_repage_gather` would raise for it."""
+        return self._repage_batch(lib().kvbm_manager_execute_repage_batch, sources, dst, seqs, plan, options, ready_flags, layer_done_flags,
+                                  num_layers)
+
+    def execute_repage_anypage(self, sources: Mapping[int, int], dst: int, seqs: Sequence[tuple], plan: Sequence,
+                               options: Optional[TransferOptions] = None, ready_flags: Optional[Mapping[int, int]] = None,
+                               layer_done_flags: int = 0, num_layers: Optional[int] = None) -> TransferCompleteNotification:
+        """`execute_repage_batch` between engines whose page sizes need not divide each other (kvbm_manager_execute_repage_anypage),
+        e.g. a hybrid model's 544-token attention block into 64-token decode pages, or 24 into 16: the same arguments, plan forms,
+        errors and streaming.  Pages past the exactness bound (big + small - gcd) * small < 2^32 raise UNSUPPORTED.  With
+        dividing pages the destination bytes are `execute_repage_batch`'s."""
+        return self._repage_batch(lib().kvbm_manager_execute_repage_anypage, sources, dst, seqs, plan, options, ready_flags,
+                                  layer_done_flags, num_layers)
+
+    def _repage_batch(self, entry, sources, dst, seqs, plan, options, ready_flags, layer_done_flags, num_layers):
+        """The body of `execute_repage_batch` and `execute_repage_anypage`: `entry` is the C entry they call."""
         if plan and isinstance(plan[0], HeadWindow):
             if num_layers is None:
                 raise ValueError("a HeadWindow plan needs num_layers, the destination's layer count")
@@ -946,8 +962,8 @@ class TransferManager:
         ls = self._layer_stream(ranks, ready_flags, layer_done_flags) if ready_flags is not None else None
         tok = C.c_uint64()
         o = (options or TransferOptions())._c()
-        _check(lib().kvbm_manager_execute_repage_batch(self._h, len(ranks), hs, dst, cs, len(seqs), ws, len(plan),
-                                                       C.byref(ls) if ls is not None else None, C.byref(o), C.byref(tok)))
+        _check(entry(self._h, len(ranks), hs, dst, cs, len(seqs), ws, len(plan), C.byref(ls) if ls is not None else None, C.byref(o),
+                     C.byref(tok)))
         return TransferCompleteNotification(self, tok.value)
 
     def execute_repage_batch_routed(self, sources: Mapping[int, int], dst: int, seqs: Sequence[tuple], plan: Sequence[ShardWindow],

@@ -691,6 +691,58 @@ cudaError_t kvbm_kernels_paged_stage_repage_gather_routed_streamed(const kvbm_st
                                                                    const float* cast_scales, const kvbm_permute_stream* st,
                                                                    cudaStream_t stream);
 
+/* ---- re-paging between pages that need not divide: a batch gather for any two page sizes -------------------------------------
+ * Engines configured independently keep pages that neither divide: a hybrid model's attention block of 544 tokens against a
+ * decode engine's 64, or 24 against 16.  Every entry above rejects such a pair; the two below take any two non-zero pages.
+ * The unit stays one block of the larger-page side.  Its block's slot 0 is sequence position F = j * big_page; the smaller-page
+ * side's block that holds F is entry small_k of its concatenated table, and F sits at slot `phase` = F % small_page of it.  The
+ * token at big slot q then sits at offset phase + q from the start of that small block: in block small_k + (phase + q) /
+ * small_page, slot (phase + q) % small_page.  With dividing pages every phase is 0.
+ * Exactness bound: (big_page + small_page - gcd(big_page, small_page)) * small_page < 2^32.  phase + q stays below
+ * big_page + small_page - gcd, and the kernels' multiply-high split by small_page is exact for it under this bound; with dividing
+ * pages it is the other entries' big_page * small_page < 2^32.  As there, every sequence's last block of the larger page ends
+ * below 2^32 tokens. */
+
+/* kvbm_repage_unit with the block's phase in place of seq: a CTA loads its unit and its phase in one 16 B load.  q0, tokens and
+ * small_k are kvbm_repage_unit's, small_k being the entry that holds the big block's slot 0 (wrapping below 0 as there); phase:
+ * that slot 0's slot in small block small_k, below small_page. */
+typedef struct kvbm_repage_anypage_unit {
+  uint32_t q0, tokens, small_k, phase;
+} kvbm_repage_anypage_unit;
+
+/* Host-only (no GPU): kvbm_kernels_repage_batch_units for any two non-zero pages, with its conventions (sizing call, counts,
+ * concatenated tables, the small_k wrap) and the records above.  For dividing pages its records and counts are that helper's
+ * with phase 0 in place of seq.  Returns non-zero, writing nothing, for a null seqs with num_seqs > 0, a page of 0, pages past
+ * the exactness bound, a reversed range, or a sequence whose last block of the larger page ends at or past 2^32 tokens. */
+int kvbm_kernels_repage_anypage_units(const kvbm_repage_seq* seqs, size_t num_seqs, uint32_t src_page_size, uint32_t dst_page_size,
+                                      kvbm_repage_anypage_unit* out, size_t cap, size_t* num_units, size_t* src_ids, size_t* dst_ids);
+
+/* kvbm_kernels_paged_stage_repage_gather_batch for any two non-zero pages: the same parameters, with `units` the device-accessible
+ * table kvbm_kernels_repage_anypage_units produced for the same seqs and pages.  Everything is the batch's: stages, layer and head
+ * windows, casts and scales, shared source blocks, no destination block in two sequences, one signal after every sequence
+ * landed, the empty batch's signal and the 2^31 unit bound.  A single range is a batch of one.  With dividing pages it writes
+ * exactly the bytes of kvbm_kernels_paged_stage_repage_gather_batch.  When the destination has the smaller page, two units may
+ * write disjoint token slots of one destination block.  cudaErrorInvalidValue, before any CUDA call, for every rule of
+ * kvbm_kernels_paged_stage_repage_gather_batch but the divisibility of the pages, with kvbm_kernels_repage_anypage_units in place
+ * of kvbm_kernels_repage_batch_units. */
+cudaError_t kvbm_kernels_paged_stage_repage_gather_anypage(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page_size,
+                                                           const kvbm_permute_side* dst, uint32_t dst_num_heads, uint32_t dst_page_size,
+                                                           const kvbm_repage_seq* seqs, size_t num_seqs, const kvbm_repage_anypage_unit* units,
+                                                           size_t num_units, int layer_begin, int layer_end, uint32_t src_row_bytes,
+                                                           int cast_mode, const float* cast_scales, uint32_t* done_flag, uint32_t epoch,
+                                                           uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream);
+
+/* kvbm_kernels_paged_stage_repage_gather_anypage streamed with kvbm_kernels_paged_stage_repage_gather_batch_streamed's flag
+ * conventions and gate forms; the stream-wait form launches the unstreamed anypage kernel per layer.  The argument rules are the
+ * anypage gather's plus the gate's. */
+cudaError_t kvbm_kernels_paged_stage_repage_gather_anypage_streamed(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page_size,
+                                                                    const kvbm_permute_side* dst, uint32_t dst_num_heads,
+                                                                    uint32_t dst_page_size, const kvbm_repage_seq* seqs, size_t num_seqs,
+                                                                    const kvbm_repage_anypage_unit* units, size_t num_units, int layer_begin,
+                                                                    int layer_end, uint32_t src_row_bytes, int cast_mode,
+                                                                    const float* cast_scales, const kvbm_permute_stream* st,
+                                                                    cudaStream_t stream);
+
 /* Host-only (no GPU): the stride table kvbm_kernels_paged_permute walks with for one side.  out[0] = 1 when offsets count
  * from the block's first byte (universal formats) or 0 when they count from the (layer, outer) region's first byte; the
  * element (layer l, outer o, head h, token t) then sits at  [out[0] ? l * out[1] + o * out[2] : 0] + h * out[3] + t * out[4].

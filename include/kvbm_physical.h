@@ -467,6 +467,18 @@ int kvbm_manager_execute_repage_batch(kvbm_transfer_manager* m, size_t num_srcs,
                                       size_t num_windows, const kvbm_layer_stream* ls, const kvbm_transfer_options* opts,
                                       kvbm_notification* out);
 
+/* kvbm_manager_execute_repage_batch between engines whose page sizes need not divide each other (a hybrid model's 544-token
+ * attention block against a 64-token decode page, or 24 against 16), through kvbm_kernels_paged_stage_repage_gather_anypage, or
+ * its streamed form with ls.  The arguments, plans, errors, codes, texts and their order are kvbm_manager_execute_repage_batch's,
+ * but for each pair's page rule: "one page size divides the other" is not asked, and pages past the exactness bound of
+ * include/kvbm_kernels.h, (big + small - gcd) * small < 2^32, fail with KVBM_ERR_UNSUPPORTED in its place.  One staged copy
+ * of every table and the unit table of kvbm_kernels_repage_anypage_units, one launch, one notification, options.done_flag
+ * written once; bytes_moved as the batch's.  With dividing pages the destination bytes are the batch's. */
+int kvbm_manager_execute_repage_anypage(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, kvbm_layout_handle dst,
+                                        const kvbm_repage_batch_seq* seqs, size_t num_seqs, const kvbm_shard_window* windows,
+                                        size_t num_windows, const kvbm_layer_stream* ls, const kvbm_transfer_options* opts,
+                                        kvbm_notification* out);
+
 /* One sequence of kvbm_manager_execute_repage_batch_routed: a kvbm_repage_batch_seq plus the sources it is read from. */
 typedef struct kvbm_repage_route_seq {
   size_t token_begin, token_end;
