@@ -3,6 +3,8 @@ records for one call, in order, with the call's bytes_moved and h2d_bytes deltas
 destination pool, byte for byte, with the oracle of its rig (tests/test_gpu_stage_gather.py's for the permuting entries,
 tests/test_gpu_repage_batch.py's for the re-paging ones).  The streamed forms run behind flags already released, in both
 gate modes."""
+import warnings
+
 import pytest
 import torch
 from torch.autograd import DeviceType
@@ -158,23 +160,65 @@ for _g, _n in ((SPIN, "spin"), (WAIT, "stream_wait")):
     CASES["batch_3_streamed_" + _n] = _batch(SEQS3, _g)
 
 
+ENQUEUE = ("cudaMemcpyAsync", "cudaLaunchKernel")
+WINDOWS = 4      # profile windows one case may take before a complete one
+
+
+def _window(events):
+    """The copies and kernels a profile window holds, in enqueue order, or None when the window is incomplete.  The order is that
+    of the window's cudaMemcpyAsync / cudaLaunchKernel runtime records (their correlation ids); a kernel is named by the device
+    record of the same correlation id, and a device record of a call made outside the window is not this call's.  CUPTI has been
+    seen to drop records in two ways, with the library's bytes right each time:
+    - in a process whose earlier profiler sessions ran many launches, the device record of every staged pinned -> device copy,
+      window after window, while keeping its cudaMemcpyAsync record: a copy is therefore named by its call (H2D), and by its
+      device record when there is one, which must then be that direction;
+    - now and then, every record of a window: a window with no enqueue call, or with a kernel launch whose device record is
+      missing, is incomplete."""
+    calls = sorted((e for e in events if e.device_type() != DeviceType.CUDA and e.name() in ENQUEUE), key=lambda e: e.correlation_id())
+    device = {e.correlation_id(): e.name() for e in events if e.device_type() == DeviceType.CUDA}
+    if not calls or any(c.name() == "cudaLaunchKernel" and c.correlation_id() not in device for c in calls):
+        return None
+    names = []
+    for c in calls:
+        d = device.get(c.correlation_id())
+        if c.name() == "cudaMemcpyAsync":
+            names.append(H2D if d is None or d.startswith(H2D) else d)
+        else:
+            names.append(d.split("(")[0].removeprefix("void ").removeprefix("kvbm::").strip())
+    return names
+
+
+def _describe(events):
+    return "; ".join(f"{'gpu' if e.device_type() == DeviceType.CUDA else 'cpu'} {e.name()[:48]} c{e.correlation_id()}"
+                     for e in sorted(events, key=lambda e: e.correlation_id()) if e.device_type() == DeviceType.CUDA or e.name() in ENQUEUE)
+
+
 def run_case(mgr, name):
-    """One call of the case under the profiler: (device activity names in order, bytes_moved delta, h2d_bytes delta), after the
-    destination pool was compared with the oracle."""
+    """One call of the case under the profiler: (the copies and kernels it enqueued, in order, bytes_moved delta, h2d_bytes delta),
+    after the destination pool was compared with the oracle.  A window the profiler delivered incomplete (_window) is reported as
+    a warning with its records and the call runs again in a new window, up to WINDOWS windows; every run is checked against the
+    oracle and must move the same bytes."""
     from torch.profiler import ProfilerActivity, profile
     r, call = CASES[name](mgr)
-    torch.cuda.synchronize()
-    moved, h2d = mgr.bytes_moved(), mgr.h2d_bytes()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        call().wait(30.0)
+    seen = []
+    for _ in range(WINDOWS):
         torch.cuda.synchronize()
-    moved, h2d = mgr.bytes_moved() - moved, mgr.h2d_bytes() - h2d
-    if isinstance(r, BatchRig):
-        r.check(singles=False)
-    else:
-        r.check()
-    events = sorted((e for e in prof.events() if e.device_type == DeviceType.CUDA), key=lambda e: e.time_range.start)
-    return [e.name.split("(")[0].removeprefix("void ").removeprefix("kvbm::").strip() for e in events], moved, h2d
+        moved, h2d = mgr.bytes_moved(), mgr.h2d_bytes()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            call().wait(30.0)
+            torch.cuda.synchronize()
+        moved, h2d = mgr.bytes_moved() - moved, mgr.h2d_bytes() - h2d
+        if isinstance(r, BatchRig):
+            r.check(singles=False)
+        else:
+            r.check()
+        events = prof.profiler.kineto_results.events()
+        names = _window(events)
+        if names is not None:
+            return names, moved, h2d
+        seen.append(_describe(events))
+        warnings.warn(f"{name}: incomplete profile window {len(seen)}: {seen[-1]}")
+    pytest.fail(f"{name}: no complete profile window in {WINDOWS}: " + " | ".join(seen))
 
 
 @pytest.fixture()
