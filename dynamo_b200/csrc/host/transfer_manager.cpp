@@ -1742,10 +1742,10 @@ struct ScatterRequest {
 static bool routed_to(const uint32_t* mask, size_t d) { return !mask || (d < 32 && ((*mask >> d) & 1u)); }
 
 // Every check of one sequence of a scatter after check_scatter_windows, under the manager's lock, in the order its header gives.
-// mask: a routed sequence's destinations, whose id lists alone are read and checked.
+// mask: a routed sequence's destinations, whose id lists alone are read and checked.  anypage: check_repage_pair's.
 static int check_scatter_request(kvbm_transfer_manager* m, kvbm_layout_handle src_h, const kvbm_scatter_batch_seq& q, size_t num_dsts,
                                  const kvbm_layout_handle* dsts, const kvbm_scatter_window* w, size_t nw, const kvbm_transfer_options& o,
-                                 const kvbm_layer_stream* ls, ScatterRequest* R, const uint32_t* mask = nullptr)
+                                 const kvbm_layer_stream* ls, ScatterRequest* R, const uint32_t* mask = nullptr, bool anypage = false)
 {
   int rc;
   Layout* S = R->S = m->find(src_h);
@@ -1766,7 +1766,8 @@ static int check_scatter_request(kvbm_transfer_manager* m, kvbm_layout_handle sr
     e[j].S = S;
     e[j].D[0] = &Dj;
     e[j].window = kvbm_head_window{0, w[j].src_head_begin, w[j].dst_head_begin, w[j].head_count};
-    if ((rc = check_repage_pair(*S, Dj, op, true, &e[j].src_kv, &e[j].dst_kv, true)) || (rc = check_head_window(*S, Dj, e[j].window, 1))) return rc;
+    if ((rc = check_repage_pair(*S, Dj, op, true, &e[j].src_kv, &e[j].dst_kv, true, anypage)) || (rc = check_head_window(*S, Dj, e[j].window, 1)))
+      return rc;
     if (Dj.cfg.page_size != D[w[0].dst_rank]->cfg.page_size)
       return fail(KVBM_ERR_INCOMPATIBLE, "the destinations of a scatter need one page size: destination " + std::to_string(w[0].dst_rank) +
                                              " has " + std::to_string(D[w[0].dst_rank]->cfg.page_size) + ", destination " +
@@ -1800,10 +1801,12 @@ static int check_scatter_request(kvbm_transfer_manager* m, kvbm_layout_handle sr
 // routing checks run after the windows', each sequence's routed id lists alone are checked, the uniqueness per destination runs
 // over its routed sequences, unrouted positions of the staged tables are padded with block 0, and the unit table carries each
 // sequence's window mask for the routed kernel entries.
+// anypage: a batch whose pages need not divide (kvbm_manager_execute_repage_scatter_anypage): check_repage_pair's anypage rule,
+// the unit table of kvbm_kernels_repage_anypage_units, and the anypage scatter entries.
 static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle src_h, size_t num_dsts, const kvbm_layout_handle* dsts,
                                   const kvbm_scatter_batch_seq* seqs, size_t num_seqs, const kvbm_scatter_window* w, size_t nw,
                                   const kvbm_transfer_options* opts_in, kvbm_notification* out, const kvbm_layer_stream* ls = nullptr,
-                                  bool batch = false, const uint32_t* masks = nullptr)
+                                  bool batch = false, const uint32_t* masks = nullptr, bool anypage = false)
 {
   kvbm_transfer_options o{};
   if (opts_in) o = *opts_in;
@@ -1832,7 +1835,7 @@ static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle s
   for (size_t i = 0; i < num_seqs; ++i) {
     const kvbm_scatter_batch_seq& q = seqs[i];
     const uint32_t* mask = masks ? masks + i : nullptr;
-    if ((rc = check_scatter_request(m, src_h, q, num_dsts, dsts, w, nw, o, ls, &R, mask))) return rc;
+    if ((rc = check_scatter_request(m, src_h, q, num_dsts, dsts, w, nw, o, ls, &R, mask, anypage))) return rc;
     if (R.empty) continue;
     any = true;
     // what lands: each routed window's destination bytes over its layers inside the range
@@ -1883,7 +1886,7 @@ static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle s
       }
       return KVBM_OK;
     };
-    if ((rc = batch_tables(seqs, num_seqs, used, 1, ups, upd, ids, unique, &bt, &n_src, &n_dst))) return rc;
+    if ((rc = batch_tables(seqs, num_seqs, used, 1, ups, upd, ids, unique, &bt, &n_src, &n_dst, anypage))) return rc;
     src_ids = bt.lists[0];
     dst_ids = bt.lists.data() + 1;
     if (masks) {  // each non-empty sequence's range with its window mask, which replaces the unit's sequence index
@@ -1924,9 +1927,14 @@ static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle s
   const int k = static_cast<int>(nw), ilb = static_cast<int>(R.lb), ile = static_cast<int>(R.le);
   const auto* du = reinterpret_cast<const kvbm_repage_unit*>(sl->dev_ids + units_at(n_src + num_dsts * n_dst));
   const auto* dr = reinterpret_cast<const kvbm_route_unit*>(du);
+  const auto* da = reinterpret_cast<const kvbm_repage_anypage_unit*>(du);
   if (ls) {
     const kvbm_permute_stream st = layer_stream(*ls, e, 1, o, *sl, seq);
-    if (masks)
+    if (anypage)
+      rc = checked(kvbm_kernels_paged_repage_scatter_anypage_streamed(&ks, snh, ups, kt, k, upd, bt.ranges.data(), bt.ranges.size(), da,
+                                                                      bt.units.size(), ilb, ile, row, o.cast_mode, o.cast_scales, &st, stream),
+                   "kvbm_kernels_paged_repage_scatter_anypage_streamed");
+    else if (masks)
       rc = checked(kvbm_kernels_paged_repage_scatter_routed_streamed(&ks, snh, ups, kt, k, upd, routes.data(), routes.size(), dr, bt.units.size(),
                                                                      ilb, ile, row, o.cast_mode, o.cast_scales, &st, stream),
                    "kvbm_kernels_paged_repage_scatter_routed_streamed");
@@ -1939,7 +1947,12 @@ static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle s
                                                               &st, stream),
                    "kvbm_kernels_paged_repage_scatter_streamed");
   } else {
-    if (masks)
+    if (anypage)
+      rc = checked(kvbm_kernels_paged_repage_scatter_anypage(&ks, snh, ups, kt, k, upd, bt.ranges.data(), bt.ranges.size(), da, bt.units.size(),
+                                                             ilb, ile, row, o.cast_mode, o.cast_scales, o.epoch, sl->host_flag,
+                                                             static_cast<uint32_t>(seq), stream),
+                   "kvbm_kernels_paged_repage_scatter_anypage");
+    else if (masks)
       rc = checked(kvbm_kernels_paged_repage_scatter_routed(&ks, snh, ups, kt, k, upd, routes.data(), routes.size(), dr, bt.units.size(), ilb, ile,
                                                             row, o.cast_mode, o.cast_scales, o.epoch, sl->host_flag, static_cast<uint32_t>(seq),
                                                             stream),
@@ -2633,6 +2646,18 @@ extern "C" int kvbm_manager_execute_repage_scatter_batch(kvbm_transfer_manager* 
   return guarded([&]() -> int {
   if (int rc = stream_entry(m, ls, 1, false, out)) return rc;
   return execute_repage_scatter(m, src, num_dsts, dsts, seqs, num_seqs, windows, num_windows, opts, out, ls, /*batch=*/true);
+  });
+}
+
+extern "C" int kvbm_manager_execute_repage_scatter_anypage(kvbm_transfer_manager* m, kvbm_layout_handle src, size_t num_dsts,
+                                                           const kvbm_layout_handle* dsts, const kvbm_scatter_batch_seq* seqs, size_t num_seqs,
+                                                           const kvbm_scatter_window* windows, size_t num_windows, const kvbm_layer_stream* ls,
+                                                           const kvbm_transfer_options* opts, kvbm_notification* out)
+{
+  return guarded([&]() -> int {
+  if (int rc = stream_entry(m, ls, 1, false, out)) return rc;
+  return execute_repage_scatter(m, src, num_dsts, dsts, seqs, num_seqs, windows, num_windows, opts, out, ls, /*batch=*/true,
+                                /*masks=*/nullptr, /*anypage=*/true);
   });
 }
 

@@ -1043,9 +1043,13 @@ __host__ __device__ __forceinline__ uint32_t source_layer(const ScatterParams&, 
 // with Ps < Pd block j is entry j of every target's table (they share Pd and the range).
 // ROUTE: only the pairs whose target's bit is set in `mask` (the unit's sequence's targets) are stored, and an entry with no such
 // pair loads nothing.  Only pair_tgt[p] < num_targets selects a bit, so bits at or above the launch's target count are never read.
-template <int CAST, bool POW2, bool SCALED, bool PPOW2, bool ROUTE = false>
+// PHASE / phase: repage_at's, the unit's phase when pages need not divide (DESIGN §4.2l).  Both halves split phase + q on the small
+// side: with Ps < Pd the loads from the source's table, else every target's stores into its own table, all with the one small_k
+// and phase (every target shares Pd and the batch layout).
+template <int CAST, bool POW2, bool SCALED, bool PPOW2, bool ROUTE = false, bool PHASE = false>
 __device__ __forceinline__ void scatter_head_rows(const ScatterParams& P, uint32_t k, uint32_t j, uint32_t l, uint32_t o, const RepageUnit& u,
-                                                  uint32_t run, const RowSplit& r, const ptx::Scale& scale, uint32_t mask = 0)
+                                                  uint32_t run, const RowSplit& r, const ptx::Scale& scale, uint32_t mask = 0,
+                                                  uint32_t phase = 0)
 {
   constexpr int IN = CAST == KVBM_CAST_BF16_TO_FP8E4M3 ? 2 : 1;
   constexpr int OUT = CAST == KVBM_CAST_FP8E4M3_TO_BF16 ? 2 : 1;
@@ -1067,7 +1071,7 @@ __device__ __forceinline__ void scatter_head_rows(const ScatterParams& P, uint32
 #pragma unroll
     for (int i = 0; i < U; ++i)
       if (v + i * 32 < run) {
-        const RepageAt a = repage_at<POW2, PPOW2>(G, r, u.q0, v + i * 32);
+        const RepageAt a = repage_at<POW2, PPOW2, PHASE>(G, r, u.q0, v + i * 32, phase);
         load_vector(ss ? repage_small(sh, S.ids, u.small_k, S.block_stride, static_cast<uint32_t>(S.tok_stride), small_shift, a)
                        : repage_big(sh, static_cast<uint32_t>(S.tok_stride), big_shift, a),
                     x[i]);
@@ -1075,7 +1079,7 @@ __device__ __forceinline__ void scatter_head_rows(const ScatterParams& P, uint32
 #pragma unroll
     for (int i = 0; i < U; ++i)
       if (v + i * 32 < run) {
-        const RepageAt a = repage_at<POW2, PPOW2>(G, r, u.q0, v + i * 32);
+        const RepageAt a = repage_at<POW2, PPOW2, PHASE>(G, r, u.q0, v + i * 32, phase);
         uint4 y[OUT];
         if constexpr (CAST == KVBM_CAST_NONE)
           y[0] = x[i][0];
@@ -1100,16 +1104,21 @@ __device__ __forceinline__ void scatter_head_rows(const ScatterParams& P, uint32
 // One (big block j, source layer l, outer o) unit of the scatter, clipped to the range, with l's stage T: one warp per covered
 // source head of T, looping by the CTA's warps past 8.  SCALED: the SOURCE's scales[l * no + o], loaded once per unit.
 // TABLE: a batch of sequences, whose unit comes from `units` (batch_unit) instead of the launch's one token range.  ROUTE: a
-// routed batch, whose unit and target mask come from record j of `routes` in the same 16 B load (scatter_head_rows' ROUTE).
-template <int CAST, bool POW2, bool SCALED, bool PPOW2, bool TABLE = false, bool ROUTE = false>
+// routed batch, whose unit and target mask come from record j of `routes` in the same 16 B load (scatter_head_rows' ROUTE).  ANY:
+// a batch whose pages need not divide, whose unit and phase come from record j of `any` (anypage_unit).
+template <int CAST, bool POW2, bool SCALED, bool PPOW2, bool TABLE = false, bool ROUTE = false, bool ANY = false>
 __device__ __forceinline__ void scatter_unit(const ScatterParams& P, const GatherStage& T, uint32_t j, uint32_t l, uint32_t o, const RowSplit& r,
                                              const float* scales, const kvbm_repage_unit* units = nullptr,
-                                             const kvbm_route_unit* routes = nullptr)
+                                             const kvbm_route_unit* routes = nullptr, const kvbm_repage_anypage_unit* any = nullptr)
 {
   const RepageGeom& G = P.geo;
   RepageUnit u;
-  uint32_t mask = 0;
-  if constexpr (ROUTE) {
+  uint32_t mask = 0, phase = 0;
+  if constexpr (ANY) {
+    const RepageAnyUnit a = anypage_unit(any, j);
+    u = a.u;
+    phase = a.phase;
+  } else if constexpr (ROUTE) {
     const uint4 w = __ldg(reinterpret_cast<const uint4*>(routes) + j);
     u = {w.x, w.y, w.z};
     mask = w.w;
@@ -1122,7 +1131,7 @@ __device__ __forceinline__ void scatter_unit(const ScatterParams& P, const Gathe
   const uint32_t run = row_run<POW2>(r, u.tokens);
   const uint32_t end = T.first + T.count;
   for (uint32_t k = T.first + (threadIdx.x >> 5); k < end; k += blockDim.x >> 5)
-    scatter_head_rows<CAST, POW2, SCALED, PPOW2, ROUTE>(P, k, j, l, o, u, run, r, scale, mask);
+    scatter_head_rows<CAST, POW2, SCALED, PPOW2, ROUTE, ANY>(P, k, j, l, o, u, run, r, scale, mask, phase);
 }
 
 // One CTA per unit, as the re-paging gather.  The re-paging gathers' bound: three CTAs per SM.
@@ -1156,6 +1165,18 @@ kvbm_paged_repage_route_kernel(const __grid_constant__ ScatterParams P, const kv
   const auto [j, l, rem] = repage_cta(P.geo);
   const uint32_t o = rem % P.geo.no;
   scatter_unit<CAST, POW2, SCALED, PPOW2, true, true>(P, stage_of(P, l), j, l, o, r, scales, nullptr, routes);
+}
+
+// kvbm_paged_repage_push_seqs_kernel over a batch whose pages need not divide: record j of `units` also carries big block j's phase
+// (DESIGN §4.2l).  The same bound: three CTAs per SM.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__global__ void __launch_bounds__(256, 3)
+kvbm_paged_repage_phased_push_kernel(const __grid_constant__ ScatterParams P, const kvbm_repage_anypage_unit* units, RowSplit r,
+                                     const float* scales)
+{
+  const auto [j, l, rem] = repage_cta(P.geo);
+  const uint32_t o = rem % P.geo.no;
+  scatter_unit<CAST, POW2, SCALED, PPOW2, false, false, true>(P, stage_of(P, l), j, l, o, r, scales, nullptr, nullptr, units);
 }
 
 // The scatter's signal after its launch: every target's done flag (epoch) and the completion word, system scope.
@@ -1384,6 +1405,21 @@ kvbm_gated_repage_route_kernel(const __grid_constant__ ScatterParams P, const __
       target_done(F, num_flags, A));
 }
 
+// kvbm_gated_repage_push_seqs_kernel over a batch whose pages need not divide (num_big: the length of `units`).
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__global__ void __launch_bounds__(256, 1)
+kvbm_gated_repage_phased_push_kernel(const __grid_constant__ ScatterParams P, const __grid_constant__ GateArgs A,
+                                     const __grid_constant__ ScatterFlags F, int num_flags, const kvbm_repage_anypage_unit* units,
+                                     uint32_t num_big, RowSplit r, const float* scales, uint32_t batch)
+{
+  gated_repage_units(
+      A, P, P.geo, num_big, batch,
+      [&](const GatherStage& T, uint32_t j, uint32_t l, uint32_t o) {
+        scatter_unit<CAST, POW2, SCALED, PPOW2, false, false, true>(P, T, j, l, o, r, scales, nullptr, nullptr, units);
+      },
+      target_done(F, num_flags, A));
+}
+
 // The stream-wait form's signal after layer l: its layer-done flag, and after the last layer the done and completion flags.
 __global__ void kvbm_layer_signal_kernel(uint32_t* layer_done, uint32_t* done, uint32_t epoch, uint32_t* completion, uint32_t completion_value)
 {
@@ -1596,6 +1632,10 @@ static cudaError_t preload_kernels()
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_anypage_kernel<c, p, sc, false>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_anypage_kernel<c, p, sc, true>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_anypage_kernel<c, p, sc, false>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_phased_push_kernel<c, p, sc, true>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_phased_push_kernel<c, p, sc, false>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_phased_push_kernel<c, p, sc, true>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_phased_push_kernel<c, p, sc, false>);
         });
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_layer_signal_kernel);
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_scatter_signal_kernel);
@@ -2294,7 +2334,8 @@ static bool fill_scatter_targets(const kvbm_scatter_target* tg, int n, uint32_t 
 // before them), then one kvbm_paged_repage_scatter_kernel launch and the signal.  st: a streamed launch (its flags are the ones
 // passed, and its done flag is written with the targets'), which takes the gated push kernel, or per source layer this launch
 // unstreamed.  B: a batch of sequences in place of the one token range (token_begin / token_end unused), which always takes the
-// push_seqs kernels, or the route kernels for a routed batch, whose every target mask must be non-zero and below bit num_targets.
+// push_seqs kernels, or the route kernels for a routed batch, whose every target mask must be non-zero and below bit num_targets,
+// or the phased push kernels for a batch whose pages need not divide (B->any).
 static cudaError_t launch_paged_repage_scatter(const kvbm_permute_side* src, uint32_t src_num_heads, uint32_t src_page,
                                                const kvbm_scatter_target* targets, int num_targets, uint32_t dst_page, uint32_t token_begin,
                                                uint32_t token_end, int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode,
@@ -2340,6 +2381,9 @@ static cudaError_t launch_paged_repage_scatter(const kvbm_permute_side* src, uin
             if (B && B->route)
               kvbm_gated_repage_route_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, Ag, F, num_targets, B->route_units, L.num_big, r,
                                                                                         cast_scales, batch);
+            else if (B && B->any)
+              kvbm_gated_repage_phased_push_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, Ag, F, num_targets, B->any_units, L.num_big,
+                                                                                              r, cast_scales, batch);
             else if (B)
               kvbm_gated_repage_push_seqs_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, Ag, F, num_targets, B->units, L.num_big, r,
                                                                                             cast_scales, batch);
@@ -2351,6 +2395,9 @@ static cudaError_t launch_paged_repage_scatter(const kvbm_permute_side* src, uin
   with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, L.page_pow2, [&](auto c, auto p, auto sc, auto pp) {
     if (B && B->route)
       kvbm_paged_repage_route_kernel<c, p, sc, pp><<<static_cast<unsigned>(L.units), threads, 0, stream>>>(P, B->route_units, r, cast_scales);
+    else if (B && B->any)
+      kvbm_paged_repage_phased_push_kernel<c, p, sc, pp><<<static_cast<unsigned>(L.units), threads, 0, stream>>>(P, B->any_units, r,
+                                                                                                                cast_scales);
     else if (B)
       kvbm_paged_repage_push_seqs_kernel<c, p, sc, pp><<<static_cast<unsigned>(L.units), threads, 0, stream>>>(P, B->units, r, cast_scales);
     else
@@ -2802,6 +2849,32 @@ kvbm_kernels_paged_repage_scatter_batch_streamed(const kvbm_permute_side* src, u
 {
   if (!stream_args_ok(st, 1)) return cudaErrorInvalidValue;
   const RepageBatch B{seqs, num_seqs, units, num_units};
+  return launch_paged_repage_scatter(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, 0, 0, layer_begin, layer_end,
+                                     src_row_bytes, cast_mode, cast_scales, st->epoch, st->completion_flag, st->completion_value, stream, st,
+                                     &B);
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_repage_scatter_anypage(const kvbm_permute_side* src, uint32_t src_num_heads, uint32_t src_page_size,
+                                          const kvbm_scatter_target* targets, int num_targets, uint32_t dst_page_size, const kvbm_repage_seq* seqs,
+                                          size_t num_seqs, const kvbm_repage_anypage_unit* units, size_t num_units, int layer_begin,
+                                          int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales, uint32_t epoch,
+                                          uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
+{
+  const RepageBatch B{seqs, num_seqs, nullptr, num_units, false, nullptr, nullptr, true, units};
+  return launch_paged_repage_scatter(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, 0, 0, layer_begin, layer_end,
+                                     src_row_bytes, cast_mode, cast_scales, epoch, completion_flag, completion_value, stream, nullptr, &B);
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_repage_scatter_anypage_streamed(const kvbm_permute_side* src, uint32_t src_num_heads, uint32_t src_page_size,
+                                                   const kvbm_scatter_target* targets, int num_targets, uint32_t dst_page_size,
+                                                   const kvbm_repage_seq* seqs, size_t num_seqs, const kvbm_repage_anypage_unit* units,
+                                                   size_t num_units, int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode,
+                                                   const float* cast_scales, const kvbm_permute_stream* st, cudaStream_t stream)
+{
+  if (!stream_args_ok(st, 1)) return cudaErrorInvalidValue;
+  const RepageBatch B{seqs, num_seqs, nullptr, num_units, false, nullptr, nullptr, true, units};
   return launch_paged_repage_scatter(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, 0, 0, layer_begin, layer_end,
                                      src_row_bytes, cast_mode, cast_scales, st->epoch, st->completion_flag, st->completion_value, stream, st,
                                      &B);

@@ -302,6 +302,10 @@ def lib() -> C.CDLL:
         L.kvbm_kernels_paged_stage_repage_gather_anypage.restype = i
         L.kvbm_kernels_paged_stage_repage_gather_anypage_streamed.argtypes = L.kvbm_kernels_paged_stage_repage_gather_batch_streamed.argtypes
         L.kvbm_kernels_paged_stage_repage_gather_anypage_streamed.restype = i
+        L.kvbm_kernels_paged_repage_scatter_anypage.argtypes = L.kvbm_kernels_paged_repage_scatter_batch.argtypes
+        L.kvbm_kernels_paged_repage_scatter_anypage.restype = i
+        L.kvbm_kernels_paged_repage_scatter_anypage_streamed.argtypes = L.kvbm_kernels_paged_repage_scatter_batch_streamed.argtypes
+        L.kvbm_kernels_paged_repage_scatter_anypage_streamed.restype = i
         L.kvbm_kernels_permute_strides.argtypes = [i, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64, C.c_uint64,
                                                    C.POINTER(C.c_uint64)]
         L.kvbm_kernels_permute_strides.restype = i
@@ -335,6 +339,7 @@ EXPORTED_SYMBOLS = [
     "kvbm_kernels_paged_repage_scatter_routed_streamed", "kvbm_kernels_paged_stage_repage_gather_routed",
     "kvbm_kernels_paged_stage_repage_gather_routed_streamed", "kvbm_kernels_repage_anypage_units",
     "kvbm_kernels_paged_stage_repage_gather_anypage", "kvbm_kernels_paged_stage_repage_gather_anypage_streamed",
+    "kvbm_kernels_paged_repage_scatter_anypage", "kvbm_kernels_paged_repage_scatter_anypage_streamed",
 ]
 
 
@@ -705,6 +710,34 @@ def paged_repage_scatter_batch_streamed(src: PermuteSide, src_num_heads: int, sr
                                                                   units or None, num_units, layer_begin, layer_end, src_row_bytes,
                                                                   int(cast_mode), scales_ptr(cast_scales),
                                                                   C.byref(st) if st is not None else None, stream)
+
+
+def paged_repage_scatter_anypage(src: PermuteSide, src_num_heads: int, src_page_size: int, targets: Sequence[ScatterTarget],
+                                 dst_page_size: int, seqs: Sequence[Tuple[int, int]], units: int, num_units: int, layer_begin: int,
+                                 layer_end: int, src_row_bytes: int, cast_mode: int = 0, cast_scales=None, epoch: int = 0,
+                                 completion_flag: int = 0, completion_value: int = 0, stream: int = 0) -> int:
+    """`paged_repage_scatter_batch` for any two non-zero pages, dividing or not: `units` is the device address of the table
+    `repage_anypage_units` made for the same ranges and pages (Ps, Pd), which serves every target.  With dividing pages it writes
+    the batch scatter's bytes.  include/kvbm_kernels.h (kvbm_kernels_paged_repage_scatter_anypage)."""
+    arr = (ScatterTarget * max(1, len(targets)))(*targets)
+    return lib().kvbm_kernels_paged_repage_scatter_anypage(C.byref(src), src_num_heads, src_page_size, arr, len(targets), dst_page_size,
+                                                           C.cast(_repage_seqs(seqs), C.c_void_p), len(seqs), units or None, num_units,
+                                                           layer_begin, layer_end, src_row_bytes, int(cast_mode), scales_ptr(cast_scales),
+                                                           epoch, completion_flag or None, completion_value, stream)
+
+
+def paged_repage_scatter_anypage_streamed(src: PermuteSide, src_num_heads: int, src_page_size: int, targets: Sequence[ScatterTarget],
+                                          dst_page_size: int, seqs: Sequence[Tuple[int, int]], units: int, num_units: int,
+                                          layer_begin: int, layer_end: int, src_row_bytes: int, cast_mode: int, cast_scales,
+                                          st: Optional[PermuteStream], stream: int = 0) -> int:
+    """`paged_repage_scatter_anypage` streamed with `paged_repage_scatter_batch_streamed`'s flags and gate forms.
+    include/kvbm_kernels.h (kvbm_kernels_paged_repage_scatter_anypage_streamed)."""
+    arr = (ScatterTarget * max(1, len(targets)))(*targets)
+    return lib().kvbm_kernels_paged_repage_scatter_anypage_streamed(C.byref(src), src_num_heads, src_page_size, arr, len(targets),
+                                                                    dst_page_size, C.cast(_repage_seqs(seqs), C.c_void_p), len(seqs),
+                                                                    units or None, num_units, layer_begin, layer_end, src_row_bytes,
+                                                                    int(cast_mode), scales_ptr(cast_scales),
+                                                                    C.byref(st) if st is not None else None, stream)
 
 
 def _route_seqs(seqs: Sequence[Tuple[int, int, int]]):

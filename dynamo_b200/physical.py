@@ -275,6 +275,7 @@ EXPORTED_SYMBOLS = [
     "kvbm_manager_execute_repage_batch", "kvbm_tp_pp_scatter_plan", "kvbm_manager_execute_repage_scatter",
     "kvbm_manager_execute_repage_scatter_streamed", "kvbm_manager_execute_repage_scatter_batch",
     "kvbm_manager_execute_repage_scatter_routed", "kvbm_manager_execute_repage_batch_routed", "kvbm_manager_execute_repage_anypage",
+    "kvbm_manager_execute_repage_scatter_anypage",
 ]
 
 
@@ -347,6 +348,7 @@ def lib() -> C.CDLL:
                                                                    sz, P(_CLayerStream), P(_COptions), P(u64)]
         L.kvbm_manager_execute_repage_scatter_batch.argtypes = [vp, u64, sz, P(u64), P(_CScatterBatchSeq), sz, P(_CScatterWindow), sz,
                                                                 P(_CLayerStream), P(_COptions), P(u64)]
+        L.kvbm_manager_execute_repage_scatter_anypage.argtypes = L.kvbm_manager_execute_repage_scatter_batch.argtypes
         L.kvbm_manager_execute_repage_scatter_routed.argtypes = [vp, u64, sz, P(u64), P(_CScatterRouteSeq), sz, P(_CScatterWindow), sz,
                                                                  P(_CLayerStream), P(_COptions), P(u64)]
         L.kvbm_notification_is_complete.argtypes = [vp, u64]
@@ -1050,6 +1052,22 @@ class TransferManager:
         as `execute_repage_scatter_streamed` does, and `layer_done_flags[l]` is written once source layer l of every sequence
         landed.  Two sequences may share source blocks; a destination block may appear once per destination in the whole batch.
         The first rejected sequence raises what `execute_repage_scatter` would raise for it."""
+        return self._repage_scatter_batch(lib().kvbm_manager_execute_repage_scatter_batch, src, dsts, seqs, plan, options, ready_flags,
+                                          layer_done_flags)
+
+    def execute_repage_scatter_anypage(self, src: int, dsts: Sequence[int], seqs: Sequence[tuple], plan: Sequence[ScatterWindow],
+                                       options: Optional[TransferOptions] = None, ready_flags: Optional[int] = None,
+                                       layer_done_flags: int = 0) -> TransferCompleteNotification:
+        """`execute_repage_scatter_batch` between engines whose page sizes need not divide each other
+        (kvbm_manager_execute_repage_scatter_anypage), e.g. a hybrid model's 544-token attention block pushed into 64-token decode
+        pages, or 24 into 16: the same arguments, plans, errors and streaming.  Pages past the exactness bound
+        (big + small - gcd) * small < 2^32 raise UNSUPPORTED.  With dividing pages the destination bytes are
+        `execute_repage_scatter_batch`'s."""
+        return self._repage_scatter_batch(lib().kvbm_manager_execute_repage_scatter_anypage, src, dsts, seqs, plan, options, ready_flags,
+                                          layer_done_flags)
+
+    def _repage_scatter_batch(self, entry, src, dsts, seqs, plan, options, ready_flags, layer_done_flags):
+        """The body of `execute_repage_scatter_batch` and `execute_repage_scatter_anypage`: `entry` is the C entry they call."""
         keep, cs, ws = [], (_CScatterBatchSeq * max(1, len(seqs)))(), None
         for c, (tokens, src_ids, dst_ids) in zip(cs, seqs):
             args = self._scatter_args(src, src_ids, dsts, dst_ids, plan, tokens)
@@ -1063,8 +1081,8 @@ class TransferManager:
         ls = self._layer_stream([0], {0: ready_flags}, layer_done_flags) if ready_flags is not None else None
         tok = C.c_uint64()
         o = (options or TransferOptions())._c()
-        _check(lib().kvbm_manager_execute_repage_scatter_batch(self._h, src, len(dsts), hs, cs, len(seqs), ws, len(plan),
-                                                               C.byref(ls) if ls is not None else None, C.byref(o), C.byref(tok)))
+        _check(entry(self._h, src, len(dsts), hs, cs, len(seqs), ws, len(plan), C.byref(ls) if ls is not None else None, C.byref(o),
+                     C.byref(tok)))
         return TransferCompleteNotification(self, tok.value)
 
     def execute_repage_scatter_routed(self, src: int, dsts: Sequence[int], seqs: Sequence[tuple], plan: Sequence[ScatterWindow],

@@ -691,9 +691,9 @@ cudaError_t kvbm_kernels_paged_stage_repage_gather_routed_streamed(const kvbm_st
                                                                    const float* cast_scales, const kvbm_permute_stream* st,
                                                                    cudaStream_t stream);
 
-/* ---- re-paging between pages that need not divide: a batch gather for any two page sizes -------------------------------------
+/* ---- re-paging between pages that need not divide: a batch gather and a batch scatter for any two page sizes ------------------
  * Engines configured independently keep pages that neither divide: a hybrid model's attention block of 544 tokens against a
- * decode engine's 64, or 24 against 16.  Every entry above rejects such a pair; the two below take any two non-zero pages.
+ * decode engine's 64, or 24 against 16.  Every entry above rejects such a pair; the entries below take any two non-zero pages.
  * The unit stays one block of the larger-page side.  Its block's slot 0 is sequence position F = j * big_page; the smaller-page
  * side's block that holds F is entry small_k of its concatenated table, and F sits at slot `phase` = F % small_page of it.  The
  * token at big slot q then sits at offset phase + q from the start of that small block: in block small_k + (phase + q) /
@@ -742,6 +742,36 @@ cudaError_t kvbm_kernels_paged_stage_repage_gather_anypage_streamed(const kvbm_s
                                                                     int layer_end, uint32_t src_row_bytes, int cast_mode,
                                                                     const float* cast_scales, const kvbm_permute_stream* st,
                                                                     cudaStream_t stream);
+
+/* kvbm_kernels_paged_repage_scatter_batch for any two non-zero pages: the push-side counterpart of the anypage gather, one source
+ * of page Ps into up to KVBM_GATHER_MAX_SOURCES targets of page Pd in ONE launch, each vector read and cast once and stored to
+ * every target.  The same parameters, with `units` the device-accessible table kvbm_kernels_repage_anypage_units(seqs, Ps, Pd)
+ * produced; as in the batch scatter, every target shares Pd and the batch layout, so one unit table (and its phases) serves every
+ * target.  Everything is the batch scatter's: windows, stages, formats, casts and scales, shared source blocks, no destination
+ * block in two sequences of one target pool, every target's done_flag and completion_flag written once after every sequence
+ * landed, the empty batch's signal and the 2^31 unit bound.  A single range is a batch of one.  With dividing pages it writes
+ * exactly the bytes of kvbm_kernels_paged_repage_scatter_batch.  When Pd < Ps two units may write disjoint token slots of one
+ * target block; when Ps < Pd several units read one source block.  cudaErrorInvalidValue, before any CUDA call, for every rule
+ * of kvbm_kernels_paged_repage_scatter_batch but the divisibility of the pages, with kvbm_kernels_repage_anypage_units (and its
+ * exactness bound) in place of kvbm_kernels_repage_batch_units. */
+cudaError_t kvbm_kernels_paged_repage_scatter_anypage(const kvbm_permute_side* src, uint32_t src_num_heads, uint32_t src_page_size,
+                                                      const kvbm_scatter_target* targets, int num_targets, uint32_t dst_page_size,
+                                                      const kvbm_repage_seq* seqs, size_t num_seqs, const kvbm_repage_anypage_unit* units,
+                                                      size_t num_units, int layer_begin, int layer_end, uint32_t src_row_bytes,
+                                                      int cast_mode, const float* cast_scales, uint32_t epoch, uint32_t* completion_flag,
+                                                      uint32_t completion_value, cudaStream_t stream);
+
+/* kvbm_kernels_paged_repage_scatter_anypage streamed with kvbm_kernels_paged_repage_scatter_batch_streamed's flag conventions and
+ * gate forms: one ready flag per source layer covers the batch, layer_done_flags[l] is written once source layer l of every
+ * sequence landed in every target, and after a gate timeout no done flag is written and completion_flag becomes 0xFFFFFFFF.  The
+ * stream-wait form launches the unstreamed anypage scatter per source layer.  The argument rules are the anypage scatter's plus
+ * the gate's with one source. */
+cudaError_t kvbm_kernels_paged_repage_scatter_anypage_streamed(const kvbm_permute_side* src, uint32_t src_num_heads, uint32_t src_page_size,
+                                                               const kvbm_scatter_target* targets, int num_targets, uint32_t dst_page_size,
+                                                               const kvbm_repage_seq* seqs, size_t num_seqs,
+                                                               const kvbm_repage_anypage_unit* units, size_t num_units, int layer_begin,
+                                                               int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
+                                                               const kvbm_permute_stream* st, cudaStream_t stream);
 
 /* Host-only (no GPU): the stride table kvbm_kernels_paged_permute walks with for one side.  out[0] = 1 when offsets count
  * from the block's first byte (universal formats) or 0 when they count from the (layer, outer) region's first byte; the

@@ -581,6 +581,20 @@ int kvbm_manager_execute_repage_scatter_batch(kvbm_transfer_manager* m, kvbm_lay
                                               size_t num_windows, const kvbm_layer_stream* ls, const kvbm_transfer_options* opts,
                                               kvbm_notification* out);
 
+/* kvbm_manager_execute_repage_scatter_batch between engines whose page sizes need not divide each other (a hybrid model's
+ * 544-token attention block pushed into 64-token decode pages, or 24 into 16), through kvbm_kernels_paged_repage_scatter_anypage,
+ * or its streamed form with ls.  The arguments, plans, errors, codes, texts and their order are
+ * kvbm_manager_execute_repage_scatter_batch's, but for each window's page rule: "one page size divides the other" is not asked,
+ * and pages past the exactness bound of include/kvbm_kernels.h, (big + small - gcd) * small < 2^32, fail with
+ * KVBM_ERR_UNSUPPORTED and kvbm_manager_execute_repage_anypage's text in its place.  One staged copy of every table and the unit
+ * table of kvbm_kernels_repage_anypage_units, one launch, one notification; per_dst_done_flags and done_flag written once, after
+ * every sequence landed (never after a gate timeout); bytes_moved as the batch's.  With dividing pages the destination bytes are
+ * the batch's.  Every other scatter entry keeps rejecting pages that do not divide. */
+int kvbm_manager_execute_repage_scatter_anypage(kvbm_transfer_manager* m, kvbm_layout_handle src, size_t num_dsts,
+                                                const kvbm_layout_handle* dsts, const kvbm_scatter_batch_seq* seqs, size_t num_seqs,
+                                                const kvbm_scatter_window* windows, size_t num_windows, const kvbm_layer_stream* ls,
+                                                const kvbm_transfer_options* opts, kvbm_notification* out);
+
 /* One sequence of kvbm_manager_execute_repage_scatter_routed: a kvbm_scatter_batch_seq plus the destinations it goes to. */
 typedef struct kvbm_scatter_route_seq {
   size_t token_begin, token_end;
