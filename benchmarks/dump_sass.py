@@ -68,6 +68,10 @@ for _c, _cn in ((0, ""), (1, "_fp8_to_bf16"), (2, "_bf16_to_fp8")):
                     f"paged_repage_phased_push{_cn}_row_{'pow2' if _r else 'mulhi'}_page_{'pow2' if _p else 'mulhi'}{'_scaled' if _sc else ''}")
                 WANT[f"gated_repage_phased_push_kernelILi{_c}ELb{_r}ELb{_sc}ELb{_p}E"] = (
                     f"gated_repage_phased_push{_cn}_row_{'pow2' if _r else 'mulhi'}_page_{'pow2' if _p else 'mulhi'}{'_scaled' if _sc else ''}")
+                # the routed gather and the routed scatter between pages that need not divide, one CTA per unit and streamed
+                for _k in ("paged_repage_collect", "gated_repage_collect", "paged_repage_deal", "gated_repage_deal"):
+                    WANT[f"{_k}_kernelILi{_c}ELb{_r}ELb{_sc}ELb{_p}E"] = (
+                        f"{_k}{_cn}_row_{'pow2' if _r else 'mulhi'}_page_{'pow2' if _p else 'mulhi'}{'_scaled' if _sc else ''}")
             # the layer-streamed (gated, persistent) gather: <cast, row pow2, scaled>
             WANT[f"gated_gather_kernelILi{_c}ELb{_r}ELb{_sc}E"] = f"gated_gather{_cn}_{'pow2' if _r else 'mulhi'}{'_scaled' if _sc else ''}"
 WANT["layer_signal_kernel"] = "layer_signal"

@@ -1477,10 +1477,14 @@ struct BatchTables {
 
 // List k of sequence q is ids(q, k): q.n_src ids for k < num_src_lists, else q.n_dst.  check(t->cat), the caller's duplicate-id
 // checks, runs before the unit table.  *n_src / *n_dst: each concatenated source and destination table's length.  anypage: the
-// unit table is kvbm_kernels_repage_anypage_units' (the same 16 B records, the phase in the fourth word).
+// unit table is kvbm_kernels_repage_anypage_units' (the same 16 B records, the phase in the fourth word).  routes (with anypage):
+// each non-empty sequence's range and window mask, in t->ranges' order; the unit table is then
+// kvbm_kernels_repage_route_anypage_units', whose fourth word packs the mask with the phase, so that no sequence index survives in
+// it to be rewritten.
 template <class Seq, class Ids, class Check>
 static int batch_tables(const Seq* seqs, size_t num_seqs, const std::vector<bool>& used, size_t num_src_lists, uint32_t ps, uint32_t pd,
-                        Ids ids, Check check, BatchTables* t, size_t* n_src, size_t* n_dst, bool anypage = false)
+                        Ids ids, Check check, BatchTables* t, size_t* n_src, size_t* n_dst, bool anypage = false,
+                        const kvbm_route_seq* routes = nullptr)
 {
   t->cat.resize(used.size());
   for (size_t i = 0; i < num_seqs; ++i) {
@@ -1491,8 +1495,12 @@ static int batch_tables(const Seq* seqs, size_t num_seqs, const std::vector<bool
       if (used[k]) t->cat[k].insert(t->cat[k].end(), ids(q, k), ids(q, k) + (k < num_src_lists ? q.n_src : q.n_dst));
   }
   if (int rc = check(t->cat)) return rc;
-  static_assert(sizeof(kvbm_repage_anypage_unit) == sizeof(kvbm_repage_unit), "one staged record layout");
+  static_assert(sizeof(kvbm_repage_anypage_unit) == sizeof(kvbm_repage_unit) && sizeof(kvbm_route_anypage_unit) == sizeof(kvbm_repage_unit),
+                "one staged record layout");
   auto units = [&](kvbm_repage_unit* out, size_t cap, size_t* num_units) {
+    if (anypage && routes)
+      return kvbm_kernels_repage_route_anypage_units(routes, t->ranges.size(), ps, pd, reinterpret_cast<kvbm_route_anypage_unit*>(out), cap,
+                                                     num_units, n_src, n_dst);
     return anypage ? kvbm_kernels_repage_anypage_units(t->ranges.data(), t->ranges.size(), ps, pd, reinterpret_cast<kvbm_repage_anypage_unit*>(out),
                                                        cap, num_units, n_src, n_dst)
                    : kvbm_kernels_repage_batch_units(t->ranges.data(), t->ranges.size(), ps, pd, out, cap, num_units, n_src, n_dst);
@@ -1516,7 +1524,8 @@ static int batch_tables(const Seq* seqs, size_t num_seqs, const std::vector<bool
 // layout, unrouted positions of the staged tables are padded with block 0, and the unit table carries each sequence's window
 // mask for the routed kernel entries.
 // anypage: a batch whose pages need not divide (kvbm_manager_execute_repage_anypage): check_repage_pair's anypage rule, the unit
-// table of kvbm_kernels_repage_anypage_units, and the anypage kernel entries.
+// table of kvbm_kernels_repage_anypage_units, and the anypage kernel entries.  Both (kvbm_manager_execute_repage_batch_routed_anypage):
+// the routed batch's checks, the unit table of kvbm_kernels_repage_route_anypage_units, and the routed anypage kernel entries.
 static int execute_repage(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, kvbm_layout_handle dst_h,
                           const kvbm_repage_batch_seq* seqs, size_t num_seqs, const kvbm_head_window* windows, size_t nw,
                           const kvbm_transfer_options* opts_in, kvbm_notification* out, const kvbm_layer_stream* ls = nullptr,
@@ -1625,15 +1634,17 @@ static int execute_repage(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_
       }
       return KVBM_OK;
     };
-    if ((rc = batch_tables(seqs, num_seqs, used, num_srcs, ups, upd, ids, unique, &bt, &n_src, &n_dst, anypage))) return rc;
+    // each non-empty sequence's range with its window mask, which replaces the unit's sequence index (or joins the phase)
+    for (size_t i = 0; masks && i < num_seqs; ++i)
+      if (seqs[i].token_begin != seqs[i].token_end)
+        routes.push_back(kvbm_route_seq{static_cast<uint32_t>(seqs[i].token_begin), static_cast<uint32_t>(seqs[i].token_end), window_mask(i)});
+    if ((rc = batch_tables(seqs, num_seqs, used, num_srcs, ups, upd, ids, unique, &bt, &n_src, &n_dst, anypage,
+                           masks ? routes.data() : nullptr)))
+      return rc;
     src_ids = bt.lists.data();
     dst_ids = bt.lists[num_srcs];
-    if (masks) {  // each non-empty sequence's range with its window mask, which replaces the unit's sequence index
-      for (size_t i = 0; i < num_seqs; ++i)
-        if (seqs[i].token_begin != seqs[i].token_end)
-          routes.push_back(kvbm_route_seq{static_cast<uint32_t>(seqs[i].token_begin), static_cast<uint32_t>(seqs[i].token_end), window_mask(i)});
+    if (masks && !anypage)
       for (kvbm_repage_unit& u : bt.units) u.seq = routes[u.seq].targets;
-    }
   }
 
   DeviceGuard g(m->device);
@@ -1654,6 +1665,17 @@ static int execute_repage(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_
       const auto* du = reinterpret_cast<const kvbm_repage_unit*>(sl.dev_ids + units_at(num_srcs * n_src + n_dst));
       const auto* dr = reinterpret_cast<const kvbm_route_unit*>(du);
       const auto* da = reinterpret_cast<const kvbm_repage_anypage_unit*>(du);
+      const auto* dra = reinterpret_cast<const kvbm_route_anypage_unit*>(du);
+      if (masks && anypage && st)
+        return checked(kvbm_kernels_paged_stage_repage_gather_routed_anypage_streamed(ss, k, ups, &kd, dnh, upd, routes.data(), routes.size(), dra,
+                                                                                      bt.units.size(), ilb, ile, row, o.cast_mode, o.cast_scales,
+                                                                                      st, stream),
+                       "kvbm_kernels_paged_stage_repage_gather_routed_anypage_streamed");
+      if (masks && anypage)
+        return checked(kvbm_kernels_paged_stage_repage_gather_routed_anypage(ss, k, ups, &kd, dnh, upd, routes.data(), routes.size(), dra,
+                                                                             bt.units.size(), ilb, ile, row, o.cast_mode, o.cast_scales,
+                                                                             o.done_flag, o.epoch, sl.host_flag, value, stream),
+                       "kvbm_kernels_paged_stage_repage_gather_routed_anypage");
       if (anypage && st)
         return checked(kvbm_kernels_paged_stage_repage_gather_anypage_streamed(ss, k, ups, &kd, dnh, upd, bt.ranges.data(), bt.ranges.size(), da,
                                                                                bt.units.size(), ilb, ile, row, o.cast_mode, o.cast_scales, st,
@@ -1802,7 +1824,9 @@ static int check_scatter_request(kvbm_transfer_manager* m, kvbm_layout_handle sr
 // over its routed sequences, unrouted positions of the staged tables are padded with block 0, and the unit table carries each
 // sequence's window mask for the routed kernel entries.
 // anypage: a batch whose pages need not divide (kvbm_manager_execute_repage_scatter_anypage): check_repage_pair's anypage rule,
-// the unit table of kvbm_kernels_repage_anypage_units, and the anypage scatter entries.
+// the unit table of kvbm_kernels_repage_anypage_units, and the anypage scatter entries.  Both
+// (kvbm_manager_execute_repage_scatter_routed_anypage): the routed batch's checks, the unit table of
+// kvbm_kernels_repage_route_anypage_units, and the routed anypage scatter entries.
 static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle src_h, size_t num_dsts, const kvbm_layout_handle* dsts,
                                   const kvbm_scatter_batch_seq* seqs, size_t num_seqs, const kvbm_scatter_window* w, size_t nw,
                                   const kvbm_transfer_options* opts_in, kvbm_notification* out, const kvbm_layer_stream* ls = nullptr,
@@ -1886,18 +1910,19 @@ static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle s
       }
       return KVBM_OK;
     };
-    if ((rc = batch_tables(seqs, num_seqs, used, 1, ups, upd, ids, unique, &bt, &n_src, &n_dst, anypage))) return rc;
+    // each non-empty sequence's range with its window mask, which replaces the unit's sequence index (or joins the phase)
+    for (size_t i = 0; masks && i < num_seqs; ++i) {
+      if (seqs[i].token_begin == seqs[i].token_end) continue;
+      uint32_t targets = 0;
+      for (size_t j = 0; j < nw; ++j) targets |= static_cast<uint32_t>(routed_to(masks + i, w[j].dst_rank)) << j;
+      routes.push_back(kvbm_route_seq{static_cast<uint32_t>(seqs[i].token_begin), static_cast<uint32_t>(seqs[i].token_end), targets});
+    }
+    if ((rc = batch_tables(seqs, num_seqs, used, 1, ups, upd, ids, unique, &bt, &n_src, &n_dst, anypage, masks ? routes.data() : nullptr)))
+      return rc;
     src_ids = bt.lists[0];
     dst_ids = bt.lists.data() + 1;
-    if (masks) {  // each non-empty sequence's range with its window mask, which replaces the unit's sequence index
-      for (size_t i = 0; i < num_seqs; ++i) {
-        if (seqs[i].token_begin == seqs[i].token_end) continue;
-        uint32_t targets = 0;
-        for (size_t j = 0; j < nw; ++j) targets |= static_cast<uint32_t>(routed_to(masks + i, w[j].dst_rank)) << j;
-        routes.push_back(kvbm_route_seq{static_cast<uint32_t>(seqs[i].token_begin), static_cast<uint32_t>(seqs[i].token_end), targets});
-      }
+    if (masks && !anypage)
       for (kvbm_repage_unit& u : bt.units) u.seq = routes[u.seq].targets;
-    }
   }
 
   DeviceGuard g(m->device);
@@ -1928,9 +1953,15 @@ static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle s
   const auto* du = reinterpret_cast<const kvbm_repage_unit*>(sl->dev_ids + units_at(n_src + num_dsts * n_dst));
   const auto* dr = reinterpret_cast<const kvbm_route_unit*>(du);
   const auto* da = reinterpret_cast<const kvbm_repage_anypage_unit*>(du);
+  const auto* dra = reinterpret_cast<const kvbm_route_anypage_unit*>(du);
   if (ls) {
     const kvbm_permute_stream st = layer_stream(*ls, e, 1, o, *sl, seq);
-    if (anypage)
+    if (masks && anypage)
+      rc = checked(kvbm_kernels_paged_repage_scatter_routed_anypage_streamed(&ks, snh, ups, kt, k, upd, routes.data(), routes.size(), dra,
+                                                                             bt.units.size(), ilb, ile, row, o.cast_mode, o.cast_scales, &st,
+                                                                             stream),
+                   "kvbm_kernels_paged_repage_scatter_routed_anypage_streamed");
+    else if (anypage)
       rc = checked(kvbm_kernels_paged_repage_scatter_anypage_streamed(&ks, snh, ups, kt, k, upd, bt.ranges.data(), bt.ranges.size(), da,
                                                                       bt.units.size(), ilb, ile, row, o.cast_mode, o.cast_scales, &st, stream),
                    "kvbm_kernels_paged_repage_scatter_anypage_streamed");
@@ -1947,7 +1978,12 @@ static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle s
                                                               &st, stream),
                    "kvbm_kernels_paged_repage_scatter_streamed");
   } else {
-    if (anypage)
+    if (masks && anypage)
+      rc = checked(kvbm_kernels_paged_repage_scatter_routed_anypage(&ks, snh, ups, kt, k, upd, routes.data(), routes.size(), dra, bt.units.size(),
+                                                                    ilb, ile, row, o.cast_mode, o.cast_scales, o.epoch, sl->host_flag,
+                                                                    static_cast<uint32_t>(seq), stream),
+                   "kvbm_kernels_paged_repage_scatter_routed_anypage");
+    else if (anypage)
       rc = checked(kvbm_kernels_paged_repage_scatter_anypage(&ks, snh, ups, kt, k, upd, bt.ranges.data(), bt.ranges.size(), da, bt.units.size(),
                                                              ilb, ile, row, o.cast_mode, o.cast_scales, o.epoch, sl->host_flag,
                                                              static_cast<uint32_t>(seq), stream),
@@ -2661,10 +2697,11 @@ extern "C" int kvbm_manager_execute_repage_scatter_anypage(kvbm_transfer_manager
   });
 }
 
-extern "C" int kvbm_manager_execute_repage_scatter_routed(kvbm_transfer_manager* m, kvbm_layout_handle src, size_t num_dsts,
-                                                          const kvbm_layout_handle* dsts, const kvbm_scatter_route_seq* seqs, size_t num_seqs,
-                                                          const kvbm_scatter_window* windows, size_t num_windows, const kvbm_layer_stream* ls,
-                                                          const kvbm_transfer_options* opts, kvbm_notification* out)
+// The body of kvbm_manager_execute_repage_scatter_routed and, with anypage, of kvbm_manager_execute_repage_scatter_routed_anypage.
+static int execute_repage_scatter_routed(kvbm_transfer_manager* m, kvbm_layout_handle src, size_t num_dsts, const kvbm_layout_handle* dsts,
+                                         const kvbm_scatter_route_seq* seqs, size_t num_seqs, const kvbm_scatter_window* windows,
+                                         size_t num_windows, const kvbm_layer_stream* ls, const kvbm_transfer_options* opts,
+                                         kvbm_notification* out, bool anypage)
 {
   return guarded([&]() -> int {
   if (int rc = stream_entry(m, ls, 1, false, out)) return rc;
@@ -2676,8 +2713,25 @@ extern "C" int kvbm_manager_execute_repage_scatter_routed(kvbm_transfer_manager*
     masks[i] = s.dst_mask;
   }
   return execute_repage_scatter(m, src, num_dsts, dsts, seqs ? qs.data() : nullptr, num_seqs, windows, num_windows, opts, out, ls,
-                                /*batch=*/true, masks.data());
+                                /*batch=*/true, masks.data(), anypage);
   });
+}
+
+extern "C" int kvbm_manager_execute_repage_scatter_routed(kvbm_transfer_manager* m, kvbm_layout_handle src, size_t num_dsts,
+                                                          const kvbm_layout_handle* dsts, const kvbm_scatter_route_seq* seqs, size_t num_seqs,
+                                                          const kvbm_scatter_window* windows, size_t num_windows, const kvbm_layer_stream* ls,
+                                                          const kvbm_transfer_options* opts, kvbm_notification* out)
+{
+  return execute_repage_scatter_routed(m, src, num_dsts, dsts, seqs, num_seqs, windows, num_windows, ls, opts, out, /*anypage=*/false);
+}
+
+extern "C" int kvbm_manager_execute_repage_scatter_routed_anypage(kvbm_transfer_manager* m, kvbm_layout_handle src, size_t num_dsts,
+                                                                  const kvbm_layout_handle* dsts, const kvbm_scatter_route_seq* seqs,
+                                                                  size_t num_seqs, const kvbm_scatter_window* windows, size_t num_windows,
+                                                                  const kvbm_layer_stream* ls, const kvbm_transfer_options* opts,
+                                                                  kvbm_notification* out)
+{
+  return execute_repage_scatter_routed(m, src, num_dsts, dsts, seqs, num_seqs, windows, num_windows, ls, opts, out, /*anypage=*/true);
 }
 
 // The head windows of a staged plan's windows, in hw[], or null without windows.  Only the first KVBM_GATHER_MAX_SOURCES are
@@ -2754,10 +2808,11 @@ extern "C" int kvbm_manager_execute_repage_anypage(kvbm_transfer_manager* m, siz
   });
 }
 
-extern "C" int kvbm_manager_execute_repage_batch_routed(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs,
-                                                        kvbm_layout_handle dst, const kvbm_repage_route_seq* seqs, size_t num_seqs,
-                                                        const kvbm_shard_window* windows, size_t num_windows, const kvbm_layer_stream* ls,
-                                                        const kvbm_transfer_options* opts, kvbm_notification* out)
+// The body of kvbm_manager_execute_repage_batch_routed and, with anypage, of kvbm_manager_execute_repage_batch_routed_anypage.
+static int execute_repage_batch_routed(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, kvbm_layout_handle dst,
+                                       const kvbm_repage_route_seq* seqs, size_t num_seqs, const kvbm_shard_window* windows,
+                                       size_t num_windows, const kvbm_layer_stream* ls, const kvbm_transfer_options* opts,
+                                       kvbm_notification* out, bool anypage)
 {
   return guarded([&]() -> int {
   if (int rc = stream_entry(m, ls, num_srcs, false, out)) return rc;
@@ -2770,8 +2825,25 @@ extern "C" int kvbm_manager_execute_repage_batch_routed(kvbm_transfer_manager* m
     masks[i] = s.src_mask;
   }
   return execute_repage(m, num_srcs, srcs, dst, seqs ? qs.data() : nullptr, num_seqs, head_windows(windows, num_windows, hw), num_windows,
-                        opts, out, ls, /*gather=*/true, windows, /*batch=*/true, masks.data());
+                        opts, out, ls, /*gather=*/true, windows, /*batch=*/true, masks.data(), anypage);
   });
+}
+
+extern "C" int kvbm_manager_execute_repage_batch_routed(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs,
+                                                        kvbm_layout_handle dst, const kvbm_repage_route_seq* seqs, size_t num_seqs,
+                                                        const kvbm_shard_window* windows, size_t num_windows, const kvbm_layer_stream* ls,
+                                                        const kvbm_transfer_options* opts, kvbm_notification* out)
+{
+  return execute_repage_batch_routed(m, num_srcs, srcs, dst, seqs, num_seqs, windows, num_windows, ls, opts, out, /*anypage=*/false);
+}
+
+extern "C" int kvbm_manager_execute_repage_batch_routed_anypage(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs,
+                                                                kvbm_layout_handle dst, const kvbm_repage_route_seq* seqs, size_t num_seqs,
+                                                                const kvbm_shard_window* windows, size_t num_windows,
+                                                                const kvbm_layer_stream* ls, const kvbm_transfer_options* opts,
+                                                                kvbm_notification* out)
+{
+  return execute_repage_batch_routed(m, num_srcs, srcs, dst, seqs, num_seqs, windows, num_windows, ls, opts, out, /*anypage=*/true);
 }
 
 extern "C" int kvbm_manager_execute_repage_gather_streamed(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs,

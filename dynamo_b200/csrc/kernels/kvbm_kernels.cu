@@ -761,6 +761,16 @@ __device__ __forceinline__ RepageAnyUnit anypage_unit(const kvbm_repage_anypage_
   return {{w.x, w.y, w.z}, w.w};
 }
 
+// A routed batch whose pages need not divide (kvbm_route_anypage_unit): the unit, its phase (the high half of the fourth word)
+// and, in *mask, its sequence's mask (the low half), in the same 16 B load.  The mask is cut to its 16 bits although the walks
+// only read bits below the launch's rank count, so that the phase never reaches a mask reader.
+__device__ __forceinline__ RepageAnyUnit route_anypage_unit(const kvbm_route_anypage_unit* units, uint32_t j, uint32_t* mask)
+{
+  const uint4 w = __ldg(reinterpret_cast<const uint4*>(units) + j);
+  *mask = w.w & 0xFFFFu;
+  return {{w.x, w.y, w.z}, w.w >> 16};
+}
+
 // The unit of a one-CTA-per-unit re-paging kernel, blockIdx.x = (big block j * nlayers + l - layer_begin) * no + o.  The caller
 // takes o = rem % no itself: the gathers after their stage lookup, the scatters before it.  Moving it changes how ptxas
 // schedules the division.
@@ -904,12 +914,14 @@ struct RepageGatherParams {
 // ROUTE: a routed batch, whose unit and source mask come from record j of `routes` in one 16 B load.  The warps walk only the
 // entries of the stage's sources in the mask, numbered densely (route_entry), so no warp idles on an unrouted window; heads[s]
 // is source s's entry count.  Only the stage's sources are consulted, so mask bits at or above the launch's sources never are.
-// ANY: a batch whose pages need not divide, whose unit and phase come from record j of `any` (anypage_unit).
+// ANY: a batch whose pages need not divide, whose unit and phase come from record j of `any` (anypage_unit).  ROUTE and ANY:
+// a routed batch whose pages need not divide, whose unit, mask and phase come from record j of `route_any` (route_anypage_unit).
 template <int CAST, bool POW2, bool SCALED, bool PPOW2, bool TABLE = false, bool ROUTE = false, bool ANY = false>
 __device__ __forceinline__ void repage_gather_unit(const RepageGatherParams& P, const GatherStage& T, uint32_t j, uint32_t l, uint32_t o,
                                                    const RowSplit& r, const float* scales, const kvbm_repage_unit* units = nullptr,
                                                    const kvbm_route_unit* routes = nullptr, const uint16_t* heads = nullptr,
-                                                   const kvbm_repage_anypage_unit* any = nullptr)
+                                                   const kvbm_repage_anypage_unit* any = nullptr,
+                                                   const kvbm_route_anypage_unit* route_any = nullptr)
 {
   constexpr int IN = CAST == KVBM_CAST_BF16_TO_FP8E4M3 ? 2 : 1;
   constexpr int OUT = CAST == KVBM_CAST_FP8E4M3_TO_BF16 ? 2 : 1;
@@ -919,7 +931,11 @@ __device__ __forceinline__ void repage_gather_unit(const RepageGatherParams& P, 
   const PermuteSide& D = g.D;
   RepageUnit u;
   uint32_t mask = 0, phase = 0;
-  if constexpr (ANY) {
+  if constexpr (ROUTE && ANY) {
+    const RepageAnyUnit a = route_anypage_unit(route_any, j, &mask);
+    u = a.u;
+    phase = a.phase;
+  } else if constexpr (ANY) {
     const RepageAnyUnit a = anypage_unit(any, j);
     u = a.u;
     phase = a.phase;
@@ -1010,6 +1026,18 @@ kvbm_paged_repage_anypage_kernel(const __grid_constant__ RepageGatherParams P, c
   const auto [j, l, rem] = repage_cta(P.geo);
   repage_gather_unit<CAST, POW2, SCALED, PPOW2, false, false, true>(P, stage_of(P.g, l), j, l, rem % P.geo.no, r, scales, nullptr, nullptr,
                                                                     nullptr, units);
+}
+
+// kvbm_paged_repage_fanin_kernel over a batch whose pages need not divide: record j of `units` carries big block j's sources and
+// phase in its fourth word (DESIGN §4.2m).  The same bound: three CTAs per SM.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__global__ void __launch_bounds__(256, 3)
+kvbm_paged_repage_collect_kernel(const __grid_constant__ RepageGatherParams P, const __grid_constant__ SourceHeads H,
+                                 const kvbm_route_anypage_unit* units, RowSplit r, const float* scales)
+{
+  const auto [j, l, rem] = repage_cta(P.geo);
+  repage_gather_unit<CAST, POW2, SCALED, PPOW2, true, true, true>(P, stage_of(P.g, l), j, l, rem % P.geo.no, r, scales, nullptr, nullptr, H.n,
+                                                                  nullptr, units);
 }
 
 // The re-paging scatter, the gather's mirror image: ONE source pool of page Ps (a prefill rank) into up to
@@ -1105,16 +1133,22 @@ __device__ __forceinline__ void scatter_head_rows(const ScatterParams& P, uint32
 // source head of T, looping by the CTA's warps past 8.  SCALED: the SOURCE's scales[l * no + o], loaded once per unit.
 // TABLE: a batch of sequences, whose unit comes from `units` (batch_unit) instead of the launch's one token range.  ROUTE: a
 // routed batch, whose unit and target mask come from record j of `routes` in the same 16 B load (scatter_head_rows' ROUTE).  ANY:
-// a batch whose pages need not divide, whose unit and phase come from record j of `any` (anypage_unit).
+// a batch whose pages need not divide, whose unit and phase come from record j of `any` (anypage_unit).  ROUTE and ANY: a routed
+// batch whose pages need not divide, whose unit, mask and phase come from record j of `route_any` (route_anypage_unit).
 template <int CAST, bool POW2, bool SCALED, bool PPOW2, bool TABLE = false, bool ROUTE = false, bool ANY = false>
 __device__ __forceinline__ void scatter_unit(const ScatterParams& P, const GatherStage& T, uint32_t j, uint32_t l, uint32_t o, const RowSplit& r,
                                              const float* scales, const kvbm_repage_unit* units = nullptr,
-                                             const kvbm_route_unit* routes = nullptr, const kvbm_repage_anypage_unit* any = nullptr)
+                                             const kvbm_route_unit* routes = nullptr, const kvbm_repage_anypage_unit* any = nullptr,
+                                             const kvbm_route_anypage_unit* route_any = nullptr)
 {
   const RepageGeom& G = P.geo;
   RepageUnit u;
   uint32_t mask = 0, phase = 0;
-  if constexpr (ANY) {
+  if constexpr (ROUTE && ANY) {
+    const RepageAnyUnit a = route_anypage_unit(route_any, j, &mask);
+    u = a.u;
+    phase = a.phase;
+  } else if constexpr (ANY) {
     const RepageAnyUnit a = anypage_unit(any, j);
     u = a.u;
     phase = a.phase;
@@ -1177,6 +1211,17 @@ kvbm_paged_repage_phased_push_kernel(const __grid_constant__ ScatterParams P, co
   const auto [j, l, rem] = repage_cta(P.geo);
   const uint32_t o = rem % P.geo.no;
   scatter_unit<CAST, POW2, SCALED, PPOW2, false, false, true>(P, stage_of(P, l), j, l, o, r, scales, nullptr, nullptr, units);
+}
+
+// kvbm_paged_repage_route_kernel over a batch whose pages need not divide: record j of `units` carries big block j's targets and
+// phase in its fourth word (DESIGN §4.2m).  The same bound: three CTAs per SM.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__global__ void __launch_bounds__(256, 3)
+kvbm_paged_repage_deal_kernel(const __grid_constant__ ScatterParams P, const kvbm_route_anypage_unit* units, RowSplit r, const float* scales)
+{
+  const auto [j, l, rem] = repage_cta(P.geo);
+  const uint32_t o = rem % P.geo.no;
+  scatter_unit<CAST, POW2, SCALED, PPOW2, true, true, true>(P, stage_of(P, l), j, l, o, r, scales, nullptr, nullptr, nullptr, units);
 }
 
 // The scatter's signal after its launch: every target's done flag (epoch) and the completion word, system scope.
@@ -1355,6 +1400,19 @@ kvbm_gated_repage_anypage_kernel(const __grid_constant__ RepageGatherParams P, c
   });
 }
 
+// kvbm_gated_repage_fanin_kernel over a batch whose pages need not divide (num_big: the length of `units`): the stages' sources are
+// the routed ones only, as there.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__global__ void __launch_bounds__(256, 1)
+kvbm_gated_repage_collect_kernel(const __grid_constant__ RepageGatherParams P, const __grid_constant__ GateArgs A,
+                                 const __grid_constant__ SourceHeads H, const kvbm_route_anypage_unit* units, uint32_t num_big, RowSplit r,
+                                 const float* scales, uint32_t batch)
+{
+  gated_repage_units(A, P.g, P.geo, num_big, batch, [&](const GatherStage& T, uint32_t j, uint32_t l, uint32_t o) {
+    repage_gather_unit<CAST, POW2, SCALED, PPOW2, true, true, true>(P, T, j, l, o, r, scales, nullptr, nullptr, H.n, nullptr, units);
+  });
+}
+
 // The push kernels' hook in arrive_transfer: the num_flags target done flags of F, with A.ss's own and before the completion word.
 __device__ __forceinline__ auto target_done(const ScatterFlags& F, const int& num_flags, const GateArgs& A)
 {
@@ -1416,6 +1474,22 @@ kvbm_gated_repage_phased_push_kernel(const __grid_constant__ ScatterParams P, co
       A, P, P.geo, num_big, batch,
       [&](const GatherStage& T, uint32_t j, uint32_t l, uint32_t o) {
         scatter_unit<CAST, POW2, SCALED, PPOW2, false, false, true>(P, T, j, l, o, r, scales, nullptr, nullptr, units);
+      },
+      target_done(F, num_flags, A));
+}
+
+// kvbm_gated_repage_route_kernel over a batch whose pages need not divide (num_big: the length of `units`): every unit of source
+// layer l counts, written or not, as there.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2>
+__global__ void __launch_bounds__(256, 1)
+kvbm_gated_repage_deal_kernel(const __grid_constant__ ScatterParams P, const __grid_constant__ GateArgs A, const __grid_constant__ ScatterFlags F,
+                              int num_flags, const kvbm_route_anypage_unit* units, uint32_t num_big, RowSplit r, const float* scales,
+                              uint32_t batch)
+{
+  gated_repage_units(
+      A, P, P.geo, num_big, batch,
+      [&](const GatherStage& T, uint32_t j, uint32_t l, uint32_t o) {
+        scatter_unit<CAST, POW2, SCALED, PPOW2, true, true, true>(P, T, j, l, o, r, scales, nullptr, nullptr, nullptr, units);
       },
       target_done(F, num_flags, A));
 }
@@ -1636,6 +1710,14 @@ static cudaError_t preload_kernels()
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_phased_push_kernel<c, p, sc, false>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_phased_push_kernel<c, p, sc, true>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_phased_push_kernel<c, p, sc, false>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_collect_kernel<c, p, sc, true>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_collect_kernel<c, p, sc, false>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_collect_kernel<c, p, sc, true>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_collect_kernel<c, p, sc, false>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_deal_kernel<c, p, sc, true>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_deal_kernel<c, p, sc, false>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_deal_kernel<c, p, sc, true>);
+          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_deal_kernel<c, p, sc, false>);
         });
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_layer_signal_kernel);
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_scatter_signal_kernel);
@@ -2055,7 +2137,8 @@ static bool repage_pages(uint32_t src_page, uint32_t dst_page, int layer_begin, 
 
 // A batch of sequences of a re-paging launch: the caller's ranges (host) and unit table (device-accessible).  route: a routed
 // batch, whose ranges and masks (a scatter's targets, a gather's sources) are route_seqs and whose unit table is route_units
-// (seqs and units unused).  any_units: a batch whose pages need not divide, whose unit table is this one (units unused).
+// (seqs and units unused).  any_units: a batch whose pages need not divide, whose unit table is this one (units unused).  route
+// and any together: a routed batch whose pages need not divide, with route_seqs and the unit table route_any_units.
 struct RepageBatch {
   const kvbm_repage_seq* seqs;
   size_t num_seqs;
@@ -2066,6 +2149,7 @@ struct RepageBatch {
   const kvbm_route_unit* route_units = nullptr;
   bool any = false;
   const kvbm_repage_anypage_unit* any_units = nullptr;
+  const kvbm_route_anypage_unit* route_any_units = nullptr;
 };
 
 // What repage_launch derives: repage_pages' results with the token range's fields, the units to launch (0: nothing to move), the
@@ -2080,8 +2164,8 @@ struct RepageLaunch {
 
 // Every re-paging launch's first checks, before any CUDA call: ranges not reversed, cast_args_ok, and B checked by
 // kvbm_kernels_repage_batch_units (a routed batch: kvbm_kernels_repage_route_units; one whose pages need not divide:
-// kvbm_kernels_repage_anypage_units, and repage_pages without the divisibility rule) with the caller's unit count.  An empty range
-// or batch then leaves L->units 0 (the caller
+// kvbm_kernels_repage_anypage_units, and repage_pages without the divisibility rule; both: kvbm_kernels_repage_route_anypage_units)
+// with the caller's unit count.  An empty range or batch then leaves L->units 0 (the caller
 // signals).  Else `side` (a gather's destination, the scatter's source) needs a table, a base, a non-zero outer dim and the layer
 // range; the pages repage_pages' rules; a single range slots in 32 bits (its last block of the larger page ends below 2^32); the
 // launch fewer than 2^31 units.  False: rejected.
@@ -2094,11 +2178,17 @@ static bool repage_launch(const kvbm_permute_side* side, uint32_t src_page, uint
   size_t num_big = 0;
   if (B) {
     size_t src_ids, dst_ids;
-    if ((B->route ? kvbm_kernels_repage_route_units(B->route_seqs, B->num_seqs, src_page, dst_page, nullptr, 0, &num_big, &src_ids, &dst_ids)
-         : B->any ? kvbm_kernels_repage_anypage_units(B->seqs, B->num_seqs, src_page, dst_page, nullptr, 0, &num_big, &src_ids, &dst_ids)
-                  : kvbm_kernels_repage_batch_units(B->seqs, B->num_seqs, src_page, dst_page, nullptr, 0, &num_big, &src_ids, &dst_ids)) != 0)
+    const bool both = B->route && B->any;
+    if ((both ? kvbm_kernels_repage_route_anypage_units(B->route_seqs, B->num_seqs, src_page, dst_page, nullptr, 0, &num_big, &src_ids,
+                                                        &dst_ids)
+         : B->route ? kvbm_kernels_repage_route_units(B->route_seqs, B->num_seqs, src_page, dst_page, nullptr, 0, &num_big, &src_ids, &dst_ids)
+         : B->any   ? kvbm_kernels_repage_anypage_units(B->seqs, B->num_seqs, src_page, dst_page, nullptr, 0, &num_big, &src_ids, &dst_ids)
+                    : kvbm_kernels_repage_batch_units(B->seqs, B->num_seqs, src_page, dst_page, nullptr, 0, &num_big, &src_ids, &dst_ids)) != 0)
       return false;
-    const void* table = B->route ? static_cast<const void*>(B->route_units) : B->any ? static_cast<const void*>(B->any_units) : B->units;
+    const void* table = both       ? static_cast<const void*>(B->route_any_units)
+                        : B->route ? static_cast<const void*>(B->route_units)
+                        : B->any   ? static_cast<const void*>(B->any_units)
+                                   : B->units;
     if (num_big != B->num_units || (num_big != 0 && !table)) return false;
   }
   L->units = 0;
@@ -2135,7 +2225,7 @@ static bool repage_launch(const kvbm_permute_side* side, uint32_t src_page, uint
 // must be non-zero and below bit num_srcs, and two windows of a stage may then share destination heads unless one mask holds both.
 // Each stage's sources are ANDed with the union of the masks, so both gate forms wait on routed sources only, and a CTA has as
 // many warps as the most routed entries of one stage under one mask (up to 8).  A batch whose pages need not divide (B->any)
-// takes the anypage kernels.
+// takes the anypage kernels, or the collect kernels when it is also routed.
 static cudaError_t launch_paged_repage_gather(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page, const kvbm_permute_side* dst,
                                               uint32_t dst_num_heads, uint32_t dst_page, uint32_t token_begin, uint32_t token_end,
                                               int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
@@ -2194,7 +2284,10 @@ static cudaError_t launch_paged_repage_gather(const kvbm_stage_source* srcs, int
         },
         [&](const GateArgs& A, unsigned ctas, uint32_t batch) {
           with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, L.page_pow2, [&](auto c, auto p, auto sc, auto pp) {
-            if (route)
+            if (route && B->any)
+              kvbm_gated_repage_collect_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, A, H, B->route_any_units, L.num_big, r,
+                                                                                            cast_scales, batch);
+            else if (route)
               kvbm_gated_repage_fanin_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, A, H, B->route_units, L.num_big, r, cast_scales, batch);
             else if (B && B->any)
               kvbm_gated_repage_anypage_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, A, B->any_units, L.num_big, r, cast_scales, batch);
@@ -2212,7 +2305,9 @@ static cudaError_t launch_paged_repage_gather(const kvbm_stage_source* srcs, int
   R.small = P.geo.src_small ? P.g.src[0].S : P.g.D;
   R.g = P.geo;
   with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, L.page_pow2, [&](auto c, auto p, auto sc, auto pp) {
-    if (route)
+    if (route && B->any)
+      kvbm_paged_repage_collect_kernel<c, p, sc, pp><<<grid, threads, 0, stream>>>(P, H, B->route_any_units, r, cast_scales);
+    else if (route)
       kvbm_paged_repage_fanin_kernel<c, p, sc, pp><<<grid, threads, 0, stream>>>(P, H, B->route_units, r, cast_scales);
     else if (B && B->any)
       kvbm_paged_repage_anypage_kernel<c, p, sc, pp><<<grid, threads, 0, stream>>>(P, B->any_units, r, cast_scales);
@@ -2335,7 +2430,7 @@ static bool fill_scatter_targets(const kvbm_scatter_target* tg, int n, uint32_t 
 // passed, and its done flag is written with the targets'), which takes the gated push kernel, or per source layer this launch
 // unstreamed.  B: a batch of sequences in place of the one token range (token_begin / token_end unused), which always takes the
 // push_seqs kernels, or the route kernels for a routed batch, whose every target mask must be non-zero and below bit num_targets,
-// or the phased push kernels for a batch whose pages need not divide (B->any).
+// or the phased push kernels for a batch whose pages need not divide (B->any), or the deal kernels for one that is both.
 static cudaError_t launch_paged_repage_scatter(const kvbm_permute_side* src, uint32_t src_num_heads, uint32_t src_page,
                                                const kvbm_scatter_target* targets, int num_targets, uint32_t dst_page, uint32_t token_begin,
                                                uint32_t token_end, int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode,
@@ -2378,7 +2473,10 @@ static cudaError_t launch_paged_repage_scatter(const kvbm_permute_side* src, uin
           const ScatterFlags F = scatter_flags(targets, num_targets, &any);
           Ag.ss.want_done |= any;
           with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, L.page_pow2, [&](auto c, auto p, auto sc, auto pp) {
-            if (B && B->route)
+            if (B && B->route && B->any)
+              kvbm_gated_repage_deal_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, Ag, F, num_targets, B->route_any_units, L.num_big, r,
+                                                                                       cast_scales, batch);
+            else if (B && B->route)
               kvbm_gated_repage_route_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, Ag, F, num_targets, B->route_units, L.num_big, r,
                                                                                         cast_scales, batch);
             else if (B && B->any)
@@ -2393,7 +2491,9 @@ static cudaError_t launch_paged_repage_scatter(const kvbm_permute_side* src, uin
         });
   }
   with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, L.page_pow2, [&](auto c, auto p, auto sc, auto pp) {
-    if (B && B->route)
+    if (B && B->route && B->any)
+      kvbm_paged_repage_deal_kernel<c, p, sc, pp><<<static_cast<unsigned>(L.units), threads, 0, stream>>>(P, B->route_any_units, r, cast_scales);
+    else if (B && B->route)
       kvbm_paged_repage_route_kernel<c, p, sc, pp><<<static_cast<unsigned>(L.units), threads, 0, stream>>>(P, B->route_units, r, cast_scales);
     else if (B && B->any)
       kvbm_paged_repage_phased_push_kernel<c, p, sc, pp><<<static_cast<unsigned>(L.units), threads, 0, stream>>>(P, B->any_units, r,
@@ -2720,6 +2820,17 @@ kvbm_kernels_repage_anypage_units(const kvbm_repage_seq* seqs, size_t num_seqs, 
                      [](size_t, uint32_t phase) { return phase; }, /*any=*/true);
 }
 
+extern "C" int
+kvbm_kernels_repage_route_anypage_units(const kvbm_route_seq* seqs, size_t num_seqs, uint32_t src_page_size, uint32_t dst_page_size,
+                                        kvbm_route_anypage_unit* out, size_t cap, size_t* num_units, size_t* src_ids, size_t* dst_ids)
+{
+  // the mask takes the low half of the fourth word; the phase, below a small page the exactness bound keeps under 2^16, the high
+  for (size_t i = 0; seqs && i < num_seqs; ++i)
+    if (seqs[i].targets >> 16) return 1;
+  return batch_units(seqs, num_seqs, src_page_size, dst_page_size, out, cap, num_units, src_ids, dst_ids,
+                     [seqs](size_t i, uint32_t phase) { return seqs[i].targets | phase << 16; }, /*any=*/true);
+}
+
 extern "C" cudaError_t
 kvbm_kernels_paged_stage_repage_gather_anypage(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page_size, const kvbm_permute_side* dst,
                                                uint32_t dst_num_heads, uint32_t dst_page_size, const kvbm_repage_seq* seqs, size_t num_seqs,
@@ -2801,6 +2912,37 @@ kvbm_kernels_paged_stage_repage_gather_routed_streamed(const kvbm_stage_source* 
   for (size_t i = 0; seqs && i < num_seqs; ++i) used |= seqs[i].targets;
   if (!stream_args_ok(st, num_srcs, used)) return cudaErrorInvalidValue;
   const RepageBatch B{nullptr, num_seqs, nullptr, num_units, true, seqs, units};
+  return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, 0, 0, layer_begin, layer_end,
+                                    src_row_bytes, cast_mode, cast_scales, st->done_flag, st->epoch, st->completion_flag,
+                                    st->completion_value, KVBM_GATHER_MAX_HEADS, stream, st, &B);
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_stage_repage_gather_routed_anypage(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page_size,
+                                                      const kvbm_permute_side* dst, uint32_t dst_num_heads, uint32_t dst_page_size,
+                                                      const kvbm_route_seq* seqs, size_t num_seqs, const kvbm_route_anypage_unit* units,
+                                                      size_t num_units, int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode,
+                                                      const float* cast_scales, uint32_t* done_flag, uint32_t epoch, uint32_t* completion_flag,
+                                                      uint32_t completion_value, cudaStream_t stream)
+{
+  const RepageBatch B{nullptr, num_seqs, nullptr, num_units, true, seqs, nullptr, true, nullptr, units};
+  return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, 0, 0, layer_begin, layer_end,
+                                    src_row_bytes, cast_mode, cast_scales, done_flag, epoch, completion_flag, completion_value,
+                                    KVBM_GATHER_MAX_HEADS, stream, nullptr, &B);
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_stage_repage_gather_routed_anypage_streamed(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page_size,
+                                                               const kvbm_permute_side* dst, uint32_t dst_num_heads, uint32_t dst_page_size,
+                                                               const kvbm_route_seq* seqs, size_t num_seqs,
+                                                               const kvbm_route_anypage_unit* units, size_t num_units, int layer_begin,
+                                                               int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
+                                                               const kvbm_permute_stream* st, cudaStream_t stream)
+{
+  uint32_t used = 0;  // the sources some sequence is routed to: only they need ready flags
+  for (size_t i = 0; seqs && i < num_seqs; ++i) used |= seqs[i].targets;
+  if (!stream_args_ok(st, num_srcs, used)) return cudaErrorInvalidValue;
+  const RepageBatch B{nullptr, num_seqs, nullptr, num_units, true, seqs, nullptr, true, nullptr, units};
   return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, 0, 0, layer_begin, layer_end,
                                     src_row_bytes, cast_mode, cast_scales, st->done_flag, st->epoch, st->completion_flag,
                                     st->completion_value, KVBM_GATHER_MAX_HEADS, stream, st, &B);
@@ -2901,6 +3043,34 @@ kvbm_kernels_paged_repage_scatter_routed_streamed(const kvbm_permute_side* src, 
 {
   if (!stream_args_ok(st, 1)) return cudaErrorInvalidValue;
   const RepageBatch B{nullptr, num_seqs, nullptr, num_units, true, seqs, units};
+  return launch_paged_repage_scatter(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, 0, 0, layer_begin, layer_end,
+                                     src_row_bytes, cast_mode, cast_scales, st->epoch, st->completion_flag, st->completion_value, stream, st,
+                                     &B);
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_repage_scatter_routed_anypage(const kvbm_permute_side* src, uint32_t src_num_heads, uint32_t src_page_size,
+                                                 const kvbm_scatter_target* targets, int num_targets, uint32_t dst_page_size,
+                                                 const kvbm_route_seq* seqs, size_t num_seqs, const kvbm_route_anypage_unit* units,
+                                                 size_t num_units, int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode,
+                                                 const float* cast_scales, uint32_t epoch, uint32_t* completion_flag,
+                                                 uint32_t completion_value, cudaStream_t stream)
+{
+  const RepageBatch B{nullptr, num_seqs, nullptr, num_units, true, seqs, nullptr, true, nullptr, units};
+  return launch_paged_repage_scatter(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, 0, 0, layer_begin, layer_end,
+                                     src_row_bytes, cast_mode, cast_scales, epoch, completion_flag, completion_value, stream, nullptr, &B);
+}
+
+extern "C" cudaError_t
+kvbm_kernels_paged_repage_scatter_routed_anypage_streamed(const kvbm_permute_side* src, uint32_t src_num_heads, uint32_t src_page_size,
+                                                          const kvbm_scatter_target* targets, int num_targets, uint32_t dst_page_size,
+                                                          const kvbm_route_seq* seqs, size_t num_seqs, const kvbm_route_anypage_unit* units,
+                                                          size_t num_units, int layer_begin, int layer_end, uint32_t src_row_bytes,
+                                                          int cast_mode, const float* cast_scales, const kvbm_permute_stream* st,
+                                                          cudaStream_t stream)
+{
+  if (!stream_args_ok(st, 1)) return cudaErrorInvalidValue;
+  const RepageBatch B{nullptr, num_seqs, nullptr, num_units, true, seqs, nullptr, true, nullptr, units};
   return launch_paged_repage_scatter(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, 0, 0, layer_begin, layer_end,
                                      src_row_bytes, cast_mode, cast_scales, st->epoch, st->completion_flag, st->completion_value, stream, st,
                                      &B);

@@ -135,6 +135,12 @@ class RepageAnypageUnit(C.Structure):
     _fields_ = [("q0", C.c_uint32), ("tokens", C.c_uint32), ("small_k", C.c_uint32), ("phase", C.c_uint32)]
 
 
+class RouteAnypageUnit(C.Structure):
+    """struct kvbm_route_anypage_unit: RouteUnit for pages that need not divide, 16 B: route = targets | phase << 16
+    (`repage_route_anypage_units` writes them)"""
+    _fields_ = [("q0", C.c_uint32), ("tokens", C.c_uint32), ("small_k", C.c_uint32), ("route", C.c_uint32)]
+
+
 class ScatterTarget(C.Structure):
     """struct kvbm_scatter_target: one target of `paged_repage_scatter` (a destination side, its head count, one head window, one
     layer window and its nullable done flag)"""
@@ -306,6 +312,17 @@ def lib() -> C.CDLL:
         L.kvbm_kernels_paged_repage_scatter_anypage.restype = i
         L.kvbm_kernels_paged_repage_scatter_anypage_streamed.argtypes = L.kvbm_kernels_paged_repage_scatter_batch_streamed.argtypes
         L.kvbm_kernels_paged_repage_scatter_anypage_streamed.restype = i
+        L.kvbm_kernels_repage_route_anypage_units.argtypes = L.kvbm_kernels_repage_route_units.argtypes
+        L.kvbm_kernels_repage_route_anypage_units.restype = i
+        L.kvbm_kernels_paged_repage_scatter_routed_anypage.argtypes = L.kvbm_kernels_paged_repage_scatter_batch.argtypes
+        L.kvbm_kernels_paged_repage_scatter_routed_anypage.restype = i
+        L.kvbm_kernels_paged_repage_scatter_routed_anypage_streamed.argtypes = L.kvbm_kernels_paged_repage_scatter_batch_streamed.argtypes
+        L.kvbm_kernels_paged_repage_scatter_routed_anypage_streamed.restype = i
+        L.kvbm_kernels_paged_stage_repage_gather_routed_anypage.argtypes = L.kvbm_kernels_paged_stage_repage_gather_batch.argtypes
+        L.kvbm_kernels_paged_stage_repage_gather_routed_anypage.restype = i
+        L.kvbm_kernels_paged_stage_repage_gather_routed_anypage_streamed.argtypes = (
+            L.kvbm_kernels_paged_stage_repage_gather_batch_streamed.argtypes)
+        L.kvbm_kernels_paged_stage_repage_gather_routed_anypage_streamed.restype = i
         L.kvbm_kernels_permute_strides.argtypes = [i, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64, C.c_uint64,
                                                    C.POINTER(C.c_uint64)]
         L.kvbm_kernels_permute_strides.restype = i
@@ -340,6 +357,9 @@ EXPORTED_SYMBOLS = [
     "kvbm_kernels_paged_stage_repage_gather_routed_streamed", "kvbm_kernels_repage_anypage_units",
     "kvbm_kernels_paged_stage_repage_gather_anypage", "kvbm_kernels_paged_stage_repage_gather_anypage_streamed",
     "kvbm_kernels_paged_repage_scatter_anypage", "kvbm_kernels_paged_repage_scatter_anypage_streamed",
+    "kvbm_kernels_repage_route_anypage_units", "kvbm_kernels_paged_repage_scatter_routed_anypage",
+    "kvbm_kernels_paged_repage_scatter_routed_anypage_streamed", "kvbm_kernels_paged_stage_repage_gather_routed_anypage",
+    "kvbm_kernels_paged_stage_repage_gather_routed_anypage_streamed",
 ]
 
 
@@ -811,6 +831,73 @@ def paged_stage_repage_gather_routed_streamed(srcs: Sequence[StageSource], src_p
                                                                         units or None, num_units, layer_begin, layer_end, src_row_bytes,
                                                                         int(cast_mode), scales_ptr(cast_scales),
                                                                         C.byref(st) if st is not None else None, stream)
+
+
+def repage_route_anypage_units(seqs: Sequence[Tuple[int, int, int]], src_page_size: int, dst_page_size: int):
+    """Host-only: `repage_anypage_units` over the (token_begin, token_end, targets) of a routed batch, each record's fourth word its
+    sequence's targets | its block's phase << 16: a numpy uint32 array [num_units, 4] (q0, tokens, small_k, route) and the two table
+    lengths, or None (also for a mask with a bit at or above 16).  include/kvbm_kernels.h (kvbm_kernels_repage_route_anypage_units)."""
+    return _unit_table(lib().kvbm_kernels_repage_route_anypage_units, _route_seqs(seqs), len(seqs), src_page_size, dst_page_size)
+
+
+def paged_repage_scatter_routed_anypage(src: PermuteSide, src_num_heads: int, src_page_size: int, targets: Sequence[ScatterTarget],
+                                        dst_page_size: int, seqs: Sequence[Tuple[int, int, int]], units: int, num_units: int,
+                                        layer_begin: int, layer_end: int, src_row_bytes: int, cast_mode: int = 0, cast_scales=None,
+                                        epoch: int = 0, completion_flag: int = 0, completion_value: int = 0, stream: int = 0) -> int:
+    """`paged_repage_scatter_routed` for any two non-zero pages, dividing or not: `units` is the device address of the table
+    `repage_route_anypage_units` made for the same sequences and pages.  include/kvbm_kernels.h
+    (kvbm_kernels_paged_repage_scatter_routed_anypage)."""
+    arr = (ScatterTarget * max(1, len(targets)))(*targets)
+    return lib().kvbm_kernels_paged_repage_scatter_routed_anypage(C.byref(src), src_num_heads, src_page_size, arr, len(targets),
+                                                                  dst_page_size, C.cast(_route_seqs(seqs), C.c_void_p), len(seqs),
+                                                                  units or None, num_units, layer_begin, layer_end, src_row_bytes,
+                                                                  int(cast_mode), scales_ptr(cast_scales), epoch, completion_flag or None,
+                                                                  completion_value, stream)
+
+
+def paged_repage_scatter_routed_anypage_streamed(src: PermuteSide, src_num_heads: int, src_page_size: int,
+                                                 targets: Sequence[ScatterTarget], dst_page_size: int, seqs: Sequence[Tuple[int, int, int]],
+                                                 units: int, num_units: int, layer_begin: int, layer_end: int, src_row_bytes: int,
+                                                 cast_mode: int, cast_scales, st: Optional[PermuteStream], stream: int = 0) -> int:
+    """`paged_repage_scatter_routed_anypage` streamed with `paged_repage_scatter_routed_streamed`'s flags and gate forms.
+    include/kvbm_kernels.h (kvbm_kernels_paged_repage_scatter_routed_anypage_streamed)."""
+    arr = (ScatterTarget * max(1, len(targets)))(*targets)
+    return lib().kvbm_kernels_paged_repage_scatter_routed_anypage_streamed(C.byref(src), src_num_heads, src_page_size, arr, len(targets),
+                                                                           dst_page_size, C.cast(_route_seqs(seqs), C.c_void_p), len(seqs),
+                                                                           units or None, num_units, layer_begin, layer_end, src_row_bytes,
+                                                                           int(cast_mode), scales_ptr(cast_scales),
+                                                                           C.byref(st) if st is not None else None, stream)
+
+
+def paged_stage_repage_gather_routed_anypage(srcs: Sequence[StageSource], src_page_size: int, dst: PermuteSide, dst_num_heads: int,
+                                             dst_page_size: int, seqs: Sequence[Tuple[int, int, int]], units: int, num_units: int,
+                                             layer_begin: int, layer_end: int, src_row_bytes: int, cast_mode: int = 0, cast_scales=None,
+                                             done_flag: int = 0, epoch: int = 0, completion_flag: int = 0, completion_value: int = 0,
+                                             stream: int = 0) -> int:
+    """`paged_stage_repage_gather_routed` for any two non-zero pages, dividing or not: `units` is the device address of the table
+    `repage_route_anypage_units` made for the same sequences and pages.  include/kvbm_kernels.h
+    (kvbm_kernels_paged_stage_repage_gather_routed_anypage)."""
+    arr = (StageSource * max(1, len(srcs)))(*srcs)
+    return lib().kvbm_kernels_paged_stage_repage_gather_routed_anypage(arr, len(srcs), src_page_size, C.byref(dst), dst_num_heads,
+                                                                       dst_page_size, C.cast(_route_seqs(seqs), C.c_void_p), len(seqs),
+                                                                       units or None, num_units, layer_begin, layer_end, src_row_bytes,
+                                                                       int(cast_mode), scales_ptr(cast_scales), done_flag or None, epoch,
+                                                                       completion_flag or None, completion_value, stream)
+
+
+def paged_stage_repage_gather_routed_anypage_streamed(srcs: Sequence[StageSource], src_page_size: int, dst: PermuteSide,
+                                                      dst_num_heads: int, dst_page_size: int, seqs: Sequence[Tuple[int, int, int]],
+                                                      units: int, num_units: int, layer_begin: int, layer_end: int, src_row_bytes: int,
+                                                      cast_mode: int, cast_scales, st: Optional[PermuteStream], stream: int = 0) -> int:
+    """`paged_stage_repage_gather_routed_anypage` streamed with `paged_stage_repage_gather_routed_streamed`'s flags and gate forms;
+    only the sources some sequence is routed to are waited on.
+    include/kvbm_kernels.h (kvbm_kernels_paged_stage_repage_gather_routed_anypage_streamed)."""
+    arr = (StageSource * max(1, len(srcs)))(*srcs)
+    return lib().kvbm_kernels_paged_stage_repage_gather_routed_anypage_streamed(arr, len(srcs), src_page_size, C.byref(dst), dst_num_heads,
+                                                                                dst_page_size, C.cast(_route_seqs(seqs), C.c_void_p),
+                                                                                len(seqs), units or None, num_units, layer_begin, layer_end,
+                                                                                src_row_bytes, int(cast_mode), scales_ptr(cast_scales),
+                                                                                C.byref(st) if st is not None else None, stream)
 
 
 def permute_strides(kv_layout: int, num_layers: int, outer_dim: int, num_heads: int, page_size: int, row_bytes: int,

@@ -275,7 +275,8 @@ EXPORTED_SYMBOLS = [
     "kvbm_manager_execute_repage_batch", "kvbm_tp_pp_scatter_plan", "kvbm_manager_execute_repage_scatter",
     "kvbm_manager_execute_repage_scatter_streamed", "kvbm_manager_execute_repage_scatter_batch",
     "kvbm_manager_execute_repage_scatter_routed", "kvbm_manager_execute_repage_batch_routed", "kvbm_manager_execute_repage_anypage",
-    "kvbm_manager_execute_repage_scatter_anypage",
+    "kvbm_manager_execute_repage_scatter_anypage", "kvbm_manager_execute_repage_scatter_routed_anypage",
+    "kvbm_manager_execute_repage_batch_routed_anypage",
 ]
 
 
@@ -341,6 +342,7 @@ def lib() -> C.CDLL:
         L.kvbm_manager_execute_repage_anypage.argtypes = L.kvbm_manager_execute_repage_batch.argtypes
         L.kvbm_manager_execute_repage_batch_routed.argtypes = [vp, sz, P(u64), u64, P(_CRepageRouteSeq), sz, P(_CShardWindow), sz,
                                                                P(_CLayerStream), P(_COptions), P(u64)]
+        L.kvbm_manager_execute_repage_batch_routed_anypage.argtypes = L.kvbm_manager_execute_repage_batch_routed.argtypes
         L.kvbm_tp_pp_scatter_plan.argtypes = [sz, sz, sz, sz, P(sz), sz, sz, P(sz), sz, P(_CScatterWindow), sz, P(sz)]
         L.kvbm_manager_execute_repage_scatter.argtypes = [vp, u64, vp, sz, sz, P(u64), P(P(sz)), sz, sz, sz, P(_CScatterWindow), sz,
                                                           P(_COptions), P(u64)]
@@ -351,6 +353,7 @@ def lib() -> C.CDLL:
         L.kvbm_manager_execute_repage_scatter_anypage.argtypes = L.kvbm_manager_execute_repage_scatter_batch.argtypes
         L.kvbm_manager_execute_repage_scatter_routed.argtypes = [vp, u64, sz, P(u64), P(_CScatterRouteSeq), sz, P(_CScatterWindow), sz,
                                                                  P(_CLayerStream), P(_COptions), P(u64)]
+        L.kvbm_manager_execute_repage_scatter_routed_anypage.argtypes = L.kvbm_manager_execute_repage_scatter_routed.argtypes
         L.kvbm_notification_is_complete.argtypes = [vp, u64]
         L.kvbm_notification_wait.argtypes = [vp, u64, C.c_int64]
         L.kvbm_manager_bytes_moved.argtypes = [vp]
@@ -978,6 +981,22 @@ class TransferManager:
         its own sources' windows only; windows of one stage may write the same destination heads as long as no sequence is routed
         to two of them.  One staged copy, one launch, one notification; with `ready_flags` (source rank -> flags) it streams as
         `execute_repage_batch` does, and only the sources some sequence names are waited on."""
+        return self._repage_batch_routed(lib().kvbm_manager_execute_repage_batch_routed, sources, dst, seqs, plan, options, ready_flags,
+                                         layer_done_flags, num_layers)
+
+    def execute_repage_batch_routed_anypage(self, sources: Mapping[int, int], dst: int, seqs: Sequence[tuple], plan: Sequence[ShardWindow],
+                                            options: Optional[TransferOptions] = None, ready_flags: Optional[Mapping[int, int]] = None,
+                                            layer_done_flags: int = 0, num_layers: Optional[int] = None) -> TransferCompleteNotification:
+        """`execute_repage_batch_routed` between engines whose page sizes need not divide each other
+        (kvbm_manager_execute_repage_batch_routed_anypage), e.g. a decode step pulling each sequence from the hybrid prefill worker
+        (544-token blocks) that served it into 64-token pages: the same arguments, plans, errors and streaming.  Pages past the
+        exactness bound (big + small - gcd) * small < 2^32 raise UNSUPPORTED.  With dividing pages the destination bytes are
+        `execute_repage_batch_routed`'s."""
+        return self._repage_batch_routed(lib().kvbm_manager_execute_repage_batch_routed_anypage, sources, dst, seqs, plan, options,
+                                         ready_flags, layer_done_flags, num_layers)
+
+    def _repage_batch_routed(self, entry, sources, dst, seqs, plan, options, ready_flags, layer_done_flags, num_layers):
+        """The body of `execute_repage_batch_routed` and `execute_repage_batch_routed_anypage`: `entry` is the C entry they call."""
         if plan and isinstance(plan[0], HeadWindow):
             if num_layers is None:
                 raise ValueError("a HeadWindow plan needs num_layers, the destination's layer count")
@@ -1006,8 +1025,8 @@ class TransferManager:
         ls = self._layer_stream(ranks, ready_flags, layer_done_flags) if ready_flags is not None else None
         tok = C.c_uint64()
         o = (options or TransferOptions())._c()
-        _check(lib().kvbm_manager_execute_repage_batch_routed(self._h, len(ranks), hs, dst, cs, len(seqs), ws, len(plan),
-                                                              C.byref(ls) if ls is not None else None, C.byref(o), C.byref(tok)))
+        _check(entry(self._h, len(ranks), hs, dst, cs, len(seqs), ws, len(plan), C.byref(ls) if ls is not None else None, C.byref(o),
+                     C.byref(tok)))
         return TransferCompleteNotification(self, tok.value)
 
     def execute_repage_scatter(self, src: int, src_block_ids: Sequence[int], dsts: Sequence[int], dst_block_ids: Sequence[Sequence[int]],
@@ -1095,6 +1114,23 @@ class TransferManager:
         `options.per_dst_done_flags` and `options.done_flag` are written once, after every sequence landed.  With `ready_flags` it
         streams as `execute_repage_scatter_batch` does.  A destination block may appear once per destination among the sequences
         routed to it."""
+        return self._repage_scatter_routed(lib().kvbm_manager_execute_repage_scatter_routed, src, dsts, seqs, plan, options, ready_flags,
+                                           layer_done_flags)
+
+    def execute_repage_scatter_routed_anypage(self, src: int, dsts: Sequence[int], seqs: Sequence[tuple], plan: Sequence[ScatterWindow],
+                                              options: Optional[TransferOptions] = None, ready_flags: Optional[int] = None,
+                                              layer_done_flags: int = 0) -> TransferCompleteNotification:
+        """`execute_repage_scatter_routed` between engines whose page sizes need not divide each other
+        (kvbm_manager_execute_repage_scatter_routed_anypage), e.g. a hybrid prefill pool's 544-token blocks pushed to several decode
+        workers with 64-token pages, each sequence to its own worker: the same arguments, plans, errors and streaming.  Pages past
+        the exactness bound (big + small - gcd) * small < 2^32 raise UNSUPPORTED.  With dividing pages the destination bytes are
+        `execute_repage_scatter_routed`'s."""
+        return self._repage_scatter_routed(lib().kvbm_manager_execute_repage_scatter_routed_anypage, src, dsts, seqs, plan, options,
+                                           ready_flags, layer_done_flags)
+
+    def _repage_scatter_routed(self, entry, src, dsts, seqs, plan, options, ready_flags, layer_done_flags):
+        """The body of `execute_repage_scatter_routed` and `execute_repage_scatter_routed_anypage`: `entry` is the C entry they
+        call."""
         keep, cs = [], (_CScatterRouteSeq * max(1, len(seqs)))()
         for c, (tokens, src_ids, routed) in zip(cs, seqs):
             if tokens.step != 1:
@@ -1120,8 +1156,8 @@ class TransferManager:
         ls = self._layer_stream([0], {0: ready_flags}, layer_done_flags) if ready_flags is not None else None
         tok = C.c_uint64()
         o = (options or TransferOptions())._c()
-        _check(lib().kvbm_manager_execute_repage_scatter_routed(self._h, src, len(dsts), hs, cs, len(seqs), ws, len(plan),
-                                                                C.byref(ls) if ls is not None else None, C.byref(o), C.byref(tok)))
+        _check(entry(self._h, src, len(dsts), hs, cs, len(seqs), ws, len(plan), C.byref(ls) if ls is not None else None, C.byref(o),
+                     C.byref(tok)))
         return TransferCompleteNotification(self, tok.value)
 
     @staticmethod

@@ -773,6 +773,81 @@ cudaError_t kvbm_kernels_paged_repage_scatter_anypage_streamed(const kvbm_permut
                                                                int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
                                                                const kvbm_permute_stream* st, cudaStream_t stream);
 
+/* ---- routed re-paging between pages that need not divide: each sequence to or from its own workers, any two page sizes -------
+ * A hybrid-attention prefill pool (544-token blocks) in front of several decode workers with 64-token pages mixes requests of
+ * those workers in one batch: the routed entries' masks and the anypage entries' phases in one launch.  Both fit the one 16 B
+ * record.  A kernel entry rejects mask bits at or above its rank count, at most KVBM_GATHER_MAX_SOURCES = 16, so a mask needs 16
+ * bits; the phase is below the small page, and the exactness bound with big >= small >= gcd gives small^2 < 2^32, so
+ * small <= 65535 and phase <= 65534 also need 16 bits. */
+
+/* kvbm_route_unit for pages that need not divide: route = targets | phase << 16 (targets: the sequence's mask, below 2^16;
+ * phase: kvbm_repage_anypage_unit's). */
+typedef struct kvbm_route_anypage_unit {
+  uint32_t q0, tokens, small_k, route;
+} kvbm_route_anypage_unit;
+
+/* Host-only (no GPU): kvbm_kernels_repage_anypage_units over the ranges of seqs, with the same rules, counts, sizing call and
+ * small_k wrap, each record's fourth word packing its sequence's targets (low 16 bits) with its phase (high 16 bits).  For
+ * dividing pages its records are kvbm_kernels_repage_route_units', byte for byte; route >> 16 is kvbm_kernels_repage_anypage_units'
+ * phase and route & 0xFFFF the mask.  Returns non-zero, writing nothing, for every rule of kvbm_kernels_repage_anypage_units and a
+ * mask with a bit at or above 16. */
+int kvbm_kernels_repage_route_anypage_units(const kvbm_route_seq* seqs, size_t num_seqs, uint32_t src_page_size,
+                                            uint32_t dst_page_size, kvbm_route_anypage_unit* out, size_t cap,
+                                            size_t* num_units, size_t* src_ids, size_t* dst_ids);
+
+/* kvbm_kernels_paged_repage_scatter_routed for any two non-zero pages: the same parameters, with `units` the device-accessible table
+ * kvbm_kernels_repage_route_anypage_units(seqs, Ps, Pd) produced.  Every rule, flag convention and error order is the routed
+ * scatter's (a sequence whose targets is 0 or has a bit at or above num_targets is rejected), except that the pages need only the
+ * exactness bound.  Equivalences: with every mask all num_targets bits, the bytes of kvbm_kernels_paged_repage_scatter_anypage;
+ * with dividing pages, the bytes of kvbm_kernels_paged_repage_scatter_routed; with one target per sequence, the bytes of one
+ * kvbm_kernels_paged_repage_scatter_anypage launch per target over the sequences routed to it. */
+cudaError_t kvbm_kernels_paged_repage_scatter_routed_anypage(const kvbm_permute_side* src, uint32_t src_num_heads, uint32_t src_page_size,
+                                                             const kvbm_scatter_target* targets, int num_targets, uint32_t dst_page_size,
+                                                             const kvbm_route_seq* seqs, size_t num_seqs, const kvbm_route_anypage_unit* units,
+                                                             size_t num_units, int layer_begin, int layer_end, uint32_t src_row_bytes,
+                                                             int cast_mode, const float* cast_scales, uint32_t epoch,
+                                                             uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream);
+
+/* kvbm_kernels_paged_repage_scatter_routed_anypage streamed with kvbm_kernels_paged_repage_scatter_routed_streamed's flag
+ * conventions and gate forms: layer_done_flags[l] is written once source layer l of every sequence landed in every target it is
+ * routed to, and after a gate timeout no done flag is written and completion_flag becomes 0xFFFFFFFF.  The stream-wait form
+ * launches the unstreamed entry per source layer.  The argument rules are the unstreamed entry's plus the gate's with one source. */
+cudaError_t kvbm_kernels_paged_repage_scatter_routed_anypage_streamed(const kvbm_permute_side* src, uint32_t src_num_heads,
+                                                                      uint32_t src_page_size, const kvbm_scatter_target* targets,
+                                                                      int num_targets, uint32_t dst_page_size, const kvbm_route_seq* seqs,
+                                                                      size_t num_seqs, const kvbm_route_anypage_unit* units,
+                                                                      size_t num_units, int layer_begin, int layer_end,
+                                                                      uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
+                                                                      const kvbm_permute_stream* st, cudaStream_t stream);
+
+/* kvbm_kernels_paged_stage_repage_gather_routed for any two non-zero pages: the same parameters, with `units` the
+ * device-accessible table kvbm_kernels_repage_route_anypage_units(seqs, Ps, Pd) produced.  Every rule and error order is the
+ * routed gather's (a mask of 0 or with a bit at or above num_srcs is rejected; two windows of one stage may share destination
+ * heads when no mask holds both), except that the pages need only the exactness bound.  Equivalences: with every mask all
+ * num_srcs bits, the bytes of kvbm_kernels_paged_stage_repage_gather_anypage; with dividing pages, the bytes of
+ * kvbm_kernels_paged_stage_repage_gather_routed; with one source per sequence, the bytes of one
+ * kvbm_kernels_paged_stage_repage_gather_anypage launch per source over the sequences routed to it. */
+cudaError_t kvbm_kernels_paged_stage_repage_gather_routed_anypage(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page_size,
+                                                                  const kvbm_permute_side* dst, uint32_t dst_num_heads,
+                                                                  uint32_t dst_page_size, const kvbm_route_seq* seqs, size_t num_seqs,
+                                                                  const kvbm_route_anypage_unit* units, size_t num_units, int layer_begin,
+                                                                  int layer_end, uint32_t src_row_bytes, int cast_mode,
+                                                                  const float* cast_scales, uint32_t* done_flag, uint32_t epoch,
+                                                                  uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream);
+
+/* kvbm_kernels_paged_stage_repage_gather_routed_anypage streamed with kvbm_kernels_paged_stage_repage_gather_routed_streamed's flag
+ * conventions and gate forms: only the sources some sequence is routed to are waited on and need st->layer_ready_flags[s]; after a
+ * gate timeout no done flag is written and completion_flag becomes 0xFFFFFFFF.  The stream-wait form launches the unstreamed entry
+ * per layer.  The argument rules are the unstreamed entry's plus the gate's. */
+cudaError_t kvbm_kernels_paged_stage_repage_gather_routed_anypage_streamed(const kvbm_stage_source* srcs, int num_srcs,
+                                                                           uint32_t src_page_size, const kvbm_permute_side* dst,
+                                                                           uint32_t dst_num_heads, uint32_t dst_page_size,
+                                                                           const kvbm_route_seq* seqs, size_t num_seqs,
+                                                                           const kvbm_route_anypage_unit* units, size_t num_units,
+                                                                           int layer_begin, int layer_end, uint32_t src_row_bytes,
+                                                                           int cast_mode, const float* cast_scales,
+                                                                           const kvbm_permute_stream* st, cudaStream_t stream);
+
 /* Host-only (no GPU): the stride table kvbm_kernels_paged_permute walks with for one side.  out[0] = 1 when offsets count
  * from the block's first byte (universal formats) or 0 when they count from the (layer, outer) region's first byte; the
  * element (layer l, outer o, head h, token t) then sits at  [out[0] ? l * out[1] + o * out[2] : 0] + h * out[3] + t * out[4].

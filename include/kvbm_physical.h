@@ -622,6 +622,28 @@ int kvbm_manager_execute_repage_scatter_routed(kvbm_transfer_manager* m, kvbm_la
                                                size_t num_windows, const kvbm_layer_stream* ls, const kvbm_transfer_options* opts,
                                                kvbm_notification* out);
 
+/* kvbm_manager_execute_repage_scatter_routed between engines whose page sizes need not divide each other (a hybrid prefill pool's
+ * 544-token blocks pushed to several decode workers with 64-token pages), through kvbm_kernels_paged_repage_scatter_routed_anypage,
+ * or its streamed form with ls.  The arguments, plans, routing, errors, codes, texts and their order are
+ * kvbm_manager_execute_repage_scatter_routed's, but for each window's page rule: "one page size divides the other" is not asked,
+ * and pages past the exactness bound, (big + small - gcd) * small < 2^32, fail with KVBM_ERR_UNSUPPORTED and
+ * kvbm_manager_execute_repage_anypage's text.  The staged unit table is kvbm_kernels_repage_route_anypage_units' over each
+ * non-empty sequence's range and window mask.  With dividing pages the destination bytes are the routed scatter's. */
+int kvbm_manager_execute_repage_scatter_routed_anypage(kvbm_transfer_manager* m, kvbm_layout_handle src, size_t num_dsts,
+                                                       const kvbm_layout_handle* dsts, const kvbm_scatter_route_seq* seqs, size_t num_seqs,
+                                                       const kvbm_scatter_window* windows, size_t num_windows, const kvbm_layer_stream* ls,
+                                                       const kvbm_transfer_options* opts, kvbm_notification* out);
+
+/* kvbm_manager_execute_repage_batch_routed between engines whose page sizes need not divide each other, through
+ * kvbm_kernels_paged_stage_repage_gather_routed_anypage, or its streamed form with ls.  The arguments, plans, routing, errors,
+ * codes, texts and their order are kvbm_manager_execute_repage_batch_routed's, but for each window's page rule, which is
+ * kvbm_manager_execute_repage_anypage's: pages past the exactness bound fail with KVBM_ERR_UNSUPPORTED and its text.  With dividing
+ * pages the destination bytes are the routed gather's. */
+int kvbm_manager_execute_repage_batch_routed_anypage(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs,
+                                                     kvbm_layout_handle dst, const kvbm_repage_route_seq* seqs, size_t num_seqs,
+                                                     const kvbm_shard_window* windows, size_t num_windows, const kvbm_layer_stream* ls,
+                                                     const kvbm_transfer_options* opts, kvbm_notification* out);
+
 /* Completion: the transfer's last warp writes a flag in pinned host memory (no cudaEventQuery polling). */
 int kvbm_notification_is_complete(kvbm_transfer_manager* m, kvbm_notification n);  /* 1 / 0 / <0 error */
 int kvbm_notification_wait(kvbm_transfer_manager* m, kvbm_notification n, int64_t timeout_us);
