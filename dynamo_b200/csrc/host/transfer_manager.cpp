@@ -1475,16 +1475,21 @@ struct BatchTables {
   std::vector<const size_t*> lists;
 };
 
+// What a re-paging request's units are, as the kernel library's re-paging launches take them: the single entries' one token
+// range, or a batch of sequences whose unit table's fourth word is each unit's sequence index (kSeqs), its sequence's window mask
+// (kRouted), its phase where pages need not divide (kPhased), or both (kRoutedPhased).  Each batch kind has its own unit table
+// helper and kernel entries.
+enum RepageUnits { kRange, kSeqs, kRouted, kPhased, kRoutedPhased };
+static bool phased_units(RepageUnits k) { return k == kPhased || k == kRoutedPhased; }
+
 // List k of sequence q is ids(q, k): q.n_src ids for k < num_src_lists, else q.n_dst.  check(t->cat), the caller's duplicate-id
-// checks, runs before the unit table.  *n_src / *n_dst: each concatenated source and destination table's length.  anypage: the
-// unit table is kvbm_kernels_repage_anypage_units' (the same 16 B records, the phase in the fourth word).  routes (with anypage):
-// each non-empty sequence's range and window mask, in t->ranges' order; the unit table is then
-// kvbm_kernels_repage_route_anypage_units', whose fourth word packs the mask with the phase, so that no sequence index survives in
-// it to be rewritten.
+// checks, runs before the unit table, which the helper of `units` writes (the same 16 B records for every kind).  routes (a
+// routed kind): each non-empty sequence's range and window mask, in t->ranges' order.  *n_src / *n_dst: each concatenated source
+// and destination table's length.
 template <class Seq, class Ids, class Check>
 static int batch_tables(const Seq* seqs, size_t num_seqs, const std::vector<bool>& used, size_t num_src_lists, uint32_t ps, uint32_t pd,
-                        Ids ids, Check check, BatchTables* t, size_t* n_src, size_t* n_dst, bool anypage = false,
-                        const kvbm_route_seq* routes = nullptr)
+                        Ids ids, Check check, BatchTables* t, size_t* n_src, size_t* n_dst, RepageUnits units,
+                        const kvbm_route_seq* routes)
 {
   t->cat.resize(used.size());
   for (size_t i = 0; i < num_seqs; ++i) {
@@ -1495,20 +1500,28 @@ static int batch_tables(const Seq* seqs, size_t num_seqs, const std::vector<bool
       if (used[k]) t->cat[k].insert(t->cat[k].end(), ids(q, k), ids(q, k) + (k < num_src_lists ? q.n_src : q.n_dst));
   }
   if (int rc = check(t->cat)) return rc;
-  static_assert(sizeof(kvbm_repage_anypage_unit) == sizeof(kvbm_repage_unit) && sizeof(kvbm_route_anypage_unit) == sizeof(kvbm_repage_unit),
+  static_assert(sizeof(kvbm_route_unit) == sizeof(kvbm_repage_unit) && sizeof(kvbm_repage_anypage_unit) == sizeof(kvbm_repage_unit) &&
+                    sizeof(kvbm_route_anypage_unit) == sizeof(kvbm_repage_unit),
                 "one staged record layout");
-  auto units = [&](kvbm_repage_unit* out, size_t cap, size_t* num_units) {
-    if (anypage && routes)
-      return kvbm_kernels_repage_route_anypage_units(routes, t->ranges.size(), ps, pd, reinterpret_cast<kvbm_route_anypage_unit*>(out), cap,
-                                                     num_units, n_src, n_dst);
-    return anypage ? kvbm_kernels_repage_anypage_units(t->ranges.data(), t->ranges.size(), ps, pd, reinterpret_cast<kvbm_repage_anypage_unit*>(out),
-                                                       cap, num_units, n_src, n_dst)
-                   : kvbm_kernels_repage_batch_units(t->ranges.data(), t->ranges.size(), ps, pd, out, cap, num_units, n_src, n_dst);
+  auto write = [&](kvbm_repage_unit* out, size_t cap, size_t* num_units) {
+    const size_t n = t->ranges.size();
+    switch (units) {
+      case kRouted:
+        return kvbm_kernels_repage_route_units(routes, n, ps, pd, reinterpret_cast<kvbm_route_unit*>(out), cap, num_units, n_src, n_dst);
+      case kPhased:
+        return kvbm_kernels_repage_anypage_units(t->ranges.data(), n, ps, pd, reinterpret_cast<kvbm_repage_anypage_unit*>(out), cap, num_units,
+                                                 n_src, n_dst);
+      case kRoutedPhased:
+        return kvbm_kernels_repage_route_anypage_units(routes, n, ps, pd, reinterpret_cast<kvbm_route_anypage_unit*>(out), cap, num_units,
+                                                       n_src, n_dst);
+      default:
+        return kvbm_kernels_repage_batch_units(t->ranges.data(), n, ps, pd, out, cap, num_units, n_src, n_dst);
+    }
   };
   size_t num_units = 0;
-  if (units(nullptr, 0, &num_units)) return fail(KVBM_ERR, "the batch's token ranges and page sizes have no unit table");
+  if (write(nullptr, 0, &num_units)) return fail(KVBM_ERR, "the batch's token ranges and page sizes have no unit table");
   t->units.resize(num_units);
-  units(t->units.data(), t->units.size(), &num_units);
+  write(t->units.data(), t->units.size(), &num_units);
   for (size_t k = 0; k < used.size(); ++k) t->lists.push_back(used[k] ? t->cat[k].data() : nullptr);
   return KVBM_OK;
 }
@@ -1517,21 +1530,22 @@ static int batch_tables(const Seq* seqs, size_t num_seqs, const std::vector<bool
 // pass their one range as one sequence, kvbm_manager_execute_repage_batch its list (`batch`).  Every sequence is checked in
 // turn and the first rejected one returns its code and text; an empty one moves nothing.  Then a batch's concatenated tables
 // are checked for a destination block named twice, and one slot takes every table (and a batch's unit table) in one copy, and
-// one launch moves every sequence: through the _batch kernel entries for a batch, else the single range's.
+// one launch moves every sequence: through the batch kind's kernel entries for a batch (units other than kRange), else the
+// single range's.
 // masks: a routed batch (kvbm_manager_execute_repage_batch_routed), sequence i read from the sources of masks[i] only: the
 // windows of a stage may share destination heads, the routing checks run after the null sequence list, each sequence's routed id
 // lists alone are checked, the destination's ids are checked against the ids of the sequences routed to a source in its
 // layout, unrouted positions of the staged tables are padded with block 0, and the unit table carries each sequence's window
-// mask for the routed kernel entries.
-// anypage: a batch whose pages need not divide (kvbm_manager_execute_repage_anypage): check_repage_pair's anypage rule, the unit
-// table of kvbm_kernels_repage_anypage_units, and the anypage kernel entries.  Both (kvbm_manager_execute_repage_batch_routed_anypage):
-// the routed batch's checks, the unit table of kvbm_kernels_repage_route_anypage_units, and the routed anypage kernel entries.
+// mask for the routed kernel entries (kRouted, or kRoutedPhased with pages that need not divide).
+// A phased kind (kvbm_manager_execute_repage_anypage, kvbm_manager_execute_repage_batch_routed_anypage): check_repage_pair's
+// anypage rule.
 static int execute_repage(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, kvbm_layout_handle dst_h,
                           const kvbm_repage_batch_seq* seqs, size_t num_seqs, const kvbm_head_window* windows, size_t nw,
                           const kvbm_transfer_options* opts_in, kvbm_notification* out, const kvbm_layer_stream* ls = nullptr,
-                          bool gather = true, const kvbm_shard_window* layers = nullptr, bool batch = false, const uint32_t* masks = nullptr,
-                          bool anypage = false)
+                          bool gather = true, const kvbm_shard_window* layers = nullptr, RepageUnits units = kRange,
+                          const uint32_t* masks = nullptr)
 {
+  const bool batch = units != kRange;
   kvbm_transfer_options o{};
   if (opts_in) o = *opts_in;
   if (out) *out = 0;
@@ -1583,7 +1597,7 @@ static int execute_repage(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_
     const kvbm_repage_batch_seq& q = seqs[i];
     const uint32_t* mask = masks ? masks + i : nullptr;
     if ((rc = check_repage_request(m, num_srcs, srcs, q.src_ids, q.n_src, dst_h, q.dst_ids, q.n_dst, q.token_begin, q.token_end, windows, nw, o,
-                                   ls, gather, layers, &R, mask, anypage)))
+                                   ls, gather, layers, &R, mask, phased_units(units))))
       return rc;
     if (R.empty) continue;
     any = true;
@@ -1634,17 +1648,14 @@ static int execute_repage(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_
       }
       return KVBM_OK;
     };
-    // each non-empty sequence's range with its window mask, which replaces the unit's sequence index (or joins the phase)
+    // each non-empty sequence's range with its window mask, which the routed unit table carries
     for (size_t i = 0; masks && i < num_seqs; ++i)
       if (seqs[i].token_begin != seqs[i].token_end)
         routes.push_back(kvbm_route_seq{static_cast<uint32_t>(seqs[i].token_begin), static_cast<uint32_t>(seqs[i].token_end), window_mask(i)});
-    if ((rc = batch_tables(seqs, num_seqs, used, num_srcs, ups, upd, ids, unique, &bt, &n_src, &n_dst, anypage,
-                           masks ? routes.data() : nullptr)))
+    if ((rc = batch_tables(seqs, num_seqs, used, num_srcs, ups, upd, ids, unique, &bt, &n_src, &n_dst, units, routes.data())))
       return rc;
     src_ids = bt.lists.data();
     dst_ids = bt.lists[num_srcs];
-    if (masks && !anypage)
-      for (kvbm_repage_unit& u : bt.units) u.seq = routes[u.seq].targets;
   }
 
   DeviceGuard g(m->device);
@@ -1661,49 +1672,35 @@ static int execute_repage(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_
                      "kvbm_kernels_paged_repage");
     kvbm_stage_source ss[KVBM_GATHER_MAX_SOURCES] = {};
     stage_sources(ks, layers, nw, D->cfg.num_layers, ss);
-    if (batch) {
-      const auto* du = reinterpret_cast<const kvbm_repage_unit*>(sl.dev_ids + units_at(num_srcs * n_src + n_dst));
-      const auto* dr = reinterpret_cast<const kvbm_route_unit*>(du);
-      const auto* da = reinterpret_cast<const kvbm_repage_anypage_unit*>(du);
-      const auto* dra = reinterpret_cast<const kvbm_route_anypage_unit*>(du);
-      if (masks && anypage && st)
-        return checked(kvbm_kernels_paged_stage_repage_gather_routed_anypage_streamed(ss, k, ups, &kd, dnh, upd, routes.data(), routes.size(), dra,
-                                                                                      bt.units.size(), ilb, ile, row, o.cast_mode, o.cast_scales,
-                                                                                      st, stream),
-                       "kvbm_kernels_paged_stage_repage_gather_routed_anypage_streamed");
-      if (masks && anypage)
-        return checked(kvbm_kernels_paged_stage_repage_gather_routed_anypage(ss, k, ups, &kd, dnh, upd, routes.data(), routes.size(), dra,
-                                                                             bt.units.size(), ilb, ile, row, o.cast_mode, o.cast_scales,
-                                                                             o.done_flag, o.epoch, sl.host_flag, value, stream),
-                       "kvbm_kernels_paged_stage_repage_gather_routed_anypage");
-      if (anypage && st)
-        return checked(kvbm_kernels_paged_stage_repage_gather_anypage_streamed(ss, k, ups, &kd, dnh, upd, bt.ranges.data(), bt.ranges.size(), da,
-                                                                               bt.units.size(), ilb, ile, row, o.cast_mode, o.cast_scales, st,
-                                                                               stream),
-                       "kvbm_kernels_paged_stage_repage_gather_anypage_streamed");
-      if (anypage)
-        return checked(kvbm_kernels_paged_stage_repage_gather_anypage(ss, k, ups, &kd, dnh, upd, bt.ranges.data(), bt.ranges.size(), da,
-                                                                      bt.units.size(), ilb, ile, row, o.cast_mode, o.cast_scales, o.done_flag,
-                                                                      o.epoch, sl.host_flag, value, stream),
-                       "kvbm_kernels_paged_stage_repage_gather_anypage");
-      if (masks && st)
-        return checked(kvbm_kernels_paged_stage_repage_gather_routed_streamed(ss, k, ups, &kd, dnh, upd, routes.data(), routes.size(), dr,
-                                                                              bt.units.size(), ilb, ile, row, o.cast_mode, o.cast_scales, st,
-                                                                              stream),
-                       "kvbm_kernels_paged_stage_repage_gather_routed_streamed");
-      if (masks)
-        return checked(kvbm_kernels_paged_stage_repage_gather_routed(ss, k, ups, &kd, dnh, upd, routes.data(), routes.size(), dr, bt.units.size(),
-                                                                     ilb, ile, row, o.cast_mode, o.cast_scales, o.done_flag, o.epoch, sl.host_flag,
-                                                                     value, stream),
-                       "kvbm_kernels_paged_stage_repage_gather_routed");
+    // a batch: its kind's entry, streamed or not
+    const int32_t* du = sl.dev_ids + units_at(num_srcs * n_src + n_dst);
+    auto run = [&](auto entry, auto streamed_entry, const char* name, const char* streamed_name, const auto* qs, size_t n, const auto* t) {
       if (st)
-        return checked(kvbm_kernels_paged_stage_repage_gather_batch_streamed(ss, k, ups, &kd, dnh, upd, bt.ranges.data(), bt.ranges.size(), du,
-                                                                             bt.units.size(), ilb, ile, row, o.cast_mode, o.cast_scales, st, stream),
-                       "kvbm_kernels_paged_stage_repage_gather_batch_streamed");
-      return checked(kvbm_kernels_paged_stage_repage_gather_batch(ss, k, ups, &kd, dnh, upd, bt.ranges.data(), bt.ranges.size(), du, bt.units.size(), ilb,
-                                                                  ile, row, o.cast_mode, o.cast_scales, o.done_flag, o.epoch, sl.host_flag, value,
-                                                                  stream),
-                     "kvbm_kernels_paged_stage_repage_gather_batch");
+        return checked(streamed_entry(ss, k, ups, &kd, dnh, upd, qs, n, t, bt.units.size(), ilb, ile, row, o.cast_mode, o.cast_scales, st, stream),
+                       streamed_name);
+      return checked(entry(ss, k, ups, &kd, dnh, upd, qs, n, t, bt.units.size(), ilb, ile, row, o.cast_mode, o.cast_scales, o.done_flag, o.epoch,
+                           sl.host_flag, value, stream),
+                     name);
+    };
+    switch (units) {
+      case kSeqs:
+        return run(kvbm_kernels_paged_stage_repage_gather_batch, kvbm_kernels_paged_stage_repage_gather_batch_streamed,
+                   "kvbm_kernels_paged_stage_repage_gather_batch", "kvbm_kernels_paged_stage_repage_gather_batch_streamed", bt.ranges.data(),
+                   bt.ranges.size(), reinterpret_cast<const kvbm_repage_unit*>(du));
+      case kRouted:
+        return run(kvbm_kernels_paged_stage_repage_gather_routed, kvbm_kernels_paged_stage_repage_gather_routed_streamed,
+                   "kvbm_kernels_paged_stage_repage_gather_routed", "kvbm_kernels_paged_stage_repage_gather_routed_streamed", routes.data(),
+                   routes.size(), reinterpret_cast<const kvbm_route_unit*>(du));
+      case kPhased:
+        return run(kvbm_kernels_paged_stage_repage_gather_anypage, kvbm_kernels_paged_stage_repage_gather_anypage_streamed,
+                   "kvbm_kernels_paged_stage_repage_gather_anypage", "kvbm_kernels_paged_stage_repage_gather_anypage_streamed",
+                   bt.ranges.data(), bt.ranges.size(), reinterpret_cast<const kvbm_repage_anypage_unit*>(du));
+      case kRoutedPhased:
+        return run(kvbm_kernels_paged_stage_repage_gather_routed_anypage, kvbm_kernels_paged_stage_repage_gather_routed_anypage_streamed,
+                   "kvbm_kernels_paged_stage_repage_gather_routed_anypage", "kvbm_kernels_paged_stage_repage_gather_routed_anypage_streamed",
+                   routes.data(), routes.size(), reinterpret_cast<const kvbm_route_anypage_unit*>(du));
+      case kRange:
+        break;
     }
     if (st)
       return checked(kvbm_kernels_paged_stage_repage_gather_streamed(ss, k, ups, &kd, dnh, upd, utb, ute, ilb, ile, row, o.cast_mode,
@@ -1822,16 +1819,15 @@ static int check_scatter_request(kvbm_transfer_manager* m, kvbm_layout_handle sr
 // masks: a routed batch (kvbm_manager_execute_repage_scatter_routed), sequence i going to the destinations of masks[i] only: the
 // routing checks run after the windows', each sequence's routed id lists alone are checked, the uniqueness per destination runs
 // over its routed sequences, unrouted positions of the staged tables are padded with block 0, and the unit table carries each
-// sequence's window mask for the routed kernel entries.
-// anypage: a batch whose pages need not divide (kvbm_manager_execute_repage_scatter_anypage): check_repage_pair's anypage rule,
-// the unit table of kvbm_kernels_repage_anypage_units, and the anypage scatter entries.  Both
-// (kvbm_manager_execute_repage_scatter_routed_anypage): the routed batch's checks, the unit table of
-// kvbm_kernels_repage_route_anypage_units, and the routed anypage scatter entries.
+// sequence's window mask for the routed kernel entries (kRouted, or kRoutedPhased with pages that need not divide).
+// A phased kind (kvbm_manager_execute_repage_scatter_anypage, kvbm_manager_execute_repage_scatter_routed_anypage):
+// check_repage_pair's anypage rule.  units: as execute_repage's.
 static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle src_h, size_t num_dsts, const kvbm_layout_handle* dsts,
                                   const kvbm_scatter_batch_seq* seqs, size_t num_seqs, const kvbm_scatter_window* w, size_t nw,
                                   const kvbm_transfer_options* opts_in, kvbm_notification* out, const kvbm_layer_stream* ls = nullptr,
-                                  bool batch = false, const uint32_t* masks = nullptr, bool anypage = false)
+                                  RepageUnits units = kRange, const uint32_t* masks = nullptr)
 {
+  const bool batch = units != kRange;
   kvbm_transfer_options o{};
   if (opts_in) o = *opts_in;
   if (out) *out = 0;
@@ -1859,7 +1855,7 @@ static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle s
   for (size_t i = 0; i < num_seqs; ++i) {
     const kvbm_scatter_batch_seq& q = seqs[i];
     const uint32_t* mask = masks ? masks + i : nullptr;
-    if ((rc = check_scatter_request(m, src_h, q, num_dsts, dsts, w, nw, o, ls, &R, mask, anypage))) return rc;
+    if ((rc = check_scatter_request(m, src_h, q, num_dsts, dsts, w, nw, o, ls, &R, mask, phased_units(units)))) return rc;
     if (R.empty) continue;
     any = true;
     // what lands: each routed window's destination bytes over its layers inside the range
@@ -1910,19 +1906,16 @@ static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle s
       }
       return KVBM_OK;
     };
-    // each non-empty sequence's range with its window mask, which replaces the unit's sequence index (or joins the phase)
+    // each non-empty sequence's range with its window mask, which the routed unit table carries
     for (size_t i = 0; masks && i < num_seqs; ++i) {
       if (seqs[i].token_begin == seqs[i].token_end) continue;
       uint32_t targets = 0;
       for (size_t j = 0; j < nw; ++j) targets |= static_cast<uint32_t>(routed_to(masks + i, w[j].dst_rank)) << j;
       routes.push_back(kvbm_route_seq{static_cast<uint32_t>(seqs[i].token_begin), static_cast<uint32_t>(seqs[i].token_end), targets});
     }
-    if ((rc = batch_tables(seqs, num_seqs, used, 1, ups, upd, ids, unique, &bt, &n_src, &n_dst, anypage, masks ? routes.data() : nullptr)))
-      return rc;
+    if ((rc = batch_tables(seqs, num_seqs, used, 1, ups, upd, ids, unique, &bt, &n_src, &n_dst, units, routes.data()))) return rc;
     src_ids = bt.lists[0];
     dst_ids = bt.lists.data() + 1;
-    if (masks && !anypage)
-      for (kvbm_repage_unit& u : bt.units) u.seq = routes[u.seq].targets;
   }
 
   DeviceGuard g(m->device);
@@ -1950,60 +1943,46 @@ static int execute_repage_scatter(kvbm_transfer_manager* m, kvbm_layout_handle s
   const uint32_t snh = static_cast<uint32_t>(S->cfg.num_heads);
   const uint32_t utb = static_cast<uint32_t>(seqs[0].token_begin), ute = static_cast<uint32_t>(seqs[0].token_end);
   const int k = static_cast<int>(nw), ilb = static_cast<int>(R.lb), ile = static_cast<int>(R.le);
-  const auto* du = reinterpret_cast<const kvbm_repage_unit*>(sl->dev_ids + units_at(n_src + num_dsts * n_dst));
-  const auto* dr = reinterpret_cast<const kvbm_route_unit*>(du);
-  const auto* da = reinterpret_cast<const kvbm_repage_anypage_unit*>(du);
-  const auto* dra = reinterpret_cast<const kvbm_route_anypage_unit*>(du);
-  if (ls) {
-    const kvbm_permute_stream st = layer_stream(*ls, e, 1, o, *sl, seq);
-    if (masks && anypage)
-      rc = checked(kvbm_kernels_paged_repage_scatter_routed_anypage_streamed(&ks, snh, ups, kt, k, upd, routes.data(), routes.size(), dra,
-                                                                             bt.units.size(), ilb, ile, row, o.cast_mode, o.cast_scales, &st,
-                                                                             stream),
-                   "kvbm_kernels_paged_repage_scatter_routed_anypage_streamed");
-    else if (anypage)
-      rc = checked(kvbm_kernels_paged_repage_scatter_anypage_streamed(&ks, snh, ups, kt, k, upd, bt.ranges.data(), bt.ranges.size(), da,
-                                                                      bt.units.size(), ilb, ile, row, o.cast_mode, o.cast_scales, &st, stream),
-                   "kvbm_kernels_paged_repage_scatter_anypage_streamed");
-    else if (masks)
-      rc = checked(kvbm_kernels_paged_repage_scatter_routed_streamed(&ks, snh, ups, kt, k, upd, routes.data(), routes.size(), dr, bt.units.size(),
-                                                                     ilb, ile, row, o.cast_mode, o.cast_scales, &st, stream),
-                   "kvbm_kernels_paged_repage_scatter_routed_streamed");
-    else if (batch)
-      rc = checked(kvbm_kernels_paged_repage_scatter_batch_streamed(&ks, snh, ups, kt, k, upd, bt.ranges.data(), bt.ranges.size(), du, bt.units.size(),
-                                                                    ilb, ile, row, o.cast_mode, o.cast_scales, &st, stream),
-                   "kvbm_kernels_paged_repage_scatter_batch_streamed");
-    else
-      rc = checked(kvbm_kernels_paged_repage_scatter_streamed(&ks, snh, ups, kt, k, upd, utb, ute, ilb, ile, row, o.cast_mode, o.cast_scales,
-                                                              &st, stream),
-                   "kvbm_kernels_paged_repage_scatter_streamed");
-  } else {
-    if (masks && anypage)
-      rc = checked(kvbm_kernels_paged_repage_scatter_routed_anypage(&ks, snh, ups, kt, k, upd, routes.data(), routes.size(), dra, bt.units.size(),
-                                                                    ilb, ile, row, o.cast_mode, o.cast_scales, o.epoch, sl->host_flag,
-                                                                    static_cast<uint32_t>(seq), stream),
-                   "kvbm_kernels_paged_repage_scatter_routed_anypage");
-    else if (anypage)
-      rc = checked(kvbm_kernels_paged_repage_scatter_anypage(&ks, snh, ups, kt, k, upd, bt.ranges.data(), bt.ranges.size(), da, bt.units.size(),
-                                                             ilb, ile, row, o.cast_mode, o.cast_scales, o.epoch, sl->host_flag,
-                                                             static_cast<uint32_t>(seq), stream),
-                   "kvbm_kernels_paged_repage_scatter_anypage");
-    else if (masks)
-      rc = checked(kvbm_kernels_paged_repage_scatter_routed(&ks, snh, ups, kt, k, upd, routes.data(), routes.size(), dr, bt.units.size(), ilb, ile,
-                                                            row, o.cast_mode, o.cast_scales, o.epoch, sl->host_flag, static_cast<uint32_t>(seq),
-                                                            stream),
-                   "kvbm_kernels_paged_repage_scatter_routed");
-    else if (batch)
-      rc = checked(kvbm_kernels_paged_repage_scatter_batch(&ks, snh, ups, kt, k, upd, bt.ranges.data(), bt.ranges.size(), du, bt.units.size(), ilb, ile,
-                                                           row, o.cast_mode, o.cast_scales, o.epoch, sl->host_flag, static_cast<uint32_t>(seq),
-                                                           stream),
-                   "kvbm_kernels_paged_repage_scatter_batch");
-    else
-      rc = checked(kvbm_kernels_paged_repage_scatter(&ks, snh, ups, kt, k, upd, utb, ute, ilb, ile, row, o.cast_mode, o.cast_scales, o.epoch,
-                                                     sl->host_flag, static_cast<uint32_t>(seq), stream),
-                   "kvbm_kernels_paged_repage_scatter");
-    if (!rc && o.done_flag) rc = checked(kvbm_kernels_set_flags(o.done_flag, 0, 1, o.epoch, stream), "kvbm_kernels_set_flags");
+  const int32_t* du = sl->dev_ids + units_at(n_src + num_dsts * n_dst);
+  const kvbm_permute_stream st = ls ? layer_stream(*ls, e, 1, o, *sl, seq) : kvbm_permute_stream{};
+  // a batch: its kind's entry, streamed or not
+  auto run = [&](auto entry, auto streamed_entry, const char* name, const char* streamed_name, const auto* qs, size_t n, const auto* t) {
+    if (ls)
+      return checked(streamed_entry(&ks, snh, ups, kt, k, upd, qs, n, t, bt.units.size(), ilb, ile, row, o.cast_mode, o.cast_scales, &st, stream),
+                     streamed_name);
+    return checked(entry(&ks, snh, ups, kt, k, upd, qs, n, t, bt.units.size(), ilb, ile, row, o.cast_mode, o.cast_scales, o.epoch, sl->host_flag,
+                         static_cast<uint32_t>(seq), stream),
+                   name);
+  };
+  switch (units) {
+    case kRange:
+      rc = ls ? checked(kvbm_kernels_paged_repage_scatter_streamed(&ks, snh, ups, kt, k, upd, utb, ute, ilb, ile, row, o.cast_mode, o.cast_scales,
+                                                                   &st, stream),
+                        "kvbm_kernels_paged_repage_scatter_streamed")
+              : checked(kvbm_kernels_paged_repage_scatter(&ks, snh, ups, kt, k, upd, utb, ute, ilb, ile, row, o.cast_mode, o.cast_scales, o.epoch,
+                                                          sl->host_flag, static_cast<uint32_t>(seq), stream),
+                        "kvbm_kernels_paged_repage_scatter");
+      break;
+    case kSeqs:
+      rc = run(kvbm_kernels_paged_repage_scatter_batch, kvbm_kernels_paged_repage_scatter_batch_streamed, "kvbm_kernels_paged_repage_scatter_batch",
+               "kvbm_kernels_paged_repage_scatter_batch_streamed", bt.ranges.data(), bt.ranges.size(), reinterpret_cast<const kvbm_repage_unit*>(du));
+      break;
+    case kRouted:
+      rc = run(kvbm_kernels_paged_repage_scatter_routed, kvbm_kernels_paged_repage_scatter_routed_streamed, "kvbm_kernels_paged_repage_scatter_routed",
+               "kvbm_kernels_paged_repage_scatter_routed_streamed", routes.data(), routes.size(), reinterpret_cast<const kvbm_route_unit*>(du));
+      break;
+    case kPhased:
+      rc = run(kvbm_kernels_paged_repage_scatter_anypage, kvbm_kernels_paged_repage_scatter_anypage_streamed,
+               "kvbm_kernels_paged_repage_scatter_anypage", "kvbm_kernels_paged_repage_scatter_anypage_streamed", bt.ranges.data(),
+               bt.ranges.size(), reinterpret_cast<const kvbm_repage_anypage_unit*>(du));
+      break;
+    case kRoutedPhased:
+      rc = run(kvbm_kernels_paged_repage_scatter_routed_anypage, kvbm_kernels_paged_repage_scatter_routed_anypage_streamed,
+               "kvbm_kernels_paged_repage_scatter_routed_anypage", "kvbm_kernels_paged_repage_scatter_routed_anypage_streamed", routes.data(),
+               routes.size(), reinterpret_cast<const kvbm_route_anypage_unit*>(du));
+      break;
   }
+  if (!rc && !ls && o.done_flag) rc = checked(kvbm_kernels_set_flags(o.done_flag, 0, 1, o.epoch, stream), "kvbm_kernels_set_flags");
   if (rc) return rc;
   if ((rc = finish_slot(m, sl, stream, bytes))) return rc;
   if (out) *out = o.use_caller_stream ? 0 : seq;
@@ -2681,7 +2660,7 @@ extern "C" int kvbm_manager_execute_repage_scatter_batch(kvbm_transfer_manager* 
 {
   return guarded([&]() -> int {
   if (int rc = stream_entry(m, ls, 1, false, out)) return rc;
-  return execute_repage_scatter(m, src, num_dsts, dsts, seqs, num_seqs, windows, num_windows, opts, out, ls, /*batch=*/true);
+  return execute_repage_scatter(m, src, num_dsts, dsts, seqs, num_seqs, windows, num_windows, opts, out, ls, kSeqs);
   });
 }
 
@@ -2692,16 +2671,16 @@ extern "C" int kvbm_manager_execute_repage_scatter_anypage(kvbm_transfer_manager
 {
   return guarded([&]() -> int {
   if (int rc = stream_entry(m, ls, 1, false, out)) return rc;
-  return execute_repage_scatter(m, src, num_dsts, dsts, seqs, num_seqs, windows, num_windows, opts, out, ls, /*batch=*/true,
-                                /*masks=*/nullptr, /*anypage=*/true);
+  return execute_repage_scatter(m, src, num_dsts, dsts, seqs, num_seqs, windows, num_windows, opts, out, ls, kPhased);
   });
 }
 
-// The body of kvbm_manager_execute_repage_scatter_routed and, with anypage, of kvbm_manager_execute_repage_scatter_routed_anypage.
+// The body of kvbm_manager_execute_repage_scatter_routed (units kRouted) and kvbm_manager_execute_repage_scatter_routed_anypage
+// (kRoutedPhased).
 static int execute_repage_scatter_routed(kvbm_transfer_manager* m, kvbm_layout_handle src, size_t num_dsts, const kvbm_layout_handle* dsts,
                                          const kvbm_scatter_route_seq* seqs, size_t num_seqs, const kvbm_scatter_window* windows,
                                          size_t num_windows, const kvbm_layer_stream* ls, const kvbm_transfer_options* opts,
-                                         kvbm_notification* out, bool anypage)
+                                         kvbm_notification* out, RepageUnits units)
 {
   return guarded([&]() -> int {
   if (int rc = stream_entry(m, ls, 1, false, out)) return rc;
@@ -2712,8 +2691,8 @@ static int execute_repage_scatter_routed(kvbm_transfer_manager* m, kvbm_layout_h
     qs[i] = kvbm_scatter_batch_seq{s.token_begin, s.token_end, s.src_ids, s.n_src, s.dst_ids, s.n_dst};
     masks[i] = s.dst_mask;
   }
-  return execute_repage_scatter(m, src, num_dsts, dsts, seqs ? qs.data() : nullptr, num_seqs, windows, num_windows, opts, out, ls,
-                                /*batch=*/true, masks.data(), anypage);
+  return execute_repage_scatter(m, src, num_dsts, dsts, seqs ? qs.data() : nullptr, num_seqs, windows, num_windows, opts, out, ls, units,
+                                masks.data());
   });
 }
 
@@ -2722,7 +2701,7 @@ extern "C" int kvbm_manager_execute_repage_scatter_routed(kvbm_transfer_manager*
                                                           const kvbm_scatter_window* windows, size_t num_windows, const kvbm_layer_stream* ls,
                                                           const kvbm_transfer_options* opts, kvbm_notification* out)
 {
-  return execute_repage_scatter_routed(m, src, num_dsts, dsts, seqs, num_seqs, windows, num_windows, ls, opts, out, /*anypage=*/false);
+  return execute_repage_scatter_routed(m, src, num_dsts, dsts, seqs, num_seqs, windows, num_windows, ls, opts, out, kRouted);
 }
 
 extern "C" int kvbm_manager_execute_repage_scatter_routed_anypage(kvbm_transfer_manager* m, kvbm_layout_handle src, size_t num_dsts,
@@ -2731,7 +2710,7 @@ extern "C" int kvbm_manager_execute_repage_scatter_routed_anypage(kvbm_transfer_
                                                                   const kvbm_layer_stream* ls, const kvbm_transfer_options* opts,
                                                                   kvbm_notification* out)
 {
-  return execute_repage_scatter_routed(m, src, num_dsts, dsts, seqs, num_seqs, windows, num_windows, ls, opts, out, /*anypage=*/true);
+  return execute_repage_scatter_routed(m, src, num_dsts, dsts, seqs, num_seqs, windows, num_windows, ls, opts, out, kRoutedPhased);
 }
 
 // The head windows of a staged plan's windows, in hw[], or null without windows.  Only the first KVBM_GATHER_MAX_SOURCES are
@@ -2791,7 +2770,7 @@ extern "C" int kvbm_manager_execute_repage_batch(kvbm_transfer_manager* m, size_
   if (int rc = stream_entry(m, ls, num_srcs, false, out)) return rc;
   kvbm_head_window hw[KVBM_GATHER_MAX_SOURCES];
   return execute_repage(m, num_srcs, srcs, dst, seqs, num_seqs, head_windows(windows, num_windows, hw), num_windows, opts, out, ls,
-                        /*gather=*/true, windows, /*batch=*/true);
+                        /*gather=*/true, windows, kSeqs);
   });
 }
 
@@ -2804,15 +2783,16 @@ extern "C" int kvbm_manager_execute_repage_anypage(kvbm_transfer_manager* m, siz
   if (int rc = stream_entry(m, ls, num_srcs, false, out)) return rc;
   kvbm_head_window hw[KVBM_GATHER_MAX_SOURCES];
   return execute_repage(m, num_srcs, srcs, dst, seqs, num_seqs, head_windows(windows, num_windows, hw), num_windows, opts, out, ls,
-                        /*gather=*/true, windows, /*batch=*/true, /*masks=*/nullptr, /*anypage=*/true);
+                        /*gather=*/true, windows, kPhased);
   });
 }
 
-// The body of kvbm_manager_execute_repage_batch_routed and, with anypage, of kvbm_manager_execute_repage_batch_routed_anypage.
+// The body of kvbm_manager_execute_repage_batch_routed (units kRouted) and kvbm_manager_execute_repage_batch_routed_anypage
+// (kRoutedPhased).
 static int execute_repage_batch_routed(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs, kvbm_layout_handle dst,
                                        const kvbm_repage_route_seq* seqs, size_t num_seqs, const kvbm_shard_window* windows,
                                        size_t num_windows, const kvbm_layer_stream* ls, const kvbm_transfer_options* opts,
-                                       kvbm_notification* out, bool anypage)
+                                       kvbm_notification* out, RepageUnits units)
 {
   return guarded([&]() -> int {
   if (int rc = stream_entry(m, ls, num_srcs, false, out)) return rc;
@@ -2825,7 +2805,7 @@ static int execute_repage_batch_routed(kvbm_transfer_manager* m, size_t num_srcs
     masks[i] = s.src_mask;
   }
   return execute_repage(m, num_srcs, srcs, dst, seqs ? qs.data() : nullptr, num_seqs, head_windows(windows, num_windows, hw), num_windows,
-                        opts, out, ls, /*gather=*/true, windows, /*batch=*/true, masks.data(), anypage);
+                        opts, out, ls, /*gather=*/true, windows, units, masks.data());
   });
 }
 
@@ -2834,7 +2814,7 @@ extern "C" int kvbm_manager_execute_repage_batch_routed(kvbm_transfer_manager* m
                                                         const kvbm_shard_window* windows, size_t num_windows, const kvbm_layer_stream* ls,
                                                         const kvbm_transfer_options* opts, kvbm_notification* out)
 {
-  return execute_repage_batch_routed(m, num_srcs, srcs, dst, seqs, num_seqs, windows, num_windows, ls, opts, out, /*anypage=*/false);
+  return execute_repage_batch_routed(m, num_srcs, srcs, dst, seqs, num_seqs, windows, num_windows, ls, opts, out, kRouted);
 }
 
 extern "C" int kvbm_manager_execute_repage_batch_routed_anypage(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs,
@@ -2843,7 +2823,7 @@ extern "C" int kvbm_manager_execute_repage_batch_routed_anypage(kvbm_transfer_ma
                                                                 const kvbm_layer_stream* ls, const kvbm_transfer_options* opts,
                                                                 kvbm_notification* out)
 {
-  return execute_repage_batch_routed(m, num_srcs, srcs, dst, seqs, num_seqs, windows, num_windows, ls, opts, out, /*anypage=*/true);
+  return execute_repage_batch_routed(m, num_srcs, srcs, dst, seqs, num_seqs, windows, num_windows, ls, opts, out, kRoutedPhased);
 }
 
 extern "C" int kvbm_manager_execute_repage_gather_streamed(kvbm_transfer_manager* m, size_t num_srcs, const kvbm_layout_handle* srcs,

@@ -740,35 +740,38 @@ __device__ __forceinline__ RepageUnit repage_unit(const RepageGeom& G, uint32_t 
   return {t0 - first, t1 - t0, (G.big_first + j) * G.ratio - G.small_first};
 }
 
-// A batch of sequences (kvbm_repage_unit): the same three words of big block j, loaded from the batch's unit table, whose
-// small_k indexes the concatenated small table.  One 16 B load where a search over per-sequence prefix sums would be log2(n)
-// dependent loads at the head of a CTA that lives a few microseconds.
-__device__ __forceinline__ RepageUnit batch_unit(const kvbm_repage_unit* units, uint32_t j)
-{
-  const uint4 w = __ldg(reinterpret_cast<const uint4*>(units) + j);
-  return {w.x, w.y, w.z};
-}
+// Where a re-paging launch's units come from.  kRange: the launch's one token range (repage_unit).  Every other kind is a batch
+// of sequences whose unit j is record j of a 16 B unit table: the same three words, whose small_k indexes the concatenated small
+// table, in one 16 B load where a search over per-sequence prefix sums would be log2(n) dependent loads at the head of a CTA that
+// lives a few microseconds.  The kinds differ in what the record's fourth word means:
+//   kSeqs         kvbm_repage_unit           the sequence index (unused by the walks)
+//   kRouted       kvbm_route_unit            the sequence's rank mask (a scatter's targets, a gather's sources)
+//   kPhased       kvbm_repage_anypage_unit   the phase, for pages that need not divide (DESIGN §4.2k)
+//   kRoutedPhased kvbm_route_anypage_unit    mask | phase << 16 (DESIGN §4.2m)
+enum RepageUnits { kRange, kSeqs, kRouted, kPhased, kRoutedPhased };
+__host__ __device__ constexpr bool routed_units(RepageUnits k) { return k == kRouted || k == kRoutedPhased; }
+__host__ __device__ constexpr bool phased_units(RepageUnits k) { return k == kPhased || k == kRoutedPhased; }
 
-// A batch whose pages need not divide (kvbm_repage_anypage_unit): batch_unit's three words and the unit's phase, the slot of
-// small block small_k that holds the big block's slot 0, in the same 16 B load.
-struct RepageAnyUnit {
+// Unit j of a re-paging launch whose units are UNITS, with its rank mask and its phase (the slot of small block small_k that
+// holds the big block's slot 0), each 0 where the kind has none.  table: the unit table (unused for kRange).
+struct RepageUnitRecord {
   RepageUnit u;
-  uint32_t phase;
+  uint32_t mask, phase;
 };
-__device__ __forceinline__ RepageAnyUnit anypage_unit(const kvbm_repage_anypage_unit* units, uint32_t j)
+template <RepageUnits UNITS>
+__device__ __forceinline__ RepageUnitRecord load_unit(const RepageGeom& G, const void* table, uint32_t j)
 {
-  const uint4 w = __ldg(reinterpret_cast<const uint4*>(units) + j);
-  return {{w.x, w.y, w.z}, w.w};
-}
-
-// A routed batch whose pages need not divide (kvbm_route_anypage_unit): the unit, its phase (the high half of the fourth word)
-// and, in *mask, its sequence's mask (the low half), in the same 16 B load.  The mask is cut to its 16 bits although the walks
-// only read bits below the launch's rank count, so that the phase never reaches a mask reader.
-__device__ __forceinline__ RepageAnyUnit route_anypage_unit(const kvbm_route_anypage_unit* units, uint32_t j, uint32_t* mask)
-{
-  const uint4 w = __ldg(reinterpret_cast<const uint4*>(units) + j);
-  *mask = w.w & 0xFFFFu;
-  return {{w.x, w.y, w.z}, w.w >> 16};
+  if constexpr (UNITS == kRange) {
+    return {repage_unit(G, j), 0, 0};
+  } else {
+    const uint4 w = __ldg(static_cast<const uint4*>(table) + j);
+    if constexpr (UNITS == kSeqs) return {{w.x, w.y, w.z}, 0, 0};
+    if constexpr (UNITS == kRouted) return {{w.x, w.y, w.z}, w.w, 0};
+    if constexpr (UNITS == kPhased) return {{w.x, w.y, w.z}, 0, w.w};
+    // kRoutedPhased: the mask is cut to its 16 bits although the walks only read bits below the launch's rank count, so that the
+    // phase never reaches a mask reader.
+    return {{w.x, w.y, w.z}, w.w & 0xFFFFu, w.w >> 16};
+  }
 }
 
 // The unit of a one-CTA-per-unit re-paging kernel, blockIdx.x = (big block j * nlayers + l - layer_begin) * no + o.  The caller
@@ -910,18 +913,14 @@ struct RepageGatherParams {
 
 // Unit (big block j, destination layer l, outer o) of the re-paging gather: the warp of map entry k of l's stage T reads its source
 // s at the source's own layer l + shift[s].  SCALED: one scale array for every source, scales[l * no + o] by the destination layer.
-// TABLE: a batch of sequences, whose unit comes from `units` (batch_unit) instead of the launch's one token range.
-// ROUTE: a routed batch, whose unit and source mask come from record j of `routes` in one 16 B load.  The warps walk only the
-// entries of the stage's sources in the mask, numbered densely (route_entry), so no warp idles on an unrouted window; heads[s]
-// is source s's entry count.  Only the stage's sources are consulted, so mask bits at or above the launch's sources never are.
-// ANY: a batch whose pages need not divide, whose unit and phase come from record j of `any` (anypage_unit).  ROUTE and ANY:
-// a routed batch whose pages need not divide, whose unit, mask and phase come from record j of `route_any` (route_anypage_unit).
-template <int CAST, bool POW2, bool SCALED, bool PPOW2, bool TABLE = false, bool ROUTE = false, bool ANY = false>
+// UNITS / table: where the unit comes from (load_unit).  A routed kind walks only the entries of the stage's sources in the
+// unit's mask, numbered densely (route_entry), so no warp idles on an unrouted window; heads[s] is source s's entry count.  Only
+// the stage's sources are consulted, so mask bits at or above the launch's sources never are.  A phased kind's walks split the
+// unit's phase (repage_head_rows' PHASE).
+template <int CAST, bool POW2, bool SCALED, bool PPOW2, RepageUnits UNITS = kRange>
 __device__ __forceinline__ void repage_gather_unit(const RepageGatherParams& P, const GatherStage& T, uint32_t j, uint32_t l, uint32_t o,
-                                                   const RowSplit& r, const float* scales, const kvbm_repage_unit* units = nullptr,
-                                                   const kvbm_route_unit* routes = nullptr, const uint16_t* heads = nullptr,
-                                                   const kvbm_repage_anypage_unit* any = nullptr,
-                                                   const kvbm_route_anypage_unit* route_any = nullptr)
+                                                   const RowSplit& r, const float* scales, const void* table = nullptr,
+                                                   const uint16_t* heads = nullptr)
 {
   constexpr int IN = CAST == KVBM_CAST_BF16_TO_FP8E4M3 ? 2 : 1;
   constexpr int OUT = CAST == KVBM_CAST_FP8E4M3_TO_BF16 ? 2 : 1;
@@ -929,25 +928,9 @@ __device__ __forceinline__ void repage_gather_unit(const RepageGatherParams& P, 
   const RepageGeom& G = P.geo;
   const uint32_t first = T.first, end = T.first + T.count;
   const PermuteSide& D = g.D;
-  RepageUnit u;
-  uint32_t mask = 0, phase = 0;
-  if constexpr (ROUTE && ANY) {
-    const RepageAnyUnit a = route_anypage_unit(route_any, j, &mask);
-    u = a.u;
-    phase = a.phase;
-  } else if constexpr (ANY) {
-    const RepageAnyUnit a = anypage_unit(any, j);
-    u = a.u;
-    phase = a.phase;
-  } else if constexpr (ROUTE) {
-    const uint4 w = __ldg(reinterpret_cast<const uint4*>(routes) + j);
-    u = {w.x, w.y, w.z};
-    mask = w.w;
-  } else if constexpr (TABLE) {
-    u = batch_unit(units, j);
-  } else {
-    u = repage_unit(G, j);
-  }
+  const RepageUnitRecord rec = load_unit<UNITS>(G, table, j);
+  const RepageUnit u = rec.u;  // named, not bound: the walk's lambda captures them
+  const uint32_t mask = rec.mask, phase = rec.phase;
   const uint8_t* d_region = side_region(D, l, o);
   const ptx::Scale scale = ptx::make_scale(SCALED ? __ldg(scales + l * G.no + o) : 1.f);
   const uint32_t big_shift = G.src_small ? 3 + OUT : 3 + IN, small_shift = G.src_small ? 3 + IN : 3 + OUT;
@@ -962,11 +945,11 @@ __device__ __forceinline__ void repage_gather_unit(const RepageGatherParams& P, 
     const PermuteSide& B = ss ? D : S.S;
     const PermuteSide& Sm = ss ? S.S : D;
     const uint8_t* bh = (ss ? dh : sh) + static_cast<uint64_t>(__ldg(B.ids + j)) * B.block_stride;
-    repage_head_rows<CAST, POW2, SCALED, PPOW2, ANY>(bh, static_cast<uint32_t>(B.tok_stride), big_shift, ss ? sh : dh, Sm.ids, u.small_k,
-                                                     Sm.block_stride, static_cast<uint32_t>(Sm.tok_stride), small_shift, G, u.q0, run, r,
-                                                     scale, phase);
+    repage_head_rows<CAST, POW2, SCALED, PPOW2, phased_units(UNITS)>(bh, static_cast<uint32_t>(B.tok_stride), big_shift, ss ? sh : dh, Sm.ids,
+                                                                     u.small_k, Sm.block_stride, static_cast<uint32_t>(Sm.tok_stride),
+                                                                     small_shift, G, u.q0, run, r, scale, phase);
   };
-  if constexpr (ROUTE) {
+  if constexpr (routed_units(UNITS)) {
     // routed entry i of the unit: the stage's map runs source by source in source order, so skip whole sources up to it
     const uint32_t warps = blockDim.x >> 5;
     uint32_t i = threadIdx.x >> 5;
@@ -997,7 +980,7 @@ __global__ void __launch_bounds__(256, 3)
 kvbm_paged_batch_repage_gather_kernel(const __grid_constant__ RepageGatherParams P, const kvbm_repage_unit* units, RowSplit r, const float* scales)
 {
   const auto [j, l, rem] = repage_cta(P.geo);
-  repage_gather_unit<CAST, POW2, SCALED, PPOW2, true>(P, stage_of(P.g, l), j, l, rem % P.geo.no, r, scales, units);
+  repage_gather_unit<CAST, POW2, SCALED, PPOW2, kSeqs>(P, stage_of(P.g, l), j, l, rem % P.geo.no, r, scales, units);
 }
 
 // Each source's entry count in the head map (its window's heads), which a routed unit needs to skip unrouted sources.
@@ -1013,7 +996,7 @@ kvbm_paged_repage_fanin_kernel(const __grid_constant__ RepageGatherParams P, con
                                RowSplit r, const float* scales)
 {
   const auto [j, l, rem] = repage_cta(P.geo);
-  repage_gather_unit<CAST, POW2, SCALED, PPOW2, true, true>(P, stage_of(P.g, l), j, l, rem % P.geo.no, r, scales, nullptr, routes, H.n);
+  repage_gather_unit<CAST, POW2, SCALED, PPOW2, kRouted>(P, stage_of(P.g, l), j, l, rem % P.geo.no, r, scales, routes, H.n);
 }
 
 // kvbm_paged_batch_repage_gather_kernel over a batch whose pages need not divide: record j of `units` also carries big block j's
@@ -1024,8 +1007,7 @@ kvbm_paged_repage_anypage_kernel(const __grid_constant__ RepageGatherParams P, c
                                  const float* scales)
 {
   const auto [j, l, rem] = repage_cta(P.geo);
-  repage_gather_unit<CAST, POW2, SCALED, PPOW2, false, false, true>(P, stage_of(P.g, l), j, l, rem % P.geo.no, r, scales, nullptr, nullptr,
-                                                                    nullptr, units);
+  repage_gather_unit<CAST, POW2, SCALED, PPOW2, kPhased>(P, stage_of(P.g, l), j, l, rem % P.geo.no, r, scales, units);
 }
 
 // kvbm_paged_repage_fanin_kernel over a batch whose pages need not divide: record j of `units` carries big block j's sources and
@@ -1036,8 +1018,7 @@ kvbm_paged_repage_collect_kernel(const __grid_constant__ RepageGatherParams P, c
                                  const kvbm_route_anypage_unit* units, RowSplit r, const float* scales)
 {
   const auto [j, l, rem] = repage_cta(P.geo);
-  repage_gather_unit<CAST, POW2, SCALED, PPOW2, true, true, true>(P, stage_of(P.g, l), j, l, rem % P.geo.no, r, scales, nullptr, nullptr, H.n,
-                                                                  nullptr, units);
+  repage_gather_unit<CAST, POW2, SCALED, PPOW2, kRoutedPhased>(P, stage_of(P.g, l), j, l, rem % P.geo.no, r, scales, units, H.n);
 }
 
 // The re-paging scatter, the gather's mirror image: ONE source pool of page Ps (a prefill rank) into up to
@@ -1131,41 +1112,19 @@ __device__ __forceinline__ void scatter_head_rows(const ScatterParams& P, uint32
 
 // One (big block j, source layer l, outer o) unit of the scatter, clipped to the range, with l's stage T: one warp per covered
 // source head of T, looping by the CTA's warps past 8.  SCALED: the SOURCE's scales[l * no + o], loaded once per unit.
-// TABLE: a batch of sequences, whose unit comes from `units` (batch_unit) instead of the launch's one token range.  ROUTE: a
-// routed batch, whose unit and target mask come from record j of `routes` in the same 16 B load (scatter_head_rows' ROUTE).  ANY:
-// a batch whose pages need not divide, whose unit and phase come from record j of `any` (anypage_unit).  ROUTE and ANY: a routed
-// batch whose pages need not divide, whose unit, mask and phase come from record j of `route_any` (route_anypage_unit).
-template <int CAST, bool POW2, bool SCALED, bool PPOW2, bool TABLE = false, bool ROUTE = false, bool ANY = false>
+// UNITS / table: where the unit comes from (load_unit); a routed kind's mask and a phased kind's phase go to scatter_head_rows.
+template <int CAST, bool POW2, bool SCALED, bool PPOW2, RepageUnits UNITS = kRange>
 __device__ __forceinline__ void scatter_unit(const ScatterParams& P, const GatherStage& T, uint32_t j, uint32_t l, uint32_t o, const RowSplit& r,
-                                             const float* scales, const kvbm_repage_unit* units = nullptr,
-                                             const kvbm_route_unit* routes = nullptr, const kvbm_repage_anypage_unit* any = nullptr,
-                                             const kvbm_route_anypage_unit* route_any = nullptr)
+                                             const float* scales, const void* table = nullptr)
 {
   const RepageGeom& G = P.geo;
-  RepageUnit u;
-  uint32_t mask = 0, phase = 0;
-  if constexpr (ROUTE && ANY) {
-    const RepageAnyUnit a = route_anypage_unit(route_any, j, &mask);
-    u = a.u;
-    phase = a.phase;
-  } else if constexpr (ANY) {
-    const RepageAnyUnit a = anypage_unit(any, j);
-    u = a.u;
-    phase = a.phase;
-  } else if constexpr (ROUTE) {
-    const uint4 w = __ldg(reinterpret_cast<const uint4*>(routes) + j);
-    u = {w.x, w.y, w.z};
-    mask = w.w;
-  } else if constexpr (TABLE) {
-    u = batch_unit(units, j);
-  } else {
-    u = repage_unit(G, j);
-  }
+  const RepageUnitRecord rec = load_unit<UNITS>(G, table, j);
   const ptx::Scale scale = ptx::make_scale(SCALED ? __ldg(scales + l * G.no + o) : 1.f);
-  const uint32_t run = row_run<POW2>(r, u.tokens);
+  const uint32_t run = row_run<POW2>(r, rec.u.tokens);
   const uint32_t end = T.first + T.count;
   for (uint32_t k = T.first + (threadIdx.x >> 5); k < end; k += blockDim.x >> 5)
-    scatter_head_rows<CAST, POW2, SCALED, PPOW2, ROUTE, ANY>(P, k, j, l, o, u, run, r, scale, mask, phase);
+    scatter_head_rows<CAST, POW2, SCALED, PPOW2, routed_units(UNITS), phased_units(UNITS)>(P, k, j, l, o, rec.u, run, r, scale, rec.mask,
+                                                                                           rec.phase);
 }
 
 // One CTA per unit, as the re-paging gather.  The re-paging gathers' bound: three CTAs per SM.
@@ -1187,7 +1146,7 @@ kvbm_paged_repage_push_seqs_kernel(const __grid_constant__ ScatterParams P, cons
 {
   const auto [j, l, rem] = repage_cta(P.geo);
   const uint32_t o = rem % P.geo.no;
-  scatter_unit<CAST, POW2, SCALED, PPOW2, true>(P, stage_of(P, l), j, l, o, r, scales, units);
+  scatter_unit<CAST, POW2, SCALED, PPOW2, kSeqs>(P, stage_of(P, l), j, l, o, r, scales, units);
 }
 
 // kvbm_paged_repage_push_seqs_kernel over a routed batch: record j of `routes` also names the targets big block j goes to, and
@@ -1198,7 +1157,7 @@ kvbm_paged_repage_route_kernel(const __grid_constant__ ScatterParams P, const kv
 {
   const auto [j, l, rem] = repage_cta(P.geo);
   const uint32_t o = rem % P.geo.no;
-  scatter_unit<CAST, POW2, SCALED, PPOW2, true, true>(P, stage_of(P, l), j, l, o, r, scales, nullptr, routes);
+  scatter_unit<CAST, POW2, SCALED, PPOW2, kRouted>(P, stage_of(P, l), j, l, o, r, scales, routes);
 }
 
 // kvbm_paged_repage_push_seqs_kernel over a batch whose pages need not divide: record j of `units` also carries big block j's phase
@@ -1210,7 +1169,7 @@ kvbm_paged_repage_phased_push_kernel(const __grid_constant__ ScatterParams P, co
 {
   const auto [j, l, rem] = repage_cta(P.geo);
   const uint32_t o = rem % P.geo.no;
-  scatter_unit<CAST, POW2, SCALED, PPOW2, false, false, true>(P, stage_of(P, l), j, l, o, r, scales, nullptr, nullptr, units);
+  scatter_unit<CAST, POW2, SCALED, PPOW2, kPhased>(P, stage_of(P, l), j, l, o, r, scales, units);
 }
 
 // kvbm_paged_repage_route_kernel over a batch whose pages need not divide: record j of `units` carries big block j's targets and
@@ -1221,7 +1180,7 @@ kvbm_paged_repage_deal_kernel(const __grid_constant__ ScatterParams P, const kvb
 {
   const auto [j, l, rem] = repage_cta(P.geo);
   const uint32_t o = rem % P.geo.no;
-  scatter_unit<CAST, POW2, SCALED, PPOW2, true, true, true>(P, stage_of(P, l), j, l, o, r, scales, nullptr, nullptr, nullptr, units);
+  scatter_unit<CAST, POW2, SCALED, PPOW2, kRoutedPhased>(P, stage_of(P, l), j, l, o, r, scales, units);
 }
 
 // The scatter's signal after its launch: every target's done flag (epoch) and the completion word, system scope.
@@ -1373,7 +1332,7 @@ kvbm_gated_batch_repage_gather_kernel(const __grid_constant__ RepageGatherParams
                                       const kvbm_repage_unit* units, uint32_t num_big, RowSplit r, const float* scales, uint32_t batch)
 {
   gated_repage_units(A, P.g, P.geo, num_big, batch, [&](const GatherStage& T, uint32_t j, uint32_t l, uint32_t o) {
-    repage_gather_unit<CAST, POW2, SCALED, PPOW2, true>(P, T, j, l, o, r, scales, units);
+    repage_gather_unit<CAST, POW2, SCALED, PPOW2, kSeqs>(P, T, j, l, o, r, scales, units);
   });
 }
 
@@ -1385,7 +1344,7 @@ kvbm_gated_repage_fanin_kernel(const __grid_constant__ RepageGatherParams P, con
                                const kvbm_route_unit* routes, uint32_t num_big, RowSplit r, const float* scales, uint32_t batch)
 {
   gated_repage_units(A, P.g, P.geo, num_big, batch, [&](const GatherStage& T, uint32_t j, uint32_t l, uint32_t o) {
-    repage_gather_unit<CAST, POW2, SCALED, PPOW2, true, true>(P, T, j, l, o, r, scales, nullptr, routes, H.n);
+    repage_gather_unit<CAST, POW2, SCALED, PPOW2, kRouted>(P, T, j, l, o, r, scales, routes, H.n);
   });
 }
 
@@ -1396,7 +1355,7 @@ kvbm_gated_repage_anypage_kernel(const __grid_constant__ RepageGatherParams P, c
                                  const kvbm_repage_anypage_unit* units, uint32_t num_big, RowSplit r, const float* scales, uint32_t batch)
 {
   gated_repage_units(A, P.g, P.geo, num_big, batch, [&](const GatherStage& T, uint32_t j, uint32_t l, uint32_t o) {
-    repage_gather_unit<CAST, POW2, SCALED, PPOW2, false, false, true>(P, T, j, l, o, r, scales, nullptr, nullptr, nullptr, units);
+    repage_gather_unit<CAST, POW2, SCALED, PPOW2, kPhased>(P, T, j, l, o, r, scales, units);
   });
 }
 
@@ -1409,7 +1368,7 @@ kvbm_gated_repage_collect_kernel(const __grid_constant__ RepageGatherParams P, c
                                  const float* scales, uint32_t batch)
 {
   gated_repage_units(A, P.g, P.geo, num_big, batch, [&](const GatherStage& T, uint32_t j, uint32_t l, uint32_t o) {
-    repage_gather_unit<CAST, POW2, SCALED, PPOW2, true, true, true>(P, T, j, l, o, r, scales, nullptr, nullptr, H.n, nullptr, units);
+    repage_gather_unit<CAST, POW2, SCALED, PPOW2, kRoutedPhased>(P, T, j, l, o, r, scales, units, H.n);
   });
 }
 
@@ -1444,7 +1403,7 @@ kvbm_gated_repage_push_seqs_kernel(const __grid_constant__ ScatterParams P, cons
 {
   gated_repage_units(
       A, P, P.geo, num_big, batch,
-      [&](const GatherStage& T, uint32_t j, uint32_t l, uint32_t o) { scatter_unit<CAST, POW2, SCALED, PPOW2, true>(P, T, j, l, o, r, scales, units); },
+      [&](const GatherStage& T, uint32_t j, uint32_t l, uint32_t o) { scatter_unit<CAST, POW2, SCALED, PPOW2, kSeqs>(P, T, j, l, o, r, scales, units); },
       target_done(F, num_flags, A));
 }
 
@@ -1458,7 +1417,7 @@ kvbm_gated_repage_route_kernel(const __grid_constant__ ScatterParams P, const __
   gated_repage_units(
       A, P, P.geo, num_big, batch,
       [&](const GatherStage& T, uint32_t j, uint32_t l, uint32_t o) {
-        scatter_unit<CAST, POW2, SCALED, PPOW2, true, true>(P, T, j, l, o, r, scales, nullptr, routes);
+        scatter_unit<CAST, POW2, SCALED, PPOW2, kRouted>(P, T, j, l, o, r, scales, routes);
       },
       target_done(F, num_flags, A));
 }
@@ -1473,7 +1432,7 @@ kvbm_gated_repage_phased_push_kernel(const __grid_constant__ ScatterParams P, co
   gated_repage_units(
       A, P, P.geo, num_big, batch,
       [&](const GatherStage& T, uint32_t j, uint32_t l, uint32_t o) {
-        scatter_unit<CAST, POW2, SCALED, PPOW2, false, false, true>(P, T, j, l, o, r, scales, nullptr, nullptr, units);
+        scatter_unit<CAST, POW2, SCALED, PPOW2, kPhased>(P, T, j, l, o, r, scales, units);
       },
       target_done(F, num_flags, A));
 }
@@ -1489,7 +1448,7 @@ kvbm_gated_repage_deal_kernel(const __grid_constant__ ScatterParams P, const __g
   gated_repage_units(
       A, P, P.geo, num_big, batch,
       [&](const GatherStage& T, uint32_t j, uint32_t l, uint32_t o) {
-        scatter_unit<CAST, POW2, SCALED, PPOW2, true, true, true>(P, T, j, l, o, r, scales, nullptr, nullptr, nullptr, units);
+        scatter_unit<CAST, POW2, SCALED, PPOW2, kRoutedPhased>(P, T, j, l, o, r, scales, units);
       },
       target_done(F, num_flags, A));
 }
@@ -1527,6 +1486,57 @@ static void with_repage_kernel(int cast_mode, bool pow2, bool scaled, bool page_
 {
   with_walk_kernel(cast_mode, pow2, scaled, [&](auto c, auto p, auto sc) {
     page_pow2 ? f(c, p, sc, std::true_type{}) : f(c, p, sc, std::false_type{});
+  });
+}
+
+// The one place that names each unit kind's kernels: the re-paging gather's and the scatter's one-CTA-per-unit kernel and gated
+// kernel, the kind's sequence and unit record types and the exported helper that writes (and counts) its unit table.  The
+// launchers and preload_kernels take every kernel from here.
+template <RepageUnits UNITS>
+struct RepageKernels;
+#define KVBM_REPAGE_KERNELS(UNITS, SEQ, RECORD, WRITE_UNITS, GATHER, GATED_GATHER, SCATTER, GATED_SCATTER)      \
+  template <>                                                                                                   \
+  struct RepageKernels<UNITS> {                                                                                 \
+    using Seq = SEQ;                                                                                            \
+    using Record = RECORD;                                                                                      \
+    static constexpr auto write_units = WRITE_UNITS;                                                            \
+    template <int C, bool P, bool S, bool PP> static constexpr auto gather = GATHER<C, P, S, PP>;               \
+    template <int C, bool P, bool S, bool PP> static constexpr auto gated_gather = GATED_GATHER<C, P, S, PP>;   \
+    template <int C, bool P, bool S, bool PP> static constexpr auto scatter = SCATTER<C, P, S, PP>;             \
+    template <int C, bool P, bool S, bool PP> static constexpr auto gated_scatter = GATED_SCATTER<C, P, S, PP>; \
+  };
+KVBM_REPAGE_KERNELS(kRange, void, void, nullptr, kvbm_paged_repage_gather_kernel, kvbm_gated_repage_gather_kernel,
+                    kvbm_paged_repage_scatter_kernel, kvbm_gated_repage_push_kernel)
+KVBM_REPAGE_KERNELS(kSeqs, kvbm_repage_seq, kvbm_repage_unit, kvbm_kernels_repage_batch_units, kvbm_paged_batch_repage_gather_kernel,
+                    kvbm_gated_batch_repage_gather_kernel, kvbm_paged_repage_push_seqs_kernel, kvbm_gated_repage_push_seqs_kernel)
+KVBM_REPAGE_KERNELS(kRouted, kvbm_route_seq, kvbm_route_unit, kvbm_kernels_repage_route_units, kvbm_paged_repage_fanin_kernel,
+                    kvbm_gated_repage_fanin_kernel, kvbm_paged_repage_route_kernel, kvbm_gated_repage_route_kernel)
+KVBM_REPAGE_KERNELS(kPhased, kvbm_repage_seq, kvbm_repage_anypage_unit, kvbm_kernels_repage_anypage_units, kvbm_paged_repage_anypage_kernel,
+                    kvbm_gated_repage_anypage_kernel, kvbm_paged_repage_phased_push_kernel, kvbm_gated_repage_phased_push_kernel)
+KVBM_REPAGE_KERNELS(kRoutedPhased, kvbm_route_seq, kvbm_route_anypage_unit, kvbm_kernels_repage_route_anypage_units,
+                    kvbm_paged_repage_collect_kernel, kvbm_gated_repage_collect_kernel, kvbm_paged_repage_deal_kernel,
+                    kvbm_gated_repage_deal_kernel)
+#undef KVBM_REPAGE_KERNELS
+
+// Calls f(integral_constant<RepageUnits, units>).
+template <class F>
+static void with_units(RepageUnits units, F&& f)
+{
+  switch (units) {
+    case kRange: return f(std::integral_constant<RepageUnits, kRange>{});
+    case kSeqs: return f(std::integral_constant<RepageUnits, kSeqs>{});
+    case kRouted: return f(std::integral_constant<RepageUnits, kRouted>{});
+    case kPhased: return f(std::integral_constant<RepageUnits, kPhased>{});
+    case kRoutedPhased: return f(std::integral_constant<RepageUnits, kRoutedPhased>{});
+  }
+}
+
+// with_repage_kernel with the unit kind first: calls f(integral_constant<RepageUnits, units>, cast, row pow2, scaled, page pow2).
+template <class F>
+static void with_repage_units(RepageUnits units, int cast_mode, bool pow2, bool scaled, bool page_pow2, F&& f)
+{
+  with_units(units, [&](auto u) {
+    with_repage_kernel(cast_mode, pow2, scaled, page_pow2, [&](auto c, auto p, auto sc, auto pp) { f(u, c, p, sc, pp); });
   });
 }
 
@@ -1668,7 +1678,8 @@ static cudaError_t preload_kernels()
   KVBM_PRELOAD((kvbm_permute_kernel<4, false>))
   KVBM_PRELOAD((kvbm_permute_kernel<2, false>))
 #undef KVBM_PRELOAD
-  // the paged permute and gather: every instantiation launch_paged_permute can select, through its own selection helper
+  // the paged permute, the gather and the plain re-page: every instantiation their launchers can select, through their own
+  // selection helpers
   for (int cast = KVBM_CAST_NONE; cast <= KVBM_CAST_BF16_TO_FP8E4M3; ++cast)
     for (int pow2 = 0; pow2 < 2; ++pow2)
       for (int scaled = 0; scaled < 2; ++scaled)
@@ -1677,48 +1688,21 @@ static cudaError_t preload_kernels()
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_gather_kernel<c, p, sc>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_kernel<c, p, sc, true>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_kernel<c, p, sc, false>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_gather_kernel<c, p, sc, true>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_gather_kernel<c, p, sc, false>);
           if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_gather_kernel<c, p, sc>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_gather_kernel<c, p, sc, true>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_gather_kernel<c, p, sc, false>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_batch_repage_gather_kernel<c, p, sc, true>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_batch_repage_gather_kernel<c, p, sc, false>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_batch_repage_gather_kernel<c, p, sc, true>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_batch_repage_gather_kernel<c, p, sc, false>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_scatter_kernel<c, p, sc, true>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_scatter_kernel<c, p, sc, false>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_push_kernel<c, p, sc, true>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_push_kernel<c, p, sc, false>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_push_seqs_kernel<c, p, sc, true>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_push_seqs_kernel<c, p, sc, false>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_push_seqs_kernel<c, p, sc, true>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_push_seqs_kernel<c, p, sc, false>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_route_kernel<c, p, sc, true>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_route_kernel<c, p, sc, false>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_route_kernel<c, p, sc, true>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_route_kernel<c, p, sc, false>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_fanin_kernel<c, p, sc, true>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_fanin_kernel<c, p, sc, false>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_fanin_kernel<c, p, sc, true>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_fanin_kernel<c, p, sc, false>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_anypage_kernel<c, p, sc, true>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_anypage_kernel<c, p, sc, false>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_anypage_kernel<c, p, sc, true>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_anypage_kernel<c, p, sc, false>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_phased_push_kernel<c, p, sc, true>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_phased_push_kernel<c, p, sc, false>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_phased_push_kernel<c, p, sc, true>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_phased_push_kernel<c, p, sc, false>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_collect_kernel<c, p, sc, true>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_collect_kernel<c, p, sc, false>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_collect_kernel<c, p, sc, true>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_collect_kernel<c, p, sc, false>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_deal_kernel<c, p, sc, true>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_paged_repage_deal_kernel<c, p, sc, false>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_deal_kernel<c, p, sc, true>);
-          if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_gated_repage_deal_kernel<c, p, sc, false>);
         });
+  // the re-paging gathers and scatters: every kernel of every unit kind (RepageKernels)
+  for (int units = kRange; units <= kRoutedPhased; ++units)
+    for (int cast = KVBM_CAST_NONE; cast <= KVBM_CAST_BF16_TO_FP8E4M3; ++cast)
+      for (int pow2 = 0; pow2 < 2; ++pow2)
+        for (int scaled = 0; scaled < 2; ++scaled)
+          for (int page_pow2 = 0; page_pow2 < 2; ++page_pow2)
+            with_repage_units(static_cast<RepageUnits>(units), cast, pow2, scaled, page_pow2, [&](auto u, auto c, auto p, auto sc, auto pp) {
+              using K = RepageKernels<u>;
+              if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, K::template gather<c, p, sc, pp>);
+              if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, K::template gated_gather<c, p, sc, pp>);
+              if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, K::template scatter<c, p, sc, pp>);
+              if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, K::template gated_scatter<c, p, sc, pp>);
+            });
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_layer_signal_kernel);
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kvbm_scatter_signal_kernel);
   return e;
@@ -2135,22 +2119,31 @@ static bool repage_pages(uint32_t src_page, uint32_t dst_page, int layer_begin, 
   return true;
 }
 
-// A batch of sequences of a re-paging launch: the caller's ranges (host) and unit table (device-accessible).  route: a routed
-// batch, whose ranges and masks (a scatter's targets, a gather's sources) are route_seqs and whose unit table is route_units
-// (seqs and units unused).  any_units: a batch whose pages need not divide, whose unit table is this one (units unused).  route
-// and any together: a routed batch whose pages need not divide, with route_seqs and the unit table route_any_units.
+// A batch of sequences of a re-paging launch: its unit kind (never kRange), the caller's ranges (host; RepageKernels<kind>::Seq,
+// which for a routed kind carries each sequence's mask: a scatter's targets, a gather's sources) and the unit table of
+// RepageKernels<kind>::Record (device-accessible).  repage_batch builds one from pointers of those types, batch_table reads
+// the table back as one.
 struct RepageBatch {
-  const kvbm_repage_seq* seqs;
+  RepageUnits kind;
+  const void* seqs;
   size_t num_seqs;
-  const kvbm_repage_unit* units;
+  const void* table;
   size_t num_units;
-  bool route = false;
-  const kvbm_route_seq* route_seqs = nullptr;
-  const kvbm_route_unit* route_units = nullptr;
-  bool any = false;
-  const kvbm_repage_anypage_unit* any_units = nullptr;
-  const kvbm_route_anypage_unit* route_any_units = nullptr;
 };
+template <RepageUnits UNITS>
+static RepageBatch repage_batch(const typename RepageKernels<UNITS>::Seq* seqs, size_t num_seqs,
+                                const typename RepageKernels<UNITS>::Record* table, size_t num_units)
+{
+  RepageBatch B;
+  B.kind = UNITS;
+  B.seqs = seqs;
+  B.num_seqs = num_seqs;
+  B.table = table;
+  B.num_units = num_units;
+  return B;
+}
+template <RepageUnits UNITS>
+static auto batch_table(const RepageBatch* B) { return static_cast<const typename RepageKernels<UNITS>::Record*>(B->table); }
 
 // What repage_launch derives: repage_pages' results with the token range's fields, the units to launch (0: nothing to move), the
 // big blocks per (layer, outer), and the layers and outer dim of the pool whose layers the launch counts.
@@ -2162,11 +2155,9 @@ struct RepageLaunch {
   bool page_pow2;
 };
 
-// Every re-paging launch's first checks, before any CUDA call: ranges not reversed, cast_args_ok, and B checked by
-// kvbm_kernels_repage_batch_units (a routed batch: kvbm_kernels_repage_route_units; one whose pages need not divide:
-// kvbm_kernels_repage_anypage_units, and repage_pages without the divisibility rule; both: kvbm_kernels_repage_route_anypage_units)
-// with the caller's unit count.  An empty range or batch then leaves L->units 0 (the caller
-// signals).  Else `side` (a gather's destination, the scatter's source) needs a table, a base, a non-zero outer dim and the layer
+// Every re-paging launch's first checks, before any CUDA call: ranges not reversed, cast_args_ok, and B checked by its kind's unit
+// table helper (RepageKernels) with the caller's unit count; a phased kind takes repage_pages without the divisibility rule.  An
+// empty range or batch then leaves L->units 0 (the caller signals).  Else `side` (a gather's destination, the scatter's source) needs a table, a base, a non-zero outer dim and the layer
 // range; the pages repage_pages' rules; a single range slots in 32 bits (its last block of the larger page ends below 2^32); the
 // launch fewer than 2^31 units.  False: rejected.
 static bool repage_launch(const kvbm_permute_side* side, uint32_t src_page, uint32_t dst_page, uint32_t token_begin, uint32_t token_end,
@@ -2178,18 +2169,14 @@ static bool repage_launch(const kvbm_permute_side* side, uint32_t src_page, uint
   size_t num_big = 0;
   if (B) {
     size_t src_ids, dst_ids;
-    const bool both = B->route && B->any;
-    if ((both ? kvbm_kernels_repage_route_anypage_units(B->route_seqs, B->num_seqs, src_page, dst_page, nullptr, 0, &num_big, &src_ids,
-                                                        &dst_ids)
-         : B->route ? kvbm_kernels_repage_route_units(B->route_seqs, B->num_seqs, src_page, dst_page, nullptr, 0, &num_big, &src_ids, &dst_ids)
-         : B->any   ? kvbm_kernels_repage_anypage_units(B->seqs, B->num_seqs, src_page, dst_page, nullptr, 0, &num_big, &src_ids, &dst_ids)
-                    : kvbm_kernels_repage_batch_units(B->seqs, B->num_seqs, src_page, dst_page, nullptr, 0, &num_big, &src_ids, &dst_ids)) != 0)
-      return false;
-    const void* table = both       ? static_cast<const void*>(B->route_any_units)
-                        : B->route ? static_cast<const void*>(B->route_units)
-                        : B->any   ? static_cast<const void*>(B->any_units)
-                                   : B->units;
-    if (num_big != B->num_units || (num_big != 0 && !table)) return false;
+    int bad = 1;
+    with_units(B->kind, [&](auto u) {
+      using K = RepageKernels<u>;
+      if constexpr (u != kRange)
+        bad = K::write_units(static_cast<const typename K::Seq*>(B->seqs), B->num_seqs, src_page, dst_page, nullptr, 0, &num_big, &src_ids,
+                            &dst_ids);
+    });
+    if (bad || num_big != B->num_units || (num_big != 0 && !B->table)) return false;
   }
   L->units = 0;
   if ((B ? num_big == 0 : token_end == token_begin) || layer_end == layer_begin) return true;
@@ -2198,7 +2185,7 @@ static bool repage_launch(const kvbm_permute_side* side, uint32_t src_page, uint
   if (nl == 0 || no == 0 || static_cast<uint32_t>(layer_end) > nl) return false;
   RepageGeom& g = L->geo;
   if (!repage_pages(src_page, dst_page, layer_begin, layer_end, no, src_row_bytes, cast_mode, &g, &L->r, &L->dst_row_bytes, &L->page_pow2,
-                    B && B->any))
+                    B && phased_units(B->kind)))
     return false;
   if (!B) {
     const uint64_t big_end = (static_cast<uint64_t>(token_end) + g.big_page - 1) / g.big_page * g.big_page;
@@ -2218,14 +2205,13 @@ static bool repage_launch(const kvbm_permute_side* side, uint32_t src_page, uint
 // Every re-paging launch: a plain re-page is one source whose window covers every head and every layer of both sides, a
 // re-paging gather one or more windows.  Runs repage_launch's checks with the destination as the launch's side, and those of
 // launch_paged_permute's sources, each side's region at its own page and head count, all before any CUDA call; signals when
-// there is nothing to move; then launches kvbm_paged_repage_kernel for a plain re-page, else kvbm_paged_repage_gather_kernel,
-// and the signal.  max_covered and st: as launch_paged_permute's (st takes the gated re-paging gather kernel, or per layer this
-// launch unstreamed).  B: a batch of sequences in place of the one token range (token_begin / token_end unused), which always
-// takes the batch gather kernels, or the fan-in kernels for a routed batch: bit s of a sequence's mask names srcs[s], every mask
-// must be non-zero and below bit num_srcs, and two windows of a stage may then share destination heads unless one mask holds both.
-// Each stage's sources are ANDed with the union of the masks, so both gate forms wait on routed sources only, and a CTA has as
-// many warps as the most routed entries of one stage under one mask (up to 8).  A batch whose pages need not divide (B->any)
-// takes the anypage kernels, or the collect kernels when it is also routed.
+// there is nothing to move; then launches kvbm_paged_repage_kernel for a plain re-page, else the gather kernel of the launch's
+// unit kind (RepageKernels), and the signal.  max_covered and st: as launch_paged_permute's (st takes the kind's gated kernel, or
+// per layer this launch unstreamed).  B: a batch of sequences in place of the one token range (token_begin / token_end unused).
+// A routed batch: bit s of a sequence's mask names srcs[s], every mask must be non-zero and below bit num_srcs, and two windows of
+// a stage may then share destination heads unless one mask holds both.  Each stage's sources are ANDed with the union of the
+// masks, so both gate forms wait on routed sources only, and a CTA has as many warps as the most routed entries of one stage under
+// one mask (up to 8).
 static cudaError_t launch_paged_repage_gather(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page, const kvbm_permute_side* dst,
                                               uint32_t dst_num_heads, uint32_t dst_page, uint32_t token_begin, uint32_t token_end,
                                               int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
@@ -2235,12 +2221,13 @@ static cudaError_t launch_paged_repage_gather(const kvbm_stage_source* srcs, int
 {
   RepageLaunch L;
   if (!srcs || num_srcs < 1 || num_srcs > KVBM_GATHER_MAX_SOURCES) return cudaErrorInvalidValue;
-  const bool route = B && B->route;
+  const RepageUnits units = B ? B->kind : kRange;
+  const bool route = routed_units(units);
   std::vector<uint32_t> masks;  // a routed batch's distinct source masks
   uint32_t routed = 0;          // and their union
-  if (route && B->route_seqs)
+  if (route && B->seqs)
     for (size_t i = 0; i < B->num_seqs; ++i) {
-      const uint32_t m = B->route_seqs[i].targets;
+      const uint32_t m = static_cast<const kvbm_route_seq*>(B->seqs)[i].targets;
       if (m == 0 || (m >> num_srcs) != 0) return cudaErrorInvalidValue;
       if (std::find(masks.begin(), masks.end(), m) == masks.end()) masks.push_back(m);
       routed |= m;
@@ -2283,18 +2270,14 @@ static cudaError_t launch_paged_repage_gather(const kvbm_stage_source* srcs, int
                                             src_row_bytes, cast_mode, cast_scales, nullptr, 0, nullptr, 0, max_covered, stream, nullptr, B);
         },
         [&](const GateArgs& A, unsigned ctas, uint32_t batch) {
-          with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, L.page_pow2, [&](auto c, auto p, auto sc, auto pp) {
-            if (route && B->any)
-              kvbm_gated_repage_collect_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, A, H, B->route_any_units, L.num_big, r,
-                                                                                            cast_scales, batch);
-            else if (route)
-              kvbm_gated_repage_fanin_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, A, H, B->route_units, L.num_big, r, cast_scales, batch);
-            else if (B && B->any)
-              kvbm_gated_repage_anypage_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, A, B->any_units, L.num_big, r, cast_scales, batch);
-            else if (B)
-              kvbm_gated_batch_repage_gather_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, A, B->units, L.num_big, r, cast_scales, batch);
+          with_repage_units(units, cast_mode, r.pow2, cast_scales != nullptr, L.page_pow2, [&](auto u, auto c, auto p, auto sc, auto pp) {
+            const auto kernel = RepageKernels<u>::template gated_gather<c, p, sc, pp>;
+            if constexpr (u == kRange)
+              kernel<<<ctas, threads, 0, stream>>>(P, A, L.num_big, r, cast_scales, batch);
+            else if constexpr (routed_units(u))
+              kernel<<<ctas, threads, 0, stream>>>(P, A, H, batch_table<u>(B), L.num_big, r, cast_scales, batch);
             else
-              kvbm_gated_repage_gather_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, A, L.num_big, r, cast_scales, batch);
+              kernel<<<ctas, threads, 0, stream>>>(P, A, batch_table<u>(B), L.num_big, r, cast_scales, batch);
           });
         });
   // a window over every layer and every head of both sides (the checks above make its starts 0)
@@ -2304,19 +2287,18 @@ static cudaError_t launch_paged_repage_gather(const kvbm_stage_source* srcs, int
   R.big = P.geo.src_small ? P.g.D : P.g.src[0].S;
   R.small = P.geo.src_small ? P.g.src[0].S : P.g.D;
   R.g = P.geo;
-  with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, L.page_pow2, [&](auto c, auto p, auto sc, auto pp) {
-    if (route && B->any)
-      kvbm_paged_repage_collect_kernel<c, p, sc, pp><<<grid, threads, 0, stream>>>(P, H, B->route_any_units, r, cast_scales);
-    else if (route)
-      kvbm_paged_repage_fanin_kernel<c, p, sc, pp><<<grid, threads, 0, stream>>>(P, H, B->route_units, r, cast_scales);
-    else if (B && B->any)
-      kvbm_paged_repage_anypage_kernel<c, p, sc, pp><<<grid, threads, 0, stream>>>(P, B->any_units, r, cast_scales);
-    else if (B)
-      kvbm_paged_batch_repage_gather_kernel<c, p, sc, pp><<<grid, threads, 0, stream>>>(P, B->units, r, cast_scales);
-    else if (plain)
-      kvbm_paged_repage_kernel<c, p, sc, pp><<<grid, threads, 0, stream>>>(R, r, cast_scales);
-    else
-      kvbm_paged_repage_gather_kernel<c, p, sc, pp><<<grid, threads, 0, stream>>>(P, r, cast_scales);
+  with_repage_units(units, cast_mode, r.pow2, cast_scales != nullptr, L.page_pow2, [&](auto u, auto c, auto p, auto sc, auto pp) {
+    const auto kernel = RepageKernels<u>::template gather<c, p, sc, pp>;
+    if constexpr (u == kRange) {
+      if (plain)
+        kvbm_paged_repage_kernel<c, p, sc, pp><<<grid, threads, 0, stream>>>(R, r, cast_scales);
+      else
+        kernel<<<grid, threads, 0, stream>>>(P, r, cast_scales);
+    } else if constexpr (routed_units(u)) {
+      kernel<<<grid, threads, 0, stream>>>(P, H, batch_table<u>(B), r, cast_scales);
+    } else {
+      kernel<<<grid, threads, 0, stream>>>(P, batch_table<u>(B), r, cast_scales);
+    }
   });
   return launched(stream, done_flag, epoch, completion_flag, completion_value);
 }
@@ -2428,9 +2410,8 @@ static bool fill_scatter_targets(const kvbm_scatter_target* tg, int n, uint32_t 
 // The scatter: every check before any CUDA call (repage_launch's with the source as the launch's side, and the target-count rule
 // before them), then one kvbm_paged_repage_scatter_kernel launch and the signal.  st: a streamed launch (its flags are the ones
 // passed, and its done flag is written with the targets'), which takes the gated push kernel, or per source layer this launch
-// unstreamed.  B: a batch of sequences in place of the one token range (token_begin / token_end unused), which always takes the
-// push_seqs kernels, or the route kernels for a routed batch, whose every target mask must be non-zero and below bit num_targets,
-// or the phased push kernels for a batch whose pages need not divide (B->any), or the deal kernels for one that is both.
+// unstreamed.  B: a batch of sequences in place of the one token range (token_begin / token_end unused), which takes its kind's
+// kernels (RepageKernels); a routed batch's every target mask must be non-zero and below bit num_targets.
 static cudaError_t launch_paged_repage_scatter(const kvbm_permute_side* src, uint32_t src_num_heads, uint32_t src_page,
                                                const kvbm_scatter_target* targets, int num_targets, uint32_t dst_page, uint32_t token_begin,
                                                uint32_t token_end, int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode,
@@ -2439,9 +2420,12 @@ static cudaError_t launch_paged_repage_scatter(const kvbm_permute_side* src, uin
 {
   RepageLaunch L;
   if (!targets || num_targets < 1 || num_targets > KVBM_GATHER_MAX_SOURCES) return cudaErrorInvalidValue;
-  if (B && B->route && B->route_seqs)
-    for (size_t i = 0; i < B->num_seqs; ++i)
-      if (B->route_seqs[i].targets == 0 || (B->route_seqs[i].targets >> num_targets) != 0) return cudaErrorInvalidValue;
+  const RepageUnits units = B ? B->kind : kRange;
+  if (routed_units(units) && B->seqs)
+    for (size_t i = 0; i < B->num_seqs; ++i) {
+      const uint32_t m = static_cast<const kvbm_route_seq*>(B->seqs)[i].targets;
+      if (m == 0 || (m >> num_targets) != 0) return cudaErrorInvalidValue;
+    }
   if (!repage_launch(src, src_page, dst_page, token_begin, token_end, layer_begin, layer_end, src_row_bytes, cast_mode, cast_scales, B, &L))
     return cudaErrorInvalidValue;
   if (L.units == 0) return scatter_signal(targets, num_targets, st ? st->done_flag : nullptr, epoch, completion_flag, completion_value, stream);
@@ -2472,36 +2456,22 @@ static cudaError_t launch_paged_repage_scatter(const kvbm_permute_side* src, uin
           bool any;
           const ScatterFlags F = scatter_flags(targets, num_targets, &any);
           Ag.ss.want_done |= any;
-          with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, L.page_pow2, [&](auto c, auto p, auto sc, auto pp) {
-            if (B && B->route && B->any)
-              kvbm_gated_repage_deal_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, Ag, F, num_targets, B->route_any_units, L.num_big, r,
-                                                                                       cast_scales, batch);
-            else if (B && B->route)
-              kvbm_gated_repage_route_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, Ag, F, num_targets, B->route_units, L.num_big, r,
-                                                                                        cast_scales, batch);
-            else if (B && B->any)
-              kvbm_gated_repage_phased_push_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, Ag, F, num_targets, B->any_units, L.num_big,
-                                                                                              r, cast_scales, batch);
-            else if (B)
-              kvbm_gated_repage_push_seqs_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, Ag, F, num_targets, B->units, L.num_big, r,
-                                                                                            cast_scales, batch);
+          with_repage_units(units, cast_mode, r.pow2, cast_scales != nullptr, L.page_pow2, [&](auto u, auto c, auto p, auto sc, auto pp) {
+            const auto kernel = RepageKernels<u>::template gated_scatter<c, p, sc, pp>;
+            if constexpr (u == kRange)
+              kernel<<<ctas, threads, 0, stream>>>(P, Ag, F, num_targets, L.num_big, r, cast_scales, batch);
             else
-              kvbm_gated_repage_push_kernel<c, p, sc, pp><<<ctas, threads, 0, stream>>>(P, Ag, F, num_targets, L.num_big, r, cast_scales, batch);
+              kernel<<<ctas, threads, 0, stream>>>(P, Ag, F, num_targets, batch_table<u>(B), L.num_big, r, cast_scales, batch);
           });
         });
   }
-  with_repage_kernel(cast_mode, r.pow2, cast_scales != nullptr, L.page_pow2, [&](auto c, auto p, auto sc, auto pp) {
-    if (B && B->route && B->any)
-      kvbm_paged_repage_deal_kernel<c, p, sc, pp><<<static_cast<unsigned>(L.units), threads, 0, stream>>>(P, B->route_any_units, r, cast_scales);
-    else if (B && B->route)
-      kvbm_paged_repage_route_kernel<c, p, sc, pp><<<static_cast<unsigned>(L.units), threads, 0, stream>>>(P, B->route_units, r, cast_scales);
-    else if (B && B->any)
-      kvbm_paged_repage_phased_push_kernel<c, p, sc, pp><<<static_cast<unsigned>(L.units), threads, 0, stream>>>(P, B->any_units, r,
-                                                                                                                cast_scales);
-    else if (B)
-      kvbm_paged_repage_push_seqs_kernel<c, p, sc, pp><<<static_cast<unsigned>(L.units), threads, 0, stream>>>(P, B->units, r, cast_scales);
+  const unsigned grid = static_cast<unsigned>(L.units);
+  with_repage_units(units, cast_mode, r.pow2, cast_scales != nullptr, L.page_pow2, [&](auto u, auto c, auto p, auto sc, auto pp) {
+    const auto kernel = RepageKernels<u>::template scatter<c, p, sc, pp>;
+    if constexpr (u == kRange)
+      kernel<<<grid, threads, 0, stream>>>(P, r, cast_scales);
     else
-      kvbm_paged_repage_scatter_kernel<c, p, sc, pp><<<static_cast<unsigned>(L.units), threads, 0, stream>>>(P, r, cast_scales);
+      kernel<<<grid, threads, 0, stream>>>(P, batch_table<u>(B), r, cast_scales);
   });
   g_launches.fetch_add(1, std::memory_order_relaxed);
   const cudaError_t e = cudaGetLastError();
@@ -2831,6 +2801,56 @@ kvbm_kernels_repage_route_anypage_units(const kvbm_route_seq* seqs, size_t num_s
                      [seqs](size_t i, uint32_t phase) { return seqs[i].targets | phase << 16; }, /*any=*/true);
 }
 
+// The body of every batch re-paging gather entry: a batch of UNITS, streamed through st (checked here, and then with st's flags),
+// else with the flags passed.  A streamed routed batch needs the ready flags of the sources some sequence is routed to only.
+template <RepageUnits UNITS>
+static cudaError_t repage_gather_batch(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page_size, const kvbm_permute_side* dst,
+                                       uint32_t dst_num_heads, uint32_t dst_page_size, const typename RepageKernels<UNITS>::Seq* seqs,
+                                       size_t num_seqs, const typename RepageKernels<UNITS>::Record* units, size_t num_units, int layer_begin,
+                                       int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales, bool streamed,
+                                       const kvbm_permute_stream* st, uint32_t* done_flag, uint32_t epoch, uint32_t* completion_flag,
+                                       uint32_t completion_value, cudaStream_t stream)
+{
+  if (streamed) {
+    uint32_t used = ~0u;
+    if constexpr (routed_units(UNITS)) {
+      used = 0;
+      for (size_t i = 0; seqs && i < num_seqs; ++i) used |= seqs[i].targets;
+    }
+    if (!stream_args_ok(st, num_srcs, used)) return cudaErrorInvalidValue;
+    done_flag = st->done_flag;
+    epoch = st->epoch;
+    completion_flag = st->completion_flag;
+    completion_value = st->completion_value;
+  }
+  const RepageBatch B = repage_batch<UNITS>(seqs, num_seqs, units, num_units);
+  return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, 0, 0, layer_begin, layer_end,
+                                    src_row_bytes, cast_mode, cast_scales, done_flag, epoch, completion_flag, completion_value,
+                                    KVBM_GATHER_MAX_HEADS, stream, st, &B);
+}
+
+// The body of every batch scatter entry: a batch of UNITS, streamed through st (checked here, and then with st's flags), else
+// with the flags passed.
+template <RepageUnits UNITS>
+static cudaError_t repage_scatter_batch(const kvbm_permute_side* src, uint32_t src_num_heads, uint32_t src_page_size,
+                                        const kvbm_scatter_target* targets, int num_targets, uint32_t dst_page_size,
+                                        const typename RepageKernels<UNITS>::Seq* seqs, size_t num_seqs,
+                                        const typename RepageKernels<UNITS>::Record* units, size_t num_units, int layer_begin, int layer_end,
+                                        uint32_t src_row_bytes, int cast_mode, const float* cast_scales, bool streamed,
+                                        const kvbm_permute_stream* st, uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value,
+                                        cudaStream_t stream)
+{
+  if (streamed) {
+    if (!stream_args_ok(st, 1)) return cudaErrorInvalidValue;
+    epoch = st->epoch;
+    completion_flag = st->completion_flag;
+    completion_value = st->completion_value;
+  }
+  const RepageBatch B = repage_batch<UNITS>(seqs, num_seqs, units, num_units);
+  return launch_paged_repage_scatter(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, 0, 0, layer_begin, layer_end,
+                                     src_row_bytes, cast_mode, cast_scales, epoch, completion_flag, completion_value, stream, st, &B);
+}
+
 extern "C" cudaError_t
 kvbm_kernels_paged_stage_repage_gather_anypage(const kvbm_stage_source* srcs, int num_srcs, uint32_t src_page_size, const kvbm_permute_side* dst,
                                                uint32_t dst_num_heads, uint32_t dst_page_size, const kvbm_repage_seq* seqs, size_t num_seqs,
@@ -2838,10 +2858,9 @@ kvbm_kernels_paged_stage_repage_gather_anypage(const kvbm_stage_source* srcs, in
                                                uint32_t src_row_bytes, int cast_mode, const float* cast_scales, uint32_t* done_flag,
                                                uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
 {
-  const RepageBatch B{seqs, num_seqs, nullptr, num_units, false, nullptr, nullptr, true, units};
-  return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, 0, 0, layer_begin, layer_end,
-                                    src_row_bytes, cast_mode, cast_scales, done_flag, epoch, completion_flag, completion_value,
-                                    KVBM_GATHER_MAX_HEADS, stream, nullptr, &B);
+  return repage_gather_batch<kPhased>(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, seqs, num_seqs, units, num_units,
+                                      layer_begin, layer_end, src_row_bytes, cast_mode, cast_scales, false, nullptr, done_flag, epoch,
+                                      completion_flag, completion_value, stream);
 }
 
 extern "C" cudaError_t
@@ -2852,11 +2871,9 @@ kvbm_kernels_paged_stage_repage_gather_anypage_streamed(const kvbm_stage_source*
                                                         int cast_mode, const float* cast_scales, const kvbm_permute_stream* st,
                                                         cudaStream_t stream)
 {
-  if (!stream_args_ok(st, num_srcs)) return cudaErrorInvalidValue;
-  const RepageBatch B{seqs, num_seqs, nullptr, num_units, false, nullptr, nullptr, true, units};
-  return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, 0, 0, layer_begin, layer_end,
-                                    src_row_bytes, cast_mode, cast_scales, st->done_flag, st->epoch, st->completion_flag,
-                                    st->completion_value, KVBM_GATHER_MAX_HEADS, stream, st, &B);
+  return repage_gather_batch<kPhased>(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, seqs, num_seqs, units, num_units,
+                                      layer_begin, layer_end, src_row_bytes, cast_mode, cast_scales, true, st, nullptr, 0, nullptr, 0,
+                                      stream);
 }
 
 extern "C" cudaError_t
@@ -2866,10 +2883,9 @@ kvbm_kernels_paged_stage_repage_gather_batch(const kvbm_stage_source* srcs, int 
                                              uint32_t src_row_bytes, int cast_mode, const float* cast_scales, uint32_t* done_flag,
                                              uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
 {
-  const RepageBatch B{seqs, num_seqs, units, num_units};
-  return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, 0, 0, layer_begin, layer_end,
-                                    src_row_bytes, cast_mode, cast_scales, done_flag, epoch, completion_flag, completion_value,
-                                    KVBM_GATHER_MAX_HEADS, stream, nullptr, &B);
+  return repage_gather_batch<kSeqs>(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, seqs, num_seqs, units, num_units,
+                                    layer_begin, layer_end, src_row_bytes, cast_mode, cast_scales, false, nullptr, done_flag, epoch,
+                                    completion_flag, completion_value, stream);
 }
 
 extern "C" cudaError_t
@@ -2880,11 +2896,9 @@ kvbm_kernels_paged_stage_repage_gather_batch_streamed(const kvbm_stage_source* s
                                                       int cast_mode, const float* cast_scales, const kvbm_permute_stream* st,
                                                       cudaStream_t stream)
 {
-  if (!stream_args_ok(st, num_srcs)) return cudaErrorInvalidValue;
-  const RepageBatch B{seqs, num_seqs, units, num_units};
-  return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, 0, 0, layer_begin, layer_end,
-                                    src_row_bytes, cast_mode, cast_scales, st->done_flag, st->epoch, st->completion_flag,
-                                    st->completion_value, KVBM_GATHER_MAX_HEADS, stream, st, &B);
+  return repage_gather_batch<kSeqs>(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, seqs, num_seqs, units, num_units,
+                                    layer_begin, layer_end, src_row_bytes, cast_mode, cast_scales, true, st, nullptr, 0, nullptr, 0,
+                                    stream);
 }
 
 extern "C" cudaError_t
@@ -2894,10 +2908,9 @@ kvbm_kernels_paged_stage_repage_gather_routed(const kvbm_stage_source* srcs, int
                                               uint32_t src_row_bytes, int cast_mode, const float* cast_scales, uint32_t* done_flag,
                                               uint32_t epoch, uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
 {
-  const RepageBatch B{nullptr, num_seqs, nullptr, num_units, true, seqs, units};
-  return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, 0, 0, layer_begin, layer_end,
-                                    src_row_bytes, cast_mode, cast_scales, done_flag, epoch, completion_flag, completion_value,
-                                    KVBM_GATHER_MAX_HEADS, stream, nullptr, &B);
+  return repage_gather_batch<kRouted>(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, seqs, num_seqs, units, num_units,
+                                      layer_begin, layer_end, src_row_bytes, cast_mode, cast_scales, false, nullptr, done_flag, epoch,
+                                      completion_flag, completion_value, stream);
 }
 
 extern "C" cudaError_t
@@ -2908,13 +2921,9 @@ kvbm_kernels_paged_stage_repage_gather_routed_streamed(const kvbm_stage_source* 
                                                        int cast_mode, const float* cast_scales, const kvbm_permute_stream* st,
                                                        cudaStream_t stream)
 {
-  uint32_t used = 0;  // the sources some sequence is routed to: only they need ready flags
-  for (size_t i = 0; seqs && i < num_seqs; ++i) used |= seqs[i].targets;
-  if (!stream_args_ok(st, num_srcs, used)) return cudaErrorInvalidValue;
-  const RepageBatch B{nullptr, num_seqs, nullptr, num_units, true, seqs, units};
-  return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, 0, 0, layer_begin, layer_end,
-                                    src_row_bytes, cast_mode, cast_scales, st->done_flag, st->epoch, st->completion_flag,
-                                    st->completion_value, KVBM_GATHER_MAX_HEADS, stream, st, &B);
+  return repage_gather_batch<kRouted>(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, seqs, num_seqs, units, num_units,
+                                      layer_begin, layer_end, src_row_bytes, cast_mode, cast_scales, true, st, nullptr, 0, nullptr, 0,
+                                      stream);
 }
 
 extern "C" cudaError_t
@@ -2925,10 +2934,9 @@ kvbm_kernels_paged_stage_repage_gather_routed_anypage(const kvbm_stage_source* s
                                                       const float* cast_scales, uint32_t* done_flag, uint32_t epoch, uint32_t* completion_flag,
                                                       uint32_t completion_value, cudaStream_t stream)
 {
-  const RepageBatch B{nullptr, num_seqs, nullptr, num_units, true, seqs, nullptr, true, nullptr, units};
-  return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, 0, 0, layer_begin, layer_end,
-                                    src_row_bytes, cast_mode, cast_scales, done_flag, epoch, completion_flag, completion_value,
-                                    KVBM_GATHER_MAX_HEADS, stream, nullptr, &B);
+  return repage_gather_batch<kRoutedPhased>(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, seqs, num_seqs, units,
+                                            num_units, layer_begin, layer_end, src_row_bytes, cast_mode, cast_scales, false, nullptr,
+                                            done_flag, epoch, completion_flag, completion_value, stream);
 }
 
 extern "C" cudaError_t
@@ -2939,13 +2947,9 @@ kvbm_kernels_paged_stage_repage_gather_routed_anypage_streamed(const kvbm_stage_
                                                                int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
                                                                const kvbm_permute_stream* st, cudaStream_t stream)
 {
-  uint32_t used = 0;  // the sources some sequence is routed to: only they need ready flags
-  for (size_t i = 0; seqs && i < num_seqs; ++i) used |= seqs[i].targets;
-  if (!stream_args_ok(st, num_srcs, used)) return cudaErrorInvalidValue;
-  const RepageBatch B{nullptr, num_seqs, nullptr, num_units, true, seqs, nullptr, true, nullptr, units};
-  return launch_paged_repage_gather(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, 0, 0, layer_begin, layer_end,
-                                    src_row_bytes, cast_mode, cast_scales, st->done_flag, st->epoch, st->completion_flag,
-                                    st->completion_value, KVBM_GATHER_MAX_HEADS, stream, st, &B);
+  return repage_gather_batch<kRoutedPhased>(srcs, num_srcs, src_page_size, dst, dst_num_heads, dst_page_size, seqs, num_seqs, units,
+                                            num_units, layer_begin, layer_end, src_row_bytes, cast_mode, cast_scales, true, st, nullptr, 0,
+                                            nullptr, 0, stream);
 }
 
 extern "C" cudaError_t
@@ -2977,9 +2981,9 @@ kvbm_kernels_paged_repage_scatter_batch(const kvbm_permute_side* src, uint32_t s
                                         uint32_t src_row_bytes, int cast_mode, const float* cast_scales, uint32_t epoch,
                                         uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
 {
-  const RepageBatch B{seqs, num_seqs, units, num_units};
-  return launch_paged_repage_scatter(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, 0, 0, layer_begin, layer_end,
-                                     src_row_bytes, cast_mode, cast_scales, epoch, completion_flag, completion_value, stream, nullptr, &B);
+  return repage_scatter_batch<kSeqs>(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, seqs, num_seqs, units,
+                                     num_units, layer_begin, layer_end, src_row_bytes, cast_mode, cast_scales, false, nullptr, epoch,
+                                     completion_flag, completion_value, stream);
 }
 
 extern "C" cudaError_t
@@ -2989,11 +2993,9 @@ kvbm_kernels_paged_repage_scatter_batch_streamed(const kvbm_permute_side* src, u
                                                  int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
                                                  const kvbm_permute_stream* st, cudaStream_t stream)
 {
-  if (!stream_args_ok(st, 1)) return cudaErrorInvalidValue;
-  const RepageBatch B{seqs, num_seqs, units, num_units};
-  return launch_paged_repage_scatter(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, 0, 0, layer_begin, layer_end,
-                                     src_row_bytes, cast_mode, cast_scales, st->epoch, st->completion_flag, st->completion_value, stream, st,
-                                     &B);
+  return repage_scatter_batch<kSeqs>(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, seqs, num_seqs, units,
+                                     num_units, layer_begin, layer_end, src_row_bytes, cast_mode, cast_scales, true, st, 0, nullptr, 0,
+                                     stream);
 }
 
 extern "C" cudaError_t
@@ -3003,9 +3005,9 @@ kvbm_kernels_paged_repage_scatter_anypage(const kvbm_permute_side* src, uint32_t
                                           int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales, uint32_t epoch,
                                           uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
 {
-  const RepageBatch B{seqs, num_seqs, nullptr, num_units, false, nullptr, nullptr, true, units};
-  return launch_paged_repage_scatter(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, 0, 0, layer_begin, layer_end,
-                                     src_row_bytes, cast_mode, cast_scales, epoch, completion_flag, completion_value, stream, nullptr, &B);
+  return repage_scatter_batch<kPhased>(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, seqs, num_seqs, units,
+                                       num_units, layer_begin, layer_end, src_row_bytes, cast_mode, cast_scales, false, nullptr, epoch,
+                                       completion_flag, completion_value, stream);
 }
 
 extern "C" cudaError_t
@@ -3015,11 +3017,9 @@ kvbm_kernels_paged_repage_scatter_anypage_streamed(const kvbm_permute_side* src,
                                                    size_t num_units, int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode,
                                                    const float* cast_scales, const kvbm_permute_stream* st, cudaStream_t stream)
 {
-  if (!stream_args_ok(st, 1)) return cudaErrorInvalidValue;
-  const RepageBatch B{seqs, num_seqs, nullptr, num_units, false, nullptr, nullptr, true, units};
-  return launch_paged_repage_scatter(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, 0, 0, layer_begin, layer_end,
-                                     src_row_bytes, cast_mode, cast_scales, st->epoch, st->completion_flag, st->completion_value, stream, st,
-                                     &B);
+  return repage_scatter_batch<kPhased>(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, seqs, num_seqs, units,
+                                       num_units, layer_begin, layer_end, src_row_bytes, cast_mode, cast_scales, true, st, 0, nullptr, 0,
+                                       stream);
 }
 
 extern "C" cudaError_t
@@ -3029,9 +3029,9 @@ kvbm_kernels_paged_repage_scatter_routed(const kvbm_permute_side* src, uint32_t 
                                          uint32_t src_row_bytes, int cast_mode, const float* cast_scales, uint32_t epoch,
                                          uint32_t* completion_flag, uint32_t completion_value, cudaStream_t stream)
 {
-  const RepageBatch B{nullptr, num_seqs, nullptr, num_units, true, seqs, units};
-  return launch_paged_repage_scatter(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, 0, 0, layer_begin, layer_end,
-                                     src_row_bytes, cast_mode, cast_scales, epoch, completion_flag, completion_value, stream, nullptr, &B);
+  return repage_scatter_batch<kRouted>(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, seqs, num_seqs, units,
+                                       num_units, layer_begin, layer_end, src_row_bytes, cast_mode, cast_scales, false, nullptr, epoch,
+                                       completion_flag, completion_value, stream);
 }
 
 extern "C" cudaError_t
@@ -3041,11 +3041,9 @@ kvbm_kernels_paged_repage_scatter_routed_streamed(const kvbm_permute_side* src, 
                                                   int layer_begin, int layer_end, uint32_t src_row_bytes, int cast_mode, const float* cast_scales,
                                                   const kvbm_permute_stream* st, cudaStream_t stream)
 {
-  if (!stream_args_ok(st, 1)) return cudaErrorInvalidValue;
-  const RepageBatch B{nullptr, num_seqs, nullptr, num_units, true, seqs, units};
-  return launch_paged_repage_scatter(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, 0, 0, layer_begin, layer_end,
-                                     src_row_bytes, cast_mode, cast_scales, st->epoch, st->completion_flag, st->completion_value, stream, st,
-                                     &B);
+  return repage_scatter_batch<kRouted>(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, seqs, num_seqs, units,
+                                       num_units, layer_begin, layer_end, src_row_bytes, cast_mode, cast_scales, true, st, 0, nullptr, 0,
+                                       stream);
 }
 
 extern "C" cudaError_t
@@ -3056,9 +3054,9 @@ kvbm_kernels_paged_repage_scatter_routed_anypage(const kvbm_permute_side* src, u
                                                  const float* cast_scales, uint32_t epoch, uint32_t* completion_flag,
                                                  uint32_t completion_value, cudaStream_t stream)
 {
-  const RepageBatch B{nullptr, num_seqs, nullptr, num_units, true, seqs, nullptr, true, nullptr, units};
-  return launch_paged_repage_scatter(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, 0, 0, layer_begin, layer_end,
-                                     src_row_bytes, cast_mode, cast_scales, epoch, completion_flag, completion_value, stream, nullptr, &B);
+  return repage_scatter_batch<kRoutedPhased>(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, seqs, num_seqs, units,
+                                             num_units, layer_begin, layer_end, src_row_bytes, cast_mode, cast_scales, false, nullptr,
+                                             epoch, completion_flag, completion_value, stream);
 }
 
 extern "C" cudaError_t
@@ -3069,11 +3067,9 @@ kvbm_kernels_paged_repage_scatter_routed_anypage_streamed(const kvbm_permute_sid
                                                           int cast_mode, const float* cast_scales, const kvbm_permute_stream* st,
                                                           cudaStream_t stream)
 {
-  if (!stream_args_ok(st, 1)) return cudaErrorInvalidValue;
-  const RepageBatch B{nullptr, num_seqs, nullptr, num_units, true, seqs, nullptr, true, nullptr, units};
-  return launch_paged_repage_scatter(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, 0, 0, layer_begin, layer_end,
-                                     src_row_bytes, cast_mode, cast_scales, st->epoch, st->completion_flag, st->completion_value, stream, st,
-                                     &B);
+  return repage_scatter_batch<kRoutedPhased>(src, src_num_heads, src_page_size, targets, num_targets, dst_page_size, seqs, num_seqs, units,
+                                             num_units, layer_begin, layer_end, src_row_bytes, cast_mode, cast_scales, true, st, 0, nullptr,
+                                             0, stream);
 }
 
 extern "C" cudaError_t
